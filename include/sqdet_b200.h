@@ -1,5 +1,5 @@
 /*
- * sqdet_b200.h — C ABI of libsqdet_b200.so: the B200 (sm_100a) SqueezeDet
+ * sqdet_b200.h — C ABI of libsqdet_b200.so: the H100 (sm_90a) SqueezeDet
  * inference hot path (conv backbone -> ConvDet -> interpret_output ->
  * filter_prediction / NMS).
  *
@@ -46,7 +46,7 @@ extern "C" {
 
 /* math_mode of the convolution kernels */
 #define SQDET_MATH_FP32_SIMT   0   /* fp32 FFMA direct/implicit-GEMM kernels            */
-#define SQDET_MATH_TF32X3_TC   1   /* tcgen05 tensor cores, 3xTF32 split (fp32-grade)    */
+#define SQDET_MATH_TF32X3_TC   1   /* wgmma tensor cores, 3xTF32 split (fp32-grade)      */
 
 typedef struct sqdet_engine sqdet_engine;   /* opaque */
 
@@ -222,11 +222,12 @@ int sqdet_conv2d(const float* x_dev, const float* w_hwio_dev, const float* bias_
                  int B, int H, int W, int Cin, int Cout, int size, int stride,
                  int padding, int relu, int y_cstride, int y_coff, int math_mode,
                  void* stream);
-/* The halo-tile tensor-core path of a 3x3, stride-1, SAME convolution (csrc/halo_tc.cu; the
- * plan the engine picks for the ConvDet head, src/nets/squeezeDet.py:73-78) as a stage-isolated
- * call: same arguments as sqdet_conv2d without size/stride/padding/math_mode.  Returns
- * SQDET_ERR_UNSUPPORTED for shapes that kernel does not take (Cin % 16, channel-window rules).
- * Synchronises the stream (test / debug entry).                                          */
+/* A 3x3, stride-1, SAME convolution (the ConvDet head's shape, src/nets/squeezeDet.py:73-78) as a
+ * stage-isolated call: same arguments as sqdet_conv2d without size/stride/padding/math_mode.  The
+ * name is kept for ABI compatibility: there is no separate halo-tile kernel any more, the call runs
+ * the same wgmma implicit-GEMM kernel as sqdet_conv2d with SQDET_MATH_TF32X3_TC.  Returns
+ * SQDET_ERR_UNSUPPORTED for shapes that kernel does not take (Cin % 16 != 0).  Synchronises the
+ * stream (test / debug entry).                                                             */
 int sqdet_conv3x3_halo(const float* x_dev, const float* w_hwio_dev, const float* bias_dev,
                        const float* scale_dev, const float* shift_dev, float* y_dev, int B,
                        int H, int W, int Cin, int Cout, int relu, int y_cstride, int y_coff,
@@ -234,9 +235,9 @@ int sqdet_conv3x3_halo(const float* x_dev, const float* w_hwio_dev, const float*
 /* SqueezeDet._fire_layer (src/nets/squeezeDet.py:81-106; same in squeezeDetPlus.py) as ONE
  * call: y[..., :E1] = relu(1x1_e1(q)+b), y[..., E1:] = relu(3x3_e3(q)+b), q = relu(1x1_s(x)+b).
  * x [B,H,W,Cin], kernels HWIO, y [B,H,W,E1+E3].  With SQDET_MATH_TF32X3_TC and a shape the
- * fused kernel takes (Cin % 32 == 0, S % 16 == 0, S <= 64, E % 32 == 0) this is ONE kernel
- * launch and the squeeze tensor never leaves the SM; other shapes run squeeze and expand
- * as separate launches.  Synchronises the stream (test / debug entry, not the hot path).    */
+ * one-kernel fire takes (Cin % 16 == 0, S in {16, 32, 48, 64}) this is ONE kernel launch and the
+ * squeeze tensor never leaves the SM; other shapes run squeeze and expand as separate launches.
+ * Synchronises the stream (test / debug entry, not the hot path).                          */
 int sqdet_fire(const float* x_dev, const float* w_sq_dev, const float* b_sq_dev,
                const float* w_e1_dev, const float* b_e1_dev, const float* w_e3_dev,
                const float* b_e3_dev, float* y_dev, int B, int H, int W, int Cin, int S,

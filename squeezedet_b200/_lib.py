@@ -1,6 +1,6 @@
 """ctypes binding of ``libsqdet_b200.so`` (the C ABI declared in
 ``include/sqdet_b200.h``).  There is no CPU fallback: if the library is missing
-or no B200 is visible, calls fail loudly with :class:`SqdetError`."""
+or no H100 is visible, calls fail loudly with :class:`SqdetError`."""
 from __future__ import annotations
 
 import ctypes as C

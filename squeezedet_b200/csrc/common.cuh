@@ -1,4 +1,4 @@
-// Shared declarations for libsqdet_b200 (sm_100a only).
+// Shared declarations for libsqdet_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -28,8 +28,7 @@ int  cuda_fail(cudaError_t err, const char* what);
 // ---- programmatic dependent launch (PDL) --------------------------------------------------
 // The forward is a chain of ~20 kernels, each reading what the previous one wrote.  With the
 // programmatic-stream-serialization launch attribute a kernel may be SCHEDULED while its
-// predecessor still runs: its prologue (mbarrier init, tensor-memory allocation, tensor-map
-// fetch) overlaps the predecessor's ragged last wave, and `griddepcontrol.wait` then holds every
+// predecessor still runs: its prologue (index math, parameter fetch) overlaps the predecessor's ragged last wave, and `griddepcontrol.wait` then holds every
 // thread until the predecessor has completed and flushed.  Every kernel of the forward calls
 // pdl_trigger() first (lets ITS successor be scheduled) and pdl_wait() before touching global
 // memory; both are no-ops for a plain launch.  The engine switches the attribute on per thread

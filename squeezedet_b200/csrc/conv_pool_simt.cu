@@ -29,14 +29,6 @@ constexpr int CT_H = 2 * PT_H + 1, CT_W = 2 * PT_W + 1;   // 9 x 33 conv pixels 
 constexpr int CT_PIX = CT_H * CT_W;               // 297
 constexpr int PIX_PER_THREAD = (CT_PIX + 63) / 64;  // 5
 
-// Two IEEE fp32 FMAs per instruction (Blackwell FFMA2): identical results to two fmaf().
-__device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b,
-                                                    unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-
 struct ConvPoolParams {
   const float* x;       // [B,H,W,3]
   const float* w;       // [k,k,3,Cout]
@@ -112,11 +104,11 @@ conv_pool_simt_kernel(const ConvPoolParams p) {
   // ---- conv: 5 pixels x 16 channels per thread ----
   const int cg = tid >> 6;                 // channel group (warp-uniform)
   const int l64 = tid & 63;
-  unsigned long long acc2[PIX_PER_THREAD][8];      // 16 channels as 8 packed fp32 pairs
+  float acc[PIX_PER_THREAD][16];
 #pragma unroll
   for (int i = 0; i < PIX_PER_THREAD; ++i)
 #pragma unroll
-    for (int c = 0; c < 8; ++c) acc2[i][c] = 0ull;
+    for (int c = 0; c < 16; ++c) acc[i][c] = 0.f;
   int pbase[PIX_PER_THREAD];
 #pragma unroll
   for (int i = 0; i < PIX_PER_THREAD; ++i) {
@@ -130,33 +122,20 @@ conv_pool_simt_kernel(const ConvPoolParams p) {
 #pragma unroll
     for (int bc = 0; bc < KS * 3; ++bc) {          // (b, c) flattened: contiguous in the patch
       const int k = a * KS * 3 + bc;
-      unsigned long long xx[PIX_PER_THREAD];
+      float xx[PIX_PER_THREAD];
 #pragma unroll
-      for (int i = 0; i < PIX_PER_THREAD; ++i) {
-        const unsigned xb = __float_as_uint(s_patch[pbase[i] + a * PW * 3 + bc]);
-        xx[i] = ((unsigned long long)xb << 32) | xb;
-      }
+      for (int i = 0; i < PIX_PER_THREAD; ++i) xx[i] = s_patch[pbase[i] + a * PW * 3 + bc];
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {       // 8 channels at a time: fewer live weights
-        const ulonglong2 wa = *reinterpret_cast<const ulonglong2*>(wg + k * p.Cout + half * 8);
-        const ulonglong2 wb = *reinterpret_cast<const ulonglong2*>(wg + k * p.Cout + half * 8 + 4);
-        const unsigned long long wv[4] = {wa.x, wa.y, wb.x, wb.y};
+      for (int q = 0; q < 4; ++q) {                // 4 channels at a time: fewer live weights
+        const float4 w4 = *reinterpret_cast<const float4*>(wg + k * p.Cout + q * 4);
+        const float wv[4] = {w4.x, w4.y, w4.z, w4.w};
 #pragma unroll
         for (int i = 0; i < PIX_PER_THREAD; ++i)
 #pragma unroll
-          for (int c = 0; c < 4; ++c)
-            acc2[i][half * 4 + c] = ffma2(xx[i], wv[c], acc2[i][half * 4 + c]);
+          for (int c = 0; c < 4; ++c) acc[i][q * 4 + c] = fmaf(xx[i], wv[c], acc[i][q * 4 + c]);
       }
     }
   }
-  float acc[PIX_PER_THREAD][16];
-#pragma unroll
-  for (int i = 0; i < PIX_PER_THREAD; ++i)
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-      acc[i][2 * c] = __uint_as_float((unsigned)(acc2[i][c] & 0xffffffffull));
-      acc[i][2 * c + 1] = __uint_as_float((unsigned)(acc2[i][c] >> 32));
-    }
 
   // ---- epilogue 1: bias [, affine], relu, mask, conv tile -> smem ----
   {

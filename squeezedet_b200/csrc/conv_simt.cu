@@ -4,7 +4,7 @@
 // (reference src/nn_skeleton.py:539-547, :441-449).  Handles every shape the four
 // nets use (any k, stride, SAME/VALID, Cin incl. 3, strided channel-offset output for
 // the fire concat).  It is the kernel for conv1 (Cin = 3: K = 27/147 is too thin for
-// a tensor-core tile) and the on-device fp32 cross-check of the tcgen05 path.
+// a tensor-core tile) and the on-device fp32 cross-check of the wgmma path.
 //
 // GEMM view: M = B*Ho*Wo output pixels, N = Cout, K = kh*kw*Cin ordered (u, v, c) —
 // the row order of the HWIO weight tensor viewed as [K, Cout].

@@ -1,866 +1,515 @@
-// tcgen05 implicit-GEMM convolution with the 3xTF32 split (SQDET_MATH_TF32X3_TC).
+// Hopper (sm_90a) wgmma implicit-GEMM convolution with the 3xTF32 split (SQDET_MATH_TF32X3_TC).
 //
 // Replaces tf.nn.conv2d + bias_add [+ batch_normalization] + relu of the reference
-// (src/nn_skeleton.py:539-547, :441-449) for every stride-1 conv whose Cin is a multiple
-// of 16 (all fire squeeze/expand convs, the ConvDet head, the VGG/ResNet body) and for 3x3
-// convs over 3-channel images ("gather mode"), and fuses a fire module's expand1x1 ||
-// expand3x3 + channel concat (src/nets/squeezeDet.py:96-106) into one launch.
+// (src/nn_skeleton.py:539-547, :441-449) for every stride-1 SAME 1x1 / 3x3 conv whose Cin is a
+// multiple of 16 (all fire squeeze/expand convs, the ConvDet head, the VGG/ResNet body) and for
+// 3x3 convs over 3-channel images ("gather mode"), and runs a fire module's expand1x1 ||
+// expand3x3 + channel concat (src/nets/squeezeDet.py:96-106) as one launch.
 //
-// GEMM view per CTA:  D[128 pixels, N] += A[128 pixels, K] * W[K, N]
-//   M tile  = an 8 x 16 patch of output pixels of one image (TMEM lane = pixel); 128 consecutive
-//             pixels of the flattened B*H*W list when the launch holds only 1x1 convs; the conv
-//             pixels under a block of pooling windows when a stride-2 max-pool is fused
-//   N       = one chunk of output channels (multiple of 16, <= 128; TMEM column = channel)
-//   K       = taps x Cin, walked as (tap, 32- or 16-channel chunk)
-//   A       : TMA tiled load of the NHWC activation tensor, box {KC ch, 16 w, 8 h, 1 n} at
-//             the tap-shifted coordinate; out-of-image coordinates are zero-filled by the
-//             TMA unit = TF "SAME" zero padding; lands K-major with the 128B/64B swizzle.
-//   W       : host-packed [chunk][tap][kchunk][N][KC] fp32 (hi and lo halves), 2-D TMA.
-// Precision: fp32 operands are split a = a_hi + a_lo with a_hi = rn_tf32(a), a_lo = a - a_hi
-//   (exact; the tensor core reads its top 19 bits); D += a_lo*b_hi + a_hi*b_lo + a_hi*b_hi with
-//   fp32 accumulation in TMEM (kind::tf32).  Dropped terms ~ 2^-21: fp32-grade results, which the
-//   1e-4 parity bar against the fp32 reference needs through ~25 stacked convs (plain TF32
-//   or BF16 miss it by 1-2 orders of magnitude).  Weights are pre-split on the host.  The
-//   activation split is done by 4 warps between the TMA landing and the MMA issue: each thread
-//   reads its pixel's row of the raw tile from smem and writes a_hi / a_lo into TENSOR MEMORY
-//   (tcgen05.st); the MMAs take A from TMEM (.ts form) and only B from smem.  (With A in smem
-//   the kernel was shared-memory-bandwidth bound; measured, see DESIGN.md.)
-// Accumulation: the tensor core adds into its fp32 accumulator with truncation (measured
-//   on B200: a systematic shrink, linear in the number of chained MMAs, 3.6e-5 of max at
-//   K=6912 vs 2e-6 for fp32 FFMA).  So a tile's K loop is cut into SEGMENTS of 36 MMAs, each
-//   accumulated from zero in one of two TMEM buffers; the drain warps add finished segments
-//   into fp32 registers (round-to-nearest) scaled by 1 + 1.4e-8 * (MMAs in the segment), the
-//   measured first-order size of the remaining bias; the drain of segment g overlaps the MMAs of
-//   segment g+1.
-// Persistent CTAs (one per SM, 512 threads = 4 warpgroups) over (chunk, tile) items, round-robin
-//   or a host-computed longest-processing-time-first schedule:  warpgroup 0: warp 0 = TMA
-//   producer, warp 1 = TMEM owner + MMA issuer (one elected lane), warps 2-3 idle;  warpgroup 1 =
-//   operand splitter;  warpgroups 2 and 3 = segment drain + epilogue (tcgen05.ld -> fp32 FFMA ->
-//   +bias [*scale+shift] -> relu -> TMA store), alternating items (measured: one drain group was
-//   the bottleneck of the small-K layers - the MMA warp spent 30-45 % of its time waiting for
-//   TMEM buffers).  setmaxnreg moves registers from warpgroups 0/1 to the drain warpgroups, whose
-//   running sums (up to 128 per thread) must stay out of local memory.
-// Pipelines: full[s] (TMA -> splitter), split[s] (splitter -> MMA), empty[s]
-//   (tcgen05.commit -> TMA), tfull[group][b] (tcgen05.commit -> drain), tempty[b] (drain -> MMA).
-// Opt-in variants kept for measurement (all parity-green, all slower today, DESIGN.md 4.1):
-//   weight-tile TMA multicast over CTA clusters, CTA-pair MMA (cta_group::2), fused max-pool
-//   epilogue; -DSQDET_ABLATE builds can switch pipeline pieces off (tools/ablate.sh).
-// Roofline: SqueezeDet fire2-9 are HBM-bound even fused (AI 24-95 FLOP/B fp32 I/O),
-//   fire10/11 ~ridge, ConvDet tensor-bound (SURVEY.md §8d); 3xTF32 costs 3 MMAs at the
-//   TF32 rate per algorithmic MAC.
-#include <cuda.h>
+// GEMM view per CTA:  D[128 pixels, NT] += A[128 pixels, K] * W[K, NT]
+//   M tile : 128 consecutive pixels of the flattened B*Ho*Wo output list; two warpgroups, each
+//            owning 64 rows (one wgmma m64 row block).
+//   N      : one chunk of NT output channels (16, 32 or 64) of one conv; blockIdx.y walks the
+//            chunks of every conv of the launch (the fire expand pair is two convs).
+//   K      : taps x Cin walked in KC-channel chunks (KC = 32 or 16); gather mode flattens
+//            (dy, dx, c) and pads it to a multiple of 32.
+//   A      : cp.async (zero-fill = TF SAME padding) into a row-major [pixel][KC + 4] tile, then
+//            into registers in the wgmma A-fragment layout (the +4 keeps the reads conflict-free).
+//   W      : host-packed per (chunk, K chunk) in the no-swizzle K-major core-matrix layout
+//            [NT/8][KC/4][8 rows][4 floats], hi then lo half; cp.async, read by wgmma through a
+//            shared-memory descriptor.
+// Precision: fp32 operands are split a = a_hi + a_lo with a_hi = rn_tf32(a), a_lo = rn_tf32(a - a_hi)
+//   (rounding a_lo here keeps the tensor core's truncation of its inputs from biasing the sum);
+//   D += a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (the dropped lo*lo term is ~2^-22 of a product): fp32-
+//   grade results, which the 1e-4 parity bar against the fp32 reference needs through ~25
+//   stacked convs (plain TF32 misses it by 1-2 orders of magnitude).  Weights are pre-split on the
+//   host, activations in registers after the A-fragment load.
+// Accumulation: each 8-wide K step (the three split MMAs) accumulates from zero in the wgmma
+//   accumulator and is then added into fp32 running sums with round-to-nearest FADDs, so the
+//   tensor core's truncating accumulation never compounds over a long K (longer chains in the
+//   accumulator left a one-signed error that fails the 1e-4 box parity of SqueezeDet+).
+// Pipeline: 3-stage cp.async ring (one commit group per K chunk); each wgmma group is waited for
+//   before its sums are read, so a stage is free again at the next block barrier.
 #include <cuda_runtime.h>
-#include <math.h>
-#include <math_constants.h>
-#include <stdio.h>
+#include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
 
-#include <algorithm>
-#include <queue>
 #include <vector>
 
 #include "common.cuh"
 #include "conv_tc.cuh"
-#include "halo_tc.cuh"
-#include "tc_ptx.cuh"
 
 namespace sqdet {
 namespace {
 
-constexpr int TILE_H = 8, TILE_W = 16, TILE_M = TILE_H * TILE_W;   // 128 pixels
-constexpr int NUM_THREADS = 512;       // 4 warpgroups: {TMA, MMA, 2 spare} | splitter | drain A | drain B
-constexpr int MAX_CHUNKS = 16;
-constexpr int MAX_N = 128;          // output channels per item (register-resident running sums)
-constexpr int POOL_MAX_N = 64;      // ... when a max-pool is fused (conv tile staged per drain group)
-constexpr int POOL_MAX_GROUPS = POOL_MAX_N / 32;
-constexpr int POOL_STAGE_BYTES = POOL_MAX_GROUPS * (16384 + 4096);   // conv + pooled tiles
-constexpr int MAX_STAGES = 8;
-constexpr int GATHER_PITCH = 128;   // floats between patch rows in the stage (gather mode)
+constexpr int TILE_M = 128;
+constexpr int NUM_THREADS = 256;   // 2 warpgroups x 64 rows
+constexpr int STAGES = 3;
+constexpr int MAX_CHUNKS = 32;
 
 struct TcChunk {
-  int ksize;        // 1 or 3 (square)
-  int pad;          // SAME: (ksize-1)/2
-  int w_row_base;   // first row of this chunk in the packed weight matrix (hi half)
-  int ch_base;      // output channel (within this conv group) of TMEM column 0
-  int ch_count;     // valid output channels in this chunk
-  int y_coff;       // channel offset of ch_base..ch_base+ch_count in the output tensor
-  int bias_base;    // index of ch_base in the bias/scale/shift arrays
-  int tap_begin;    // first filter tap of this chunk (split-K partials cover tap sub-ranges)
-  int tap_count;    // number of taps (ksize*ksize unless split)
-  int kc_begin;     // first K chunk (of KC input channels) of this chunk; split-K partials cover ranges
-  int kc_count;     // number of K chunks (Cin / KC unless split)
+  int ksize, pad_t, pad_l;  // this conv's filter size and top / left zero padding
+  int nk;                   // K chunks of KC channels
+  int ncount;               // valid output channels of this chunk (<= NT)
+  int y_off;                // first output channel in y
+  int p_off;                // first entry of bias / scale / shift
+  long long w_off;          // float offset of the chunk's packed weights
 };
 
 struct TcParams {
-  CUtensorMap tmA;
-  CUtensorMap tmW;
-  CUtensorMap tmWs;     // weight slice map for cluster multicast: box {KC, 2N/cluster} rows
-  CUtensorMap tmY;      // output tensor, box {32 ch, 16 w, 8 h, 1}, SWIZZLE_128B (TMA-store epilogue)
-  const float* bias;    // may be null
-  const float* scale;   // may be null (frozen BN)
-  const float* shift;
+  const float* x;
   float* y;
-  int B, Ho, Wo, tiles_h, tiles_w;
-  int kch;              // Cin / KC
-  int N;                // UMMA N (uniform over chunks)
-  int tmem_cols;        // power of two >= 2*N (two accumulator buffers) + stages*2*KC (A slots)
-  int seg_stages;       // pipeline stages (K blocks) per accumulation segment
-  float bias_comp;      // first-order compensation of the accumulator's truncation bias, per chained MMA
-  int ntiles;           // B * tiles_h * tiles_w
-  int tma_store;        // 1: epilogue stages 32-channel groups in smem and issues TMA stores
-  // conv tile (rows of the M=128 MMA tile): ct_h x ct_w output pixels (8x16, or 7x17 / 8x16
-  // when a 3x3 / 2x2 stride-2 max-pool is fused into the epilogue); tile step in conv pixels
-  int ct_h, ct_w, step_h, step_w, org_h, org_w;   // origin = tile*step - org
-  int sq_w, sq_h;       // TMA-store epilogue: offset of drain warp q's 32-pixel slab in the tile
-  // gather mode (first layer: 3x3 conv over a 3-channel image): the A tile is the im2col
-  // of an input patch; the producer fetches the patch row by row with 1-D TMA loads (rows of a
-  // 3-channel fp32 image are only 4-byte aligned, which rules out the tiled 4-D map), K = 27
-  // padded to one 32-wide K block
-  CUtensorMap tmX;      // the whole input as a 1-D array of floats, box = g_box floats
-  int gather;           // 1 = gather mode
-  int g_H, g_W, g_stride, g_pad_t, g_pad_l;
-  int g_ph, g_box;      // patch rows; floats fetched per patch row (patch columns * 3, padded to 4)
-  // fused max-pool (0 = none, else window 2 or 3; stride 2): pooled tile pt_h x pt_w, pooled dims
-  int pool, pt_h, pt_w, Hp, Wp;
-  int store_ring;       // per-warp TMA-store staging tiles (2, or 1 to buy one more pipeline stage)
-  int ablate;           // profiling builds only (-DSQDET_ABLATE): bitmask of pipeline pieces to skip
-  int two_cta;          // 1: CTA-pair MMA (cta_group::2), implies cluster == 2
-  int cluster;          // CTAs per cluster (1, 2 or 4): weight tiles are TMA-multicast across it
-  int exp_mode;         // timing experiments only (SQDET_TC_EXP): 1 no fence, 2 no store, 4 no STS
-  int two_split;        // 1: warpgroup 3 is a SECOND operand splitter (alternate stages) and warpgroup 2 the
-                        // only drain group: thin-N, K-heavy launches whose stage the splitter paced
-  // static schedule (launches whose chunks differ in cost): sched[0 .. nbins] = first entry of each
-  // cluster's item list, followed by the lists (longest-processing-time-first assignment);
-  // null = round-robin `item = cluster id + k * clusters`
-  const int* sched;
-  long long* dbg;       // optional per-CTA cycle counters (SQDET_TC_DEBUG=1), else null
-  int y_cstride, relu;
-  int lo_row_offset;    // rows between the hi and the lo copy of the packed weights
-  int stages;
+  const float* w;
+  const float* bias;   // may be null
+  const float* scale;  // null unless a frozen-BN affine follows the bias
+  const float* shift;
+  int B, H, W, Cin, Ho, Wo, stride, relu, y_cstride;
+  long long M;         // B * Ho * Wo
   int nchunks;
-  TcChunk chunk[MAX_CHUNKS];
+  TcChunk chunks[MAX_CHUNKS];
 };
 
-// Debug-only stall accounting: cycles spent inside a barrier wait, per role.
-#define SQ_TIMED_WAIT(counter, bar, parity)                 \
-  do {                                                      \
-    if (p.dbg) {                                            \
-      const long long _t0 = clock64();                      \
-      mbar_wait(bar, parity);                               \
-      counter += clock64() - _t0;                           \
-    } else {                                                \
-      mbar_wait(bar, parity);                               \
-    }                                                       \
-  } while (0)
+// ---------------------------------------------------------------------------------------------
+// PTX wrappers
+__device__ __forceinline__ uint32_t smem_u32(const void* p) {
+  return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src),
+               "r"(valid ? 16 : 0)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async4(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src),
+               "r"(valid ? 4 : 0)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+// cp.async writes are generic-proxy writes; wgmma reads shared memory through the async proxy
+__device__ __forceinline__ void fence_proxy_async() {
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void wgmma_wait_all() {
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+}
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
-// One pooled 16-byte channel chunk: max over the PK x PK window (stride 2) of conv-tile rows.
-// Conv staging: per 32-channel group a 128-row x 128 B tile (16 KB, 128B-swizzled), conv tile
-// width 14 + PK; pooled staging: per group a (pt_h*8)-row x 128 B tile (4 KB apart).
-template <int PK>
-__device__ __forceinline__ void pool_unit(uint32_t conv_base, uint32_t pool_base, int u, int n_pp) {
-  constexpr int CTW = 14 + PK;
-  const int k2 = u & 7;
-  const int pu = u >> 3;
-  const int jg = pu / n_pp, pp = pu - jg * n_pp;
-  const int py = pp >> 3, px = pp & 7;
-  const uint32_t tc = conv_base + (uint32_t)(jg * 16384);
-  float4 m = make_float4(-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F);
+// No-swizzle K-major descriptor: core matrices of 8 rows x 16 bytes, K-adjacent ones 128 B apart
+// (LBO), 8-row groups `sbo` bytes apart (SBO).
+__device__ __forceinline__ uint64_t make_desc(uint32_t addr, uint32_t sbo) {
+  return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)(128 >> 4) << 16) |
+         ((uint64_t)(sbo >> 4) << 32);
+}
+
+__device__ __forceinline__ float rn_tf32(float x) {
+  // round-to-nearest (ties away) onto the 10-bit TF32 mantissa; the low 13 bits end up zero so
+  // the value is exact whatever the tensor core does with the low bits of its fp32 inputs
+  return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
+}
+
+// D[64 x N] (+)= A[64 x 8] (registers) * B[8 x N] (shared-memory descriptor), tf32 -> fp32
+template <int N>
+struct Mma;
+template <>
+struct Mma<16> {
+  static __device__ __forceinline__ void run(float (&d)[8], const uint32_t (&a)[4], uint64_t b,
+                                             int acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+  }
+};
+template <>
+struct Mma<32> {
+  static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b,
+                                             int acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "{%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
+          "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+  }
+};
+template <>
+struct Mma<64> {
+  static __device__ __forceinline__ void run(float (&d)[32], const uint32_t (&a)[4], uint64_t b,
+                                             int acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
+          "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
+          "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),
+          "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+  }
+};
+
+template <int NT, int KC>
+__host__ __device__ constexpr int stage_floats() {
+  return TILE_M * (KC + 4) + 2 * NT * KC;
+}
+
+// One K chunk of KC channels for this thread's A-fragment rows g (a0) and g + 8 (a1), each
+// pointing at the chunk's first column in shared memory; B = hi tile at shared address `bhi`,
+// lo tile right after it.  Every 8-wide K step runs its three split MMAs from a zeroed
+// accumulator and is added into the fp32 running sums.
+template <int NT, int KC>
+__device__ __forceinline__ void mma_chunk(const float* a0, const float* a1, uint32_t bhi, int t,
+                                          float (&acc)[NT / 2], float (&sum)[NT / 2]) {
+  constexpr int KSTEPS = KC / 8;
+  constexpr uint32_t SBO = (KC / 4) * 128;
+  uint32_t ahi[KSTEPS][4], alo[KSTEPS][4];
 #pragma unroll
-  for (int a = 0; a < PK; ++a)
+  for (int ks = 0; ks < KSTEPS; ++ks) {
+    const float v[4] = {a0[ks * 8 + t], a1[ks * 8 + t], a0[ks * 8 + t + 4], a1[ks * 8 + t + 4]};
 #pragma unroll
-    for (int b = 0; b < PK; ++b) {
-      const int rr = (2 * py + a) * CTW + 2 * px + b;
-      const float4 q4 = lds128(tc + (uint32_t)(rr * 128 + ((k2 ^ (rr & 7)) << 4)));
-      m.x = fmaxf(m.x, q4.x); m.y = fmaxf(m.y, q4.y);
-      m.z = fmaxf(m.z, q4.z); m.w = fmaxf(m.w, q4.w);
+    for (int i = 0; i < 4; ++i) {
+      const float hi = rn_tf32(v[i]);
+      ahi[ks][i] = __float_as_uint(hi);
+      alo[ks][i] = __float_as_uint(rn_tf32(v[i] - hi));   // rounded, not truncated by the MMA
     }
-  sts128(pool_base + (uint32_t)(jg * 4096 + pp * 128 + ((k2 ^ (pp & 7)) << 4)), m);
+  }
+  const uint32_t blo = bhi + NT * KC * 4;
+#pragma unroll
+  for (int ks = 0; ks < KSTEPS; ++ks) {
+    const uint64_t dhi = make_desc(bhi + ks * 256, SBO), dlo = make_desc(blo + ks * 256, SBO);
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) fence_operand(acc[i]);
+    wgmma_fence();
+    Mma<NT>::run(acc, alo[ks], dhi, 0);
+    Mma<NT>::run(acc, ahi[ks], dlo, 1);
+    Mma<NT>::run(acc, ahi[ks], dhi, 1);
+    wgmma_commit();
+    wgmma_wait_all();
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) {
+      fence_operand(acc[i]);
+      sum[i] += acc[i];
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
-template <int KC, bool TWO, bool GATHER>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+template <int NT, int KC, bool GATHER>
+__global__ void __launch_bounds__(NUM_THREADS)
 conv_tc_kernel(const __grid_constant__ TcParams p) {
-  extern __shared__ uint8_t smem_dyn[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) &
-                                             ~uintptr_t(1023));
-  constexpr int A_BYTES = TILE_M * KC * 4;
-  // B tile bytes held by THIS CTA: all N rows, or N/2 in CTA-pair mode
-  const int B_BYTES = (TWO ? p.N / 2 : p.N) * KC * 4;
-  const int STAGE_BYTES = A_BYTES + 2 * B_BYTES;   // [A raw][B hi][B lo]
-  const int S = p.stages;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)S * STAGE_BYTES);
-  uint64_t* full = bars;                    // [S]  TMA -> splitter
-  uint64_t* split = bars + MAX_STAGES;      // [S]  splitter -> MMA
-  uint64_t* empty = bars + 2 * MAX_STAGES;  // [S]  MMA -> TMA
-  // tfull is per (drain group, TMEM buffer): an mbarrier waiter must observe every phase in
-  // order, so each group gets barriers only it waits on; tempty's only waiter is the MMA warp.
-  uint64_t* tfull = bars + 3 * MAX_STAGES;  // [2 groups][2]  MMA -> drain (segment accumulated)
-  uint64_t* tempty = tfull + 4;             // [2]  drain -> MMA (buffer read out)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  // per-item epilogue parameters (bias, scale, shift), double-buffered by item parity
-  float* s_par = reinterpret_cast<float*>(tempty + 4);   // [2 groups][2][3][MAX_N]
-  // two 16 KB output staging tiles (128 pixels x 32 channels, 128B-swizzled) for TMA stores
-  uint8_t* s_out = reinterpret_cast<uint8_t*>(
-      (reinterpret_cast<uintptr_t>(s_par + 4 * 3 * MAX_N) + 1023) & ~uintptr_t(1023));
-
-  // 32-bit shared-window addresses of the regions above (see lds128 / sts128)
-  const uint32_t smem_b = smem_u32(smem);
-  const uint32_t par_b = smem_b + (uint32_t)(reinterpret_cast<uint8_t*>(s_par) - smem);
-  const uint32_t out_b = smem_b + (uint32_t)(s_out - smem);
-
+  constexpr int APITCH = KC + 4;
+  constexpr int NACC = NT / 2;
+  extern __shared__ __align__(128) float smem[];
   pdl_trigger();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // Work decomposition: a cluster of C CTAs walks "super-items" = C consecutive tiles of one
-  // chunk in lockstep, so that every weight tile is fetched from L2 once per cluster and
-  // multicast into all C shared memories.  Tiles past the end are clamped (recomputed, not stored).
-  const int C = p.cluster;
-  const uint32_t crank = C > 1 ? cluster_ctarank() : 0u;
-  const int cid = (int)blockIdx.x / C, n_clusters = (int)gridDim.x / C;
-  const int spc = (p.ntiles + C - 1) / C;              // super-items per chunk
-  const int total_items = spc * p.nchunks;             // super-items
-  const uint16_t cmask = (uint16_t)((1u << C) - 1u);
-  const int G = p.seg_stages;
-  // this cluster's items: entries [k_begin, k_end) of the static schedule, or round-robin
-  const int k_begin = p.sched ? __ldg(p.sched + cid) : 0;
-  const int k_end = p.sched ? __ldg(p.sched + cid + 1)
-                            : (total_items - cid + n_clusters - 1) / n_clusters;
-#define SQ_FOR_ITEMS(...)                                                                \
-  for (int k_ = k_begin, nxt_ = (p.sched && k_begin < k_end) ? __ldg(p.sched + k_begin) : 0, \
-           item = p.sched ? nxt_ : cid;                                                  \
-       k_ < k_end;                                                                       \
-       ++k_, item = p.sched ? nxt_ : cid + k_ * n_clusters __VA_ARGS__)                  \
-    if (p.sched && k_ + 1 < k_end ? (nxt_ = __ldg(p.sched + k_ + 1), true) : true)
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&split[s], TWO ? 256 : 128);  // pair mode: both CTAs' splitters arrive at the leader
-      mbar_init(&empty[s], TWO ? 1u : (uint32_t)C);   // commit arrivals (pair mode: one multicast)
-    }
-    for (int b = 0; b < 4; ++b) mbar_init(&tfull[b], 1);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tempty[b], TWO ? 256 : 128);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  const TcChunk& ch = p.chunks[blockIdx.y];
+  const int tid = threadIdx.x;
+  const long long m0 = (long long)blockIdx.x * TILE_M;
+
+  // ---- loader role: pixel `lp`, half `lh` of the KC channels of each K chunk
+  const int lp = tid >> 1, lh = tid & 1;
+  const long long lm = m0 + lp;
+  const bool lvalid = lm < p.M;
+  int ln = 0, liy0 = 0, lix0 = 0;
+  if (lvalid) {
+    const int hw = p.Ho * p.Wo;
+    ln = (int)(lm / hw);
+    const int r = (int)(lm - (long long)ln * hw);
+    liy0 = (r / p.Wo) * p.stride - ch.pad_t;
+    lix0 = (r % p.Wo) * p.stride - ch.pad_l;
   }
-  if (warp == 1) {
-    if (TWO) tmem_alloc_2(tmem_slot, (uint32_t)p.tmem_cols);
-    else tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (C > 1) cluster_sync_all();           // peers' barriers exist before anyone multicasts
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // prologue done (overlapped the previous kernel's tail under PDL): from here on global memory
+  const float* xn = p.x + (size_t)ln * p.H * p.W * p.Cin;
+  const int cpt = GATHER ? 1 : p.Cin / KC;   // K chunks per tap
+  const float* wch = p.w + ch.w_off;
+
+  auto load_stage = [&](int kk, int s) {
+    float* st = smem + (size_t)s * stage_floats<NT, KC>();
+    float* sa = st + 2 * NT * KC;
+    const uint32_t arow = smem_u32(sa + lp * APITCH);
+    if (!GATHER) {
+      const int tap = kk / cpt, c0 = (kk - tap * cpt) * KC + lh * (KC / 2);
+      const int iy = liy0 + tap / ch.ksize, ix = lix0 + tap % ch.ksize;
+      const bool ok = lvalid && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
+      const float* src = ok ? xn + ((size_t)iy * p.W + ix) * p.Cin + c0 : p.x;
+#pragma unroll
+      for (int v = 0; v < KC / 8; ++v)
+        cp_async16(arow + (lh * (KC / 2) + 4 * v) * 4, ok ? src + 4 * v : p.x, ok);
+    } else {
+      const int taps = ch.ksize * ch.ksize;
+#pragma unroll
+      for (int j = 0; j < KC / 2; ++j) {
+        const int k = kk * KC + lh * (KC / 2) + j;
+        const int tap = k / p.Cin, c = k - tap * p.Cin;
+        const int iy = liy0 + tap / ch.ksize, ix = lix0 + tap % ch.ksize;
+        const bool ok = lvalid && tap < taps && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
+        cp_async4(arow + (lh * (KC / 2) + j) * 4, ok ? xn + ((size_t)iy * p.W + ix) * p.Cin + c : p.x,
+                  ok);
+      }
+    }
+    // weights: 2 * NT * KC contiguous floats
+    const float* wsrc = wch + (size_t)kk * 2 * NT * KC;
+    const uint32_t wdst = smem_u32(st);
+    for (int v = tid; v < NT * KC / 2; v += NUM_THREADS) cp_async16(wdst + v * 16, wsrc + 4 * v, true);
+  };
+
   pdl_wait();
-
-  // Register re-balancing between the warpgroups (launch bound: 168/thread) happens at the top
-  // of every role branch, so that ptxas sees one register budget per branch.
-  // Items are ordered chunk-major (all tiles of chunk 0, then chunk 1, ...) so that the static
-  // round-robin gives every CTA the same mix of cheap (1x1) and expensive (3x3) items.
-  if (warp < 4) {
-   asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");   // one instruction for the whole warpgroup
-   if (warp == 0) {
-    // ================================ TMA producer =====================================
-    if (lane == 0) {
-      int it = 0, st_i = 0;
-      uint32_t st_ph = 0;
-      long long w_empty = 0;
-      const long long t_begin = clock64();
-      SQ_FOR_ITEMS() {
-        const TcChunk ck = p.chunk[item / spc];
-        int tile = (item % spc) * C + (int)crank;
-        if (tile >= p.ntiles) tile = p.ntiles - 1;
-        const int tw = tile % p.tiles_w;
-        tile /= p.tiles_w;
-        const int h0 = (tile % p.tiles_h) * p.step_h - p.org_h, w0 = tw * p.step_w - p.org_w;
-        const int img = tile / p.tiles_h;
-        const int iters = ck.tap_count * ck.kc_count;
-        const uint32_t a_bytes = (uint32_t)(p.ct_h * p.ct_w * KC * 4);   // the TMA box
-        for (int i = 0; i < iters; ++i, ++it) {
-          const int s = st_i;
-          const uint32_t ph = st_ph;
-          if (++st_i == S) { st_i = 0; st_ph ^= 1u; }
-          SQ_TIMED_WAIT(w_empty, &empty[s], ph ^ 1u);
-          uint8_t* st = smem + (size_t)s * STAGE_BYTES;
-#ifdef SQDET_ABLATE
-          mbar_expect_tx(&full[s], ((p.ablate & 4) ? 0u : a_bytes) +
-                                       ((p.ablate & 2) ? 0u : (uint32_t)(2 * B_BYTES)));
-#else
-          mbar_expect_tx(&full[s], (GATHER ? (uint32_t)(p.g_ph * p.g_box * 4) : a_bytes) +
-                                       (uint32_t)(2 * B_BYTES));
-#endif
-          const int tl = i / ck.kc_count, kc = ck.kc_begin + (i - tl * ck.kc_count);
-          const int tap = ck.tap_begin + tl;
-          const int dy = tap / ck.ksize, dx = tap - dy * ck.ksize;
-#ifdef SQDET_ABLATE
-          if (!(p.ablate & 4))
-#endif
-          if (GATHER) {
-            // patch rows at a 512-byte pitch in the stage's A region.  TMA needs a 16-byte aligned global start: every row is fetched from its start
-            // rounded down to 4 floats (the splitter adds the 0..3 float offset back); rows
-            // above / below the image fetch a neighbour's data or zero fill, which the splitter
-            // masks (padding) or which only feed conv pixels the epilogue masks
-            const int e0 = ((img * p.g_H + h0 * p.g_stride - p.g_pad_t) * p.g_W +
-                            (w0 * p.g_stride - p.g_pad_l)) * 3;
-            for (int r = 0; r < p.g_ph; ++r)
-              tma_load_1d(st + r * (GATHER_PITCH * 4), &p.tmX, &full[s],
-                          (e0 + r * p.g_W * 3) & ~3);
-          } else {
-            tma_load_4d(st, &p.tmA, &full[s], kc * KC, w0 + dx - ck.pad, h0 + dy - ck.pad, img);
-          }
-          const int row = ck.w_row_base + i * p.N;
-#ifdef SQDET_ABLATE
-          if (p.ablate & 2) continue;
-#endif
-          if (TWO) {
-            // this CTA's half (rows crank*N/2 ...) of the hi and of the lo tile
-            const int r0 = (int)crank * (p.N / 2);
-            tma_load_2d(st + A_BYTES, &p.tmWs, &full[s], 0, row + r0);
-            tma_load_2d(st + A_BYTES + B_BYTES, &p.tmWs, &full[s], 0, row + r0 + p.lo_row_offset);
-          } else if (C == 1) {
-            tma_load_2d(st + A_BYTES, &p.tmW, &full[s], 0, row);
-            tma_load_2d(st + A_BYTES + B_BYTES, &p.tmW, &full[s], 0, row + p.lo_row_offset);
-          } else {
-            // this CTA fetches slice `crank` of the stacked [hi (N rows); lo (N rows)] tile and
-            // multicasts it to the whole cluster
-            const int srows = 2 * p.N / C;
-            const int r0 = (int)crank * srows;
-            const int which = r0 / p.N, rr = r0 - which * p.N;
-            tma_load_2d_mc(st + A_BYTES + which * B_BYTES + rr * KC * 4, &p.tmWs, &full[s], 0,
-                           row + rr + which * p.lo_row_offset, cmask);
-          }
-        }
-      }
-      if (p.dbg) {
-        p.dbg[blockIdx.x * 12 + 0] = w_empty;
-        p.dbg[blockIdx.x * 12 + 5] = clock64() - t_begin;
-        p.dbg[blockIdx.x * 12 + 6] = it;
-      }
-    }
-   } else if (warp == 1) {
-    // ================================ MMA issuer =========================================
-    // The whole warp walks the loop (warp-uniform addresses/descriptors live in uniform
-    // registers); only lane 0 issues tcgen05.mma / tcgen05.commit.  In CTA-pair mode only the
-    // leader CTA (cluster rank 0) issues, for both CTAs.
-    if (!TWO || crank == 0) {
-      const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.N >> 3) << 17) |
-                             ((uint32_t)((TWO ? 2 * TILE_M : TILE_M) >> 4) << 24);
-      const uint32_t smem_base = __shfl_sync(0xffffffffu, smem_u32(smem), 0);
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);   // provably warp-uniform
-      const uint64_t desc_hi = make_desc<KC>(0) & 0xFFFFFFFF00000000ull;   // layout/SBO/version
-      const uint32_t desc_lo0 = (uint32_t)(make_desc<KC>(0) & 0xFFFFFFFFull);  // LBO field
-      int it = 0, g = 0, st_i = 0, n_item = 0;
-      uint32_t st_ph = 0;
-      long long w_split = 0, w_tempty = 0;
-      SQ_FOR_ITEMS(, ++n_item) {
-        const TcChunk ck = p.chunk[item / spc];
-        const int iters = ck.tap_count * ck.kc_count;
-        const int owner = p.two_split ? 0 : (n_item & 1);   // drain group of this item
-        for (int i0 = 0; i0 < iters; i0 += G, ++g) {
-          const int buf = g & 1;
-          SQ_TIMED_WAIT(w_tempty, &tempty[buf], (((uint32_t)g >> 1) & 1u) ^ 1u);   // buffer drained
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_u + (uint32_t)(buf * p.N);
-          const int i1 = (i0 + G < iters) ? (i0 + G) : iters;
-          for (int i = i0; i < i1; ++i, ++it) {
-            const int s = st_i;
-            const uint32_t ph = st_ph;
-            if (++st_i == S) { st_i = 0; st_ph ^= 1u; }
-            SQ_TIMED_WAIT(w_split, &split[s], ph);
-            tc_fence_after();
-            // B descriptor low words (start address >> 4 | LBO), +2 per 32-byte K step;
-            // A operand: TMEM slot s = 2*KC columns [hi | lo], 8 columns per K step
-            const uint32_t b_hi =
-                desc_lo0 | ((smem_base + (uint32_t)(s * STAGE_BYTES) + (uint32_t)A_BYTES) >> 4);
-            const uint32_t b_lo = b_hi + (uint32_t)(B_BYTES >> 4);
-            const uint32_t a_hi = tmem_u + (uint32_t)(2 * p.N + s * 2 * KC);
-            const uint32_t a_lo = a_hi + KC;
-            if (elect_one()) {
+  const int nk = ch.nk;
 #pragma unroll
-              for (int j = 0; j < KC / 8; ++j) {
-                const uint64_t dbh = desc_hi | (uint64_t)(b_hi + 2 * j);
-                const uint64_t dbl = desc_hi | (uint64_t)(b_lo + 2 * j);
-                if (TWO) {
-                  umma_tf32_ts_2(d_tmem, a_lo + 8 * j, dbh, idesc, (i != i0 || j != 0) ? 1u : 0u);
-                  umma_tf32_ts_2(d_tmem, a_hi + 8 * j, dbl, idesc, 1u);
-                  umma_tf32_ts_2(d_tmem, a_hi + 8 * j, dbh, idesc, 1u);
-                } else {
-                  umma_tf32_ts(d_tmem, a_lo + 8 * j, dbh, idesc, (i != i0 || j != 0) ? 1u : 0u);
-#ifdef SQDET_ABLATE
-                  if (p.ablate & 32) continue;
-#endif
-                  umma_tf32_ts(d_tmem, a_hi + 8 * j, dbl, idesc, 1u);
-                  umma_tf32_ts(d_tmem, a_hi + 8 * j, dbh, idesc, 1u);
-                }
-              }
-              if (TWO) umma_commit_2(&empty[s]);    // frees the stage in both CTAs of the pair
-              else if (C == 1) umma_commit(&empty[s]);   // frees the smem stage once the MMAs read it
-              else umma_commit_mc(&empty[s], cmask);   // ... in every CTA of the cluster
-            }
-            __syncwarp();
-          }
-          if (elect_one()) {                       // segment complete -> its drain group
-            if (TWO) umma_commit_2(&tfull[owner * 2 + buf]);
-            else umma_commit(&tfull[owner * 2 + buf]);
-          }
-          __syncwarp();
-        }
-      }
-      if (p.dbg && lane == 0) {
-        p.dbg[blockIdx.x * 12 + 1] = w_split;
-        p.dbg[blockIdx.x * 12 + 2] = w_tempty;
-      }
-    }
-   }   // warps 2-3 of warpgroup 0 are spare: straight to the teardown barrier
-  } else if (warp < 8 || (p.two_split && warp >= 12)) {
-    // ================================ operand splitter ====================================
-    // (two_split: warpgroups 1 and 3 take alternate stages; BOTH wait on every full[s] in order - an
-    // mbarrier waiter that skips phases can mistake phase n-2 for phase n)
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
-    const int sgroup = warp >= 12 ? 1 : 0;
-    const int t = threadIdx.x & 127;   // 0..127
-    int it = 0, st_i = 0;
-    uint32_t st_ph = 0;
-    long long w_full = 0;
-    SQ_FOR_ITEMS() {
-      const TcChunk ck = p.chunk[item / spc];
-      const int iters = ck.tap_count * ck.kc_count;
-      for (int i = 0; i < iters; ++i, ++it) {
-        const int s = st_i;
-        const uint32_t ph = st_ph;
-        if (++st_i == S) { st_i = 0; st_ph ^= 1u; }
-        SQ_TIMED_WAIT(w_full, &full[s], ph);
-        if (p.two_split && (it & 1) != sgroup) continue;
-        // row t of the raw tile (KC*4 bytes, swizzled 16-byte chunks) -> registers ->
-        // a_hi / a_lo -> TMEM slot s, lane t (this warp owns lanes 32*(warp%4)..+31)
-        if (KC == 32 && GATHER) {
-          // gather mode: row t of A = the 27 taps (dy, dx, c) of conv pixel t, read from the
-          // patch rows; taps outside the image (SAME padding), taps 27..31 and rows past the
-          // tile are zero
-          const uint32_t patch = smem_b + (uint32_t)(s * STAGE_BYTES);
-          int tile = (item % spc) * C + (int)crank;
-          if (tile >= p.ntiles) tile = p.ntiles - 1;
-          const int tw = tile % p.tiles_w;
-          tile /= p.tiles_w;
-          const int h0 = (tile % p.tiles_h) * p.step_h - p.org_h, w0 = tw * p.step_w - p.org_w;
-          const int img = tile / p.tiles_h;
-          const int r_h = t / p.ct_w, r_w = t - r_h * p.ct_w;
-          const bool live = r_h < p.ct_h;
-          const int iy0 = (h0 + r_h) * p.g_stride - p.g_pad_t;      // input row of tap dy = 0
-          const int ix0 = (w0 + r_w) * p.g_stride - p.g_pad_l;      // input column of tap dx = 0
-          // global element index of (row iy0, tile's first patch column): its low 2 bits are the
-          // offset the producer's 16-byte alignment shifted this patch row by
-          const int g0 = ((img * p.g_H + iy0) * p.g_W + (w0 * p.g_stride - p.g_pad_l)) * 3;
-          uint32_t prow[3];
-          bool rok[3], cok[3];
-#pragma unroll
-          for (int d = 0; d < 3; ++d) {
-            const int g = g0 + d * p.g_W * 3;
-            prow[d] = patch + 4u * (uint32_t)(live ? (r_h * p.g_stride + d) * GATHER_PITCH + (g & 3) +
-                                                        r_w * p.g_stride * 3
-                                                  : 0);
-            rok[d] = live && (iy0 + d) >= 0 && (iy0 + d) < p.g_H;
-            cok[d] = (ix0 + d) >= 0 && (ix0 + d) < p.g_W;
-          }
-          const uint32_t a_slot = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) +
-                                  (uint32_t)(2 * p.N + s * 2 * KC);
-#pragma unroll
-          for (int hblk = 0; hblk < 2; ++hblk) {
-            uint32_t hi[16], lo[16];
-#pragma unroll
-            for (int e = 0; e < 16; ++e) {
-              const int k = hblk * 16 + e;
-              float v = 0.f;
-              if (k < 27) {
-                v = lds32(prow[k / 9] + 4u * (uint32_t)(k % 9));
-                if (!(rok[k / 9] && cok[(k % 9) / 3])) v = 0.f;
-              }
-              const float h = rn_tf32(v);
-              hi[e] = __float_as_uint(h);
-              lo[e] = __float_as_uint(v - h);
-            }
-            tmem_st16(a_slot + (uint32_t)(hblk * 16), hi);
-            tmem_st16(a_slot + (uint32_t)(KC + hblk * 16), lo);
-          }
-          tmem_wait_st();
-          tc_fence_before();
-          if (TWO) mbar_arrive_remote(&split[s], 0u);
-          else mbar_arrive(&split[s]);
-          continue;
-        }
-        const uint32_t arow = smem_b + (uint32_t)(s * STAGE_BYTES + t * (KC * 4));
-        const int sw = (KC == 32) ? (t & 7) : ((t >> 1) & 3);
-        const uint32_t a_slot = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) +
-                                (uint32_t)(2 * p.N + s * 2 * KC);
-#ifdef SQDET_ABLATE
-        if (!(p.ablate & 1))
-#endif
-#pragma unroll
-        for (int hblk = 0; hblk < KC / 16; ++hblk) {       // 16 columns at a time
-          uint32_t hi[16], lo[16];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int chunk = hblk * 4 + k;
-            const float4 v = lds128(arow + (uint32_t)((chunk ^ sw) << 4));
-            const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              // a = h + l exactly (h: 11-bit RN of a, l = a - h fits fp32); the tensor core
-              // reads the top 19 bits of l, i.e. |l| * 2^-10 <= 2^-21 |a| is dropped
-              const float h = rn_tf32(vv[e]);
-              hi[k * 4 + e] = __float_as_uint(h);
-              lo[k * 4 + e] = __float_as_uint(vv[e] - h);
-            }
-          }
-          tmem_st16(a_slot + (uint32_t)(hblk * 16), hi);
-          tmem_st16(a_slot + (uint32_t)(KC + hblk * 16), lo);
-        }
-        tmem_wait_st();
-        tc_fence_before();             // order the TMEM writes before the barrier hand-off
-        if (TWO) mbar_arrive_remote(&split[s], 0u);   // the leader CTA's barrier
-        else mbar_arrive(&split[s]);
-      }
-    }
-    if (p.dbg && t == 0 && sgroup == 0) p.dbg[blockIdx.x * 12 + 3] = w_full;
-  } else {
-    // ============================ segment drain + epilogue ================================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 192;");
-    // two drain groups (warps 8-11 and 12-15) take alternate items
-    const int dgroup = (warp >= 12) ? 1 : 0;     // (two_split: warpgroup 3 never gets here)
-    const int ngroups = p.two_split ? 1 : 2;
-    const int q = warp & 3;                      // TMEM lane quarter this warp may access
-    const int r = q * 32 + lane;                 // accumulator row = pixel within the tile
-    const int tt = threadIdx.x - 256 - 128 * dgroup;   // 0..127 within the drain group
-    float acc[MAX_N];
-    int g = 0;
-    long long w_tfull = 0, c_epi = 0, c_stw = 0, c_pool = 0, c_par = 0;
-    int n_item = 0, n_own = 0, n_store = 0;
-    uint32_t use0 = 0u, use1 = 0u;               // own segments seen per TMEM buffer
-    SQ_FOR_ITEMS(, ++n_item) {
-      const TcChunk ck = p.chunk[item / spc];
-      const int iters = ck.tap_count * ck.kc_count;
-      if ((n_item % ngroups) != dgroup) {
-        g += (iters + G - 1) / G;                // segments of an item the other group drains
-        continue;
-      }
-      int tile = (item % spc) * C + (int)crank;
-      const bool tile_valid = tile < p.ntiles;
-      if (!tile_valid) tile = p.ntiles - 1;
-      const int tw = tile % p.tiles_w;
-      tile /= p.tiles_w;
-      const int th_i = tile % p.tiles_h;
-      const int h0 = th_i * p.step_h - p.org_h, w0 = tw * p.step_w - p.org_w;
-      const int img = tile / p.tiles_h;
-      const int ncols = (ck.ch_count + 15) & ~15;
-      // stage this item's bias / scale / shift in smem (one element per drain thread); the
-      // named barrier also orders it against the previous item's epilogue reads.
-      const uint32_t par = par_b + 4u * (uint32_t)((dgroup * 2 + (n_own & 1)) * 3 * MAX_N);
-      const long long tpar0 = p.dbg ? clock64() : 0;
-      {
-        const bool in = tt < ck.ch_count;
-        sts32(par + 4u * (uint32_t)tt, (in && p.bias) ? __ldg(p.bias + ck.bias_base + tt) : 0.f);
-        sts32(par + 4u * (uint32_t)(MAX_N + tt),
-              (in && p.scale) ? __ldg(p.scale + ck.bias_base + tt) : 1.f);
-        sts32(par + 4u * (uint32_t)(2 * MAX_N + tt),
-              (in && p.scale) ? __ldg(p.shift + ck.bias_base + tt) : 0.f);
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + dgroup) : "memory");
-      }
-      if (p.dbg) c_par += clock64() - tpar0;
-      ++n_own;
-      for (int i0 = 0; i0 < iters; i0 += G, ++g) {
-        const int buf = g & 1;
-        SQ_TIMED_WAIT(w_tfull, &tfull[dgroup * 2 + buf], (buf ? use1 : use0) & 1u);
-        if (buf) ++use1; else ++use0;
-        tc_fence_after();
-        const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * p.N);
-        // The tensor core truncates when it adds into its fp32 accumulator: a segment of m chained
-        // MMAs comes out short by ~bias_comp * m relative (measured, tests/debug_accuracy.py);
-        // scale the segment sum back while adding it (one FFMA instead of the FADD).
-        const int seg_st = (iters - i0) < G ? (iters - i0) : G;
-        const float seg_gain = 1.f + p.bias_comp * (float)(3 * (KC / 8) * seg_st);
-#ifdef SQDET_ABLATE
-        if (!(p.ablate & 8))
-#endif
-#pragma unroll
-        for (int c0 = 0; c0 < MAX_N; c0 += 16) {
-          if (c0 < ncols) {                      // warp-uniform
-            uint32_t v0[16];
-            tmem_ld16_nowait(trow + (uint32_t)c0, v0);
-            tmem_wait_ld();
-#pragma unroll
-            for (int e = 0; e < 16; ++e)
-              acc[c0 + e] = fmaf(__uint_as_float(v0[e]), seg_gain, i0 == 0 ? 0.f : acc[c0 + e]);
-          }
-        }
-        tc_fence_before();
-        if (TWO) mbar_arrive_remote(&tempty[buf], 0u);
-        else mbar_arrive(&tempty[buf]);          // buffer may be overwritten by segment g+2
-      }
-      // ---- epilogue: bias [, affine], relu, 128-bit stores of this pixel's channel run ----
-      const long long t_epi = p.dbg ? clock64() : 0;
-      const int r_h = r / p.ct_w, r_w = r - r_h * p.ct_w;
-      const int oh = h0 + r_h, ow = w0 + r_w;
-      const bool pix_ok = (r_h < p.ct_h) && oh >= 0 && ow >= 0 && oh < p.Ho && ow < p.Wo;
-#ifdef SQDET_ABLATE
-      if (p.ablate & 16) continue;
-#endif
-      if (p.tma_store) {
-        // TMEM-drained sums -> (+bias [*scale+shift], relu) -> swizzled smem tiles -> TMA
-        // stores.  The TMA unit writes whole 128-byte lines asynchronously and clips ragged
-        // tiles / the channel tail; the drain warps never wait on global memory.
-        const bool affine = p.scale != nullptr;
-        const float lo_clip = p.relu ? 0.f : -CUDART_INF_F;
-        if (!p.pool) {
-          // ---- plain: each warp owns tile rows 2q, 2q+1 (its 32 TMEM lanes) and stores them
-          // itself: no CTA-level barrier, only __syncwarp.  Ring of two 4 KB tiles per warp.
-#pragma unroll
-          for (int jg = 0; jg < MAX_N / 32; ++jg) {
-            if (jg * 32 < ck.ch_count) {                  // warp-uniform
-              if (lane == 0) {
-                const long long t0 = p.dbg ? clock64() : 0;
-                if (p.store_ring == 2) tma_store_wait_read_le1();   // tile used 2 stores ago is free
-                else tma_store_wait_read_all();
-                if (p.dbg) c_stw += clock64() - t0;
-              }
-              __syncwarp();
-              const uint32_t tile_w = out_b + (uint32_t)((dgroup * 4 + q) * (4096 * p.store_ring) +
-                                                         (p.store_ring == 2 ? (n_store & 1) * 4096 : 0));
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                const int c = jg * 32 + k * 4;
-                const float4 b0 = lds128(par + 4u * (uint32_t)c);
-                float o[4] = {acc[c] + b0.x, acc[c + 1] + b0.y, acc[c + 2] + b0.z,
-                              acc[c + 3] + b0.w};
-                if (affine) {
-                  const float4 s0 = lds128(par + 4u * (uint32_t)(MAX_N + c));
-                  const float4 h0v = lds128(par + 4u * (uint32_t)(2 * MAX_N + c));
-                  o[0] = o[0] * s0.x + h0v.x; o[1] = o[1] * s0.y + h0v.y;
-                  o[2] = o[2] * s0.z + h0v.z; o[3] = o[3] * s0.w + h0v.w;
-                }
-                float4 v;
-                v.x = fmaxf(o[0], lo_clip); v.y = fmaxf(o[1], lo_clip);
-                v.z = fmaxf(o[2], lo_clip); v.w = fmaxf(o[3], lo_clip);
-                sts128(tile_w + (uint32_t)(lane * 128 + ((k ^ (lane & 7)) << 4)), v);
-              }
-              fence_async_proxy();
-              __syncwarp();
-              if (lane == 0 && tile_valid)
-                tma_store_4d(tile_w, &p.tmY, ck.y_coff + jg * 32, w0 + q * p.sq_w, h0 + q * p.sq_h, img);
-              ++n_store;
-            }
-          }
-        } else {
-          // ---- fused tf.nn.max_pool (window p.pool, stride 2): stage the whole conv tile
-          // (all channel groups), pool across pixels from smem, store the pooled tile.
-          const bool issuer = tt == 0;
-          if (issuer) {
-            const long long t0 = p.dbg ? clock64() : 0;
-            tma_store_wait_read_all();                    // previous item's pooled tiles are free
-            if (p.dbg) c_stw += clock64() - t0;
-          }
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + dgroup) : "memory");
-          const float ninf = -CUDART_INF_F;
-#pragma unroll
-          for (int jg = 0; jg < MAX_N / 32; ++jg) {
-            if (jg * 32 < ck.ch_count) {
-              const uint32_t tile_c = out_b + (uint32_t)(dgroup * POOL_STAGE_BYTES + jg * 16384);
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                const int c = jg * 32 + k * 4;
-                const float4 b0 = lds128(par + 4u * (uint32_t)c);
-                float o[4] = {acc[c] + b0.x, acc[c + 1] + b0.y, acc[c + 2] + b0.z,
-                              acc[c + 3] + b0.w};
-                if (affine) {
-                  const float4 s0 = lds128(par + 4u * (uint32_t)(MAX_N + c));
-                  const float4 h0v = lds128(par + 4u * (uint32_t)(2 * MAX_N + c));
-                  o[0] = o[0] * s0.x + h0v.x; o[1] = o[1] * s0.y + h0v.y;
-                  o[2] = o[2] * s0.z + h0v.z; o[3] = o[3] * s0.w + h0v.w;
-                }
-                float4 v;
-                // tf.nn.max_pool ignores cells outside the image: they become -inf
-                v.x = pix_ok ? fmaxf(o[0], lo_clip) : ninf;
-                v.y = pix_ok ? fmaxf(o[1], lo_clip) : ninf;
-                v.z = pix_ok ? fmaxf(o[2], lo_clip) : ninf;
-                v.w = pix_ok ? fmaxf(o[3], lo_clip) : ninf;
-                sts128(tile_c + (uint32_t)(r * 128 + ((k ^ (r & 7)) << 4)), v);
-              }
-            }
-          }
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + dgroup) : "memory");
-          const long long tp0 = p.dbg ? clock64() : 0;
-          // unit = (channel group jg, pooled pixel pp, 16-byte chunk k2); pt_w == 8
-          const int n_pp = p.pt_h * 8;
-          const int n_units = ((ck.ch_count + 31) >> 5) * n_pp * 8;
-          const uint32_t conv_base = out_b + (uint32_t)(dgroup * POOL_STAGE_BYTES);
-          const uint32_t pool_base = conv_base + (uint32_t)(POOL_MAX_GROUPS * 16384);
-          if (p.pool == 3) {
-            for (int u = tt; u < n_units; u += 128)
-              pool_unit<3>(conv_base, pool_base, u, n_pp);
-          } else {
-            for (int u = tt; u < n_units; u += 128)
-              pool_unit<2>(conv_base, pool_base, u, n_pp);
-          }
-          if (p.dbg) c_pool += clock64() - tp0;
-          fence_async_proxy();
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + dgroup) : "memory");
-          if (issuer && tile_valid) {
-            for (int jg = 0; jg * 32 < ck.ch_count; ++jg)
-              tma_store_4d(pool_base + jg * 4096, &p.tmY, ck.y_coff + jg * 32, tw * 8,
-                           th_i * p.pt_h, img);
-          }
-        }
-      } else if (pix_ok && tile_valid) {
-        float* yrow =
-            p.y + (((size_t)img * p.Ho + oh) * p.Wo + ow) * (size_t)p.y_cstride + ck.y_coff;
-        // 256-bit stores: each thread writes whole 32-byte sectors of its pixel's channel run.
-        // Branch-free per element: parameters come from smem (padded with bias 0 / scale 1).
-        const bool wide = ((p.y_cstride | ck.y_coff | ck.ch_count) & 7) == 0;
-        const bool affine = p.scale != nullptr;
-        const float lo_clip = p.relu ? 0.f : -CUDART_INF_F;
-#pragma unroll
-        for (int c = 0; c < MAX_N; c += 8) {
-          if (c < ck.ch_count) {
-            float o[8];
-            const float4 b0 = lds128(par + 4u * (uint32_t)c);
-            const float4 b1 = lds128(par + 4u * (uint32_t)(c + 4));
-            const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-            for (int e = 0; e < 8; ++e) o[e] = acc[c + e] + bb[e];
-            if (affine) {
-              const float4 s0 = lds128(par + 4u * (uint32_t)(MAX_N + c));
-              const float4 s1 = lds128(par + 4u * (uint32_t)(MAX_N + c + 4));
-              const float4 h0v = lds128(par + 4u * (uint32_t)(2 * MAX_N + c));
-              const float4 h1v = lds128(par + 4u * (uint32_t)(2 * MAX_N + c + 4));
-              const float ss[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-              const float hh[8] = {h0v.x, h0v.y, h0v.z, h0v.w, h1v.x, h1v.y, h1v.z, h1v.w};
-#pragma unroll
-              for (int e = 0; e < 8; ++e) o[e] = o[e] * ss[e] + hh[e];
-            }
-#pragma unroll
-            for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], lo_clip);
-            if (wide) {
-              asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(yrow + c),
-                           "f"(o[0]), "f"(o[1]), "f"(o[2]), "f"(o[3]), "f"(o[4]), "f"(o[5]),
-                           "f"(o[6]), "f"(o[7])
-                           : "memory");
-            } else {
-#pragma unroll
-              for (int e = 0; e < 8; ++e)
-                if (c + e < ck.ch_count) yrow[c + e] = o[e];
-            }
-          }
-        }
-      }
-      if (p.dbg) c_epi += clock64() - t_epi;
-    }
-    if (p.tma_store && lane == 0) tma_store_wait_all();
-    if (p.dbg && threadIdx.x == 256) {   // group 0 only
-      p.dbg[blockIdx.x * 12 + 4] = w_tfull;
-      p.dbg[blockIdx.x * 12 + 7] = c_epi;
-      p.dbg[blockIdx.x * 12 + 8] = c_stw;
-      p.dbg[blockIdx.x * 12 + 9] = c_pool;
-      p.dbg[blockIdx.x * 12 + 10] = c_par;
-    }
+  for (int s = 0; s < STAGES - 1; ++s) {
+    if (s < nk) load_stage(s, s);
+    cp_async_commit();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (C > 1) cluster_sync_all();           // no CTA leaves while peers may still multicast to it
-  if (warp == 1) {
-    tc_fence_after();
-    if (TWO) tmem_dealloc_2(tmem_base, (uint32_t)p.tmem_cols);
-    else tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+
+  // ---- MMA role: warpgroup `wg` owns rows [64 wg, 64 wg + 64); A-fragment row g / g + 8 of
+  // warp `wq`'s 16-row slice, columns t / t + 4 of each 8-wide K step
+  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const int arow0 = wg * 64 + wq * 16 + g;
+  float acc[NACC], sum[NACC];
+#pragma unroll
+  for (int i = 0; i < NACC; ++i) acc[i] = 0.f, sum[i] = 0.f;
+
+  for (int kk = 0; kk < nk; ++kk) {
+    cp_async_wait<STAGES - 2>();
+    fence_proxy_async();
+    __syncthreads();
+    if (kk + STAGES - 1 < nk) load_stage(kk + STAGES - 1, (kk + STAGES - 1) % STAGES);
+    cp_async_commit();
+
+    const float* st = smem + (size_t)(kk % STAGES) * stage_floats<NT, KC>();
+    const float* sa = st + 2 * NT * KC;
+    mma_chunk<NT, KC>(sa + arow0 * APITCH, sa + (arow0 + 8) * APITCH, smem_u32(st), t, acc, sum);
+  }
+  cp_async_wait<0>();
+
+  // ---- epilogue: accumulator element 4j + 2h + e is (row g + 8h, column 8j + 2t + e)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const long long m = m0 + arow0 + 8 * h;
+    if (m >= p.M) continue;
+    float* yrow = p.y + (size_t)m * p.y_cstride + ch.y_off;
+#pragma unroll
+    for (int j = 0; j < NT / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int c = 8 * j + 2 * t + e;
+        if (c >= ch.ncount) continue;
+        float v = sum[4 * j + 2 * h + e];
+        if (p.bias) v += p.bias[ch.p_off + c];
+        if (p.scale) v = v * p.scale[ch.p_off + c] + p.shift[ch.p_off + c];
+        if (p.relu) v = fmaxf(v, 0.f);
+        yrow[c] = v;
+      }
   }
 }
 
-// Split-K reduction: y[p][c] = act( (bias[c] + sum_s part[p][s*pitch + c]) [*scale + shift] ).
-// Deterministic (fixed summation order), 128-bit loads/stores; the partials are L2-resident.
-__global__ void __launch_bounds__(256)
-splitk_reduce_kernel(const float* __restrict__ part, float* __restrict__ y,
-                     const float* __restrict__ bias, const float* __restrict__ scale,
-                     const float* __restrict__ shift, long long npix, int cout, int pitch,
-                     int ksplit, int y_cstride, int y_coff, int relu) {
+// ---------------------------------------------------------------------------------------------
+// The fire module as ONE kernel: a CTA owns an 8 x 16 tile of output pixels of one image.
+//   squeeze: 1x1 conv over the 10 x 18 halo of the tile (192 rows = three m64 blocks; warpgroup 0
+//            takes blocks 0 and 2, warpgroup 1 block 1), bias + ReLU, zero outside the image (SAME
+//            padding of the 3x3 expand pads the post-ReLU squeeze output), kept in shared memory
+//            as Q[halo pixel][SQN + 4] fp32;
+//   expand:  1x1 and 3x3 convs over Q in chunks of 64 output channels; the A fragments of tap
+//            (dy, dx) are read from Q at the tap-shifted halo row, so the squeeze tensor never
+//            leaves the SM; weights stream through the cp.async ring.
+constexpr int FT_W = 16, FQ_W = FT_W + 2, FQ_P = 10 * FQ_W, FQ_ROWS = 192;
+constexpr int MAX_FCHUNKS = 16;
+
+struct FireChunk {
+  int taps, nk, ncount, y_off;
+};
+
+struct FireParams {
+  const float* x;
+  float* y;
+  const float* wsq;   // squeeze tiles [Cin / KCI][2][SQN][KCI]
+  const float* bsq;   // [SQN], zero past S
+  const float* wex;   // expand tiles, chunk after chunk, [nk][2][64][KCE] each
+  const float* bex;   // [E1 + E3]
+  int B, H, W, Cin, S, Etot, tiles_w, tiles_h, nchunks;
+  FireChunk chunks[MAX_FCHUNKS];
+};
+
+template <int KCI, int SQN, int KCE>
+__host__ __device__ constexpr int fire_ring_floats() {
+  return FQ_ROWS * (KCI + 4) + 2 * SQN * KCI > 2 * 64 * KCE ? FQ_ROWS * (KCI + 4) + 2 * SQN * KCI
+                                                             : 2 * 64 * KCE;
+}
+
+template <int KCI, int SQN, int KCE>
+__global__ void __launch_bounds__(NUM_THREADS)
+fire_tc_kernel(const __grid_constant__ FireParams p) {
+  constexpr int API = KCI + 4, QP = SQN + 4;
+  constexpr int RING = fire_ring_floats<KCI, SQN, KCE>();
+  extern __shared__ __align__(128) float smem[];
+  float* q = smem + STAGES * RING;
   pdl_trigger();
+
+  int tile = blockIdx.x;
+  const int tx = tile % p.tiles_w;
+  tile /= p.tiles_w;
+  const int ty = tile % p.tiles_h, n = tile / p.tiles_h;
+  const int oy0 = ty * 8, ox0 = tx * FT_W;
+  const int tid = threadIdx.x;
+  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const float* xn = p.x + (size_t)n * p.H * p.W * p.Cin;
+
+  auto load_sq = [&](int kk, int s) {
+    float* st = smem + (size_t)s * RING;
+    float* sa = st + 2 * SQN * KCI;
+    for (int v = tid; v < FQ_ROWS * KCI / 4; v += NUM_THREADS) {
+      const int row = v / (KCI / 4), j = v % (KCI / 4);
+      const int iy = oy0 - 1 + row / FQ_W, ix = ox0 - 1 + row % FQ_W;
+      const bool ok = row < FQ_P && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
+      cp_async16(smem_u32(sa + row * API + 4 * j),
+                 ok ? xn + ((size_t)iy * p.W + ix) * p.Cin + kk * KCI + 4 * j : p.x, ok);
+    }
+    const float* wsrc = p.wsq + (size_t)kk * 2 * SQN * KCI;
+    for (int v = tid; v < SQN * KCI / 2; v += NUM_THREADS) cp_async16(smem_u32(st) + v * 16, wsrc + 4 * v, true);
+  };
+
   pdl_wait();
-  const int c4n = cout / 4;
-  const long long total = npix * c4n;
-  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(idx % c4n) * 4;
-    const long long px = idx / c4n;
-    float4 a = bias ? *reinterpret_cast<const float4*>(bias + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const float* src = part + px * (long long)(ksplit * pitch) + c;
-    for (int s2 = 0; s2 < ksplit; ++s2) {
-      const float4 v = *reinterpret_cast<const float4*>(src + s2 * pitch);
-      a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
-    }
-    if (scale) {
-      const float4 sc = *reinterpret_cast<const float4*>(scale + c);
-      const float4 sh = *reinterpret_cast<const float4*>(shift + c);
-      a.x = a.x * sc.x + sh.x; a.y = a.y * sc.y + sh.y;
-      a.z = a.z * sc.z + sh.z; a.w = a.w * sc.w + sh.w;
-    }
-    if (relu) {
-      a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); a.z = fmaxf(a.z, 0.f); a.w = fmaxf(a.w, 0.f);
-    }
-    *reinterpret_cast<float4*>(y + px * y_cstride + y_coff + c) = a;
+  // ---- squeeze
+  const int nks = p.Cin / KCI;
+#pragma unroll
+  for (int s = 0; s < STAGES - 1; ++s) {
+    if (s < nks) load_sq(s, s);
+    cp_async_commit();
   }
+  float accq[SQN / 2], sq[2][SQN / 2];
+#pragma unroll
+  for (int i = 0; i < SQN / 2; ++i) accq[i] = 0.f, sq[0][i] = 0.f, sq[1][i] = 0.f;
+  for (int kk = 0; kk < nks; ++kk) {
+    cp_async_wait<STAGES - 2>();
+    fence_proxy_async();
+    __syncthreads();
+    if (kk + STAGES - 1 < nks) load_sq(kk + STAGES - 1, (kk + STAGES - 1) % STAGES);
+    cp_async_commit();
+    const float* st = smem + (size_t)(kk % STAGES) * RING;
+    const float* sa = st + 2 * SQN * KCI;
+#pragma unroll
+    for (int bi = 0; bi < 2; ++bi) {
+      const int b = wg + 2 * bi;   // warpgroup-uniform
+      if (b < 3) {
+        const int r0 = b * 64 + wq * 16 + g;
+        mma_chunk<SQN, KCI>(sa + r0 * API, sa + (r0 + 8) * API, smem_u32(st), t, accq, sq[bi]);
+      }
+    }
+  }
+  cp_async_wait<0>();
+#pragma unroll
+  for (int bi = 0; bi < 2; ++bi) {
+    const int b = wg + 2 * bi;
+    if (b >= 3) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = b * 64 + wq * 16 + g + 8 * h;
+      const int iy = oy0 - 1 + row / FQ_W, ix = ox0 - 1 + row % FQ_W;
+      const bool ok = row < FQ_P && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
+#pragma unroll
+      for (int j = 0; j < SQN / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * j + 2 * t + e;
+          q[row * QP + c] = ok ? fmaxf(sq[bi][4 * j + 2 * h + e] + p.bsq[c], 0.f) : 0.f;
+        }
+    }
+  }
+  __syncthreads();   // Q complete; every squeeze MMA has retired, so the ring is free
+
+  // ---- expand: pixel rows g / g + 8 of this warp are tile row (4 wg + wq), columns g / g + 8
+  const int spt = p.S / KCE;   // K chunks per tap
+  int total = 0;
+  for (int c = 0; c < p.nchunks; ++c) total += p.chunks[c].nk;
+  auto load_ex = [&](int it, int s) {
+    const float* wsrc = p.wex + (size_t)it * 2 * 64 * KCE;
+    const uint32_t dst = smem_u32(smem + (size_t)s * RING);
+    for (int v = tid; v < 64 * KCE / 2; v += NUM_THREADS) cp_async16(dst + v * 16, wsrc + 4 * v, true);
+  };
+#pragma unroll
+  for (int s = 0; s < STAGES - 1; ++s) {
+    if (s < total) load_ex(s, s);
+    cp_async_commit();
+  }
+  const int r = wg * 4 + wq;
+  float acc[32], sum[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f, sum[i] = 0.f;
+  int c = 0, kk = 0;
+  for (int it = 0; it < total; ++it) {
+    cp_async_wait<STAGES - 2>();
+    fence_proxy_async();
+    __syncthreads();
+    if (it + STAGES - 1 < total) load_ex(it + STAGES - 1, (it + STAGES - 1) % STAGES);
+    cp_async_commit();
+    const FireChunk& ch = p.chunks[c];
+    const int tap = kk / spt, k0 = (kk - tap * spt) * KCE;
+    const int dy = ch.taps == 1 ? 1 : tap / 3, dx = ch.taps == 1 ? 1 : tap % 3;
+    const int qr = (r + dy) * FQ_W + g + dx;
+    mma_chunk<64, KCE>(q + qr * QP + k0, q + (qr + 8) * QP + k0,
+                       smem_u32(smem + (size_t)(it % STAGES) * RING), t, acc, sum);
+    if (++kk == ch.nk) {
+      const int oy = oy0 + r;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int ox = ox0 + g + 8 * h;
+        if (oy >= p.H || ox >= p.W) continue;
+        float* yrow = p.y + (((size_t)n * p.H + oy) * p.W + ox) * p.Etot + ch.y_off;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * j + 2 * t + e;
+            if (col < ch.ncount) yrow[col] = fmaxf(sum[4 * j + 2 * h + e] + p.bex[ch.y_off + col], 0.f);
+          }
+      }
+#pragma unroll
+      for (int i = 0; i < 32; ++i) sum[i] = 0.f;
+      kk = 0;
+      ++c;
+    }
+  }
+  cp_async_wait<0>();
 }
 
 // ---------------------------------------------------------------------------------------------
 // Host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn) return fn;
-  void* p = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) !=
-          cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess)
-    return nullptr;
-  fn = reinterpret_cast<EncodeTiledFn>(p);
-  return fn;
-}
-
-struct ConvGroup {        // one conv reading the shared input; >= 1 chunks
-  int ksize, Cout, y_coff, bias_base;
-  int tap_begin = 0, tap_count = -1;   // tap sub-range (split-K); -1 = all ksize*ksize taps
-  int kc_begin = 0, kc_count = -1;     // input-channel chunk sub-range (split-K); -1 = all Cin / KC
+struct ConvGroup {   // one conv reading the shared input
+  int ksize, Cout, y_off;
 };
 
 struct TcImpl {
-  TcParams prm;
-  int KC = 32;
-  int Cin = 0;
-  size_t smem_bytes = 0;
+  TcParams prm{};
+  int NT = 0, KC = 0;
+  bool gather = false;
   dim3 grid;
-  float* d_w = nullptr;        // packed weights: hi rows then lo rows, [rows][KC]
-  float* d_bias = nullptr;     // concatenated per-group bias (or null)
+  size_t smem_bytes = 0;
+  std::vector<ConvGroup> groups;
+  std::vector<int> group_chunk0;   // first chunk of each group
+  int cout_total = 0;
+  float* d_w = nullptr;
+  float* d_bias = nullptr;
   float* d_scale = nullptr;
   float* d_shift = nullptr;
-  int rows_half = 0;
-  int bias_total = 0;
-  std::vector<ConvGroup> groups;
-  std::vector<TcChunk> chunks;
-  // split-K: the kernel writes `ksplit` partial sums into d_scratch [pixels][ksplit*pitch];
-  // splitk_reduce_kernel adds them (+bias [,affine], relu) into the real output
-  int ksplit = 1, pitch = 0, relu_final = 0, cout = 0, y_cstride_final = 0, y_coff_final = 0;
-  long long npix = 0;
-  float* d_scratch = nullptr;
-  float* y_final = nullptr;
-  int* d_sched = nullptr;      // static LPT schedule (see TcParams::sched)
-  // gather mode: the input address is baked into the 1-D tensor map; the engine feeds the first
-  // layer from several buffers (pipelined inputs), so maps are cached per address
-  long long x_floats = 0;
-  mutable std::vector<std::pair<const float*, CUtensorMap>> xmaps;
+  long long w_floats = 0;
 };
 
 static inline float host_rn_tf32(float x) {
@@ -872,560 +521,25 @@ static inline float host_rn_tf32(float x) {
   return r;
 }
 
-static int encode_act_map(CUtensorMap* map, const float* x, int B, int H, int W, int C, int KC,
-                          int box_w = TILE_W, int box_h = TILE_H) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(SQDET_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4};
-  cuuint32_t box[4] = {(cuuint32_t)KC, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x), dims, strides,
-                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   KC == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char buf[96];
-    snprintf(buf, sizeof buf, "cuTensorMapEncodeTiled(activation) failed: CUresult %d", (int)r);
-    return fail(SQDET_ERR_CUDA, buf);
+// Output-channel tile: the narrowest of 16 / 32 / 64 that covers the launch's chunks with the
+// least padded MMA work plus A-tile re-reads (each chunk reloads the pixels' K values).
+static int pick_nt(const std::vector<ConvGroup>& groups) {
+  int best = 0;
+  long long best_cost = 0;
+  for (int nt : {64, 32, 16}) {
+    long long chunks = 0;
+    for (const auto& g : groups) chunks += (g.Cout + nt - 1) / nt;
+    if (chunks > MAX_CHUNKS) continue;
+    const long long cost = chunks * (nt + 32);
+    if (!best || cost < best_cost) best = nt, best_cost = cost;
   }
-  return SQDET_OK;
+  return best;
 }
 
-static int encode_w_map(CUtensorMap* map, const float* w, int rows, int KC, int N) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(SQDET_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[2] = {(cuuint64_t)KC, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)KC * 4};
-  cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)N};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(w), dims, strides,
-                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   KC == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char buf[96];
-    snprintf(buf, sizeof buf, "cuTensorMapEncodeTiled(weights) failed: CUresult %d", (int)r);
-    return fail(SQDET_ERR_CUDA, buf);
-  }
-  return SQDET_OK;
-}
-
-// Common planner: `groups` convs (same ksize rules as the fire pair) over one input.
-// First-layer (gather) mode: the conv really is `ks x ks` over a 3-channel image with this
-// stride / padding; plan_common is then called on the conv OUTPUT grid with a fake 1x1 group.
-struct GatherSpec {
-  int B_in, H_in, W_in, stride, pad_t, pad_l;
-};
-
-static int encode_flat_map(CUtensorMap* map, const float* x, long long n, int box) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(SQDET_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[1] = {(cuuint64_t)n};
-  cuuint64_t strides[1] = {0};
-  cuuint32_t bx[1] = {(cuuint32_t)box};
-  cuuint32_t estr[1] = {1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 1, const_cast<float*>(x), dims, strides, bx,
-                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    char buf[96];
-    snprintf(buf, sizeof buf, "cuTensorMapEncodeTiled(flat input) failed: CUresult %d", (int)r);
-    return fail(SQDET_ERR_CUDA, buf);
-  }
-  return SQDET_OK;
-}
-
-static int plan_common(TcImpl* im, int B, int H, int W, int Cin, const std::vector<ConvGroup>& groups,
-                       int relu, bool has_affine, int y_cstride, const float* x_dev, float* y_dev,
-                       const TcPool* pool, const GatherSpec* gs = nullptr) {
-  // A launch made only of 1x1 convs has no spatial structure: walk the B*H*W pixels as one flat
-  // row in tiles of 128 consecutive pixels (no ragged image-edge tiles; e.g. 22x76x20 is 262
-  // tiles instead of 300, which is two waves of 148 CTAs instead of three).
-  bool flat = !(pool && pool->size > 0) && !gs;
-  for (auto& g : groups) flat = flat && g.ksize == 1;
-  {
-    static int env_flat = -1;
-    if (env_flat < 0) {
-      const char* a = getenv("SQDET_TC_FLAT");
-      env_flat = a ? atoi(a) : 1;
-    }
-    if (!env_flat) flat = false;
-  }
-  if (flat) {
-    W = B * H * W;
-    H = 1;
-    B = 1;
-  }
-  im->Cin = Cin;
-  im->KC = (Cin % 32 == 0) ? 32 : 16;
-  const int KC = im->KC;
-  im->groups = groups;
-  // uniform N over all chunks
-  int maxc = 0;
-  for (auto& g : groups) maxc = g.Cout > maxc ? g.Cout : maxc;
-  int N = 0;
-  {
-    const int nmax = (pool && pool->size > 0) ? POOL_MAX_N : MAX_N;
-    const int nsplit = (maxc + nmax - 1) / nmax;
-    N = ((maxc + nsplit - 1) / nsplit + 15) / 16 * 16;
-  }
-  TcParams& P = im->prm;
-  memset(&P, 0, sizeof P);
-  im->chunks.clear();
-  int row = 0;
-  const int kch = Cin / KC;
-  for (auto& g : groups) {
-    for (int cb = 0; cb < g.Cout; cb += N) {
-      TcChunk c;
-      c.ksize = g.ksize;
-      c.pad = (g.ksize - 1) / 2;
-      c.w_row_base = row;
-      c.ch_base = cb;
-      c.ch_count = (g.Cout - cb) < N ? (g.Cout - cb) : N;
-      c.y_coff = g.y_coff + cb;
-      c.bias_base = g.bias_base + cb;
-      c.tap_begin = g.tap_begin;
-      c.tap_count = g.tap_count < 0 ? g.ksize * g.ksize : g.tap_count;
-      c.kc_begin = g.kc_begin;
-      c.kc_count = g.kc_count < 0 ? kch : g.kc_count;
-      row += c.tap_count * c.kc_count * N;
-      im->chunks.push_back(c);
-    }
-  }
-  if ((int)im->chunks.size() > MAX_CHUNKS) return 0;   // not taken by this path
-  im->rows_half = row;
-  im->bias_total = 0;
-  for (auto& g : groups) im->bias_total = (g.bias_base + g.Cout) > im->bias_total ? (g.bias_base + g.Cout) : im->bias_total;
-  P.B = B; P.Ho = H; P.Wo = W;                      // stride-1 SAME: output grid == input grid
-  P.ct_h = TILE_H; P.ct_w = TILE_W; P.step_h = TILE_H; P.step_w = TILE_W;
-  P.org_h = P.org_w = 0;
-  P.tiles_h = (H + TILE_H - 1) / TILE_H;
-  P.tiles_w = (W + TILE_W - 1) / TILE_W;
-  P.sq_w = 0; P.sq_h = 2;                           // drain warp q stores tile rows 2q, 2q+1
-  if (flat) {
-    P.ct_h = 1; P.ct_w = TILE_M; P.step_h = 1; P.step_w = TILE_M;
-    P.tiles_h = 1; P.tiles_w = (W + TILE_M - 1) / TILE_M;
-    P.sq_w = 32; P.sq_h = 0;
-  }
-  const bool pooled = pool && pool->size > 0;
-  // TMA-store epilogue: needs every chunk to be a whole number of 32-channel groups unless it
-  // ends at the tensor's last channel (where the TMA unit clips the tail).
-  bool store_ok = (y_cstride % 4 == 0);
-  {
-    static int env_tma = -1;
-    if (env_tma < 0) {
-      const char* a = getenv("SQDET_TC_TMA_STORE");
-      env_tma = a ? atoi(a) : 1;
-    }
-    if (!env_tma) store_ok = false;
-    for (auto& c : im->chunks)
-      if ((c.ch_count % 32) != 0 && (c.y_coff + c.ch_count != y_cstride)) store_ok = false;
-    for (auto& c : im->chunks)
-      if (c.y_coff % 4 != 0) store_ok = false;
-  }
-  if (!store_ok && !pooled && !flat && !gs) {
-    // Direct-store epilogue: any ct_h x ct_w <= 128 tile works, so pick the shape with the fewest
-    // rounds of the persistent grid (ConvDet head on 22x76x20: 8x16 tiles = 900 split-K items =
-    // 7 rounds on 148 SMs; 11x11 tiles = 840 items = 6 rounds), then the fewest tiles.
-    static int env_search = -1;
-    if (env_search < 0) {
-      const char* a = getenv("SQDET_TC_TILESEARCH");
-      env_search = a ? atoi(a) : 1;
-    }
-    int sms = 148, dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const long long nch = (long long)im->chunks.size();
-    auto rounds_of = [&](long long tiles) { return (tiles * nch + sms - 1) / sms; };
-    long long best_tiles = (long long)B * P.tiles_h * P.tiles_w;
-    long long best_rounds = rounds_of(best_tiles);
-    for (int th = 1; env_search && th <= 32; ++th) {
-      int twd = TILE_M / th;
-      if (twd > 128) twd = 128;
-      if (twd < 4) break;
-      const long long tiles = (long long)B * ((H + th - 1) / th) * ((W + twd - 1) / twd);
-      const long long rounds = rounds_of(tiles);
-      if (rounds < best_rounds || (rounds == best_rounds && tiles < best_tiles * 9 / 10)) {
-        best_rounds = rounds; best_tiles = tiles;
-        P.ct_h = th; P.ct_w = twd; P.step_h = th; P.step_w = twd;
-        P.tiles_h = (H + th - 1) / th; P.tiles_w = (W + twd - 1) / twd;
-      }
-    }
-  }
-  if (pooled) {
-    // conv tile = the conv pixels under a pt_h x pt_w block of stride-2 pooling windows
-    if (pool->size != 2 && pool->size != 3) return 0;
-    P.pool = pool->size;
-    P.pt_h = pool->size == 3 ? 3 : 4;
-    P.pt_w = 8;
-    P.ct_h = 2 * (P.pt_h - 1) + pool->size;      // 7 or 8
-    P.ct_w = 2 * (P.pt_w - 1) + pool->size;      // 17 or 16
-    P.step_h = 2 * P.pt_h; P.step_w = 2 * P.pt_w;
-    P.org_h = pool->pad_t; P.org_w = pool->pad_l;
-    P.Hp = pool->Hp; P.Wp = pool->Wp;
-    P.tiles_h = (pool->Hp + P.pt_h - 1) / P.pt_h;
-    P.tiles_w = (pool->Wp + P.pt_w - 1) / P.pt_w;
-  }
-  P.kch = kch;
-  P.N = N;
-
-  // 36 chained MMAs per accumulation segment (3 MMAs per 8-wide K step).  Measured relative
-  // error of one conv: 24 -> 4e-7, 48 -> 7e-7, 96 -> 1.3e-6 (fp32 SIMT accumulation: 1e-6 ..
-  // 2e-6); 48 is 5% faster end to end than 24 but the truncation bias is systematic, and at
-  // 48 the 50-layer ResNet body lands one box coordinate 8e-3 px from the fp32 reference
-  // (the test bar is ~6e-3): 36 keeps the margin.
-  P.seg_stages = (KC == 32) ? 3 : 6;
-  P.ntiles = B * P.tiles_h * P.tiles_w;
-  P.y_cstride = y_cstride;
-  P.relu = relu;
-  P.lo_row_offset = row;
-  P.nchunks = (int)im->chunks.size();
-  for (int i = 0; i < P.nchunks; ++i) P.chunk[i] = im->chunks[i];
-  // CTA-pair mode (cta_group::2): needs N % 32 == 0 (2-SM TF32 MMA shape rule) and two tiles
-  static int env_two = -1;
-  if (env_two < 0) {
-    const char* a = getenv("SQDET_TC_2CTA");
-    env_two = a ? atoi(a) : 0;
-  }
-  const bool two_cta = env_two != 0 && (N % 32 == 0) && P.ntiles >= 2;
-  P.two_cta = two_cta ? 1 : 0;
-  {
-    // second splitter warpgroup instead of the second drain group: launches whose MMA stage
-    // (12 MMAs of N/2 clocks) is shorter than the splitter's ~650 clocks AND whose items are K-heavy
-    // (few epilogues per MMA: one drain group keeps up).  Measured (profiles/r2_two_split.txt): ConvDet
-    // 0.280 vs 0.271 ms, fire6/7 +5 %, VGG16 +18 % - the stage is a latency chain, not splitter throughput.
-    static int env_2s = -1;
-    if (env_2s < 0) {
-      const char* a = getenv("SQDET_TC_2SPLIT");
-      env_2s = a ? atoi(a) : 0;   // opt-in (2 = the rule below): measured slower everywhere it applies
-    }
-    int max_iters = 0;
-    for (auto& c : im->chunks)
-      max_iters = (c.tap_count * c.kc_count) > max_iters ? (c.tap_count * c.kc_count) : max_iters;
-    const bool want = env_2s == 1 || (env_2s == 2 && N <= 96 && max_iters >= 24);
-    P.two_split = (want && !two_cta && !pooled && !gs) ? 1 : 0;
-  }
-  const size_t stage = (size_t)TILE_M * KC * 4 + (size_t)2 * (two_cta ? N / 2 : N) * KC * 4;
-  // Pipeline depth and residency: with two CTAs per SM (<= ~110 KB each) there are two
-  // independent TMA->split->MMA->drain pipelines per SM to hide latency; otherwise one deep one.
-  static int env_ctas = -1, env_stages = -1, env_seg = -1;
-  if (env_ctas < 0) {
-    const char* a = getenv("SQDET_TC_CTAS");   env_ctas = a ? atoi(a) : 0;
-    const char* b = getenv("SQDET_TC_STAGES"); env_stages = b ? atoi(b) : 0;
-    const char* c = getenv("SQDET_TC_SEG");    env_seg = c ? atoi(c) : 0;
-  }
-  int ctas = env_ctas > 0 ? env_ctas : 1;   // 384 threads x 168 regs: one CTA per SM
-  static int env_ring = -1;
-  if (env_ring < 0) {
-    const char* a = getenv("SQDET_TC_STORE_RING");
-    env_ring = a ? atoi(a) : 0;
-  }
-  auto overhead_for = [&](int ring) {
-    return (size_t)(1024 /*alignment*/ + 512 /*barriers*/ + 4 * 3 * MAX_N * 4 /*epilogue params*/ +
-                    1024 + (pooled ? 2 * POOL_STAGE_BYTES : 8 * 4096 * ring) /*store staging*/);
-  };
-  int ring = 2;
-  {
-    const size_t budget = 227 * 1024;
-    const int s2 = (int)((budget - overhead_for(2)) / stage), s1 = (int)((budget - overhead_for(1)) / stage);
-    if (env_ring == 1 || (env_ring == 0 && s2 < 4 && s1 > s2)) ring = 1;
-  }
-  P.store_ring = ring;
-  const size_t overhead = overhead_for(ring);
-  int stages = 0;
-  for (; ctas >= 1; --ctas) {
-    const size_t budget = (ctas == 1 ? 227 * 1024 : (227 * 1024) / ctas - 1024) - overhead;
-    stages = (int)(budget / stage);
-    if (stages >= 3 || ctas == 1) break;
-  }
-  if (ctas < 1) ctas = 1;
-  const int max_stages = env_stages > 0 ? env_stages : MAX_STAGES;
-  if (stages > max_stages) stages = max_stages;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  // TMEM: two accumulator buffers (2N columns) + one [a_hi | a_lo] slot (2*KC columns) per stage
-  while (stages > 2 && 2 * N + stages * 2 * KC > 512) --stages;
-  if (stages < 2 || 2 * N + stages * 2 * KC > 512) return 0;
-  P.stages = stages;
-  {
-    int cols = 32;
-    while (cols < 2 * N + stages * 2 * KC) cols <<= 1;
-    P.tmem_cols = cols;
-  }
-  if (env_seg > 0) P.seg_stages = env_seg;
-  {
-    static float env_comp = -1.f;
-    if (env_comp < 0.f) {
-      const char* a = getenv("SQDET_TC_BIAS_COMP");
-      env_comp = a ? (float)atof(a) : 1.4e-8f;
-    }
-    P.bias_comp = env_comp;
-  }
-  {
-    const char* a = getenv("SQDET_TC_ABLATE");
-    P.ablate = a ? atoi(a) : 0;
-  }
-  im->smem_bytes = stages * stage + overhead;
-  {
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    // Cluster size for the weight multicast: 2 packs all 148 SMs (74 TPC pairs); 4 quarters the
-    // L2->SM weight traffic but strands SMs of GPCs whose SM count is not a multiple of 4.
-    static int env_cluster = -1;
-    if (env_cluster < 0) {
-      const char* a = getenv("SQDET_TC_CLUSTER");
-      env_cluster = a ? atoi(a) : 1;   // measured: multicast (2, 4) is slower, see DESIGN.md
-    }
-    int cluster = (env_cluster == 4 || env_cluster == 2) ? env_cluster : 1;
-    if (P.two_cta) cluster = 2;
-    if (P.ntiles < cluster) cluster = 1;
-    P.cluster = cluster;
-    const long long supers = (long long)((P.ntiles + cluster - 1) / cluster) * P.nchunks;
-    long long nclusters = (long long)(sms * ctas) / cluster;
-    if (supers < nclusters) nclusters = supers;
-    im->grid = dim3((unsigned)(nclusters * cluster));
-    // Static longest-processing-time-first schedule when chunks differ in cost (a fire expand
-    // pair: 1x1 items of kch stages, 3x3 items of 9*kch): round-robin leaves e.g. 12 of 148 CTAs
-    // with 7 expensive items against 6 (207 vs 182 stages on fire10); LPT hands those CTAs
-    // fewer cheap items instead.
-    static int env_lpt = -1;
-    if (env_lpt < 0) {
-      const char* a = getenv("SQDET_TC_LPT");
-      env_lpt = a ? atoi(a) : 1;
-    }
-    bool differ = false;
-    for (auto& c : im->chunks)
-      if (c.tap_count * c.kc_count != im->chunks[0].tap_count * im->chunks[0].kc_count) differ = true;
-    // (only when a CTA gets few items: with dozens per CTA round-robin is already balanced, and
-    // keeping a tile's 1x1 and 3x3 items adjacent in time is better for L2 - measured on fire2/3)
-    if (env_lpt && differ && supers > nclusters && supers < 24 * nclusters) {
-      const int spc_h = (P.ntiles + cluster - 1) / cluster;
-      std::vector<int> order(im->chunks.size());
-      for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
-      auto cost_of = [&](int c) { return 2 * im->chunks[c].tap_count * im->chunks[c].kc_count + 3; };   // + epilogue
-      std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return cost_of(a) > cost_of(b); });
-      typedef std::pair<long long, int> Bin;     // (load, cluster id): least loaded first
-      std::priority_queue<Bin, std::vector<Bin>, std::greater<Bin>> heap;
-      for (int b = 0; b < (int)nclusters; ++b) heap.push(Bin(0, b));
-      std::vector<std::vector<int>> lists((size_t)nclusters);
-      for (int c : order)
-        for (int t = 0; t < spc_h; ++t) {
-          Bin b = heap.top();
-          heap.pop();
-          lists[(size_t)b.second].push_back(c * spc_h + t);
-          b.first += cost_of(c);
-          heap.push(b);
-        }
-      std::vector<int> sched((size_t)nclusters + 1);
-      int pos = (int)nclusters + 1;
-      for (int b = 0; b < (int)nclusters; ++b) {
-        sched[(size_t)b] = pos;
-        pos += (int)lists[(size_t)b].size();
-      }
-      sched[(size_t)nclusters] = pos;
-      for (auto& l : lists) sched.insert(sched.end(), l.begin(), l.end());
-      SQ_CUDA(cudaMalloc(&im->d_sched, sizeof(int) * sched.size()));
-      SQ_CUDA(cudaMemcpy(im->d_sched, sched.data(), sizeof(int) * sched.size(), cudaMemcpyHostToDevice));
-      P.sched = im->d_sched;
-    }
-  }
-  P.y = y_dev;
-  SQ_CUDA(cudaMalloc(&im->d_w, sizeof(float) * (size_t)row * 2 * KC));
-  SQ_CUDA(cudaMemset(im->d_w, 0, sizeof(float) * (size_t)row * 2 * KC));
-  SQ_CUDA(cudaMalloc(&im->d_bias, sizeof(float) * im->bias_total));
-  SQ_CUDA(cudaMemset(im->d_bias, 0, sizeof(float) * im->bias_total));
-  P.bias = im->d_bias;
-  if (has_affine) {
-    SQ_CUDA(cudaMalloc(&im->d_scale, sizeof(float) * im->bias_total));
-    SQ_CUDA(cudaMalloc(&im->d_shift, sizeof(float) * im->bias_total));
-    P.scale = im->d_scale;
-    P.shift = im->d_shift;
-  }
-  int rc = 0;
-  if (gs) {
-    P.gather = 1;
-    P.g_H = gs->H_in; P.g_W = gs->W_in; P.g_stride = gs->stride;
-    P.g_pad_t = gs->pad_t; P.g_pad_l = gs->pad_l;
-    P.g_ph = (P.ct_h - 1) * gs->stride + 3;
-    // patch columns * 3 floats, + up to 3 floats of alignment shift, rounded to 16 bytes
-    P.g_box = (((P.ct_w - 1) * gs->stride + 3) * 3 + 3 + 3) / 4 * 4;
-    if ((long long)gs->B_in * gs->H_in * gs->W_in * 3 + 4096 >= (1LL << 31)) return 0;
-    if (P.g_box > GATHER_PITCH || (size_t)P.g_ph * GATHER_PITCH * 4 > (size_t)TILE_M * KC * 4)
-      return 0;                                       // patch must fit the stage's A region
-    im->x_floats = (long long)gs->B_in * gs->H_in * gs->W_in * 3;
-    rc = encode_flat_map(&P.tmX, x_dev, im->x_floats, P.g_box);
-    if (rc) return rc;
-    im->xmaps.emplace_back(x_dev, P.tmX);
-  } else {
-    rc = encode_act_map(&P.tmA, x_dev, B, H, W, Cin, KC, P.ct_w, P.ct_h);
-    if (rc) return rc;
-  }
-  {
-    const bool ok = store_ok;
-    if (pooled && !ok) return 0;          // the fused pool exists only on the TMA-store path
-    if (ok) {
-      if (pooled)
-        rc = encode_act_map(&P.tmY, y_dev, B, pool->Hp, pool->Wp, y_cstride, 32, P.pt_w, P.pt_h);
-      else
-        rc = flat ? encode_act_map(&P.tmY, y_dev, B, H, W, y_cstride, 32, 32, 1)
-                  : encode_act_map(&P.tmY, y_dev, B, H, W, y_cstride, 32, TILE_W, 2);   // per-warp rows
-      if (rc) return rc;
-    }
-    P.tma_store = ok ? 1 : 0;
-  }
-  rc = encode_w_map(&P.tmW, im->d_w, row * 2, KC, N);
-  if (rc) return rc;
-  if (P.cluster > 1) {
-    rc = encode_w_map(&P.tmWs, im->d_w, row * 2, KC, P.two_cta ? N / 2 : 2 * N / P.cluster);
-    if (rc) return rc;
-  }
-  // opt in to the full 227 KB once per DEVICE for every instantiation (the attribute is per
-  // function and per device context, not per launch, so it must cover the largest plan)
-  static unsigned long long attr_devs = 0ull;
-  int attr_dev = 0;
-  SQ_CUDA(cudaGetDevice(&attr_dev));
-  if (attr_dev >= 64 || !((attr_devs >> attr_dev) & 1ull)) {
-    SQ_CUDA(cudaFuncSetAttribute(conv_tc_kernel<32, false, false>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    SQ_CUDA(cudaFuncSetAttribute(conv_tc_kernel<16, false, false>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    SQ_CUDA(cudaFuncSetAttribute(conv_tc_kernel<32, true, false>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    SQ_CUDA(cudaFuncSetAttribute(conv_tc_kernel<16, true, false>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    SQ_CUDA(cudaFuncSetAttribute(conv_tc_kernel<32, false, true>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
-    if (attr_dev < 64) attr_devs |= 1ull << attr_dev;
-  }
-  return 1;
-}
-
-// Pack group `gi` weights (HWIO [k,k,Cin,Cout]) into the [chunk][tap][kchunk][N][KC] hi/lo rows.
-static void pack_group(const TcImpl* im, int gi, const float* w_hwio, std::vector<float>& packed) {
-  const int KC = im->KC, N = im->prm.N, Cin = im->Cin;
-  const ConvGroup& g = im->groups[gi];
-  const size_t lo_off = (size_t)im->rows_half * KC;
-  // chunks of this group appear in order; find the first
-  int ci = 0;
-  for (int i = 0; i < gi; ++i) ci += (im->groups[i].Cout + N - 1) / N;
-  for (int cb = 0; cb < g.Cout; cb += N, ++ci) {
-    const TcChunk& c = im->chunks[ci];
-    for (int tl = 0; tl < c.tap_count; ++tl)
-      for (int kc = c.kc_begin; kc < c.kc_begin + c.kc_count; ++kc)
-        for (int n = 0; n < c.ch_count; ++n) {
-          const int tap = c.tap_begin + tl;
-          const size_t rowi = (size_t)c.w_row_base + ((size_t)tl * c.kc_count + (kc - c.kc_begin)) * N + n;
-          for (int k = 0; k < KC; ++k) {
-            const float v = (kc * KC + k < Cin)
-                                ? w_hwio[((size_t)tap * Cin + (size_t)kc * KC + k) * g.Cout + cb + n]
-                                : 0.f;   // gather mode: K = 27 padded to 32
-            const float hi = host_rn_tf32(v);
-            packed[rowi * KC + k] = hi;
-            packed[lo_off + rowi * KC + k] = host_rn_tf32(v - hi);
-          }
-        }
-  }
-}
-
-static int launch_impl(const TcImpl* im, const float* x_dev, float* y_dev, cudaStream_t stream) {
-  // the tensor map bakes in the activation address the plan was made for
-  (void)x_dev;
-  (void)y_dev;
-  static int debug = -1;
-  if (debug < 0) {
-    const char* d = getenv("SQDET_TC_DEBUG");
-    debug = d ? atoi(d) : 0;
-  }
-  TcParams prm = im->prm;
-  if (prm.gather && x_dev) {
-    bool found = false;
-    for (auto& m : im->xmaps)
-      if (m.first == x_dev) { prm.tmX = m.second; found = true; break; }
-    if (!found) {
-      CUtensorMap m;
-      int rc = encode_flat_map(&m, x_dev, im->x_floats, prm.g_box);
-      if (rc) return rc;
-      if (im->xmaps.size() >= 8) im->xmaps.erase(im->xmaps.begin());
-      im->xmaps.emplace_back(x_dev, m);
-      prm.tmX = m;
-    }
-  }
-  {
-    static int exp_mode = -1;
-    if (exp_mode < 0) {
-      const char* x = getenv("SQDET_TC_EXP");
-      exp_mode = x ? atoi(x) : 0;
-    }
-    prm.exp_mode = exp_mode;
-  }
-  long long* dbg = nullptr;
-  const int nb = (int)im->grid.x;
-  if (debug) {
-    SQ_CUDA(cudaMalloc(&dbg, sizeof(long long) * 12 * nb));
-    SQ_CUDA(cudaMemsetAsync(dbg, 0, sizeof(long long) * 12 * nb, stream));
-    prm.dbg = dbg;
-  }
-  if (prm.cluster <= 1) {
-    // classic launch (no cluster attribute: keeps the non-cluster CTA->SM placement path)
-    if (prm.gather)
-      SQ_CUDA(launch_kernel(conv_tc_kernel<32, false, true>, im->grid, dim3(NUM_THREADS), im->smem_bytes,
-                            stream, prm));
-    else if (im->KC == 32)
-      SQ_CUDA(launch_kernel(conv_tc_kernel<32, false, false>, im->grid, dim3(NUM_THREADS), im->smem_bytes,
-                            stream, prm));
-    else
-      SQ_CUDA(launch_kernel(conv_tc_kernel<16, false, false>, im->grid, dim3(NUM_THREADS), im->smem_bytes,
-                            stream, prm));
-  } else {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = im->grid;
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = im->smem_bytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)prm.cluster;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaError_t le;
-    if (prm.two_cta)
-      le = (im->KC == 32) ? cudaLaunchKernelEx(&cfg, conv_tc_kernel<32, true, false>, prm)
-                          : cudaLaunchKernelEx(&cfg, conv_tc_kernel<16, true, false>, prm);
-    else
-      le = (im->KC == 32) ? cudaLaunchKernelEx(&cfg, conv_tc_kernel<32, false, false>, prm)
-                          : cudaLaunchKernelEx(&cfg, conv_tc_kernel<16, false, false>, prm);
-    if (le != cudaSuccess) return cuda_fail(le, "cudaLaunchKernelEx(conv_tc_kernel)");
-  }
-  SQ_CHECK_LAUNCH("conv_tc_kernel");
-  if (im->ksplit > 1) {
-    const long long total = im->npix * (im->cout / 4);
-    long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
-    SQ_CUDA(launch_kernel(splitk_reduce_kernel, dim3((unsigned)blocks), dim3(256), 0, stream,
-                          (const float*)im->d_scratch, im->y_final, (const float*)im->d_bias,
-                          (const float*)im->d_scale, (const float*)im->d_shift, im->npix, im->cout,
-                          im->pitch, im->ksplit, im->y_cstride_final, im->y_coff_final, im->relu_final));
-    SQ_CHECK_LAUNCH("splitk_reduce_kernel");
-  }
-  if (debug) {
-    std::vector<long long> h((size_t)12 * nb);
-    SQ_CUDA(cudaStreamSynchronize(stream));
-    SQ_CUDA(cudaMemcpy(h.data(), dbg, sizeof(long long) * h.size(), cudaMemcpyDeviceToHost));
-    cudaFree(dbg);
-    double a[12] = {0};
-    for (int b = 0; b < nb; ++b)
-      for (int k = 0; k < 12; ++k) a[k] += (double)h[(size_t)b * 12 + k] / nb;
-    fprintf(stderr,
-            "[tc] grid %d tile %dx%d ntiles %d%s cluster %d%s smem %zu KC %d N %d kch %d chunks %d stages %d seg %d | per-CTA avg cycles: "
-            "total %.0f stages %.0f | waits: producer(empty) %.0f mma(split) %.0f mma(tempty) %.0f "
-            "splitter(full) %.0f drain(tfull) %.0f | epilogue %.0f (store-wait %.0f, pool %.0f, params %.0f)\n",
-            nb, prm.ct_h, prm.ct_w, prm.ntiles, prm.sched ? " LPT" : "", prm.cluster, prm.two_cta ? " (cta_group::2)" : "", im->smem_bytes, im->KC, prm.N, prm.kch, prm.nchunks, prm.stages, prm.seg_stages,
-            a[5], a[6], a[0], a[1], a[2], a[3], a[4], a[7], a[8], a[9], a[10]);
-  }
-  return SQDET_OK;
+template <int NT, int KC, bool GATHER>
+static cudaError_t set_smem(size_t bytes) {
+  return cudaFuncSetAttribute(conv_tc_kernel<NT, KC, GATHER>,
+                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
 }
 
 static void release_impl(void** impl) {
@@ -1435,151 +549,196 @@ static void release_impl(void** impl) {
   cudaFree(im->d_bias);
   cudaFree(im->d_scale);
   cudaFree(im->d_shift);
-  cudaFree(im->d_scratch);
-  cudaFree(im->d_sched);
   delete im;
   *impl = nullptr;
 }
 
+// Plans `groups` convs over one [B, H, W, Cin] input into a [B, Ho, Wo, y_cstride] output.
+// Returns 1 (planned), 0 (declined) or a negative status.
+static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo, int stride,
+                       int pad_t, int pad_l, bool gather, const std::vector<ConvGroup>& groups,
+                       int relu, bool has_affine, int y_cstride) {
+  const int NT = pick_nt(groups);
+  if (!NT) return 0;
+  const int KC = (gather || Cin % 32 == 0) ? 32 : 16;
+  const long long M = (long long)B * Ho * Wo;
+  const long long mtiles = (M + TILE_M - 1) / TILE_M;
+  if (M <= 0 || mtiles > 0x7fffffffLL) return 0;
+  im->NT = NT;
+  im->KC = KC;
+  im->gather = gather;
+  im->groups = groups;
+  TcParams& p = im->prm;
+  p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Ho = Ho; p.Wo = Wo; p.stride = stride;
+  p.relu = relu; p.y_cstride = y_cstride; p.M = M;
+  int nch = 0, poff = 0;
+  long long woff = 0;
+  for (const auto& g : groups) {
+    im->group_chunk0.push_back(nch);
+    const int nk = gather ? (g.ksize * g.ksize * Cin + KC - 1) / KC : g.ksize * g.ksize * (Cin / KC);
+    for (int cb = 0; cb < g.Cout; cb += NT, ++nch) {
+      TcChunk& c = p.chunks[nch];
+      c.ksize = g.ksize;
+      c.pad_t = gather ? pad_t : g.ksize / 2;
+      c.pad_l = gather ? pad_l : g.ksize / 2;
+      c.nk = nk;
+      c.ncount = g.Cout - cb < NT ? g.Cout - cb : NT;
+      c.y_off = g.y_off + cb;
+      c.p_off = poff + cb;
+      c.w_off = woff;
+      woff += (long long)nk * 2 * NT * KC;
+    }
+    poff += g.Cout;
+  }
+  p.nchunks = nch;
+  im->cout_total = poff;
+  im->w_floats = woff;
+  im->grid = dim3((unsigned)mtiles, (unsigned)nch);
+  im->smem_bytes = (size_t)STAGES * (TILE_M * (KC + 4) + 2 * NT * KC) * sizeof(float);
+  cudaError_t ce = cudaSuccess;
+  if (gather) {
+    ce = NT == 64 ? set_smem<64, 32, true>(im->smem_bytes)
+                  : NT == 32 ? set_smem<32, 32, true>(im->smem_bytes) : set_smem<16, 32, true>(im->smem_bytes);
+  } else if (KC == 32) {
+    ce = NT == 64 ? set_smem<64, 32, false>(im->smem_bytes)
+                  : NT == 32 ? set_smem<32, 32, false>(im->smem_bytes) : set_smem<16, 32, false>(im->smem_bytes);
+  } else {
+    ce = NT == 64 ? set_smem<64, 16, false>(im->smem_bytes)
+                  : NT == 32 ? set_smem<32, 16, false>(im->smem_bytes) : set_smem<16, 16, false>(im->smem_bytes);
+  }
+  if (ce != cudaSuccess) return cuda_fail(ce, "cudaFuncSetAttribute(conv_tc_kernel)");
+  SQ_CUDA(cudaMalloc(&im->d_w, sizeof(float) * (size_t)woff));
+  SQ_CUDA(cudaMalloc(&im->d_bias, sizeof(float) * poff));
+  SQ_CUDA(cudaMemset(im->d_bias, 0, sizeof(float) * poff));
+  if (has_affine) {
+    SQ_CUDA(cudaMalloc(&im->d_scale, sizeof(float) * poff));
+    SQ_CUDA(cudaMalloc(&im->d_shift, sizeof(float) * poff));
+  }
+  p.w = im->d_w;
+  p.bias = im->d_bias;
+  p.scale = im->d_scale;
+  p.shift = im->d_shift;
+  return 1;
+}
+
+// Packs K chunks [0, nk) of one output-channel chunk [n0, n0 + NT) of a weight matrix whose rows
+// are the flattened HWIO K index (tap * Cin + channel, `kreal` of them) into the tiles the
+// kernels read: per K chunk [NT/8 row groups][KC/4 K core matrices][8 rows][4 floats], hi tile
+// then lo tile.  Rows past `kreal` and channels past `cout` are zero.
+static void pack_tiles(const float* w, long long kreal, int cout, int n0, int NT, int KC, int nk,
+                       float* dst) {
+  for (int kk = 0; kk < nk; ++kk) {
+    float* hi_t = dst + (size_t)kk * 2 * NT * KC;
+    float* lo_t = hi_t + NT * KC;
+    for (int n = 0; n < NT; ++n)
+      for (int k = 0; k < KC; ++k) {
+        const long long kg = (long long)kk * KC + k;
+        const float v = (n0 + n < cout && kg < kreal) ? w[kg * cout + n0 + n] : 0.f;
+        const float hi = host_rn_tf32(v);
+        const size_t at = ((size_t)(n / 8) * (KC / 4) + k / 4) * 32 + (n % 8) * 4 + k % 4;
+        hi_t[at] = hi;
+        lo_t[at] = host_rn_tf32(v - hi);
+      }
+  }
+}
+
+// Pack group `gi` weights (HWIO [k,k,Cin,Cout]) into each of its chunks' tiles.  With Cin a
+// multiple of KC (or gather mode) K chunk kk holds flattened K rows [kk * KC, kk * KC + KC).
+static void pack_group(const TcImpl* im, int gi, const float* w_hwio, std::vector<float>& packed) {
+  const ConvGroup& g = im->groups[gi];
+  int ci = im->group_chunk0[gi];
+  for (int cb = 0; cb < g.Cout; cb += im->NT, ++ci) {
+    const TcChunk& c = im->prm.chunks[ci];
+    pack_tiles(w_hwio, (long long)g.ksize * g.ksize * im->prm.Cin, g.Cout, cb, im->NT, im->KC, c.nk,
+               packed.data() + c.w_off);
+  }
+}
+
+static int upload_weights(TcImpl* im, const std::vector<const float*>& w_hwio) {
+  std::vector<float> packed((size_t)im->w_floats, 0.f);
+  for (int gi = 0; gi < (int)im->groups.size(); ++gi) pack_group(im, gi, w_hwio[gi], packed);
+  SQ_CUDA(cudaMemcpy(im->d_w, packed.data(), packed.size() * sizeof(float), cudaMemcpyHostToDevice));
+  return SQDET_OK;
+}
+
+static int launch_impl(const TcImpl* im, const float* x_dev, float* y_dev, cudaStream_t stream) {
+  TcParams prm = im->prm;
+  prm.x = x_dev;
+  prm.y = y_dev;
+  const dim3 block(NUM_THREADS);
+  const size_t sm = im->smem_bytes;
+  cudaError_t ce;
+  if (im->gather)
+    ce = im->NT == 64 ? launch_kernel(conv_tc_kernel<64, 32, true>, im->grid, block, sm, stream, prm)
+         : im->NT == 32 ? launch_kernel(conv_tc_kernel<32, 32, true>, im->grid, block, sm, stream, prm)
+                        : launch_kernel(conv_tc_kernel<16, 32, true>, im->grid, block, sm, stream, prm);
+  else if (im->KC == 32)
+    ce = im->NT == 64 ? launch_kernel(conv_tc_kernel<64, 32, false>, im->grid, block, sm, stream, prm)
+         : im->NT == 32 ? launch_kernel(conv_tc_kernel<32, 32, false>, im->grid, block, sm, stream, prm)
+                        : launch_kernel(conv_tc_kernel<16, 32, false>, im->grid, block, sm, stream, prm);
+  else
+    ce = im->NT == 64 ? launch_kernel(conv_tc_kernel<64, 16, false>, im->grid, block, sm, stream, prm)
+         : im->NT == 32 ? launch_kernel(conv_tc_kernel<32, 16, false>, im->grid, block, sm, stream, prm)
+                        : launch_kernel(conv_tc_kernel<16, 16, false>, im->grid, block, sm, stream, prm);
+  if (ce != cudaSuccess) return cuda_fail(ce, "launch conv_tc_kernel");
+  return SQDET_OK;
+}
+
+// ---- one-kernel fire module: host state -----------------------------
+struct FusedImpl {
+  FireParams fp{};
+  int KCI = 0, SQN = 0, KCE = 0;
+  unsigned grid = 0;
+  size_t smem = 0;
+  float* d_w = nullptr;    // squeeze tiles
+  float* d_w2 = nullptr;   // expand tiles
+  float* d_b = nullptr;
+  float* d_b2 = nullptr;
+  long long w_floats = 0, w2_floats = 0;
+};
+
+static void release_fused(void** impl) {
+  if (!*impl) return;
+  FusedImpl* im = static_cast<FusedImpl*>(*impl);
+  cudaFree(im->d_w); cudaFree(im->d_w2); cudaFree(im->d_b); cudaFree(im->d_b2);
+  delete im;
+  *impl = nullptr;
+}
+
+// (KCI, SQN, KCE) of the squeeze width S: S = 16, 32, 48, 64 -> SQN 16, 32, 64, 64 and KCE the
+// largest of 32 / 16 dividing S
+#define SQ_FIRE_DISPATCH(KCI_, SQN_, KCE_, CALL)                                              \
+  do {                                                                                          \
+    if (KCI_ == 32 && SQN_ == 16) CALL(32, 16, 16);                                             \
+    else if (KCI_ == 32 && SQN_ == 32) CALL(32, 32, 32);                                        \
+    else if (KCI_ == 32 && SQN_ == 64 && KCE_ == 16) CALL(32, 64, 16);                          \
+    else if (KCI_ == 32) CALL(32, 64, 32);                                                      \
+    else if (SQN_ == 16) CALL(16, 16, 16);                                                      \
+    else if (SQN_ == 32) CALL(16, 32, 32);                                                      \
+    else if (KCE_ == 16) CALL(16, 64, 16);                                                      \
+    else CALL(16, 64, 32);                                                                      \
+  } while (0)
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
-int tc_encode_act_map(CUtensorMap* map, const float* x, int B, int H, int W, int C, int KC,
-                      int box_w, int box_h) {
-  return encode_act_map(map, x, B, H, W, C, KC, box_w, box_h);
-}
-int tc_encode_w_map(CUtensorMap* map, const float* w, int rows, int KC, int N) {
-  return encode_w_map(map, w, rows, KC, N);
-}
-int tc_encode_flat_map(CUtensorMap* map, const float* x, long long n, int box) {
-  return encode_flat_map(map, x, n, box);
-}
-
-bool tc_conv_eligible(int Cin, int Cout, int size, int stride, int padding, int y_cstride,
-                      int y_coff) {
-  // shapes this path takes: stride-1 SAME, 1x1 or 3x3, Cin a multiple of 16, 16B-aligned stores
+bool tc_conv_eligible(int Cin, int Cout, int size, int stride, int padding) {
+  // shapes this path takes: stride-1 SAME, 1x1 or 3x3, Cin a multiple of 16
   if (stride != 1 || padding != SQDET_PAD_SAME || (size != 1 && size != 3)) return false;
-  if (Cin % 16 != 0 || Cin < 16 || (y_cstride % 4) || (y_coff % 4) || (Cout % 4)) return false;
-  return true;
-}
-
-bool tc_pool_fusable(const int* couts, const int* coffs, int ngroups, int y_cstride, int pool_size,
-                     int pool_stride) {
-  // mirrors plan_common: uniform chunk width N; every chunk must be whole 32-channel groups
-  // unless it ends the output tensor (TMA clips the tail there)
-  if ((pool_size != 2 && pool_size != 3) || pool_stride != 2 || (y_cstride % 4)) return false;
-  int maxc = 0;
-  for (int g = 0; g < ngroups; ++g) maxc = couts[g] > maxc ? couts[g] : maxc;
-  const int nsplit = (maxc + POOL_MAX_N - 1) / POOL_MAX_N;
-  const int N = ((maxc + nsplit - 1) / nsplit + 15) / 16 * 16;
-  int nchunks = 0;
-  for (int g = 0; g < ngroups; ++g)
-    for (int cb = 0; cb < couts[g]; cb += N, ++nchunks) {
-      const int cnt = (couts[g] - cb) < N ? (couts[g] - cb) : N;
-      if ((cnt % 32) != 0 && (coffs[g] + cb + cnt != y_cstride)) return false;
-      if ((coffs[g] + cb) % 4) return false;
-    }
-  return nchunks <= MAX_CHUNKS;
+  return Cin % 16 == 0 && Cin >= 16 && Cout > 0;
 }
 
 int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, int Cout, int size, int stride,
-                 int padding, int relu, bool has_affine, int y_cstride, int y_coff,
-                 const float* x_dev, float* y_dev, const TcPool* pool) {
+                 int padding, int relu, bool has_affine, int y_cstride, int y_coff) {
   plan->enabled = false;
-  // First layer: 3x3 conv over a 3-channel image (stride 1 or 2, SAME or VALID) -> gather mode
-  if (Cin == 3 && size == 3 && (stride == 1 || stride == 2) && (Cout % 4) == 0 &&
-      (y_cstride % 4) == 0 && (y_coff % 4) == 0) {
-    static int env_gather = -1;
-    if (env_gather < 0) {
-      const char* a = getenv("SQDET_TC_GATHER");
-      env_gather = a ? atoi(a) : 1;
-    }
-    if (!env_gather) return 0;
-    const Geom gh = tf_geometry(H, size, stride, padding);
-    const Geom gw = tf_geometry(W, size, stride, padding);
-    if (gh.out <= 0 || gw.out <= 0) return 0;
-    TcImpl* im = new TcImpl();
-    GatherSpec gs{B, H, W, stride, gh.pad_before, gw.pad_before};
-    std::vector<ConvGroup> groups = {{1, Cout, y_coff, 0}};   // one K block of 32 (27 real taps)
-    int rc = plan_common(im, B, gh.out, gw.out, 32, groups, relu, has_affine, y_cstride, x_dev,
-                         y_dev, pool, &gs);
-    if (rc <= 0) {
-      void* p = im;
-      release_impl(&p);
-      return rc;
-    }
-    im->Cin = 27;          // weight packing: HWIO flattened is already [k = (dy, dx, c)][Cout]
-    plan->enabled = true;
-    plan->B = B; plan->H = H; plan->W = W; plan->Cin = Cin; plan->Cout = Cout;
-    plan->size = size; plan->stride = stride; plan->relu = relu;
-    plan->Ho = gh.out; plan->Wo = gw.out; plan->pad_t = gh.pad_before; plan->pad_l = gw.pad_before;
-    plan->y_cstride = y_cstride; plan->y_coff = y_coff;
-    plan->launches = 1;
-    plan->impl = im;
-    return 1;
-  }
-  if (!tc_conv_eligible(Cin, Cout, size, stride, padding, y_cstride, y_coff)) return 0;
+  const bool gather = Cin == 3 && size == 3 && (stride == 1 || stride == 2) && Cout > 0;
+  if (!gather && !tc_conv_eligible(Cin, Cout, size, stride, padding)) return 0;
+  const Geom gh = tf_geometry(H, size, stride, padding);
+  const Geom gw = tf_geometry(W, size, stride, padding);
+  if (gh.out <= 0 || gw.out <= 0) return 0;
   TcImpl* im = new TcImpl();
-  // Split-K for 3x3 convs whose item count leaves the last round of the persistent grid mostly
-  // idle (SqueezeDet's ConvDet head: 300 items on 148 SMs = 3 rounds for 2.03 rounds of work):
-  // three partial convs over the filter rows, then a deterministic reduction.
-  int ksplit = 1;
-  {
-    static int env_split = -1;
-    if (env_split < 0) {
-      const char* a = getenv("SQDET_TC_SPLITK");
-      env_split = a ? atoi(a) : 1;
-    }
-    int sms = 148, dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const long long ntiles = (long long)B * ((H + TILE_H - 1) / TILE_H) * ((W + TILE_W - 1) / TILE_W);
-    const bool few_items = Cout <= MAX_N && ntiles < 4LL * sms && (ntiles % sms) != 0 &&
-                           (double)(ntiles % sms) / sms < 0.5;
-    if (env_split && !pool && size == 3 && few_items && Cin >= 96 && (Cout % 4) == 0) ksplit = 3;
-  }
-  std::vector<ConvGroup> groups;
-  int rc;
-  if (ksplit == 1) {
-    groups = {{size, Cout, y_coff, 0}};
-    rc = plan_common(im, B, H, W, Cin, groups, relu, has_affine, y_cstride, x_dev, y_dev, pool);
-  } else {
-    const int pitch = (Cout + 7) / 8 * 8;
-    im->ksplit = ksplit;
-    im->pitch = pitch;
-    im->relu_final = relu;
-    im->cout = Cout;
-    im->y_cstride_final = y_cstride;
-    im->y_coff_final = y_coff;
-    im->npix = (long long)B * H * W;
-    im->y_final = y_dev;
-    cudaError_t ce = cudaMalloc(&im->d_scratch, sizeof(float) * (size_t)im->npix * ksplit * pitch);
-    if (ce != cudaSuccess) {
-      delete im;
-      return cuda_fail(ce, "cudaMalloc(split-K scratch)");
-    }
-    static int env_rows = -1;
-    if (env_rows < 0) {
-      const char* a = getenv("SQDET_TC_SPLITK_ROWS");
-      env_rows = a ? atoi(a) : 0;
-    }
-    const int KCs = (Cin % 32 == 0) ? 32 : 16, kch_all = Cin / KCs;
-    for (int s2 = 0; s2 < ksplit; ++s2) {
-      ConvGroup g{size, Cout, s2 * pitch, 0};
-      if (env_rows || kch_all % ksplit != 0) {
-        g.tap_begin = s2 * size;         // one filter row per partial (reads the input ksplit times)
-        g.tap_count = size;
-      } else {
-        g.kc_begin = s2 * (kch_all / ksplit);   // one input-channel range per partial: every input
-        g.kc_count = kch_all / ksplit;          // byte is read once (ConvDet: 329 -> ~130 MB of DRAM reads)
-      }
-      groups.push_back(g);
-    }
-    // partials: no bias / affine / relu in the conv epilogue (they are applied by the reduction)
-    rc = plan_common(im, B, H, W, Cin, groups, 0, has_affine, ksplit * pitch, x_dev, im->d_scratch,
-                     nullptr);
-    if (rc > 0) im->prm.bias = nullptr, im->prm.scale = nullptr, im->prm.shift = nullptr;
-  }
+  int rc = plan_common(im, B, H, W, Cin, gh.out, gw.out, stride, gh.pad_before, gw.pad_before,
+                       gather, {{size, Cout, y_coff}}, relu, has_affine, y_cstride);
   if (rc <= 0) {
     void* p = im;
     release_impl(&p);
@@ -1587,20 +746,20 @@ int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, int Cout, int s
   }
   plan->enabled = true;
   plan->B = B; plan->H = H; plan->W = W; plan->Cin = Cin; plan->Cout = Cout;
-  plan->size = size; plan->stride = stride; plan->relu = relu; plan->Ho = H; plan->Wo = W;
+  plan->size = size; plan->stride = stride; plan->relu = relu;
+  plan->Ho = gh.out; plan->Wo = gw.out; plan->pad_t = gh.pad_before; plan->pad_l = gw.pad_before;
   plan->y_cstride = y_cstride; plan->y_coff = y_coff;
-  plan->launches = im->ksplit > 1 ? 2 : 1;
   plan->impl = im;
   return 1;
 }
 
-int tc_fire_plan(TcFirePlan* plan, int B, int H, int W, int S, int E1, int E3, const float* q_dev,
-                 float* y_dev, const TcPool* pool) {
+int tc_fire_plan(TcFirePlan* plan, int B, int H, int W, int S, int E1, int E3) {
   plan->enabled = false;
-  if (S % 16 != 0 || S < 16 || (E1 % 4) || (E3 % 4)) return 0;
+  if (!tc_conv_eligible(S, E1, 1, 1, SQDET_PAD_SAME) || !tc_conv_eligible(S, E3, 3, 1, SQDET_PAD_SAME))
+    return 0;
   TcImpl* im = new TcImpl();
-  std::vector<ConvGroup> groups = {{1, E1, 0, 0}, {3, E3, E1, E1}};
-  int rc = plan_common(im, B, H, W, S, groups, 1, false, E1 + E3, q_dev, y_dev, pool);
+  int rc = plan_common(im, B, H, W, S, H, W, 1, 0, 0, false, {{1, E1, 0}, {3, E3, E1}}, 1, false,
+                       E1 + E3);
   if (rc <= 0) {
     void* p = im;
     release_impl(&p);
@@ -1614,11 +773,9 @@ int tc_fire_plan(TcFirePlan* plan, int B, int H, int W, int S, int E1, int E3, c
 
 int tc_conv_pack_weights(TcConvPlan* plan, const float* w_hwio, const float* bias) {
   TcImpl* im = static_cast<TcImpl*>(plan->impl);
-  std::vector<float> packed((size_t)im->rows_half * 2 * im->KC, 0.f);
-  for (int gi = 0; gi < (int)im->groups.size(); ++gi) pack_group(im, gi, w_hwio, packed);
-  SQ_CUDA(cudaMemcpy(im->d_w, packed.data(), packed.size() * sizeof(float), cudaMemcpyHostToDevice));
-  if (bias)
-    SQ_CUDA(cudaMemcpy(im->d_bias, bias, sizeof(float) * plan->Cout, cudaMemcpyHostToDevice));
+  int rc = upload_weights(im, {w_hwio});
+  if (rc) return rc;
+  if (bias) SQ_CUDA(cudaMemcpy(im->d_bias, bias, sizeof(float) * plan->Cout, cudaMemcpyHostToDevice));
   return SQDET_OK;
 }
 
@@ -1633,23 +790,10 @@ int tc_conv_set_affine(TcConvPlan* plan, const float* scale, const float* shift)
 int tc_fire_pack_weights(TcFirePlan* plan, const float* w_e1, const float* b_e1, const float* w_e3,
                          const float* b_e3) {
   TcImpl* im = static_cast<TcImpl*>(plan->impl);
-  std::vector<float> packed((size_t)im->rows_half * 2 * im->KC, 0.f);
-  pack_group(im, 0, w_e1, packed);
-  pack_group(im, 1, w_e3, packed);
-  SQ_CUDA(cudaMemcpy(im->d_w, packed.data(), packed.size() * sizeof(float), cudaMemcpyHostToDevice));
+  int rc = upload_weights(im, {w_e1, w_e3});
+  if (rc) return rc;
   SQ_CUDA(cudaMemcpy(im->d_bias, b_e1, sizeof(float) * plan->E1, cudaMemcpyHostToDevice));
   SQ_CUDA(cudaMemcpy(im->d_bias + plan->E1, b_e3, sizeof(float) * plan->E3, cudaMemcpyHostToDevice));
-  return SQDET_OK;
-}
-
-int launch_splitk_reduce(const float* part, float* y, const float* bias, const float* scale,
-                         const float* shift, long long npix, int cout, int pitch, int ksplit,
-                         int y_cstride, int y_coff, int relu, cudaStream_t stream) {
-  const long long total = npix * (cout / 4);
-  long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
-  SQ_CUDA(launch_kernel(splitk_reduce_kernel, dim3((unsigned)blocks), dim3(256), 0, stream, part, y, bias,
-                        scale, shift, npix, cout, pitch, ksplit, y_cstride, y_coff, relu));
   return SQDET_OK;
 }
 
@@ -1677,10 +821,10 @@ int conv2d_tc_oneshot(const float* x_dev, const float* w_hwio_dev, const float* 
                       int y_cstride, int y_coff, cudaStream_t stream) {
   TcConvPlan plan;
   int rc = tc_conv_plan(&plan, B, H, W, Cin, Cout, size, stride, padding, relu,
-                        scale_dev != nullptr, y_cstride, y_coff, x_dev, y_dev, nullptr);
+                        scale_dev != nullptr, y_cstride, y_coff);
   if (rc < 0) return rc;
   if (rc == 0) {
-    // shape not taken by the tensor-core path (e.g. conv1, Cin = 3): same dispatch as the engine
+    // shape not taken by the tensor-core path (e.g. a strided conv): same dispatch as the engine
     ConvArgs a;
     a.x = x_dev; a.w = w_hwio_dev; a.bias = bias_dev; a.scale = scale_dev; a.shift = shift_dev;
     a.y = y_dev; a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.size = size;
@@ -1688,20 +832,152 @@ int conv2d_tc_oneshot(const float* x_dev, const float* w_hwio_dev, const float* 
     return launch_conv_simt(a, stream);
   }
   std::vector<float> w((size_t)size * size * Cin * Cout), b(Cout, 0.f), sc, sh;
-  SQ_CUDA(cudaMemcpy(w.data(), w_hwio_dev, w.size() * sizeof(float), cudaMemcpyDeviceToHost));
-  if (bias_dev) SQ_CUDA(cudaMemcpy(b.data(), bias_dev, Cout * sizeof(float), cudaMemcpyDeviceToHost));
-  rc = tc_conv_pack_weights(&plan, w.data(), bias_dev ? b.data() : nullptr);
-  if (!rc && scale_dev) {
+  cudaError_t ce = cudaMemcpy(w.data(), w_hwio_dev, w.size() * sizeof(float), cudaMemcpyDeviceToHost);
+  if (ce == cudaSuccess && bias_dev)
+    ce = cudaMemcpy(b.data(), bias_dev, Cout * sizeof(float), cudaMemcpyDeviceToHost);
+  if (ce == cudaSuccess && scale_dev) {
     sc.resize(Cout); sh.resize(Cout);
-    SQ_CUDA(cudaMemcpy(sc.data(), scale_dev, Cout * sizeof(float), cudaMemcpyDeviceToHost));
-    SQ_CUDA(cudaMemcpy(sh.data(), shift_dev, Cout * sizeof(float), cudaMemcpyDeviceToHost));
-    rc = tc_conv_set_affine(&plan, sc.data(), sh.data());
+    ce = cudaMemcpy(sc.data(), scale_dev, Cout * sizeof(float), cudaMemcpyDeviceToHost);
+    if (ce == cudaSuccess) ce = cudaMemcpy(sh.data(), shift_dev, Cout * sizeof(float), cudaMemcpyDeviceToHost);
   }
+  if (ce != cudaSuccess) {
+    tc_conv_release(&plan);
+    return cuda_fail(ce, "conv2d_tc_oneshot: parameter download");
+  }
+  rc = tc_conv_pack_weights(&plan, w.data(), bias_dev ? b.data() : nullptr);
+  if (!rc && scale_dev) rc = tc_conv_set_affine(&plan, sc.data(), sh.data());
   if (!rc) rc = launch_conv_tc(plan, x_dev, y_dev, stream);
-  cudaError_t ce = cudaStreamSynchronize(stream);
+  ce = cudaStreamSynchronize(stream);
   tc_conv_release(&plan);
   if (rc) return rc;
   if (ce != cudaSuccess) return cuda_fail(ce, "conv2d_tc_oneshot sync");
+  return SQDET_OK;
+}
+
+// ---- one-kernel fire module ----------------------------------------------------------------------
+int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int S, int E1, int E3) {
+  plan->enabled = false;
+  if (Cin % 16 || Cin < 16 || S % 16 || S < 16 || S > 64 || E1 <= 0 || E3 <= 0) return 0;
+  const int nch = (E1 + 63) / 64 + (E3 + 63) / 64;
+  if (nch > MAX_FCHUNKS) return 0;
+  FusedImpl* im = new FusedImpl();
+  im->KCI = Cin % 32 == 0 ? 32 : 16;
+  im->SQN = S <= 16 ? 16 : S <= 32 ? 32 : 64;
+  im->KCE = S % 32 == 0 ? 32 : 16;
+  FireParams& p = im->fp;
+  p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.S = S; p.Etot = E1 + E3;
+  p.tiles_w = (W + FT_W - 1) / FT_W;
+  p.tiles_h = (H + 7) / 8;
+  p.nchunks = nch;
+  int c = 0;
+  for (int gi = 0; gi < 2; ++gi) {
+    const int E = gi ? E3 : E1, taps = gi ? 9 : 1;
+    for (int cb = 0; cb < E; cb += 64, ++c) {
+      p.chunks[c] = FireChunk{taps, taps * (S / im->KCE), E - cb < 64 ? E - cb : 64, (gi ? E1 : 0) + cb};
+      im->w2_floats += (long long)p.chunks[c].nk * 2 * 64 * im->KCE;
+    }
+  }
+  im->w_floats = (long long)(Cin / im->KCI) * 2 * im->SQN * im->KCI;
+  im->grid = (unsigned)((long long)B * p.tiles_h * p.tiles_w);
+  cudaError_t ce = cudaSuccess;
+#define SQ_FIRE_SMEM(A, Bq, C)                                                                  \
+  (im->smem = sizeof(float) * ((size_t)STAGES * fire_ring_floats<A, Bq, C>() + FQ_ROWS * (Bq + 4)), \
+   ce = cudaFuncSetAttribute(fire_tc_kernel<A, Bq, C>,                                           \
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)im->smem))
+  SQ_FIRE_DISPATCH(im->KCI, im->SQN, im->KCE, SQ_FIRE_SMEM);
+#undef SQ_FIRE_SMEM
+  void* vp = im;
+  if (ce != cudaSuccess) {
+    release_fused(&vp);
+    return cuda_fail(ce, "cudaFuncSetAttribute(fire_tc_kernel)");
+  }
+  if ((ce = cudaMalloc(&im->d_w, sizeof(float) * im->w_floats)) != cudaSuccess ||
+      (ce = cudaMalloc(&im->d_w2, sizeof(float) * im->w2_floats)) != cudaSuccess ||
+      (ce = cudaMalloc(&im->d_b, sizeof(float) * im->SQN)) != cudaSuccess ||
+      (ce = cudaMalloc(&im->d_b2, sizeof(float) * (E1 + E3))) != cudaSuccess) {
+    release_fused(&vp);
+    return cuda_fail(ce, "cudaMalloc(fused fire)");
+  }
+  p.wsq = im->d_w; p.wex = im->d_w2; p.bsq = im->d_b; p.bex = im->d_b2;
+  plan->enabled = true;
+  plan->B = B; plan->H = H; plan->W = W; plan->Cin = Cin; plan->S = S; plan->E1 = E1; plan->E3 = E3;
+  plan->impl = im;
+  return 1;
+}
+
+int tc_fused_fire_pack_weights(TcFusedFirePlan* plan, const float* w_sq, const float* b_sq,
+                               const float* w_e1, const float* b_e1, const float* w_e3,
+                               const float* b_e3) {
+  FusedImpl* im = static_cast<FusedImpl*>(plan->impl);
+  const FireParams& p = im->fp;
+  std::vector<float> wsq((size_t)im->w_floats), wex((size_t)im->w2_floats);
+  std::vector<float> bsq(im->SQN, 0.f), bex;
+  pack_tiles(w_sq, p.Cin, p.S, 0, im->SQN, im->KCI, p.Cin / im->KCI, wsq.data());
+  long long off = 0;
+  for (int c = 0; c < p.nchunks; ++c) {
+    const FireChunk& ch = p.chunks[c];
+    const bool e3 = ch.taps == 9;
+    pack_tiles(e3 ? w_e3 : w_e1, (long long)ch.taps * p.S, e3 ? plan->E3 : plan->E1,
+               ch.y_off - (e3 ? plan->E1 : 0), 64, im->KCE, ch.nk, wex.data() + off);
+    off += (long long)ch.nk * 2 * 64 * im->KCE;
+  }
+  for (int i = 0; i < p.S; ++i) bsq[i] = b_sq[i];
+  bex.assign(b_e1, b_e1 + plan->E1);
+  bex.insert(bex.end(), b_e3, b_e3 + plan->E3);
+  SQ_CUDA(cudaMemcpy(im->d_w, wsq.data(), wsq.size() * sizeof(float), cudaMemcpyHostToDevice));
+  SQ_CUDA(cudaMemcpy(im->d_w2, wex.data(), wex.size() * sizeof(float), cudaMemcpyHostToDevice));
+  SQ_CUDA(cudaMemcpy(im->d_b, bsq.data(), bsq.size() * sizeof(float), cudaMemcpyHostToDevice));
+  SQ_CUDA(cudaMemcpy(im->d_b2, bex.data(), bex.size() * sizeof(float), cudaMemcpyHostToDevice));
+  return SQDET_OK;
+}
+
+int launch_fused_fire_tc(const TcFusedFirePlan& plan, const float* x_dev, float* y_dev,
+                         cudaStream_t stream) {
+  const FusedImpl* im = static_cast<const FusedImpl*>(plan.impl);
+  FireParams p = im->fp;
+  p.x = x_dev;
+  p.y = y_dev;
+  cudaError_t ce = cudaSuccess;
+#define SQ_FIRE_LAUNCH(A, Bq, C) \
+  ce = launch_kernel(fire_tc_kernel<A, Bq, C>, dim3(im->grid), dim3(NUM_THREADS), im->smem, stream, p)
+  SQ_FIRE_DISPATCH(im->KCI, im->SQN, im->KCE, SQ_FIRE_LAUNCH);
+#undef SQ_FIRE_LAUNCH
+  if (ce != cudaSuccess) return cuda_fail(ce, "launch fire_tc_kernel");
+  return SQDET_OK;
+}
+
+void tc_fused_fire_release(TcFusedFirePlan* plan) {
+  release_fused(&plan->impl);
+  plan->enabled = false;
+}
+
+int fire_fused_oneshot(const float* x_dev, const float* w_sq_dev, const float* b_sq_dev,
+                       const float* w_e1_dev, const float* b_e1_dev, const float* w_e3_dev,
+                       const float* b_e3_dev, float* y_dev, int B, int H, int W, int Cin, int S,
+                       int E1, int E3, cudaStream_t stream) {
+  TcFusedFirePlan plan;
+  int rc = tc_fused_fire_plan(&plan, B, H, W, Cin, S, E1, E3);
+  if (rc <= 0) return rc < 0 ? rc : 1;
+  std::vector<float> wsq((size_t)Cin * S), bsq(S), w1((size_t)S * E1), b1(E1), w3((size_t)9 * S * E3),
+      b3(E3);
+  const std::pair<void*, const float*> io[6] = {{wsq.data(), w_sq_dev}, {bsq.data(), b_sq_dev},
+                                                {w1.data(), w_e1_dev},  {b1.data(), b_e1_dev},
+                                                {w3.data(), w_e3_dev},  {b3.data(), b_e3_dev}};
+  const size_t n[6] = {wsq.size(), bsq.size(), w1.size(), b1.size(), w3.size(), b3.size()};
+  cudaError_t ce = cudaSuccess;
+  for (int i = 0; i < 6 && ce == cudaSuccess; ++i)
+    ce = cudaMemcpy(io[i].first, io[i].second, n[i] * sizeof(float), cudaMemcpyDeviceToHost);
+  if (ce != cudaSuccess) {
+    tc_fused_fire_release(&plan);
+    return cuda_fail(ce, "fire_fused_oneshot: parameter download");
+  }
+  rc = tc_fused_fire_pack_weights(&plan, wsq.data(), bsq.data(), w1.data(), b1.data(), w3.data(),
+                                  b3.data());
+  if (!rc) rc = launch_fused_fire_tc(plan, x_dev, y_dev, stream);
+  ce = cudaStreamSynchronize(stream);
+  tc_fused_fire_release(&plan);
+  if (rc) return rc;
+  if (ce != cudaSuccess) return cuda_fail(ce, "fire_fused_oneshot sync");
   return SQDET_OK;
 }
 

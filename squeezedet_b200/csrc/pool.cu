@@ -55,7 +55,7 @@ maxpool_vec4_kernel(const float* __restrict__ x, float* __restrict__ y, int B, i
 // Stride-2 windows of 2x2 or 3x3 (every pool of the four nets): all K*K loads of a thread are
 // issued before the first max (addresses clamped into the image, out-of-image taps replaced by -inf
 // afterwards), 32-bit index arithmetic.  The generic kernel below branches around each tap, which
-// serialises its loads (pool3: 3.39 TB/s -> see profiles/r2_pool.txt).
+// serialises its loads.
 template <int K>
 __global__ void __launch_bounds__(256)
 maxpool_s2_vec4_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W,
@@ -273,7 +273,10 @@ int launch_maxpool(const float* x, float* y, int B, int H, int W, int C, int siz
                    ((reinterpret_cast<uintptr_t>(y) & 15) == 0);
   const long long total = (long long)B * gh.out * gw.out * (vec ? C / 4 : C);
   long long blocks = (total + 255) / 256;
-  const long long cap = 148LL * 8 * 16;   // grid-stride beyond 16 waves of 8 CTAs/SM
+  int sms = 132, dev = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const long long cap = (long long)sms * 8 * 16;   // grid-stride beyond 16 waves of 8 CTAs/SM
   if (blocks > cap) blocks = cap;
   static int env_fast = -1;
   if (env_fast < 0) {

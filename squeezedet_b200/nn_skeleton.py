@@ -6,7 +6,7 @@ graph attributes (`image_input`, `preds`, `det_boxes`, `det_probs`, `det_class`,
 `model_params`, `model_size_counter`, `flop_counter`, `activation_counter`) and the
 same `filter_prediction(boxes, probs, cls_idx)`.  Instead of building a TF-1.0
 graph, each constructor records the layer into a `libsqdet_b200` engine plan
-(C ABI, `include/sqdet_b200.h`); the arithmetic runs in hand-written sm_100a
+(C ABI, `include/sqdet_b200.h`); the arithmetic runs in hand-written sm_90a
 kernels.  There is no TensorFlow and no CPU fallback.
 
 What replaces `sess.run([model.det_boxes, model.det_probs, model.det_class],

@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-  config.addinivalue_line('markers', 'gpu: needs a B200 (run with -m gpu on the GPU box)')
+  config.addinivalue_line('markers', 'gpu: needs an H100 (run with -m gpu on a GPU machine)')
 
 
 @pytest.fixture(scope='session')

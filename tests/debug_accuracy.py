@@ -1,6 +1,6 @@
 """GPU debug driver: end-to-end accuracy of the SqueezeDet forward against the fp64 oracle
 (truth) next to the fp32 oracle's own error, at the smoke() configuration.
-Usage: python tests/debug_accuracy.py [tc|simt]   (SQDET_TC_SEG=n varies the segment length)"""
+Usage: python tests/debug_accuracy.py [tc|simt]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -32,7 +32,7 @@ def run(dtype):
 p32, (b32, s32, c32) = run(np.float32)
 p64, (b64, s64, c64) = run(np.float64)
 sc = np.abs(p64).max()
-print('mode %s seg %s' % (mode, os.environ.get('SQDET_TC_SEG', 'default')))
+print('mode %s' % mode)
 print('preds  max|gpu-f64|/max %.3e   max|f32-f64|/max %.3e   mean signed (gpu-f64)/|f64| %.3e'
       % (np.abs(got_preds - p64).max() / sc, np.abs(p32 - p64).max() / sc,
          np.mean((got_preds - p64) * np.sign(p64)) / np.mean(np.abs(p64))))

@@ -1,5 +1,4 @@
-"""GPU debug driver: one profiled (non-graph) forward at the bench configuration; with
-SQDET_TC_DEBUG=1 every tensor-core launch prints its per-role stall accounting."""
+"""GPU debug driver: one profiled (non-graph) forward at the bench configuration."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

@@ -1,8 +1,7 @@
-"""Adversarial operand distributions for the tensor-core convolution (conv_tc.cu): the tcgen05
-accumulator adds with truncation, and the kernels compensate a segment of m chained MMAs with the
-scalar 1 + bias_comp*m measured by tools/mma_bias.cu on one-signed chains.  That model is exact
-only when the addends share the sum's sign, so these cases stress the others: all-positive (bias
-fully present), heavy-tailed (log-normal: a few products dominate), cancellation-dominated (the sum
+"""Adversarial operand distributions for the tensor-core convolution (conv_tc.cu): the tensor
+core's own accumulation must not leave a one-signed bias over a long K (the kernel adds each K
+chunk's MMA result into fp32 running sums).  These cases stress it: all-positive (any truncation
+bias fully present), heavy-tailed (log-normal: a few products dominate), cancellation-dominated (the sum
 is tiny against sum |products|), plus a long K.  Error is measured per output element against the
 fp64 oracle on the scale that bounds ANY fp32 summation of the same products,
     |err| <= tol * (|x| (*) |w|),
@@ -18,9 +17,8 @@ pytestmark = pytest.mark.gpu
 
 # Forward-error bar in units of sum |products|, for K products per output: fp32 round-to-nearest
 # accumulation random-walks to ~ sqrt(K) * 2^-24 (measured 2.7e-6 at K = 2304 on all-positive
-# operands with the FFMA kernel); the 3xTF32 path drops terms of 2^-21 per product and carries the
-# residual of the scalar bias compensation (tools/mma_bias.cu: a one-signed 36-MMA segment is short
-# by 1.6e-6, 1.1e-6 after the compensation).  One bar for both math modes:
+# operands with the FFMA kernel); the 3xTF32 path drops terms of 2^-21 per product.  One bar for
+# both math modes:
 def adv_tol(K):
   return 1.2e-7 * np.sqrt(K)
 

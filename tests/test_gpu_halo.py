@@ -1,6 +1,5 @@
-"""The halo-tile 3x3 convolution (csrc/halo_tc.cu, entry sqdet_conv3x3_halo) against the numpy
-oracle: both tile orientations, split-K over input-channel ranges and the direct epilogue, the
-ConvDet head's 72-channel output (partial last 32-channel group), BN-style scale/shift, a channel
+"""The stage-isolated 3x3 tensor-core convolution (entry sqdet_conv3x3_halo) against the numpy
+oracle: ragged tiles on both axes, the ConvDet head's 72-channel output (partial last channel chunk), BN-style scale/shift, a channel
 window of a wider tensor, and a grid with more items than SMs."""
 import numpy as np
 import pytest
@@ -20,7 +19,7 @@ CASES = [
     (1, 9, 40, 32, 128),      # one row of tiles, N = 128
     (2, 17, 23, 48, 256),     # two output-channel chunks of 128
     (1, 8, 16, 16, 32),       # exactly one tile, one K chunk
-    (6, 40, 48, 32, 32),      # 180 tiles > 148 SMs: several items per CTA
+    (6, 40, 48, 32, 32),      # more 128-pixel tiles than SMs
 ]
 
 

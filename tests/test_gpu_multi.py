@@ -1,7 +1,7 @@
 """More than one device: (1) two engines on two devices of ONE process (the per-device opt-in of
-the >48 KB dynamic shared memory, ADVICE r1); (2) N ranks, NCCL all-gather captured in the
-forward graph: the gathered records are byte-equal to a 1-rank run of the same global batch.
-Both skip below 2 visible GPUs (the single-GPU box of the round-end run)."""
+the >48 KB dynamic shared memory); (2) N ranks, NCCL all-gather captured in the forward graph:
+the gathered records are byte-equal to a 1-rank run of the same global batch.
+Both skip on a machine with fewer than 2 visible GPUs."""
 import os
 import subprocess
 import sys

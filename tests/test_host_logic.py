@@ -83,32 +83,3 @@ def test_gloo_world2_allgather_roundtrip(tmp_path):
   assert a['counts'].tolist() == [2, 0, 5, 1, 3]          # 5 images: shards 3 + 2
   assert a['dets'].shape == (5, 8)
   assert a['dets']['anchor'][2, :5].tolist() == [200, 201, 202, 203, 204]
-
-
-def test_ncu_summary_maps_launches_to_ops():
-  """tools/ncu_summary.py: kernel names of one SqueezeDet forward -> engine ops (the mapping the
-  tracked profiles/r2_launch_shares.csv and r2_traffic.json depend on), for the round-2 launch
-  sequence (fire2/3 as one kernel each) and for the all-two-launch plan."""
-  import importlib.util
-  spec = importlib.util.spec_from_file_location(
-      'ncu_summary', os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
-                                  'tools', 'ncu_summary.py'))
-  mod = importlib.util.module_from_spec(spec)
-  spec.loader.exec_module(mod)
-  tc = 'void sqdet::conv_tc_kernel<32, 0, 0>(TcParams)'
-  fused = (['first_tc_kernel<3, 2>', 'fire_fused_kernel', 'fire_fused_kernel', 'maxpool_s2_vec4_kernel<3>'] +
-           [tc] * 4 + ['maxpool_s2_vec4_kernel<3>'] + [tc] * 12 +
-           [tc, 'splitk_reduce_kernel', 'interpret_kernel', 'filter_kernel'])
-  ops = mod.ops_of(fused)
-  assert len(ops) == 25
-  assert ops[:4] == ['conv1+pool1', 'fire2.fused', 'fire3.fused', 'pool3']
-  assert ops[4:8] == ['fire4.squeeze', 'fire4.expand', 'fire5.squeeze', 'fire5.expand']
-  assert ops[8] == 'pool5' and ops[9] == 'fire6.squeeze' and ops[20] == 'fire11.expand'
-  assert ops[21:] == ['conv12.partials', 'conv12.reduce', 'interpret_output', 'filter_prediction']
-  unfused = (['conv_pool_simt_kernel<3, 256, 2>'] + [tc] * 4 + ['maxpool_vec4_kernel'] + [tc] * 4 +
-             ['maxpool_vec4_kernel'] + [tc] * 12 + [tc, 'splitk_reduce_kernel', 'interpret_kernel',
-                                                    'filter_kernel'])
-  ops = mod.ops_of(unfused)
-  assert len(ops) == 27 and ops[1:3] == ['fire2.squeeze', 'fire2.expand'] and ops[-4] == 'conv12.partials'
-  s, n = mod.forward_span(['x'] + unfused + ['y'] + fused)
-  assert (s, n) == (len(unfused) + 2, 25)

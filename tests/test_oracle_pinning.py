@@ -1,14 +1,13 @@
-"""The oracle's numpy half against (a) the committed fixtures produced by the
-reference's own functions (tests/golden/make_golden.py) and (b) the live reference
-import when /root/reference is present (dev container only)."""
+"""The oracle's numpy half against the committed fixtures produced by the reference's own
+functions (tests/golden/make_golden.py, tests/golden/make_filter_trials.py)."""
 import hashlib
+import os
 
 import numpy as np
 import pytest
 
 import oracle
 from oracle import postproc as P
-from oracle import ref_import
 
 
 def _run_oracle(c):
@@ -70,24 +69,28 @@ def test_set_anchors_matches_reference_fixtures(anchors_golden):
     assert a[0].tolist() == g['first'] and a[-1].tolist() == g['last']
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference tree not mounted')
-def test_live_reference_import_agrees():
-  ns = ref_import.load()
+def filter_trials():
+  """60 seeded filter_prediction cases: (boxes, probs, cls, top_n)."""
   rng = np.random.default_rng(7)
-  for trial in range(60):
+  for _ in range(60):
     n = int(rng.integers(1, 400))
     boxes = np.stack([rng.uniform(0, 1242, n), rng.uniform(0, 375, n),
                       rng.uniform(5, 300, n), rng.uniform(5, 200, n)], 1).astype(np.float32)
     probs = rng.permutation(np.linspace(0.001, 0.999, n)).astype(np.float32)
     cls = rng.integers(0, 3, n).astype(np.int64)
     top_n = int(rng.choice([64, 0, 1000, 10]))
-    fb, fp, fc = ref_import.ref_filter_prediction(ns, boxes, probs, cls, 3, top_n, 0.005, 0.4)
+    yield boxes, probs, cls, top_n
+
+
+def test_reference_filter_trials_agree():
+  """The reference's own filter_prediction outputs on the seeded trials
+  (tests/golden/make_filter_trials.py) against the oracle, bit for bit."""
+  z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'filter_trials.npz'))
+  for t, (boxes, probs, cls, top_n) in enumerate(filter_trials()):
     ob, op, oc, _ = oracle.filter_prediction(boxes, probs, cls, 3, top_n, 0.005, 0.4)
-    assert fc == oc
-    assert all(np.array_equal(x, y) for x, y in zip(fb, ob))
-    assert [float(x) for x in fp] == [float(x) for x in op]
-  for fn, (w, h, gh, gw, shapes) in CONFIGS.items():
-    assert np.array_equal(ns.configs[fn]().ANCHOR_BOX, oracle.set_anchors(w, h, gh, gw, shapes))
+    assert oc == z['t%d_cls' % t].tolist(), t
+    assert np.array_equal(np.asarray(ob, np.float32).reshape(-1, 4), z['t%d_boxes' % t]), t
+    assert np.array_equal(np.asarray(op, np.float32), z['t%d_probs' % t]), t
 
 
 def test_interpret_output_hand_case():
