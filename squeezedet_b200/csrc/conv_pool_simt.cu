@@ -233,6 +233,8 @@ int launch_conv_pool_simt(const float* x, const float* w, const float* bias, con
   const int threads = 64 * (Cout / 16);
   const size_t smem = ksize == 3 ? smem_bytes_for<3>(Cout) : smem_bytes_for<7>(Cout);
   if (smem > 232448) return fail(SQDET_ERR_UNSUPPORTED, "conv+pool: tile does not fit in smem");
+  // Exactly `threads` threads: each 64 of them own one 16-channel group (cg = tid >> 6), and
+  // s_conv / bias hold Cout / 16 groups.  NT_ is only the __launch_bounds__ ceiling.
 #define SQ_LAUNCH_CP(KS_, NT_, MINB_)                                                          \
   do {                                                                                         \
     /* the opt-in is per device: remember which devices of this process already have it */    \
@@ -244,8 +246,8 @@ int launch_conv_pool_simt(const float* x, const float* w, const float* bias, con
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));      \
       if (dev_ < 64) attr_devs |= 1ull << dev_;                                                \
     }                                                                                          \
-    SQ_CUDA(launch_kernel(conv_pool_simt_kernel<KS_, NT_, MINB_>, grid, dim3(NT_), smem, stream, \
-                          p));                                                               \
+    SQ_CUDA(launch_kernel(conv_pool_simt_kernel<KS_, NT_, MINB_>, grid, dim3(threads), smem,    \
+                          stream, p));                                                         \
   } while (0)
   if (ksize == 3 && threads <= 256) SQ_LAUNCH_CP(3, 256, 2);
   else if (ksize == 3) SQ_LAUNCH_CP(3, 384, 1);

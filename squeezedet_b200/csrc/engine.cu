@@ -181,6 +181,17 @@ static int add_param(sqdet_engine* e, const std::string& name, std::vector<int64
   return idx;
 }
 
+// True when an op other than `self` reads tensor `t`.
+static bool read_by_other_op(const sqdet_engine* e, int t, const Op* self) {
+  for (const auto& o : e->ops) {
+    if (&o == self) continue;
+    if (o.src == t || o.src2 == t) return true;
+    for (const auto& c : o.convs)
+      if (c.src == t) return true;
+  }
+  return false;
+}
+
 static int new_tensor(sqdet_engine* e, const std::string& name, int B, int H, int W, int C) {
   Tensor t;
   t.name = name;
@@ -747,6 +758,8 @@ int sqdet_set_preds(sqdet_engine* e, int preds, const double* anchor_box, int64_
   return SQDET_OK;
 }
 
+static int plan_ops(sqdet_engine* e);
+
 int sqdet_finalize(sqdet_engine* e) {
   if (!e) return fail(SQDET_ERR_INVALID_ARG, "null engine");
   if (e->finalized) return fail(SQDET_ERR_STATE, "already finalized");
@@ -793,6 +806,8 @@ int sqdet_finalize(sqdet_engine* e) {
       e->tensors[prod.dst].materialized = false;
     }
   }
+  int rc = plan_ops(e);
+  if (rc) return rc;
   // activations
   for (size_t i = 0; i < e->tensors.size(); ++i) {
     Tensor& t = e->tensors[i];
@@ -818,7 +833,15 @@ int sqdet_finalize(sqdet_engine* e) {
     e->d_counts = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(blob) + rec_bytes);
   }
   SQ_CUDA(cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
-  // per-op accounting + tensor-core planning
+  e->finalized = true;
+  e->params_dirty = true;
+  return SQDET_OK;
+}
+
+// Per-op accounting and tensor-core planning.  Runs before the activations are allocated: a
+// fire module planned as one kernel never materialises its squeeze tensor.
+static int plan_ops(sqdet_engine* e) {
+  const sqdet_config& c = e->cfg;
   for (auto& op : e->ops) {
     int64_t bytes = 0;
     op.launches = 0;
@@ -844,10 +867,12 @@ int sqdet_finalize(sqdet_engine* e) {
           cudaGetDevice(&dev);
           cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
           const long long tiles = (long long)xin.B * ((xin.H + 7) / 8) * ((xin.W + 15) / 16);
-          if (sq.Cout <= 16 && tiles >= 4LL * sms) {
+          if (sq.Cout <= 16 && tiles >= 4LL * sms && sq.dst != e->preds &&
+              !read_by_other_op(e, sq.dst, &op)) {
             int rcf = tc_fused_fire_plan(&op.fused, xin.B, xin.H, xin.W, xin.C, sq.Cout,
                                          op.convs[1].Cout, op.convs[2].Cout);
             if (rcf < 0) return rcf;
+            if (op.fused.enabled) e->tensors[sq.dst].materialized = false;
           }
         }
         if (op.kind == OP_FIRE && !op.fused.enabled) {
@@ -872,8 +897,6 @@ int sqdet_finalize(sqdet_engine* e) {
     }
     op.min_bytes = bytes;
   }
-  e->finalized = true;
-  e->params_dirty = true;
   return SQDET_OK;
 }
 

@@ -46,10 +46,15 @@ def _case(kind, rng, shape_x, shape_w):
 
 
 SHAPES = [
-    # B, H, W, Cin, Cout, k
-    (1, 12, 20, 96, 64, 3),      # 864 products per output, 3 segments of 36 MMAs
-    (1, 9, 17, 256, 32, 3),      # 2304 products, K chunks of 32
-    (1, 16, 24, 768, 16, 1),     # the longest 1x1 of SqueezeDet (fire11 squeeze)
+    # B, H, W, Cin, Cout, k, stride (SAME padding)
+    (1, 12, 20, 96, 64, 3, 1),    # 864 products per output, 3 segments of 36 MMAs
+    (1, 9, 17, 256, 32, 3, 1),    # 2304 products, K chunks of 32
+    (1, 16, 24, 768, 16, 1, 1),   # the longest 1x1 of SqueezeDet (fire11 squeeze)
+    (1, 12, 20, 48, 64, 3, 1),    # K chunks of 16 (Cin % 32 == 16)
+    (1, 10, 18, 80, 48, 3, 1),    # K chunks of 16, 45 of them
+    (1, 12, 20, 48, 32, 3, 1),    # K chunks of 16 with a 32-wide output tile
+    (2, 17, 29, 3, 64, 3, 1),     # gather mode: K = 27 zero-padded to one 32-row chunk
+    (1, 33, 47, 3, 32, 3, 2),     # gather mode, stride 2, 32-wide output tile
 ]
 
 
@@ -57,12 +62,13 @@ SHAPES = [
 @pytest.mark.parametrize('kind', ['positive', 'lognormal', 'lognormal_positive', 'cancel'])
 @pytest.mark.parametrize('shape', SHAPES)
 def test_conv_adversarial_operands(shape, kind, math_mode, gpu_device):
-  B, H, W, Cin, Cout, k = shape
+  B, H, W, Cin, Cout, k, stride = shape
   rng = np.random.default_rng(1000 + Cin + k)
   x, w = _case(kind, rng, (B, H, W, Cin), (k, k, Cin, Cout))
-  want = oracle.conv2d(x, w, None, 1, 'SAME', apply_relu=False, dtype=np.float64)
-  bound = oracle.conv2d(np.abs(x), np.abs(w), None, 1, 'SAME', apply_relu=False, dtype=np.float64)
-  got = conv2d_gpu(x, w, None, 1, 'SAME', relu=False, math_mode=math_mode)
+  want = oracle.conv2d(x, w, None, stride, 'SAME', apply_relu=False, dtype=np.float64)
+  bound = oracle.conv2d(np.abs(x), np.abs(w), None, stride, 'SAME', apply_relu=False,
+                        dtype=np.float64)
+  got = conv2d_gpu(x, w, None, stride, 'SAME', relu=False, math_mode=math_mode)
   ratio = np.abs(got.astype(np.float64) - want) / bound
   assert not np.isnan(got).any()
   tol = adv_tol(k * k * Cin)

@@ -53,6 +53,73 @@ def test_fire_vs_oracle(shape, math_mode, gpu_device):
   assert rel_err(got, want64) < FIRE_RTOL, rel_err(got, want64)
   assert rel_err(got, want32) < 1e-4
   assert rel_err(want32, want64) < FIRE_RTOL          # sanity of the bar
+  r = fire_bound_ratio(args, got, want64)
+  assert r < 1.0, r
+
+
+# Shapes the shipped nets never produce, chosen to reach every fire_tc_kernel<KCI, SQN, KCE>
+# instantiation and the planner's edges (conv_tc.cu, tc_fused_fire_plan):
+#   KCI = 16 (Cin % 32 == 16) at every squeeze width: <16,16,16> <16,32,32> <16,64,16> <16,64,32>
+#   E1 != E3, expand widths that are not multiples of 64 or of 8,
+#   16 expand chunks of 64 (the one-kernel limit) and 17 (sqdet_fire falls back to separate
+#   launches).
+FIRE_EDGE_CASES = [
+    # (Cin, S, E1, E3), (B, H, W)
+    *[((cin, s, 64, 64), (2, 11, 21)) for cin in (16, 48, 80, 112) for s in (16, 32, 48, 64)],
+    ((64, 16, 40, 88), (2, 13, 19)),
+    ((96, 32, 24, 200), (1, 10, 33)),
+    ((48, 48, 40, 88), (2, 9, 17)),
+    ((128, 64, 40, 88), (2, 9, 17)),
+    ((64, 16, 512, 512), (1, 9, 18)),
+    ((64, 16, 576, 512), (1, 9, 18)),
+    # tiny images: 1x1, one row, one column, one exact 8x16 tile, one pixel past it on both axes
+    *[((48, 32, 40, 88), (3, h, w)) for h, w in ((1, 1), (1, 17), (9, 1), (8, 16), (9, 17))],
+    *[((64, 48, 64, 64), (3, h, w)) for h, w in ((1, 1), (8, 16), (9, 17))],
+]
+
+
+def fire_error_bound(x, ws, w1, w3, q64):
+  """Per-element scale of the error of squeeze -> ReLU -> expand in any fp32 summation order:
+  the expand's own rounding, tol * (|q| (*) |w_e|), plus the squeeze's error carried through the
+  expand, tol * ((|x| (*) |w_s|) (*) |w_e|); ReLU is 1-Lipschitz, so it cannot amplify the
+  squeeze error."""
+  def conv(a, w):
+    return oracle.conv2d(a, w, None, 1, 'SAME', False, np.float64)
+  sx = conv(np.abs(x), np.abs(ws))
+  return np.concatenate([conv(np.abs(q64), np.abs(w1)) + conv(sx, np.abs(w1)),
+                         conv(np.abs(q64), np.abs(w3)) + conv(sx, np.abs(w3))], axis=3)
+
+
+def fire_bound_ratio(args, got, want64):
+  """max |got - want64| / fire_error_bound, in units of the bar 1.2e-7 * sqrt(K) with K the
+  longer of the two convs' sums (test_gpu_adversarial.adv_tol); must stay below 1."""
+  x, ws, bs, w1, b1, w3, b3 = args
+  q64 = oracle.conv2d(x, ws, bs, 1, 'SAME', True, np.float64)
+  err = np.abs(got.astype(np.float64) - want64)
+  bound = fire_error_bound(x, ws, w1, w3, q64)
+  with np.errstate(divide='ignore'):
+    ratio = np.divide(err, bound, out=np.zeros_like(err), where=err > 0)
+  return float(ratio.max()) / (1.2e-7 * np.sqrt(max(x.shape[3], 9 * ws.shape[3])))
+
+
+@pytest.mark.parametrize('math_mode', [_lib.MATH_FP32_SIMT, _lib.MATH_TF32X3_TC])
+@pytest.mark.parametrize('shape,spatial', FIRE_EDGE_CASES)
+def test_fire_edge_shapes_vs_oracle(shape, spatial, math_mode, gpu_device):
+  """Every one-kernel fire variant and the planner's edges, against fp64 with the per-tensor
+  bar of test_fire_vs_oracle and the per-element bound of fire_error_bound; the same call twice
+  is bit-identical."""
+  Cin, S, E1, E3 = shape
+  args = make_case(shape, spatial, seed=Cin * 131 + S * 7 + E1 + E3 + sum(spatial))
+  want64 = fire_oracle(*args, dtype=np.float64)
+  want32 = fire_oracle(*args, dtype=np.float32)
+  got = fire_gpu(*args, math_mode=math_mode, device=gpu_device)
+  assert got.shape == want64.shape and not np.isnan(got).any()
+  assert rel_err(got, want64) < FIRE_RTOL, rel_err(got, want64)
+  assert rel_err(got, want32) < 1e-4
+  r = fire_bound_ratio(args, got, want64)
+  assert r < 1.0, r
+  again = fire_gpu(*args, math_mode=math_mode, device=gpu_device)
+  assert np.array_equal(got, again)            # deterministic: fixed summation order
 
 
 @pytest.mark.parametrize('shape', [SQUEEZEDET_FIRES[0], SQUEEZEDET_FIRES[3], SQUEEZEDET_FIRES[9]])

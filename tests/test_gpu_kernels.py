@@ -31,6 +31,31 @@ CONV_CASES = [
     (1, 48, 100, 3, 96, 3, 1, 'VALID'),
     (1, 64, 96, 64, 64, 1, 1, 'SAME'),     # flat 1x1 tiling, 48 whole tiles
     (3, 11, 13, 32, 48, 1, 1, 'SAME'),     # flat 1x1 tiling, ragged last tile
+    # gather mode with 16- and 32-wide output tiles (conv_tc_kernel<16|32, 32, true>)
+    (2, 19, 35, 3, 16, 3, 1, 'SAME'),
+    (1, 21, 40, 3, 16, 3, 2, 'VALID'),
+    (1, 22, 37, 3, 32, 3, 2, 'SAME'),
+    (2, 17, 30, 3, 32, 3, 1, 'VALID'),
+    # Cin % 32 == 16 with a 16-wide output tile: KC = 16, NT = 16 (conv_tc_kernel<16, 16, false>)
+    (2, 14, 23, 16, 16, 3, 1, 'SAME'),
+    (1, 13, 29, 48, 16, 1, 1, 'SAME'),
+    # one-pixel-high / -wide images under a 3x3 window: every tap but the centre row / column pads
+    (2, 1, 37, 32, 64, 3, 1, 'SAME'),
+    (1, 29, 1, 16, 32, 3, 1, 'SAME'),
+    (1, 1, 40, 3, 16, 3, 1, 'SAME'),
+    # M = B * Ho * Wo around one 128-pixel tile: 1, 127, 128, 129
+    (1, 1, 1, 64, 64, 3, 1, 'SAME'),
+    (1, 1, 127, 32, 48, 1, 1, 'SAME'),
+    (2, 8, 8, 16, 32, 3, 1, 'SAME'),
+    (1, 3, 43, 48, 64, 3, 1, 'SAME'),
+    # ragged last output-channel chunk with NT = 64: 100 = 64 + 36 (not a multiple of 8),
+    # 200 = 3 * 64 + 8
+    (1, 9, 15, 64, 100, 3, 1, 'SAME'),
+    (1, 10, 13, 32, 200, 1, 1, 'SAME'),
+    # the 32-chunk launch limit: 2048 = 32 chunks of 64 runs on wgmma, 2049 is declined and
+    # runs on the SIMT kernel
+    (1, 3, 5, 32, 2048, 1, 1, 'SAME'),
+    (1, 3, 5, 32, 2049, 1, 1, 'SAME'),
 ]
 
 

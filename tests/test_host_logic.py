@@ -65,6 +65,81 @@ def test_shard_ranges():
   assert sum(b - a for a, b in r) == 20
 
 
+# ---- tensor-core kernel selection, restated from squeezedet_b200/csrc/conv_tc.cu --------------
+MAX_CHUNKS = 32          # conv_tc.cu:49   output-channel chunks per conv_tc_kernel launch
+MAX_FCHUNKS = 16         # conv_tc.cu:334  64-wide expand chunks per fire_tc_kernel launch
+
+
+def tc_pick_nt(couts):
+  """pick_nt (conv_tc.cu:526-537): the narrowest-cost output tile of 64 / 32 / 16 whose chunk
+  count fits one launch; None when none fits (the conv is declined)."""
+  best = best_cost = None
+  for nt in (64, 32, 16):
+    chunks = sum(-(-c // nt) for c in couts)
+    if chunks > MAX_CHUNKS:
+      continue
+    cost = chunks * (nt + 32)
+    if best is None or cost < best_cost:
+      best, best_cost = nt, cost
+  return best
+
+
+def tc_conv_variant(Cin, Cout, k, stride, padding):
+  """conv_tc_kernel<NT, KC, GATHER> that sqdet_conv2d runs with MATH_TF32X3_TC, or None when the
+  shape goes to the SIMT kernel: tc_conv_plan (conv_tc.cu:731-741) with tc_conv_eligible
+  (conv_tc.cu:725-729) and plan_common's KC rule (conv_tc.cu:561-563)."""
+  gather = Cin == 3 and k == 3 and stride in (1, 2)
+  eligible = stride == 1 and padding == 'SAME' and k in (1, 3) and Cin % 16 == 0 and Cin >= 16
+  if not (gather or eligible):
+    return None
+  nt = tc_pick_nt([Cout])
+  if nt is None:
+    return None
+  return nt, 32 if gather or Cin % 32 == 0 else 16, gather
+
+
+def tc_fire_variant(Cin, S, E1, E3):
+  """fire_tc_kernel<KCI, SQN, KCE> that sqdet_fire runs with MATH_TF32X3_TC, or None when
+  tc_fused_fire_plan declines (conv_tc.cu:858-866) and the fire runs as separate convs."""
+  if Cin % 16 or Cin < 16 or S % 16 or not 16 <= S <= 64:
+    return None
+  if -(-E1 // 64) + -(-E3 // 64) > MAX_FCHUNKS:
+    return None
+  return (32 if Cin % 32 == 0 else 16, 16 if S <= 16 else 32 if S <= 32 else 64,
+          32 if S % 32 == 0 else 16)
+
+
+ALL_CONV_TC_VARIANTS = {(nt, kc, g) for nt in (64, 32, 16) for kc, g in ((32, True), (32, False),
+                                                                        (16, False))}
+# SQ_FIRE_DISPATCH (conv_tc.cu:710-720)
+ALL_FIRE_TC_VARIANTS = {(32, 16, 16), (32, 32, 32), (32, 64, 16), (32, 64, 32),
+                        (16, 16, 16), (16, 32, 32), (16, 64, 16), (16, 64, 32)}
+
+
+def test_gpu_case_tables_reach_every_tc_kernel_variant():
+  """The GPU parity tables run every conv_tc_kernel and fire_tc_kernel instantiation, and both
+  sides of the chunk limits, by the host rules above."""
+  from test_gpu_adversarial import SHAPES
+  from test_gpu_fire import FIRE_EDGE_CASES
+  from test_gpu_kernels import CONV_CASES
+  conv = {tc_conv_variant(Cin, Cout, k, s, pad) for _, _, _, Cin, Cout, k, s, pad in CONV_CASES}
+  assert conv - {None} == ALL_CONV_TC_VARIANTS, ALL_CONV_TC_VARIANTS - conv
+  adv = {tc_conv_variant(Cin, Cout, k, s, 'SAME') for _, _, _, Cin, Cout, k, s in SHAPES}
+  assert {(16, False), (32, True)} <= {(kc, g) for _, kc, g in adv - {None}}
+  assert any(v is not None and v[:2] == (32, 16) for v in adv)     # NT = 32 with KC = 16
+  fire = {tc_fire_variant(*shape) for shape, _ in FIRE_EDGE_CASES}
+  assert fire - {None} == ALL_FIRE_TC_VARIANTS, ALL_FIRE_TC_VARIANTS - fire
+  # chunk limits: a 2048-wide 1x1 is 32 chunks of 64 on wgmma, 2049 falls back to SIMT; a fire
+  # with 16 expand chunks is one kernel, 17 fall back
+  assert tc_conv_variant(32, 2048, 1, 1, 'SAME') == (64, 32, False)
+  assert tc_conv_variant(32, 2049, 1, 1, 'SAME') is None
+  assert (1, 3, 5, 32, 2048, 1, 1, 'SAME') in CONV_CASES
+  assert (1, 3, 5, 32, 2049, 1, 1, 'SAME') in CONV_CASES
+  shapes = [s for s, _ in FIRE_EDGE_CASES]
+  assert (64, 16, 512, 512) in shapes and tc_fire_variant(64, 16, 512, 512) is not None
+  assert (64, 16, 576, 512) in shapes and tc_fire_variant(64, 16, 576, 512) is None
+
+
 def test_gloo_world2_allgather_roundtrip(tmp_path):
   """N>1 path on CPU: 2 processes, gloo, 127.0.0.1 — each packs its shard's detection
   blob, one all_gather, both unpack identical global results."""
