@@ -24,41 +24,6 @@ int  cuda_fail(cudaError_t err, const char* what);
     if (_e != cudaSuccess) return ::sqdet::cuda_fail(_e, what);         \
   } while (0)
 
-
-// ---- programmatic dependent launch (PDL) --------------------------------------------------
-// The forward is a chain of ~20 kernels, each reading what the previous one wrote.  With the
-// programmatic-stream-serialization launch attribute a kernel may be SCHEDULED while its
-// predecessor still runs: its prologue (index math, parameter fetch) overlaps the predecessor's ragged last wave, and `griddepcontrol.wait` then holds every
-// thread until the predecessor has completed and flushed.  Every kernel of the forward calls
-// pdl_trigger() first (lets ITS successor be scheduled) and pdl_wait() before touching global
-// memory; both are no-ops for a plain launch.  The engine switches the attribute on per thread
-// around sqdet_forward (never for the first kernel, whose input comes from a copy).
-void set_pdl_launch(bool on);
-bool pdl_launch();
-
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                                 cudaStream_t stream, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  if (pdl_launch()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-  }
-  return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
-}
-
-#ifdef __CUDACC__
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-#endif
-
 // ---- TF NHWC geometry (SURVEY App. A.1; tf.nn.conv2d / tf.nn.max_pool) ------------------
 struct Geom {
   int out, pad_before, pad_after;

@@ -48,8 +48,6 @@ struct ConvPoolParams {
 template <int KS, int NT, int MINB>
 __global__ void __launch_bounds__(NT, MINB)
 conv_pool_simt_kernel(const ConvPoolParams p) {
-  pdl_trigger();
-  pdl_wait();
   constexpr int PH = 2 * (CT_H - 1) + KS;          // input patch rows
   constexpr int PW = 2 * (CT_W - 1) + KS;          // input patch cols (pixels)
   constexpr int K = KS * KS * 3;
@@ -203,6 +201,14 @@ size_t smem_bytes_for(int Cout) {
                           (size_t)(Cout / 16) * CT_PIX * 16);
 }
 
+// The <KS, NT, MINB> instantiations, indexed by conv_pool_instance.
+void (*const kConvPoolKernels[4])(ConvPoolParams) = {
+    conv_pool_simt_kernel<3, 256, 2>, conv_pool_simt_kernel<3, 384, 1>,
+    conv_pool_simt_kernel<7, 256, 1>, conv_pool_simt_kernel<7, 384, 1>};
+
+// Index of the kernel for a ksize x ksize conv on `threads` threads: the narrowest NT that holds them.
+int conv_pool_instance(int ksize, int threads) { return (ksize == 7 ? 2 : 0) + (threads > 256); }
+
 }  // namespace
 
 bool conv_pool_simt_eligible(int Cin, int Cout, int ksize, int stride, int pool_size,
@@ -234,26 +240,18 @@ int launch_conv_pool_simt(const float* x, const float* w, const float* bias, con
   const size_t smem = ksize == 3 ? smem_bytes_for<3>(Cout) : smem_bytes_for<7>(Cout);
   if (smem > 232448) return fail(SQDET_ERR_UNSUPPORTED, "conv+pool: tile does not fit in smem");
   // Exactly `threads` threads: each 64 of them own one 16-channel group (cg = tid >> 6), and
-  // s_conv / bias hold Cout / 16 groups.  NT_ is only the __launch_bounds__ ceiling.
-#define SQ_LAUNCH_CP(KS_, NT_, MINB_)                                                          \
-  do {                                                                                         \
-    /* the opt-in is per device: remember which devices of this process already have it */    \
-    static unsigned long long attr_devs = 0ull;                                                \
-    int dev_ = 0;                                                                              \
-    SQ_CUDA(cudaGetDevice(&dev_));                                                             \
-    if (dev_ >= 64 || !((attr_devs >> dev_) & 1ull)) {                                         \
-      SQ_CUDA(cudaFuncSetAttribute(conv_pool_simt_kernel<KS_, NT_, MINB_>,                     \
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));      \
-      if (dev_ < 64) attr_devs |= 1ull << dev_;                                                \
-    }                                                                                          \
-    SQ_CUDA(launch_kernel(conv_pool_simt_kernel<KS_, NT_, MINB_>, grid, dim3(threads), smem,    \
-                          stream, p));                                                         \
-  } while (0)
-  if (ksize == 3 && threads <= 256) SQ_LAUNCH_CP(3, 256, 2);
-  else if (ksize == 3) SQ_LAUNCH_CP(3, 384, 1);
-  else if (threads <= 256) SQ_LAUNCH_CP(7, 256, 1);
-  else SQ_LAUNCH_CP(7, 384, 1);
-#undef SQ_LAUNCH_CP
+  // s_conv / bias hold Cout / 16 groups.  The instance's NT is only the __launch_bounds__ ceiling.
+  const int inst = conv_pool_instance(ksize, threads);
+  // the opt-in is per device: remember which devices of this process already have it
+  static unsigned long long attr_devs[4] = {};
+  int dev = 0;
+  SQ_CUDA(cudaGetDevice(&dev));
+  if (dev >= 64 || !((attr_devs[inst] >> dev) & 1ull)) {
+    SQ_CUDA(cudaFuncSetAttribute(kConvPoolKernels[inst], cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 232448));
+    if (dev < 64) attr_devs[inst] |= 1ull << dev;
+  }
+  kConvPoolKernels[inst]<<<grid, threads, smem, stream>>>(p);
   SQ_CHECK_LAUNCH("conv_pool_simt_kernel");
   return SQDET_OK;
 }

@@ -24,8 +24,6 @@ conv_simt_kernel(const float* __restrict__ x, const float* __restrict__ w,
                  int B, int H, int W, int Cin, int Cout, int ksz, int stride,
                  int pad_t, int pad_l, int Ho, int Wo, int relu, int y_cstride,
                  int y_coff) {
-  pdl_trigger();
-  pdl_wait();
   __shared__ __align__(16) float As[BK][BM + 4];
   __shared__ __align__(16) float Bs[BK][BN];
 
@@ -165,16 +163,9 @@ int launch_conv_simt(const ConvArgs& a, cudaStream_t stream) {
   const bool vec4 = (a.Cin % 4 == 0) && (a.Cout % 4 == 0) &&
                     ((reinterpret_cast<uintptr_t>(a.x) & 15) == 0) &&
                     ((reinterpret_cast<uintptr_t>(a.w) & 15) == 0);
-  if (vec4)
-    SQ_CUDA(launch_kernel(conv_simt_kernel<true>, grid, dim3(NT), 0, stream,
-                          a.x, a.w, a.bias, a.scale, a.shift, a.y, a.B, a.H, a.W, a.Cin, a.Cout, a.size,
-                          a.stride, gh.pad_before, gw.pad_before, gh.out, gw.out, a.relu, a.y_cstride,
-                          a.y_coff));
-  else
-    SQ_CUDA(launch_kernel(conv_simt_kernel<false>, grid, dim3(NT), 0, stream,
-                          a.x, a.w, a.bias, a.scale, a.shift, a.y, a.B, a.H, a.W, a.Cin, a.Cout, a.size,
-                          a.stride, gh.pad_before, gw.pad_before, gh.out, gw.out, a.relu, a.y_cstride,
-                          a.y_coff));
+  (vec4 ? conv_simt_kernel<true> : conv_simt_kernel<false>)<<<grid, NT, 0, stream>>>(
+      a.x, a.w, a.bias, a.scale, a.shift, a.y, a.B, a.H, a.W, a.Cin, a.Cout, a.size, a.stride,
+      gh.pad_before, gw.pad_before, gh.out, gw.out, a.relu, a.y_cstride, a.y_coff);
   SQ_CHECK_LAUNCH("conv_simt_kernel");
   return SQDET_OK;
 }

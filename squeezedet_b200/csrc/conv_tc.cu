@@ -219,7 +219,6 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   constexpr int APITCH = KC + 4;
   constexpr int NACC = NT / 2;
   extern __shared__ __align__(128) float smem[];
-  pdl_trigger();
 
   const TcChunk& ch = p.chunks[blockIdx.y];
   const int tid = threadIdx.x;
@@ -271,7 +270,6 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
     for (int v = tid; v < NT * KC / 2; v += NUM_THREADS) cp_async16(wdst + v * 16, wsrc + 4 * v, true);
   };
 
-  pdl_wait();
   const int nk = ch.nk;
 #pragma unroll
   for (int s = 0; s < STAGES - 1; ++s) {
@@ -361,7 +359,6 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
   constexpr int RING = fire_ring_floats<KCI, SQN, KCE>();
   extern __shared__ __align__(128) float smem[];
   float* q = smem + STAGES * RING;
-  pdl_trigger();
 
   int tile = blockIdx.x;
   const int tx = tile % p.tiles_w;
@@ -386,7 +383,6 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
     for (int v = tid; v < SQN * KCI / 2; v += NUM_THREADS) cp_async16(smem_u32(st) + v * 16, wsrc + 4 * v, true);
   };
 
-  pdl_wait();
   // ---- squeeze
   const int nks = p.Cin / KCI;
 #pragma unroll
@@ -492,14 +488,44 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
 
 // ---------------------------------------------------------------------------------------------
 // Host side
-struct ConvGroup {   // one conv reading the shared input
-  int ksize, Cout, y_off;
-};
+using ConvKernel = void (*)(TcParams);
+using FireKernel = void (*)(FireParams);
+
+template <int KC, bool GATHER>
+ConvKernel conv_tc_instance(int NT) {
+  return NT == 64 ? conv_tc_kernel<64, KC, GATHER>
+         : NT == 32 ? conv_tc_kernel<32, KC, GATHER> : conv_tc_kernel<16, KC, GATHER>;
+}
+
+// The conv_tc_kernel instantiation of a plan (gather mode always walks K in chunks of 32).
+ConvKernel conv_tc_instance(int NT, int KC, bool gather) {
+  if (gather) return conv_tc_instance<32, true>(NT);
+  return KC == 32 ? conv_tc_instance<32, false>(NT) : conv_tc_instance<16, false>(NT);
+}
+
+template <int KCI, int SQN, int KCE>
+FireKernel fire_tc_instance(size_t* smem) {
+  *smem = sizeof(float) * ((size_t)STAGES * fire_ring_floats<KCI, SQN, KCE>() + FQ_ROWS * (SQN + 4));
+  return fire_tc_kernel<KCI, SQN, KCE>;
+}
+
+// The fire_tc_kernel instantiation for (KCI, SQN, KCE) and its dynamic shared memory in bytes.
+// S = 16, 32, 48, 64 -> SQN 16, 32, 64, 64 and KCE the largest of 32 / 16 dividing S.
+FireKernel fire_tc_instance(int KCI, int SQN, int KCE, size_t* smem) {
+  if (KCI == 32) {
+    if (SQN == 16) return fire_tc_instance<32, 16, 16>(smem);
+    if (SQN == 32) return fire_tc_instance<32, 32, 32>(smem);
+    return KCE == 16 ? fire_tc_instance<32, 64, 16>(smem) : fire_tc_instance<32, 64, 32>(smem);
+  }
+  if (SQN == 16) return fire_tc_instance<16, 16, 16>(smem);
+  if (SQN == 32) return fire_tc_instance<16, 32, 32>(smem);
+  return KCE == 16 ? fire_tc_instance<16, 64, 16>(smem) : fire_tc_instance<16, 64, 32>(smem);
+}
 
 struct TcImpl {
   TcParams prm{};
   int NT = 0, KC = 0;
-  bool gather = false;
+  ConvKernel kernel = nullptr;
   dim3 grid;
   size_t smem_bytes = 0;
   std::vector<ConvGroup> groups;
@@ -536,12 +562,6 @@ static int pick_nt(const std::vector<ConvGroup>& groups) {
   return best;
 }
 
-template <int NT, int KC, bool GATHER>
-static cudaError_t set_smem(size_t bytes) {
-  return cudaFuncSetAttribute(conv_tc_kernel<NT, KC, GATHER>,
-                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-}
-
 static void release_impl(void** impl) {
   if (!*impl) return;
   TcImpl* im = static_cast<TcImpl*>(*impl);
@@ -566,7 +586,7 @@ static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo,
   if (M <= 0 || mtiles > 0x7fffffffLL) return 0;
   im->NT = NT;
   im->KC = KC;
-  im->gather = gather;
+  im->kernel = conv_tc_instance(NT, KC, gather);
   im->groups = groups;
   TcParams& p = im->prm;
   p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Ho = Ho; p.Wo = Wo; p.stride = stride;
@@ -595,17 +615,8 @@ static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo,
   im->w_floats = woff;
   im->grid = dim3((unsigned)mtiles, (unsigned)nch);
   im->smem_bytes = (size_t)STAGES * (TILE_M * (KC + 4) + 2 * NT * KC) * sizeof(float);
-  cudaError_t ce = cudaSuccess;
-  if (gather) {
-    ce = NT == 64 ? set_smem<64, 32, true>(im->smem_bytes)
-                  : NT == 32 ? set_smem<32, 32, true>(im->smem_bytes) : set_smem<16, 32, true>(im->smem_bytes);
-  } else if (KC == 32) {
-    ce = NT == 64 ? set_smem<64, 32, false>(im->smem_bytes)
-                  : NT == 32 ? set_smem<32, 32, false>(im->smem_bytes) : set_smem<16, 32, false>(im->smem_bytes);
-  } else {
-    ce = NT == 64 ? set_smem<64, 16, false>(im->smem_bytes)
-                  : NT == 32 ? set_smem<32, 16, false>(im->smem_bytes) : set_smem<16, 16, false>(im->smem_bytes);
-  }
+  cudaError_t ce = cudaFuncSetAttribute(im->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)im->smem_bytes);
   if (ce != cudaSuccess) return cuda_fail(ce, "cudaFuncSetAttribute(conv_tc_kernel)");
   SQ_CUDA(cudaMalloc(&im->d_w, sizeof(float) * (size_t)woff));
   SQ_CUDA(cudaMalloc(&im->d_bias, sizeof(float) * poff));
@@ -654,40 +665,12 @@ static void pack_group(const TcImpl* im, int gi, const float* w_hwio, std::vecto
   }
 }
 
-static int upload_weights(TcImpl* im, const std::vector<const float*>& w_hwio) {
-  std::vector<float> packed((size_t)im->w_floats, 0.f);
-  for (int gi = 0; gi < (int)im->groups.size(); ++gi) pack_group(im, gi, w_hwio[gi], packed);
-  SQ_CUDA(cudaMemcpy(im->d_w, packed.data(), packed.size() * sizeof(float), cudaMemcpyHostToDevice));
-  return SQDET_OK;
-}
-
-static int launch_impl(const TcImpl* im, const float* x_dev, float* y_dev, cudaStream_t stream) {
-  TcParams prm = im->prm;
-  prm.x = x_dev;
-  prm.y = y_dev;
-  const dim3 block(NUM_THREADS);
-  const size_t sm = im->smem_bytes;
-  cudaError_t ce;
-  if (im->gather)
-    ce = im->NT == 64 ? launch_kernel(conv_tc_kernel<64, 32, true>, im->grid, block, sm, stream, prm)
-         : im->NT == 32 ? launch_kernel(conv_tc_kernel<32, 32, true>, im->grid, block, sm, stream, prm)
-                        : launch_kernel(conv_tc_kernel<16, 32, true>, im->grid, block, sm, stream, prm);
-  else if (im->KC == 32)
-    ce = im->NT == 64 ? launch_kernel(conv_tc_kernel<64, 32, false>, im->grid, block, sm, stream, prm)
-         : im->NT == 32 ? launch_kernel(conv_tc_kernel<32, 32, false>, im->grid, block, sm, stream, prm)
-                        : launch_kernel(conv_tc_kernel<16, 32, false>, im->grid, block, sm, stream, prm);
-  else
-    ce = im->NT == 64 ? launch_kernel(conv_tc_kernel<64, 16, false>, im->grid, block, sm, stream, prm)
-         : im->NT == 32 ? launch_kernel(conv_tc_kernel<32, 16, false>, im->grid, block, sm, stream, prm)
-                        : launch_kernel(conv_tc_kernel<16, 16, false>, im->grid, block, sm, stream, prm);
-  if (ce != cudaSuccess) return cuda_fail(ce, "launch conv_tc_kernel");
-  return SQDET_OK;
-}
-
 // ---- one-kernel fire module: host state -----------------------------
 struct FusedImpl {
   FireParams fp{};
   int KCI = 0, SQN = 0, KCE = 0;
+  int E1 = 0, E3 = 0;
+  FireKernel kernel = nullptr;
   unsigned grid = 0;
   size_t smem = 0;
   float* d_w = nullptr;    // squeeze tiles
@@ -705,20 +688,6 @@ static void release_fused(void** impl) {
   *impl = nullptr;
 }
 
-// (KCI, SQN, KCE) of the squeeze width S: S = 16, 32, 48, 64 -> SQN 16, 32, 64, 64 and KCE the
-// largest of 32 / 16 dividing S
-#define SQ_FIRE_DISPATCH(KCI_, SQN_, KCE_, CALL)                                              \
-  do {                                                                                          \
-    if (KCI_ == 32 && SQN_ == 16) CALL(32, 16, 16);                                             \
-    else if (KCI_ == 32 && SQN_ == 32) CALL(32, 32, 32);                                        \
-    else if (KCI_ == 32 && SQN_ == 64 && KCE_ == 16) CALL(32, 64, 16);                          \
-    else if (KCI_ == 32) CALL(32, 64, 32);                                                      \
-    else if (SQN_ == 16) CALL(16, 16, 16);                                                      \
-    else if (SQN_ == 32) CALL(16, 32, 32);                                                      \
-    else if (KCE_ == 16) CALL(16, 64, 16);                                                      \
-    else CALL(16, 64, 32);                                                                      \
-  } while (0)
-
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
@@ -728,100 +697,71 @@ bool tc_conv_eligible(int Cin, int Cout, int size, int stride, int padding) {
   return Cin % 16 == 0 && Cin >= 16 && Cout > 0;
 }
 
-int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, int Cout, int size, int stride,
-                 int padding, int relu, bool has_affine, int y_cstride, int y_coff) {
-  plan->enabled = false;
-  const bool gather = Cin == 3 && size == 3 && (stride == 1 || stride == 2) && Cout > 0;
-  if (!gather && !tc_conv_eligible(Cin, Cout, size, stride, padding)) return 0;
+int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, const std::vector<ConvGroup>& convs,
+                 int stride, int padding, int relu, bool has_affine, int y_cstride) {
+  plan->impl = nullptr;
+  const int size = convs[0].ksize;
+  const bool gather = convs.size() == 1 && Cin == 3 && size == 3 && (stride == 1 || stride == 2) &&
+                      convs[0].Cout > 0;
+  if (!gather)
+    for (const auto& g : convs)
+      if (!tc_conv_eligible(Cin, g.Cout, g.ksize, stride, padding)) return 0;
   const Geom gh = tf_geometry(H, size, stride, padding);
   const Geom gw = tf_geometry(W, size, stride, padding);
   if (gh.out <= 0 || gw.out <= 0) return 0;
-  TcImpl* im = new TcImpl();
-  int rc = plan_common(im, B, H, W, Cin, gh.out, gw.out, stride, gh.pad_before, gw.pad_before,
-                       gather, {{size, Cout, y_coff}}, relu, has_affine, y_cstride);
+  void* im = new TcImpl();
+  int rc = plan_common(static_cast<TcImpl*>(im), B, H, W, Cin, gh.out, gw.out, stride,
+                       gh.pad_before, gw.pad_before, gather, convs, relu, has_affine, y_cstride);
   if (rc <= 0) {
-    void* p = im;
-    release_impl(&p);
+    release_impl(&im);
     return rc;
   }
-  plan->enabled = true;
-  plan->B = B; plan->H = H; plan->W = W; plan->Cin = Cin; plan->Cout = Cout;
-  plan->size = size; plan->stride = stride; plan->relu = relu;
-  plan->Ho = gh.out; plan->Wo = gw.out; plan->pad_t = gh.pad_before; plan->pad_l = gw.pad_before;
-  plan->y_cstride = y_cstride; plan->y_coff = y_coff;
   plan->impl = im;
   return 1;
 }
 
-int tc_fire_plan(TcFirePlan* plan, int B, int H, int W, int S, int E1, int E3) {
-  plan->enabled = false;
-  if (!tc_conv_eligible(S, E1, 1, 1, SQDET_PAD_SAME) || !tc_conv_eligible(S, E3, 3, 1, SQDET_PAD_SAME))
-    return 0;
-  TcImpl* im = new TcImpl();
-  int rc = plan_common(im, B, H, W, S, H, W, 1, 0, 0, false, {{1, E1, 0}, {3, E3, E1}}, 1, false,
-                       E1 + E3);
-  if (rc <= 0) {
-    void* p = im;
-    release_impl(&p);
-    return rc;
-  }
-  plan->enabled = true;
-  plan->B = B; plan->H = H; plan->W = W; plan->S = S; plan->E1 = E1; plan->E3 = E3;
-  plan->impl = im;
-  return 1;
-}
-
-int tc_conv_pack_weights(TcConvPlan* plan, const float* w_hwio, const float* bias) {
+int tc_conv_pack_weights(TcConvPlan* plan, const std::vector<const float*>& w_hwio,
+                         const std::vector<const float*>& bias) {
   TcImpl* im = static_cast<TcImpl*>(plan->impl);
-  int rc = upload_weights(im, {w_hwio});
-  if (rc) return rc;
-  if (bias) SQ_CUDA(cudaMemcpy(im->d_bias, bias, sizeof(float) * plan->Cout, cudaMemcpyHostToDevice));
+  std::vector<float> packed((size_t)im->w_floats, 0.f);
+  for (int gi = 0; gi < (int)im->groups.size(); ++gi) pack_group(im, gi, w_hwio[gi], packed);
+  SQ_CUDA(cudaMemcpy(im->d_w, packed.data(), packed.size() * sizeof(float), cudaMemcpyHostToDevice));
+  int off = 0;
+  for (int gi = 0; gi < (int)im->groups.size(); ++gi) {
+    const int n = im->groups[gi].Cout;
+    if (bias[gi]) SQ_CUDA(cudaMemcpy(im->d_bias + off, bias[gi], sizeof(float) * n, cudaMemcpyHostToDevice));
+    off += n;
+  }
   return SQDET_OK;
 }
 
 int tc_conv_set_affine(TcConvPlan* plan, const float* scale, const float* shift) {
   TcImpl* im = static_cast<TcImpl*>(plan->impl);
   if (!im->d_scale) return fail(SQDET_ERR_STATE, "tc conv planned without an affine epilogue");
-  SQ_CUDA(cudaMemcpy(im->d_scale, scale, sizeof(float) * plan->Cout, cudaMemcpyHostToDevice));
-  SQ_CUDA(cudaMemcpy(im->d_shift, shift, sizeof(float) * plan->Cout, cudaMemcpyHostToDevice));
-  return SQDET_OK;
-}
-
-int tc_fire_pack_weights(TcFirePlan* plan, const float* w_e1, const float* b_e1, const float* w_e3,
-                         const float* b_e3) {
-  TcImpl* im = static_cast<TcImpl*>(plan->impl);
-  int rc = upload_weights(im, {w_e1, w_e3});
-  if (rc) return rc;
-  SQ_CUDA(cudaMemcpy(im->d_bias, b_e1, sizeof(float) * plan->E1, cudaMemcpyHostToDevice));
-  SQ_CUDA(cudaMemcpy(im->d_bias + plan->E1, b_e3, sizeof(float) * plan->E3, cudaMemcpyHostToDevice));
+  SQ_CUDA(cudaMemcpy(im->d_scale, scale, sizeof(float) * im->cout_total, cudaMemcpyHostToDevice));
+  SQ_CUDA(cudaMemcpy(im->d_shift, shift, sizeof(float) * im->cout_total, cudaMemcpyHostToDevice));
   return SQDET_OK;
 }
 
 int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, cudaStream_t stream) {
-  return launch_impl(static_cast<const TcImpl*>(plan.impl), x_dev, y_dev, stream);
+  const TcImpl* im = static_cast<const TcImpl*>(plan.impl);
+  TcParams prm = im->prm;
+  prm.x = x_dev;
+  prm.y = y_dev;
+  im->kernel<<<im->grid, NUM_THREADS, im->smem_bytes, stream>>>(prm);
+  SQ_CHECK_LAUNCH("conv_tc_kernel");
+  return SQDET_OK;
 }
 
-int launch_fire_expand_tc(const TcFirePlan& plan, const float* q_dev, float* y_dev,
-                          cudaStream_t stream) {
-  return launch_impl(static_cast<const TcImpl*>(plan.impl), q_dev, y_dev, stream);
-}
-
-void tc_conv_release(TcConvPlan* plan) {
-  release_impl(&plan->impl);
-  plan->enabled = false;
-}
-void tc_fire_release(TcFirePlan* plan) {
-  release_impl(&plan->impl);
-  plan->enabled = false;
-}
+void tc_conv_release(TcConvPlan* plan) { release_impl(&plan->impl); }
 
 int conv2d_tc_oneshot(const float* x_dev, const float* w_hwio_dev, const float* bias_dev,
                       const float* scale_dev, const float* shift_dev, float* y_dev, int B, int H,
                       int W, int Cin, int Cout, int size, int stride, int padding, int relu,
                       int y_cstride, int y_coff, cudaStream_t stream) {
   TcConvPlan plan;
-  int rc = tc_conv_plan(&plan, B, H, W, Cin, Cout, size, stride, padding, relu,
-                        scale_dev != nullptr, y_cstride, y_coff);
+  int rc = tc_conv_plan(&plan, B, H, W, Cin, {{size, Cout, y_coff}}, stride, padding, relu,
+                        scale_dev != nullptr, y_cstride);
   if (rc < 0) return rc;
   if (rc == 0) {
     // shape not taken by the tensor-core path (e.g. a strided conv): same dispatch as the engine
@@ -844,7 +784,7 @@ int conv2d_tc_oneshot(const float* x_dev, const float* w_hwio_dev, const float* 
     tc_conv_release(&plan);
     return cuda_fail(ce, "conv2d_tc_oneshot: parameter download");
   }
-  rc = tc_conv_pack_weights(&plan, w.data(), bias_dev ? b.data() : nullptr);
+  rc = tc_conv_pack_weights(&plan, {w.data()}, {bias_dev ? b.data() : nullptr});
   if (!rc && scale_dev) rc = tc_conv_set_affine(&plan, sc.data(), sh.data());
   if (!rc) rc = launch_conv_tc(plan, x_dev, y_dev, stream);
   ce = cudaStreamSynchronize(stream);
@@ -856,7 +796,7 @@ int conv2d_tc_oneshot(const float* x_dev, const float* w_hwio_dev, const float* 
 
 // ---- one-kernel fire module ----------------------------------------------------------------------
 int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int S, int E1, int E3) {
-  plan->enabled = false;
+  plan->impl = nullptr;
   if (Cin % 16 || Cin < 16 || S % 16 || S < 16 || S > 64 || E1 <= 0 || E3 <= 0) return 0;
   const int nch = (E1 + 63) / 64 + (E3 + 63) / 64;
   if (nch > MAX_FCHUNKS) return 0;
@@ -864,6 +804,8 @@ int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int 
   im->KCI = Cin % 32 == 0 ? 32 : 16;
   im->SQN = S <= 16 ? 16 : S <= 32 ? 32 : 64;
   im->KCE = S % 32 == 0 ? 32 : 16;
+  im->E1 = E1;
+  im->E3 = E3;
   FireParams& p = im->fp;
   p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.S = S; p.Etot = E1 + E3;
   p.tiles_w = (W + FT_W - 1) / FT_W;
@@ -879,14 +821,10 @@ int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int 
   }
   im->w_floats = (long long)(Cin / im->KCI) * 2 * im->SQN * im->KCI;
   im->grid = (unsigned)((long long)B * p.tiles_h * p.tiles_w);
-  cudaError_t ce = cudaSuccess;
-#define SQ_FIRE_SMEM(A, Bq, C)                                                                  \
-  (im->smem = sizeof(float) * ((size_t)STAGES * fire_ring_floats<A, Bq, C>() + FQ_ROWS * (Bq + 4)), \
-   ce = cudaFuncSetAttribute(fire_tc_kernel<A, Bq, C>,                                           \
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)im->smem))
-  SQ_FIRE_DISPATCH(im->KCI, im->SQN, im->KCE, SQ_FIRE_SMEM);
-#undef SQ_FIRE_SMEM
+  im->kernel = fire_tc_instance(im->KCI, im->SQN, im->KCE, &im->smem);
   void* vp = im;
+  cudaError_t ce = cudaFuncSetAttribute(im->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)im->smem);
   if (ce != cudaSuccess) {
     release_fused(&vp);
     return cuda_fail(ce, "cudaFuncSetAttribute(fire_tc_kernel)");
@@ -899,8 +837,6 @@ int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int 
     return cuda_fail(ce, "cudaMalloc(fused fire)");
   }
   p.wsq = im->d_w; p.wex = im->d_w2; p.bsq = im->d_b; p.bex = im->d_b2;
-  plan->enabled = true;
-  plan->B = B; plan->H = H; plan->W = W; plan->Cin = Cin; plan->S = S; plan->E1 = E1; plan->E3 = E3;
   plan->impl = im;
   return 1;
 }
@@ -917,13 +853,13 @@ int tc_fused_fire_pack_weights(TcFusedFirePlan* plan, const float* w_sq, const f
   for (int c = 0; c < p.nchunks; ++c) {
     const FireChunk& ch = p.chunks[c];
     const bool e3 = ch.taps == 9;
-    pack_tiles(e3 ? w_e3 : w_e1, (long long)ch.taps * p.S, e3 ? plan->E3 : plan->E1,
-               ch.y_off - (e3 ? plan->E1 : 0), 64, im->KCE, ch.nk, wex.data() + off);
+    pack_tiles(e3 ? w_e3 : w_e1, (long long)ch.taps * p.S, e3 ? im->E3 : im->E1,
+               ch.y_off - (e3 ? im->E1 : 0), 64, im->KCE, ch.nk, wex.data() + off);
     off += (long long)ch.nk * 2 * 64 * im->KCE;
   }
   for (int i = 0; i < p.S; ++i) bsq[i] = b_sq[i];
-  bex.assign(b_e1, b_e1 + plan->E1);
-  bex.insert(bex.end(), b_e3, b_e3 + plan->E3);
+  bex.assign(b_e1, b_e1 + im->E1);
+  bex.insert(bex.end(), b_e3, b_e3 + im->E3);
   SQ_CUDA(cudaMemcpy(im->d_w, wsq.data(), wsq.size() * sizeof(float), cudaMemcpyHostToDevice));
   SQ_CUDA(cudaMemcpy(im->d_w2, wex.data(), wex.size() * sizeof(float), cudaMemcpyHostToDevice));
   SQ_CUDA(cudaMemcpy(im->d_b, bsq.data(), bsq.size() * sizeof(float), cudaMemcpyHostToDevice));
@@ -937,19 +873,12 @@ int launch_fused_fire_tc(const TcFusedFirePlan& plan, const float* x_dev, float*
   FireParams p = im->fp;
   p.x = x_dev;
   p.y = y_dev;
-  cudaError_t ce = cudaSuccess;
-#define SQ_FIRE_LAUNCH(A, Bq, C) \
-  ce = launch_kernel(fire_tc_kernel<A, Bq, C>, dim3(im->grid), dim3(NUM_THREADS), im->smem, stream, p)
-  SQ_FIRE_DISPATCH(im->KCI, im->SQN, im->KCE, SQ_FIRE_LAUNCH);
-#undef SQ_FIRE_LAUNCH
-  if (ce != cudaSuccess) return cuda_fail(ce, "launch fire_tc_kernel");
+  im->kernel<<<im->grid, NUM_THREADS, im->smem, stream>>>(p);
+  SQ_CHECK_LAUNCH("fire_tc_kernel");
   return SQDET_OK;
 }
 
-void tc_fused_fire_release(TcFusedFirePlan* plan) {
-  release_fused(&plan->impl);
-  plan->enabled = false;
-}
+void tc_fused_fire_release(TcFusedFirePlan* plan) { release_fused(&plan->impl); }
 
 int fire_fused_oneshot(const float* x_dev, const float* w_sq_dev, const float* b_sq_dev,
                        const float* w_e1_dev, const float* b_e1_dev, const float* w_e3_dev,

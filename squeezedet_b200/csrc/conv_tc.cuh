@@ -3,47 +3,39 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <vector>
+
 namespace sqdet {
 
-// One convolution executed as an implicit GEMM on wgmma with the 3xTF32 split.
-struct TcConvPlan {
-  bool enabled = false;
-  int B = 0, H = 0, W = 0, Cin = 0, Cout = 0, size = 1, stride = 1, relu = 1;
-  int Ho = 0, Wo = 0, pad_t = 0, pad_l = 0;
-  int y_cstride = 0, y_coff = 0;
-  void* impl = nullptr;          // opaque device/host state (packed weights, launch parameters)
+// One conv of an implicit-GEMM launch: all convs of a launch read the same input and write
+// channels [y_off, y_off + Cout) of the same output.
+struct ConvGroup {
+  int ksize, Cout, y_off;
 };
 
-// The expand pair of a fire module (1x1 || 3x3 on the same squeeze tensor) as one launch
-// writing the channel-concatenated output.
-struct TcFirePlan {
-  bool enabled = false;
-  int B = 0, H = 0, W = 0, S = 0, E1 = 0, E3 = 0;
-  void* impl = nullptr;
+// Convs over one input executed as one implicit GEMM on wgmma with the 3xTF32 split: a single
+// conv, or a fire module's expand pair (1x1 || 3x3 on the squeeze tensor) writing the
+// channel-concatenated output.  A null impl means "not planned".
+struct TcConvPlan {
+  void* impl = nullptr;          // opaque device/host state (packed weights, launch parameters)
 };
 
 bool tc_conv_eligible(int Cin, int Cout, int size, int stride, int padding);
 
-// Returns 1 when the shape is taken by the tensor-core path (plan->enabled), 0 when it is
-// left to the fp32 SIMT kernel, negative on error.
-int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, int Cout, int size, int stride,
-                 int padding, int relu, bool has_affine, int y_cstride, int y_coff);
-int tc_fire_plan(TcFirePlan* plan, int B, int H, int W, int S, int E1, int E3);
-int tc_conv_pack_weights(TcConvPlan* plan, const float* w_hwio, const float* bias);
+// Returns 1 when the tensor-core path takes the convs (plan->impl set), 0 when they are left to
+// the fp32 SIMT kernel, negative on error.  Gather mode (3-channel input) takes a single conv.
+int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, const std::vector<ConvGroup>& convs,
+                 int stride, int padding, int relu, bool has_affine, int y_cstride);
+// HWIO weights and bias (or null) of each planned conv, in plan order.
+int tc_conv_pack_weights(TcConvPlan* plan, const std::vector<const float*>& w_hwio,
+                         const std::vector<const float*>& bias);
 int tc_conv_set_affine(TcConvPlan* plan, const float* scale, const float* shift);
-int tc_fire_pack_weights(TcFirePlan* plan, const float* w_e1, const float* b_e1,
-                         const float* w_e3, const float* b_e3);
 int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, cudaStream_t stream);
-int launch_fire_expand_tc(const TcFirePlan& plan, const float* q_dev, float* y_dev,
-                          cudaStream_t stream);
 void tc_conv_release(TcConvPlan* plan);
-void tc_fire_release(TcFirePlan* plan);
 
 // The whole fire module (squeeze 1x1 -> expand 1x1 || 3x3 + concat) as ONE kernel: the squeeze
 // tile of each 8 x 16 output tile stays in shared memory.  Cin % 16 == 0, S in {16, 32, 48, 64}.
 struct TcFusedFirePlan {
-  bool enabled = false;
-  int B = 0, H = 0, W = 0, Cin = 0, S = 0, E1 = 0, E3 = 0;
   void* impl = nullptr;
 };
 int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int S, int E1, int E3);

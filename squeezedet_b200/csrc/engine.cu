@@ -30,9 +30,6 @@ static thread_local std::string g_last_error;
 
 void set_error(const std::string& msg) { g_last_error = msg; }
 
-static thread_local bool g_pdl_launch = false;
-void set_pdl_launch(bool on) { g_pdl_launch = on; }
-bool pdl_launch() { return g_pdl_launch; }
 int fail(int code, const std::string& msg) {
   g_last_error = msg;
   return code;
@@ -74,7 +71,18 @@ struct ConvSpec {
   int p_kernel = -1, p_bias = -1, p_gamma = -1, p_beta = -1, p_mean = -1, p_var = -1;
   float* scale = nullptr;      // device, BN only
   float* shift = nullptr;
-  TcConvPlan tc;               // tensor-core plan (valid when tc.enabled)
+};
+
+enum LaunchKind { L_CONV_SIMT, L_CONV_TC, L_CONV_POOL, L_FIRE_TC, L_MAXPOOL, L_ADD_RELU };
+
+// One kernel launch of an op.
+struct Launch {
+  LaunchKind kind;
+  int src = -1, dst = -1;        // tensor read (add+ReLU also reads the op's src2) and written
+  int conv = 0, nconv = 0;       // computes the op's convs [conv, conv + nconv)
+  int pool_padding = 0;          // L_CONV_POOL: padding of the absorbed 3x3/2 max-pool
+  TcConvPlan tc;                 // L_CONV_TC
+  TcFusedFirePlan fire;          // L_FIRE_TC
 };
 
 struct Op {
@@ -84,13 +92,7 @@ struct Op {
   int src = -1, src2 = -1, dst = -1;
   int size = 0, stride = 0, padding = 0;
   int64_t flops = 0, params = 0, min_bytes = 0;
-  int launches = 0;
-  TcFirePlan tcfire;             // fused expand pair (valid when tcfire.enabled)
-  TcFusedFirePlan fused;         // whole fire module in one kernel (valid when fused.enabled)
-  bool skip = false;             // pool op whose work happens in the producer's epilogue
-  int fused_pool_op = -1;        // index of the pool op fused into this conv / fire
-  bool first_layer_fused = false;  // Cin=3 stride-2 conv + 3x3/2 pool as one FFMA kernel
-  int out = -1;                  // tensor actually written (dst, or the fused pool's dst)
+  std::vector<Launch> launches;  // what the op runs, in order; empty for a pool its producer absorbed
 };
 
 }  // namespace sqdet
@@ -100,6 +102,7 @@ using namespace sqdet;
 struct sqdet_engine {
   sqdet_config cfg;
   int device = 0;
+  int sms = 0;                    // the device's SM count
   bool finalized = false;
   bool params_dirty = true;
   std::vector<Tensor> tensors;
@@ -250,69 +253,89 @@ static void conv_cost(const sqdet_engine* e, const ConvSpec& c, int Ho, int Wo, 
   op->params += (int64_t)(1 + c.size * c.size * c.Cin) * c.Cout;
 }
 
-static int run_conv(sqdet_engine* e, const ConvSpec& c, const float* x_override,
-                    cudaStream_t stream) {
-  const Tensor& in = e->tensors[c.src];
-  const Tensor& out = e->tensors[c.dst];
-  const float* x = (c.src == 0 && x_override) ? x_override : in.dev;
-  if (c.tc.enabled) return launch_conv_tc(c.tc, x, out.dev, stream);
-  ConvArgs a;
-  a.x = x;
-  a.w = e->params[c.p_kernel].dev;
-  a.bias = c.p_bias >= 0 ? e->params[c.p_bias].dev : nullptr;
-  a.scale = c.scale;
-  a.shift = c.shift;
-  a.y = out.dev;
-  a.B = in.B; a.H = in.H; a.W = in.W; a.Cin = c.Cin; a.Cout = c.Cout;
-  a.size = c.size; a.stride = c.stride; a.padding = c.padding; a.relu = c.relu;
-  a.y_cstride = out.C;
-  a.y_coff = c.y_coff;
-  return launch_conv_simt(a, stream);
+// sqdet_add_conv / sqdet_add_conv_bn: one conv op and its output tensor.
+static int add_conv_op(sqdet_engine* e, const char* what, const char* name, int src, int filters,
+                       int size, int stride, int padding, int relu, bool bn, bool with_bias,
+                       int* out) {
+  int rc = check_build(e, src);
+  if (rc) return rc;
+  if (!name || !out) return fail(SQDET_ERR_INVALID_ARG, std::string(what) + ": null argument");
+  Op op;
+  op.kind = OP_CONV;
+  op.name = name;
+  ConvSpec cs;
+  int Ho, Wo;
+  rc = make_conv(e, name, src, filters, size, stride, padding, relu, bn, with_bias, &cs, &Ho, &Wo);
+  if (rc) return rc;
+  cs.dst = new_tensor(e, name, e->tensors[src].B, Ho, Wo, filters);
+  conv_cost(e, cs, Ho, Wo, &op);
+  op.src = src;
+  op.dst = cs.dst;
+  op.convs.push_back(cs);
+  e->ops.push_back(op);
+  *out = cs.dst;
+  return SQDET_OK;
 }
 
-static int run_op(sqdet_engine* e, const Op& op, const float* x_override, cudaStream_t stream) {
-  if (op.skip) return SQDET_OK;
-  switch (op.kind) {
-    case OP_CONV:
-      if (op.first_layer_fused) {
-        const ConvSpec& c = op.convs[0];
-        const Op& po = e->ops[op.fused_pool_op];
-        const Tensor& in = e->tensors[c.src];
-        const float* x = (c.src == 0 && x_override) ? x_override : in.dev;
-        return launch_conv_pool_simt(x, e->params[c.p_kernel].dev,
-                                     c.p_bias >= 0 ? e->params[c.p_bias].dev : nullptr, c.scale,
-                                     c.shift, e->tensors[op.out].dev, in.B, in.H, in.W, c.Cout,
-                                     c.size, c.padding, c.relu, po.padding, stream);
-      }
-      return run_conv(e, op.convs[0], x_override, stream);
-    case OP_FIRE: {
-      if (op.fused.enabled) {
-        const ConvSpec& sq = op.convs[0];
-        const float* x = (sq.src == 0 && x_override) ? x_override : e->tensors[sq.src].dev;
-        return launch_fused_fire_tc(op.fused, x, e->tensors[op.out].dev, stream);
-      }
-      int rc = run_conv(e, op.convs[0], x_override, stream);
-      if (rc) return rc;
-      if (op.tcfire.enabled)
-        return launch_fire_expand_tc(op.tcfire, e->tensors[op.convs[1].src].dev,
-                                     e->tensors[op.out].dev, stream);
-      rc = run_conv(e, op.convs[1], nullptr, stream);
-      if (rc) return rc;
-      return run_conv(e, op.convs[2], nullptr, stream);
+// Tensor `t` as the forward reads it: the caller's images stand in for tensor 0.
+static const float* input_ptr(const sqdet_engine* e, int t, const float* images) {
+  return (t == 0 && images) ? images : e->tensors[t].dev;
+}
+
+static int run_launch(sqdet_engine* e, const Op& op, const Launch& l, const float* images,
+                      cudaStream_t stream) {
+  const Tensor& in = e->tensors[l.src];
+  const float* x = input_ptr(e, l.src, images);
+  float* y = e->tensors[l.dst].dev;
+  switch (l.kind) {
+    case L_CONV_SIMT: {
+      const ConvSpec& c = op.convs[l.conv];
+      ConvArgs a;
+      a.x = x;
+      a.w = e->params[c.p_kernel].dev;
+      a.bias = c.p_bias >= 0 ? e->params[c.p_bias].dev : nullptr;
+      a.scale = c.scale;
+      a.shift = c.shift;
+      a.y = y;
+      a.B = in.B; a.H = in.H; a.W = in.W; a.Cin = c.Cin; a.Cout = c.Cout;
+      a.size = c.size; a.stride = c.stride; a.padding = c.padding; a.relu = c.relu;
+      a.y_cstride = e->tensors[l.dst].C;
+      a.y_coff = c.y_coff;
+      return launch_conv_simt(a, stream);
     }
-    case OP_POOL: {
-      const Tensor& in = e->tensors[op.src];
-      const float* x = (op.src == 0 && x_override) ? x_override : in.dev;
-      return launch_maxpool(x, e->tensors[op.dst].dev, in.B, in.H, in.W, in.C, op.size,
-                            op.stride, op.padding, stream);
+    case L_CONV_TC:
+      return launch_conv_tc(l.tc, x, y, stream);
+    case L_CONV_POOL: {
+      const ConvSpec& c = op.convs[0];
+      return launch_conv_pool_simt(x, e->params[c.p_kernel].dev,
+                                   c.p_bias >= 0 ? e->params[c.p_bias].dev : nullptr, c.scale,
+                                   c.shift, y, in.B, in.H, in.W, c.Cout, c.size, c.padding, c.relu,
+                                   l.pool_padding, stream);
     }
-    case OP_ADD_RELU: {
-      const Tensor& a = e->tensors[op.src];
-      return launch_add_relu(a.dev, e->tensors[op.src2].dev, e->tensors[op.dst].dev,
-                             a.numel(), stream);
-    }
+    case L_FIRE_TC:
+      return launch_fused_fire_tc(l.fire, x, y, stream);
+    case L_MAXPOOL:
+      return launch_maxpool(x, y, in.B, in.H, in.W, in.C, op.size, op.stride, op.padding, stream);
+    case L_ADD_RELU:
+      return launch_add_relu(x, input_ptr(e, op.src2, images), y, in.numel(), stream);
   }
-  return fail(SQDET_ERR_STATE, "unknown op kind");
+  return fail(SQDET_ERR_STATE, "unknown launch kind");
+}
+
+static int run_op(sqdet_engine* e, const Op& op, const float* images, cudaStream_t stream) {
+  for (const Launch& l : op.launches) {
+    int rc = run_launch(e, op, l, images, stream);
+    if (rc) return rc;
+  }
+  return SQDET_OK;
+}
+
+static void release_launches(Op& op) {
+  for (auto& l : op.launches) {
+    tc_conv_release(&l.tc);
+    tc_fused_fire_release(&l.fire);
+  }
+  op.launches.clear();
 }
 
 // ---- NCCL, bound at run time (dlopen): the library must load on boxes without NCCL ----------
@@ -366,20 +389,28 @@ static int run_allgather(sqdet_engine* e, void* comm, cudaStream_t stream) {
   return SQDET_OK;
 }
 
-static int run_postproc(sqdet_engine* e, cudaStream_t stream) {
+// interpret_output, then the eval-order rescale when it is on
+static int run_interpret(sqdet_engine* e, cudaStream_t stream) {
   const sqdet_config& c = e->cfg;
   int rc = launch_interpret(e->tensors[e->preds].dev, e->d_anchors, e->d_boxes, e->d_probs,
                             e->d_cls, c.batch_size, e->grid_h, e->grid_w, c.anchors_per_grid,
                             c.classes, c.image_width, c.image_height, c.exp_thresh, stream);
-  if (rc) return rc;
-  if (e->rescale_on) {
-    rc = launch_rescale_boxes(e->d_boxes, e->d_scales + (size_t)e->scale_slot * c.batch_size * 2,
+  if (rc || !e->rescale_on) return rc;
+  return launch_rescale_boxes(e->d_boxes, e->d_scales + (size_t)e->scale_slot * c.batch_size * 2,
                               c.batch_size, (int)e->num_anchors, stream);
-    if (rc) return rc;
-  }
-  rc = launch_topk_nms(e->d_boxes, e->d_probs, e->d_cls, c.batch_size, (int)e->num_anchors,
-                       c.classes, c.top_n_detection, c.prob_thresh, c.nms_thresh, e->d_dets,
-                       e->d_counts, e->max_dets, stream);
+}
+
+// filter_prediction
+static int run_filter(sqdet_engine* e, cudaStream_t stream) {
+  const sqdet_config& c = e->cfg;
+  return launch_topk_nms(e->d_boxes, e->d_probs, e->d_cls, c.batch_size, (int)e->num_anchors,
+                         c.classes, c.top_n_detection, c.prob_thresh, c.nms_thresh, e->d_dets,
+                         e->d_counts, e->max_dets, stream);
+}
+
+static int run_postproc(sqdet_engine* e, cudaStream_t stream) {
+  int rc = run_interpret(e, stream);
+  if (!rc) rc = run_filter(e, stream);
   if (rc) return rc;
   if (e->gather_in_forward && e->comm) return run_allgather(e, e->comm, stream);
   return SQDET_OK;
@@ -393,59 +424,47 @@ static int prepare_params(sqdet_engine* e) {
     SQ_CUDA(cudaMemcpy(p.dev, p.host.data(), sizeof(float) * (size_t)p.numel(),
                        cudaMemcpyHostToDevice));
   }
+  auto host = [e](int p) { return p >= 0 ? e->params[p].host.data() : nullptr; };
   for (auto& op : e->ops) {
-    for (auto& c : op.convs) {
-      if (c.p_gamma >= 0) {
-        // tf.nn.batch_normalization: inv = rsqrt(var+eps)*gamma; y = x*inv + (beta - mean*inv)
-        const int n = c.Cout;
-        std::vector<float> sc(n), sh(n);
-        const auto& g = e->params[c.p_gamma].host;
-        const auto& b = e->params[c.p_beta].host;
-        const auto& m = e->params[c.p_mean].host;
-        const auto& v = e->params[c.p_var].host;
-        for (int i = 0; i < n; ++i) {
-          const float inv = (1.0f / sqrtf(v[i] + e->cfg.batch_norm_epsilon)) * g[i];
-          sc[i] = inv;
-          sh[i] = b[i] - m[i] * inv;
-        }
-        if (!c.scale) SQ_CUDA(cudaMalloc(&c.scale, sizeof(float) * n));
-        if (!c.shift) SQ_CUDA(cudaMalloc(&c.shift, sizeof(float) * n));
-        SQ_CUDA(cudaMemcpy(c.scale, sc.data(), sizeof(float) * n, cudaMemcpyHostToDevice));
-        SQ_CUDA(cudaMemcpy(c.shift, sh.data(), sizeof(float) * n, cudaMemcpyHostToDevice));
-        if (c.tc.enabled) {
-          int rc = tc_conv_set_affine(&c.tc, sc.data(), sh.data());
-          if (rc) return rc;
-        }
+    std::vector<std::vector<float>> scale(op.convs.size()), shift(op.convs.size());
+    for (size_t k = 0; k < op.convs.size(); ++k) {
+      ConvSpec& c = op.convs[k];
+      if (c.p_gamma < 0) continue;
+      // tf.nn.batch_normalization: inv = rsqrt(var+eps)*gamma; y = x*inv + (beta - mean*inv)
+      const int n = c.Cout;
+      std::vector<float>& sc = scale[k];
+      std::vector<float>& sh = shift[k];
+      sc.resize(n);
+      sh.resize(n);
+      const auto& g = e->params[c.p_gamma].host;
+      const auto& b = e->params[c.p_beta].host;
+      const auto& m = e->params[c.p_mean].host;
+      const auto& v = e->params[c.p_var].host;
+      for (int i = 0; i < n; ++i) {
+        const float inv = (1.0f / sqrtf(v[i] + e->cfg.batch_norm_epsilon)) * g[i];
+        sc[i] = inv;
+        sh[i] = b[i] - m[i] * inv;
       }
+      if (!c.scale) SQ_CUDA(cudaMalloc(&c.scale, sizeof(float) * n));
+      if (!c.shift) SQ_CUDA(cudaMalloc(&c.shift, sizeof(float) * n));
+      SQ_CUDA(cudaMemcpy(c.scale, sc.data(), sizeof(float) * n, cudaMemcpyHostToDevice));
+      SQ_CUDA(cudaMemcpy(c.shift, sh.data(), sizeof(float) * n, cudaMemcpyHostToDevice));
     }
-  }
-  // tensor-core weight packs
-  for (auto& op : e->ops) {
-    if (op.fused.enabled) {
-      const ConvSpec& sq = op.convs[0];
-      const ConvSpec& e1 = op.convs[1];
-      const ConvSpec& e3 = op.convs[2];
-      int rc = tc_fused_fire_pack_weights(&op.fused, e->params[sq.p_kernel].host.data(),
-                                          e->params[sq.p_bias].host.data(),
-                                          e->params[e1.p_kernel].host.data(),
-                                          e->params[e1.p_bias].host.data(),
-                                          e->params[e3.p_kernel].host.data(),
-                                          e->params[e3.p_bias].host.data());
-      if (rc) return rc;
-    }
-    for (auto& c : op.convs) {
-      const float* bias = c.p_bias >= 0 ? e->params[c.p_bias].host.data() : nullptr;
-      if (!c.tc.enabled) continue;
-      int rc = tc_conv_pack_weights(&c.tc, e->params[c.p_kernel].host.data(), bias);
-      if (rc) return rc;
-    }
-    if (op.tcfire.enabled) {
-      const ConvSpec& e1 = op.convs[1];
-      const ConvSpec& e3 = op.convs[2];
-      int rc = tc_fire_pack_weights(&op.tcfire, e->params[e1.p_kernel].host.data(),
-                                    e->params[e1.p_bias].host.data(),
-                                    e->params[e3.p_kernel].host.data(),
-                                    e->params[e3.p_bias].host.data());
+    // tensor-core weight packs
+    for (auto& l : op.launches) {
+      std::vector<const float*> w, b;
+      for (int k = l.conv; k < l.conv + l.nconv; ++k) {
+        w.push_back(host(op.convs[k].p_kernel));
+        b.push_back(host(op.convs[k].p_bias));
+      }
+      int rc = SQDET_OK;
+      if (l.kind == L_FIRE_TC) {
+        rc = tc_fused_fire_pack_weights(&l.fire, w[0], b[0], w[1], b[1], w[2], b[2]);
+      } else if (l.kind == L_CONV_TC) {
+        rc = tc_conv_pack_weights(&l.tc, w, b);
+        if (!rc && !scale[l.conv].empty())
+          rc = tc_conv_set_affine(&l.tc, scale[l.conv].data(), shift[l.conv].data());
+      }
       if (rc) return rc;
     }
   }
@@ -462,27 +481,11 @@ static void drop_graph(sqdet_engine* e) {
 }
 
 static int enqueue_all(sqdet_engine* e, const float* images_dev, cudaStream_t stream) {
-  // Programmatic dependent launch for every kernel after the first (whose input comes from a
-  // copy or from the caller): see common.cuh.  Opt-in (SQDET_PDL=1): the captured forward graph
-  // already removes the launch gaps.
-  static int env_pdl = -1;
-  if (env_pdl < 0) {
-    const char* a = getenv("SQDET_PDL");
-    env_pdl = a ? atoi(a) : 0;
-  }
-  int rc = SQDET_OK;
-  bool first = true;
   for (const auto& op : e->ops) {
-    rc = run_op(e, op, images_dev, stream);
-    if (rc) break;
-    if (first && !op.skip) {
-      first = false;
-      set_pdl_launch(env_pdl != 0);
-    }
+    int rc = run_op(e, op, images_dev, stream);
+    if (rc) return rc;
   }
-  if (!rc) rc = run_postproc(e, stream);
-  set_pdl_launch(false);
-  return rc;
+  return run_postproc(e, stream);
 }
 
 static int forward_impl(sqdet_engine* e, const float* images_dev, cudaStream_t stream) {
@@ -521,6 +524,42 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, cudaStream_t s
     hit = &slot;
   }
   SQ_CUDA(cudaGraphLaunch(hit->exec, stream));
+  return SQDET_OK;
+}
+
+// Pipelined host path (sqdet_submit, sqdet_submit_frames): refuses a third batch in flight, sets
+// the pipeline up on first use and picks the slot of this submission.
+static int begin_submit(sqdet_engine* e, const char* what, int* slot) {
+  if (e->n_submitted - e->n_waited >= 2)
+    return fail(SQDET_ERR_STATE, std::string(what) + ": two batches already in flight; call sqdet_wait");
+  if (!e->copy_stream) {
+    SQ_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
+    e->d_in_slot[0] = e->tensors[0].dev;
+    SQ_CUDA(cudaMalloc(&e->d_in_slot[1], sizeof(float) * (size_t)e->tensors[0].numel()));
+    for (int k = 0; k < 2; ++k) {
+      SQ_CUDA(cudaEventCreateWithFlags(&e->ev_h2d[k], cudaEventDisableTiming));
+      SQ_CUDA(cudaEventCreateWithFlags(&e->ev_done[k], cudaEventDisableTiming));
+    }
+  }
+  *slot = (int)(e->n_submitted & 1);
+  return SQDET_OK;
+}
+
+// The forward over the slot's input on the compute stream, then the records and counts back to
+// the caller's buffers; ev_done marks the slot's buffers free again.
+static int finish_submit(sqdet_engine* e, int slot, sqdet_det* dets, int32_t* counts) {
+  const size_t B = (size_t)e->cfg.batch_size;
+  cudaStream_t ks = e->own_stream;
+  int rc = forward_impl(e, e->d_in_slot[slot], ks);
+  if (rc) return rc;
+  if (dets)
+    SQ_CUDA(cudaMemcpyAsync(dets, e->d_dets, sizeof(sqdet_det) * B * e->max_dets,
+                            cudaMemcpyDeviceToHost, ks));
+  if (counts)
+    SQ_CUDA(cudaMemcpyAsync(counts, e->d_counts, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, ks));
+  SQ_CUDA(cudaEventRecord(e->ev_done[slot], ks));
+  e->slot_used[slot] = true;
+  ++e->n_submitted;
   return SQDET_OK;
 }
 
@@ -564,6 +603,7 @@ int sqdet_create(const sqdet_config* cfg, int device, sqdet_engine** out) {
   std::unique_ptr<sqdet_engine> e(new sqdet_engine());
   e->cfg = *cfg;
   e->device = device;
+  e->sms = prop.multiProcessorCount;
   new_tensor(e.get(), "image_input", cfg->batch_size, cfg->image_height, cfg->image_width, 3);
   *out = e.release();
   return SQDET_OK;
@@ -581,10 +621,8 @@ int sqdet_destroy(sqdet_engine* e) {
     for (auto& c : op.convs) {
       if (c.scale) cudaFree(c.scale);
       if (c.shift) cudaFree(c.shift);
-      tc_conv_release(&c.tc);
     }
-    tc_fire_release(&op.tcfire);
-    tc_fused_fire_release(&op.fused);
+    release_launches(op);
   }
   cudaFree(e->d_anchors);
   cudaFree(e->d_boxes);
@@ -612,48 +650,14 @@ int sqdet_destroy(sqdet_engine* e) {
 
 int sqdet_add_conv(sqdet_engine* e, const char* layer_name, int src, int filters, int size,
                    int stride, int padding, int relu, int* out) {
-  int rc = check_build(e, src);
-  if (rc) return rc;
-  if (!layer_name || !out) return fail(SQDET_ERR_INVALID_ARG, "sqdet_add_conv: null argument");
-  Op op;
-  op.kind = OP_CONV;
-  op.name = layer_name;
-  ConvSpec cs;
-  int Ho, Wo;
-  rc = make_conv(e, layer_name, src, filters, size, stride, padding, relu, false, true, &cs,
-                 &Ho, &Wo);
-  if (rc) return rc;
-  cs.dst = new_tensor(e, layer_name, e->tensors[src].B, Ho, Wo, filters);
-  conv_cost(e, cs, Ho, Wo, &op);
-  op.src = src;
-  op.dst = cs.dst;
-  op.convs.push_back(cs);
-  e->ops.push_back(op);
-  *out = cs.dst;
-  return SQDET_OK;
+  return add_conv_op(e, "sqdet_add_conv", layer_name, src, filters, size, stride, padding, relu,
+                     false, true, out);
 }
 
 int sqdet_add_conv_bn(sqdet_engine* e, const char* scope_name, int src, int filters, int size,
                       int stride, int relu, int conv_with_bias, int* out) {
-  int rc = check_build(e, src);
-  if (rc) return rc;
-  if (!scope_name || !out) return fail(SQDET_ERR_INVALID_ARG, "sqdet_add_conv_bn: null argument");
-  Op op;
-  op.kind = OP_CONV;
-  op.name = scope_name;
-  ConvSpec cs;
-  int Ho, Wo;
-  rc = make_conv(e, scope_name, src, filters, size, stride, SQDET_PAD_SAME, relu, true,
-                 conv_with_bias != 0, &cs, &Ho, &Wo);
-  if (rc) return rc;
-  cs.dst = new_tensor(e, scope_name, e->tensors[src].B, Ho, Wo, filters);
-  conv_cost(e, cs, Ho, Wo, &op);
-  op.src = src;
-  op.dst = cs.dst;
-  op.convs.push_back(cs);
-  e->ops.push_back(op);
-  *out = cs.dst;
-  return SQDET_OK;
+  return add_conv_op(e, "sqdet_add_conv_bn", scope_name, src, filters, size, stride,
+                     SQDET_PAD_SAME, relu, true, conv_with_bias != 0, out);
 }
 
 int sqdet_add_pool(sqdet_engine* e, const char* layer_name, int src, int size, int stride,
@@ -774,38 +778,6 @@ int sqdet_finalize(sqdet_engine* e) {
     return fail(SQDET_ERR_INVALID_ARG, "max_dets smaller than TOP_N_DETECTION");
   if (topn && c.top_n_detection > 1024)
     return fail(SQDET_ERR_UNSUPPORTED, "TOP_N_DETECTION above 1024 is not supported");
-  // Pool fusion: the first layer's stride-2 conv and the max-pool that alone reads its output run
-  // as one kernel; the un-pooled tensor is never materialised.
-  for (auto& op : e->ops) op.out = op.dst;
-  {
-    static int env_fuse = -1;
-    if (env_fuse < 0) {
-      const char* a = getenv("SQDET_FUSE_POOL");
-      env_fuse = a ? atoi(a) : 1;
-    }
-    const int nops = (int)e->ops.size();
-    // first layer: Cin = 3, stride-2 conv + 3x3/2 pool -> one FFMA kernel (both math modes)
-    for (int i = 0; env_fuse && i + 1 < nops; ++i) {
-      Op& prod = e->ops[i];
-      Op& pool = e->ops[i + 1];
-      if (prod.kind != OP_CONV || pool.kind != OP_POOL || pool.src != prod.dst) continue;
-      const ConvSpec& cs = prod.convs[0];
-      if (!conv_pool_simt_eligible(cs.Cin, cs.Cout, cs.size, cs.stride, pool.size, pool.stride))
-        continue;
-      int readers = 0;
-      for (const auto& o : e->ops) {
-        if (o.src == prod.dst || o.src2 == prod.dst) ++readers;
-        for (const auto& c2 : o.convs)
-          if (&o != &prod && c2.src == prod.dst) ++readers;
-      }
-      if (readers != 1 || prod.dst == e->preds) continue;
-      prod.first_layer_fused = true;
-      prod.fused_pool_op = i + 1;
-      prod.out = pool.dst;
-      pool.skip = true;
-      e->tensors[prod.dst].materialized = false;
-    }
-  }
   int rc = plan_ops(e);
   if (rc) return rc;
   // activations
@@ -838,65 +810,112 @@ int sqdet_finalize(sqdet_engine* e) {
   return SQDET_OK;
 }
 
-// Per-op accounting and tensor-core planning.  Runs before the activations are allocated: a
-// fire module planned as one kernel never materialises its squeeze tensor.
-static int plan_ops(sqdet_engine* e) {
-  const sqdet_config& c = e->cfg;
-  for (auto& op : e->ops) {
-    int64_t bytes = 0;
-    op.launches = 0;
-    if (op.kind == OP_CONV || op.kind == OP_FIRE) {
-      bytes += 4 * e->tensors[op.src].numel() + 4 * e->tensors[op.dst].numel() + 4 * op.params;
-      if (op.first_layer_fused)
-        bytes = 4 * e->tensors[op.src].numel() + 4 * e->tensors[op.out].numel() + 4 * op.params;
-      if (c.math_mode == SQDET_MATH_TF32X3_TC && !op.first_layer_fused) {
-        if (op.kind == OP_CONV) {
-          ConvSpec& cs = op.convs[0];
-          int rc = tc_conv_plan(&cs.tc, e->tensors[cs.src].B, e->tensors[cs.src].H,
-                                e->tensors[cs.src].W, cs.Cin, cs.Cout, cs.size, cs.stride,
-                                cs.padding, cs.relu, cs.p_gamma >= 0, e->tensors[op.out].C,
-                                cs.y_coff);
-          if (rc < 0) return rc;
-        } else {
-          // The whole module as one kernel where the squeeze is 16 channels wide and the grid
-          // holds at least 4 tiles per SM (SqueezeDet fire2/3); otherwise the squeeze conv, then
-          // the expand pair as one launch over the squeeze tensor.
-          ConvSpec& sq = op.convs[0];
-          const Tensor& xin = e->tensors[sq.src];
-          int sms = 132, dev = 0;
-          cudaGetDevice(&dev);
-          cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-          const long long tiles = (long long)xin.B * ((xin.H + 7) / 8) * ((xin.W + 15) / 16);
-          if (sq.Cout <= 16 && tiles >= 4LL * sms && sq.dst != e->preds &&
-              !read_by_other_op(e, sq.dst, &op)) {
-            int rcf = tc_fused_fire_plan(&op.fused, xin.B, xin.H, xin.W, xin.C, sq.Cout,
-                                         op.convs[1].Cout, op.convs[2].Cout);
-            if (rcf < 0) return rcf;
-            if (op.fused.enabled) e->tensors[sq.dst].materialized = false;
-          }
-        }
-        if (op.kind == OP_FIRE && !op.fused.enabled) {
-          ConvSpec& sq = op.convs[0];
-          int rc = tc_conv_plan(&sq.tc, e->tensors[sq.src].B, e->tensors[sq.src].H,
-                                e->tensors[sq.src].W, sq.Cin, sq.Cout, 1, 1, SQDET_PAD_SAME, 1,
-                                false, e->tensors[sq.dst].C, 0);
-          if (rc < 0) return rc;
-          const Tensor& q = e->tensors[sq.dst];
-          rc = tc_fire_plan(&op.tcfire, q.B, q.H, q.W, q.C, op.convs[1].Cout, op.convs[2].Cout);
-          if (rc < 0) return rc;
-        }
-      }
-      if (op.kind == OP_CONV) op.launches = 1;
-      else op.launches = op.fused.enabled ? 1 : 1 + (op.tcfire.enabled ? 1 : 2);
-    } else if (op.kind == OP_POOL) {
-      bytes = op.skip ? 0 : 4 * e->tensors[op.src].numel() + 4 * e->tensors[op.dst].numel();
-      op.launches = op.skip ? 0 : 1;
-    } else {
-      bytes = 4 * 3 * e->tensors[op.dst].numel();
-      op.launches = 1;
+// One conv as one launch: the wgmma implicit GEMM where the tensor-core path takes the shape,
+// else the FFMA kernel.
+static int plan_conv(sqdet_engine* e, const ConvSpec& c, int index, bool tc, Launch* l) {
+  *l = Launch{L_CONV_SIMT, c.src, c.dst, index, 1};
+  if (!tc) return SQDET_OK;
+  const Tensor& in = e->tensors[c.src];
+  const int rc = tc_conv_plan(&l->tc, in.B, in.H, in.W, c.Cin, {{c.size, c.Cout, c.y_coff}},
+                              c.stride, c.padding, c.relu, c.p_gamma >= 0, e->tensors[c.dst].C);
+  if (rc > 0) l->kind = L_CONV_TC;
+  return rc < 0 ? rc : SQDET_OK;
+}
+
+// A fire module on tensor cores runs as one kernel where the squeeze is 16 channels wide and the
+// grid holds at least 4 tiles per SM (SqueezeDet fire2/3); otherwise as the squeeze conv, then
+// the expand pair as one launch over the squeeze tensor.  What the wgmma kernels decline, and
+// every fire in the SIMT math mode, runs as three FFMA convs.
+static int plan_fire(sqdet_engine* e, Op& op, bool tc) {
+  const ConvSpec& sq = op.convs[0];
+  const ConvSpec& e1 = op.convs[1];
+  const ConvSpec& e3 = op.convs[2];
+  const Tensor& x = e->tensors[op.src];
+  const long long tiles = (long long)x.B * ((x.H + 7) / 8) * ((x.W + 15) / 16);
+  if (tc && sq.Cout <= 16 && tiles >= 4LL * e->sms && sq.dst != e->preds &&
+      !read_by_other_op(e, sq.dst, &op)) {
+    Launch l{L_FIRE_TC, op.src, op.dst, 0, 3};
+    const int rc = tc_fused_fire_plan(&l.fire, x.B, x.H, x.W, x.C, sq.Cout, e1.Cout, e3.Cout);
+    if (rc < 0) return rc;
+    if (rc) {
+      op.launches.push_back(l);
+      e->tensors[sq.dst].materialized = false;
+      return SQDET_OK;
     }
-    op.min_bytes = bytes;
   }
+  Launch l;
+  int rc = plan_conv(e, sq, 0, tc, &l);
+  op.launches.push_back(l);
+  if (rc) return rc;
+  if (tc) {
+    const Tensor& q = e->tensors[sq.dst];
+    Launch pair{L_CONV_TC, sq.dst, op.dst, 1, 2};
+    rc = tc_conv_plan(&pair.tc, q.B, q.H, q.W, q.C,
+                      {{e1.size, e1.Cout, e1.y_coff}, {e3.size, e3.Cout, e3.y_coff}}, 1,
+                      SQDET_PAD_SAME, 1, false, e->tensors[op.dst].C);
+    if (rc < 0) return rc;
+    if (rc) {
+      op.launches.push_back(pair);
+      return SQDET_OK;
+    }
+  }
+  op.launches.push_back(Launch{L_CONV_SIMT, sq.dst, op.dst, 1, 1});
+  op.launches.push_back(Launch{L_CONV_SIMT, sq.dst, op.dst, 2, 1});
+  return SQDET_OK;
+}
+
+// The bytes an op has to move at the least: its input, the tensor it finally writes (a fused
+// pool's output) and its parameters; add+ReLU reads two tensors and writes one.
+static int64_t min_bytes(const sqdet_engine* e, const Op& op) {
+  auto bytes = [e](int t) { return 4 * e->tensors[t].numel(); };
+  if (op.kind == OP_ADD_RELU) return 3 * bytes(op.dst);
+  if (op.launches.empty()) return 0;
+  return bytes(op.src) + bytes(op.launches.back().dst) + 4 * op.params;
+}
+
+// Every kernel choice of the forward: first-layer pool fusion, tensor-core plans, one-kernel fire
+// or expand pair, and which tensors are never materialised.  Runs before the activations are
+// allocated.
+static int plan_ops(sqdet_engine* e) {
+  const bool tc = e->cfg.math_mode == SQDET_MATH_TF32X3_TC;
+  for (auto& op : e->ops) release_launches(op);
+  for (size_t i = 0; i < e->ops.size(); ++i) {
+    Op& op = e->ops[i];
+    int rc = SQDET_OK;
+    switch (op.kind) {
+      case OP_CONV: {
+        const ConvSpec& c = op.convs[0];
+        Op* pool = i + 1 < e->ops.size() ? &e->ops[i + 1] : nullptr;
+        Launch l;
+        if (pool && pool->kind == OP_POOL && pool->src == op.dst && op.dst != e->preds &&
+            conv_pool_simt_eligible(c.Cin, c.Cout, c.size, c.stride, pool->size, pool->stride) &&
+            !read_by_other_op(e, op.dst, pool)) {
+          // the first layer (Cin = 3, stride 2) and the 3x3/2 pool that alone reads it: one FFMA
+          // kernel in both math modes.  The pool keeps no launch and the un-pooled tensor is never
+          // materialised.
+          l = Launch{L_CONV_POOL, op.src, pool->dst, 0, 1};
+          l.pool_padding = pool->padding;
+          e->tensors[op.dst].materialized = false;
+          ++i;
+        } else {
+          rc = plan_conv(e, c, 0, tc, &l);
+        }
+        op.launches.push_back(l);
+        break;
+      }
+      case OP_FIRE:
+        rc = plan_fire(e, op, tc);
+        break;
+      case OP_POOL:
+        op.launches.push_back(Launch{L_MAXPOOL, op.src, op.dst});
+        break;
+      case OP_ADD_RELU:
+        op.launches.push_back(Launch{L_ADD_RELU, op.src, op.dst});
+        break;
+    }
+    if (rc) return rc;
+  }
+  for (auto& op : e->ops) op.min_bytes = min_bytes(e, op);
   return SQDET_OK;
 }
 
@@ -1019,20 +1038,10 @@ int sqdet_forward_profiled(sqdet_engine* e, const float* images_dev, void* strea
     if (rc) return rc;
     SQ_CUDA(cudaEventRecord(e->prof_events[i + 1], stream));
   }
-  const sqdet_config& c = e->cfg;
-  rc = launch_interpret(e->tensors[e->preds].dev, e->d_anchors, e->d_boxes, e->d_probs, e->d_cls,
-                        c.batch_size, e->grid_h, e->grid_w, c.anchors_per_grid, c.classes,
-                        c.image_width, c.image_height, c.exp_thresh, stream);
+  rc = run_interpret(e, stream);
   if (rc) return rc;
-  if (e->rescale_on) {
-    rc = launch_rescale_boxes(e->d_boxes, e->d_scales + (size_t)e->scale_slot * c.batch_size * 2,
-                              c.batch_size, (int)e->num_anchors, stream);
-    if (rc) return rc;
-  }
   SQ_CUDA(cudaEventRecord(e->prof_events[n - 1], stream));
-  rc = launch_topk_nms(e->d_boxes, e->d_probs, e->d_cls, c.batch_size, (int)e->num_anchors,
-                       c.classes, c.top_n_detection, c.prob_thresh, c.nms_thresh, e->d_dets,
-                       e->d_counts, e->max_dets, stream);
+  rc = run_filter(e, stream);
   if (rc) return rc;
   SQ_CUDA(cudaEventRecord(e->prof_events[n], stream));
   SQ_CUDA(cudaEventSynchronize(e->prof_events[n]));
@@ -1094,21 +1103,12 @@ int sqdet_submit(sqdet_engine* e, const void* images, int img_type, sqdet_det* d
   if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_submit before sqdet_finalize");
   if (img_type != SQDET_IMG_F32 && img_type != SQDET_IMG_U8)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit: unknown img_type");
-  if (e->n_submitted - e->n_waited >= 2)
-    return fail(SQDET_ERR_STATE, "sqdet_submit: two batches already in flight; call sqdet_wait");
   DeviceGuard guard(e->device);
   const sqdet_config& c = e->cfg;
-  const int slot = (int)(e->n_submitted & 1);
+  int slot;
+  int rc = begin_submit(e, "sqdet_submit", &slot);
+  if (rc) return rc;
   const int64_t n_pix = (int64_t)c.batch_size * c.image_height * c.image_width;
-  if (!e->copy_stream) {
-    SQ_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-    e->d_in_slot[0] = e->tensors[0].dev;
-    SQ_CUDA(cudaMalloc(&e->d_in_slot[1], sizeof(float) * (size_t)n_pix * 3));
-    for (int k = 0; k < 2; ++k) {
-      SQ_CUDA(cudaEventCreateWithFlags(&e->ev_h2d[k], cudaEventDisableTiming));
-      SQ_CUDA(cudaEventCreateWithFlags(&e->ev_done[k], cudaEventDisableTiming));
-    }
-  }
   if (img_type == SQDET_IMG_U8 && !e->d_u8_slot[slot])
     SQ_CUDA(cudaMalloc(&e->d_u8_slot[slot], (size_t)n_pix * 3));
   cudaStream_t cs = e->copy_stream, ks = e->own_stream;
@@ -1121,7 +1121,6 @@ int sqdet_submit(sqdet_engine* e, const void* images, int img_type, sqdet_det* d
                             cudaMemcpyHostToDevice, cs));
   SQ_CUDA(cudaEventRecord(e->ev_h2d[slot], cs));
   SQ_CUDA(cudaStreamWaitEvent(ks, e->ev_h2d[slot], 0));
-  int rc = SQDET_OK;
   if (img_type == SQDET_IMG_U8) {
     // on the COMPUTE stream: on the copy stream (to overlap the previous batch's forward) it was
     // measured slower, 2.08 vs 1.93 ms per step end to end - its CTAs wait for the persistent
@@ -1130,18 +1129,7 @@ int sqdet_submit(sqdet_engine* e, const void* images, int img_type, sqdet_det* d
                            e->bgr_means[1], e->bgr_means[2], ks);
     if (rc) return rc;
   }
-  rc = forward_impl(e, e->d_in_slot[slot], ks);
-  if (rc) return rc;
-  if (dets)
-    SQ_CUDA(cudaMemcpyAsync(dets, e->d_dets, sizeof(sqdet_det) * (size_t)c.batch_size * e->max_dets,
-                            cudaMemcpyDeviceToHost, ks));
-  if (counts)
-    SQ_CUDA(cudaMemcpyAsync(counts, e->d_counts, sizeof(int32_t) * (size_t)c.batch_size,
-                            cudaMemcpyDeviceToHost, ks));
-  SQ_CUDA(cudaEventRecord(e->ev_done[slot], ks));
-  e->slot_used[slot] = true;
-  ++e->n_submitted;
-  return SQDET_OK;
+  return finish_submit(e, slot, dets, counts);
 }
 
 int sqdet_wait(sqdet_engine* e) {
@@ -1157,7 +1145,7 @@ int sqdet_wait(sqdet_engine* e) {
 int sqdet_launches_per_forward(sqdet_engine* e) {
   if (!e) return SQDET_ERR_INVALID_ARG;
   int n = 2 + (e->rescale_on ? 1 : 0);   // interpret [+ rescale] + filter (NCCL's own kernel not counted)
-  for (const auto& op : e->ops) n += op.launches;
+  for (const auto& op : e->ops) n += (int)op.launches.size();
   return n;
 }
 
@@ -1194,9 +1182,10 @@ int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames, const int
   if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_submit_frames before sqdet_finalize");
   if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit_frames: order must be 0 (demo) or 1 (eval)");
-  if (e->n_submitted - e->n_waited >= 2)
-    return fail(SQDET_ERR_STATE, "sqdet_submit_frames: two batches already in flight; call sqdet_wait");
   DeviceGuard guard(e->device);
+  int slot;
+  int rc = begin_submit(e, "sqdet_submit_frames", &slot);
+  if (rc) return rc;
   const sqdet_config& c = e->cfg;
   const int B = c.batch_size;
   size_t total = 0;
@@ -1206,17 +1195,6 @@ int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames, const int
       return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit_frames: empty frame");
     off[(size_t)i] = total;
     total += ((size_t)heights[i] * widths[i] * 3 + 255) & ~(size_t)255;
-  }
-  const int slot = (int)(e->n_submitted & 1);
-  const int64_t n_pix = (int64_t)B * c.image_height * c.image_width;
-  if (!e->copy_stream) {
-    SQ_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-    e->d_in_slot[0] = e->tensors[0].dev;
-    SQ_CUDA(cudaMalloc(&e->d_in_slot[1], sizeof(float) * (size_t)n_pix * 3));
-    for (int k = 0; k < 2; ++k) {
-      SQ_CUDA(cudaEventCreateWithFlags(&e->ev_h2d[k], cudaEventDisableTiming));
-      SQ_CUDA(cudaEventCreateWithFlags(&e->ev_done[k], cudaEventDisableTiming));
-    }
   }
   cudaStream_t cs = e->copy_stream, ks = e->own_stream;
   if (e->slot_used[slot]) SQ_CUDA(cudaStreamWaitEvent(cs, e->ev_done[slot], 0));
@@ -1241,37 +1219,26 @@ int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames, const int
       sc[(size_t)2 * i + 1] = (float)((double)c.image_height / (double)heights[i]);
     }
     if (!e->rescale_on) {
-      int rc = sqdet_set_box_scale(e, sc.data());      // first use: allocate + enable
+      rc = sqdet_set_box_scale(e, sc.data());      // first use: allocate + enable
       if (rc) return rc;
     }
     // this slot's half of the table, in stream order behind the forward that last read it
     SQ_CUDA(cudaMemcpyAsync(e->d_scales + (size_t)slot * B * 2, sc.data(), sizeof(float) * B * 2,
                             cudaMemcpyHostToDevice, ks));
   } else if (e->rescale_on) {
-    int rc = sqdet_set_box_scale(e, nullptr);
+    rc = sqdet_set_box_scale(e, nullptr);
     if (rc) return rc;
   }
   SQ_CUDA(cudaStreamWaitEvent(ks, e->ev_h2d[slot], 0));
   const size_t img_floats = (size_t)c.image_height * c.image_width * 3;
   for (int i = 0; i < B; ++i) {
-    int rc = launch_resize_meansub_u8(e->d_frames[slot] + off[(size_t)i], heights[i], widths[i],
-                                      e->d_in_slot[slot] + (size_t)i * img_floats, c.image_height,
-                                      c.image_width, e->bgr_means[0], e->bgr_means[1],
-                                      e->bgr_means[2], order == SQDET_PRE_SUB_THEN_RESIZE, ks);
+    rc = launch_resize_meansub_u8(e->d_frames[slot] + off[(size_t)i], heights[i], widths[i],
+                                  e->d_in_slot[slot] + (size_t)i * img_floats, c.image_height,
+                                  c.image_width, e->bgr_means[0], e->bgr_means[1],
+                                  e->bgr_means[2], order == SQDET_PRE_SUB_THEN_RESIZE, ks);
     if (rc) return rc;
   }
-  int rc = forward_impl(e, e->d_in_slot[slot], ks);
-  if (rc) return rc;
-  if (dets)
-    SQ_CUDA(cudaMemcpyAsync(dets, e->d_dets, sizeof(sqdet_det) * (size_t)B * e->max_dets,
-                            cudaMemcpyDeviceToHost, ks));
-  if (counts)
-    SQ_CUDA(cudaMemcpyAsync(counts, e->d_counts, sizeof(int32_t) * (size_t)B,
-                            cudaMemcpyDeviceToHost, ks));
-  SQ_CUDA(cudaEventRecord(e->ev_done[slot], ks));
-  e->slot_used[slot] = true;
-  ++e->n_submitted;
-  return SQDET_OK;
+  return finish_submit(e, slot, dets, counts);
 }
 
 // ---- multi-GPU: ONE all-gather of the filtered records ---------------------------------------------

@@ -6,7 +6,6 @@
 // Roofline: HBM.  Algorithmic bytes = 4*(B*H*W*C + B*Ho*Wo*C); each input element is
 // read ~(k/stride)^2 times but the re-reads hit L1/L2 (adjacent threads share rows).
 #include <math_constants.h>
-#include <stdlib.h>
 #include "common.cuh"
 
 namespace sqdet {
@@ -23,8 +22,6 @@ __device__ __forceinline__ float4 ld_stream(const float4* p) {
 __global__ void __launch_bounds__(256)
 maxpool_vec4_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W,
                     int C4, int k, int stride, int pad_t, int pad_l, int Ho, int Wo) {
-  pdl_trigger();
-  pdl_wait();
   const long long total = (long long)B * Ho * Wo * C4;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
@@ -60,8 +57,6 @@ template <int K>
 __global__ void __launch_bounds__(256)
 maxpool_s2_vec4_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W,
                        int C4, int pad_t, int pad_l, int Ho, int Wo) {
-  pdl_trigger();
-  pdl_wait();
   const int total = B * Ho * Wo * C4;
   const float4* __restrict__ x4 = reinterpret_cast<const float4*>(x);
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
@@ -102,8 +97,6 @@ maxpool_s2_vec4_kernel(const float* __restrict__ x, float* __restrict__ y, int B
 __global__ void __launch_bounds__(256)
 maxpool_scalar_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W,
                       int C, int k, int stride, int pad_t, int pad_l, int Ho, int Wo) {
-  pdl_trigger();
-  pdl_wait();
   const long long total = (long long)B * Ho * Wo * C;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
@@ -131,8 +124,6 @@ maxpool_scalar_kernel(const float* __restrict__ x, float* __restrict__ y, int B,
 __global__ void __launch_bounds__(256)
 add_relu_kernel(const float* __restrict__ a, const float* __restrict__ b,
                 float* __restrict__ y, long long n4, long long n) {
-  pdl_trigger();
-  pdl_wait();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n4) {
     const float4 p = ld_stream(reinterpret_cast<const float4*>(a) + i);
@@ -278,26 +269,17 @@ int launch_maxpool(const float* x, float* y, int B, int H, int W, int C, int siz
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long cap = (long long)sms * 8 * 16;   // grid-stride beyond 16 waves of 8 CTAs/SM
   if (blocks > cap) blocks = cap;
-  static int env_fast = -1;
-  if (env_fast < 0) {
-    const char* a = getenv("SQDET_POOL_FAST");
-    env_fast = a ? atoi(a) : 1;
-  }
   const long long in_elems = (long long)B * H * W * (C / 4);
-  if (vec && env_fast && stride == 2 && (size == 2 || size == 3) && total < (1LL << 30) &&
-      in_elems < (1LL << 30)) {
-    if (size == 3)
-      SQ_CUDA(launch_kernel(maxpool_s2_vec4_kernel<3>, dim3((unsigned)blocks), dim3(256), 0, stream, x, y,
-                            B, H, W, C / 4, gh.pad_before, gw.pad_before, gh.out, gw.out));
-    else
-      SQ_CUDA(launch_kernel(maxpool_s2_vec4_kernel<2>, dim3((unsigned)blocks), dim3(256), 0, stream, x, y,
-                            B, H, W, C / 4, gh.pad_before, gw.pad_before, gh.out, gw.out));
-  } else if (vec)
-    SQ_CUDA(launch_kernel(maxpool_vec4_kernel, dim3((unsigned)blocks), dim3(256), 0, stream,
-                          x, y, B, H, W, C / 4, size, stride, gh.pad_before, gw.pad_before, gh.out, gw.out));
+  if (vec && stride == 2 && (size == 2 || size == 3) && total < (1LL << 30) &&
+      in_elems < (1LL << 30))
+    (size == 3 ? maxpool_s2_vec4_kernel<3> : maxpool_s2_vec4_kernel<2>)<<<(unsigned)blocks, 256, 0, stream>>>(
+        x, y, B, H, W, C / 4, gh.pad_before, gw.pad_before, gh.out, gw.out);
+  else if (vec)
+    maxpool_vec4_kernel<<<(unsigned)blocks, 256, 0, stream>>>(
+        x, y, B, H, W, C / 4, size, stride, gh.pad_before, gw.pad_before, gh.out, gw.out);
   else
-    SQ_CUDA(launch_kernel(maxpool_scalar_kernel, dim3((unsigned)blocks), dim3(256), 0, stream,
-                          x, y, B, H, W, C, size, stride, gh.pad_before, gw.pad_before, gh.out, gw.out));
+    maxpool_scalar_kernel<<<(unsigned)blocks, 256, 0, stream>>>(
+        x, y, B, H, W, C, size, stride, gh.pad_before, gw.pad_before, gh.out, gw.out);
   SQ_CHECK_LAUNCH("maxpool_kernel");
   return SQDET_OK;
 }
@@ -308,7 +290,7 @@ int launch_add_relu(const float* a, const float* b, float* y, int64_t n, cudaStr
                           reinterpret_cast<uintptr_t>(y)) & 15) == 0);
   const long long n4 = aligned ? n / 4 : 0;
   long long threads = n4 > 0 ? n4 : 1;
-  SQ_CUDA(launch_kernel(add_relu_kernel, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, a, b, y, n4, n));
+  add_relu_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(a, b, y, n4, n);
   SQ_CHECK_LAUNCH("add_relu_kernel");
   return SQDET_OK;
 }

@@ -32,8 +32,6 @@ interpret_kernel(const float* __restrict__ preds, const float* __restrict__ anch
                  float* __restrict__ boxes, float* __restrict__ probs,
                  long long* __restrict__ cls, int B, int A, int K, int C, float wm1,
                  float hm1, float exp_thresh, float slope) {
-  pdl_trigger();
-  pdl_wait();
   const long long total = (long long)B * A;
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
@@ -90,8 +88,6 @@ interpret_kernel(const float* __restrict__ preds, const float* __restrict__ anch
 __global__ void __launch_bounds__(256)
 rescale_boxes_kernel(float4* __restrict__ boxes, const float* __restrict__ scales, int A,
                      long long total) {
-  pdl_trigger();
-  pdl_wait();
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const int b = (int)(idx / A);
@@ -149,8 +145,6 @@ filter_kernel(const float* __restrict__ boxes, const float* __restrict__ probs,
               const long long* __restrict__ cls, int A, int classes, int top_n,
               float prob_thresh, float nms_thresh, sqdet_det* __restrict__ dets,
               int* __restrict__ counts, int max_dets) {
-  pdl_trigger();
-  pdl_wait();
   __shared__ unsigned long long s_key[FCAP];   // (order_key << 32) | (~anchor)
   __shared__ float4 s_box[FCAP];
   __shared__ int s_cls[FCAP];
@@ -395,9 +389,9 @@ int launch_interpret(const float* preds, const float* anchors, float* boxes, flo
   const long long total = (long long)B * A;
   // slope = np.exp(thresh) in float64, cast to fp32 where it meets the tensor (util.py:222)
   const float slope = (float)exp((double)exp_thresh);
-  SQ_CUDA(launch_kernel(interpret_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, stream,
-                        preds, anchors, boxes, probs, reinterpret_cast<long long*>(cls), B, A, K, C,
-                        (float)(image_width - 1.0), (float)(image_height - 1.0), exp_thresh, slope));
+  interpret_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(
+      preds, anchors, boxes, probs, reinterpret_cast<long long*>(cls), B, A, K, C,
+      (float)(image_width - 1.0), (float)(image_height - 1.0), exp_thresh, slope);
   SQ_CHECK_LAUNCH("interpret_kernel");
   return SQDET_OK;
 }
@@ -408,8 +402,8 @@ int launch_rescale_boxes(float* boxes, const float* scales_xy, int B, int A,
   if (reinterpret_cast<uintptr_t>(boxes) & 15)
     return fail(SQDET_ERR_INVALID_ARG, "rescale_boxes: boxes must be 16-byte aligned");
   const long long total = (long long)B * A;
-  SQ_CUDA(launch_kernel(rescale_boxes_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0,
-                        stream, reinterpret_cast<float4*>(boxes), scales_xy, A, total));
+  rescale_boxes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(
+      reinterpret_cast<float4*>(boxes), scales_xy, A, total);
   SQ_CHECK_LAUNCH("rescale_boxes_kernel");
   return SQDET_OK;
 }
@@ -425,9 +419,9 @@ int launch_topk_nms(const float* boxes, const float* probs, const int64_t* cls, 
   if (topn_branch && (top_n > FCAP || top_n > max_dets))
     return fail(SQDET_ERR_UNSUPPORTED,
                 "topk_nms: TOP_N_DETECTION above capacity (max 1024 and <= max_dets)");
-  SQ_CUDA(launch_kernel(filter_kernel, dim3((unsigned)B), dim3(FT), 0, stream, boxes, probs,
-                        reinterpret_cast<const long long*>(cls), A, classes, top_n, prob_thresh,
-                        nms_thresh, dets, reinterpret_cast<int*>(counts), max_dets));
+  filter_kernel<<<(unsigned)B, FT, 0, stream>>>(boxes, probs, reinterpret_cast<const long long*>(cls),
+                                                A, classes, top_n, prob_thresh, nms_thresh, dets,
+                                                reinterpret_cast<int*>(counts), max_dets);
   SQ_CHECK_LAUNCH("filter_kernel");
   return SQDET_OK;
 }

@@ -167,6 +167,37 @@ def test_session_run_contract_and_filter_prediction(math_mode, gpu_device):
   assert len(model.model_params) == 64
 
 
+@pytest.mark.parametrize('math_mode', MODES)
+def test_forward_profiled_matches_detect(math_mode, gpu_device):
+  """sqdet_forward_profiled: one time per op_table() row, and the same det tensors and filtered
+  records as sqdet_detect on the same images.  Every result buffer is overwritten with 0xff bytes
+  first, so a skipped interpret or filter launch shows.  VGG16 fuses no pool into its producer, so
+  every op issues work and every time is positive."""
+  mc = make_mc('vgg16', 96, 64, 2)
+  model = VGG16ConvDet(mc, gpu_device, math_mode=math_mode)
+  model.load_weights(synth.synthetic_weights(synth.model_param_specs(model), seed=5))
+  images = synth.synthetic_images(2, 64, 96, seed=6)
+  want = dict(zip(('det_boxes', 'det_probs', 'det_class', 'dets', 'counts'),
+                  model.detect(images, want_dets=True)))
+  assert want['counts'].sum() > 0
+  lib, res = model._lib, model.results_device()
+  for key, arr in want.items():
+    fill = np.full(arr.nbytes, 0xff, np.uint8)
+    _lib.check(lib.sqdet_memcpy_h2d(res[key], fill.ctypes.data, fill.nbytes, None))
+  _lib.check(lib.sqdet_stream_sync(gpu_device, None))
+  x = _lib.DeviceBuffer.from_numpy(images, gpu_device)
+  rows = model.forward_profiled(x.ptr)
+  table = model.op_table()
+  assert len(rows) == lib.sqdet_num_ops(model._engine) == len(table)
+  assert [row[0] for row, _ in rows] == [row[0] for row in table]
+  assert all(ms > 0 for _, ms in rows), rows
+  for key, arr in want.items():
+    got = np.empty_like(arr)
+    _lib.check(lib.sqdet_memcpy_d2h(got.ctypes.data, res[key], got.nbytes, None))
+    _lib.check(lib.sqdet_stream_sync(gpu_device, None))
+    assert got.tobytes() == arr.tobytes(), key
+
+
 def test_batch_invariance_and_determinism(gpu_device):
   mc1 = make_mc('squeezeDet', 320, 96, 1)
   mc3 = make_mc('squeezeDet', 320, 96, 3)
