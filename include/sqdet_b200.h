@@ -136,6 +136,21 @@ int sqdet_op_info(sqdet_engine* e, int index, char* name_buf, int name_cap,
 /* Asynchronous on `stream`: backbone + ConvDet + interpret_output + filter for the
  * whole batch.  images_dev [B,H,W,3] fp32 (BGR, mean-subtracted).                     */
 int sqdet_forward(sqdet_engine* e, const float* images_dev, void* stream);
+/* Partial batch: an engine built for B images runs any n with 1 <= n <= B and processes images
+ * [0, n) only.  images_dev then needs to hold just those n images [n,H,W,3]; nothing at or past
+ * image n is read.
+ *   - Same kernels as the full batch: the plan sqdet_finalize made for B (kernel per layer,
+ *     output-channel tile, one-kernel fire or not) runs unchanged; only the grids shrink.  So
+ *     image i of an n-image forward is bitwise identical to image i of a full forward whose
+ *     first n images are the same.
+ *   - No activation row, det_boxes / det_probs / det_class row or record row at or past n is
+ *     written: sqdet_read_tensor and sqdet_results_dev still return B rows, and rows [n, B)
+ *     hold what the last forward that covered them left there.  counts[n, B) are set to 0 on the
+ *     device (inside the forward's CUDA graph), so the all-gather blob stays fully defined.
+ *   - sqdet_read_tensor, sqdet_op_info and sqdet_launches_per_forward keep their B-sized meaning.
+ *   - SQDET_ERR_INVALID_ARG when n < 1 or n > B.
+ * sqdet_forward is sqdet_forward_n with n = B.                                              */
+int sqdet_forward_n(sqdet_engine* e, const float* images_dev, int n, void* stream);
 /* Same, but records a CUDA event around every op (not graph-captured) and returns
  * per-op milliseconds (synchronous).  op_ms has sqdet_num_ops() entries.              */
 int sqdet_forward_profiled(sqdet_engine* e, const float* images_dev, void* stream,
@@ -177,6 +192,14 @@ int sqdet_wait(sqdet_engine* e);
 int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames,
                         const int32_t* heights, const int32_t* widths, int order,
                         int rescale, sqdet_det* dets, int32_t* counts);
+/* sqdet_submit_frames over n frames, 1 <= n <= B, with the partial-batch semantics of
+ * sqdet_forward_n: frames/heights/widths have n entries, and n rows of records (dets
+ * [n,max_dets]) and n counts are copied back.  Same sqdet_wait contract; submits with different
+ * n may be in flight together.  SQDET_ERR_INVALID_ARG when n < 1 or n > B.
+ * sqdet_submit_frames is sqdet_submit_frames_n with n = B.                                   */
+int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
+                          const int32_t* heights, const int32_t* widths, int order,
+                          int rescale, sqdet_det* dets, int32_t* counts);
 /* src/eval.py:83-84 for callers that resize on the host: xy_scales = B pairs (x_scale,
  * y_scale), host memory; every later forward divides det_boxes[b,:,0::2] by x_scale and
  * [b,:,1::2] by y_scale (float32, as numpy does) between interpret_output and

@@ -74,6 +74,7 @@ SIGNATURES = {
     'sqdet_num_ops': (_i, [_vp]),
     'sqdet_op_info': (_i, [_vp, _i, C.c_char_p, _i, _i64p, _i64p, _i64p]),
     'sqdet_forward': (_i, [_vp, _fp, _vp]),
+    'sqdet_forward_n': (_i, [_vp, _fp, _i, _vp]),
     'sqdet_forward_profiled': (_i, [_vp, _fp, _vp, _fp]),
     'sqdet_results_dev': (_i, [_vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp),
                                C.POINTER(_vp), C.POINTER(_vp), C.POINTER(C.c_int32)]),
@@ -82,6 +83,7 @@ SIGNATURES = {
     'sqdet_submit': (_i, [_vp, _vp, _i, _vp, _vp]),
     'sqdet_wait': (_i, [_vp]),
     'sqdet_submit_frames': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),
+    'sqdet_submit_frames_n': (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _vp, _vp]),
     'sqdet_set_box_scale': (_i, [_vp, _vp]),
     'sqdet_launches_per_forward': (_i, [_vp]),
     'sqdet_engine_stream': (_vp, [_vp]),

@@ -526,7 +526,6 @@ struct TcImpl {
   TcParams prm{};
   int NT = 0, KC = 0;
   ConvKernel kernel = nullptr;
-  dim3 grid;
   size_t smem_bytes = 0;
   std::vector<ConvGroup> groups;
   std::vector<int> group_chunk0;   // first chunk of each group
@@ -613,7 +612,6 @@ static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo,
   p.nchunks = nch;
   im->cout_total = poff;
   im->w_floats = woff;
-  im->grid = dim3((unsigned)mtiles, (unsigned)nch);
   im->smem_bytes = (size_t)STAGES * (TILE_M * (KC + 4) + 2 * NT * KC) * sizeof(float);
   cudaError_t ce = cudaFuncSetAttribute(im->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)im->smem_bytes);
@@ -671,7 +669,6 @@ struct FusedImpl {
   int KCI = 0, SQN = 0, KCE = 0;
   int E1 = 0, E3 = 0;
   FireKernel kernel = nullptr;
-  unsigned grid = 0;
   size_t smem = 0;
   float* d_w = nullptr;    // squeeze tiles
   float* d_w2 = nullptr;   // expand tiles
@@ -743,12 +740,17 @@ int tc_conv_set_affine(TcConvPlan* plan, const float* scale, const float* shift)
   return SQDET_OK;
 }
 
-int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, cudaStream_t stream) {
+int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, int n,
+                   cudaStream_t stream) {
   const TcImpl* im = static_cast<const TcImpl*>(plan.impl);
   TcParams prm = im->prm;
+  if (n < 1 || n > prm.B) return fail(SQDET_ERR_INVALID_ARG, "launch_conv_tc: image count outside [1, B]");
   prm.x = x_dev;
   prm.y = y_dev;
-  im->kernel<<<im->grid, NUM_THREADS, im->smem_bytes, stream>>>(prm);
+  prm.B = n;
+  prm.M = (long long)n * prm.Ho * prm.Wo;
+  const dim3 grid((unsigned)((prm.M + TILE_M - 1) / TILE_M), (unsigned)prm.nchunks);
+  im->kernel<<<grid, NUM_THREADS, im->smem_bytes, stream>>>(prm);
   SQ_CHECK_LAUNCH("conv_tc_kernel");
   return SQDET_OK;
 }
@@ -786,7 +788,7 @@ int conv2d_tc_oneshot(const float* x_dev, const float* w_hwio_dev, const float* 
   }
   rc = tc_conv_pack_weights(&plan, {w.data()}, {bias_dev ? b.data() : nullptr});
   if (!rc && scale_dev) rc = tc_conv_set_affine(&plan, sc.data(), sh.data());
-  if (!rc) rc = launch_conv_tc(plan, x_dev, y_dev, stream);
+  if (!rc) rc = launch_conv_tc(plan, x_dev, y_dev, B, stream);
   ce = cudaStreamSynchronize(stream);
   tc_conv_release(&plan);
   if (rc) return rc;
@@ -820,7 +822,6 @@ int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int 
     }
   }
   im->w_floats = (long long)(Cin / im->KCI) * 2 * im->SQN * im->KCI;
-  im->grid = (unsigned)((long long)B * p.tiles_h * p.tiles_w);
   im->kernel = fire_tc_instance(im->KCI, im->SQN, im->KCE, &im->smem);
   void* vp = im;
   cudaError_t ce = cudaFuncSetAttribute(im->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -867,13 +868,16 @@ int tc_fused_fire_pack_weights(TcFusedFirePlan* plan, const float* w_sq, const f
   return SQDET_OK;
 }
 
-int launch_fused_fire_tc(const TcFusedFirePlan& plan, const float* x_dev, float* y_dev,
+int launch_fused_fire_tc(const TcFusedFirePlan& plan, const float* x_dev, float* y_dev, int n,
                          cudaStream_t stream) {
   const FusedImpl* im = static_cast<const FusedImpl*>(plan.impl);
   FireParams p = im->fp;
+  if (n < 1 || n > p.B) return fail(SQDET_ERR_INVALID_ARG, "launch_fused_fire_tc: image count outside [1, B]");
   p.x = x_dev;
   p.y = y_dev;
-  im->kernel<<<im->grid, NUM_THREADS, im->smem, stream>>>(p);
+  p.B = n;
+  const unsigned grid = (unsigned)((long long)n * p.tiles_h * p.tiles_w);
+  im->kernel<<<grid, NUM_THREADS, im->smem, stream>>>(p);
   SQ_CHECK_LAUNCH("fire_tc_kernel");
   return SQDET_OK;
 }
@@ -902,7 +906,7 @@ int fire_fused_oneshot(const float* x_dev, const float* w_sq_dev, const float* b
   }
   rc = tc_fused_fire_pack_weights(&plan, wsq.data(), bsq.data(), w1.data(), b1.data(), w3.data(),
                                   b3.data());
-  if (!rc) rc = launch_fused_fire_tc(plan, x_dev, y_dev, stream);
+  if (!rc) rc = launch_fused_fire_tc(plan, x_dev, y_dev, B, stream);
   ce = cudaStreamSynchronize(stream);
   tc_fused_fire_release(&plan);
   if (rc) return rc;

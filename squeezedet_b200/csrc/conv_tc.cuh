@@ -30,7 +30,10 @@ int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, const std::vect
 int tc_conv_pack_weights(TcConvPlan* plan, const std::vector<const float*>& w_hwio,
                          const std::vector<const float*>& bias);
 int tc_conv_set_affine(TcConvPlan* plan, const float* scale, const float* shift);
-int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, cudaStream_t stream);
+// Runs the plan over images [0, n) of its batch, 1 <= n <= the planned B: the same kernel and
+// chunks, with M = n * Ho * Wo and the grid sized to it.
+int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, int n,
+                   cudaStream_t stream);
 void tc_conv_release(TcConvPlan* plan);
 
 // The whole fire module (squeeze 1x1 -> expand 1x1 || 3x3 + concat) as ONE kernel: the squeeze
@@ -42,7 +45,8 @@ int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int 
 int tc_fused_fire_pack_weights(TcFusedFirePlan* plan, const float* w_sq, const float* b_sq,
                                const float* w_e1, const float* b_e1, const float* w_e3,
                                const float* b_e3);
-int launch_fused_fire_tc(const TcFusedFirePlan& plan, const float* x_dev, float* y_dev,
+// Runs the plan over images [0, n) of its batch, 1 <= n <= the planned B: n * tiles blocks.
+int launch_fused_fire_tc(const TcFusedFirePlan& plan, const float* x_dev, float* y_dev, int n,
                          cudaStream_t stream);
 void tc_fused_fire_release(TcFusedFirePlan* plan);
 // Stage-isolated one-kernel fire from device weights; synchronises.  Returns 1 when the shape is

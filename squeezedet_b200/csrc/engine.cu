@@ -121,11 +121,12 @@ struct sqdet_engine {
   int32_t* d_counts = nullptr;
   int max_dets = 0;
   float* d_input = nullptr;       // engine-owned input buffer (host-path + graph)
-  // CUDA graphs of one forward, keyed by (input pointer, stream); small LRU-less cache
+  // CUDA graphs of one forward, keyed by (input pointer, stream, image count); small LRU-less cache
   struct GraphEntry {
     cudaGraphExec_t exec = nullptr;
     const float* input = nullptr;
     cudaStream_t stream = nullptr;
+    int n = 0;
   };
   GraphEntry graphs[4];
   int graph_next = 0;
@@ -282,7 +283,9 @@ static const float* input_ptr(const sqdet_engine* e, int t, const float* images)
   return (t == 0 && images) ? images : e->tensors[t].dev;
 }
 
-static int run_launch(sqdet_engine* e, const Op& op, const Launch& l, const float* images,
+// One launch over images [0, n): every kernel takes the image count as a launch argument, so a
+// forward of n < B images runs the kernels planned for B on smaller grids.
+static int run_launch(sqdet_engine* e, const Op& op, const Launch& l, const float* images, int n,
                       cudaStream_t stream) {
   const Tensor& in = e->tensors[l.src];
   const float* x = input_ptr(e, l.src, images);
@@ -297,34 +300,35 @@ static int run_launch(sqdet_engine* e, const Op& op, const Launch& l, const floa
       a.scale = c.scale;
       a.shift = c.shift;
       a.y = y;
-      a.B = in.B; a.H = in.H; a.W = in.W; a.Cin = c.Cin; a.Cout = c.Cout;
+      a.B = n; a.H = in.H; a.W = in.W; a.Cin = c.Cin; a.Cout = c.Cout;
       a.size = c.size; a.stride = c.stride; a.padding = c.padding; a.relu = c.relu;
       a.y_cstride = e->tensors[l.dst].C;
       a.y_coff = c.y_coff;
       return launch_conv_simt(a, stream);
     }
     case L_CONV_TC:
-      return launch_conv_tc(l.tc, x, y, stream);
+      return launch_conv_tc(l.tc, x, y, n, stream);
     case L_CONV_POOL: {
       const ConvSpec& c = op.convs[0];
       return launch_conv_pool_simt(x, e->params[c.p_kernel].dev,
                                    c.p_bias >= 0 ? e->params[c.p_bias].dev : nullptr, c.scale,
-                                   c.shift, y, in.B, in.H, in.W, c.Cout, c.size, c.padding, c.relu,
+                                   c.shift, y, n, in.H, in.W, c.Cout, c.size, c.padding, c.relu,
                                    l.pool_padding, stream);
     }
     case L_FIRE_TC:
-      return launch_fused_fire_tc(l.fire, x, y, stream);
+      return launch_fused_fire_tc(l.fire, x, y, n, stream);
     case L_MAXPOOL:
-      return launch_maxpool(x, y, in.B, in.H, in.W, in.C, op.size, op.stride, op.padding, stream);
+      return launch_maxpool(x, y, n, in.H, in.W, in.C, op.size, op.stride, op.padding, stream);
     case L_ADD_RELU:
-      return launch_add_relu(x, input_ptr(e, op.src2, images), y, in.numel(), stream);
+      return launch_add_relu(x, input_ptr(e, op.src2, images), y, (int64_t)n * in.H * in.W * in.C,
+                             stream);
   }
   return fail(SQDET_ERR_STATE, "unknown launch kind");
 }
 
-static int run_op(sqdet_engine* e, const Op& op, const float* images, cudaStream_t stream) {
+static int run_op(sqdet_engine* e, const Op& op, const float* images, int n, cudaStream_t stream) {
   for (const Launch& l : op.launches) {
-    int rc = run_launch(e, op, l, images, stream);
+    int rc = run_launch(e, op, l, images, n, stream);
     if (rc) return rc;
   }
   return SQDET_OK;
@@ -389,28 +393,32 @@ static int run_allgather(sqdet_engine* e, void* comm, cudaStream_t stream) {
   return SQDET_OK;
 }
 
-// interpret_output, then the eval-order rescale when it is on
-static int run_interpret(sqdet_engine* e, cudaStream_t stream) {
+// interpret_output of images [0, n), then the eval-order rescale when it is on
+static int run_interpret(sqdet_engine* e, int n, cudaStream_t stream) {
   const sqdet_config& c = e->cfg;
   int rc = launch_interpret(e->tensors[e->preds].dev, e->d_anchors, e->d_boxes, e->d_probs,
-                            e->d_cls, c.batch_size, e->grid_h, e->grid_w, c.anchors_per_grid,
+                            e->d_cls, n, e->grid_h, e->grid_w, c.anchors_per_grid,
                             c.classes, c.image_width, c.image_height, c.exp_thresh, stream);
   if (rc || !e->rescale_on) return rc;
   return launch_rescale_boxes(e->d_boxes, e->d_scales + (size_t)e->scale_slot * c.batch_size * 2,
-                              c.batch_size, (int)e->num_anchors, stream);
+                              n, (int)e->num_anchors, stream);
 }
 
-// filter_prediction
-static int run_filter(sqdet_engine* e, cudaStream_t stream) {
+// filter_prediction of images [0, n); the counts of images [n, B) are set to 0, so the result blob
+// (records + counts) stays fully defined for the all-gather
+static int run_filter(sqdet_engine* e, int n, cudaStream_t stream) {
   const sqdet_config& c = e->cfg;
-  return launch_topk_nms(e->d_boxes, e->d_probs, e->d_cls, c.batch_size, (int)e->num_anchors,
-                         c.classes, c.top_n_detection, c.prob_thresh, c.nms_thresh, e->d_dets,
-                         e->d_counts, e->max_dets, stream);
+  int rc = launch_topk_nms(e->d_boxes, e->d_probs, e->d_cls, n, (int)e->num_anchors,
+                           c.classes, c.top_n_detection, c.prob_thresh, c.nms_thresh, e->d_dets,
+                           e->d_counts, e->max_dets, stream);
+  if (rc || n == c.batch_size) return rc;
+  SQ_CUDA(cudaMemsetAsync(e->d_counts + n, 0, sizeof(int32_t) * (size_t)(c.batch_size - n), stream));
+  return SQDET_OK;
 }
 
-static int run_postproc(sqdet_engine* e, cudaStream_t stream) {
-  int rc = run_interpret(e, stream);
-  if (!rc) rc = run_filter(e, stream);
+static int run_postproc(sqdet_engine* e, int n, cudaStream_t stream) {
+  int rc = run_interpret(e, n, stream);
+  if (!rc) rc = run_filter(e, n, stream);
   if (rc) return rc;
   if (e->gather_in_forward && e->comm) return run_allgather(e, e->comm, stream);
   return SQDET_OK;
@@ -480,28 +488,31 @@ static void drop_graph(sqdet_engine* e) {
   }
 }
 
-static int enqueue_all(sqdet_engine* e, const float* images_dev, cudaStream_t stream) {
+static int enqueue_all(sqdet_engine* e, const float* images_dev, int n, cudaStream_t stream) {
   for (const auto& op : e->ops) {
-    int rc = run_op(e, op, images_dev, stream);
+    int rc = run_op(e, op, images_dev, n, stream);
     if (rc) return rc;
   }
-  return run_postproc(e, stream);
+  return run_postproc(e, n, stream);
 }
 
-static int forward_impl(sqdet_engine* e, const float* images_dev, cudaStream_t stream) {
+// The forward over images [0, n) of `images_dev`, 1 <= n <= B.
+static int forward_impl(sqdet_engine* e, const float* images_dev, int n, cudaStream_t stream) {
   if (!e) return fail(SQDET_ERR_INVALID_ARG, "null engine");
   if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_forward before sqdet_finalize");
   if (!images_dev) return fail(SQDET_ERR_INVALID_ARG, "null images pointer");
+  if (n < 1 || n > e->cfg.batch_size)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_n: n must be in [1, batch_size]");
   DeviceGuard guard(e->device);
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
   int rc = prepare_params(e);
   if (rc) return rc;
   e->scale_slot = (e->d_in_slot[1] && images_dev == e->d_in_slot[1]) ? 1 : 0;
   const bool can_graph = e->use_graph && stream != nullptr;   // legacy stream cannot capture
-  if (!can_graph) return enqueue_all(e, images_dev, stream);
+  if (!can_graph) return enqueue_all(e, images_dev, n, stream);
   sqdet_engine::GraphEntry* hit = nullptr;
   for (auto& g : e->graphs)
-    if (g.exec && g.input == images_dev && g.stream == stream) hit = &g;
+    if (g.exec && g.input == images_dev && g.stream == stream && g.n == n) hit = &g;
   if (!hit) {
     sqdet_engine::GraphEntry& slot = e->graphs[e->graph_next];
     e->graph_next = (e->graph_next + 1) % 4;
@@ -509,7 +520,7 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, cudaStream_t s
     slot = sqdet_engine::GraphEntry();
     cudaGraph_t graph = nullptr;
     SQ_CUDA(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-    rc = enqueue_all(e, images_dev, stream);
+    rc = enqueue_all(e, images_dev, n, stream);
     cudaError_t ce = cudaStreamEndCapture(stream, &graph);
     if (rc) {
       if (graph) cudaGraphDestroy(graph);
@@ -521,6 +532,7 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, cudaStream_t s
     if (ce != cudaSuccess) return cuda_fail(ce, "cudaGraphInstantiate");
     slot.input = images_dev;
     slot.stream = stream;
+    slot.n = n;
     hit = &slot;
   }
   SQ_CUDA(cudaGraphLaunch(hit->exec, stream));
@@ -545,18 +557,18 @@ static int begin_submit(sqdet_engine* e, const char* what, int* slot) {
   return SQDET_OK;
 }
 
-// The forward over the slot's input on the compute stream, then the records and counts back to
-// the caller's buffers; ev_done marks the slot's buffers free again.
-static int finish_submit(sqdet_engine* e, int slot, sqdet_det* dets, int32_t* counts) {
-  const size_t B = (size_t)e->cfg.batch_size;
+// The forward over images [0, n) of the slot's input on the compute stream, then their records
+// and counts back to the caller's buffers; ev_done marks the slot's buffers free again.
+static int finish_submit(sqdet_engine* e, int slot, int n, sqdet_det* dets, int32_t* counts) {
   cudaStream_t ks = e->own_stream;
-  int rc = forward_impl(e, e->d_in_slot[slot], ks);
+  int rc = forward_impl(e, e->d_in_slot[slot], n, ks);
   if (rc) return rc;
   if (dets)
-    SQ_CUDA(cudaMemcpyAsync(dets, e->d_dets, sizeof(sqdet_det) * B * e->max_dets,
+    SQ_CUDA(cudaMemcpyAsync(dets, e->d_dets, sizeof(sqdet_det) * (size_t)n * e->max_dets,
                             cudaMemcpyDeviceToHost, ks));
   if (counts)
-    SQ_CUDA(cudaMemcpyAsync(counts, e->d_counts, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, ks));
+    SQ_CUDA(cudaMemcpyAsync(counts, e->d_counts, sizeof(int32_t) * (size_t)n,
+                            cudaMemcpyDeviceToHost, ks));
   SQ_CUDA(cudaEventRecord(e->ev_done[slot], ks));
   e->slot_used[slot] = true;
   ++e->n_submitted;
@@ -1014,7 +1026,11 @@ int sqdet_op_info(sqdet_engine* e, int index, char* name_buf, int name_cap, int6
 }
 
 int sqdet_forward(sqdet_engine* e, const float* images_dev, void* stream) {
-  return forward_impl(e, images_dev, (cudaStream_t)stream);
+  return sqdet_forward_n(e, images_dev, e ? e->cfg.batch_size : 0, stream);
+}
+
+int sqdet_forward_n(sqdet_engine* e, const float* images_dev, int n, void* stream) {
+  return forward_impl(e, images_dev, n, (cudaStream_t)stream);
 }
 
 int sqdet_forward_profiled(sqdet_engine* e, const float* images_dev, void* stream_v,
@@ -1032,16 +1048,17 @@ int sqdet_forward_profiled(sqdet_engine* e, const float* images_dev, void* strea
     SQ_CUDA(cudaEventCreate(&ev));
     e->prof_events.push_back(ev);
   }
+  const int B = e->cfg.batch_size;
   SQ_CUDA(cudaEventRecord(e->prof_events[0], stream));
   for (int i = 0; i < (int)e->ops.size(); ++i) {
-    rc = run_op(e, e->ops[i], images_dev, stream);
+    rc = run_op(e, e->ops[i], images_dev, B, stream);
     if (rc) return rc;
     SQ_CUDA(cudaEventRecord(e->prof_events[i + 1], stream));
   }
-  rc = run_interpret(e, stream);
+  rc = run_interpret(e, B, stream);
   if (rc) return rc;
   SQ_CUDA(cudaEventRecord(e->prof_events[n - 1], stream));
-  rc = run_filter(e, stream);
+  rc = run_filter(e, B, stream);
   if (rc) return rc;
   SQ_CUDA(cudaEventRecord(e->prof_events[n], stream));
   SQ_CUDA(cudaEventSynchronize(e->prof_events[n]));
@@ -1072,7 +1089,7 @@ int sqdet_detect(sqdet_engine* e, const float* images, float* det_boxes, float* 
   const sqdet_config& c = e->cfg;
   const size_t in_bytes = sizeof(float) * (size_t)e->tensors[0].numel();
   SQ_CUDA(cudaMemcpyAsync(e->d_input, images, in_bytes, cudaMemcpyHostToDevice, stream));
-  int rc = forward_impl(e, e->d_input, stream);
+  int rc = forward_impl(e, e->d_input, c.batch_size, stream);
   if (rc) return rc;
   const size_t BA = (size_t)c.batch_size * (size_t)e->num_anchors;
   if (det_boxes)
@@ -1129,7 +1146,7 @@ int sqdet_submit(sqdet_engine* e, const void* images, int img_type, sqdet_det* d
                            e->bgr_means[1], e->bgr_means[2], ks);
     if (rc) return rc;
   }
-  return finish_submit(e, slot, dets, counts);
+  return finish_submit(e, slot, c.batch_size, dets, counts);
 }
 
 int sqdet_wait(sqdet_engine* e) {
@@ -1177,20 +1194,29 @@ int sqdet_set_box_scale(sqdet_engine* e, const float* xy_scales) {
 int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames, const int32_t* heights,
                         const int32_t* widths, int order, int rescale, sqdet_det* dets,
                         int32_t* counts) {
+  return sqdet_submit_frames_n(e, e ? e->cfg.batch_size : 0, frames, heights, widths, order,
+                               rescale, dets, counts);
+}
+
+int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
+                          const int32_t* heights, const int32_t* widths, int order, int rescale,
+                          sqdet_det* dets, int32_t* counts) {
   if (!e || !frames || !heights || !widths)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit_frames: null argument");
   if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_submit_frames before sqdet_finalize");
   if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit_frames: order must be 0 (demo) or 1 (eval)");
+  const sqdet_config& c = e->cfg;
+  const int B = c.batch_size;
+  if (n < 1 || n > B)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit_frames_n: n must be in [1, batch_size]");
   DeviceGuard guard(e->device);
   int slot;
   int rc = begin_submit(e, "sqdet_submit_frames", &slot);
   if (rc) return rc;
-  const sqdet_config& c = e->cfg;
-  const int B = c.batch_size;
   size_t total = 0;
-  std::vector<size_t> off((size_t)B);
-  for (int i = 0; i < B; ++i) {
+  std::vector<size_t> off((size_t)n);
+  for (int i = 0; i < n; ++i) {
     if (!frames[i] || heights[i] <= 0 || widths[i] <= 0)
       return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit_frames: empty frame");
     off[(size_t)i] = total;
@@ -1206,14 +1232,14 @@ int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames, const int
     SQ_CUDA(cudaMalloc(&e->d_frames[slot], total));
     e->frames_cap[slot] = total;
   }
-  for (int i = 0; i < B; ++i)
+  for (int i = 0; i < n; ++i)
     SQ_CUDA(cudaMemcpyAsync(e->d_frames[slot] + off[(size_t)i], frames[i],
                             (size_t)heights[i] * widths[i] * 3, cudaMemcpyHostToDevice, cs));
   SQ_CUDA(cudaEventRecord(e->ev_h2d[slot], cs));
   // eval order: boxes go back to each frame's own pixel grid before the filter (eval.py:80-87)
   if (rescale) {
-    std::vector<float> sc((size_t)B * 2);
-    for (int i = 0; i < B; ++i) {
+    std::vector<float> sc((size_t)B * 2, 1.f);   // images [n, B) are not run; 1 keeps the table valid
+    for (int i = 0; i < n; ++i) {
       // eval.py:72-74 / imdb.py:93-95: x_scale = mc.IMAGE_WIDTH / orig_w (Python floats = double)
       sc[(size_t)2 * i] = (float)((double)c.image_width / (double)widths[i]);
       sc[(size_t)2 * i + 1] = (float)((double)c.image_height / (double)heights[i]);
@@ -1223,7 +1249,7 @@ int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames, const int
       if (rc) return rc;
     }
     // this slot's half of the table, in stream order behind the forward that last read it
-    SQ_CUDA(cudaMemcpyAsync(e->d_scales + (size_t)slot * B * 2, sc.data(), sizeof(float) * B * 2,
+    SQ_CUDA(cudaMemcpyAsync(e->d_scales + (size_t)slot * B * 2, sc.data(), sizeof(float) * n * 2,
                             cudaMemcpyHostToDevice, ks));
   } else if (e->rescale_on) {
     rc = sqdet_set_box_scale(e, nullptr);
@@ -1231,14 +1257,14 @@ int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames, const int
   }
   SQ_CUDA(cudaStreamWaitEvent(ks, e->ev_h2d[slot], 0));
   const size_t img_floats = (size_t)c.image_height * c.image_width * 3;
-  for (int i = 0; i < B; ++i) {
+  for (int i = 0; i < n; ++i) {
     rc = launch_resize_meansub_u8(e->d_frames[slot] + off[(size_t)i], heights[i], widths[i],
                                   e->d_in_slot[slot] + (size_t)i * img_floats, c.image_height,
                                   c.image_width, e->bgr_means[0], e->bgr_means[1],
                                   e->bgr_means[2], order == SQDET_PRE_SUB_THEN_RESIZE, ks);
     if (rc) return rc;
   }
-  return finish_submit(e, slot, dets, counts);
+  return finish_submit(e, slot, n, dets, counts);
 }
 
 // ---- multi-GPU: ONE all-gather of the filtered records ---------------------------------------------

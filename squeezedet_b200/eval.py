@@ -1,14 +1,17 @@
 #!/usr/bin/env python
 """Evaluation loop — drop-in for the detection part of reference ``src/eval.py``
 (`eval_once`, lines 48-134), same flags: --dataset --data_path --image_set --eval_dir
---checkpoint_path --run_once --net --gpu.
+--checkpoint_path --run_once --net --gpu, plus --batch_size.
 
 Per image, in the reference's order (eval.py:69-92): the uint8 frame goes to the GPU, where it
 is converted to float32, has the BGR means subtracted and is resized (src/dataset/imdb.py:85-97);
 forward; ALL det boxes are rescaled to the original image (eval.py:83-84) and only then
 filtered (filter_prediction + NMS on original-image coordinates, eval.py:86-87) - one
-`sqdet_submit_frames(..., order=eval, rescale=1)` call; corner format + score go into
-all_boxes[cls][image].  Then the KITTI detection files are written
+`sqdet_submit_frames_n(..., order=eval, rescale=1)` call per group of --batch_size images
+(default 1, the reference's image-by-image loop, eval.py:150); the last group is short and runs
+on the same engine.  Two groups are in flight on the GPU while a thread pool decodes the next one
+with cv2.imread.  Corner format + score go into all_boxes[cls][image].  Then the KITTI detection
+files are written
 (src/dataset/kitti.py:100-127) and the reference's unmodified `evaluate_object` binary
 (built by oracle/build_kitti_eval.sh) is invoked and its stats_*_ap.txt parsed
 (kitti.py:129-159).  The TensorBoard summaries and the checkpoint-polling loop
@@ -17,8 +20,11 @@ all_boxes[cls][image].  Then the KITTI detection files are written
 from __future__ import annotations
 
 import argparse
+import collections
 import os
 import subprocess
+import time
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
@@ -37,6 +43,8 @@ def parse_flags(argv=None):
   ap.add_argument('--run_once', action='store_true', default=True)
   ap.add_argument('--net', default='squeezeDet', help='Neural net architecture.')
   ap.add_argument('--gpu', default='0', help='gpu id.')
+  ap.add_argument('--batch_size', type=int, default=1,
+                  help='Images per forward; the last group of the image set may be shorter.')
   return ap.parse_args(argv)
 
 
@@ -77,6 +85,21 @@ def detections_to_all_boxes(records, count, scale, num_classes):
   return out
 
 
+def _read_frame(path):
+  """cv2.imread of one frame (uint8 BGR, original size) and the seconds it took."""
+  import cv2
+  t0 = time.time()
+  frame = cv2.imread(path)
+  return frame, time.time() - t0
+
+
+def _charge(timer, seconds, images):
+  """Adds `seconds` spent on `images` images to `timer`, keeping its average per image."""
+  timer.total_time += seconds
+  timer.calls += images
+  timer.average_time = timer.total_time / timer.calls
+
+
 EVAL_TOOL = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'oracle',
                          '_ref', 'evaluate_object')   # built by oracle/build_kitti_eval.sh
 
@@ -89,7 +112,9 @@ def eval_once(flags):
   assert flags.net in NETS, 'Selected neural net architecture not supported: {}'.format(flags.net)
   cls_name, cfg_name = NETS[flags.net]
   mc = getattr(cfg, cfg_name)()
-  mc.BATCH_SIZE = 1                     # the reference evaluates image by image (eval.py:150)
+  k = int(flags.batch_size)
+  assert k >= 1, '--batch_size must be at least 1'
+  mc.BATCH_SIZE = k                     # 1: the reference evaluates image by image (eval.py:150)
   mc.LOAD_PRETRAINED_MODEL = False
   model = getattr(nets, cls_name)(mc, int(flags.gpu))
   if flags.checkpoint_path == 'synthetic':
@@ -102,24 +127,61 @@ def eval_once(flags):
   image_dir = os.path.join(flags.data_path, 'training', 'image_2')
   num_images = len(image_ids)
   all_boxes = [[[] for _ in range(num_images)] for _ in range(mc.CLASSES)]
+  # every timer is an average per image: im_read = cv2.imread time, im_detect = host time spent
+  # in the submit and wait calls, misc = records -> all_boxes
   _t = {'im_detect': Timer(), 'im_read': Timer(), 'misc': Timer()}
-  for i, index in enumerate(image_ids):
-    import cv2
-    _t['im_read'].tic()
-    frame = cv2.imread(os.path.join(image_dir, index + '.png'))     # uint8 BGR, original size
-    _t['im_read'].toc()
-    _t['im_detect'].tic()
-    # imdb.py:85-97 pre-processing, forward, eval.py:83-84 rescale, filter: one GPU pass
-    dets, counts = model.detect_frames([frame], order='eval', rescale=True)
-    _t['im_detect'].toc()
-    _t['misc'].tic()
-    per_class = detections_to_all_boxes(dets[0], int(counts[0]), None, mc.CLASSES)
-    for c in range(mc.CLASSES):
-      all_boxes[c][i] = per_class[c]
-    _t['misc'].toc()
-    print('im_detect: {:d}/{:d} im_read: {:.3f}s detect: {:.3f}s misc: {:.3f}s'.format(
-        i + 1, num_images, _t['im_read'].average_time, _t['im_detect'].average_time,
-        _t['misc'].average_time))
+  from ._lib import DET_DTYPE, PinnedArray
+  groups = [list(range(s, min(s + k, num_images))) for s in range(0, num_images, k)]
+  # one pinned result slot per group in flight (pinned, so the copies back stay asynchronous)
+  dets_buf = [PinnedArray((k, model.max_dets), DET_DTYPE) for _ in range(2)]
+  counts_buf = [PinnedArray((k,), np.int32) for _ in range(2)]
+
+  def collect(gi):
+    """The results of group gi, after its wait()."""
+    dets, counts = dets_buf[gi & 1].array, counts_buf[gi & 1].array
+    for j, i in enumerate(groups[gi]):
+      _t['misc'].tic()
+      per_class = detections_to_all_boxes(dets[j], int(counts[j]), None, mc.CLASSES)
+      for c in range(mc.CLASSES):
+        all_boxes[c][i] = per_class[c]
+      _t['misc'].toc()
+      print('im_detect: {:d}/{:d} im_read: {:.3f}s detect: {:.3f}s misc: {:.3f}s'.format(
+          i + 1, num_images, _t['im_read'].average_time, _t['im_detect'].average_time,
+          _t['misc'].average_time))
+
+  with ThreadPoolExecutor(max_workers=max(1, min(k, os.cpu_count() or 1, 8))) as pool:
+    def start_read(gi):
+      return [pool.submit(_read_frame, os.path.join(image_dir, image_ids[i] + '.png'))
+              for i in groups[gi]]
+
+    in_flight = collections.deque()        # (group, its frames), oldest first
+    reading = start_read(0) if groups else []
+    for gi in range(len(groups)):
+      read = [f.result() for f in reading]
+      _charge(_t['im_read'], sum(s for _, s in read), len(read))
+      frames = [f for f, _ in read]
+      if gi + 1 < len(groups):
+        reading = start_read(gi + 1)       # decodes while this group runs on the GPU
+      t0 = time.time()
+      # imdb.py:85-97 pre-processing, forward, eval.py:83-84 rescale, filter: one GPU pass
+      model.submit_frames(frames, dets_buf[gi & 1].ptr, counts_buf[gi & 1].ptr, order='eval',
+                          rescale=True)
+      in_flight.append((gi, frames))
+      done = None
+      if len(in_flight) == 2:
+        model.wait()
+        done = in_flight.popleft()[0]
+      _charge(_t['im_detect'], time.time() - t0, len(frames))
+      if done is not None:
+        collect(done)
+    while in_flight:
+      t0 = time.time()
+      model.wait()
+      done = in_flight.popleft()[0]
+      _charge(_t['im_detect'], time.time() - t0, len(groups[done]))
+      collect(done)
+  for buf in dets_buf + counts_buf:
+    buf.free()
 
   det_dir = os.path.join(flags.eval_dir, 'detection_files_{:s}'.format('0'), 'data')
   result_dir = write_kitti_detections(det_dir, image_ids, mc.CLASS_NAMES, all_boxes)

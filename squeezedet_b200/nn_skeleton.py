@@ -360,34 +360,36 @@ class ModelSkeleton:
 
   # ---- variable-size uint8 frames: pre-processing on the GPU (demo.py:187-190 / imdb.py:85-97) ----
   def submit_frames(self, frames, dets_ptr, counts_ptr, order='demo', rescale=False):
-    """frames: list of B uint8 BGR arrays [h_i, w_i, 3] as cv2.imread returns them.  The engine
-    resizes (cv2 float32 INTER_LINEAR) to (mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT) and subtracts
-    mc.BGR_MEANS in the reference order ('demo': resize then subtract, demo.py:187-190; 'eval':
-    subtract then resize, imdb.py:85-97).  rescale=True: boxes are divided by each frame's
-    (x_scale, y_scale) BEFORE filter_prediction, like eval.py:80-87.  Same wait() contract as
-    submit(); the frame arrays must stay alive until then."""
-    B = self.mc.BATCH_SIZE
-    if len(frames) != B:
-      raise ValueError('need %d frames, got %d' % (B, len(frames)))
+    """frames: list of n uint8 BGR arrays [h_i, w_i, 3] as cv2.imread returns them,
+    1 <= n <= mc.BATCH_SIZE.  The engine resizes (cv2 float32 INTER_LINEAR) to
+    (mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT) and subtracts mc.BGR_MEANS in the reference order ('demo':
+    resize then subtract, demo.py:187-190; 'eval': subtract then resize, imdb.py:85-97).
+    rescale=True: boxes are divided by each frame's (x_scale, y_scale) BEFORE filter_prediction,
+    like eval.py:80-87.  dets_ptr / counts_ptr receive n rows (sqdet_submit_frames_n: a short
+    batch runs the kernels planned for BATCH_SIZE, so image i's records equal those of a full
+    batch).  Same wait() contract as submit(); the frame arrays must stay alive until then."""
+    B, n = self.mc.BATCH_SIZE, len(frames)
+    if not 1 <= n <= B:
+      raise ValueError('need 1 to %d frames, got %d' % (B, n))
     arrs = []
     for f in frames:
       a = np.ascontiguousarray(np.asarray(f, dtype=np.uint8))
       if a.ndim != 3 or a.shape[2] != 3:
         raise ValueError('a frame must be uint8 [h, w, 3], got %r' % (a.shape,))
       arrs.append(a)
-    ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in arrs])
-    hs = (C.c_int32 * B)(*[a.shape[0] for a in arrs])
-    ws = (C.c_int32 * B)(*[a.shape[1] for a in arrs])
+    ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
+    hs = (C.c_int32 * n)(*[a.shape[0] for a in arrs])
+    ws = (C.c_int32 * n)(*[a.shape[1] for a in arrs])
     code = {'demo': 0, 'eval': 1}[order]
     self._frames_alive = arrs
-    _lib.check(self._lib.sqdet_submit_frames(self._engine, ptrs, hs, ws, code,
-                                             int(bool(rescale)), dets_ptr, counts_ptr))
+    _lib.check(self._lib.sqdet_submit_frames_n(self._engine, n, ptrs, hs, ws, code,
+                                               int(bool(rescale)), dets_ptr, counts_ptr))
 
   def detect_frames(self, frames, order='demo', rescale=False):
-    """Synchronous convenience over submit_frames: -> (dets [B,max_dets], counts [B])."""
-    B = self.mc.BATCH_SIZE
-    dets = np.empty((B, self.max_dets), _lib.DET_DTYPE)
-    counts = np.empty((B,), np.int32)
+    """Synchronous convenience over submit_frames: n frames -> (dets [n,max_dets], counts [n])."""
+    n = len(frames)
+    dets = np.empty((n, self.max_dets), _lib.DET_DTYPE)
+    counts = np.empty((n,), np.int32)
     self.submit_frames(frames, dets.ctypes.data, counts.ctypes.data, order, rescale)
     self.wait()
     return dets, counts
@@ -482,8 +484,14 @@ class ModelSkeleton:
     return out
 
   # device-resident path (no host copies; used by bench / multi-GPU runner)
-  def forward_device(self, images_dev_ptr, stream=None):
-    _lib.check(self._lib.sqdet_forward(self._engine, images_dev_ptr, stream))
+  def forward_device(self, images_dev_ptr, stream=None, n=None):
+    """Forward of the device images at `images_dev_ptr`: all BATCH_SIZE of them, or only the
+    first n (1 <= n <= BATCH_SIZE; sqdet_forward_n), in which case the buffer needs to hold just
+    those n images and result rows [n, BATCH_SIZE) are left untouched (counts set to 0)."""
+    if n is None:
+      _lib.check(self._lib.sqdet_forward(self._engine, images_dev_ptr, stream))
+    else:
+      _lib.check(self._lib.sqdet_forward_n(self._engine, images_dev_ptr, int(n), stream))
 
   def forward_profiled(self, images_dev_ptr, stream=None):
     n = self._lib.sqdet_num_ops(self._engine)
