@@ -188,7 +188,8 @@ int sqdet_wait(sqdet_engine* e);
  * SQDET_PRE_SUB_THEN_RESIZE: src/dataset/imdb.py:85-97) on the GPU, then the forward; same
  * depth-2 pipelining and sqdet_wait contract as sqdet_submit.  rescale != 0 additionally divides
  * every det box by (x_scale, y_scale) = (IMAGE_WIDTH / widths[i], IMAGE_HEIGHT / heights[i])
- * BEFORE filter_prediction, i.e. the order of src/eval.py:80-87.                            */
+ * BEFORE filter_prediction, i.e. the order of src/eval.py:80-87.  `rescale` applies to this one
+ * submission only; the table of sqdet_set_box_scale is never applied here.                  */
 int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames,
                         const int32_t* heights, const int32_t* widths, int order,
                         int rescale, sqdet_det* dets, int32_t* counts);
@@ -201,10 +202,13 @@ int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
                           const int32_t* heights, const int32_t* widths, int order,
                           int rescale, sqdet_det* dets, int32_t* counts);
 /* src/eval.py:83-84 for callers that resize on the host: xy_scales = B pairs (x_scale,
- * y_scale), host memory; every later forward divides det_boxes[b,:,0::2] by x_scale and
- * [b,:,1::2] by y_scale (float32, as numpy does) between interpret_output and
- * filter_prediction, so det_boxes, the records and the NMS all live on the original image.
- * NULL switches it off.  Synchronous (waits for in-flight forwards).                       */
+ * y_scale), host memory; every later forward of the paths fed already-resized images
+ * (sqdet_forward(_n), sqdet_forward_profiled, sqdet_detect, sqdet_submit) divides
+ * det_boxes[b,:,0::2] by x_scale and [b,:,1::2] by y_scale (float32, as numpy does) between
+ * interpret_output and filter_prediction, so det_boxes, the records and the NMS all live on the
+ * original image.  sqdet_submit_frames(_n) does not use this table: its `rescale` argument
+ * decides per submission.  NULL switches it off.  Synchronous (waits for in-flight forwards).
+ * sqdet_launches_per_forward counts the rescale launch while a table is set.               */
 int sqdet_set_box_scale(sqdet_engine* e, const float* xy_scales);
 /* Kernel launches issued by one sqdet_forward (for accounting).                        */
 int sqdet_launches_per_forward(sqdet_engine* e);

@@ -95,6 +95,16 @@ struct Op {
   std::vector<Launch> launches;  // what the op runs, in order; empty for a pool its producer absorbed
 };
 
+// One of the two pipeline slots of the host path (sqdet_submit, sqdet_submit_frames_n).
+struct Slot {
+  float* input = nullptr;        // fp32 network input; slot 0's is tensors[0].dev
+  uint8_t* staging = nullptr;    // uint8 images or frames as uploaded; grow-only
+  size_t staging_cap = 0;
+  float* scales = nullptr;       // B (x_scale, y_scale) pairs of a rescaled frames submission
+  cudaEvent_t h2d = nullptr, done = nullptr;   // the upload; the forward and its copies back
+  bool used = false;
+};
+
 }  // namespace sqdet
 
 using namespace sqdet;
@@ -120,35 +130,25 @@ struct sqdet_engine {
   sqdet_det* d_dets = nullptr;
   int32_t* d_counts = nullptr;
   int max_dets = 0;
-  float* d_input = nullptr;       // engine-owned input buffer (host-path + graph)
-  // CUDA graphs of one forward, keyed by (input pointer, stream, image count); small LRU-less cache
+  // CUDA graphs of one forward, keyed by (input, stream, image count, scales); small LRU-less cache
   struct GraphEntry {
     cudaGraphExec_t exec = nullptr;
     const float* input = nullptr;
     cudaStream_t stream = nullptr;
     int n = 0;
+    const float* scales = nullptr;
   };
   GraphEntry graphs[4];
   int graph_next = 0;
   bool use_graph = true;
   // pipelined host path (sqdet_submit / sqdet_wait), depth 2
   cudaStream_t copy_stream = nullptr;
-  float* d_in_slot[2] = {nullptr, nullptr};       // slot 0 aliases tensors[0].dev
-  uint8_t* d_u8_slot[2] = {nullptr, nullptr};
-  cudaEvent_t ev_h2d[2] = {nullptr, nullptr};
-  cudaEvent_t ev_done[2] = {nullptr, nullptr};
-  bool slot_used[2] = {false, false};
+  Slot slots[2];
   long long n_submitted = 0, n_waited = 0;
   double bgr_means[3] = {103.939, 116.779, 123.68};   // config.py:72
   cudaStream_t own_stream = nullptr;
   std::vector<cudaEvent_t> prof_events;
-  // eval-order rescale (src/eval.py:83-84): det_boxes / (x_scale, y_scale) BEFORE the filter
-  float* d_scales = nullptr;      // [2 pipeline slots][B][2] device
-  int scale_slot = 0;             // half read by the forward being enqueued
-  bool rescale_on = false;
-  // variable-size uint8 frames (sqdet_submit_frames): one staging buffer per pipeline slot
-  uint8_t* d_frames[2] = {nullptr, nullptr};
-  size_t frames_cap[2] = {0, 0};
+  float* box_scale = nullptr;     // sqdet_set_box_scale's B (x_scale, y_scale) pairs, or null
   // multi-GPU: the ONE collective of the path, ncclAllGather of the result blob
   void* comm = nullptr;           // ncclComm_t
   bool comm_owned = false;
@@ -393,15 +393,14 @@ static int run_allgather(sqdet_engine* e, void* comm, cudaStream_t stream) {
   return SQDET_OK;
 }
 
-// interpret_output of images [0, n), then the eval-order rescale when it is on
-static int run_interpret(sqdet_engine* e, int n, cudaStream_t stream) {
+// interpret_output of images [0, n), then the eval-order rescale by `scales` unless it is null
+static int run_interpret(sqdet_engine* e, int n, const float* scales, cudaStream_t stream) {
   const sqdet_config& c = e->cfg;
   int rc = launch_interpret(e->tensors[e->preds].dev, e->d_anchors, e->d_boxes, e->d_probs,
                             e->d_cls, n, e->grid_h, e->grid_w, c.anchors_per_grid,
                             c.classes, c.image_width, c.image_height, c.exp_thresh, stream);
-  if (rc || !e->rescale_on) return rc;
-  return launch_rescale_boxes(e->d_boxes, e->d_scales + (size_t)e->scale_slot * c.batch_size * 2,
-                              n, (int)e->num_anchors, stream);
+  if (rc || !scales) return rc;
+  return launch_rescale_boxes(e->d_boxes, scales, n, (int)e->num_anchors, stream);
 }
 
 // filter_prediction of images [0, n); the counts of images [n, B) are set to 0, so the result blob
@@ -416,8 +415,8 @@ static int run_filter(sqdet_engine* e, int n, cudaStream_t stream) {
   return SQDET_OK;
 }
 
-static int run_postproc(sqdet_engine* e, int n, cudaStream_t stream) {
-  int rc = run_interpret(e, n, stream);
+static int run_postproc(sqdet_engine* e, int n, const float* scales, cudaStream_t stream) {
+  int rc = run_interpret(e, n, scales, stream);
   if (!rc) rc = run_filter(e, n, stream);
   if (rc) return rc;
   if (e->gather_in_forward && e->comm) return run_allgather(e, e->comm, stream);
@@ -488,16 +487,18 @@ static void drop_graph(sqdet_engine* e) {
   }
 }
 
-static int enqueue_all(sqdet_engine* e, const float* images_dev, int n, cudaStream_t stream) {
+static int enqueue_all(sqdet_engine* e, const float* images_dev, int n, const float* scales,
+                       cudaStream_t stream) {
   for (const auto& op : e->ops) {
     int rc = run_op(e, op, images_dev, n, stream);
     if (rc) return rc;
   }
-  return run_postproc(e, n, stream);
+  return run_postproc(e, n, scales, stream);
 }
 
-// The forward over images [0, n) of `images_dev`, 1 <= n <= B.
-static int forward_impl(sqdet_engine* e, const float* images_dev, int n, cudaStream_t stream) {
+// The forward over images [0, n) of `images_dev`, 1 <= n <= B, rescaled by `scales` unless null.
+static int forward_impl(sqdet_engine* e, const float* images_dev, int n, const float* scales,
+                        cudaStream_t stream) {
   if (!e) return fail(SQDET_ERR_INVALID_ARG, "null engine");
   if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_forward before sqdet_finalize");
   if (!images_dev) return fail(SQDET_ERR_INVALID_ARG, "null images pointer");
@@ -507,12 +508,12 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, int n, cudaStr
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
   int rc = prepare_params(e);
   if (rc) return rc;
-  e->scale_slot = (e->d_in_slot[1] && images_dev == e->d_in_slot[1]) ? 1 : 0;
   const bool can_graph = e->use_graph && stream != nullptr;   // legacy stream cannot capture
-  if (!can_graph) return enqueue_all(e, images_dev, n, stream);
+  if (!can_graph) return enqueue_all(e, images_dev, n, scales, stream);
   sqdet_engine::GraphEntry* hit = nullptr;
   for (auto& g : e->graphs)
-    if (g.exec && g.input == images_dev && g.stream == stream && g.n == n) hit = &g;
+    if (g.exec && g.input == images_dev && g.stream == stream && g.n == n && g.scales == scales)
+      hit = &g;
   if (!hit) {
     sqdet_engine::GraphEntry& slot = e->graphs[e->graph_next];
     e->graph_next = (e->graph_next + 1) % 4;
@@ -520,7 +521,7 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, int n, cudaStr
     slot = sqdet_engine::GraphEntry();
     cudaGraph_t graph = nullptr;
     SQ_CUDA(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-    rc = enqueue_all(e, images_dev, n, stream);
+    rc = enqueue_all(e, images_dev, n, scales, stream);
     cudaError_t ce = cudaStreamEndCapture(stream, &graph);
     if (rc) {
       if (graph) cudaGraphDestroy(graph);
@@ -533,6 +534,7 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, int n, cudaStr
     slot.input = images_dev;
     slot.stream = stream;
     slot.n = n;
+    slot.scales = scales;
     hit = &slot;
   }
   SQ_CUDA(cudaGraphLaunch(hit->exec, stream));
@@ -541,27 +543,52 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, int n, cudaStr
 
 // Pipelined host path (sqdet_submit, sqdet_submit_frames): refuses a third batch in flight, sets
 // the pipeline up on first use and picks the slot of this submission.
-static int begin_submit(sqdet_engine* e, const char* what, int* slot) {
+static int begin_submit(sqdet_engine* e, const char* what, Slot** slot) {
   if (e->n_submitted - e->n_waited >= 2)
     return fail(SQDET_ERR_STATE, std::string(what) + ": two batches already in flight; call sqdet_wait");
   if (!e->copy_stream) {
     SQ_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-    e->d_in_slot[0] = e->tensors[0].dev;
-    SQ_CUDA(cudaMalloc(&e->d_in_slot[1], sizeof(float) * (size_t)e->tensors[0].numel()));
-    for (int k = 0; k < 2; ++k) {
-      SQ_CUDA(cudaEventCreateWithFlags(&e->ev_h2d[k], cudaEventDisableTiming));
-      SQ_CUDA(cudaEventCreateWithFlags(&e->ev_done[k], cudaEventDisableTiming));
+    SQ_CUDA(cudaMalloc(&e->slots[1].input, sizeof(float) * (size_t)e->tensors[0].numel()));
+    for (Slot& s : e->slots) {
+      SQ_CUDA(cudaEventCreateWithFlags(&s.h2d, cudaEventDisableTiming));
+      SQ_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
     }
   }
-  *slot = (int)(e->n_submitted & 1);
+  *slot = &e->slots[e->n_submitted & 1];
+  return SQDET_OK;
+}
+
+// One submission's host-to-device copies on the copy stream, behind the slot's previous forward:
+// host buffer i (bytes[i] long) goes to offset off[i] of the slot's fp32 input when `to_input`, else
+// of its uint8 staging buffer, grown when too small.  The compute stream then waits for them.
+static int upload(sqdet_engine* e, Slot& s, bool to_input, int count, const uint8_t* const* src,
+                  const size_t* bytes, const size_t* off) {
+  cudaStream_t cs = e->copy_stream;
+  // the slot's buffers are free once the forward that last read them has finished
+  if (s.used) SQ_CUDA(cudaStreamWaitEvent(cs, s.done, 0));
+  const size_t total = off[count - 1] + bytes[count - 1];
+  if (!to_input && s.staging_cap < total) {
+    // growing the staging buffer: the slot's previous forward must be done with it
+    if (s.used) SQ_CUDA(cudaEventSynchronize(s.done));
+    cudaFree(s.staging);
+    s.staging = nullptr;
+    SQ_CUDA(cudaMalloc(&s.staging, total));
+    s.staging_cap = total;
+  }
+  uint8_t* dst = to_input ? reinterpret_cast<uint8_t*>(s.input) : s.staging;
+  for (int i = 0; i < count; ++i)
+    SQ_CUDA(cudaMemcpyAsync(dst + off[i], src[i], bytes[i], cudaMemcpyHostToDevice, cs));
+  SQ_CUDA(cudaEventRecord(s.h2d, cs));
+  SQ_CUDA(cudaStreamWaitEvent(e->own_stream, s.h2d, 0));
   return SQDET_OK;
 }
 
 // The forward over images [0, n) of the slot's input on the compute stream, then their records
-// and counts back to the caller's buffers; ev_done marks the slot's buffers free again.
-static int finish_submit(sqdet_engine* e, int slot, int n, sqdet_det* dets, int32_t* counts) {
+// and counts back to the caller's buffers; `done` marks the slot's buffers free again.
+static int finish_submit(sqdet_engine* e, Slot& s, int n, const float* scales, sqdet_det* dets,
+                         int32_t* counts) {
   cudaStream_t ks = e->own_stream;
-  int rc = forward_impl(e, e->d_in_slot[slot], n, ks);
+  int rc = forward_impl(e, s.input, n, scales, ks);
   if (rc) return rc;
   if (dets)
     SQ_CUDA(cudaMemcpyAsync(dets, e->d_dets, sizeof(sqdet_det) * (size_t)n * e->max_dets,
@@ -569,8 +596,8 @@ static int finish_submit(sqdet_engine* e, int slot, int n, sqdet_det* dets, int3
   if (counts)
     SQ_CUDA(cudaMemcpyAsync(counts, e->d_counts, sizeof(int32_t) * (size_t)n,
                             cudaMemcpyDeviceToHost, ks));
-  SQ_CUDA(cudaEventRecord(e->ev_done[slot], ks));
-  e->slot_used[slot] = true;
+  SQ_CUDA(cudaEventRecord(s.done, ks));
+  s.used = true;
   ++e->n_submitted;
   return SQDET_OK;
 }
@@ -640,19 +667,18 @@ int sqdet_destroy(sqdet_engine* e) {
   cudaFree(e->d_boxes);
   cudaFree(e->d_probs);
   cudaFree(e->d_cls);
-  cudaFree(e->d_dets);   // also owns d_counts (one blob); d_input aliases tensors[0].dev
+  cudaFree(e->d_dets);   // also owns d_counts (one blob)
   for (auto ev : e->prof_events) cudaEventDestroy(ev);
-  for (int k = 0; k < 2; ++k) {
-    if (k == 1 && e->d_in_slot[1]) cudaFree(e->d_in_slot[1]);
-    if (e->d_u8_slot[k]) cudaFree(e->d_u8_slot[k]);
-    if (e->ev_h2d[k]) cudaEventDestroy(e->ev_h2d[k]);
-    if (e->ev_done[k]) cudaEventDestroy(e->ev_done[k]);
+  for (Slot& s : e->slots) {
+    if (&s != &e->slots[0]) cudaFree(s.input);   // slot 0's input is tensors[0].dev
+    cudaFree(s.staging);
+    cudaFree(s.scales);
+    if (s.h2d) cudaEventDestroy(s.h2d);
+    if (s.done) cudaEventDestroy(s.done);
   }
   if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
   if (e->own_stream) cudaStreamDestroy(e->own_stream);
-  cudaFree(e->d_scales);
-  cudaFree(e->d_frames[0]);
-  cudaFree(e->d_frames[1]);
+  cudaFree(e->box_scale);
   cudaFree(e->d_gathered);
   if (e->comm && e->comm_owned && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
   (void)cudaGetLastError();   // never leave a stale error for the next engine's launch checks
@@ -798,7 +824,7 @@ int sqdet_finalize(sqdet_engine* e) {
     if (!t.materialized) continue;
     SQ_CUDA(cudaMalloc(&t.dev, sizeof(float) * (size_t)t.numel()));
   }
-  e->d_input = e->tensors[0].dev;
+  e->slots[0].input = e->tensors[0].dev;
   const int64_t A = e->num_anchors, B = c.batch_size;
   std::vector<float> anc((size_t)A * 4);
   for (size_t i = 0; i < anc.size(); ++i) anc[i] = (float)e->anchors_f64[i];   // fp64 -> fp32 cast
@@ -1030,7 +1056,7 @@ int sqdet_forward(sqdet_engine* e, const float* images_dev, void* stream) {
 }
 
 int sqdet_forward_n(sqdet_engine* e, const float* images_dev, int n, void* stream) {
-  return forward_impl(e, images_dev, n, (cudaStream_t)stream);
+  return forward_impl(e, images_dev, n, e ? e->box_scale : nullptr, (cudaStream_t)stream);
 }
 
 int sqdet_forward_profiled(sqdet_engine* e, const float* images_dev, void* stream_v,
@@ -1055,7 +1081,7 @@ int sqdet_forward_profiled(sqdet_engine* e, const float* images_dev, void* strea
     if (rc) return rc;
     SQ_CUDA(cudaEventRecord(e->prof_events[i + 1], stream));
   }
-  rc = run_interpret(e, B, stream);
+  rc = run_interpret(e, B, e->box_scale, stream);
   if (rc) return rc;
   SQ_CUDA(cudaEventRecord(e->prof_events[n - 1], stream));
   rc = run_filter(e, B, stream);
@@ -1088,8 +1114,8 @@ int sqdet_detect(sqdet_engine* e, const float* images, float* det_boxes, float* 
   cudaStream_t stream = stream_v ? (cudaStream_t)stream_v : e->own_stream;
   const sqdet_config& c = e->cfg;
   const size_t in_bytes = sizeof(float) * (size_t)e->tensors[0].numel();
-  SQ_CUDA(cudaMemcpyAsync(e->d_input, images, in_bytes, cudaMemcpyHostToDevice, stream));
-  int rc = forward_impl(e, e->d_input, c.batch_size, stream);
+  SQ_CUDA(cudaMemcpyAsync(e->slots[0].input, images, in_bytes, cudaMemcpyHostToDevice, stream));
+  int rc = forward_impl(e, e->slots[0].input, c.batch_size, e->box_scale, stream);
   if (rc) return rc;
   const size_t BA = (size_t)c.batch_size * (size_t)e->num_anchors;
   if (det_boxes)
@@ -1122,46 +1148,39 @@ int sqdet_submit(sqdet_engine* e, const void* images, int img_type, sqdet_det* d
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit: unknown img_type");
   DeviceGuard guard(e->device);
   const sqdet_config& c = e->cfg;
-  int slot;
-  int rc = begin_submit(e, "sqdet_submit", &slot);
+  Slot* s;
+  int rc = begin_submit(e, "sqdet_submit", &s);
   if (rc) return rc;
+  const bool u8 = img_type == SQDET_IMG_U8;
   const int64_t n_pix = (int64_t)c.batch_size * c.image_height * c.image_width;
-  if (img_type == SQDET_IMG_U8 && !e->d_u8_slot[slot])
-    SQ_CUDA(cudaMalloc(&e->d_u8_slot[slot], (size_t)n_pix * 3));
-  cudaStream_t cs = e->copy_stream, ks = e->own_stream;
-  // the slot's input buffers are free once the forward that last read them has finished
-  if (e->slot_used[slot]) SQ_CUDA(cudaStreamWaitEvent(cs, e->ev_done[slot], 0));
-  if (img_type == SQDET_IMG_U8)
-    SQ_CUDA(cudaMemcpyAsync(e->d_u8_slot[slot], images, (size_t)n_pix * 3, cudaMemcpyHostToDevice, cs));
-  else
-    SQ_CUDA(cudaMemcpyAsync(e->d_in_slot[slot], images, sizeof(float) * (size_t)n_pix * 3,
-                            cudaMemcpyHostToDevice, cs));
-  SQ_CUDA(cudaEventRecord(e->ev_h2d[slot], cs));
-  SQ_CUDA(cudaStreamWaitEvent(ks, e->ev_h2d[slot], 0));
-  if (img_type == SQDET_IMG_U8) {
+  const size_t bytes = (size_t)n_pix * 3 * (u8 ? 1 : sizeof(float));
+  const uint8_t* src = static_cast<const uint8_t*>(images);
+  const size_t off = 0;
+  rc = upload(e, *s, !u8, 1, &src, &bytes, &off);
+  if (rc) return rc;
+  if (u8) {
     // on the COMPUTE stream: on the copy stream (to overlap the previous batch's forward) it was
     // measured slower, 2.08 vs 1.93 ms per step end to end - its CTAs wait for the persistent
     // one-CTA-per-SM kernels of that forward and then delay this batch's first layer
-    rc = launch_u8_meansub(e->d_u8_slot[slot], e->d_in_slot[slot], n_pix, e->bgr_means[0],
-                           e->bgr_means[1], e->bgr_means[2], ks);
+    rc = launch_u8_meansub(s->staging, s->input, n_pix, e->bgr_means[0], e->bgr_means[1],
+                           e->bgr_means[2], e->own_stream);
     if (rc) return rc;
   }
-  return finish_submit(e, slot, c.batch_size, dets, counts);
+  return finish_submit(e, *s, c.batch_size, e->box_scale, dets, counts);
 }
 
 int sqdet_wait(sqdet_engine* e) {
   if (!e) return fail(SQDET_ERR_INVALID_ARG, "null engine");
   if (e->n_waited >= e->n_submitted) return fail(SQDET_ERR_STATE, "sqdet_wait: nothing in flight");
   DeviceGuard guard(e->device);
-  const int slot = (int)(e->n_waited & 1);
-  SQ_CUDA(cudaEventSynchronize(e->ev_done[slot]));
+  SQ_CUDA(cudaEventSynchronize(e->slots[e->n_waited & 1].done));
   ++e->n_waited;
   return SQDET_OK;
 }
 
 int sqdet_launches_per_forward(sqdet_engine* e) {
   if (!e) return SQDET_ERR_INVALID_ARG;
-  int n = 2 + (e->rescale_on ? 1 : 0);   // interpret [+ rescale] + filter (NCCL's own kernel not counted)
+  int n = 2 + (e->box_scale ? 1 : 0);   // interpret [+ rescale] + filter (NCCL's own kernel not counted)
   for (const auto& op : e->ops) n += (int)op.launches.size();
   return n;
 }
@@ -1172,21 +1191,19 @@ int sqdet_set_box_scale(sqdet_engine* e, const float* xy_scales) {
   if (!e) return fail(SQDET_ERR_INVALID_ARG, "null engine");
   if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_set_box_scale before sqdet_finalize");
   DeviceGuard guard(e->device);
-  const bool on = xy_scales != nullptr;
-  if (on) {
-    const size_t n = (size_t)e->cfg.batch_size * 2;
-    for (size_t i = 0; i < n; ++i)
-      if (!(xy_scales[i] > 0.f)) return fail(SQDET_ERR_INVALID_ARG, "sqdet_set_box_scale: scales must be positive");
-    if (!e->d_scales) SQ_CUDA(cudaMalloc(&e->d_scales, sizeof(float) * n * 2));
-    // synchronous: no forward may be in flight while the table changes (both pipeline halves)
-    SQ_CUDA(cudaDeviceSynchronize());
-    SQ_CUDA(cudaMemcpy(e->d_scales, xy_scales, sizeof(float) * n, cudaMemcpyHostToDevice));
-    SQ_CUDA(cudaMemcpy(e->d_scales + n, xy_scales, sizeof(float) * n, cudaMemcpyHostToDevice));
+  const size_t n = (size_t)e->cfg.batch_size * 2;
+  for (size_t i = 0; xy_scales && i < n; ++i)
+    if (!(xy_scales[i] > 0.f)) return fail(SQDET_ERR_INVALID_ARG, "sqdet_set_box_scale: scales must be positive");
+  // synchronous: no forward may be in flight while the table changes or goes.  No graph is
+  // dropped: a graph reads the table at its key's address, whichever table is allocated there.
+  SQ_CUDA(cudaDeviceSynchronize());
+  if (!xy_scales) {
+    cudaFree(e->box_scale);
+    e->box_scale = nullptr;
+    return SQDET_OK;
   }
-  if (on != e->rescale_on) {
-    e->rescale_on = on;
-    drop_graph(e);           // the captured forward has one kernel more / less
-  }
+  if (!e->box_scale) SQ_CUDA(cudaMalloc(&e->box_scale, sizeof(float) * n));
+  SQ_CUDA(cudaMemcpy(e->box_scale, xy_scales, sizeof(float) * n, cudaMemcpyHostToDevice));
   return SQDET_OK;
 }
 
@@ -1211,60 +1228,41 @@ int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
   if (n < 1 || n > B)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit_frames_n: n must be in [1, batch_size]");
   DeviceGuard guard(e->device);
-  int slot;
-  int rc = begin_submit(e, "sqdet_submit_frames", &slot);
+  Slot* s;
+  int rc = begin_submit(e, "sqdet_submit_frames", &s);
   if (rc) return rc;
-  size_t total = 0;
-  std::vector<size_t> off((size_t)n);
+  std::vector<size_t> bytes((size_t)n), off((size_t)n);
+  std::vector<float> sc((size_t)n * 2);
+  size_t end = 0;
   for (int i = 0; i < n; ++i) {
     if (!frames[i] || heights[i] <= 0 || widths[i] <= 0)
       return fail(SQDET_ERR_INVALID_ARG, "sqdet_submit_frames: empty frame");
-    off[(size_t)i] = total;
-    total += ((size_t)heights[i] * widths[i] * 3 + 255) & ~(size_t)255;
+    bytes[(size_t)i] = (size_t)heights[i] * widths[i] * 3;
+    off[(size_t)i] = end;                                   // 256-byte aligned staging offsets
+    end += (bytes[(size_t)i] + 255) & ~(size_t)255;
+    // eval.py:72-74 / imdb.py:93-95: x_scale = mc.IMAGE_WIDTH / orig_w (Python floats = double)
+    sc[(size_t)2 * i] = (float)((double)c.image_width / (double)widths[i]);
+    sc[(size_t)2 * i + 1] = (float)((double)c.image_height / (double)heights[i]);
   }
-  cudaStream_t cs = e->copy_stream, ks = e->own_stream;
-  if (e->slot_used[slot]) SQ_CUDA(cudaStreamWaitEvent(cs, e->ev_done[slot], 0));
-  if (e->frames_cap[slot] < total) {
-    // growing the staging buffer: the slot's previous forward must be done with it
-    if (e->slot_used[slot]) SQ_CUDA(cudaEventSynchronize(e->ev_done[slot]));
-    cudaFree(e->d_frames[slot]);
-    e->d_frames[slot] = nullptr;
-    SQ_CUDA(cudaMalloc(&e->d_frames[slot], total));
-    e->frames_cap[slot] = total;
-  }
-  for (int i = 0; i < n; ++i)
-    SQ_CUDA(cudaMemcpyAsync(e->d_frames[slot] + off[(size_t)i], frames[i],
-                            (size_t)heights[i] * widths[i] * 3, cudaMemcpyHostToDevice, cs));
-  SQ_CUDA(cudaEventRecord(e->ev_h2d[slot], cs));
-  // eval order: boxes go back to each frame's own pixel grid before the filter (eval.py:80-87)
+  cudaStream_t ks = e->own_stream;
+  // eval order: boxes go back to each frame's own pixel grid before the filter (eval.py:80-87).
+  // The slot's table is written in stream order behind the forward that last read it.
   if (rescale) {
-    std::vector<float> sc((size_t)B * 2, 1.f);   // images [n, B) are not run; 1 keeps the table valid
-    for (int i = 0; i < n; ++i) {
-      // eval.py:72-74 / imdb.py:93-95: x_scale = mc.IMAGE_WIDTH / orig_w (Python floats = double)
-      sc[(size_t)2 * i] = (float)((double)c.image_width / (double)widths[i]);
-      sc[(size_t)2 * i + 1] = (float)((double)c.image_height / (double)heights[i]);
-    }
-    if (!e->rescale_on) {
-      rc = sqdet_set_box_scale(e, sc.data());      // first use: allocate + enable
-      if (rc) return rc;
-    }
-    // this slot's half of the table, in stream order behind the forward that last read it
-    SQ_CUDA(cudaMemcpyAsync(e->d_scales + (size_t)slot * B * 2, sc.data(), sizeof(float) * n * 2,
+    if (!s->scales) SQ_CUDA(cudaMalloc(&s->scales, sizeof(float) * (size_t)B * 2));
+    SQ_CUDA(cudaMemcpyAsync(s->scales, sc.data(), sizeof(float) * sc.size(),
                             cudaMemcpyHostToDevice, ks));
-  } else if (e->rescale_on) {
-    rc = sqdet_set_box_scale(e, nullptr);
-    if (rc) return rc;
   }
-  SQ_CUDA(cudaStreamWaitEvent(ks, e->ev_h2d[slot], 0));
+  rc = upload(e, *s, false, n, frames, bytes.data(), off.data());
+  if (rc) return rc;
   const size_t img_floats = (size_t)c.image_height * c.image_width * 3;
   for (int i = 0; i < n; ++i) {
-    rc = launch_resize_meansub_u8(e->d_frames[slot] + off[(size_t)i], heights[i], widths[i],
-                                  e->d_in_slot[slot] + (size_t)i * img_floats, c.image_height,
+    rc = launch_resize_meansub_u8(s->staging + off[(size_t)i], heights[i], widths[i],
+                                  s->input + (size_t)i * img_floats, c.image_height,
                                   c.image_width, e->bgr_means[0], e->bgr_means[1],
                                   e->bgr_means[2], order == SQDET_PRE_SUB_THEN_RESIZE, ks);
     if (rc) return rc;
   }
-  return finish_submit(e, slot, n, dets, counts);
+  return finish_submit(e, *s, n, rescale ? s->scales : nullptr, dets, counts);
 }
 
 // ---- multi-GPU: ONE all-gather of the filtered records ---------------------------------------------

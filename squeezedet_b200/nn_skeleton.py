@@ -291,9 +291,9 @@ class ModelSkeleton:
     return missing
 
   # ---- execution ----------------------------------------------------------------------
-  def _images_array(self, images):
+  def _images_array(self, images, dtype=np.float32):
     mc = self.mc
-    arr = np.asarray(images, dtype=np.float32)
+    arr = np.asarray(images, dtype=dtype)
     want = (mc.BATCH_SIZE, mc.IMAGE_HEIGHT, mc.IMAGE_WIDTH, 3)
     if arr.shape != want:
       # TF raises ValueError on a feed-shape mismatch against the static placeholder
@@ -346,14 +346,10 @@ class ModelSkeleton:
   def detect_u8(self, images_u8):
     """uint8 BGR images [B,H,W,3] (already at mc.IMAGE_WIDTH x IMAGE_HEIGHT) ->
     (dets, counts): the demo.py:187-199 loop body from `im - mc.BGR_MEANS` on, on the GPU."""
-    mc = self.mc
-    arr = np.ascontiguousarray(np.asarray(images_u8, dtype=np.uint8))
-    want = (mc.BATCH_SIZE, mc.IMAGE_HEIGHT, mc.IMAGE_WIDTH, 3)
-    if arr.shape != want:
-      raise ValueError('Cannot feed value of shape %r for image_input, which has shape %r'
-                       % (arr.shape, want))
-    dets = np.empty((mc.BATCH_SIZE, self.max_dets), _lib.DET_DTYPE)
-    counts = np.empty((mc.BATCH_SIZE,), np.int32)
+    B = self.mc.BATCH_SIZE
+    arr = self._images_array(images_u8, np.uint8)
+    dets = np.empty((B, self.max_dets), _lib.DET_DTYPE)
+    counts = np.empty((B,), np.int32)
     self.submit(arr.ctypes.data, dets.ctypes.data, counts.ctypes.data, _lib.IMG_U8)
     self.wait()
     return dets, counts
@@ -365,9 +361,9 @@ class ModelSkeleton:
     (mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT) and subtracts mc.BGR_MEANS in the reference order ('demo':
     resize then subtract, demo.py:187-190; 'eval': subtract then resize, imdb.py:85-97).
     rescale=True: boxes are divided by each frame's (x_scale, y_scale) BEFORE filter_prediction,
-    like eval.py:80-87.  dets_ptr / counts_ptr receive n rows (sqdet_submit_frames_n: a short
-    batch runs the kernels planned for BATCH_SIZE, so image i's records equal those of a full
-    batch).  Same wait() contract as submit(); the frame arrays must stay alive until then."""
+    like eval.py:80-87, in this submission only; set_box_scale's table does not apply.
+    dets_ptr / counts_ptr receive n rows (sqdet_submit_frames_n: a short batch runs the kernels
+    planned for BATCH_SIZE, so image i's records equal those of a full batch).  Same wait() contract as submit(); the frame arrays must stay alive until then."""
     B, n = self.mc.BATCH_SIZE, len(frames)
     if not 1 <= n <= B:
       raise ValueError('need 1 to %d frames, got %d' % (B, n))
@@ -396,7 +392,8 @@ class ModelSkeleton:
 
   def set_box_scale(self, scales):
     """eval.py:83-84 for host-resized inputs: `scales` = B (x_scale, y_scale) pairs, or None to
-    switch the rescale off.  Later forwards divide det_boxes by them before the filter."""
+    switch the rescale off.  Later forwards of already-resized images (detect, detect_records,
+    submit, forward_device) divide det_boxes by them before the filter; submit_frames does not."""
     if scales is None:
       _lib.check(self._lib.sqdet_set_box_scale(self._engine, None))
       return

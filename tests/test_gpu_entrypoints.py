@@ -168,3 +168,38 @@ def test_rescale_before_filter_changes_nothing_but_coordinates(gpu_device):
   m.set_box_scale(None)
   b2, _, _ = m.detect(imgs)
   assert np.array_equal(b2, b0)
+
+
+def test_frames_rescale_and_box_scale_table_stay_apart(gpu_device):
+  """`rescale` of a frames submission applies to that submission only, and the table of
+  sqdet_set_box_scale to the paths fed already-resized images only."""
+  from squeezedet_b200.nets import SqueezeDet
+  from test_gpu_e2e import make_mc
+  mc = make_mc('squeezeDet', 416, 128, 2)
+  m = SqueezeDet(mc, gpu_device)
+  m.load_weights(synth.synthetic_weights(synth.model_param_specs(m), seed=5))
+  imgs = synth.synthetic_images(2, 128, 416, seed=6)
+  rng = np.random.default_rng(7)
+  # not 128 x 416, so the frames' box scales are not 1
+  frames = [rng.integers(0, 256, hw + (3,), dtype=np.uint8) for hw in ((150, 500), (100, 380))]
+  b0, p0, c0 = m.detect(imgs)
+  launches = m.launches_per_forward()
+  want_d, want_c = m.detect_frames(frames, order='eval', rescale=True)
+  b1, p1, c1 = m.detect(imgs)
+  assert b1.tobytes() == b0.tobytes() and p1.tobytes() == p0.tobytes()
+  assert c1.tobytes() == c0.tobytes()
+  assert m.launches_per_forward() == launches
+  scales = np.array([[1248 / 1242.0, 384 / 375.0], [0.75, 1.5]], np.float32)
+  m.set_box_scale(scales)
+  assert m.launches_per_forward() == launches + 1
+  m.detect_frames(frames, order='eval', rescale=False)
+  b2, p2, c2 = m.detect(imgs)
+  want = b0.copy()
+  for j in range(2):
+    want[j, :, 0::2] /= float(scales[j, 0])
+    want[j, :, 1::2] /= float(scales[j, 1])
+  assert np.array_equal(b2, want) and np.array_equal(p2, p0) and np.array_equal(c2, c0)
+  d, c = m.detect_frames(frames, order='eval', rescale=True)
+  assert np.array_equal(c, want_c) and want_c.sum() > 0
+  for j in range(2):
+    assert d[j][:c[j]].tobytes() == want_d[j][:c[j]].tobytes()
