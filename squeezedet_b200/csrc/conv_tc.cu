@@ -9,8 +9,9 @@
 // GEMM view per CTA:  D[128 pixels, NT] += A[128 pixels, K] * W[K, NT]
 //   M tile : 128 consecutive pixels of the flattened B*Ho*Wo output list; two warpgroups, each
 //            owning 64 rows (one wgmma m64 row block).
-//   N      : one chunk of NT output channels (16, 32 or 64) of one conv; blockIdx.y walks the
-//            chunks of every conv of the launch (the fire expand pair is two convs).
+//   N      : one chunk of NT output channels (16, 32, 64, or 72 for the ConvDet head) of one
+//            conv; blockIdx.y walks the chunks of every conv of the launch (the fire expand pair
+//            is two convs).
 //   K      : taps x Cin walked in KC-channel chunks (KC = 32 or 16); gather mode flattens
 //            (dy, dx, c) and pads it to a multiple of 32.
 //   A      : cp.async (zero-fill = TF SAME padding) into a row-major [pixel][KC + 4] tile, then
@@ -28,8 +29,11 @@
 //   accumulator and is then added into fp32 running sums with round-to-nearest FADDs, so the
 //   tensor core's truncating accumulation never compounds over a long K (longer chains in the
 //   accumulator left a one-signed error that fails the 1e-4 box parity of SqueezeDet+).
-// Pipeline: 3-stage cp.async ring (one commit group per K chunk); each wgmma group is waited for
-//   before its sums are read, so a stage is free again at the next block barrier.
+// Pipeline: 3-stage cp.async ring (one commit group per K chunk).  Within a K chunk the steps
+//   alternate between two accumulator sets: step k + 1's MMAs are issued before step k is
+//   waited for (wait_group 1) and added in, and the next A fragment is loaded and split while
+//   they run.  Each chunk ends with wait_group 0, so a stage is free again at the next block
+//   barrier.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -98,11 +102,15 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() {
   asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void wgmma_wait_all() {
-  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+// waits until at most N committed wgmma groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+// keeps the compiler from moving accumulator / A-fragment reads and writes across the
+// asynchronous MMAs
 __device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+__device__ __forceinline__ void fence_operand(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
 
 // No-swizzle K-major descriptor: core matrices of 8 rows x 16 bytes, K-adjacent ones 128 B apart
 // (LBO), 8-row groups `sbo` bytes apart (SBO).
@@ -166,55 +174,114 @@ struct Mma<64> {
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
   }
 };
+// the ConvDet head's 72 = 9 anchors x (classes + 1 + 4) channels as one tile
+template <>
+struct Mma<72> {
+  static __device__ __forceinline__ void run(float (&d)[36], const uint32_t (&a)[4], uint64_t b,
+                                             int acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %41, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n72k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35}, "
+        "{%36, %37, %38, %39}, %40, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
+          "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
+          "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),
+          "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
+  }
+};
 
 template <int NT, int KC>
 __host__ __device__ constexpr int stage_floats() {
   return TILE_M * (KC + 4) + 2 * NT * KC;
 }
 
-// One K chunk of KC channels for this thread's A-fragment rows g (a0) and g + 8 (a1), each
-// pointing at the chunk's first column in shared memory; B = hi tile at shared address `bhi`,
-// lo tile right after it.  Every 8-wide K step runs its three split MMAs from a zeroed
-// accumulator and is added into the fp32 running sums.
-template <int NT, int KC>
-__device__ __forceinline__ void mma_chunk(const float* a0, const float* a1, uint32_t bhi, int t,
-                                          float (&acc)[NT / 2], float (&sum)[NT / 2]) {
-  constexpr int KSTEPS = KC / 8;
-  constexpr uint32_t SBO = (KC / 4) * 128;
-  uint32_t ahi[KSTEPS][4], alo[KSTEPS][4];
+// A fragment of 8-wide K step `ks` for this thread's rows g (a0) and g + 8 (a1), split into its
+// TF32 hi part and rounded lo remainder.
+__device__ __forceinline__ void load_split(const float* a0, const float* a1, int ks, int t,
+                                           uint32_t (&ahi)[4], uint32_t (&alo)[4]) {
+  const float v[4] = {a0[ks * 8 + t], a1[ks * 8 + t], a0[ks * 8 + t + 4], a1[ks * 8 + t + 4]};
 #pragma unroll
-  for (int ks = 0; ks < KSTEPS; ++ks) {
-    const float v[4] = {a0[ks * 8 + t], a1[ks * 8 + t], a0[ks * 8 + t + 4], a1[ks * 8 + t + 4]};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float hi = rn_tf32(v[i]);
-      ahi[ks][i] = __float_as_uint(hi);
-      alo[ks][i] = __float_as_uint(rn_tf32(v[i] - hi));   // rounded, not truncated by the MMA
-    }
-  }
-  const uint32_t blo = bhi + NT * KC * 4;
-#pragma unroll
-  for (int ks = 0; ks < KSTEPS; ++ks) {
-    const uint64_t dhi = make_desc(bhi + ks * 256, SBO), dlo = make_desc(blo + ks * 256, SBO);
-#pragma unroll
-    for (int i = 0; i < NT / 2; ++i) fence_operand(acc[i]);
-    wgmma_fence();
-    Mma<NT>::run(acc, alo[ks], dhi, 0);
-    Mma<NT>::run(acc, ahi[ks], dlo, 1);
-    Mma<NT>::run(acc, ahi[ks], dhi, 1);
-    wgmma_commit();
-    wgmma_wait_all();
-#pragma unroll
-    for (int i = 0; i < NT / 2; ++i) {
-      fence_operand(acc[i]);
-      sum[i] += acc[i];
-    }
+  for (int i = 0; i < 4; ++i) {
+    const float hi = rn_tf32(v[i]);
+    ahi[i] = __float_as_uint(hi);
+    alo[i] = __float_as_uint(rn_tf32(v[i] - hi));   // rounded, not truncated by the MMA
   }
 }
 
+// Issues K step `ks` of a KC-channel chunk as one wgmma group: the three split MMAs into `acc`,
+// the first from zero.  B = hi tile at shared address `bhi`, lo tile right after it.
+template <int NT, int KC>
+__device__ __forceinline__ void mma_step(float (&acc)[NT / 2], const uint32_t (&ahi)[4],
+                                         const uint32_t (&alo)[4], uint32_t bhi, int ks) {
+  constexpr uint32_t SBO = (KC / 4) * 128;
+  const uint32_t blo = bhi + NT * KC * 4;
+  const uint64_t dhi = make_desc(bhi + ks * 256, SBO), dlo = make_desc(blo + ks * 256, SBO);
+#pragma unroll
+  for (int i = 0; i < NT / 2; ++i) fence_operand(acc[i]);
+  wgmma_fence();
+  Mma<NT>::run(acc, alo, dhi, 0);
+  Mma<NT>::run(acc, ahi, dlo, 1);
+  Mma<NT>::run(acc, ahi, dhi, 1);
+  wgmma_commit();
+}
+
+// Adds the accumulator of a retired K step into the fp32 running sums; its A fragment is free.
+template <int N>
+__device__ __forceinline__ void flush(float (&acc)[N], float (&sum)[N], uint32_t (&ahi)[4],
+                                      uint32_t (&alo)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) fence_operand(ahi[i]), fence_operand(alo[i]);
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    fence_operand(acc[i]);
+    sum[i] += acc[i];
+  }
+}
+
+// One K chunk of KC channels for this thread's A-fragment rows g (a0) and g + 8 (a1), each
+// pointing at the chunk's first column in shared memory; B at `bhi`.  Software-pipelined over
+// two accumulator sets: step ks runs into acc[ks & 1], and while its MMAs are in flight the
+// previous step is retired (wgmma.wait_group 1) and added into the fp32 running sums, and the
+// next step's A fragment is loaded and split.  Every step still runs from a zeroed accumulator
+// and is added in K order, as in an unpipelined loop.
+//
+// The chunk ends with every group retired (wait_group 0).  That drain leaves one MMA latency
+// exposed per chunk, but it is what makes the caller's 3-stage ring safe: past the next block
+// barrier no wgmma reads the stage that the prefetch then overwrites.  (ptxas also serialises
+// every wgmma of a kernel whose accumulators are read in a loop that a group stays in flight
+// across.)
+template <int NT, int KC>
+__device__ __forceinline__ void mma_chunk(const float* a0, const float* a1, uint32_t bhi, int t,
+                                          float (&acc)[2][NT / 2], float (&sum)[NT / 2]) {
+  constexpr int KSTEPS = KC / 8;
+  uint32_t ahi[2][4], alo[2][4];
+#pragma unroll
+  for (int ks = 0; ks < KSTEPS; ++ks) {
+    const int cur = ks & 1;
+    load_split(a0, a1, ks, t, ahi[cur], alo[cur]);
+    mma_step<NT, KC>(acc[cur], ahi[cur], alo[cur], bhi, ks);
+    if (ks > 0) {
+      wgmma_wait<1>();
+      flush(acc[cur ^ 1], sum, ahi[cur ^ 1], alo[cur ^ 1]);
+    }
+  }
+  constexpr int last = (KSTEPS - 1) & 1;
+  wgmma_wait<0>();
+  flush(acc[last], sum, ahi[last], alo[last]);
+}
+
 // ---------------------------------------------------------------------------------------------
+// Two CTAs per SM (the shared memory of 3 stages allows it up to NT = 72, KC = 32): at most 128
+// registers a thread.  The 72-wide tile needs more (108 accumulator and sum registers alone) and
+// runs one CTA per SM.
 template <int NT, int KC, bool GATHER>
-__global__ void __launch_bounds__(NUM_THREADS)
+__global__ void __launch_bounds__(NUM_THREADS, NT == 72 ? 1 : 2)
 conv_tc_kernel(const __grid_constant__ TcParams p) {
   constexpr int APITCH = KC + 4;
   constexpr int NACC = NT / 2;
@@ -260,8 +327,8 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
         const int tap = k / p.Cin, c = k - tap * p.Cin;
         const int iy = liy0 + tap / ch.ksize, ix = lix0 + tap % ch.ksize;
         const bool ok = lvalid && tap < taps && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
-        cp_async4(arow + (lh * (KC / 2) + j) * 4, ok ? xn + ((size_t)iy * p.W + ix) * p.Cin + c : p.x,
-                  ok);
+        // 32-bit offset: one image of a 3-channel input is far below 2^31 floats
+        cp_async4(arow + (lh * (KC / 2) + j) * 4, ok ? xn + ((iy * p.W + ix) * p.Cin + c) : p.x, ok);
       }
     }
     // weights: 2 * NT * KC contiguous floats
@@ -281,14 +348,16 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   // warp `wq`'s 16-row slice, columns t / t + 4 of each 8-wide K step
   const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
   const int arow0 = wg * 64 + wq * 16 + g;
-  float acc[NACC], sum[NACC];
+  float acc[2][NACC], sum[NACC];
 #pragma unroll
-  for (int i = 0; i < NACC; ++i) acc[i] = 0.f, sum[i] = 0.f;
+  for (int i = 0; i < NACC; ++i) acc[0][i] = acc[1][i] = sum[i] = 0.f;
 
   for (int kk = 0; kk < nk; ++kk) {
     cp_async_wait<STAGES - 2>();
     fence_proxy_async();
     __syncthreads();
+    // overwrites stage (kk - 1) % STAGES: both warpgroups have retired its MMAs (mma_chunk
+    // drains) and read its A fragments before the barrier
     if (kk + STAGES - 1 < nk) load_stage(kk + STAGES - 1, (kk + STAGES - 1) % STAGES);
     cp_async_commit();
 
@@ -343,6 +412,7 @@ struct FireParams {
   const float* wex;   // expand tiles, chunk after chunk, [nk][2][64][KCE] each
   const float* bex;   // [E1 + E3]
   int B, H, W, Cin, S, Etot, tiles_w, tiles_h, nchunks;
+  int total_nk;   // K chunks of all expand chunks (read from the parameter bank, not a register)
   FireChunk chunks[MAX_FCHUNKS];
 };
 
@@ -352,8 +422,10 @@ __host__ __device__ constexpr int fire_ring_floats() {
                                                              : 2 * 64 * KCE;
 }
 
+// A 16-channel squeeze leaves room for two CTAs per SM (110.6 KB of shared memory, at most 128
+// registers a thread); the wider squeezes need more shared memory than that anyway.
 template <int KCI, int SQN, int KCE>
-__global__ void __launch_bounds__(NUM_THREADS)
+__global__ void __launch_bounds__(NUM_THREADS, SQN == 16 ? 2 : 1)
 fire_tc_kernel(const __grid_constant__ FireParams p) {
   constexpr int API = KCI + 4, QP = SQN + 4;
   constexpr int RING = fire_ring_floats<KCI, SQN, KCE>();
@@ -390,9 +462,10 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
     if (s < nks) load_sq(s, s);
     cp_async_commit();
   }
-  float accq[SQN / 2], sq[2][SQN / 2];
+  float accq[2][SQN / 2], sq[2][SQN / 2];
 #pragma unroll
-  for (int i = 0; i < SQN / 2; ++i) accq[i] = 0.f, sq[0][i] = 0.f, sq[1][i] = 0.f;
+  for (int i = 0; i < SQN / 2; ++i) accq[0][i] = accq[1][i] = sq[0][i] = sq[1][i] = 0.f;
+  const int rb = wq * 16 + g;
   for (int kk = 0; kk < nks; ++kk) {
     cp_async_wait<STAGES - 2>();
     fence_proxy_async();
@@ -401,13 +474,25 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
     cp_async_commit();
     const float* st = smem + (size_t)(kk % STAGES) * RING;
     const float* sa = st + 2 * SQN * KCI;
+    if (wg == 0) {
+      // blocks 0 and 2 interleaved, block 2 * bi in accumulator set bi: one block's step is in
+      // flight while the other block's previous step is added in; drained like mma_chunk
+      uint32_t qhi[2][4], qlo[2][4];
 #pragma unroll
-    for (int bi = 0; bi < 2; ++bi) {
-      const int b = wg + 2 * bi;   // warpgroup-uniform
-      if (b < 3) {
-        const int r0 = b * 64 + wq * 16 + g;
-        mma_chunk<SQN, KCI>(sa + r0 * API, sa + (r0 + 8) * API, smem_u32(st), t, accq, sq[bi]);
+      for (int j = 0; j < 2 * (KCI / 8); ++j) {
+        const int bi = j & 1, ks = j >> 1, r0 = 128 * bi + rb;
+        load_split(sa + r0 * API, sa + (r0 + 8) * API, ks, t, qhi[bi], qlo[bi]);
+        mma_step<SQN, KCI>(accq[bi], qhi[bi], qlo[bi], smem_u32(st), ks);
+        if (j > 0) {
+          wgmma_wait<1>();
+          flush(accq[bi ^ 1], sq[bi ^ 1], qhi[bi ^ 1], qlo[bi ^ 1]);
+        }
       }
+      wgmma_wait<0>();
+      flush(accq[1], sq[1], qhi[1], qlo[1]);
+    } else {
+      const int r0 = 64 + rb;
+      mma_chunk<SQN, KCI>(sa + r0 * API, sa + (r0 + 8) * API, smem_u32(st), t, accq, sq[0]);
     }
   }
   cp_async_wait<0>();
@@ -433,8 +518,7 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
 
   // ---- expand: pixel rows g / g + 8 of this warp are tile row (4 wg + wq), columns g / g + 8
   const int spt = p.S / KCE;   // K chunks per tap
-  int total = 0;
-  for (int c = 0; c < p.nchunks; ++c) total += p.chunks[c].nk;
+  const int total = p.total_nk;
   auto load_ex = [&](int it, int s) {
     const float* wsrc = p.wex + (size_t)it * 2 * 64 * KCE;
     const uint32_t dst = smem_u32(smem + (size_t)s * RING);
@@ -446,9 +530,9 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
     cp_async_commit();
   }
   const int r = wg * 4 + wq;
-  float acc[32], sum[32];
+  float acc[2][32], sum[32];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) acc[i] = 0.f, sum[i] = 0.f;
+  for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i] = sum[i] = 0.f;
   int c = 0, kk = 0;
   for (int it = 0; it < total; ++it) {
     cp_async_wait<STAGES - 2>();
@@ -499,6 +583,7 @@ ConvKernel conv_tc_instance(int NT) {
 
 // The conv_tc_kernel instantiation of a plan (gather mode always walks K in chunks of 32).
 ConvKernel conv_tc_instance(int NT, int KC, bool gather) {
+  if (NT == 72) return conv_tc_kernel<72, 32, false>;   // pick_nt's head tile
   if (gather) return conv_tc_instance<32, true>(NT);
   return KC == 32 ? conv_tc_instance<32, false>(NT) : conv_tc_instance<16, false>(NT);
 }
@@ -547,11 +632,17 @@ static inline float host_rn_tf32(float x) {
 }
 
 // Output-channel tile: the narrowest of 16 / 32 / 64 that covers the launch's chunks with the
-// least padded MMA work plus A-tile re-reads (each chunk reloads the pixels' K values).
-static int pick_nt(const std::vector<ConvGroup>& groups) {
+// least padded MMA work plus A-tile re-reads (each chunk reloads the pixels' K values).  A
+// 72-wide tile is also a candidate for one conv of 65..72 output channels walked in 32-channel
+// K chunks, the ConvDet head (9 anchors x 8 values), which it covers in one chunk instead of
+// two 64-wide ones that are 44 % padding.
+static int pick_nt(const std::vector<ConvGroup>& groups, int KC, bool gather) {
   int best = 0;
   long long best_cost = 0;
-  for (int nt : {64, 32, 16}) {
+  const bool head = !gather && KC == 32 && groups.size() == 1 && groups[0].Cout > 64 &&
+                    groups[0].Cout <= 72;
+  for (int nt : {72, 64, 32, 16}) {
+    if (nt == 72 && !head) continue;
     long long chunks = 0;
     for (const auto& g : groups) chunks += (g.Cout + nt - 1) / nt;
     if (chunks > MAX_CHUNKS) continue;
@@ -577,9 +668,9 @@ static void release_impl(void** impl) {
 static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo, int stride,
                        int pad_t, int pad_l, bool gather, const std::vector<ConvGroup>& groups,
                        int relu, bool has_affine, int y_cstride) {
-  const int NT = pick_nt(groups);
-  if (!NT) return 0;
   const int KC = (gather || Cin % 32 == 0) ? 32 : 16;
+  const int NT = pick_nt(groups, KC, gather);
+  if (!NT) return 0;
   const long long M = (long long)B * Ho * Wo;
   const long long mtiles = (M + TILE_M - 1) / TILE_M;
   if (M <= 0 || mtiles > 0x7fffffffLL) return 0;
@@ -819,6 +910,7 @@ int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int 
     for (int cb = 0; cb < E; cb += 64, ++c) {
       p.chunks[c] = FireChunk{taps, taps * (S / im->KCE), E - cb < 64 ? E - cb : 64, (gi ? E1 : 0) + cb};
       im->w2_floats += (long long)p.chunks[c].nk * 2 * 64 * im->KCE;
+      p.total_nk += p.chunks[c].nk;
     }
   }
   im->w_floats = (long long)(Cin / im->KCI) * 2 * im->SQN * im->KCI;
