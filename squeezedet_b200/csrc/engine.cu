@@ -1374,6 +1374,18 @@ int sqdet_gathered_dev(sqdet_engine* e, void** gathered, int64_t* bytes_per_rank
 void* sqdet_engine_stream(sqdet_engine* e) { return e ? (void*)e->own_stream : nullptr; }
 
 // ---- stage-isolated kernels ------------------------------------------------------------------
+// The epilogue arguments every conv entry point checks before any device work, whichever kernel
+// then runs: scale and shift come together, and the Cout output channels at y_coff lie inside
+// each pixel's y_cstride channels.
+static int check_conv_epilogue(const char* who, const float* scale_dev, const float* shift_dev,
+                               int Cout, int y_cstride, int y_coff) {
+  if ((scale_dev == nullptr) != (shift_dev == nullptr))
+    return fail(SQDET_ERR_INVALID_ARG, std::string(who) + ": scale and shift must be given together");
+  if (y_coff < 0 || (long long)y_coff + Cout > y_cstride)
+    return fail(SQDET_ERR_INVALID_ARG, std::string(who) + ": output channel window out of range");
+  return SQDET_OK;
+}
+
 int sqdet_conv2d(const float* x_dev, const float* w_hwio_dev, const float* bias_dev,
                  const float* scale_dev, const float* shift_dev, float* y_dev, int B, int H, int W,
                  int Cin, int Cout, int size, int stride, int padding, int relu, int y_cstride,
@@ -1381,6 +1393,8 @@ int sqdet_conv2d(const float* x_dev, const float* w_hwio_dev, const float* bias_
   if (!x_dev || !w_hwio_dev || !y_dev) return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv2d: null pointer");
   if (padding != SQDET_PAD_SAME && padding != SQDET_PAD_VALID)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv2d: padding must be SAME(0) or VALID(1)");
+  if (int rc = check_conv_epilogue("sqdet_conv2d", scale_dev, shift_dev, Cout, y_cstride, y_coff))
+    return rc;
   if (math_mode == SQDET_MATH_TF32X3_TC)
     return conv2d_tc_oneshot(x_dev, w_hwio_dev, bias_dev, scale_dev, shift_dev, y_dev, B, H, W,
                              Cin, Cout, size, stride, padding, relu, y_cstride, y_coff,
@@ -1402,6 +1416,9 @@ int sqdet_conv3x3_halo(const float* x_dev, const float* w_hwio_dev, const float*
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv3x3_halo: null pointer");
   if (B <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv3x3_halo: non-positive dimension");
+  if (int rc = check_conv_epilogue("sqdet_conv3x3_halo", scale_dev, shift_dev, Cout, y_cstride,
+                                   y_coff))
+    return rc;
   if (!tc_conv_eligible(Cin, Cout, 3, 1, SQDET_PAD_SAME))
     return fail(SQDET_ERR_UNSUPPORTED, "sqdet_conv3x3_halo: shape not taken by the tensor-core path");
   return conv2d_tc_oneshot(x_dev, w_hwio_dev, bias_dev, scale_dev, shift_dev, y_dev, B, H, W, Cin,

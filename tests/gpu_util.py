@@ -51,17 +51,23 @@ def conv3x3_halo_gpu(x, w, b=None, relu=True, scale=None, shift=None, y_cstride=
   return dy.to_numpy(np.float32, (B, H, W, cs))
 
 
-def maxpool_gpu(x, k, stride, padding, device=0):
+def maxpool_gpu(x, k, stride, padding, device=0, offset=0):
+  """sqdet_maxpool_nhwc; `offset` > 0 places x and y that many floats into larger buffers (an
+  offset of 1 leaves both pointers 4 bytes past 16-byte alignment)."""
   lib = _lib.load()
   import oracle
   B, H, W, Cc = x.shape
   Ho = oracle.conv_geometry(H, k, stride, padding)[0]
   Wo = oracle.conv_geometry(W, k, stride, padding)[0]
-  dx = DeviceBuffer.from_numpy(x.astype(np.float32), device)
-  dy = DeviceBuffer(B * Ho * Wo * Cc * 4, device)
-  _lib.check(lib.sqdet_maxpool_nhwc(dx.ptr, dy.ptr, B, H, W, Cc, k, stride,
-                                    _lib.pad_code(padding), None))
-  return dy.to_numpy(np.float32, (B, Ho, Wo, Cc))
+  n_out = B * Ho * Wo * Cc
+  dx = DeviceBuffer.from_numpy(np.concatenate([np.zeros(offset, np.float32),
+                                               x.astype(np.float32).ravel()]), device)
+  dy = DeviceBuffer.from_numpy(np.full(offset + n_out, np.nan, np.float32), device)
+  _lib.check(lib.sqdet_maxpool_nhwc(dx.ptr + 4 * offset, dy.ptr + 4 * offset, B, H, W, Cc, k,
+                                    stride, _lib.pad_code(padding), None))
+  y = dy.to_numpy(np.float32, (offset + n_out,))
+  assert np.isnan(y[:offset]).all()
+  return y[offset:].reshape(B, Ho, Wo, Cc)
 
 
 def interpret_gpu(preds, anchors_f64, K, classes, img_w, img_h, exp_thresh=1.0, device=0):

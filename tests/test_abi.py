@@ -66,6 +66,26 @@ def test_argument_validation_needs_no_gpu():
   assert lib.sqdet_topk_nms(None, None, None, 1, 8, 3, 64, 0.005, 0.4, None, None, 64, None) == -1
 
 
+def test_conv_epilogue_validation_needs_no_gpu():
+  """sqdet_conv2d (both math modes) and sqdet_conv3x3_halo reject a channel window outside
+  [0, y_cstride) and a scale without a shift (or the reverse) before any device work: on a box
+  with no device that is SQDET_ERR_INVALID_ARG, not a CUDA error.  The pointers are never
+  dereferenced, so the test only runs where no device could be handed them."""
+  lib = _lib.load()
+  if lib.sqdet_device_count() > 0:
+    pytest.skip('a GPU is visible; the no-device behaviour is checked on CPU boxes')
+  p = ctypes.c_void_p(4096)
+  B, H, W, Cin, Cout = 1, 12, 20, 32, 72        # a shape the tensor-core path plans
+  bad = [(72, 1, None, None), (80, -1, None, None), (71, 0, None, None),
+         (72, 0, p, None), (72, 0, None, p)]
+  for cs, coff, sc, sh in bad:
+    for mode in (_lib.MATH_FP32_SIMT, _lib.MATH_TF32X3_TC):
+      assert lib.sqdet_conv2d(p, p, p, sc, sh, p, B, H, W, Cin, Cout, 3, 1, 0, 1, cs, coff, mode,
+                              None) == -1, (cs, coff, sc, sh, mode)
+    assert lib.sqdet_conv3x3_halo(p, p, p, sc, sh, p, B, H, W, Cin, Cout, 1, cs, coff,
+                                  None) == -1, (cs, coff, sc, sh)
+
+
 def test_padding_code():
   assert _lib.pad_code('same') == 0 and _lib.pad_code('VALID') == 1
   with pytest.raises(ValueError):

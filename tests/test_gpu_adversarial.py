@@ -55,6 +55,10 @@ SHAPES = [
     (1, 12, 20, 48, 32, 3, 1),    # K chunks of 16 with a 32-wide output tile
     (2, 17, 29, 3, 64, 3, 1),     # gather mode: K = 27 zero-padded to one 32-row chunk
     (1, 33, 47, 3, 32, 3, 2),     # gather mode, stride 2, 32-wide output tile
+    # the ConvDet heads on the 72-wide tile, the longest reductions the shipped nets run
+    (1, 12, 20, 768, 72, 3, 1),   # K = 6912 (SqueezeDet)
+    (1, 12, 20, 512, 72, 3, 1),   # K = 4608 (SqueezeDet+, VGG16)
+    (1, 12, 20, 1024, 72, 3, 1),  # K = 9216 (ResNet50)
 ]
 
 

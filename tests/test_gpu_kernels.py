@@ -56,6 +56,15 @@ CONV_CASES = [
     # runs on the SIMT kernel
     (1, 3, 5, 32, 2048, 1, 1, 'SAME'),
     (1, 3, 5, 32, 2049, 1, 1, 'SAME'),
+    # the 72-wide ConvDet head tile (one conv of 65..72 channels, Cin % 32 == 0): ragged and odd
+    # channel counts inside the tile, a 1x1 on it, and both sides of its 64 / 65 and 72 / 73 edges
+    (1, 12, 20, 64, 65, 3, 1, 'SAME'),
+    (2, 11, 17, 32, 69, 3, 1, 'SAME'),
+    (1, 13, 21, 96, 71, 3, 1, 'SAME'),
+    (1, 16, 24, 128, 72, 1, 1, 'SAME'),
+    (1, 12, 20, 48, 72, 3, 1, 'SAME'),     # Cin % 32 == 16: KC = 16, so the 64-wide tile
+    (1, 12, 20, 64, 73, 3, 1, 'SAME'),     # one channel past the 72 tile
+    (1, 96, 200, 32, 72, 3, 1, 'SAME'),    # 150 pixel tiles: more CTAs than SMs
 ]
 
 
@@ -75,41 +84,73 @@ def test_conv2d_vs_oracle(case, math_mode, gpu_device):
   assert rel_err(oracle.conv2d(x, w, b, stride, padding, True, np.float32), want) < CONV_RTOL
 
 
+def check_affine_and_channel_window(math_mode, Cin, Cout, y_cstride, y_coff):
+  rng = np.random.default_rng(11)
+  x = rng.normal(size=(1, 15, 18, Cin)).astype(np.float32)
+  w = (rng.normal(size=(3, 3, Cin, Cout)) / np.sqrt(9 * Cin)).astype(np.float32)
+  b = rng.normal(size=(Cout,)).astype(np.float32)
+  sc = rng.uniform(0.5, 1.5, Cout).astype(np.float32)
+  sh = rng.normal(size=Cout).astype(np.float32)
+  want = oracle.conv2d(x, w, b, 1, 'SAME', False, np.float64) * sc + sh
+  y0 = np.full((1, 15, 18, y_cstride), 7.0, np.float32)
+  got = conv2d_gpu(x, w, b, 1, 'SAME', relu=False, scale=sc, shift=sh, y_cstride=y_cstride,
+                   y_coff=y_coff, math_mode=math_mode, y_init=y0)
+  assert rel_err(got[..., y_coff:y_coff + Cout], want) < CONV_RTOL
+  assert np.all(got[..., :y_coff] == 7.0) and np.all(got[..., y_coff + Cout:] == 7.0)  # untouched
+
+
 @pytest.mark.parametrize('math_mode', [_lib.MATH_FP32_SIMT, _lib.MATH_TF32X3_TC])
 def test_conv2d_no_relu_affine_and_channel_window(math_mode, gpu_device):
   """BN-style scale/shift epilogue, no ReLU, and a strided channel window (fire concat)."""
-  rng = np.random.default_rng(11)
-  x = rng.normal(size=(1, 15, 18, 32)).astype(np.float32)
-  w = (rng.normal(size=(3, 3, 32, 48)) / 17).astype(np.float32)
-  b = rng.normal(size=(48,)).astype(np.float32)
-  sc = rng.uniform(0.5, 1.5, 48).astype(np.float32)
-  sh = rng.normal(size=48).astype(np.float32)
-  want = oracle.conv2d(x, w, b, 1, 'SAME', False, np.float64) * sc + sh
-  y0 = np.full((1, 15, 18, 80), 7.0, np.float32)
-  got = conv2d_gpu(x, w, b, 1, 'SAME', relu=False, scale=sc, shift=sh, y_cstride=80, y_coff=16,
-                   math_mode=math_mode, y_init=y0)
-  assert rel_err(got[..., 16:64], want) < CONV_RTOL
-  assert np.all(got[..., :16] == 7.0) and np.all(got[..., 64:] == 7.0)   # untouched channels
+  check_affine_and_channel_window(math_mode, 32, 48, 80, 16)
 
 
-@pytest.mark.parametrize('shape,k,stride,padding', [
+@pytest.mark.parametrize('math_mode', [_lib.MATH_FP32_SIMT, _lib.MATH_TF32X3_TC])
+def test_conv2d_affine_and_channel_window_on_72_tile(math_mode, gpu_device):
+  """The same epilogue on the 72-wide head tile: 72 channels at offset 8 of 88."""
+  check_affine_and_channel_window(math_mode, 64, 72, 88, 8)
+
+
+MAXPOOL_CASES = [
+    # stride 2 with 2x2 / 3x3 windows (maxpool_s2_vec4_kernel), C % 4 != 0 (scalar kernel)
     ((2, 47, 61, 64), 3, 2, 'SAME'), ((1, 47, 62, 128), 3, 2, 'SAME'),
     ((1, 45, 61, 96), 3, 2, 'VALID'), ((2, 31, 37, 64), 2, 2, 'SAME'),
-    ((1, 9, 11, 6), 3, 2, 'SAME')])
+    ((1, 9, 11, 6), 3, 2, 'SAME'),
+    # every other window / stride: the generic maxpool_vec4_kernel
+    ((2, 23, 37, 64), 2, 1, 'SAME'), ((1, 23, 37, 32), 2, 1, 'VALID'),
+    ((2, 19, 29, 64), 3, 1, 'SAME'), ((1, 19, 29, 16), 3, 1, 'VALID'),
+    ((1, 31, 44, 64), 3, 3, 'SAME'), ((2, 13, 17, 32), 1, 1, 'SAME'),
+    # 5.1 M float4 outputs: more than the grid cap of 16 waves of 8 CTAs per SM, so grid-strided
+    ((2, 200, 200, 256), 2, 1, 'SAME'),
+]
+# C % 4 == 0 with x and y one float past 16-byte alignment: the scalar kernel
+MAXPOOL_MISALIGNED_CASES = [((2, 31, 37, 64), 3, 2, 'SAME', 1), ((1, 23, 37, 32), 2, 1, 'VALID', 1)]
+
+
+@pytest.mark.parametrize('shape,k,stride,padding', MAXPOOL_CASES)
 def test_maxpool_exact(shape, k, stride, padding, gpu_device):
   rng = np.random.default_rng(5)
   x = (rng.normal(size=shape) - 2.0).astype(np.float32)
   assert np.array_equal(maxpool_gpu(x, k, stride, padding), oracle.max_pool(x, k, stride, padding))
 
 
-@pytest.mark.parametrize('classes,K,gh,gw', [(3, 9, 24, 78), (20, 9, 5, 7), (3, 9, 22, 76)])
+@pytest.mark.parametrize('shape,k,stride,padding,offset', MAXPOOL_MISALIGNED_CASES)
+def test_maxpool_exact_misaligned(shape, k, stride, padding, offset, gpu_device):
+  rng = np.random.default_rng(6)
+  x = (rng.normal(size=shape) - 2.0).astype(np.float32)
+  assert np.array_equal(maxpool_gpu(x, k, stride, padding, offset=offset),
+                        oracle.max_pool(x, k, stride, padding))
+
+
+@pytest.mark.parametrize('classes,K,gh,gw', [(3, 9, 24, 78), (20, 9, 5, 7), (3, 9, 22, 76),
+                                             (3, 1, 24, 78), (3, 5, 13, 41), (1, 9, 11, 37)])
 def test_interpret_vs_oracle(classes, K, gh, gw, gpu_device):
   rng = np.random.default_rng(classes)
   B, W, H = 2, 1242, 375
   preds = (rng.normal(size=(B, gh, gw, K * (classes + 5))) * 1.5).astype(np.float32)
   preds[0, 0, 0, K * classes + K + 2] = 3.0         # dw above EXP_THRESH -> linear tail
   preds[0, 0, 1, K * classes + K + 3] = -40.0
-  anchors = oracle.set_anchors(W, H, gh, gw, oracle.postproc.ANCHOR_SHAPES_SQUEEZE)
+  anchors = oracle.set_anchors(W, H, gh, gw, oracle.postproc.ANCHOR_SHAPES_SQUEEZE[:K])
   wb, wp, wc = oracle.interpret_output(preds, anchors, classes, K, W, H, 1.0)
   gb, gp, gc = interpret_gpu(preds, anchors, K, classes, W, H, 1.0)
   # bar (BASELINE.json): coordinates and scores within 1e-4 relative; 1e-3 px absolute covers
