@@ -7,15 +7,22 @@
 // expand3x3 + channel concat (src/nets/squeezeDet.py:96-106) as one launch.
 //
 // GEMM view per CTA:  D[128 pixels, NT] += A[128 pixels, K] * W[K, NT]
-//   M tile : 128 consecutive pixels of the flattened B*Ho*Wo output list; two warpgroups, each
-//            owning 64 rows (one wgmma m64 row block).
+//   M tile : 128 output pixels; two warpgroups, each owning 64 rows (one wgmma m64 row block).
+//            Halo mode (every launch with a 3x3 conv over a Cin % 16 == 0 input): an 8-row x
+//            16-column tile of one image, warp 4 wg + wq owning tile row 4 wg + wq.  Row mode
+//            (1x1-only launches) and gather mode: 128 consecutive pixels of the flattened
+//            B*Ho*Wo output list.
 //   N      : one chunk of NT output channels (16, 32, 64, or 72 for the ConvDet head) of one
 //            conv; blockIdx.y walks the chunks of every conv of the launch (the fire expand pair
 //            is two convs).
-//   K      : taps x Cin walked in KC-channel chunks (KC = 32 or 16); gather mode flattens
-//            (dy, dx, c) and pads it to a multiple of 32.
+//   K      : walked in KC-channel chunks (KC = 32 or 16).  Halo mode walks a 3x3 conv channel
+//            chunk by channel chunk with the nine taps inner; a 1x1 conv is its channel chunks.
+//            Gather mode flattens (dy, dx, c) and pads it to a multiple of 32.
 //   A      : cp.async (zero-fill = TF SAME padding) into a row-major [pixel][KC + 4] tile, then
 //            into registers in the wgmma A-fragment layout (the +4 keeps the reads conflict-free).
+//            In halo mode a 3x3 conv loads the 10 x 18 halo of its tile once per channel chunk
+//            and reads tap (dy, dx) at a row offset into it, so each input value crosses from L2
+//            once per channel chunk instead of once per tap.
 //   W      : host-packed per (chunk, K chunk) in the no-swizzle K-major core-matrix layout
 //            [NT/8][KC/4][8 rows][4 floats], hi then lo half; cp.async, read by wgmma through a
 //            shared-memory descriptor.
@@ -29,7 +36,9 @@
 //   accumulator and is then added into fp32 running sums with round-to-nearest FADDs, so the
 //   tensor core's truncating accumulation never compounds over a long K (longer chains in the
 //   accumulator left a one-signed error that fails the 1e-4 box parity of SqueezeDet+).
-// Pipeline: 3-stage cp.async ring (one commit group per K chunk).  Within a K chunk the steps
+// Pipeline: 3-stage cp.async ring (one commit group per K chunk; a halo tile travels in the
+//   group of the first K chunk that reads it, and two halo buffers alternate between channel
+//   chunks).  Within a K chunk the steps
 //   alternate between two accumulator sets: step k + 1's MMAs are issued before step k is
 //   waited for (wait_group 1) and added in, and the next A fragment is loaded and split while
 //   they run.  Each chunk ends with wait_group 0, so a stage is free again at the next block
@@ -51,9 +60,15 @@ constexpr int TILE_M = 128;
 constexpr int NUM_THREADS = 256;   // 2 warpgroups x 64 rows
 constexpr int STAGES = 3;
 constexpr int MAX_CHUNKS = 32;
+// output tiles of the halo-mode convolution and the fire kernel: 8 rows x FT_W columns, read
+// through a (8 + 2) x FQ_W halo of FQ_P pixels
+constexpr int FT_W = 16, FQ_W = FT_W + 2, FQ_P = 10 * FQ_W;
+
+// conv_tc_kernel's operand tiling: see the file comment
+enum TcMode { TC_ROWS, TC_GATHER, TC_HALO };
 
 struct TcChunk {
-  int ksize, pad_t, pad_l;  // this conv's filter size and top / left zero padding
+  int ksize, pad_t, pad_l;  // this conv's filter size and top / left zero padding (gather mode)
   int nk;                   // K chunks of KC channels
   int ncount;               // valid output channels of this chunk (<= NT)
   int y_off;                // first output channel in y
@@ -70,6 +85,7 @@ struct TcParams {
   const float* shift;
   int B, H, W, Cin, Ho, Wo, stride, relu, y_cstride;
   long long M;         // B * Ho * Wo
+  int tiles_w, tiles_h;   // halo mode: output tiles per image row / column
   int nchunks;
   TcChunk chunks[MAX_CHUNKS];
 };
@@ -196,9 +212,12 @@ struct Mma<72> {
   }
 };
 
-template <int NT, int KC>
-__host__ __device__ constexpr int stage_floats() {
-  return TILE_M * (KC + 4) + 2 * NT * KC;
+// conv_tc_kernel's shared memory: the weight ring, STAGES x [2 NT KC], then the A tiles:
+// STAGES x [TILE_M][KC + 4] (one per stage), or in halo mode for a 3x3 conv two [FQ_P][KC + 4]
+// halo tiles in the same space.
+static_assert(2 * FQ_P <= STAGES * TILE_M, "two halo tiles fit in the A ring");
+constexpr size_t conv_smem_floats(int NT, int KC) {
+  return (size_t)STAGES * (2 * NT * KC + TILE_M * (KC + 4));
 }
 
 // A fragment of 8-wide K step `ks` for this thread's rows g (a0) and g + 8 (a1), split into its
@@ -276,68 +295,101 @@ __device__ __forceinline__ void mma_chunk(const float* a0, const float* a1, uint
   flush(acc[last], sum, ahi[last], alo[last]);
 }
 
+// Halo mode: the CTA's 8 x FT_W output tile, of image n at (oy0, ox0)
+struct HaloTile {
+  int n, oy0, ox0;
+};
+__device__ __forceinline__ HaloTile halo_tile(const TcParams& p) {
+  const int tx = blockIdx.x % p.tiles_w, rest = blockIdx.x / p.tiles_w;
+  return {rest / p.tiles_h, rest % p.tiles_h * 8, tx * FT_W};
+}
+
 // ---------------------------------------------------------------------------------------------
 // Two CTAs per SM (the shared memory of 3 stages allows it up to NT = 72, KC = 32): at most 128
 // registers a thread.  The 72-wide tile needs more (108 accumulator and sum registers alone) and
 // runs one CTA per SM.
-template <int NT, int KC, bool GATHER>
+template <int NT, int KC, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, NT == 72 ? 1 : 2)
 conv_tc_kernel(const __grid_constant__ TcParams p) {
   constexpr int APITCH = KC + 4;
   constexpr int NACC = NT / 2;
+  constexpr int WST = 2 * NT * KC;   // floats of one stage's hi + lo weight tiles
   extern __shared__ __align__(128) float smem[];
+  float* const sa = smem + STAGES * WST;   // A tiles
 
   const TcChunk& ch = p.chunks[blockIdx.y];
   const int tid = threadIdx.x;
-  const long long m0 = (long long)blockIdx.x * TILE_M;
+  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  const float* wch = p.w + ch.w_off;
+  const int nk = ch.nk;
 
-  // ---- loader role: pixel `lp`, half `lh` of the KC channels of each K chunk
+  // ---- row and gather mode: 128 consecutive output pixels from m0; loader thread role: pixel
+  // `lp`, half `lh` of the KC channels of each K chunk
+  const long long m0 = (long long)blockIdx.x * TILE_M;
   const int lp = tid >> 1, lh = tid & 1;
   const long long lm = m0 + lp;
-  const bool lvalid = lm < p.M;
-  int ln = 0, liy0 = 0, lix0 = 0;
-  if (lvalid) {
-    const int hw = p.Ho * p.Wo;
-    ln = (int)(lm / hw);
-    const int r = (int)(lm - (long long)ln * hw);
-    liy0 = (r / p.Wo) * p.stride - ch.pad_t;
-    lix0 = (r % p.Wo) * p.stride - ch.pad_l;
-  }
-  const float* xn = p.x + (size_t)ln * p.H * p.W * p.Cin;
-  const int cpt = GATHER ? 1 : p.Cin / KC;   // K chunks per tap
-  const float* wch = p.w + ch.w_off;
+  const bool lvalid = MODE != TC_HALO && lm < p.M;
+  const int taps = ch.ksize * ch.ksize;   // 1 or 9
 
+  // rows x cols input pixels from (y0, x0) of image n, channels [c0, c0 + KC), into a
+  // [rows * cols][APITCH] tile; zero outside the image.  Kept rolled: unrolled, its address
+  // registers push the 64-wide tile past 128 registers into spills.
+  auto load_block = [&](float* dst, int rows, int cols, int y0, int x0, int n, int c0) {
+    const float* xn = p.x + (size_t)n * p.H * p.W * p.Cin;
+#pragma unroll 1
+    for (int v = tid; v < rows * cols * (KC / 4); v += NUM_THREADS) {
+      const int row = v / (KC / 4), j = v % (KC / 4);
+      const int iy = y0 + row / cols, ix = x0 + row % cols;
+      const bool ok = iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
+      cp_async16(smem_u32(dst + row * APITCH + 4 * j),
+                 ok ? xn + ((size_t)iy * p.W + ix) * p.Cin + c0 + 4 * j : p.x, ok);
+    }
+  };
+
+  // K chunk kk into stage s: its weights, and the A values it is the first to read
   auto load_stage = [&](int kk, int s) {
-    float* st = smem + (size_t)s * stage_floats<NT, KC>();
-    float* sa = st + 2 * NT * KC;
-    const uint32_t arow = smem_u32(sa + lp * APITCH);
-    if (!GATHER) {
-      const int tap = kk / cpt, c0 = (kk - tap * cpt) * KC + lh * (KC / 2);
-      const int iy = liy0 + tap / ch.ksize, ix = lix0 + tap % ch.ksize;
-      const bool ok = lvalid && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
-      const float* src = ok ? xn + ((size_t)iy * p.W + ix) * p.Cin + c0 : p.x;
-#pragma unroll
-      for (int v = 0; v < KC / 8; ++v)
-        cp_async16(arow + (lh * (KC / 2) + 4 * v) * 4, ok ? src + 4 * v : p.x, ok);
+    if (MODE == TC_HALO) {
+      // (re-derived from blockIdx rather than kept in registers across the K loop)
+      const HaloTile tl = halo_tile(p);
+      if (taps == 1)
+        load_block(sa + s * TILE_M * APITCH, 8, FT_W, tl.oy0, tl.ox0, tl.n, kk * KC);
+      else if (kk % 9 == 0)   // channel chunk c = kk / 9: its halo, into buffer c & 1
+        load_block(sa + (kk / 9 & 1) * FQ_P * APITCH, 10, FQ_W, tl.oy0 - 1, tl.ox0 - 1, tl.n, kk / 9 * KC);
     } else {
-      const int taps = ch.ksize * ch.ksize;
+      const uint32_t arow = smem_u32(sa + (s * TILE_M + lp) * APITCH);
+      if (MODE == TC_ROWS) {
+        // 1x1, stride 1: output pixel m reads input pixel m
+        const float* src = p.x + (size_t)(lvalid ? lm : 0) * p.Cin + kk * KC + lh * (KC / 2);
 #pragma unroll
-      for (int j = 0; j < KC / 2; ++j) {
-        const int k = kk * KC + lh * (KC / 2) + j;
-        const int tap = k / p.Cin, c = k - tap * p.Cin;
-        const int iy = liy0 + tap / ch.ksize, ix = lix0 + tap % ch.ksize;
-        const bool ok = lvalid && tap < taps && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
-        // 32-bit offset: one image of a 3-channel input is far below 2^31 floats
-        cp_async4(arow + (lh * (KC / 2) + j) * 4, ok ? xn + ((iy * p.W + ix) * p.Cin + c) : p.x, ok);
+        for (int v = 0; v < KC / 8; ++v)
+          cp_async16(arow + (lh * (KC / 2) + 4 * v) * 4, src + 4 * v, lvalid);
+      } else {
+        int ln = 0, liy0 = 0, lix0 = 0;
+        if (lvalid) {
+          const int hw = p.Ho * p.Wo;
+          ln = (int)(lm / hw);
+          const int r = (int)(lm - (long long)ln * hw);
+          liy0 = (r / p.Wo) * p.stride - ch.pad_t;
+          lix0 = (r % p.Wo) * p.stride - ch.pad_l;
+        }
+        const float* xn = p.x + (size_t)ln * p.H * p.W * p.Cin;
+#pragma unroll
+        for (int j = 0; j < KC / 2; ++j) {
+          const int k = kk * KC + lh * (KC / 2) + j;
+          const int tap = k / p.Cin, c = k - tap * p.Cin;
+          const int iy = liy0 + tap / ch.ksize, ix = lix0 + tap % ch.ksize;
+          const bool ok = lvalid && tap < taps && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
+          // 32-bit offset: one image of a 3-channel input is far below 2^31 floats
+          cp_async4(arow + (lh * (KC / 2) + j) * 4, ok ? xn + ((iy * p.W + ix) * p.Cin + c) : p.x, ok);
+        }
       }
     }
     // weights: 2 * NT * KC contiguous floats
-    const float* wsrc = wch + (size_t)kk * 2 * NT * KC;
-    const uint32_t wdst = smem_u32(st);
+    const float* wsrc = wch + (size_t)kk * WST;
+    const uint32_t wdst = smem_u32(smem + s * WST);
     for (int v = tid; v < NT * KC / 2; v += NUM_THREADS) cp_async16(wdst + v * 16, wsrc + 4 * v, true);
   };
 
-  const int nk = ch.nk;
 #pragma unroll
   for (int s = 0; s < STAGES - 1; ++s) {
     if (s < nk) load_stage(s, s);
@@ -345,9 +397,10 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   }
 
   // ---- MMA role: warpgroup `wg` owns rows [64 wg, 64 wg + 64); A-fragment row g / g + 8 of
-  // warp `wq`'s 16-row slice, columns t / t + 4 of each 8-wide K step
-  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
+  // warp `wq`'s 16-row slice, columns t / t + 4 of each 8-wide K step.  In halo mode the slice
+  // is tile row r = 4 wg + wq and rows g / g + 8 are its columns g / g + 8.
   const int arow0 = wg * 64 + wq * 16 + g;
+  const int r = wg * 4 + wq;
   float acc[2][NACC], sum[NACC];
 #pragma unroll
   for (int i = 0; i < NACC; ++i) acc[0][i] = acc[1][i] = sum[i] = 0.f;
@@ -357,21 +410,33 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
     fence_proxy_async();
     __syncthreads();
     // overwrites stage (kk - 1) % STAGES: both warpgroups have retired its MMAs (mma_chunk
-    // drains) and read its A fragments before the barrier
+    // drains) and read its A fragments before the barrier.  A halo buffer is overwritten
+    // taps - 1 K chunks after the last read of the channel chunk it held.
     if (kk + STAGES - 1 < nk) load_stage(kk + STAGES - 1, (kk + STAGES - 1) % STAGES);
     cp_async_commit();
 
-    const float* st = smem + (size_t)(kk % STAGES) * stage_floats<NT, KC>();
-    const float* sa = st + 2 * NT * KC;
-    mma_chunk<NT, KC>(sa + arow0 * APITCH, sa + (arow0 + 8) * APITCH, smem_u32(st), t, acc, sum);
+    // (in halo mode row arow0 of an 8 x FT_W tile is pixel (r, g), as a 1x1 conv loads it)
+    const float* a0 = sa + (kk % STAGES * TILE_M + arow0) * APITCH;
+    if (MODE == TC_HALO && taps > 1) {
+      const int c = kk / 9, tap = kk - c * 9;
+      a0 = sa + ((c & 1) * FQ_P + (r + tap / 3) * FQ_W + g + tap % 3) * APITCH;
+    }
+    mma_chunk<NT, KC>(a0, a0 + 8 * APITCH, smem_u32(smem + kk % STAGES * WST), t, acc, sum);
   }
   cp_async_wait<0>();
 
   // ---- epilogue: accumulator element 4j + 2h + e is (row g + 8h, column 8j + 2t + e)
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const long long m = m0 + arow0 + 8 * h;
-    if (m >= p.M) continue;
+    long long m = m0 + arow0 + 8 * h;   // output pixel
+    if (MODE == TC_HALO) {
+      const HaloTile tl = halo_tile(p);
+      const int oy = tl.oy0 + r, ox = tl.ox0 + g + 8 * h;
+      if (oy >= p.Ho || ox >= p.Wo) continue;
+      m = ((long long)tl.n * p.Ho + oy) * p.Wo + ox;
+    } else if (m >= p.M) {
+      continue;
+    }
     float* yrow = p.y + (size_t)m * p.y_cstride + ch.y_off;
 #pragma unroll
     for (int j = 0; j < NT / 8; ++j)
@@ -397,7 +462,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
 //   expand:  1x1 and 3x3 convs over Q in chunks of 64 output channels; the A fragments of tap
 //            (dy, dx) are read from Q at the tap-shifted halo row, so the squeeze tensor never
 //            leaves the SM; weights stream through the cp.async ring.
-constexpr int FT_W = 16, FQ_W = FT_W + 2, FQ_P = 10 * FQ_W, FQ_ROWS = 192;
+constexpr int FQ_ROWS = 192;   // FQ_P halo pixels padded to three m64 blocks
 constexpr int MAX_FCHUNKS = 16;
 
 struct FireChunk {
@@ -575,17 +640,20 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
 using ConvKernel = void (*)(TcParams);
 using FireKernel = void (*)(FireParams);
 
-template <int KC, bool GATHER>
+template <int KC, int MODE>
 ConvKernel conv_tc_instance(int NT) {
-  return NT == 64 ? conv_tc_kernel<64, KC, GATHER>
-         : NT == 32 ? conv_tc_kernel<32, KC, GATHER> : conv_tc_kernel<16, KC, GATHER>;
+  return NT == 64 ? conv_tc_kernel<64, KC, MODE>
+         : NT == 32 ? conv_tc_kernel<32, KC, MODE> : conv_tc_kernel<16, KC, MODE>;
 }
 
-// The conv_tc_kernel instantiation of a plan (gather mode always walks K in chunks of 32).
-ConvKernel conv_tc_instance(int NT, int KC, bool gather) {
-  if (NT == 72) return conv_tc_kernel<72, 32, false>;   // pick_nt's head tile
-  if (gather) return conv_tc_instance<32, true>(NT);
-  return KC == 32 ? conv_tc_instance<32, false>(NT) : conv_tc_instance<16, false>(NT);
+// The conv_tc_kernel instantiation of a plan (gather mode always walks K in chunks of 32; the
+// 72-wide head tile only comes with KC = 32).
+ConvKernel conv_tc_instance(int NT, int KC, int mode) {
+  if (NT == 72) return mode == TC_HALO ? conv_tc_kernel<72, 32, TC_HALO> : conv_tc_kernel<72, 32, TC_ROWS>;
+  if (mode == TC_GATHER) return conv_tc_instance<32, TC_GATHER>(NT);
+  if (mode == TC_HALO)
+    return KC == 32 ? conv_tc_instance<32, TC_HALO>(NT) : conv_tc_instance<16, TC_HALO>(NT);
+  return KC == 32 ? conv_tc_instance<32, TC_ROWS>(NT) : conv_tc_instance<16, TC_ROWS>(NT);
 }
 
 template <int KCI, int SQN, int KCE>
@@ -609,7 +677,7 @@ FireKernel fire_tc_instance(int KCI, int SQN, int KCE, size_t* smem) {
 
 struct TcImpl {
   TcParams prm{};
-  int NT = 0, KC = 0;
+  int NT = 0, KC = 0, mode = TC_ROWS;
   ConvKernel kernel = nullptr;
   size_t smem_bytes = 0;
   std::vector<ConvGroup> groups;
@@ -671,16 +739,22 @@ static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo,
   const int KC = (gather || Cin % 32 == 0) ? 32 : 16;
   const int NT = pick_nt(groups, KC, gather);
   if (!NT) return 0;
+  int mode = gather ? TC_GATHER : TC_ROWS;
+  for (const auto& g : groups)
+    if (!gather && g.ksize == 3) mode = TC_HALO;   // stride-1 SAME (tc_conv_eligible)
   const long long M = (long long)B * Ho * Wo;
-  const long long mtiles = (M + TILE_M - 1) / TILE_M;
-  if (M <= 0 || mtiles > 0x7fffffffLL) return 0;
+  const int tiles_w = (Wo + FT_W - 1) / FT_W, tiles_h = (Ho + 7) / 8;
+  const long long blocks = mode == TC_HALO ? (long long)B * tiles_h * tiles_w : (M + TILE_M - 1) / TILE_M;
+  if (M <= 0 || blocks > 0x7fffffffLL) return 0;
   im->NT = NT;
   im->KC = KC;
-  im->kernel = conv_tc_instance(NT, KC, gather);
+  im->mode = mode;
+  im->kernel = conv_tc_instance(NT, KC, mode);
   im->groups = groups;
   TcParams& p = im->prm;
   p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Ho = Ho; p.Wo = Wo; p.stride = stride;
   p.relu = relu; p.y_cstride = y_cstride; p.M = M;
+  p.tiles_w = tiles_w; p.tiles_h = tiles_h;
   int nch = 0, poff = 0;
   long long woff = 0;
   for (const auto& g : groups) {
@@ -703,7 +777,7 @@ static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo,
   p.nchunks = nch;
   im->cout_total = poff;
   im->w_floats = woff;
-  im->smem_bytes = (size_t)STAGES * (TILE_M * (KC + 4) + 2 * NT * KC) * sizeof(float);
+  im->smem_bytes = conv_smem_floats(NT, KC) * sizeof(float);
   cudaError_t ce = cudaFuncSetAttribute(im->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)im->smem_bytes);
   if (ce != cudaSuccess) return cuda_fail(ce, "cudaFuncSetAttribute(conv_tc_kernel)");
@@ -724,15 +798,18 @@ static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo,
 // Packs K chunks [0, nk) of one output-channel chunk [n0, n0 + NT) of a weight matrix whose rows
 // are the flattened HWIO K index (tap * Cin + channel, `kreal` of them) into the tiles the
 // kernels read: per K chunk [NT/8 row groups][KC/4 K core matrices][8 rows][4 floats], hi tile
-// then lo tile.  Rows past `kreal` and channels past `cout` are zero.
+// then lo tile.  Rows past `kreal` and channels past `cout` are zero.  With taps == 1 K chunk kk
+// holds rows [kk * KC, kk * KC + KC); otherwise the chunks walk channel chunk c with the taps
+// inner (the halo-mode order): K chunk c * taps + tap holds rows tap * cin + c * KC + [0, KC).
 static void pack_tiles(const float* w, long long kreal, int cout, int n0, int NT, int KC, int nk,
-                       float* dst) {
+                       int taps, int cin, float* dst) {
   for (int kk = 0; kk < nk; ++kk) {
     float* hi_t = dst + (size_t)kk * 2 * NT * KC;
     float* lo_t = hi_t + NT * KC;
+    const long long k0 = (long long)(kk % taps) * cin + (long long)(kk / taps) * KC;
     for (int n = 0; n < NT; ++n)
       for (int k = 0; k < KC; ++k) {
-        const long long kg = (long long)kk * KC + k;
+        const long long kg = k0 + k;
         const float v = (n0 + n < cout && kg < kreal) ? w[kg * cout + n0 + n] : 0.f;
         const float hi = host_rn_tf32(v);
         const size_t at = ((size_t)(n / 8) * (KC / 4) + k / 4) * 32 + (n % 8) * 4 + k % 4;
@@ -742,15 +819,17 @@ static void pack_tiles(const float* w, long long kreal, int cout, int n0, int NT
   }
 }
 
-// Pack group `gi` weights (HWIO [k,k,Cin,Cout]) into each of its chunks' tiles.  With Cin a
-// multiple of KC (or gather mode) K chunk kk holds flattened K rows [kk * KC, kk * KC + KC).
+// Pack group `gi` weights (HWIO [k,k,Cin,Cout]) into each of its chunks' tiles: in halo mode a
+// 3x3 conv channel chunk by channel chunk with the taps inner, otherwise (1x1, gather mode) K
+// chunk kk holds flattened K rows [kk * KC, kk * KC + KC).
 static void pack_group(const TcImpl* im, int gi, const float* w_hwio, std::vector<float>& packed) {
   const ConvGroup& g = im->groups[gi];
+  const int taps = im->mode == TC_HALO ? g.ksize * g.ksize : 1;
   int ci = im->group_chunk0[gi];
   for (int cb = 0; cb < g.Cout; cb += im->NT, ++ci) {
     const TcChunk& c = im->prm.chunks[ci];
     pack_tiles(w_hwio, (long long)g.ksize * g.ksize * im->prm.Cin, g.Cout, cb, im->NT, im->KC, c.nk,
-               packed.data() + c.w_off);
+               taps, im->prm.Cin, packed.data() + c.w_off);
   }
 }
 
@@ -840,7 +919,9 @@ int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, int
   prm.y = y_dev;
   prm.B = n;
   prm.M = (long long)n * prm.Ho * prm.Wo;
-  const dim3 grid((unsigned)((prm.M + TILE_M - 1) / TILE_M), (unsigned)prm.nchunks);
+  const long long blocks = im->mode == TC_HALO ? (long long)n * prm.tiles_h * prm.tiles_w
+                                               : (prm.M + TILE_M - 1) / TILE_M;
+  const dim3 grid((unsigned)blocks, (unsigned)prm.nchunks);
   im->kernel<<<grid, NUM_THREADS, im->smem_bytes, stream>>>(prm);
   SQ_CHECK_LAUNCH("conv_tc_kernel");
   return SQDET_OK;
@@ -941,13 +1022,13 @@ int tc_fused_fire_pack_weights(TcFusedFirePlan* plan, const float* w_sq, const f
   const FireParams& p = im->fp;
   std::vector<float> wsq((size_t)im->w_floats), wex((size_t)im->w2_floats);
   std::vector<float> bsq(im->SQN, 0.f), bex;
-  pack_tiles(w_sq, p.Cin, p.S, 0, im->SQN, im->KCI, p.Cin / im->KCI, wsq.data());
+  pack_tiles(w_sq, p.Cin, p.S, 0, im->SQN, im->KCI, p.Cin / im->KCI, 1, p.Cin, wsq.data());
   long long off = 0;
   for (int c = 0; c < p.nchunks; ++c) {
     const FireChunk& ch = p.chunks[c];
     const bool e3 = ch.taps == 9;
     pack_tiles(e3 ? w_e3 : w_e1, (long long)ch.taps * p.S, e3 ? im->E3 : im->E1,
-               ch.y_off - (e3 ? im->E1 : 0), 64, im->KCE, ch.nk, wex.data() + off);
+               ch.y_off - (e3 ? im->E1 : 0), 64, im->KCE, ch.nk, 1, p.S, wex.data() + off);
     off += (long long)ch.nk * 2 * 64 * im->KCE;
   }
   for (int i = 0; i < p.S; ++i) bsq[i] = b_sq[i];
