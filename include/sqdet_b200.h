@@ -113,7 +113,9 @@ int sqdet_finalize(sqdet_engine* e);
 /* ---- parameters: replaces tf.train.Saver(model.model_params).restore ---------------
  * (src/demo.py:181-184, src/eval.py:205).  Names are the reference's TF variable
  * names: "<layer>/kernels" [kh,kw,Cin,Cout], "<layer>/biases" [Cout], BN
- * "<scope>/gamma|beta|mean|var" [Cout].  Callable before or after finalize.           */
+ * "<scope>/gamma|beta|mean|var" [Cout].  Callable before or after finalize.  A change
+ * takes effect at the next forward, which first waits for the engine's forwards already
+ * in flight.                                                                          */
 int sqdet_num_params(sqdet_engine* e);
 int sqdet_param_info(sqdet_engine* e, int index, char* name_buf, int name_cap,
                      int64_t shape[4], int* ndim);

@@ -147,6 +147,9 @@ struct sqdet_engine {
   long long n_submitted = 0, n_waited = 0;
   double bgr_means[3] = {103.939, 116.779, 123.68};   // config.py:72
   cudaStream_t own_stream = nullptr;
+  // recorded behind every forward: a reload, sqdet_read_tensor and sqdet_set_box_scale wait for it
+  // rather than for the device, which is invalid while another thread captures a graph
+  cudaEvent_t last_forward = nullptr;
   std::vector<cudaEvent_t> prof_events;
   float* box_scale = nullptr;     // sqdet_set_box_scale's B (x_scale, y_scale) pairs, or null
   // multi-GPU: the ONE collective of the path, ncclAllGather of the result blob
@@ -423,9 +426,14 @@ static int run_postproc(sqdet_engine* e, int n, const float* scales, cudaStream_
   return SQDET_OK;
 }
 
-// Upload parameters and derive what the kernels consume (BN scale/shift, TC packs).
+// Upload parameters and derive what the kernels consume (BN scale/shift, TC packs).  The uploads
+// are synchronous copies on the legacy stream, which is not ordered with the engine's own stream
+// or a caller's non-blocking one.  So the forwards already enqueued are waited for first, or they
+// would read the new weights part-way through, and the legacy stream after the uploads, because a
+// copy from pageable memory can return before its DMA lands and this forward must not read ahead.
 static int prepare_params(sqdet_engine* e) {
   if (!e->params_dirty) return SQDET_OK;
+  SQ_CUDA(cudaEventSynchronize(e->last_forward));
   for (auto& p : e->params) {
     if (!p.dev) SQ_CUDA(cudaMalloc(&p.dev, sizeof(float) * (size_t)p.numel()));
     SQ_CUDA(cudaMemcpy(p.dev, p.host.data(), sizeof(float) * (size_t)p.numel(),
@@ -475,6 +483,7 @@ static int prepare_params(sqdet_engine* e) {
       if (rc) return rc;
     }
   }
+  SQ_CUDA(cudaStreamSynchronize(nullptr));
   e->params_dirty = false;
   // weights changed -> any captured graph still points at the same buffers, so it stays valid
   return SQDET_OK;
@@ -509,7 +518,11 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, int n, const f
   int rc = prepare_params(e);
   if (rc) return rc;
   const bool can_graph = e->use_graph && stream != nullptr;   // legacy stream cannot capture
-  if (!can_graph) return enqueue_all(e, images_dev, n, scales, stream);
+  if (!can_graph) {
+    rc = enqueue_all(e, images_dev, n, scales, stream);
+    if (!rc) SQ_CUDA(cudaEventRecord(e->last_forward, stream));
+    return rc;
+  }
   sqdet_engine::GraphEntry* hit = nullptr;
   for (auto& g : e->graphs)
     if (g.exec && g.input == images_dev && g.stream == stream && g.n == n && g.scales == scales)
@@ -538,6 +551,7 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, int n, const f
     hit = &slot;
   }
   SQ_CUDA(cudaGraphLaunch(hit->exec, stream));
+  SQ_CUDA(cudaEventRecord(e->last_forward, stream));
   return SQDET_OK;
 }
 
@@ -678,6 +692,7 @@ int sqdet_destroy(sqdet_engine* e) {
   }
   if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
   if (e->own_stream) cudaStreamDestroy(e->own_stream);
+  if (e->last_forward) cudaEventDestroy(e->last_forward);
   cudaFree(e->box_scale);
   cudaFree(e->d_gathered);
   if (e->comm && e->comm_owned && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
@@ -843,6 +858,7 @@ int sqdet_finalize(sqdet_engine* e) {
     e->d_counts = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(blob) + rec_bytes);
   }
   SQ_CUDA(cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
+  SQ_CUDA(cudaEventCreateWithFlags(&e->last_forward, cudaEventDisableTiming));
   e->finalized = true;
   e->params_dirty = true;
   return SQDET_OK;
@@ -1011,7 +1027,7 @@ int sqdet_read_tensor(sqdet_engine* e, int id, float* host_out) {
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_read_tensor: bad argument");
   if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_read_tensor before sqdet_finalize");
   DeviceGuard guard(e->device);
-  SQ_CUDA(cudaDeviceSynchronize());
+  SQ_CUDA(cudaEventSynchronize(e->last_forward));
   const Tensor& t = e->tensors[id];
   if (!t.materialized)
     return fail(SQDET_ERR_NOT_FOUND, "tensor '" + t.name + "' is not materialised (fused into its consumer)");
@@ -1196,7 +1212,7 @@ int sqdet_set_box_scale(sqdet_engine* e, const float* xy_scales) {
     if (!(xy_scales[i] > 0.f)) return fail(SQDET_ERR_INVALID_ARG, "sqdet_set_box_scale: scales must be positive");
   // synchronous: no forward may be in flight while the table changes or goes.  No graph is
   // dropped: a graph reads the table at its key's address, whichever table is allocated there.
-  SQ_CUDA(cudaDeviceSynchronize());
+  SQ_CUDA(cudaEventSynchronize(e->last_forward));
   if (!xy_scales) {
     cudaFree(e->box_scale);
     e->box_scale = nullptr;
@@ -1204,6 +1220,8 @@ int sqdet_set_box_scale(sqdet_engine* e, const float* xy_scales) {
   }
   if (!e->box_scale) SQ_CUDA(cudaMalloc(&e->box_scale, sizeof(float) * n));
   SQ_CUDA(cudaMemcpy(e->box_scale, xy_scales, sizeof(float) * n, cudaMemcpyHostToDevice));
+  // the copy from pageable memory may return before its DMA lands; the next forward must not
+  SQ_CUDA(cudaStreamSynchronize(nullptr));
   return SQDET_OK;
 }
 
