@@ -18,14 +18,17 @@
 //   K      : walked in KC-channel chunks (KC = 32 or 16).  Halo mode walks a 3x3 conv channel
 //            chunk by channel chunk with the nine taps inner; a 1x1 conv is its channel chunks.
 //            Gather mode flattens (dy, dx, c) and pads it to a multiple of 32.
-//   A      : cp.async (zero-fill = TF SAME padding) into a row-major [pixel][KC + 4] tile, then
-//            into registers in the wgmma A-fragment layout (the +4 keeps the reads conflict-free).
-//            In halo mode a 3x3 conv loads the 10 x 18 halo of its tile once per channel chunk
-//            and reads tap (dy, dx) at a row offset into it, so each input value crosses from L2
-//            once per channel chunk instead of once per tap.
+//   A      : TMA tensor-map loads (out-of-bounds zero fill = TF SAME padding) into a row-major
+//            [pixel][KC] tile stored with the 128-byte (KC = 32) or 64-byte (KC = 16) swizzle,
+//            then into registers in the wgmma A-fragment layout (the swizzle keeps the reads
+//            conflict-free).  In halo mode a 3x3 conv loads the 10 x 18 halo of its tile once per
+//            channel chunk and reads tap (dy, dx) at a row offset into it, so each input value
+//            crosses from L2 once per channel chunk instead of once per tap.  Gather mode (a
+//            12-byte pixel is below TMA's 16-byte granule) gathers with cp.async into the same
+//            swizzled layout.
 //   W      : host-packed per (chunk, K chunk) in the no-swizzle K-major core-matrix layout
-//            [NT/8][KC/4][8 rows][4 floats], hi then lo half; cp.async, read by wgmma through a
-//            shared-memory descriptor.
+//            [NT/8][KC/4][8 rows][4 floats], hi then lo half; one bulk copy per K chunk, read by
+//            wgmma through a shared-memory descriptor.
 // Precision: fp32 operands are split a = a_hi + a_lo with a_hi = rn_tf32(a), a_lo = rn_tf32(a - a_hi)
 //   (rounding a_lo here keeps the tensor core's truncation of its inputs from biasing the sum);
 //   D += a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (the dropped lo*lo term is ~2^-22 of a product): fp32-
@@ -36,13 +39,15 @@
 //   accumulator and is then added into fp32 running sums with round-to-nearest FADDs, so the
 //   tensor core's truncating accumulation never compounds over a long K (longer chains in the
 //   accumulator left a one-signed error that fails the 1e-4 box parity of SqueezeDet+).
-// Pipeline: 3-stage cp.async ring (one commit group per K chunk; a halo tile travels in the
-//   group of the first K chunk that reads it, and two halo buffers alternate between channel
-//   chunks).  Within a K chunk the steps
-//   alternate between two accumulator sets: step k + 1's MMAs are issued before step k is
-//   waited for (wait_group 1) and added in, and the next A fragment is loaded and split while
-//   they run.  Each chunk ends with wait_group 0, so a stage is free again at the next block
-//   barrier.
+// Pipeline: 3-stage ring tracked by mbarriers.  A stage's `full` barrier completes on the bytes
+//   of its copies; its `empty` barrier on one arrival per consumer warp once the warp has retired
+//   the MMAs that read it.  One thread waits for a stage to be empty and issues its copies, so the
+//   K loop has no block barrier.  A halo tile travels with the first K chunk that reads it, and
+//   two halo buffers alternate between channel chunks.  Within a K chunk the steps alternate
+//   between two accumulator sets: step k + 1's MMAs are issued before step k is waited for
+//   (wait_group 1) and added in, and the next A fragment is loaded and split while they run.
+//   Each chunk ends with wait_group 0 before its warp releases the stage.
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -77,6 +82,10 @@ struct TcChunk {
 };
 
 struct TcParams {
+  // tensor maps over x (encoded per launch input): row mode (C, B*H*W) boxes of (KC, 128); halo
+  // mode (C, W, H, B) boxes of (KC, 18, 10, 1) for 3x3 halos in `amap`, (KC, 16, 8, 1) for the
+  // tile of a 1x1 conv in `amap1`
+  CUtensorMap amap, amap1;
   const float* x;
   float* y;
   const float* w;
@@ -113,6 +122,63 @@ __device__ __forceinline__ void cp_async_wait() {
 // cp.async writes are generic-proxy writes; wgmma reads shared memory through the async proxy
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+// makes cp.async operations this thread issued so far arrive on `bar` when they complete (the
+// barrier's count includes the arrival)
+__device__ __forceinline__ void cp_async_arrive(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
+// mbarriers
+__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+// orders the initialisations before the barriers' use by other threads and the async proxy
+__device__ __forceinline__ void mbar_init_fence() {
+  asm volatile("fence.mbarrier_init.release.cluster;\n\tfence.proxy.async.shared::cta;" ::: "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// arrives and adds `bytes` to the transaction count the current phase waits for
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
+               "r"(bytes)
+               : "memory");
+}
+// waits for the completion of the phase of parity `parity`
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred done;\n\t"
+      "WAIT_%=:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 done, [%0], %1;\n\t"
+      "@!done bra WAIT_%=;\n\t}" ::"r"(smem_u32(bar)),
+      "r"(parity)
+      : "memory");
+}
+
+// `bytes` contiguous bytes from global memory into shared memory, completing on `bar`
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
+      "l"(src), "r"(bytes), "r"(smem_u32(bar))
+      : "memory");
+}
+// one box of a 2-D / 4-D tensor map at the given coordinates (innermost first), completing on `bar`
+__device__ __forceinline__ void tma_load(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes "
+      "[%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
+      "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+      : "memory");
+}
+__device__ __forceinline__ void tma_load(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2,
+                                         int c3, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes "
+      "[%0], [%1, {%2, %3, %4, %5}], [%6];" ::"r"(dst),
+      "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar))
+      : "memory");
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() {
@@ -212,25 +278,50 @@ struct Mma<72> {
   }
 };
 
-// conv_tc_kernel's shared memory: the weight ring, STAGES x [2 NT KC], then the A tiles:
-// STAGES x [TILE_M][KC + 4] (one per stage), or in halo mode for a 3x3 conv two [FQ_P][KC + 4]
-// halo tiles in the same space.
-static_assert(2 * FQ_P <= STAGES * TILE_M, "two halo tiles fit in the A ring");
-constexpr size_t conv_smem_floats(int NT, int KC) {
-  return (size_t)STAGES * (2 * NT * KC + TILE_M * (KC + 4));
+// conv_tc_kernel's shared memory, from a 1024-byte aligned base (the swizzle pattern repeats
+// every 1024 bytes): the weight ring, STAGES x [2 NT KC]; the A tiles, STAGES x [TILE_M][KC] (one
+// per stage), or in halo mode for a 3x3 conv two halo tiles of halo_rows(KC) rows in the same
+// space; then the full and empty barrier of each stage.
+__host__ __device__ constexpr int halo_rows(int KC) {   // FQ_P rows rounded up to a multiple of 1024 bytes
+  return (FQ_P * KC * 4 + 1023) / 1024 * 1024 / (KC * 4);
+}
+static_assert(2 * halo_rows(16) <= STAGES * TILE_M && 2 * halo_rows(32) <= STAGES * TILE_M,
+              "two halo tiles fit in the A ring");
+constexpr size_t conv_smem_bytes(int NT, int KC) {
+  return 1024 + (size_t)STAGES * (2 * NT * KC + TILE_M * KC) * sizeof(float) + 2 * STAGES * sizeof(uint64_t);
 }
 
-// A fragment of 8-wide K step `ks` for this thread's rows g (a0) and g + 8 (a1), split into its
-// TF32 hi part and rounded lo remainder.
-__device__ __forceinline__ void load_split(const float* a0, const float* a1, int ks, int t,
-                                           uint32_t (&ahi)[4], uint32_t (&alo)[4]) {
-  const float v[4] = {a0[ks * 8 + t], a1[ks * 8 + t], a0[ks * 8 + t + 4], a1[ks * 8 + t + 4]};
+// Splits four fp32 A values into their TF32 hi parts and rounded lo remainders.
+__device__ __forceinline__ void split(const float (&v)[4], uint32_t (&ahi)[4], uint32_t (&alo)[4]) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const float hi = rn_tf32(v[i]);
     ahi[i] = __float_as_uint(hi);
     alo[i] = __float_as_uint(rn_tf32(v[i] - hi));   // rounded, not truncated by the MMA
   }
+}
+
+// A fragment of 8-wide K step `ks` for this thread's rows g (a0) and g + 8 (a1) of a padded tile.
+__device__ __forceinline__ void load_split(const float* a0, const float* a1, int ks, int t,
+                                           uint32_t (&ahi)[4], uint32_t (&alo)[4]) {
+  split({a0[ks * 8 + t], a1[ks * 8 + t], a0[ks * 8 + t + 4], a1[ks * 8 + t + 4]}, ahi, alo);
+}
+
+// The swizzled [pixel][KC] tiles: 16-byte column chunk j of row p is stored at chunk j ^ swz(p),
+// TMA's 128-byte swizzle for KC = 32 (128-byte rows), its 64-byte swizzle for KC = 16.  Rows
+// p .. p + 7 then cover every bank once, at any p (so at every halo tap offset too).
+template <int KC>
+__device__ __forceinline__ int swz(int p) {
+  return KC == 32 ? (p & 7) : ((p >> 1) & 3);
+}
+// A fragment of K step `ks` for rows p and p + 8 (which share the swizzle) of a swizzled tile
+template <int KC>
+__device__ __forceinline__ void load_split_swz(const float* tile, int p, int ks, int t,
+                                               uint32_t (&ahi)[4], uint32_t (&alo)[4]) {
+  const float* a0 = tile + p * KC + t;
+  const float* a1 = a0 + 8 * KC;
+  const int j0 = (2 * ks ^ swz<KC>(p)) * 4, j1 = ((2 * ks + 1) ^ swz<KC>(p)) * 4;
+  split({a0[j0], a1[j0], a0[j1], a1[j1]}, ahi, alo);
 }
 
 // Issues K step `ks` of a KC-channel chunk as one wgmma group: the three split MMAs into `acc`,
@@ -263,27 +354,26 @@ __device__ __forceinline__ void flush(float (&acc)[N], float (&sum)[N], uint32_t
   }
 }
 
-// One K chunk of KC channels for this thread's A-fragment rows g (a0) and g + 8 (a1), each
-// pointing at the chunk's first column in shared memory; B at `bhi`.  Software-pipelined over
-// two accumulator sets: step ks runs into acc[ks & 1], and while its MMAs are in flight the
-// previous step is retired (wgmma.wait_group 1) and added into the fp32 running sums, and the
-// next step's A fragment is loaded and split.  Every step still runs from a zeroed accumulator
-// and is added in K order, as in an unpipelined loop.
+// One K chunk of KC channels; `load_a(ks, ahi, alo)` loads and splits this thread's A fragment
+// of step ks, B is at `bhi`.  Software-pipelined over two accumulator sets: step ks runs into
+// acc[ks & 1], and while its MMAs are in flight the previous step is retired
+// (wgmma.wait_group 1) and added into the fp32 running sums, and the next step's A fragment is
+// loaded and split.  Every step still runs from a zeroed accumulator and is added in K order, as
+// in an unpipelined loop.
 //
 // The chunk ends with every group retired (wait_group 0).  That drain leaves one MMA latency
-// exposed per chunk, but it is what makes the caller's 3-stage ring safe: past the next block
-// barrier no wgmma reads the stage that the prefetch then overwrites.  (ptxas also serialises
-// every wgmma of a kernel whose accumulators are read in a loop that a group stays in flight
-// across.)
-template <int NT, int KC>
-__device__ __forceinline__ void mma_chunk(const float* a0, const float* a1, uint32_t bhi, int t,
-                                          float (&acc)[2][NT / 2], float (&sum)[NT / 2]) {
+// exposed per chunk, but after it no wgmma of this warpgroup reads the chunk's stage, so the
+// caller may release it.  (ptxas also serialises every wgmma of a kernel whose accumulators are
+// read in a loop that a group stays in flight across.)
+template <int NT, int KC, typename LoadA>
+__device__ __forceinline__ void mma_chunk(LoadA load_a, uint32_t bhi, float (&acc)[2][NT / 2],
+                                          float (&sum)[NT / 2]) {
   constexpr int KSTEPS = KC / 8;
   uint32_t ahi[2][4], alo[2][4];
 #pragma unroll
   for (int ks = 0; ks < KSTEPS; ++ks) {
     const int cur = ks & 1;
-    load_split(a0, a1, ks, t, ahi[cur], alo[cur]);
+    load_a(ks, ahi[cur], alo[cur]);
     mma_step<NT, KC>(acc[cur], ahi[cur], alo[cur], bhi, ks);
     if (ks > 0) {
       wgmma_wait<1>();
@@ -311,90 +401,105 @@ __device__ __forceinline__ HaloTile halo_tile(const TcParams& p) {
 template <int NT, int KC, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, NT == 72 ? 1 : 2)
 conv_tc_kernel(const __grid_constant__ TcParams p) {
-  constexpr int APITCH = KC + 4;
   constexpr int NACC = NT / 2;
   constexpr int WST = 2 * NT * KC;   // floats of one stage's hi + lo weight tiles
-  extern __shared__ __align__(128) float smem[];
+  constexpr uint32_t W_BYTES = WST * 4, TILE_BYTES = TILE_M * KC * 4, HALO_BYTES = FQ_P * KC * 4;
+  constexpr int HROWS = halo_rows(KC);
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  float* const smem = reinterpret_cast<float*>(smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023));
   float* const sa = smem + STAGES * WST;   // A tiles
+  uint64_t* const full = reinterpret_cast<uint64_t*>(sa + STAGES * TILE_M * KC);
+  uint64_t* const empty = full + STAGES;
 
   const TcChunk& ch = p.chunks[blockIdx.y];
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
   const float* wch = p.w + ch.w_off;
   const int nk = ch.nk;
-
-  // ---- row and gather mode: 128 consecutive output pixels from m0; loader thread role: pixel
-  // `lp`, half `lh` of the KC channels of each K chunk
-  const long long m0 = (long long)blockIdx.x * TILE_M;
-  const int lp = tid >> 1, lh = tid & 1;
-  const long long lm = m0 + lp;
-  const bool lvalid = MODE != TC_HALO && lm < p.M;
   const int taps = ch.ksize * ch.ksize;   // 1 or 9
 
-  // rows x cols input pixels from (y0, x0) of image n, channels [c0, c0 + KC), into a
-  // [rows * cols][APITCH] tile; zero outside the image.  Kept rolled: unrolled, its address
-  // registers push the 64-wide tile past 128 registers into spills.
-  auto load_block = [&](float* dst, int rows, int cols, int y0, int x0, int n, int c0) {
-    const float* xn = p.x + (size_t)n * p.H * p.W * p.Cin;
-#pragma unroll 1
-    for (int v = tid; v < rows * cols * (KC / 4); v += NUM_THREADS) {
-      const int row = v / (KC / 4), j = v % (KC / 4);
-      const int iy = y0 + row / cols, ix = x0 + row % cols;
-      const bool ok = iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
-      cp_async16(smem_u32(dst + row * APITCH + 4 * j),
-                 ok ? xn + ((size_t)iy * p.W + ix) * p.Cin + c0 + 4 * j : p.x, ok);
+  if (tid == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      // gather mode: every thread's cp.async arrival besides the weight copy's
+      mbar_init(&full[s], MODE == TC_GATHER ? NUM_THREADS + 1 : 1);
+      mbar_init(&empty[s], NUM_THREADS / 32);
     }
-  };
-
-  // K chunk kk into stage s: its weights, and the A values it is the first to read
-  auto load_stage = [&](int kk, int s) {
-    if (MODE == TC_HALO) {
-      // (re-derived from blockIdx rather than kept in registers across the K loop)
-      const HaloTile tl = halo_tile(p);
-      if (taps == 1)
-        load_block(sa + s * TILE_M * APITCH, 8, FT_W, tl.oy0, tl.ox0, tl.n, kk * KC);
-      else if (kk % 9 == 0)   // channel chunk c = kk / 9: its halo, into buffer c & 1
-        load_block(sa + (kk / 9 & 1) * FQ_P * APITCH, 10, FQ_W, tl.oy0 - 1, tl.ox0 - 1, tl.n, kk / 9 * KC);
-    } else {
-      const uint32_t arow = smem_u32(sa + (s * TILE_M + lp) * APITCH);
-      if (MODE == TC_ROWS) {
-        // 1x1, stride 1: output pixel m reads input pixel m
-        const float* src = p.x + (size_t)(lvalid ? lm : 0) * p.Cin + kk * KC + lh * (KC / 2);
-#pragma unroll
-        for (int v = 0; v < KC / 8; ++v)
-          cp_async16(arow + (lh * (KC / 2) + 4 * v) * 4, src + 4 * v, lvalid);
-      } else {
-        int ln = 0, liy0 = 0, lix0 = 0;
-        if (lvalid) {
-          const int hw = p.Ho * p.Wo;
-          ln = (int)(lm / hw);
-          const int r = (int)(lm - (long long)ln * hw);
-          liy0 = (r / p.Wo) * p.stride - ch.pad_t;
-          lix0 = (r % p.Wo) * p.stride - ch.pad_l;
-        }
-        const float* xn = p.x + (size_t)ln * p.H * p.W * p.Cin;
-#pragma unroll
-        for (int j = 0; j < KC / 2; ++j) {
-          const int k = kk * KC + lh * (KC / 2) + j;
-          const int tap = k / p.Cin, c = k - tap * p.Cin;
-          const int iy = liy0 + tap / ch.ksize, ix = lix0 + tap % ch.ksize;
-          const bool ok = lvalid && tap < taps && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
-          // 32-bit offset: one image of a 3-channel input is far below 2^31 floats
-          cp_async4(arow + (lh * (KC / 2) + j) * 4, ok ? xn + ((iy * p.W + ix) * p.Cin + c) : p.x, ok);
-        }
-      }
-    }
-    // weights: 2 * NT * KC contiguous floats
-    const float* wsrc = wch + (size_t)kk * WST;
-    const uint32_t wdst = smem_u32(smem + s * WST);
-    for (int v = tid; v < NT * KC / 2; v += NUM_THREADS) cp_async16(wdst + v * 16, wsrc + 4 * v, true);
-  };
-
-#pragma unroll
-  for (int s = 0; s < STAGES - 1; ++s) {
-    if (s < nk) load_stage(s, s);
-    cp_async_commit();
+    mbar_init_fence();
   }
+  __syncthreads();
+
+  // ---- row and gather mode: 128 consecutive output pixels from m0
+  const long long m0 = (long long)blockIdx.x * TILE_M;
+
+  // Gather mode, every thread: pixel `lp`, half `lh` of the 32 K values of K chunk kk into stage s
+  auto gather_stage = [&](int kk, int s) {
+    const int lp = tid >> 1, lh = tid & 1;
+    const long long lm = m0 + lp;
+    const bool lvalid = lm < p.M;
+    int ln = 0, liy0 = 0, lix0 = 0;
+    if (lvalid) {
+      const int hw = p.Ho * p.Wo;
+      ln = (int)(lm / hw);
+      const int r = (int)(lm - (long long)ln * hw);
+      liy0 = (r / p.Wo) * p.stride - ch.pad_t;
+      lix0 = (r % p.Wo) * p.stride - ch.pad_l;
+    }
+    const float* xn = p.x + (size_t)ln * p.H * p.W * p.Cin;
+    float* const arow = sa + (s * TILE_M + lp) * KC;
+#pragma unroll
+    for (int j = 0; j < KC / 2; ++j) {
+      const int col = lh * (KC / 2) + j, k = kk * KC + col;
+      const int tap = k / p.Cin, c = k - tap * p.Cin;
+      const int iy = liy0 + tap / ch.ksize, ix = lix0 + tap % ch.ksize;
+      const bool ok = lvalid && tap < taps && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
+      // 32-bit offset: one image of a 3-channel input is far below 2^31 floats
+      cp_async4(smem_u32(arow + ((col >> 2 ^ swz<KC>(lp)) << 2) + (col & 3)),
+                ok ? xn + ((iy * p.W + ix) * p.Cin + c) : p.x, ok);
+    }
+    cp_async_arrive(&full[s]);
+  };
+
+  // K chunk j into stage s once the warps have released the stage's previous K chunk: its
+  // weights and the A values it is the first to read.  Thread 0 issues the bulk and tensor copies.
+  auto load_stage = [&](int j) {
+    const int s = j % STAGES;
+    if (MODE == TC_GATHER) {
+      if (j >= STAGES) mbar_wait(&empty[s], (j / STAGES & 1) ^ 1);
+      gather_stage(j, s);
+    } else if (tid == 0 && j >= STAGES) {
+      mbar_wait(&empty[s], (j / STAGES & 1) ^ 1);
+    }
+    if (tid != 0) return;
+    uint32_t bytes = W_BYTES;
+    if (MODE == TC_ROWS) {
+      // 1x1, stride 1: output pixel m reads input pixel m
+      bytes += TILE_BYTES;
+      mbar_expect_tx(&full[s], bytes);
+      tma_load(smem_u32(sa + s * TILE_M * KC), &p.amap, j * KC, (int)m0, &full[s]);
+    } else if (MODE == TC_HALO) {
+      const HaloTile tl = halo_tile(p);
+      if (taps == 1) {
+        bytes += TILE_BYTES;
+        mbar_expect_tx(&full[s], bytes);
+        tma_load(smem_u32(sa + s * TILE_M * KC), &p.amap1, j * KC, tl.ox0, tl.oy0, tl.n, &full[s]);
+      } else if (j % 9 == 0) {
+        // channel chunk c = j / 9: its halo, into buffer c & 1, whose last reader (K chunk j - 10)
+        // was released before K chunk j - STAGES was
+        bytes += HALO_BYTES;
+        mbar_expect_tx(&full[s], bytes);
+        tma_load(smem_u32(sa + (j / 9 & 1) * HROWS * KC), &p.amap, j / 9 * KC, tl.ox0 - 1, tl.oy0 - 1,
+                 tl.n, &full[s]);
+      } else {
+        mbar_expect_tx(&full[s], bytes);
+      }
+    } else {
+      mbar_expect_tx(&full[s], bytes);
+    }
+    bulk_load(smem_u32(smem + s * WST), wch + (size_t)j * WST, W_BYTES, &full[s]);
+  };
+
+#pragma unroll 1
+  for (int j = 0; j < STAGES - 1 && j < nk; ++j) load_stage(j);
 
   // ---- MMA role: warpgroup `wg` owns rows [64 wg, 64 wg + 64); A-fragment row g / g + 8 of
   // warp `wq`'s 16-row slice, columns t / t + 4 of each 8-wide K step.  In halo mode the slice
@@ -406,24 +511,24 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   for (int i = 0; i < NACC; ++i) acc[0][i] = acc[1][i] = sum[i] = 0.f;
 
   for (int kk = 0; kk < nk; ++kk) {
-    cp_async_wait<STAGES - 2>();
-    fence_proxy_async();
-    __syncthreads();
-    // overwrites stage (kk - 1) % STAGES: both warpgroups have retired its MMAs (mma_chunk
-    // drains) and read its A fragments before the barrier.  A halo buffer is overwritten
-    // taps - 1 K chunks after the last read of the channel chunk it held.
-    if (kk + STAGES - 1 < nk) load_stage(kk + STAGES - 1, (kk + STAGES - 1) % STAGES);
-    cp_async_commit();
+    if (kk + STAGES - 1 < nk) load_stage(kk + STAGES - 1);
+    const int s = kk % STAGES;
+    mbar_wait(&full[s], kk / STAGES & 1);
 
     // (in halo mode row arow0 of an 8 x FT_W tile is pixel (r, g), as a 1x1 conv loads it)
-    const float* a0 = sa + (kk % STAGES * TILE_M + arow0) * APITCH;
+    const float* tile = sa + s * TILE_M * KC;
+    int prow = arow0;
     if (MODE == TC_HALO && taps > 1) {
       const int c = kk / 9, tap = kk - c * 9;
-      a0 = sa + ((c & 1) * FQ_P + (r + tap / 3) * FQ_W + g + tap % 3) * APITCH;
+      tile = sa + (c & 1) * HROWS * KC;
+      prow = (r + tap / 3) * FQ_W + g + tap % 3;
     }
-    mma_chunk<NT, KC>(a0, a0 + 8 * APITCH, smem_u32(smem + kk % STAGES * WST), t, acc, sum);
+    mma_chunk<NT, KC>(
+        [&](int ks, uint32_t(&ahi)[4], uint32_t(&alo)[4]) { load_split_swz<KC>(tile, prow, ks, t, ahi, alo); },
+        smem_u32(smem + s * WST), acc, sum);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
   }
-  cp_async_wait<0>();
 
   // ---- epilogue: accumulator element 4j + 2h + e is (row g + 8h, column 8j + 2t + e)
 #pragma unroll
@@ -461,7 +566,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
 //            as Q[halo pixel][SQN + 4] fp32;
 //   expand:  1x1 and 3x3 convs over Q in chunks of 64 output channels; the A fragments of tap
 //            (dy, dx) are read from Q at the tap-shifted halo row, so the squeeze tensor never
-//            leaves the SM; weights stream through the cp.async ring.
+//            leaves the SM; weights stream through the mbarrier ring, one bulk copy per K chunk.
 constexpr int FQ_ROWS = 192;   // FQ_P halo pixels padded to three m64 blocks
 constexpr int MAX_FCHUNKS = 16;
 
@@ -496,6 +601,8 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
   constexpr int RING = fire_ring_floats<KCI, SQN, KCE>();
   extern __shared__ __align__(128) float smem[];
   float* q = smem + STAGES * RING;
+  uint64_t* const full = reinterpret_cast<uint64_t*>(q + FQ_ROWS * QP);   // expand weight ring
+  uint64_t* const empty = full + STAGES;
 
   int tile = blockIdx.x;
   const int tx = tile % p.tiles_w;
@@ -505,6 +612,13 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
   const float* xn = p.x + (size_t)n * p.H * p.W * p.Cin;
+  if (tid == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], NUM_THREADS / 32);
+    }
+    mbar_init_fence();
+  }
 
   auto load_sq = [&](int kk, int s) {
     float* st = smem + (size_t)s * RING;
@@ -557,7 +671,11 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
       flush(accq[1], sq[1], qhi[1], qlo[1]);
     } else {
       const int r0 = 64 + rb;
-      mma_chunk<SQN, KCI>(sa + r0 * API, sa + (r0 + 8) * API, smem_u32(st), t, accq, sq[0]);
+      mma_chunk<SQN, KCI>(
+          [&](int ks, uint32_t(&ahi)[4], uint32_t(&alo)[4]) {
+            load_split(sa + r0 * API, sa + (r0 + 8) * API, ks, t, ahi, alo);
+          },
+          smem_u32(st), accq, sq[0]);
     }
   }
   cp_async_wait<0>();
@@ -581,18 +699,22 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
   }
   __syncthreads();   // Q complete; every squeeze MMA has retired, so the ring is free
 
-  // ---- expand: pixel rows g / g + 8 of this warp are tile row (4 wg + wq), columns g / g + 8
+  // ---- expand: pixel rows g / g + 8 of this warp are tile row (4 wg + wq), columns g / g + 8.
+  // Its weight tiles stream through the ring, K chunk `it` into stage it % STAGES once the warps
+  // have released the stage's previous K chunk; thread 0 waits for that and issues the copy.
   const int spt = p.S / KCE;   // K chunks per tap
   const int total = p.total_nk;
-  auto load_ex = [&](int it, int s) {
-    const float* wsrc = p.wex + (size_t)it * 2 * 64 * KCE;
-    const uint32_t dst = smem_u32(smem + (size_t)s * RING);
-    for (int v = tid; v < 64 * KCE / 2; v += NUM_THREADS) cp_async16(dst + v * 16, wsrc + 4 * v, true);
+  constexpr uint32_t EX_BYTES = 2 * 64 * KCE * 4;
+  auto load_ex = [&](int it) {
+    const int s = it % STAGES;
+    if (it >= STAGES) mbar_wait(&empty[s], (it / STAGES & 1) ^ 1);
+    mbar_expect_tx(&full[s], EX_BYTES);
+    bulk_load(smem_u32(smem + (size_t)s * RING), p.wex + (size_t)it * 2 * 64 * KCE, EX_BYTES, &full[s]);
   };
-#pragma unroll
-  for (int s = 0; s < STAGES - 1; ++s) {
-    if (s < total) load_ex(s, s);
-    cp_async_commit();
+  if (tid == 0) {
+    // the squeeze's cp.async writes to the ring were fenced before the barrier above
+#pragma unroll 1
+    for (int it = 0; it < STAGES - 1 && it < total; ++it) load_ex(it);
   }
   const int r = wg * 4 + wq;
   float acc[2][32], sum[32];
@@ -600,24 +722,30 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
   for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i] = sum[i] = 0.f;
   int c = 0, kk = 0;
   for (int it = 0; it < total; ++it) {
-    cp_async_wait<STAGES - 2>();
-    fence_proxy_async();
-    __syncthreads();
-    if (it + STAGES - 1 < total) load_ex(it + STAGES - 1, (it + STAGES - 1) % STAGES);
-    cp_async_commit();
+    if (tid == 0 && it + STAGES - 1 < total) load_ex(it + STAGES - 1);
+    const int s = it % STAGES;
+    mbar_wait(&full[s], it / STAGES & 1);
     const FireChunk& ch = p.chunks[c];
     const int tap = kk / spt, k0 = (kk - tap * spt) * KCE;
     const int dy = ch.taps == 1 ? 1 : tap / 3, dx = ch.taps == 1 ? 1 : tap % 3;
     const int qr = (r + dy) * FQ_W + g + dx;
-    mma_chunk<64, KCE>(q + qr * QP + k0, q + (qr + 8) * QP + k0,
-                       smem_u32(smem + (size_t)(it % STAGES) * RING), t, acc, sum);
+    mma_chunk<64, KCE>(
+        [&](int ks, uint32_t(&ahi)[4], uint32_t(&alo)[4]) {
+          load_split(q + qr * QP + k0, q + (qr + 8) * QP + k0, ks, t, ahi, alo);
+        },
+        smem_u32(smem + (size_t)s * RING), acc, sum);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
     if (++kk == ch.nk) {
-      const int oy = oy0 + r;
+      // (the tile re-derived from blockIdx rather than kept in registers across the K loop)
+      const int tl = blockIdx.x / p.tiles_w;
+      const int oy = tl % p.tiles_h * 8 + r;
+      const size_t prow = ((size_t)(tl / p.tiles_h) * p.H + oy) * p.W;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int ox = ox0 + g + 8 * h;
         if (oy >= p.H || ox >= p.W) continue;
-        float* yrow = p.y + (((size_t)n * p.H + oy) * p.W + ox) * p.Etot + ch.y_off;
+        float* yrow = p.y + (prow + ox) * p.Etot + ch.y_off;
 #pragma unroll
         for (int j = 0; j < 8; ++j)
 #pragma unroll
@@ -632,7 +760,6 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
       ++c;
     }
   }
-  cp_async_wait<0>();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -658,7 +785,8 @@ ConvKernel conv_tc_instance(int NT, int KC, int mode) {
 
 template <int KCI, int SQN, int KCE>
 FireKernel fire_tc_instance(size_t* smem) {
-  *smem = sizeof(float) * ((size_t)STAGES * fire_ring_floats<KCI, SQN, KCE>() + FQ_ROWS * (SQN + 4));
+  *smem = sizeof(float) * ((size_t)STAGES * fire_ring_floats<KCI, SQN, KCE>() + FQ_ROWS * (SQN + 4)) +
+          2 * STAGES * sizeof(uint64_t);
   return fire_tc_kernel<KCI, SQN, KCE>;
 }
 
@@ -688,6 +816,9 @@ struct TcImpl {
   float* d_scale = nullptr;
   float* d_shift = nullptr;
   long long w_floats = 0;
+  // the input and image count prm's tensor maps were encoded for (null: none yet)
+  const float* map_x = nullptr;
+  int map_n = 0;
 };
 
 static inline float host_rn_tf32(float x) {
@@ -718,6 +849,61 @@ static int pick_nt(const std::vector<ConvGroup>& groups, int KC, bool gather) {
     if (!best || cost < best_cost) best = nt, best_cost = cost;
   }
   return best;
+}
+
+using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
+                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                   CUtensorMapFloatOOBfill);
+
+// A tiled tensor map over the fp32 tensor at x: `rank` dims (innermost first, dims[0] the
+// channels) of densely packed `dims`, boxes of `box`, stored with the swizzle the kernel reads
+// KC-channel rows with; elements outside the tensor read as zero.
+static int encode_map(CUtensorMap* map, const float* x, int rank, const cuuint64_t* dims,
+                      const cuuint32_t* box, int KC) {
+  static EncodeTiledFn encode = [] {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      fn = nullptr;
+    return reinterpret_cast<EncodeTiledFn>(fn);
+  }();
+  if (!encode) return fail(SQDET_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
+  cuuint64_t strides[3];
+  cuuint64_t stride = sizeof(float);
+  for (int i = 0; i + 1 < rank; ++i) strides[i] = stride *= dims[i];
+  const cuuint32_t elem_strides[4] = {1, 1, 1, 1};
+  const CUresult rc = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<float*>(x), dims, strides,
+                             box, elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                             KC == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (rc != CUDA_SUCCESS)
+    return fail(SQDET_ERR_CUDA, "cuTensorMapEncodeTiled failed (error " + std::to_string((int)rc) + ")");
+  return SQDET_OK;
+}
+
+// Encodes the plan's tensor maps for input x of n images, unless they already are.
+static int update_maps(TcImpl* im, const float* x, int n) {
+  if (im->mode == TC_GATHER || (im->map_x == x && im->map_n == n)) return SQDET_OK;
+  TcParams& p = im->prm;
+  const cuuint32_t KC = im->KC;
+  im->map_x = nullptr;
+  int rc;
+  if (im->mode == TC_ROWS) {
+    const cuuint64_t dims[2] = {(cuuint64_t)p.Cin, (cuuint64_t)n * p.H * p.W};
+    const cuuint32_t box[2] = {KC, TILE_M};
+    rc = encode_map(&p.amap, x, 2, dims, box, im->KC);
+  } else {
+    const cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)n};
+    const cuuint32_t halo[4] = {KC, FQ_W, 10, 1}, tile[4] = {KC, FT_W, 8, 1};
+    rc = encode_map(&p.amap, x, 4, dims, halo, im->KC);
+    if (!rc) rc = encode_map(&p.amap1, x, 4, dims, tile, im->KC);
+  }
+  if (rc) return rc;
+  im->map_x = x;
+  im->map_n = n;
+  return SQDET_OK;
 }
 
 static void release_impl(void** impl) {
@@ -777,7 +963,7 @@ static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo,
   p.nchunks = nch;
   im->cout_total = poff;
   im->w_floats = woff;
-  im->smem_bytes = conv_smem_floats(NT, KC) * sizeof(float);
+  im->smem_bytes = conv_smem_bytes(NT, KC);
   cudaError_t ce = cudaFuncSetAttribute(im->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)im->smem_bytes);
   if (ce != cudaSuccess) return cuda_fail(ce, "cudaFuncSetAttribute(conv_tc_kernel)");
@@ -912,9 +1098,11 @@ int tc_conv_set_affine(TcConvPlan* plan, const float* scale, const float* shift)
 
 int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, int n,
                    cudaStream_t stream) {
-  const TcImpl* im = static_cast<const TcImpl*>(plan.impl);
+  TcImpl* im = static_cast<TcImpl*>(plan.impl);
+  if (n < 1 || n > im->prm.B) return fail(SQDET_ERR_INVALID_ARG, "launch_conv_tc: image count outside [1, B]");
+  const int rc = update_maps(im, x_dev, n);
+  if (rc) return rc;
   TcParams prm = im->prm;
-  if (n < 1 || n > prm.B) return fail(SQDET_ERR_INVALID_ARG, "launch_conv_tc: image count outside [1, B]");
   prm.x = x_dev;
   prm.y = y_dev;
   prm.B = n;

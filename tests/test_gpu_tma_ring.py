@@ -1,0 +1,121 @@
+"""The operand ring of the tensor-core convolution (conv_tc.cu): TMA tensor-map loads of the
+activations, one bulk copy per weight tile, and full / empty mbarriers per stage instead of a block
+barrier.  K chunk counts below, at and just above the three stages, a 216-chunk K (the ConvDet
+head's, over which each barrier's phase wraps 72 times), several output-channel chunks in one
+launch, both K chunk widths (so both the 128-byte and the 64-byte swizzle), a row-mode pixel count
+that is not a multiple of 128, tiles hanging over the image (TMA zero fill), gather mode, and the
+one-shot entry called on a second set of buffers.  Each element is checked against the fp64 oracle
+with the bar of test_gpu_adversarial, and bitwise against a repeat run."""
+import numpy as np
+import pytest
+
+import oracle
+from squeezedet_b200 import _lib
+from squeezedet_b200.utils import synth
+from gpu_util import conv2d_gpu
+from test_gpu_adversarial import adv_tol
+from test_gpu_dispatch import build, engine_tensor
+
+pytestmark = pytest.mark.gpu
+TC = _lib.MATH_TF32X3_TC
+
+
+def check_conv(x, w, stride=1, padding='SAME', seed=0):
+  k, Cin = w.shape[0], w.shape[2]
+  rng = np.random.default_rng(seed)
+  b = rng.normal(size=w.shape[3]).astype(np.float32)
+  want = oracle.conv2d(x, w, b, stride, padding, apply_relu=False, dtype=np.float64)
+  bound = oracle.conv2d(np.abs(x), np.abs(w), np.abs(b), stride, padding, apply_relu=False,
+                        dtype=np.float64)
+  got = conv2d_gpu(x, w, b, stride, padding, relu=False, math_mode=TC)
+  assert got.shape == want.shape and not np.isnan(got).any()
+  ratio = np.abs(got.astype(np.float64) - want) / np.maximum(bound, 1e-30)
+  assert ratio.max() < adv_tol(k * k * Cin), (x.shape, w.shape, float(ratio.max()))
+  again = conv2d_gpu(x, w, b, stride, padding, relu=False, math_mode=TC)
+  assert got.tobytes() == again.tobytes()
+  return got
+
+
+def make(B, H, W, Cin, Cout, k, seed):
+  rng = np.random.default_rng(seed)
+  x = rng.normal(size=(B, H, W, Cin)).astype(np.float32)
+  w = (rng.normal(size=(k, k, Cin, Cout)) / np.sqrt(k * k * Cin)).astype(np.float32)
+  return x, w
+
+
+ROW_CASES = [
+    # B, H, W, Cin, Cout: row mode (1x1), K chunks = Cin / KC (KC 32 when Cin % 32 == 0, else 16)
+    (1, 4, 5, 16, 16),       # 1 K chunk of 16, M = 20 < one 128-pixel tile
+    (2, 7, 11, 32, 40),      # 1 K chunk of 32, M = 154 (a 26-pixel tail tile); NT 64
+    (1, 9, 15, 64, 24),      # 2 K chunks of 32
+    (3, 5, 13, 48, 16),      # 3 K chunks of 16: exactly the stage count
+    (1, 16, 16, 128, 200),   # 4 K chunks of 32 (one past the stages); 4 output-channel chunks
+    (2, 3, 29, 112, 96),     # 7 K chunks of 16 (one past two rings)
+]
+
+
+@pytest.mark.parametrize('case', ROW_CASES)
+def test_row_mode_ring(case, gpu_device):
+  B, H, W, Cin, Cout = case
+  check_conv(*make(B, H, W, Cin, Cout, 1, sum(case)), seed=1)
+
+
+HALO_CASES = [
+    # B, H, W, Cin, Cout: halo mode (3x3), 9 K chunks per channel chunk
+    (1, 3, 5, 16, 16),       # 9 K chunks of 16, one tile mostly outside the image
+    (2, 8, 16, 32, 16),      # 9 K chunks of 32, exactly one tile
+    (1, 9, 17, 48, 130),     # 27 K chunks of 16, tiles over the right and bottom edges; 3 chunks
+    (1, 9, 17, 768, 72),     # 216 K chunks of 32 (the ConvDet head's K); the 72-wide tile
+    (2, 11, 35, 64, 64),     # 18 K chunks of 32, both halo buffers in use
+]
+
+
+@pytest.mark.parametrize('case', HALO_CASES)
+def test_halo_mode_ring(case, gpu_device):
+  B, H, W, Cin, Cout = case
+  x, w = make(B, H, W, Cin, Cout, 3, sum(case))
+  got = check_conv(x, w, seed=2)
+  # an image's tiles do not depend on the batch around it (a tensor map of one image)
+  if B > 1:
+    first = conv2d_gpu(x[:1], w, np.random.default_rng(2).normal(size=Cout).astype(np.float32), 1,
+                       'SAME', relu=False, math_mode=TC)
+    assert first.tobytes() == got[:1].tobytes()
+
+
+@pytest.mark.parametrize('stride', [1, 2])
+def test_gather_mode_ring(stride, gpu_device):
+  """3-channel 3x3 convs: cp.async into the swizzled tile, completing on the stage's mbarrier."""
+  x, w = make(2, 13, 37, 3, 64, 3, stride)
+  check_conv(x, w, stride=stride, seed=3)
+
+
+def test_oneshot_on_second_buffers(gpu_device):
+  """Two one-shot calls of the same shape on different inputs (and so different buffers): each
+  encodes its tensor maps for its own input."""
+  x1, w = make(1, 10, 20, 32, 32, 3, 11)
+  x2 = -2.0 * x1[:, ::-1]
+  y1 = check_conv(x1, w, seed=4)
+  y2 = check_conv(np.ascontiguousarray(x2), w, seed=4)
+  assert not np.array_equal(y1, y2)
+
+
+def test_cached_maps_follow_image_count(gpu_device):
+  """An engine plan caches its tensor maps per (input, image count): forwards of n = 3, 1, 2, 3
+  images give bitwise the rows of the first full forward, through row mode (the squeeze),
+  halo mode (the expand pair and the head)."""
+  B, H, W = 3, 19, 41
+  body = [('conv', 'conv1', 32, 3, 1, 'SAME'), ('fire', 'fire2', 32, 64, 64)]
+  _, model, _ = build(body, B, H, W, TC, gpu_device)
+  images = synth.synthetic_images(B, H, W, seed=9)
+  names = ('fire2/squeeze1x1', 'fire2', 'conv12')
+  buf = _lib.DeviceBuffer.from_numpy(np.ascontiguousarray(images, np.float32), gpu_device)
+  full = None
+  for n in (3, 1, 2, 3):
+    model.forward_device(buf.ptr, None, n)
+    _lib.check(model._lib.sqdet_stream_sync(gpu_device, None))
+    got = {nm: model.read_tensor(engine_tensor(model, nm)) for nm in names}
+    if full is None:
+      full = got
+    for nm in names:
+      assert got[nm][:n].tobytes() == full[nm][:n].tobytes(), (nm, n)
+  buf.free()
