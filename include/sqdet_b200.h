@@ -265,8 +265,9 @@ int sqdet_conv3x3_halo(const float* x_dev, const float* w_hwio_dev, const float*
 /* SqueezeDet._fire_layer (src/nets/squeezeDet.py:81-106; same in squeezeDetPlus.py) as ONE
  * call: y[..., :E1] = relu(1x1_e1(q)+b), y[..., E1:] = relu(3x3_e3(q)+b), q = relu(1x1_s(x)+b).
  * x [B,H,W,Cin], kernels HWIO, y [B,H,W,E1+E3].  With SQDET_MATH_TF32X3_TC and a shape the
- * one-kernel fire takes (Cin % 16 == 0, S in {16, 32, 48, 64}) this is ONE kernel launch and the
- * squeeze tensor never leaves the SM; other shapes run squeeze and expand as separate launches.
+ * one-kernel fire takes (Cin % 16 == 0, S == 16, E1 and E3 together at most 16 chunks of 64
+ * channels) this is ONE kernel launch and the squeeze tensor never leaves the SM; other shapes
+ * run the squeeze, the 1x1 expand and the 3x3 expand as three sqdet_conv2d launches.
  * Synchronises the stream (test / debug entry, not the hot path).                          */
 int sqdet_fire(const float* x_dev, const float* w_sq_dev, const float* b_sq_dev,
                const float* w_e1_dev, const float* b_e1_dev, const float* w_e3_dev,

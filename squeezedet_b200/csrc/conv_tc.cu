@@ -104,24 +104,10 @@ struct TcParams {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src),
-               "r"(valid ? 16 : 0)
-               : "memory");
-}
 __device__ __forceinline__ void cp_async4(uint32_t dst, const void* src, bool valid) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src),
                "r"(valid ? 4 : 0)
                : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-// cp.async writes are generic-proxy writes; wgmma reads shared memory through the async proxy
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 // makes cp.async operations this thread issued so far arrive on `bar` when they complete (the
 // barrier's count includes the arrival)
@@ -155,6 +141,35 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "@!done bra WAIT_%=;\n\t}" ::"r"(smem_u32(bar)),
       "r"(parity)
       : "memory");
+}
+
+// The operand ring: K chunk j of a kernel's sequence goes through stage j % STAGES.  A stage's
+// full barrier completes once its copies (and in gather mode every thread's cp.async arrival)
+// have landed; its empty barrier once each warp has released the stage's K chunk.
+__device__ __forceinline__ void ring_init(uint64_t* full, uint64_t* empty, int full_count) {
+  for (int s = 0; s < STAGES; ++s) {
+    mbar_init(&full[s], full_count);
+    mbar_init(&empty[s], NUM_THREADS / 32);
+  }
+  mbar_init_fence();
+}
+// Loader: waits until the warps have released K chunk j - STAGES, the last one in j's stage, and
+// returns the stage.
+__device__ __forceinline__ int ring_acquire(uint64_t* empty, int j) {
+  const int s = j % STAGES;
+  if (j >= STAGES) mbar_wait(&empty[s], (j / STAGES & 1) ^ 1);
+  return s;
+}
+// Consumer: waits for K chunk j's copies and returns its stage.
+__device__ __forceinline__ int ring_wait_full(uint64_t* full, int j) {
+  const int s = j % STAGES;
+  mbar_wait(&full[s], j / STAGES & 1);
+  return s;
+}
+// Consumer warp: releases K chunk j's stage once every lane is done with it (its MMAs retired).
+__device__ __forceinline__ void ring_release(uint64_t* empty, int j) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[j % STAGES]);
 }
 
 // `bytes` contiguous bytes from global memory into shared memory, completing on `bar`
@@ -385,13 +400,13 @@ __device__ __forceinline__ void mma_chunk(LoadA load_a, uint32_t bhi, float (&ac
   flush(acc[last], sum, ahi[last], alo[last]);
 }
 
-// Halo mode: the CTA's 8 x FT_W output tile, of image n at (oy0, ox0)
+// Halo mode and the fire kernel: the CTA's 8 x FT_W output tile, of image n at (oy0, ox0)
 struct HaloTile {
   int n, oy0, ox0;
 };
-__device__ __forceinline__ HaloTile halo_tile(const TcParams& p) {
-  const int tx = blockIdx.x % p.tiles_w, rest = blockIdx.x / p.tiles_w;
-  return {rest / p.tiles_h, rest % p.tiles_h * 8, tx * FT_W};
+__device__ __forceinline__ HaloTile halo_tile(int tiles_w, int tiles_h) {
+  const int tx = blockIdx.x % tiles_w, rest = blockIdx.x / tiles_w;
+  return {rest / tiles_h, rest % tiles_h * 8, tx * FT_W};
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -418,14 +433,8 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   const int nk = ch.nk;
   const int taps = ch.ksize * ch.ksize;   // 1 or 9
 
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      // gather mode: every thread's cp.async arrival besides the weight copy's
-      mbar_init(&full[s], MODE == TC_GATHER ? NUM_THREADS + 1 : 1);
-      mbar_init(&empty[s], NUM_THREADS / 32);
-    }
-    mbar_init_fence();
-  }
+  // gather mode: every thread's cp.async arrival besides the weight copy's
+  if (tid == 0) ring_init(full, empty, MODE == TC_GATHER ? NUM_THREADS + 1 : 1);
   __syncthreads();
 
   // ---- row and gather mode: 128 consecutive output pixels from m0
@@ -462,13 +471,9 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   // K chunk j into stage s once the warps have released the stage's previous K chunk: its
   // weights and the A values it is the first to read.  Thread 0 issues the bulk and tensor copies.
   auto load_stage = [&](int j) {
-    const int s = j % STAGES;
-    if (MODE == TC_GATHER) {
-      if (j >= STAGES) mbar_wait(&empty[s], (j / STAGES & 1) ^ 1);
-      gather_stage(j, s);
-    } else if (tid == 0 && j >= STAGES) {
-      mbar_wait(&empty[s], (j / STAGES & 1) ^ 1);
-    }
+    if (MODE != TC_GATHER && tid != 0) return;
+    const int s = ring_acquire(empty, j);
+    if (MODE == TC_GATHER) gather_stage(j, s);
     if (tid != 0) return;
     uint32_t bytes = W_BYTES;
     if (MODE == TC_ROWS) {
@@ -477,7 +482,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
       mbar_expect_tx(&full[s], bytes);
       tma_load(smem_u32(sa + s * TILE_M * KC), &p.amap, j * KC, (int)m0, &full[s]);
     } else if (MODE == TC_HALO) {
-      const HaloTile tl = halo_tile(p);
+      const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
       if (taps == 1) {
         bytes += TILE_BYTES;
         mbar_expect_tx(&full[s], bytes);
@@ -512,8 +517,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
 
   for (int kk = 0; kk < nk; ++kk) {
     if (kk + STAGES - 1 < nk) load_stage(kk + STAGES - 1);
-    const int s = kk % STAGES;
-    mbar_wait(&full[s], kk / STAGES & 1);
+    const int s = ring_wait_full(full, kk);
 
     // (in halo mode row arow0 of an 8 x FT_W tile is pixel (r, g), as a 1x1 conv loads it)
     const float* tile = sa + s * TILE_M * KC;
@@ -526,8 +530,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
     mma_chunk<NT, KC>(
         [&](int ks, uint32_t(&ahi)[4], uint32_t(&alo)[4]) { load_split_swz<KC>(tile, prow, ks, t, ahi, alo); },
         smem_u32(smem + s * WST), acc, sum);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);
+    ring_release(empty, kk);
   }
 
   // ---- epilogue: accumulator element 4j + 2h + e is (row g + 8h, column 8j + 2t + e)
@@ -535,7 +538,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   for (int h = 0; h < 2; ++h) {
     long long m = m0 + arow0 + 8 * h;   // output pixel
     if (MODE == TC_HALO) {
-      const HaloTile tl = halo_tile(p);
+      const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
       const int oy = tl.oy0 + r, ox = tl.ox0 + g + 8 * h;
       if (oy >= p.Ho || ox >= p.Wo) continue;
       m = ((long long)tl.n * p.Ho + oy) * p.Wo + ox;
@@ -559,109 +562,114 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// The fire module as ONE kernel: a CTA owns an 8 x 16 tile of output pixels of one image.
+// The fire module with a 16-channel squeeze as ONE kernel: a CTA owns an 8 x 16 tile of output
+// pixels of one image.
 //   squeeze: 1x1 conv over the 10 x 18 halo of the tile (192 rows = three m64 blocks; warpgroup 0
 //            takes blocks 0 and 2, warpgroup 1 block 1), bias + ReLU, zero outside the image (SAME
 //            padding of the 3x3 expand pads the post-ReLU squeeze output), kept in shared memory
-//            as Q[halo pixel][SQN + 4] fp32;
-//   expand:  1x1 and 3x3 convs over Q in chunks of 64 output channels; the A fragments of tap
-//            (dy, dx) are read from Q at the tap-shifted halo row, so the squeeze tensor never
-//            leaves the SM; weights stream through the mbarrier ring, one bulk copy per K chunk.
+//            as Q[halo pixel][FS + 4] fp32.  Each K chunk of KCI channels brings its halo by TMA
+//            through the halo-mode tensor map of conv_tc_kernel and its weight tile by one bulk copy;
+//   expand:  1x1 and 3x3 convs over Q in chunks of 64 output channels; K chunk kk of a 3x3 chunk
+//            is tap kk = (dy, dx), whose A fragments are read from Q at the tap-shifted halo row,
+//            so the squeeze tensor never leaves the SM; one bulk copy of weights per K chunk.
+// Squeeze and expand K chunks are one sequence through the mbarrier ring (squeeze chunk kk, then
+// expand K chunk it as nks + it), so thread 0 prefetches the expand's first weight tiles while the
+// squeeze runs; the block barrier that publishes Q is the only one after the ring is set up.
+constexpr int FS = 16;         // squeeze channels
 constexpr int FQ_ROWS = 192;   // FQ_P halo pixels padded to three m64 blocks
 constexpr int MAX_FCHUNKS = 16;
 
 struct FireChunk {
-  int taps, nk, ncount, y_off;
+  int taps, ncount, y_off;   // a chunk has `taps` K chunks of FS channels, one per tap
 };
 
 struct FireParams {
-  const float* x;
+  CUtensorMap amap;   // (C, W, H, B) over x, boxes of (KCI, 18, 10, 1)
   float* y;
-  const float* wsq;   // squeeze tiles [Cin / KCI][2][SQN][KCI]
-  const float* bsq;   // [SQN], zero past S
-  const float* wex;   // expand tiles, chunk after chunk, [nk][2][64][KCE] each
+  const float* wsq;   // squeeze tiles [Cin / KCI][2][FS][KCI]
+  const float* bsq;   // [FS]
+  const float* wex;   // expand tiles, chunk after chunk, [taps][2][64][FS] each
   const float* bex;   // [E1 + E3]
-  int B, H, W, Cin, S, Etot, tiles_w, tiles_h, nchunks;
-  int total_nk;   // K chunks of all expand chunks (read from the parameter bank, not a register)
+  int B, H, W, Cin, Etot, tiles_w, tiles_h, nchunks;
+  int total_nk;   // K chunks of all expand chunks
   FireChunk chunks[MAX_FCHUNKS];
 };
 
-template <int KCI, int SQN, int KCE>
-__host__ __device__ constexpr int fire_ring_floats() {
-  return FQ_ROWS * (KCI + 4) + 2 * SQN * KCI > 2 * 64 * KCE ? FQ_ROWS * (KCI + 4) + 2 * SQN * KCI
-                                                             : 2 * 64 * KCE;
+// fire_tc_kernel's shared memory, from a 1024-byte aligned base: STAGES x [squeeze weight tile
+// 2 FS KCI][A tile FQ_ROWS x KCI] (an expand weight tile reuses the stage's first 8 KiB), then Q
+// and the full and empty barrier of each stage.
+__host__ __device__ constexpr int fire_stage_floats(int KCI) { return 2 * FS * KCI + FQ_ROWS * KCI; }
+constexpr size_t fire_smem_bytes(int KCI) {
+  return 1024 + ((size_t)STAGES * fire_stage_floats(KCI) + FQ_ROWS * (FS + 4)) * sizeof(float) +
+         2 * STAGES * sizeof(uint64_t);
 }
 
-// A 16-channel squeeze leaves room for two CTAs per SM (110.6 KB of shared memory, at most 128
-// registers a thread); the wider squeezes need more shared memory than that anyway.
-template <int KCI, int SQN, int KCE>
-__global__ void __launch_bounds__(NUM_THREADS, SQN == 16 ? 2 : 1)
+// Two CTAs per SM: at most 128 registers a thread, and 102.4 KB of shared memory at KCI = 32.
+template <int KCI>
+__global__ void __launch_bounds__(NUM_THREADS, 2)
 fire_tc_kernel(const __grid_constant__ FireParams p) {
-  constexpr int API = KCI + 4, QP = SQN + 4;
-  constexpr int RING = fire_ring_floats<KCI, SQN, KCE>();
-  extern __shared__ __align__(128) float smem[];
-  float* q = smem + STAGES * RING;
-  uint64_t* const full = reinterpret_cast<uint64_t*>(q + FQ_ROWS * QP);   // expand weight ring
+  constexpr int QP = FS + 4;
+  constexpr int SQW = 2 * FS * KCI;   // floats of a squeeze weight tile, hi + lo
+  constexpr int STAGE = fire_stage_floats(KCI);
+  constexpr uint32_t SQW_BYTES = SQW * 4, HALO_BYTES = FQ_P * KCI * 4, EX_BYTES = 2 * 64 * FS * 4;
+  // the expand's weight tiles leave the A tiles' rows FQ_P.. zeroed below alone
+  static_assert(EX_BYTES <= (SQW + FQ_P * KCI) * 4, "expand tile fits before the zeroed rows");
+  static_assert(SQW_BYTES % 1024 == 0 && STAGE * 4 % 1024 == 0, "A tiles keep the swizzle's alignment");
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  float* const smem = reinterpret_cast<float*>(smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023));
+  float* const q = smem + STAGES * STAGE;
+  uint64_t* const full = reinterpret_cast<uint64_t*>(q + FQ_ROWS * QP);
   uint64_t* const empty = full + STAGES;
 
-  int tile = blockIdx.x;
-  const int tx = tile % p.tiles_w;
-  tile /= p.tiles_w;
-  const int ty = tile % p.tiles_h, n = tile / p.tiles_h;
-  const int oy0 = ty * 8, ox0 = tx * FT_W;
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
-  const float* xn = p.x + (size_t)n * p.H * p.W * p.Cin;
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], NUM_THREADS / 32);
-    }
-    mbar_init_fence();
+  const int nks = p.Cin / KCI, total = nks + p.total_nk;
+  if (tid == 0) ring_init(full, empty, 1);
+  // A-tile rows FQ_P.. feed only the discarded squeeze rows; the halo box never writes them
+  for (int i = tid; i < STAGES * (FQ_ROWS - FQ_P) * KCI; i += NUM_THREADS) {
+    const int s = i / ((FQ_ROWS - FQ_P) * KCI);
+    smem[s * STAGE + SQW + FQ_P * KCI + i % ((FQ_ROWS - FQ_P) * KCI)] = 0.f;
   }
+  __syncthreads();
 
-  auto load_sq = [&](int kk, int s) {
-    float* st = smem + (size_t)s * RING;
-    float* sa = st + 2 * SQN * KCI;
-    for (int v = tid; v < FQ_ROWS * KCI / 4; v += NUM_THREADS) {
-      const int row = v / (KCI / 4), j = v % (KCI / 4);
-      const int iy = oy0 - 1 + row / FQ_W, ix = ox0 - 1 + row % FQ_W;
-      const bool ok = row < FQ_P && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
-      cp_async16(smem_u32(sa + row * API + 4 * j),
-                 ok ? xn + ((size_t)iy * p.W + ix) * p.Cin + kk * KCI + 4 * j : p.x, ok);
+  // K chunk j of the sequence into its stage (thread 0): for j < nks the squeeze's halo of
+  // channels [j KCI, j KCI + KCI) and weight tile, then expand K chunk j - nks's weight tile
+  auto load_stage = [&](int j) {
+    const int s = ring_acquire(empty, j);
+    float* const st = smem + s * STAGE;
+    if (j < nks) {
+      const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
+      mbar_expect_tx(&full[s], SQW_BYTES + HALO_BYTES);
+      tma_load(smem_u32(st + SQW), &p.amap, j * KCI, tl.ox0 - 1, tl.oy0 - 1, tl.n, &full[s]);
+      bulk_load(smem_u32(st), p.wsq + (size_t)j * SQW, SQW_BYTES, &full[s]);
+    } else {
+      mbar_expect_tx(&full[s], EX_BYTES);
+      bulk_load(smem_u32(st), p.wex + (size_t)(j - nks) * 2 * 64 * FS, EX_BYTES, &full[s]);
     }
-    const float* wsrc = p.wsq + (size_t)kk * 2 * SQN * KCI;
-    for (int v = tid; v < SQN * KCI / 2; v += NUM_THREADS) cp_async16(smem_u32(st) + v * 16, wsrc + 4 * v, true);
   };
+  if (tid == 0) {
+#pragma unroll 1
+    for (int j = 0; j < STAGES - 1 && j < total; ++j) load_stage(j);
+  }
 
   // ---- squeeze
-  const int nks = p.Cin / KCI;
+  float accq[2][FS / 2], sq[2][FS / 2];
 #pragma unroll
-  for (int s = 0; s < STAGES - 1; ++s) {
-    if (s < nks) load_sq(s, s);
-    cp_async_commit();
-  }
-  float accq[2][SQN / 2], sq[2][SQN / 2];
-#pragma unroll
-  for (int i = 0; i < SQN / 2; ++i) accq[0][i] = accq[1][i] = sq[0][i] = sq[1][i] = 0.f;
+  for (int i = 0; i < FS / 2; ++i) accq[0][i] = accq[1][i] = sq[0][i] = sq[1][i] = 0.f;
   const int rb = wq * 16 + g;
   for (int kk = 0; kk < nks; ++kk) {
-    cp_async_wait<STAGES - 2>();
-    fence_proxy_async();
-    __syncthreads();
-    if (kk + STAGES - 1 < nks) load_sq(kk + STAGES - 1, (kk + STAGES - 1) % STAGES);
-    cp_async_commit();
-    const float* st = smem + (size_t)(kk % STAGES) * RING;
-    const float* sa = st + 2 * SQN * KCI;
+    if (tid == 0 && kk + STAGES - 1 < total) load_stage(kk + STAGES - 1);
+    const float* st = smem + ring_wait_full(full, kk) * STAGE;
+    const float* sa = st + SQW;
     if (wg == 0) {
       // blocks 0 and 2 interleaved, block 2 * bi in accumulator set bi: one block's step is in
       // flight while the other block's previous step is added in; drained like mma_chunk
       uint32_t qhi[2][4], qlo[2][4];
 #pragma unroll
       for (int j = 0; j < 2 * (KCI / 8); ++j) {
-        const int bi = j & 1, ks = j >> 1, r0 = 128 * bi + rb;
-        load_split(sa + r0 * API, sa + (r0 + 8) * API, ks, t, qhi[bi], qlo[bi]);
-        mma_step<SQN, KCI>(accq[bi], qhi[bi], qlo[bi], smem_u32(st), ks);
+        const int bi = j & 1, ks = j >> 1;
+        load_split_swz<KCI>(sa, 128 * bi + rb, ks, t, qhi[bi], qlo[bi]);
+        mma_step<FS, KCI>(accq[bi], qhi[bi], qlo[bi], smem_u32(st), ks);
         if (j > 0) {
           wgmma_wait<1>();
           flush(accq[bi ^ 1], sq[bi ^ 1], qhi[bi ^ 1], qlo[bi ^ 1]);
@@ -670,88 +678,70 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
       wgmma_wait<0>();
       flush(accq[1], sq[1], qhi[1], qlo[1]);
     } else {
-      const int r0 = 64 + rb;
-      mma_chunk<SQN, KCI>(
+      mma_chunk<FS, KCI>(
           [&](int ks, uint32_t(&ahi)[4], uint32_t(&alo)[4]) {
-            load_split(sa + r0 * API, sa + (r0 + 8) * API, ks, t, ahi, alo);
+            load_split_swz<KCI>(sa, 64 + rb, ks, t, ahi, alo);
           },
           smem_u32(st), accq, sq[0]);
     }
+    ring_release(empty, kk);
   }
-  cp_async_wait<0>();
+  {
+    const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
 #pragma unroll
-  for (int bi = 0; bi < 2; ++bi) {
-    const int b = wg + 2 * bi;
-    if (b >= 3) continue;
+    for (int bi = 0; bi < 2; ++bi) {
+      const int b = wg + 2 * bi;
+      if (b >= 3) continue;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = b * 64 + wq * 16 + g + 8 * h;
-      const int iy = oy0 - 1 + row / FQ_W, ix = ox0 - 1 + row % FQ_W;
-      const bool ok = row < FQ_P && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
+      for (int h = 0; h < 2; ++h) {
+        const int row = b * 64 + wq * 16 + g + 8 * h;
+        const int iy = tl.oy0 - 1 + row / FQ_W, ix = tl.ox0 - 1 + row % FQ_W;
+        const bool ok = row < FQ_P && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
 #pragma unroll
-      for (int j = 0; j < SQN / 8; ++j)
+        for (int j = 0; j < FS / 8; ++j)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int c = 8 * j + 2 * t + e;
-          q[row * QP + c] = ok ? fmaxf(sq[bi][4 * j + 2 * h + e] + p.bsq[c], 0.f) : 0.f;
-        }
+          for (int e = 0; e < 2; ++e) {
+            const int c = 8 * j + 2 * t + e;
+            q[row * QP + c] = ok ? fmaxf(sq[bi][4 * j + 2 * h + e] + p.bsq[c], 0.f) : 0.f;
+          }
+      }
     }
   }
-  __syncthreads();   // Q complete; every squeeze MMA has retired, so the ring is free
+  __syncthreads();   // Q complete
 
-  // ---- expand: pixel rows g / g + 8 of this warp are tile row (4 wg + wq), columns g / g + 8.
-  // Its weight tiles stream through the ring, K chunk `it` into stage it % STAGES once the warps
-  // have released the stage's previous K chunk; thread 0 waits for that and issues the copy.
-  const int spt = p.S / KCE;   // K chunks per tap
-  const int total = p.total_nk;
-  constexpr uint32_t EX_BYTES = 2 * 64 * KCE * 4;
-  auto load_ex = [&](int it) {
-    const int s = it % STAGES;
-    if (it >= STAGES) mbar_wait(&empty[s], (it / STAGES & 1) ^ 1);
-    mbar_expect_tx(&full[s], EX_BYTES);
-    bulk_load(smem_u32(smem + (size_t)s * RING), p.wex + (size_t)it * 2 * 64 * KCE, EX_BYTES, &full[s]);
-  };
-  if (tid == 0) {
-    // the squeeze's cp.async writes to the ring were fenced before the barrier above
-#pragma unroll 1
-    for (int it = 0; it < STAGES - 1 && it < total; ++it) load_ex(it);
-  }
+  // ---- expand: pixel rows g / g + 8 of this warp are tile row (4 wg + wq), columns g / g + 8
   const int r = wg * 4 + wq;
   float acc[2][32], sum[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i] = sum[i] = 0.f;
   int c = 0, kk = 0;
-  for (int it = 0; it < total; ++it) {
-    if (tid == 0 && it + STAGES - 1 < total) load_ex(it + STAGES - 1);
-    const int s = it % STAGES;
-    mbar_wait(&full[s], it / STAGES & 1);
+  for (int j = nks; j < total; ++j) {
+    if (tid == 0 && j + STAGES - 1 < total) load_stage(j + STAGES - 1);
+    const int s = ring_wait_full(full, j);
     const FireChunk& ch = p.chunks[c];
-    const int tap = kk / spt, k0 = (kk - tap * spt) * KCE;
-    const int dy = ch.taps == 1 ? 1 : tap / 3, dx = ch.taps == 1 ? 1 : tap % 3;
+    const int dy = ch.taps == 1 ? 1 : kk / 3, dx = ch.taps == 1 ? 1 : kk % 3;
     const int qr = (r + dy) * FQ_W + g + dx;
-    mma_chunk<64, KCE>(
+    mma_chunk<64, FS>(
         [&](int ks, uint32_t(&ahi)[4], uint32_t(&alo)[4]) {
-          load_split(q + qr * QP + k0, q + (qr + 8) * QP + k0, ks, t, ahi, alo);
+          load_split(q + qr * QP, q + (qr + 8) * QP, ks, t, ahi, alo);
         },
-        smem_u32(smem + (size_t)s * RING), acc, sum);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);
-    if (++kk == ch.nk) {
-      // (the tile re-derived from blockIdx rather than kept in registers across the K loop)
-      const int tl = blockIdx.x / p.tiles_w;
-      const int oy = tl % p.tiles_h * 8 + r;
-      const size_t prow = ((size_t)(tl / p.tiles_h) * p.H + oy) * p.W;
+        smem_u32(smem + s * STAGE), acc, sum);
+    ring_release(empty, j);
+    if (++kk == ch.taps) {
+      const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
+      const int oy = tl.oy0 + r;
+      const size_t prow = ((size_t)tl.n * p.H + oy) * p.W;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int ox = ox0 + g + 8 * h;
+        const int ox = tl.ox0 + g + 8 * h;
         if (oy >= p.H || ox >= p.W) continue;
         float* yrow = p.y + (prow + ox) * p.Etot + ch.y_off;
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
+        for (int jn = 0; jn < 8; ++jn)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int col = 8 * j + 2 * t + e;
-            if (col < ch.ncount) yrow[col] = fmaxf(sum[4 * j + 2 * h + e] + p.bex[ch.y_off + col], 0.f);
+            const int col = 8 * jn + 2 * t + e;
+            if (col < ch.ncount) yrow[col] = fmaxf(sum[4 * jn + 2 * h + e] + p.bex[ch.y_off + col], 0.f);
           }
       }
 #pragma unroll
@@ -781,26 +771,6 @@ ConvKernel conv_tc_instance(int NT, int KC, int mode) {
   if (mode == TC_HALO)
     return KC == 32 ? conv_tc_instance<32, TC_HALO>(NT) : conv_tc_instance<16, TC_HALO>(NT);
   return KC == 32 ? conv_tc_instance<32, TC_ROWS>(NT) : conv_tc_instance<16, TC_ROWS>(NT);
-}
-
-template <int KCI, int SQN, int KCE>
-FireKernel fire_tc_instance(size_t* smem) {
-  *smem = sizeof(float) * ((size_t)STAGES * fire_ring_floats<KCI, SQN, KCE>() + FQ_ROWS * (SQN + 4)) +
-          2 * STAGES * sizeof(uint64_t);
-  return fire_tc_kernel<KCI, SQN, KCE>;
-}
-
-// The fire_tc_kernel instantiation for (KCI, SQN, KCE) and its dynamic shared memory in bytes.
-// S = 16, 32, 48, 64 -> SQN 16, 32, 64, 64 and KCE the largest of 32 / 16 dividing S.
-FireKernel fire_tc_instance(int KCI, int SQN, int KCE, size_t* smem) {
-  if (KCI == 32) {
-    if (SQN == 16) return fire_tc_instance<32, 16, 16>(smem);
-    if (SQN == 32) return fire_tc_instance<32, 32, 32>(smem);
-    return KCE == 16 ? fire_tc_instance<32, 64, 16>(smem) : fire_tc_instance<32, 64, 32>(smem);
-  }
-  if (SQN == 16) return fire_tc_instance<16, 16, 16>(smem);
-  if (SQN == 32) return fire_tc_instance<16, 32, 32>(smem);
-  return KCE == 16 ? fire_tc_instance<16, 64, 16>(smem) : fire_tc_instance<16, 64, 32>(smem);
 }
 
 struct TcImpl {
@@ -883,22 +853,27 @@ static int encode_map(CUtensorMap* map, const float* x, int rank, const cuuint64
   return SQDET_OK;
 }
 
+// A (C, W, H, n) map over n NHWC images of H x W x C at x, with (KC, box_w, box_h, 1) boxes.
+static int encode_nhwc_map(CUtensorMap* map, const float* x, int n, int H, int W, int C, int KC,
+                           int box_w, int box_h) {
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n};
+  const cuuint32_t box[4] = {(cuuint32_t)KC, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  return encode_map(map, x, 4, dims, box, KC);
+}
+
 // Encodes the plan's tensor maps for input x of n images, unless they already are.
 static int update_maps(TcImpl* im, const float* x, int n) {
   if (im->mode == TC_GATHER || (im->map_x == x && im->map_n == n)) return SQDET_OK;
   TcParams& p = im->prm;
-  const cuuint32_t KC = im->KC;
   im->map_x = nullptr;
   int rc;
   if (im->mode == TC_ROWS) {
     const cuuint64_t dims[2] = {(cuuint64_t)p.Cin, (cuuint64_t)n * p.H * p.W};
-    const cuuint32_t box[2] = {KC, TILE_M};
+    const cuuint32_t box[2] = {(cuuint32_t)im->KC, TILE_M};
     rc = encode_map(&p.amap, x, 2, dims, box, im->KC);
   } else {
-    const cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)n};
-    const cuuint32_t halo[4] = {KC, FQ_W, 10, 1}, tile[4] = {KC, FT_W, 8, 1};
-    rc = encode_map(&p.amap, x, 4, dims, halo, im->KC);
-    if (!rc) rc = encode_map(&p.amap1, x, 4, dims, tile, im->KC);
+    rc = encode_nhwc_map(&p.amap, x, n, p.H, p.W, p.Cin, im->KC, FQ_W, 10);
+    if (!rc) rc = encode_nhwc_map(&p.amap1, x, n, p.H, p.W, p.Cin, im->KC, FT_W, 8);
   }
   if (rc) return rc;
   im->map_x = x;
@@ -1022,7 +997,7 @@ static void pack_group(const TcImpl* im, int gi, const float* w_hwio, std::vecto
 // ---- one-kernel fire module: host state -----------------------------
 struct FusedImpl {
   FireParams fp{};
-  int KCI = 0, SQN = 0, KCE = 0;
+  int KCI = 0;
   int E1 = 0, E3 = 0;
   FireKernel kernel = nullptr;
   size_t smem = 0;
@@ -1031,6 +1006,9 @@ struct FusedImpl {
   float* d_b = nullptr;
   float* d_b2 = nullptr;
   long long w_floats = 0, w2_floats = 0;
+  // the input and image count fp.amap was encoded for (null: none yet)
+  const float* map_x = nullptr;
+  int map_n = 0;
 };
 
 static void release_fused(void** impl) {
@@ -1159,17 +1137,15 @@ int conv2d_tc_oneshot(const float* x_dev, const float* w_hwio_dev, const float* 
 // ---- one-kernel fire module ----------------------------------------------------------------------
 int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int S, int E1, int E3) {
   plan->impl = nullptr;
-  if (Cin % 16 || Cin < 16 || S % 16 || S < 16 || S > 64 || E1 <= 0 || E3 <= 0) return 0;
+  if (Cin % 16 || Cin < 16 || S != FS || E1 <= 0 || E3 <= 0) return 0;
   const int nch = (E1 + 63) / 64 + (E3 + 63) / 64;
   if (nch > MAX_FCHUNKS) return 0;
   FusedImpl* im = new FusedImpl();
   im->KCI = Cin % 32 == 0 ? 32 : 16;
-  im->SQN = S <= 16 ? 16 : S <= 32 ? 32 : 64;
-  im->KCE = S % 32 == 0 ? 32 : 16;
   im->E1 = E1;
   im->E3 = E3;
   FireParams& p = im->fp;
-  p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.S = S; p.Etot = E1 + E3;
+  p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Etot = E1 + E3;
   p.tiles_w = (W + FT_W - 1) / FT_W;
   p.tiles_h = (H + 7) / 8;
   p.nchunks = nch;
@@ -1177,13 +1153,14 @@ int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int 
   for (int gi = 0; gi < 2; ++gi) {
     const int E = gi ? E3 : E1, taps = gi ? 9 : 1;
     for (int cb = 0; cb < E; cb += 64, ++c) {
-      p.chunks[c] = FireChunk{taps, taps * (S / im->KCE), E - cb < 64 ? E - cb : 64, (gi ? E1 : 0) + cb};
-      im->w2_floats += (long long)p.chunks[c].nk * 2 * 64 * im->KCE;
-      p.total_nk += p.chunks[c].nk;
+      p.chunks[c] = FireChunk{taps, E - cb < 64 ? E - cb : 64, (gi ? E1 : 0) + cb};
+      p.total_nk += taps;
     }
   }
-  im->w_floats = (long long)(Cin / im->KCI) * 2 * im->SQN * im->KCI;
-  im->kernel = fire_tc_instance(im->KCI, im->SQN, im->KCE, &im->smem);
+  im->w_floats = (long long)(Cin / im->KCI) * 2 * FS * im->KCI;
+  im->w2_floats = (long long)p.total_nk * 2 * 64 * FS;
+  im->kernel = im->KCI == 32 ? fire_tc_kernel<32> : fire_tc_kernel<16>;
+  im->smem = fire_smem_bytes(im->KCI);
   void* vp = im;
   cudaError_t ce = cudaFuncSetAttribute(im->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)im->smem);
@@ -1193,7 +1170,7 @@ int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int 
   }
   if ((ce = cudaMalloc(&im->d_w, sizeof(float) * im->w_floats)) != cudaSuccess ||
       (ce = cudaMalloc(&im->d_w2, sizeof(float) * im->w2_floats)) != cudaSuccess ||
-      (ce = cudaMalloc(&im->d_b, sizeof(float) * im->SQN)) != cudaSuccess ||
+      (ce = cudaMalloc(&im->d_b, sizeof(float) * FS)) != cudaSuccess ||
       (ce = cudaMalloc(&im->d_b2, sizeof(float) * (E1 + E3))) != cudaSuccess) {
     release_fused(&vp);
     return cuda_fail(ce, "cudaMalloc(fused fire)");
@@ -1208,33 +1185,38 @@ int tc_fused_fire_pack_weights(TcFusedFirePlan* plan, const float* w_sq, const f
                                const float* b_e3) {
   FusedImpl* im = static_cast<FusedImpl*>(plan->impl);
   const FireParams& p = im->fp;
-  std::vector<float> wsq((size_t)im->w_floats), wex((size_t)im->w2_floats);
-  std::vector<float> bsq(im->SQN, 0.f), bex;
-  pack_tiles(w_sq, p.Cin, p.S, 0, im->SQN, im->KCI, p.Cin / im->KCI, 1, p.Cin, wsq.data());
+  std::vector<float> wsq((size_t)im->w_floats), wex((size_t)im->w2_floats), bex;
+  pack_tiles(w_sq, p.Cin, FS, 0, FS, im->KCI, p.Cin / im->KCI, 1, p.Cin, wsq.data());
   long long off = 0;
   for (int c = 0; c < p.nchunks; ++c) {
     const FireChunk& ch = p.chunks[c];
     const bool e3 = ch.taps == 9;
-    pack_tiles(e3 ? w_e3 : w_e1, (long long)ch.taps * p.S, e3 ? im->E3 : im->E1,
-               ch.y_off - (e3 ? im->E1 : 0), 64, im->KCE, ch.nk, 1, p.S, wex.data() + off);
-    off += (long long)ch.nk * 2 * 64 * im->KCE;
+    pack_tiles(e3 ? w_e3 : w_e1, (long long)ch.taps * FS, e3 ? im->E3 : im->E1,
+               ch.y_off - (e3 ? im->E1 : 0), 64, FS, ch.taps, 1, FS, wex.data() + off);
+    off += (long long)ch.taps * 2 * 64 * FS;
   }
-  for (int i = 0; i < p.S; ++i) bsq[i] = b_sq[i];
   bex.assign(b_e1, b_e1 + im->E1);
   bex.insert(bex.end(), b_e3, b_e3 + im->E3);
   SQ_CUDA(cudaMemcpy(im->d_w, wsq.data(), wsq.size() * sizeof(float), cudaMemcpyHostToDevice));
   SQ_CUDA(cudaMemcpy(im->d_w2, wex.data(), wex.size() * sizeof(float), cudaMemcpyHostToDevice));
-  SQ_CUDA(cudaMemcpy(im->d_b, bsq.data(), bsq.size() * sizeof(float), cudaMemcpyHostToDevice));
+  SQ_CUDA(cudaMemcpy(im->d_b, b_sq, FS * sizeof(float), cudaMemcpyHostToDevice));
   SQ_CUDA(cudaMemcpy(im->d_b2, bex.data(), bex.size() * sizeof(float), cudaMemcpyHostToDevice));
   return SQDET_OK;
 }
 
 int launch_fused_fire_tc(const TcFusedFirePlan& plan, const float* x_dev, float* y_dev, int n,
                          cudaStream_t stream) {
-  const FusedImpl* im = static_cast<const FusedImpl*>(plan.impl);
-  FireParams p = im->fp;
-  if (n < 1 || n > p.B) return fail(SQDET_ERR_INVALID_ARG, "launch_fused_fire_tc: image count outside [1, B]");
-  p.x = x_dev;
+  FusedImpl* im = static_cast<FusedImpl*>(plan.impl);
+  FireParams& fp = im->fp;
+  if (n < 1 || n > fp.B) return fail(SQDET_ERR_INVALID_ARG, "launch_fused_fire_tc: image count outside [1, B]");
+  if (im->map_x != x_dev || im->map_n != n) {
+    im->map_x = nullptr;
+    const int rc = encode_nhwc_map(&fp.amap, x_dev, n, fp.H, fp.W, fp.Cin, im->KCI, FQ_W, 10);
+    if (rc) return rc;
+    im->map_x = x_dev;
+    im->map_n = n;
+  }
+  FireParams p = fp;
   p.y = y_dev;
   p.B = n;
   const unsigned grid = (unsigned)((long long)n * p.tiles_h * p.tiles_w);

@@ -37,7 +37,8 @@ int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, int
 void tc_conv_release(TcConvPlan* plan);
 
 // The whole fire module (squeeze 1x1 -> expand 1x1 || 3x3 + concat) as ONE kernel: the squeeze
-// tile of each 8 x 16 output tile stays in shared memory.  Cin % 16 == 0, S in {16, 32, 48, 64}.
+// tile of each 8 x 16 output tile stays in shared memory.  Cin % 16 == 0, S == 16, at most 16
+// expand chunks of 64 channels.  The plan caches the tensor map of its last (input, image count).
 struct TcFusedFirePlan {
   void* impl = nullptr;
 };

@@ -57,12 +57,13 @@ def test_fire_vs_oracle(shape, math_mode, gpu_device):
   assert r < 1.0, r
 
 
-# Shapes the shipped nets never produce, chosen to reach every fire_tc_kernel<KCI, SQN, KCE>
-# instantiation and the planner's edges (conv_tc.cu, tc_fused_fire_plan):
-#   KCI = 16 (Cin % 32 == 16) at every squeeze width: <16,16,16> <16,32,32> <16,64,16> <16,64,32>
+# Shapes the shipped nets never produce, chosen to reach both fire_tc_kernel<KCI> instantiations
+# (KCI = 16 for Cin % 32 == 16, else 32) and the planner's edges (conv_tc.cu, tc_fused_fire_plan):
+#   S = 16 (one kernel) and S = 32, 48, 64 (squeeze and expands as three sqdet_conv2d launches),
 #   E1 != E3, expand widths that are not multiples of 64 or of 8,
 #   16 expand chunks of 64 (the one-kernel limit) and 17 (sqdet_fire falls back to separate
 #   launches).
+TINY_IMAGES = ((1, 1), (1, 17), (9, 1), (8, 16), (9, 17))
 FIRE_EDGE_CASES = [
     # (Cin, S, E1, E3), (B, H, W)
     *[((cin, s, 64, 64), (2, 11, 21)) for cin in (16, 48, 80, 112) for s in (16, 32, 48, 64)],
@@ -73,8 +74,9 @@ FIRE_EDGE_CASES = [
     ((64, 16, 512, 512), (1, 9, 18)),
     ((64, 16, 576, 512), (1, 9, 18)),
     # tiny images: 1x1, one row, one column, one exact 8x16 tile, one pixel past it on both axes
-    *[((48, 32, 40, 88), (3, h, w)) for h, w in ((1, 1), (1, 17), (9, 1), (8, 16), (9, 17))],
+    *[((48, 32, 40, 88), (3, h, w)) for h, w in TINY_IMAGES],
     *[((64, 48, 64, 64), (3, h, w)) for h, w in ((1, 1), (8, 16), (9, 17))],
+    *[((cin, 16, 40, 88), (3, h, w)) for cin in (48, 64) for h, w in TINY_IMAGES],
 ]
 
 

@@ -4,8 +4,9 @@ barrier.  K chunk counts below, at and just above the three stages, a 216-chunk 
 head's, over which each barrier's phase wraps 72 times), several output-channel chunks in one
 launch, both K chunk widths (so both the 128-byte and the 64-byte swizzle), a row-mode pixel count
 that is not a multiple of 128, tiles hanging over the image (TMA zero fill), gather mode, and the
-one-shot entry called on a second set of buffers.  Each element is checked against the fp64 oracle
-with the bar of test_gpu_adversarial, and bitwise against a repeat run."""
+one-shot entry called on a second set of buffers; engines whose forwards change the image count
+and the input buffer, through the convolution and the one-kernel fire.  Each element is checked
+against the fp64 oracle with the bar of test_gpu_adversarial, and bitwise against a repeat run."""
 import numpy as np
 import pytest
 
@@ -14,7 +15,8 @@ from squeezedet_b200 import _lib
 from squeezedet_b200.utils import synth
 from gpu_util import conv2d_gpu
 from test_gpu_adversarial import adv_tol
-from test_gpu_dispatch import build, engine_tensor
+from test_gpu_dispatch import (ONE_KERNEL_MIN_TILES, POST_LAUNCHES, build, engine_tensor,
+                               fire_tiles)
 
 pytestmark = pytest.mark.gpu
 TC = _lib.MATH_TF32X3_TC
@@ -99,6 +101,25 @@ def test_oneshot_on_second_buffers(gpu_device):
   assert not np.array_equal(y1, y2)
 
 
+def assert_rows_follow_full_forward(model, B, H, W, names, runs, device):
+  """For each (i, n) of `runs`, the first a full forward, runs a forward of n images from input
+  buffer i (all buffers hold the same images) and checks that the tensors `names` hold bitwise the
+  first forward's rows."""
+  images = np.ascontiguousarray(synth.synthetic_images(B, H, W, seed=9), np.float32)
+  bufs = [_lib.DeviceBuffer.from_numpy(images, device) for _ in range(1 + max(i for i, _ in runs))]
+  full = None
+  for i, n in runs:
+    model.forward_device(bufs[i].ptr, None, n)
+    _lib.check(model._lib.sqdet_stream_sync(device, None))
+    got = {nm: model.read_tensor(engine_tensor(model, nm)) for nm in names}
+    if full is None:
+      full = got
+    for nm in names:
+      assert got[nm][:n].tobytes() == full[nm][:n].tobytes(), (nm, i, n)
+  for buf in bufs:
+    buf.free()
+
+
 def test_cached_maps_follow_image_count(gpu_device):
   """An engine plan caches its tensor maps per (input, image count): forwards of n = 3, 1, 2, 3
   images give bitwise the rows of the first full forward, through row mode (the squeeze),
@@ -106,16 +127,20 @@ def test_cached_maps_follow_image_count(gpu_device):
   B, H, W = 3, 19, 41
   body = [('conv', 'conv1', 32, 3, 1, 'SAME'), ('fire', 'fire2', 32, 64, 64)]
   _, model, _ = build(body, B, H, W, TC, gpu_device)
-  images = synth.synthetic_images(B, H, W, seed=9)
-  names = ('fire2/squeeze1x1', 'fire2', 'conv12')
-  buf = _lib.DeviceBuffer.from_numpy(np.ascontiguousarray(images, np.float32), gpu_device)
-  full = None
-  for n in (3, 1, 2, 3):
-    model.forward_device(buf.ptr, None, n)
-    _lib.check(model._lib.sqdet_stream_sync(gpu_device, None))
-    got = {nm: model.read_tensor(engine_tensor(model, nm)) for nm in names}
-    if full is None:
-      full = got
-    for nm in names:
-      assert got[nm][:n].tobytes() == full[nm][:n].tobytes(), (nm, n)
-  buf.free()
+  assert_rows_follow_full_forward(model, B, H, W, ('fire2/squeeze1x1', 'fire2', 'conv12'),
+                                  [(0, 3), (0, 1), (0, 2), (0, 3)], gpu_device)
+
+
+def test_cached_fire_map_follows_image_count(gpu_device):
+  """The same through the one-kernel fire, whose plan caches the halo map of its squeeze: a
+  16-channel squeeze on 3 x 64 x 352 (528 tiles, 4 per SM on 132 SMs).  Forwards of n = 3, 1, 2,
+  3 images, then from a second input buffer, give bitwise the rows of the first full forward.
+  (The fire reads conv1's output, so the second buffer is the input of conv1 only.)"""
+  B, H, W = 3, 64, 352
+  assert fire_tiles(B, H, W) >= ONE_KERNEL_MIN_TILES
+  body = [('conv', 'conv1', 32, 3, 1, 'SAME'), ('fire', 'fire2', 16, 64, 64)]
+  _, model, _ = build(body, B, H, W, TC, gpu_device)
+  assert model.launches_per_forward() == 3 + POST_LAUNCHES     # conv1, fire2 as one kernel, head
+  assert_rows_follow_full_forward(model, B, H, W, ('conv1', 'fire2', 'conv12'),
+                                  [(0, 3), (0, 1), (0, 2), (0, 3), (1, 3), (1, 2), (0, 1)],
+                                  gpu_device)

@@ -104,22 +104,21 @@ def tc_conv_variant(Cin, Cout, k, stride, padding):
 
 
 def tc_fire_variant(Cin, S, E1, E3):
-  """fire_tc_kernel<KCI, SQN, KCE> that sqdet_fire runs with MATH_TF32X3_TC, or None when
-  tc_fused_fire_plan (conv_tc.cu) declines and the fire runs as separate convs."""
-  if Cin % 16 or Cin < 16 or S % 16 or not 16 <= S <= 64:
+  """KCI of the fire_tc_kernel<KCI> that sqdet_fire runs with MATH_TF32X3_TC, or None when
+  tc_fused_fire_plan (conv_tc.cu) declines and the fire runs as separate convs: it takes a
+  16-channel squeeze over Cin % 16 == 0 channels with at most MAX_FCHUNKS expand chunks of 64."""
+  if Cin % 16 or Cin < 16 or S != 16:
     return None
   if -(-E1 // 64) + -(-E3 // 64) > MAX_FCHUNKS:
     return None
-  return (32 if Cin % 32 == 0 else 16, 16 if S <= 16 else 32 if S <= 32 else 64,
-          32 if S % 32 == 0 else 16)
+  return 32 if Cin % 32 == 0 else 16
 
 
 ALL_CONV_TC_VARIANTS = {(nt, kc, g) for nt in (64, 32, 16) for kc, g in ((32, True), (32, False),
                                                                         (16, False))}
 ALL_CONV_TC_VARIANTS.add((72, 32, False))          # conv_tc_instance: the head tile
-# fire_tc_instance (conv_tc.cu)
-ALL_FIRE_TC_VARIANTS = {(32, 16, 16), (32, 32, 32), (32, 64, 16), (32, 64, 32),
-                        (16, 16, 16), (16, 32, 32), (16, 64, 16), (16, 64, 32)}
+# the fire_tc_kernel<KCI> instantiations (tc_fused_fire_plan, conv_tc.cu)
+ALL_FIRE_TC_VARIANTS = {32, 16}
 
 
 def test_gpu_case_tables_reach_every_tc_kernel_variant():
