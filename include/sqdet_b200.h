@@ -293,7 +293,9 @@ int sqdet_interpret(const float* preds_dev, const float* anchors_f32_dev,
                     int image_width, int image_height, float exp_thresh, void* stream);
 /* ModelSkeleton.filter_prediction + util.nms (src/nn_skeleton.py:696-734,
  * src/utils/util.py:32-76) for B images at once: boxes [B,A,4], probs [B,A],
- * cls [B,A] -> dets [B,max_dets], counts [B] (count<0: SQDET_ERR_OVERFLOW case).      */
+ * cls [B,A] -> dets [B,max_dets], counts [B] (count<0: SQDET_ERR_OVERFLOW case).
+ * Rank order for the top-N cut and NMS: probability descending, -0.0 == +0.0, NaN last,
+ * ties by ascending anchor.                                                            */
 int sqdet_topk_nms(const float* boxes_dev, const float* probs_dev,
                    const int64_t* cls_dev, int B, int A, int classes, int top_n,
                    float prob_thresh, float nms_thresh, sqdet_det* dets_dev,
