@@ -251,17 +251,6 @@ int sqdet_conv2d(const float* x_dev, const float* w_hwio_dev, const float* bias_
                  int B, int H, int W, int Cin, int Cout, int size, int stride,
                  int padding, int relu, int y_cstride, int y_coff, int math_mode,
                  void* stream);
-/* A 3x3, stride-1, SAME convolution (the ConvDet head's shape, src/nets/squeezeDet.py:73-78) as a
- * stage-isolated call: same arguments as sqdet_conv2d without size/stride/padding/math_mode.  It
- * runs the wgmma implicit-GEMM kernel of sqdet_conv2d with SQDET_MATH_TF32X3_TC, which takes
- * every such conv in halo mode: a CTA computes an 8 x 16 output tile of one image from the
- * 10 x 18 halo of each input-channel chunk, loaded once, and reads the nine taps as row offsets
- * into it.  Returns SQDET_ERR_UNSUPPORTED for shapes that kernel does not take (Cin % 16 != 0).
- * Synchronises the stream (test / debug entry).                                            */
-int sqdet_conv3x3_halo(const float* x_dev, const float* w_hwio_dev, const float* bias_dev,
-                       const float* scale_dev, const float* shift_dev, float* y_dev, int B,
-                       int H, int W, int Cin, int Cout, int relu, int y_cstride, int y_coff,
-                       void* stream);
 /* SqueezeDet._fire_layer (src/nets/squeezeDet.py:81-106; same in squeezeDetPlus.py) as ONE
  * call: y[..., :E1] = relu(1x1_e1(q)+b), y[..., E1:] = relu(3x3_e3(q)+b), q = relu(1x1_s(x)+b).
  * x [B,H,W,Cin], kernels HWIO, y [B,H,W,E1+E3].  With SQDET_MATH_TF32X3_TC and a shape the

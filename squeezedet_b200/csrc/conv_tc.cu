@@ -69,8 +69,8 @@ constexpr int MAX_CHUNKS = 32;
 // through a (8 + 2) x FQ_W halo of FQ_P pixels
 constexpr int FT_W = 16, FQ_W = FT_W + 2, FQ_P = 10 * FQ_W;
 
-// conv_tc_kernel's operand tiling: see the file comment
-enum TcMode { TC_ROWS, TC_GATHER, TC_HALO };
+// conv_tc_kernel's operand tiling (see the file comment), or a plan of fire_tc_kernel
+enum TcMode { TC_ROWS, TC_GATHER, TC_HALO, TC_FIRE };
 
 struct TcChunk {
   int ksize, pad_t, pad_l;  // this conv's filter size and top / left zero padding (gather mode)
@@ -575,25 +575,13 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
 // Squeeze and expand K chunks are one sequence through the mbarrier ring (squeeze chunk kk, then
 // expand K chunk it as nks + it), so thread 0 prefetches the expand's first weight tiles while the
 // squeeze runs; the block barrier that publishes Q is the only one after the ring is set up.
+//
+// The kernel reads the TcParams of a fire plan (tc_fire_plan): chunk 0 is the squeeze (Cin / KCI
+// K chunks, FS output channels), chunks 1.. the 64-wide expand chunks, each with one K chunk of
+// FS channels per tap; w holds the squeeze tiles [Cin / KCI][2][FS][KCI], then the expand tiles
+// [taps][2][64][FS] chunk after chunk; bias is [b_sq | b_e1 | b_e3]; amap is the halo-mode map.
 constexpr int FS = 16;         // squeeze channels
 constexpr int FQ_ROWS = 192;   // FQ_P halo pixels padded to three m64 blocks
-constexpr int MAX_FCHUNKS = 16;
-
-struct FireChunk {
-  int taps, ncount, y_off;   // a chunk has `taps` K chunks of FS channels, one per tap
-};
-
-struct FireParams {
-  CUtensorMap amap;   // (C, W, H, B) over x, boxes of (KCI, 18, 10, 1)
-  float* y;
-  const float* wsq;   // squeeze tiles [Cin / KCI][2][FS][KCI]
-  const float* bsq;   // [FS]
-  const float* wex;   // expand tiles, chunk after chunk, [taps][2][64][FS] each
-  const float* bex;   // [E1 + E3]
-  int B, H, W, Cin, Etot, tiles_w, tiles_h, nchunks;
-  int total_nk;   // K chunks of all expand chunks
-  FireChunk chunks[MAX_FCHUNKS];
-};
 
 // fire_tc_kernel's shared memory, from a 1024-byte aligned base: STAGES x [squeeze weight tile
 // 2 FS KCI][A tile FQ_ROWS x KCI] (an expand weight tile reuses the stage's first 8 KiB), then Q
@@ -607,7 +595,7 @@ constexpr size_t fire_smem_bytes(int KCI) {
 // Two CTAs per SM: at most 128 registers a thread, and 102.4 KB of shared memory at KCI = 32.
 template <int KCI>
 __global__ void __launch_bounds__(NUM_THREADS, 2)
-fire_tc_kernel(const __grid_constant__ FireParams p) {
+fire_tc_kernel(const __grid_constant__ TcParams p) {
   constexpr int QP = FS + 4;
   constexpr int SQW = 2 * FS * KCI;   // floats of a squeeze weight tile, hi + lo
   constexpr int STAGE = fire_stage_floats(KCI);
@@ -623,7 +611,10 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
 
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
-  const int nks = p.Cin / KCI, total = nks + p.total_nk;
+  const int nks = p.Cin / KCI;
+  int total = 0;   // K chunks of the squeeze and every expand chunk
+#pragma unroll 1
+  for (int c = 0; c < p.nchunks; ++c) total += p.chunks[c].nk;
   if (tid == 0) ring_init(full, empty, 1);
   // A-tile rows FQ_P.. feed only the discarded squeeze rows; the halo box never writes them
   for (int i = tid; i < STAGES * (FQ_ROWS - FQ_P) * KCI; i += NUM_THREADS) {
@@ -641,10 +632,11 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
       const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
       mbar_expect_tx(&full[s], SQW_BYTES + HALO_BYTES);
       tma_load(smem_u32(st + SQW), &p.amap, j * KCI, tl.ox0 - 1, tl.oy0 - 1, tl.n, &full[s]);
-      bulk_load(smem_u32(st), p.wsq + (size_t)j * SQW, SQW_BYTES, &full[s]);
+      bulk_load(smem_u32(st), p.w + (size_t)j * SQW, SQW_BYTES, &full[s]);
     } else {
       mbar_expect_tx(&full[s], EX_BYTES);
-      bulk_load(smem_u32(st), p.wex + (size_t)(j - nks) * 2 * 64 * FS, EX_BYTES, &full[s]);
+      bulk_load(smem_u32(st), p.w + (size_t)nks * SQW + (size_t)(j - nks) * 2 * 64 * FS, EX_BYTES,
+                &full[s]);
     }
   };
   if (tid == 0) {
@@ -702,7 +694,7 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int c = 8 * j + 2 * t + e;
-            q[row * QP + c] = ok ? fmaxf(sq[bi][4 * j + 2 * h + e] + p.bsq[c], 0.f) : 0.f;
+            q[row * QP + c] = ok ? fmaxf(sq[bi][4 * j + 2 * h + e] + p.bias[c], 0.f) : 0.f;
           }
       }
     }
@@ -714,12 +706,12 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
   float acc[2][32], sum[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i] = sum[i] = 0.f;
-  int c = 0, kk = 0;
+  int c = 1, kk = 0;
   for (int j = nks; j < total; ++j) {
     if (tid == 0 && j + STAGES - 1 < total) load_stage(j + STAGES - 1);
     const int s = ring_wait_full(full, j);
-    const FireChunk& ch = p.chunks[c];
-    const int dy = ch.taps == 1 ? 1 : kk / 3, dx = ch.taps == 1 ? 1 : kk % 3;
+    const TcChunk& ch = p.chunks[c];   // nk: its taps, one K chunk of FS channels each
+    const int dy = ch.nk == 1 ? 1 : kk / 3, dx = ch.nk == 1 ? 1 : kk % 3;
     const int qr = (r + dy) * FQ_W + g + dx;
     mma_chunk<64, FS>(
         [&](int ks, uint32_t(&ahi)[4], uint32_t(&alo)[4]) {
@@ -727,7 +719,7 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
         },
         smem_u32(smem + s * STAGE), acc, sum);
     ring_release(empty, j);
-    if (++kk == ch.taps) {
+    if (++kk == ch.nk) {
       const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
       const int oy = tl.oy0 + r;
       const size_t prow = ((size_t)tl.n * p.H + oy) * p.W;
@@ -735,13 +727,13 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
       for (int h = 0; h < 2; ++h) {
         const int ox = tl.ox0 + g + 8 * h;
         if (oy >= p.H || ox >= p.W) continue;
-        float* yrow = p.y + (prow + ox) * p.Etot + ch.y_off;
+        float* yrow = p.y + (prow + ox) * p.y_cstride + ch.y_off;
 #pragma unroll
         for (int jn = 0; jn < 8; ++jn)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int col = 8 * jn + 2 * t + e;
-            if (col < ch.ncount) yrow[col] = fmaxf(sum[4 * jn + 2 * h + e] + p.bex[ch.y_off + col], 0.f);
+            if (col < ch.ncount) yrow[col] = fmaxf(sum[4 * jn + 2 * h + e] + p.bias[ch.p_off + col], 0.f);
           }
       }
 #pragma unroll
@@ -754,18 +746,17 @@ fire_tc_kernel(const __grid_constant__ FireParams p) {
 
 // ---------------------------------------------------------------------------------------------
 // Host side
-using ConvKernel = void (*)(TcParams);
-using FireKernel = void (*)(FireParams);
+using TcKernel = void (*)(TcParams);
 
 template <int KC, int MODE>
-ConvKernel conv_tc_instance(int NT) {
+TcKernel conv_tc_instance(int NT) {
   return NT == 64 ? conv_tc_kernel<64, KC, MODE>
          : NT == 32 ? conv_tc_kernel<32, KC, MODE> : conv_tc_kernel<16, KC, MODE>;
 }
 
 // The conv_tc_kernel instantiation of a plan (gather mode always walks K in chunks of 32; the
 // 72-wide head tile only comes with KC = 32).
-ConvKernel conv_tc_instance(int NT, int KC, int mode) {
+TcKernel conv_tc_instance(int NT, int KC, int mode) {
   if (NT == 72) return mode == TC_HALO ? conv_tc_kernel<72, 32, TC_HALO> : conv_tc_kernel<72, 32, TC_ROWS>;
   if (mode == TC_GATHER) return conv_tc_instance<32, TC_GATHER>(NT);
   if (mode == TC_HALO)
@@ -773,13 +764,22 @@ ConvKernel conv_tc_instance(int NT, int KC, int mode) {
   return KC == 32 ? conv_tc_instance<32, TC_ROWS>(NT) : conv_tc_instance<16, TC_ROWS>(NT);
 }
 
+// One conv of a plan: its output channels in chunks [chunk0, chunk0 + ceil(Cout / NT)) of NT,
+// its K over its cin input channels in chunks of KC.
+struct PlanGroup {
+  ConvGroup conv;
+  int NT, KC, cin, chunk0;
+};
+
+}  // namespace
+
 struct TcImpl {
   TcParams prm{};
-  int NT = 0, KC = 0, mode = TC_ROWS;
-  ConvKernel kernel = nullptr;
+  int KC = 0;          // channels of a box of the input's tensor maps
+  int mode = TC_ROWS;
+  TcKernel kernel = nullptr;
   size_t smem_bytes = 0;
-  std::vector<ConvGroup> groups;
-  std::vector<int> group_chunk0;   // first chunk of each group
+  std::vector<PlanGroup> groups;
   int cout_total = 0;
   float* d_w = nullptr;
   float* d_bias = nullptr;
@@ -861,7 +861,8 @@ static int encode_nhwc_map(CUtensorMap* map, const float* x, int n, int H, int W
   return encode_map(map, x, 4, dims, box, KC);
 }
 
-// Encodes the plan's tensor maps for input x of n images, unless they already are.
+// Encodes the plan's tensor maps for input x of n images, unless they already are: row mode its
+// row map; halo mode and the fire the halo map, halo mode also the map of a 1x1 conv's tile.
 static int update_maps(TcImpl* im, const float* x, int n) {
   if (im->mode == TC_GATHER || (im->map_x == x && im->map_n == n)) return SQDET_OK;
   TcParams& p = im->prm;
@@ -873,7 +874,7 @@ static int update_maps(TcImpl* im, const float* x, int n) {
     rc = encode_map(&p.amap, x, 2, dims, box, im->KC);
   } else {
     rc = encode_nhwc_map(&p.amap, x, n, p.H, p.W, p.Cin, im->KC, FQ_W, 10);
-    if (!rc) rc = encode_nhwc_map(&p.amap1, x, n, p.H, p.W, p.Cin, im->KC, FT_W, 8);
+    if (!rc && im->mode == TC_HALO) rc = encode_nhwc_map(&p.amap1, x, n, p.H, p.W, p.Cin, im->KC, FT_W, 8);
   }
   if (rc) return rc;
   im->map_x = x;
@@ -881,67 +882,52 @@ static int update_maps(TcImpl* im, const float* x, int n) {
   return SQDET_OK;
 }
 
-static void release_impl(void** impl) {
-  if (!*impl) return;
-  TcImpl* im = static_cast<TcImpl*>(*impl);
-  cudaFree(im->d_w);
-  cudaFree(im->d_bias);
-  cudaFree(im->d_scale);
-  cudaFree(im->d_shift);
-  delete im;
-  *impl = nullptr;
+// The grid's CTAs over n images: one per 8 x FT_W output tile in halo mode and the fire, one per
+// TILE_M output pixels otherwise.
+static long long grid_blocks(const TcImpl* im, int n) {
+  const TcParams& p = im->prm;
+  if (im->mode == TC_HALO || im->mode == TC_FIRE) return (long long)n * p.tiles_h * p.tiles_w;
+  return ((long long)n * p.Ho * p.Wo + TILE_M - 1) / TILE_M;
 }
 
-// Plans `groups` convs over one [B, H, W, Cin] input into a [B, Ho, Wo, y_cstride] output.
-// Returns 1 (planned), 0 (declined) or a negative status.
+// Plans the convs of im->groups over one [B, H, W, Cin] input into a [B, Ho, Wo, y_cstride]
+// output, for the mode, kernel and group tiling already in im: their chunks in group order, the
+// kernel's shared memory, and the weight, bias and affine buffers.  Returns 1 (planned),
+// 0 (declined) or a negative status.
 static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo, int stride,
-                       int pad_t, int pad_l, bool gather, const std::vector<ConvGroup>& groups,
-                       int relu, bool has_affine, int y_cstride) {
-  const int KC = (gather || Cin % 32 == 0) ? 32 : 16;
-  const int NT = pick_nt(groups, KC, gather);
-  if (!NT) return 0;
-  int mode = gather ? TC_GATHER : TC_ROWS;
-  for (const auto& g : groups)
-    if (!gather && g.ksize == 3) mode = TC_HALO;   // stride-1 SAME (tc_conv_eligible)
-  const long long M = (long long)B * Ho * Wo;
-  const int tiles_w = (Wo + FT_W - 1) / FT_W, tiles_h = (Ho + 7) / 8;
-  const long long blocks = mode == TC_HALO ? (long long)B * tiles_h * tiles_w : (M + TILE_M - 1) / TILE_M;
-  if (M <= 0 || blocks > 0x7fffffffLL) return 0;
-  im->NT = NT;
-  im->KC = KC;
-  im->mode = mode;
-  im->kernel = conv_tc_instance(NT, KC, mode);
-  im->groups = groups;
+                       int pad_t, int pad_l, int relu, bool has_affine, int y_cstride) {
+  const bool gather = im->mode == TC_GATHER;
   TcParams& p = im->prm;
   p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Ho = Ho; p.Wo = Wo; p.stride = stride;
-  p.relu = relu; p.y_cstride = y_cstride; p.M = M;
-  p.tiles_w = tiles_w; p.tiles_h = tiles_h;
+  p.relu = relu; p.y_cstride = y_cstride; p.M = (long long)B * Ho * Wo;
+  p.tiles_w = (Wo + FT_W - 1) / FT_W; p.tiles_h = (Ho + 7) / 8;
+  if (p.M <= 0 || grid_blocks(im, B) > 0x7fffffffLL) return 0;
   int nch = 0, poff = 0;
   long long woff = 0;
-  for (const auto& g : groups) {
-    im->group_chunk0.push_back(nch);
-    const int nk = gather ? (g.ksize * g.ksize * Cin + KC - 1) / KC : g.ksize * g.ksize * (Cin / KC);
-    for (int cb = 0; cb < g.Cout; cb += NT, ++nch) {
+  for (auto& g : im->groups) {
+    g.chunk0 = nch;
+    const int taps = g.conv.ksize * g.conv.ksize;
+    const int nk = gather ? (taps * g.cin + g.KC - 1) / g.KC : taps * (g.cin / g.KC);
+    for (int cb = 0; cb < g.conv.Cout; cb += g.NT, ++nch) {
       TcChunk& c = p.chunks[nch];
-      c.ksize = g.ksize;
-      c.pad_t = gather ? pad_t : g.ksize / 2;
-      c.pad_l = gather ? pad_l : g.ksize / 2;
+      c.ksize = g.conv.ksize;
+      c.pad_t = gather ? pad_t : g.conv.ksize / 2;
+      c.pad_l = gather ? pad_l : g.conv.ksize / 2;
       c.nk = nk;
-      c.ncount = g.Cout - cb < NT ? g.Cout - cb : NT;
-      c.y_off = g.y_off + cb;
+      c.ncount = g.conv.Cout - cb < g.NT ? g.conv.Cout - cb : g.NT;
+      c.y_off = g.conv.y_off + cb;
       c.p_off = poff + cb;
       c.w_off = woff;
-      woff += (long long)nk * 2 * NT * KC;
+      woff += (long long)nk * 2 * g.NT * g.KC;
     }
-    poff += g.Cout;
+    poff += g.conv.Cout;
   }
   p.nchunks = nch;
   im->cout_total = poff;
   im->w_floats = woff;
-  im->smem_bytes = conv_smem_bytes(NT, KC);
   cudaError_t ce = cudaFuncSetAttribute(im->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)im->smem_bytes);
-  if (ce != cudaSuccess) return cuda_fail(ce, "cudaFuncSetAttribute(conv_tc_kernel)");
+  if (ce != cudaSuccess) return cuda_fail(ce, "cudaFuncSetAttribute(tensor-core kernel)");
   SQ_CUDA(cudaMalloc(&im->d_w, sizeof(float) * (size_t)woff));
   SQ_CUDA(cudaMalloc(&im->d_bias, sizeof(float) * poff));
   SQ_CUDA(cudaMemset(im->d_bias, 0, sizeof(float) * poff));
@@ -980,46 +966,19 @@ static void pack_tiles(const float* w, long long kreal, int cout, int n0, int NT
   }
 }
 
-// Pack group `gi` weights (HWIO [k,k,Cin,Cout]) into each of its chunks' tiles: in halo mode a
-// 3x3 conv channel chunk by channel chunk with the taps inner, otherwise (1x1, gather mode) K
-// chunk kk holds flattened K rows [kk * KC, kk * KC + KC).
-static void pack_group(const TcImpl* im, int gi, const float* w_hwio, std::vector<float>& packed) {
-  const ConvGroup& g = im->groups[gi];
-  const int taps = im->mode == TC_HALO ? g.ksize * g.ksize : 1;
-  int ci = im->group_chunk0[gi];
-  for (int cb = 0; cb < g.Cout; cb += im->NT, ++ci) {
+// Packs group g's weights (HWIO [k, k, cin, Cout]) into each of its chunks' tiles: a 3x3 conv
+// channel chunk by channel chunk with the taps inner (in the fire's expand, whose K chunks are
+// the squeeze's FS channels, that is the flat HWIO order), a 1x1 conv and gather mode the
+// flattened K rows in order.
+static void pack_group(const TcImpl* im, const PlanGroup& g, const float* w_hwio, std::vector<float>& packed) {
+  const int taps = im->mode == TC_GATHER ? 1 : g.conv.ksize * g.conv.ksize;
+  int ci = g.chunk0;
+  for (int cb = 0; cb < g.conv.Cout; cb += g.NT, ++ci) {
     const TcChunk& c = im->prm.chunks[ci];
-    pack_tiles(w_hwio, (long long)g.ksize * g.ksize * im->prm.Cin, g.Cout, cb, im->NT, im->KC, c.nk,
-               taps, im->prm.Cin, packed.data() + c.w_off);
+    pack_tiles(w_hwio, (long long)g.conv.ksize * g.conv.ksize * g.cin, g.conv.Cout, cb, g.NT, g.KC,
+               c.nk, taps, g.cin, packed.data() + c.w_off);
   }
 }
-
-// ---- one-kernel fire module: host state -----------------------------
-struct FusedImpl {
-  FireParams fp{};
-  int KCI = 0;
-  int E1 = 0, E3 = 0;
-  FireKernel kernel = nullptr;
-  size_t smem = 0;
-  float* d_w = nullptr;    // squeeze tiles
-  float* d_w2 = nullptr;   // expand tiles
-  float* d_b = nullptr;
-  float* d_b2 = nullptr;
-  long long w_floats = 0, w2_floats = 0;
-  // the input and image count fp.amap was encoded for (null: none yet)
-  const float* map_x = nullptr;
-  int map_n = 0;
-};
-
-static void release_fused(void** impl) {
-  if (!*impl) return;
-  FusedImpl* im = static_cast<FusedImpl*>(*impl);
-  cudaFree(im->d_w); cudaFree(im->d_w2); cudaFree(im->d_b); cudaFree(im->d_b2);
-  delete im;
-  *impl = nullptr;
-}
-
-}  // namespace
 
 // ---------------------------------------------------------------------------------------------
 bool tc_conv_eligible(int Cin, int Cout, int size, int stride, int padding) {
@@ -1040,26 +999,50 @@ int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, const std::vect
   const Geom gh = tf_geometry(H, size, stride, padding);
   const Geom gw = tf_geometry(W, size, stride, padding);
   if (gh.out <= 0 || gw.out <= 0) return 0;
-  void* im = new TcImpl();
-  int rc = plan_common(static_cast<TcImpl*>(im), B, H, W, Cin, gh.out, gw.out, stride,
-                       gh.pad_before, gw.pad_before, gather, convs, relu, has_affine, y_cstride);
-  if (rc <= 0) {
-    release_impl(&im);
-    return rc;
-  }
-  plan->impl = im;
-  return 1;
+  const int KC = (gather || Cin % 32 == 0) ? 32 : 16;
+  const int NT = pick_nt(convs, KC, gather);
+  if (!NT) return 0;
+  int mode = gather ? TC_GATHER : TC_ROWS;
+  for (const auto& g : convs)
+    if (!gather && g.ksize == 3) mode = TC_HALO;   // stride-1 SAME (tc_conv_eligible)
+  TcImpl* im = plan->impl = new TcImpl();
+  im->KC = KC;
+  im->mode = mode;
+  im->kernel = conv_tc_instance(NT, KC, mode);
+  im->smem_bytes = conv_smem_bytes(NT, KC);
+  for (const auto& g : convs) im->groups.push_back({g, NT, KC, Cin, 0});
+  const int rc = plan_common(im, B, H, W, Cin, gh.out, gw.out, stride, gh.pad_before, gw.pad_before,
+                             relu, has_affine, y_cstride);
+  if (rc <= 0) tc_conv_release(plan);
+  return rc;
+}
+
+int tc_fire_plan(TcConvPlan* plan, int B, int H, int W, int Cin, int S, int E1, int E3) {
+  plan->impl = nullptr;
+  if (Cin % 16 || Cin < 16 || S != FS || E1 <= 0 || E3 <= 0) return 0;
+  if ((E1 + 63) / 64 + (E3 + 63) / 64 > 16) return 0;   // expand chunks of 64 channels
+  const int KCI = Cin % 32 == 0 ? 32 : 16;
+  TcImpl* im = plan->impl = new TcImpl();
+  im->KC = KCI;
+  im->mode = TC_FIRE;
+  im->kernel = KCI == 32 ? fire_tc_kernel<32> : fire_tc_kernel<16>;
+  im->smem_bytes = fire_smem_bytes(KCI);
+  // chunk 0 the squeeze, then the 64-wide expand chunks, expand1x1's before expand3x3's
+  im->groups = {{{1, FS, 0}, FS, KCI, Cin, 0}, {{1, E1, 0}, 64, FS, FS, 0}, {{3, E3, E1}, 64, FS, FS, 0}};
+  const int rc = plan_common(im, B, H, W, Cin, H, W, 1, 0, 0, 1, false, E1 + E3);
+  if (rc <= 0) tc_conv_release(plan);
+  return rc;
 }
 
 int tc_conv_pack_weights(TcConvPlan* plan, const std::vector<const float*>& w_hwio,
                          const std::vector<const float*>& bias) {
-  TcImpl* im = static_cast<TcImpl*>(plan->impl);
+  TcImpl* im = plan->impl;
   std::vector<float> packed((size_t)im->w_floats, 0.f);
-  for (int gi = 0; gi < (int)im->groups.size(); ++gi) pack_group(im, gi, w_hwio[gi], packed);
+  for (size_t gi = 0; gi < im->groups.size(); ++gi) pack_group(im, im->groups[gi], w_hwio[gi], packed);
   SQ_CUDA(cudaMemcpy(im->d_w, packed.data(), packed.size() * sizeof(float), cudaMemcpyHostToDevice));
   int off = 0;
-  for (int gi = 0; gi < (int)im->groups.size(); ++gi) {
-    const int n = im->groups[gi].Cout;
+  for (size_t gi = 0; gi < im->groups.size(); ++gi) {
+    const int n = im->groups[gi].conv.Cout;
     if (bias[gi]) SQ_CUDA(cudaMemcpy(im->d_bias + off, bias[gi], sizeof(float) * n, cudaMemcpyHostToDevice));
     off += n;
   }
@@ -1067,7 +1050,7 @@ int tc_conv_pack_weights(TcConvPlan* plan, const std::vector<const float*>& w_hw
 }
 
 int tc_conv_set_affine(TcConvPlan* plan, const float* scale, const float* shift) {
-  TcImpl* im = static_cast<TcImpl*>(plan->impl);
+  TcImpl* im = plan->impl;
   if (!im->d_scale) return fail(SQDET_ERR_STATE, "tc conv planned without an affine epilogue");
   SQ_CUDA(cudaMemcpy(im->d_scale, scale, sizeof(float) * im->cout_total, cudaMemcpyHostToDevice));
   SQ_CUDA(cudaMemcpy(im->d_shift, shift, sizeof(float) * im->cout_total, cudaMemcpyHostToDevice));
@@ -1076,7 +1059,7 @@ int tc_conv_set_affine(TcConvPlan* plan, const float* scale, const float* shift)
 
 int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, int n,
                    cudaStream_t stream) {
-  TcImpl* im = static_cast<TcImpl*>(plan.impl);
+  TcImpl* im = plan.impl;
   if (n < 1 || n > im->prm.B) return fail(SQDET_ERR_INVALID_ARG, "launch_conv_tc: image count outside [1, B]");
   const int rc = update_maps(im, x_dev, n);
   if (rc) return rc;
@@ -1085,175 +1068,53 @@ int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, int
   prm.y = y_dev;
   prm.B = n;
   prm.M = (long long)n * prm.Ho * prm.Wo;
-  const long long blocks = im->mode == TC_HALO ? (long long)n * prm.tiles_h * prm.tiles_w
-                                               : (prm.M + TILE_M - 1) / TILE_M;
-  const dim3 grid((unsigned)blocks, (unsigned)prm.nchunks);
+  // a fire CTA walks every chunk of its tile
+  const dim3 grid((unsigned)grid_blocks(im, n), im->mode == TC_FIRE ? 1u : (unsigned)prm.nchunks);
   im->kernel<<<grid, NUM_THREADS, im->smem_bytes, stream>>>(prm);
-  SQ_CHECK_LAUNCH("conv_tc_kernel");
+  SQ_CHECK_LAUNCH(im->mode == TC_FIRE ? "fire_tc_kernel" : "conv_tc_kernel");
   return SQDET_OK;
 }
 
-void tc_conv_release(TcConvPlan* plan) { release_impl(&plan->impl); }
-
-int conv2d_tc_oneshot(const float* x_dev, const float* w_hwio_dev, const float* bias_dev,
-                      const float* scale_dev, const float* shift_dev, float* y_dev, int B, int H,
-                      int W, int Cin, int Cout, int size, int stride, int padding, int relu,
-                      int y_cstride, int y_coff, cudaStream_t stream) {
-  TcConvPlan plan;
-  int rc = tc_conv_plan(&plan, B, H, W, Cin, {{size, Cout, y_coff}}, stride, padding, relu,
-                        scale_dev != nullptr, y_cstride);
-  if (rc < 0) return rc;
-  if (rc == 0) {
-    // shape not taken by the tensor-core path (e.g. a strided conv): same dispatch as the engine
-    ConvArgs a;
-    a.x = x_dev; a.w = w_hwio_dev; a.bias = bias_dev; a.scale = scale_dev; a.shift = shift_dev;
-    a.y = y_dev; a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.size = size;
-    a.stride = stride; a.padding = padding; a.relu = relu; a.y_cstride = y_cstride; a.y_coff = y_coff;
-    return launch_conv_simt(a, stream);
-  }
-  std::vector<float> w((size_t)size * size * Cin * Cout), b(Cout, 0.f), sc, sh;
-  cudaError_t ce = cudaMemcpy(w.data(), w_hwio_dev, w.size() * sizeof(float), cudaMemcpyDeviceToHost);
-  if (ce == cudaSuccess && bias_dev)
-    ce = cudaMemcpy(b.data(), bias_dev, Cout * sizeof(float), cudaMemcpyDeviceToHost);
-  if (ce == cudaSuccess && scale_dev) {
-    sc.resize(Cout); sh.resize(Cout);
-    ce = cudaMemcpy(sc.data(), scale_dev, Cout * sizeof(float), cudaMemcpyDeviceToHost);
-    if (ce == cudaSuccess) ce = cudaMemcpy(sh.data(), shift_dev, Cout * sizeof(float), cudaMemcpyDeviceToHost);
-  }
-  if (ce != cudaSuccess) {
-    tc_conv_release(&plan);
-    return cuda_fail(ce, "conv2d_tc_oneshot: parameter download");
-  }
-  rc = tc_conv_pack_weights(&plan, {w.data()}, {bias_dev ? b.data() : nullptr});
-  if (!rc && scale_dev) rc = tc_conv_set_affine(&plan, sc.data(), sh.data());
-  if (!rc) rc = launch_conv_tc(plan, x_dev, y_dev, B, stream);
-  ce = cudaStreamSynchronize(stream);
-  tc_conv_release(&plan);
-  if (rc) return rc;
-  if (ce != cudaSuccess) return cuda_fail(ce, "conv2d_tc_oneshot sync");
-  return SQDET_OK;
-}
-
-// ---- one-kernel fire module ----------------------------------------------------------------------
-int tc_fused_fire_plan(TcFusedFirePlan* plan, int B, int H, int W, int Cin, int S, int E1, int E3) {
+void tc_conv_release(TcConvPlan* plan) {
+  TcImpl* im = plan->impl;
+  if (!im) return;
+  cudaFree(im->d_w);
+  cudaFree(im->d_bias);
+  cudaFree(im->d_scale);
+  cudaFree(im->d_shift);
+  delete im;
   plan->impl = nullptr;
-  if (Cin % 16 || Cin < 16 || S != FS || E1 <= 0 || E3 <= 0) return 0;
-  const int nch = (E1 + 63) / 64 + (E3 + 63) / 64;
-  if (nch > MAX_FCHUNKS) return 0;
-  FusedImpl* im = new FusedImpl();
-  im->KCI = Cin % 32 == 0 ? 32 : 16;
-  im->E1 = E1;
-  im->E3 = E3;
-  FireParams& p = im->fp;
-  p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Etot = E1 + E3;
-  p.tiles_w = (W + FT_W - 1) / FT_W;
-  p.tiles_h = (H + 7) / 8;
-  p.nchunks = nch;
-  int c = 0;
-  for (int gi = 0; gi < 2; ++gi) {
-    const int E = gi ? E3 : E1, taps = gi ? 9 : 1;
-    for (int cb = 0; cb < E; cb += 64, ++c) {
-      p.chunks[c] = FireChunk{taps, E - cb < 64 ? E - cb : 64, (gi ? E1 : 0) + cb};
-      p.total_nk += taps;
-    }
-  }
-  im->w_floats = (long long)(Cin / im->KCI) * 2 * FS * im->KCI;
-  im->w2_floats = (long long)p.total_nk * 2 * 64 * FS;
-  im->kernel = im->KCI == 32 ? fire_tc_kernel<32> : fire_tc_kernel<16>;
-  im->smem = fire_smem_bytes(im->KCI);
-  void* vp = im;
-  cudaError_t ce = cudaFuncSetAttribute(im->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)im->smem);
-  if (ce != cudaSuccess) {
-    release_fused(&vp);
-    return cuda_fail(ce, "cudaFuncSetAttribute(fire_tc_kernel)");
-  }
-  if ((ce = cudaMalloc(&im->d_w, sizeof(float) * im->w_floats)) != cudaSuccess ||
-      (ce = cudaMalloc(&im->d_w2, sizeof(float) * im->w2_floats)) != cudaSuccess ||
-      (ce = cudaMalloc(&im->d_b, sizeof(float) * FS)) != cudaSuccess ||
-      (ce = cudaMalloc(&im->d_b2, sizeof(float) * (E1 + E3))) != cudaSuccess) {
-    release_fused(&vp);
-    return cuda_fail(ce, "cudaMalloc(fused fire)");
-  }
-  p.wsq = im->d_w; p.wex = im->d_w2; p.bsq = im->d_b; p.bex = im->d_b2;
-  plan->impl = im;
-  return 1;
 }
 
-int tc_fused_fire_pack_weights(TcFusedFirePlan* plan, const float* w_sq, const float* b_sq,
-                               const float* w_e1, const float* b_e1, const float* w_e3,
-                               const float* b_e3) {
-  FusedImpl* im = static_cast<FusedImpl*>(plan->impl);
-  const FireParams& p = im->fp;
-  std::vector<float> wsq((size_t)im->w_floats), wex((size_t)im->w2_floats), bex;
-  pack_tiles(w_sq, p.Cin, FS, 0, FS, im->KCI, p.Cin / im->KCI, 1, p.Cin, wsq.data());
-  long long off = 0;
-  for (int c = 0; c < p.nchunks; ++c) {
-    const FireChunk& ch = p.chunks[c];
-    const bool e3 = ch.taps == 9;
-    pack_tiles(e3 ? w_e3 : w_e1, (long long)ch.taps * FS, e3 ? im->E3 : im->E1,
-               ch.y_off - (e3 ? im->E1 : 0), 64, FS, ch.taps, 1, FS, wex.data() + off);
-    off += (long long)ch.taps * 2 * 64 * FS;
-  }
-  bex.assign(b_e1, b_e1 + im->E1);
-  bex.insert(bex.end(), b_e3, b_e3 + im->E3);
-  SQ_CUDA(cudaMemcpy(im->d_w, wsq.data(), wsq.size() * sizeof(float), cudaMemcpyHostToDevice));
-  SQ_CUDA(cudaMemcpy(im->d_w2, wex.data(), wex.size() * sizeof(float), cudaMemcpyHostToDevice));
-  SQ_CUDA(cudaMemcpy(im->d_b, b_sq, FS * sizeof(float), cudaMemcpyHostToDevice));
-  SQ_CUDA(cudaMemcpy(im->d_b2, bex.data(), bex.size() * sizeof(float), cudaMemcpyHostToDevice));
-  return SQDET_OK;
-}
-
-int launch_fused_fire_tc(const TcFusedFirePlan& plan, const float* x_dev, float* y_dev, int n,
-                         cudaStream_t stream) {
-  FusedImpl* im = static_cast<FusedImpl*>(plan.impl);
-  FireParams& fp = im->fp;
-  if (n < 1 || n > fp.B) return fail(SQDET_ERR_INVALID_ARG, "launch_fused_fire_tc: image count outside [1, B]");
-  if (im->map_x != x_dev || im->map_n != n) {
-    im->map_x = nullptr;
-    const int rc = encode_nhwc_map(&fp.amap, x_dev, n, fp.H, fp.W, fp.Cin, im->KCI, FQ_W, 10);
-    if (rc) return rc;
-    im->map_x = x_dev;
-    im->map_n = n;
-  }
-  FireParams p = fp;
-  p.y = y_dev;
-  p.B = n;
-  const unsigned grid = (unsigned)((long long)n * p.tiles_h * p.tiles_w);
-  im->kernel<<<grid, NUM_THREADS, im->smem, stream>>>(p);
-  SQ_CHECK_LAUNCH("fire_tc_kernel");
-  return SQDET_OK;
-}
-
-void tc_fused_fire_release(TcFusedFirePlan* plan) { release_fused(&plan->impl); }
-
-int fire_fused_oneshot(const float* x_dev, const float* w_sq_dev, const float* b_sq_dev,
-                       const float* w_e1_dev, const float* b_e1_dev, const float* w_e3_dev,
-                       const float* b_e3_dev, float* y_dev, int B, int H, int W, int Cin, int S,
-                       int E1, int E3, cudaStream_t stream) {
-  TcFusedFirePlan plan;
-  int rc = tc_fused_fire_plan(&plan, B, H, W, Cin, S, E1, E3);
-  if (rc <= 0) return rc < 0 ? rc : 1;
-  std::vector<float> wsq((size_t)Cin * S), bsq(S), w1((size_t)S * E1), b1(E1), w3((size_t)9 * S * E3),
-      b3(E3);
-  const std::pair<void*, const float*> io[6] = {{wsq.data(), w_sq_dev}, {bsq.data(), b_sq_dev},
-                                                {w1.data(), w_e1_dev},  {b1.data(), b_e1_dev},
-                                                {w3.data(), w_e3_dev},  {b3.data(), b_e3_dev}};
-  const size_t n[6] = {wsq.size(), bsq.size(), w1.size(), b1.size(), w3.size(), b3.size()};
+int tc_conv_oneshot(TcConvPlan* plan, const std::vector<const float*>& w_hwio_dev,
+                    const std::vector<const float*>& bias_dev, const float* scale_dev,
+                    const float* shift_dev, const float* x_dev, float* y_dev, cudaStream_t stream) {
+  TcImpl* im = plan->impl;
+  if (!im) return 1;
+  const size_t ng = im->groups.size();
+  std::vector<std::vector<float>> w(ng), b(ng);
+  std::vector<float> sc, sh;
+  std::vector<const float*> w_host(ng), b_host(ng);
   cudaError_t ce = cudaSuccess;
-  for (int i = 0; i < 6 && ce == cudaSuccess; ++i)
-    ce = cudaMemcpy(io[i].first, io[i].second, n[i] * sizeof(float), cudaMemcpyDeviceToHost);
-  if (ce != cudaSuccess) {
-    tc_fused_fire_release(&plan);
-    return cuda_fail(ce, "fire_fused_oneshot: parameter download");
+  auto download = [&ce](std::vector<float>& dst, const float* src, size_t n) {
+    dst.resize(n);
+    if (ce == cudaSuccess) ce = cudaMemcpy(dst.data(), src, n * sizeof(float), cudaMemcpyDeviceToHost);
+    return dst.data();
+  };
+  for (size_t gi = 0; gi < ng; ++gi) {
+    const ConvGroup& g = im->groups[gi].conv;
+    w_host[gi] = download(w[gi], w_hwio_dev[gi], (size_t)g.ksize * g.ksize * im->groups[gi].cin * g.Cout);
+    b_host[gi] = bias_dev[gi] ? download(b[gi], bias_dev[gi], g.Cout) : nullptr;
   }
-  rc = tc_fused_fire_pack_weights(&plan, wsq.data(), bsq.data(), w1.data(), b1.data(), w3.data(),
-                                  b3.data());
-  if (!rc) rc = launch_fused_fire_tc(plan, x_dev, y_dev, B, stream);
+  if (scale_dev) download(sc, scale_dev, im->cout_total), download(sh, shift_dev, im->cout_total);
+  int rc = ce == cudaSuccess ? tc_conv_pack_weights(plan, w_host, b_host)
+                             : cuda_fail(ce, "tc_conv_oneshot: parameter download");
+  if (!rc && scale_dev) rc = tc_conv_set_affine(plan, sc.data(), sh.data());
+  if (!rc) rc = launch_conv_tc(*plan, x_dev, y_dev, im->prm.B, stream);
   ce = cudaStreamSynchronize(stream);
-  tc_fused_fire_release(&plan);
+  tc_conv_release(plan);
   if (rc) return rc;
-  if (ce != cudaSuccess) return cuda_fail(ce, "fire_fused_oneshot sync");
+  if (ce != cudaSuccess) return cuda_fail(ce, "tc_conv_oneshot sync");
   return SQDET_OK;
 }
 

@@ -73,7 +73,7 @@ struct ConvSpec {
   float* shift = nullptr;
 };
 
-enum LaunchKind { L_CONV_SIMT, L_CONV_TC, L_CONV_POOL, L_FIRE_TC, L_MAXPOOL, L_ADD_RELU };
+enum LaunchKind { L_CONV_SIMT, L_CONV_TC, L_CONV_POOL, L_MAXPOOL, L_ADD_RELU };
 
 // One kernel launch of an op.
 struct Launch {
@@ -81,8 +81,7 @@ struct Launch {
   int src = -1, dst = -1;        // tensor read (add+ReLU also reads the op's src2) and written
   int conv = 0, nconv = 0;       // computes the op's convs [conv, conv + nconv)
   int pool_padding = 0;          // L_CONV_POOL: padding of the absorbed 3x3/2 max-pool
-  TcConvPlan tc;                 // L_CONV_TC
-  TcFusedFirePlan fire;          // L_FIRE_TC
+  TcConvPlan tc;                 // L_CONV_TC: a conv, an expand pair or a whole fire module
 };
 
 struct Op {
@@ -318,8 +317,6 @@ static int run_launch(sqdet_engine* e, const Op& op, const Launch& l, const floa
                                    c.shift, y, n, in.H, in.W, c.Cout, c.size, c.padding, c.relu,
                                    l.pool_padding, stream);
     }
-    case L_FIRE_TC:
-      return launch_fused_fire_tc(l.fire, x, y, n, stream);
     case L_MAXPOOL:
       return launch_maxpool(x, y, n, in.H, in.W, in.C, op.size, op.stride, op.padding, stream);
     case L_ADD_RELU:
@@ -338,10 +335,7 @@ static int run_op(sqdet_engine* e, const Op& op, const float* images, int n, cud
 }
 
 static void release_launches(Op& op) {
-  for (auto& l : op.launches) {
-    tc_conv_release(&l.tc);
-    tc_fused_fire_release(&l.fire);
-  }
+  for (auto& l : op.launches) tc_conv_release(&l.tc);
   op.launches.clear();
 }
 
@@ -467,19 +461,15 @@ static int prepare_params(sqdet_engine* e) {
     }
     // tensor-core weight packs
     for (auto& l : op.launches) {
+      if (l.kind != L_CONV_TC) continue;
       std::vector<const float*> w, b;
       for (int k = l.conv; k < l.conv + l.nconv; ++k) {
         w.push_back(host(op.convs[k].p_kernel));
         b.push_back(host(op.convs[k].p_bias));
       }
-      int rc = SQDET_OK;
-      if (l.kind == L_FIRE_TC) {
-        rc = tc_fused_fire_pack_weights(&l.fire, w[0], b[0], w[1], b[1], w[2], b[2]);
-      } else if (l.kind == L_CONV_TC) {
-        rc = tc_conv_pack_weights(&l.tc, w, b);
-        if (!rc && !scale[l.conv].empty())
-          rc = tc_conv_set_affine(&l.tc, scale[l.conv].data(), shift[l.conv].data());
-      }
+      int rc = tc_conv_pack_weights(&l.tc, w, b);
+      if (!rc && !scale[l.conv].empty())
+        rc = tc_conv_set_affine(&l.tc, scale[l.conv].data(), shift[l.conv].data());
       if (rc) return rc;
     }
   }
@@ -888,8 +878,8 @@ static int plan_fire(sqdet_engine* e, Op& op, bool tc) {
   const long long tiles = (long long)x.B * ((x.H + 7) / 8) * ((x.W + 15) / 16);
   if (tc && sq.Cout <= 16 && tiles >= 4LL * e->sms && sq.dst != e->preds &&
       !read_by_other_op(e, sq.dst, &op)) {
-    Launch l{L_FIRE_TC, op.src, op.dst, 0, 3};
-    const int rc = tc_fused_fire_plan(&l.fire, x.B, x.H, x.W, x.C, sq.Cout, e1.Cout, e3.Cout);
+    Launch l{L_CONV_TC, op.src, op.dst, 0, 3};
+    const int rc = tc_fire_plan(&l.tc, x.B, x.H, x.W, x.C, sq.Cout, e1.Cout, e3.Cout);
     if (rc < 0) return rc;
     if (rc) {
       op.launches.push_back(l);
@@ -1413,35 +1403,23 @@ int sqdet_conv2d(const float* x_dev, const float* w_hwio_dev, const float* bias_
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv2d: padding must be SAME(0) or VALID(1)");
   if (int rc = check_conv_epilogue("sqdet_conv2d", scale_dev, shift_dev, Cout, y_cstride, y_coff))
     return rc;
-  if (math_mode == SQDET_MATH_TF32X3_TC)
-    return conv2d_tc_oneshot(x_dev, w_hwio_dev, bias_dev, scale_dev, shift_dev, y_dev, B, H, W,
-                             Cin, Cout, size, stride, padding, relu, y_cstride, y_coff,
-                             (cudaStream_t)stream);
-  if (math_mode != SQDET_MATH_FP32_SIMT)
+  if (math_mode != SQDET_MATH_FP32_SIMT && math_mode != SQDET_MATH_TF32X3_TC)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv2d: unknown math_mode");
+  if (math_mode == SQDET_MATH_TF32X3_TC) {
+    TcConvPlan plan;
+    int rc = tc_conv_plan(&plan, B, H, W, Cin, {{size, Cout, y_coff}}, stride, padding, relu,
+                          scale_dev != nullptr, y_cstride);
+    if (rc >= 0)
+      rc = tc_conv_oneshot(&plan, {w_hwio_dev}, {bias_dev}, scale_dev, shift_dev, x_dev, y_dev,
+                           (cudaStream_t)stream);
+    if (rc != 1) return rc;   // 1 = shape not taken by the tensor-core path (e.g. a strided conv)
+  }
+  // the fp32 SIMT kernel: the same dispatch as the engine
   ConvArgs a;
   a.x = x_dev; a.w = w_hwio_dev; a.bias = bias_dev; a.scale = scale_dev; a.shift = shift_dev;
   a.y = y_dev; a.B = B; a.H = H; a.W = W; a.Cin = Cin; a.Cout = Cout; a.size = size;
   a.stride = stride; a.padding = padding; a.relu = relu; a.y_cstride = y_cstride; a.y_coff = y_coff;
   return launch_conv_simt(a, (cudaStream_t)stream);
-}
-
-
-int sqdet_conv3x3_halo(const float* x_dev, const float* w_hwio_dev, const float* bias_dev,
-                       const float* scale_dev, const float* shift_dev, float* y_dev, int B, int H,
-                       int W, int Cin, int Cout, int relu, int y_cstride, int y_coff, void* stream_v) {
-  if (!x_dev || !w_hwio_dev || !y_dev)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv3x3_halo: null pointer");
-  if (B <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv3x3_halo: non-positive dimension");
-  if (int rc = check_conv_epilogue("sqdet_conv3x3_halo", scale_dev, shift_dev, Cout, y_cstride,
-                                   y_coff))
-    return rc;
-  if (!tc_conv_eligible(Cin, Cout, 3, 1, SQDET_PAD_SAME))
-    return fail(SQDET_ERR_UNSUPPORTED, "sqdet_conv3x3_halo: shape not taken by the tensor-core path");
-  return conv2d_tc_oneshot(x_dev, w_hwio_dev, bias_dev, scale_dev, shift_dev, y_dev, B, H, W, Cin,
-                           Cout, 3, 1, SQDET_PAD_SAME, relu, y_cstride, y_coff,
-                           (cudaStream_t)stream_v);
 }
 
 /* SqueezeDet._fire_layer as ONE stage-isolated call (src/nets/squeezeDet.py:81-106). */
@@ -1457,8 +1435,11 @@ int sqdet_fire(const float* x_dev, const float* w_sq_dev, const float* b_sq_dev,
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_fire: unknown math_mode");
   cudaStream_t stream = (cudaStream_t)stream_v;
   if (math_mode == SQDET_MATH_TF32X3_TC) {
-    int rc = fire_fused_oneshot(x_dev, w_sq_dev, b_sq_dev, w_e1_dev, b_e1_dev, w_e3_dev, b_e3_dev,
-                                y_dev, B, H, W, Cin, S, E1, E3, stream);
+    TcConvPlan plan;
+    int rc = tc_fire_plan(&plan, B, H, W, Cin, S, E1, E3);
+    if (rc >= 0)
+      rc = tc_conv_oneshot(&plan, {w_sq_dev, w_e1_dev, w_e3_dev}, {b_sq_dev, b_e1_dev, b_e3_dev},
+                           nullptr, nullptr, x_dev, y_dev, stream);
     if (rc != 1) return rc;   // 1 = shape not taken by the one-kernel fire
   }
   // squeeze tensor through HBM, then the two expand convs into the concat tensor

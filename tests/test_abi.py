@@ -67,7 +67,7 @@ def test_argument_validation_needs_no_gpu():
 
 
 def test_conv_epilogue_validation_needs_no_gpu():
-  """sqdet_conv2d (both math modes) and sqdet_conv3x3_halo reject a channel window outside
+  """sqdet_conv2d (both math modes) rejects a channel window outside
   [0, y_cstride) and a scale without a shift (or the reverse) before any device work: on a box
   with no device that is SQDET_ERR_INVALID_ARG, not a CUDA error.  The pointers are never
   dereferenced, so the test only runs where no device could be handed them."""
@@ -82,8 +82,6 @@ def test_conv_epilogue_validation_needs_no_gpu():
     for mode in (_lib.MATH_FP32_SIMT, _lib.MATH_TF32X3_TC):
       assert lib.sqdet_conv2d(p, p, p, sc, sh, p, B, H, W, Cin, Cout, 3, 1, 0, 1, cs, coff, mode,
                               None) == -1, (cs, coff, sc, sh, mode)
-    assert lib.sqdet_conv3x3_halo(p, p, p, sc, sh, p, B, H, W, Cin, Cout, 1, cs, coff,
-                                  None) == -1, (cs, coff, sc, sh)
 
 
 def test_padding_code():

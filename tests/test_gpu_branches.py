@@ -5,7 +5,7 @@
   * add_relu_kernel's float4 body, tail and unaligned paths, including an add+ReLU whose operand
     is the image input and therefore reads the caller's images buffer;
   * u8_meansub_kernel's tail (B * H * W not a multiple of 4);
-  * sqdet_conv2d / sqdet_conv3x3_halo argument validation, the same in both math modes.
+  * sqdet_conv2d argument validation, the same in both math modes.
 tests/test_host_logic.py restates each branch predicate and checks that the tables below reach
 every branch."""
 import numpy as np
@@ -222,7 +222,7 @@ BAD_EPILOGUES = [
     (72, 0, False, True)]
 
 
-@pytest.mark.parametrize('entry', ['conv2d_simt', 'conv2d_tc', 'conv3x3_halo'])
+@pytest.mark.parametrize('entry', ['conv2d_simt', 'conv2d_tc'])
 @pytest.mark.parametrize('bad', BAD_EPILOGUES)
 def test_conv_rejects_bad_epilogue(entry, bad, gpu_device):
   """A channel window outside [0, y_cstride) or an unpaired scale / shift is refused with
@@ -242,13 +242,9 @@ def test_conv_rejects_bad_epilogue(entry, bad, gpu_device):
   sc = vec[1].ptr if has_scale else None
   sh = vec[2].ptr if has_shift else None
   y = dy.ptr + 4 * pad
-  if entry == 'conv3x3_halo':
-    rc = lib.sqdet_conv3x3_halo(dx.ptr, dw.ptr, vec[0].ptr, sc, sh, y, B, H, W, Cin, Cout, 1, cs,
-                                coff, None)
-  else:
-    mode = _lib.MATH_FP32_SIMT if entry == 'conv2d_simt' else _lib.MATH_TF32X3_TC
-    rc = lib.sqdet_conv2d(dx.ptr, dw.ptr, vec[0].ptr, sc, sh, y, B, H, W, Cin, Cout, 3, 1, 0, 1,
-                          cs, coff, mode, None)
+  mode = _lib.MATH_FP32_SIMT if entry == 'conv2d_simt' else _lib.MATH_TF32X3_TC
+  rc = lib.sqdet_conv2d(dx.ptr, dw.ptr, vec[0].ptr, sc, sh, y, B, H, W, Cin, Cout, 3, 1, 0, 1, cs,
+                        coff, mode, None)
   assert rc == ERR_INVALID_ARG, (rc, lib.sqdet_last_error())
   _lib.check(lib.sqdet_stream_sync(gpu_device, None))
   assert dy.to_numpy(np.float32, sentinel.shape).tobytes() == sentinel.tobytes()

@@ -58,7 +58,7 @@ def test_fire_vs_oracle(shape, math_mode, gpu_device):
 
 
 # Shapes the shipped nets never produce, chosen to reach both fire_tc_kernel<KCI> instantiations
-# (KCI = 16 for Cin % 32 == 16, else 32) and the planner's edges (conv_tc.cu, tc_fused_fire_plan):
+# (KCI = 16 for Cin % 32 == 16, else 32) and the planner's edges (conv_tc.cu, tc_fire_plan):
 #   S = 16 (one kernel) and S = 32, 48, 64 (squeeze and expands as three sqdet_conv2d launches),
 #   E1 != E3, expand widths that are not multiples of 64 or of 8,
 #   16 expand chunks of 64 (the one-kernel limit) and 17 (sqdet_fire falls back to separate

@@ -4,14 +4,15 @@ nine taps as row offsets into it.  Tiles cut by every image edge, images smaller
 (down to 1 x 1), every output-tile width with both K chunk widths, a ragged fire expand pair (a
 1x1 and a 3x3 conv in one launch), the affine epilogue with a channel window, and images of a
 partial batch.  Each element is checked against the fp64 oracle on the scale that bounds any
-fp32 summation of its products, with the bar of test_gpu_adversarial."""
+fp32 summation of its products, with the bar of test_gpu_adversarial; the ConvDet heads, wide
+outputs and a channel window also against a relative bar over the whole tensor and its borders."""
 import numpy as np
 import pytest
 
 import oracle
 from squeezedet_b200 import _lib
 from squeezedet_b200.utils import synth
-from gpu_util import conv2d_gpu
+from gpu_util import conv2d_gpu, rel_err
 from test_gpu_adversarial import adv_tol
 from test_gpu_dispatch import build, engine_tensor
 
@@ -77,6 +78,54 @@ def test_halo_tile_affine_and_channel_window(cin, gpu_device):
                    math_mode=TC, y_init=y0)
   assert_within_bound(got[..., coff:coff + Cout], want, bound, 9 * cin, cin)
   assert np.all(got[..., :coff] == 7.0) and np.all(got[..., coff + Cout:] == 7.0)
+
+
+CONV_RTOL = 2e-5
+HALO_CONV_CASES = [
+    # B, H, W, Cin, Cout: output tile NT (pick_nt) and K chunk KC (32 when Cin % 32 == 0, else 16)
+    (1, 24, 78, 768, 72),     # NT 72, KC 32; the ConvDet head of SqueezeDet
+    (2, 22, 76, 384, 72),     # NT 72, KC 32; the ConvDet head of SqueezeDet+ (ragged both ways)
+    (1, 33, 19, 64, 64),      # NT 64, KC 32; one chunk, tiles over the right and bottom edges
+    (1, 9, 40, 32, 128),      # NT 64, KC 32; two chunks, a second tile row of one image row
+    (2, 17, 23, 48, 256),     # NT 64, KC 16; four chunks, three channel chunks
+    (1, 8, 16, 16, 32),       # NT 32, KC 16; exactly one tile, one channel chunk
+    (6, 40, 48, 32, 32),      # NT 32, KC 32; 90 tiles over six images
+]
+WINDOW_CASE = (1, 15, 18, 32, 64)   # NT 64, KC 32
+
+
+@pytest.mark.parametrize('case', HALO_CONV_CASES)
+def test_halo_conv_vs_oracle(case, gpu_device):
+  B, H, W, Cin, Cout = case
+  rng = np.random.default_rng(sum(case))
+  x = rng.normal(size=(B, H, W, Cin)).astype(np.float32)
+  w = (rng.normal(size=(3, 3, Cin, Cout)) / np.sqrt(9 * Cin)).astype(np.float32)
+  b = rng.normal(size=(Cout,)).astype(np.float32)
+  want = oracle.conv2d(x, w, b, 1, 'SAME', apply_relu=True, dtype=np.float64)
+  got = conv2d_gpu(x, w, b, 1, 'SAME', relu=True, math_mode=TC)
+  assert got.shape == want.shape and not np.isnan(got).any()
+  assert rel_err(got, want) < CONV_RTOL, rel_err(got, want)
+  # image borders carry the SAME zero padding: check them on their own scale
+  for sl in (np.s_[:, 0], np.s_[:, -1], np.s_[:, :, 0], np.s_[:, :, -1]):
+    assert rel_err(got[sl], want[sl]) < CONV_RTOL
+  again = conv2d_gpu(x, w, b, 1, 'SAME', relu=True, math_mode=TC)
+  assert np.array_equal(got, again)            # deterministic
+
+
+def test_halo_conv_no_relu_affine_and_channel_window(gpu_device):
+  B, H, W, Cin, Cout = WINDOW_CASE
+  rng = np.random.default_rng(3)
+  x = rng.normal(size=(B, H, W, Cin)).astype(np.float32)
+  w = (rng.normal(size=(3, 3, Cin, Cout)) / 17).astype(np.float32)
+  b = rng.normal(size=(Cout,)).astype(np.float32)
+  sc = rng.uniform(0.5, 1.5, Cout).astype(np.float32)
+  sh = rng.normal(size=Cout).astype(np.float32)
+  want = oracle.conv2d(x, w, b, 1, 'SAME', False, np.float64) * sc + sh
+  y0 = np.full((B, H, W, 96), 7.0, np.float32)
+  got = conv2d_gpu(x, w, b, 1, 'SAME', relu=False, scale=sc, shift=sh, y_cstride=96, y_coff=32,
+                   math_mode=TC, y_init=y0)
+  assert rel_err(got[..., 32:], want) < CONV_RTOL
+  assert np.all(got[..., :32] == 7.0)          # untouched channels
 
 
 def test_ragged_expand_pair_and_partial_batch(gpu_device):

@@ -67,7 +67,7 @@ def test_shard_ranges():
 
 # ---- tensor-core kernel selection, restated from squeezedet_b200/csrc/conv_tc.cu --------------
 MAX_CHUNKS = 32          # conv_tc.cu MAX_CHUNKS: output-channel chunks per conv_tc_kernel launch
-MAX_FCHUNKS = 16         # conv_tc.cu MAX_FCHUNKS: 64-wide expand chunks per fire_tc_kernel launch
+MAX_FCHUNKS = 16         # conv_tc.cu tc_fire_plan: 64-wide expand chunks of a one-kernel fire
 
 
 def tc_pick_nt(couts, kc=32, gather=False):
@@ -105,8 +105,8 @@ def tc_conv_variant(Cin, Cout, k, stride, padding):
 
 def tc_fire_variant(Cin, S, E1, E3):
   """KCI of the fire_tc_kernel<KCI> that sqdet_fire runs with MATH_TF32X3_TC, or None when
-  tc_fused_fire_plan (conv_tc.cu) declines and the fire runs as separate convs: it takes a
-  16-channel squeeze over Cin % 16 == 0 channels with at most MAX_FCHUNKS expand chunks of 64."""
+  tc_fire_plan (conv_tc.cu) declines and the fire runs as separate convs: it takes a 16-channel
+  squeeze over Cin % 16 == 0 channels with at most MAX_FCHUNKS expand chunks of 64."""
   if Cin % 16 or Cin < 16 or S != 16:
     return None
   if -(-E1 // 64) + -(-E3 // 64) > MAX_FCHUNKS:
@@ -117,7 +117,7 @@ def tc_fire_variant(Cin, S, E1, E3):
 ALL_CONV_TC_VARIANTS = {(nt, kc, g) for nt in (64, 32, 16) for kc, g in ((32, True), (32, False),
                                                                         (16, False))}
 ALL_CONV_TC_VARIANTS.add((72, 32, False))          # conv_tc_instance: the head tile
-# the fire_tc_kernel<KCI> instantiations (tc_fused_fire_plan, conv_tc.cu)
+# the fire_tc_kernel<KCI> instantiations (tc_fire_plan, conv_tc.cu)
 ALL_FIRE_TC_VARIANTS = {32, 16}
 
 
@@ -126,9 +126,13 @@ def test_gpu_case_tables_reach_every_tc_kernel_variant():
   sides of the chunk limits, by the host rules above."""
   from test_gpu_adversarial import SHAPES
   from test_gpu_fire import FIRE_EDGE_CASES
+  from test_gpu_halo_tile import HALO_CONV_CASES, WINDOW_CASE
   from test_gpu_kernels import CONV_CASES
   conv = {tc_conv_variant(Cin, Cout, k, s, pad) for _, _, _, Cin, Cout, k, s, pad in CONV_CASES}
   assert conv - {None} == ALL_CONV_TC_VARIANTS, ALL_CONV_TC_VARIANTS - conv
+  # sqdet_conv2d would run a declined shape on the SIMT kernel: every halo-conv case is taken
+  for _, _, _, Cin, Cout in HALO_CONV_CASES + [WINDOW_CASE]:
+    assert tc_conv_variant(Cin, Cout, 3, 1, 'SAME') is not None, (Cin, Cout)
   adv = {tc_conv_variant(Cin, Cout, k, s, 'SAME') for _, _, _, Cin, Cout, k, s in SHAPES}
   assert {(16, False), (32, True)} <= {(kc, g) for _, kc, g in adv - {None}}
   assert any(v is not None and v[:2] == (32, 16) for v in adv)     # NT = 32 with KC = 16
