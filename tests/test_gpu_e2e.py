@@ -73,7 +73,7 @@ def test_layerwise_parity_small_image(net, width, height, math_mode, gpu_device)
       try:
         got = model.read_tensor(name)
       except _lib.SqdetError as exc:
-        assert exc.code == -5, exc          # fused away (e.g. fire3 when pool3 is fused)
+        assert exc.code == -5, exc          # fused away (conv1, run in one kernel with pool1)
         continue
       assert got.shape == want.shape, name
       # (1) the bar: within 1e-4 (relative to the tensor's scale) of the fp32 reference

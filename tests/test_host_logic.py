@@ -232,6 +232,40 @@ def test_gpu_case_tables_reach_every_pool_add_relu_meansub_filter_branch():
   assert any(c[5] for c in br.FILTER_CASES)                        # class ids == classes
 
 
+def conv_pool_classes(cout, k, cpad, ppad, bn, height, width):
+  """What one first-layer row reaches in conv_pool_simt_kernel (conv_pool_simt.cu): the pooled
+  size and its remainders against the 4 x 16 pooled tile (PT_H, PT_W), and the instance
+  conv_pool_instance picks (64 threads per 16 channels, NT = 384 above 256 threads)."""
+  import oracle
+  hc = oracle.conv_geometry(height, k, 2, cpad)[0]
+  wc = oracle.conv_geometry(width, k, 2, cpad)[0]
+  hp = oracle.conv_geometry(hc, 3, 2, ppad)[0]
+  wp = oracle.conv_geometry(wc, 3, 2, ppad)[0]
+  return dict(hp=hp, wp=wp, pt_h=hp % 4, pt_w=wp % 16, instance=(k, 4 * cout > 256))
+
+
+def test_first_layer_table_reaches_every_class():
+  """The fused first-layer table of test_gpu_layer_bounds reaches, across its rows: both parities
+  of H and W, every pooled height mod 4 and pooled widths with and without a ragged 16-column
+  tile, a single pooled pixel, an image smaller than one pooled tile both ways, every ksize x
+  conv padding x pool padding, all four kernel instances, and the BN epilogue."""
+  from test_gpu_layer_bounds import FIRST_LAYER_ROWS
+  rows = [(r, conv_pool_classes(*r)) for r in FIRST_LAYER_ROWS]
+  assert {r[5] % 2 for r, _ in rows} == {0, 1} and {r[6] % 2 for r, _ in rows} == {0, 1}
+  assert {c['pt_h'] for _, c in rows} == {0, 1, 2, 3}
+  assert {c['pt_w'] == 0 for _, c in rows} == {True, False}
+  assert any(c['hp'] == c['wp'] == 1 for _, c in rows)
+  assert any(c['hp'] < 4 and c['wp'] < 16 and (c['hp'], c['wp']) != (1, 1) for _, c in rows)
+  assert {(r[1], r[2], r[3]) for r, _ in rows} == {(k, cp, pp) for k in (3, 7)
+                                                     for cp in ('SAME', 'VALID')
+                                                     for pp in ('SAME', 'VALID')}
+  assert {c['instance'] for _, c in rows} == {(k, wide) for k in (3, 7) for wide in (False, True)}
+  assert all(16 <= r[0] <= 96 and r[0] % 16 == 0 for r, _ in rows)     # all fused
+  assert any(r[4] for r, _ in rows)
+  assert all(r[2] == 'SAME' for r, _ in rows if r[4])                   # _conv_bn_layer: SAME only
+  assert all(c['hp'] >= 1 and c['wp'] >= 1 for _, c in rows)
+
+
 def test_gloo_world2_allgather_roundtrip(tmp_path):
   """N>1 path on CPU: 2 processes, gloo, 127.0.0.1 — each packs its shard's detection
   blob, one all_gather, both unpack identical global results."""
