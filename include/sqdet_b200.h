@@ -131,6 +131,10 @@ int sqdet_read_tensor(sqdet_engine* e, int id, float* host_out);   /* synchronou
 int sqdet_num_ops(sqdet_engine* e);
 int sqdet_op_info(sqdet_engine* e, int index, char* name_buf, int name_cap,
                   int64_t* flops, int64_t* params, int64_t* min_bytes);
+/* The K split S the plan chose for op `index` (a ConvDet head whose K is summed by a cluster of S
+ * CTAs, see sqdet_conv2d_k_split), 1 for every other op; negative on error.  Fixed at
+ * sqdet_finalize for BATCH_SIZE images, so every sqdet_forward_n runs the same partition.     */
+int sqdet_op_k_split(sqdet_engine* e, int index);
 
 /* ---- execution: replaces sess.run([det_boxes, det_probs, det_class], feed_dict) ----
  * (src/demo.py:193-195, src/eval.py:75-77) and model.filter_prediction on every image
@@ -251,6 +255,17 @@ int sqdet_conv2d(const float* x_dev, const float* w_hwio_dev, const float* bias_
                  int B, int H, int W, int Cin, int Cout, int size, int stride,
                  int padding, int relu, int y_cstride, int y_coff, int math_mode,
                  void* stream);
+/* sqdet_conv2d with the K split of the tensor-core path chosen by the caller.  A stride-1 SAME
+ * 3x3 conv of Cin % 32 == 0 and 65..72 output channels (the ConvDet head's 72-wide tile) may sum
+ * its Cin / 32 channel chunks over a cluster of S CTAs, each taking a contiguous range of them,
+ * and add the S partial sums in rank order.  k_split 0 chooses S as the engine does (from B and
+ * the device's resident clusters; sqdet_conv2d), 1 runs unsplit, 2..4 force S (at most Cin / 32,
+ * SQDET_MATH_TF32X3_TC and such a shape only).                                               */
+int sqdet_conv2d_k_split(const float* x_dev, const float* w_hwio_dev, const float* bias_dev,
+                         const float* scale_dev, const float* shift_dev, float* y_dev,
+                         int B, int H, int W, int Cin, int Cout, int size, int stride,
+                         int padding, int relu, int y_cstride, int y_coff, int math_mode,
+                         int k_split, void* stream);
 /* SqueezeDet._fire_layer (src/nets/squeezeDet.py:81-106; same in squeezeDetPlus.py) as ONE
  * call: y[..., :E1] = relu(1x1_e1(q)+b), y[..., E1:] = relu(3x3_e3(q)+b), q = relu(1x1_s(x)+b).
  * x [B,H,W,Cin], kernels HWIO, y [B,H,W,E1+E3].  With SQDET_MATH_TF32X3_TC and a shape the

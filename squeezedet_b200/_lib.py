@@ -73,6 +73,7 @@ SIGNATURES = {
     'sqdet_read_tensor': (_i, [_vp, _i, _fp]),
     'sqdet_num_ops': (_i, [_vp]),
     'sqdet_op_info': (_i, [_vp, _i, C.c_char_p, _i, _i64p, _i64p, _i64p]),
+    'sqdet_op_k_split': (_i, [_vp, _i]),
     'sqdet_forward': (_i, [_vp, _fp, _vp]),
     'sqdet_forward_n': (_i, [_vp, _fp, _i, _vp]),
     'sqdet_forward_profiled': (_i, [_vp, _fp, _vp, _fp]),
@@ -97,6 +98,7 @@ SIGNATURES = {
                                 C.POINTER(C.c_int32)]),
     'sqdet_fire': (_i, [_fp] * 8 + [_i] * 8 + [_vp]),
     'sqdet_conv2d': (_i, [_fp, _fp, _fp, _fp, _fp, _fp] + [_i] * 12 + [_vp]),
+    'sqdet_conv2d_k_split': (_i, [_fp, _fp, _fp, _fp, _fp, _fp] + [_i] * 13 + [_vp]),
     'sqdet_maxpool_nhwc': (_i, [_fp, _fp] + [_i] * 7 + [_vp]),
     'sqdet_preprocess_u8': (_i, [_vp, _i, _i, _fp, _i, _i, _vp, _i, _vp]),
     'sqdet_interpret': (_i, [_fp, _fp, _fp, _fp, _fp] + [_i] * 7 + [_f, _vp]),

@@ -47,6 +47,12 @@
 //   between two accumulator sets: step k + 1's MMAs are issued before step k is waited for
 //   (wait_group 1) and added in, and the next A fragment is loaded and split while they run.
 //   Each chunk ends with wait_group 0 before its warp releases the stage.
+//   The 72-wide tile runs its steps one at a time in one accumulator set instead, which lets two
+//   of its CTAs share an SM.
+// K split (the 72-wide halo-mode tile only): a cluster of S CTAs along blockIdx.z shares one
+//   output tile; rank r walks a contiguous range of the conv's channel chunks, all nine taps of
+//   each, through its own ring.  The ranks then reduce their partial tiles through distributed
+//   shared memory in rank order 0, 1, ..., S - 1, each rank finishing 1/S of the tile.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -194,6 +200,23 @@ __device__ __forceinline__ void tma_load(uint32_t dst, const CUtensorMap* map, i
       "[%0], [%1, {%2, %3, %4, %5}], [%6];" ::"r"(dst),
       "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar))
       : "memory");
+}
+// every thread of every CTA of the cluster; orders each thread's shared-memory writes before the
+// other CTAs' reads after it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the four floats at this CTA's shared address `addr` as seen in the shared memory of cluster rank `rank`
+__device__ __forceinline__ float4 ld_cluster_f4(uint32_t addr, int rank) {
+  float4 v;
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %4, %5;\n\t"
+      "ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [ra];\n\t}"
+      : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+      : "r"(addr), "r"(rank)
+      : "memory");
+  return v;
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() {
@@ -380,24 +403,37 @@ __device__ __forceinline__ void flush(float (&acc)[N], float (&sum)[N], uint32_t
 // exposed per chunk, but after it no wgmma of this warpgroup reads the chunk's stage, so the
 // caller may release it.  (ptxas also serialises every wgmma of a kernel whose accumulators are
 // read in a loop that a group stays in flight across.)
-template <int NT, int KC, typename LoadA>
+//
+// PIPE = false runs one step at a time in acc[0] (wait_group 0 after each): the 72-wide tile's
+// registers then allow two CTAs per SM, and the other CTA fills the exposed MMA latency.
+template <int NT, int KC, bool PIPE = true, typename LoadA>
 __device__ __forceinline__ void mma_chunk(LoadA load_a, uint32_t bhi, float (&acc)[2][NT / 2],
                                           float (&sum)[NT / 2]) {
   constexpr int KSTEPS = KC / 8;
   uint32_t ahi[2][4], alo[2][4];
+  if constexpr (!PIPE) {
 #pragma unroll
-  for (int ks = 0; ks < KSTEPS; ++ks) {
-    const int cur = ks & 1;
-    load_a(ks, ahi[cur], alo[cur]);
-    mma_step<NT, KC>(acc[cur], ahi[cur], alo[cur], bhi, ks);
-    if (ks > 0) {
-      wgmma_wait<1>();
-      flush(acc[cur ^ 1], sum, ahi[cur ^ 1], alo[cur ^ 1]);
+    for (int ks = 0; ks < KSTEPS; ++ks) {
+      load_a(ks, ahi[0], alo[0]);
+      mma_step<NT, KC>(acc[0], ahi[0], alo[0], bhi, ks);
+      wgmma_wait<0>();
+      flush(acc[0], sum, ahi[0], alo[0]);
     }
+  } else {
+#pragma unroll
+    for (int ks = 0; ks < KSTEPS; ++ks) {
+      const int cur = ks & 1;
+      load_a(ks, ahi[cur], alo[cur]);
+      mma_step<NT, KC>(acc[cur], ahi[cur], alo[cur], bhi, ks);
+      if (ks > 0) {
+        wgmma_wait<1>();
+        flush(acc[cur ^ 1], sum, ahi[cur ^ 1], alo[cur ^ 1]);
+      }
+    }
+    constexpr int last = (KSTEPS - 1) & 1;
+    wgmma_wait<0>();
+    flush(acc[last], sum, ahi[last], alo[last]);
   }
-  constexpr int last = (KSTEPS - 1) & 1;
-  wgmma_wait<0>();
-  flush(acc[last], sum, ahi[last], alo[last]);
 }
 
 // Halo mode and the fire kernel: the CTA's 8 x FT_W output tile, of image n at (oy0, ox0)
@@ -409,13 +445,25 @@ __device__ __forceinline__ HaloTile halo_tile(int tiles_w, int tiles_h) {
   return {rest / tiles_h, rest % tiles_h * 8, tx * FT_W};
 }
 
+// Output channel c of chunk ch from its sum: bias, frozen-BN affine, ReLU.
+__device__ __forceinline__ float finish(const TcParams& p, const TcChunk& ch, int c, float v) {
+  if (p.bias) v += p.bias[ch.p_off + c];
+  if (p.scale) v = v * p.scale[ch.p_off + c] + p.shift[ch.p_off + c];
+  if (p.relu) v = fmaxf(v, 0.f);
+  return v;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Two CTAs per SM (the shared memory of 3 stages allows it up to NT = 72, KC = 32): at most 128
-// registers a thread.  The 72-wide tile needs more (108 accumulator and sum registers alone) and
-// runs one CTA per SM.
-template <int NT, int KC, int MODE>
-__global__ void __launch_bounds__(NUM_THREADS, NT == 72 ? 1 : 2)
+// registers a thread.  The 72-wide tile fits them only with one accumulator set (mma_chunk's
+// PIPE = false: 72 accumulator and sum registers instead of 108).
+//
+// KSPLIT (halo mode): launched in clusters of gridDim.z CTAs along z; rank blockIdx.z sums the
+// channel chunks [z nc / S, (z + 1) nc / S) of the conv's nc (see the file comment).
+template <int NT, int KC, int MODE, bool KSPLIT = false>
+__global__ void __launch_bounds__(NUM_THREADS, 2)
 conv_tc_kernel(const __grid_constant__ TcParams p) {
+  static_assert(!KSPLIT || MODE == TC_HALO, "the K split walks halo-mode channel chunks");
   constexpr int NACC = NT / 2;
   constexpr int WST = 2 * NT * KC;   // floats of one stage's hi + lo weight tiles
   constexpr uint32_t W_BYTES = WST * 4, TILE_BYTES = TILE_M * KC * 4, HALO_BYTES = FQ_P * KC * 4;
@@ -430,8 +478,15 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, t = lane & 3;
   const float* wch = p.w + ch.w_off;
-  const int nk = ch.nk;
+  // this CTA's K chunks [k0, k0 + nk) of the conv's ch.nk; the loop below counts them from 0
+  int k0 = 0, nk = ch.nk;
   const int taps = ch.ksize * ch.ksize;   // 1 or 9
+  if (KSPLIT) {
+    const int nc = ch.nk / taps, S = gridDim.z, z = blockIdx.z;
+    k0 = z * nc / S * taps;
+    nk = (z + 1) * nc / S * taps - k0;
+    wch += (size_t)k0 * WST;
+  }
 
   // gather mode: every thread's cp.async arrival besides the weight copy's
   if (tid == 0) ring_init(full, empty, MODE == TC_GATHER ? NUM_THREADS + 1 : 1);
@@ -486,14 +541,14 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
       if (taps == 1) {
         bytes += TILE_BYTES;
         mbar_expect_tx(&full[s], bytes);
-        tma_load(smem_u32(sa + s * TILE_M * KC), &p.amap1, j * KC, tl.ox0, tl.oy0, tl.n, &full[s]);
+        tma_load(smem_u32(sa + s * TILE_M * KC), &p.amap1, (k0 + j) * KC, tl.ox0, tl.oy0, tl.n, &full[s]);
       } else if (j % 9 == 0) {
         // channel chunk c = j / 9: its halo, into buffer c & 1, whose last reader (K chunk j - 10)
         // was released before K chunk j - STAGES was
         bytes += HALO_BYTES;
         mbar_expect_tx(&full[s], bytes);
-        tma_load(smem_u32(sa + (j / 9 & 1) * HROWS * KC), &p.amap, j / 9 * KC, tl.ox0 - 1, tl.oy0 - 1,
-                 tl.n, &full[s]);
+        tma_load(smem_u32(sa + (j / 9 & 1) * HROWS * KC), &p.amap, (k0 + j) / 9 * KC, tl.ox0 - 1,
+                 tl.oy0 - 1, tl.n, &full[s]);
       } else {
         mbar_expect_tx(&full[s], bytes);
       }
@@ -527,37 +582,68 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
       tile = sa + (c & 1) * HROWS * KC;
       prow = (r + tap / 3) * FQ_W + g + tap % 3;
     }
-    mma_chunk<NT, KC>(
+    mma_chunk<NT, KC, NT != 72>(
         [&](int ks, uint32_t(&ahi)[4], uint32_t(&alo)[4]) { load_split_swz<KC>(tile, prow, ks, t, ahi, alo); },
         smem_u32(smem + s * WST), acc, sum);
     ring_release(empty, kk);
   }
 
   // ---- epilogue: accumulator element 4j + 2h + e is (row g + 8h, column 8j + 2t + e)
+  if constexpr (KSPLIT) {
+    // this rank's partial tile, [TILE_M][NT] over the ring once every warp is done with the ring
+    static_assert(TILE_M * NT <= STAGES * (WST + TILE_M * KC), "the partial tile fits in the ring");
+    float* const part = smem;
+    __syncthreads();
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    long long m = m0 + arow0 + 8 * h;   // output pixel
-    if (MODE == TC_HALO) {
-      const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
-      const int oy = tl.oy0 + r, ox = tl.ox0 + g + 8 * h;
-      if (oy >= p.Ho || ox >= p.Wo) continue;
-      m = ((long long)tl.n * p.Ho + oy) * p.Wo + ox;
-    } else if (m >= p.M) {
-      continue;
-    }
-    float* yrow = p.y + (size_t)m * p.y_cstride + ch.y_off;
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-    for (int j = 0; j < NT / 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int c = 8 * j + 2 * t + e;
-        if (c >= ch.ncount) continue;
-        float v = sum[4 * j + 2 * h + e];
-        if (p.bias) v += p.bias[ch.p_off + c];
-        if (p.scale) v = v * p.scale[ch.p_off + c] + p.shift[ch.p_off + c];
-        if (p.relu) v = fmaxf(v, 0.f);
-        yrow[c] = v;
+      for (int j = 0; j < NT / 8; ++j)
+        *reinterpret_cast<float2*>(part + (arow0 + 8 * h) * NT + 8 * j + 2 * t) =
+            make_float2(sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
+    cluster_sync();
+    // rank z finishes the 4-channel groups [z G / S, (z + 1) G / S) of the tile's G, adding the
+    // ranks' partials in rank order
+    constexpr int G = TILE_M * NT / 4;
+    const int S = gridDim.z, z = blockIdx.z;
+    const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
+    for (int i = z * G / S + tid; i < (z + 1) * G / S; i += NUM_THREADS) {
+      const uint32_t at = smem_u32(part + 4 * i);
+      float4 v = ld_cluster_f4(at, 0);
+      for (int q = 1; q < S; ++q) {
+        const float4 u = ld_cluster_f4(at, q);
+        v.x += u.x, v.y += u.y, v.z += u.z, v.w += u.w;
       }
+      const int px = 4 * i / NT, c0 = 4 * i % NT;   // tile pixel, first channel
+      const int oy = tl.oy0 + px / FT_W, ox = tl.ox0 + px % FT_W;
+      if (oy >= p.Ho || ox >= p.Wo) continue;
+      float* yrow = p.y + (((size_t)tl.n * p.Ho + oy) * p.Wo + ox) * p.y_cstride + ch.y_off;
+      const float vs[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        if (c0 + e < ch.ncount) yrow[c0 + e] = finish(p, ch, c0 + e, vs[e]);
+    }
+    cluster_sync();   // no CTA exits while another may still read its partial tile
+  } else {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      long long m = m0 + arow0 + 8 * h;   // output pixel
+      if (MODE == TC_HALO) {
+        const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
+        const int oy = tl.oy0 + r, ox = tl.ox0 + g + 8 * h;
+        if (oy >= p.Ho || ox >= p.Wo) continue;
+        m = ((long long)tl.n * p.Ho + oy) * p.Wo + ox;
+      } else if (m >= p.M) {
+        continue;
+      }
+      float* yrow = p.y + (size_t)m * p.y_cstride + ch.y_off;
+#pragma unroll
+      for (int j = 0; j < NT / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * j + 2 * t + e;
+          if (c < ch.ncount) yrow[c] = finish(p, ch, c, sum[4 * j + 2 * h + e]);
+        }
+    }
   }
 }
 
@@ -778,6 +864,7 @@ struct TcImpl {
   int KC = 0;          // channels of a box of the input's tensor maps
   int mode = TC_ROWS;
   TcKernel kernel = nullptr;
+  int ksplit = 1;      // CTAs of a cluster that split K (kernel is then the KSPLIT instance)
   size_t smem_bytes = 0;
   std::vector<PlanGroup> groups;
   int cout_total = 0;
@@ -980,6 +1067,63 @@ static void pack_group(const TcImpl* im, const PlanGroup& g, const float* w_hwio
   }
 }
 
+// A launch of `grid` whose clusters are the S CTAs along z that split K (S = 1: no cluster).
+struct ClusterLaunch {
+  cudaLaunchAttribute attr;
+  cudaLaunchConfig_t cfg;
+  ClusterLaunch(dim3 grid, size_t smem, int S, cudaStream_t stream) : attr{}, cfg{} {
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = (unsigned)S;
+    cfg.gridDim = dim3(grid.x, grid.y, grid.z * S);
+    cfg.blockDim = dim3(NUM_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+  }
+};
+
+constexpr int MAX_KSPLIT = 4;
+constexpr int MIN_RANK_CHUNKS = 4;   // channel chunks a rank walks at the least when S is chosen
+
+// The K split of a 72-wide halo-mode plan (the ConvDet head, whose few long tiles leave a short
+// last wave: 300 tiles on 264 CTA slots at b = 20, 120 on 264 at b = 8).  forced == 0 picks, for the planned B,
+// the S in 1..MAX_KSPLIT with the fewest waves of S-CTA clusters over the device's resident
+// clusters, counting a wave of split CTAs as 1/S of a whole one and keeping the smaller S on a
+// tie, among the S that leave every rank MIN_RANK_CHUNKS channel chunks.  forced > 0 takes that
+// S, at most one rank per channel chunk.
+static int plan_ksplit(TcImpl* im, int forced) {
+  const TcKernel split = conv_tc_kernel<72, 32, TC_HALO, true>;
+  const int nc = im->prm.chunks[0].nk / 9;
+  if (forced < 0 || forced > MAX_KSPLIT || forced > nc)
+    return fail(SQDET_ERR_INVALID_ARG, "K split outside [1, min(4, channel chunks)]");
+  SQ_CUDA(cudaFuncSetAttribute(split, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)im->smem_bytes));
+  int S = forced;
+  if (!forced) {
+    int dev = 0, sms = 0, per_sm = 0;
+    SQ_CUDA(cudaGetDevice(&dev));
+    SQ_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    SQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, im->kernel, NUM_THREADS, im->smem_bytes));
+    const long long ctas = grid_blocks(im, im->prm.B) * im->prm.nchunks;
+    S = 1;
+    long long best_waves = (ctas + per_sm * sms - 1) / (per_sm * sms);
+    for (int s = 2; s <= MAX_KSPLIT && s * MIN_RANK_CHUNKS <= nc; ++s) {
+      // clusters of s resident at once: a cluster's CTAs share one GPC, whose SM count need not
+      // be a multiple of s
+      int clusters = 0;
+      const ClusterLaunch l(dim3(1), im->smem_bytes, s, nullptr);
+      SQ_CUDA(cudaOccupancyMaxActiveClusters(&clusters, split, &l.cfg));
+      if (clusters < 1) continue;
+      const long long waves = (ctas + clusters - 1) / clusters;
+      if (waves * S < best_waves * s) S = s, best_waves = waves;   // waves / s < best_waves / S
+    }
+  }
+  if (S > 1) im->kernel = split;
+  im->ksplit = S;
+  return 1;
+}
+
 // ---------------------------------------------------------------------------------------------
 bool tc_conv_eligible(int Cin, int Cout, int size, int stride, int padding) {
   // shapes this path takes: stride-1 SAME, 1x1 or 3x3, Cin a multiple of 16
@@ -988,7 +1132,7 @@ bool tc_conv_eligible(int Cin, int Cout, int size, int stride, int padding) {
 }
 
 int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, const std::vector<ConvGroup>& convs,
-                 int stride, int padding, int relu, bool has_affine, int y_cstride) {
+                 int stride, int padding, int relu, bool has_affine, int y_cstride, int k_split) {
   plan->impl = nullptr;
   const int size = convs[0].ksize;
   const bool gather = convs.size() == 1 && Cin == 3 && size == 3 && (stride == 1 || stride == 2) &&
@@ -1011,11 +1155,18 @@ int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, const std::vect
   im->kernel = conv_tc_instance(NT, KC, mode);
   im->smem_bytes = conv_smem_bytes(NT, KC);
   for (const auto& g : convs) im->groups.push_back({g, NT, KC, Cin, 0});
-  const int rc = plan_common(im, B, H, W, Cin, gh.out, gw.out, stride, gh.pad_before, gw.pad_before,
-                             relu, has_affine, y_cstride);
+  int rc = plan_common(im, B, H, W, Cin, gh.out, gw.out, stride, gh.pad_before, gw.pad_before,
+                       relu, has_affine, y_cstride);
+  if (rc > 0 && NT == 72 && mode == TC_HALO) {
+    rc = plan_ksplit(im, k_split);
+  } else if (rc > 0 && k_split > 1) {
+    rc = fail(SQDET_ERR_INVALID_ARG, "a K split needs a 72-wide 3x3 tensor-core plan");
+  }
   if (rc <= 0) tc_conv_release(plan);
   return rc;
 }
+
+int tc_conv_k_split(const TcConvPlan& plan) { return plan.impl ? plan.impl->ksplit : 1; }
 
 int tc_fire_plan(TcConvPlan* plan, int B, int H, int W, int Cin, int S, int E1, int E3) {
   plan->impl = nullptr;
@@ -1070,7 +1221,12 @@ int launch_conv_tc(const TcConvPlan& plan, const float* x_dev, float* y_dev, int
   prm.M = (long long)n * prm.Ho * prm.Wo;
   // a fire CTA walks every chunk of its tile
   const dim3 grid((unsigned)grid_blocks(im, n), im->mode == TC_FIRE ? 1u : (unsigned)prm.nchunks);
-  im->kernel<<<grid, NUM_THREADS, im->smem_bytes, stream>>>(prm);
+  if (im->ksplit > 1) {
+    const ClusterLaunch l(grid, im->smem_bytes, im->ksplit, stream);
+    SQ_CUDA(cudaLaunchKernelEx(&l.cfg, im->kernel, prm));
+  } else {
+    im->kernel<<<grid, NUM_THREADS, im->smem_bytes, stream>>>(prm);
+  }
   SQ_CHECK_LAUNCH(im->mode == TC_FIRE ? "fire_tc_kernel" : "conv_tc_kernel");
   return SQDET_OK;
 }

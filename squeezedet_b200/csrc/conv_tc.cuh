@@ -26,8 +26,13 @@ bool tc_conv_eligible(int Cin, int Cout, int size, int stride, int padding);
 
 // Returns 1 when the tensor-core path takes the convs (plan->impl set), 0 when they are left to
 // the fp32 SIMT kernel, negative on error.  Gather mode (3-channel input) takes a single conv.
+// A single 3x3 conv of 65..72 output channels (the ConvDet head) may split its K over a cluster
+// of S CTAs: k_split 0 chooses S from B and the device's resident clusters, 1..4 forces it (an
+// error for any other plan when above 1).  S stays fixed for every image count the plan runs.
 int tc_conv_plan(TcConvPlan* plan, int B, int H, int W, int Cin, const std::vector<ConvGroup>& convs,
-                 int stride, int padding, int relu, bool has_affine, int y_cstride);
+                 int stride, int padding, int relu, bool has_affine, int y_cstride, int k_split = 0);
+// The plan's K split S (1 when unsplit or not planned).
+int tc_conv_k_split(const TcConvPlan& plan);
 // The whole fire module (squeeze 1x1 -> expand 1x1 || 3x3 + concat into E1 + E3 channels) as ONE
 // kernel: the squeeze tile of each 8 x 16 output tile stays in shared memory.  Takes Cin % 16 ==
 // 0, S == 16 and at most 16 expand chunks of 64 channels; returns as tc_conv_plan.  Its convs, in

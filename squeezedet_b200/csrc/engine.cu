@@ -1057,6 +1057,16 @@ int sqdet_op_info(sqdet_engine* e, int index, char* name_buf, int name_cap, int6
   return SQDET_OK;
 }
 
+int sqdet_op_k_split(sqdet_engine* e, int index) {
+  if (!e || index < 0 || index >= (int)e->ops.size() + 2)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_op_k_split: bad index");
+  int s = 1;
+  if (index < (int)e->ops.size())
+    for (const auto& l : e->ops[index].launches)
+      if (l.kind == L_CONV_TC) s = std::max(s, tc_conv_k_split(l.tc));
+  return s;
+}
+
 int sqdet_forward(sqdet_engine* e, const float* images_dev, void* stream) {
   return sqdet_forward_n(e, images_dev, e ? e->cfg.batch_size : 0, stream);
 }
@@ -1398,7 +1408,18 @@ int sqdet_conv2d(const float* x_dev, const float* w_hwio_dev, const float* bias_
                  const float* scale_dev, const float* shift_dev, float* y_dev, int B, int H, int W,
                  int Cin, int Cout, int size, int stride, int padding, int relu, int y_cstride,
                  int y_coff, int math_mode, void* stream) {
+  return sqdet_conv2d_k_split(x_dev, w_hwio_dev, bias_dev, scale_dev, shift_dev, y_dev, B, H, W, Cin,
+                              Cout, size, stride, padding, relu, y_cstride, y_coff, math_mode, 0, stream);
+}
+
+int sqdet_conv2d_k_split(const float* x_dev, const float* w_hwio_dev, const float* bias_dev,
+                         const float* scale_dev, const float* shift_dev, float* y_dev, int B, int H,
+                         int W, int Cin, int Cout, int size, int stride, int padding, int relu,
+                         int y_cstride, int y_coff, int math_mode, int k_split, void* stream) {
   if (!x_dev || !w_hwio_dev || !y_dev) return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv2d: null pointer");
+  if (k_split < 0 || k_split > 4) return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv2d: k_split outside [0, 4]");
+  if (k_split > 1 && math_mode != SQDET_MATH_TF32X3_TC)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv2d: a K split needs SQDET_MATH_TF32X3_TC");
   if (padding != SQDET_PAD_SAME && padding != SQDET_PAD_VALID)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv2d: padding must be SAME(0) or VALID(1)");
   if (int rc = check_conv_epilogue("sqdet_conv2d", scale_dev, shift_dev, Cout, y_cstride, y_coff))
@@ -1408,10 +1429,12 @@ int sqdet_conv2d(const float* x_dev, const float* w_hwio_dev, const float* bias_
   if (math_mode == SQDET_MATH_TF32X3_TC) {
     TcConvPlan plan;
     int rc = tc_conv_plan(&plan, B, H, W, Cin, {{size, Cout, y_coff}}, stride, padding, relu,
-                          scale_dev != nullptr, y_cstride);
+                          scale_dev != nullptr, y_cstride, k_split);
     if (rc >= 0)
       rc = tc_conv_oneshot(&plan, {w_hwio_dev}, {bias_dev}, scale_dev, shift_dev, x_dev, y_dev,
                            (cudaStream_t)stream);
+    if (rc == 1 && k_split > 1)
+      return fail(SQDET_ERR_INVALID_ARG, "sqdet_conv2d: a K split needs a shape the tensor-core path takes");
     if (rc != 1) return rc;   // 1 = shape not taken by the tensor-core path (e.g. a strided conv)
   }
   // the fp32 SIMT kernel: the same dispatch as the engine

@@ -508,6 +508,17 @@ class ModelSkeleton:
       rows.append((buf.value.decode(), fl.value, pa.value, by.value))
     return rows
 
+  def op_k_splits(self):
+    """{op name: S} for the ops whose K the plan splits over a cluster of S > 1 CTAs."""
+    out = {}
+    for i, (name, _, _, _) in enumerate(self.op_table()):
+      s = self._lib.sqdet_op_k_split(self._engine, i)
+      if s < 0:
+        _lib.check(s)
+      if s > 1:
+        out[name] = s
+    return out
+
   def results_device(self):
     """Device pointers of the last forward's results: dict of ints + max_dets."""
     ptrs = [C.c_void_p() for _ in range(5)]
