@@ -1,18 +1,299 @@
-"""Helpers for the -m gpu parity tests: every call goes through the C ABI."""
+"""Helpers shared by the tests: engines and forwards, the fp64 oracles and their per-element
+bound, and stage-isolated calls of the C ABI."""
 import ctypes as C
 
 import numpy as np
+import pytest
 
+import oracle
+from oracle import preproc
+from oracle.torch_port import TorchForward
 from squeezedet_b200 import _lib
+from squeezedet_b200 import config as cfg
 from squeezedet_b200._lib import DeviceBuffer
+from squeezedet_b200.nets import SqueezeDet, SqueezeDetPlus, VGG16ConvDet, ResNet50ConvDet
+from squeezedet_b200.nets.squeezeDet import FireNetBase
+from squeezedet_b200.utils import synth
+
+NETS = {
+    'squeezeDet': (SqueezeDet, cfg.kitti_squeezeDet_config),
+    'squeezeDet+': (SqueezeDetPlus, cfg.kitti_squeezeDetPlus_config),
+    'vgg16': (VGG16ConvDet, cfg.kitti_vgg16_config),
+    'resnet50': (ResNet50ConvDet, cfg.kitti_res50_config),
+}
+MODES = [_lib.MATH_FP32_SIMT, _lib.MATH_TF32X3_TC]
+
+# Tolerances (BASELINE.json north_star): scores and box coordinates within 1e-4 relative;
+# class ids / kept-box indices exact wherever the oracle's own margin exceeds fp noise.
+TOL = 1e-4
+
+ERR_NOT_FOUND = -5          # SQDET_ERR_NOT_FOUND: tensor fused into its consumer
+POST_LAUNCHES = 2           # interpret + filter (sqdet_launches_per_forward)
+FIRE_TILE_H, FIRE_TILE_W = 8, 16
+# The engine runs a fire as one kernel when the squeeze is <= 16 wide and the grid holds at least
+# 4 tiles per SM.  H100 SXM has 132 SMs, H100 PCIe 114: sizes below stay on one side of the rule
+# on both.
+ONE_KERNEL_MIN_TILES = 4 * 132
+PAIR_MAX_TILES = 4 * 114
 
 
+def fire_tiles(batch, h, w):
+  return batch * -(-h // FIRE_TILE_H) * -(-w // FIRE_TILE_W)
+
+
+# ---- engines -------------------------------------------------------------------------------------
+def make_mc(net, width, height, batch):
+  mc = NETS[net][1]()
+  mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT, mc.BATCH_SIZE = width, height, batch
+  rows = oracle.layer_table(net, height, width)
+  mc.GRID_H, mc.GRID_W = rows[-1][2][0], rows[-1][2][1]
+  mc.ANCHOR_BOX = cfg.set_anchors(mc)
+  mc.ANCHORS = len(mc.ANCHOR_BOX)
+  return mc
+
+
+def make_net(net, width, height, batch, device, math_mode=None, seed=0):
+  """(model, weights): benchmark net `net` with synthetic weights `seed` loaded.  The weight table
+  of synth.model_param_specs(model) is the one of oracle.param_specs(net)."""
+  model = NETS[net][0](make_mc(net, width, height, batch), device, math_mode=math_mode)
+  weights = synth.synthetic_weights(synth.model_param_specs(model), seed=seed)
+  model.load_weights(weights)
+  return model, weights
+
+
+class TableNet(FireNetBase):
+  """FireNetBase over any BODY.  Conv rows named in `bn_convs` become _conv_bn_layer (conv +
+  bias + frozen BN + ReLU, ResNet-50's first layer)."""
+
+  def __init__(self, mc, body, bn_convs=(), gpu_id=0, math_mode=None):
+    self.BODY = tuple(body)
+    self.bn_convs = set(bn_convs)
+    FireNetBase.__init__(self, mc, gpu_id, math_mode)
+
+  def _conv_layer(self, layer_name, inputs, filters, size, stride, padding='SAME', **kw):
+    if layer_name in self.bn_convs:
+      return self._conv_bn_layer(inputs, layer_name, 'bn_' + layer_name, 'scale_' + layer_name,
+                                 filters, size, stride, padding, relu=True, conv_with_bias=True)
+    return FireNetBase._conv_layer(self, layer_name, inputs, filters, size, stride, padding, **kw)
+
+
+def body_grid(body, height, width):
+  """(H, W) of the body's last tensor (= the ConvDet head's grid)."""
+  h, w = height, width
+  for row in body:
+    if row[0] in ('conv', 'pool'):
+      k, s, pad = row[-3:]
+      h = oracle.conv_geometry(h, k, s, pad)[0]
+      w = oracle.conv_geometry(w, k, s, pad)[0]
+  return h, w
+
+
+def build(body, batch, height, width, math_mode, device, bn_convs=()):
+  """(mc, model, weights) of a TableNet over `body` with synthetic weights."""
+  mc = cfg.kitti_squeezeDet_config()
+  mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT, mc.BATCH_SIZE = width, height, batch
+  mc.GRID_H, mc.GRID_W = body_grid(body, height, width)
+  mc.ANCHOR_BOX = cfg.set_anchors(mc)
+  mc.ANCHORS = len(mc.ANCHOR_BOX)
+  model = TableNet(mc, body, bn_convs, device, math_mode=math_mode)
+  weights = synth.synthetic_weights(synth.model_param_specs(model), seed=7)
+  model.load_weights(weights)
+  return mc, model, weights
+
+
+def engine_tensor(model, name):
+  """Handle of any engine tensor by name, including ones the Python net does not register
+  (a fire's squeeze output)."""
+  lib = model._lib
+  buf = C.create_string_buffer(256)
+  for tid in range(lib.sqdet_num_tensors(model._engine)):
+    _lib.check(lib.sqdet_tensor_info(model._engine, tid, buf, 256, None))
+    if buf.value.decode() == name:
+      return model._new_tensor(name, tid)
+  raise KeyError(name)
+
+
+def read_tensors(model, names):
+  return {nm: model.read_tensor(engine_tensor(model, nm)) for nm in names}
+
+
+def assert_fused_away(model, name):
+  with pytest.raises(_lib.SqdetError) as exc:
+    model.read_tensor(engine_tensor(model, name))
+  assert exc.value.code == ERR_NOT_FOUND, exc.value
+
+
+def forward_n(model, images, n=None, stream=None):
+  """forward_device of the first n images (all with n = None) from a device buffer that holds
+  just those images, then a sync of `stream` (None: the legacy stream, never graph-captured)."""
+  x = images if n is None else images[:n]
+  buf = DeviceBuffer.from_numpy(np.ascontiguousarray(x, np.float32), model.gpu_id)
+  model.forward_device(buf.ptr, stream, n)
+  _lib.check(model._lib.sqdet_stream_sync(model.gpu_id, stream))
+  buf.free()
+
+
+def assert_rows_equal(got, full, n, *what):
+  """Rows [0, n) of each array of an n-image forward bitwise those of the full forward."""
+  for key, want in full.items():
+    assert got[key][:n].tobytes() == want[:n].tobytes(), (key, n) + what
+
+
+RESULTS = (('det_boxes', np.float32, 4), ('det_probs', np.float32, None),
+           ('det_class', np.int64, None))
+
+
+def fetch_results(model, device):
+  """Every device result buffer of the engine, all B rows."""
+  B, A = model.det_probs.shape
+  res = model.results_device()
+  lib = model._lib
+  out = {}
+  for key, dtype, last in RESULTS:
+    out[key] = np.empty((B, A, last) if last else (B, A), dtype)
+  out['dets'] = np.empty((B, res['max_dets']), _lib.DET_DTYPE)
+  out['counts'] = np.empty((B,), np.int32)
+  _lib.check(lib.sqdet_stream_sync(device, None))
+  for key, arr in out.items():
+    _lib.check(lib.sqdet_memcpy_d2h(arr.ctypes.data, res[key], arr.nbytes, None))
+  _lib.check(lib.sqdet_stream_sync(device, None))
+  return out
+
+
+# ---- the per-element fp64 bound ------------------------------------------------------------------
+# Forward-error bar in units of sum |products|, for K products per output: fp32 round-to-nearest
+# accumulation random-walks to ~ sqrt(K) * 2^-24 (measured 2.7e-6 at K = 2304 on all-positive
+# operands with the FFMA kernel); the 3xTF32 path drops terms of 2^-21 per product.  One bar for
+# both math modes:
+def adv_tol(K):
+  return 1.2e-7 * np.sqrt(K)
+
+
+def bound_ratio(got, want64, bar):
+  """|got - want64| / bar per element: 0 where the error is 0, inf where got is NaN or a non-zero
+  error meets a zero bar."""
+  err = np.abs(np.asarray(got, np.float64) - want64)
+  with np.errstate(divide='ignore', invalid='ignore'):
+    ratio = np.where(err > 0, err / bar, 0.0)
+  ratio[np.isnan(err)] = np.inf
+  return ratio
+
+
+def assert_within_bound(got, want64, bar, K, what):
+  """|got - want64| < adv_tol(K) * bar everywhere; a failure names the worst element."""
+  ratio = bound_ratio(got, want64, bar)
+  worst = np.unravel_index(np.argmax(ratio), ratio.shape)
+  assert ratio[worst] < adv_tol(K), (what, 'element', tuple(int(i) for i in worst),
+                                     float(ratio[worst]), adv_tol(K))
+
+
+def conv_oracle(x, w, b=None, stride=1, padding='SAME', relu=False, scale=None, shift=None):
+  """(fp64 conv, its bar): relu?(conv(x, w) + b) [* scale + shift], and |x| (*) |w| + |b|
+  [* |scale| + |shift|], the scale that bounds any fp32 summation of the products.  ReLU is
+  1-Lipschitz, so it leaves the bar as it is."""
+  want = oracle.conv2d(x, w, b, stride, padding, False, np.float64)
+  bar = oracle.conv2d(np.abs(x), np.abs(w), None if b is None else np.abs(b), stride, padding,
+                      False, np.float64)
+  if scale is not None:
+    want, bar = want * scale + shift, bar * np.abs(scale) + np.abs(shift)
+  if relu:
+    want = np.maximum(want, 0)
+  return want, bar
+
+
+def fire_oracle(x, ws, bs, w1, b1, w3, b3, dtype):
+  q = oracle.conv2d(x, ws, bs, 1, 'SAME', True, dtype)
+  a = oracle.conv2d(q, w1, b1, 1, 'SAME', True, dtype)
+  b = oracle.conv2d(q, w3, b3, 1, 'SAME', True, dtype)
+  return np.concatenate([a, b], axis=3)
+
+
+def fire_error_bound(x, ws, w1, w3, q64):
+  """Per-element scale of the error of squeeze -> ReLU -> expand in any fp32 summation order:
+  the expand's own rounding, tol * (|q| (*) |w_e|), plus the squeeze's error carried through the
+  expand, tol * ((|x| (*) |w_s|) (*) |w_e|); ReLU is 1-Lipschitz, so it cannot amplify the
+  squeeze error."""
+  def conv(a, w):
+    return oracle.conv2d(a, w, None, 1, 'SAME', False, np.float64)
+  sx = conv(np.abs(x), np.abs(ws))
+  return np.concatenate([conv(np.abs(q64), np.abs(w1)) + conv(sx, np.abs(w1)),
+                         conv(np.abs(q64), np.abs(w3)) + conv(sx, np.abs(w3))], axis=3)
+
+
+# ---- detections ----------------------------------------------------------------------------------
+def assert_boxes_close(got, ref32, ref64):
+  """Box coordinates: within 1e-4 relative of the fp32 reference, plus the reference's OWN
+  fp32 uncertainty (|ref32 - ref64|, x4) — boxes that clip from ~4000 px wide pre-clip values
+  carry ~1e-3 px of fp32 rounding in any implementation — plus 4e-3 px absolute (3e-6 of the
+  image width)."""
+  got = np.asarray(got, np.float64)
+  tol = TOL * np.abs(ref32) + 4.0 * np.abs(np.asarray(ref32, np.float64) - ref64) + 4e-3
+  bad = np.abs(got - ref32) > tol
+  assert not bad.any(), (int(bad.sum()), float(np.abs(got - ref32)[bad].max()))
+
+
+def make_png(path, h, w, seed):
+  """A frame with structure (rectangles on noise) so detections spread over the image."""
+  import cv2
+  rng = np.random.default_rng(seed)
+  im = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+  for _ in range(12):
+    y0, x0 = int(rng.integers(0, h - 40)), int(rng.integers(0, w - 80))
+    im[y0:y0 + int(rng.integers(20, 120)), x0:x0 + int(rng.integers(40, 300))] = \
+        rng.integers(0, 256, 3, dtype=np.uint8)
+  assert cv2.imwrite(path, im)
+  return im
+
+
+def make_kitti(root):
+  """A KITTI tree under `root` of three full-size frames, each with one label: (data directory,
+  image ids, {id: frame})."""
+  data = root / 'KITTI'
+  (data / 'training' / 'image_2').mkdir(parents=True)
+  (data / 'training' / 'label_2').mkdir(parents=True)
+  (data / 'ImageSets').mkdir()
+  ids, frames = [], {}
+  for k, (h, w) in enumerate([(375, 1242), (370, 1224), (376, 1241)]):
+    idx = '%06d' % k
+    ids.append(idx)
+    frames[idx] = make_png(str(data / 'training' / 'image_2' / (idx + '.png')), h, w, seed=20 + k)
+    (data / 'training' / 'label_2' / (idx + '.txt')).write_text(
+        'Car 0.00 0 -1.57 100.00 120.00 300.00 250.00 1.5 1.6 3.9 1.0 1.7 10.0 -1.5\n')
+  (data / 'ImageSets' / 'val.txt').write_text('\n'.join(ids) + '\n')
+  return data, ids, frames
+
+
+def oracle_pipeline(net, mc, weights, frame_u8, order, rescale):
+  """The reference pipeline on one frame: oracle pre-processing (pinned to cv2) -> torch-CPU
+  forward -> interpret_output -> [rescale ALL boxes, eval.py:83-84] -> filter_prediction.
+  Returns the filtered (boxes, probs, classes) and whether the top-66 scores hold a near tie."""
+  fed = preproc.preprocess(frame_u8, mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT, mc.BGR_MEANS, order)
+  preds = TorchForward(net, weights)(fed[None])
+  boxes, probs, cls = oracle.interpret_output(preds, mc.ANCHOR_BOX, mc.CLASSES,
+                                              mc.ANCHOR_PER_GRID, mc.IMAGE_WIDTH,
+                                              mc.IMAGE_HEIGHT, mc.EXP_THRESH)
+  boxes, probs, cls = boxes[0].copy(), probs[0], cls[0]
+  if rescale:
+    # eval.py:72-74,83-84 (scales are Python floats; numpy divides the float32 array in float32)
+    x_scale = mc.IMAGE_WIDTH / float(frame_u8.shape[1])
+    y_scale = mc.IMAGE_HEIGHT / float(frame_u8.shape[0])
+    boxes[:, 0::2] /= x_scale
+    boxes[:, 1::2] /= y_scale
+  fb, fp, fc, src = oracle.filter_prediction(boxes, probs, cls, mc.CLASSES, mc.TOP_N_DETECTION,
+                                             mc.PROB_THRESH, mc.NMS_THRESH)
+  order66 = np.argsort(-probs.astype(np.float64), kind='stable')[:66]
+  top = probs[order66].astype(np.float64)
+  gap = np.abs(top[:, None] - top[None, :]) <= 10 * TOL * top[:, None]
+  np.fill_diagonal(gap, False)
+  return fb, fp, fc, bool(gap.any())
+
+
+# ---- stage-isolated calls ------------------------------------------------------------------------
 def conv2d_gpu(x, w, b=None, stride=1, padding='SAME', relu=True, scale=None, shift=None,
                y_cstride=None, y_coff=0, math_mode=0, device=0, y_init=None):
   lib = _lib.load()
   B, H, W, Cin = x.shape
   k, _, _, Cout = w.shape
-  import oracle
   Ho = oracle.conv_geometry(H, k, stride, padding)[0]
   Wo = oracle.conv_geometry(W, k, stride, padding)[0]
   cs = y_cstride or Cout
@@ -34,7 +315,6 @@ def maxpool_gpu(x, k, stride, padding, device=0, offset=0):
   """sqdet_maxpool_nhwc; `offset` > 0 places x and y that many floats into larger buffers (an
   offset of 1 leaves both pointers 4 bytes past 16-byte alignment)."""
   lib = _lib.load()
-  import oracle
   B, H, W, Cc = x.shape
   Ho = oracle.conv_geometry(H, k, stride, padding)[0]
   Wo = oracle.conv_geometry(W, k, stride, padding)[0]

@@ -21,12 +21,11 @@ import torch
 import oracle
 from squeezedet_b200 import _lib
 from squeezedet_b200.utils import synth
-from test_gpu_dispatch import assert_fused_away, fire_tiles
-from test_gpu_e2e import MODES, NETS, make_mc
+from gpu_util import MODES, assert_fused_away, fire_tiles, forward_n, make_net
 
 pytestmark = pytest.mark.gpu
 
-SPIN_CYCLES = 400_000_000        # about 0.2 s at 1.98 GHz
+SPIN_CYCLES = 1_000_000_000      # 0.5 s at 1.98 GHz, longer at the clocks of a power-capped card
 W1, W2 = 31, 32                  # weight seeds before and after a reload
 # (height, width, batch).  SqueezeDet: fire2 and fire3 read 3 x 12 x 20 = 720 tiles of pool1's
 # output, at least 4 per SM, so on tensor cores each runs as one kernel with its own weight pack.
@@ -47,14 +46,10 @@ def engine(net, mode, seed, device, size=None, scales=None):
   """An engine with weights `seed`, warmed by one forward on the legacy stream.  That forward is
   ordered behind the parameter uploads, so nothing is in flight afterwards."""
   h, w, b = size or SIZES[net]
-  model = NETS[net][0](make_mc(net, w, h, b), device, math_mode=mode)
-  model.load_weights(weights(net, seed))
+  model, _ = make_net(net, w, h, b, device, mode, seed)
   if scales is not None:
     model.set_box_scale(scales)
-  x = _lib.DeviceBuffer.from_numpy(np.zeros((b, h, w, 3), np.float32), device)
-  model.forward_device(x.ptr, None)
-  sync(model, None)
-  x.free()
+  forward_n(model, np.zeros((b, h, w, 3), np.float32))
   return model
 
 
@@ -75,7 +70,7 @@ def fresh():
 
 class Hold:
   """A bounded spin queued on `stream`: what is enqueued behind it stays in flight until the spin
-  ends, about 0.2 s later."""
+  ends, about 0.5 s later."""
 
   def __init__(self, stream, device):
     s = torch.cuda.ExternalStream(stream, device=device)
@@ -256,9 +251,10 @@ def test_reload_with_forwards_in_flight(net, math_mode, path, fresh, gpu_device)
   for i in (0, 1):                 # both submissions once: graphs captured, buffers sized
     run.enqueue(i)
   run.finish()
+  w2 = weights(net, W2)            # outside the hold: ResNet-50's table takes over 0.2 s to make
   hold = Hold(run.stream, gpu_device)
   run.enqueue(0)
-  model.load_weights(weights(net, W2))
+  model.load_weights(w2)
   hold.assert_active('the reload')
   run.enqueue(1)
   run.finish()
@@ -353,8 +349,9 @@ def test_waits_cover_only_the_engines_own_work(gpu_device):
   foreign = torch.cuda.Stream(device=gpu_device)
   stream = model.engine_stream()
   assert foreign.cuda_stream != stream
+  w2 = weights('squeezeDet', W2)
   hold = Hold(foreign.cuda_stream, gpu_device)
-  model.load_weights(weights('squeezeDet', W2))
+  model.load_weights(w2)
   model.forward_device(x.ptr, stream)
   r.copy(model, stream)
   sync(model, stream)

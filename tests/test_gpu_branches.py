@@ -15,12 +15,8 @@ import oracle
 from squeezedet_b200 import _lib
 from squeezedet_b200 import config as cfg
 from squeezedet_b200.nn_skeleton import ModelSkeleton
-from squeezedet_b200.nets import SqueezeDet
 from squeezedet_b200.utils import synth
-from gpu_util import topk_nms_gpu
-from test_gpu_dispatch import build
-from test_gpu_e2e import MODES, make_mc
-from test_gpu_partial import fetch_results
+from gpu_util import build, fetch_results, make_net, topk_nms_gpu
 
 pytestmark = pytest.mark.gpu
 ERR_INVALID_ARG = -1
@@ -94,10 +90,9 @@ def test_filter_capacity_edges(case, gpu_device):
 def test_full_squeezedet_1600x480_uncached_filter(gpu_device):
   """SqueezeDet at 1600x480 has 27000 anchors, past the 24576 whose scores the filter keeps in
   registers: the GPU filter on the engine's own det tensors equals the oracle's on them."""
-  mc = make_mc('squeezeDet', 1600, 480, 1)
+  model, _ = make_net('squeezeDet', 1600, 480, 1, gpu_device, seed=0)
+  mc = model.mc
   assert mc.ANCHORS == 27000
-  model = SqueezeDet(mc, gpu_device)
-  model.load_weights(synth.synthetic_weights(synth.model_param_specs(model), seed=0))
   images = synth.synthetic_images(1, 480, 1600, seed=77)
   boxes, probs, cls, dets, counts = model.detect(images, want_dets=True)
   assert 0 < mc.TOP_N_DETECTION < mc.ANCHORS

@@ -2,16 +2,15 @@
 one output tile, each rank sums a contiguous range of the conv's 32-channel chunks, and the ranks
 add their partial tiles in rank order through distributed shared memory.  The engine chooses S
 from its batch and the device's resident clusters; sqdet_conv2d_k_split forces it.  Each element
-is checked against the fp64 oracle with the bar of test_gpu_adversarial, repeat runs bitwise, and
+is checked against the fp64 oracle with the bar gpu_util.adv_tol, repeat runs bitwise, and
 forwards of fewer images than the engine's batch bitwise against the full batch's rows."""
 import numpy as np
 import pytest
 
-import oracle
 from squeezedet_b200 import _lib
 from squeezedet_b200.utils import synth
-from test_gpu_adversarial import adv_tol
-from test_gpu_e2e import NETS, make_mc
+from gpu_util import (assert_rows_equal, assert_within_bound, conv_oracle, fetch_results,
+                      forward_n, make_net)
 
 pytestmark = pytest.mark.gpu
 TC = _lib.MATH_TF32X3_TC
@@ -54,16 +53,12 @@ def test_forced_k_split_vs_oracle(case, k_split, gpu_device):
   affine = cs != Cout
   sc = rng.uniform(0.5, 1.5, Cout).astype(np.float32) if affine else None
   sh = rng.normal(size=Cout).astype(np.float32) if affine else None
-  want = oracle.conv2d(x, w, b, 1, 'SAME', False, np.float64)
-  bound = oracle.conv2d(np.abs(x), np.abs(w), np.abs(b), 1, 'SAME', False, np.float64)
-  if affine:
-    want, bound = want * sc + sh, bound * sc + np.abs(sh)
+  want, bound = conv_oracle(x, w, b, scale=sc, shift=sh)
   got = conv_k_split(x, w, b, k_split, scale=sc, shift=sh, y_cstride=cs, y_coff=coff,
                      device=gpu_device)
   win = got[..., coff:coff + Cout]
   assert not np.isnan(win).any()
-  ratio = np.abs(win.astype(np.float64) - want) / np.maximum(bound, 1e-30)
-  assert ratio.max() < adv_tol(9 * Cin), (case, k_split, float(ratio.max()))
+  assert_within_bound(win, want, bound, 9 * Cin, (case, k_split))
   assert np.all(got[..., :coff] == 7.0) and np.all(got[..., coff + Cout:] == 7.0)
   again = conv_k_split(x, w, b, k_split, scale=sc, shift=sh, y_cstride=cs, y_coff=coff,
                        device=gpu_device)
@@ -85,33 +80,12 @@ def test_k_split_rejected_where_not_planned(gpu_device):
     assert exc.value.code == -1, (cout, k_split)
 
 
-def engine(net, width, height, batch, device, seed=5):
-  mc = make_mc(net, width, height, batch)
-  model = NETS[net][0](mc, device)
-  model.load_weights(synth.synthetic_weights(synth.model_param_specs(model), seed=seed))
-  return model
-
-
 def forward(model, images, n, device):
-  buf = _lib.DeviceBuffer.from_numpy(np.ascontiguousarray(images[:n], np.float32), device)
-  model.forward_device(buf.ptr, None, n)
-  _lib.check(model._lib.sqdet_stream_sync(device, None))
-  buf.free()
-  res = model.results_device()
-  B, A = model.mc.BATCH_SIZE, model.mc.ANCHORS
-  out = {'preds': model.read_tensor(model.preds)}
-  for key, dtype, shape in (('det_probs', np.float32, (B, A)), ('det_boxes', np.float32, (B, A, 4)),
-                            ('det_class', np.int64, (B, A))):
-    a = np.empty(shape, dtype)
-    _lib.check(model._lib.sqdet_memcpy_d2h(a.ctypes.data, res[key], a.nbytes, None))
-    out[key] = a
-  _lib.check(model._lib.sqdet_stream_sync(device, None))
-  return out
-
-
-def assert_rows_equal(got, want, n):
-  for key in want:
-    assert got[key][:n].tobytes() == want[key][:n].tobytes(), (key, n)
+  """The head's output and the det tensors of a forward of the first n images."""
+  forward_n(model, images, n)
+  res = fetch_results(model, device)
+  return {'preds': model.read_tensor(model.preds),
+          **{key: res[key] for key in ('det_probs', 'det_boxes', 'det_class')}}
 
 
 def test_squeezedet_head_splits_at_the_benchmark_size(gpu_device):
@@ -119,7 +93,7 @@ def test_squeezedet_head_splits_at_the_benchmark_size(gpu_device):
   wave idle, so the plan splits the head's K.  Two forwards are bitwise equal, and a forward
   of 7 images gives bitwise the first 7 rows of the full batch."""
   B, H, W = 20, 375, 1242
-  model = engine('squeezeDet', W, H, B, gpu_device)
+  model, _ = make_net('squeezeDet', W, H, B, gpu_device, seed=5)
   splits = model.op_k_splits()
   assert list(splits) == ['conv12'] and splits['conv12'] > 1, splits
   images = synth.synthetic_images(B, H, W, seed=2)
@@ -132,7 +106,7 @@ def test_squeezedet_head_splits_at_the_benchmark_size(gpu_device):
 def test_only_the_head_splits(net, gpu_device):
   """At b = 8 the 120 head tiles fill fewer than half of the two CTA slots per SM, so the plan
   splits the head's K; no other op of the net is planned with a split."""
-  model = engine(net, 1242, 375, 8, gpu_device)
+  model, _ = make_net(net, 1242, 375, 8, gpu_device, seed=5)
   splits = model.op_k_splits()
   head = model.op_table()[-3][0]          # the last plan op, before interpret and filter
   assert list(splits) == [head] and 1 < splits[head] <= 4, splits
@@ -142,7 +116,7 @@ def test_split_head_rows_follow_full_batch(gpu_device):
   """A small grid (2 head tiles an image) splits the head four ways; forwards of n = 1, 2 of the
   3 images, and a repeat of the full batch, give bitwise the full forward's rows."""
   B, H, W = 3, 96, 320
-  model = engine('squeezeDet', W, H, B, gpu_device, seed=8)
+  model, _ = make_net('squeezeDet', W, H, B, gpu_device, seed=8)
   assert model.op_k_splits().get('conv12', 1) > 1
   images = synth.synthetic_images(B, H, W, seed=4)
   full = forward(model, images, B, gpu_device)

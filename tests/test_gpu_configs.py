@@ -9,8 +9,7 @@ import oracle
 from oracle.torch_port import TorchForward
 from squeezedet_b200 import _lib
 from squeezedet_b200.utils import synth
-from gpu_util import assert_classes_match
-from test_gpu_e2e import NETS, TOL, assert_boxes_close, make_mc
+from gpu_util import TOL, assert_boxes_close, assert_classes_match, make_mc, make_net
 
 pytestmark = pytest.mark.gpu
 
@@ -47,9 +46,9 @@ def test_baseline_config_detections(net, batch, math_mode, gpu_device):
   mc, weights, images, (p32, (wb, wp, wc)), (p64, (wb64, _, _)) = oracle_at_config(net, batch)
   grid = {'squeezeDet+': (22, 76)}.get(net, (24, 78))
   assert (mc.GRID_H, mc.GRID_W) == grid and mc.ANCHORS == grid[0] * grid[1] * 9
-  model = NETS[net][0](mc, gpu_device, math_mode=math_mode)
+  model, model_weights = make_net(net, 1242, 375, batch, gpu_device, math_mode, seed=0)
   assert [n for n, _ in synth.model_param_specs(model)] == [n for n, _ in oracle.param_specs(net)]
-  model.load_weights(weights)
+  assert all(model_weights[n].tobytes() == weights[n].tobytes() for n in weights)
   boxes, probs, cls, dets, counts = model.detect(images, want_dets=True)
   assert boxes.shape == (batch, mc.ANCHORS, 4) and cls.dtype == np.int64
   # scores / boxes within 1e-4 relative of the fp32 reference semantics

@@ -7,70 +7,17 @@ chained numpy oracle, and launches_per_forward() tells which kernel path each op
     squeeze conv + expand pair (two launches), and the SIMT path (three launches).
 Bar per tensor (test_gpu_e2e.test_layerwise_parity_small_image): within 1e-4 of the fp32
 reference, and no further from fp64 than 4x the fp32 reference's own distance."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import oracle
 from squeezedet_b200 import _lib
-from squeezedet_b200 import config as cfg
-from squeezedet_b200.nets.squeezeDet import FireNetBase
 from squeezedet_b200.utils import synth
-from gpu_util import rel_err
-from test_gpu_fire import fire_oracle
+from gpu_util import (MODES, ONE_KERNEL_MIN_TILES, PAIR_MAX_TILES, POST_LAUNCHES, TOL,
+                      assert_fused_away, body_grid, build, engine_tensor, fire_oracle, fire_tiles,
+                      rel_err)
 
 pytestmark = pytest.mark.gpu
-
-MODES = [_lib.MATH_FP32_SIMT, _lib.MATH_TF32X3_TC]
-TOL = 1e-4
-ERR_NOT_FOUND = -5          # SQDET_ERR_NOT_FOUND: tensor fused into its consumer
-POST_LAUNCHES = 2           # interpret + filter (sqdet_launches_per_forward)
-FIRE_TILE_H, FIRE_TILE_W = 8, 16
-# The engine runs a fire as one kernel when the squeeze is <= 16 wide and the grid holds at least
-# 4 tiles per SM.  H100 SXM has 132 SMs, H100 PCIe 114: sizes below stay on one side of the rule
-# on both.
-ONE_KERNEL_MIN_TILES = 4 * 132
-PAIR_MAX_TILES = 4 * 114
-
-
-class TableNet(FireNetBase):
-  """FireNetBase over any BODY.  Conv rows named in `bn_convs` become _conv_bn_layer (conv +
-  bias + frozen BN + ReLU, ResNet-50's first layer)."""
-
-  def __init__(self, mc, body, bn_convs=(), gpu_id=0, math_mode=None):
-    self.BODY = tuple(body)
-    self.bn_convs = set(bn_convs)
-    FireNetBase.__init__(self, mc, gpu_id, math_mode)
-
-  def _conv_layer(self, layer_name, inputs, filters, size, stride, padding='SAME', **kw):
-    if layer_name in self.bn_convs:
-      return self._conv_bn_layer(inputs, layer_name, 'bn_' + layer_name, 'scale_' + layer_name,
-                                 filters, size, stride, padding, relu=True, conv_with_bias=True)
-    return FireNetBase._conv_layer(self, layer_name, inputs, filters, size, stride, padding, **kw)
-
-
-def body_grid(body, height, width):
-  """(H, W) of the body's last tensor (= the ConvDet head's grid)."""
-  h, w = height, width
-  for row in body:
-    if row[0] in ('conv', 'pool'):
-      k, s, pad = row[-3:]
-      h = oracle.conv_geometry(h, k, s, pad)[0]
-      w = oracle.conv_geometry(w, k, s, pad)[0]
-  return h, w
-
-
-def build(body, batch, height, width, math_mode, device, bn_convs=()):
-  mc = cfg.kitti_squeezeDet_config()
-  mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT, mc.BATCH_SIZE = width, height, batch
-  mc.GRID_H, mc.GRID_W = body_grid(body, height, width)
-  mc.ANCHOR_BOX = cfg.set_anchors(mc)
-  mc.ANCHORS = len(mc.ANCHOR_BOX)
-  model = TableNet(mc, body, bn_convs, device, math_mode=math_mode)
-  weights = synth.synthetic_weights(synth.model_param_specs(model), seed=7)
-  model.load_weights(weights)
-  return mc, model, weights
 
 
 def oracle_layers(body, weights, images, dtype, bn_convs=(), eps=1e-5):
@@ -103,30 +50,12 @@ def oracle_layers(body, weights, images, dtype, bn_convs=(), eps=1e-5):
   return out
 
 
-def engine_tensor(model, name):
-  """Handle of any engine tensor by name, including ones the Python net does not register
-  (a fire's squeeze output)."""
-  lib = model._lib
-  buf = C.create_string_buffer(256)
-  for tid in range(lib.sqdet_num_tensors(model._engine)):
-    _lib.check(lib.sqdet_tensor_info(model._engine, tid, buf, 256, None))
-    if buf.value.decode() == name:
-      return model._new_tensor(name, tid)
-  raise KeyError(name)
-
-
 def assert_layer(model, name, want64, want32):
   got = model.read_tensor(engine_tensor(model, name))
   assert got.shape == want64[name].shape, name
   assert rel_err(got, want32[name]) < TOL, (name, rel_err(got, want32[name]))
   e_gpu, e_ref = rel_err(got, want64[name]), rel_err(want32[name], want64[name])
   assert e_gpu < max(4 * e_ref, 2e-5), (name, e_gpu, e_ref)
-
-
-def assert_fused_away(model, name):
-  with pytest.raises(_lib.SqdetError) as exc:
-    model.read_tensor(engine_tensor(model, name))
-  assert exc.value.code == ERR_NOT_FOUND, exc.value
 
 
 def run(body, batch, height, width, math_mode, device, bn_convs=()):
@@ -171,10 +100,6 @@ def test_first_layer_conv_pool(cout, size, cpad, ppad, bn, math_mode, gpu_device
 
 
 # ---- fire modules: one kernel vs squeeze + expand pair ---------------------------------------
-def fire_tiles(batch, h, w):
-  return batch * -(-h // FIRE_TILE_H) * -(-w // FIRE_TILE_W)
-
-
 @pytest.mark.parametrize('math_mode', MODES)
 @pytest.mark.parametrize('cin', [32, 48])
 def test_fire_one_kernel_layerwise(cin, math_mode, gpu_device):

@@ -5,45 +5,12 @@ import pytest
 
 import oracle
 from squeezedet_b200 import _lib, Session
-from squeezedet_b200 import config as cfg
-from squeezedet_b200.nets import SqueezeDet, SqueezeDetPlus, VGG16ConvDet, ResNet50ConvDet
+from squeezedet_b200.nets import SqueezeDet
 from squeezedet_b200.utils import synth
-from gpu_util import assert_classes_match, rel_err
+from gpu_util import (MODES, TOL, assert_boxes_close, assert_classes_match, make_mc, make_net,
+                      rel_err)
 
 pytestmark = pytest.mark.gpu
-
-NETS = {
-    'squeezeDet': (SqueezeDet, cfg.kitti_squeezeDet_config),
-    'squeezeDet+': (SqueezeDetPlus, cfg.kitti_squeezeDetPlus_config),
-    'vgg16': (VGG16ConvDet, cfg.kitti_vgg16_config),
-    'resnet50': (ResNet50ConvDet, cfg.kitti_res50_config),
-}
-MODES = [_lib.MATH_FP32_SIMT, _lib.MATH_TF32X3_TC]
-
-# Tolerances (BASELINE.json north_star): scores and box coordinates within 1e-4 relative;
-# class ids / kept-box indices exact wherever the oracle's own margin exceeds fp noise.
-TOL = 1e-4
-
-
-def make_mc(net, width, height, batch):
-  mc = NETS[net][1]()
-  mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT, mc.BATCH_SIZE = width, height, batch
-  rows = oracle.layer_table(net, height, width)
-  mc.GRID_H, mc.GRID_W = rows[-1][2][0], rows[-1][2][1]
-  mc.ANCHOR_BOX = cfg.set_anchors(mc)
-  mc.ANCHORS = len(mc.ANCHOR_BOX)
-  return mc
-
-
-def assert_boxes_close(got, ref32, ref64):
-  """Box coordinates: within 1e-4 relative of the fp32 reference, plus the reference's OWN
-  fp32 uncertainty (|ref32 - ref64|, x4) — boxes that clip from ~4000 px wide pre-clip values
-  carry ~1e-3 px of fp32 rounding in any implementation — plus 4e-3 px absolute (3e-6 of the
-  image width)."""
-  got = np.asarray(got, np.float64)
-  tol = TOL * np.abs(ref32) + 4.0 * np.abs(np.asarray(ref32, np.float64) - ref64) + 4e-3
-  bad = np.abs(got - ref32) > tol
-  assert not bad.any(), (int(bad.sum()), float(np.abs(got - ref32)[bad].max()))
 
 
 def oracle_run(net, mc, weights, images, dtype=np.float32, keep=None):
@@ -57,11 +24,9 @@ def oracle_run(net, mc, weights, images, dtype=np.float32, keep=None):
     ('squeezeDet', 208, 112), ('squeezeDet+', 215, 119), ('vgg16', 96, 64),
     ('resnet50', 131, 99)])
 def test_layerwise_parity_small_image(net, width, height, math_mode, gpu_device):
-  mc = make_mc(net, width, height, 2)
-  model = NETS[net][0](mc, gpu_device, math_mode=math_mode)
-  weights = synth.synthetic_weights(synth.model_param_specs(model), seed=3)
+  model, weights = make_net(net, width, height, 2, gpu_device, math_mode, seed=3)
+  mc = model.mc
   assert [n for n, _ in synth.model_param_specs(model)] == [n for n, _ in oracle.param_specs(net)]
-  model.load_weights(weights)
   images = synth.synthetic_images(2, height, width, seed=9)
   keep64, keep32 = {}, {}
   p64, (b64, s64, c64) = oracle_run(net, mc, weights, images, np.float64, keep64)
@@ -94,11 +59,9 @@ def test_full_size_squeezedet_detections(math_mode, gpu_device):
   the fp32 oracle; filtered records identical to running the oracle's filter_prediction on
   the oracle's det tensors wherever the oracle's top-65 score gaps exceed the tolerance."""
   net = 'squeezeDet'
-  mc = make_mc(net, 1242, 375, 2)
+  model, weights = make_net(net, 1242, 375, 2, gpu_device, math_mode, seed=0)
+  mc = model.mc
   assert (mc.GRID_H, mc.GRID_W, mc.ANCHORS) == (24, 78, 16848)
-  model = SqueezeDet(mc, gpu_device, math_mode=math_mode)
-  weights = synth.synthetic_weights(synth.model_param_specs(model), seed=0)
-  model.load_weights(weights)
   images = synth.synthetic_images(2, 375, 1242, seed=1234)
   _, (wb, wp, wc) = oracle_run(net, mc, weights, images, np.float32)
   p64, (wb64, _, _) = oracle_run(net, mc, weights, images, np.float64)
@@ -138,9 +101,8 @@ def test_full_size_squeezedet_detections(math_mode, gpu_device):
 def test_session_run_contract_and_filter_prediction(math_mode, gpu_device):
   """The reference call shape: sess.run([det_boxes, det_probs, det_class], feed_dict) then
   model.filter_prediction per image (demo.py:193-199)."""
-  mc = make_mc('squeezeDet', 416, 128, 1)
-  model = SqueezeDet(mc, gpu_device, math_mode=math_mode)
-  model.load_weights(synth.synthetic_weights(synth.model_param_specs(model), seed=5))
+  model, _ = make_net('squeezeDet', 416, 128, 1, gpu_device, math_mode, seed=5)
+  mc = model.mc
   img = synth.synthetic_images(1, 128, 416, seed=6)[0]
   with Session() as sess:
     det_boxes, det_probs, det_class = sess.run(
@@ -173,9 +135,7 @@ def test_forward_profiled_matches_detect(math_mode, gpu_device):
   records as sqdet_detect on the same images.  Every result buffer is overwritten with 0xff bytes
   first, so a skipped interpret or filter launch shows.  VGG16 fuses no pool into its producer, so
   every op issues work and every time is positive."""
-  mc = make_mc('vgg16', 96, 64, 2)
-  model = VGG16ConvDet(mc, gpu_device, math_mode=math_mode)
-  model.load_weights(synth.synthetic_weights(synth.model_param_specs(model), seed=5))
+  model, _ = make_net('vgg16', 96, 64, 2, gpu_device, math_mode, seed=5)
   images = synth.synthetic_images(2, 64, 96, seed=6)
   want = dict(zip(('det_boxes', 'det_probs', 'det_class', 'dets', 'counts'),
                   model.detect(images, want_dets=True)))
@@ -199,13 +159,8 @@ def test_forward_profiled_matches_detect(math_mode, gpu_device):
 
 
 def test_batch_invariance_and_determinism(gpu_device):
-  mc1 = make_mc('squeezeDet', 320, 96, 1)
-  mc3 = make_mc('squeezeDet', 320, 96, 3)
-  m1 = SqueezeDet(mc1, gpu_device)
-  m3 = SqueezeDet(mc3, gpu_device)
-  w = synth.synthetic_weights(synth.model_param_specs(m1), seed=8)
-  m1.load_weights(w)
-  m3.load_weights(w)
+  m1, _ = make_net('squeezeDet', 320, 96, 1, gpu_device, seed=8)
+  m3, _ = make_net('squeezeDet', 320, 96, 3, gpu_device, seed=8)
   imgs = synth.synthetic_images(3, 96, 320, seed=4)
   b3, p3, c3 = m3.detect(imgs)
   b3b, p3b, c3b = m3.detect(imgs)
@@ -227,9 +182,8 @@ def test_set_param_errors(gpu_device):
 def test_pipelined_submit_and_uint8_input(gpu_device):
   """sqdet_submit/sqdet_wait (depth-2 pipeline) and the uint8 path: same records as the
   synchronous fp32 feed of `im - BGR_MEANS` (demo.py:187-190)."""
-  mc = make_mc('squeezeDet', 320, 96, 2)
-  m = SqueezeDet(mc, gpu_device)
-  m.load_weights(synth.synthetic_weights(synth.model_param_specs(m), seed=8))
+  m, _ = make_net('squeezeDet', 320, 96, 2, gpu_device, seed=8)
+  mc = m.mc
   rng = np.random.default_rng(3)
   batches = [rng.integers(0, 256, (2, 96, 320, 3), dtype=np.uint8) for _ in range(4)]
   feeds = [(b.astype(np.float32) - np.asarray(mc.BGR_MEANS)).astype(np.float32) for b in batches]

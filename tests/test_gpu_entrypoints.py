@@ -9,50 +9,13 @@ import numpy as np
 import pytest
 
 import oracle
-from oracle import preproc
-from oracle.torch_port import TorchForward
-from squeezedet_b200 import _lib, demo, eval as sq_eval
+from squeezedet_b200 import demo, eval as sq_eval
 from squeezedet_b200 import config as cfg
 from squeezedet_b200.utils import synth, viz
 from squeezedet_b200.utils.util import bbox_transform
+from gpu_util import TOL, make_kitti, make_net, make_png, oracle_pipeline
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-4
-
-
-def make_png(path, h, w, seed):
-  """A frame with structure (rectangles on noise) so detections spread over the image."""
-  import cv2
-  rng = np.random.default_rng(seed)
-  im = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
-  for _ in range(12):
-    y0, x0 = int(rng.integers(0, h - 40)), int(rng.integers(0, w - 80))
-    im[y0:y0 + int(rng.integers(20, 120)), x0:x0 + int(rng.integers(40, 300))] = \
-        rng.integers(0, 256, 3, dtype=np.uint8)
-  assert cv2.imwrite(path, im)
-  return im
-
-
-def oracle_pipeline(net, mc, weights, frame_u8, order, rescale):
-  fed = preproc.preprocess(frame_u8, mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT, mc.BGR_MEANS, order)
-  preds = TorchForward(net, weights)(fed[None])
-  boxes, probs, cls = oracle.interpret_output(preds, mc.ANCHOR_BOX, mc.CLASSES,
-                                              mc.ANCHOR_PER_GRID, mc.IMAGE_WIDTH,
-                                              mc.IMAGE_HEIGHT, mc.EXP_THRESH)
-  boxes, probs, cls = boxes[0].copy(), probs[0], cls[0]
-  if rescale:
-    # eval.py:72-74,83-84 (scales are Python floats; numpy divides the float32 array in float32)
-    x_scale = mc.IMAGE_WIDTH / float(frame_u8.shape[1])
-    y_scale = mc.IMAGE_HEIGHT / float(frame_u8.shape[0])
-    boxes[:, 0::2] /= x_scale
-    boxes[:, 1::2] /= y_scale
-  fb, fp, fc, src = oracle.filter_prediction(boxes, probs, cls, mc.CLASSES, mc.TOP_N_DETECTION,
-                                             mc.PROB_THRESH, mc.NMS_THRESH)
-  order66 = np.argsort(-probs.astype(np.float64), kind='stable')[:66]
-  top = probs[order66].astype(np.float64)
-  gap = np.abs(top[:, None] - top[None, :]) <= 10 * TOL * top[:, None]
-  np.fill_diagonal(gap, False)
-  return fb, fp, fc, bool(gap.any())
 
 
 def compare(got_boxes, got_probs, got_cls, want, what):
@@ -89,18 +52,7 @@ def test_image_demo_runs_and_matches_oracle(tmp_path, gpu_device):
 
 
 def test_eval_once_reference_order_files_and_scorer(tmp_path, gpu_device):
-  data = tmp_path / 'KITTI'
-  (data / 'training' / 'image_2').mkdir(parents=True)
-  (data / 'training' / 'label_2').mkdir(parents=True)
-  (data / 'ImageSets').mkdir()
-  ids, frames = [], {}
-  for k, (h, w) in enumerate([(375, 1242), (370, 1224), (376, 1241)]):
-    idx = '%06d' % k
-    ids.append(idx)
-    frames[idx] = make_png(str(data / 'training' / 'image_2' / (idx + '.png')), h, w, seed=20 + k)
-    (data / 'training' / 'label_2' / (idx + '.txt')).write_text(
-        'Car 0.00 0 -1.57 100.00 120.00 300.00 250.00 1.5 1.6 3.9 1.0 1.7 10.0 -1.5\n')
-  (data / 'ImageSets' / 'val.txt').write_text('\n'.join(ids) + '\n')
+  data, ids, frames = make_kitti(tmp_path)
   flags = sq_eval.parse_flags(['--data_path', str(data), '--image_set', 'val',
                                '--eval_dir', str(tmp_path / 'eval'),
                                '--checkpoint_path', 'synthetic', '--net', 'squeezeDet',
@@ -145,11 +97,8 @@ def test_eval_once_reference_order_files_and_scorer(tmp_path, gpu_device):
 def test_rescale_before_filter_changes_nothing_but_coordinates(gpu_device):
   """sqdet_set_box_scale: det_boxes come back divided by the scales (float32 division, as numpy
   does in eval.py:83-84) and the records equal the oracle filter run on those rescaled boxes."""
-  from squeezedet_b200.nets import SqueezeDet
-  from test_gpu_e2e import make_mc
-  mc = make_mc('squeezeDet', 416, 128, 2)
-  m = SqueezeDet(mc, gpu_device)
-  m.load_weights(synth.synthetic_weights(synth.model_param_specs(m), seed=5))
+  m, _ = make_net('squeezeDet', 416, 128, 2, gpu_device, seed=5)
+  mc = m.mc
   imgs = synth.synthetic_images(2, 128, 416, seed=6)
   b0, p0, c0 = m.detect(imgs)
   scales = np.array([[1248 / 1242.0, 384 / 375.0], [0.75, 1.5]], np.float32)
@@ -173,11 +122,8 @@ def test_rescale_before_filter_changes_nothing_but_coordinates(gpu_device):
 def test_frames_rescale_and_box_scale_table_stay_apart(gpu_device):
   """`rescale` of a frames submission applies to that submission only, and the table of
   sqdet_set_box_scale to the paths fed already-resized images only."""
-  from squeezedet_b200.nets import SqueezeDet
-  from test_gpu_e2e import make_mc
-  mc = make_mc('squeezeDet', 416, 128, 2)
-  m = SqueezeDet(mc, gpu_device)
-  m.load_weights(synth.synthetic_weights(synth.model_param_specs(m), seed=5))
+  m, _ = make_net('squeezeDet', 416, 128, 2, gpu_device, seed=5)
+  mc = m.mc
   imgs = synth.synthetic_images(2, 128, 416, seed=6)
   rng = np.random.default_rng(7)
   # not 128 x 416, so the frames' box scales are not 1

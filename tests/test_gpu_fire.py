@@ -6,7 +6,7 @@ import pytest
 
 import oracle
 from squeezedet_b200 import _lib
-from gpu_util import fire_gpu, rel_err
+from gpu_util import adv_tol, bound_ratio, fire_error_bound, fire_gpu, fire_oracle, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -20,13 +20,6 @@ SQUEEZEDET_PLUS_FIRES = [(96, 96, 64, 64), (128, 96, 64, 64), (128, 192, 128, 12
 # spatial cases: ragged tiles on both axes, a single-tile image, a batch > 1
 SPATIAL = [(2, 19, 37), (1, 8, 16), (1, 24, 78)]
 FIRE_RTOL = 3e-5      # two stacked convs vs fp64, relative to the tensor's max
-
-
-def fire_oracle(x, ws, bs, w1, b1, w3, b3, dtype):
-  q = oracle.conv2d(x, ws, bs, 1, 'SAME', True, dtype)
-  a = oracle.conv2d(q, w1, b1, 1, 'SAME', True, dtype)
-  b = oracle.conv2d(q, w3, b3, 1, 'SAME', True, dtype)
-  return np.concatenate([a, b], axis=3)
 
 
 def make_case(shape, spatial, seed):
@@ -80,28 +73,13 @@ FIRE_EDGE_CASES = [
 ]
 
 
-def fire_error_bound(x, ws, w1, w3, q64):
-  """Per-element scale of the error of squeeze -> ReLU -> expand in any fp32 summation order:
-  the expand's own rounding, tol * (|q| (*) |w_e|), plus the squeeze's error carried through the
-  expand, tol * ((|x| (*) |w_s|) (*) |w_e|); ReLU is 1-Lipschitz, so it cannot amplify the
-  squeeze error."""
-  def conv(a, w):
-    return oracle.conv2d(a, w, None, 1, 'SAME', False, np.float64)
-  sx = conv(np.abs(x), np.abs(ws))
-  return np.concatenate([conv(np.abs(q64), np.abs(w1)) + conv(sx, np.abs(w1)),
-                         conv(np.abs(q64), np.abs(w3)) + conv(sx, np.abs(w3))], axis=3)
-
-
 def fire_bound_ratio(args, got, want64):
-  """max |got - want64| / fire_error_bound, in units of the bar 1.2e-7 * sqrt(K) with K the
-  longer of the two convs' sums (test_gpu_adversarial.adv_tol); must stay below 1."""
+  """max |got - want64| / gpu_util.fire_error_bound, in units of the bar adv_tol(K) with K the
+  longer of the two convs' sums; must stay below 1."""
   x, ws, bs, w1, b1, w3, b3 = args
   q64 = oracle.conv2d(x, ws, bs, 1, 'SAME', True, np.float64)
-  err = np.abs(got.astype(np.float64) - want64)
-  bound = fire_error_bound(x, ws, w1, w3, q64)
-  with np.errstate(divide='ignore'):
-    ratio = np.divide(err, bound, out=np.zeros_like(err), where=err > 0)
-  return float(ratio.max()) / (1.2e-7 * np.sqrt(max(x.shape[3], 9 * ws.shape[3])))
+  ratio = bound_ratio(got, want64, fire_error_bound(x, ws, w1, w3, q64))
+  return float(ratio.max()) / adv_tol(max(x.shape[3], 9 * ws.shape[3]))
 
 
 @pytest.mark.parametrize('math_mode', [_lib.MATH_FP32_SIMT, _lib.MATH_TF32X3_TC])

@@ -4,7 +4,7 @@ nine taps as row offsets into it.  Tiles cut by every image edge, images smaller
 (down to 1 x 1), every output-tile width with both K chunk widths, a ragged fire expand pair (a
 1x1 and a 3x3 conv in one launch), the affine epilogue with a channel window, and images of a
 partial batch.  Each element is checked against the fp64 oracle on the scale that bounds any
-fp32 summation of its products, with the bar of test_gpu_adversarial; the ConvDet heads, wide
+fp32 summation of its products, with the bar gpu_util.adv_tol; the ConvDet heads, wide
 outputs and a channel window also against a relative bar over the whole tensor and its borders."""
 import numpy as np
 import pytest
@@ -12,18 +12,11 @@ import pytest
 import oracle
 from squeezedet_b200 import _lib
 from squeezedet_b200.utils import synth
-from gpu_util import conv2d_gpu, rel_err
-from test_gpu_adversarial import adv_tol
-from test_gpu_dispatch import build, engine_tensor
+from gpu_util import (assert_rows_equal, assert_within_bound, build, conv2d_gpu, conv_oracle,
+                      forward_n, read_tensors, rel_err)
 
 pytestmark = pytest.mark.gpu
 TC = _lib.MATH_TF32X3_TC
-
-
-def assert_within_bound(got, want, bound, K, what):
-  ratio = np.abs(np.asarray(got, np.float64) - want) / np.maximum(bound, 1e-30)
-  assert not np.isnan(got).any(), what
-  assert ratio.max() < adv_tol(K), (what, float(ratio.max()), adv_tol(K))
 
 
 CASES = [
@@ -46,8 +39,7 @@ def test_halo_tile_vs_oracle(case, gpu_device):
   rng = np.random.default_rng(7 + sum(case))
   x = rng.normal(size=(B, H, W, Cin)).astype(np.float32)
   w = (rng.normal(size=(3, 3, Cin, Cout)) / np.sqrt(9 * Cin)).astype(np.float32)
-  want = oracle.conv2d(x, w, None, 1, 'SAME', apply_relu=False, dtype=np.float64)
-  bound = oracle.conv2d(np.abs(x), np.abs(w), None, 1, 'SAME', apply_relu=False, dtype=np.float64)
+  want, bound = conv_oracle(x, w)
   got = conv2d_gpu(x, w, None, 1, 'SAME', relu=False, math_mode=TC)
   assert got.shape == want.shape
   assert_within_bound(got, want, bound, 9 * Cin, case)
@@ -69,10 +61,7 @@ def test_halo_tile_affine_and_channel_window(cin, gpu_device):
   b = rng.normal(size=Cout).astype(np.float32)
   sc = rng.uniform(0.5, 1.5, Cout).astype(np.float32)
   sh = rng.normal(size=Cout).astype(np.float32)
-  conv = oracle.conv2d(x, w, b, 1, 'SAME', False, np.float64)
-  want = conv * sc + sh
-  bound = (oracle.conv2d(np.abs(x), np.abs(w), np.abs(b), 1, 'SAME', False, np.float64) * sc
-           + np.abs(sh))
+  want, bound = conv_oracle(x, w, b, scale=sc, shift=sh)
   y0 = np.full((B, H, W, cs), 7.0, np.float32)
   got = conv2d_gpu(x, w, b, 1, 'SAME', relu=False, scale=sc, shift=sh, y_cstride=cs, y_coff=coff,
                    math_mode=TC, y_init=y0)
@@ -140,29 +129,17 @@ def test_ragged_expand_pair_and_partial_batch(gpu_device):
   images = synth.synthetic_images(B, H, W, seed=3)
   model.detect(images)
   names = ('fire2/squeeze1x1', 'fire2', 'conv12')
-  full = {nm: model.read_tensor(engine_tensor(model, nm)) for nm in names}
+  full = read_tensors(model, names)
 
   q = full['fire2/squeeze1x1'].astype(np.float64)
-  parts = []
-  for sub, k in (('expand1x1', 1), ('expand3x3', 3)):
+  for sub, k, got in (('expand1x1', 1, full['fire2'][..., :24]),
+                      ('expand3x3', 3, full['fire2'][..., 24:])):
     kern, bias = weights['fire2/%s/kernels' % sub], weights['fire2/%s/biases' % sub]
-    want = oracle.conv2d(q, kern, bias, 1, 'SAME', True, np.float64)
-    bound = oracle.conv2d(np.abs(q), np.abs(kern), np.abs(bias), 1, 'SAME', False, np.float64)
-    parts.append((want, bound, k * k * 48))
-  assert_within_bound(full['fire2'][..., :24], *parts[0][:2], parts[0][2], 'expand1x1')
-  assert_within_bound(full['fire2'][..., 24:], *parts[1][:2], parts[1][2], 'expand3x3')
-  e = full['fire2'].astype(np.float64)
+    assert_within_bound(got, *conv_oracle(q, kern, bias, relu=True), k * k * 48, sub)
   kern, bias = weights['conv12/kernels'], weights['conv12/biases']
   assert kern.shape == (3, 3, 96, 72)
-  assert_within_bound(full['conv12'], oracle.conv2d(e, kern, bias, 1, 'SAME', False, np.float64),
-                      oracle.conv2d(np.abs(e), np.abs(kern), np.abs(bias), 1, 'SAME', False,
-                                    np.float64), 9 * 96, 'conv12')
+  assert_within_bound(full['conv12'], *conv_oracle(full['fire2'], kern, bias), 9 * 96, 'conv12')
 
   for n in (1, 2):
-    buf = _lib.DeviceBuffer.from_numpy(np.ascontiguousarray(images[:n], np.float32), gpu_device)
-    model.forward_device(buf.ptr, None, n)
-    _lib.check(model._lib.sqdet_stream_sync(gpu_device, None))
-    buf.free()
-    for nm in names:
-      got = model.read_tensor(engine_tensor(model, nm))
-      assert got[:n].tobytes() == full[nm][:n].tobytes(), (nm, n)
+    forward_n(model, images, n)
+    assert_rows_equal(read_tensors(model, names), full, n)

@@ -2,7 +2,7 @@
 
 The oracle of each layer is fed the engine's own read-back input for that layer (teacher
 forcing), so errors do not compound from layer to layer and the per-element bound of the
-stage-isolated tests (test_gpu_adversarial.adv_tol) applies unchanged at the benchmark's shapes,
+stage-isolated tests (gpu_util.adv_tol) applies unchanged at the benchmark's shapes,
 batch and dispatch:
 
     |got - want64| <= tol(K) * (|x| (*) |w| + |b|),    tol(K) = 1.2e-7 * sqrt(K),  K = k*k*Cin.
@@ -20,7 +20,7 @@ Rules per layer kind:
   * conv fused with the 3x3/2 pool (the conv tensor reads as not found): max_pool of the fp64 conv
     against max_pool of the conv bound (a max over a window moves by at most the largest move of
     its inputs);
-  * one-kernel fire (the squeeze tensor reads as not found): test_gpu_fire.fire_oracle in fp64,
+  * one-kernel fire (the squeeze tensor reads as not found): gpu_util.fire_oracle in fp64,
     per element against the bar of test_gpu_fire.fire_bound_ratio;
   * squeeze + expand pair, or three SIMT convs: the conv rule for the squeeze on the fire input and
     for each expand on the engine's squeeze tensor;
@@ -39,12 +39,9 @@ from oracle.nets import NET_BUILDERS
 from oracle.torch_port import _TorchTracer
 from squeezedet_b200 import _lib
 from squeezedet_b200.utils import synth
-from gpu_util import conv2d_gpu, maxpool_gpu
-from test_gpu_adversarial import adv_tol
-from test_gpu_dispatch import (ERR_NOT_FOUND, ONE_KERNEL_MIN_TILES, PAIR_MAX_TILES,
-                               assert_fused_away, build, engine_tensor, fire_tiles)
-from test_gpu_e2e import MODES, NETS, make_mc
-from test_gpu_fire import fire_error_bound, fire_oracle
+from gpu_util import (ERR_NOT_FOUND, MODES, ONE_KERNEL_MIN_TILES, PAIR_MAX_TILES, adv_tol,
+                      assert_fused_away, bound_ratio, build, conv2d_gpu, engine_tensor,
+                      fire_error_bound, fire_oracle, fire_tiles, make_net, maxpool_gpu)
 
 U = 2.0 ** -24         # unit roundoff of fp32 round-to-nearest
 
@@ -108,10 +105,7 @@ class LayerChecker:
     if got.shape != want.shape:
       self.failures.append('%s (%s): shape %s, want %s' % (name, rule, got.shape, want.shape))
       return
-    err = np.abs(got.astype(np.float64) - want)
-    with np.errstate(divide='ignore', invalid='ignore'):
-      ratio = np.where(err > 0, err / bar, 0.0)
-    ratio[np.isnan(err)] = np.inf
+    ratio = bound_ratio(got, want, bar)
     worst = np.unravel_index(np.argmax(ratio), ratio.shape)
     r = float(ratio[worst])
     if record:
@@ -122,7 +116,8 @@ class LayerChecker:
       self.failures.append(
           '%s (%s): image %d, element (y, x, c) = %s: |got - want| = %.4g is %.3g x the bar %.4g '
           '(got %r, want %r), K = %d' % (name, rule, self.images[worst[0]],
-                                          tuple(int(v) for v in worst[1:]), err[worst], r,
+                                          tuple(int(v) for v in worst[1:]),
+                                          abs(float(got[worst]) - want[worst]), r,
                                           bar[worst], float(got[worst]), float(want[worst]), K))
 
   def _sanity(self, name, rule, want32, want, bar, K):
@@ -275,10 +270,8 @@ HEIGHT, WIDTH = 375, 1242
 def test_benchmark_layers_within_fp64_bound(net, batch, math_mode, gpu_device):
   """Each layer of the net at 1242 x 375 and the batch the benchmark runs, with the dispatch this
   check is meant to see asserted first."""
-  mc = make_mc(net, WIDTH, HEIGHT, batch)
-  model = NETS[net][0](mc, gpu_device, math_mode=math_mode)
-  weights = synth.synthetic_weights(oracle.param_specs(net), seed=0)
-  model.load_weights(weights)
+  model, weights = make_net(net, WIDTH, HEIGHT, batch, gpu_device, math_mode, seed=0)
+  mc = model.mc
   images = synth.synthetic_images(batch, HEIGHT, WIDTH, seed=1234)
   model.detect(images)
   tc = math_mode == _lib.MATH_TF32X3_TC

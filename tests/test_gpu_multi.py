@@ -10,9 +10,8 @@ import numpy as np
 import pytest
 
 from squeezedet_b200 import _lib
-from squeezedet_b200.nets import SqueezeDet
 from squeezedet_b200.utils import synth
-from test_gpu_e2e import make_mc
+from gpu_util import make_net
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -26,12 +25,10 @@ def need_gpus(n):
 
 def test_two_devices_one_process():
   need_gpus(2)
-  mc = make_mc('squeezeDet', 320, 96, 2)
   imgs = synth.synthetic_images(2, 96, 320, seed=4)
   outs = []
   for dev in (0, 1):
-    m = SqueezeDet(mc, dev)
-    m.load_weights(synth.synthetic_weights(synth.model_param_specs(m), seed=8))
+    m, _ = make_net('squeezeDet', 320, 96, 2, dev, seed=8)
     outs.append((m, m.detect(imgs)))
   (m0, (b0, p0, c0)), (m1, (b1, p1, c1)) = outs
   assert np.array_equal(p0, p1) and np.array_equal(b0, b1) and np.array_equal(c0, c1)

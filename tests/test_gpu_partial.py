@@ -15,31 +15,11 @@ from squeezedet_b200 import config as cfg
 from squeezedet_b200.nets import SqueezeDet
 from squeezedet_b200.utils import synth, viz
 from squeezedet_b200.utils.util import bbox_transform
-from test_gpu_dispatch import assert_fused_away, build, fire_tiles
-from test_gpu_e2e import NETS, MODES, make_mc
-from test_gpu_entrypoints import TOL, make_png, oracle_pipeline
+from gpu_util import (MODES, RESULTS, TOL, assert_fused_away, assert_rows_equal, build,
+                      fetch_results, fire_tiles, forward_n, make_kitti, make_net, oracle_pipeline)
 
 pytestmark = pytest.mark.gpu
 ERR_INVALID_ARG = -1
-RESULTS = (('det_boxes', np.float32, 4), ('det_probs', np.float32, None),
-           ('det_class', np.int64, None))
-
-
-def fetch_results(model, device):
-  """Every device result buffer of the engine, all B rows."""
-  B, A = model.det_probs.shape
-  res = model.results_device()
-  lib = model._lib
-  out = {}
-  for key, dtype, last in RESULTS:
-    out[key] = np.empty((B, A, last) if last else (B, A), dtype)
-  out['dets'] = np.empty((B, res['max_dets']), _lib.DET_DTYPE)
-  out['counts'] = np.empty((B,), np.int32)
-  _lib.check(lib.sqdet_stream_sync(device, None))
-  for key, arr in out.items():
-    _lib.check(lib.sqdet_memcpy_d2h(arr.ctypes.data, res[key], arr.nbytes, None))
-  _lib.check(lib.sqdet_stream_sync(device, None))
-  return out
 
 
 def fill_results(model, device, byte=0xff):
@@ -64,14 +44,6 @@ def activations(model):
   return out
 
 
-def forward(model, images, n, stream, device):
-  """forward_device over a device buffer that holds exactly the images passed."""
-  buf = _lib.DeviceBuffer.from_numpy(np.ascontiguousarray(images, np.float32), device)
-  model.forward_device(buf.ptr, stream, n)
-  _lib.check(model._lib.sqdet_stream_sync(device, stream))
-  buf.free()
-
-
 def assert_rows_match(got, want, n):
   """Rows [0, n) bitwise equal (records up to each image's count); rows [n, B) untouched since
   fill_results (0xff bytes), except counts, which are 0."""
@@ -91,17 +63,16 @@ def check_partial_rows(model, images, other, device, stream_for):
   forward; then `other` at n = 1, after which every activation's rows >= 1 still hold `images`'
   values.  stream_for(n): the stream of the n-image forward (None = legacy, not graph-captured)."""
   B = images.shape[0]
-  forward(model, images, None, model.engine_stream(), device)
+  forward_n(model, images, None, model.engine_stream())
   want = fetch_results(model, device)
   acts = activations(model)
   assert acts
   for n in range(1, B):
     fill_results(model, device)
-    forward(model, images[:n], n, stream_for(n), device)
+    forward_n(model, images, n, stream_for(n))
     assert_rows_match(fetch_results(model, device), want, n)
-    for name, a in activations(model).items():
-      assert a[:n].tobytes() == acts[name][:n].tobytes(), (name, n)
-  forward(model, other[:1], 1, model.engine_stream(), device)
+    assert_rows_equal(activations(model), acts, n)
+  forward_n(model, other, 1, model.engine_stream())
   for name, a in activations(model).items():
     assert a[1:].tobytes() == acts[name][1:].tobytes(), name
   return want
@@ -112,9 +83,7 @@ def check_partial_rows(model, images, other, device, stream_for):
     ('squeezeDet', 208, 112), ('squeezeDet+', 215, 119), ('vgg16', 96, 64),
     ('resnet50', 131, 99)])
 def test_forward_n_rows_bitwise(net, width, height, math_mode, gpu_device):
-  mc = make_mc(net, width, height, 3)
-  model = NETS[net][0](mc, gpu_device, math_mode=math_mode)
-  model.load_weights(synth.synthetic_weights(synth.model_param_specs(model), seed=3))
+  model, _ = make_net(net, width, height, 3, gpu_device, math_mode, seed=3)
   x = synth.synthetic_images(3, height, width, seed=9)
   y = synth.synthetic_images(3, height, width, seed=10)
   # n = 1 on the legacy stream (launched directly), n = 2 on the engine stream (CUDA graph)
@@ -155,9 +124,7 @@ def test_submit_frames_n_pipeline(gpu_device):
   """n = B, 1, B, 2 with two submits in flight and rescale alternating: each result equals the
   same frames submitted alone, only n rows come back, and the device counts past n are 0."""
   B = 3
-  mc = make_mc('squeezeDet', 320, 96, B)
-  m = SqueezeDet(mc, gpu_device)
-  m.load_weights(synth.synthetic_weights(synth.model_param_specs(m), seed=8))
+  m, _ = make_net('squeezeDet', 320, 96, B, gpu_device, seed=8)
   rng = np.random.default_rng(4)
   sizes = [(96, 320), (120, 400), (80, 300)]
   plan = [(B, True), (1, False), (B, False), (2, True)]
@@ -203,24 +170,6 @@ def test_submit_frames_n_pipeline(gpu_device):
     m.detect_frames([])
   with pytest.raises(ValueError):
     m.detect_frames([subs[0][0]] * (B + 1))
-
-
-def make_kitti(root):
-  """The three full-size frames and labels of
-  test_gpu_entrypoints.test_eval_once_reference_order_files_and_scorer."""
-  data = root / 'KITTI'
-  (data / 'training' / 'image_2').mkdir(parents=True)
-  (data / 'training' / 'label_2').mkdir(parents=True)
-  (data / 'ImageSets').mkdir()
-  ids, frames = [], {}
-  for k, (h, w) in enumerate([(375, 1242), (370, 1224), (376, 1241)]):
-    idx = '%06d' % k
-    ids.append(idx)
-    frames[idx] = make_png(str(data / 'training' / 'image_2' / (idx + '.png')), h, w, seed=20 + k)
-    (data / 'training' / 'label_2' / (idx + '.txt')).write_text(
-        'Car 0.00 0 -1.57 100.00 120.00 300.00 250.00 1.5 1.6 3.9 1.0 1.7 10.0 -1.5\n')
-  (data / 'ImageSets' / 'val.txt').write_text('\n'.join(ids) + '\n')
-  return data, ids, frames
 
 
 def run_eval(data, eval_dir, batch, device):

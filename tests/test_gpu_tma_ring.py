@@ -6,17 +6,14 @@ launch, both K chunk widths (so both the 128-byte and the 64-byte swizzle), a ro
 that is not a multiple of 128, tiles hanging over the image (TMA zero fill), gather mode, and the
 one-shot entry called on a second set of buffers; engines whose forwards change the image count
 and the input buffer, through the convolution and the one-kernel fire.  Each element is checked
-against the fp64 oracle with the bar of test_gpu_adversarial, and bitwise against a repeat run."""
+against the fp64 oracle with the bar gpu_util.adv_tol, and bitwise against a repeat run."""
 import numpy as np
 import pytest
 
-import oracle
 from squeezedet_b200 import _lib
 from squeezedet_b200.utils import synth
-from gpu_util import conv2d_gpu
-from test_gpu_adversarial import adv_tol
-from test_gpu_dispatch import (ONE_KERNEL_MIN_TILES, POST_LAUNCHES, build, engine_tensor,
-                               fire_tiles)
+from gpu_util import (ONE_KERNEL_MIN_TILES, POST_LAUNCHES, assert_rows_equal, assert_within_bound,
+                      build, conv2d_gpu, conv_oracle, fire_tiles, read_tensors)
 
 pytestmark = pytest.mark.gpu
 TC = _lib.MATH_TF32X3_TC
@@ -26,13 +23,10 @@ def check_conv(x, w, stride=1, padding='SAME', seed=0):
   k, Cin = w.shape[0], w.shape[2]
   rng = np.random.default_rng(seed)
   b = rng.normal(size=w.shape[3]).astype(np.float32)
-  want = oracle.conv2d(x, w, b, stride, padding, apply_relu=False, dtype=np.float64)
-  bound = oracle.conv2d(np.abs(x), np.abs(w), np.abs(b), stride, padding, apply_relu=False,
-                        dtype=np.float64)
+  want, bound = conv_oracle(x, w, b, stride, padding)
   got = conv2d_gpu(x, w, b, stride, padding, relu=False, math_mode=TC)
   assert got.shape == want.shape and not np.isnan(got).any()
-  ratio = np.abs(got.astype(np.float64) - want) / np.maximum(bound, 1e-30)
-  assert ratio.max() < adv_tol(k * k * Cin), (x.shape, w.shape, float(ratio.max()))
+  assert_within_bound(got, want, bound, k * k * Cin, (x.shape, w.shape))
   again = conv2d_gpu(x, w, b, stride, padding, relu=False, math_mode=TC)
   assert got.tobytes() == again.tobytes()
   return got
@@ -111,11 +105,10 @@ def assert_rows_follow_full_forward(model, B, H, W, names, runs, device):
   for i, n in runs:
     model.forward_device(bufs[i].ptr, None, n)
     _lib.check(model._lib.sqdet_stream_sync(device, None))
-    got = {nm: model.read_tensor(engine_tensor(model, nm)) for nm in names}
+    got = read_tensors(model, names)
     if full is None:
       full = got
-    for nm in names:
-      assert got[nm][:n].tobytes() == full[nm][:n].tobytes(), (nm, i, n)
+    assert_rows_equal(got, full, n, i)
   for buf in bufs:
     buf.free()
 

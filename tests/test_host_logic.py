@@ -160,6 +160,34 @@ def test_gpu_case_tables_reach_every_tc_kernel_variant():
              for _, _, _, Cin, Cout, k, s in SHAPES)
 
 
+def test_bound_ratio_and_assert_within_bound():
+  """The per-element fp64 bound every stage-isolated and layer check goes through: an exact result
+  is 0 even on a zero bar, NaN and a non-zero error on a zero bar are inf, and assert_within_bound
+  fails at 1.01x the bar, naming the element, and passes at 0.99x it."""
+  from gpu_util import adv_tol, assert_within_bound, bound_ratio
+  want = np.array([1.0, 0.0, 2.0, -3.0, 5.0, 0.0])
+  bar = np.array([1.0, 0.0, 0.0, 2.0, 4.0, 0.0])
+  got = np.array([1.5, 0.0, 2.0, np.nan, 5.0, 1e-30], np.float32)
+  assert bound_ratio(got, want, bar).tolist() == [0.5, 0.0, 0.0, np.inf, 0.0, np.inf]
+  assert_within_bound(got[1:3], want[1:3], bar[1:3], 1, 'exact results on zero bars')
+  with pytest.raises(AssertionError):
+    assert_within_bound(got[3:5], want[3:5], bar[3:5], 1, 'a NaN')
+
+  K = 9 * 64
+  rng = np.random.default_rng(0)
+  want = rng.normal(size=(2, 3, 4, 5))
+  bar = rng.uniform(0.5, 2.0, want.shape)
+  sign = rng.choice([-1.0, 1.0], want.shape)
+  for scale, ok in ((0.99, True), (1.01, False)):
+    got = want + sign * 0.5 * adv_tol(K) * bar
+    got[1, 2, 0, 3] = want[1, 2, 0, 3] + sign[1, 2, 0, 3] * scale * adv_tol(K) * bar[1, 2, 0, 3]
+    if ok:
+      assert_within_bound(got, want, bar, K, 'at 0.99x')
+    else:
+      with pytest.raises(AssertionError, match=r'\(1, 2, 0, 3\)'):
+        assert_within_bound(got, want, bar, K, 'at 1.01x')
+
+
 # ---- branches of the other kernels, restated from their launchers -------------------------------
 def maxpool_branch(C, size, stride, offset=0):
   """launch_maxpool (pool.cu): float4 kernels need C % 4 == 0 and 16-byte aligned x and y; the
