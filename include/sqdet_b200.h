@@ -157,7 +157,20 @@ int sqdet_forward(sqdet_engine* e, const float* images_dev, void* stream);
  *   - SQDET_ERR_INVALID_ARG when n < 1 or n > B.
  * sqdet_forward is sqdet_forward_n with n = B.                                              */
 int sqdet_forward_n(sqdet_engine* e, const float* images_dev, int n, void* stream);
-/* Same, but records a CUDA event around every op (not graph-captured) and returns
+/* images_dev: n uint8 BGR images [n,H,W,3] as cv2.imread / cv2.resize leave them (any byte
+ * alignment); the engine subtracts mc.BGR_MEANS (src/demo.py:190).  Otherwise sqdet_forward_n:
+ * asynchronous on `stream`, graph-captured, the same partial-batch rules, box-scale table and
+ * in-forward all-gather, and the same results as sqdet_forward_n on
+ * float32(float64(images) - BGR_MEANS), bit for bit.  The plan picks one of two paths:
+ *   - when a fused conv+pool first layer is the only reader of the image tensor, that kernel reads
+ *     the bytes itself and tensor 0 is not written (sqdet_read_tensor(0) keeps what it held);
+ *   - otherwise (a first conv without a pool, VGG16's tensor-core conv1_1, an image read by two
+ *     ops) one extra launch converts the n images into tensor 0, which sqdet_read_tensor(0) then
+ *     returns, and the forward issues one launch more than sqdet_launches_per_forward counts.
+ * A sqdet_set_bgr_means call takes effect at the next sqdet_forward_u8.
+ * SQDET_ERR_INVALID_ARG / SQDET_ERR_STATE before any device work as for sqdet_forward_n.     */
+int sqdet_forward_u8(sqdet_engine* e, const uint8_t* images_dev, int n, void* stream);
+/* sqdet_forward, but records a CUDA event around every op (not graph-captured) and returns
  * per-op milliseconds (synchronous).  op_ms has sqdet_num_ops() entries.              */
 int sqdet_forward_profiled(sqdet_engine* e, const float* images_dev, void* stream,
                            float* op_ms);

@@ -76,6 +76,7 @@ SIGNATURES = {
     'sqdet_op_k_split': (_i, [_vp, _i]),
     'sqdet_forward': (_i, [_vp, _fp, _vp]),
     'sqdet_forward_n': (_i, [_vp, _fp, _i, _vp]),
+    'sqdet_forward_u8': (_i, [_vp, _vp, _i, _vp]),
     'sqdet_forward_profiled': (_i, [_vp, _fp, _vp, _fp]),
     'sqdet_results_dev': (_i, [_vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp),
                                C.POINTER(_vp), C.POINTER(_vp), C.POINTER(C.c_int32)]),

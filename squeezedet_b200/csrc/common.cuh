@@ -57,7 +57,10 @@ int launch_conv_simt(const ConvArgs& a, cudaStream_t stream);
 
 bool conv_pool_simt_eligible(int Cin, int Cout, int ksize, int stride, int pool_size,
                              int pool_stride);
-int launch_conv_pool_simt(const float* x, const float* w, const float* bias, const float* scale,
+// The input is fp32 x, or, when x8 is non-null, uint8 BGR x8 (any byte alignment) from which the
+// kernel subtracts bgr_means as it loads it.
+int launch_conv_pool_simt(const float* x, const uint8_t* x8, const double* bgr_means,
+                          const float* w, const float* bias, const float* scale,
                           const float* shift, float* y, int B, int H, int W, int Cout, int ksize,
                           int conv_padding, int relu, int pool_padding, cudaStream_t stream);
 

@@ -13,11 +13,15 @@
 //
 // CTA = one pooled tile of 4 x 16 pixels of one image:
 //   input patch  (2*8+k) x (2*32+k) x 3 floats        -> smem (coalesced row loads, 0 = pad)
+//                 (uint8 input: the 4-byte words holding each row's bytes -> smem, then
+//                 float32(double(byte) - mean[c]) per cell, 0 = pad)
 //   conv tile    9 x 33 conv pixels x Cout             -> registers (5 px x 16 ch per thread)
 //                 -> +bias [*scale+shift], ReLU, -inf outside the image -> smem
 //   pooled tile  4 x 16 x Cout, max over 3x3 windows   -> 128-bit coalesced global stores
 // Threads: 64 per 16-channel group (Cout/16 groups).  Weights [k*k*3][Cout] live in smem.
 #include <math_constants.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -45,12 +49,27 @@ struct ConvPoolParams {
   int tiles_w, tiles_h;
 };
 
-template <int KS, int NT, int MINB>
+// The uint8-input instances' parameters (x unused).  A type of their own: a larger block in the
+// fp32 instances would change their code.
+struct ConvPoolU8Params : ConvPoolParams {
+  const uint8_t* x8;    // [B,H,W,3] BGR bytes, any byte alignment
+  double mean[3];       // subtracted per channel
+};
+
+// U8: the input is uint8 BGR (p.x8) and the patch cell of an in-image byte b of channel c is
+// float32(double(b) - mean[c]), exactly what u8_meansub_kernel writes for the fp32 path to read;
+// a padding cell is 0 either way.  Only the patch staging differs, so the outputs are bitwise
+// those of the fp32 instance on the converted images.
+template <int KS, int NT, int MINB, bool U8 = false>
 __global__ void __launch_bounds__(NT, MINB)
-conv_pool_simt_kernel(const ConvPoolParams p) {
+conv_pool_simt_kernel(const std::conditional_t<U8, ConvPoolU8Params, ConvPoolParams> p) {
   constexpr int PH = 2 * (CT_H - 1) + KS;          // input patch rows
   constexpr int PW = 2 * (CT_W - 1) + KS;          // input patch cols (pixels)
   constexpr int K = KS * KS * 3;
+  // U8 staging: the aligned 4-byte words covering a row's PW*3 bytes at any alignment, one row of
+  // SW words per patch row, in s_conv's space (free until epilogue 1)
+  constexpr int SW = (PW * 3 + 6) / 4;
+  static_assert(PH * SW <= CT_PIX * 16, "uint8 staging must fit in one channel group of s_conv");
   extern __shared__ __align__(16) float sm[];
   float* s_patch = sm;                             // [PH][PW*3]
   float* s_w = s_patch + ((PH * PW * 3 + 3) & ~3); // [K][Cout]
@@ -73,7 +92,51 @@ conv_pool_simt_kernel(const ConvPoolParams p) {
     const unsigned dst = (unsigned)__cvta_generic_to_shared(s_w + i * 4);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(p.w + i * 4) : "memory");
   }
-  {
+  if constexpr (U8) {
+    // One warp per in-image patch row: the words from the one holding the row's first needed
+    // byte to the one holding its last.  Each holds at least one byte of the row, so no load
+    // touches a padding row, another image or (allocations being 4-byte aligned) past an end.
+    const uint8_t* xin = p.x8 + (size_t)img * p.H * p.W * 3;
+    unsigned* s_stage = reinterpret_cast<unsigned*>(s_conv);
+    const int wid = tid >> 5, lane = tid & 31, nwarps = nthreads >> 5;
+    const int b0 = max(ix0 * 3, 0), b1 = min((ix0 + PW) * 3, p.W * 3);   // needed bytes of a row
+    for (int row = wid; row < PH; row += nwarps) {
+      const int iy = iy0 + row;
+      if (iy < 0 || iy >= p.H || b0 >= b1) continue;
+      const uintptr_t a0 = (uintptr_t)(xin + (size_t)iy * p.W * 3 + b0);
+      const uintptr_t w0 = a0 & ~(uintptr_t)3;
+      const int nw = (int)((a0 + (b1 - b0) + 3 - w0) >> 2);
+      for (int j = lane; j < nw; j += 32) {
+        const unsigned dst = (unsigned)__cvta_generic_to_shared(s_stage + row * SW + j);
+        asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(w0 + 4 * j)
+                     : "memory");
+      }
+    }
+    // each warp converts the rows it staged once its own copies have landed: no block barrier
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    __syncwarp();
+    const uint8_t* s_bytes = reinterpret_cast<const uint8_t*>(s_stage);
+    for (int row = wid; row < PH; row += nwarps) {
+      const int iy = iy0 + row;
+      const bool row_ok = iy >= 0 && iy < p.H;
+      // byte b of the row sits at (row start + b0) % 4 + b - b0 in the row's staged words
+      const int skew = row_ok ? (int)((uintptr_t)(xin + (size_t)iy * p.W * 3 + b0) & 3) - b0 : 0;
+#pragma unroll
+      for (int it = 0; it < (PW * 3 + 31) / 32; ++it) {
+        const int col = lane + it * 32;
+        if (col < PW * 3) {
+          const int ixc = ix0 * 3 + col;
+          float v = 0.f;                             // TF pads the mean-subtracted image with 0
+          if (row_ok && ixc >= b0 && ixc < b1) {
+            const int c = col % 3;
+            v = (float)((double)s_bytes[row * SW * 4 + skew + ixc] -
+                        (c == 0 ? p.mean[0] : c == 1 ? p.mean[1] : p.mean[2]));
+          }
+          s_patch[row * (PW * 3) + col] = v;
+        }
+      }
+    }
+  } else {
     const float* xin = p.x + (size_t)img * p.H * p.W * 3;
     const int wid = tid >> 5, lane = tid & 31, nwarps = nthreads >> 5;
     for (int row = wid; row < PH; row += nwarps) {       // one warp per patch row: coalesced
@@ -201,7 +264,12 @@ size_t smem_bytes_for(int Cout) {
                           (size_t)(Cout / 16) * CT_PIX * 16);
 }
 
-// The <KS, NT, MINB> instantiations, indexed by conv_pool_instance.
+// The <KS, NT, MINB> instantiations, indexed by conv_pool_instance.  The uint8 ones come first:
+// ptxas compiles a module's kernels last to first, and so compiles the fp32 ones as it did
+// before they existed (their SASS is unchanged).
+void (*const kConvPoolU8Kernels[4])(ConvPoolU8Params) = {
+    conv_pool_simt_kernel<3, 256, 2, true>, conv_pool_simt_kernel<3, 384, 1, true>,
+    conv_pool_simt_kernel<7, 256, 1, true>, conv_pool_simt_kernel<7, 384, 1, true>};
 void (*const kConvPoolKernels[4])(ConvPoolParams) = {
     conv_pool_simt_kernel<3, 256, 2>, conv_pool_simt_kernel<3, 384, 1>,
     conv_pool_simt_kernel<7, 256, 1>, conv_pool_simt_kernel<7, 384, 1>};
@@ -217,7 +285,8 @@ bool conv_pool_simt_eligible(int Cin, int Cout, int ksize, int stride, int pool_
          pool_stride == 2 && Cout % 16 == 0 && Cout >= 16 && Cout <= 96;
 }
 
-int launch_conv_pool_simt(const float* x, const float* w, const float* bias, const float* scale,
+int launch_conv_pool_simt(const float* x, const uint8_t* x8, const double* bgr_means,
+                          const float* w, const float* bias, const float* scale,
                           const float* shift, float* y, int B, int H, int W, int Cout, int ksize,
                           int conv_padding, int relu, int pool_padding, cudaStream_t stream) {
   if (!conv_pool_simt_eligible(3, Cout, ksize, 2, 3, 2))
@@ -241,17 +310,25 @@ int launch_conv_pool_simt(const float* x, const float* w, const float* bias, con
   if (smem > 232448) return fail(SQDET_ERR_UNSUPPORTED, "conv+pool: tile does not fit in smem");
   // Exactly `threads` threads: each 64 of them own one 16-channel group (cg = tid >> 6), and
   // s_conv / bias hold Cout / 16 groups.  The instance's NT is only the __launch_bounds__ ceiling.
-  const int inst = conv_pool_instance(ksize, threads);
+  const int u8 = x8 != nullptr, inst = conv_pool_instance(ksize, threads);
+  const void* fn = u8 ? (const void*)kConvPoolU8Kernels[inst] : (const void*)kConvPoolKernels[inst];
   // the opt-in is per device: remember which devices of this process already have it
-  static unsigned long long attr_devs[4] = {};
+  static unsigned long long attr_devs[2][4] = {};
   int dev = 0;
   SQ_CUDA(cudaGetDevice(&dev));
-  if (dev >= 64 || !((attr_devs[inst] >> dev) & 1ull)) {
-    SQ_CUDA(cudaFuncSetAttribute(kConvPoolKernels[inst], cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 232448));
-    if (dev < 64) attr_devs[inst] |= 1ull << dev;
+  if (dev >= 64 || !((attr_devs[u8][inst] >> dev) & 1ull)) {
+    SQ_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+    if (dev < 64) attr_devs[u8][inst] |= 1ull << dev;
   }
-  kConvPoolKernels[inst]<<<grid, threads, smem, stream>>>(p);
+  if (u8) {
+    ConvPoolU8Params q;
+    static_cast<ConvPoolParams&>(q) = p;
+    q.x8 = x8;
+    for (int c = 0; c < 3; ++c) q.mean[c] = bgr_means[c];
+    kConvPoolU8Kernels[inst]<<<grid, threads, smem, stream>>>(q);
+  } else {
+    kConvPoolKernels[inst]<<<grid, threads, smem, stream>>>(p);
+  }
   SQ_CHECK_LAUNCH("conv_pool_simt_kernel");
   return SQDET_OK;
 }

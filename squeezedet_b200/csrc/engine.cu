@@ -129,10 +129,12 @@ struct sqdet_engine {
   sqdet_det* d_dets = nullptr;
   int32_t* d_counts = nullptr;
   int max_dets = 0;
-  // CUDA graphs of one forward, keyed by (input, stream, image count, scales); small LRU-less cache
+  // CUDA graphs of one forward, keyed by (input, input type, stream, image count, scales); small
+  // LRU-less cache
   struct GraphEntry {
     cudaGraphExec_t exec = nullptr;
-    const float* input = nullptr;
+    const void* input = nullptr;
+    bool u8 = false;              // input is uint8 BGR (sqdet_forward_u8)
     cudaStream_t stream = nullptr;
     int n = 0;
     const float* scales = nullptr;
@@ -140,6 +142,9 @@ struct sqdet_engine {
   GraphEntry graphs[4];
   int graph_next = 0;
   bool use_graph = true;
+  // sqdet_forward_u8 hands its uint8 images to the first layer: the plan's only reader of tensor 0
+  // is a conv+pool launch.  Otherwise they are converted into tensor 0 first.
+  bool u8_fused = false;
   // pipelined host path (sqdet_submit / sqdet_wait), depth 2
   cudaStream_t copy_stream = nullptr;
   Slot slots[2];
@@ -286,9 +291,10 @@ static const float* input_ptr(const sqdet_engine* e, int t, const float* images)
 }
 
 // One launch over images [0, n): every kernel takes the image count as a launch argument, so a
-// forward of n < B images runs the kernels planned for B on smaller grids.
-static int run_launch(sqdet_engine* e, const Op& op, const Launch& l, const float* images, int n,
-                      cudaStream_t stream) {
+// forward of n < B images runs the kernels planned for B on smaller grids.  `u8`, when non-null,
+// is uint8 BGR images the conv+pool launch reads in place of tensor 0 (e->u8_fused).
+static int run_launch(sqdet_engine* e, const Op& op, const Launch& l, const float* images,
+                      const uint8_t* u8, int n, cudaStream_t stream) {
   const Tensor& in = e->tensors[l.src];
   const float* x = input_ptr(e, l.src, images);
   float* y = e->tensors[l.dst].dev;
@@ -312,7 +318,8 @@ static int run_launch(sqdet_engine* e, const Op& op, const Launch& l, const floa
       return launch_conv_tc(l.tc, x, y, n, stream);
     case L_CONV_POOL: {
       const ConvSpec& c = op.convs[0];
-      return launch_conv_pool_simt(x, e->params[c.p_kernel].dev,
+      const uint8_t* x8 = l.src == 0 ? u8 : nullptr;
+      return launch_conv_pool_simt(x8 ? nullptr : x, x8, e->bgr_means, e->params[c.p_kernel].dev,
                                    c.p_bias >= 0 ? e->params[c.p_bias].dev : nullptr, c.scale,
                                    c.shift, y, n, in.H, in.W, c.Cout, c.size, c.padding, c.relu,
                                    l.pool_padding, stream);
@@ -326,9 +333,10 @@ static int run_launch(sqdet_engine* e, const Op& op, const Launch& l, const floa
   return fail(SQDET_ERR_STATE, "unknown launch kind");
 }
 
-static int run_op(sqdet_engine* e, const Op& op, const float* images, int n, cudaStream_t stream) {
+static int run_op(sqdet_engine* e, const Op& op, const float* images, const uint8_t* u8, int n,
+                  cudaStream_t stream) {
   for (const Launch& l : op.launches) {
-    int rc = run_launch(e, op, l, images, n, stream);
+    int rc = run_launch(e, op, l, images, u8, n, stream);
     if (rc) return rc;
   }
   return SQDET_OK;
@@ -479,43 +487,66 @@ static int prepare_params(sqdet_engine* e) {
   return SQDET_OK;
 }
 
-static void drop_graph(sqdet_engine* e) {
+// Destroys the cached graphs, or only those of uint8 inputs.  A graph still running finishes first.
+static void drop_graph(sqdet_engine* e, bool only_u8 = false) {
   for (auto& g : e->graphs) {
+    if (only_u8 && !g.u8) continue;
     if (g.exec) cudaGraphExecDestroy(g.exec);
     g = sqdet_engine::GraphEntry();
   }
 }
 
-static int enqueue_all(sqdet_engine* e, const float* images_dev, int n, const float* scales,
+// The forward of fp32 images, or of uint8 BGR images (`u8`): handed to the first layer when the
+// plan fuses it, else converted into tensor 0 by one launch.  The uint8 images of a row or of an
+// image may start at any byte; the conversion kernel's word loads need a 4-byte aligned base, so
+// another base goes through the byte-wise same-size path of the resize kernel, over n*H rows.
+static int enqueue_all(sqdet_engine* e, const void* images, bool u8, int n, const float* scales,
                        cudaStream_t stream) {
+  const float* x = u8 ? nullptr : static_cast<const float*>(images);
+  const uint8_t* x8 = u8 ? static_cast<const uint8_t*>(images) : nullptr;
+  if (x8 && !e->u8_fused) {
+    const Tensor& t = e->tensors[0];
+    const double* m = e->bgr_means;
+    const int rc = ((uintptr_t)x8 & 3) == 0
+        ? launch_u8_meansub(x8, t.dev, (int64_t)n * t.H * t.W, m[0], m[1], m[2], stream)
+        : launch_resize_meansub_u8(x8, n * t.H, t.W, t.dev, n * t.H, t.W, m[0], m[1], m[2], 0,
+                                   stream);
+    if (rc) return rc;
+    x8 = nullptr;
+  }
   for (const auto& op : e->ops) {
-    int rc = run_op(e, op, images_dev, n, stream);
+    int rc = run_op(e, op, x, x8, n, stream);
     if (rc) return rc;
   }
   return run_postproc(e, n, scales, stream);
 }
 
-// The forward over images [0, n) of `images_dev`, 1 <= n <= B, rescaled by `scales` unless null.
-static int forward_impl(sqdet_engine* e, const float* images_dev, int n, const float* scales,
+// The forward over images [0, n) of `images` (uint8 BGR when `u8`, else fp32), 1 <= n <= B,
+// rescaled by `scales` unless null.
+static int forward_impl(sqdet_engine* e, const void* images, bool u8, int n, const float* scales,
                         cudaStream_t stream) {
   if (!e) return fail(SQDET_ERR_INVALID_ARG, "null engine");
-  if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_forward before sqdet_finalize");
-  if (!images_dev) return fail(SQDET_ERR_INVALID_ARG, "null images pointer");
+  if (!e->finalized)
+    return fail(SQDET_ERR_STATE, u8 ? "sqdet_forward_u8 before sqdet_finalize"
+                                    : "sqdet_forward before sqdet_finalize");
+  if (!images) return fail(SQDET_ERR_INVALID_ARG, "null images pointer");
   if (n < 1 || n > e->cfg.batch_size)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_n: n must be in [1, batch_size]");
+    return fail(SQDET_ERR_INVALID_ARG, u8 ? "sqdet_forward_u8: n must be in [1, batch_size]"
+                                          : "sqdet_forward_n: n must be in [1, batch_size]");
   DeviceGuard guard(e->device);
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
   int rc = prepare_params(e);
   if (rc) return rc;
   const bool can_graph = e->use_graph && stream != nullptr;   // legacy stream cannot capture
   if (!can_graph) {
-    rc = enqueue_all(e, images_dev, n, scales, stream);
+    rc = enqueue_all(e, images, u8, n, scales, stream);
     if (!rc) SQ_CUDA(cudaEventRecord(e->last_forward, stream));
     return rc;
   }
   sqdet_engine::GraphEntry* hit = nullptr;
   for (auto& g : e->graphs)
-    if (g.exec && g.input == images_dev && g.stream == stream && g.n == n && g.scales == scales)
+    if (g.exec && g.input == images && g.u8 == u8 && g.stream == stream && g.n == n &&
+        g.scales == scales)
       hit = &g;
   if (!hit) {
     sqdet_engine::GraphEntry& slot = e->graphs[e->graph_next];
@@ -524,7 +555,7 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, int n, const f
     slot = sqdet_engine::GraphEntry();
     cudaGraph_t graph = nullptr;
     SQ_CUDA(cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-    rc = enqueue_all(e, images_dev, n, scales, stream);
+    rc = enqueue_all(e, images, u8, n, scales, stream);
     cudaError_t ce = cudaStreamEndCapture(stream, &graph);
     if (rc) {
       if (graph) cudaGraphDestroy(graph);
@@ -534,7 +565,8 @@ static int forward_impl(sqdet_engine* e, const float* images_dev, int n, const f
     ce = cudaGraphInstantiate(&slot.exec, graph, 0);
     cudaGraphDestroy(graph);
     if (ce != cudaSuccess) return cuda_fail(ce, "cudaGraphInstantiate");
-    slot.input = images_dev;
+    slot.input = images;
+    slot.u8 = u8;
     slot.stream = stream;
     slot.n = n;
     slot.scales = scales;
@@ -592,7 +624,7 @@ static int upload(sqdet_engine* e, Slot& s, bool to_input, int count, const uint
 static int finish_submit(sqdet_engine* e, Slot& s, int n, const float* scales, sqdet_det* dets,
                          int32_t* counts) {
   cudaStream_t ks = e->own_stream;
-  int rc = forward_impl(e, s.input, n, scales, ks);
+  int rc = forward_impl(e, s.input, false, n, scales, ks);
   if (rc) return rc;
   if (dets)
     SQ_CUDA(cudaMemcpyAsync(dets, e->d_dets, sizeof(sqdet_det) * (size_t)n * e->max_dets,
@@ -960,6 +992,15 @@ static int plan_ops(sqdet_engine* e) {
     if (rc) return rc;
   }
   for (auto& op : e->ops) op.min_bytes = min_bytes(e, op);
+  int readers = 0;
+  bool pool_reads = false;
+  for (const auto& op : e->ops)
+    for (const auto& l : op.launches)
+      if (l.src == 0 || (l.kind == L_ADD_RELU && op.src2 == 0)) {
+        ++readers;
+        pool_reads = pool_reads || l.kind == L_CONV_POOL;
+      }
+  e->u8_fused = readers == 1 && pool_reads;
   return SQDET_OK;
 }
 
@@ -1072,7 +1113,11 @@ int sqdet_forward(sqdet_engine* e, const float* images_dev, void* stream) {
 }
 
 int sqdet_forward_n(sqdet_engine* e, const float* images_dev, int n, void* stream) {
-  return forward_impl(e, images_dev, n, e ? e->box_scale : nullptr, (cudaStream_t)stream);
+  return forward_impl(e, images_dev, false, n, e ? e->box_scale : nullptr, (cudaStream_t)stream);
+}
+
+int sqdet_forward_u8(sqdet_engine* e, const uint8_t* images_dev, int n, void* stream) {
+  return forward_impl(e, images_dev, true, n, e ? e->box_scale : nullptr, (cudaStream_t)stream);
 }
 
 int sqdet_forward_profiled(sqdet_engine* e, const float* images_dev, void* stream_v,
@@ -1093,7 +1138,7 @@ int sqdet_forward_profiled(sqdet_engine* e, const float* images_dev, void* strea
   const int B = e->cfg.batch_size;
   SQ_CUDA(cudaEventRecord(e->prof_events[0], stream));
   for (int i = 0; i < (int)e->ops.size(); ++i) {
-    rc = run_op(e, e->ops[i], images_dev, B, stream);
+    rc = run_op(e, e->ops[i], images_dev, nullptr, B, stream);
     if (rc) return rc;
     SQ_CUDA(cudaEventRecord(e->prof_events[i + 1], stream));
   }
@@ -1131,7 +1176,7 @@ int sqdet_detect(sqdet_engine* e, const float* images, float* det_boxes, float* 
   const sqdet_config& c = e->cfg;
   const size_t in_bytes = sizeof(float) * (size_t)e->tensors[0].numel();
   SQ_CUDA(cudaMemcpyAsync(e->slots[0].input, images, in_bytes, cudaMemcpyHostToDevice, stream));
-  int rc = forward_impl(e, e->slots[0].input, c.batch_size, e->box_scale, stream);
+  int rc = forward_impl(e, e->slots[0].input, false, c.batch_size, e->box_scale, stream);
   if (rc) return rc;
   const size_t BA = (size_t)c.batch_size * (size_t)e->num_anchors;
   if (det_boxes)
@@ -1152,6 +1197,11 @@ int sqdet_detect(sqdet_engine* e, const float* images, float* det_boxes, float* 
 
 int sqdet_set_bgr_means(sqdet_engine* e, const double bgr_means[3]) {
   if (!e || !bgr_means) return fail(SQDET_ERR_INVALID_ARG, "sqdet_set_bgr_means: null argument");
+  // a uint8 forward's graph holds the means it was captured with
+  if (memcmp(e->bgr_means, bgr_means, sizeof(e->bgr_means)) != 0) {
+    DeviceGuard guard(e->device);
+    drop_graph(e, true);
+  }
   for (int i = 0; i < 3; ++i) e->bgr_means[i] = bgr_means[i];
   return SQDET_OK;
 }

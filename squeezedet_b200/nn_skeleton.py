@@ -490,6 +490,13 @@ class ModelSkeleton:
     else:
       _lib.check(self._lib.sqdet_forward_n(self._engine, images_dev_ptr, int(n), stream))
 
+  def forward_device_u8(self, images_dev_ptr, stream=None, n=None):
+    """forward_device of uint8 BGR images [n, H, W, 3] at `images_dev_ptr` (any byte alignment),
+    as cv2.imread / cv2.resize leave them; the engine subtracts mc.BGR_MEANS (demo.py:190).  The
+    results are bitwise those of forward_device on the converted fp32 images (sqdet_forward_u8)."""
+    n = self.mc.BATCH_SIZE if n is None else int(n)
+    _lib.check(self._lib.sqdet_forward_u8(self._engine, images_dev_ptr, n, stream))
+
   def forward_profiled(self, images_dev_ptr, stream=None):
     n = self._lib.sqdet_num_ops(self._engine)
     ms = np.zeros(n, np.float32)
