@@ -453,6 +453,23 @@ __device__ __forceinline__ float finish(const TcParams& p, const TcChunk& ch, in
   return v;
 }
 
+// Stores channels c and c + 1 (c even) of an output row whose first `ncount` channels are valid,
+// value(c) giving each: one 8-byte store when `pair` (every row of the chunk starts 8-byte
+// aligned) and both are valid, else one 4-byte store per valid channel.
+template <typename Value>
+__device__ __forceinline__ void store_pair(float* yrow, int c, int ncount, bool pair, Value value) {
+  if (pair && c + 1 < ncount) {
+    *reinterpret_cast<float2*>(yrow + c) = make_float2(value(c), value(c + 1));
+  } else {
+    if (c < ncount) yrow[c] = value(c);
+    if (c + 1 < ncount) yrow[c + 1] = value(c + 1);
+  }
+}
+// Whether every output row of chunk ch starts 8-byte aligned.
+__device__ __forceinline__ bool rows_pair_aligned(const TcParams& p, const TcChunk& ch) {
+  return ((p.y_cstride | ch.y_off) & 1) == 0 && (reinterpret_cast<uintptr_t>(p.y) & 7) == 0;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Two CTAs per SM (the shared memory of 3 stages allows it up to NT = 72, KC = 32): at most 128
 // registers a thread.  The 72-wide tile fits them only with one accumulator set (mma_chunk's
@@ -624,6 +641,7 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
     }
     cluster_sync();   // no CTA exits while another may still read its partial tile
   } else {
+    const bool pair = rows_pair_aligned(p, ch);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       long long m = m0 + arow0 + 8 * h;   // output pixel
@@ -638,11 +656,8 @@ conv_tc_kernel(const __grid_constant__ TcParams p) {
       float* yrow = p.y + (size_t)m * p.y_cstride + ch.y_off;
 #pragma unroll
       for (int j = 0; j < NT / 8; ++j)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int c = 8 * j + 2 * t + e;
-          if (c < ch.ncount) yrow[c] = finish(p, ch, c, sum[4 * j + 2 * h + e]);
-        }
+        store_pair(yrow, 8 * j + 2 * t, ch.ncount, pair,
+                   [&](int c) { return finish(p, ch, c, sum[4 * j + 2 * h + (c & 1)]); });
     }
   }
 }
@@ -809,6 +824,7 @@ fire_tc_kernel(const __grid_constant__ TcParams p) {
       const HaloTile tl = halo_tile(p.tiles_w, p.tiles_h);
       const int oy = tl.oy0 + r;
       const size_t prow = ((size_t)tl.n * p.H + oy) * p.W;
+      const bool pair = rows_pair_aligned(p, ch);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int ox = tl.ox0 + g + 8 * h;
@@ -816,11 +832,9 @@ fire_tc_kernel(const __grid_constant__ TcParams p) {
         float* yrow = p.y + (prow + ox) * p.y_cstride + ch.y_off;
 #pragma unroll
         for (int jn = 0; jn < 8; ++jn)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int col = 8 * jn + 2 * t + e;
-            if (col < ch.ncount) yrow[col] = fmaxf(sum[4 * jn + 2 * h + e] + p.bias[ch.p_off + col], 0.f);
-          }
+          store_pair(yrow, 8 * jn + 2 * t, ch.ncount, pair, [&](int col) {
+            return fmaxf(sum[4 * jn + 2 * h + (col & 1)] + p.bias[ch.p_off + col], 0.f);
+          });
       }
 #pragma unroll
       for (int i = 0; i < 32; ++i) sum[i] = 0.f;
@@ -978,9 +992,14 @@ static long long grid_blocks(const TcImpl* im, int n) {
 }
 
 // Plans the convs of im->groups over one [B, H, W, Cin] input into a [B, Ho, Wo, y_cstride]
-// output, for the mode, kernel and group tiling already in im: their chunks in group order, the
-// kernel's shared memory, and the weight, bias and affine buffers.  Returns 1 (planned),
-// 0 (declined) or a negative status.
+// output, for the mode, kernel and group tiling already in im: their chunks, the kernel's shared
+// memory, and the weight, bias and affine buffers.  Returns 1 (planned), 0 (declined) or a
+// negative status.
+//
+// The chunks follow group order, except that halo mode numbers its 3x3 convs' chunks first.  The
+// block scheduler starts a grid's CTAs in blockIdx order, so an expand pair's long 3x3 CTAs (9x
+// the K chunks of its 1x1 CTAs) start first and the short 1x1 CTAs fill the last wave, instead of
+// a last wave of 3x3 CTAs running on a partly idle GPU.
 static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo, int stride,
                        int pad_t, int pad_l, int relu, bool has_affine, int y_cstride) {
   const bool gather = im->mode == TC_GATHER;
@@ -989,9 +1008,18 @@ static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo,
   p.relu = relu; p.y_cstride = y_cstride; p.M = (long long)B * Ho * Wo;
   p.tiles_w = (Wo + FT_W - 1) / FT_W; p.tiles_h = (Ho + 7) / 8;
   if (p.M <= 0 || grid_blocks(im, B) > 0x7fffffffLL) return 0;
-  int nch = 0, poff = 0;
+  // each group's first bias / scale / shift entry, in group order (tc_conv_pack_weights)
+  std::vector<int> poffs;
+  int poff = 0;
+  for (const auto& g : im->groups) poffs.push_back(poff), poff += g.conv.Cout;
+  std::vector<size_t> order;
+  for (int pass = 0; pass < 2; ++pass)
+    for (size_t gi = 0; gi < im->groups.size(); ++gi)
+      if ((im->mode == TC_HALO && im->groups[gi].conv.ksize == 3) == (pass == 0)) order.push_back(gi);
+  int nch = 0;
   long long woff = 0;
-  for (auto& g : im->groups) {
+  for (const size_t gi : order) {
+    PlanGroup& g = im->groups[gi];
     g.chunk0 = nch;
     const int taps = g.conv.ksize * g.conv.ksize;
     const int nk = gather ? (taps * g.cin + g.KC - 1) / g.KC : taps * (g.cin / g.KC);
@@ -1003,11 +1031,10 @@ static int plan_common(TcImpl* im, int B, int H, int W, int Cin, int Ho, int Wo,
       c.nk = nk;
       c.ncount = g.conv.Cout - cb < g.NT ? g.conv.Cout - cb : g.NT;
       c.y_off = g.conv.y_off + cb;
-      c.p_off = poff + cb;
+      c.p_off = poffs[gi] + cb;
       c.w_off = woff;
       woff += (long long)nk * 2 * g.NT * g.KC;
     }
-    poff += g.conv.Cout;
   }
   p.nchunks = nch;
   im->cout_total = poff;
