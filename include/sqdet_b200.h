@@ -186,14 +186,17 @@ int sqdet_detect(sqdet_engine* e, const float* images, float* det_boxes,
                  float* det_probs, int64_t* det_class, sqdet_det* dets,
                  int32_t* counts, void* stream);
 /* Pipelined host-buffer path (depth 2): sqdet_submit enqueues H2D (own copy stream) ->
- * [uint8 -> fp32 - mc.BGR_MEANS on the GPU] -> forward -> D2H of the filtered records and
- * returns at once; sqdet_wait blocks until the OLDEST outstanding submit has delivered into its
- * dets/counts buffers.  With two submits in flight the copy of batch i+1 overlaps the compute
- * of batch i.  img_type SQDET_IMG_F32: [B,H,W,3] fp32 BGR, mean-subtracted (feed_dict
- * semantics, src/demo.py:190-195); SQDET_IMG_U8: [B,H,W,3] uint8 BGR exactly as cv2.imread /
- * cv2.resize leave it (src/demo.py:187-189) - the engine applies `im - mc.BGR_MEANS`
- * (src/demo.py:190, src/dataset/imdb.py:88).  Host buffers must stay valid (and should be
- * pinned) until the matching sqdet_wait.  SQDET_ERR_STATE if two submits are already pending. */
+ * forward -> D2H of the filtered records and returns at once; sqdet_wait blocks until the
+ * OLDEST outstanding submit has delivered into its dets/counts buffers.  With two submits in
+ * flight the copy of batch i+1 overlaps the compute of batch i.  img_type SQDET_IMG_F32:
+ * [B,H,W,3] fp32 BGR, mean-subtracted (feed_dict semantics, src/demo.py:190-195), uploaded into
+ * a buffer of the submission's own, not tensor 0; SQDET_IMG_U8: [B,H,W,3] uint8 BGR exactly as
+ * cv2.imread / cv2.resize leave it (src/demo.py:187-189), uploaded as bytes and run by the
+ * forward of sqdet_forward_u8, under its rules: the engine applies `im - mc.BGR_MEANS`
+ * (src/demo.py:190, src/dataset/imdb.py:88) in the fused first layer, leaving tensor 0 as it
+ * was, or in one launch that converts the batch into tensor 0.  Host buffers must stay valid
+ * (and should be pinned) until the matching sqdet_wait.  SQDET_ERR_STATE if two submits are
+ * already pending.                                                                           */
 #define SQDET_IMG_F32 0
 #define SQDET_IMG_U8  1
 int sqdet_set_bgr_means(sqdet_engine* e, const double bgr_means[3]);   /* mc.BGR_MEANS */

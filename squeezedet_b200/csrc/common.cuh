@@ -68,8 +68,6 @@ int launch_maxpool(const float* x, float* y, int B, int H, int W, int C, int siz
                    int stride, int padding, cudaStream_t stream);
 int launch_resize_meansub_u8(const uint8_t* src, int H0, int W0, float* dst, int H, int W,
                              double m0, double m1, double m2, int sub_first, cudaStream_t stream);
-int launch_u8_meansub(const uint8_t* src, float* dst, int64_t n_pixels, double m0, double m1,
-                      double m2, cudaStream_t stream);
 int launch_add_relu(const float* a, const float* b, float* y, int64_t n, cudaStream_t stream);
 
 int launch_interpret(const float* preds, const float* anchors, float* boxes, float* probs,

@@ -57,9 +57,9 @@ struct ConvPoolU8Params : ConvPoolParams {
 };
 
 // U8: the input is uint8 BGR (p.x8) and the patch cell of an in-image byte b of channel c is
-// float32(double(b) - mean[c]), exactly what u8_meansub_kernel writes for the fp32 path to read;
-// a padding cell is 0 either way.  Only the patch staging differs, so the outputs are bitwise
-// those of the fp32 instance on the converted images.
+// float32(double(b) - mean[c]), exactly what the engine's conversion launch writes for the fp32
+// path to read; a padding cell is 0 either way.  Only the patch staging differs, so the outputs
+// are bitwise those of the fp32 instance on the converted images.
 template <int KS, int NT, int MINB, bool U8 = false>
 __global__ void __launch_bounds__(NT, MINB)
 conv_pool_simt_kernel(const std::conditional_t<U8, ConvPoolU8Params, ConvPoolParams> p) {

@@ -96,7 +96,7 @@ struct Op {
 
 // One of the two pipeline slots of the host path (sqdet_submit, sqdet_submit_frames_n).
 struct Slot {
-  float* input = nullptr;        // fp32 network input; slot 0's is tensors[0].dev
+  float* input = nullptr;        // fp32 network input
   uint8_t* staging = nullptr;    // uint8 images or frames as uploaded; grow-only
   size_t staging_cap = 0;
   float* scales = nullptr;       // B (x_scale, y_scale) pairs of a rescaled frames submission
@@ -497,9 +497,8 @@ static void drop_graph(sqdet_engine* e, bool only_u8 = false) {
 }
 
 // The forward of fp32 images, or of uint8 BGR images (`u8`): handed to the first layer when the
-// plan fuses it, else converted into tensor 0 by one launch.  The uint8 images of a row or of an
-// image may start at any byte; the conversion kernel's word loads need a 4-byte aligned base, so
-// another base goes through the byte-wise same-size path of the resize kernel, over n*H rows.
+// plan fuses it, else converted into tensor 0 by one launch: the byte-wise same-size path of the
+// resize kernel over n*H rows, which reads images starting at any byte.
 static int enqueue_all(sqdet_engine* e, const void* images, bool u8, int n, const float* scales,
                        cudaStream_t stream) {
   const float* x = u8 ? nullptr : static_cast<const float*>(images);
@@ -507,10 +506,8 @@ static int enqueue_all(sqdet_engine* e, const void* images, bool u8, int n, cons
   if (x8 && !e->u8_fused) {
     const Tensor& t = e->tensors[0];
     const double* m = e->bgr_means;
-    const int rc = ((uintptr_t)x8 & 3) == 0
-        ? launch_u8_meansub(x8, t.dev, (int64_t)n * t.H * t.W, m[0], m[1], m[2], stream)
-        : launch_resize_meansub_u8(x8, n * t.H, t.W, t.dev, n * t.H, t.W, m[0], m[1], m[2], 0,
-                                   stream);
+    const int rc = launch_resize_meansub_u8(x8, n * t.H, t.W, t.dev, n * t.H, t.W, m[0], m[1],
+                                            m[2], 0, stream);
     if (rc) return rc;
     x8 = nullptr;
   }
@@ -584,8 +581,8 @@ static int begin_submit(sqdet_engine* e, const char* what, Slot** slot) {
     return fail(SQDET_ERR_STATE, std::string(what) + ": two batches already in flight; call sqdet_wait");
   if (!e->copy_stream) {
     SQ_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-    SQ_CUDA(cudaMalloc(&e->slots[1].input, sizeof(float) * (size_t)e->tensors[0].numel()));
     for (Slot& s : e->slots) {
+      SQ_CUDA(cudaMalloc(&s.input, sizeof(float) * (size_t)e->tensors[0].numel()));
       SQ_CUDA(cudaEventCreateWithFlags(&s.h2d, cudaEventDisableTiming));
       SQ_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
     }
@@ -619,12 +616,13 @@ static int upload(sqdet_engine* e, Slot& s, bool to_input, int count, const uint
   return SQDET_OK;
 }
 
-// The forward over images [0, n) of the slot's input on the compute stream, then their records
-// and counts back to the caller's buffers; `done` marks the slot's buffers free again.
-static int finish_submit(sqdet_engine* e, Slot& s, int n, const float* scales, sqdet_det* dets,
-                         int32_t* counts) {
+// The forward over images [0, n) of `input`, one of the slot's buffers (uint8 BGR when `u8`, else
+// fp32), on the compute stream, then their records and counts back to the caller's buffers;
+// `done` marks the slot's buffers free again.
+static int finish_submit(sqdet_engine* e, Slot& s, const void* input, bool u8, int n,
+                         const float* scales, sqdet_det* dets, int32_t* counts) {
   cudaStream_t ks = e->own_stream;
-  int rc = forward_impl(e, s.input, false, n, scales, ks);
+  int rc = forward_impl(e, input, u8, n, scales, ks);
   if (rc) return rc;
   if (dets)
     SQ_CUDA(cudaMemcpyAsync(dets, e->d_dets, sizeof(sqdet_det) * (size_t)n * e->max_dets,
@@ -706,7 +704,7 @@ int sqdet_destroy(sqdet_engine* e) {
   cudaFree(e->d_dets);   // also owns d_counts (one blob)
   for (auto ev : e->prof_events) cudaEventDestroy(ev);
   for (Slot& s : e->slots) {
-    if (&s != &e->slots[0]) cudaFree(s.input);   // slot 0's input is tensors[0].dev
+    cudaFree(s.input);
     cudaFree(s.staging);
     cudaFree(s.scales);
     if (s.h2d) cudaEventDestroy(s.h2d);
@@ -861,7 +859,6 @@ int sqdet_finalize(sqdet_engine* e) {
     if (!t.materialized) continue;
     SQ_CUDA(cudaMalloc(&t.dev, sizeof(float) * (size_t)t.numel()));
   }
-  e->slots[0].input = e->tensors[0].dev;
   const int64_t A = e->num_anchors, B = c.batch_size;
   std::vector<float> anc((size_t)A * 4);
   for (size_t i = 0; i < anc.size(); ++i) anc[i] = (float)e->anchors_f64[i];   // fp64 -> fp32 cast
@@ -1175,8 +1172,8 @@ int sqdet_detect(sqdet_engine* e, const float* images, float* det_boxes, float* 
   cudaStream_t stream = stream_v ? (cudaStream_t)stream_v : e->own_stream;
   const sqdet_config& c = e->cfg;
   const size_t in_bytes = sizeof(float) * (size_t)e->tensors[0].numel();
-  SQ_CUDA(cudaMemcpyAsync(e->slots[0].input, images, in_bytes, cudaMemcpyHostToDevice, stream));
-  int rc = forward_impl(e, e->slots[0].input, false, c.batch_size, e->box_scale, stream);
+  SQ_CUDA(cudaMemcpyAsync(e->tensors[0].dev, images, in_bytes, cudaMemcpyHostToDevice, stream));
+  int rc = forward_impl(e, e->tensors[0].dev, false, c.batch_size, e->box_scale, stream);
   if (rc) return rc;
   const size_t BA = (size_t)c.batch_size * (size_t)e->num_anchors;
   if (det_boxes)
@@ -1224,15 +1221,8 @@ int sqdet_submit(sqdet_engine* e, const void* images, int img_type, sqdet_det* d
   const size_t off = 0;
   rc = upload(e, *s, !u8, 1, &src, &bytes, &off);
   if (rc) return rc;
-  if (u8) {
-    // on the COMPUTE stream: on the copy stream (to overlap the previous batch's forward) it was
-    // measured slower, 2.08 vs 1.93 ms per step end to end - its CTAs wait for the persistent
-    // one-CTA-per-SM kernels of that forward and then delay this batch's first layer
-    rc = launch_u8_meansub(s->staging, s->input, n_pix, e->bgr_means[0], e->bgr_means[1],
-                           e->bgr_means[2], e->own_stream);
-    if (rc) return rc;
-  }
-  return finish_submit(e, *s, c.batch_size, e->box_scale, dets, counts);
+  return finish_submit(e, *s, u8 ? (const void*)s->staging : s->input, u8, c.batch_size,
+                       e->box_scale, dets, counts);
 }
 
 int sqdet_wait(sqdet_engine* e) {
@@ -1330,7 +1320,7 @@ int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
                                   e->bgr_means[2], order == SQDET_PRE_SUB_THEN_RESIZE, ks);
     if (rc) return rc;
   }
-  return finish_submit(e, *s, n, rescale ? s->scales : nullptr, dets, counts);
+  return finish_submit(e, *s, s->input, false, n, rescale ? s->scales : nullptr, dets, counts);
 }
 
 // ---- multi-GPU: ONE all-gather of the filtered records ---------------------------------------------

@@ -138,35 +138,6 @@ add_relu_kernel(const float* __restrict__ a, const float* __restrict__ b,
   }
 }
 
-// uint8 BGR -> fp32, minus the per-channel mean: float32(double(u8) - mean), the value the
-// reference feeds (src/demo.py:187-190: float32 image, float64 BGR_MEANS, cast at the feed).
-// One thread = 4 pixels = 12 input bytes = three 128-bit output stores.
-__global__ void __launch_bounds__(256)
-u8_meansub_kernel(const uint8_t* __restrict__ src, float* __restrict__ dst, long long n_quads,
-                  long long n_pixels, double m0, double m1, double m2) {
-  const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= n_quads) return;
-  const double mean[3] = {m0, m1, m2};
-  if ((q + 1) * 4 <= n_pixels) {
-    const uint3 w = *reinterpret_cast<const uint3*>(src + q * 12);     // 12 bytes, 4-aligned
-    const unsigned words[3] = {w.x, w.y, w.z};
-    float o[12];
-#pragma unroll
-    for (int i = 0; i < 12; ++i) {
-      const unsigned b = (words[i >> 2] >> (8 * (i & 3))) & 0xffu;
-      o[i] = (float)((double)b - mean[i % 3]);
-    }
-    float4* d = reinterpret_cast<float4*>(dst + q * 12);
-    d[0] = make_float4(o[0], o[1], o[2], o[3]);
-    d[1] = make_float4(o[4], o[5], o[6], o[7]);
-    d[2] = make_float4(o[8], o[9], o[10], o[11]);
-  } else {
-    for (long long px = q * 4; px < n_pixels; ++px)
-      for (int c = 0; c < 3; ++c)
-        dst[px * 3 + c] = (float)((double)src[px * 3 + c] - mean[c]);
-  }
-}
-
 // uint8 BGR [H0, W0, 3] -> fp32 [H, W, 3]: cv2.resize (float32, INTER_LINEAR) and the mean
 // subtraction, in the reference's two orders (src/demo.py:187-190: resize, then `- BGR_MEANS`
 // in float64; src/dataset/imdb.py:87-91: float32 `-= BGR_MEANS`, then resize).  Restates
@@ -240,16 +211,6 @@ int launch_resize_meansub_u8(const uint8_t* src, int H0, int W0, float* dst, int
   resize_meansub_u8_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
       src, dst, H0, W0, H, W, scale_x, scale_y, m0, m1, m2, sub_first);
   SQ_CHECK_LAUNCH("resize_meansub_u8_kernel");
-  return SQDET_OK;
-}
-
-int launch_u8_meansub(const uint8_t* src, float* dst, int64_t n_pixels, double m0, double m1,
-                      double m2, cudaStream_t stream) {
-  if (n_pixels <= 0) return fail(SQDET_ERR_INVALID_ARG, "u8_meansub: empty image");
-  const long long quads = (n_pixels + 3) / 4;
-  u8_meansub_kernel<<<(unsigned)((quads + 255) / 256), 256, 0, stream>>>(src, dst, quads, n_pixels,
-                                                                         m0, m1, m2);
-  SQ_CHECK_LAUNCH("u8_meansub_kernel");
   return SQDET_OK;
 }
 

@@ -4,7 +4,6 @@
     oracle.filter_prediction;
   * add_relu_kernel's float4 body, tail and unaligned paths, including an add+ReLU whose operand
     is the image input and therefore reads the caller's images buffer;
-  * u8_meansub_kernel's tail (B * H * W not a multiple of 4);
   * sqdet_conv2d argument validation, the same in both math modes.
 tests/test_host_logic.py restates each branch predicate and checks that the tables below reach
 every branch."""
@@ -16,7 +15,7 @@ from squeezedet_b200 import _lib
 from squeezedet_b200 import config as cfg
 from squeezedet_b200.nn_skeleton import ModelSkeleton
 from squeezedet_b200.utils import synth
-from gpu_util import build, fetch_results, make_net, topk_nms_gpu
+from gpu_util import fetch_results, make_net, topk_nms_gpu
 
 pytestmark = pytest.mark.gpu
 ERR_INVALID_ARG = -1
@@ -187,27 +186,6 @@ def test_add_relu_paths(case, gpu_device):
       assert got_res[key].tobytes() == want_res[key].tobytes(), key
     for key in want_act:
       assert got_act[key].tobytes() == want_act[key].tobytes(), key
-
-
-# ---- uint8 mean subtraction tail ----------------------------------------------------------------
-U8_CASES = [(1, 9, 29), (1, 10, 31), (1, 11, 25), (3, 7, 13)]   # B * H * W % 4 = 1, 2, 3, 1
-
-
-@pytest.mark.parametrize('B,H,W', U8_CASES)
-def test_u8_meansub_tail(B, H, W, gpu_device):
-  """One submit(IMG_U8) on a fresh engine lands in tensor 0's buffer: it holds
-  float32(float64(u8) - BGR_MEANS) bit for bit, and the records equal those of the fp32 feed."""
-  mc, model, _ = build([('conv', 'conv1', 16, 3, 1, 'SAME')], B, H, W, _lib.MATH_TF32X3_TC,
-                       gpu_device)
-  rng = np.random.default_rng(B * H * W)
-  u8 = rng.integers(0, 256, (B, H, W, 3), dtype=np.uint8)
-  dets_u8, counts_u8 = model.detect_u8(u8)
-  feed = (u8.astype(np.float64) - np.asarray(mc.BGR_MEANS, np.float64).reshape(3)).astype(
-      np.float32)
-  assert model.read_tensor('image_input').tobytes() == feed.tobytes()
-  dets, counts = model.detect_records(feed)
-  assert np.array_equal(counts, counts_u8) and counts.min() >= 0
-  assert dets.tobytes() == dets_u8.tobytes()
 
 
 # ---- conv argument validation -------------------------------------------------------------------

@@ -271,6 +271,64 @@ def test_path_choice(case, gpu_device):
   assert model.launches_per_forward() == base
 
 
+TAIL_CASES = [(1, 9, 29), (1, 10, 31), (1, 11, 25), (3, 7, 13)]   # B * H * W % 4 = 1, 2, 3, 1
+
+
+@pytest.mark.parametrize('B,H,W', TAIL_CASES)
+def test_converted_tail(B, H, W, gpu_device):
+  """The converted path at pixel counts that are not a multiple of 4: tensor 0 holds
+  float32(float64(u8) - BGR_MEANS) bit for bit, and the records equal those of the fp32 feed."""
+  mc, model, _ = build([('conv', 'conv1', 16, 3, 1, 'SAME')], B, H, W, _lib.MATH_TF32X3_TC,
+                       gpu_device)
+  u8 = random_u8((B, H, W, 3), seed=B * H * W)
+  forward_u8(model, u8)
+  got = fetch_results(model, gpu_device)
+  feed = converted(u8, mc.BGR_MEANS)
+  assert image_input(model).tobytes() == feed.tobytes()
+  dets, counts = model.detect_records(feed)
+  assert np.array_equal(counts, got['counts']) and counts.min() >= 0
+  assert dets.tobytes() == got['dets'].tobytes()
+
+
+# ---- pipelined submissions (sqdet_submit) take the same path ----------------------------------
+def test_submit_u8_fused_leaves_tensor0(gpu_device):
+  """On a fused plan a uint8 submission runs no conversion: after sqdet_detect of fp32 images A,
+  submissions of other bytes B (one per slot) leave A in tensor 0, and their records equal those
+  of the fp32 feed of B."""
+  model = squeezedet_small(2, gpu_device)
+  mc = model.mc
+  shape = (2, mc.IMAGE_HEIGHT, mc.IMAGE_WIDTH, 3)
+  u8 = random_u8(shape, seed=18)
+  want_dets, want_counts = model.detect_records(converted(u8, mc.BGR_MEANS))
+  feed = synth.synthetic_images(2, mc.IMAGE_HEIGHT, mc.IMAGE_WIDTH, seed=19)
+  model.detect(feed)
+  for slot in (0, 1):
+    dets, counts = model.detect_u8(u8)
+    assert np.array_equal(counts, want_counts) and dets.tobytes() == want_dets.tobytes(), slot
+    assert image_input(model).tobytes() == feed.tobytes(), slot
+
+
+def test_submit_mixed_types_converted(gpu_device):
+  """On a plan that converts into tensor 0, four submissions with two in flight, fp32 in slot 0
+  and uint8 in slot 1: every submission's records equal its synchronous run's."""
+  B, H, W = 2, 96, 320
+  mc, model, _ = build([('conv', 'conv1', 32, 3, 1, 'SAME'), ('pool', 'pool1', 3, 2, 'SAME')], B,
+                       H, W, _lib.MATH_TF32X3_TC, gpu_device)
+  srcs = [synth.synthetic_images(B, H, W, seed=20 + i) if i % 2 == 0 else
+          random_u8((B, H, W, 3), seed=20 + i) for i in range(4)]
+  want = [model.detect_records(x if i % 2 == 0 else converted(x, mc.BGR_MEANS))
+          for i, x in enumerate(srcs)]
+  outs = [(np.empty((B, model.max_dets), _lib.DET_DTYPE), np.empty((B,), np.int32)) for _ in srcs]
+  for i, x in enumerate(srcs):
+    model.submit(x.ctypes.data, outs[i][0].ctypes.data, outs[i][1].ctypes.data,
+                 _lib.IMG_F32 if i % 2 == 0 else _lib.IMG_U8)
+    if i >= 1:
+      model.wait()
+  model.wait()
+  for i, ((d, c), (wd, wc)) in enumerate(zip(outs, want)):
+    assert np.array_equal(c, wc) and wc.min() >= 0 and d.tobytes() == wd.tobytes(), i
+
+
 # ---- refused calls write nothing ------------------------------------------------------------------
 def test_errors_before_device_work(gpu_device):
   model = squeezedet_small(2, gpu_device)

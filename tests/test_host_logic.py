@@ -207,11 +207,6 @@ def add_relu_branch(n, aligned):
   return 'vector + tail' if n % 4 else 'vector'
 
 
-def u8_meansub_branch(n_pixels):
-  """u8_meansub_kernel (pool.cu): quads of 4 pixels, then a tail of n_pixels % 4."""
-  return 'with tail' if n_pixels % 4 else 'vector only'
-
-
 FILTER_THREADS, FILTER_KCACHE, FILTER_CAP = 1024, 24, 1024     # postproc.cu FT, KCACHE, FCAP
 
 
@@ -225,9 +220,9 @@ def filter_branch(A, top_n, n_above, max_dets):
   return 'threshold overflow' if n_above > min(FILTER_CAP, max_dets) else 'threshold'
 
 
-def test_gpu_case_tables_reach_every_pool_add_relu_meansub_filter_branch():
-  """The GPU tables run every branch of the max-pool, add+ReLU, uint8 mean subtraction and filter
-  launchers, by the host rules above, and both sides of the filter's register cache."""
+def test_gpu_case_tables_reach_every_pool_add_relu_filter_branch():
+  """The GPU tables run every branch of the max-pool, add+ReLU and filter launchers, by the host
+  rules above, and both sides of the filter's register cache."""
   import test_gpu_branches as br
   from test_gpu_kernels import MAXPOOL_CASES, MAXPOOL_MISALIGNED_CASES
   pool = {maxpool_branch(shape[3], k, s) for shape, k, s, _ in MAXPOOL_CASES}
@@ -241,10 +236,6 @@ def test_gpu_case_tables_reach_every_pool_add_relu_meansub_filter_branch():
          for body, B, H, W, off in br.ADD_RELU_CASES}
   assert add == {'vector', 'vector + tail', 'unaligned'}, add
   assert any(body == 'image' and off is not None for body, _, _, _, off in br.ADD_RELU_CASES)
-  u8 = {u8_meansub_branch(B * H * W) for B, H, W in br.U8_CASES}
-  assert u8 == {'with tail'} and {B * H * W % 4 for B, H, W in br.U8_CASES} == {1, 2, 3}
-  # every other test feeds whole quads (2 x 96 x 320 in test_gpu_e2e)
-  assert u8_meansub_branch(2 * 96 * 320) == 'vector only'
   filt = {}
   for A, top_n, n_above, max_dets, _, _ in br.FILTER_CASES:
     if max_dets is None:
