@@ -223,6 +223,26 @@ int sqdet_submit_frames(sqdet_engine* e, const uint8_t* const* frames,
 int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
                           const int32_t* heights, const int32_t* widths, int order,
                           int rescale, sqdet_det* dets, int32_t* counts);
+/* n uint8 BGR frames already in device memory on the engine's device (a hardware decoder's
+ * output, torch CUDA tensors, crops of larger frames): frame i is heights[i] rows of widths[i]*3
+ * bytes, row r at frames_dev[i] + r*row_pitches[i] (NULL row_pitches = 3*widths[i]; any byte
+ * alignment).  Host arrays of n entries, 1 <= n <= B.  Resize + `- mc.BGR_MEANS` in `order` as
+ * sqdet_submit_frames_n, bit for bit, into tensor 0, then the forward of sqdet_forward_n on
+ * `stream`; rescale != 0 divides det boxes by each frame's scales before the filter (this call
+ * only; the sqdet_set_box_scale table is not applied).  Asynchronous; no host synchronisation.
+ *   - Afterwards rows [0, n) of tensor 0 (sqdet_read_tensor(0)) hold the resized fp32 images.
+ *   - Launches: sqdet_launches_per_forward (without a box-scale table), plus one resize launch
+ *     per 64 frames (so one for every n <= B <= 64), plus the rescale launch when rescale != 0.
+ *   - Refused before any device work, leaving graphs, pipeline and tensor 0 untouched:
+ *     SQDET_ERR_INVALID_ARG for a null engine or array, n outside [1, B], an unknown order, a
+ *     null frame, heights[i] or widths[i] <= 0, row_pitches[i] < 3*widths[i], or a frame whose
+ *     bytes [p, p + (h-1)*pitch + 3*w) are not device memory of the engine's device inside one
+ *     allocation (a host pointer, a frame longer than its buffer); SQDET_ERR_STATE before
+ *     sqdet_finalize.
+ * Like sqdet_forward_u8, one engine per stream: results are read through sqdet_results_dev.   */
+int sqdet_forward_frames_u8(sqdet_engine* e, int n, const uint8_t* const* frames_dev,
+                            const int32_t* heights, const int32_t* widths,
+                            const int64_t* row_pitches, int order, int rescale, void* stream);
 /* src/eval.py:83-84 for callers that resize on the host: xy_scales = B pairs (x_scale,
  * y_scale), host memory; every later forward of the paths fed already-resized images
  * (sqdet_forward(_n), sqdet_forward_profiled, sqdet_detect, sqdet_submit) divides

@@ -66,8 +66,26 @@ int launch_conv_pool_simt(const float* x, const uint8_t* x8, const double* bgr_m
 
 int launch_maxpool(const float* x, float* y, int B, int H, int W, int C, int size,
                    int stride, int padding, cudaStream_t stream);
-int launch_resize_meansub_u8(const uint8_t* src, int H0, int W0, float* dst, int H, int W,
-                             double m0, double m1, double m2, int sub_first, cudaStream_t stream);
+// One uint8 BGR frame of the batched resize: h rows of w * 3 bytes, row r at src + r * pitch
+// (any byte alignment), sampled at cv::resize's double scales; box_scale_* are the eval-order
+// box scales (IMAGE_WIDTH / w, IMAGE_HEIGHT / h) as float32.
+struct ResizeFrame {
+  const uint8_t* src;
+  int64_t pitch;
+  double scale_x, scale_y;
+  float box_scale_x, box_scale_y;
+  int h, w;
+};
+// Frames per launch: their descriptors stay inside the classic 4 KiB parameter block.
+constexpr int kResizeFramesPerLaunch = 64;
+// The descriptor of frame (src, pitch, h, w) resized to H x W.
+ResizeFrame resize_frame(const uint8_t* src, int64_t pitch, int h, int w, int H, int W);
+// cv2.resize (float32 INTER_LINEAR) to H x W + `- means` in either order of n frames into the fp32
+// batch [n, H, W, 3] at dst, one launch per kResizeFramesPerLaunch frames.  With scales_xy, each
+// frame's (box_scale_x, box_scale_y) also goes to scales_xy[2i], [2i + 1] on the device.
+int launch_resize_meansub_u8_batch(const ResizeFrame* frames, int n, float* dst, int H, int W,
+                                   const double* means, int sub_first, float* scales_xy,
+                                   cudaStream_t stream);
 int launch_add_relu(const float* a, const float* b, float* y, int64_t n, cudaStream_t stream);
 
 int launch_interpret(const float* preds, const float* anchors, float* boxes, float* probs,

@@ -8,6 +8,7 @@
 // weight storage in HBM, BN folding to (scale, shift), kernel selection per op
 // (wgmma 3xTF32 implicit GEMM or fp32 SIMT), CUDA-graph capture of the whole forward,
 // and the fused post-processing.
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <math.h>
@@ -156,6 +157,9 @@ struct sqdet_engine {
   cudaEvent_t last_forward = nullptr;
   std::vector<cudaEvent_t> prof_events;
   float* box_scale = nullptr;     // sqdet_set_box_scale's B (x_scale, y_scale) pairs, or null
+  // sqdet_forward_frames_u8's B (x_scale, y_scale) pairs, written by its resize launch; one
+  // address for the engine's life, so the forward graphs keyed on it stay valid
+  float* frame_scales = nullptr;
   // multi-GPU: the ONE collective of the path, ncclAllGather of the result blob
   void* comm = nullptr;           // ncclComm_t
   bool comm_owned = false;
@@ -498,16 +502,16 @@ static void drop_graph(sqdet_engine* e, bool only_u8 = false) {
 
 // The forward of fp32 images, or of uint8 BGR images (`u8`): handed to the first layer when the
 // plan fuses it, else converted into tensor 0 by one launch: the byte-wise same-size path of the
-// resize kernel over n*H rows, which reads images starting at any byte.
+// resize kernel on one frame of n*H rows, which reads images starting at any byte.
 static int enqueue_all(sqdet_engine* e, const void* images, bool u8, int n, const float* scales,
                        cudaStream_t stream) {
   const float* x = u8 ? nullptr : static_cast<const float*>(images);
   const uint8_t* x8 = u8 ? static_cast<const uint8_t*>(images) : nullptr;
   if (x8 && !e->u8_fused) {
     const Tensor& t = e->tensors[0];
-    const double* m = e->bgr_means;
-    const int rc = launch_resize_meansub_u8(x8, n * t.H, t.W, t.dev, n * t.H, t.W, m[0], m[1],
-                                            m[2], 0, stream);
+    const ResizeFrame f = resize_frame(x8, 3 * (int64_t)t.W, n * t.H, t.W, n * t.H, t.W);
+    const int rc = launch_resize_meansub_u8_batch(&f, 1, t.dev, n * t.H, t.W, e->bgr_means, 0,
+                                                  nullptr, stream);
     if (rc) return rc;
     x8 = nullptr;
   }
@@ -714,6 +718,7 @@ int sqdet_destroy(sqdet_engine* e) {
   if (e->own_stream) cudaStreamDestroy(e->own_stream);
   if (e->last_forward) cudaEventDestroy(e->last_forward);
   cudaFree(e->box_scale);
+  cudaFree(e->frame_scales);
   cudaFree(e->d_gathered);
   if (e->comm && e->comm_owned && g_nccl.CommDestroy) g_nccl.CommDestroy(e->comm);
   (void)cudaGetLastError();   // never leave a stale error for the next engine's launch checks
@@ -1290,7 +1295,6 @@ int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
   int rc = begin_submit(e, "sqdet_submit_frames", &s);
   if (rc) return rc;
   std::vector<size_t> bytes((size_t)n), off((size_t)n);
-  std::vector<float> sc((size_t)n * 2);
   size_t end = 0;
   for (int i = 0; i < n; ++i) {
     if (!frames[i] || heights[i] <= 0 || widths[i] <= 0)
@@ -1298,29 +1302,98 @@ int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
     bytes[(size_t)i] = (size_t)heights[i] * widths[i] * 3;
     off[(size_t)i] = end;                                   // 256-byte aligned staging offsets
     end += (bytes[(size_t)i] + 255) & ~(size_t)255;
-    // eval.py:72-74 / imdb.py:93-95: x_scale = mc.IMAGE_WIDTH / orig_w (Python floats = double)
-    sc[(size_t)2 * i] = (float)((double)c.image_width / (double)widths[i]);
-    sc[(size_t)2 * i + 1] = (float)((double)c.image_height / (double)heights[i]);
   }
-  cudaStream_t ks = e->own_stream;
   // eval order: boxes go back to each frame's own pixel grid before the filter (eval.py:80-87).
-  // The slot's table is written in stream order behind the forward that last read it.
-  if (rescale) {
-    if (!s->scales) SQ_CUDA(cudaMalloc(&s->scales, sizeof(float) * (size_t)B * 2));
-    SQ_CUDA(cudaMemcpyAsync(s->scales, sc.data(), sizeof(float) * sc.size(),
-                            cudaMemcpyHostToDevice, ks));
-  }
+  // The resize launch writes the slot's table in stream order behind the forward that last read it.
+  if (rescale && !s->scales) SQ_CUDA(cudaMalloc(&s->scales, sizeof(float) * (size_t)B * 2));
   rc = upload(e, *s, false, n, frames, bytes.data(), off.data());
   if (rc) return rc;
-  const size_t img_floats = (size_t)c.image_height * c.image_width * 3;
-  for (int i = 0; i < n; ++i) {
-    rc = launch_resize_meansub_u8(s->staging + off[(size_t)i], heights[i], widths[i],
-                                  s->input + (size_t)i * img_floats, c.image_height,
-                                  c.image_width, e->bgr_means[0], e->bgr_means[1],
-                                  e->bgr_means[2], order == SQDET_PRE_SUB_THEN_RESIZE, ks);
-    if (rc) return rc;
+  std::vector<ResizeFrame> fr((size_t)n);
+  for (int i = 0; i < n; ++i)
+    fr[(size_t)i] = resize_frame(s->staging + off[(size_t)i], 3 * (int64_t)widths[i], heights[i],
+                                 widths[i], c.image_height, c.image_width);
+  float* scales = rescale ? s->scales : nullptr;
+  rc = launch_resize_meansub_u8_batch(fr.data(), n, s->input, c.image_height, c.image_width,
+                                      e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE, scales,
+                                      e->own_stream);
+  if (rc) return rc;
+  return finish_submit(e, *s, s->input, false, n, scales, dets, counts);
+}
+
+// ---- variable-size uint8 frames already in device memory ----------------------------------------
+using MemGetAddressRangeFn = CUresult (*)(CUdeviceptr*, size_t*, CUdeviceptr);
+
+// True when the `bytes` bytes at p are device memory of `device` inside one allocation.  The
+// pointer comes from outside the program: a host pointer or an overlong frame is refused here
+// rather than faulting the resize kernel.
+static bool device_range_ok(const uint8_t* p, int64_t bytes, int device) {
+  static MemGetAddressRangeFn range = [] {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      fn = nullptr;
+    return reinterpret_cast<MemGetAddressRangeFn>(fn);
+  }();
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) {
+    (void)cudaGetLastError();      // an unknown pointer: no stale error for the next launch check
+    return false;
   }
-  return finish_submit(e, *s, s->input, false, n, rescale ? s->scales : nullptr, dets, counts);
+  if (attr.type != cudaMemoryTypeDevice || attr.device != device || !range) return false;
+  CUdeviceptr base = 0;
+  size_t size = 0;
+  if (range(&base, &size, (CUdeviceptr)(uintptr_t)p) != CUDA_SUCCESS) return false;
+  const uint64_t off = (uint64_t)(uintptr_t)p - (uint64_t)base;
+  return off <= size && (uint64_t)bytes <= size - off;
+}
+
+int sqdet_forward_frames_u8(sqdet_engine* e, int n, const uint8_t* const* frames_dev,
+                            const int32_t* heights, const int32_t* widths,
+                            const int64_t* row_pitches, int order, int rescale, void* stream_v) {
+  if (!e || !frames_dev || !heights || !widths)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_u8: null argument");
+  if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_forward_frames_u8 before sqdet_finalize");
+  const sqdet_config& c = e->cfg;
+  if (n < 1 || n > c.batch_size)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_u8: n must be in [1, batch_size]");
+  if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_u8: order must be 0 (demo) or 1 (eval)");
+  for (int i = 0; i < n; ++i) {
+    const int64_t h = heights[i], w = widths[i];
+    const int64_t pitch = row_pitches ? row_pitches[i] : 3 * w;
+    const std::string which = "sqdet_forward_frames_u8: frame " + std::to_string(i);
+    if (!frames_dev[i]) return fail(SQDET_ERR_INVALID_ARG, which + " is a null pointer");
+    if (h <= 0 || w <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
+    if (pitch < 3 * w) return fail(SQDET_ERR_INVALID_ARG, which + ": row pitch below 3 * width");
+  }
+  DeviceGuard guard(e->device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
+  std::vector<ResizeFrame> fr((size_t)n);
+  for (int i = 0; i < n; ++i) {
+    const int64_t h = heights[i], w = widths[i];
+    const int64_t pitch = row_pitches ? row_pitches[i] : 3 * w;
+    // the frame's bytes end at (h - 1) * pitch + 3 * w; refused when that overflows int64
+    const bool fits = h == 1 || pitch <= (INT64_MAX - 3 * w) / (h - 1);
+    if (!fits || !device_range_ok(frames_dev[i], (h - 1) * pitch + 3 * w, e->device))
+      return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_u8: frame " + std::to_string(i) +
+                                             " is not inside one device allocation on the engine's device");
+    fr[(size_t)i] = resize_frame(frames_dev[i], pitch, (int)h, (int)w, c.image_height, c.image_width);
+  }
+  cudaStream_t stream = (cudaStream_t)stream_v;
+  // the weights first: their upload waits for the forwards in flight, and the resize below must
+  // not be left behind a failed one
+  int rc = prepare_params(e);
+  if (rc) return rc;
+  if (rescale && !e->frame_scales)
+    SQ_CUDA(cudaMalloc(&e->frame_scales, sizeof(float) * (size_t)c.batch_size * 2));
+  float* scales = rescale ? e->frame_scales : nullptr;
+  Tensor& t0 = e->tensors[0];
+  rc = launch_resize_meansub_u8_batch(fr.data(), n, t0.dev, c.image_height, c.image_width,
+                                      e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE, scales,
+                                      stream);
+  if (rc) return rc;
+  return forward_impl(e, t0.dev, false, n, scales, stream);
 }
 
 // ---- multi-GPU: ONE all-gather of the filtered records ---------------------------------------------
@@ -1537,9 +1610,10 @@ int sqdet_preprocess_u8(const uint8_t* src_dev, int src_h, int src_w, float* dst
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_preprocess_u8: null pointer");
   if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_preprocess_u8: order must be 0 (demo) or 1 (eval)");
-  return launch_resize_meansub_u8(src_dev, src_h, src_w, dst_dev, dst_h, dst_w, bgr_means[0],
-                                  bgr_means[1], bgr_means[2], order == SQDET_PRE_SUB_THEN_RESIZE,
-                                  (cudaStream_t)stream);
+  const ResizeFrame f = resize_frame(src_dev, 3 * (int64_t)src_w, src_h, src_w, dst_h, dst_w);
+  return launch_resize_meansub_u8_batch(&f, 1, dst_dev, dst_h, dst_w, bgr_means,
+                                        order == SQDET_PRE_SUB_THEN_RESIZE, nullptr,
+                                        (cudaStream_t)stream);
 }
 
 int sqdet_interpret(const float* preds_dev, const float* anchors_f32_dev, float* det_boxes_dev,

@@ -6,6 +6,9 @@
 // Roofline: HBM.  Algorithmic bytes = 4*(B*H*W*C + B*Ho*Wo*C); each input element is
 // read ~(k/stride)^2 times but the re-reads hit L1/L2 (adjacent threads share rows).
 #include <math_constants.h>
+
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace sqdet {
@@ -143,15 +146,13 @@ add_relu_kernel(const float* __restrict__ a, const float* __restrict__ b,
 // in float64; src/dataset/imdb.py:87-91: float32 `-= BGR_MEANS`, then resize).  Restates
 // oracle/preproc.py operation for operation (double sampling position, float32 weight, clamps,
 // horizontal pass then vertical pass, round-to-nearest multiplies and adds, no contraction).
-// One thread = one output pixel (3 channels); the 4 taps are 12 byte loads served by L1.
-__global__ void __launch_bounds__(256)
-resize_meansub_u8_kernel(const uint8_t* __restrict__ src, float* __restrict__ dst, int H0, int W0,
-                         int H, int W, double scale_x, double scale_y, double m0, double m1,
-                         double m2, int sub_first) {
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (long long)H * W) return;
-  const int dx = (int)(idx % W), dy = (int)(idx / W);
-  const double mean[3] = {m0, m1, m2};
+// Output pixel (dx, dy) of one frame whose row r starts at src + r * pitch (any byte alignment):
+// the 4 taps are 12 byte loads served by L1.
+__device__ __forceinline__ void resize_meansub_pixel(const uint8_t* __restrict__ src,
+                                                     long long pitch, int H0, int W0, int H, int W,
+                                                     double scale_x, double scale_y,
+                                                     const double (&mean)[3], int sub_first, int dx,
+                                                     int dy, float* __restrict__ d) {
   int sx, sx1, y0, y1;
   float fx, fy;
   bool x_edge = false;
@@ -184,7 +185,7 @@ resize_meansub_u8_kernel(const uint8_t* __restrict__ src, float* __restrict__ ds
     for (int r = 0; r < 2; ++r)
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
-        const float v = (float)src[((long long)ys[r] * W0 + xs[q]) * 3 + c];
+        const float v = (float)src[(long long)ys[r] * pitch + (long long)xs[q] * 3 + c];
         t[r][q] = sub_first ? (float)((double)v - mean[c]) : v;
       }
     float row[2];
@@ -194,23 +195,74 @@ resize_meansub_u8_kernel(const uint8_t* __restrict__ src, float* __restrict__ ds
     const float v = same ? row[0] : __fadd_rn(__fmul_rn(row[0], b0), __fmul_rn(row[1], b1));
     o[c] = sub_first ? v : (float)((double)v - mean[c]);
   }
-  float* d = dst + idx * 3;
   d[0] = o[0]; d[1] = o[1]; d[2] = o[2];
+}
+
+struct ResizeFrameBatch {
+  ResizeFrame f[kResizeFramesPerLaunch];
+};
+// Descriptors travel in the parameter block: no device table, no copy, no host synchronisation.
+static_assert(sizeof(ResizeFrameBatch) + 128 <= 4096, "resize descriptors exceed 4 KiB of parameters");
+
+// Up to kResizeFramesPerLaunch frames in one launch: blockIdx.y is the frame, x runs over its
+// H x W output pixels, written as image blockIdx.y of the fp32 [count, H, W, 3] batch at dst.
+// With scales_xy, the frame's (x_scale, y_scale) box scales go to scales_xy[2 * frame].
+__global__ void __launch_bounds__(256)
+resize_meansub_u8_batch_kernel(const __grid_constant__ ResizeFrameBatch batch,
+                               float* __restrict__ dst, int H, int W, double m0, double m1,
+                               double m2, int sub_first, float* __restrict__ scales_xy) {
+  const ResizeFrame& f = batch.f[blockIdx.y];
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (scales_xy && idx == 0) {
+    scales_xy[2 * blockIdx.y] = f.box_scale_x;
+    scales_xy[2 * blockIdx.y + 1] = f.box_scale_y;
+  }
+  if (idx >= (long long)H * W) return;
+  const double mean[3] = {m0, m1, m2};
+  resize_meansub_pixel(f.src, f.pitch, f.h, f.w, H, W, f.scale_x, f.scale_y, mean, sub_first,
+                       (int)(idx % W), (int)(idx / W),
+                       dst + ((long long)blockIdx.y * H * W + idx) * 3);
 }
 
 }  // namespace
 
-int launch_resize_meansub_u8(const uint8_t* src, int H0, int W0, float* dst, int H, int W,
-                             double m0, double m1, double m2, int sub_first, cudaStream_t stream) {
-  if (H0 <= 0 || W0 <= 0 || H <= 0 || W <= 0)
-    return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_u8: non-positive image size");
+ResizeFrame resize_frame(const uint8_t* src, int64_t pitch, int h, int w, int H, int W) {
+  ResizeFrame f;
+  f.src = src;
+  f.pitch = pitch;
+  f.h = h;
+  f.w = w;
   // cv::resize: inv_scale = dst / src, scale = 1 / inv_scale (both double)
-  const double scale_x = 1.0 / ((double)W / (double)W0);
-  const double scale_y = 1.0 / ((double)H / (double)H0);
-  const long long n = (long long)H * W;
-  resize_meansub_u8_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
-      src, dst, H0, W0, H, W, scale_x, scale_y, m0, m1, m2, sub_first);
-  SQ_CHECK_LAUNCH("resize_meansub_u8_kernel");
+  f.scale_x = 1.0 / ((double)W / (double)w);
+  f.scale_y = 1.0 / ((double)H / (double)h);
+  // eval.py:72-74 / imdb.py:93-95: x_scale = mc.IMAGE_WIDTH / orig_w (Python floats = double)
+  f.box_scale_x = (float)((double)W / (double)w);
+  f.box_scale_y = (float)((double)H / (double)h);
+  return f;
+}
+
+int launch_resize_meansub_u8_batch(const ResizeFrame* frames, int n, float* dst, int H, int W,
+                                   const double* means, int sub_first, float* scales_xy,
+                                   cudaStream_t stream) {
+  if (n <= 0 || H <= 0 || W <= 0)
+    return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_u8: non-positive image size");
+  for (int i = 0; i < n; ++i)
+    if (frames[i].h <= 0 || frames[i].w <= 0)
+      return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_u8: non-positive image size");
+    else if (frames[i].pitch < 3 * (int64_t)frames[i].w)
+      return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_u8: row pitch below 3 * width");
+  const long long pixels = (long long)H * W;
+  const long long blocks = (pixels + 255) / 256;
+  if (blocks > 0x7fffffffLL) return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_u8: image too large");
+  for (int g = 0; g < n; g += kResizeFramesPerLaunch) {
+    const int count = std::min(n - g, kResizeFramesPerLaunch);
+    ResizeFrameBatch batch;
+    for (int i = 0; i < count; ++i) batch.f[i] = frames[g + i];
+    resize_meansub_u8_batch_kernel<<<dim3((unsigned)blocks, (unsigned)count), 256, 0, stream>>>(
+        batch, dst + (size_t)g * pixels * 3, H, W, means[0], means[1], means[2], sub_first,
+        scales_xy ? scales_xy + 2 * g : nullptr);
+    SQ_CHECK_LAUNCH("resize_meansub_u8_batch_kernel");
+  }
   return SQDET_OK;
 }
 

@@ -497,6 +497,42 @@ class ModelSkeleton:
     n = self.mc.BATCH_SIZE if n is None else int(n)
     _lib.check(self._lib.sqdet_forward_u8(self._engine, images_dev_ptr, n, stream))
 
+  def forward_device_frames(self, frames, order='demo', rescale=False, stream=None):
+    """Forward of 1..BATCH_SIZE uint8 BGR frames of any size already on this engine's device:
+    CUDA tensors [h, w, 3] with stride(2) == 1 and stride(1) == 3; the row stride is free, so a
+    crop view such as frame[500:-205, 239:-439] passes without a copy.  The engine resizes them
+    to (mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT) and subtracts mc.BGR_MEANS in `order` ('demo' or
+    'eval', as submit_frames) in one launch into image_input, then runs the forward on `stream`
+    (sqdet_forward_frames_u8).  rescale=True divides the boxes by each frame's scales before the
+    filter, in this call only.  Asynchronous: read the results through results_device()."""
+    frames = list(frames)
+    B, n = self.mc.BATCH_SIZE, len(frames)
+    if not 1 <= n <= B:
+      raise ValueError('need 1 to %d frames, got %d' % (B, n))
+    if order not in ('demo', 'eval'):
+      raise ValueError("order must be 'demo' or 'eval', got %r" % (order,))
+    ptrs, hs, ws, pitches = [], [], [], []
+    for i, f in enumerate(frames):
+      dtype, device, shape = getattr(f, 'dtype', None), getattr(f, 'device', None), tuple(f.shape)
+      if str(dtype) != 'torch.uint8':
+        raise ValueError('frame %d: need a uint8 tensor, got %s' % (i, dtype))
+      if getattr(device, 'type', None) != 'cuda' or device.index != self.gpu_id:
+        raise ValueError('frame %d: need a tensor on cuda:%d, got %s' % (i, self.gpu_id, device))
+      if len(shape) != 3 or shape[2] != 3 or shape[0] < 1 or shape[1] < 1:
+        raise ValueError('frame %d: need shape [h, w, 3], got %r' % (i, shape))
+      stride = tuple(f.stride())
+      pitch = stride[0] if shape[0] > 1 else 3 * shape[1]   # a single row's stride is never used
+      if stride[2] != 1 or stride[1] != 3 or pitch < 3 * shape[1]:
+        raise ValueError('frame %d: need strides (row, 3, 1) with row >= 3 * w, got %r'
+                         % (i, stride))
+      ptrs.append(f.data_ptr())
+      hs.append(shape[0])
+      ws.append(shape[1])
+      pitches.append(pitch)
+    _lib.check(self._lib.sqdet_forward_frames_u8(
+        self._engine, n, (C.c_void_p * n)(*ptrs), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws),
+        (C.c_int64 * n)(*pitches), {'demo': 0, 'eval': 1}[order], int(bool(rescale)), stream))
+
   def forward_profiled(self, images_dev_ptr, stream=None):
     n = self._lib.sqdet_num_ops(self._engine)
     ms = np.zeros(n, np.float32)
