@@ -243,6 +243,31 @@ int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
 int sqdet_forward_frames_u8(sqdet_engine* e, int n, const uint8_t* const* frames_dev,
                             const int32_t* heights, const int32_t* widths,
                             const int64_t* row_pitches, int order, int rescale, void* stream);
+/* n NV12 frames already in device memory on the engine's device, as a hardware video decoder
+ * (NVDEC) writes them: frame i is heights[i] x widths[i] (both even), a luma plane of heights[i]
+ * rows of widths[i] bytes at luma_dev[i] + r*luma_pitches[i] and a chroma plane of heights[i]/2
+ * rows of widths[i] interleaved U,V bytes at chroma_dev[i] + r*chroma_pitches[i] (NULL pitches =
+ * widths[i]; either plane may start at any byte).  crops: NULL (whole frames) or n x (x, y, w, h),
+ * a non-empty rectangle inside the frame at any origin.  Each crop is exactly
+ * cv2.cvtColor(nv12, cv2.COLOR_YUV2BGR_NV12)[y:y+h, x:x+w] (OpenCV's BT.601 limited-range
+ * fixed-point conversion; FFmpeg's swscale, inside cv2.VideoCapture, rounds differently), and the
+ * call is bit for bit sqdet_forward_frames_u8 on those BGR crops: resize + `- mc.BGR_MEANS` in
+ * `order` into tensor 0, rescale by the crop's size, then the forward on `stream`.  No BGR frame
+ * is written.  Asynchronous; no host synchronisation.
+ *   - Launches: sqdet_launches_per_forward (without a box-scale table), plus one conversion launch
+ *     per 56 frames, plus the rescale launch when rescale != 0.
+ *   - Refused before any device work, leaving graphs, pipeline and tensor 0 untouched:
+ *     SQDET_ERR_INVALID_ARG for a null engine or array, n outside [1, B], an unknown order, a
+ *     null plane, a height or width <= 0 or odd, a pitch below the width, an empty crop or one
+ *     outside the frame, or a plane whose bytes (luma (H-1)*pitch + W, chroma (H/2-1)*pitch + W)
+ *     are not device memory of the engine's device inside one allocation; SQDET_ERR_STATE before
+ *     sqdet_finalize.
+ * Like sqdet_forward_u8, one engine per stream: results are read through sqdet_results_dev.   */
+int sqdet_forward_frames_nv12(sqdet_engine* e, int n, const uint8_t* const* luma_dev,
+                              const int64_t* luma_pitches, const uint8_t* const* chroma_dev,
+                              const int64_t* chroma_pitches, const int32_t* heights,
+                              const int32_t* widths, const int32_t* crops, int order, int rescale,
+                              void* stream);
 /* src/eval.py:83-84 for callers that resize on the host: xy_scales = B pairs (x_scale,
  * y_scale), host memory; every later forward of the paths fed already-resized images
  * (sqdet_forward(_n), sqdet_forward_profiled, sqdet_detect, sqdet_submit) divides

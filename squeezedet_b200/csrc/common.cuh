@@ -86,6 +86,32 @@ ResizeFrame resize_frame(const uint8_t* src, int64_t pitch, int h, int w, int H,
 int launch_resize_meansub_u8_batch(const ResizeFrame* frames, int n, float* dst, int H, int W,
                                    const double* means, int sub_first, float* scales_xy,
                                    cudaStream_t stream);
+// One h x w crop of an NV12 frame for the same resize: luma points at the crop origin's byte,
+// chroma at the U,V pair of the origin's 2x2 chroma block, and (x_odd, y_odd) is the origin's
+// parity in the frame, so the crop reads the frame's own chroma samples at any origin.  Both
+// planes may start at any byte and have any pitch.
+struct Nv12Frame {
+  const uint8_t* luma;
+  const uint8_t* chroma;
+  int64_t luma_pitch, chroma_pitch;
+  double scale_x, scale_y;
+  float box_scale_x, box_scale_y;
+  int h, w;
+  int x_odd, y_odd;
+};
+// Frames per launch: 56 descriptors of 72 bytes and the kernel's other parameters fill the
+// classic 4 KiB parameter block.
+constexpr int kNv12FramesPerLaunch = 56;
+// The descriptor of the h x w crop at (x, y) of the NV12 frame with planes (luma, luma_pitch),
+// (chroma, chroma_pitch), resized to H x W.
+Nv12Frame nv12_frame(const uint8_t* luma, int64_t luma_pitch, const uint8_t* chroma,
+                     int64_t chroma_pitch, int x, int y, int h, int w, int H, int W);
+// cv2.cvtColor(COLOR_YUV2BGR_NV12) of each crop, then launch_resize_meansub_u8_batch's resize and
+// mean subtraction, bit for bit, one launch per kNv12FramesPerLaunch frames.  No BGR frame is
+// written: each tap is fetched from the planes and converted.
+int launch_resize_meansub_nv12_batch(const Nv12Frame* frames, int n, float* dst, int H, int W,
+                                     const double* means, int sub_first, float* scales_xy,
+                                     cudaStream_t stream);
 int launch_add_relu(const float* a, const float* b, float* y, int64_t n, cudaStream_t stream);
 
 int launch_interpret(const float* preds, const float* anchors, float* boxes, float* probs,

@@ -157,7 +157,7 @@ struct sqdet_engine {
   cudaEvent_t last_forward = nullptr;
   std::vector<cudaEvent_t> prof_events;
   float* box_scale = nullptr;     // sqdet_set_box_scale's B (x_scale, y_scale) pairs, or null
-  // sqdet_forward_frames_u8's B (x_scale, y_scale) pairs, written by its resize launch; one
+  // sqdet_forward_frames_{u8,nv12}'s B (x_scale, y_scale) pairs, written by their resize launch; one
   // address for the engine's life, so the forward graphs keyed on it stay valid
   float* frame_scales = nullptr;
   // multi-GPU: the ONE collective of the path, ncclAllGather of the result blob
@@ -1348,6 +1348,18 @@ static bool device_range_ok(const uint8_t* p, int64_t bytes, int device) {
   return off <= size && (uint64_t)bytes <= size - off;
 }
 
+// Before the resize launch of a device-frames forward: the weights first, since their upload waits
+// for the forwards in flight and the resize must not be left behind a failed one; then, with
+// rescale, the box-scale table the launch writes, at *scales (null without rescale).
+static int prepare_frames(sqdet_engine* e, int rescale, float** scales) {
+  const int rc = prepare_params(e);
+  if (rc) return rc;
+  if (rescale && !e->frame_scales)
+    SQ_CUDA(cudaMalloc(&e->frame_scales, sizeof(float) * (size_t)e->cfg.batch_size * 2));
+  *scales = rescale ? e->frame_scales : nullptr;
+  return SQDET_OK;
+}
+
 int sqdet_forward_frames_u8(sqdet_engine* e, int n, const uint8_t* const* frames_dev,
                             const int32_t* heights, const int32_t* widths,
                             const int64_t* row_pitches, int order, int rescale, void* stream_v) {
@@ -1381,17 +1393,70 @@ int sqdet_forward_frames_u8(sqdet_engine* e, int n, const uint8_t* const* frames
     fr[(size_t)i] = resize_frame(frames_dev[i], pitch, (int)h, (int)w, c.image_height, c.image_width);
   }
   cudaStream_t stream = (cudaStream_t)stream_v;
-  // the weights first: their upload waits for the forwards in flight, and the resize below must
-  // not be left behind a failed one
-  int rc = prepare_params(e);
+  float* scales = nullptr;
+  int rc = prepare_frames(e, rescale, &scales);
   if (rc) return rc;
-  if (rescale && !e->frame_scales)
-    SQ_CUDA(cudaMalloc(&e->frame_scales, sizeof(float) * (size_t)c.batch_size * 2));
-  float* scales = rescale ? e->frame_scales : nullptr;
   Tensor& t0 = e->tensors[0];
   rc = launch_resize_meansub_u8_batch(fr.data(), n, t0.dev, c.image_height, c.image_width,
                                       e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE, scales,
                                       stream);
+  if (rc) return rc;
+  return forward_impl(e, t0.dev, false, n, scales, stream);
+}
+
+int sqdet_forward_frames_nv12(sqdet_engine* e, int n, const uint8_t* const* luma_dev,
+                              const int64_t* luma_pitches, const uint8_t* const* chroma_dev,
+                              const int64_t* chroma_pitches, const int32_t* heights,
+                              const int32_t* widths, const int32_t* crops, int order, int rescale,
+                              void* stream_v) {
+  if (!e || !luma_dev || !chroma_dev || !heights || !widths)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_nv12: null argument");
+  if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_forward_frames_nv12 before sqdet_finalize");
+  const sqdet_config& c = e->cfg;
+  if (n < 1 || n > c.batch_size)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_nv12: n must be in [1, batch_size]");
+  if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_nv12: order must be 0 (demo) or 1 (eval)");
+  for (int i = 0; i < n; ++i) {
+    const int64_t H = heights[i], W = widths[i];
+    const int64_t lp = luma_pitches ? luma_pitches[i] : W, cp = chroma_pitches ? chroma_pitches[i] : W;
+    const std::string which = "sqdet_forward_frames_nv12: frame " + std::to_string(i);
+    if (!luma_dev[i] || !chroma_dev[i]) return fail(SQDET_ERR_INVALID_ARG, which + " has a null plane");
+    if (H <= 0 || W <= 0 || H % 2 || W % 2)
+      return fail(SQDET_ERR_INVALID_ARG, which + ": height and width must be positive and even");
+    if (lp < W || cp < W) return fail(SQDET_ERR_INVALID_ARG, which + ": row pitch below the width");
+    if (crops) {
+      const int64_t x = crops[4 * i], y = crops[4 * i + 1], w = crops[4 * i + 2], h = crops[4 * i + 3];
+      if (w <= 0 || h <= 0) return fail(SQDET_ERR_INVALID_ARG, which + ": empty crop");
+      if (x < 0 || y < 0 || x + w > W || y + h > H)
+        return fail(SQDET_ERR_INVALID_ARG, which + ": crop outside the frame");
+    }
+  }
+  DeviceGuard guard(e->device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
+  std::vector<Nv12Frame> fr((size_t)n);
+  for (int i = 0; i < n; ++i) {
+    const int64_t H = heights[i], W = widths[i];
+    const int64_t lp = luma_pitches ? luma_pitches[i] : W, cp = chroma_pitches ? chroma_pitches[i] : W;
+    // the planes' bytes end at (H - 1) * lp + W and (H / 2 - 1) * cp + W; refused when either
+    // overflows int64 (H >= 2)
+    const bool fits = lp <= (INT64_MAX - W) / (H - 1) && (H == 2 || cp <= (INT64_MAX - W) / (H / 2 - 1));
+    if (!fits || !device_range_ok(luma_dev[i], (H - 1) * lp + W, e->device) ||
+        !device_range_ok(chroma_dev[i], (H / 2 - 1) * cp + W, e->device))
+      return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_nv12: frame " + std::to_string(i) +
+                                             ": a plane is not inside one device allocation on the engine's device");
+    const int32_t* r = crops ? crops + 4 * i : nullptr;
+    fr[(size_t)i] = nv12_frame(luma_dev[i], lp, chroma_dev[i], cp, r ? r[0] : 0, r ? r[1] : 0,
+                               r ? r[3] : (int)H, r ? r[2] : (int)W, c.image_height, c.image_width);
+  }
+  cudaStream_t stream = (cudaStream_t)stream_v;
+  float* scales = nullptr;
+  int rc = prepare_frames(e, rescale, &scales);
+  if (rc) return rc;
+  Tensor& t0 = e->tensors[0];
+  rc = launch_resize_meansub_nv12_batch(fr.data(), n, t0.dev, c.image_height, c.image_width,
+                                        e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE, scales,
+                                        stream);
   if (rc) return rc;
   return forward_impl(e, t0.dev, false, n, scales, stream);
 }

@@ -146,10 +146,11 @@ add_relu_kernel(const float* __restrict__ a, const float* __restrict__ b,
 // in float64; src/dataset/imdb.py:87-91: float32 `-= BGR_MEANS`, then resize).  Restates
 // oracle/preproc.py operation for operation (double sampling position, float32 weight, clamps,
 // horizontal pass then vertical pass, round-to-nearest multiplies and adds, no contraction).
-// Output pixel (dx, dy) of one frame whose row r starts at src + r * pitch (any byte alignment):
-// the 4 taps are 12 byte loads served by L1.
-__device__ __forceinline__ void resize_meansub_pixel(const uint8_t* __restrict__ src,
-                                                     long long pitch, int H0, int W0, int H, int W,
+// Output pixel (dx, dy) of one H0 x W0 frame whose source pixels `taps` fetches:
+// taps(ys, xs, r, q, c) is channel c (B, G, R) of source pixel (ys[r], xs[q]), asked for channel 0
+// of every tap first.
+template <class Taps>
+__device__ __forceinline__ void resize_meansub_pixel(const Taps& taps, int H0, int W0, int H, int W,
                                                      double scale_x, double scale_y,
                                                      const double (&mean)[3], int sub_first, int dx,
                                                      int dy, float* __restrict__ d) {
@@ -185,7 +186,7 @@ __device__ __forceinline__ void resize_meansub_pixel(const uint8_t* __restrict__
     for (int r = 0; r < 2; ++r)
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
-        const float v = (float)src[(long long)ys[r] * pitch + (long long)xs[q] * 3 + c];
+        const float v = taps(ys, xs, r, q, c);
         t[r][q] = sub_first ? (float)((double)v - mean[c]) : v;
       }
     float row[2];
@@ -198,20 +199,72 @@ __device__ __forceinline__ void resize_meansub_pixel(const uint8_t* __restrict__
   d[0] = o[0]; d[1] = o[1]; d[2] = o[2];
 }
 
+// The taps of a uint8 BGR frame whose row r starts at src + r * pitch (any byte alignment): a
+// channel is a byte load served by L1.
+struct BgrTaps {
+  const uint8_t* __restrict__ src;
+  long long pitch;
+  __device__ __forceinline__ float operator()(const int (&ys)[2], const int (&xs)[2], int r, int q,
+                                             int c) const {
+    return (float)src[(long long)ys[r] * pitch + (long long)xs[q] * 3 + c];
+  }
+};
+
+// The taps of an NV12 crop: one luma byte and the U,V pair of its 2x2 chroma block, converted as
+// cv2.cvtColor(COLOR_YUV2BGR_NV12) does (OpenCV's BT.601 limited-range ITUR_BT_601_* constants,
+// 20 fraction bits; oracle.nv12.nv12_to_bgr).  Crop pixel (y, x) is frame pixel
+// (y0 + y, x0 + x); luma and chroma point at the crop origin's byte and chroma pair, and the
+// origin's parity (x_odd, y_odd) picks the chroma block, so an odd origin reads the frame's own
+// samples.  int32 suffices: every sum stays below 2^30 in magnitude.  Each tap is loaded and
+// converted once, when its channel 0 is asked for.
+struct Nv12Taps {
+  const uint8_t* __restrict__ luma;
+  const uint8_t* __restrict__ chroma;
+  long long luma_pitch, chroma_pitch;
+  int x_odd, y_odd;
+  mutable float bgr[2][2][3];   // tap (r, q), converted at its channel 0
+  __device__ __forceinline__ float operator()(const int (&ys)[2], const int (&xs)[2], int r, int q,
+                                             int c) const {
+    if (c == 0) {
+      const int y = ys[r], x = xs[q];
+      const int Y = luma[(long long)y * luma_pitch + x];
+      const uint8_t* uv =
+          chroma + (long long)((y + y_odd) >> 1) * chroma_pitch + ((x + x_odd) & ~1);
+      const int u = (int)uv[0] - 128, v = (int)uv[1] - 128;
+      const int yy = max(Y - 16, 0) * 1220542 + (1 << 19);
+      bgr[r][q][0] = (float)min(max((yy + 2116026 * u) >> 20, 0), 255);
+      bgr[r][q][1] = (float)min(max((yy - 852492 * v - 409993 * u) >> 20, 0), 255);
+      bgr[r][q][2] = (float)min(max((yy + 1673527 * v) >> 20, 0), 255);
+    }
+    return bgr[r][q][c];
+  }
+};
+
+__device__ __forceinline__ BgrTaps taps(const ResizeFrame& f) { return {f.src, f.pitch}; }
+__device__ __forceinline__ Nv12Taps taps(const Nv12Frame& f) {
+  return {f.luma, f.chroma, f.luma_pitch, f.chroma_pitch, f.x_odd, f.y_odd, {}};
+}
+
 struct ResizeFrameBatch {
   ResizeFrame f[kResizeFramesPerLaunch];
 };
+struct Nv12FrameBatch {
+  Nv12Frame f[kNv12FramesPerLaunch];
+};
 // Descriptors travel in the parameter block: no device table, no copy, no host synchronisation.
 static_assert(sizeof(ResizeFrameBatch) + 128 <= 4096, "resize descriptors exceed 4 KiB of parameters");
+// The kernel's other parameters take 56 bytes.
+static_assert(sizeof(Nv12FrameBatch) + 64 <= 4096, "NV12 descriptors exceed 4 KiB of parameters");
 
-// Up to kResizeFramesPerLaunch frames in one launch: blockIdx.y is the frame, x runs over its
-// H x W output pixels, written as image blockIdx.y of the fp32 [count, H, W, 3] batch at dst.
-// With scales_xy, the frame's (x_scale, y_scale) box scales go to scales_xy[2 * frame].
+// Up to the batch's frame count in one launch: blockIdx.y is the frame, x runs over its H x W
+// output pixels, written as image blockIdx.y of the fp32 [count, H, W, 3] batch at dst.  With
+// scales_xy, the frame's (x_scale, y_scale) box scales go to scales_xy[2 * frame].
+template <class Batch>
 __global__ void __launch_bounds__(256)
-resize_meansub_u8_batch_kernel(const __grid_constant__ ResizeFrameBatch batch,
-                               float* __restrict__ dst, int H, int W, double m0, double m1,
-                               double m2, int sub_first, float* __restrict__ scales_xy) {
-  const ResizeFrame& f = batch.f[blockIdx.y];
+resize_meansub_u8_batch_kernel(const __grid_constant__ Batch batch, float* __restrict__ dst, int H,
+                               int W, double m0, double m1, double m2, int sub_first,
+                               float* __restrict__ scales_xy) {
+  const auto& f = batch.f[blockIdx.y];
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (scales_xy && idx == 0) {
     scales_xy[2 * blockIdx.y] = f.box_scale_x;
@@ -219,9 +272,30 @@ resize_meansub_u8_batch_kernel(const __grid_constant__ ResizeFrameBatch batch,
   }
   if (idx >= (long long)H * W) return;
   const double mean[3] = {m0, m1, m2};
-  resize_meansub_pixel(f.src, f.pitch, f.h, f.w, H, W, f.scale_x, f.scale_y, mean, sub_first,
+  resize_meansub_pixel(taps(f), f.h, f.w, H, W, f.scale_x, f.scale_y, mean, sub_first,
                        (int)(idx % W), (int)(idx / W),
                        dst + ((long long)blockIdx.y * H * W + idx) * 3);
+}
+
+// The frames in launches of the batch's frame count each (the frames' own checks are the
+// caller's); `what` names the kernel in errors.
+template <class Batch, class Frame>
+int launch_batches(const char* what, const Frame* frames, int n, float* dst, int H, int W,
+                   const double* means, int sub_first, float* scales_xy, cudaStream_t stream) {
+  constexpr int per_launch = (int)(sizeof(Batch) / sizeof(Frame));
+  const long long pixels = (long long)H * W;
+  const long long blocks = (pixels + 255) / 256;
+  if (blocks > 0x7fffffffLL) return fail(SQDET_ERR_INVALID_ARG, std::string(what) + ": image too large");
+  for (int g = 0; g < n; g += per_launch) {
+    const int count = std::min(n - g, per_launch);
+    Batch batch;
+    for (int i = 0; i < count; ++i) batch.f[i] = frames[g + i];
+    resize_meansub_u8_batch_kernel<<<dim3((unsigned)blocks, (unsigned)count), 256, 0, stream>>>(
+        batch, dst + (size_t)g * pixels * 3, H, W, means[0], means[1], means[2], sub_first,
+        scales_xy ? scales_xy + 2 * g : nullptr);
+    SQ_CHECK_LAUNCH(what);
+  }
+  return SQDET_OK;
 }
 
 }  // namespace
@@ -241,6 +315,25 @@ ResizeFrame resize_frame(const uint8_t* src, int64_t pitch, int h, int w, int H,
   return f;
 }
 
+Nv12Frame nv12_frame(const uint8_t* luma, int64_t luma_pitch, const uint8_t* chroma,
+                     int64_t chroma_pitch, int x, int y, int h, int w, int H, int W) {
+  const ResizeFrame r = resize_frame(nullptr, 0, h, w, H, W);
+  Nv12Frame f;
+  f.luma = luma + (int64_t)y * luma_pitch + x;
+  f.chroma = chroma + (int64_t)(y >> 1) * chroma_pitch + (x & ~1);
+  f.luma_pitch = luma_pitch;
+  f.chroma_pitch = chroma_pitch;
+  f.scale_x = r.scale_x;
+  f.scale_y = r.scale_y;
+  f.box_scale_x = r.box_scale_x;
+  f.box_scale_y = r.box_scale_y;
+  f.h = h;
+  f.w = w;
+  f.x_odd = x & 1;
+  f.y_odd = y & 1;
+  return f;
+}
+
 int launch_resize_meansub_u8_batch(const ResizeFrame* frames, int n, float* dst, int H, int W,
                                    const double* means, int sub_first, float* scales_xy,
                                    cudaStream_t stream) {
@@ -251,19 +344,22 @@ int launch_resize_meansub_u8_batch(const ResizeFrame* frames, int n, float* dst,
       return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_u8: non-positive image size");
     else if (frames[i].pitch < 3 * (int64_t)frames[i].w)
       return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_u8: row pitch below 3 * width");
-  const long long pixels = (long long)H * W;
-  const long long blocks = (pixels + 255) / 256;
-  if (blocks > 0x7fffffffLL) return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_u8: image too large");
-  for (int g = 0; g < n; g += kResizeFramesPerLaunch) {
-    const int count = std::min(n - g, kResizeFramesPerLaunch);
-    ResizeFrameBatch batch;
-    for (int i = 0; i < count; ++i) batch.f[i] = frames[g + i];
-    resize_meansub_u8_batch_kernel<<<dim3((unsigned)blocks, (unsigned)count), 256, 0, stream>>>(
-        batch, dst + (size_t)g * pixels * 3, H, W, means[0], means[1], means[2], sub_first,
-        scales_xy ? scales_xy + 2 * g : nullptr);
-    SQ_CHECK_LAUNCH("resize_meansub_u8_batch_kernel");
-  }
-  return SQDET_OK;
+  return launch_batches<ResizeFrameBatch>("resize_meansub_u8_batch_kernel", frames, n, dst, H, W,
+                                          means, sub_first, scales_xy, stream);
+}
+
+int launch_resize_meansub_nv12_batch(const Nv12Frame* frames, int n, float* dst, int H, int W,
+                                     const double* means, int sub_first, float* scales_xy,
+                                     cudaStream_t stream) {
+  if (n <= 0 || H <= 0 || W <= 0)
+    return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_nv12: non-positive image size");
+  for (int i = 0; i < n; ++i)
+    if (frames[i].h <= 0 || frames[i].w <= 0)
+      return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_nv12: non-positive crop size");
+    else if (frames[i].luma_pitch < frames[i].w || frames[i].chroma_pitch < frames[i].w)
+      return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_nv12: row pitch below the crop width");
+  return launch_batches<Nv12FrameBatch>("resize_meansub_u8_batch_kernel<Nv12FrameBatch>", frames,
+                                        n, dst, H, W, means, sub_first, scales_xy, stream);
 }
 
 int launch_maxpool(const float* x, float* y, int B, int H, int W, int C, int size,

@@ -533,6 +533,83 @@ class ModelSkeleton:
         self._engine, n, (C.c_void_p * n)(*ptrs), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws),
         (C.c_int64 * n)(*pitches), {'demo': 0, 'eval': 1}[order], int(bool(rescale)), stream))
 
+  def forward_device_frames_nv12(self, frames, crops=None, order='demo', rescale=False,
+                                 stream=None):
+    """forward_device_frames of NV12 frames already on this engine's device, as a hardware video
+    decoder writes them.  Each frame is a uint8 CUDA tensor [3H/2, W] (the luma plane's H rows
+    stacked on the chroma plane's H/2 rows of interleaved U,V bytes, the layout cv2 uses) or a
+    pair (luma [H, W], chroma [H/2, W]); H and W even, rows may be strided, columns must be
+    adjacent.  crops: None, or per frame None (the whole frame) or (x, y, w, h) inside it, at any
+    origin.  The engine converts each crop exactly as cv2.cvtColor(nv12, COLOR_YUV2BGR_NV12)
+    [y:y+h, x:x+w] (BT.601 limited range), then resizes and subtracts the means as
+    forward_device_frames, bit for bit, in one launch into image_input, without writing a BGR
+    frame (sqdet_forward_frames_nv12).  rescale=True scales the boxes back to each crop.
+    Asynchronous: read the results through results_device()."""
+    frames = list(frames)
+    B, n = self.mc.BATCH_SIZE, len(frames)
+    if not 1 <= n <= B:
+      raise ValueError('need 1 to %d frames, got %d' % (B, n))
+    if order not in ('demo', 'eval'):
+      raise ValueError("order must be 'demo' or 'eval', got %r" % (order,))
+    crops = [None] * n if crops is None else list(crops)
+    if len(crops) != n:
+      raise ValueError('need one crop (or None) per frame, got %d for %d frames' % (len(crops), n))
+
+    def plane(i, name, t, rows):
+      dtype, device = getattr(t, 'dtype', None), getattr(t, 'device', None)
+      if str(dtype) != 'torch.uint8':
+        raise ValueError('frame %d: need a uint8 %s tensor, got %s' % (i, name, dtype))
+      if getattr(device, 'type', None) != 'cuda' or device.index != self.gpu_id:
+        raise ValueError('frame %d: need a %s tensor on cuda:%d, got %s'
+                         % (i, name, self.gpu_id, device))
+      shape, stride = tuple(t.shape), tuple(t.stride())
+      if len(shape) != 2 or (rows is not None and shape[0] != rows):
+        raise ValueError('frame %d: %s plane of shape %r does not fit' % (i, name, shape))
+      pitch = stride[0] if shape[0] > 1 else shape[1]       # a single row's stride is never used
+      if stride[1] != 1 or pitch < shape[1]:
+        raise ValueError('frame %d: need %s strides (row, 1) with row >= w, got %r'
+                         % (i, name, stride))
+      return t.data_ptr(), pitch
+
+    lp, lpitch, cp, cpitch, hs, ws, rects = [], [], [], [], [], [], []
+    for i, f in enumerate(frames):
+      if isinstance(f, (tuple, list)):
+        if len(f) != 2:
+          raise ValueError('frame %d: need a tensor or a (luma, chroma) pair' % i)
+        luma, chroma = f
+        shape = tuple(getattr(luma, 'shape', ()))
+        h, w = (shape + (0, 0))[:2]
+      else:
+        shape = tuple(getattr(f, 'shape', ()))
+        if len(shape) != 2 or shape[0] % 3:
+          raise ValueError('frame %d: need shape [3H/2, W], got %r' % (i, shape))
+        h, w = 2 * shape[0] // 3, shape[1]
+        luma, chroma = f[:h], f[h:]
+      if h < 2 or w < 2 or h % 2 or w % 2:
+        raise ValueError('frame %d: need an even height and width of at least 2, got %dx%d'
+                         % (i, w, h))
+      lp_i, lpitch_i = plane(i, 'luma', luma, h)
+      cp_i, cpitch_i = plane(i, 'chroma', chroma, h // 2)
+      if tuple(chroma.shape)[1] != w:
+        raise ValueError('frame %d: chroma width %d, luma width %d' % (i, chroma.shape[1], w))
+      rect = (0, 0, w, h) if crops[i] is None else tuple(int(v) for v in crops[i])
+      x, y, cw, ch = rect if len(rect) == 4 else (0, 0, 0, 0)
+      if len(rect) != 4 or cw < 1 or ch < 1 or x < 0 or y < 0 or x + cw > w or y + ch > h:
+        raise ValueError('frame %d: crop %r is not a non-empty (x, y, w, h) inside %dx%d'
+                         % (i, crops[i], w, h))
+      lp.append(lp_i)
+      lpitch.append(lpitch_i)
+      cp.append(cp_i)
+      cpitch.append(cpitch_i)
+      hs.append(h)
+      ws.append(w)
+      rects.extend(rect)
+    _lib.check(self._lib.sqdet_forward_frames_nv12(
+        self._engine, n, (C.c_void_p * n)(*lp), (C.c_int64 * n)(*lpitch), (C.c_void_p * n)(*cp),
+        (C.c_int64 * n)(*cpitch), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws),
+        (C.c_int32 * (4 * n))(*rects), {'demo': 0, 'eval': 1}[order], int(bool(rescale)),
+        stream))
+
   def forward_profiled(self, images_dev_ptr, stream=None):
     n = self._lib.sqdet_num_ops(self._engine)
     ms = np.zeros(n, np.float32)
