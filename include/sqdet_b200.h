@@ -268,6 +268,45 @@ int sqdet_forward_frames_nv12(sqdet_engine* e, int n, const uint8_t* const* luma
                               const int64_t* chroma_pitches, const int32_t* heights,
                               const int32_t* widths, const int32_t* crops, int order, int rescale,
                               void* stream);
+/* Pixel formats of sqdet_forward_frames and the cv2.cvtColor code each frame is converted by.   */
+#define SQDET_FMT_BGR        0  /* plane 0: packed B,G,R  (== sqdet_forward_frames_u8)        */
+#define SQDET_FMT_RGB        1  /* plane 0: packed R,G,B                  cv2 COLOR_RGB2BGR    */
+#define SQDET_FMT_BGRA       2  /* plane 0: packed B,G,R,A, A never read  cv2 COLOR_BGRA2BGR   */
+#define SQDET_FMT_RGBA       3  /* plane 0: packed R,G,B,A, A never read  cv2 COLOR_RGBA2BGR   */
+#define SQDET_FMT_RGB_PLANAR 4  /* planes 0,1,2: R, G, B, h rows of w bytes (torch [3,h,w])   */
+#define SQDET_FMT_NV12       5  /* luma + interleaved U,V (== sqdet_forward_frames_nv12)       */
+#define SQDET_FMT_I420       6  /* luma, U, V; U and V h/2 rows of w/2     cv2 COLOR_YUV2BGR_I420 */
+/* n frames of pixel format `format` already in device memory on the engine's device: decoder
+ * output (torchvision.io.decode_jpeg(device='cuda') gives SQDET_FMT_RGB_PLANAR, NVDEC NV12),
+ * render targets and capture surfaces (BGRA, RGBA).  Frame i is heights[i] x widths[i]; its planes
+ * are planes[3i + p] (p below the format's plane count; unused entries are not read and may be
+ * NULL), plane p's row r at planes[3i + p] + r*pitches[3i + p], any start byte.  Each plane has
+ *   - packed BGR, RGB: h rows of 3w bytes; BGRA, RGBA: h rows of 4w bytes;
+ *   - RGB_PLANAR: three planes of h rows of w bytes;
+ *   - NV12: h rows of w bytes, then h/2 rows of w interleaved U,V bytes (h, w even);
+ *   - I420: h rows of w bytes, then U and V of h/2 rows of w/2 bytes (h, w even).
+ * NULL pitches = tight rows.  crops: NULL (whole frames) or n x (x, y, w, h), a non-empty
+ * rectangle inside the frame at any origin (a 4:2:0 crop at an odd origin reads the frame's own
+ * chroma samples).  Each crop is exactly cv2.cvtColor(frame, code)[y:y+h, x:x+w] with the code
+ * listed beside the format (the YUV formats by OpenCV's BT.601 limited-range fixed-point
+ * conversion), and the call is bit for bit sqdet_forward_frames_u8 on those BGR crops: resize +
+ * `- mc.BGR_MEANS` in `order` into tensor 0, rescale by the crop's size, then the forward on
+ * `stream`.  No BGR frame is written.  Asynchronous; no host synchronisation.
+ *   - sqdet_forward_frames_u8 is this call with SQDET_FMT_BGR and no crops, and
+ *     sqdet_forward_frames_nv12 with SQDET_FMT_NV12: same launches, same results.
+ *   - Launches: sqdet_launches_per_forward (without a box-scale table), plus one conversion launch
+ *     per 64 frames (BGR, RGB, BGRA, RGBA), 56 (NV12) or 45 (RGB_PLANAR, I420), plus the rescale
+ *     launch when rescale != 0.
+ *   - Refused before any device work, leaving graphs, pipeline and tensor 0 untouched:
+ *     SQDET_ERR_INVALID_ARG for a null engine or array, n outside [1, B], an unknown order or
+ *     format, a null plane the format needs, a height or width <= 0 (or odd for NV12 and I420), a
+ *     pitch below the plane's row bytes, an empty crop or one outside the frame, or a plane whose
+ *     bytes ((rows-1)*pitch + row bytes) are not device memory of the engine's device inside one
+ *     allocation; SQDET_ERR_STATE before sqdet_finalize.
+ * Like sqdet_forward_u8, one engine per stream: results are read through sqdet_results_dev.   */
+int sqdet_forward_frames(sqdet_engine* e, int n, int format, const uint8_t* const* planes,
+                         const int64_t* pitches, const int32_t* heights, const int32_t* widths,
+                         const int32_t* crops, int order, int rescale, void* stream);
 /* src/eval.py:83-84 for callers that resize on the host: xy_scales = B pairs (x_scale,
  * y_scale), host memory; every later forward of the paths fed already-resized images
  * (sqdet_forward(_n), sqdet_forward_profiled, sqdet_detect, sqdet_submit) divides

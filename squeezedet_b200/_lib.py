@@ -88,6 +88,7 @@ SIGNATURES = {
     'sqdet_submit_frames_n': (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _vp, _vp]),
     'sqdet_forward_frames_u8': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     'sqdet_forward_frames_nv12': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    'sqdet_forward_frames': (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     'sqdet_set_box_scale': (_i, [_vp, _vp]),
     'sqdet_launches_per_forward': (_i, [_vp]),
     'sqdet_engine_stream': (_vp, [_vp]),

@@ -112,6 +112,35 @@ Nv12Frame nv12_frame(const uint8_t* luma, int64_t luma_pitch, const uint8_t* chr
 int launch_resize_meansub_nv12_batch(const Nv12Frame* frames, int n, float* dst, int H, int W,
                                      const double* means, int sub_first, float* scales_xy,
                                      cudaStream_t stream);
+// The memory layout of a pixel format of sqdet_forward_frames (SQDET_FMT_*).  Plane p of an h x w
+// frame holds h >> y_shift rows of (w >> x_shift) * bytes_per_px bytes, and a crop at (x, y) starts
+// (y >> y_shift) * pitch + (x >> x_shift) * bytes_per_px bytes into it.
+struct PixPlane {
+  int bytes_per_px, x_shift, y_shift;
+};
+struct PixFormat {
+  int planes;
+  bool even;                 // 4:2:0 chroma: the height and width must be even
+  const char* least_pitch;   // the least row pitch, as a refusal names it
+  PixPlane plane[3];
+};
+// The layout of SQDET_FMT_* `format`, or null for an unknown format.
+const PixFormat* pix_format(int format);
+// One frame of sqdet_forward_frames: its planes (as many as the format has) and their row
+// pitches, and the h x w crop at (x, y) to run.
+struct FrameSource {
+  const uint8_t* plane[3];
+  int64_t pitch[3];
+  int x, y, h, w;
+};
+// Each crop converted to BGR as the format's cv2.cvtColor code does, then
+// launch_resize_meansub_u8_batch's resize and mean subtraction, bit for bit, without writing a
+// BGR frame.  SQDET_FMT_BGR and SQDET_FMT_NV12 are exactly launch_resize_meansub_u8_batch and
+// launch_resize_meansub_nv12_batch; the other formats launch per 64 (packed) or 45 (three-plane)
+// frames.  The frames' checks against pix_format are the caller's.
+int launch_resize_meansub_frames(int format, const FrameSource* frames, int n, float* dst, int H,
+                                 int W, const double* means, int sub_first, float* scales_xy,
+                                 cudaStream_t stream);
 int launch_add_relu(const float* a, const float* b, float* y, int64_t n, cudaStream_t stream);
 
 int launch_interpret(const float* preds, const float* anchors, float* boxes, float* probs,

@@ -1360,105 +1360,120 @@ static int prepare_frames(sqdet_engine* e, int rescale, float** scales) {
   return SQDET_OK;
 }
 
-int sqdet_forward_frames_u8(sqdet_engine* e, int n, const uint8_t* const* frames_dev,
-                            const int32_t* heights, const int32_t* widths,
-                            const int64_t* row_pitches, int order, int rescale, void* stream_v) {
-  if (!e || !frames_dev || !heights || !widths)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_u8: null argument");
-  if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_forward_frames_u8 before sqdet_finalize");
+// Where the planes of sqdet_forward_frames' frames are: plane p of frame i at
+// ptr[p][i * stride], its row pitch at pitch[p][i * stride] (tight rows when pitch[p] is null).
+struct FramePlanes {
+  const uint8_t* const* ptr[3];
+  const int64_t* pitch[3];
+  int stride;
+};
+
+// sqdet_forward_frames and the two calls that are it for one format; `what` names the call in
+// refusals.  Every check is driven by the format's pix_format layout.
+static int forward_frames(sqdet_engine* e, const char* what, int n, int format,
+                          const FramePlanes& pl, const int32_t* heights, const int32_t* widths,
+                          const int32_t* crops, int order, int rescale, void* stream_v) {
+  const std::string name = what;
+  const PixFormat* pf = pix_format(format);
+  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
+  bool null_array = !e || !heights || !widths;
+  for (int p = 0; p < pf->planes; ++p) null_array = null_array || !pl.ptr[p];
+  if (null_array) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (!e->finalized) return fail(SQDET_ERR_STATE, name + " before sqdet_finalize");
   const sqdet_config& c = e->cfg;
   if (n < 1 || n > c.batch_size)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_u8: n must be in [1, batch_size]");
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, batch_size]");
   if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_u8: order must be 0 (demo) or 1 (eval)");
+    return fail(SQDET_ERR_INVALID_ARG, name + ": order must be 0 (demo) or 1 (eval)");
+  // plane p of an H x W frame: rows(H, p) rows of row_bytes(W, p) bytes
+  auto rows = [&](int64_t H, int p) { return H >> pf->plane[p].y_shift; };
+  auto row_bytes = [&](int64_t W, int p) {
+    return (W >> pf->plane[p].x_shift) * pf->plane[p].bytes_per_px;
+  };
+  std::vector<FrameSource> fr((size_t)n);
   for (int i = 0; i < n; ++i) {
-    const int64_t h = heights[i], w = widths[i];
-    const int64_t pitch = row_pitches ? row_pitches[i] : 3 * w;
-    const std::string which = "sqdet_forward_frames_u8: frame " + std::to_string(i);
-    if (!frames_dev[i]) return fail(SQDET_ERR_INVALID_ARG, which + " is a null pointer");
-    if (h <= 0 || w <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
-    if (pitch < 3 * w) return fail(SQDET_ERR_INVALID_ARG, which + ": row pitch below 3 * width");
+    const int64_t H = heights[i], W = widths[i];
+    const std::string which = name + ": frame " + std::to_string(i);
+    FrameSource& s = fr[(size_t)i];
+    for (int p = 0; p < pf->planes; ++p) {
+      s.plane[p] = pl.ptr[p][(size_t)i * pl.stride];
+      if (!s.plane[p])
+        return fail(SQDET_ERR_INVALID_ARG, which + (pf->planes == 1 ? " is a null pointer" : " has a null plane"));
+    }
+    if (!pf->even && (H <= 0 || W <= 0)) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
+    if (pf->even && (H <= 0 || W <= 0 || H % 2 || W % 2))
+      return fail(SQDET_ERR_INVALID_ARG, which + ": height and width must be positive and even");
+    for (int p = 0; p < pf->planes; ++p) {
+      s.pitch[p] = pl.pitch[p] ? pl.pitch[p][(size_t)i * pl.stride] : row_bytes(W, p);
+      if (s.pitch[p] < row_bytes(W, p))
+        return fail(SQDET_ERR_INVALID_ARG, which + ": row pitch below " + pf->least_pitch);
+    }
+    const int32_t* r = crops ? crops + 4 * i : nullptr;
+    if (r) {
+      const int64_t x = r[0], y = r[1], w = r[2], h = r[3];
+      if (w <= 0 || h <= 0) return fail(SQDET_ERR_INVALID_ARG, which + ": empty crop");
+      if (x < 0 || y < 0 || x + w > W || y + h > H)
+        return fail(SQDET_ERR_INVALID_ARG, which + ": crop outside the frame");
+    }
+    s.x = r ? r[0] : 0;
+    s.y = r ? r[1] : 0;
+    s.w = r ? r[2] : (int)W;
+    s.h = r ? r[3] : (int)H;
   }
   DeviceGuard guard(e->device);
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
-  std::vector<ResizeFrame> fr((size_t)n);
   for (int i = 0; i < n; ++i) {
-    const int64_t h = heights[i], w = widths[i];
-    const int64_t pitch = row_pitches ? row_pitches[i] : 3 * w;
-    // the frame's bytes end at (h - 1) * pitch + 3 * w; refused when that overflows int64
-    const bool fits = h == 1 || pitch <= (INT64_MAX - 3 * w) / (h - 1);
-    if (!fits || !device_range_ok(frames_dev[i], (h - 1) * pitch + 3 * w, e->device))
-      return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_u8: frame " + std::to_string(i) +
-                                             " is not inside one device allocation on the engine's device");
-    fr[(size_t)i] = resize_frame(frames_dev[i], pitch, (int)h, (int)w, c.image_height, c.image_width);
+    const FrameSource& s = fr[(size_t)i];
+    const int64_t H = heights[i], W = widths[i];
+    for (int p = 0; p < pf->planes; ++p) {
+      // the plane's bytes end at (rows - 1) * pitch + row bytes; refused when that overflows int64
+      const int64_t k = rows(H, p), b = row_bytes(W, p);
+      const bool fits = k == 1 || s.pitch[p] <= (INT64_MAX - b) / (k - 1);
+      if (!fits || !device_range_ok(s.plane[p], (k - 1) * s.pitch[p] + b, e->device))
+        return fail(SQDET_ERR_INVALID_ARG,
+                    name + ": frame " + std::to_string(i) +
+                        (pf->planes == 1 ? " is not inside" : ": a plane is not inside") +
+                        " one device allocation on the engine's device");
+    }
   }
   cudaStream_t stream = (cudaStream_t)stream_v;
   float* scales = nullptr;
   int rc = prepare_frames(e, rescale, &scales);
   if (rc) return rc;
   Tensor& t0 = e->tensors[0];
-  rc = launch_resize_meansub_u8_batch(fr.data(), n, t0.dev, c.image_height, c.image_width,
-                                      e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE, scales,
-                                      stream);
+  rc = launch_resize_meansub_frames(format, fr.data(), n, t0.dev, c.image_height, c.image_width,
+                                    e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE, scales,
+                                    stream);
   if (rc) return rc;
   return forward_impl(e, t0.dev, false, n, scales, stream);
+}
+
+int sqdet_forward_frames(sqdet_engine* e, int n, int format, const uint8_t* const* planes,
+                         const int64_t* pitches, const int32_t* heights, const int32_t* widths,
+                         const int32_t* crops, int order, int rescale, void* stream) {
+  const FramePlanes pl = {{planes, planes ? planes + 1 : nullptr, planes ? planes + 2 : nullptr},
+                          {pitches, pitches ? pitches + 1 : nullptr, pitches ? pitches + 2 : nullptr},
+                          3};
+  return forward_frames(e, "sqdet_forward_frames", n, format, pl, heights, widths, crops, order,
+                        rescale, stream);
+}
+
+int sqdet_forward_frames_u8(sqdet_engine* e, int n, const uint8_t* const* frames_dev,
+                            const int32_t* heights, const int32_t* widths,
+                            const int64_t* row_pitches, int order, int rescale, void* stream) {
+  const FramePlanes pl = {{frames_dev, nullptr, nullptr}, {row_pitches, nullptr, nullptr}, 1};
+  return forward_frames(e, "sqdet_forward_frames_u8", n, SQDET_FMT_BGR, pl, heights, widths,
+                        nullptr, order, rescale, stream);
 }
 
 int sqdet_forward_frames_nv12(sqdet_engine* e, int n, const uint8_t* const* luma_dev,
                               const int64_t* luma_pitches, const uint8_t* const* chroma_dev,
                               const int64_t* chroma_pitches, const int32_t* heights,
                               const int32_t* widths, const int32_t* crops, int order, int rescale,
-                              void* stream_v) {
-  if (!e || !luma_dev || !chroma_dev || !heights || !widths)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_nv12: null argument");
-  if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_forward_frames_nv12 before sqdet_finalize");
-  const sqdet_config& c = e->cfg;
-  if (n < 1 || n > c.batch_size)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_nv12: n must be in [1, batch_size]");
-  if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_nv12: order must be 0 (demo) or 1 (eval)");
-  for (int i = 0; i < n; ++i) {
-    const int64_t H = heights[i], W = widths[i];
-    const int64_t lp = luma_pitches ? luma_pitches[i] : W, cp = chroma_pitches ? chroma_pitches[i] : W;
-    const std::string which = "sqdet_forward_frames_nv12: frame " + std::to_string(i);
-    if (!luma_dev[i] || !chroma_dev[i]) return fail(SQDET_ERR_INVALID_ARG, which + " has a null plane");
-    if (H <= 0 || W <= 0 || H % 2 || W % 2)
-      return fail(SQDET_ERR_INVALID_ARG, which + ": height and width must be positive and even");
-    if (lp < W || cp < W) return fail(SQDET_ERR_INVALID_ARG, which + ": row pitch below the width");
-    if (crops) {
-      const int64_t x = crops[4 * i], y = crops[4 * i + 1], w = crops[4 * i + 2], h = crops[4 * i + 3];
-      if (w <= 0 || h <= 0) return fail(SQDET_ERR_INVALID_ARG, which + ": empty crop");
-      if (x < 0 || y < 0 || x + w > W || y + h > H)
-        return fail(SQDET_ERR_INVALID_ARG, which + ": crop outside the frame");
-    }
-  }
-  DeviceGuard guard(e->device);
-  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
-  std::vector<Nv12Frame> fr((size_t)n);
-  for (int i = 0; i < n; ++i) {
-    const int64_t H = heights[i], W = widths[i];
-    const int64_t lp = luma_pitches ? luma_pitches[i] : W, cp = chroma_pitches ? chroma_pitches[i] : W;
-    // the planes' bytes end at (H - 1) * lp + W and (H / 2 - 1) * cp + W; refused when either
-    // overflows int64 (H >= 2)
-    const bool fits = lp <= (INT64_MAX - W) / (H - 1) && (H == 2 || cp <= (INT64_MAX - W) / (H / 2 - 1));
-    if (!fits || !device_range_ok(luma_dev[i], (H - 1) * lp + W, e->device) ||
-        !device_range_ok(chroma_dev[i], (H / 2 - 1) * cp + W, e->device))
-      return fail(SQDET_ERR_INVALID_ARG, "sqdet_forward_frames_nv12: frame " + std::to_string(i) +
-                                             ": a plane is not inside one device allocation on the engine's device");
-    const int32_t* r = crops ? crops + 4 * i : nullptr;
-    fr[(size_t)i] = nv12_frame(luma_dev[i], lp, chroma_dev[i], cp, r ? r[0] : 0, r ? r[1] : 0,
-                               r ? r[3] : (int)H, r ? r[2] : (int)W, c.image_height, c.image_width);
-  }
-  cudaStream_t stream = (cudaStream_t)stream_v;
-  float* scales = nullptr;
-  int rc = prepare_frames(e, rescale, &scales);
-  if (rc) return rc;
-  Tensor& t0 = e->tensors[0];
-  rc = launch_resize_meansub_nv12_batch(fr.data(), n, t0.dev, c.image_height, c.image_width,
-                                        e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE, scales,
-                                        stream);
-  if (rc) return rc;
-  return forward_impl(e, t0.dev, false, n, scales, stream);
+                              void* stream) {
+  const FramePlanes pl = {{luma_dev, chroma_dev, nullptr}, {luma_pitches, chroma_pitches, nullptr}, 1};
+  return forward_frames(e, "sqdet_forward_frames_nv12", n, SQDET_FMT_NV12, pl, heights, widths,
+                        crops, order, rescale, stream);
 }
 
 // ---- multi-GPU: ONE all-gather of the filtered records ---------------------------------------------

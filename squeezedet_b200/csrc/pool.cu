@@ -8,6 +8,7 @@
 #include <math_constants.h>
 
 #include <algorithm>
+#include <vector>
 
 #include "common.cuh"
 
@@ -199,38 +200,67 @@ __device__ __forceinline__ void resize_meansub_pixel(const Taps& taps, int H0, i
   d[0] = o[0]; d[1] = o[1]; d[2] = o[2];
 }
 
-// The taps of a uint8 BGR frame whose row r starts at src + r * pitch (any byte alignment): a
-// channel is a byte load served by L1.
-struct BgrTaps {
+// The taps of a packed uint8 frame of kBpp bytes per pixel whose row r starts at src + r * pitch
+// (any byte alignment), with B, G, R at byte offsets kB, kG, kR of a pixel (other bytes, such as
+// alpha, are never read): a channel is a byte load served by L1.  The layout is a compile-time
+// instance, so a tap costs the same address arithmetic as BGR's.
+template <int kBpp, int kB, int kG, int kR>
+struct PackedTaps {
   const uint8_t* __restrict__ src;
   long long pitch;
   __device__ __forceinline__ float operator()(const int (&ys)[2], const int (&xs)[2], int r, int q,
                                              int c) const {
-    return (float)src[(long long)ys[r] * pitch + (long long)xs[q] * 3 + c];
+    return (float)src[(long long)ys[r] * pitch + (long long)xs[q] * kBpp +
+                      (c == 0 ? kB : c == 1 ? kG : kR)];
+  }
+};
+using BgrTaps = PackedTaps<3, 0, 1, 2>;
+
+// The taps of three uint8 planes holding R, G and B (torch's [3, h, w] image layout): channel c
+// (B, G, R) of pixel (y, x) is byte x of row y of plane 2 - c, each plane at any byte and pitch.
+struct PlanarTaps {
+  const uint8_t* __restrict__ plane[3];
+  long long pitch[3];
+  __device__ __forceinline__ float operator()(const int (&ys)[2], const int (&xs)[2], int r, int q,
+                                             int c) const {
+    return (float)plane[2 - c][(long long)ys[r] * pitch[2 - c] + xs[q]];
   }
 };
 
-// The taps of an NV12 crop: one luma byte and the U,V pair of its 2x2 chroma block, converted as
-// cv2.cvtColor(COLOR_YUV2BGR_NV12) does (OpenCV's BT.601 limited-range ITUR_BT_601_* constants,
-// 20 fraction bits; oracle.nv12.nv12_to_bgr).  Crop pixel (y, x) is frame pixel
-// (y0 + y, x0 + x); luma and chroma point at the crop origin's byte and chroma pair, and the
-// origin's parity (x_odd, y_odd) picks the chroma block, so an odd origin reads the frame's own
-// samples.  int32 suffices: every sum stays below 2^30 in magnitude.  Each tap is loaded and
-// converted once, when its channel 0 is asked for.
-struct Nv12Taps {
+// The taps of a YUV 4:2:0 crop: one luma byte and the U,V samples of its 2x2 chroma block,
+// converted as cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420) does (OpenCV's BT.601 limited-range
+// ITUR_BT_601_* constants, 20 fraction bits; oracle.nv12.nv12_to_bgr).  kInterleaved: NV12, one
+// chroma plane of U,V pairs at u; otherwise I420, separate U and V planes of half the width.
+// Crop pixel (y, x) is frame pixel (y0 + y, x0 + x); luma and the chroma planes point at the crop
+// origin's byte and chroma sample, and the origin's parity (x_odd, y_odd) picks the chroma block,
+// so an odd origin reads the frame's own samples.  int32 suffices: every sum stays below 2^30 in
+// magnitude.  Each tap is loaded and converted once, when its channel 0 is asked for.
+template <bool kInterleaved>
+struct Yuv420Taps {
   const uint8_t* __restrict__ luma;
-  const uint8_t* __restrict__ chroma;
-  long long luma_pitch, chroma_pitch;
+  const uint8_t* __restrict__ u_plane;
+  long long luma_pitch, u_pitch;
   int x_odd, y_odd;
   mutable float bgr[2][2][3];   // tap (r, q), converted at its channel 0
+  // I420's V plane, last: with it after the fields NV12 uses, the NV12 instance compiles to the
+  // code it had before I420 shared this struct
+  const uint8_t* __restrict__ v_plane;
+  long long v_pitch;
   __device__ __forceinline__ float operator()(const int (&ys)[2], const int (&xs)[2], int r, int q,
                                              int c) const {
     if (c == 0) {
       const int y = ys[r], x = xs[q];
       const int Y = luma[(long long)y * luma_pitch + x];
-      const uint8_t* uv =
-          chroma + (long long)((y + y_odd) >> 1) * chroma_pitch + ((x + x_odd) & ~1);
-      const int u = (int)uv[0] - 128, v = (int)uv[1] - 128;
+      const long long cy = (long long)((y + y_odd) >> 1);
+      int u, v;
+      if (kInterleaved) {
+        const uint8_t* uv = u_plane + cy * u_pitch + ((x + x_odd) & ~1);
+        u = (int)uv[0] - 128;
+        v = (int)uv[1] - 128;
+      } else {
+        u = (int)u_plane[cy * u_pitch + ((x + x_odd) >> 1)] - 128;
+        v = (int)v_plane[cy * v_pitch + ((x + x_odd) >> 1)] - 128;
+      }
       const int yy = max(Y - 16, 0) * 1220542 + (1 << 19);
       bgr[r][q][0] = (float)min(max((yy + 2116026 * u) >> 20, 0), 255);
       bgr[r][q][1] = (float)min(max((yy - 852492 * v - 409993 * u) >> 20, 0), 255);
@@ -240,9 +270,42 @@ struct Nv12Taps {
   }
 };
 
+// A packed RGB, BGRA or RGBA frame: ResizeFrame's descriptor, typed by its layout.
+template <int kBpp, int kB, int kG, int kR>
+struct PackedFrame : ResizeFrame {};
+using RgbFrame = PackedFrame<3, 2, 1, 0>;
+using BgraFrame = PackedFrame<4, 0, 1, 2>;
+using RgbaFrame = PackedFrame<4, 2, 1, 0>;
+// The h x w crop of a planar RGB or an I420 frame: plane[p] points at the crop origin's sample of
+// plane p, and (x_odd, y_odd), the origin's parity, picks I420's chroma block.  88 bytes.
+struct ThreePlaneFrame {
+  const uint8_t* plane[3];
+  int64_t pitch[3];
+  double scale_x, scale_y;
+  float box_scale_x, box_scale_y;
+  int h, w;
+  int x_odd, y_odd;
+};
+// Frames per launch: 45 descriptors of 88 bytes and the kernel's other parameters fill the
+// classic 4 KiB parameter block.
+constexpr int kThreePlaneFramesPerLaunch = 45;
+struct PlanarFrame : ThreePlaneFrame {};
+struct I420Frame : ThreePlaneFrame {};
+
 __device__ __forceinline__ BgrTaps taps(const ResizeFrame& f) { return {f.src, f.pitch}; }
-__device__ __forceinline__ Nv12Taps taps(const Nv12Frame& f) {
-  return {f.luma, f.chroma, f.luma_pitch, f.chroma_pitch, f.x_odd, f.y_odd, {}};
+template <int kBpp, int kB, int kG, int kR>
+__device__ __forceinline__ PackedTaps<kBpp, kB, kG, kR> taps(const PackedFrame<kBpp, kB, kG, kR>& f) {
+  return {f.src, f.pitch};
+}
+__device__ __forceinline__ Yuv420Taps<true> taps(const Nv12Frame& f) {
+  return {f.luma, f.chroma, f.luma_pitch, f.chroma_pitch, f.x_odd, f.y_odd, {}, nullptr, 0};
+}
+__device__ __forceinline__ PlanarTaps taps(const PlanarFrame& f) {
+  return {{f.plane[0], f.plane[1], f.plane[2]}, {f.pitch[0], f.pitch[1], f.pitch[2]}};
+}
+__device__ __forceinline__ Yuv420Taps<false> taps(const I420Frame& f) {
+  return {f.plane[0], f.plane[1], f.pitch[0], f.pitch[1], f.x_odd, f.y_odd, {}, f.plane[2],
+          f.pitch[2]};
 }
 
 struct ResizeFrameBatch {
@@ -251,10 +314,22 @@ struct ResizeFrameBatch {
 struct Nv12FrameBatch {
   Nv12Frame f[kNv12FramesPerLaunch];
 };
+template <class Frame>
+struct PackedFrameBatch {
+  Frame f[kResizeFramesPerLaunch];
+};
+template <class Frame>
+struct ThreePlaneFrameBatch {
+  Frame f[kThreePlaneFramesPerLaunch];
+};
 // Descriptors travel in the parameter block: no device table, no copy, no host synchronisation.
 static_assert(sizeof(ResizeFrameBatch) + 128 <= 4096, "resize descriptors exceed 4 KiB of parameters");
 // The kernel's other parameters take 56 bytes.
 static_assert(sizeof(Nv12FrameBatch) + 64 <= 4096, "NV12 descriptors exceed 4 KiB of parameters");
+static_assert(sizeof(PackedFrameBatch<RgbaFrame>) == sizeof(ResizeFrameBatch),
+              "packed descriptors are ResizeFrame's");
+static_assert(sizeof(ThreePlaneFrameBatch<I420Frame>) + 64 <= 4096,
+              "three-plane descriptors exceed 4 KiB of parameters");
 
 // Up to the batch's frame count in one launch: blockIdx.y is the frame, x runs over its H x W
 // output pixels, written as image blockIdx.y of the fp32 [count, H, W, 3] batch at dst.  With
@@ -360,6 +435,116 @@ int launch_resize_meansub_nv12_batch(const Nv12Frame* frames, int n, float* dst,
       return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_nv12: row pitch below the crop width");
   return launch_batches<Nv12FrameBatch>("resize_meansub_u8_batch_kernel<Nv12FrameBatch>", frames,
                                         n, dst, H, W, means, sub_first, scales_xy, stream);
+}
+
+const PixFormat* pix_format(int format) {
+  static_assert(SQDET_FMT_BGR == 0 && SQDET_FMT_RGB == 1 && SQDET_FMT_BGRA == 2 &&
+                    SQDET_FMT_RGBA == 3 && SQDET_FMT_RGB_PLANAR == 4 && SQDET_FMT_NV12 == 5 &&
+                    SQDET_FMT_I420 == 6,
+                "the table is indexed by SQDET_FMT_*");
+  static const PixFormat table[] = {
+      {1, false, "3 * width", {{3, 0, 0}}},                                       // BGR
+      {1, false, "3 * width", {{3, 0, 0}}},                                       // RGB
+      {1, false, "4 * width", {{4, 0, 0}}},                                       // BGRA
+      {1, false, "4 * width", {{4, 0, 0}}},                                       // RGBA
+      {3, false, "the width", {{1, 0, 0}, {1, 0, 0}, {1, 0, 0}}},                 // RGB_PLANAR
+      {2, true, "the width", {{1, 0, 0}, {2, 1, 1}}},                             // NV12
+      {3, true, "the width (Y) or half of it (U, V)", {{1, 0, 0}, {1, 1, 1}, {1, 1, 1}}},  // I420
+  };
+  return format >= 0 && format < (int)(sizeof table / sizeof table[0]) ? &table[format] : nullptr;
+}
+
+namespace {
+
+// The byte of plane p at the origin of frame s's crop.
+const uint8_t* crop_origin(const PixFormat& pf, const FrameSource& s, int p) {
+  const PixPlane& q = pf.plane[p];
+  return s.plane[p] + (int64_t)(s.y >> q.y_shift) * s.pitch[p] +
+         (int64_t)(s.x >> q.x_shift) * q.bytes_per_px;
+}
+
+template <class Frame>
+int launch_packed(const char* what, const PixFormat& pf, const FrameSource* s, int n, float* dst,
+                  int H, int W, const double* means, int sub_first, float* scales_xy,
+                  cudaStream_t stream) {
+  std::vector<Frame> fr((size_t)n);
+  for (int i = 0; i < n; ++i)
+    static_cast<ResizeFrame&>(fr[(size_t)i]) =
+        resize_frame(crop_origin(pf, s[i], 0), s[i].pitch[0], s[i].h, s[i].w, H, W);
+  return launch_batches<PackedFrameBatch<Frame>>(what, fr.data(), n, dst, H, W, means, sub_first,
+                                                 scales_xy, stream);
+}
+
+template <class Frame>
+int launch_three_plane(const char* what, const PixFormat& pf, const FrameSource* s, int n,
+                       float* dst, int H, int W, const double* means, int sub_first,
+                       float* scales_xy, cudaStream_t stream) {
+  std::vector<Frame> fr((size_t)n);
+  for (int i = 0; i < n; ++i) {
+    const ResizeFrame r = resize_frame(nullptr, 0, s[i].h, s[i].w, H, W);
+    Frame& f = fr[(size_t)i];
+    for (int p = 0; p < 3; ++p) {
+      f.plane[p] = crop_origin(pf, s[i], p);
+      f.pitch[p] = s[i].pitch[p];
+    }
+    f.scale_x = r.scale_x;
+    f.scale_y = r.scale_y;
+    f.box_scale_x = r.box_scale_x;
+    f.box_scale_y = r.box_scale_y;
+    f.h = s[i].h;
+    f.w = s[i].w;
+    f.x_odd = s[i].x & 1;
+    f.y_odd = s[i].y & 1;
+  }
+  return launch_batches<ThreePlaneFrameBatch<Frame>>(what, fr.data(), n, dst, H, W, means,
+                                                     sub_first, scales_xy, stream);
+}
+
+}  // namespace
+
+int launch_resize_meansub_frames(int format, const FrameSource* frames, int n, float* dst, int H,
+                                 int W, const double* means, int sub_first, float* scales_xy,
+                                 cudaStream_t stream) {
+  const PixFormat* pf = pix_format(format);
+  if (!pf) return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_frames: unknown format");
+  if (n <= 0 || H <= 0 || W <= 0)
+    return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_frames: non-positive image size");
+  for (int i = 0; i < n; ++i)
+    if (frames[i].h <= 0 || frames[i].w <= 0)
+      return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_frames: non-positive crop size");
+  const FrameSource* s = frames;
+  switch (format) {
+    case SQDET_FMT_BGR: {
+      std::vector<ResizeFrame> fr((size_t)n);
+      for (int i = 0; i < n; ++i)
+        fr[(size_t)i] = resize_frame(crop_origin(*pf, s[i], 0), s[i].pitch[0], s[i].h, s[i].w, H, W);
+      return launch_resize_meansub_u8_batch(fr.data(), n, dst, H, W, means, sub_first, scales_xy,
+                                            stream);
+    }
+    case SQDET_FMT_NV12: {
+      std::vector<Nv12Frame> fr((size_t)n);
+      for (int i = 0; i < n; ++i)
+        fr[(size_t)i] = nv12_frame(s[i].plane[0], s[i].pitch[0], s[i].plane[1], s[i].pitch[1],
+                                   s[i].x, s[i].y, s[i].h, s[i].w, H, W);
+      return launch_resize_meansub_nv12_batch(fr.data(), n, dst, H, W, means, sub_first, scales_xy,
+                                              stream);
+    }
+    case SQDET_FMT_RGB:
+      return launch_packed<RgbFrame>("resize_meansub_u8_batch_kernel<RGB>", *pf, s, n, dst, H, W,
+                                     means, sub_first, scales_xy, stream);
+    case SQDET_FMT_BGRA:
+      return launch_packed<BgraFrame>("resize_meansub_u8_batch_kernel<BGRA>", *pf, s, n, dst, H, W,
+                                      means, sub_first, scales_xy, stream);
+    case SQDET_FMT_RGBA:
+      return launch_packed<RgbaFrame>("resize_meansub_u8_batch_kernel<RGBA>", *pf, s, n, dst, H, W,
+                                      means, sub_first, scales_xy, stream);
+    case SQDET_FMT_RGB_PLANAR:
+      return launch_three_plane<PlanarFrame>("resize_meansub_u8_batch_kernel<PlanarFrame>", *pf, s,
+                                             n, dst, H, W, means, sub_first, scales_xy, stream);
+    default:
+      return launch_three_plane<I420Frame>("resize_meansub_u8_batch_kernel<I420Frame>", *pf, s, n,
+                                           dst, H, W, means, sub_first, scales_xy, stream);
+  }
 }
 
 int launch_maxpool(const float* x, float* y, int B, int H, int W, int C, int size,

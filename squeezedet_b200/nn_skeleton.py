@@ -28,6 +28,9 @@ import numpy as np
 from . import _lib
 from ._lib import SqdetError  # noqa: F401
 
+# forward_device_frames_fmt's pixel formats, in SQDET_FMT_* order
+PIXEL_FORMATS = ('bgr', 'rgb', 'bgra', 'rgba', 'rgb_planar', 'nv12', 'i420')
+
 
 class GraphTensor:
   """Opaque handle to a tensor of the engine plan (stands in for a tf.Tensor)."""
@@ -545,6 +548,31 @@ class ModelSkeleton:
     forward_device_frames, bit for bit, in one launch into image_input, without writing a BGR
     frame (sqdet_forward_frames_nv12).  rescale=True scales the boxes back to each crop.
     Asynchronous: read the results through results_device()."""
+    return self.forward_device_frames_fmt(frames, 'nv12', crops=crops, order=order,
+                                          rescale=rescale, stream=stream)
+
+  def forward_device_frames_fmt(self, frames, fmt, crops=None, order='demo', rescale=False,
+                                stream=None):
+    """forward_device_frames of frames in pixel format `fmt` already on this engine's device.
+    Each frame is made of uint8 CUDA tensors whose rows may be strided and whose bytes within a
+    row are adjacent:
+      'bgr', 'rgb'    [h, w, 3] with strides (row, 3, 1);
+      'bgra', 'rgba'  [h, w, 4] with strides (row, 4, 1) (capture surfaces; alpha is never read);
+      'rgb_planar'    [3, h, w] with strides (plane, row, 1), as torchvision.io.decode_jpeg(...,
+                      device='cuda') returns it (or a frame of list(batch) of [n, 3, h, w]), or an
+                      (r, g, b) tuple of [h, w] planes;
+      'nv12'          as forward_device_frames_nv12;
+      'i420'          a tight [3h/2, w] tensor (Y's rows, then U's and V's bytes, as cv2 lays it
+                      out) or a (y [h, w], u [h/2, w/2], v [h/2, w/2]) tuple at any pitches;
+                      h and w even.
+    crops: None, or per frame None (the whole frame) or (x, y, w, h) inside it, at any origin.  The
+    engine converts each crop to BGR exactly as cv2.cvtColor does (COLOR_RGB2BGR, _BGRA2BGR,
+    _RGBA2BGR, _YUV2BGR_NV12, _YUV2BGR_I420), then resizes and subtracts the means as
+    forward_device_frames, bit for bit, in one launch into image_input, without writing a BGR
+    frame (sqdet_forward_frames).  rescale=True scales the boxes back to each crop.
+    Asynchronous: read the results through results_device()."""
+    if fmt not in PIXEL_FORMATS:
+      raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
     frames = list(frames)
     B, n = self.mc.BATCH_SIZE, len(frames)
     if not 1 <= n <= B:
@@ -554,16 +582,41 @@ class ModelSkeleton:
     crops = [None] * n if crops is None else list(crops)
     if len(crops) != n:
       raise ValueError('need one crop (or None) per frame, got %d for %d frames' % (len(crops), n))
+    planes, pitches, hs, ws, rects = [], [], [], [], []
+    for i, f in enumerate(frames):
+      h, w, ps = self._frame_planes(i, f, fmt)
+      rect = (0, 0, w, h) if crops[i] is None else tuple(int(v) for v in crops[i])
+      x, y, cw, ch = rect if len(rect) == 4 else (0, 0, 0, 0)
+      if len(rect) != 4 or cw < 1 or ch < 1 or x < 0 or y < 0 or x + cw > w or y + ch > h:
+        raise ValueError('frame %d: crop %r is not a non-empty (x, y, w, h) inside %dx%d'
+                         % (i, crops[i], w, h))
+      ps = ps + [(None, 0)] * (3 - len(ps))
+      planes.extend(p for p, _ in ps)
+      pitches.extend(q for _, q in ps)
+      hs.append(h)
+      ws.append(w)
+      rects.extend(rect)
+    _lib.check(self._lib.sqdet_forward_frames(
+        self._engine, n, PIXEL_FORMATS.index(fmt), (C.c_void_p * (3 * n))(*planes),
+        (C.c_int64 * (3 * n))(*pitches), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws),
+        (C.c_int32 * (4 * n))(*rects), {'demo': 0, 'eval': 1}[order], int(bool(rescale)),
+        stream))
 
-    def plane(i, name, t, rows):
+  def _frame_planes(self, i, f, fmt):
+    """(h, w, [(pointer, row pitch) per plane]) of frame i in `fmt`, or ValueError naming it."""
+    def on_device(name, t):
       dtype, device = getattr(t, 'dtype', None), getattr(t, 'device', None)
       if str(dtype) != 'torch.uint8':
         raise ValueError('frame %d: need a uint8 %s tensor, got %s' % (i, name, dtype))
       if getattr(device, 'type', None) != 'cuda' or device.index != self.gpu_id:
         raise ValueError('frame %d: need a %s tensor on cuda:%d, got %s'
                          % (i, name, self.gpu_id, device))
+
+    def plane(name, t, rows=None, cols=None):
+      on_device(name, t)
       shape, stride = tuple(t.shape), tuple(t.stride())
-      if len(shape) != 2 or (rows is not None and shape[0] != rows):
+      if (len(shape) != 2 or min(shape) < 1 or (rows is not None and shape[0] != rows)
+          or (cols is not None and shape[1] != cols)):
         raise ValueError('frame %d: %s plane of shape %r does not fit' % (i, name, shape))
       pitch = stride[0] if shape[0] > 1 else shape[1]       # a single row's stride is never used
       if stride[1] != 1 or pitch < shape[1]:
@@ -571,44 +624,64 @@ class ModelSkeleton:
                          % (i, name, stride))
       return t.data_ptr(), pitch
 
-    lp, lpitch, cp, cpitch, hs, ws, rects = [], [], [], [], [], [], []
-    for i, f in enumerate(frames):
-      if isinstance(f, (tuple, list)):
-        if len(f) != 2:
-          raise ValueError('frame %d: need a tensor or a (luma, chroma) pair' % i)
-        luma, chroma = f
-        shape = tuple(getattr(luma, 'shape', ()))
-        h, w = (shape + (0, 0))[:2]
-      else:
-        shape = tuple(getattr(f, 'shape', ()))
-        if len(shape) != 2 or shape[0] % 3:
-          raise ValueError('frame %d: need shape [3H/2, W], got %r' % (i, shape))
-        h, w = 2 * shape[0] // 3, shape[1]
-        luma, chroma = f[:h], f[h:]
+    def even(h, w):
       if h < 2 or w < 2 or h % 2 or w % 2:
         raise ValueError('frame %d: need an even height and width of at least 2, got %dx%d'
                          % (i, w, h))
-      lp_i, lpitch_i = plane(i, 'luma', luma, h)
-      cp_i, cpitch_i = plane(i, 'chroma', chroma, h // 2)
-      if tuple(chroma.shape)[1] != w:
-        raise ValueError('frame %d: chroma width %d, luma width %d' % (i, chroma.shape[1], w))
-      rect = (0, 0, w, h) if crops[i] is None else tuple(int(v) for v in crops[i])
-      x, y, cw, ch = rect if len(rect) == 4 else (0, 0, 0, 0)
-      if len(rect) != 4 or cw < 1 or ch < 1 or x < 0 or y < 0 or x + cw > w or y + ch > h:
-        raise ValueError('frame %d: crop %r is not a non-empty (x, y, w, h) inside %dx%d'
-                         % (i, crops[i], w, h))
-      lp.append(lp_i)
-      lpitch.append(lpitch_i)
-      cp.append(cp_i)
-      cpitch.append(cpitch_i)
-      hs.append(h)
-      ws.append(w)
-      rects.extend(rect)
-    _lib.check(self._lib.sqdet_forward_frames_nv12(
-        self._engine, n, (C.c_void_p * n)(*lp), (C.c_int64 * n)(*lpitch), (C.c_void_p * n)(*cp),
-        (C.c_int64 * n)(*cpitch), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws),
-        (C.c_int32 * (4 * n))(*rects), {'demo': 0, 'eval': 1}[order], int(bool(rescale)),
-        stream))
+
+    def parts(k, what):
+      if not isinstance(f, (tuple, list)):
+        return None
+      if len(f) != k:
+        raise ValueError('frame %d: need a tensor or a %s tuple' % (i, what))
+      return f
+
+    shape = tuple(getattr(f, 'shape', ()))
+    if fmt in ('bgr', 'rgb', 'bgra', 'rgba'):
+      c = 4 if fmt in ('bgra', 'rgba') else 3
+      on_device('frame', f)
+      if len(shape) != 3 or shape[2] != c or shape[0] < 1 or shape[1] < 1:
+        raise ValueError('frame %d: need shape [h, w, %d], got %r' % (i, c, shape))
+      stride = tuple(f.stride())
+      pitch = stride[0] if shape[0] > 1 else c * shape[1]   # a single row's stride is never used
+      if stride[2] != 1 or stride[1] != c or pitch < c * shape[1]:
+        raise ValueError('frame %d: need strides (row, %d, 1) with row >= %d * w, got %r'
+                         % (i, c, c, stride))
+      return shape[0], shape[1], [(f.data_ptr(), pitch)]
+    if fmt == 'rgb_planar':
+      rgb = parts(3, '(r, g, b)')
+      if rgb is None:
+        if len(shape) != 3 or shape[0] != 3:
+          raise ValueError('frame %d: need shape [3, h, w], got %r' % (i, shape))
+        rgb = (f[0], f[1], f[2])
+      h, w = (tuple(getattr(rgb[0], 'shape', ())) + (0, 0))[:2]
+      return h, w, [plane(name, t, h, w) for name, t in zip(('R', 'G', 'B'), rgb)]
+    if fmt == 'nv12':
+      yc = parts(2, '(luma, chroma)')
+      if yc is None:
+        if len(shape) != 2 or shape[0] % 3:
+          raise ValueError('frame %d: need shape [3H/2, W], got %r' % (i, shape))
+        h = 2 * shape[0] // 3
+        yc = (f[:h], f[h:])
+      h, w = (tuple(getattr(yc[0], 'shape', ())) + (0, 0))[:2]
+      even(h, w)
+      return h, w, [plane('luma', yc[0], h, w), plane('chroma', yc[1], h // 2, w)]
+    yuv = parts(3, '(y, u, v)')
+    if yuv is not None:
+      h, w = (tuple(getattr(yuv[0], 'shape', ())) + (0, 0))[:2]
+      even(h, w)
+      return h, w, [plane('Y', yuv[0], h, w), plane('U', yuv[1], h // 2, w // 2),
+                    plane('V', yuv[2], h // 2, w // 2)]
+    on_device('frame', f)
+    if len(shape) != 2 or shape[0] % 3:
+      raise ValueError('frame %d: need shape [3h/2, w], got %r' % (i, shape))
+    h, w = 2 * shape[0] // 3, shape[1]
+    even(h, w)
+    if tuple(f.stride()) != (w, 1):
+      raise ValueError('frame %d: a stacked I420 frame must be tight, strides (%d, 1), got %r'
+                       % (i, w, tuple(f.stride())))
+    y = f.data_ptr()
+    return h, w, [(y, w), (y + h * w, w // 2), (y + h * w + h * w // 4, w // 2)]
 
   def forward_profiled(self, images_dev_ptr, stream=None):
     n = self._lib.sqdet_num_ops(self._engine)
