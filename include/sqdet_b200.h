@@ -307,6 +307,43 @@ int sqdet_forward_frames_nv12(sqdet_engine* e, int n, const uint8_t* const* luma
 int sqdet_forward_frames(sqdet_engine* e, int n, int format, const uint8_t* const* planes,
                          const int64_t* pitches, const int32_t* heights, const int32_t* widths,
                          const int32_t* crops, int order, int rescale, void* stream);
+/* Detection over whole frames larger than the network input, as overlapping tiles at native
+ * scale (an extra "overview" tile of a whole frame, resized, mixes in freely).  n frames in one
+ * SQDET_FMT_* format, laid out exactly as sqdet_forward_frames takes them (planes[3f + p],
+ * pitches[3f + p], heights[f], widths[f]), and t tiles, tiles[5k .. 5k+4] = (frame, x, y, w, h): a
+ * non-empty rectangle inside its frame.  1 <= n <= t <= B, and every frame has a tile.
+ *   1. Rows [0, t) of det_boxes / det_probs / det_class and of the per-tile records and counts
+ *      (sqdet_results_dev) are bitwise sqdet_forward_frames over the tiles as crops of their
+ *      frames, with rescale = 1 (boxes in tile pixels).
+ *   2. Frame f's union U_f is its tiles' rows concatenated in call order, union index
+ *      j = p * A + anchor for the frame's p-th tile; each box is (cx + float(x), cy + float(y), w,
+ *      h), a float32 add (det_boxes itself is not modified).
+ *   3. filter_prediction of U_f exactly as sqdet_topk_nms filters one image: the top-N branch
+ *      when 0 < TOP_N_DETECTION < |U_f|, else the PROB_THRESH branch in union order (more
+ *      candidates than min(1024, max_dets): count -1); same rank order, NMS rule and
+ *      class-grouped output.
+ *   4. The merged records [B, max_dets] and counts [B] go to a buffer of their own
+ *      (sqdet_tile_results_dev): record.anchor is the union index j, so the record came from the
+ *      frame's (j / A)-th tile, anchor j % A.  Counts of rows [n, B) are 0; padding as
+ *      sqdet_topk_nms writes it.
+ * With one tile per frame at (0, 0) the merged records are bitwise the per-tile records.
+ * Asynchronous on `stream`, no host synchronisation; a weight reload or sqdet_set_box_scale
+ * waits for the merge too.  At most 128 tiles per call (SQDET_ERR_UNSUPPORTED above).
+ *   - Launches: those of sqdet_forward_frames over the t tiles with rescale, plus the merge: one
+ *     launch, and one per-tile top-N launch before it when some frame's union is longer than
+ *     TOP_N_DETECTION > 0.
+ *   - Refused before any device work, leaving graphs, tensor 0 and both result buffers
+ *     untouched: SQDET_ERR_INVALID_ARG for a null engine or array, t outside [1, B], n outside
+ *     [1, t], a tile's frame index outside [0, n), a frame with no tile, an empty tile or one
+ *     outside its frame, and every refusal of sqdet_forward_frames (naming "tile k (frame f)");
+ *     SQDET_ERR_STATE before sqdet_finalize.                                                  */
+int sqdet_forward_tiles(sqdet_engine* e, int n, int format, const uint8_t* const* planes,
+                        const int64_t* pitches, const int32_t* heights, const int32_t* widths,
+                        int t, const int32_t* tiles, int order, void* stream);
+/* sqdet_forward_tiles' merged records [B, max_dets] and counts [B]; valid until the next
+ * sqdet_forward_tiles (counts 0 before the first).                                           */
+int sqdet_tile_results_dev(sqdet_engine* e, sqdet_det** dets, int32_t** counts,
+                           int32_t* max_dets);
 /* src/eval.py:83-84 for callers that resize on the host: xy_scales = B pairs (x_scale,
  * y_scale), host memory; every later forward of the paths fed already-resized images
  * (sqdet_forward(_n), sqdet_forward_profiled, sqdet_detect, sqdet_submit) divides
@@ -404,6 +441,14 @@ int sqdet_topk_nms(const float* boxes_dev, const float* probs_dev,
                    const int64_t* cls_dev, int B, int A, int classes, int top_n,
                    float prob_thresh, float nms_thresh, sqdet_det* dets_dev,
                    int32_t* counts_dev, int max_dets, void* stream);
+/* The merge of sqdet_forward_tiles (steps 2-4) on its own: boxes [t,A,4], probs [t,A], cls [t,A]
+ * are t tile rows, tile k of frame tile_frames[k] at offset (tile_xy[2k], tile_xy[2k+1]) (host
+ * arrays) -> dets [n,max_dets], counts [n] for n frames, 1 <= n <= t <= 128.  The per-tile
+ * top-N scratch comes from the stream-ordered allocator on `stream`.  Asynchronous.            */
+int sqdet_merge_tiles(const float* boxes_dev, const float* probs_dev, const int64_t* cls_dev,
+                      int A, int t, const int32_t* tile_frames, const int32_t* tile_xy, int n,
+                      int classes, int top_n, float prob_thresh, float nms_thresh,
+                      sqdet_det* dets_dev, int32_t* counts_dev, int max_dets, void* stream);
 
 /* ---- tiny device-memory helpers so a ctypes caller needs nothing else -------------- */
 int sqdet_malloc(int device, int64_t bytes, void** out_dev);

@@ -89,6 +89,8 @@ SIGNATURES = {
     'sqdet_forward_frames_u8': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     'sqdet_forward_frames_nv12': (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     'sqdet_forward_frames': (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    'sqdet_forward_tiles': (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _vp]),
+    'sqdet_tile_results_dev': (_i, [_vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(C.c_int32)]),
     'sqdet_set_box_scale': (_i, [_vp, _vp]),
     'sqdet_launches_per_forward': (_i, [_vp]),
     'sqdet_engine_stream': (_vp, [_vp]),
@@ -107,6 +109,8 @@ SIGNATURES = {
     'sqdet_preprocess_u8': (_i, [_vp, _i, _i, _fp, _i, _i, _vp, _i, _vp]),
     'sqdet_interpret': (_i, [_fp, _fp, _fp, _fp, _fp] + [_i] * 7 + [_f, _vp]),
     'sqdet_topk_nms': (_i, [_fp, _fp, _fp, _i, _i, _i, _i, _f, _f, _fp, _fp, _i, _vp]),
+    'sqdet_merge_tiles': (_i, [_fp, _fp, _fp, _i, _i, _vp, _vp, _i, _i, _i, _f, _f, _fp, _fp, _i,
+                               _vp]),
     'sqdet_malloc': (_i, [_i, _i64, C.POINTER(_vp)]),
     'sqdet_free': (_i, [_i, _vp]),
     'sqdet_malloc_host': (_i, [_i64, C.POINTER(_vp)]),

@@ -152,4 +152,25 @@ int launch_topk_nms(const float* boxes, const float* probs, const int64_t* cls, 
                     int A, int classes, int top_n, float prob_thresh, float nms_thresh,
                     sqdet_det* dets, int32_t* counts, int max_dets, cudaStream_t stream);
 
+// Tiles of whole frames (sqdet_merge_tiles, sqdet_forward_tiles): tile k is det_* row k of frame
+// tile_frames[k], shifted by (tile_xy[2k], tile_xy[2k + 1]).  At most kMaxMergeTiles tiles per call,
+// whose descriptors travel in the kernels' parameter blocks.
+constexpr int kMaxMergeTiles = 128;
+constexpr int kMergeCandBytes = 32;     // one per-tile top-N candidate in the scratch
+// Bytes of scratch the per-tile top-N stage of t tiles needs (0 when top_n <= 0).
+size_t merge_tiles_scratch_bytes(int t, int A, int top_n);
+// Every refusal of a merge of t tiles of A anchors over n frames, before any device work; `what`
+// names the call.
+int check_merge_tiles(const char* what, int A, int t, const int32_t* tile_frames, int n,
+                      int top_n, int max_dets);
+// filter_prediction of each frame's union of tile rows into dets [rows, max_dets] / counts [rows];
+// rows [n, rows) get count 0.  `scratch` holds merge_tiles_scratch_bytes, or is null to take it
+// from the stream-ordered allocator.  One launch, plus the per-tile top-N launch when some frame's
+// union is longer than top_n > 0.
+int launch_merge_tiles(const char* what, const float* boxes, const float* probs,
+                       const int64_t* cls, int A, int t, const int32_t* tile_frames,
+                       const int32_t* tile_xy, int n, int rows, int classes, int top_n,
+                       float prob_thresh, float nms_thresh, void* scratch, sqdet_det* dets,
+                       int32_t* counts, int max_dets, cudaStream_t stream);
+
 }  // namespace sqdet

@@ -130,6 +130,11 @@ struct sqdet_engine {
   sqdet_det* d_dets = nullptr;
   int32_t* d_counts = nullptr;
   int max_dets = 0;
+  // sqdet_forward_tiles' merged records [B, max_dets] and counts [B] (one allocation), and the
+  // scratch of its per-tile top-N stage (null when TOP_N_DETECTION is off or above 1024)
+  sqdet_det* d_tile_dets = nullptr;
+  int32_t* d_tile_counts = nullptr;
+  void* d_tile_cand = nullptr;
   // CUDA graphs of one forward, keyed by (input, input type, stream, image count, scales); small
   // LRU-less cache
   struct GraphEntry {
@@ -706,6 +711,8 @@ int sqdet_destroy(sqdet_engine* e) {
   cudaFree(e->d_probs);
   cudaFree(e->d_cls);
   cudaFree(e->d_dets);   // also owns d_counts (one blob)
+  cudaFree(e->d_tile_dets);   // also owns d_tile_counts
+  cudaFree(e->d_tile_cand);
   for (auto ev : e->prof_events) cudaEventDestroy(ev);
   for (Slot& s : e->slots) {
     cudaFree(s.input);
@@ -880,7 +887,15 @@ int sqdet_finalize(sqdet_engine* e) {
     SQ_CUDA(cudaMalloc(&blob, rec_bytes + sizeof(int32_t) * (size_t)B));
     e->d_dets = reinterpret_cast<sqdet_det*>(blob);
     e->d_counts = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(blob) + rec_bytes);
+    // the same layout for sqdet_forward_tiles' merged records, all counts 0 until its first call
+    SQ_CUDA(cudaMalloc(&blob, rec_bytes + sizeof(int32_t) * (size_t)B));
+    SQ_CUDA(cudaMemset(blob, 0, rec_bytes + sizeof(int32_t) * (size_t)B));
+    e->d_tile_dets = reinterpret_cast<sqdet_det*>(blob);
+    e->d_tile_counts = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(blob) + rec_bytes);
   }
+  if (c.top_n_detection > 0 && c.top_n_detection <= 1024)
+    SQ_CUDA(cudaMalloc(&e->d_tile_cand,
+                       merge_tiles_scratch_bytes((int)B, (int)A, c.top_n_detection)));
   SQ_CUDA(cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
   SQ_CUDA(cudaEventCreateWithFlags(&e->last_forward, cudaEventDisableTiming));
   e->finalized = true;
@@ -1369,10 +1384,12 @@ struct FramePlanes {
 };
 
 // sqdet_forward_frames and the two calls that are it for one format; `what` names the call in
-// refusals.  Every check is driven by the format's pix_format layout.
+// refusals.  Every check is driven by the format's pix_format layout.  With `tile_frames`
+// (sqdet_forward_tiles) image i is tile i of frame tile_frames[i], and refusals name both.
 static int forward_frames(sqdet_engine* e, const char* what, int n, int format,
                           const FramePlanes& pl, const int32_t* heights, const int32_t* widths,
-                          const int32_t* crops, int order, int rescale, void* stream_v) {
+                          const int32_t* crops, int order, int rescale, void* stream_v,
+                          const int32_t* tile_frames = nullptr) {
   const std::string name = what;
   const PixFormat* pf = pix_format(format);
   if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
@@ -1390,10 +1407,14 @@ static int forward_frames(sqdet_engine* e, const char* what, int n, int format,
   auto row_bytes = [&](int64_t W, int p) {
     return (W >> pf->plane[p].x_shift) * pf->plane[p].bytes_per_px;
   };
+  auto image = [&](int i) {
+    return tile_frames ? "tile " + std::to_string(i) + " (frame " + std::to_string(tile_frames[i]) + ")"
+                       : "frame " + std::to_string(i);
+  };
   std::vector<FrameSource> fr((size_t)n);
   for (int i = 0; i < n; ++i) {
     const int64_t H = heights[i], W = widths[i];
-    const std::string which = name + ": frame " + std::to_string(i);
+    const std::string which = name + ": " + image(i);
     FrameSource& s = fr[(size_t)i];
     for (int p = 0; p < pf->planes; ++p) {
       s.plane[p] = pl.ptr[p][(size_t)i * pl.stride];
@@ -1431,7 +1452,7 @@ static int forward_frames(sqdet_engine* e, const char* what, int n, int format,
       const bool fits = k == 1 || s.pitch[p] <= (INT64_MAX - b) / (k - 1);
       if (!fits || !device_range_ok(s.plane[p], (k - 1) * s.pitch[p] + b, e->device))
         return fail(SQDET_ERR_INVALID_ARG,
-                    name + ": frame " + std::to_string(i) +
+                    name + ": " + image(i) +
                         (pf->planes == 1 ? " is not inside" : ": a plane is not inside") +
                         " one device allocation on the engine's device");
     }
@@ -1474,6 +1495,76 @@ int sqdet_forward_frames_nv12(sqdet_engine* e, int n, const uint8_t* const* luma
   const FramePlanes pl = {{luma_dev, chroma_dev, nullptr}, {luma_pitches, chroma_pitches, nullptr}, 1};
   return forward_frames(e, "sqdet_forward_frames_nv12", n, SQDET_FMT_NV12, pl, heights, widths,
                         crops, order, rescale, stream);
+}
+
+// ---- whole frames as overlapping tiles, merged per frame ---------------------------------------
+int sqdet_forward_tiles(sqdet_engine* e, int n, int format, const uint8_t* const* planes,
+                        const int64_t* pitches, const int32_t* heights, const int32_t* widths,
+                        int t, const int32_t* tiles, int order, void* stream) {
+  const std::string name = "sqdet_forward_tiles";
+  if (!e || !planes || !heights || !widths || !tiles)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (!e->finalized) return fail(SQDET_ERR_STATE, name + " before sqdet_finalize");
+  const sqdet_config& c = e->cfg;
+  if (t < 1 || t > c.batch_size)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": t must be in [1, batch_size]");
+  std::vector<int32_t> frame_of((size_t)t), xy((size_t)t * 2), crops((size_t)t * 4);
+  std::vector<int32_t> hs((size_t)t), ws((size_t)t);
+  for (int k = 0; k < t; ++k) frame_of[(size_t)k] = tiles[5 * k];
+  int rc = check_merge_tiles(name.c_str(), (int)e->num_anchors, t, frame_of.data(), n,
+                             c.top_n_detection, e->max_dets);
+  if (rc) return rc;
+  for (int k = 0; k < t; ++k) {
+    const int f = frame_of[(size_t)k];
+    const int64_t x = tiles[5 * k + 1], y = tiles[5 * k + 2], w = tiles[5 * k + 3],
+                  h = tiles[5 * k + 4];
+    const std::string which = name + ": tile " + std::to_string(k) + " (frame " + std::to_string(f) + ")";
+    if (w <= 0 || h <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
+    if (x < 0 || y < 0 || x + w > widths[f] || y + h > heights[f])
+      return fail(SQDET_ERR_INVALID_ARG, which + " is outside its frame");
+    xy[2 * (size_t)k] = (int32_t)x;
+    xy[2 * (size_t)k + 1] = (int32_t)y;
+    for (int j = 0; j < 4; ++j) crops[4 * (size_t)k + j] = tiles[5 * k + 1 + j];
+    hs[(size_t)k] = heights[f];
+    ws[(size_t)k] = widths[f];
+  }
+  // image k of the forward is tile k: its frame's planes and pitches, cropped to the tile
+  std::vector<const uint8_t*> tp((size_t)t * 3);
+  std::vector<int64_t> tq(pitches ? (size_t)t * 3 : 0);
+  for (int k = 0; k < t; ++k)
+    for (int p = 0; p < 3; ++p) {
+      const size_t src = 3 * (size_t)frame_of[(size_t)k] + p;
+      tp[3 * (size_t)k + p] = planes[src];
+      if (pitches) tq[3 * (size_t)k + p] = pitches[src];
+    }
+  const int64_t* tqp = pitches ? tq.data() : nullptr;
+  const FramePlanes pl = {{tp.data(), tp.data() + 1, tp.data() + 2},
+                          {tqp, tqp ? tqp + 1 : nullptr, tqp ? tqp + 2 : nullptr},
+                          3};
+  rc = forward_frames(e, "sqdet_forward_tiles", t, format, pl, hs.data(), ws.data(), crops.data(),
+                      order, 1, stream, frame_of.data());
+  if (rc) return rc;
+  DeviceGuard guard(e->device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
+  cudaStream_t s = (cudaStream_t)stream;
+  rc = launch_merge_tiles("sqdet_forward_tiles", e->d_boxes, e->d_probs, e->d_cls,
+                          (int)e->num_anchors, t, frame_of.data(), xy.data(), n, c.batch_size,
+                          c.classes, c.top_n_detection, c.prob_thresh, c.nms_thresh,
+                          e->d_tile_cand, e->d_tile_dets, e->d_tile_counts, e->max_dets, s);
+  if (rc) return rc;
+  // a weight reload or sqdet_set_box_scale waits for the merge too
+  SQ_CUDA(cudaEventRecord(e->last_forward, s));
+  return SQDET_OK;
+}
+
+int sqdet_tile_results_dev(sqdet_engine* e, sqdet_det** dets, int32_t** counts,
+                           int32_t* max_dets) {
+  if (!e) return fail(SQDET_ERR_INVALID_ARG, "sqdet_tile_results_dev: null engine");
+  if (!e->finalized) return fail(SQDET_ERR_STATE, "sqdet_tile_results_dev before sqdet_finalize");
+  if (dets) *dets = e->d_tile_dets;
+  if (counts) *counts = e->d_tile_counts;
+  if (max_dets) *max_dets = e->max_dets;
+  return SQDET_OK;
 }
 
 // ---- multi-GPU: ONE all-gather of the filtered records ---------------------------------------------
@@ -1714,6 +1805,17 @@ int sqdet_topk_nms(const float* boxes_dev, const float* probs_dev, const int64_t
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_topk_nms: null pointer");
   return launch_topk_nms(boxes_dev, probs_dev, cls_dev, B, A, classes, top_n, prob_thresh,
                          nms_thresh, dets_dev, counts_dev, max_dets, (cudaStream_t)stream);
+}
+
+int sqdet_merge_tiles(const float* boxes_dev, const float* probs_dev, const int64_t* cls_dev,
+                      int A, int t, const int32_t* tile_frames, const int32_t* tile_xy, int n,
+                      int classes, int top_n, float prob_thresh, float nms_thresh,
+                      sqdet_det* dets_dev, int32_t* counts_dev, int max_dets, void* stream) {
+  if (!boxes_dev || !probs_dev || !cls_dev || !tile_frames || !tile_xy || !dets_dev || !counts_dev)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_merge_tiles: null pointer");
+  return launch_merge_tiles("sqdet_merge_tiles", boxes_dev, probs_dev, cls_dev, A, t, tile_frames,
+                            tile_xy, n, n, classes, top_n, prob_thresh, nms_thresh, nullptr,
+                            dets_dev, counts_dev, max_dets, (cudaStream_t)stream);
 }
 
 // ---- memory helpers ------------------------------------------------------------------------------

@@ -11,8 +11,14 @@
 //                     "suppressed-still-suppresses" NMS per class (the reference's rule,
 //                     NOT greedy NMS), class-grouped output order.  IoU arithmetic is
 //                     bit-exact with numpy float32 (IEEE mul/add/div, no FMA).
+// tile_top_n_kernel / merge_tiles_kernel : filter_prediction of each frame's union of tile rows
+//                     (sqdet_merge_tiles): per-tile top-N candidates, then one CTA per frame
+//                     selects, suppresses and orders them as filter_kernel does one image.
 // Roofline: HBM / latency (B*A*(K*(C+5))/K*4 bytes in, <= B*top_n*28 bytes out).
 #include <math_constants.h>
+#include <algorithm>
+#include <string>
+#include <vector>
 #include "common.cuh"
 
 namespace sqdet {
@@ -382,6 +388,395 @@ filter_kernel(const float* __restrict__ boxes, const float* __restrict__ probs,
   }
 }
 
+// ---- helpers of the tile merge: filter_kernel's stages as functions ---------------------------
+// filter_kernel keeps its own inline copy of each, so that its code stays as it was.
+// Top-N selection of one image's A scores at pr (0 < top_n < A): radix select of the key of the
+// top_n-th largest score, then ordered compaction.  Runs of up to KCACHE keys per thread stay in
+// registers.  put(slot, key, i) receives every selected anchor
+// i, slots [0, n_gt) the scores above that key in anchor order and [n_gt, top_n) the ties at it,
+// lowest anchors first.
+template <int KCACHE, class Put>
+__device__ __forceinline__ void select_top_n(const float* __restrict__ pr, int A, int top_n,
+                                             int* s_hist, int* s_warp, unsigned& s_prefix,
+                                             int& s_remaining, Put put) {
+  const int tid = threadIdx.x;
+  // Each thread owns a contiguous run of `per` anchors, so one block scan orders the whole
+  // image (17 runs of block scans per image were most of this kernel's 80 us).  Keys are
+  // cached in registers when the run is short enough, else re-read from L2.
+  const int per = (A + FT - 1) / FT;
+  const int i_lo = tid * per, i_hi = min(A, i_lo + per);
+  const bool cached = per <= KCACHE;
+  unsigned kc[KCACHE];
+  if (cached) {
+#pragma unroll
+    for (int j = 0; j < KCACHE; ++j)
+      kc[j] = (i_lo + j < i_hi) ? order_key(pr[i_lo + j]) : 0u;
+  }
+  // ---- radix select: key of the top_n-th largest score --------------------------------
+  if (tid == 0) { s_prefix = 0u; s_remaining = top_n; }
+  unsigned mask = 0u;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    if (tid < 256) s_hist[tid] = 0;
+    __syncthreads();
+    const unsigned prefix = s_prefix;
+    if (cached) {
+#pragma unroll
+      for (int j = 0; j < KCACHE; ++j) {
+        const bool in = (i_lo + j < i_hi) && ((kc[j] & mask) == prefix);
+        // warp-aggregated histogram: one atomic per distinct digit per warp
+        const unsigned digit = (kc[j] >> shift) & 255u;
+        const unsigned act = __ballot_sync(0xffffffffu, in);
+        if (in) {
+          const unsigned peers = __match_any_sync(act, digit);
+          if ((threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1))
+            atomicAdd(&s_hist[digit], __popc(peers));
+        }
+      }
+    } else {
+      for (int i = i_lo; i < i_hi; ++i) {
+        const unsigned k = order_key(pr[i]);
+        if ((k & mask) == prefix) atomicAdd(&s_hist[(k >> shift) & 255u], 1);
+      }
+    }
+    __syncthreads();
+    if (tid == 0) {
+      int rem = s_remaining, d = 255;
+      for (; d > 0; --d) {
+        const int h = s_hist[d];
+        if (h >= rem) break;
+        rem -= h;
+      }
+      s_remaining = rem;                       // how many to take among digit d
+      s_prefix = prefix | ((unsigned)d << shift);
+    }
+    mask |= 255u << shift;
+    __syncthreads();
+  }
+  const unsigned T = s_prefix;
+  const int take_eq = s_remaining;             // ties at T: lowest anchor ids first
+  const int n_gt = top_n - take_eq;
+  // ---- ordered compaction: [0,n_gt) scores > T, [n_gt, top_n) scores == T --------------
+  int c_gt = 0, c_eq = 0;
+  if (cached) {
+#pragma unroll
+    for (int j = 0; j < KCACHE; ++j)
+      if (i_lo + j < i_hi) { c_gt += (kc[j] > T); c_eq += (kc[j] == T); }
+  } else {
+    for (int i = i_lo; i < i_hi; ++i) {
+      const unsigned k = order_key(pr[i]);
+      c_gt += (k > T);
+      c_eq += (k == T);
+    }
+  }
+  // exclusive block scan of (c_gt, c_eq) in thread order
+  int o_gt, o_eq;
+  {
+    const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    int v_gt = c_gt, v_eq = c_eq;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int a = __shfl_up_sync(0xffffffffu, v_gt, off);
+      const int b2 = __shfl_up_sync(0xffffffffu, v_eq, off);
+      if (lane >= (unsigned)off) { v_gt += a; v_eq += b2; }
+    }
+    __syncthreads();
+    if (lane == 31) { s_warp[wid] = v_gt; s_hist[wid] = v_eq; }
+    __syncthreads();
+    int base_gt = 0, base_eq = 0;
+    for (int w = 0; w < (int)wid; ++w) { base_gt += s_warp[w]; base_eq += s_hist[w]; }
+    o_gt = base_gt + v_gt - c_gt;
+    o_eq = base_eq + v_eq - c_eq;
+  }
+  auto place = [&](unsigned k, int i) {
+    int slot = -1;
+    if (k > T) slot = o_gt++;
+    else if (k == T) { if (o_eq < take_eq) slot = n_gt + o_eq; ++o_eq; }
+    if (slot >= 0) put(slot, k, i);
+  };
+  if (cached) {
+#pragma unroll
+    for (int j = 0; j < KCACHE; ++j)
+      if (i_lo + j < i_hi && kc[j] >= T) place(kc[j], i_lo + j);
+  } else {
+    for (int i = i_lo; i < i_hi; ++i) place(order_key(pr[i]), i);
+  }
+}
+
+// Bitonic sort of M <= FCAP candidates, descending in (score, -index), pads last.
+__device__ __forceinline__ void sort_candidates(unsigned long long* s_key, float4* s_box,
+                                                int* s_cls, int M) {
+  const int tid = threadIdx.x;
+  int P = 1;
+  while (P < M) P <<= 1;
+  for (int i = M + tid; i < P; i += FT) s_key[i] = 0ull;   // pads sort last
+  __syncthreads();
+  for (int size = 2; size <= P; size <<= 1) {
+    for (int strd = size >> 1; strd > 0; strd >>= 1) {
+      for (int t = tid; t < P; t += FT) {
+        const int partner = t ^ strd;
+        if (partner > t) {
+          const bool desc = ((t & size) == 0);
+          const unsigned long long ka = s_key[t], kb = s_key[partner];
+          if (desc ? (ka < kb) : (ka > kb)) {
+            s_key[t] = kb; s_key[partner] = ka;
+            const float4 tb4 = s_box[t]; s_box[t] = s_box[partner]; s_box[partner] = tb4;
+            const int tc = s_cls[t]; s_cls[t] = s_cls[partner]; s_cls[partner] = tc;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// The M candidates in smem -> per-class NMS, class-grouped records at out, the kept count at
+// *count and deterministic padding up to max_dets.  A record's anchor is the index in the low word
+// of its key; prob_of(anchor) gives its det_probs value.
+template <class ProbOf>
+__device__ __forceinline__ void nms_and_output(const unsigned long long* s_key,
+                                               const float4* s_box, const int* s_cls,
+                                               unsigned char* s_keep, int* s_warp, int M,
+                                               int classes, float nms_thresh,
+                                               sqdet_det* __restrict__ out, int* __restrict__ count,
+                                               int max_dets, ProbOf prob_of) {
+  const int tid = threadIdx.x;
+  // ---- NMS (util.py:56-76): j is dropped iff some higher-ranked same-class i overlaps ----
+  for (int j = tid; j < M; j += FT) {
+    const int cj = s_cls[j];
+    bool keep = (cj >= 0 && cj < classes);
+    if (keep) {
+      const unsigned long long kj = s_key[j];
+      const float4 bj = s_box[j];
+      for (int i = 0; i < M; ++i) {
+        if (i == j || s_cls[i] != cj || !(s_key[i] > kj)) continue;
+        if (iou_ref(bj, s_box[i]) > nms_thresh) { keep = false; break; }
+      }
+    }
+    s_keep[j] = keep ? 1 : 0;
+  }
+  __syncthreads();
+  // ---- class-grouped output order (nn_skeleton.py:726-733) --------------------------------
+  for (int j = tid; j < M; j += FT) {
+    if (!s_keep[j]) continue;
+    const int cj = s_cls[j];
+    int pos = 0;
+    for (int i = 0; i < M; ++i)
+      pos += (s_keep[i] && (s_cls[i] < cj || (s_cls[i] == cj && i < j))) ? 1 : 0;
+    const unsigned long long kj = s_key[j];
+    const int anchor = (int)(~(unsigned)(kj & 0xffffffffull));
+    sqdet_det r;
+    r.anchor = anchor;
+    r.cls = cj;
+    r.prob = prob_of(anchor);
+    const float4 b4 = s_box[j];
+    r.cx = b4.x; r.cy = b4.y; r.w = b4.z; r.h = b4.w;
+    out[pos] = r;
+  }
+  int my = 0;
+  for (int j = tid; j < M; j += FT) my += s_keep[j];
+  // total kept (block reduction through the scan helper's table)
+  int tot = 0;
+  {
+    // reduce `my` over the block
+    for (int o = 16; o > 0; o >>= 1) my += __shfl_xor_sync(0xffffffffu, my, o);
+    __syncthreads();
+    if ((tid & 31) == 0) s_warp[tid >> 5] = my;
+    __syncthreads();
+    for (int i = 0; i < FT / 32; ++i) tot += s_warp[i];
+  }
+  if (tid == 0) *count = tot;
+  for (int i = tot + tid; i < max_dets; i += FT) {   // deterministic padding
+    sqdet_det z; z.anchor = -1; z.cls = -1; z.prob = 0.f; z.cx = z.cy = z.w = z.h = 0.f;
+    out[i] = z;
+  }
+}
+
+// The record rows of a threshold-branch overflow: count -1, every record padding.
+__device__ __forceinline__ void write_overflow(sqdet_det* __restrict__ out, int* __restrict__ count,
+                                               int max_dets) {
+  if (threadIdx.x == 0) *count = -1;
+  for (int i = threadIdx.x; i < max_dets; i += FT) {
+    sqdet_det z; z.anchor = -1; z.cls = -1; z.prob = 0.f; z.cx = z.cy = z.w = z.h = 0.f;
+    out[i] = z;
+  }
+}
+
+// ---- tiles of whole frames: one filter over each frame's union of tile rows -------------------
+// Tile descriptors in frame-major order (a frame's tiles in call order), by value in the
+// parameter block.  Entry e is det_* row `row[e]`, at union position pos[e] among its frame's
+// tiles, shifted by (x[e], y[e]); frame f's entries are [first[f], first[f + 1]).
+struct TileSet {
+  int row[kMaxMergeTiles];
+  int pos[kMaxMergeTiles];
+  float x[kMaxMergeTiles], y[kMaxMergeTiles];
+  int first[kMaxMergeTiles + 1];
+};
+static_assert(sizeof(TileSet) + 128 <= 4096, "tile descriptors exceed 4 KiB of parameters");
+
+// One per-tile top-N candidate: its box in frame pixels, (order_key << 32) | ~union index, class.
+struct TileCand {
+  float4 box;
+  unsigned long long key;
+  int cls;
+  int pad;
+};
+static_assert(sizeof(TileCand) == kMergeCandBytes, "TileCand layout");
+
+// Stage 1, one CTA per tile: the tile's top min(top_n, A) anchors under the filter's rank order,
+// with the tile offset applied, into cand[e * min(top_n, A) ...].  A frame's union top-N is inside
+// the union of its tiles' top-Ns under the same total order, so stage 2 needs only these.
+__global__ void __launch_bounds__(FT)
+tile_top_n_kernel(const float* __restrict__ boxes, const float* __restrict__ probs,
+                  const long long* __restrict__ cls, int A, int top_n,
+                  const __grid_constant__ TileSet ts, TileCand* __restrict__ cand) {
+  __shared__ int s_hist[256];
+  __shared__ int s_warp[FT / 32];
+  __shared__ unsigned s_prefix;
+  __shared__ int s_remaining;
+  const int e = blockIdx.x;
+  const long long row = ts.row[e];
+  const float* pr = probs + row * A;
+  const float4* bx = reinterpret_cast<const float4*>(boxes) + row * A;
+  const long long* cl = cls + row * A;
+  const unsigned base = (unsigned)ts.pos[e] * (unsigned)A;
+  const float ox = ts.x[e], oy = ts.y[e];
+  const int m = min(top_n, A);
+  TileCand* out = cand + (long long)e * m;
+  auto put = [&](int slot, unsigned k, int i) {
+    float4 b = bx[i];
+    b.x = __fadd_rn(b.x, ox);
+    b.y = __fadd_rn(b.y, oy);
+    TileCand c;
+    c.box = b;
+    c.key = ((unsigned long long)k << 32) | (unsigned)(~(base + (unsigned)i));
+    c.cls = (int)cl[i];
+    c.pad = 0;
+    out[slot] = c;
+  };
+  if (top_n < A)   // 20 cached keys per thread: 24, as filter_kernel caches, spills here
+    select_top_n<20>(pr, A, top_n, s_hist, s_warp, s_prefix, s_remaining, put);
+  else
+    for (int i = threadIdx.x; i < A; i += FT) put(i, order_key(pr[i]), i);
+}
+
+// Stage 2, one CTA per output row: filter_prediction of frame f's union U_f (its tiles' rows in
+// call order, union index j = pos * A + anchor, boxes shifted by the tile offset), as filter_kernel
+// filters one image.  The top-N branch selects the union's top_n among the stage-1 candidates by a
+// 64-bit radix select (keys are distinct), the threshold branch scans U_f in union order.  Rows
+// f >= n only get count 0.
+// __maxnreg__ rather than __launch_bounds__(FT): with the bound, ptxas keeps this kernel at 32
+// registers and spills around the division's slow path.  64 registers still fit FT threads.
+__global__ void __maxnreg__(64)
+merge_tiles_kernel(const float* __restrict__ boxes, const float* __restrict__ probs,
+                   const long long* __restrict__ cls, int A, int n,
+                   const __grid_constant__ TileSet ts, const TileCand* __restrict__ cand,
+                   int classes, int top_n, float prob_thresh, float nms_thresh,
+                   sqdet_det* __restrict__ dets, int* __restrict__ counts, int max_dets) {
+  __shared__ unsigned long long s_key[FCAP];   // (order_key << 32) | (~union index)
+  __shared__ float4 s_box[FCAP];
+  __shared__ int s_cls[FCAP];
+  __shared__ unsigned char s_keep[FCAP];
+  __shared__ int s_hist[256];
+  __shared__ int s_warp[FT / 32];
+  __shared__ unsigned long long s_prefix;
+  __shared__ int s_remaining;
+
+  const int f = blockIdx.x;
+  const int tid = threadIdx.x;
+  if (f >= n) {
+    if (tid == 0) counts[f] = 0;
+    return;
+  }
+  const int e0 = ts.first[f];
+  const int tiles = ts.first[f + 1] - e0;
+  const int U = tiles * A;
+  sqdet_det* out = dets + (long long)f * max_dets;
+  // union index j -> its det_* element
+  auto elem = [&](int j) {
+    const int p = j / A;
+    return (long long)ts.row[e0 + p] * A + (j - p * A);
+  };
+
+  const bool topn_branch = (top_n > 0 && top_n < U);
+  int M = 0;
+  if (topn_branch) {
+    const int m = min(top_n, A);
+    const int C = tiles * m;                    // >= top_n candidates
+    const TileCand* c0 = cand + (long long)e0 * m;
+    // ---- radix select of the top_n-th largest key, 8 bits at a time -------------------------
+    if (tid == 0) { s_prefix = 0ull; s_remaining = top_n; }
+    unsigned long long mask = 0ull;
+    for (int shift = 56; shift >= 0; shift -= 8) {
+      if (tid < 256) s_hist[tid] = 0;
+      __syncthreads();
+      const unsigned long long prefix = s_prefix;
+      for (int c = tid; c < C; c += FT) {
+        const unsigned long long k = c0[c].key;
+        if ((k & mask) == prefix) atomicAdd(&s_hist[(unsigned)(k >> shift) & 255u], 1);
+      }
+      __syncthreads();
+      if (tid == 0) {
+        int rem = s_remaining, d = 255;
+        for (; d > 0; --d) {
+          const int h = s_hist[d];
+          if (h >= rem) break;
+          rem -= h;
+        }
+        s_remaining = rem;
+        s_prefix = prefix | ((unsigned long long)d << shift);
+      }
+      mask |= 255ull << shift;
+      __syncthreads();
+    }
+    // keys are distinct, so exactly top_n of them are >= T; any slot order, the sort fixes it
+    const unsigned long long T = s_prefix;
+    __syncthreads();
+    if (tid == 0) s_remaining = 0;
+    __syncthreads();
+    for (int c = tid; c < C; c += FT) {
+      const unsigned long long k = c0[c].key;
+      if (k >= T) {
+        const int slot = atomicAdd(&s_remaining, 1);
+        s_key[slot] = k;
+        s_box[slot] = c0[c].box;
+        s_cls[slot] = c0[c].cls;
+      }
+    }
+    M = top_n;
+    __syncthreads();
+    sort_candidates(s_key, s_box, s_cls, M);
+  } else {
+    // ---- threshold branch: probs > PROB_THRESH in union order --------------------------------
+    int run = 0;
+    for (int base = 0; base < U; base += FT) {
+      const int j = base + tid;
+      const long long x = j < U ? elem(j) : 0;
+      const bool ok = (j < U) && (probs[x] > prob_thresh);
+      int tot;
+      const int o = block_scan_flag(ok, s_warp, tot);
+      const int slot = run + o;
+      if (ok && slot < FCAP && slot < max_dets) {
+        const int p = j / A;
+        float4 b = reinterpret_cast<const float4*>(boxes)[x];
+        b.x = __fadd_rn(b.x, ts.x[e0 + p]);
+        b.y = __fadd_rn(b.y, ts.y[e0 + p]);
+        s_key[slot] = ((unsigned long long)order_key(probs[x]) << 32) | (unsigned)(~(unsigned)j);
+        s_box[slot] = b;
+        s_cls[slot] = (int)cls[x];
+      }
+      run += tot;
+    }
+    if (run > FCAP || run > max_dets) {
+      write_overflow(out, counts + f, max_dets);
+      return;
+    }
+    M = run;
+    __syncthreads();
+  }
+  nms_and_output(s_key, s_box, s_cls, s_keep, s_warp, M, classes, nms_thresh, out, counts + f,
+                 max_dets, [&](int j) { return probs[elem(j)]; });
+}
+
 }  // namespace
 
 int launch_interpret(const float* preds, const float* anchors, float* boxes, float* probs,
@@ -430,6 +825,85 @@ int launch_topk_nms(const float* boxes, const float* probs, const int64_t* cls, 
                                                 A, classes, top_n, prob_thresh, nms_thresh, dets,
                                                 reinterpret_cast<int*>(counts), max_dets);
   SQ_CHECK_LAUNCH("filter_kernel");
+  return SQDET_OK;
+}
+
+size_t merge_tiles_scratch_bytes(int t, int A, int top_n) {
+  return top_n > 0 ? (size_t)t * (size_t)std::min(top_n, A) * kMergeCandBytes : 0;
+}
+
+int check_merge_tiles(const char* what, int A, int t, const int32_t* tile_frames, int n,
+                      int top_n, int max_dets) {
+  const std::string name = what;
+  if (t < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": t must be at least 1");
+  if (t > kMaxMergeTiles)
+    return fail(SQDET_ERR_UNSUPPORTED,
+                name + ": at most " + std::to_string(kMaxMergeTiles) + " tiles per call");
+  if (n < 1 || n > t) return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, t]");
+  if ((long long)t * A > INT32_MAX)
+    return fail(SQDET_ERR_UNSUPPORTED, name + ": more than 2^31 - 1 union entries");
+  std::vector<int> per((size_t)n, 0);
+  for (int k = 0; k < t; ++k) {
+    const int f = tile_frames[k];
+    if (f < 0 || f >= n)
+      return fail(SQDET_ERR_INVALID_ARG, name + ": tile " + std::to_string(k) + ": frame index " +
+                                             std::to_string(f) + " outside [0, n)");
+    ++per[(size_t)f];
+  }
+  int most = 0;
+  for (int f = 0; f < n; ++f) {
+    if (!per[(size_t)f])
+      return fail(SQDET_ERR_INVALID_ARG, name + ": frame " + std::to_string(f) + " has no tile");
+    most = std::max(most, per[(size_t)f]);
+  }
+  if (top_n > 0 && top_n < (long long)most * A && (top_n > FCAP || top_n > max_dets))
+    return fail(SQDET_ERR_UNSUPPORTED,
+                name + ": TOP_N_DETECTION above capacity (max 1024 and <= max_dets)");
+  return SQDET_OK;
+}
+
+int launch_merge_tiles(const char* what, const float* boxes, const float* probs,
+                       const int64_t* cls, int A, int t, const int32_t* tile_frames,
+                       const int32_t* tile_xy, int n, int rows, int classes, int top_n,
+                       float prob_thresh, float nms_thresh, void* scratch, sqdet_det* dets,
+                       int32_t* counts, int max_dets, cudaStream_t stream) {
+  const std::string name = what;
+  if (A <= 0 || classes <= 0 || max_dets <= 0)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": non-positive dimension");
+  if (reinterpret_cast<uintptr_t>(boxes) & 15)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": boxes must be 16-byte aligned");
+  int rc = check_merge_tiles(what, A, t, tile_frames, n, top_n, max_dets);
+  if (rc) return rc;
+  // frame-major descriptors: a frame's tiles keep their call order (counting sort by frame)
+  TileSet ts = {};
+  for (int k = 0; k < t; ++k) ++ts.first[tile_frames[k] + 1];
+  for (int f = 0; f < n; ++f) ts.first[f + 1] += ts.first[f];
+  std::vector<int> fill(ts.first, ts.first + n);
+  int most = 0;
+  for (int k = 0; k < t; ++k) {
+    const int f = tile_frames[k];
+    const int e = fill[(size_t)f]++;
+    ts.row[e] = k;
+    ts.pos[e] = e - ts.first[f];
+    ts.x[e] = (float)tile_xy[2 * k];
+    ts.y[e] = (float)tile_xy[2 * k + 1];
+    most = std::max(most, ts.pos[e] + 1);
+  }
+  const long long* cl = reinterpret_cast<const long long*>(cls);
+  TileCand* cand = static_cast<TileCand*>(scratch);
+  const bool stage1 = top_n > 0 && top_n < (long long)most * A;
+  const bool own = stage1 && !cand;
+  if (own) SQ_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&cand),
+                                   merge_tiles_scratch_bytes(t, A, top_n), stream));
+  if (stage1) {
+    tile_top_n_kernel<<<(unsigned)t, FT, 0, stream>>>(boxes, probs, cl, A, top_n, ts, cand);
+    SQ_CHECK_LAUNCH("tile_top_n_kernel");
+  }
+  merge_tiles_kernel<<<(unsigned)rows, FT, 0, stream>>>(boxes, probs, cl, A, n, ts, cand, classes,
+                                                        top_n, prob_thresh, nms_thresh, dets,
+                                                        reinterpret_cast<int*>(counts), max_dets);
+  SQ_CHECK_LAUNCH("merge_tiles_kernel");
+  if (own) SQ_CUDA(cudaFreeAsync(cand, stream));
   return SQDET_OK;
 }
 

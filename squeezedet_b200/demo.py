@@ -12,6 +12,11 @@ config 1).  Per image: cv2.imread -> float32 -> cv2.resize to
 (mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT) -> minus mc.BGR_MEANS (reference demo.py:187-190) -> ONE GPU
 pass doing detect + filter_prediction (demo.py:193-199) -> keep prob > PLOT_PROB_THRESH -> draw ->
 imwrite out_<name>.
+
+`--mode video --tiles` looks at whole frames instead of the reference's fixed crop: each frame is
+uploaded once and covered by overlapping network-sized tiles at native scale
+(utils.util.tile_grid, 128 px overlap), whose detections are merged per frame on the GPU
+(ModelSkeleton.forward_device_tiles) and drawn on the full frame.
 """
 from __future__ import annotations
 
@@ -34,17 +39,20 @@ def parse_flags(argv=None):
   ap.add_argument('--out_dir', default='./data/out/', help='Directory to dump output image or video.')
   ap.add_argument('--demo_net', default='squeezeDet', help='Neural net architecture.')
   ap.add_argument('--gpu', default='0', help='gpu id.')
+  ap.add_argument('--tiles', action='store_true',
+                  help='Video mode: detect over whole frames as overlapping tiles, merged per '
+                       'frame on the GPU, instead of the reference crop.')
   return ap.parse_args(argv)
 
 
-def build_model(demo_net, gpu, checkpoint):
+def build_model(demo_net, gpu, checkpoint, batch=1):
   from . import config as cfg
   from .nets import SqueezeDet, SqueezeDetPlus
   from .utils import checkpoint as ckpt, synth
   assert demo_net in ('squeezeDet', 'squeezeDet+'), \
       'Selected nueral net architecture not supported: {}'.format(demo_net)
   mc = cfg.kitti_squeezeDet_config() if demo_net == 'squeezeDet' else cfg.kitti_squeezeDetPlus_config()
-  mc.BATCH_SIZE = 1
+  mc.BATCH_SIZE = batch
   mc.LOAD_PRETRAINED_MODEL = False          # parameters come from the checkpoint only
   model = (SqueezeDet if demo_net == 'squeezeDet' else SqueezeDetPlus)(mc, int(gpu))
   if checkpoint == 'synthetic':
@@ -62,12 +70,9 @@ def preprocess(im_bgr_u8, mc):
   return im, (im - mc.BGR_MEANS).astype(np.float32)
 
 
-def detect_and_draw(model, mc, im, frame_u8):
-  """`frame_u8`: the uint8 BGR frame as read; resize + mean subtraction (demo.py:187-190) run on
-  the GPU in front of the forward (sqdet_submit_frames, order = resize then subtract)."""
+def draw_detections(mc, im, final_boxes, final_probs, final_class):
+  """Draws the detections above mc.PLOT_PROB_THRESH on `im`; returns them."""
   from .utils.viz import CLASS_COLORS, draw_box
-  dets, counts = model.detect_frames([frame_u8], order='demo', rescale=False)
-  final_boxes, final_probs, final_class = model.records_to_lists(dets[0], int(counts[0]))
   keep = [i for i in range(len(final_probs)) if final_probs[i] > mc.PLOT_PROB_THRESH]
   final_boxes = [final_boxes[i] for i in keep]
   final_probs = [final_probs[i] for i in keep]
@@ -76,6 +81,13 @@ def detect_and_draw(model, mc, im, frame_u8):
            [mc.CLASS_NAMES[idx] + ': (%.2f)' % prob for idx, prob in zip(final_class, final_probs)],
            cdict=CLASS_COLORS)
   return im, final_boxes, final_probs, final_class
+
+
+def detect_and_draw(model, mc, im, frame_u8):
+  """`frame_u8`: the uint8 BGR frame as read; resize + mean subtraction (demo.py:187-190) run on
+  the GPU in front of the forward (sqdet_submit_frames, order = resize then subtract)."""
+  dets, counts = model.detect_frames([frame_u8], order='demo', rescale=False)
+  return draw_detections(mc, im, *model.records_to_lists(dets[0], int(counts[0])))
 
 
 def image_demo(flags):
@@ -97,6 +109,8 @@ def image_demo(flags):
 
 def video_demo(flags):
   """Detect videos (reference demo.py:44-158: same per-frame crop and per-stage wall clock)."""
+  if flags.tiles:
+    return video_demo_tiles(flags)
   import cv2
   mc, model = build_model(flags.demo_net, flags.gpu, flags.checkpoint)
   cap = cv2.VideoCapture(flags.input_path)
@@ -118,6 +132,41 @@ def video_demo(flags):
     t_draw = time.time()
     print('Total time: {:.4f}, detail: reshape {:.4f} detect+filter {:.4f} draw {:.4f}'.format(
         t_draw - t_start, t_reshape - t_start, t_detect - t_reshape, t_draw - t_detect))
+  cap.release()
+
+
+def video_demo_tiles(flags):
+  """Detect videos over whole frames: the frame goes to the GPU once and runs as a tile_grid of
+  network-sized tiles, merged per frame (forward_device_tiles); boxes are drawn on the full
+  frame."""
+  import cv2
+  import torch
+  from . import config as cfg
+  from .utils.util import tile_grid
+  cap = cv2.VideoCapture(flags.input_path)
+  w, h = int(cap.get(cv2.CAP_PROP_FRAME_WIDTH)), int(cap.get(cv2.CAP_PROP_FRAME_HEIGHT))
+  net_mc = cfg.kitti_squeezeDet_config()
+  grid = [(0,) + tile for tile in tile_grid(w, h, net_mc.IMAGE_WIDTH, net_mc.IMAGE_HEIGHT, 128)]
+  mc, model = build_model(flags.demo_net, flags.gpu, flags.checkpoint, batch=len(grid))
+  os.makedirs(flags.out_dir, exist_ok=True)
+  dev = 'cuda:%d' % int(flags.gpu)
+  count = 0
+  while cap.isOpened():
+    t_start = time.time()
+    count += 1
+    ret, frame = cap.read()
+    if not ret:
+      break
+    frame_dev = torch.from_numpy(frame).to(dev)
+    t_upload = time.time()
+    model.forward_device_tiles([frame_dev], 'bgr', grid, order='demo')
+    dets, counts = model.tile_results(1)
+    t_detect = time.time()
+    im, _, _, _ = draw_detections(mc, frame.copy(), *model.records_to_lists(dets[0], int(counts[0])))
+    cv2.imwrite(os.path.join(flags.out_dir, str(count).zfill(6) + '.jpg'), im)
+    t_draw = time.time()
+    print('Total time: {:.4f}, detail: upload {:.4f} detect+merge {:.4f} draw {:.4f}'.format(
+        t_draw - t_start, t_upload - t_start, t_detect - t_upload, t_draw - t_detect))
   cap.release()
 
 

@@ -602,6 +602,73 @@ class ModelSkeleton:
         (C.c_int32 * (4 * n))(*rects), {'demo': 0, 'eval': 1}[order], int(bool(rescale)),
         stream))
 
+  def forward_device_tiles(self, frames, fmt, tiles, order='demo', stream=None):
+    """Detection over whole frames as overlapping tiles (sqdet_forward_tiles).  frames: as
+    forward_device_frames_fmt takes them, in pixel format `fmt`; tiles: 1..BATCH_SIZE tuples
+    (frame_index, x, y, w, h), each a non-empty rectangle inside its frame (utils.util.tile_grid
+    makes a covering grid; a whole-frame "overview" tile may be added), every frame with at least
+    one tile.  Tile k runs as row k of forward_device_frames_fmt over the tiles as crops with
+    rescale=True, then each frame's detections, shifted into frame pixels, are merged by one
+    top-N and NMS on the GPU.  Asynchronous: read the merged records through
+    tile_results_device() (record 'anchor' = p * A + anchor of the frame's p-th tile) and the
+    per-tile rows through results_device()."""
+    if fmt not in PIXEL_FORMATS:
+      raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
+    if order not in ('demo', 'eval'):
+      raise ValueError("order must be 'demo' or 'eval', got %r" % (order,))
+    frames, tiles = list(frames), [tuple(int(v) for v in tile) for tile in tiles]
+    B, n, t = self.mc.BATCH_SIZE, len(frames), len(tiles)
+    if not 1 <= t <= B:
+      raise ValueError('need 1 to %d tiles, got %d' % (B, t))
+    if not 1 <= n <= t:
+      raise ValueError('need 1 to %d frames (at most one per tile), got %d' % (t, n))
+    planes, pitches, hs, ws = [], [], [], []
+    for i, f in enumerate(frames):
+      h, w, ps = self._frame_planes(i, f, fmt)
+      ps = ps + [(None, 0)] * (3 - len(ps))
+      planes.extend(p for p, _ in ps)
+      pitches.extend(q for _, q in ps)
+      hs.append(h)
+      ws.append(w)
+    flat = []
+    for k, tile in enumerate(tiles):
+      if len(tile) != 5:
+        raise ValueError('tile %d: need (frame_index, x, y, w, h), got %r' % (k, tile))
+      f, x, y, w, h = tile
+      if not 0 <= f < n:
+        raise ValueError('tile %d: frame index %d outside [0, %d)' % (k, f, n))
+      if w < 1 or h < 1 or x < 0 or y < 0 or x + w > ws[f] or y + h > hs[f]:
+        raise ValueError('tile %d: %r is not a non-empty rectangle inside frame %d (%dx%d)'
+                         % (k, tile, f, ws[f], hs[f]))
+      flat.extend(tile)
+    missing = sorted(set(range(n)) - {tile[0] for tile in tiles})
+    if missing:
+      raise ValueError('frame %d has no tile' % missing[0])
+    _lib.check(self._lib.sqdet_forward_tiles(
+        self._engine, n, PIXEL_FORMATS.index(fmt), (C.c_void_p * (3 * n))(*planes),
+        (C.c_int64 * (3 * n))(*pitches), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws), t,
+        (C.c_int32 * (5 * t))(*flat), {'demo': 0, 'eval': 1}[order], stream))
+
+  def tile_results_device(self):
+    """Device pointers of forward_device_tiles' merged results: {'dets': [B, max_dets] records,
+    'counts': [B] int32, 'max_dets': int}.  Valid until the next forward_device_tiles."""
+    d, c, md = C.c_void_p(), C.c_void_p(), C.c_int32()
+    _lib.check(self._lib.sqdet_tile_results_dev(self._engine, C.byref(d), C.byref(c),
+                                                C.byref(md)))
+    return {'dets': d.value, 'counts': c.value, 'max_dets': int(md.value)}
+
+  def tile_results(self, n, stream=None):
+    """Host copies (dets [n, max_dets], counts [n]) of the merged results of the first n frames,
+    after `stream` (the one forward_device_tiles ran on) has finished."""
+    res = self.tile_results_device()
+    dets = np.empty((n, res['max_dets']), _lib.DET_DTYPE)
+    counts = np.empty((n,), np.int32)
+    _lib.check(self._lib.sqdet_stream_sync(self.gpu_id, stream))
+    _lib.check(self._lib.sqdet_memcpy_d2h(dets.ctypes.data, res['dets'], dets.nbytes, None))
+    _lib.check(self._lib.sqdet_memcpy_d2h(counts.ctypes.data, res['counts'], counts.nbytes, None))
+    _lib.check(self._lib.sqdet_stream_sync(self.gpu_id, None))
+    return dets, counts
+
   def _frame_planes(self, i, f, fmt):
     """(h, w, [(pointer, row pitch) per plane]) of frame i in `fmt`, or ValueError naming it."""
     def on_device(name, t):

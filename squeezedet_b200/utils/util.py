@@ -53,6 +53,28 @@ class Timer(object):
     return self.average_time if average else self.duration
 
 
+def tile_grid(frame_w, frame_h, tile_w, tile_h, min_overlap):
+  """Overlapping tiles that cover a frame_w x frame_h frame at native scale, as (x, y, w, h) in
+  row-major order, for ModelSkeleton.forward_device_tiles.  Per axis: the fewest tiles whose
+  neighbours overlap by at least `min_overlap` pixels, evenly spaced, the first at 0 and the last
+  flush with the far edge.  A frame smaller than a tile on an axis gets one tile of the frame's
+  size there (the forward then resizes it up).  1920x1080 with 1242x375 tiles and
+  min_overlap = 128 gives 2 x 4 tiles."""
+  def axis(frame, tile):
+    if frame <= tile:
+      return [(0, frame)]
+    if not 0 <= min_overlap < tile:
+      raise ValueError('min_overlap must be in [0, %d), got %r' % (tile, min_overlap))
+    span, step = frame - tile, tile - min_overlap
+    c = 1 + -(-span // step)
+    return [(i * span // (c - 1), tile) for i in range(c)]
+
+  if min(frame_w, frame_h, tile_w, tile_h) < 1:
+    raise ValueError('frame and tile sizes must be positive')
+  return [(x, y, w, h) for y, h in axis(int(frame_h), int(tile_h))
+          for x, w in axis(int(frame_w), int(tile_w))]
+
+
 def nms(boxes, probs, threshold, device=0):
   """Reference util.nms semantics (util.py:56-76) on the GPU: returns the keep
   mask (list of bool) for centre-format `boxes` ranked by `probs`."""
