@@ -449,6 +449,52 @@ int sqdet_merge_tiles(const float* boxes_dev, const float* probs_dev, const int6
                       int A, int t, const int32_t* tile_frames, const int32_t* tile_xy, int n,
                       int classes, int top_n, float prob_thresh, float nms_thresh,
                       sqdet_det* dets_dev, int32_t* counts_dev, int max_dets, void* stream);
+/* Detections drawn onto frames in device memory, as the reference's demo draws them
+ * (src/demo.py draw_detections + src/train.py _draw_box: cv2.rectangle + cv2.putText), bit for bit.
+ * n <= 128 frames in one SQDET_FMT_* format, laid out exactly as sqdet_forward_frames takes them
+ * (planes[3i + p], pitches[3i + p] or NULL for tight rows, heights[i], widths[i], the same
+ * refusals).  Frame i's canvas is the frame, or with crops its crop (x, y, w, h): drawing on a crop
+ * is cv2 drawing on the numpy view frame[y:y+h, x:x+w], coordinates crop-relative and clipped at
+ * the crop's edges (the records of sqdet_forward_frames(..., rescale=1) over the same crops; tile
+ * records, sqdet_tile_results_dev, are in frame pixels and draw with no crops).
+ * Frame i's records are dets_dev[i * max_dets + k], k < min(counts_dev[i], max_dets) (device
+ * memory); count < 0 (the filter's overflow marker) draws nothing.  Each record, in record order,
+ * on a uint8 BGR canvas:
+ *   - kept only if prob > plot_prob_thresh (float32, as numpy 2 compares np.float32 > float) and
+ *     0 <= cls < classes;
+ *   - (xmin, ymin, xmax, ymax) = int() of bbox_transform([cx, cy, w, h]): float32 cx - w / 2 etc.
+ *     (no contraction), truncated toward zero; skipped if a corner is not finite or |corner| >= 2^31;
+ *   - cv2.rectangle(canvas, (xmin, ymin), (xmax, ymax), colour, 1);
+ *   - cv2.putText(canvas, name + ": (%.2f)" % prob, (xmin, ymax), FONT_HERSHEY_SIMPLEX,
+ *     font_scale, colour, 1) with LINE_8; '%.2f' is correctly rounded (half to even) on the exact
+ *     float32 value, e.g. 0.125 -> "0.12", -0.0 -> "-0.00".  A prob outside [0, 1] draws the
+ *     rectangle and no label (the engine's probs are always inside);
+ *   - later records overwrite earlier ones where they overlap.
+ * Formats: BGR is exactly those bytes.  RGB, BGRA, RGBA, RGB_PLANAR: the B, G, R bytes are those of
+ * drawing on cv2.cvtColor(frame, -> BGR), written back in the frame's channel order; alpha is never
+ * written.  NV12, I420 (no cv2 equivalent): with (Y, U, V) of the colour =
+ * cv2.cvtColor(solid 2x2 BGR patch, COLOR_BGR2YUV_I420), a record sets Y on every pixel of its cv2
+ * mask and (U, V) on every chroma sample whose 2x2 luma block, in frame coordinates, holds a mask
+ * pixel; later records overwrite earlier ones (oracle/draw.py restates the rule).
+ * Runs on the device frame 0's first plane lives on, whichever device is current (`stream`
+ * belongs to it).  Asynchronous on `stream`, no host synchronisation.  Refused before any device
+ * work, leaving every frame untouched: SQDET_ERR_INVALID_ARG for a null array, n outside [1, 128],
+ * an unknown format, every frame refusal of sqdet_forward_frames (planes that are not device
+ * memory of that device inside one allocation included), max_dets < 1, classes outside [1, 64], a
+ * null class name or one that is not printable ASCII of at most 31 characters, a font_scale that
+ * is not finite, positive and at most 1024, and dets_dev (n * max_dets records) or counts_dev
+ * (n int32) not inside one allocation of device memory on that device.                        */
+typedef struct sqdet_draw_style {
+  int32_t            classes;          /* 1..64                                              */
+  const char* const* class_names;      /* printable ASCII, at most 31 chars each              */
+  const uint8_t*     class_bgr;        /* [classes][3]                                        */
+  float              plot_prob_thresh; /* mc.PLOT_PROB_THRESH                                 */
+  float              font_scale;       /* draw_box's 0.3; thickness is always 1               */
+} sqdet_draw_style;
+int sqdet_draw_dets(int n, int format, uint8_t* const* planes, const int64_t* pitches,
+                    const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                    const sqdet_det* dets_dev, const int32_t* counts_dev, int max_dets,
+                    const sqdet_draw_style* style, void* stream);
 
 /* ---- tiny device-memory helpers so a ctypes caller needs nothing else -------------- */
 int sqdet_malloc(int device, int64_t bytes, void** out_dev);

@@ -46,6 +46,13 @@ class Config(C.Structure):
               ('math_mode', C.c_int32), ('max_dets', C.c_int32)]
 
 
+class DrawStyle(C.Structure):
+  """struct sqdet_draw_style."""
+  _fields_ = [('classes', C.c_int32), ('class_names', C.POINTER(C.c_char_p)),
+              ('class_bgr', C.POINTER(C.c_uint8)), ('plot_prob_thresh', C.c_float),
+              ('font_scale', C.c_float)]
+
+
 _vp, _i, _f, _i64 = C.c_void_p, C.c_int, C.c_float, C.c_int64
 _ip = C.POINTER(C.c_int)
 _i64p = C.POINTER(C.c_int64)
@@ -111,6 +118,8 @@ SIGNATURES = {
     'sqdet_topk_nms': (_i, [_fp, _fp, _fp, _i, _i, _i, _i, _f, _f, _fp, _fp, _i, _vp]),
     'sqdet_merge_tiles': (_i, [_fp, _fp, _fp, _i, _i, _vp, _vp, _i, _i, _i, _f, _f, _fp, _fp, _i,
                                _vp]),
+    'sqdet_draw_dets': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, C.POINTER(DrawStyle),
+                             _vp]),
     'sqdet_malloc': (_i, [_i, _i64, C.POINTER(_vp)]),
     'sqdet_free': (_i, [_i, _vp]),
     'sqdet_malloc_host': (_i, [_i64, C.POINTER(_vp)]),

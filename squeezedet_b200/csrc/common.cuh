@@ -141,6 +141,29 @@ struct FrameSource {
 int launch_resize_meansub_frames(int format, const FrameSource* frames, int n, float* dst, int H,
                                  int W, const double* means, int sub_first, float* scales_xy,
                                  cudaStream_t stream);
+// sqdet_draw_dets' style as its kernel takes it, by value: per class the colour (B, G, R and its
+// (Y, U, V) for 4:2:0 frames) and the name, plus the threshold and cvRound(font_scale * 65536).
+constexpr int kDrawMaxClasses = 64;
+constexpr int kDrawMaxName = 31;
+constexpr int kMaxDrawFrames = 128;     // frames per sqdet_draw_dets call
+struct DrawStyle {
+  int64_t hscale;
+  float thresh;
+  int classes;
+  uint8_t bgr[kDrawMaxClasses][3];
+  uint8_t yuv[kDrawMaxClasses][3];
+  uint8_t name_len[kDrawMaxClasses];
+  char name[kDrawMaxClasses][kDrawMaxName];
+};
+// Frames per draw launch: their descriptors and the style stay inside the classic 4 KiB parameter
+// block.
+constexpr int kDrawFramesPerLaunch = 24;
+// Draws frame i's records dets[i * max_dets + k], k < min(counts[i], max_dets), on the crop of
+// frames[i] (FrameSource: planes, pitches, canvas = the h x w crop at (x, y)), one CTA per frame,
+// one launch per kDrawFramesPerLaunch frames.  The frames' checks are the caller's.
+int launch_draw_dets(int format, const FrameSource* frames, int n, const sqdet_det* dets,
+                     const int32_t* counts, int max_dets, const DrawStyle& style,
+                     cudaStream_t stream);
 int launch_add_relu(const float* a, const float* b, float* y, int64_t n, cudaStream_t stream);
 
 int launch_interpret(const float* preds, const float* anchors, float* boxes, float* probs,

@@ -16,6 +16,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -1383,35 +1384,15 @@ struct FramePlanes {
   int stride;
 };
 
-// sqdet_forward_frames and the two calls that are it for one format; `what` names the call in
-// refusals.  Every check is driven by the format's pix_format layout.  With `tile_frames`
-// (sqdet_forward_tiles) image i is tile i of frame tile_frames[i], and refusals name both.
-static int forward_frames(sqdet_engine* e, const char* what, int n, int format,
-                          const FramePlanes& pl, const int32_t* heights, const int32_t* widths,
-                          const int32_t* crops, int order, int rescale, void* stream_v,
-                          const int32_t* tile_frames = nullptr) {
-  const std::string name = what;
-  const PixFormat* pf = pix_format(format);
-  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
-  bool null_array = !e || !heights || !widths;
-  for (int p = 0; p < pf->planes; ++p) null_array = null_array || !pl.ptr[p];
-  if (null_array) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  if (!e->finalized) return fail(SQDET_ERR_STATE, name + " before sqdet_finalize");
-  const sqdet_config& c = e->cfg;
-  if (n < 1 || n > c.batch_size)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, batch_size]");
-  if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": order must be 0 (demo) or 1 (eval)");
-  // plane p of an H x W frame: rows(H, p) rows of row_bytes(W, p) bytes
-  auto rows = [&](int64_t H, int p) { return H >> pf->plane[p].y_shift; };
+// The per-frame checks of sqdet_forward_frames and sqdet_draw_dets against the format's pix_format
+// layout, before any device work: fills fr[i] (planes, pitches, crop) or refuses, naming image(i).
+static int check_frames(const std::string& name, const PixFormat* pf, int n, const FramePlanes& pl,
+                        const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                        const std::function<std::string(int)>& image, std::vector<FrameSource>& fr) {
   auto row_bytes = [&](int64_t W, int p) {
     return (W >> pf->plane[p].x_shift) * pf->plane[p].bytes_per_px;
   };
-  auto image = [&](int i) {
-    return tile_frames ? "tile " + std::to_string(i) + " (frame " + std::to_string(tile_frames[i]) + ")"
-                       : "frame " + std::to_string(i);
-  };
-  std::vector<FrameSource> fr((size_t)n);
+  fr.assign((size_t)n, FrameSource{});
   for (int i = 0; i < n; ++i) {
     const int64_t H = heights[i], W = widths[i];
     const std::string which = name + ": " + image(i);
@@ -1441,25 +1422,66 @@ static int forward_frames(sqdet_engine* e, const char* what, int n, int format,
     s.w = r ? r[2] : (int)W;
     s.h = r ? r[3] : (int)H;
   }
-  DeviceGuard guard(e->device);
-  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
+  return SQDET_OK;
+}
+
+// Every plane of the checked frames fr is device memory of `device` (`where` names it) inside one
+// allocation.
+static int check_frame_memory(const std::string& name, const PixFormat* pf, int n,
+                              const int32_t* heights, const int32_t* widths,
+                              const std::vector<FrameSource>& fr, int device, const char* where,
+                              const std::function<std::string(int)>& image) {
   for (int i = 0; i < n; ++i) {
     const FrameSource& s = fr[(size_t)i];
     const int64_t H = heights[i], W = widths[i];
     for (int p = 0; p < pf->planes; ++p) {
       // the plane's bytes end at (rows - 1) * pitch + row bytes; refused when that overflows int64
-      const int64_t k = rows(H, p), b = row_bytes(W, p);
+      const int64_t k = H >> pf->plane[p].y_shift;
+      const int64_t b = (W >> pf->plane[p].x_shift) * pf->plane[p].bytes_per_px;
       const bool fits = k == 1 || s.pitch[p] <= (INT64_MAX - b) / (k - 1);
-      if (!fits || !device_range_ok(s.plane[p], (k - 1) * s.pitch[p] + b, e->device))
+      if (!fits || !device_range_ok(s.plane[p], (k - 1) * s.pitch[p] + b, device))
         return fail(SQDET_ERR_INVALID_ARG,
                     name + ": " + image(i) +
                         (pf->planes == 1 ? " is not inside" : ": a plane is not inside") +
-                        " one device allocation on the engine's device");
+                        " one device allocation on " + where);
     }
   }
+  return SQDET_OK;
+}
+
+// sqdet_forward_frames and the two calls that are it for one format; `what` names the call in
+// refusals.  Every check is driven by the format's pix_format layout.  With `tile_frames`
+// (sqdet_forward_tiles) image i is tile i of frame tile_frames[i], and refusals name both.
+static int forward_frames(sqdet_engine* e, const char* what, int n, int format,
+                          const FramePlanes& pl, const int32_t* heights, const int32_t* widths,
+                          const int32_t* crops, int order, int rescale, void* stream_v,
+                          const int32_t* tile_frames = nullptr) {
+  const std::string name = what;
+  const PixFormat* pf = pix_format(format);
+  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
+  bool null_array = !e || !heights || !widths;
+  for (int p = 0; p < pf->planes; ++p) null_array = null_array || !pl.ptr[p];
+  if (null_array) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (!e->finalized) return fail(SQDET_ERR_STATE, name + " before sqdet_finalize");
+  const sqdet_config& c = e->cfg;
+  if (n < 1 || n > c.batch_size)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, batch_size]");
+  if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": order must be 0 (demo) or 1 (eval)");
+  auto image = [&](int i) {
+    return tile_frames ? "tile " + std::to_string(i) + " (frame " + std::to_string(tile_frames[i]) + ")"
+                       : "frame " + std::to_string(i);
+  };
+  std::vector<FrameSource> fr;
+  int rc = check_frames(name, pf, n, pl, heights, widths, crops, image, fr);
+  if (rc) return rc;
+  DeviceGuard guard(e->device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
+  rc = check_frame_memory(name, pf, n, heights, widths, fr, e->device, "the engine's device", image);
+  if (rc) return rc;
   cudaStream_t stream = (cudaStream_t)stream_v;
   float* scales = nullptr;
-  int rc = prepare_frames(e, rescale, &scales);
+  rc = prepare_frames(e, rescale, &scales);
   if (rc) return rc;
   Tensor& t0 = e->tensors[0];
   rc = launch_resize_meansub_frames(format, fr.data(), n, t0.dev, c.image_height, c.image_width,
@@ -1816,6 +1838,78 @@ int sqdet_merge_tiles(const float* boxes_dev, const float* probs_dev, const int6
   return launch_merge_tiles("sqdet_merge_tiles", boxes_dev, probs_dev, cls_dev, A, t, tile_frames,
                             tile_xy, n, n, classes, top_n, prob_thresh, nms_thresh, nullptr,
                             dets_dev, counts_dev, max_dets, (cudaStream_t)stream);
+}
+
+// ---- detections drawn on frames in device memory --------------------------------------------------
+int sqdet_draw_dets(int n, int format, uint8_t* const* planes, const int64_t* pitches,
+                    const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                    const sqdet_det* dets_dev, const int32_t* counts_dev, int max_dets,
+                    const sqdet_draw_style* style, void* stream) {
+  const std::string name = "sqdet_draw_dets";
+  const PixFormat* pf = pix_format(format);
+  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
+  if (!planes || !heights || !widths || !dets_dev || !counts_dev || !style || !style->class_names ||
+      !style->class_bgr)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (n < 1 || n > kMaxDrawFrames)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxDrawFrames) + "]");
+  if (max_dets < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": max_dets must be at least 1");
+  if (style->classes < 1 || style->classes > kDrawMaxClasses)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": classes must be in [1, " + std::to_string(kDrawMaxClasses) + "]");
+  const float fs = style->font_scale;
+  if (!(fs > 0.f && fs <= 1024.f))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": font_scale must be finite, positive and at most 1024");
+  DrawStyle st = {};
+  st.hscale = (int64_t)nearbyint((double)fs * 65536.0);   // cvRound: half to even
+  st.thresh = style->plot_prob_thresh;
+  st.classes = style->classes;
+  for (int c = 0; c < st.classes; ++c) {
+    const char* s = style->class_names[c];
+    const size_t len = s ? strnlen(s, kDrawMaxName + 1) : kDrawMaxName + 1;
+    bool printable = len <= (size_t)kDrawMaxName;
+    for (size_t i = 0; printable && i < len; ++i) printable = s[i] >= 32 && s[i] <= 126;
+    if (!printable)
+      return fail(SQDET_ERR_INVALID_ARG, name + ": class name " + std::to_string(c) +
+                                             " is not printable ASCII of at most " +
+                                             std::to_string(kDrawMaxName) + " characters");
+    memcpy(st.name[c], s, len);
+    st.name_len[c] = (uint8_t)len;
+    const int b = style->class_bgr[3 * c], g = style->class_bgr[3 * c + 1], r = style->class_bgr[3 * c + 2];
+    st.bgr[c][0] = (uint8_t)b;
+    st.bgr[c][1] = (uint8_t)g;
+    st.bgr[c][2] = (uint8_t)r;
+    // cv2.cvtColor(solid BGR patch, COLOR_BGR2YUV_I420): OpenCV's BT.601 coefficients, 20 bits
+    const int half = 1 << 19;
+    st.yuv[c][0] = (uint8_t)((269484 * r + 528482 * g + 102760 * b + (16 << 20) + half) >> 20);
+    st.yuv[c][1] = (uint8_t)((-155188 * r - 305135 * g + 460324 * b + (128 << 20) + half) >> 20);
+    st.yuv[c][2] = (uint8_t)((460324 * r - 385875 * g - 74448 * b + (128 << 20) + half) >> 20);
+  }
+  const FramePlanes pl = {{planes, planes + 1, planes + 2},
+                          {pitches, pitches ? pitches + 1 : nullptr, pitches ? pitches + 2 : nullptr},
+                          3};
+  auto image = [](int i) { return "frame " + std::to_string(i); };
+  std::vector<FrameSource> fr;
+  int rc = check_frames(name, pf, n, pl, heights, widths, crops, image, fr);
+  if (rc) return rc;
+  // the device the call runs on is the one frame 0's first plane lives on, whatever is current
+  int device = -1;
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, fr[0].plane[0]) == cudaSuccess && attr.type == cudaMemoryTypeDevice)
+    device = attr.device;
+  else
+    (void)cudaGetLastError();      // an unknown pointer: no stale error for the next launch check
+  rc = check_frame_memory(name, pf, n, heights, widths, fr, device, "frame 0's device", image);
+  if (rc) return rc;
+  if (!device_range_ok(reinterpret_cast<const uint8_t*>(dets_dev),
+                       (int64_t)n * max_dets * (int64_t)sizeof(sqdet_det), device) ||
+      !device_range_ok(reinterpret_cast<const uint8_t*>(counts_dev), (int64_t)n * sizeof(int32_t),
+                       device))
+    return fail(SQDET_ERR_INVALID_ARG,
+                name + ": dets_dev or counts_dev is not inside one device allocation on frame 0's device");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
+  return launch_draw_dets(format, fr.data(), n, dets_dev, counts_dev, max_dets, st,
+                          (cudaStream_t)stream);
 }
 
 // ---- memory helpers ------------------------------------------------------------------------------

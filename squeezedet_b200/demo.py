@@ -16,7 +16,8 @@ imwrite out_<name>.
 `--mode video --tiles` looks at whole frames instead of the reference's fixed crop: each frame is
 uploaded once and covered by overlapping network-sized tiles at native scale
 (utils.util.tile_grid, 128 px overlap), whose detections are merged per frame on the GPU
-(ModelSkeleton.forward_device_tiles) and drawn on the full frame.
+(ModelSkeleton.forward_device_tiles) and drawn on the full frame in device memory
+(ModelSkeleton.draw_detections_device, bitwise draw_detections), which comes back once for imwrite.
 """
 from __future__ import annotations
 
@@ -138,7 +139,7 @@ def video_demo(flags):
 def video_demo_tiles(flags):
   """Detect videos over whole frames: the frame goes to the GPU once and runs as a tile_grid of
   network-sized tiles, merged per frame (forward_device_tiles); boxes are drawn on the full
-  frame."""
+  frame on the device (draw_detections_device), which comes back once for imwrite."""
   import cv2
   import torch
   from . import config as cfg
@@ -160,9 +161,11 @@ def video_demo_tiles(flags):
     frame_dev = torch.from_numpy(frame).to(dev)
     t_upload = time.time()
     model.forward_device_tiles([frame_dev], 'bgr', grid, order='demo')
-    dets, counts = model.tile_results(1)
+    torch.cuda.synchronize(dev)                    # the forward and merge are asynchronous
     t_detect = time.time()
-    im, _, _, _ = draw_detections(mc, frame.copy(), *model.records_to_lists(dets[0], int(counts[0])))
+    # boxes and labels drawn on the device frame, bitwise draw_detections on its host copy
+    model.draw_detections_device([frame_dev], 'bgr', which='tiles')
+    im = frame_dev.cpu().numpy()
     cv2.imwrite(os.path.join(flags.out_dir, str(count).zfill(6) + '.jpg'), im)
     t_draw = time.time()
     print('Total time: {:.4f}, detail: upload {:.4f} detect+merge {:.4f} draw {:.4f}'.format(

@@ -669,6 +669,61 @@ class ModelSkeleton:
     _lib.check(self._lib.sqdet_stream_sync(self.gpu_id, None))
     return dets, counts
 
+  def draw_detections_device(self, frames, fmt, which='tiles', crops=None, cdict=None,
+                             stream=None):
+    """Draws the last forward's detections onto `frames` in place, in device memory, exactly as
+    demo.draw_detections + utils.viz.draw_box draw them with cv2 on a uint8 BGR image
+    (sqdet_draw_dets): boxes and 'CLASS: (PROB)' labels of the records above mc.PLOT_PROB_THRESH,
+    FONT_HERSHEY_SIMPLEX at 0.3, colours looked up as draw_box does (the label's class name in
+    `cdict`, default utils.viz.CLASS_COLORS, else (0, 255, 0)).  frames and crops: as
+    forward_device_frames_fmt takes them, in pixel format `fmt`.  which='tiles' draws frame f's
+    merged records of forward_device_tiles (frame pixels: no crops); which='frames' draws image i's
+    records of forward_device_frames_fmt with rescale=True on its crop.  RGB and RGBA frames get
+    the colours in their own channel order (alpha untouched); NV12 and I420 frames get each
+    colour's (Y, U, V) on the boxes' pixels and the chroma samples around them.  Asynchronous on
+    `stream`: run it on the stream the forward ran on."""
+    from .utils.viz import CLASS_COLORS
+    if fmt not in PIXEL_FORMATS:
+      raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
+    if which not in ('tiles', 'frames'):
+      raise ValueError("which must be 'tiles' or 'frames', got %r" % (which,))
+    frames = list(frames)
+    B, n = self.mc.BATCH_SIZE, len(frames)
+    if not 1 <= n <= B:
+      raise ValueError('need 1 to %d frames, got %d' % (B, n))
+    crops = [None] * n if crops is None else list(crops)
+    if len(crops) != n:
+      raise ValueError('need one crop (or None) per frame, got %d for %d frames' % (len(crops), n))
+    planes, pitches, hs, ws, rects = [], [], [], [], []
+    for i, f in enumerate(frames):
+      h, w, ps = self._frame_planes(i, f, fmt)
+      rect = (0, 0, w, h) if crops[i] is None else tuple(int(v) for v in crops[i])
+      x, y, cw, ch = rect if len(rect) == 4 else (0, 0, 0, 0)
+      if len(rect) != 4 or cw < 1 or ch < 1 or x < 0 or y < 0 or x + cw > w or y + ch > h:
+        raise ValueError('frame %d: crop %r is not a non-empty (x, y, w, h) inside %dx%d'
+                         % (i, crops[i], w, h))
+      ps = ps + [(None, 0)] * (3 - len(ps))
+      planes.extend(p for p, _ in ps)
+      pitches.extend(q for _, q in ps)
+      hs.append(h)
+      ws.append(w)
+      rects.extend(rect)
+    res = self.tile_results_device() if which == 'tiles' else self.results_device()
+    cdict = CLASS_COLORS if cdict is None else cdict
+    names = list(self.mc.CLASS_NAMES)
+    bgr = []
+    for name in names:
+      key = name.split(':')[0]                    # draw_box's label.split(':')[0]
+      bgr.extend(int(v) for v in (cdict[key] if cdict and key in cdict else (0, 255, 0)))
+    enc = [s.encode('ascii') for s in names]
+    style = _lib.DrawStyle(len(names), (C.c_char_p * len(enc))(*enc),
+                           (C.c_uint8 * len(bgr))(*bgr), float(self.mc.PLOT_PROB_THRESH), 0.3)
+    _lib.check(self._lib.sqdet_draw_dets(
+        n, PIXEL_FORMATS.index(fmt), (C.c_void_p * (3 * n))(*planes),
+        (C.c_int64 * (3 * n))(*pitches), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws),
+        (C.c_int32 * (4 * n))(*rects), res['dets'], res['counts'], res['max_dets'],
+        C.byref(style), stream))
+
   def _frame_planes(self, i, f, fmt):
     """(h, w, [(pointer, row pitch) per plane]) of frame i in `fmt`, or ValueError naming it."""
     def on_device(name, t):
