@@ -41,8 +41,7 @@ from .bench_device_frames import HBM_BYTES_PER_S, make_model
 from .bench_device_u8 import gpu_info
 
 FORMS = ('a_torch_convert_then_forward_frames', 'b_forward_frames_fmt')
-# resize_meansub_u8_batch_kernel<...> instance of each format, as the profiler names it
-KERNEL = {'rgb_planar': 'PlanarFrame', 'rgba': 'PackedFrameBatch', 'i420': 'I420Frame'}
+KERNEL = 'resize_meansub_u8_batch_kernel'   # form (b)'s only launch of that name
 IN_BYTES_PER_PX = {'rgb_planar': 3, 'rgba': 4, 'i420': 1.5}
 VIDEO_DEMO_CROP = (239, 500, 1242, 375)     # (x, y, w, h): frame[500:-205, 239:-439]
 
@@ -152,9 +151,9 @@ def measure_workload(args, name, model, fmt, batch, crop, torch):
       form_b()
     stream.synchronize()
   durs = [ev.time_range.elapsed_us() for ev in prof.events()
-          if ev.device_type == DeviceType.CUDA and KERNEL[fmt] in ev.name]
+          if ev.device_type == DeviceType.CUDA and KERNEL in ev.name]
   # the profiler may drop an activity record at the edge of its window; the median needs most
-  assert len(durs) >= (args.steps + 1) // 2, 'found %d %s in %d steps' % (len(durs), KERNEL[fmt],
+  assert len(durs) >= (args.steps + 1) // 2, 'found %d %s in %d steps' % (len(durs), KERNEL,
                                                                         args.steps)
   kernel_us = float(np.median(durs))
   kernel_bytes = n * H * W * 12 + int(n * cw * ch * IN_BYTES_PER_PX[fmt])

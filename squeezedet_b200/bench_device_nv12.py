@@ -38,7 +38,7 @@ from .bench_device_frames import HBM_BYTES_PER_S, make_model
 from .bench_device_u8 import gpu_info
 
 FORMS = ('a_torch_convert_then_forward_frames', 'b_forward_frames_nv12')
-KERNEL = 'Nv12FrameBatch'          # resize_meansub_u8_batch_kernel<Nv12FrameBatch>
+KERNEL = 'resize_meansub_u8_batch_kernel'   # form (b)'s only launch of that name
 FRAME_H, FRAME_W = 1080, 1920
 VIDEO_DEMO_CROP = (239, 500, 1242, 375)     # (x, y, w, h): frame[500:-205, 239:-439]
 

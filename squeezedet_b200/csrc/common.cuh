@@ -66,52 +66,6 @@ int launch_conv_pool_simt(const float* x, const uint8_t* x8, const double* bgr_m
 
 int launch_maxpool(const float* x, float* y, int B, int H, int W, int C, int size,
                    int stride, int padding, cudaStream_t stream);
-// One uint8 BGR frame of the batched resize: h rows of w * 3 bytes, row r at src + r * pitch
-// (any byte alignment), sampled at cv::resize's double scales; box_scale_* are the eval-order
-// box scales (IMAGE_WIDTH / w, IMAGE_HEIGHT / h) as float32.
-struct ResizeFrame {
-  const uint8_t* src;
-  int64_t pitch;
-  double scale_x, scale_y;
-  float box_scale_x, box_scale_y;
-  int h, w;
-};
-// Frames per launch: their descriptors stay inside the classic 4 KiB parameter block.
-constexpr int kResizeFramesPerLaunch = 64;
-// The descriptor of frame (src, pitch, h, w) resized to H x W.
-ResizeFrame resize_frame(const uint8_t* src, int64_t pitch, int h, int w, int H, int W);
-// cv2.resize (float32 INTER_LINEAR) to H x W + `- means` in either order of n frames into the fp32
-// batch [n, H, W, 3] at dst, one launch per kResizeFramesPerLaunch frames.  With scales_xy, each
-// frame's (box_scale_x, box_scale_y) also goes to scales_xy[2i], [2i + 1] on the device.
-int launch_resize_meansub_u8_batch(const ResizeFrame* frames, int n, float* dst, int H, int W,
-                                   const double* means, int sub_first, float* scales_xy,
-                                   cudaStream_t stream);
-// One h x w crop of an NV12 frame for the same resize: luma points at the crop origin's byte,
-// chroma at the U,V pair of the origin's 2x2 chroma block, and (x_odd, y_odd) is the origin's
-// parity in the frame, so the crop reads the frame's own chroma samples at any origin.  Both
-// planes may start at any byte and have any pitch.
-struct Nv12Frame {
-  const uint8_t* luma;
-  const uint8_t* chroma;
-  int64_t luma_pitch, chroma_pitch;
-  double scale_x, scale_y;
-  float box_scale_x, box_scale_y;
-  int h, w;
-  int x_odd, y_odd;
-};
-// Frames per launch: 56 descriptors of 72 bytes and the kernel's other parameters fill the
-// classic 4 KiB parameter block.
-constexpr int kNv12FramesPerLaunch = 56;
-// The descriptor of the h x w crop at (x, y) of the NV12 frame with planes (luma, luma_pitch),
-// (chroma, chroma_pitch), resized to H x W.
-Nv12Frame nv12_frame(const uint8_t* luma, int64_t luma_pitch, const uint8_t* chroma,
-                     int64_t chroma_pitch, int x, int y, int h, int w, int H, int W);
-// cv2.cvtColor(COLOR_YUV2BGR_NV12) of each crop, then launch_resize_meansub_u8_batch's resize and
-// mean subtraction, bit for bit, one launch per kNv12FramesPerLaunch frames.  No BGR frame is
-// written: each tap is fetched from the planes and converted.
-int launch_resize_meansub_nv12_batch(const Nv12Frame* frames, int n, float* dst, int H, int W,
-                                     const double* means, int sub_first, float* scales_xy,
-                                     cudaStream_t stream);
 // The memory layout of a pixel format of sqdet_forward_frames (SQDET_FMT_*).  Plane p of an h x w
 // frame holds h >> y_shift rows of (w >> x_shift) * bytes_per_px bytes, and a crop at (x, y) starts
 // (y >> y_shift) * pitch + (x >> x_shift) * bytes_per_px bytes into it.
@@ -133,11 +87,12 @@ struct FrameSource {
   int64_t pitch[3];
   int x, y, h, w;
 };
-// Each crop converted to BGR as the format's cv2.cvtColor code does, then
-// launch_resize_meansub_u8_batch's resize and mean subtraction, bit for bit, without writing a
-// BGR frame.  SQDET_FMT_BGR and SQDET_FMT_NV12 are exactly launch_resize_meansub_u8_batch and
-// launch_resize_meansub_nv12_batch; the other formats launch per 64 (packed) or 45 (three-plane)
-// frames.  The frames' checks against pix_format are the caller's.
+// The crops of n frames in SQDET_FMT_* `format`, each converted to BGR as the format's
+// cv2.cvtColor code does, then cv2.resize (float32 INTER_LINEAR) to H x W and `- means` in either
+// order, into the fp32 batch [n, H, W, 3] at dst, without writing a BGR frame: one launch per 64
+// (packed), 56 (NV12) or 45 (RGB_PLANAR, I420) frames.  With scales_xy, each frame's box scales
+// (W / w, H / h as float32) also go to scales_xy[2i], [2i + 1] on the device.  Refuses an unknown
+// format and non-positive sizes; the frames' other checks against pix_format are the caller's.
 int launch_resize_meansub_frames(int format, const FrameSource* frames, int n, float* dst, int H,
                                  int W, const double* means, int sub_first, float* scales_xy,
                                  cudaStream_t stream);

@@ -515,9 +515,9 @@ static int enqueue_all(sqdet_engine* e, const void* images, bool u8, int n, cons
   const uint8_t* x8 = u8 ? static_cast<const uint8_t*>(images) : nullptr;
   if (x8 && !e->u8_fused) {
     const Tensor& t = e->tensors[0];
-    const ResizeFrame f = resize_frame(x8, 3 * (int64_t)t.W, n * t.H, t.W, n * t.H, t.W);
-    const int rc = launch_resize_meansub_u8_batch(&f, 1, t.dev, n * t.H, t.W, e->bgr_means, 0,
-                                                  nullptr, stream);
+    const FrameSource f = {{x8}, {3 * (int64_t)t.W}, 0, 0, n * t.H, t.W};
+    const int rc = launch_resize_meansub_frames(SQDET_FMT_BGR, &f, 1, t.dev, n * t.H, t.W,
+                                                e->bgr_means, 0, nullptr, stream);
     if (rc) return rc;
     x8 = nullptr;
   }
@@ -1324,14 +1324,14 @@ int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
   if (rescale && !s->scales) SQ_CUDA(cudaMalloc(&s->scales, sizeof(float) * (size_t)B * 2));
   rc = upload(e, *s, false, n, frames, bytes.data(), off.data());
   if (rc) return rc;
-  std::vector<ResizeFrame> fr((size_t)n);
+  std::vector<FrameSource> fr((size_t)n);
   for (int i = 0; i < n; ++i)
-    fr[(size_t)i] = resize_frame(s->staging + off[(size_t)i], 3 * (int64_t)widths[i], heights[i],
-                                 widths[i], c.image_height, c.image_width);
+    fr[(size_t)i] = {{s->staging + off[(size_t)i]}, {3 * (int64_t)widths[i]}, 0, 0, heights[i],
+                     widths[i]};
   float* scales = rescale ? s->scales : nullptr;
-  rc = launch_resize_meansub_u8_batch(fr.data(), n, s->input, c.image_height, c.image_width,
-                                      e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE, scales,
-                                      e->own_stream);
+  rc = launch_resize_meansub_frames(SQDET_FMT_BGR, fr.data(), n, s->input, c.image_height,
+                                    c.image_width, e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE,
+                                    scales, e->own_stream);
   if (rc) return rc;
   return finish_submit(e, *s, s->input, false, n, scales, dets, counts);
 }
@@ -1803,10 +1803,10 @@ int sqdet_preprocess_u8(const uint8_t* src_dev, int src_h, int src_w, float* dst
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_preprocess_u8: null pointer");
   if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
     return fail(SQDET_ERR_INVALID_ARG, "sqdet_preprocess_u8: order must be 0 (demo) or 1 (eval)");
-  const ResizeFrame f = resize_frame(src_dev, 3 * (int64_t)src_w, src_h, src_w, dst_h, dst_w);
-  return launch_resize_meansub_u8_batch(&f, 1, dst_dev, dst_h, dst_w, bgr_means,
-                                        order == SQDET_PRE_SUB_THEN_RESIZE, nullptr,
-                                        (cudaStream_t)stream);
+  const FrameSource f = {{src_dev}, {3 * (int64_t)src_w}, 0, 0, src_h, src_w};
+  return launch_resize_meansub_frames(SQDET_FMT_BGR, &f, 1, dst_dev, dst_h, dst_w, bgr_means,
+                                      order == SQDET_PRE_SUB_THEN_RESIZE, nullptr,
+                                      (cudaStream_t)stream);
 }
 
 int sqdet_interpret(const float* preds_dev, const float* anchors_f32_dev, float* det_boxes_dev,

@@ -506,35 +506,11 @@ class ModelSkeleton:
     crop view such as frame[500:-205, 239:-439] passes without a copy.  The engine resizes them
     to (mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT) and subtracts mc.BGR_MEANS in `order` ('demo' or
     'eval', as submit_frames) in one launch into image_input, then runs the forward on `stream`
-    (sqdet_forward_frames_u8).  rescale=True divides the boxes by each frame's scales before the
+    (forward_device_frames_fmt with 'bgr': sqdet_forward_frames with SQDET_FMT_BGR, which is
+    sqdet_forward_frames_u8).  rescale=True divides the boxes by each frame's scales before the
     filter, in this call only.  Asynchronous: read the results through results_device()."""
-    frames = list(frames)
-    B, n = self.mc.BATCH_SIZE, len(frames)
-    if not 1 <= n <= B:
-      raise ValueError('need 1 to %d frames, got %d' % (B, n))
-    if order not in ('demo', 'eval'):
-      raise ValueError("order must be 'demo' or 'eval', got %r" % (order,))
-    ptrs, hs, ws, pitches = [], [], [], []
-    for i, f in enumerate(frames):
-      dtype, device, shape = getattr(f, 'dtype', None), getattr(f, 'device', None), tuple(f.shape)
-      if str(dtype) != 'torch.uint8':
-        raise ValueError('frame %d: need a uint8 tensor, got %s' % (i, dtype))
-      if getattr(device, 'type', None) != 'cuda' or device.index != self.gpu_id:
-        raise ValueError('frame %d: need a tensor on cuda:%d, got %s' % (i, self.gpu_id, device))
-      if len(shape) != 3 or shape[2] != 3 or shape[0] < 1 or shape[1] < 1:
-        raise ValueError('frame %d: need shape [h, w, 3], got %r' % (i, shape))
-      stride = tuple(f.stride())
-      pitch = stride[0] if shape[0] > 1 else 3 * shape[1]   # a single row's stride is never used
-      if stride[2] != 1 or stride[1] != 3 or pitch < 3 * shape[1]:
-        raise ValueError('frame %d: need strides (row, 3, 1) with row >= 3 * w, got %r'
-                         % (i, stride))
-      ptrs.append(f.data_ptr())
-      hs.append(shape[0])
-      ws.append(shape[1])
-      pitches.append(pitch)
-    _lib.check(self._lib.sqdet_forward_frames_u8(
-        self._engine, n, (C.c_void_p * n)(*ptrs), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws),
-        (C.c_int64 * n)(*pitches), {'demo': 0, 'eval': 1}[order], int(bool(rescale)), stream))
+    self.forward_device_frames_fmt(frames, 'bgr', None, order=order, rescale=rescale,
+                                   stream=stream)
 
   def forward_device_frames_nv12(self, frames, crops=None, order='demo', rescale=False,
                                  stream=None):
@@ -571,36 +547,16 @@ class ModelSkeleton:
     forward_device_frames, bit for bit, in one launch into image_input, without writing a BGR
     frame (sqdet_forward_frames).  rescale=True scales the boxes back to each crop.
     Asynchronous: read the results through results_device()."""
-    if fmt not in PIXEL_FORMATS:
-      raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
     frames = list(frames)
     B, n = self.mc.BATCH_SIZE, len(frames)
     if not 1 <= n <= B:
       raise ValueError('need 1 to %d frames, got %d' % (B, n))
     if order not in ('demo', 'eval'):
       raise ValueError("order must be 'demo' or 'eval', got %r" % (order,))
-    crops = [None] * n if crops is None else list(crops)
-    if len(crops) != n:
-      raise ValueError('need one crop (or None) per frame, got %d for %d frames' % (len(crops), n))
-    planes, pitches, hs, ws, rects = [], [], [], [], []
-    for i, f in enumerate(frames):
-      h, w, ps = self._frame_planes(i, f, fmt)
-      rect = (0, 0, w, h) if crops[i] is None else tuple(int(v) for v in crops[i])
-      x, y, cw, ch = rect if len(rect) == 4 else (0, 0, 0, 0)
-      if len(rect) != 4 or cw < 1 or ch < 1 or x < 0 or y < 0 or x + cw > w or y + ch > h:
-        raise ValueError('frame %d: crop %r is not a non-empty (x, y, w, h) inside %dx%d'
-                         % (i, crops[i], w, h))
-      ps = ps + [(None, 0)] * (3 - len(ps))
-      planes.extend(p for p, _ in ps)
-      pitches.extend(q for _, q in ps)
-      hs.append(h)
-      ws.append(w)
-      rects.extend(rect)
+    planes, pitches, hs, ws, rects = self._pack_frames(frames, fmt, crops)
     _lib.check(self._lib.sqdet_forward_frames(
-        self._engine, n, PIXEL_FORMATS.index(fmt), (C.c_void_p * (3 * n))(*planes),
-        (C.c_int64 * (3 * n))(*pitches), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws),
-        (C.c_int32 * (4 * n))(*rects), {'demo': 0, 'eval': 1}[order], int(bool(rescale)),
-        stream))
+        self._engine, n, PIXEL_FORMATS.index(fmt), planes, pitches, hs, ws, rects,
+        {'demo': 0, 'eval': 1}[order], int(bool(rescale)), stream))
 
   def forward_device_tiles(self, frames, fmt, tiles, order='demo', stream=None):
     """Detection over whole frames as overlapping tiles (sqdet_forward_tiles).  frames: as
@@ -612,8 +568,6 @@ class ModelSkeleton:
     top-N and NMS on the GPU.  Asynchronous: read the merged records through
     tile_results_device() (record 'anchor' = p * A + anchor of the frame's p-th tile) and the
     per-tile rows through results_device()."""
-    if fmt not in PIXEL_FORMATS:
-      raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
     if order not in ('demo', 'eval'):
       raise ValueError("order must be 'demo' or 'eval', got %r" % (order,))
     frames, tiles = list(frames), [tuple(int(v) for v in tile) for tile in tiles]
@@ -622,14 +576,7 @@ class ModelSkeleton:
       raise ValueError('need 1 to %d tiles, got %d' % (B, t))
     if not 1 <= n <= t:
       raise ValueError('need 1 to %d frames (at most one per tile), got %d' % (t, n))
-    planes, pitches, hs, ws = [], [], [], []
-    for i, f in enumerate(frames):
-      h, w, ps = self._frame_planes(i, f, fmt)
-      ps = ps + [(None, 0)] * (3 - len(ps))
-      planes.extend(p for p, _ in ps)
-      pitches.extend(q for _, q in ps)
-      hs.append(h)
-      ws.append(w)
+    planes, pitches, hs, ws, _ = self._pack_frames(frames, fmt, None)
     flat = []
     for k, tile in enumerate(tiles):
       if len(tile) != 5:
@@ -645,8 +592,7 @@ class ModelSkeleton:
     if missing:
       raise ValueError('frame %d has no tile' % missing[0])
     _lib.check(self._lib.sqdet_forward_tiles(
-        self._engine, n, PIXEL_FORMATS.index(fmt), (C.c_void_p * (3 * n))(*planes),
-        (C.c_int64 * (3 * n))(*pitches), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws), t,
+        self._engine, n, PIXEL_FORMATS.index(fmt), planes, pitches, hs, ws, t,
         (C.c_int32 * (5 * t))(*flat), {'demo': 0, 'eval': 1}[order], stream))
 
   def tile_results_device(self):
@@ -683,14 +629,34 @@ class ModelSkeleton:
     colour's (Y, U, V) on the boxes' pixels and the chroma samples around them.  Asynchronous on
     `stream`: run it on the stream the forward ran on."""
     from .utils.viz import CLASS_COLORS
-    if fmt not in PIXEL_FORMATS:
-      raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
     if which not in ('tiles', 'frames'):
       raise ValueError("which must be 'tiles' or 'frames', got %r" % (which,))
     frames = list(frames)
     B, n = self.mc.BATCH_SIZE, len(frames)
     if not 1 <= n <= B:
       raise ValueError('need 1 to %d frames, got %d' % (B, n))
+    planes, pitches, hs, ws, rects = self._pack_frames(frames, fmt, crops)
+    res = self.tile_results_device() if which == 'tiles' else self.results_device()
+    cdict = CLASS_COLORS if cdict is None else cdict
+    names = list(self.mc.CLASS_NAMES)
+    bgr = []
+    for name in names:
+      key = name.split(':')[0]                    # draw_box's label.split(':')[0]
+      bgr.extend(int(v) for v in (cdict[key] if cdict and key in cdict else (0, 255, 0)))
+    enc = [s.encode('ascii') for s in names]
+    style = _lib.DrawStyle(len(names), (C.c_char_p * len(enc))(*enc),
+                           (C.c_uint8 * len(bgr))(*bgr), float(self.mc.PLOT_PROB_THRESH), 0.3)
+    _lib.check(self._lib.sqdet_draw_dets(
+        n, PIXEL_FORMATS.index(fmt), planes, pitches, hs, ws, rects, res['dets'], res['counts'],
+        res['max_dets'], C.byref(style), stream))
+
+  def _pack_frames(self, frames, fmt, crops):
+    """The C arrays (planes [3n], pitches [3n], heights [n], widths [n], crops [4n]) of the n frames
+    in pixel format `fmt` and their crops (None, or per frame None for the whole frame or
+    (x, y, w, h) inside it), or ValueError naming what does not fit."""
+    if fmt not in PIXEL_FORMATS:
+      raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
+    n = len(frames)
     crops = [None] * n if crops is None else list(crops)
     if len(crops) != n:
       raise ValueError('need one crop (or None) per frame, got %d for %d frames' % (len(crops), n))
@@ -708,21 +674,8 @@ class ModelSkeleton:
       hs.append(h)
       ws.append(w)
       rects.extend(rect)
-    res = self.tile_results_device() if which == 'tiles' else self.results_device()
-    cdict = CLASS_COLORS if cdict is None else cdict
-    names = list(self.mc.CLASS_NAMES)
-    bgr = []
-    for name in names:
-      key = name.split(':')[0]                    # draw_box's label.split(':')[0]
-      bgr.extend(int(v) for v in (cdict[key] if cdict and key in cdict else (0, 255, 0)))
-    enc = [s.encode('ascii') for s in names]
-    style = _lib.DrawStyle(len(names), (C.c_char_p * len(enc))(*enc),
-                           (C.c_uint8 * len(bgr))(*bgr), float(self.mc.PLOT_PROB_THRESH), 0.3)
-    _lib.check(self._lib.sqdet_draw_dets(
-        n, PIXEL_FORMATS.index(fmt), (C.c_void_p * (3 * n))(*planes),
-        (C.c_int64 * (3 * n))(*pitches), (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws),
-        (C.c_int32 * (4 * n))(*rects), res['dets'], res['counts'], res['max_dets'],
-        C.byref(style), stream))
+    return ((C.c_void_p * (3 * n))(*planes), (C.c_int64 * (3 * n))(*pitches),
+            (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws), (C.c_int32 * (4 * n))(*rects))
 
   def _frame_planes(self, i, f, fmt):
     """(h, w, [(pointer, row pitch) per plane]) of frame i in `fmt`, or ValueError naming it."""

@@ -1,6 +1,7 @@
-"""sqdet_forward_frames / ModelSkeleton.forward_device_frames_fmt: RGB, BGRA, RGBA, planar RGB and
-I420 frames already in device memory, converted, cropped, resized and mean-subtracted by one
-batched launch into tensor 0, then the forward.  Every check is bitwise against
+"""sqdet_forward_frames / ModelSkeleton.forward_device_frames_fmt: RGB, BGRA, RGBA, planar RGB, NV12
+and I420 frames already in device memory, converted, cropped, resized and mean-subtracted by one
+batched launch into tensor 0, then the forward; and sqdet_forward_frames_nv12 /
+forward_device_frames_nv12, which are that call for NV12.  Every check is bitwise against
 forward_device_frames on the BGR crops that oracle.pixfmt.to_bgr (pinned to cv2.cvtColor) makes of
 the same bytes, uploaded tight."""
 import ctypes as C
@@ -19,7 +20,7 @@ pytestmark = pytest.mark.gpu
 
 ERR_INVALID_ARG, ERR_STATE = -1, -4
 FMT = {name: code for code, name in enumerate(pixfmt.FORMATS)}    # SQDET_FMT_*
-NEW_FORMATS = ('rgb', 'bgra', 'rgba', 'rgb_planar', 'i420')
+FORMATS = ('rgb', 'bgra', 'rgba', 'rgb_planar', 'nv12', 'i420')    # every one but BGR, the reference
 YUV = ('nv12', 'i420')
 RESULT_ROWS = ('det_boxes', 'det_probs', 'det_class', 'dets')
 # How a frame sits in device memory: the one-tensor form (packed [h, w, C], planar [3, h, w],
@@ -28,7 +29,9 @@ RESULT_ROWS = ('det_boxes', 'det_probs', 'det_class', 'dets')
 # start byte with an odd pitch; each plane in its own allocation at a padded even pitch.
 LAYOUTS = ('tight', 'padded', 'odd', 'separate')
 VIDEO_DEMO_CROP = (239, 500, 1242, 375)      # frame[500:-205, 239:-439] of a 1080p frame
-LAUNCH_LIMIT = 64                             # the most frames of any format one launch holds
+# frames per conversion launch, as sqdet_b200.h documents them
+FRAMES_PER_LAUNCH = {'bgr': 64, 'rgb': 64, 'bgra': 64, 'rgba': 64, 'rgb_planar': 45, 'nv12': 56,
+                     'i420': 45}
 
 
 def small_engine(batch, device):
@@ -142,7 +145,7 @@ T0_ODD_CASES = [(47, 133, None), (31, 77, (3, 2, 40, 21)), (1, 1, None), (5, 3, 
 
 
 @pytest.mark.parametrize('order', ['demo', 'eval'])
-@pytest.mark.parametrize('fmt', NEW_FORMATS)
+@pytest.mark.parametrize('fmt', FORMATS)
 def test_tensor0_bitwise(fmt, order, gpu_device):
   """Every case under every layout: rows [0, n) of tensor 0 are those of forward_device_frames on
   the BGR crops bit for bit, and within 2 float32 ulp of 255 of oracle.preproc on them."""
@@ -174,7 +177,7 @@ RES_CASES = [(50, 140, None), (48, 134, None), (94, 266, (3, 1, 261, 91)), (30, 
 
 @pytest.mark.parametrize('rescale', [False, True], ids=['plain', 'rescale'])
 @pytest.mark.parametrize('order', ['demo', 'eval'])
-@pytest.mark.parametrize('fmt', NEW_FORMATS)
+@pytest.mark.parametrize('fmt', FORMATS)
 def test_results_bitwise(fmt, order, rescale, gpu_device):
   B = len(RES_CASES)
   model = small_engine(B, gpu_device)
@@ -182,7 +185,7 @@ def test_results_bitwise(fmt, order, rescale, gpu_device):
   rng = np.random.default_rng(2)
   frames = [random_planes(fmt, h, w, rng) for h, w, _ in RES_CASES]
   crops = [c for _, _, c in RES_CASES]
-  for n in (1, 7, B):
+  for n in (1, 5, 7, B):
     want_t0, want = bgr_reference(model, fmt, frames[:n], crops[:n], order, rescale)
     got_t0, got = run_fmt(model, fmt, frames[:n], crops[:n], order, rescale, stream=stream)
     assert got_t0.tobytes() == want_t0.tobytes(), (fmt, n, order, rescale)
@@ -249,16 +252,17 @@ def test_bgr_and_nv12_formats_equal_their_calls(gpu_device):
 
 
 # ---- 4. more frames than one launch holds -----------------------------------------------------------
-@pytest.mark.parametrize('fmt', ['rgba', 'rgb_planar', 'i420'])
+@pytest.mark.parametrize('fmt', ['rgba', 'rgb_planar', 'nv12', 'i420'])
 def test_more_frames_than_one_launch(fmt, gpu_device):
-  """68 frames: two launches of 64 packed or of 45 three-plane descriptors."""
-  B = LAUNCH_LIMIT + 4
+  """68 frames, and one more than the format's launch holds: two launches of 64 packed, 56 NV12
+  or 45 three-plane descriptors."""
+  B = max(FRAMES_PER_LAUNCH.values()) + 4
   model = small_engine(B, gpu_device)
   rng = np.random.default_rng(3)
   shapes = [(2 * int(rng.integers(10, 60)), 2 * int(rng.integers(20, 90))) for _ in range(B)]
   frames = [random_planes(fmt, h, w, rng) for h, w in shapes]
   crops = [None if i % 3 == 0 else (i % 2, i % 5, w // 2, h // 2) for i, (h, w) in enumerate(shapes)]
-  for n, order, rescale in ((B, 'eval', True), (46, 'demo', False)):
+  for n, order, rescale in ((B, 'eval', True), (FRAMES_PER_LAUNCH[fmt] + 1, 'demo', False)):
     want_t0, want = bgr_reference(model, fmt, frames[:n], crops[:n], order, rescale)
     got_t0, got = run_fmt(model, fmt, frames[:n], crops[:n], order, rescale)
     assert got_t0.tobytes() == want_t0.tobytes(), (fmt, n)
@@ -266,7 +270,7 @@ def test_more_frames_than_one_launch(fmt, gpu_device):
 
 
 # ---- 5. stream order --------------------------------------------------------------------------------
-@pytest.mark.parametrize('fmt', NEW_FORMATS)
+@pytest.mark.parametrize('fmt', FORMATS)
 def test_frames_written_on_the_callers_stream(fmt, gpu_device):
   """The planes are written by torch kernels queued on the caller's stream behind a long-running
   kernel, and the call follows on that stream with no synchronisation in between."""
@@ -293,7 +297,25 @@ def test_frames_written_on_the_callers_stream(fmt, gpu_device):
   assert_results(fetch_results(model, gpu_device), want, B, fmt)
 
 
-# ---- 6. refusals --------------------------------------------------------------------------------
+# ---- 6. a first layer without a fused pool -------------------------------------------------------
+@pytest.mark.parametrize('fmt', FORMATS)
+def test_first_conv_without_pool(fmt, gpu_device):
+  """A lone first conv reads tensor 0 as an ordinary fp32 input: the same bits there and in the
+  results."""
+  B = 3
+  model = build([('conv', 'conv1', 16, 3, 2, 'SAME')], B, 19, 45, _lib.MATH_FP32_SIMT,
+                gpu_device)[1]
+  rng = np.random.default_rng(7)
+  frames = [random_planes(fmt, h, w, rng) for h, w in ((40, 90), (1080, 1920), (18, 44))]
+  crops = [(3, 1, 45, 19), VIDEO_DEMO_CROP, None]
+  for order, rescale in (('demo', False), ('eval', True)):
+    want_t0, want = bgr_reference(model, fmt, frames, crops, order, rescale)
+    got_t0, got = run_fmt(model, fmt, frames, crops, order, rescale)
+    assert got_t0.tobytes() == want_t0.tobytes(), (fmt, order)
+    assert_results(got, want, B, fmt, order, rescale)
+
+
+# ---- 7. refusals --------------------------------------------------------------------------------
 def test_refusals_before_device_work(gpu_device):
   """Each invalid argument is refused with no device work: tensor 0 and every result buffer stay
   bitwise as they were, and valid calls afterwards are right."""
@@ -380,7 +402,96 @@ def test_refusals_before_device_work(gpu_device):
     b.free()
 
 
-# ---- 7. the facade ---------------------------------------------------------------------------------
+def call_nv12(lib, eng, luma, lpitch, chroma, cpitch, hs, ws, crops, n=None, order=0, rescale=0):
+  """sqdet_forward_frames_nv12 with per-frame lists."""
+  k = len(hs) if hs is not None else 1
+  arr = lambda t, v, m=1: None if v is None else (t * (m * k))(*v)  # noqa: E731
+  return lib.sqdet_forward_frames_nv12(eng, k if n is None else n, arr(C.c_void_p, luma),
+                                       arr(C.c_int64, lpitch), arr(C.c_void_p, chroma),
+                                       arr(C.c_int64, cpitch), arr(C.c_int32, hs),
+                                       arr(C.c_int32, ws), arr(C.c_int32, crops, 4), order,
+                                       rescale, None)
+
+
+def test_nv12_entry_refusals(gpu_device):
+  """sqdet_forward_frames_nv12 refuses each invalid argument with no device work: tensor 0 and
+  every result buffer stay bitwise as they were, and a valid call afterwards is right."""
+  B = 2
+  model = small_engine(B, gpu_device)
+  mc = model.mc
+  lib, eng = model._lib, model._engine
+  rng = np.random.default_rng(5)
+  frames = [random_planes('nv12', 60, 150, rng), random_planes('nv12', 30, 90, rng)]
+  crops = [None, (1, 1, 40, 20)]
+  _, want = bgr_reference(model, 'nv12', frames, crops, 'eval', True)
+  feed = synth.synthetic_images(B, mc.IMAGE_HEIGHT, mc.IMAGE_WIDTH, seed=6)
+  model.detect(feed)
+  before = fetch_results(model, gpu_device)
+  H, W = 60, 150
+  luma = DeviceBuffer.from_numpy(frames[0][0], gpu_device)
+  chroma = DeviceBuffer.from_numpy(frames[0][1], gpu_device)
+  short = DeviceBuffer(2048, gpu_device)        # the chroma plane is 30 * 150 = 4500 bytes
+  pinned = PinnedArray((H, W), np.uint8)
+  pageable = np.zeros((H, W), np.uint8)
+  cases = [
+      ('null engine', dict(eng=None)),
+      ('null luma array', dict(luma=None)),
+      ('null chroma array', dict(chroma=None)),
+      ('null heights', dict(hs=None)),
+      ('null widths', dict(ws=None)),
+      ('n = 0', dict(n=0)),
+      ('n > B', dict(n=B + 1)),
+      ('order', dict(order=2)),
+      ('null luma plane', dict(luma=[None])),
+      ('null chroma plane', dict(chroma=[None])),
+      ('zero height', dict(hs=[0])),
+      ('negative width', dict(ws=[-150])),
+      ('odd height', dict(hs=[59])),
+      ('odd width', dict(ws=[149])),
+      ('short luma pitch', dict(lpitch=[W - 1])),
+      ('short chroma pitch', dict(cpitch=[W - 1])),
+      ('empty crop', dict(crops=[0, 0, 0, 10])),
+      ('crop past the right edge', dict(crops=[1, 0, W, H])),
+      ('crop past the bottom', dict(crops=[0, 1, W, H])),
+      ('negative crop origin', dict(crops=[-1, 0, 10, 10])),
+      ('pinned host luma', dict(luma=[pinned.ptr])),
+      ('pageable host chroma', dict(chroma=[pageable.ctypes.data])),
+      ('short chroma plane', dict(chroma=[short.ptr])),
+      ('luma pitch past the buffer', dict(lpitch=[W + 1])),
+      ('pitch overflow', dict(lpitch=[1 << 62])),
+      ('chroma pitch overflow', dict(cpitch=[1 << 62])),
+  ]
+  for name, kw in cases:
+    args = dict(eng=eng, luma=[luma.ptr], lpitch=None, chroma=[chroma.ptr], cpitch=None, hs=[H],
+                ws=[W], crops=None)
+    args.update({k: v for k, v in kw.items() if k not in ('n', 'order')})
+    assert call_nv12(lib, args['eng'], args['luma'], args['lpitch'], args['chroma'],
+                     args['cpitch'], args['hs'], args['ws'], args['crops'], n=kw.get('n'),
+                     order=kw.get('order', 0)) == ERR_INVALID_ARG, name
+    assert lib.sqdet_last_error(), name
+  torch.cuda.synchronize(gpu_device)
+  assert model.read_tensor('image_input').tobytes() == feed.tobytes()
+  after = fetch_results(model, gpu_device)
+  for key in before:
+    assert after[key].tobytes() == before[key].tobytes(), key
+  # an engine not yet finalized
+  hd = C.c_void_p()
+  conf = _lib.Config(batch_size=1, image_height=8, image_width=8, classes=3, anchors_per_grid=9,
+                     top_n_detection=64, prob_thresh=0.005, nms_thresh=0.4, exp_thresh=1.0,
+                     batch_norm_epsilon=1e-5, math_mode=0, max_dets=0)
+  _lib.check(lib.sqdet_create(C.byref(conf), gpu_device, C.byref(hd)))
+  assert call_nv12(lib, hd, [luma.ptr], None, [chroma.ptr], None, [H], [W], None) == ERR_STATE
+  assert b'finalize' in lib.sqdet_last_error()
+  lib.sqdet_destroy(hd)
+  # still working
+  _, got = run_fmt(model, 'nv12', frames, crops, 'eval', True)
+  assert_results(got, want, B)
+  pinned.free()
+  for b in (luma, chroma, short):
+    b.free()
+
+
+# ---- 8. the facade ---------------------------------------------------------------------------------
 def test_planar_batch_rows(gpu_device):
   """The frames of list(batch) of an [n, 3, h, w] batch go in as they are."""
   B = 3
@@ -405,8 +516,10 @@ def test_facade_checks(gpu_device):
   planar = torch.from_numpy(np.stack(random_planes('rgb_planar', 120, 300, rng))).to(gpu_device)
   y, u, v = (torch.from_numpy(p).to(gpu_device) for p in random_planes('i420', 120, 300, rng))
   i420 = torch.cat([y.reshape(-1), u.reshape(-1), v.reshape(-1)]).reshape(180, 300)
+  nv12 = torch.from_numpy(np.concatenate(random_planes('nv12', 120, 300, rng))).to(gpu_device)
   model.forward_device_frames_fmt([rgba, rgba[1:, 2:]], 'rgba', crops=[(7, 11, 200, 90), None])
   model.forward_device_frames_fmt([i420, (y, u, v)], 'i420')
+  model.forward_device_frames_fmt([nv12, (nv12[:120], nv12[120:])], 'nv12')
   torch.cuda.synchronize(gpu_device)
   bad = {
       'unknown format': dict(frames=[rgba], fmt='yuy2'),
@@ -429,6 +542,14 @@ def test_facade_checks(gpu_device):
       'odd I420 width': dict(frames=[(y[:, :-1], u, v)], fmt='i420'),
       'I420 U of another size': dict(frames=[(y, u[:, :-1], v)], fmt='i420'),
       'I420 tuple of 2': dict(frames=[(y, u)], fmt='i420'),
+      'NV12 float32': dict(frames=[nv12.float()], fmt='nv12'),
+      'NV12 host tensor': dict(frames=[nv12.cpu()], fmt='nv12'),
+      'NV12 rows not a multiple of 3': dict(frames=[nv12[:-1]], fmt='nv12'),
+      'odd NV12 width': dict(frames=[nv12[:, :-1]], fmt='nv12'),
+      'NV12 column stride 2': dict(frames=[nv12[:, ::2]], fmt='nv12'),
+      'three-dimensional NV12': dict(frames=[nv12[:, :, None]], fmt='nv12'),
+      'NV12 chroma of another width': dict(frames=[(nv12[:120], nv12[120:, :298])], fmt='nv12'),
+      'NV12 chroma of another height': dict(frames=[(nv12[:120], nv12[121:])], fmt='nv12'),
       'crop outside': dict(frames=[rgba], fmt='rgba', crops=[(200, 0, 101, 10)]),
       'empty crop': dict(frames=[i420], fmt='i420', crops=[(0, 0, 0, 10)]),
       'crops of another count': dict(frames=[rgba], fmt='rgba', crops=[None, None]),
@@ -442,7 +563,25 @@ def test_facade_checks(gpu_device):
       pytest.fail(name)
 
 
-# ---- 8. a JPEG decoded on the GPU -------------------------------------------------------------------
+def test_nv12_method_is_the_nv12_format(gpu_device):
+  """forward_device_frames_nv12 gives tensor 0 and the results of forward_device_frames_fmt with
+  'nv12', which are those of the BGR crop."""
+  model = small_engine(2, gpu_device)
+  rng = np.random.default_rng(8)
+  planes = random_planes('nv12', 120, 300, rng)
+  x = torch.from_numpy(np.concatenate(planes)).to(gpu_device)
+  crops = [(7, 11, 200, 90)]
+  want_t0, want = bgr_reference(model, 'nv12', [planes], crops, 'demo', False)
+  model.forward_device_frames_nv12([x], crops=crops)
+  torch.cuda.synchronize(gpu_device)
+  assert model.read_tensor('image_input')[:1].tobytes() == want_t0.tobytes()
+  assert_results(fetch_results(model, gpu_device), want, 1)
+  got_t0, got = run_fmt(model, 'nv12', [planes], crops, 'demo', False, layouts=['tight'])
+  assert got_t0.tobytes() == want_t0.tobytes()
+  assert_results(got, want, 1)
+
+
+# ---- 9. a JPEG decoded on the GPU -------------------------------------------------------------------
 def test_decode_jpeg_output_as_rgb_planar(gpu_device):
   """torchvision.io.decode_jpeg(device='cuda')'s [3, h, w] RGB tensor goes straight in; the
   reference is the same decoded bytes through cv2.cvtColor(COLOR_RGB2BGR)."""
