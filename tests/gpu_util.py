@@ -7,6 +7,7 @@ import pytest
 
 import oracle
 from oracle import preproc
+from oracle import tiles as oracle_tiles
 from oracle.torch_port import TorchForward
 from squeezedet_b200 import _lib
 from squeezedet_b200 import config as cfg
@@ -361,6 +362,80 @@ def topk_nms_gpu(boxes, probs, cls, classes, top_n, prob_thresh, nms_thresh, max
                                 C.c_float(prob_thresh), C.c_float(nms_thresh), dd.ptr, dn.ptr,
                                 max_dets, None))
   return dd.to_numpy(_lib.DET_DTYPE, (B, max_dets)), dn.to_numpy(np.int32, (B,))
+
+
+# ---- tiles of whole frames -----------------------------------------------------------------------
+def assert_merge_matches_oracle(dets, counts, rows, tiles, n, mc):
+  """The merged records of frames [0, n) bitwise those of oracle.tiles.merge_tiles on `rows`."""
+  want = oracle_tiles.merge_tiles(rows['det_boxes'], rows['det_probs'], rows['det_class'], tiles,
+                                  n, mc.CLASSES, mc.TOP_N_DETECTION, mc.PROB_THRESH, mc.NMS_THRESH)
+  for f, (fb, fp, fc, src) in enumerate(want):
+    k = int(counts[f])
+    assert k == len(src), (f, k, len(src))
+    d = dets[f]
+    assert d['anchor'][:k].tolist() == src, f
+    assert d['cls'][:k].tolist() == list(fc), f
+    assert np.asarray(fp, np.float32).tobytes() == d['prob'][:k].tobytes(), f
+    got_b = np.stack([d['cx'][:k], d['cy'][:k], d['w'][:k], d['h'][:k]], -1)
+    assert np.asarray(fb, np.float32).reshape(-1, 4).tobytes() == got_b.tobytes(), f
+    assert_padding(d, k, f)
+  return want
+
+
+def assert_padding(records, k, what):
+  """Records [k, max_dets) are padding: anchor and class -1, every float +0.0."""
+  pad = records[k:]
+  assert (pad['anchor'] == -1).all() and (pad['cls'] == -1).all(), what
+  for key in ('prob', 'cx', 'cy', 'w', 'h'):
+    assert not pad[key].copy().view(np.uint32).any(), (what, key)
+
+
+def merge_gpu_rc(boxes, probs, cls, tiles, n, classes, top_n, prob_thresh, nms_thresh, max_dets,
+                 device):
+  """(return code, dets [n, max_dets], counts [n]) of sqdet_merge_tiles on host rows, tile k =
+  tiles[k] = (frame, x, y); the output buffers start as 0x77 bytes and counts 12345."""
+  lib = _lib.load()
+  t, A = probs.shape
+  db = DeviceBuffer.from_numpy(np.ascontiguousarray(boxes, np.float32), device)
+  dp = DeviceBuffer.from_numpy(np.ascontiguousarray(probs, np.float32), device)
+  dc = DeviceBuffer.from_numpy(np.ascontiguousarray(cls, np.int64), device)
+  dd = DeviceBuffer.from_numpy(np.full(n * max_dets * 28, 0x77, np.uint8), device)
+  dn = DeviceBuffer.from_numpy(np.full(n, 12345, np.int32), device)
+  fr = (C.c_int32 * t)(*[tl[0] for tl in tiles])
+  xy = (C.c_int32 * (2 * t))(*[v for tl in tiles for v in tl[1:3]])
+  rc = lib.sqdet_merge_tiles(db.ptr, dp.ptr, dc.ptr, A, t, fr, xy, n, classes, top_n,
+                             C.c_float(prob_thresh), C.c_float(nms_thresh), dd.ptr, dn.ptr,
+                             max_dets, None)
+  return rc, dd.to_numpy(_lib.DET_DTYPE, (n, max_dets)), dn.to_numpy(np.int32, (n,))
+
+
+def merge_gpu(boxes, probs, cls, tiles, n, classes, top_n, prob_thresh, nms_thresh, max_dets,
+              device):
+  rc, dets, counts = merge_gpu_rc(boxes, probs, cls, tiles, n, classes, top_n, prob_thresh,
+                                  nms_thresh, max_dets, device)
+  _lib.check(rc)
+  return dets, counts
+
+
+def adversarial_rows(t, A, classes, rng):
+  """Tile rows with probabilities tied within and across tiles, +-0, NaN, classes out of range,
+  and pairs that meet across tiles at IoU exactly float32(0.4) once the offsets are added."""
+  boxes = np.stack([rng.integers(1, 60, (t, A)) + 0.5, rng.integers(1, 30, (t, A)) + 0.5,
+                    rng.integers(2, 20, (t, A)).astype(float),
+                    rng.integers(2, 20, (t, A)).astype(float)], -1).astype(np.float32)
+  probs = rng.choice(np.float32([0.9, 0.5, 0.25, 0.125, 0.0, -0.0, np.nan, 0.75]),
+                     (t, A)).astype(np.float32)
+  cls = rng.integers(0, classes, (t, A)).astype(np.int64)
+  cls[rng.random((t, A)) < 0.05] = -1
+  cls[rng.random((t, A)) < 0.05] = classes + 2
+  # tile k's anchor 0 at x = 10.5, tile k+1's anchor 1 at 3.5 + 10 (offset): 7-wide boxes 3 apart,
+  # IoU 4/10 exactly; top score so the pair survives the top-N cut
+  for k in range(0, t - 1, 2):
+    boxes[k, 0] = (10.5, 8.5, 7, 7)
+    boxes[k + 1, 1] = (3.5, 8.5, 7, 7)
+    probs[k, 0], probs[k + 1, 1] = 0.9, 0.9
+    cls[k, 0] = cls[k + 1, 1] = 1
+  return boxes, probs, cls
 
 
 def rel_err(got, want):

@@ -9,11 +9,10 @@ import numpy as np
 import pytest
 import torch
 
-from gpu_util import TableNet, body_grid, fetch_results
-from oracle import tiles as oracle_tiles
+from gpu_util import (TableNet, adversarial_rows, assert_merge_matches_oracle, body_grid,
+                      fetch_results, merge_gpu)
 from squeezedet_b200 import _lib, demo
 from squeezedet_b200 import config as cfg
-from squeezedet_b200._lib import DeviceBuffer
 from squeezedet_b200.utils import synth
 from squeezedet_b200.utils.util import tile_grid
 
@@ -60,26 +59,6 @@ def by_tile(model, frames, fmt, tiles, order):
                                   crops=[t[1:] for t in tiles], order=order, rescale=True)
   torch.cuda.synchronize(model.gpu_id)
   return fetch_results(model, model.gpu_id)
-
-
-def assert_merge_matches_oracle(dets, counts, rows, tiles, n, mc):
-  """The merged records of frames [0, n) bitwise those of oracle.tiles.merge_tiles on `rows`."""
-  want = oracle_tiles.merge_tiles(rows['det_boxes'], rows['det_probs'], rows['det_class'], tiles,
-                                  n, mc.CLASSES, mc.TOP_N_DETECTION, mc.PROB_THRESH, mc.NMS_THRESH)
-  for f, (fb, fp, fc, src) in enumerate(want):
-    k = int(counts[f])
-    assert k == len(src), (f, k, len(src))
-    d = dets[f]
-    assert d['anchor'][:k].tolist() == src, f
-    assert d['cls'][:k].tolist() == list(fc), f
-    assert np.asarray(fp, np.float32).tobytes() == d['prob'][:k].tobytes(), f
-    got_b = np.stack([d['cx'][:k], d['cy'][:k], d['w'][:k], d['h'][:k]], -1)
-    assert np.asarray(fb, np.float32).reshape(-1, 4).tobytes() == got_b.tobytes(), f
-    pad = d[k:]
-    assert (pad['anchor'] == -1).all() and (pad['cls'] == -1).all(), f
-    for key in ('prob', 'cx', 'cy', 'w', 'h'):
-      assert not pad[key].any(), (f, key)
-  return want
 
 
 def run_tiles(model, frames, fmt, tiles, order, stream=None):
@@ -215,47 +194,16 @@ def test_non_default_stream(gpu_device):
 
 
 # ---- sqdet_merge_tiles on adversarial rows --------------------------------------------------------
-def merge_gpu(boxes, probs, cls, tiles, n, classes, top_n, prob_thresh, nms_thresh, max_dets,
-              device):
-  lib = _lib.load()
-  t, A = probs.shape
-  db = DeviceBuffer.from_numpy(np.ascontiguousarray(boxes, np.float32), device)
-  dp = DeviceBuffer.from_numpy(np.ascontiguousarray(probs, np.float32), device)
-  dc = DeviceBuffer.from_numpy(np.ascontiguousarray(cls, np.int64), device)
-  dd = DeviceBuffer.from_numpy(np.full(n * max_dets * 28, 0x77, np.uint8), device)
-  dn = DeviceBuffer.from_numpy(np.full(n, 12345, np.int32), device)
-  fr = (C.c_int32 * t)(*[tl[0] for tl in tiles])
-  xy = (C.c_int32 * (2 * t))(*[v for tl in tiles for v in tl[1:3]])
-  _lib.check(lib.sqdet_merge_tiles(db.ptr, dp.ptr, dc.ptr, A, t, fr, xy, n, classes, top_n,
-                                   C.c_float(prob_thresh), C.c_float(nms_thresh), dd.ptr, dn.ptr,
-                                   max_dets, None))
-  return dd.to_numpy(_lib.DET_DTYPE, (n, max_dets)), dn.to_numpy(np.int32, (n,))
-
-
-def adversarial_rows(t, A, classes, rng):
-  """Tile rows with probabilities tied within and across tiles, +-0, NaN, classes out of range,
-  and pairs that meet across tiles at IoU exactly float32(0.4) once the offsets are added."""
-  boxes = np.stack([rng.integers(1, 60, (t, A)) + 0.5, rng.integers(1, 30, (t, A)) + 0.5,
-                    rng.integers(2, 20, (t, A)).astype(float),
-                    rng.integers(2, 20, (t, A)).astype(float)], -1).astype(np.float32)
-  probs = rng.choice(np.float32([0.9, 0.5, 0.25, 0.125, 0.0, -0.0, np.nan, 0.75]),
-                     (t, A)).astype(np.float32)
-  cls = rng.integers(0, classes, (t, A)).astype(np.int64)
-  cls[rng.random((t, A)) < 0.05] = -1
-  cls[rng.random((t, A)) < 0.05] = classes + 2
-  # tile k's anchor 0 at x = 10.5, tile k+1's anchor 1 at 3.5 + 10 (offset): 7-wide boxes 3 apart,
-  # IoU 4/10 exactly; top score so the pair survives the top-N cut
-  for k in range(0, t - 1, 2):
-    boxes[k, 0] = (10.5, 8.5, 7, 7)
-    boxes[k + 1, 1] = (3.5, 8.5, 7, 7)
-    probs[k, 0], probs[k + 1, 1] = 0.9, 0.9
-    cls[k, 0] = cls[k + 1, 1] = 1
-  return boxes, probs, cls
-
-
 @pytest.mark.parametrize('t,n,A,top_n,thresh', [
     (6, 2, 200, 64, 0.005), (20, 1, 200, 64, 0.005), (5, 5, 40, 64, 0.005),
-    (4, 2, 150, 0, 0.2), (7, 3, 30, 0, -1.0), (3, 1, 10, 25, 0.3)])
+    (4, 2, 150, 0, 0.2), (7, 3, 30, 0, -1.0), (3, 1, 10, 25, 0.3),
+    # either side of the per-tile selection's 20 cached keys per thread (A <= 20480) and of the
+    # filter's 24 (A <= 24576), with the top-N cut inside a run of tied scores; top_n 1024 is the
+    # table's capacity, with t * 1024 stage-1 candidates per frame
+    *[(t, t // 4 + 1, A, top_n, 0.005) for A in (20480, 20481, 24576, 24577) for t in (2, 9)
+      for top_n in (64, 1024)],
+    # 128 tiles, the most one call takes: one frame, one tile per frame, frames of 4 and 2 tiles
+    (128, 1, 200, 64, 0.005), (128, 128, 100, 64, 0.005), (128, 40, 150, 64, 0.005)])
 def test_merge_tiles_adversarial(gpu_device, t, n, A, top_n, thresh):
   classes, nms = 3, 0.4
   rng = np.random.default_rng(t * 100 + A)
