@@ -4,13 +4,16 @@
 //                     bbox_transform[_inv], util.py:219-231 safe_exp).  One thread per
 //                     anchor; fp32, operation-for-operation (explicit _rn intrinsics so
 //                     nvcc cannot contract a*b+c into an FMA the reference did not do).
-// filter_kernel     : reference src/nn_skeleton.py:696-734 + src/utils/util.py:32-76.
-//                     One CTA per image: radix-select of the top-N score, ordered
-//                     compaction, bitonic sort (prob desc with -0.0 == +0.0 and NaN
-//                     last, ties by ascending anchor: oracle.postproc._rank_order), all-pairs
-//                     "suppressed-still-suppresses" NMS per class (the reference's rule,
-//                     NOT greedy NMS), class-grouped output order.  IoU arithmetic is
-//                     bit-exact with numpy float32 (IEEE mul/add/div, no FMA).
+// filter stages     : reference src/nn_skeleton.py:696-734 + src/utils/util.py:32-76, one
+//                     set of device functions that all three filter kernels call:
+//                     select_top_n (radix-select of the top-N score, ordered compaction),
+//                     sort_candidates (bitonic sort, prob desc with -0.0 == +0.0 and NaN
+//                     last, ties by ascending anchor: oracle.postproc._rank_order),
+//                     nms_and_output (all-pairs "suppressed-still-suppresses" NMS per class,
+//                     the reference's rule, NOT greedy NMS; class-grouped output order, count
+//                     and padding) and write_overflow.  IoU arithmetic is bit-exact with
+//                     numpy float32 (IEEE mul/add/div, no FMA).
+// filter_kernel     : one CTA per image (sqdet_topk_nms).
 // tile_top_n_kernel / merge_tiles_kernel : filter_prediction of each frame's union of tile rows
 //                     (sqdet_merge_tiles): per-tile top-N candidates, then one CTA per frame
 //                     selects, suppresses and orders them as filter_kernel does one image.
@@ -153,243 +156,7 @@ __device__ __forceinline__ int block_scan_flag(bool flag, int* warp_tot, int& to
   return off + in_warp;
 }
 
-__global__ void __launch_bounds__(FT)
-filter_kernel(const float* __restrict__ boxes, const float* __restrict__ probs,
-              const long long* __restrict__ cls, int A, int classes, int top_n,
-              float prob_thresh, float nms_thresh, sqdet_det* __restrict__ dets,
-              int* __restrict__ counts, int max_dets) {
-  __shared__ unsigned long long s_key[FCAP];   // (order_key << 32) | (~anchor)
-  __shared__ float4 s_box[FCAP];
-  __shared__ int s_cls[FCAP];
-  __shared__ unsigned char s_keep[FCAP];
-  __shared__ int s_hist[256];
-  __shared__ int s_warp[FT / 32];
-  __shared__ unsigned s_prefix;
-  __shared__ int s_remaining;
-
-  const int img = blockIdx.x;
-  const int tid = threadIdx.x;
-  const float* pr = probs + (long long)img * A;
-  const float4* bx = reinterpret_cast<const float4*>(boxes) + (long long)img * A;
-  const long long* cl = cls + (long long)img * A;
-  sqdet_det* out = dets + (long long)img * max_dets;
-
-  const bool topn_branch = (top_n > 0 && top_n < A);     // nn_skeleton.py:711
-  int M = 0;                                              // number of candidates
-
-  if (topn_branch) {
-    // Each thread owns a contiguous run of `per` anchors, so one block scan orders the whole
-    // image (17 runs of block scans per image were most of this kernel's 80 us).  Keys are
-    // cached in registers when the run is short enough, else re-read from L2.
-    constexpr int KCACHE = 24;
-    const int per = (A + FT - 1) / FT;
-    const int i_lo = tid * per, i_hi = min(A, i_lo + per);
-    const bool cached = per <= KCACHE;
-    unsigned kc[KCACHE];
-    if (cached) {
-#pragma unroll
-      for (int j = 0; j < KCACHE; ++j)
-        kc[j] = (i_lo + j < i_hi) ? order_key(pr[i_lo + j]) : 0u;
-    }
-    // ---- radix select: key of the top_n-th largest score --------------------------------
-    if (tid == 0) { s_prefix = 0u; s_remaining = top_n; }
-    unsigned mask = 0u;
-    for (int shift = 24; shift >= 0; shift -= 8) {
-      if (tid < 256) s_hist[tid] = 0;
-      __syncthreads();
-      const unsigned prefix = s_prefix;
-      if (cached) {
-#pragma unroll
-        for (int j = 0; j < KCACHE; ++j) {
-          const bool in = (i_lo + j < i_hi) && ((kc[j] & mask) == prefix);
-          // warp-aggregated histogram: one atomic per distinct digit per warp
-          const unsigned digit = (kc[j] >> shift) & 255u;
-          const unsigned act = __ballot_sync(0xffffffffu, in);
-          if (in) {
-            const unsigned peers = __match_any_sync(act, digit);
-            if ((threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1))
-              atomicAdd(&s_hist[digit], __popc(peers));
-          }
-        }
-      } else {
-        for (int i = i_lo; i < i_hi; ++i) {
-          const unsigned k = order_key(pr[i]);
-          if ((k & mask) == prefix) atomicAdd(&s_hist[(k >> shift) & 255u], 1);
-        }
-      }
-      __syncthreads();
-      if (tid == 0) {
-        int rem = s_remaining, d = 255;
-        for (; d > 0; --d) {
-          const int h = s_hist[d];
-          if (h >= rem) break;
-          rem -= h;
-        }
-        s_remaining = rem;                       // how many to take among digit d
-        s_prefix = prefix | ((unsigned)d << shift);
-      }
-      mask |= 255u << shift;
-      __syncthreads();
-    }
-    const unsigned T = s_prefix;
-    const int take_eq = s_remaining;             // ties at T: lowest anchor ids first
-    const int n_gt = top_n - take_eq;
-    // ---- ordered compaction: [0,n_gt) scores > T, [n_gt, top_n) scores == T --------------
-    int c_gt = 0, c_eq = 0;
-    if (cached) {
-#pragma unroll
-      for (int j = 0; j < KCACHE; ++j)
-        if (i_lo + j < i_hi) { c_gt += (kc[j] > T); c_eq += (kc[j] == T); }
-    } else {
-      for (int i = i_lo; i < i_hi; ++i) {
-        const unsigned k = order_key(pr[i]);
-        c_gt += (k > T);
-        c_eq += (k == T);
-      }
-    }
-    // exclusive block scan of (c_gt, c_eq) in thread order
-    int o_gt, o_eq;
-    {
-      const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-      int v_gt = c_gt, v_eq = c_eq;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int a = __shfl_up_sync(0xffffffffu, v_gt, off);
-        const int b2 = __shfl_up_sync(0xffffffffu, v_eq, off);
-        if (lane >= (unsigned)off) { v_gt += a; v_eq += b2; }
-      }
-      __syncthreads();
-      if (lane == 31) { s_warp[wid] = v_gt; s_hist[wid] = v_eq; }
-      __syncthreads();
-      int base_gt = 0, base_eq = 0;
-      for (int w = 0; w < (int)wid; ++w) { base_gt += s_warp[w]; base_eq += s_hist[w]; }
-      o_gt = base_gt + v_gt - c_gt;
-      o_eq = base_eq + v_eq - c_eq;
-    }
-    auto place = [&](unsigned k, int i) {
-      int slot = -1;
-      if (k > T) slot = o_gt++;
-      else if (k == T) { if (o_eq < take_eq) slot = n_gt + o_eq; ++o_eq; }
-      if (slot >= 0) {
-        s_key[slot] = ((unsigned long long)k << 32) | (unsigned)(~(unsigned)i);
-        s_box[slot] = bx[i];
-        s_cls[slot] = (int)cl[i];
-      }
-    };
-    if (cached) {
-#pragma unroll
-      for (int j = 0; j < KCACHE; ++j)
-        if (i_lo + j < i_hi && kc[j] >= T) place(kc[j], i_lo + j);
-    } else {
-      for (int i = i_lo; i < i_hi; ++i) place(order_key(pr[i]), i);
-    }
-    M = top_n;
-    __syncthreads();
-    // ---- bitonic sort, descending in (score, -anchor) ------------------------------------
-    int P = 1;
-    while (P < M) P <<= 1;
-    for (int i = M + tid; i < P; i += FT) s_key[i] = 0ull;   // pads sort last
-    __syncthreads();
-    for (int size = 2; size <= P; size <<= 1) {
-      for (int strd = size >> 1; strd > 0; strd >>= 1) {
-        for (int t = tid; t < P; t += FT) {
-          const int partner = t ^ strd;
-          if (partner > t) {
-            const bool desc = ((t & size) == 0);
-            const unsigned long long ka = s_key[t], kb = s_key[partner];
-            if (desc ? (ka < kb) : (ka > kb)) {
-              s_key[t] = kb; s_key[partner] = ka;
-              const float4 tb4 = s_box[t]; s_box[t] = s_box[partner]; s_box[partner] = tb4;
-              const int tc = s_cls[t]; s_cls[t] = s_cls[partner]; s_cls[partner] = tc;
-            }
-          }
-        }
-        __syncthreads();
-      }
-    }
-  } else {
-    // ---- threshold branch (nn_skeleton.py:716-720): probs > PROB_THRESH, original order ---
-    int run = 0;
-    bool overflow = false;
-    for (int base = 0; base < A; base += FT) {
-      const int i = base + tid;
-      const bool ok = (i < A) && (pr[i] > prob_thresh);
-      int tot;
-      const int o = block_scan_flag(ok, s_warp, tot);
-      const int slot = run + o;
-      if (ok && slot < FCAP && slot < max_dets) {
-        s_key[slot] = ((unsigned long long)order_key(pr[i]) << 32) | (unsigned)(~(unsigned)i);
-        s_box[slot] = bx[i];
-        s_cls[slot] = (int)cl[i];
-      }
-      run += tot;
-    }
-    if (run > FCAP || run > max_dets) overflow = true;
-    if (overflow) {
-      if (tid == 0) counts[img] = -1;
-      for (int i = tid; i < max_dets; i += FT) {
-        sqdet_det z; z.anchor = -1; z.cls = -1; z.prob = 0.f; z.cx = z.cy = z.w = z.h = 0.f;
-        out[i] = z;
-      }
-      return;
-    }
-    M = run;
-    __syncthreads();
-  }
-
-  // ---- NMS (util.py:56-76): j is dropped iff some higher-ranked same-class i overlaps ----
-  for (int j = tid; j < M; j += FT) {
-    const int cj = s_cls[j];
-    bool keep = (cj >= 0 && cj < classes);
-    if (keep) {
-      const unsigned long long kj = s_key[j];
-      const float4 bj = s_box[j];
-      for (int i = 0; i < M; ++i) {
-        if (i == j || s_cls[i] != cj || !(s_key[i] > kj)) continue;
-        if (iou_ref(bj, s_box[i]) > nms_thresh) { keep = false; break; }
-      }
-    }
-    s_keep[j] = keep ? 1 : 0;
-  }
-  __syncthreads();
-  // ---- class-grouped output order (nn_skeleton.py:726-733) --------------------------------
-  for (int j = tid; j < M; j += FT) {
-    if (!s_keep[j]) continue;
-    const int cj = s_cls[j];
-    int pos = 0;
-    for (int i = 0; i < M; ++i)
-      pos += (s_keep[i] && (s_cls[i] < cj || (s_cls[i] == cj && i < j))) ? 1 : 0;
-    const unsigned long long kj = s_key[j];
-    const int anchor = (int)(~(unsigned)(kj & 0xffffffffull));
-    sqdet_det r;
-    r.anchor = anchor;
-    r.cls = cj;
-    r.prob = pr[anchor];
-    const float4 b4 = s_box[j];
-    r.cx = b4.x; r.cy = b4.y; r.w = b4.z; r.h = b4.w;
-    out[pos] = r;
-  }
-  int my = 0;
-  for (int j = tid; j < M; j += FT) my += s_keep[j];
-  // total kept (block reduction through the scan helper's table)
-  int tot = 0;
-  {
-    // reduce `my` over the block
-    for (int o = 16; o > 0; o >>= 1) my += __shfl_xor_sync(0xffffffffu, my, o);
-    __syncthreads();
-    if ((tid & 31) == 0) s_warp[tid >> 5] = my;
-    __syncthreads();
-    for (int i = 0; i < FT / 32; ++i) tot += s_warp[i];
-  }
-  if (tid == 0) counts[img] = tot;
-  for (int i = tot + tid; i < max_dets; i += FT) {   // deterministic padding
-    sqdet_det z; z.anchor = -1; z.cls = -1; z.prob = 0.f; z.cx = z.cy = z.w = z.h = 0.f;
-    out[i] = z;
-  }
-}
-
-// ---- helpers of the tile merge: filter_kernel's stages as functions ---------------------------
-// filter_kernel keeps its own inline copy of each, so that its code stays as it was.
+// ---- the filter's stages, shared by filter_kernel and the tile merge ---------------------------
 // Top-N selection of one image's A scores at pr (0 < top_n < A): radix select of the key of the
 // top_n-th largest score, then ordered compaction.  Runs of up to KCACHE keys per thread stay in
 // registers.  put(slot, key, i) receives every selected anchor
@@ -401,7 +168,7 @@ __device__ __forceinline__ void select_top_n(const float* __restrict__ pr, int A
                                              int& s_remaining, Put put) {
   const int tid = threadIdx.x;
   // Each thread owns a contiguous run of `per` anchors, so one block scan orders the whole
-  // image (17 runs of block scans per image were most of this kernel's 80 us).  Keys are
+  // image (17 runs of block scans per image were most of filter_kernel's 80 us).  Keys are
   // cached in registers when the run is short enough, else re-read from L2.
   const int per = (A + FT - 1) / FT;
   const int i_lo = tid * per, i_hi = min(A, i_lo + per);
@@ -529,9 +296,18 @@ __device__ __forceinline__ void sort_candidates(unsigned long long* s_key, float
   }
 }
 
+// Deterministic padding: records [from, max_dets) get anchor and class -1, every float +0.0.
+__device__ __forceinline__ void pad_records(sqdet_det* __restrict__ out, int from, int max_dets) {
+  // a signed sum: from + threadIdx.x in unsigned costs merge_tiles_kernel a register
+  for (int i = from + (int)threadIdx.x; i < max_dets; i += FT) {
+    sqdet_det z; z.anchor = -1; z.cls = -1; z.prob = 0.f; z.cx = z.cy = z.w = z.h = 0.f;
+    out[i] = z;
+  }
+}
+
 // The M candidates in smem -> per-class NMS, class-grouped records at out, the kept count at
-// *count and deterministic padding up to max_dets.  A record's anchor is the index in the low word
-// of its key; prob_of(anchor) gives its det_probs value.
+// *count and padding up to max_dets.  A record's anchor is the index in the low word of its key;
+// prob_of(anchor) gives its det_probs value.
 template <class ProbOf>
 __device__ __forceinline__ void nms_and_output(const unsigned long long* s_key,
                                                const float4* s_box, const int* s_cls,
@@ -585,20 +361,73 @@ __device__ __forceinline__ void nms_and_output(const unsigned long long* s_key,
     for (int i = 0; i < FT / 32; ++i) tot += s_warp[i];
   }
   if (tid == 0) *count = tot;
-  for (int i = tot + tid; i < max_dets; i += FT) {   // deterministic padding
-    sqdet_det z; z.anchor = -1; z.cls = -1; z.prob = 0.f; z.cx = z.cy = z.w = z.h = 0.f;
-    out[i] = z;
-  }
+  pad_records(out, tot, max_dets);
 }
 
 // The record rows of a threshold-branch overflow: count -1, every record padding.
 __device__ __forceinline__ void write_overflow(sqdet_det* __restrict__ out, int* __restrict__ count,
                                                int max_dets) {
   if (threadIdx.x == 0) *count = -1;
-  for (int i = threadIdx.x; i < max_dets; i += FT) {
-    sqdet_det z; z.anchor = -1; z.cls = -1; z.prob = 0.f; z.cx = z.cy = z.w = z.h = 0.f;
-    out[i] = z;
+  pad_records(out, 0, max_dets);
+}
+
+__global__ void __launch_bounds__(FT)
+filter_kernel(const float* __restrict__ boxes, const float* __restrict__ probs,
+              const long long* __restrict__ cls, int A, int classes, int top_n,
+              float prob_thresh, float nms_thresh, sqdet_det* __restrict__ dets,
+              int* __restrict__ counts, int max_dets) {
+  __shared__ unsigned long long s_key[FCAP];   // (order_key << 32) | (~anchor)
+  __shared__ float4 s_box[FCAP];
+  __shared__ int s_cls[FCAP];
+  __shared__ unsigned char s_keep[FCAP];
+  __shared__ int s_hist[256];
+  __shared__ int s_warp[FT / 32];
+  __shared__ unsigned s_prefix;
+  __shared__ int s_remaining;
+
+  const int img = blockIdx.x;
+  const int tid = threadIdx.x;
+  const float* pr = probs + (long long)img * A;
+  const float4* bx = reinterpret_cast<const float4*>(boxes) + (long long)img * A;
+  const long long* cl = cls + (long long)img * A;
+  sqdet_det* out = dets + (long long)img * max_dets;
+  auto put = [&](int slot, unsigned k, int i) {
+    s_key[slot] = ((unsigned long long)k << 32) | (unsigned)(~(unsigned)i);
+    s_box[slot] = bx[i];
+    s_cls[slot] = (int)cl[i];
+  };
+
+  const bool topn_branch = (top_n > 0 && top_n < A);     // nn_skeleton.py:711
+  int M = 0;                                              // number of candidates
+
+  if (topn_branch) {
+    // keys cached per thread: ceil(A / FT) <= KCACHE (A <= 24 576) runs from registers
+    constexpr int KCACHE = 24;
+    select_top_n<KCACHE>(pr, A, top_n, s_hist, s_warp, s_prefix, s_remaining, put);
+    M = top_n;
+    __syncthreads();
+    sort_candidates(s_key, s_box, s_cls, M);
+  } else {
+    // ---- threshold branch (nn_skeleton.py:716-720): probs > PROB_THRESH, original order ---
+    int run = 0;
+    for (int base = 0; base < A; base += FT) {
+      const int i = base + tid;
+      const bool ok = (i < A) && (pr[i] > prob_thresh);
+      int tot;
+      const int o = block_scan_flag(ok, s_warp, tot);
+      const int slot = run + o;
+      if (ok && slot < FCAP && slot < max_dets) put(slot, order_key(pr[i]), i);
+      run += tot;
+    }
+    if (run > FCAP || run > max_dets) {
+      write_overflow(out, counts + img, max_dets);
+      return;
+    }
+    M = run;
+    __syncthreads();
   }
+  nms_and_output(s_key, s_box, s_cls, s_keep, s_warp, M, classes, nms_thresh, out, counts + img,
+                 max_dets, [&](int anchor) { return pr[anchor]; });
 }
 
 // ---- tiles of whole frames: one filter over each frame's union of tile rows -------------------
@@ -747,6 +576,8 @@ merge_tiles_kernel(const float* __restrict__ boxes, const float* __restrict__ pr
     sort_candidates(s_key, s_box, s_cls, M);
   } else {
     // ---- threshold branch: probs > PROB_THRESH in union order --------------------------------
+    // Not shared with filter_kernel's scan: a shared scan function made this branch 4 % slower
+    // (DESIGN.md, One set of filter stages).
     int run = 0;
     for (int base = 0; base < U; base += FT) {
       const int j = base + tid;
