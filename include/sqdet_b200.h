@@ -496,6 +496,40 @@ int sqdet_draw_dets(int n, int format, uint8_t* const* planes, const int64_t* pi
                     const sqdet_det* dets_dev, const int32_t* counts_dev, int max_dets,
                     const sqdet_draw_style* style, void* stream);
 
+/* ---- JPEG encoding of frames in device memory (no engine needed) -------------------
+ * sqdet_encode_jpeg: frame i's crop (x, y, w, h) becomes exactly the bytes of
+ *   cv2.imencode('.jpg', cv2.cvtColor(frame, code)[y:y+h, x:x+w], [IMWRITE_JPEG_QUALITY, quality])
+ * with `code` the frame format's code of sqdet_forward_frames (BGR: no conversion): cv2's default
+ * encoder, libjpeg-turbo's integer pipeline — baseline sequential, 4:2:0, Annex K Huffman tables
+ * (not optimized), no restart markers, JFIF APP0 1.01 with 1:1 density, quantization tables of
+ * jpeg_quality_scaling(quality) clamped to 1..255.  Frames are laid out as sqdet_forward_frames
+ * takes them.  Frame i's file goes to out_dev + i * cap and its length to lengths_dev[i]; a file
+ * longer than cap gives lengths_dev[i] = -1 and unspecified bytes in that frame's slot, and the
+ * other frames are unaffected.  cap = sqdet_jpeg_max_bytes(h, w) fits every crop of h x w or less.
+ * scratch_dev is 256-byte aligned (as cudaMalloc returns) and holds at least
+ * sqdet_jpeg_scratch_bytes(n, heights, widths, crops) bytes; lengths_dev is 8-byte aligned; out_dev
+ * may start at any byte.
+ * Runs on the device frame 0's first plane lives on (`stream` belongs to it); asynchronous on
+ * `stream`, no host synchronisation, no allocation.  Refused before any device work with
+ * SQDET_ERR_INVALID_ARG: a null array, n outside [1, 128], an unknown format, every frame refusal of
+ * sqdet_forward_frames (planes that are not device memory of that device inside one allocation
+ * included), a crop wider or taller than 65535, quality outside [1, 100], cap < 1, a misaligned
+ * scratch_dev or lengths_dev, scratch_bytes below sqdet_jpeg_scratch_bytes, and out_dev (n * cap bytes), lengths_dev (n int64) or scratch_dev
+ * (scratch_bytes) not inside one allocation of device memory on that device.
+ * sqdet_jpeg_max_bytes: the largest file of an h x w image, 0xFF stuffing of every byte included
+ * (-1 for h or w outside [1, 65535]).  sqdet_jpeg_scratch_bytes: the scratch of that call (-1 when
+ * its sizes are refused as sqdet_encode_jpeg refuses them).  Both are worst cases, so that no
+ * launch size waits for the device: for 1920 x 1080, about 20 MB of output (a quality-95 file of a
+ * natural picture is under 1 MB) and about 17 MB of scratch per frame; frames run in groups of
+ * 16 that reuse one scratch, so the scratch is that of the largest group.                     */
+int64_t sqdet_jpeg_max_bytes(int h, int w);
+int64_t sqdet_jpeg_scratch_bytes(int n, const int32_t* heights, const int32_t* widths,
+                                 const int32_t* crops);
+int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
+                      const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                      int quality, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
+                      void* scratch_dev, int64_t scratch_bytes, void* stream);
+
 /* ---- tiny device-memory helpers so a ctypes caller needs nothing else -------------- */
 int sqdet_malloc(int device, int64_t bytes, void** out_dev);
 int sqdet_free(int device, void* dev);

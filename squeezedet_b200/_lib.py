@@ -120,6 +120,9 @@ SIGNATURES = {
                                _vp]),
     'sqdet_draw_dets': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, C.POINTER(DrawStyle),
                              _vp]),
+    'sqdet_jpeg_max_bytes': (_i64, [_i, _i]),
+    'sqdet_jpeg_scratch_bytes': (_i64, [_i, _vp, _vp, _vp]),
+    'sqdet_encode_jpeg': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i64, _vp, _vp, _i64, _vp]),
     'sqdet_malloc': (_i, [_i, _i64, C.POINTER(_vp)]),
     'sqdet_free': (_i, [_i, _vp]),
     'sqdet_malloc_host': (_i, [_i64, C.POINTER(_vp)]),

@@ -119,6 +119,13 @@ constexpr int kDrawFramesPerLaunch = 24;
 int launch_draw_dets(int format, const FrameSource* frames, int n, const sqdet_det* dets,
                      const int32_t* counts, int max_dets, const DrawStyle& style,
                      cudaStream_t stream);
+// sqdet_encode_jpeg: frames per call, the largest file of an h x w crop, the scratch of the crops
+// of `frames`, and the encode of their crops (the frames' checks are the caller's).
+constexpr int kMaxJpegFrames = 128;
+int64_t jpeg_max_bytes(int h, int w);
+int64_t jpeg_scratch_bytes(const FrameSource* frames, int n);
+int launch_encode_jpeg(int format, const FrameSource* frames, int n, int quality, uint8_t* out,
+                       int64_t cap, int64_t* lengths, void* scratch, cudaStream_t stream);
 int launch_add_relu(const float* a, const float* b, float* y, int64_t n, cudaStream_t stream);
 
 int launch_interpret(const float* preds, const float* anchors, float* boxes, float* probs,

@@ -1912,6 +1912,98 @@ int sqdet_draw_dets(int n, int format, uint8_t* const* planes, const int64_t* pi
                           (cudaStream_t)stream);
 }
 
+// ---- JPEG encoding of frames in device memory ---------------------------------------------------
+constexpr int kJpegMaxSide = 65535;     // SOF0's 16-bit height and width
+
+int64_t sqdet_jpeg_max_bytes(int h, int w) {
+  if (h < 1 || w < 1 || h > kJpegMaxSide || w > kJpegMaxSide) {
+    fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_max_bytes: h and w must be in [1, 65535]");
+    return -1;
+  }
+  return jpeg_max_bytes(h, w);
+}
+
+// The crops (x, y, w, h) of sqdet_encode_jpeg's frames, or a refusal naming the first that is empty,
+// outside its frame or larger than a JPEG holds.
+static int jpeg_crops(const std::string& name, int n, const int32_t* heights, const int32_t* widths,
+                      const int32_t* crops, std::vector<FrameSource>& fr) {
+  if (!heights || !widths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (n < 1 || n > kMaxJpegFrames)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxJpegFrames) + "]");
+  fr.assign((size_t)n, FrameSource{});
+  for (int i = 0; i < n; ++i) {
+    const std::string which = name + ": frame " + std::to_string(i);
+    const int64_t H = heights[i], W = widths[i];
+    if (H <= 0 || W <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
+    const int32_t* r = crops ? crops + 4 * i : nullptr;
+    FrameSource& s = fr[(size_t)i];
+    s.x = r ? r[0] : 0;
+    s.y = r ? r[1] : 0;
+    s.w = r ? r[2] : (int)W;
+    s.h = r ? r[3] : (int)H;
+    if (s.w <= 0 || s.h <= 0) return fail(SQDET_ERR_INVALID_ARG, which + ": empty crop");
+    if (s.x < 0 || s.y < 0 || (int64_t)s.x + s.w > W || (int64_t)s.y + s.h > H)
+      return fail(SQDET_ERR_INVALID_ARG, which + ": crop outside the frame");
+    if (s.w > kJpegMaxSide || s.h > kJpegMaxSide)
+      return fail(SQDET_ERR_INVALID_ARG, which + ": a JPEG is at most 65535 pixels wide and high");
+  }
+  return SQDET_OK;
+}
+
+int64_t sqdet_jpeg_scratch_bytes(int n, const int32_t* heights, const int32_t* widths,
+                                 const int32_t* crops) {
+  std::vector<FrameSource> fr;
+  if (jpeg_crops("sqdet_jpeg_scratch_bytes", n, heights, widths, crops, fr)) return -1;
+  return jpeg_scratch_bytes(fr.data(), n);
+}
+
+int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
+                      const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                      int quality, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
+                      void* scratch_dev, int64_t scratch_bytes, void* stream) {
+  const std::string name = "sqdet_encode_jpeg";
+  const PixFormat* pf = pix_format(format);
+  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
+  if (!planes || !heights || !widths || !out_dev || !lengths_dev || !scratch_dev)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  std::vector<FrameSource> sizes;
+  int rc = jpeg_crops(name, n, heights, widths, crops, sizes);
+  if (rc) return rc;
+  if (quality < 1 || quality > 100) return fail(SQDET_ERR_INVALID_ARG, name + ": quality must be in [1, 100]");
+  if (cap < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": cap must be at least 1");
+  // the scratch holds int4, int64 and 32-bit atomic regions at 256-byte offsets from its start
+  if ((uintptr_t)scratch_dev % 256)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
+  if ((uintptr_t)lengths_dev % alignof(int64_t))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": lengths_dev must be 8-byte aligned");
+  if (scratch_bytes < jpeg_scratch_bytes(sizes.data(), n))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below sqdet_jpeg_scratch_bytes");
+  const FramePlanes pl = {{planes, planes + 1, planes + 2},
+                          {pitches, pitches ? pitches + 1 : nullptr, pitches ? pitches + 2 : nullptr},
+                          3};
+  auto image = [](int i) { return "frame " + std::to_string(i); };
+  std::vector<FrameSource> fr;
+  rc = check_frames(name, pf, n, pl, heights, widths, crops, image, fr);
+  if (rc) return rc;
+  int device = -1;
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, fr[0].plane[0]) == cudaSuccess && attr.type == cudaMemoryTypeDevice)
+    device = attr.device;
+  else
+    (void)cudaGetLastError();
+  rc = check_frame_memory(name, pf, n, heights, widths, fr, device, "frame 0's device", image);
+  if (rc) return rc;
+  const bool out_fits = cap <= INT64_MAX / n && device_range_ok(out_dev, (int64_t)n * cap, device);
+  if (!out_fits || !device_range_ok(reinterpret_cast<const uint8_t*>(lengths_dev), (int64_t)n * 8, device) ||
+      !device_range_ok(static_cast<const uint8_t*>(scratch_dev), scratch_bytes, device))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": out_dev, lengths_dev or scratch_dev is not inside one "
+                                              "device allocation on frame 0's device");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
+  return launch_encode_jpeg(format, fr.data(), n, quality, out_dev, cap, lengths_dev, scratch_dev,
+                            (cudaStream_t)stream);
+}
+
 // ---- memory helpers ------------------------------------------------------------------------------
 int sqdet_malloc(int device, int64_t bytes, void** out_dev) {
   if (!out_dev || bytes <= 0) return fail(SQDET_ERR_INVALID_ARG, "sqdet_malloc: bad argument");

@@ -17,7 +17,9 @@ imwrite out_<name>.
 uploaded once and covered by overlapping network-sized tiles at native scale
 (utils.util.tile_grid, 128 px overlap), whose detections are merged per frame on the GPU
 (ModelSkeleton.forward_device_tiles) and drawn on the full frame in device memory
-(ModelSkeleton.draw_detections_device, bitwise draw_detections), which comes back once for imwrite.
+(ModelSkeleton.draw_detections_device, bitwise draw_detections), then encoded to JPEG on the device
+(jpeg.encode_jpeg_device, byte for byte cv2.imwrite's file): only the file's bytes come back.
+`--host_encode` copies the drawn frame back and writes it with cv2.imwrite instead.
 """
 from __future__ import annotations
 
@@ -43,6 +45,9 @@ def parse_flags(argv=None):
   ap.add_argument('--tiles', action='store_true',
                   help='Video mode: detect over whole frames as overlapping tiles, merged per '
                        'frame on the GPU, instead of the reference crop.')
+  ap.add_argument('--host_encode', action='store_true',
+                  help='With --tiles: copy each drawn frame back and cv2.imwrite it instead of '
+                       'encoding it on the GPU (the same bytes).')
   return ap.parse_args(argv)
 
 
@@ -139,10 +144,12 @@ def video_demo(flags):
 def video_demo_tiles(flags):
   """Detect videos over whole frames: the frame goes to the GPU once and runs as a tile_grid of
   network-sized tiles, merged per frame (forward_device_tiles); boxes are drawn on the full
-  frame on the device (draw_detections_device), which comes back once for imwrite."""
+  frame on the device (draw_detections_device) and encoded there (encode_jpeg_device), so only
+  the JPEG's bytes come back; with --host_encode the frame comes back for cv2.imwrite."""
   import cv2
   import torch
   from . import config as cfg
+  from .jpeg import encode_jpeg_device, jpeg_bytes
   from .utils.util import tile_grid
   cap = cv2.VideoCapture(flags.input_path)
   w, h = int(cap.get(cv2.CAP_PROP_FRAME_WIDTH)), int(cap.get(cv2.CAP_PROP_FRAME_HEIGHT))
@@ -165,8 +172,13 @@ def video_demo_tiles(flags):
     t_detect = time.time()
     # boxes and labels drawn on the device frame, bitwise draw_detections on its host copy
     model.draw_detections_device([frame_dev], 'bgr', which='tiles')
-    im = frame_dev.cpu().numpy()
-    cv2.imwrite(os.path.join(flags.out_dir, str(count).zfill(6) + '.jpg'), im)
+    out_file = os.path.join(flags.out_dir, str(count).zfill(6) + '.jpg')
+    if flags.host_encode:
+      cv2.imwrite(out_file, frame_dev.cpu().numpy())
+    else:                                          # cv2.imwrite's bytes, encoded on the device
+      (data,) = jpeg_bytes(*encode_jpeg_device([frame_dev], 'bgr'))
+      with open(out_file, 'wb') as f:
+        f.write(data)
     t_draw = time.time()
     print('Total time: {:.4f}, detail: upload {:.4f} detect+merge {:.4f} draw {:.4f}'.format(
         t_draw - t_start, t_upload - t_start, t_detect - t_upload, t_draw - t_detect))
