@@ -530,6 +530,82 @@ int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int
                       int quality, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
                       void* scratch_dev, int64_t scratch_bytes, void* stream);
 
+/* ---- JPEG decoding into frames in device memory (no engine needed) -----------------
+ * sqdet_decode_jpeg: file i becomes exactly the pixels of cv2.imdecode(file, cv2.IMREAD_COLOR)
+ * (cv2's bundled libjpeg-turbo at its defaults: its SIMD islow IDCT, fancy upsampling, EXIF
+ * orientation applied), a BGR uint8 [height, width, 3] frame at out_planes[i] with rows out_pitches[i] bytes
+ * apart (pitch >= 3 * width; any start byte).
+ *
+ * Decoded: SOF0/SOF1 Huffman-coded sequential files with 8-bit samples and one scan of 1 or 3
+ * components; luma sampling 1x1, 2x1, 1x2, 2x2 or 4x1 with 1x1 chroma; any DQT and DHT; DRI.
+ * APPn and COM segments are skipped; the first APP1 'Exif' segment's Orientation is applied.
+ * Everything else is refused before any device work with SQDET_ERR_UNSUPPORTED and a message
+ * naming the file; route those files to cv2.imdecode.
+ *
+ * sqdet_jpeg_parse (host only): the headers of one file.  Returns SQDET_OK for a file
+ * sqdet_decode_jpeg decodes, SQDET_ERR_UNSUPPORTED with out->reason set for one it refuses, and
+ * SQDET_ERR_INVALID_ARG for a null pointer or len < 0.
+ *
+ * sqdet_jpeg_decode_staging_bytes / sqdet_jpeg_decode_scratch_bytes: the pinned host staging and
+ * the device scratch sqdet_decode_jpeg needs for these files (-1 when a file is refused).  Both
+ * come from the headers alone, so nothing on the host waits for the device: the staging holds
+ * every file's entropy-coded bytes plus about 9 KiB of tables, and the scratch about 5 bytes per
+ * decoded pixel for 4:2:0 and 10 for 4:4:4 (coefficients and sample planes; a quality-95 1080p
+ * 4:2:0 file of 0.54 MB takes 0.55 MB of staging and 10.6 MB of scratch).
+ *
+ * sqdet_decode_jpeg parses every header on the host, builds each file's Huffman lookup tables and
+ * quantization tables, packs them and the entropy-coded bytes into staging_pinned, issues one
+ * cudaMemcpyAsync of it into scratch_dev and then the kernels, all on `stream`, with no host
+ * synchronisation.  Staging reuse: the call returns before the copy has read staging_pinned, so
+ * the caller must not write to it again (in another call or otherwise) until that copy is done;
+ * record an event on `stream` after the call and wait on it before reusing the staging.
+ * status_dev[i] is 0 when file i decoded, negative when its entropy-coded data is corrupt (an
+ * invalid code, a DC category above 15, a run past coefficient 63, an RSTn out of sequence or
+ * missing, too few blocks in an interval, or data that runs out): its pixels are then unspecified
+ * and the other files are unaffected.  As in libjpeg, data after an interval's last block and
+ * RSTn markers after the last interval's are skipped.  Files libjpeg refuses when it builds its
+ * tables (a Huffman table with more codes than its lengths allow, a DC symbol above 15) are
+ * refused as malformed; 3-component files libjpeg takes as RGB (an Adobe transform 0, or ids
+ * 'R','G','B', without a JFIF APP0) as SQDET_JPEG_COLOR_TRANSFORM.  n is in [1, 128]; scratch_dev is 256-byte aligned device memory on the device of
+ * the outputs, status_dev 4-byte aligned; staging_pinned is page-locked host memory.  Refused
+ * with SQDET_ERR_INVALID_ARG before any device work: null arrays, n outside [1, 128], lengths
+ * outside [4, 2^28], a pitch below 3 * width, outputs, status or scratch not inside one device
+ * allocation of the outputs' device, a misaligned scratch or status, staging that is not pinned
+ * host memory, and staging or scratch bytes below the sizes above.                             */
+#define SQDET_JPEG_OK               0
+#define SQDET_JPEG_MALFORMED        1   /* truncated or malformed header */
+#define SQDET_JPEG_PROGRESSIVE      2   /* progressive or hierarchical */
+#define SQDET_JPEG_ARITHMETIC       3
+#define SQDET_JPEG_LOSSLESS         4
+#define SQDET_JPEG_PRECISION        5   /* not 8-bit samples */
+#define SQDET_JPEG_COMPONENTS       6   /* not 1 or 3 components (CMYK, YCCK, ...) */
+#define SQDET_JPEG_COLOR_TRANSFORM  7   /* RGB-coded: Adobe transform 0 or ids 'R','G','B' */
+#define SQDET_JPEG_SAMPLING         8   /* other sampling layouts, multi-scan sequential files */
+#define SQDET_JPEG_SIZE             9   /* zero height or width */
+typedef struct {
+  int32_t height, width;              /* of the decoded frame, after orientation */
+  int32_t coded_height, coded_width;  /* as SOF gives them */
+  int32_t components;                 /* 1 or 3 */
+  int32_t h_samp, v_samp;             /* luma sampling factors (chroma is 1x1) */
+  int32_t orientation;                /* EXIF Orientation 1..8 (1 without one) */
+  int32_t restart_interval;           /* MCUs per restart interval, 0 for none */
+  int32_t supported;                  /* 1 when sqdet_decode_jpeg decodes the file */
+  int32_t reason;                     /* SQDET_JPEG_* */
+  int32_t reserved;
+  int64_t scan_offset;                /* the entropy-coded segment's first byte */
+} sqdet_jpeg_info;
+int sqdet_jpeg_parse(const uint8_t* file, int64_t len, sqdet_jpeg_info* out);
+int64_t sqdet_jpeg_decode_staging_bytes(int n, const uint8_t* const* files_host, const int64_t* lengths);
+int64_t sqdet_jpeg_decode_scratch_bytes(int n, const uint8_t* const* files_host, const int64_t* lengths);
+int sqdet_decode_jpeg(int n, const uint8_t* const* files_host, const int64_t* lengths,
+                      uint8_t* const* out_planes, const int64_t* out_pitches, void* staging_pinned,
+                      int64_t staging_bytes, void* scratch_dev, int64_t scratch_bytes,
+                      int32_t* status_dev, void* stream);
+/* Test hook: the bits per subsequence of the parallel Huffman decode (a multiple of 32 in
+ * [32, 8192]; 0 restores the default 1024).  Process-wide; sizes from the functions above hold
+ * for the value set when they were called.                                                    */
+int sqdet_jpeg_decode_set_subsequence_bits(int bits);
+
 /* ---- tiny device-memory helpers so a ctypes caller needs nothing else -------------- */
 int sqdet_malloc(int device, int64_t bytes, void** out_dev);
 int sqdet_free(int device, void* dev);

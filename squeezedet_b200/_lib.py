@@ -53,6 +53,14 @@ class DrawStyle(C.Structure):
               ('font_scale', C.c_float)]
 
 
+class JpegInfo(C.Structure):
+  """struct sqdet_jpeg_info."""
+  _fields_ = [(k, C.c_int32) for k in (
+      'height', 'width', 'coded_height', 'coded_width', 'components', 'h_samp', 'v_samp',
+      'orientation', 'restart_interval', 'supported', 'reason', 'reserved')] + \
+      [('scan_offset', C.c_int64)]
+
+
 _vp, _i, _f, _i64 = C.c_void_p, C.c_int, C.c_float, C.c_int64
 _ip = C.POINTER(C.c_int)
 _i64p = C.POINTER(C.c_int64)
@@ -123,6 +131,11 @@ SIGNATURES = {
     'sqdet_jpeg_max_bytes': (_i64, [_i, _i]),
     'sqdet_jpeg_scratch_bytes': (_i64, [_i, _vp, _vp, _vp]),
     'sqdet_encode_jpeg': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i64, _vp, _vp, _i64, _vp]),
+    'sqdet_jpeg_parse': (_i, [_vp, _i64, C.POINTER(JpegInfo)]),
+    'sqdet_jpeg_decode_staging_bytes': (_i64, [_i, _vp, _vp]),
+    'sqdet_jpeg_decode_scratch_bytes': (_i64, [_i, _vp, _vp]),
+    'sqdet_decode_jpeg': (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp]),
+    'sqdet_jpeg_decode_set_subsequence_bits': (_i, [_i]),
     'sqdet_malloc': (_i, [_i, _i64, C.POINTER(_vp)]),
     'sqdet_free': (_i, [_i, _vp]),
     'sqdet_malloc_host': (_i, [_i64, C.POINTER(_vp)]),

@@ -1,0 +1,157 @@
+#!/usr/bin/env python
+"""What feeding JPEG files to the engine costs, two ways.
+
+  python -m squeezedet_b200.bench_jpeg_decode --rounds 5 --steps 10 --warmup 3
+
+A SqueezeDet engine at 1242x375 (b = --frames) runs forward_device_frames on --frames JPEG files
+per step, quality 95, of smooth synthetic pictures (bilinear upsampled noise plus grain, as
+bench_jpeg makes them, seeded on the host).  Two workloads: 1242x375 files and 1920x1080 files.
+Each step starts from the files' bytes on the host and ends one of two ways:
+  (a) a thread pool of cv2.imdecode (one file per task, os.cpu_count() threads), the BGR frames
+      uploaded, then forward_device_frames;
+  (b) decode_jpeg_device on the engine's stream, then forward_device_frames.
+The step ends at a device synchronisation; the forms alternate within each round.  Every step's
+records of (b) are checked bitwise against (a)'s.
+
+The decode kernels alone are timed in a separate pass under torch.profiler: the device durations of
+the decode_jpeg_device calls' kernels, copies and memsets, summed, per frame.
+
+Prints one JSON line with the card's name and power limit, read in the same run; writes nothing.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import time
+from concurrent.futures import ThreadPoolExecutor
+
+import numpy as np
+
+from .bench_device_frames import make_model
+from .bench_device_u8 import gpu_info
+
+FORMS = ('a_cv2_imdecode_pool', 'b_decode_jpeg_device')
+QUALITY = 95
+KERNELS = ('destuff_count_kernel', 'scan_chunks_kernel', 'destuff_compact_kernel',
+           'intervals_kernel', 'sync_tiles_kernel', 'sync_chain_kernel', 'scan_counts_kernel',
+           'decode_write_kernel', 'idct_kernel', 'color_kernel')
+
+
+def parse_args(argv=None):
+  ap = argparse.ArgumentParser()
+  ap.add_argument('--rounds', type=int, default=5)
+  ap.add_argument('--steps', type=int, default=10)
+  ap.add_argument('--warmup', type=int, default=3)
+  ap.add_argument('--frames', type=int, default=8)
+  ap.add_argument('--gpu', type=int, default=0)
+  return ap.parse_args(argv)
+
+
+def picture(h, w, rng):
+  """A smooth uint8 [h, w, 3] picture: bilinear upsampled noise plus grain."""
+  import cv2
+  low = rng.uniform(0, 255, (max(h // 24, 2), max(w // 24, 2), 3)).astype(np.float32)
+  up = cv2.resize(low, (w, h), interpolation=cv2.INTER_LINEAR)
+  return np.clip(up + rng.normal(0, 4, (h, w, 3)), 0, 255).astype(np.uint8)
+
+
+def measure_workload(args, name, model, files, torch):
+  import cv2
+  from . import _lib
+  from .jpeg import decode_jpeg_device
+  dev = torch.device('cuda', args.gpu)
+  lib = model._lib
+  stream = torch.cuda.ExternalStream(lib.sqdet_engine_stream(model._engine), device=dev)
+  pool = ThreadPoolExecutor(os.cpu_count() or 1)
+
+  def records():
+    res = model.results_device()
+    out = np.empty((len(files), res['max_dets']), _lib.DET_DTYPE)
+    _lib.check(lib.sqdet_memcpy_d2h(out.ctypes.data, res['dets'], out.nbytes, None))
+    return out
+
+  def form_a():
+    imgs = list(pool.map(lambda f: cv2.imdecode(np.frombuffer(f, np.uint8), cv2.IMREAD_COLOR), files))
+    with torch.cuda.stream(stream):
+      frames = [torch.from_numpy(im).to(dev, non_blocking=False) for im in imgs]
+    model.forward_device_frames(frames, stream=stream.cuda_stream)
+    stream.synchronize()
+
+  def form_b():
+    frames, status = decode_jpeg_device(files, dev, stream=stream)
+    model.forward_device_frames(frames, stream=stream.cuda_stream)
+    stream.synchronize()
+    return status
+
+  form_a()
+  want = records()
+  st = form_b()
+  assert st.cpu().tolist() == [0] * len(files)
+  assert records().tobytes() == want.tobytes(), '%s: the records differ' % name
+  forms = {FORMS[0]: form_a, FORMS[1]: form_b}
+  for form in FORMS:
+    for _ in range(args.warmup):
+      forms[form]()
+  step = {form: [] for form in FORMS}
+  for r in range(args.rounds):
+    for form in (FORMS if r % 2 == 0 else FORMS[::-1]):
+      for _ in range(args.steps):
+        t0 = time.perf_counter()
+        forms[form]()
+        step[form].append(time.perf_counter() - t0)
+      assert records().tobytes() == want.tobytes(), '%s: the records of %s differ' % (name, form)
+  pool.shutdown()
+
+  from torch.autograd import DeviceType
+  from torch.profiler import ProfilerActivity, profile
+  calls = 20
+  keep = []
+  with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    for _ in range(calls):
+      keep.append(decode_jpeg_device(files, dev, stream=stream))
+    stream.synchronize()
+  evs = [ev for ev in prof.events() if ev.device_type == DeviceType.CUDA and
+         any(k in ev.name for k in KERNELS + ('emset', 'emcpy', 'Memcpy', 'Memset'))]
+  kern = [ev for ev in evs if any(k in ev.name for k in KERNELS)]
+  assert len(kern) >= calls * len(KERNELS) * 9 // 10, 'found %d decode launches' % len(kern)
+  us = sum(ev.time_range.elapsed_us() for ev in evs) / calls
+  us_k = sum(ev.time_range.elapsed_us() for ev in kern) / calls
+  n = len(files)
+  row = {'workload': name, 'frames': n, 'file_bytes_mean': float(np.mean([len(f) for f in files]))}
+  for form in FORMS:
+    row[form] = {'ms_per_frame_step_median': 1e3 * float(np.median(step[form])) / n,
+                 'ms_per_frame_step_min': 1e3 * min(step[form]) / n}
+  row['decode_device'] = {'us_per_frame_kernels': us_k / n, 'us_per_frame_with_copy_and_memsets': us / n,
+                          'calls_timed': calls}
+  return row
+
+
+def measure(args):
+  import torch
+  from . import _lib
+  import cv2
+  if _lib.device_count() < 1:
+    raise SystemExit('bench_jpeg_decode: no CUDA device visible; the engine has no CPU fallback')
+  rng = np.random.default_rng(7)
+  model = make_model(1242, 375, args.frames, args.gpu)
+  rows = []
+  for name, (h, w) in (('kitti_1242x375', (375, 1242)), ('1080p', (1080, 1920))):
+    files = [cv2.imencode('.jpg', picture(h, w, rng), [cv2.IMWRITE_JPEG_QUALITY, QUALITY])[1].tobytes()
+             for _ in range(args.frames)]
+    rows.append(measure_workload(args, name, model, files, torch))
+  return {'workload': 'squeezeDet 1242x375 forward_device_frames on JPEG files (quality 95, 4:2:0, '
+                      'smooth synthetic pictures) decoded by a cv2.imdecode thread pool and '
+                      'uploaded, or by decode_jpeg_device',
+          'gpu': gpu_info(args.gpu), 'cpu_threads': os.cpu_count(),
+          'timer': 'host clock per step from the files on the host to a device synchronisation '
+                   'after the forward; decode kernels: torch.profiler device durations, summed, per frame',
+          'rounds': args.rounds, 'steps': args.steps, 'forms': list(FORMS), 'rows': rows}
+
+
+def main(argv=None):
+  print(json.dumps(measure(parse_args(argv))))
+
+
+if __name__ == '__main__':
+  main()

@@ -1341,8 +1341,8 @@ using MemGetAddressRangeFn = CUresult (*)(CUdeviceptr*, size_t*, CUdeviceptr);
 
 // True when the `bytes` bytes at p are device memory of `device` inside one allocation.  The
 // pointer comes from outside the program: a host pointer or an overlong frame is refused here
-// rather than faulting the resize kernel.
-static bool device_range_ok(const uint8_t* p, int64_t bytes, int device) {
+// rather than faulting the resize kernel.  jpeg_decode.cu checks its outputs with it too.
+bool device_range_ok(const uint8_t* p, int64_t bytes, int device) {
   static MemGetAddressRangeFn range = [] {
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult q;

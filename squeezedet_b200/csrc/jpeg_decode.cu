@@ -1,0 +1,1225 @@
+// Baseline / extended sequential JPEG decoding into BGR frames in device memory
+// (sqdet_decode_jpeg): file i becomes exactly cv2.imdecode(file_i, cv2.IMREAD_COLOR), which is
+// libjpeg-turbo's (SIMD) islow IDCT, fancy upsampling, fixed-point YCbCr->RGB and the EXIF orientation.
+// oracle/jpeg_decode.py restates it in numpy.
+//
+// The host parses the headers, builds each file's Huffman lookup and quantization tables and
+// packs them with the raw entropy-coded bytes into the caller's pinned staging; one copy takes
+// them to the scratch.  Then, per call, on the stream:
+//   1. destuff_count   per 4 KiB chunk of each file: its data bytes (stuffed 0x00 and markers
+//                      dropped) and RSTn markers, packed in one int64; the first byte of the
+//                      terminating marker (atomicMin)
+//   2. scan            per file, the exclusive scan of the chunk sums
+//   3. destuff_compact each chunk copies its data bytes to the file's clean stream and records
+//                      where each restart interval starts, checking the RSTn numbering
+//   4. intervals       per file: each interval's subsequences of kSubBits bits (at least one),
+//                      scanned into the first subsequence of each interval
+//   5. sync_tiles      the self-synchronising Huffman decode (Weissenberger & Schmidt): one
+//                      thread per subsequence decodes from a guessed state (bit offset, block of
+//                      the MCU, coefficient index) to its first symbol boundary past its end;
+//                      rounds in shared memory re-run the subsequences whose entry state changed
+//                      until every exit state matches its successor's entry (at most kTile rounds)
+//   6. sync_chain      one CTA per file walks its tiles in order: a tile whose first entry
+//                      differs from the previous tile's last exit re-runs the rounds of step 5
+//   7. scan_counts     per file, the exclusive scan of each subsequence's completed blocks and
+//                      per-component DC difference sums
+//   8. decode_write    each subsequence decodes again from its final entry state, with its first
+//                      block and DC predictors from the scan, and writes its coefficients
+//   9. idct            jpeg_idct_islow per 8x8 block (as libjpeg-turbo's SIMD code computes it)
+//                      into the component planes
+//  10. color           per output pixel: orientation, fancy upsampling, YCbCr->BGR
+// All loops are bounded by host-known sizes; a corrupt entropy-coded segment sets a negative
+// status for its file and nothing else.
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "common.cuh"
+
+extern "C" bool device_range_ok(const uint8_t* p, int64_t bytes, int device);   // engine.cu
+
+namespace sqdet {
+
+namespace {
+
+constexpr int kMaxFiles = 128;
+constexpr int kMaxFileBytes = 1 << 28;   // bit offsets within a file fit int32
+constexpr int kChunkThreads = 256;
+constexpr int kChunkBytes = 16;          // raw bytes per destuffing thread
+constexpr int kChunk = kChunkThreads * kChunkBytes;
+constexpr int kScanThreads = 1024;
+constexpr int kTile = 128;               // subsequences per sync CTA
+constexpr int kDefaultSubBits = 1024;
+constexpr int kFastBits = 9;
+constexpr int kPixThreads = 256;
+
+int g_sub_bits = kDefaultSubBits;
+
+constexpr int kNatural[64] = {
+    0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5,
+    12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14, 21, 28,
+    35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
+    58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+__constant__ uint8_t kNaturalDev[64] = {
+    0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5,
+    12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14, 21, 28,
+    35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
+    58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+
+// A Huffman table: codes of up to kFastBits bits by a lookup of the next kFastBits bits
+// (length << 8 | symbol, 0 for longer or invalid codes); longer ones canonically, through the
+// largest code of each length (-1: none) and the offset from a code to its symbol's index.
+struct HuffTab {
+  uint16_t fast[1 << kFastBits];
+  int32_t maxcode[17];
+  int32_t valoff[17];
+  uint8_t vals[256];
+};
+
+// Everything the kernels know of one file.  Offsets are bytes from the scratch's start.
+struct DecFile {
+  int32_t h, w, oh, ow, ncomp, orient;
+  int32_t mcu_cols, mcus, bpm, restart, intervals;
+  int32_t raw_len, chunks, blocks, sub_max;
+  int32_t sub_bits;
+  int8_t bcomp[10], bdy[10], bdx[10];  // per block of an MCU: component, block row and column in it
+  int8_t ch[3], cv[3];                 // sampling factors
+  int32_t pw[3], ph[3];                // padded plane width and height (whole blocks)
+  int32_t cw[3], chh[3];               // component width and height in samples
+  int16_t q[3][64];                    // dequantization, natural order (libjpeg's short multiplier)
+  int64_t raw, clean, sums, term, ist, sbase, entry, exit_, counts, coef, plane[3], tabs;
+  uint8_t* out;
+  int64_t pitch;
+};
+
+struct DecParams {
+  DecFile* f;
+  uint8_t* s;                           // the scratch
+  int32_t* status;
+};
+
+__device__ __forceinline__ void fail_file(int32_t* status, int i, int code) { status[i] = code; }
+
+// ---- block-wide exclusive scan (blockDim.x a multiple of 32) ------------------------------------
+template <class T>
+__device__ T block_scan(T v, T* warp, T* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  T x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) warp[wid] = x;
+  __syncthreads();
+  if (wid == 0) {
+    T w = lane < nw ? warp[lane] : T(0);
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const T y = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += y;
+    }
+    if (lane < nw) warp[lane] = w;
+  }
+  __syncthreads();
+  const T before = (wid ? warp[wid - 1] : T(0)) + x - v;
+  *total = warp[nw - 1];
+  __syncthreads();
+  return before;
+}
+
+// ---- 1. destuff counts ---------------------------------------------------------------------------
+// Byte j of a file's entropy-coded segment is data unless it is the byte after a 0xFF that starts
+// a marker or a stuffed 0x00, or a fill 0xFF before one.  A 0xFF followed by something other
+// than 0x00, 0xFF or RSTn ends the segment (EOI, normally), as does a 0xFF that ends the file.
+constexpr int64_t kRstOne = int64_t(1) << 40;   // chunk sums: RSTn count << 40 | data bytes
+
+__device__ __forceinline__ int byte_at(const uint8_t* raw, int len, int j) {
+  return j >= 0 && j < len ? raw[j] : -1;
+}
+
+// 0 data, 1 dropped, 2 RSTn (its 0xFF), 3 terminator (its 0xFF)
+__device__ __forceinline__ int classify(const uint8_t* raw, int len, int j) {
+  const int b = raw[j];
+  if (b == 0xFF) {
+    const int nx = byte_at(raw, len, j + 1);
+    if (nx == 0x00) return 0;
+    if (nx == 0xFF) return 1;
+    if (nx >= 0xD0 && nx <= 0xD7) return 2;
+    return 3;
+  }
+  return byte_at(raw, len, j - 1) == 0xFF ? 1 : 0;
+}
+
+__global__ void __launch_bounds__(kChunkThreads) destuff_count_kernel(DecParams p) {
+  __shared__ int64_t warp[32];
+  const DecFile& f = p.f[blockIdx.y];
+  if ((int)blockIdx.x >= f.chunks) return;
+  const uint8_t* raw = p.s + f.raw;
+  const int first = blockIdx.x * kChunk + threadIdx.x * kChunkBytes;
+  int64_t v = 0;
+  int term = INT32_MAX;
+  for (int j = first; j < first + kChunkBytes && j < f.raw_len; ++j) {
+    const int c = classify(raw, f.raw_len, j);
+    v += c == 0 ? 1 : c == 2 ? kRstOne : 0;
+    if (c == 3 && term == INT32_MAX) term = j;
+  }
+  if (term != INT32_MAX) atomicMin(reinterpret_cast<uint32_t*>(p.s + f.term), (uint32_t)term);
+  int64_t total;
+  block_scan<int64_t>(v, warp, &total);
+  if (threadIdx.x == 0) reinterpret_cast<int64_t*>(p.s + f.sums)[blockIdx.x] = total;
+}
+
+// ---- 2. per-file exclusive scan of chunk sums ------------------------------------------------------
+__global__ void __launch_bounds__(kScanThreads) scan_chunks_kernel(DecParams p) {
+  __shared__ int64_t warp[32];
+  const DecFile& f = p.f[blockIdx.x];
+  int64_t* s = reinterpret_cast<int64_t*>(p.s + f.sums);
+  int64_t carry = 0;
+  for (int base = 0; base < f.chunks; base += kScanThreads) {
+    const int i = base + threadIdx.x;
+    const int64_t v = i < f.chunks ? s[i] : 0;
+    int64_t total;
+    const int64_t ex = block_scan<int64_t>(v, warp, &total);
+    if (i < f.chunks) s[i] = carry + ex;
+    carry += total;
+  }
+  if (threadIdx.x == 0) s[f.chunks] = carry;
+}
+
+// ---- 3. compact ------------------------------------------------------------------------------------
+// ist[r] is the clean byte where interval r starts (ist[0] = 0, ist[intervals] = the end); the
+// intervals kernel finds any left at -1.
+__global__ void __launch_bounds__(kChunkThreads) destuff_compact_kernel(DecParams p) {
+  __shared__ int64_t warp[32];
+  const DecFile& f = p.f[blockIdx.y];
+  if ((int)blockIdx.x >= f.chunks) return;
+  const uint8_t* raw = p.s + f.raw;
+  uint8_t* clean = p.s + f.clean;
+  int32_t* ist = reinterpret_cast<int32_t*>(p.s + f.ist);
+  const int term = (int)min(*reinterpret_cast<const uint32_t*>(p.s + f.term), (uint32_t)f.raw_len);
+  const int first = blockIdx.x * kChunk + threadIdx.x * kChunkBytes;
+  uint8_t cls[kChunkBytes];
+  int64_t v = 0;
+#pragma unroll
+  for (int i = 0; i < kChunkBytes; ++i) {
+    const int j = first + i;
+    cls[i] = j < f.raw_len ? (uint8_t)classify(raw, f.raw_len, j) : 1;
+    v += cls[i] == 0 ? 1 : cls[i] == 2 ? kRstOne : 0;
+  }
+  int64_t total;
+  const int64_t at = reinterpret_cast<const int64_t*>(p.s + f.sums)[blockIdx.x] + block_scan<int64_t>(v, warp, &total);
+  int64_t o = at & (kRstOne - 1);
+  int r = (int)(at >> 40);
+  for (int i = 0; i < kChunkBytes; ++i) {
+    const int j = first + i;
+    if (j >= term) {
+      if (j == term) ist[f.intervals] = (int32_t)o;
+      break;
+    }
+    if (cls[i] == 0) {
+      clean[o++] = raw[j];
+    } else if (cls[i] == 2) {
+      // the r-th marker ends interval r and must be RST(r mod 8); markers after the last
+      // interval's are skipped, as libjpeg skips them
+      if (r + 1 < f.intervals) {
+        if (raw[j + 1] != 0xD0 + (r & 7)) fail_file(p.status, blockIdx.y, -2);
+        ist[r + 1] = (int32_t)o;
+      }
+      ++r;
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    ist[0] = 0;
+    if (term >= f.raw_len) {                            // no terminator: the data runs to the end
+      ist[f.intervals] = (int32_t)(reinterpret_cast<const int64_t*>(p.s + f.sums)[f.chunks] & (kRstOne - 1));
+    }
+  }
+}
+
+// ---- 4. intervals -> subsequences ------------------------------------------------------------------
+// sbase[r] is the first subsequence of interval r, sbase[intervals] their count (<= sub_max).
+__global__ void __launch_bounds__(kScanThreads) intervals_kernel(DecParams p) {
+  __shared__ int32_t warp[32];
+  const int i = blockIdx.x;
+  const DecFile& f = p.f[i];
+  const int32_t* ist = reinterpret_cast<const int32_t*>(p.s + f.ist);
+  int32_t* sbase = reinterpret_cast<int32_t*>(p.s + f.sbase);
+  int32_t carry = 0;
+  bool bad = false;
+  for (int base = 0; base < f.intervals; base += kScanThreads) {
+    const int r = base + threadIdx.x;
+    int32_t v = 0;
+    if (r < f.intervals) {
+      const int a = ist[r], b = ist[r + 1];
+      if (a < 0 || b < a) {
+        bad = true;
+        v = 1;
+      } else {
+        v = max(1, (int)(((int64_t)(b - a) * 8 + f.sub_bits - 1) / f.sub_bits));
+      }
+    }
+    int32_t total;
+    const int32_t ex = block_scan<int32_t>(v, warp, &total);
+    if (r < f.intervals) sbase[r] = carry + ex;
+    carry += total;
+  }
+  if (bad) fail_file(p.status, i, -3);
+  if (threadIdx.x == 0) sbase[f.intervals] = min(carry, f.sub_max);
+}
+
+// ---- the Huffman decoder ---------------------------------------------------------------------------
+// The 32 bits of the clean stream from bit p on (MSB first); words past the end are padding.
+__device__ __forceinline__ uint32_t peek32(const uint8_t* clean, int p) {
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(clean) + (p >> 5);
+  const uint32_t a = __byte_perm(w[0], 0, 0x0123), b = __byte_perm(w[1], 0, 0x0123);
+  return __funnelshift_l(b, a, p & 31);
+}
+
+// One decoder state at a symbol boundary: bit offset, block of the MCU, next coefficient (0: DC).
+struct State {
+  int p, uk;                             // uk = u << 8 | k
+  __device__ bool operator==(const State& o) const { return p == o.p && uk == o.uk; }
+};
+
+// The symbol and code length at the front of `bits`, length 0 for an invalid code.
+__device__ __forceinline__ int huff_decode(const HuffTab& t, uint32_t bits, int& len) {
+  const int e = t.fast[bits >> (32 - kFastBits)];
+  if (e) {
+    len = e >> 8;
+    return e & 255;
+  }
+  int l = kFastBits + 1;
+  int code = (int)(bits >> (32 - l));
+#pragma unroll 1
+  for (; l <= 16 && code > t.maxcode[l]; ++l) code = (int)(bits >> (32 - (l + 1)));
+  if (l > 16) {
+    len = 0;
+    return 0;
+  }
+  len = l;
+  return t.vals[(t.valoff[l] + code) & 255];
+}
+
+__device__ __forceinline__ int extend(uint32_t v, int s) {
+  return s && v < (1u << (s - 1)) ? (int)v - (1 << s) + 1 : (int)v;
+}
+
+struct Counts {
+  int blocks, dc[3];
+};
+
+// Decodes from state st while st.p < end and fewer than block_limit blocks are complete.  kWrite:
+// writes the block's coefficients (JCOEF, natural order) to coef + 64 * (block0 + blocks), with
+// the DC predictors in c.dc, and reports corrupt data through the return value (negative);
+// otherwise c.dc sums the DC differences and corrupt data decodes on deterministically.
+template <bool kWrite>
+__device__ int decode_run(const DecFile& f, const HuffTab* tabs, const uint8_t* clean, State& st,
+                          int end, int block_limit, Counts& c, int16_t* coef, int64_t block0,
+                          int max_iter) {
+  int p = st.p, u = st.uk >> 8, k = st.uk & 255;
+#pragma unroll 1
+  for (int it = 0; it < max_iter && p < end && c.blocks < block_limit; ++it) {
+    const int comp = f.bcomp[u];
+    const uint32_t bits = peek32(clean, p);
+    int len;
+    const int sym = huff_decode(tabs[2 * comp + (k ? 1 : 0)], bits, len);
+    if (!len) {
+      if (kWrite) return -4;
+      ++p;                                // speculative: step one bit
+      continue;
+    }
+    const int s = sym & 15, run = sym >> 4;
+    const uint32_t extra = s ? (bits << len) >> (32 - s) : 0;
+    p += len + s;
+    if (k == 0) {
+      if (sym > 15) {
+        if (kWrite) return -4;
+      }
+      c.dc[comp] += extend(extra, s);
+      if (kWrite) coef[(block0 + c.blocks) * 64] = (int16_t)c.dc[comp];
+      k = 1;
+    } else if (s) {
+      k += run;
+      if (k > 63) {
+        if (kWrite) return -5;
+        k = 64;
+      } else {
+        if (kWrite) coef[(block0 + c.blocks) * 64 + kNaturalDev[k]] = (int16_t)extend(extra, s);
+        ++k;
+      }
+    } else if (run == 15) {
+      k += 16;
+      if (k > 64) {
+        if (kWrite) return -5;
+        k = 64;
+      }
+    } else {
+      k = 64;
+    }
+    if (k >= 64) {
+      ++c.blocks;
+      k = 0;
+      u = u + 1 == f.bpm ? 0 : u + 1;
+    }
+  }
+  st.p = p;
+  st.uk = u << 8 | k;
+  return 0;
+}
+
+// Subsequence g of a file: its interval r, its first bit and the end of its range.
+struct Sub {
+  int r, j, start, end, nsub;
+};
+__device__ Sub locate(const DecFile& f, const int32_t* ist, const int32_t* sbase, int g) {
+  int lo = 0, hi = f.intervals - 1;           // the last r with sbase[r] <= g
+#pragma unroll 1
+  for (int it = 0; it < 32 && lo < hi; ++it) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (sbase[mid] <= g) lo = mid; else hi = mid - 1;
+  }
+  Sub s;
+  s.r = lo;
+  s.j = g - sbase[lo];
+  s.nsub = sbase[lo + 1] - sbase[lo];
+  const int a = max(ist[lo], 0), b = max(ist[lo + 1], a);
+  s.start = a * 8 + s.j * f.sub_bits;
+  s.end = min(s.start + f.sub_bits, b * 8);
+  return s;
+}
+
+// The rounds of the synchronisation within one tile of kTile subsequences from g0: entries whose
+// `dirty` flag is set are decoded again, and each exit that differs from its successor's entry
+// (unless that successor starts an interval) becomes that entry.  Each round makes at least one
+// more entry final, so kTile rounds suffice.
+__device__ void sync_rounds(const DecFile& f, const HuffTab* tabs, const uint8_t* clean,
+                            const Sub& sub, bool valid, bool dirty0, State* entry, State* exit_,
+                            Counts& cnt, int* starts_interval) {
+  const int t = threadIdx.x;
+  bool dirty = dirty0;
+  starts_interval[t] = !valid || sub.j == 0;
+  __syncthreads();
+#pragma unroll 1
+  for (int round = 0; round < kTile; ++round) {
+    if (dirty && valid) {
+      State st = entry[t];
+      cnt = Counts{0, {0, 0, 0}};
+      decode_run<false>(f, tabs, clean, st, sub.end, INT32_MAX, cnt, nullptr, 0, f.sub_bits + 64);
+      exit_[t] = st;
+    }
+    dirty = false;
+    __syncthreads();
+    bool changed = false;
+    if (t > 0 && valid && !starts_interval[t] && !(exit_[t - 1] == entry[t])) {
+      changed = true;
+    }
+    const State prev = t > 0 ? exit_[t - 1] : State{0, 0};
+    __syncthreads();
+    if (changed) {
+      entry[t] = prev;
+      dirty = true;
+    }
+    if (!__syncthreads_or(changed)) break;
+  }
+}
+
+// ---- 5. sync within tiles ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(kTile) sync_tiles_kernel(DecParams p) {
+  __shared__ State entry[kTile], exit_[kTile];
+  __shared__ int starts[kTile];
+  const DecFile& f = p.f[blockIdx.y];
+  const int32_t* sbase = reinterpret_cast<const int32_t*>(p.s + f.sbase);
+  const int nsub = sbase[f.intervals];
+  const int g0 = blockIdx.x * kTile;
+  if (g0 >= nsub) return;
+  const int32_t* ist = reinterpret_cast<const int32_t*>(p.s + f.ist);
+  const HuffTab* tabs = reinterpret_cast<const HuffTab*>(p.s + f.tabs);
+  const uint8_t* clean = p.s + f.clean;
+  const int g = g0 + threadIdx.x;
+  const bool valid = g < nsub;
+  const Sub sub = valid ? locate(f, ist, sbase, g) : Sub{0, 0, 0, 0, 0};
+  entry[threadIdx.x] = State{sub.start, 0};
+  Counts cnt{0, {0, 0, 0}};
+  sync_rounds(f, tabs, clean, sub, valid, true, entry, exit_, cnt, starts);
+  if (valid) {
+    reinterpret_cast<State*>(p.s + f.entry)[g] = entry[threadIdx.x];
+    reinterpret_cast<State*>(p.s + f.exit_)[g] = exit_[threadIdx.x];
+    reinterpret_cast<int4*>(p.s + f.counts)[g] = make_int4(cnt.blocks, cnt.dc[0], cnt.dc[1], cnt.dc[2]);
+  }
+}
+
+// ---- 6. sync across tiles ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(kTile) sync_chain_kernel(DecParams p) {
+  __shared__ State entry[kTile], exit_[kTile];
+  __shared__ int starts[kTile];
+  const DecFile& f = p.f[blockIdx.x];
+  const int32_t* sbase = reinterpret_cast<const int32_t*>(p.s + f.sbase);
+  const int nsub = sbase[f.intervals];
+  const int32_t* ist = reinterpret_cast<const int32_t*>(p.s + f.ist);
+  const HuffTab* tabs = reinterpret_cast<const HuffTab*>(p.s + f.tabs);
+  const uint8_t* clean = p.s + f.clean;
+  State* gentry = reinterpret_cast<State*>(p.s + f.entry);
+  State* gexit = reinterpret_cast<State*>(p.s + f.exit_);
+  int4* gcounts = reinterpret_cast<int4*>(p.s + f.counts);
+  const int tiles = (f.sub_max + kTile - 1) / kTile;
+#pragma unroll 1
+  for (int tile = 1; tile < tiles; ++tile) {
+    const int g0 = tile * kTile;
+    if (g0 >= nsub) break;
+    const int g = g0 + threadIdx.x;
+    const bool valid = g < nsub;
+    // the tile's first entry is final once the previous tile's last exit is
+    const Sub first = locate(f, ist, sbase, g0);
+    const State want = gexit[g0 - 1];
+    const bool stale = first.j != 0 && !(gentry[g0] == want);
+    if (!stale) continue;                  // uniform across the CTA
+    const Sub sub = valid ? locate(f, ist, sbase, g) : Sub{0, 0, 0, 0, 0};
+    if (valid) {
+      entry[threadIdx.x] = threadIdx.x == 0 ? want : gentry[g];
+      exit_[threadIdx.x] = gexit[g];
+    }
+    const int4 c4 = valid ? gcounts[g] : make_int4(0, 0, 0, 0);
+    Counts cnt{c4.x, {c4.y, c4.z, c4.w}};
+    __syncthreads();
+    sync_rounds(f, tabs, clean, sub, valid, threadIdx.x == 0, entry, exit_, cnt, starts);
+    if (valid) {
+      gentry[g] = entry[threadIdx.x];
+      gexit[g] = exit_[threadIdx.x];
+      gcounts[g] = make_int4(cnt.blocks, cnt.dc[0], cnt.dc[1], cnt.dc[2]);
+    }
+    __syncthreads();
+  }
+}
+
+// ---- 7. per-file exclusive scan of the counts ---------------------------------------------------------
+__global__ void __launch_bounds__(kScanThreads) scan_counts_kernel(DecParams p) {
+  __shared__ int32_t warp[32];
+  const DecFile& f = p.f[blockIdx.x];
+  const int nsub = reinterpret_cast<const int32_t*>(p.s + f.sbase)[f.intervals];
+  int4* c = reinterpret_cast<int4*>(p.s + f.counts);
+  int4 carry = make_int4(0, 0, 0, 0);
+  for (int base = 0; base < nsub; base += kScanThreads) {
+    const int i = base + threadIdx.x;
+    const int4 v = i < nsub ? c[i] : make_int4(0, 0, 0, 0);
+    int4 ex, tot;
+    ex.x = block_scan<int32_t>(v.x, warp, &tot.x);
+    ex.y = block_scan<int32_t>(v.y, warp, &tot.y);
+    ex.z = block_scan<int32_t>(v.z, warp, &tot.z);
+    ex.w = block_scan<int32_t>(v.w, warp, &tot.w);
+    if (i < nsub) c[i] = make_int4(carry.x + ex.x, carry.y + ex.y, carry.z + ex.z, carry.w + ex.w);
+    carry = make_int4(carry.x + tot.x, carry.y + tot.y, carry.z + tot.z, carry.w + tot.w);
+  }
+}
+
+// ---- 8. decode and write coefficients -----------------------------------------------------------------
+__global__ void __launch_bounds__(kTile) decode_write_kernel(DecParams p) {
+  const DecFile& f = p.f[blockIdx.y];
+  const int32_t* sbase = reinterpret_cast<const int32_t*>(p.s + f.sbase);
+  const int nsub = sbase[f.intervals];
+  const int g = blockIdx.x * kTile + threadIdx.x;
+  if (g >= nsub) return;
+  const int32_t* ist = reinterpret_cast<const int32_t*>(p.s + f.ist);
+  const HuffTab* tabs = reinterpret_cast<const HuffTab*>(p.s + f.tabs);
+  const int4* counts = reinterpret_cast<const int4*>(p.s + f.counts);
+  const Sub sub = locate(f, ist, sbase, g);
+  const int4 mine = counts[g], base = counts[sbase[sub.r]];
+  const int interval_blocks = min(f.restart, f.mcus - sub.r * f.restart) * f.bpm;
+  Counts c{mine.x - base.x, {mine.y - base.y, mine.z - base.z, mine.w - base.w}};
+  const int b0 = c.blocks;
+  if (b0 < 0) {
+    fail_file(p.status, blockIdx.y, -6);
+    return;
+  }
+  State st = reinterpret_cast<const State*>(p.s + f.entry)[g];
+  // every block of the interval lies in [first block of the interval, + interval_blocks)
+  c.blocks = 0;
+  int16_t* coef = reinterpret_cast<int16_t*>(p.s + f.coef);
+  const int64_t block0 = (int64_t)sub.r * f.restart * f.bpm + b0;
+  const int limit = interval_blocks - b0;
+  const int rc = limit > 0 ? decode_run<true>(f, tabs, p.s + f.clean, st, sub.end, limit, c, coef,
+                                              block0, f.sub_bits + 64)
+                           : 0;
+  const int end_bits = max(ist[sub.r + 1], 0) * 8;
+  if (rc) {
+    fail_file(p.status, blockIdx.y, rc);
+  } else if (st.p > end_bits) {
+    fail_file(p.status, blockIdx.y, -7);                 // ran off the interval's data
+  } else if (sub.j == sub.nsub - 1 && b0 + c.blocks < interval_blocks) {
+    fail_file(p.status, blockIdx.y, -8);                 // too few blocks in the interval
+  }
+  // data after an interval's last block is skipped, as libjpeg skips it before the next marker
+}
+
+// ---- 9. IDCT ----------------------------------------------------------------------------------------
+constexpr int F0_298 = 2446, F0_390 = 3196, F0_541 = 4433, F0_765 = 6270, F0_899 = 7373,
+              F1_175 = 9633, F1_501 = 12299, F1_847 = 15137, F1_961 = 16069, F2_053 = 16819,
+              F2_562 = 20995, F3_072 = 25172;
+
+__device__ __forceinline__ int w16(int x) { return (int)(int16_t)x; }   // a 16-bit SIMD add
+__device__ __forceinline__ int s16(int x) { return min(max(x, -32768), 32767); }   // packssdw
+
+// One 1-D pass of jpeg_idct_islow over d[0], d[stride], ... d[7 stride], descaled by `shift`, as
+// libjpeg-turbo's SIMD islow computes it (cv2 runs that code): products and their sums in 32 bits,
+// in0 +- in4, in7 + in3 and in5 + in1 in 16 bits.  For coefficients an 8-bit encoder writes this
+// is jidctint.c's arithmetic; it differs only where those sums overflow 16 bits.
+__device__ __forceinline__ void idct8(int* d, int stride, int shift) {
+  int z2 = d[2 * stride], z3 = d[6 * stride];
+  int z1 = (z2 + z3) * F0_541;
+  const int tmp2 = z1 - z3 * F1_847, tmp3 = z1 + z2 * F0_765;
+  const int tmp0 = w16(d[0] + d[4 * stride]) << 13, tmp1 = w16(d[0] - d[4 * stride]) << 13;
+  const int t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
+  int a0 = d[7 * stride], a1 = d[5 * stride], a2 = d[3 * stride], a3 = d[stride];
+  z1 = a0 + a3;
+  z2 = a1 + a2;
+  z3 = w16(a0 + a2);
+  int z4 = w16(a1 + a3);
+  const int z5 = (z3 + z4) * F1_175;
+  a0 *= F0_298;
+  a1 *= F2_053;
+  a2 *= F3_072;
+  a3 *= F1_501;
+  z1 *= -F0_899;
+  z2 *= -F2_562;
+  z3 = z3 * -F1_961 + z5;
+  z4 = z4 * -F0_390 + z5;
+  a0 += z1 + z3;
+  a1 += z2 + z4;
+  a2 += z2 + z3;
+  a3 += z1 + z4;
+  const int rnd = 1 << (shift - 1);
+  d[0] = (t10 + a3 + rnd) >> shift;
+  d[7 * stride] = (t10 - a3 + rnd) >> shift;
+  d[stride] = (t11 + a2 + rnd) >> shift;
+  d[6 * stride] = (t11 - a2 + rnd) >> shift;
+  d[2 * stride] = (t12 + a1 + rnd) >> shift;
+  d[5 * stride] = (t12 - a1 + rnd) >> shift;
+  d[3 * stride] = (t13 + a0 + rnd) >> shift;
+  d[4 * stride] = (t13 - a0 + rnd) >> shift;
+}
+
+// The SIMD islow's block: dequantization by a 16-bit multiply; the column pass saturated to 16
+// bits, or, when every AC coefficient is zero, the DC << 2 in 16 bits; the output clamped.
+__global__ void __launch_bounds__(kPixThreads) idct_kernel(DecParams p) {
+  const DecFile& f = p.f[blockIdx.y];
+  const int b = blockIdx.x * kPixThreads + threadIdx.x;
+  if (b >= f.blocks) return;
+  const int m = b / f.bpm, u = b - m * f.bpm;
+  const int c = f.bcomp[u];
+  int by, bx;
+  if (f.ncomp == 1) {
+    by = m / f.mcu_cols;
+    bx = m - by * f.mcu_cols;
+  } else {
+    const int my = m / f.mcu_cols, mx = m - my * f.mcu_cols;
+    by = my * f.cv[c] + f.bdy[u];
+    bx = mx * f.ch[c] + f.bdx[u];
+  }
+  const int4* src = reinterpret_cast<const int4*>(p.s + f.coef) + (int64_t)b * 8;
+  int d[64];
+  int ac = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int4 v = src[i];
+    if (i) ac |= v.x | v.y | v.z | v.w;
+    const int16_t* h = reinterpret_cast<const int16_t*>(&v);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) d[8 * i + e] = w16((int)h[e] * (int)f.q[c][8 * i + e]);
+  }
+  if (ac) {
+#pragma unroll
+    for (int col = 0; col < 8; ++col) idct8(d + col, 8, 11);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) d[i] = s16(d[i]);
+  } else {
+#pragma unroll
+    for (int i = 63; i >= 0; --i) d[i] = w16(d[i & 7] << 2);   // row 0 last: the others read it
+  }
+#pragma unroll
+  for (int row = 0; row < 8; ++row) idct8(d + 8 * row, 1, 18);
+  uint8_t* plane = p.s + f.plane[c];
+  const int pw = f.pw[c];
+#pragma unroll
+  for (int row = 0; row < 8; ++row) {
+    uint32_t w[2] = {0, 0};
+#pragma unroll
+    for (int col = 0; col < 8; ++col) {
+      const int v = min(max(s16(d[8 * row + col]), -128), 127) + 128;
+      w[col >> 2] |= (uint32_t)v << (8 * (col & 3));
+    }
+    *reinterpret_cast<uint2*>(plane + (int64_t)(by * 8 + row) * pw + bx * 8) = make_uint2(w[0], w[1]);
+  }
+}
+
+// ---- 10. upsample, convert, orient ----------------------------------------------------------------------
+// Chroma of full-resolution pixel (y, x) from plane c (cw x chh samples) with sampling (fh, fv).
+__device__ __forceinline__ int chroma_at(const uint8_t* pl, int pw, int cw, int chh, int fh, int fv,
+                                         int y, int x) {
+  const bool fancy_h = fh == 2 && cw > 2;
+  if (fh == 1 && fv == 1) return pl[(int64_t)y * pw + x];
+  if (fv == 2 && (fh == 1 || fancy_h)) {
+    const int r = y >> 1, rn = (y & 1) ? min(r + 1, chh - 1) : max(r - 1, 0);
+    if (fh == 1) return (3 * pl[(int64_t)r * pw + x] + pl[(int64_t)rn * pw + x] + 1 + (y & 1)) >> 2;
+    const int cx = x >> 1, xn = (x & 1) ? min(cx + 1, cw - 1) : max(cx - 1, 0);
+    const int near = 3 * pl[(int64_t)r * pw + cx] + pl[(int64_t)rn * pw + cx];
+    const int far = 3 * pl[(int64_t)r * pw + xn] + pl[(int64_t)rn * pw + xn];
+    return (3 * near + far + 8 - (x & 1)) >> 4;
+  }
+  if (fv == 1 && fancy_h) {
+    const int cx = x >> 1, xn = (x & 1) ? min(cx + 1, cw - 1) : max(cx - 1, 0);
+    const uint8_t* row = pl + (int64_t)y * pw;
+    return (3 * row[cx] + row[xn] + 1 + (x & 1)) >> 2;
+  }
+  return pl[(int64_t)(y / fv) * pw + x / fh];
+}
+
+__global__ void __launch_bounds__(kPixThreads) color_kernel(DecParams p) {
+  const DecFile& f = p.f[blockIdx.y];
+  const int64_t i = (int64_t)blockIdx.x * kPixThreads + threadIdx.x;
+  if (i >= (int64_t)f.oh * f.ow) return;
+  const int oy = (int)(i / f.ow), ox = (int)(i - (int64_t)oy * f.ow);
+  int sy = oy, sx = ox;
+  switch (f.orient) {
+    case 2: sx = f.w - 1 - ox; break;
+    case 3: sy = f.h - 1 - oy; sx = f.w - 1 - ox; break;
+    case 4: sy = f.h - 1 - oy; break;
+    case 5: sy = ox; sx = oy; break;
+    case 6: sy = f.h - 1 - ox; sx = oy; break;
+    case 7: sy = f.h - 1 - ox; sx = f.w - 1 - oy; break;
+    case 8: sy = ox; sx = f.w - 1 - oy; break;
+    default: break;
+  }
+  const int y = p.s[f.plane[0] + (int64_t)sy * f.pw[0] + sx];
+  int b = y, g = y, r = y;
+  if (f.ncomp == 3) {
+    const int fh = f.ch[0], fv = f.cv[0];
+    const int cb = chroma_at(p.s + f.plane[1], f.pw[1], f.cw[1], f.chh[1], fh, fv, sy, sx) - 128;
+    const int cr = chroma_at(p.s + f.plane[2], f.pw[2], f.cw[2], f.chh[2], fh, fv, sy, sx) - 128;
+    // jdcolor.c's tables: FIX(x) = x * 2^16 rounded
+    r = y + ((91881 * cr + 32768) >> 16);
+    b = y + ((116130 * cb + 32768) >> 16);
+    g = y + ((-22554 * cb + 32768 - 46802 * cr) >> 16);
+    r = min(max(r, 0), 255);
+    g = min(max(g, 0), 255);
+    b = min(max(b, 0), 255);
+  }
+  uint8_t* o = f.out + (int64_t)oy * f.pitch + 3 * (int64_t)ox;
+  o[0] = (uint8_t)b;
+  o[1] = (uint8_t)g;
+  o[2] = (uint8_t)r;
+}
+
+// ---- host: parsing -----------------------------------------------------------------------------------
+struct Comp {
+  int id, h, v, tq, td, ta;
+};
+struct Parsed {
+  sqdet_jpeg_info info;
+  Comp comp[3];
+  uint16_t qt[4][64];                  // natural order
+  bool have_q[4], have_dc[4], have_ac[4];
+  uint8_t dc_bits[4][16], ac_bits[4][16];
+  uint8_t dc_vals[4][256], ac_vals[4][256];
+};
+
+int u16(const uint8_t* b, int64_t i) { return (b[i] << 8) | b[i + 1]; }
+
+int exif_orientation(const uint8_t* s, int64_t n) {
+  if (n < 14 || memcmp(s, "Exif\0\0", 6) != 0) return 1;
+  const uint8_t* t = s + 6;
+  const int64_t tn = n - 6;
+  bool le;
+  if (t[0] == 'I' && t[1] == 'I') le = true;
+  else if (t[0] == 'M' && t[1] == 'M') le = false;
+  else return 1;
+  auto rd = [&](int64_t i, int k) -> int64_t {
+    if (i < 0 || i + k > tn) return -1;
+    int64_t v = 0;
+    for (int j = 0; j < k; ++j) v |= (int64_t)t[i + (le ? j : k - 1 - j)] << (8 * j);
+    return v;
+  };
+  if (rd(2, 2) != 42) return 1;
+  const int64_t ifd = rd(4, 4);
+  const int64_t count = rd(ifd, 2);
+  if (ifd < 0 || count < 0) return 1;
+  for (int64_t e = 0; e < count; ++e) {
+    const int64_t q = ifd + 2 + 12 * e;
+    if (q + 12 > tn) break;
+    if (rd(q, 2) == 0x0112 && rd(q + 2, 2) == 3) {
+      const int64_t o = rd(q + 8, 2);
+      return o >= 1 && o <= 8 ? (int)o : 1;
+    }
+  }
+  return 1;
+}
+
+// jpeg.jpeg_info reports these words; oracle/jpeg_decode.py's REASONS are tested equal to them
+const char* kReasons[] = {"ok", "malformed or truncated header", "progressive", "arithmetic coding",
+                          "lossless", "not 8-bit samples", "not 1 or 3 components",
+                          "RGB-coded", "unsupported sampling",
+                          "zero height or width"};
+
+// libjpeg's checks of a Huffman table a scan uses: no length's codes run past its all-ones code,
+// and a DC table's symbols are categories 0..15.
+bool huff_ok(const uint8_t* bits, const uint8_t* vals, bool dc) {
+  int code = 0, count = 0;
+  for (int l = 1; l <= 16; ++l) {
+    code += bits[l - 1];
+    count += bits[l - 1];
+    if (code >= (1 << l)) return false;
+    code <<= 1;
+  }
+  for (int k = 0; dc && k < count; ++k)
+    if (vals[k] > 15) return false;
+  return true;
+}
+
+// The headers up to the first SOS; the reason (SQDET_JPEG_*) and what was read.
+int parse(const uint8_t* b, int64_t n, Parsed& P) {
+  memset(&P, 0, sizeof(P));
+  sqdet_jpeg_info& I = P.info;
+  I.orientation = 1;
+  if (n < 4 || b[0] != 0xFF || b[1] != 0xD8) return SQDET_JPEG_MALFORMED;
+  int adobe = -1, ncomp = 0;
+  bool frame = false, exif = false, jfif = false;
+  int64_t i = 2;
+  for (;;) {
+    while (i + 1 < n && b[i] == 0xFF && b[i + 1] == 0xFF) ++i;
+    if (i + 2 > n || b[i] != 0xFF) return SQDET_JPEG_MALFORMED;
+    const int m = b[i + 1];
+    i += 2;
+    if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) return SQDET_JPEG_MALFORMED;
+    if (i + 2 > n) return SQDET_JPEG_MALFORMED;
+    const int len = u16(b, i);
+    if (len < 2 || i + len > n) return SQDET_JPEG_MALFORMED;
+    const uint8_t* body = b + i + 2;
+    const int bn = len - 2;
+    i += len;
+    if (m == 0xC2 || m == 0xC6 || m == 0xCA || m == 0xCE) return SQDET_JPEG_PROGRESSIVE;
+    if (m == 0xC9 || m == 0xCB || m == 0xCD || m == 0xCF) return SQDET_JPEG_ARITHMETIC;
+    if (m == 0xC3 || m == 0xC7) return SQDET_JPEG_LOSSLESS;
+    if (m == 0xC5) return SQDET_JPEG_PROGRESSIVE;
+    if (m == 0xC0 || m == 0xC1) {
+      if (frame || bn < 6) return SQDET_JPEG_MALFORMED;
+      I.coded_height = u16(body, 1);
+      I.coded_width = u16(body, 3);
+      ncomp = body[5];
+      if (body[0] != 8) return SQDET_JPEG_PRECISION;
+      if (bn != 6 + 3 * ncomp) return SQDET_JPEG_MALFORMED;
+      if (ncomp != 1 && ncomp != 3) return SQDET_JPEG_COMPONENTS;
+      I.components = ncomp;
+      for (int k = 0; k < ncomp; ++k) {
+        Comp& c = P.comp[k];
+        c.id = body[6 + 3 * k];
+        c.h = body[7 + 3 * k] >> 4;
+        c.v = body[7 + 3 * k] & 15;
+        c.tq = body[8 + 3 * k];
+        if (c.tq > 3 || c.h < 1 || c.h > 4 || c.v < 1 || c.v > 4) return SQDET_JPEG_MALFORMED;
+      }
+      if (I.coded_height == 0 || I.coded_width == 0) return SQDET_JPEG_SIZE;
+      if (ncomp == 3) {
+        const int h = P.comp[0].h, v = P.comp[0].v;
+        const bool luma_ok = (h == 1 && v == 1) || (h == 2 && v == 1) || (h == 1 && v == 2) ||
+                             (h == 2 && v == 2) || (h == 4 && v == 1);
+        for (int k = 1; k < 3; ++k)
+          if (P.comp[k].h != 1 || P.comp[k].v != 1) return SQDET_JPEG_SAMPLING;
+        if (!luma_ok) return SQDET_JPEG_SAMPLING;
+      }
+      frame = true;
+    } else if (m == 0xDB) {
+      for (int j = 0; j < bn;) {
+        const int pq = body[j] >> 4, tq = body[j] & 15, size = pq ? 128 : 64;
+        if (pq > 1 || tq > 3 || j + 1 + size > bn) return SQDET_JPEG_MALFORMED;
+        for (int k = 0; k < 64; ++k)
+          P.qt[tq][kNatural[k]] = pq ? (uint16_t)u16(body, j + 1 + 2 * k) : body[j + 1 + k];
+        P.have_q[tq] = true;
+        j += 1 + size;
+      }
+    } else if (m == 0xC4) {
+      for (int j = 0; j < bn;) {
+        if (j + 17 > bn) return SQDET_JPEG_MALFORMED;
+        const int tc = body[j] >> 4, th = body[j] & 15;
+        int cnt = 0;
+        for (int l = 0; l < 16; ++l) cnt += body[j + 1 + l];
+        if (tc > 1 || th > 3 || cnt > 256 || j + 17 + cnt > bn) return SQDET_JPEG_MALFORMED;
+        memcpy(tc ? P.ac_bits[th] : P.dc_bits[th], body + j + 1, 16);
+        memcpy(tc ? P.ac_vals[th] : P.dc_vals[th], body + j + 17, (size_t)cnt);
+        (tc ? P.have_ac : P.have_dc)[th] = true;
+        j += 17 + cnt;
+      }
+    } else if (m == 0xDD) {
+      if (bn != 2) return SQDET_JPEG_MALFORMED;
+      I.restart_interval = u16(body, 0);
+    } else if (m == 0xE1 && !exif && bn >= 6 && memcmp(body, "Exif\0\0", 6) == 0) {
+      exif = true;
+      I.orientation = exif_orientation(body, bn);
+    } else if (m == 0xE0 && bn >= 14 && memcmp(body, "JFIF\0", 5) == 0) {
+      jfif = true;
+    } else if (m == 0xEE && bn >= 12 && memcmp(body, "Adobe", 5) == 0) {
+      adobe = body[11];
+    } else if (m == 0xDA) {
+      if (!frame || bn < 1) return SQDET_JPEG_MALFORMED;
+      const int ns = body[0];
+      if (bn != 4 + 2 * ns) return SQDET_JPEG_MALFORMED;
+      if (ns != ncomp) return SQDET_JPEG_SAMPLING;
+      for (int k = 0; k < ns; ++k) {
+        Comp& c = P.comp[k];
+        if (body[1 + 2 * k] != c.id) return SQDET_JPEG_SAMPLING;
+        c.td = body[2 + 2 * k] >> 4;
+        c.ta = body[2 + 2 * k] & 15;
+        if (c.td > 3 || c.ta > 3 || !P.have_dc[c.td] || !P.have_ac[c.ta] || !P.have_q[c.tq])
+          return SQDET_JPEG_MALFORMED;
+        if (!huff_ok(P.dc_bits[c.td], P.dc_vals[c.td], true) || !huff_ok(P.ac_bits[c.ta], P.ac_vals[c.ta], false))
+          return SQDET_JPEG_MALFORMED;
+      }
+      if (body[1 + 2 * ns] != 0 || body[2 + 2 * ns] != 63 || body[3 + 2 * ns] != 0)
+        return SQDET_JPEG_MALFORMED;
+      // libjpeg's colour space of 3 components: YCbCr after a JFIF APP0; else as an Adobe APP14's
+      // transform says (0: RGB); else RGB for component ids 'R', 'G', 'B'
+      if (ncomp == 3 && !jfif &&
+          (adobe >= 0 ? adobe == 0
+                      : P.comp[0].id == 'R' && P.comp[1].id == 'G' && P.comp[2].id == 'B'))
+        return SQDET_JPEG_COLOR_TRANSFORM;
+      I.scan_offset = i;
+      I.h_samp = P.comp[0].h;
+      I.v_samp = P.comp[0].v;
+      if (ncomp == 1) I.h_samp = I.v_samp = 1;
+      const bool swap = I.orientation >= 5;
+      I.height = swap ? I.coded_width : I.coded_height;
+      I.width = swap ? I.coded_height : I.coded_width;
+      I.supported = 1;
+      return SQDET_JPEG_OK;
+    }
+  }
+}
+
+void build_tab(const uint8_t* bits, const uint8_t* vals, HuffTab& t) {
+  memset(&t, 0, sizeof(t));
+  int code = 0, k = 0;
+  for (int l = 1; l <= 16; ++l) {
+    t.maxcode[l] = -1;
+    const int first_k = k, first_code = code;
+    for (int j = 0; j < bits[l - 1]; ++j) {
+      if (code < (1 << l)) {
+        if (l <= kFastBits) {
+          const int lo = code << (kFastBits - l), hi = (code + 1) << (kFastBits - l);
+          for (int e = lo; e < hi; ++e) t.fast[e] = (uint16_t)(l << 8 | vals[k]);
+        }
+        t.maxcode[l] = code;
+      }
+      ++code;
+      ++k;
+    }
+    t.valoff[l] = first_k - first_code;
+    code <<= 1;
+  }
+  memcpy(t.vals, vals, 256);
+}
+
+int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
+
+// One file's layout: sizes that follow from its headers alone.
+struct Layout {
+  int mcu_cols, mcu_rows, mcus, bpm, restart, intervals, chunks, blocks, sub_max;
+  int pw[3], ph[3];
+  int64_t raw_len;
+  int64_t staging;                       // this file's tables and raw bytes
+  int64_t marks, coef, rest;             // its scratch: set to 0xFF, zeroed, and the rest
+};
+
+Layout layout(const Parsed& P, int64_t file_len, int sub_bits) {
+  const sqdet_jpeg_info& I = P.info;
+  Layout L{};
+  const int H = I.coded_height, W = I.coded_width;
+  if (I.components == 1) {
+    L.mcu_cols = (W + 7) / 8;
+    L.mcu_rows = (H + 7) / 8;
+    L.bpm = 1;
+    L.pw[0] = L.mcu_cols * 8;
+    L.ph[0] = L.mcu_rows * 8;
+  } else {
+    const int hs = P.comp[0].h, vs = P.comp[0].v;
+    L.mcu_cols = (W + 8 * hs - 1) / (8 * hs);
+    L.mcu_rows = (H + 8 * vs - 1) / (8 * vs);
+    L.bpm = hs * vs + 2;
+    for (int c = 0; c < 3; ++c) {
+      L.pw[c] = L.mcu_cols * P.comp[c].h * 8;
+      L.ph[c] = L.mcu_rows * P.comp[c].v * 8;
+    }
+  }
+  L.mcus = L.mcu_cols * L.mcu_rows;
+  L.blocks = L.mcus * L.bpm;
+  L.restart = I.restart_interval ? std::min(I.restart_interval, L.mcus) : L.mcus;
+  L.intervals = (L.mcus + L.restart - 1) / L.restart;
+  L.raw_len = file_len - I.scan_offset;
+  L.chunks = (int)std::max<int64_t>(1, (L.raw_len + kChunk - 1) / kChunk);
+  L.sub_max = (int)((L.raw_len * 8 + sub_bits - 1) / sub_bits) + L.intervals;
+  L.staging = align256((int64_t)sizeof(HuffTab) * 6) + align256(L.raw_len + 16);
+  L.marks = 256 + align256((int64_t)(L.intervals + 1) * 4);          // terminator, ist
+  L.coef = align256((int64_t)L.blocks * 128);
+  int64_t s = 0;
+  s += align256((int64_t)(L.chunks + 1) * 8);                     // chunk sums
+  s += align256(L.raw_len + 16);                                  // clean stream, padded
+  s += align256((int64_t)(L.intervals + 1) * 4);                  // sbase
+  s += align256((int64_t)L.sub_max * 8) * 2;                      // entry, exit
+  s += align256((int64_t)L.sub_max * 16);                         // counts
+  for (int c = 0; c < I.components; ++c) s += align256((int64_t)L.pw[c] * L.ph[c]);
+  L.rest = s;
+  return L;
+}
+
+
+// The whole call: parsed files, their layouts and where everything goes.
+struct Plan {
+  std::vector<Parsed> parsed;
+  std::vector<Layout> lay;
+  int64_t staging = 0, scratch = 0;
+  int64_t marks = 0, marks_bytes = 0, coef = 0, coef_bytes = 0;
+};
+
+// Parses every file; a refusal names the first file refused.
+int make_plan(const std::string& name, int n, const uint8_t* const* files, const int64_t* lengths,
+              Plan& plan) {
+  if (!files || !lengths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (n < 1 || n > kMaxFiles)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxFiles) + "]");
+  plan.parsed.resize((size_t)n);
+  plan.lay.resize((size_t)n);
+  for (int i = 0; i < n; ++i) {
+    if (!files[i]) return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + " is null");
+    if (lengths[i] < 4 || lengths[i] > kMaxFileBytes)
+      return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + ": length must be in [4, 2^28]");
+    const int reason = parse(files[i], lengths[i], plan.parsed[(size_t)i]);
+    if (reason)
+      return fail(SQDET_ERR_UNSUPPORTED, name + ": file " + std::to_string(i) + " is not supported: " +
+                                             kReasons[reason]);
+    plan.lay[(size_t)i] = layout(plan.parsed[(size_t)i], lengths[i], g_sub_bits);
+  }
+  int64_t st = align256((int64_t)sizeof(DecFile) * n);
+  for (const Layout& L : plan.lay) st += L.staging;
+  plan.staging = st;
+  plan.marks = st;
+  for (const Layout& L : plan.lay) plan.marks_bytes += L.marks;
+  plan.coef = plan.marks + plan.marks_bytes;
+  for (const Layout& L : plan.lay) plan.coef_bytes += L.coef;
+  plan.scratch = plan.coef + plan.coef_bytes;
+  for (const Layout& L : plan.lay) plan.scratch += L.rest;
+  return SQDET_OK;
+}
+
+// Fills the staging (descriptors, tables, raw bytes) for outputs out/pitch.
+void fill_staging(const Plan& plan, int n, const uint8_t* const* files, uint8_t* const* out,
+                  const int64_t* pitch, uint8_t* stage) {
+  DecFile* fd = reinterpret_cast<DecFile*>(stage);
+  int64_t so = align256((int64_t)sizeof(DecFile) * n);   // staging cursor
+  int64_t mo = plan.marks, co = plan.coef, ro = plan.coef + plan.coef_bytes;
+  for (int i = 0; i < n; ++i) {
+    const Parsed& P = plan.parsed[(size_t)i];
+    const Layout& L = plan.lay[(size_t)i];
+    const sqdet_jpeg_info& I = P.info;
+    DecFile f;
+    memset(&f, 0, sizeof(f));
+    f.h = I.coded_height;
+    f.w = I.coded_width;
+    f.oh = I.height;
+    f.ow = I.width;
+    f.ncomp = I.components;
+    f.orient = I.orientation;
+    f.mcu_cols = L.mcu_cols;
+    f.mcus = L.mcus;
+    f.bpm = L.bpm;
+    f.restart = L.restart;
+    f.intervals = L.intervals;
+    f.raw_len = (int32_t)L.raw_len;
+    f.chunks = L.chunks;
+    f.blocks = L.blocks;
+    f.sub_max = L.sub_max;
+    f.sub_bits = g_sub_bits;
+    int u = 0;
+    for (int c = 0; c < I.components; ++c) {
+      const Comp& cp = P.comp[c];
+      const int hc = I.components == 1 ? 1 : cp.h, vc = I.components == 1 ? 1 : cp.v;
+      f.ch[c] = (int8_t)hc;
+      f.cv[c] = (int8_t)vc;
+      for (int by = 0; by < vc; ++by)
+        for (int bx = 0; bx < hc; ++bx, ++u) {
+          f.bcomp[u] = (int8_t)c;
+          f.bdy[u] = (int8_t)by;
+          f.bdx[u] = (int8_t)bx;
+        }
+      f.pw[c] = L.pw[c];
+      f.ph[c] = L.ph[c];
+      const int hmax = I.components == 1 ? 1 : P.comp[0].h, vmax = I.components == 1 ? 1 : P.comp[0].v;
+      f.cw[c] = (int)(((int64_t)f.w * hc + hmax - 1) / hmax);
+      f.chh[c] = (int)(((int64_t)f.h * vc + vmax - 1) / vmax);
+      for (int k = 0; k < 64; ++k) f.q[c][k] = (int16_t)P.qt[cp.tq][k];
+    }
+    // staging: tables, raw bytes (+16 zero bytes of padding)
+    f.tabs = so;
+    HuffTab* tabs = reinterpret_cast<HuffTab*>(stage + so);
+    for (int c = 0; c < I.components; ++c) {
+      build_tab(P.dc_bits[P.comp[c].td], P.dc_vals[P.comp[c].td], tabs[2 * c]);
+      build_tab(P.ac_bits[P.comp[c].ta], P.ac_vals[P.comp[c].ta], tabs[2 * c + 1]);
+    }
+    f.raw = so + align256((int64_t)sizeof(HuffTab) * 6);
+    memcpy(stage + f.raw, files[i] + I.scan_offset, (size_t)L.raw_len);
+    memset(stage + f.raw + L.raw_len, 0, 16);
+    so += L.staging;
+    // scratch
+    f.term = mo;
+    f.ist = mo + 256;
+    mo += L.marks;
+    f.coef = co;
+    co += L.coef;
+    f.sums = ro;
+    ro += align256((int64_t)(L.chunks + 1) * 8);
+    f.clean = ro;
+    ro += align256(L.raw_len + 16);
+    f.sbase = ro;
+    ro += align256((int64_t)(L.intervals + 1) * 4);
+    f.entry = ro;
+    ro += align256((int64_t)L.sub_max * 8);
+    f.exit_ = ro;
+    ro += align256((int64_t)L.sub_max * 8);
+    f.counts = ro;
+    ro += align256((int64_t)L.sub_max * 16);
+    for (int c = 0; c < I.components; ++c) {
+      f.plane[c] = ro;
+      ro += align256((int64_t)L.pw[c] * L.ph[c]);
+    }
+    f.out = out[i];
+    f.pitch = pitch[i];
+    fd[i] = f;
+  }
+}
+
+int launch_decode(const Plan& plan, int n, uint8_t* stage, uint8_t* scratch, int32_t* status,
+                  cudaStream_t stream) {
+  int max_chunks = 0, max_tiles = 0, max_blocks = 0;
+  int64_t max_pix = 0;
+  for (int i = 0; i < n; ++i) {
+    const Layout& L = plan.lay[(size_t)i];
+    const sqdet_jpeg_info& I = plan.parsed[(size_t)i].info;
+    max_chunks = std::max(max_chunks, L.chunks);
+    max_tiles = std::max(max_tiles, (L.sub_max + kTile - 1) / kTile);
+    max_blocks = std::max(max_blocks, L.blocks);
+    max_pix = std::max(max_pix, (int64_t)I.height * I.width);
+  }
+  SQ_CUDA(cudaMemcpyAsync(scratch, stage, (size_t)plan.staging, cudaMemcpyHostToDevice, stream));
+  SQ_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t) * (size_t)n, stream));
+  SQ_CUDA(cudaMemsetAsync(scratch + plan.marks, 0xFF, (size_t)plan.marks_bytes, stream));
+  SQ_CUDA(cudaMemsetAsync(scratch + plan.coef, 0, (size_t)plan.coef_bytes, stream));
+  DecParams p{reinterpret_cast<DecFile*>(scratch), scratch, status};
+  const unsigned un = (unsigned)n;
+  destuff_count_kernel<<<dim3((unsigned)max_chunks, un), kChunkThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg destuff_count_kernel");
+  scan_chunks_kernel<<<un, kScanThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg scan_chunks_kernel");
+  destuff_compact_kernel<<<dim3((unsigned)max_chunks, un), kChunkThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg destuff_compact_kernel");
+  intervals_kernel<<<un, kScanThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg intervals_kernel");
+  sync_tiles_kernel<<<dim3((unsigned)max_tiles, un), kTile, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg sync_tiles_kernel");
+  sync_chain_kernel<<<un, kTile, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg sync_chain_kernel");
+  scan_counts_kernel<<<un, kScanThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg scan_counts_kernel");
+  decode_write_kernel<<<dim3((unsigned)max_tiles, un), kTile, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg decode_write_kernel");
+  idct_kernel<<<dim3((unsigned)((max_blocks + kPixThreads - 1) / kPixThreads), un), kPixThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg idct_kernel");
+  color_kernel<<<dim3((unsigned)((max_pix + kPixThreads - 1) / kPixThreads), un), kPixThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg color_kernel");
+  return SQDET_OK;
+}
+
+}  // namespace
+}  // namespace sqdet
+
+using namespace sqdet;
+
+int sqdet_jpeg_parse(const uint8_t* file, int64_t len, sqdet_jpeg_info* out) {
+  if (!file || !out || len < 0) return fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_parse: bad argument");
+  Parsed P;
+  const int reason = parse(file, len, P);
+  P.info.reason = reason;
+  if (reason) P.info.supported = 0;
+  *out = P.info;
+  if (reason)
+    return fail(SQDET_ERR_UNSUPPORTED, std::string("sqdet_jpeg_parse: not supported: ") + kReasons[reason]);
+  return SQDET_OK;
+}
+
+int64_t sqdet_jpeg_decode_staging_bytes(int n, const uint8_t* const* files_host, const int64_t* lengths) {
+  Plan plan;
+  if (make_plan("sqdet_jpeg_decode_staging_bytes", n, files_host, lengths, plan)) return -1;
+  return plan.staging;
+}
+
+int64_t sqdet_jpeg_decode_scratch_bytes(int n, const uint8_t* const* files_host, const int64_t* lengths) {
+  Plan plan;
+  if (make_plan("sqdet_jpeg_decode_scratch_bytes", n, files_host, lengths, plan)) return -1;
+  return plan.scratch;
+}
+
+int sqdet_jpeg_decode_set_subsequence_bits(int bits) {
+  if (bits == 0) bits = kDefaultSubBits;
+  if (bits < 32 || bits > 8192 || bits % 32)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_decode_set_subsequence_bits: bits must be a multiple of 32 in [32, 8192]");
+  g_sub_bits = bits;
+  return SQDET_OK;
+}
+
+int sqdet_decode_jpeg(int n, const uint8_t* const* files_host, const int64_t* lengths,
+                      uint8_t* const* out_planes, const int64_t* out_pitches, void* staging_pinned,
+                      int64_t staging_bytes, void* scratch_dev, int64_t scratch_bytes,
+                      int32_t* status_dev, void* stream) {
+  const std::string name = "sqdet_decode_jpeg";
+  if (!out_planes || !out_pitches || !staging_pinned || !scratch_dev || !status_dev)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  Plan plan;
+  int rc = make_plan(name, n, files_host, lengths, plan);
+  if (rc) return rc;
+  if ((uintptr_t)scratch_dev % 256) return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
+  if ((uintptr_t)status_dev % alignof(int32_t))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": status_dev must be 4-byte aligned");
+  if (staging_bytes < plan.staging)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": staging_bytes is below sqdet_jpeg_decode_staging_bytes");
+  if (scratch_bytes < plan.scratch)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below sqdet_jpeg_decode_scratch_bytes");
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, staging_pinned) != cudaSuccess || attr.type != cudaMemoryTypeHost) {
+    (void)cudaGetLastError();
+    return fail(SQDET_ERR_INVALID_ARG, name + ": staging_pinned is not page-locked host memory");
+  }
+  int device = -1;
+  if (!out_planes[0]) return fail(SQDET_ERR_INVALID_ARG, name + ": output 0 is null");
+  if (cudaPointerGetAttributes(&attr, out_planes[0]) == cudaSuccess && attr.type == cudaMemoryTypeDevice)
+    device = attr.device;
+  else
+    (void)cudaGetLastError();
+  if (device < 0) return fail(SQDET_ERR_INVALID_ARG, name + ": output 0 is not device memory");
+  for (int i = 0; i < n; ++i) {
+    const sqdet_jpeg_info& I = plan.parsed[(size_t)i].info;
+    const std::string which = name + ": output " + std::to_string(i);
+    if (!out_planes[i]) return fail(SQDET_ERR_INVALID_ARG, which + " is null");
+    if (out_pitches[i] < 3 * (int64_t)I.width) return fail(SQDET_ERR_INVALID_ARG, which + ": pitch below 3 * width");
+    const int64_t bytes = (int64_t)(I.height - 1) * out_pitches[i] + 3 * (int64_t)I.width;
+    if (!device_range_ok(out_planes[i], bytes, device))
+      return fail(SQDET_ERR_INVALID_ARG, which + " is not inside one device allocation on output 0's device");
+  }
+  if (!device_range_ok(reinterpret_cast<const uint8_t*>(status_dev), (int64_t)n * 4, device) ||
+      !device_range_ok(static_cast<const uint8_t*>(scratch_dev), scratch_bytes, device))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": status_dev or scratch_dev is not inside one device "
+                                              "allocation on output 0's device");
+  fill_staging(plan, n, files_host, out_planes, out_pitches, static_cast<uint8_t*>(staging_pinned));
+  int prev = -1;
+  if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(device) != cudaSuccess)
+    return fail(SQDET_ERR_CUDA, "cannot select output 0's device");
+  rc = launch_decode(plan, n, static_cast<uint8_t*>(staging_pinned), static_cast<uint8_t*>(scratch_dev),
+                     status_dev, (cudaStream_t)stream);
+  cudaSetDevice(prev);
+  return rc;
+}

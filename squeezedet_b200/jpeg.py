@@ -105,3 +105,109 @@ def jpeg_bytes(data, lengths, stream=None):
         raise ValueError('frame %d: the file did not fit the output capacity' % i)
       out.append(data[i, :n].cpu().numpy().tobytes())
   return out
+
+
+# ---- decoding ------------------------------------------------------------------------------------
+def jpeg_info(file_bytes):
+  """sqdet_jpeg_parse of one file -> dict: height and width of the decoded frame (after the EXIF
+  orientation), coded_height, coded_width, components, h_samp, v_samp (luma sampling),
+  orientation, restart_interval, supported (bool), reason (a SQDET_JPEG_* code) and reason_text
+  (the library's words for it).  Host only."""
+  b = bytes(file_bytes)
+  info = _lib.JpegInfo()
+  buf = C.create_string_buffer(b, len(b))
+  lib = _lib.load()
+  rc = lib.sqdet_jpeg_parse(buf, len(b), C.byref(info))
+  if rc not in (_lib.OK, -3):
+    _lib.check(rc)
+  out = {k: int(getattr(info, k)) for k, _ in _lib.JpegInfo._fields_ if k != 'reserved'}
+  out['supported'] = bool(out['supported'])
+  out['reason_text'] = 'ok' if rc == _lib.OK else \
+      lib.sqdet_last_error().decode('utf-8', 'replace').split('not supported: ', 1)[-1]
+  return out
+
+
+class _Staging:
+  """Two pinned host staging buffers used in turn, each with the event recorded after the call
+  that last read it.  A call waits (on the host) only for the call before the previous one, so it
+  packs its files while the previous call's decode runs."""
+
+  def __init__(self):
+    self.bufs = [None, None]
+    self.events = [None, None]
+    self.turn = 0
+
+  def get(self, nbytes):
+    """-> (slot, buffer of at least nbytes), free to write."""
+    import torch
+    k = self.turn
+    self.turn ^= 1
+    if self.events[k] is not None:
+      self.events[k].synchronize()
+    if self.bufs[k] is None or self.bufs[k].numel() < nbytes:
+      self.bufs[k] = torch.empty((max(nbytes, 1 << 20),), dtype=torch.uint8, pin_memory=True)
+    return k, self.bufs[k]
+
+
+_staging = {}
+
+
+def decode_jpeg_device(files, device, stream=None):
+  """JPEG files (bytes-like, on the host) -> (frames, status): frames[i] is a uint8 [H, W, 3] BGR
+  CUDA tensor on `device` with exactly the pixels of cv2.imdecode(files[i], cv2.IMREAD_COLOR), and
+  status an int32 [n] CUDA tensor, 0 where the file decoded and negative where its entropy-coded
+  data is corrupt (that frame's pixels are then unspecified; the others are unaffected).
+
+  Decoded are baseline and extended sequential Huffman files with 8-bit samples, 1 or 3
+  components and 4:4:4, 4:2:2, 4:4:0, 4:2:0 or 4:1:1 sampling, with or without restart markers;
+  the EXIF orientation is applied.  ValueError, naming the file's index, for any other file
+  (progressive, arithmetic, 12-bit, CMYK, ...): route those to cv2.imdecode.  1 to 128 files.
+
+  Asynchronous on `stream` (a torch.cuda.Stream, a raw cudaStream_t, or None for torch's current
+  stream): the frames, status and scratch are allocated on it, so read them on it or after
+  synchronising it.  The files go to the device through two pinned staging buffers this module
+  owns per device and uses in turn; a call waits (on the host) only until the call before the
+  previous one has finished on its stream."""
+  import torch
+  files = [bytes(f) for f in files]
+  n = len(files)
+  if not 1 <= n <= 128:
+    raise ValueError('need 1 to 128 files, got %d' % n)
+  device = torch.device(device)
+  if device.type != 'cuda':
+    raise ValueError('device must be a CUDA device, got %s' % (device,))
+  if device.index is None:
+    device = torch.device('cuda', torch.cuda.current_device())
+  infos = []
+  for i, f in enumerate(files):
+    if len(f) < 4:
+      raise ValueError('file %d: not a JPEG file (%d bytes)' % (i, len(f)))
+    info = jpeg_info(f)
+    if not info['supported']:
+      raise ValueError('file %d: not supported (%s); decode it with cv2.imdecode'
+                       % (i, info['reason_text']))
+    infos.append(info)
+  lib = _lib.load()
+  bufs = [C.create_string_buffer(f, len(f)) for f in files]
+  ptrs = (C.c_void_p * n)(*[C.addressof(b) for b in bufs])
+  lens = (C.c_int64 * n)(*[len(f) for f in files])
+  staging_bytes = lib.sqdet_jpeg_decode_staging_bytes(n, ptrs, lens)
+  scratch_bytes = lib.sqdet_jpeg_decode_scratch_bytes(n, ptrs, lens)
+  if staging_bytes < 0 or scratch_bytes < 0:
+    raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
+  s = _torch_stream(stream, device)
+  staging = _staging.setdefault(device.index, _Staging())
+  slot, buf = staging.get(staging_bytes)
+  with torch.cuda.device(device), torch.cuda.stream(s):
+    frames = [torch.empty((info['height'], info['width'], 3), dtype=torch.uint8, device=device)
+              for info in infos]
+    status = torch.empty((n,), dtype=torch.int32, device=device)
+    scratch = torch.empty((scratch_bytes,), dtype=torch.uint8, device=device)
+    outs = (C.c_void_p * n)(*[t.data_ptr() for t in frames])
+    pitches = (C.c_int64 * n)(*[3 * t.shape[1] for t in frames])
+    _lib.check(lib.sqdet_decode_jpeg(n, ptrs, lens, outs, pitches, buf.data_ptr(), buf.numel(),
+                                     scratch.data_ptr(), scratch_bytes, status.data_ptr(),
+                                     s.cuda_stream))
+    staging.events[slot] = torch.cuda.Event()
+    staging.events[slot].record(s)
+  return frames, status
