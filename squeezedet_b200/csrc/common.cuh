@@ -2,7 +2,9 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <functional>
 #include <string>
+#include <vector>
 #include "../../include/sqdet_b200.h"
 
 namespace sqdet {
@@ -71,6 +73,7 @@ int launch_maxpool(const float* x, float* y, int B, int H, int W, int C, int siz
 // (y >> y_shift) * pitch + (x >> x_shift) * bytes_per_px bytes into it.
 struct PixPlane {
   int bytes_per_px, x_shift, y_shift;
+  int64_t row_bytes(int64_t w) const { return (w >> x_shift) * bytes_per_px; }
 };
 struct PixFormat {
   int planes;
@@ -96,36 +99,46 @@ struct FrameSource {
 int launch_resize_meansub_frames(int format, const FrameSource* frames, int n, float* dst, int H,
                                  int W, const double* means, int sub_first, float* scales_xy,
                                  cudaStream_t stream);
-// sqdet_draw_dets' style as its kernel takes it, by value: per class the colour (B, G, R and its
-// (Y, U, V) for 4:2:0 frames) and the name, plus the threshold and cvRound(font_scale * 65536).
-constexpr int kDrawMaxClasses = 64;
-constexpr int kDrawMaxName = 31;
-constexpr int kMaxDrawFrames = 128;     // frames per sqdet_draw_dets call
-struct DrawStyle {
-  int64_t hscale;
-  float thresh;
-  int classes;
-  uint8_t bgr[kDrawMaxClasses][3];
-  uint8_t yuv[kDrawMaxClasses][3];
-  uint8_t name_len[kDrawMaxClasses];
-  char name[kDrawMaxClasses][kDrawMaxName];
+
+// ---- frames and buffers the caller passes in device memory (frames.cu) -------------------------
+// Hidden: the library exports the sqdet_* C ABI, not these.
+#pragma GCC visibility push(hidden)
+// Makes `dev` the current device for the guard's scope; ok is false when that failed.
+struct DeviceGuard {
+  int prev = -1;
+  bool ok = true;
+  explicit DeviceGuard(int dev) {
+    if (cudaGetDevice(&prev) != cudaSuccess) { ok = false; return; }
+    if (prev != dev && cudaSetDevice(dev) != cudaSuccess) ok = false;
+  }
+  ~DeviceGuard() {
+    if (prev >= 0) cudaSetDevice(prev);
+  }
 };
-// Frames per draw launch: their descriptors and the style stay inside the classic 4 KiB parameter
-// block.
-constexpr int kDrawFramesPerLaunch = 24;
-// Draws frame i's records dets[i * max_dets + k], k < min(counts[i], max_dets), on the crop of
-// frames[i] (FrameSource: planes, pitches, canvas = the h x w crop at (x, y)), one CTA per frame,
-// one launch per kDrawFramesPerLaunch frames.  The frames' checks are the caller's.
-int launch_draw_dets(int format, const FrameSource* frames, int n, const sqdet_det* dets,
-                     const int32_t* counts, int max_dets, const DrawStyle& style,
-                     cudaStream_t stream);
-// sqdet_encode_jpeg: frames per call, the largest file of an h x w crop, the scratch of the crops
-// of `frames`, and the encode of their crops (the frames' checks are the caller's).
-constexpr int kMaxJpegFrames = 128;
-int64_t jpeg_max_bytes(int h, int w);
-int64_t jpeg_scratch_bytes(const FrameSource* frames, int n);
-int launch_encode_jpeg(int format, const FrameSource* frames, int n, int quality, uint8_t* out,
-                       int64_t cap, int64_t* lengths, void* scratch, cudaStream_t stream);
+// The device whose memory p points into, or -1 when it is not device memory.
+int pointer_device(const void* p);
+// True when the `bytes` bytes at p are device memory of `device` inside one allocation.  The
+// pointer comes from outside the program: a host pointer or an overlong buffer is refused here
+// rather than faulting a kernel.
+bool device_range_ok(const void* p, int64_t bytes, int device);
+// The crop r = (x, y, w, h) of an H x W frame, or the whole frame when r is null, into s.x, s.y,
+// s.w and s.h; refuses an empty crop or one outside the frame, naming `which`.
+int check_crop(const std::string& which, int64_t H, int64_t W, const int32_t* r, FrameSource& s);
+// accept_frames' device: the one plane 0 of frame 0 is on.
+constexpr int kFrame0Device = -1;
+// Every check of n frames in format pf before any device work, filling fr or refusing with a
+// message that names the call and image(i) (by default "frame i").  Frame i is heights[i] x
+// widths[i], its plane p at planes[3i + p] with row pitch pitches[3i + p] (tight rows when
+// pitches is null), cropped to crops[4i .. 4i + 3] (the whole frame when crops is null).  Every
+// plane must be inside one device allocation on *device (an engine's, as refusals call it), or
+// with kFrame0Device on the device plane 0 of frame 0 is on, which *device then holds.
+int accept_frames(const std::string& name, const PixFormat& pf, int n,
+                  const uint8_t* const* planes, const int64_t* pitches, const int32_t* heights,
+                  const int32_t* widths, const int32_t* crops,
+                  const std::function<std::string(int)>& image, int* device,
+                  std::vector<FrameSource>& fr);
+#pragma GCC visibility pop
+
 int launch_add_relu(const float* a, const float* b, float* y, int64_t n, cudaStream_t stream);
 
 int launch_interpret(const float* preds, const float* anchors, float* boxes, float* probs,

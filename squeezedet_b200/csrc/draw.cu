@@ -12,7 +12,9 @@
 // later record overwrites an earlier one exactly as the sequential cv2 calls do.  Within a record
 // every pixel takes the same colour, so threads split its rectangle pixels and stroke segments
 // freely.
+#include <math.h>
 #include <stdint.h>
+#include <string.h>
 #include "common.cuh"
 
 #define SQDET_HERSHEY_SPACE __constant__
@@ -21,6 +23,23 @@
 namespace sqdet {
 namespace {
 
+// sqdet_draw_dets' style as its kernel takes it, by value: per class the colour (B, G, R and its
+// (Y, U, V) for 4:2:0 frames) and the name, plus the threshold and cvRound(font_scale * 65536).
+constexpr int kDrawMaxClasses = 64;
+constexpr int kDrawMaxName = 31;
+constexpr int kMaxDrawFrames = 128;     // frames per sqdet_draw_dets call
+struct DrawStyle {
+  int64_t hscale;
+  float thresh;
+  int classes;
+  uint8_t bgr[kDrawMaxClasses][3];
+  uint8_t yuv[kDrawMaxClasses][3];
+  uint8_t name_len[kDrawMaxClasses];
+  char name[kDrawMaxClasses][kDrawMaxName];
+};
+// Frames per draw launch: their descriptors and the style stay inside the classic 4 KiB parameter
+// block.
+constexpr int kDrawFramesPerLaunch = 24;
 constexpr int kDrawThreads = 256;
 constexpr int kMaxLabel = kDrawMaxName + 9;   // name + ": (" + "-0.00" + ")"
 
@@ -298,8 +317,9 @@ int launch_format(const FrameSource* frames, int n, const sqdet_det* dets, const
   return SQDET_OK;
 }
 
-}  // namespace
-
+// Draws frame i's records dets[i * max_dets + k], k < min(counts[i], max_dets), on the crop of
+// frames[i] (FrameSource: planes, pitches, canvas = the h x w crop at (x, y)), one CTA per frame,
+// one launch per kDrawFramesPerLaunch frames.  The frames' checks are the caller's.
 int launch_draw_dets(int format, const FrameSource* frames, int n, const sqdet_det* dets,
                      const int32_t* counts, int max_dets, const DrawStyle& style,
                      cudaStream_t stream) {
@@ -316,4 +336,66 @@ int launch_draw_dets(int format, const FrameSource* frames, int n, const sqdet_d
   }
 }
 
+}  // namespace
 }  // namespace sqdet
+
+using namespace sqdet;
+
+int sqdet_draw_dets(int n, int format, uint8_t* const* planes, const int64_t* pitches,
+                    const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                    const sqdet_det* dets_dev, const int32_t* counts_dev, int max_dets,
+                    const sqdet_draw_style* style, void* stream) {
+  const std::string name = "sqdet_draw_dets";
+  const PixFormat* pf = pix_format(format);
+  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
+  if (!planes || !heights || !widths || !dets_dev || !counts_dev || !style || !style->class_names ||
+      !style->class_bgr)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (n < 1 || n > kMaxDrawFrames)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxDrawFrames) + "]");
+  if (max_dets < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": max_dets must be at least 1");
+  if (style->classes < 1 || style->classes > kDrawMaxClasses)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": classes must be in [1, " + std::to_string(kDrawMaxClasses) + "]");
+  const float fs = style->font_scale;
+  if (!(fs > 0.f && fs <= 1024.f))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": font_scale must be finite, positive and at most 1024");
+  DrawStyle st = {};
+  st.hscale = (int64_t)nearbyint((double)fs * 65536.0);   // cvRound: half to even
+  st.thresh = style->plot_prob_thresh;
+  st.classes = style->classes;
+  for (int c = 0; c < st.classes; ++c) {
+    const char* s = style->class_names[c];
+    const size_t len = s ? strnlen(s, kDrawMaxName + 1) : kDrawMaxName + 1;
+    bool printable = len <= (size_t)kDrawMaxName;
+    for (size_t i = 0; printable && i < len; ++i) printable = s[i] >= 32 && s[i] <= 126;
+    if (!printable)
+      return fail(SQDET_ERR_INVALID_ARG, name + ": class name " + std::to_string(c) +
+                                             " is not printable ASCII of at most " +
+                                             std::to_string(kDrawMaxName) + " characters");
+    memcpy(st.name[c], s, len);
+    st.name_len[c] = (uint8_t)len;
+    const int b = style->class_bgr[3 * c], g = style->class_bgr[3 * c + 1], r = style->class_bgr[3 * c + 2];
+    st.bgr[c][0] = (uint8_t)b;
+    st.bgr[c][1] = (uint8_t)g;
+    st.bgr[c][2] = (uint8_t)r;
+    // cv2.cvtColor(solid BGR patch, COLOR_BGR2YUV_I420): OpenCV's BT.601 coefficients, 20 bits
+    const int half = 1 << 19;
+    st.yuv[c][0] = (uint8_t)((269484 * r + 528482 * g + 102760 * b + (16 << 20) + half) >> 20);
+    st.yuv[c][1] = (uint8_t)((-155188 * r - 305135 * g + 460324 * b + (128 << 20) + half) >> 20);
+    st.yuv[c][2] = (uint8_t)((460324 * r - 385875 * g - 74448 * b + (128 << 20) + half) >> 20);
+  }
+  // the device the call runs on is the one frame 0's first plane lives on, whatever is current
+  std::vector<FrameSource> fr;
+  int device = kFrame0Device;
+  const int rc = accept_frames(name, *pf, n, planes, pitches, heights, widths, crops, nullptr,
+                               &device, fr);
+  if (rc) return rc;
+  if (!device_range_ok(dets_dev, (int64_t)n * max_dets * (int64_t)sizeof(sqdet_det), device) ||
+      !device_range_ok(counts_dev, (int64_t)n * sizeof(int32_t), device))
+    return fail(SQDET_ERR_INVALID_ARG,
+                name + ": dets_dev or counts_dev is not inside one device allocation on frame 0's device");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
+  return launch_draw_dets(format, fr.data(), n, dets_dev, counts_dev, max_dets, st,
+                          (cudaStream_t)stream);
+}

@@ -8,7 +8,6 @@
 // weight storage in HBM, BN folding to (scale, shift), kernel selection per op
 // (wgmma 3xTF32 implicit GEMM or fp32 SIMT), CUDA-graph capture of the whole forward,
 // and the fused post-processing.
-#include <cuda.h>
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <math.h>
@@ -176,18 +175,6 @@ struct sqdet_engine {
 };
 
 namespace sqdet {
-
-struct DeviceGuard {
-  int prev = -1;
-  bool ok = true;
-  explicit DeviceGuard(int dev) {
-    if (cudaGetDevice(&prev) != cudaSuccess) { ok = false; return; }
-    if (prev != dev && cudaSetDevice(dev) != cudaSuccess) ok = false;
-  }
-  ~DeviceGuard() {
-    if (prev >= 0) cudaSetDevice(prev);
-  }
-};
 
 static int add_param(sqdet_engine* e, const std::string& name, std::vector<int64_t> shape) {
   auto it = e->param_index.find(name);
@@ -1337,33 +1324,6 @@ int sqdet_submit_frames_n(sqdet_engine* e, int n, const uint8_t* const* frames,
 }
 
 // ---- variable-size uint8 frames already in device memory ----------------------------------------
-using MemGetAddressRangeFn = CUresult (*)(CUdeviceptr*, size_t*, CUdeviceptr);
-
-// True when the `bytes` bytes at p are device memory of `device` inside one allocation.  The
-// pointer comes from outside the program: a host pointer or an overlong frame is refused here
-// rather than faulting the resize kernel.  jpeg_decode.cu checks its outputs with it too.
-bool device_range_ok(const uint8_t* p, int64_t bytes, int device) {
-  static MemGetAddressRangeFn range = [] {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      fn = nullptr;
-    return reinterpret_cast<MemGetAddressRangeFn>(fn);
-  }();
-  cudaPointerAttributes attr;
-  if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) {
-    (void)cudaGetLastError();      // an unknown pointer: no stale error for the next launch check
-    return false;
-  }
-  if (attr.type != cudaMemoryTypeDevice || attr.device != device || !range) return false;
-  CUdeviceptr base = 0;
-  size_t size = 0;
-  if (range(&base, &size, (CUdeviceptr)(uintptr_t)p) != CUDA_SUCCESS) return false;
-  const uint64_t off = (uint64_t)(uintptr_t)p - (uint64_t)base;
-  return off <= size && (uint64_t)bytes <= size - off;
-}
-
 // Before the resize launch of a device-frames forward: the weights first, since their upload waits
 // for the forwards in flight and the resize must not be left behind a failed one; then, with
 // rescale, the box-scale table the launch writes, at *scales (null without rescale).
@@ -1376,113 +1336,41 @@ static int prepare_frames(sqdet_engine* e, int rescale, float** scales) {
   return SQDET_OK;
 }
 
-// Where the planes of sqdet_forward_frames' frames are: plane p of frame i at
-// ptr[p][i * stride], its row pitch at pitch[p][i * stride] (tight rows when pitch[p] is null).
-struct FramePlanes {
-  const uint8_t* const* ptr[3];
-  const int64_t* pitch[3];
-  int stride;
-};
-
-// The per-frame checks of sqdet_forward_frames and sqdet_draw_dets against the format's pix_format
-// layout, before any device work: fills fr[i] (planes, pitches, crop) or refuses, naming image(i).
-static int check_frames(const std::string& name, const PixFormat* pf, int n, const FramePlanes& pl,
-                        const int32_t* heights, const int32_t* widths, const int32_t* crops,
-                        const std::function<std::string(int)>& image, std::vector<FrameSource>& fr) {
-  auto row_bytes = [&](int64_t W, int p) {
-    return (W >> pf->plane[p].x_shift) * pf->plane[p].bytes_per_px;
-  };
-  fr.assign((size_t)n, FrameSource{});
-  for (int i = 0; i < n; ++i) {
-    const int64_t H = heights[i], W = widths[i];
-    const std::string which = name + ": " + image(i);
-    FrameSource& s = fr[(size_t)i];
-    for (int p = 0; p < pf->planes; ++p) {
-      s.plane[p] = pl.ptr[p][(size_t)i * pl.stride];
-      if (!s.plane[p])
-        return fail(SQDET_ERR_INVALID_ARG, which + (pf->planes == 1 ? " is a null pointer" : " has a null plane"));
-    }
-    if (!pf->even && (H <= 0 || W <= 0)) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
-    if (pf->even && (H <= 0 || W <= 0 || H % 2 || W % 2))
-      return fail(SQDET_ERR_INVALID_ARG, which + ": height and width must be positive and even");
-    for (int p = 0; p < pf->planes; ++p) {
-      s.pitch[p] = pl.pitch[p] ? pl.pitch[p][(size_t)i * pl.stride] : row_bytes(W, p);
-      if (s.pitch[p] < row_bytes(W, p))
-        return fail(SQDET_ERR_INVALID_ARG, which + ": row pitch below " + pf->least_pitch);
-    }
-    const int32_t* r = crops ? crops + 4 * i : nullptr;
-    if (r) {
-      const int64_t x = r[0], y = r[1], w = r[2], h = r[3];
-      if (w <= 0 || h <= 0) return fail(SQDET_ERR_INVALID_ARG, which + ": empty crop");
-      if (x < 0 || y < 0 || x + w > W || y + h > H)
-        return fail(SQDET_ERR_INVALID_ARG, which + ": crop outside the frame");
-    }
-    s.x = r ? r[0] : 0;
-    s.y = r ? r[1] : 0;
-    s.w = r ? r[2] : (int)W;
-    s.h = r ? r[3] : (int)H;
-  }
-  return SQDET_OK;
-}
-
-// Every plane of the checked frames fr is device memory of `device` (`where` names it) inside one
-// allocation.
-static int check_frame_memory(const std::string& name, const PixFormat* pf, int n,
-                              const int32_t* heights, const int32_t* widths,
-                              const std::vector<FrameSource>& fr, int device, const char* where,
-                              const std::function<std::string(int)>& image) {
-  for (int i = 0; i < n; ++i) {
-    const FrameSource& s = fr[(size_t)i];
-    const int64_t H = heights[i], W = widths[i];
-    for (int p = 0; p < pf->planes; ++p) {
-      // the plane's bytes end at (rows - 1) * pitch + row bytes; refused when that overflows int64
-      const int64_t k = H >> pf->plane[p].y_shift;
-      const int64_t b = (W >> pf->plane[p].x_shift) * pf->plane[p].bytes_per_px;
-      const bool fits = k == 1 || s.pitch[p] <= (INT64_MAX - b) / (k - 1);
-      if (!fits || !device_range_ok(s.plane[p], (k - 1) * s.pitch[p] + b, device))
-        return fail(SQDET_ERR_INVALID_ARG,
-                    name + ": " + image(i) +
-                        (pf->planes == 1 ? " is not inside" : ": a plane is not inside") +
-                        " one device allocation on " + where);
-    }
-  }
-  return SQDET_OK;
-}
-
-// sqdet_forward_frames and the two calls that are it for one format; `what` names the call in
-// refusals.  Every check is driven by the format's pix_format layout.  With `tile_frames`
-// (sqdet_forward_tiles) image i is tile i of frame tile_frames[i], and refusals name both.
-static int forward_frames(sqdet_engine* e, const char* what, int n, int format,
-                          const FramePlanes& pl, const int32_t* heights, const int32_t* widths,
-                          const int32_t* crops, int order, int rescale, void* stream_v,
-                          const int32_t* tile_frames = nullptr) {
-  const std::string name = what;
-  const PixFormat* pf = pix_format(format);
-  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
-  bool null_array = !e || !heights || !widths;
-  for (int p = 0; p < pf->planes; ++p) null_array = null_array || !pl.ptr[p];
-  if (null_array) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+// The refusals of a device-frames forward before it reads any per-frame entry; null_arg: the engine
+// or an array the call needs is null.
+static int check_frames_call(sqdet_engine* e, const std::string& name, bool null_arg, int n,
+                             int order) {
+  if (null_arg) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
   if (!e->finalized) return fail(SQDET_ERR_STATE, name + " before sqdet_finalize");
-  const sqdet_config& c = e->cfg;
-  if (n < 1 || n > c.batch_size)
+  if (n < 1 || n > e->cfg.batch_size)
     return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, batch_size]");
   if (order != SQDET_PRE_RESIZE_THEN_SUB && order != SQDET_PRE_SUB_THEN_RESIZE)
     return fail(SQDET_ERR_INVALID_ARG, name + ": order must be 0 (demo) or 1 (eval)");
-  auto image = [&](int i) {
-    return tile_frames ? "tile " + std::to_string(i) + " (frame " + std::to_string(tile_frames[i]) + ")"
-                       : "frame " + std::to_string(i);
-  };
-  std::vector<FrameSource> fr;
-  int rc = check_frames(name, pf, n, pl, heights, widths, crops, image, fr);
+  return SQDET_OK;
+}
+
+// sqdet_forward_frames, whose refusals name the call `name` and image i as image(i) (by default
+// "frame i").
+static int forward_frames(sqdet_engine* e, const std::string& name, int n, int format,
+                          const uint8_t* const* planes, const int64_t* pitches,
+                          const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                          int order, int rescale, void* stream_v,
+                          const std::function<std::string(int)>& image = nullptr) {
+  const PixFormat* pf = pix_format(format);
+  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
+  int rc = check_frames_call(e, name, !e || !planes || !heights || !widths, n, order);
   if (rc) return rc;
   DeviceGuard guard(e->device);
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
-  rc = check_frame_memory(name, pf, n, heights, widths, fr, e->device, "the engine's device", image);
+  std::vector<FrameSource> fr;
+  int device = e->device;
+  rc = accept_frames(name, *pf, n, planes, pitches, heights, widths, crops, image, &device, fr);
   if (rc) return rc;
   cudaStream_t stream = (cudaStream_t)stream_v;
   float* scales = nullptr;
   rc = prepare_frames(e, rescale, &scales);
   if (rc) return rc;
+  const sqdet_config& c = e->cfg;
   Tensor& t0 = e->tensors[0];
   rc = launch_resize_meansub_frames(format, fr.data(), n, t0.dev, c.image_height, c.image_width,
                                     e->bgr_means, order == SQDET_PRE_SUB_THEN_RESIZE, scales,
@@ -1491,22 +1379,43 @@ static int forward_frames(sqdet_engine* e, const char* what, int n, int format,
   return forward_impl(e, t0.dev, false, n, scales, stream);
 }
 
+// sqdet_forward_frames_u8 and _nv12, which pass plane p of frame i at planes[p][i] and its row
+// pitch at pitches[p][i] (tight rows when pitches[p] is null): once the arrays are known to hold n
+// entries, they are laid out as sqdet_forward_frames takes them.
+static int forward_plane_arrays(sqdet_engine* e, const std::string& name, int n, int format,
+                                const uint8_t* const* const (&planes)[2],
+                                const int64_t* const (&pitches)[2], const int32_t* heights,
+                                const int32_t* widths, const int32_t* crops, int order,
+                                int rescale, void* stream) {
+  const PixFormat& pf = *pix_format(format);
+  bool null_arg = !e || !heights || !widths;
+  for (int p = 0; p < pf.planes; ++p) null_arg = null_arg || !planes[p];
+  const int rc = check_frames_call(e, name, null_arg, n, order);
+  if (rc) return rc;
+  std::vector<const uint8_t*> fp(3 * (size_t)n);
+  std::vector<int64_t> fq(3 * (size_t)n);
+  for (int i = 0; i < n; ++i)
+    for (int p = 0; p < pf.planes; ++p) {
+      fp[3 * (size_t)i + p] = planes[p][i];
+      fq[3 * (size_t)i + p] = pitches[p] ? pitches[p][i] : pf.plane[p].row_bytes(widths[i]);
+    }
+  return forward_frames(e, name, n, format, fp.data(), fq.data(), heights, widths, crops, order,
+                        rescale, stream);
+}
+
 int sqdet_forward_frames(sqdet_engine* e, int n, int format, const uint8_t* const* planes,
                          const int64_t* pitches, const int32_t* heights, const int32_t* widths,
                          const int32_t* crops, int order, int rescale, void* stream) {
-  const FramePlanes pl = {{planes, planes ? planes + 1 : nullptr, planes ? planes + 2 : nullptr},
-                          {pitches, pitches ? pitches + 1 : nullptr, pitches ? pitches + 2 : nullptr},
-                          3};
-  return forward_frames(e, "sqdet_forward_frames", n, format, pl, heights, widths, crops, order,
-                        rescale, stream);
+  return forward_frames(e, "sqdet_forward_frames", n, format, planes, pitches, heights, widths,
+                        crops, order, rescale, stream);
 }
 
 int sqdet_forward_frames_u8(sqdet_engine* e, int n, const uint8_t* const* frames_dev,
                             const int32_t* heights, const int32_t* widths,
                             const int64_t* row_pitches, int order, int rescale, void* stream) {
-  const FramePlanes pl = {{frames_dev, nullptr, nullptr}, {row_pitches, nullptr, nullptr}, 1};
-  return forward_frames(e, "sqdet_forward_frames_u8", n, SQDET_FMT_BGR, pl, heights, widths,
-                        nullptr, order, rescale, stream);
+  return forward_plane_arrays(e, "sqdet_forward_frames_u8", n, SQDET_FMT_BGR, {frames_dev, nullptr},
+                              {row_pitches, nullptr}, heights, widths, nullptr, order, rescale,
+                              stream);
 }
 
 int sqdet_forward_frames_nv12(sqdet_engine* e, int n, const uint8_t* const* luma_dev,
@@ -1514,9 +1423,9 @@ int sqdet_forward_frames_nv12(sqdet_engine* e, int n, const uint8_t* const* luma
                               const int64_t* chroma_pitches, const int32_t* heights,
                               const int32_t* widths, const int32_t* crops, int order, int rescale,
                               void* stream) {
-  const FramePlanes pl = {{luma_dev, chroma_dev, nullptr}, {luma_pitches, chroma_pitches, nullptr}, 1};
-  return forward_frames(e, "sqdet_forward_frames_nv12", n, SQDET_FMT_NV12, pl, heights, widths,
-                        crops, order, rescale, stream);
+  return forward_plane_arrays(e, "sqdet_forward_frames_nv12", n, SQDET_FMT_NV12,
+                              {luma_dev, chroma_dev}, {luma_pitches, chroma_pitches}, heights,
+                              widths, crops, order, rescale, stream);
 }
 
 // ---- whole frames as overlapping tiles, merged per frame ---------------------------------------
@@ -1536,11 +1445,14 @@ int sqdet_forward_tiles(sqdet_engine* e, int n, int format, const uint8_t* const
   int rc = check_merge_tiles(name.c_str(), (int)e->num_anchors, t, frame_of.data(), n,
                              c.top_n_detection, e->max_dets);
   if (rc) return rc;
+  auto tile = [&](int k) {
+    return "tile " + std::to_string(k) + " (frame " + std::to_string(frame_of[(size_t)k]) + ")";
+  };
   for (int k = 0; k < t; ++k) {
     const int f = frame_of[(size_t)k];
     const int64_t x = tiles[5 * k + 1], y = tiles[5 * k + 2], w = tiles[5 * k + 3],
                   h = tiles[5 * k + 4];
-    const std::string which = name + ": tile " + std::to_string(k) + " (frame " + std::to_string(f) + ")";
+    const std::string which = name + ": " + tile(k);
     if (w <= 0 || h <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
     if (x < 0 || y < 0 || x + w > widths[f] || y + h > heights[f])
       return fail(SQDET_ERR_INVALID_ARG, which + " is outside its frame");
@@ -1559,12 +1471,8 @@ int sqdet_forward_tiles(sqdet_engine* e, int n, int format, const uint8_t* const
       tp[3 * (size_t)k + p] = planes[src];
       if (pitches) tq[3 * (size_t)k + p] = pitches[src];
     }
-  const int64_t* tqp = pitches ? tq.data() : nullptr;
-  const FramePlanes pl = {{tp.data(), tp.data() + 1, tp.data() + 2},
-                          {tqp, tqp ? tqp + 1 : nullptr, tqp ? tqp + 2 : nullptr},
-                          3};
-  rc = forward_frames(e, "sqdet_forward_tiles", t, format, pl, hs.data(), ws.data(), crops.data(),
-                      order, 1, stream, frame_of.data());
+  rc = forward_frames(e, name, t, format, tp.data(), pitches ? tq.data() : nullptr, hs.data(),
+                      ws.data(), crops.data(), order, 1, stream, tile);
   if (rc) return rc;
   DeviceGuard guard(e->device);
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the engine's device");
@@ -1838,170 +1746,6 @@ int sqdet_merge_tiles(const float* boxes_dev, const float* probs_dev, const int6
   return launch_merge_tiles("sqdet_merge_tiles", boxes_dev, probs_dev, cls_dev, A, t, tile_frames,
                             tile_xy, n, n, classes, top_n, prob_thresh, nms_thresh, nullptr,
                             dets_dev, counts_dev, max_dets, (cudaStream_t)stream);
-}
-
-// ---- detections drawn on frames in device memory --------------------------------------------------
-int sqdet_draw_dets(int n, int format, uint8_t* const* planes, const int64_t* pitches,
-                    const int32_t* heights, const int32_t* widths, const int32_t* crops,
-                    const sqdet_det* dets_dev, const int32_t* counts_dev, int max_dets,
-                    const sqdet_draw_style* style, void* stream) {
-  const std::string name = "sqdet_draw_dets";
-  const PixFormat* pf = pix_format(format);
-  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
-  if (!planes || !heights || !widths || !dets_dev || !counts_dev || !style || !style->class_names ||
-      !style->class_bgr)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  if (n < 1 || n > kMaxDrawFrames)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxDrawFrames) + "]");
-  if (max_dets < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": max_dets must be at least 1");
-  if (style->classes < 1 || style->classes > kDrawMaxClasses)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": classes must be in [1, " + std::to_string(kDrawMaxClasses) + "]");
-  const float fs = style->font_scale;
-  if (!(fs > 0.f && fs <= 1024.f))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": font_scale must be finite, positive and at most 1024");
-  DrawStyle st = {};
-  st.hscale = (int64_t)nearbyint((double)fs * 65536.0);   // cvRound: half to even
-  st.thresh = style->plot_prob_thresh;
-  st.classes = style->classes;
-  for (int c = 0; c < st.classes; ++c) {
-    const char* s = style->class_names[c];
-    const size_t len = s ? strnlen(s, kDrawMaxName + 1) : kDrawMaxName + 1;
-    bool printable = len <= (size_t)kDrawMaxName;
-    for (size_t i = 0; printable && i < len; ++i) printable = s[i] >= 32 && s[i] <= 126;
-    if (!printable)
-      return fail(SQDET_ERR_INVALID_ARG, name + ": class name " + std::to_string(c) +
-                                             " is not printable ASCII of at most " +
-                                             std::to_string(kDrawMaxName) + " characters");
-    memcpy(st.name[c], s, len);
-    st.name_len[c] = (uint8_t)len;
-    const int b = style->class_bgr[3 * c], g = style->class_bgr[3 * c + 1], r = style->class_bgr[3 * c + 2];
-    st.bgr[c][0] = (uint8_t)b;
-    st.bgr[c][1] = (uint8_t)g;
-    st.bgr[c][2] = (uint8_t)r;
-    // cv2.cvtColor(solid BGR patch, COLOR_BGR2YUV_I420): OpenCV's BT.601 coefficients, 20 bits
-    const int half = 1 << 19;
-    st.yuv[c][0] = (uint8_t)((269484 * r + 528482 * g + 102760 * b + (16 << 20) + half) >> 20);
-    st.yuv[c][1] = (uint8_t)((-155188 * r - 305135 * g + 460324 * b + (128 << 20) + half) >> 20);
-    st.yuv[c][2] = (uint8_t)((460324 * r - 385875 * g - 74448 * b + (128 << 20) + half) >> 20);
-  }
-  const FramePlanes pl = {{planes, planes + 1, planes + 2},
-                          {pitches, pitches ? pitches + 1 : nullptr, pitches ? pitches + 2 : nullptr},
-                          3};
-  auto image = [](int i) { return "frame " + std::to_string(i); };
-  std::vector<FrameSource> fr;
-  int rc = check_frames(name, pf, n, pl, heights, widths, crops, image, fr);
-  if (rc) return rc;
-  // the device the call runs on is the one frame 0's first plane lives on, whatever is current
-  int device = -1;
-  cudaPointerAttributes attr;
-  if (cudaPointerGetAttributes(&attr, fr[0].plane[0]) == cudaSuccess && attr.type == cudaMemoryTypeDevice)
-    device = attr.device;
-  else
-    (void)cudaGetLastError();      // an unknown pointer: no stale error for the next launch check
-  rc = check_frame_memory(name, pf, n, heights, widths, fr, device, "frame 0's device", image);
-  if (rc) return rc;
-  if (!device_range_ok(reinterpret_cast<const uint8_t*>(dets_dev),
-                       (int64_t)n * max_dets * (int64_t)sizeof(sqdet_det), device) ||
-      !device_range_ok(reinterpret_cast<const uint8_t*>(counts_dev), (int64_t)n * sizeof(int32_t),
-                       device))
-    return fail(SQDET_ERR_INVALID_ARG,
-                name + ": dets_dev or counts_dev is not inside one device allocation on frame 0's device");
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
-  return launch_draw_dets(format, fr.data(), n, dets_dev, counts_dev, max_dets, st,
-                          (cudaStream_t)stream);
-}
-
-// ---- JPEG encoding of frames in device memory ---------------------------------------------------
-constexpr int kJpegMaxSide = 65535;     // SOF0's 16-bit height and width
-
-int64_t sqdet_jpeg_max_bytes(int h, int w) {
-  if (h < 1 || w < 1 || h > kJpegMaxSide || w > kJpegMaxSide) {
-    fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_max_bytes: h and w must be in [1, 65535]");
-    return -1;
-  }
-  return jpeg_max_bytes(h, w);
-}
-
-// The crops (x, y, w, h) of sqdet_encode_jpeg's frames, or a refusal naming the first that is empty,
-// outside its frame or larger than a JPEG holds.
-static int jpeg_crops(const std::string& name, int n, const int32_t* heights, const int32_t* widths,
-                      const int32_t* crops, std::vector<FrameSource>& fr) {
-  if (!heights || !widths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  if (n < 1 || n > kMaxJpegFrames)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxJpegFrames) + "]");
-  fr.assign((size_t)n, FrameSource{});
-  for (int i = 0; i < n; ++i) {
-    const std::string which = name + ": frame " + std::to_string(i);
-    const int64_t H = heights[i], W = widths[i];
-    if (H <= 0 || W <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
-    const int32_t* r = crops ? crops + 4 * i : nullptr;
-    FrameSource& s = fr[(size_t)i];
-    s.x = r ? r[0] : 0;
-    s.y = r ? r[1] : 0;
-    s.w = r ? r[2] : (int)W;
-    s.h = r ? r[3] : (int)H;
-    if (s.w <= 0 || s.h <= 0) return fail(SQDET_ERR_INVALID_ARG, which + ": empty crop");
-    if (s.x < 0 || s.y < 0 || (int64_t)s.x + s.w > W || (int64_t)s.y + s.h > H)
-      return fail(SQDET_ERR_INVALID_ARG, which + ": crop outside the frame");
-    if (s.w > kJpegMaxSide || s.h > kJpegMaxSide)
-      return fail(SQDET_ERR_INVALID_ARG, which + ": a JPEG is at most 65535 pixels wide and high");
-  }
-  return SQDET_OK;
-}
-
-int64_t sqdet_jpeg_scratch_bytes(int n, const int32_t* heights, const int32_t* widths,
-                                 const int32_t* crops) {
-  std::vector<FrameSource> fr;
-  if (jpeg_crops("sqdet_jpeg_scratch_bytes", n, heights, widths, crops, fr)) return -1;
-  return jpeg_scratch_bytes(fr.data(), n);
-}
-
-int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
-                      const int32_t* heights, const int32_t* widths, const int32_t* crops,
-                      int quality, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
-                      void* scratch_dev, int64_t scratch_bytes, void* stream) {
-  const std::string name = "sqdet_encode_jpeg";
-  const PixFormat* pf = pix_format(format);
-  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
-  if (!planes || !heights || !widths || !out_dev || !lengths_dev || !scratch_dev)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  std::vector<FrameSource> sizes;
-  int rc = jpeg_crops(name, n, heights, widths, crops, sizes);
-  if (rc) return rc;
-  if (quality < 1 || quality > 100) return fail(SQDET_ERR_INVALID_ARG, name + ": quality must be in [1, 100]");
-  if (cap < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": cap must be at least 1");
-  // the scratch holds int4, int64 and 32-bit atomic regions at 256-byte offsets from its start
-  if ((uintptr_t)scratch_dev % 256)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
-  if ((uintptr_t)lengths_dev % alignof(int64_t))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": lengths_dev must be 8-byte aligned");
-  if (scratch_bytes < jpeg_scratch_bytes(sizes.data(), n))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below sqdet_jpeg_scratch_bytes");
-  const FramePlanes pl = {{planes, planes + 1, planes + 2},
-                          {pitches, pitches ? pitches + 1 : nullptr, pitches ? pitches + 2 : nullptr},
-                          3};
-  auto image = [](int i) { return "frame " + std::to_string(i); };
-  std::vector<FrameSource> fr;
-  rc = check_frames(name, pf, n, pl, heights, widths, crops, image, fr);
-  if (rc) return rc;
-  int device = -1;
-  cudaPointerAttributes attr;
-  if (cudaPointerGetAttributes(&attr, fr[0].plane[0]) == cudaSuccess && attr.type == cudaMemoryTypeDevice)
-    device = attr.device;
-  else
-    (void)cudaGetLastError();
-  rc = check_frame_memory(name, pf, n, heights, widths, fr, device, "frame 0's device", image);
-  if (rc) return rc;
-  const bool out_fits = cap <= INT64_MAX / n && device_range_ok(out_dev, (int64_t)n * cap, device);
-  if (!out_fits || !device_range_ok(reinterpret_cast<const uint8_t*>(lengths_dev), (int64_t)n * 8, device) ||
-      !device_range_ok(static_cast<const uint8_t*>(scratch_dev), scratch_bytes, device))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": out_dev, lengths_dev or scratch_dev is not inside one "
-                                              "device allocation on frame 0's device");
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
-  return launch_encode_jpeg(format, fr.data(), n, quality, out_dev, cap, lengths_dev, scratch_dev,
-                            (cudaStream_t)stream);
 }
 
 // ---- memory helpers ------------------------------------------------------------------------------

@@ -6,6 +6,11 @@
 // One kernel template over the format code: taps<F> (frames.cuh, shared with jpeg.cu) picks the
 // fetch from a FrameDesc<P> of the format's P planes, and resize_meansub_pixel does the arithmetic
 // every format shares.
+//
+// It also owns the checks that frames and buffers coming from the caller get before any device
+// work (accept_frames, device_range_ok), which every entry point taking device frames shares.
+#include <cuda.h>
+
 #include <algorithm>
 
 #include "frames.cuh"
@@ -176,6 +181,94 @@ int launch_resize_meansub_frames(int format, const FrameSource* frames, int n, f
     default:
       return launch_format<SQDET_FMT_I420>(*pf, frames, n, dst, H, W, b, means, sub_first, scales_xy, stream);
   }
+}
+
+// ---- frames and buffers from the caller ----------------------------------------------------------
+int pointer_device(const void* p) {
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, p) == cudaSuccess && attr.type == cudaMemoryTypeDevice)
+    return attr.device;
+  (void)cudaGetLastError();      // an unknown pointer: no stale error for the next launch check
+  return -1;
+}
+
+using MemGetAddressRangeFn = CUresult (*)(CUdeviceptr*, size_t*, CUdeviceptr);
+
+bool device_range_ok(const void* p, int64_t bytes, int device) {
+  static MemGetAddressRangeFn range = [] {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      fn = nullptr;
+    return reinterpret_cast<MemGetAddressRangeFn>(fn);
+  }();
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) {
+    (void)cudaGetLastError();      // an unknown pointer: no stale error for the next launch check
+    return false;
+  }
+  if (attr.type != cudaMemoryTypeDevice || attr.device != device || !range) return false;
+  CUdeviceptr base = 0;
+  size_t size = 0;
+  if (range(&base, &size, (CUdeviceptr)(uintptr_t)p) != CUDA_SUCCESS) return false;
+  const uint64_t off = (uint64_t)(uintptr_t)p - (uint64_t)base;
+  return off <= size && (uint64_t)bytes <= size - off;
+}
+
+int check_crop(const std::string& which, int64_t H, int64_t W, const int32_t* r, FrameSource& s) {
+  s.x = r ? r[0] : 0;
+  s.y = r ? r[1] : 0;
+  s.w = r ? r[2] : (int)W;
+  s.h = r ? r[3] : (int)H;
+  if (s.w <= 0 || s.h <= 0) return fail(SQDET_ERR_INVALID_ARG, which + ": empty crop");
+  if (s.x < 0 || s.y < 0 || (int64_t)s.x + s.w > W || (int64_t)s.y + s.h > H)
+    return fail(SQDET_ERR_INVALID_ARG, which + ": crop outside the frame");
+  return SQDET_OK;
+}
+
+int accept_frames(const std::string& name, const PixFormat& pf, int n,
+                  const uint8_t* const* planes, const int64_t* pitches, const int32_t* heights,
+                  const int32_t* widths, const int32_t* crops,
+                  const std::function<std::string(int)>& image, int* device,
+                  std::vector<FrameSource>& fr) {
+  auto which = [&](int i) { return name + ": " + (image ? image(i) : "frame " + std::to_string(i)); };
+  fr.assign((size_t)n, FrameSource{});
+  for (int i = 0; i < n; ++i) {
+    const int64_t H = heights[i], W = widths[i];
+    const std::string what = which(i);
+    FrameSource& s = fr[(size_t)i];
+    for (int p = 0; p < pf.planes; ++p) {
+      s.plane[p] = planes[3 * (size_t)i + p];
+      if (!s.plane[p])
+        return fail(SQDET_ERR_INVALID_ARG, what + (pf.planes == 1 ? " is a null pointer" : " has a null plane"));
+    }
+    if (pf.even && (H <= 0 || W <= 0 || H % 2 || W % 2))
+      return fail(SQDET_ERR_INVALID_ARG, what + ": height and width must be positive and even");
+    if (H <= 0 || W <= 0) return fail(SQDET_ERR_INVALID_ARG, what + " is empty");
+    for (int p = 0; p < pf.planes; ++p) {
+      s.pitch[p] = pitches ? pitches[3 * (size_t)i + p] : pf.plane[p].row_bytes(W);
+      if (s.pitch[p] < pf.plane[p].row_bytes(W))
+        return fail(SQDET_ERR_INVALID_ARG, what + ": row pitch below " + pf.least_pitch);
+    }
+    const int rc = check_crop(what, H, W, crops ? crops + 4 * (size_t)i : nullptr, s);
+    if (rc) return rc;
+  }
+  const char* where = *device == kFrame0Device ? "frame 0's device" : "the engine's device";
+  if (*device == kFrame0Device) *device = pointer_device(fr[0].plane[0]);
+  for (int i = 0; i < n; ++i) {
+    const FrameSource& s = fr[(size_t)i];
+    for (int p = 0; p < pf.planes; ++p) {
+      // the plane's bytes end at (rows - 1) * pitch + row bytes; refused when that overflows int64
+      const int64_t k = (int64_t)heights[i] >> pf.plane[p].y_shift, b = pf.plane[p].row_bytes(widths[i]);
+      const bool fits = k == 1 || s.pitch[p] <= (INT64_MAX - b) / (k - 1);
+      if (!fits || !device_range_ok(s.plane[p], (k - 1) * s.pitch[p] + b, *device))
+        return fail(SQDET_ERR_INVALID_ARG,
+                    which(i) + (pf.planes == 1 ? " is not inside" : ": a plane is not inside") +
+                        " one device allocation on " + where);
+    }
+  }
+  return SQDET_OK;
 }
 
 }  // namespace sqdet

@@ -131,6 +131,8 @@ struct JpegGeom {
   int64_t* length;
 };
 constexpr int kJpegFramesPerLaunch = 16;
+constexpr int kMaxJpegFrames = 128;     // frames per sqdet_encode_jpeg call
+constexpr int kJpegMaxSide = 65535;     // SOF0's 16-bit height and width
 
 struct JpegParams {
   JpegGeom g[kJpegFramesPerLaunch];
@@ -620,13 +622,13 @@ int launch_group(const PixFormat& pf, const FrameSource* fr, int first, int coun
   return SQDET_OK;
 }
 
-}  // namespace
-
+// The largest file of an h x w crop.
 int64_t jpeg_max_bytes(int h, int w) {
   const FrameSizes s = frame_sizes(h, w);
   return kHeaderBytes + 2 * (((int64_t)s.blocks * kMaxBlockBits + 7) / 8) + 2;
 }
 
+// The scratch the encode of the crops of `frames` needs.
 int64_t jpeg_scratch_bytes(const FrameSource* frames, int n) {
   int64_t most = 0;
   for (int first = 0; first < n; first += kJpegFramesPerLaunch)
@@ -634,6 +636,7 @@ int64_t jpeg_scratch_bytes(const FrameSource* frames, int n) {
   return most;
 }
 
+// The encode of the crops of `frames` (the frames' checks are the caller's).
 int launch_encode_jpeg(int format, const FrameSource* frames, int n, int quality, uint8_t* out,
                        int64_t cap, int64_t* lengths, void* scratch, cudaStream_t stream) {
   const PixFormat* pf = pix_format(format);
@@ -689,4 +692,76 @@ int launch_encode_jpeg(int format, const FrameSource* frames, int n, int quality
   return SQDET_OK;
 }
 
+// The crops (x, y, w, h) of sqdet_encode_jpeg's frames, or a refusal naming the first that is empty,
+// outside its frame or larger than a JPEG holds.
+int jpeg_crops(const std::string& name, int n, const int32_t* heights, const int32_t* widths,
+               const int32_t* crops, std::vector<FrameSource>& fr) {
+  if (!heights || !widths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (n < 1 || n > kMaxJpegFrames)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxJpegFrames) + "]");
+  fr.assign((size_t)n, FrameSource{});
+  for (int i = 0; i < n; ++i) {
+    const std::string which = name + ": frame " + std::to_string(i);
+    if (heights[i] <= 0 || widths[i] <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
+    const int rc = check_crop(which, heights[i], widths[i], crops ? crops + 4 * i : nullptr, fr[(size_t)i]);
+    if (rc) return rc;
+    if (fr[(size_t)i].w > kJpegMaxSide || fr[(size_t)i].h > kJpegMaxSide)
+      return fail(SQDET_ERR_INVALID_ARG, which + ": a JPEG is at most 65535 pixels wide and high");
+  }
+  return SQDET_OK;
+}
+
+}  // namespace
 }  // namespace sqdet
+
+using namespace sqdet;
+
+int64_t sqdet_jpeg_max_bytes(int h, int w) {
+  if (h < 1 || w < 1 || h > kJpegMaxSide || w > kJpegMaxSide) {
+    fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_max_bytes: h and w must be in [1, 65535]");
+    return -1;
+  }
+  return jpeg_max_bytes(h, w);
+}
+
+int64_t sqdet_jpeg_scratch_bytes(int n, const int32_t* heights, const int32_t* widths,
+                                 const int32_t* crops) {
+  std::vector<FrameSource> fr;
+  if (jpeg_crops("sqdet_jpeg_scratch_bytes", n, heights, widths, crops, fr)) return -1;
+  return jpeg_scratch_bytes(fr.data(), n);
+}
+
+int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
+                      const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                      int quality, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
+                      void* scratch_dev, int64_t scratch_bytes, void* stream) {
+  const std::string name = "sqdet_encode_jpeg";
+  const PixFormat* pf = pix_format(format);
+  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
+  if (!planes || !heights || !widths || !out_dev || !lengths_dev || !scratch_dev)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  std::vector<FrameSource> fr;
+  int rc = jpeg_crops(name, n, heights, widths, crops, fr);
+  if (rc) return rc;
+  if (quality < 1 || quality > 100) return fail(SQDET_ERR_INVALID_ARG, name + ": quality must be in [1, 100]");
+  if (cap < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": cap must be at least 1");
+  // the scratch holds int4, int64 and 32-bit atomic regions at 256-byte offsets from its start
+  if ((uintptr_t)scratch_dev % 256)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
+  if ((uintptr_t)lengths_dev % alignof(int64_t))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": lengths_dev must be 8-byte aligned");
+  if (scratch_bytes < jpeg_scratch_bytes(fr.data(), n))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below sqdet_jpeg_scratch_bytes");
+  int device = kFrame0Device;
+  rc = accept_frames(name, *pf, n, planes, pitches, heights, widths, crops, nullptr, &device, fr);
+  if (rc) return rc;
+  const bool out_fits = cap <= INT64_MAX / n && device_range_ok(out_dev, (int64_t)n * cap, device);
+  if (!out_fits || !device_range_ok(lengths_dev, (int64_t)n * 8, device) ||
+      !device_range_ok(scratch_dev, scratch_bytes, device))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": out_dev, lengths_dev or scratch_dev is not inside one "
+                                              "device allocation on frame 0's device");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
+  return launch_encode_jpeg(format, fr.data(), n, quality, out_dev, cap, lengths_dev, scratch_dev,
+                            (cudaStream_t)stream);
+}

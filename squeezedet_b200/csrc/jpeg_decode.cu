@@ -37,8 +37,6 @@
 
 #include "common.cuh"
 
-extern "C" bool device_range_ok(const uint8_t* p, int64_t bytes, int device);   // engine.cu
-
 namespace sqdet {
 
 namespace {
@@ -1194,12 +1192,8 @@ int sqdet_decode_jpeg(int n, const uint8_t* const* files_host, const int64_t* le
     (void)cudaGetLastError();
     return fail(SQDET_ERR_INVALID_ARG, name + ": staging_pinned is not page-locked host memory");
   }
-  int device = -1;
   if (!out_planes[0]) return fail(SQDET_ERR_INVALID_ARG, name + ": output 0 is null");
-  if (cudaPointerGetAttributes(&attr, out_planes[0]) == cudaSuccess && attr.type == cudaMemoryTypeDevice)
-    device = attr.device;
-  else
-    (void)cudaGetLastError();
+  const int device = pointer_device(out_planes[0]);
   if (device < 0) return fail(SQDET_ERR_INVALID_ARG, name + ": output 0 is not device memory");
   for (int i = 0; i < n; ++i) {
     const sqdet_jpeg_info& I = plan.parsed[(size_t)i].info;
@@ -1210,16 +1204,13 @@ int sqdet_decode_jpeg(int n, const uint8_t* const* files_host, const int64_t* le
     if (!device_range_ok(out_planes[i], bytes, device))
       return fail(SQDET_ERR_INVALID_ARG, which + " is not inside one device allocation on output 0's device");
   }
-  if (!device_range_ok(reinterpret_cast<const uint8_t*>(status_dev), (int64_t)n * 4, device) ||
-      !device_range_ok(static_cast<const uint8_t*>(scratch_dev), scratch_bytes, device))
+  if (!device_range_ok(status_dev, (int64_t)n * 4, device) ||
+      !device_range_ok(scratch_dev, scratch_bytes, device))
     return fail(SQDET_ERR_INVALID_ARG, name + ": status_dev or scratch_dev is not inside one device "
                                               "allocation on output 0's device");
   fill_staging(plan, n, files_host, out_planes, out_pitches, static_cast<uint8_t*>(staging_pinned));
-  int prev = -1;
-  if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(device) != cudaSuccess)
-    return fail(SQDET_ERR_CUDA, "cannot select output 0's device");
-  rc = launch_decode(plan, n, static_cast<uint8_t*>(staging_pinned), static_cast<uint8_t*>(scratch_dev),
-                     status_dev, (cudaStream_t)stream);
-  cudaSetDevice(prev);
-  return rc;
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select output 0's device");
+  return launch_decode(plan, n, static_cast<uint8_t*>(staging_pinned), static_cast<uint8_t*>(scratch_dev),
+                       status_dev, (cudaStream_t)stream);
 }

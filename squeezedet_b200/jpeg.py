@@ -13,16 +13,7 @@ from __future__ import annotations
 import ctypes as C
 
 from . import _lib
-from .nn_skeleton import PIXEL_FORMATS, ModelSkeleton
-
-
-class _Frames:
-  """ModelSkeleton's frame packing and checks, for frames on cuda:`gpu_id` without an engine."""
-  _pack_frames = ModelSkeleton._pack_frames
-  _frame_planes = ModelSkeleton._frame_planes
-
-  def __init__(self, gpu_id):
-    self.gpu_id = gpu_id
+from .frames import PIXEL_FORMATS, frame_count, pack_frames
 
 
 def _first_tensor(f):
@@ -63,8 +54,7 @@ def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None):
   of output; encode fewer frames per call where that matters."""
   import torch
   frames = list(frames)
-  if not 1 <= len(frames) <= 128:
-    raise ValueError('need 1 to 128 frames, got %d' % len(frames))
+  n = frame_count(frames, 128)
   if fmt not in PIXEL_FORMATS:
     raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
   if not 1 <= int(quality) <= 100:
@@ -72,8 +62,7 @@ def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None):
   device = getattr(_first_tensor(frames[0]), 'device', None)
   if getattr(device, 'type', None) != 'cuda':
     raise ValueError('frame 0: need a CUDA tensor, got %s' % (device,))
-  n = len(frames)
-  planes, pitches, hs, ws, rects = _Frames(device.index)._pack_frames(frames, fmt, crops)
+  planes, pitches, hs, ws, rects = pack_frames(frames, fmt, crops, device.index)
   lib = _lib.load()
   cap = max(max_bytes(rects[4 * i + 3], rects[4 * i + 2]) for i in range(n))
   scratch_bytes = lib.sqdet_jpeg_scratch_bytes(n, hs, ws, rects)
