@@ -73,7 +73,10 @@ def _u16(b, i):
 
 
 def exif_orientation(seg):
-  """The Orientation tag (0x0112) of IFD0 in an APP1 'Exif\\0\\0' body, or 1."""
+  """The Orientation tag (0x0112) of IFD0 in an APP1 'Exif\\0\\0' body, or 1.  As cv2 reads it:
+  the first 0x0112 entry, its u16 at entry offset 8 in the TIFF byte order whatever the entry's
+  type and count, with only the entry's bytes [0, 10) needed inside the segment; a value outside
+  1..8 means 1."""
   if len(seg) < 14 or seg[:6] != b'Exif\x00\x00':
     return 1
   t = seg[6:]
@@ -90,9 +93,9 @@ def exif_orientation(seg):
     return 1
   for e in range(rd(ifd, 2)):
     p = ifd + 2 + 12 * e
-    if p + 12 > len(t):
+    if p + 10 > len(t):
       break
-    if rd(p, 2) == 0x0112 and rd(p + 2, 2) == 3:
+    if rd(p, 2) == 0x0112:
       o = rd(p + 8, 2)
       return o if 1 <= o <= 8 else 1
   return 1

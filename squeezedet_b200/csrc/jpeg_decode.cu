@@ -723,6 +723,9 @@ struct Parsed {
 
 int u16(const uint8_t* b, int64_t i) { return (b[i] << 8) | b[i + 1]; }
 
+// As cv2 reads it: the first Orientation (0x0112) entry of IFD0, its u16 at entry offset 8 in the
+// TIFF byte order whatever the entry's type and count, with only the entry's bytes [0, 10) needed
+// inside the segment; a value outside 1..8 means 1.
 int exif_orientation(const uint8_t* s, int64_t n) {
   if (n < 14 || memcmp(s, "Exif\0\0", 6) != 0) return 1;
   const uint8_t* t = s + 6;
@@ -743,8 +746,8 @@ int exif_orientation(const uint8_t* s, int64_t n) {
   if (ifd < 0 || count < 0) return 1;
   for (int64_t e = 0; e < count; ++e) {
     const int64_t q = ifd + 2 + 12 * e;
-    if (q + 12 > tn) break;
-    if (rd(q, 2) == 0x0112 && rd(q + 2, 2) == 3) {
+    if (q + 10 > tn) break;
+    if (rd(q, 2) == 0x0112) {
       const int64_t o = rd(q + 8, 2);
       return o >= 1 && o <= 8 ? (int)o : 1;
     }

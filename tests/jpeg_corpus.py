@@ -1,11 +1,16 @@
-"""JPEG files for the decoder's tests, all made by cv2.imencode from seeded content: the content
-kinds of test_gpu_jpeg (noise, gradients, flat, checkerboards of pixels and of 8x8 blocks, dots)
-plus a smooth picture, over sizes, qualities, samplings, restart intervals, optimized Huffman
-tables, separate luma and chroma qualities, grayscale and EXIF orientations."""
+"""JPEG files for the decoder's tests, made by cv2.imencode from seeded content: the content kinds
+of test_gpu_jpeg (noise, gradients, flat, checkerboards of pixels and of 8x8 blocks, dots) plus a
+smooth picture, over sizes, qualities, samplings, restart intervals, optimized Huffman tables,
+separate luma and chroma qualities, grayscale and EXIF orientations.  foreign() rewrites such
+files with tests/jpeg_writer.py into what other encoders write; camera() is at camera sizes;
+exif_variants() and refused() pin how cv2 reads EXIF and what the decoder refuses."""
 import cv2
 import numpy as np
 
+from oracle import jpeg_decode as D
 from oracle.jpeg_decode import with_orientation
+
+import jpeg_writer as W
 
 KINDS = ('noise', 'grad', 'flat', 'check', 'blocks', 'dots', 'smooth')
 SAMPLINGS = (0x111111, 0x211111, 0x121111, 0x221111, 0x411111)
@@ -175,3 +180,150 @@ def handmade(seed=0):
           ('extra data and RST', extra_rst_data(encode(content('smooth', 40, 56, 3, rng),
                                                        cv2.IMWRITE_JPEG_RST_INTERVAL, 2)))]
   return out
+
+
+# ---- files other encoders write, camera sizes, EXIF as cv2 reads it, and refusals ------------------
+def _foreign_sources(rng):
+  """(name, cv2 file) covering every sampling, odd sizes, grayscale and q50-100."""
+  out = []
+  for kind, (h, w), samp, q in (('noise', (37, 53), 0x111111, 100), ('check', (45, 70), 0x211111, 90),
+                                ('smooth', (61, 97), 0x121111, 75), ('noise', (33, 47), 0x221111, 50),
+                                ('smooth', (29, 83), 0x411111, 95), ('check', (26, 35), 0x221111, 100)):
+    out.append(('%s %dx%d s%06x q%d' % (kind, h, w, samp, q),
+                encode(content(kind, h, w, 3, rng), cv2.IMWRITE_JPEG_QUALITY, q,
+                       cv2.IMWRITE_JPEG_SAMPLING_FACTOR, samp)))
+  for kind, (h, w), q in (('check', (23, 41), 60), ('smooth', (50, 38), 85)):
+    out.append(('%s %dx%d gray q%d' % (kind, h, w, q),
+                encode(content(kind, h, w, 1, rng)[..., 0], cv2.IMWRITE_JPEG_QUALITY, q)))
+  return out
+
+
+def _variants(nc, mcols, mcus, thumb):
+  """name -> write() settings for a source of nc components and mcols x (mcus / mcols) MCUs."""
+  odd = next(r for r in range(3, 64) if mcols % r and r % mcols)
+  v = {
+      'tables 0 for all': dict(huff=[(0, 0)] * nc),
+      'luma on 3,2': dict(huff=[(3, 2)] + [(1, 1)] * (nc - 1)),
+      'optimal': dict(tables='optimal'),
+      'skewed': dict(tables='skewed'),
+      'full 256': dict(tables='full'),
+      'joint segments': dict(pack='joint', tables='optimal'),
+      'redefined tables': dict(redefine=True),
+      'sof1': dict(sof=0xC1),
+      'rst 1': dict(restart=1),
+      'rst %d (not a row)' % odd: dict(restart=odd, tables='optimal'),
+      'rst past the end': dict(restart=mcus + 7),
+      'rst 2 fill bytes': dict(restart=2, rst_fill=3),
+      'rst 1 0-padded': dict(restart=1, pad_bit=0, tables='skewed'),
+      '0-padded': dict(pad_bit=0),
+      'COM APP2 XMP': dict(before=(W.COM, W.ICC, W.XMP), after_sof=(W.COM,)),
+      'EXIF thumbnail': dict(before=(W.exif(1, True, thumb),), jfif=False),
+      'fill between segments': dict(fill=2, redefine=True),
+      'everything': dict(huff=[(3, 1), (1, 2), (2, 0)][:nc], tables='skewed', pack='joint',
+                         redefine=True, sof=0xC1, restart=odd, rst_fill=1, pad_bit=0,
+                         before=(W.COM, W.exif(1, False, thumb), W.XMP), fill=1, jfif=False,
+                         quant=[3, 0, 2][:nc], halve_cr=nc == 3),
+  }
+  if nc == 3:
+    v.update({
+        'chroma on 2,3': dict(huff=[(0, 0), (2, 3), (2, 3)]),
+        'Cb, Cr apart': dict(huff=[(3, 1), (1, 2), (2, 0)], tables='optimal'),
+        'Cr on quant 2': dict(quant=[0, 1, 2]),
+        'quant 3, 0, 2': dict(quant=[3, 0, 2], tables='full'),
+        'Cr quant halved': dict(quant=[0, 1, 2], halve_cr=True),
+    })
+  return v
+
+
+def foreign(seed=0):
+  """[(name, file bytes, source file)]: cv2 files of every sampling, odd sizes, grayscale, noise, checkerboard
+  and smooth content at q50-100, transcoded by tests/jpeg_writer.py into what other encoders
+  write.  Each decodes (in cv2) to its source's pixels."""
+  rng = np.random.default_rng(seed)
+  thumb = encode(content('smooth', 12, 16, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 70)
+  out = []
+  for sname, f in _foreign_sources(rng):
+    info, grids = W.source(f)
+    _, mcols, mrows = D.mcu_geometry(info)
+    for vname, kw in _variants(len(info.comps), mcols, mcols * mrows, thumb).items():
+      out.append(('%s, %s' % (sname, vname), W.write(info, grids, **kw), f))
+  return out
+
+
+def _tiff_entry(tag, typ, count, value4, e):
+  return tag.to_bytes(2, e) + typ.to_bytes(2, e) + count.to_bytes(4, e) + value4
+
+
+def _exif_body(entries, e, ifd1=None):
+  """'Exif\\0\\0' and a TIFF header in byte order e with IFD0 `entries` (and IFD1 `ifd1`)."""
+  r = lambda v, n: v.to_bytes(n, e)
+  t = (b'II' if e == 'little' else b'MM') + r(42, 2) + r(8, 4) + r(len(entries), 2) + b''.join(entries)
+  if ifd1 is None:
+    return b'Exif\x00\x00' + t + r(0, 4)
+  return b'Exif\x00\x00' + t + r(len(t) + 4, 4) + r(len(ifd1), 2) + b''.join(ifd1) + r(0, 4)
+
+
+def exif_variants(seed=0):
+  """[(name, file bytes, the orientation cv2 applies)]: Orientation entries of every type, count,
+  byte order and placement, on a 13x21 noise file at q100 4:4:4 whose eight orientations all
+  differ."""
+  rng = np.random.default_rng(seed)
+  f = encode(content('noise', 13, 21, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 100,
+             cv2.IMWRITE_JPEG_SAMPLING_FACTOR, 0x111111)
+  B, L = 'big', 'little'
+  o = lambda typ, cnt, v4, e=B: _tiff_entry(0x0112, typ, cnt, v4, e)
+  short = lambda v, e=B: v.to_bytes(2, e) + b'\x00\x00'
+  rows = [
+      ('SHORT 6 big-endian', _exif_body([o(3, 1, short(6))], B), 6),
+      ('SHORT 6 little-endian', _exif_body([o(3, 1, short(6, L), L)], L), 6),
+      ('LONG 6 little-endian', _exif_body([o(4, 1, (6).to_bytes(4, L), L)], L), 6),
+      ('type 0, 6 in the first two bytes', _exif_body([o(0, 1, short(6))], B), 6),
+      ('ends after the value\'s first two bytes', _exif_body([o(3, 1, short(6))], B)[:6 + 8 + 2 + 10], 6),
+      ('LONG 6 big-endian', _exif_body([o(4, 1, (6).to_bytes(4, B))], B), 1),
+      ('BYTE 6 big-endian', _exif_body([o(1, 1, b'\x06\x00\x00\x00')], B), 1),
+      ('SHORT 6 count 0', _exif_body([o(3, 0, short(6))], B), 6),
+      ('SHORT 6 count 2', _exif_body([o(3, 2, short(6))], B), 6),
+      ('6 then 3', _exif_body([o(3, 1, short(6)), o(3, 1, short(3))], B), 6),
+      ('only in IFD1', _exif_body([_tiff_entry(0x010F, 2, 4, b'abc\x00', B)], B, [o(3, 1, short(6))]), 1),
+      ('value 0', _exif_body([o(3, 1, short(0))], B), 1),
+      ('value 9', _exif_body([o(3, 1, short(9))], B), 1),
+      ('SHORT 8 little-endian', _exif_body([o(3, 1, short(8, L), L)], L), 8),
+  ]
+  out = [(name, f[:2] + W.segment(0xE1, body) + f[2:], want) for name, body, want in rows]
+  out.append(('XMP before the Exif', f[:2] + W.XMP + W.segment(0xE1, rows[0][1]) + f[2:], 6))
+  return out
+
+
+def camera(seed=0):
+  """[(name, file bytes)] at camera sizes, none a multiple of 16 in both sides: 12 MP smooth 4:2:0
+  with EXIF orientation 6 and a thumbnail, 12 MP 4:2:2 at orientation 8 with a restart interval of
+  one MCU row, a 4032x3024 noise file at q100 4:4:4 (about 50 MB), and 1x8191 and 8191x1."""
+  rng = np.random.default_rng(seed)
+  thumb = encode(content('smooth', 120, 160, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 80)
+  a = encode(content('smooth', 3000, 4000, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 92)
+  b = encode(content('smooth', 4000, 3000, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 95,
+             cv2.IMWRITE_JPEG_SAMPLING_FACTOR, 0x211111, cv2.IMWRITE_JPEG_RST_INTERVAL, 3000 // 16 + 1)
+  return [('4000x3000 q92 s221111 exif 6', a[:2] + W.exif(6, True, thumb) + a[2:]),
+          ('3000x4000 q95 s211111 rst row exif 8', with_orientation(b, 8)),
+          ('4032x3024 noise q100 s111111', encode(content('noise', 3024, 4032, 3, rng),
+                                                  cv2.IMWRITE_JPEG_QUALITY, 100,
+                                                  cv2.IMWRITE_JPEG_SAMPLING_FACTOR, 0x111111)),
+          ('1x8191', encode(content('smooth', 1, 8191, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 90)),
+          ('8191x1', encode(content('smooth', 8191, 1, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 90))]
+
+
+def refused(seed=0):
+  """[(name, file bytes, reason, whether cv2 decodes it)]: files the decoder refuses by design.
+  libjpeg-turbo refuses a scan whose components are in another order than the frame's (its
+  component lookup skips an id already placed at the same index), so cv2 returns None for those."""
+  rng = np.random.default_rng(seed)
+  f = encode(content('smooth', 30, 44, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 90,
+             cv2.IMWRITE_JPEG_SAMPLING_FACTOR, 0x111111)
+  g = encode(content('smooth', 30, 44, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 90)
+  info, grids = W.source(f)
+  info2, grids2 = W.source(g)
+  return [('SOS order Y, Cr, Cb', W.write(info, grids, order=(0, 2, 1)), D.SAMPLING, False),
+          ('SOS order Cb, Y, Cr', W.write(info, grids, order=(1, 0, 2)), D.SAMPLING, False),
+          ('Y and Cb 2x2, Cr 1x1', W.write(info2, [grids2[0], grids2[0], grids2[2]],
+                                           sampling=[(2, 2), (2, 2), (1, 1)]), D.SAMPLING, True),
+          ('bytes before a marker', W.write(info, grids, before=(b'\x00\x5a',)), D.MALFORMED, True)]
