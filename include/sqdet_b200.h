@@ -513,11 +513,12 @@ int sqdet_draw_dets(int n, int format, uint8_t* const* planes, const int64_t* pi
  * `stream`, no host synchronisation, no allocation.  Refused before any device work with
  * SQDET_ERR_INVALID_ARG: a null array, n outside [1, 128], an unknown format, every frame refusal of
  * sqdet_forward_frames (planes that are not device memory of that device inside one allocation
- * included), a crop wider or taller than 65535, quality outside [1, 100], cap < 1, a misaligned
+ * included), a crop wider or taller than 65500 (libjpeg's JPEG_MAX_DIMENSION: cv2.imencode fails
+ * there too), quality outside [1, 100], cap < 1, a misaligned
  * scratch_dev or lengths_dev, scratch_bytes below sqdet_jpeg_scratch_bytes, and out_dev (n * cap bytes), lengths_dev (n int64) or scratch_dev
  * (scratch_bytes) not inside one allocation of device memory on that device.
  * sqdet_jpeg_max_bytes: the largest file of an h x w image, 0xFF stuffing of every byte included
- * (-1 for h or w outside [1, 65535]).  sqdet_jpeg_scratch_bytes: the scratch of that call (-1 when
+ * (-1 for h or w outside [1, 65500]).  sqdet_jpeg_scratch_bytes: the scratch of that call (-1 when
  * its sizes are refused as sqdet_encode_jpeg refuses them).  Both are worst cases, so that no
  * launch size waits for the device: for 1920 x 1080, about 20 MB of output (a quality-95 file of a
  * natural picture is under 1 MB) and about 17 MB of scratch per frame; frames run in groups of
@@ -540,7 +541,10 @@ int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int
  * components; luma sampling 1x1, 2x1, 1x2, 2x2 or 4x1 with 1x1 chroma; any DQT and DHT; DRI.
  * APPn and COM segments are skipped; the first APP1 'Exif' segment's Orientation is applied.
  * Everything else is refused before any device work with SQDET_ERR_UNSUPPORTED and a message
- * naming the file; route those files to cv2.imdecode.
+ * naming the file; route those files to cv2.imdecode.  Except SQDET_JPEG_TOO_LARGE: a coded side
+ * above 65500 (libjpeg's JPEG_MAX_DIMENSION) or more than 2^30 coded pixels (cv2's default
+ * CV_IO_MAX_IMAGE_PIXELS) is refused because cv2.imdecode decodes none of these files either (it
+ * returns None or raises), and a few header bytes must not size gigabytes of device memory.
  *
  * sqdet_jpeg_parse (host only): the headers of one file.  Returns SQDET_OK for a file
  * sqdet_decode_jpeg decodes, SQDET_ERR_UNSUPPORTED with out->reason set for one it refuses, and
@@ -582,6 +586,7 @@ int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int
 #define SQDET_JPEG_COLOR_TRANSFORM  7   /* RGB-coded: Adobe transform 0 or ids 'R','G','B' */
 #define SQDET_JPEG_SAMPLING         8   /* other sampling layouts, multi-scan sequential files */
 #define SQDET_JPEG_SIZE             9   /* zero height or width */
+#define SQDET_JPEG_TOO_LARGE        10  /* a side above 65500 or more than 2^30 pixels, as coded */
 typedef struct {
   int32_t height, width;              /* of the decoded frame, after orientation */
   int32_t coded_height, coded_width;  /* as SOF gives them */

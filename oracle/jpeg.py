@@ -348,13 +348,14 @@ def header(h, w, quality):
 
 def encode(bgr, quality=95):
   """The bytes cv2.imencode('.jpg', bgr, [cv2.IMWRITE_JPEG_QUALITY, quality]) writes for a uint8
-  BGR image [h, w, 3]."""
+  BGR image [h, w, 3].  Sides above 65500 (libjpeg's JPEG_MAX_DIMENSION) raise ValueError where
+  cv2.imencode fails."""
   bgr = np.asarray(bgr)
   if bgr.dtype != np.uint8 or bgr.ndim != 3 or bgr.shape[2] != 3 or min(bgr.shape[:2]) < 1:
     raise ValueError('need a non-empty uint8 [h, w, 3] image, got %s %r' % (bgr.dtype, bgr.shape))
   h, w = bgr.shape[:2]
-  if h > 65535 or w > 65535:
-    raise ValueError('JPEG sizes are at most 65535, got %dx%d' % (w, h))
+  if h > 65500 or w > 65500:
+    raise ValueError('JPEG sizes are at most 65500, got %dx%d' % (w, h))
   yq, cb, cr = coefficients(bgr, quality)
   vals, lens = _scan_symbols(h, w, yq, cb, cr)
   return header(h, w, quality) + _pack(vals, lens) + bytes([0xFF, 0xD9])

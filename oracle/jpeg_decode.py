@@ -17,10 +17,14 @@ import numpy as np
 
 # refusal reasons, as sqdet_jpeg_info.reason reports them
 OK, MALFORMED, PROGRESSIVE, ARITHMETIC, LOSSLESS, PRECISION, COMPONENTS, COLOR_TRANSFORM, \
-    SAMPLING, SIZE = range(10)
+    SAMPLING, SIZE, TOO_LARGE = range(11)
 REASONS = ('ok', 'malformed or truncated header', 'progressive', 'arithmetic coding', 'lossless',
            'not 8-bit samples', 'not 1 or 3 components', 'RGB-coded',
-           'unsupported sampling', 'zero height or width')
+           'unsupported sampling', 'zero height or width', 'larger than cv2 decodes')
+# the largest coded file cv2.imdecode decodes: libjpeg's JPEG_MAX_DIMENSION per side (None above
+# it) and cv2's default CV_IO_MAX_IMAGE_PIXELS (cv2.error above it)
+MAX_SIDE = 65500
+MAX_PIXELS = 1 << 30
 
 ZIGZAG = np.array([0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5,
                    12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14, 21, 28,
@@ -147,6 +151,8 @@ def parse(b):
                          body[8 + 3 * k]) for k in range(nc)]
       if hh == 0 or ww == 0:
         raise Unsupported(SIZE)
+      if hh > MAX_SIDE or ww > MAX_SIDE or hh * ww > MAX_PIXELS:
+        raise Unsupported(TOO_LARGE)
       if any(c.tq > 3 or not 1 <= c.h <= 4 or not 1 <= c.v <= 4 for c in comps):
         raise Unsupported(MALFORMED)
       if nc == 3 and ((comps[0].h, comps[0].v) not in LAYOUTS

@@ -132,7 +132,9 @@ struct JpegGeom {
 };
 constexpr int kJpegFramesPerLaunch = 16;
 constexpr int kMaxJpegFrames = 128;     // frames per sqdet_encode_jpeg call
-constexpr int kJpegMaxSide = 65535;     // SOF0's 16-bit height and width
+// libjpeg-turbo's JPEG_MAX_DIMENSION: cv2.imencode refuses a longer side, and libjpeg does not
+// read a file whose SOF0 says one (its 16-bit fields would hold up to 65535)
+constexpr int kJpegMaxSide = 65500;
 
 struct JpegParams {
   JpegGeom g[kJpegFramesPerLaunch];
@@ -693,7 +695,7 @@ int launch_encode_jpeg(int format, const FrameSource* frames, int n, int quality
 }
 
 // The crops (x, y, w, h) of sqdet_encode_jpeg's frames, or a refusal naming the first that is empty,
-// outside its frame or larger than a JPEG holds.
+// outside its frame or longer than libjpeg writes.
 int jpeg_crops(const std::string& name, int n, const int32_t* heights, const int32_t* widths,
                const int32_t* crops, std::vector<FrameSource>& fr) {
   if (!heights || !widths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
@@ -706,7 +708,7 @@ int jpeg_crops(const std::string& name, int n, const int32_t* heights, const int
     const int rc = check_crop(which, heights[i], widths[i], crops ? crops + 4 * i : nullptr, fr[(size_t)i]);
     if (rc) return rc;
     if (fr[(size_t)i].w > kJpegMaxSide || fr[(size_t)i].h > kJpegMaxSide)
-      return fail(SQDET_ERR_INVALID_ARG, which + ": a JPEG is at most 65535 pixels wide and high");
+      return fail(SQDET_ERR_INVALID_ARG, which + ": a JPEG is at most 65500 pixels wide and high");
   }
   return SQDET_OK;
 }
@@ -718,7 +720,7 @@ using namespace sqdet;
 
 int64_t sqdet_jpeg_max_bytes(int h, int w) {
   if (h < 1 || w < 1 || h > kJpegMaxSide || w > kJpegMaxSide) {
-    fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_max_bytes: h and w must be in [1, 65535]");
+    fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_max_bytes: h and w must be in [1, 65500]");
     return -1;
   }
   return jpeg_max_bytes(h, w);

@@ -759,7 +759,12 @@ int exif_orientation(const uint8_t* s, int64_t n) {
 const char* kReasons[] = {"ok", "malformed or truncated header", "progressive", "arithmetic coding",
                           "lossless", "not 8-bit samples", "not 1 or 3 components",
                           "RGB-coded", "unsupported sampling",
-                          "zero height or width"};
+                          "zero height or width", "larger than cv2 decodes"};
+
+// The largest file cv2.imdecode decodes: libjpeg's JPEG_MAX_DIMENSION per side, and cv2's default
+// CV_IO_MAX_IMAGE_PIXELS (it raises above that many pixels).
+constexpr int kMaxSide = 65500;
+constexpr int64_t kMaxPixels = int64_t{1} << 30;
 
 // libjpeg's checks of a Huffman table a scan uses: no length's codes run past its all-ones code,
 // and a DC table's symbols are categories 0..15.
@@ -819,6 +824,9 @@ int parse(const uint8_t* b, int64_t n, Parsed& P) {
         if (c.tq > 3 || c.h < 1 || c.h > 4 || c.v < 1 || c.v > 4) return SQDET_JPEG_MALFORMED;
       }
       if (I.coded_height == 0 || I.coded_width == 0) return SQDET_JPEG_SIZE;
+      if (I.coded_height > kMaxSide || I.coded_width > kMaxSide ||
+          (int64_t)I.coded_height * I.coded_width > kMaxPixels)
+        return SQDET_JPEG_TOO_LARGE;
       if (ncomp == 3) {
         const int h = P.comp[0].h, v = P.comp[0].v;
         const bool luma_ok = (h == 1 && v == 1) || (h == 2 && v == 1) || (h == 1 && v == 2) ||

@@ -21,9 +21,10 @@ def _first_tensor(f):
 
 
 def max_bytes(h, w):
-  """The largest JPEG file of an h x w image (sqdet_jpeg_max_bytes)."""
-  if not (1 <= int(h) <= 65535 and 1 <= int(w) <= 65535):
-    raise ValueError('a JPEG is 1 to 65535 pixels wide and high, got %dx%d' % (w, h))
+  """The largest JPEG file of an h x w image (sqdet_jpeg_max_bytes).  Sides are at most 65500,
+  libjpeg's JPEG_MAX_DIMENSION, as for cv2.imencode."""
+  if not (1 <= int(h) <= 65500 and 1 <= int(w) <= 65500):
+    raise ValueError('a JPEG is 1 to 65500 pixels wide and high, got %dx%d' % (w, h))
   return int(_lib.load().sqdet_jpeg_max_bytes(int(h), int(w)))
 
 
@@ -97,6 +98,9 @@ def jpeg_bytes(data, lengths, stream=None):
 
 
 # ---- decoding ------------------------------------------------------------------------------------
+JPEG_TOO_LARGE = 10       # SQDET_JPEG_TOO_LARGE: past cv2's limits, so cv2.imdecode refuses it too
+
+
 def jpeg_info(file_bytes):
   """sqdet_jpeg_parse of one file -> dict: height and width of the decoded frame (after the EXIF
   orientation), coded_height, coded_width, components, h_samp, v_samp (luma sampling),
@@ -150,7 +154,10 @@ def decode_jpeg_device(files, device, stream=None):
   Decoded are baseline and extended sequential Huffman files with 8-bit samples, 1 or 3
   components and 4:4:4, 4:2:2, 4:4:0, 4:2:0 or 4:1:1 sampling, with or without restart markers;
   the EXIF orientation is applied.  ValueError, naming the file's index, for any other file
-  (progressive, arithmetic, 12-bit, CMYK, ...): route those to cv2.imdecode.  1 to 128 files.
+  (progressive, arithmetic, 12-bit, CMYK, ...): route those to cv2.imdecode.  A file whose coded
+  side is above 65500 (libjpeg's JPEG_MAX_DIMENSION) or with more than 2^30 coded pixels (cv2's
+  default CV_IO_MAX_IMAGE_PIXELS) raises ValueError too, before anything is allocated; cv2.imdecode
+  decodes none of those either.  1 to 128 files.
 
   Asynchronous on `stream` (a torch.cuda.Stream, a raw cudaStream_t, or None for torch's current
   stream): the frames, status and scratch are allocated on it, so read them on it or after
@@ -173,8 +180,9 @@ def decode_jpeg_device(files, device, stream=None):
       raise ValueError('file %d: not a JPEG file (%d bytes)' % (i, len(f)))
     info = jpeg_info(f)
     if not info['supported']:
-      raise ValueError('file %d: not supported (%s); decode it with cv2.imdecode'
-                       % (i, info['reason_text']))
+      raise ValueError('file %d: not supported (%s); %s' % (
+          i, info['reason_text'], 'nor does cv2.imdecode decode it'
+          if info['reason'] == JPEG_TOO_LARGE else 'decode it with cv2.imdecode'))
     infos.append(info)
   lib = _lib.load()
   bufs = [C.create_string_buffer(f, len(f)) for f in files]

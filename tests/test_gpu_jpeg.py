@@ -15,6 +15,8 @@ from squeezedet_b200 import _lib
 from squeezedet_b200._lib import DeviceBuffer
 from squeezedet_b200.jpeg import encode_jpeg_device, jpeg_bytes, max_bytes
 
+from gpu_util import Frame, content, raw_encode, want
+
 pytestmark = pytest.mark.gpu
 
 FORMATS = ('bgr', 'rgb', 'bgra', 'rgba', 'rgb_planar', 'nv12', 'i420')
@@ -23,71 +25,8 @@ SIZES = [(1, 1), (1, 17), (17, 1), (2, 3), (8, 8), (15, 31), (16, 16), (17, 23),
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def content(kind, h, w, c, rng):
-  """uint8 [h, w, c] test content: noise, gradients, flat, 0/255 checkerboards of pixels (the
-  largest AC coefficients, ZRL at low quality) or of 8x8 blocks (DC differences of category 11),
-  or isolated dots on flat grey."""
-  if kind == 'noise':
-    return rng.integers(0, 256, (h, w, c), dtype=np.uint8)
-  y, x = np.mgrid[:h, :w]
-  if kind == 'grad':
-    return ((y[..., None] * 3 + x[..., None] * 5 + np.arange(c) * 40) % 256).astype(np.uint8)
-  if kind == 'flat':
-    return np.full((h, w, c), 77, np.uint8)
-  if kind in ('check', 'blocks'):     # 0/255 per pixel, or per 8x8 block (DC category 11)
-    cell = (y + x) % 2 if kind == 'check' else (y // 8 + x // 8) % 2
-    return np.repeat((cell * 255).astype(np.uint8)[..., None], c, axis=2)
-  img = np.full((h, w, c), 128, np.uint8)
-  img[(y % 8 == 7) & (x % 8 == 7)] = 255
-  return img
-
-
-class Frame:
-  """One frame in `fmt` (an h x w image; 4:2:0 formats need even sizes) on the device, with rows
-  `pad` bytes longer than tight and starting `off` bytes into their allocation, and its BGR image
-  as cv2.cvtColor makes it."""
-
-  def __init__(self, fmt, h, w, rng, device, kind='noise', pad=0, off=0):
-    self.fmt = fmt
-    if fmt in ('bgr', 'rgb', 'bgra', 'rgba'):
-      c = 4 if fmt in ('bgra', 'rgba') else 3
-      host = content(kind, h, w, c, rng)
-      code = {'bgr': None, 'rgb': cv2.COLOR_RGB2BGR, 'bgra': cv2.COLOR_BGRA2BGR,
-              'rgba': cv2.COLOR_RGBA2BGR}[fmt]
-      self.bgr = host if code is None else cv2.cvtColor(host, code)
-      self.dev = self._pitched(host.reshape(h, w * c), pad, off, device).unflatten(1, (w, c))
-    elif fmt == 'rgb_planar':
-      host = content(kind, h, w, 3, rng)
-      self.bgr = cv2.cvtColor(host, cv2.COLOR_RGB2BGR)
-      self.dev = tuple(self._pitched(np.ascontiguousarray(host[..., i]), pad, off, device)
-                       for i in range(3))
-    else:
-      host = content(kind, h * 3 // 2, w, 1, rng)[..., 0]
-      code = cv2.COLOR_YUV2BGR_NV12 if fmt == 'nv12' else cv2.COLOR_YUV2BGR_I420
-      self.bgr = cv2.cvtColor(host, code)
-      if fmt == 'nv12':
-        self.dev = (self._pitched(host[:h], pad, off, device),
-                    self._pitched(host[h:], pad, off, device))
-      else:
-        self.dev = torch.from_numpy(host).to(device)
-
-  @staticmethod
-  def _pitched(a, pad, off, device):
-    rows, cols = a.shape
-    buf = torch.zeros(off + rows * (cols + pad), dtype=torch.uint8, device=device)
-    t = buf[off:].view(rows, cols + pad)[:, :cols]
-    t.copy_(torch.from_numpy(np.ascontiguousarray(a)))
-    return t
-
-
 def even(v):
   return v + (v & 1)
-
-
-def want(frame, crop, quality):
-  x, y, w, h = crop
-  return cv2.imencode('.jpg', np.ascontiguousarray(frame.bgr[y:y + h, x:x + w]),
-                      [cv2.IMWRITE_JPEG_QUALITY, quality])[1].tobytes()
 
 
 @pytest.mark.parametrize('quality', [50, 95, 100])
@@ -169,23 +108,6 @@ def test_raw_stream_that_is_not_current(gpu_device):
   del junk
   for f, g in zip(frames, got):
     assert g == want(f, (0, 0, 1280, 720), 95)
-
-
-def raw_encode(frames, cap, quality=95, stream=None):
-  """sqdet_encode_jpeg of BGR device frames at capacity cap -> (data, lengths, scratch)."""
-  lib = _lib.load()
-  n = len(frames)
-  planes = (C.c_void_p * (3 * n))(*sum([[f.data_ptr(), None, None] for f in frames], []))
-  hs = (C.c_int32 * n)(*[f.shape[0] for f in frames])
-  ws = (C.c_int32 * n)(*[f.shape[1] for f in frames])
-  sb = lib.sqdet_jpeg_scratch_bytes(n, hs, ws, None)
-  dev = frames[0].device
-  data = torch.zeros((n, cap), dtype=torch.uint8, device=dev)
-  lengths = torch.zeros((n,), dtype=torch.int64, device=dev)
-  scratch = torch.empty((sb,), dtype=torch.uint8, device=dev)
-  _lib.check(lib.sqdet_encode_jpeg(n, 0, planes, None, hs, ws, None, quality, data.data_ptr(), cap,
-                                   lengths.data_ptr(), scratch.data_ptr(), sb, stream))
-  return data, lengths, scratch
 
 
 def test_cap_overflow_is_one_frame(gpu_device):

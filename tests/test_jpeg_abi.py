@@ -65,7 +65,7 @@ def test_frame_refusals():
   refused(encode(h=0), 'frame 0 is empty')
   refused(encode(crops=[0, 0, 0, 4]), 'empty crop')
   refused(encode(crops=[10, 0, 8, 4]), 'crop outside the frame')
-  refused(encode(h=70000, w=8), '65535')
+  refused(encode(h=70000, w=8), '65500')
   refused(encode(fmt=FMT_NV12, h=15, w=16), 'even')
   null_plane = (C.c_void_p * 3)(None, None, None)
   refused(encode(planes=null_plane, fmt=FMT_BGR), 'null pointer')
