@@ -531,6 +531,31 @@ int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int
                       int quality, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
                       void* scratch_dev, int64_t scratch_bytes, void* stream);
 
+/* ---- PNG encoding of frames in device memory (no engine needed) ---------------------
+ * sqdet_encode_png: frame i's crop (x, y, w, h) becomes exactly the bytes of
+ *   cv2.imencode('.png', cv2.cvtColor(frame, code)[y:y+h, x:x+w])
+ * with `code` the frame format's code of sqdet_forward_frames (BGR: no conversion): cv2's default
+ * PNG writer, libpng 1.6 over zlib 1.2.11 — 8-bit RGB (colour type 2), no interlace, the SUB filter
+ * on every row (NONE for a 1-pixel-wide image), zlib level 1 with strategy Z_RLE, 8192-byte IDAT
+ * chunks, no ancillary chunk.  Arguments, layout, output slots, lengths (-1 for a file longer than
+ * cap, the other frames unaffected), alignment, device and stream rules and refusals are those of
+ * sqdet_encode_jpeg without quality, except that a crop may be up to 1000000 pixels wide and high
+ * (libpng's user limits: cv2.imencode fails beyond them too).  cap = sqdet_png_max_bytes(h, w) fits
+ * every crop of h x w or less.
+ * sqdet_png_max_bytes: the largest file of an h x w image, about 9/8 of its 3 h w + h bytes of
+ * filtered data (-1 for h or w outside [1, 1000000]).  sqdet_png_scratch_bytes: the scratch of that
+ * call (-1 when its sizes are refused as sqdet_encode_png refuses them).  Both are worst cases, so
+ * that no launch size waits for the device: for 1920 x 1080, about 7 MB of output and about 26 MB of
+ * scratch per frame; frames run in groups of 16 that reuse one scratch, so the scratch is that of
+ * the largest group.                                                                      */
+int64_t sqdet_png_max_bytes(int h, int w);
+int64_t sqdet_png_scratch_bytes(int n, const int32_t* heights, const int32_t* widths,
+                                const int32_t* crops);
+int sqdet_encode_png(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
+                     const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                     uint8_t* out_dev, int64_t cap, int64_t* lengths_dev, void* scratch_dev,
+                     int64_t scratch_bytes, void* stream);
+
 /* ---- JPEG decoding into frames in device memory (no engine needed) -----------------
  * sqdet_decode_jpeg: file i becomes exactly the pixels of cv2.imdecode(file, cv2.IMREAD_COLOR)
  * (cv2's bundled libjpeg-turbo at its defaults: its SIMD islow IDCT, fancy upsampling, EXIF

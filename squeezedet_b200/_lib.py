@@ -131,6 +131,9 @@ SIGNATURES = {
     'sqdet_jpeg_max_bytes': (_i64, [_i, _i]),
     'sqdet_jpeg_scratch_bytes': (_i64, [_i, _vp, _vp, _vp]),
     'sqdet_encode_jpeg': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i64, _vp, _vp, _i64, _vp]),
+    'sqdet_png_max_bytes': (_i64, [_i, _i]),
+    'sqdet_png_scratch_bytes': (_i64, [_i, _vp, _vp, _vp]),
+    'sqdet_encode_png': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp]),
     'sqdet_jpeg_parse': (_i, [_vp, _i64, C.POINTER(JpegInfo)]),
     'sqdet_jpeg_decode_staging_bytes': (_i64, [_i, _vp, _vp]),
     'sqdet_jpeg_decode_scratch_bytes': (_i64, [_i, _vp, _vp]),

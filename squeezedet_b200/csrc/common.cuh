@@ -124,6 +124,13 @@ bool device_range_ok(const void* p, int64_t bytes, int device);
 // The crop r = (x, y, w, h) of an H x W frame, or the whole frame when r is null, into s.x, s.y,
 // s.w and s.h; refuses an empty crop or one outside the frame, naming `which`.
 int check_crop(const std::string& which, int64_t H, int64_t W, const int32_t* r, FrameSource& s);
+// The crops of an encoder's n frames (heights[i] x widths[i], crops as check_crop takes them) into
+// fr, or a refusal naming the call: n outside [1, max_frames], an empty frame, a crop that
+// check_crop refuses, or one wider or higher than max_side, which the file `format` (its name, as
+// the message gives it) cannot hold.  Host arrays only: the encoders' size functions call it too.
+int encode_crops(const std::string& name, const char* format, int max_frames, int max_side, int n,
+                 const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                 std::vector<FrameSource>& fr);
 // accept_frames' device: the one plane 0 of frame 0 is on.
 constexpr int kFrame0Device = -1;
 // Every check of n frames in format pf before any device work, filling fr or refusing with a

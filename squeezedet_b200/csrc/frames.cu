@@ -227,6 +227,25 @@ int check_crop(const std::string& which, int64_t H, int64_t W, const int32_t* r,
   return SQDET_OK;
 }
 
+int encode_crops(const std::string& name, const char* format, int max_frames, int max_side, int n,
+                 const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                 std::vector<FrameSource>& fr) {
+  if (!heights || !widths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (n < 1 || n > max_frames)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(max_frames) + "]");
+  fr.assign((size_t)n, FrameSource{});
+  for (int i = 0; i < n; ++i) {
+    const std::string which = name + ": frame " + std::to_string(i);
+    if (heights[i] <= 0 || widths[i] <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
+    const int rc = check_crop(which, heights[i], widths[i], crops ? crops + 4 * i : nullptr, fr[(size_t)i]);
+    if (rc) return rc;
+    if (fr[(size_t)i].w > max_side || fr[(size_t)i].h > max_side)
+      return fail(SQDET_ERR_INVALID_ARG, which + ": a " + format + " is at most " +
+                                             std::to_string(max_side) + " pixels wide and high");
+  }
+  return SQDET_OK;
+}
+
 int accept_frames(const std::string& name, const PixFormat& pf, int n,
                   const uint8_t* const* planes, const int64_t* pitches, const int32_t* heights,
                   const int32_t* widths, const int32_t* crops,

@@ -1,8 +1,8 @@
 // The per-format pixel fetch of uint8 frames in any SQDET_FMT_* format, shared by the kernels that
 // read frames without writing a BGR copy (frames.cu: resize + mean subtraction into tensor 0;
-// jpeg.cu: JPEG encoding).  A FrameDesc<P> holds a crop's P planes at its origin, taps<F> turns it
-// into the format's fetch, and each fetch converts to B, G, R as the format's cv2.cvtColor code
-// does.
+// jpeg.cu, png.cu: JPEG and PNG encoding).  A FrameDesc<P> holds a crop's P planes at its origin,
+// taps<F> turns it into the format's fetch, and each fetch converts to B, G, R as the format's
+// cv2.cvtColor code does.
 #pragma once
 #include "common.cuh"
 
@@ -110,6 +110,15 @@ __device__ __forceinline__ auto taps(const FrameDesc<kPlanes<F>>& f) {
   else
     return Yuv420Taps<false>{f.plane[0], f.plane[1], f.pitch[0], f.pitch[1], f.x_odd, f.y_odd, {},
                              f.plane[2], f.pitch[2]};
+}
+
+// The B, G, R bytes of crop pixel (y, x).
+template <class Taps>
+__device__ __forceinline__ void fetch_bgr(const Taps& tp, int y, int x, int& b, int& g, int& r) {
+  const int ys[2] = {y, y}, xs[2] = {x, x};
+  b = (int)tp(ys, xs, 0, 0, 0);
+  g = (int)tp(ys, xs, 0, 0, 1);
+  r = (int)tp(ys, xs, 0, 0, 2);
 }
 
 // The byte of plane p at the origin of frame s's crop.

@@ -27,6 +27,7 @@
 #include <cstring>
 
 #include "frames.cuh"
+#include "scan.cuh"
 
 namespace sqdet {
 namespace {
@@ -214,15 +215,6 @@ __device__ __forceinline__ void fdct8(int* d, int stride) {
   d[stride] = desc(t7 * 12299 + a1 + a4, SH);
 }
 
-// The B, G, R bytes of crop pixel (y, x).
-template <class Taps>
-__device__ __forceinline__ void fetch_bgr(const Taps& tp, int y, int x, int& b, int& g, int& r) {
-  const int ys[2] = {y, y}, xs[2] = {x, x};
-  b = (int)tp(ys, xs, 0, 0, 0);
-  g = (int)tp(ys, xs, 0, 0, 1);
-  r = (int)tp(ys, xs, 0, 0, 2);
-}
-
 // rgb_ycc_convert: 16 fraction bits, Cb and Cr rounded with ONE_HALF - 1.
 __device__ __forceinline__ int to_y(int b, int g, int r) {
   return (19595 * r + 38470 * g + 7471 * b + 32768) >> 16;
@@ -297,35 +289,6 @@ __global__ void __launch_bounds__(kChunk) transform_kernel(const __grid_constant
   int4* o4 = reinterpret_cast<int4*>(tp.p.coef + gb * 64);
 #pragma unroll
   for (int i = 0; i < 8; ++i) o4[i] = reinterpret_cast<const int4*>(z)[i];
-}
-
-// ---- block-wide scans ---------------------------------------------------------------------------
-// Exclusive scan of v over the CTA's threads (blockDim.x a multiple of 32, at most 1024); *total
-// gets the sum.  Ends with a barrier, so `warp` may be reused right after.
-__device__ int64_t block_exclusive_scan(int64_t v, int64_t* warp, int64_t* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  int64_t x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int64_t y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    int64_t w = lane < nw ? warp[lane] : 0;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int64_t y = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += y;
-    }
-    if (lane < nw) warp[lane] = w;
-  }
-  __syncthreads();
-  const int64_t before = (wid ? warp[wid - 1] : 0) + x - v;
-  *total = warp[nw - 1];
-  __syncthreads();
-  return before;
 }
 
 // ---- 2. code lengths and chunk sums -------------------------------------------------------------
@@ -694,25 +657,6 @@ int launch_encode_jpeg(int format, const FrameSource* frames, int n, int quality
   return SQDET_OK;
 }
 
-// The crops (x, y, w, h) of sqdet_encode_jpeg's frames, or a refusal naming the first that is empty,
-// outside its frame or longer than libjpeg writes.
-int jpeg_crops(const std::string& name, int n, const int32_t* heights, const int32_t* widths,
-               const int32_t* crops, std::vector<FrameSource>& fr) {
-  if (!heights || !widths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  if (n < 1 || n > kMaxJpegFrames)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxJpegFrames) + "]");
-  fr.assign((size_t)n, FrameSource{});
-  for (int i = 0; i < n; ++i) {
-    const std::string which = name + ": frame " + std::to_string(i);
-    if (heights[i] <= 0 || widths[i] <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
-    const int rc = check_crop(which, heights[i], widths[i], crops ? crops + 4 * i : nullptr, fr[(size_t)i]);
-    if (rc) return rc;
-    if (fr[(size_t)i].w > kJpegMaxSide || fr[(size_t)i].h > kJpegMaxSide)
-      return fail(SQDET_ERR_INVALID_ARG, which + ": a JPEG is at most 65500 pixels wide and high");
-  }
-  return SQDET_OK;
-}
-
 }  // namespace
 }  // namespace sqdet
 
@@ -729,7 +673,8 @@ int64_t sqdet_jpeg_max_bytes(int h, int w) {
 int64_t sqdet_jpeg_scratch_bytes(int n, const int32_t* heights, const int32_t* widths,
                                  const int32_t* crops) {
   std::vector<FrameSource> fr;
-  if (jpeg_crops("sqdet_jpeg_scratch_bytes", n, heights, widths, crops, fr)) return -1;
+  if (encode_crops("sqdet_jpeg_scratch_bytes", "JPEG", kMaxJpegFrames, kJpegMaxSide, n, heights, widths, crops, fr))
+    return -1;
   return jpeg_scratch_bytes(fr.data(), n);
 }
 
@@ -743,7 +688,7 @@ int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int
   if (!planes || !heights || !widths || !out_dev || !lengths_dev || !scratch_dev)
     return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
   std::vector<FrameSource> fr;
-  int rc = jpeg_crops(name, n, heights, widths, crops, fr);
+  int rc = encode_crops(name, "JPEG", kMaxJpegFrames, kJpegMaxSide, n, heights, widths, crops, fr);
   if (rc) return rc;
   if (quality < 1 || quality > 100) return fail(SQDET_ERR_INVALID_ARG, name + ": quality must be in [1, 100]");
   if (cap < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": cap must be at least 1");
