@@ -636,6 +636,72 @@ int sqdet_decode_jpeg(int n, const uint8_t* const* files_host, const int64_t* le
  * for the value set when they were called.                                                    */
 int sqdet_jpeg_decode_set_subsequence_bits(int bits);
 
+/* ---- KITTI 2-D object scoring of filtered records (no engine needed) ---------------
+ * sqdet_kitti_eval scores n images of records exactly as the KITTI devkit's evaluate_object does
+ * the detection files eval.py writes from them (see oracle/kitti_eval.py for the rules): for each
+ * class (car, pedestrian, cyclist) and difficulty (easy, moderate, hard), index 3 * class +
+ * difficulty, it gives the threshold count and, per threshold, TP, FP, FN and the similarity sum
+ * in image order.  The host forms precision = tp / (double)(tp + fp), aos = similarity /
+ * (double)(tp + fp), their suffix maxima and the AP from these (squeezedet_b200.kitti).
+ *
+ * dets [n, max_dets] and counts [n]: records as the engine writes them, in device memory.
+ * class_map [classes] (host): per class id, SQDET_KITTI_CAR / _PEDESTRIAN / _CYCLIST, or -1 for a
+ * class the devkit never evaluates; at most one id per KITTI class.  objs [n_objects] and
+ * offsets [n + 1] (device): image i's label lines are objs[offsets[i] .. offsets[i + 1]) in file
+ * order, with aos_term = (1 + cos(alpha)) / 2 computed by the caller.  scratch: 256-byte aligned,
+ * sqdet_kitti_eval_scratch_bytes(n, max_dets, n_objects) bytes (-1 for sizes refused as below).
+ * out: one sqdet_kitti_result in device memory.  Everything runs on `stream`, with no host wait.
+ *
+ * Refused with SQDET_ERR_INVALID_ARG before any launch: n < 1, max_dets outside [1, 1024], null
+ * pointers, a bad class map, buffers not on one device.  A record that cannot be scored sets
+ * out->status to 8 * image + reason (the first image; -1 when every record is usable): a count
+ * outside [0, max_dets] (the filter's -1 overflow marker included), a class id outside the map,
+ * a non-finite box or prob, a prob outside [0, 1], offsets that are not increasing in
+ * [0, n_objects].  The other outputs are then meaningless, but nothing outside the arguments is
+ * read: an image whose offsets are refused is scored as having no objects.                  */
+#define SQDET_KITTI_CAR             0
+#define SQDET_KITTI_PEDESTRIAN      1
+#define SQDET_KITTI_CYCLIST         2
+#define SQDET_KITTI_VAN             3
+#define SQDET_KITTI_PERSON_SITTING  4
+#define SQDET_KITTI_DONTCARE        5
+#define SQDET_KITTI_OTHER           6
+#define SQDET_KITTI_MAX_THRESHOLDS 41
+#define SQDET_KITTI_MAX_CLASSES    64
+/* out->status reasons */
+#define SQDET_KITTI_BAD_COUNT       1
+#define SQDET_KITTI_BAD_CLASS       2
+#define SQDET_KITTI_NOT_FINITE      3
+#define SQDET_KITTI_BAD_SCORE       4
+#define SQDET_KITTI_BAD_OFFSETS     5
+#define SQDET_KITTI_TOO_MANY_THRESHOLDS 6   /* never: at most 41 thresholds exist */
+
+typedef struct sqdet_kitti_obj {   /* one label line (56 bytes) */
+  double  x1, y1, x2, y2;          /* box, as strtod reads it */
+  double  truncation;
+  double  aos_term;                /* (1 + cos(alpha)) / 2 */
+  int32_t type;                    /* SQDET_KITTI_* type code, case-insensitive */
+  int32_t occlusion;
+} sqdet_kitti_obj;
+
+typedef struct sqdet_kitti_result {
+  double  similarity[9][SQDET_KITTI_MAX_THRESHOLDS];
+  int32_t tp[9][SQDET_KITTI_MAX_THRESHOLDS];
+  int32_t fp[9][SQDET_KITTI_MAX_THRESHOLDS];
+  int32_t fn[9][SQDET_KITTI_MAX_THRESHOLDS];
+  int32_t n_thresholds[9];
+  int32_t n_gt[9];
+  int32_t evaluated[3];            /* a usable record of the class exists */
+  int32_t status;
+  int32_t reserved;                /* pads the struct to a multiple of 8 bytes (7472) */
+} sqdet_kitti_result;
+
+int64_t sqdet_kitti_eval_scratch_bytes(int n, int max_dets, int64_t n_objects);
+int sqdet_kitti_eval(int n, int max_dets, const sqdet_det* dets, const int32_t* counts,
+                     int classes, const int32_t* class_map, const sqdet_kitti_obj* objs,
+                     const int64_t* offsets, int64_t n_objects, void* scratch,
+                     int64_t scratch_bytes, sqdet_kitti_result* out, void* stream);
+
 /* ---- tiny device-memory helpers so a ctypes caller needs nothing else -------------- */
 int sqdet_malloc(int device, int64_t bytes, void** out_dev);
 int sqdet_free(int device, void* dev);

@@ -1,0 +1,425 @@
+// The KITTI 2-D object scorer (the reference's evaluate_object, src/dataset/kitti-eval/cpp/
+// evaluate_object.cpp, restated in oracle/kitti_eval.py) on the engine's filtered records: the
+// per-(class, difficulty, threshold) TP / FP / FN counts and ordered similarity sums from which
+// the host forms precision, AOS and AP exactly as the binary does.  Five launches on the caller's
+// stream, no host wait:
+//   prepare_kernel    the values the binary reads back from eval.py's text (corners
+//                     rint(v * 100) / 100, scores k / 1000 as bins k), class codes, record checks
+//   recall_kernel     one warp per (image, class, difficulty): computeStatistics without FP
+//                     (:345-437) into a 1001-bin histogram of TP scores, and n_gt
+//   threshold_kernel  one CTA per (class, difficulty): getThresholds (:239-272) as a histogram
+//                     suffix sum and one binary search per threshold
+//   pr_kernel         one warp per (image, class, difficulty): computeStatistics with FP
+//                     (:345-498) at each threshold
+//   sum_kernel        the similarity of each threshold summed in image order (:540-555)
+// In the warp kernels the gt loop is serial and lane l owns detections l, l + 32, ..., so with at
+// most 1024 records per image each lane's assigned flags are one 32-bit word.  Every double
+// operation whose rounding decides a comparison is an explicit _rn intrinsic, so --fmad=true
+// cannot contract it.
+#include "common.cuh"
+
+namespace sqdet {
+namespace {
+
+constexpr int kCd = 9;                  // 3 classes x 3 difficulties, index 3 * class + difficulty
+constexpr int kBins = 1001;             // scores k / 1000, k in 0..1000
+constexpr int kMaxThresholds = SQDET_KITTI_MAX_THRESHOLDS;
+constexpr int kMaxDets = 1024;
+constexpr int kWarpsPerBlock = 8;
+
+// class id k -> 0 car, 1 pedestrian, 2 cyclist or -1, stored + 1 in 2 bits at bit 2 (k % 32) of
+// word k / 32 (no array, so reading it needs no stack frame)
+struct ClassMap {
+  uint64_t lo, hi;
+  int classes;
+  __device__ int code(int k) const { return (int)(((k < 32 ? lo : hi) >> (2 * (k & 31))) & 3) - 1; }
+};
+
+struct Scratch {
+  double* box;          // [n * max_dets][4] x1 y1 x2 y2 as the binary reads them
+  int32_t* meta;        // [n * max_dets] code << 16 | score bin, or -1 (not car/pedestrian/cyclist)
+  int32_t* hist;        // [kCd][kBins] TP scores of the recall pass
+  int32_t* thr;         // [kCd][kMaxThresholds] threshold score bins
+  double* sim;          // [kCd][kMaxThresholds][n] per-image similarity
+};
+
+inline int64_t align256(int64_t b) { return (b + 255) & ~int64_t(255); }
+
+Scratch carve(void* base, int n, int max_dets) {
+  char* p = static_cast<char*>(base);
+  const int64_t recs = (int64_t)n * max_dets;
+  Scratch s;
+  s.box = reinterpret_cast<double*>(p);  p += align256(recs * 32);
+  s.meta = reinterpret_cast<int32_t*>(p); p += align256(recs * 4);
+  s.hist = reinterpret_cast<int32_t*>(p); p += align256(kCd * kBins * 4);
+  s.thr = reinterpret_cast<int32_t*>(p);  p += align256(kCd * kMaxThresholds * 4);
+  s.sim = reinterpret_cast<double*>(p);
+  return s;
+}
+
+int64_t scratch_bytes(int n, int max_dets) {
+  const int64_t recs = (int64_t)n * max_dets;
+  return align256(recs * 32) + align256(recs * 4) + align256(kCd * kBins * 4) +
+         align256(kCd * kMaxThresholds * 4) + align256((int64_t)kCd * kMaxThresholds * n * 8);
+}
+
+__device__ __forceinline__ void refuse(sqdet_kitti_result* out, int image, int reason) {
+  atomicMin(reinterpret_cast<unsigned*>(&out->status), (unsigned)(image * 8 + reason));
+}
+
+// std::max / std::min as the binary calls them: (a < b) ? b : a and (b < a) ? b : a
+__device__ __forceinline__ double dmax(double a, double b) { return a < b ? b : a; }
+__device__ __forceinline__ double dmin(double a, double b) { return b < a ? b : a; }
+
+// boxoverlap (:203-237): criterion -1 (union) for det vs gt, 0 (det area) for det vs DontCare
+template <bool kUnion>
+__device__ __forceinline__ double box_overlap(const double* a, const sqdet_kitti_obj& b) {
+  const double w = __dsub_rn(dmin(a[2], b.x2), dmax(a[0], b.x1));
+  const double h = __dsub_rn(dmin(a[3], b.y2), dmax(a[1], b.y1));
+  if (w <= 0 || h <= 0) return 0;
+  const double inter = __dmul_rn(w, h);
+  const double a_area = __dmul_rn(__dsub_rn(a[2], a[0]), __dsub_rn(a[3], a[1]));
+  if (!kUnion) return __ddiv_rn(inter, a_area);
+  const double b_area = __dmul_rn(__dsub_rn(b.x2, b.x1), __dsub_rn(b.y2, b.y1));
+  return __ddiv_rn(inter, __dsub_rn(__dadd_rn(a_area, b_area), inter));
+}
+
+__device__ __forceinline__ double min_overlap(int c) { return c == 0 ? 0.7 : 0.5; }   // :37
+
+// cleanData's ignored_gt entry (:277-320): 0 counted, 1 ignored, -1 skipped
+__device__ __forceinline__ int gt_state(const sqdet_kitti_obj& g, int c, int d) {
+  const int valid = g.type == c ? 1
+                  : ((c == 0 && g.type == SQDET_KITTI_VAN) ||
+                     (c == 1 && g.type == SQDET_KITTI_PERSON_SITTING)) ? 0 : -1;
+  const int min_height = d == 0 ? 40 : 25;                          // :28
+  const double max_trunc = d == 0 ? 0.15 : d == 1 ? 0.3 : 0.5;      // :30
+  const double height = __dsub_rn(g.y2, g.y1);
+  const bool ignore = g.occlusion > d || g.truncation > max_trunc || height < min_height;   // :29
+  if (valid == 1 && !ignore) return 0;
+  if (valid == 0 || (ignore && valid == 1)) return 1;
+  return -1;
+}
+
+__device__ __forceinline__ int clamp_count(int c, int max_dets) {
+  return c < 0 ? 0 : c > max_dets ? max_dets : c;
+}
+
+__device__ __forceinline__ bool bad_range(int64_t a, int64_t b, int64_t n_objects) {
+  return a < 0 || b < a || b > n_objects;
+}
+
+// Image i's objects [g0, g1): empty when its offsets are refused, so that a bad range only sets
+// the status word and no kernel reads outside objs (which may be null when n_objects is 0).
+__device__ __forceinline__ void object_range(const int64_t* offsets, int i, int64_t n_objects,
+                                             int64_t& g0, int64_t& g1) {
+  g0 = offsets[i];
+  g1 = offsets[i + 1];
+  if (bad_range(g0, g1, n_objects)) g0 = g1 = 0;
+}
+
+// One thread per record: what the binary reads back from `{:.2f}` / `{:.3f}` of the float32
+// values (v * 100 and p * 1000 are exact in double, so rint, round-half-even like Python's
+// formatting of exact ties, gives the printed decimal; divided back it is strtod's double).
+__global__ void prepare_kernel(const sqdet_det* __restrict__ dets, const int32_t* __restrict__ counts,
+                               const int64_t* __restrict__ offsets, int64_t n_objects, int n,
+                               int max_dets, ClassMap map, Scratch s, sqdet_kitti_result* out) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= (int64_t)n * max_dets) return;
+  const int i = (int)(r / max_dets), j = (int)(r % max_dets);
+  const int count = counts[i];
+  if (j == 0) {
+    if (count < 0 || count > max_dets) refuse(out, i, SQDET_KITTI_BAD_COUNT);
+    const int64_t a = offsets[i], b = offsets[i + 1];
+    if (bad_range(a, b, n_objects)) refuse(out, i, SQDET_KITTI_BAD_OFFSETS);
+  }
+  s.meta[r] = -1;
+  if (j >= count) return;
+  const sqdet_det d = dets[r];
+  if (d.cls < 0 || d.cls >= map.classes) { refuse(out, i, SQDET_KITTI_BAD_CLASS); return; }
+  if (!isfinite(d.prob) || !isfinite(d.cx) || !isfinite(d.cy) || !isfinite(d.w) ||
+      !isfinite(d.h)) { refuse(out, i, SQDET_KITTI_NOT_FINITE); return; }
+  if (!(d.prob >= 0.f && d.prob <= 1.f)) { refuse(out, i, SQDET_KITTI_BAD_SCORE); return; }
+  // bbox_transform in float32 (utils/util.py): cx - w / 2 etc., not contracted
+  const float hw = __fdiv_rn(d.w, 2.f), hh = __fdiv_rn(d.h, 2.f);
+  const float v[4] = {__fsub_rn(d.cx, hw), __fsub_rn(d.cy, hh), __fadd_rn(d.cx, hw),
+                      __fadd_rn(d.cy, hh)};
+  double* box = s.box + r * 4;
+  for (int k = 0; k < 4; ++k) {
+    const double c = rint(__dmul_rn((double)v[k], 100.0));
+    if (!isfinite(c)) { refuse(out, i, SQDET_KITTI_NOT_FINITE); return; }
+    box[k] = __ddiv_rn(c, 100.0);
+  }
+  const int code = map.code(d.cls);
+  if (code < 0) return;
+  const int bin = (int)rint(__dmul_rn((double)d.prob, 1000.0));
+  s.meta[r] = code << 16 | bin;
+  out->evaluated[code] = 1;
+}
+
+// The recall pass (computeStatistics, compute_fp = false): each gt that is not skipped takes the
+// unassigned detection of its class overlapping it by more than the minimum with the highest
+// score, the first index on equal scores; a TP puts its score bin into the histogram.
+__global__ void __launch_bounds__(kWarpsPerBlock * 32)
+recall_kernel(const int32_t* __restrict__ counts, const sqdet_kitti_obj* __restrict__ objs,
+              const int64_t* __restrict__ offsets, int64_t n_objects, int n, int max_dets, Scratch s,
+              sqdet_kitti_result* out) {
+  const int w = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (w >= n * kCd) return;
+  const int i = w / kCd, cd = w % kCd, c = cd / 3, d = cd % 3;
+  const int count = clamp_count(counts[i], max_dets);
+  const int slots = (count + 31) >> 5;
+  const int64_t base = (int64_t)i * max_dets;
+  const double minov = min_overlap(c);
+  uint32_t assigned = 0;
+  int n_gt = 0;
+  int64_t g0, g1;
+  object_range(offsets, i, n_objects, g0, g1);
+  for (int64_t g = g0; g < g1; ++g) {
+    const sqdet_kitti_obj gt = objs[g];
+    const int st = gt_state(gt, c, d);
+    if (st == -1) continue;
+    n_gt += st == 0;
+    uint32_t key = 0;                  // (bin + 1) << 10 | (1023 - j): max = best score, first j
+    for (int k = 0; k < slots; ++k) {
+      const int j = lane + 32 * k;
+      if (j >= count || (assigned >> k & 1)) continue;
+      const int m = s.meta[base + j];
+      if (m < 0 || (m >> 16) != c) continue;
+      const uint32_t cand = (uint32_t)((m & 0xffff) + 1) << 10 | (uint32_t)(1023 - j);
+      if (cand > key && box_overlap<true>(s.box + (base + j) * 4, gt) > minov) key = cand;
+    }
+    key = __reduce_max_sync(0xffffffffu, key);
+    if (key == 0) continue;                                     // an FN when st == 0
+    const int j = 1023 - (int)(key & 1023);
+    if ((j & 31) == lane) assigned |= 1u << (j >> 5);
+    if (st == 0 && lane == 0) atomicAdd(&s.hist[cd * kBins + (int)(key >> 10) - 1], 1);
+  }
+  if (lane == 0 && n_gt) atomicAdd(&out->n_gt[cd], n_gt);
+}
+
+// getThresholds: v (the TP scores) in descending order is the histogram read from bin 1000 down,
+// so v[i] is the bin b with above[b + 1] <= i < above[b], above[b] = TPs scoring b or more.  Index
+// i is skipped while it is not the last and (i + 2) / n - r < r - (i + 1) / n; both sides move
+// monotonically with i, so the next index taken is one binary search.  r is the binary's running
+// sum of 1 / 40.
+__global__ void __launch_bounds__(1024) threshold_kernel(Scratch s, sqdet_kitti_result* out) {
+  __shared__ int above[kBins + 1];
+  const int cd = blockIdx.x;
+  for (int b = threadIdx.x; b <= kBins; b += blockDim.x)
+    above[b] = b < kBins ? s.hist[cd * kBins + b] : 0;
+  __syncthreads();
+  for (int step = 1; step < kBins; step <<= 1) {       // suffix sum, Hillis-Steele
+    int v[2] = {0, 0};
+    for (int t = 0; t < 2; ++t) {
+      const int b = threadIdx.x + t * blockDim.x;
+      if (b < kBins) v[t] = above[b] + (b + step < kBins ? above[b + step] : 0);
+    }
+    __syncthreads();
+    for (int t = 0; t < 2; ++t) {
+      const int b = threadIdx.x + t * blockDim.x;
+      if (b < kBins) above[b] = v[t];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x != 0) return;
+  const int nv = above[0];
+  const double n = (double)out->n_gt[cd];
+  double r = 0;
+  int nt = 0;
+  auto skipped = [&](int i) {
+    if (i >= nv - 1) return false;
+    return __dsub_rn(__ddiv_rn((double)(i + 2), n), r) < __dsub_rn(r, __ddiv_rn((double)(i + 1), n));
+  };
+  for (int i = 0; i < nv; ++i) {
+    int lo = i, hi = nv - 1;                 // the first index not skipped, in [i, nv - 1]
+    while (lo < hi) {
+      const int mid = lo + (hi - lo) / 2;
+      if (skipped(mid)) lo = mid + 1; else hi = mid;
+    }
+    i = lo;
+    int bl = 0, bh = kBins - 1;              // the largest bin b with above[b] > i
+    while (bl < bh) {
+      const int mid = bl + (bh - bl + 1) / 2;
+      if (above[mid] > i) bl = mid; else bh = mid - 1;
+    }
+    if (nt == kMaxThresholds) {              // cannot happen (oracle/kitti_eval.get_thresholds)
+      refuse(out, 0, SQDET_KITTI_TOO_MANY_THRESHOLDS);
+      break;
+    }
+    s.thr[cd * kMaxThresholds + nt++] = bl;
+    r = __dadd_rn(r, 1.0 / 40.0);
+  }
+  out->n_thresholds[cd] = nt;
+}
+
+// The PR pass (computeStatistics, compute_fp = true) at each threshold: detections scoring below
+// it are left out, each gt takes the unassigned detection with the largest overlap above the
+// minimum (the first index on equal overlaps), and FP counts the eligible detections left
+// unassigned that no DontCare box holds by more than the minimum.  The similarity is 0.0 plus
+// each TP's gt term in gt order.
+__global__ void __launch_bounds__(kWarpsPerBlock * 32)
+pr_kernel(const int32_t* __restrict__ counts, const sqdet_kitti_obj* __restrict__ objs,
+          const int64_t* __restrict__ offsets, int64_t n_objects, int n, int max_dets, Scratch s,
+          sqdet_kitti_result* out) {
+  const int w = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (w >= n * kCd) return;
+  const int i = w / kCd, cd = w % kCd, c = cd / 3, d = cd % 3;
+  const int nt = out->n_thresholds[cd];
+  if (nt == 0) return;
+  const int count = clamp_count(counts[i], max_dets);
+  const int slots = (count + 31) >> 5;
+  const int64_t base = (int64_t)i * max_dets;
+  int64_t g0, g1;
+  object_range(offsets, i, n_objects, g0, g1);
+  const double minov = min_overlap(c);
+  uint32_t mine = 0, stuff = 0;          // this lane's detections of class c; held by DontCare
+  for (int k = 0; k < slots; ++k) {
+    const int j = lane + 32 * k;
+    if (j >= count) break;
+    const int m = s.meta[base + j];
+    if (m < 0 || (m >> 16) != c) continue;
+    mine |= 1u << k;
+    for (int64_t g = g0; g < g1; ++g) {
+      const sqdet_kitti_obj gt = objs[g];
+      if (gt.type == SQDET_KITTI_DONTCARE && box_overlap<false>(s.box + (base + j) * 4, gt) > minov) {
+        stuff |= 1u << k;
+        break;
+      }
+    }
+  }
+  for (int t = 0; t < nt; ++t) {
+    const int thr = s.thr[cd * kMaxThresholds + t];
+    uint32_t elig = 0;
+    for (int k = 0; k < slots; ++k)
+      if ((mine >> k & 1) && (s.meta[base + lane + 32 * k] & 0xffff) >= thr) elig |= 1u << k;
+    uint32_t assigned = 0;
+    int tp = 0, fn = 0;
+    double sim = 0;
+    for (int64_t g = g0; g < g1; ++g) {
+      const sqdet_kitti_obj gt = objs[g];
+      const int st = gt_state(gt, c, d);
+      if (st == -1) continue;
+      double best = 0;
+      int bj = kMaxDets;
+      for (int k = 0; k < slots; ++k) {
+        if (!((elig & ~assigned) >> k & 1)) continue;
+        const int j = lane + 32 * k;
+        const double o = box_overlap<true>(s.box + (base + j) * 4, gt);
+        if (o > minov && o > best) { best = o; bj = j; }
+      }
+      for (int off = 16; off; off >>= 1) {
+        const double ob = __shfl_xor_sync(0xffffffffu, best, off);
+        const int oj = __shfl_xor_sync(0xffffffffu, bj, off);
+        if (ob > best || (ob == best && oj < bj)) { best = ob; bj = oj; }
+      }
+      if (bj == kMaxDets) {
+        fn += st == 0;
+        continue;
+      }
+      if ((bj & 31) == lane) assigned |= 1u << (bj >> 5);
+      if (st == 0) {
+        ++tp;
+        sim = __dadd_rn(sim, gt.aos_term);
+      }
+    }
+    int fp = __popc(elig & ~assigned & ~stuff);
+    for (int off = 16; off; off >>= 1) fp += __shfl_xor_sync(0xffffffffu, fp, off);
+    if (lane == 0) {
+      const int o = cd * kMaxThresholds + t;
+      if (tp) atomicAdd(&out->tp[0][0] + o, tp);
+      if (fp) atomicAdd(&out->fp[0][0] + o, fp);
+      if (fn) atomicAdd(&out->fn[0][0] + o, fn);
+      s.sim[(int64_t)o * n + i] = sim;
+    }
+  }
+}
+
+// pr[t].similarity += the image's similarity, in image order (a sum of +0.0 changes nothing, so
+// the images without TP or FP, whose similarity the binary skips, add their 0.0)
+__global__ void sum_kernel(int n, Scratch s, sqdet_kitti_result* out) {
+  const int o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= kCd * kMaxThresholds || o % kMaxThresholds >= out->n_thresholds[o / kMaxThresholds]) return;
+  const double* p = s.sim + (int64_t)o * n;
+  double sum = 0;
+  for (int i = 0; i < n; ++i) sum = __dadd_rn(sum, p[i]);
+  (&out->similarity[0][0])[o] = sum;
+}
+
+}  // namespace
+}  // namespace sqdet
+
+using namespace sqdet;
+
+int64_t sqdet_kitti_eval_scratch_bytes(int n, int max_dets, int64_t n_objects) {
+  if (n < 1 || max_dets < 1 || max_dets > kMaxDets || n_objects < 0) {
+    fail(SQDET_ERR_INVALID_ARG, "sqdet_kitti_eval_scratch_bytes: need n >= 1, max_dets in "
+                                "[1, 1024] and n_objects >= 0");
+    return -1;
+  }
+  return scratch_bytes(n, max_dets);
+}
+
+int sqdet_kitti_eval(int n, int max_dets, const sqdet_det* dets, const int32_t* counts,
+                     int classes, const int32_t* class_map, const sqdet_kitti_obj* objs,
+                     const int64_t* offsets, int64_t n_objects, void* scratch,
+                     int64_t scratch_bytes_, sqdet_kitti_result* out, void* stream) {
+  const std::string name = "sqdet_kitti_eval";
+  if (n < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": n must be at least 1");
+  if (max_dets < 1 || max_dets > kMaxDets)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": max_dets must be in [1, 1024]");
+  if (n_objects < 0) return fail(SQDET_ERR_INVALID_ARG, name + ": n_objects must be >= 0");
+  if (!dets || !counts || !class_map || !offsets || !scratch || !out || (n_objects && !objs))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (classes < 1 || classes > SQDET_KITTI_MAX_CLASSES)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": classes must be in [1, 64]");
+  ClassMap map{};
+  map.classes = classes;
+  int seen[3] = {0, 0, 0};
+  for (int k = 0; k < classes; ++k) {
+    const int v = class_map[k];
+    if (v < -1 || v > 2) return fail(SQDET_ERR_INVALID_ARG, name + ": class_map entries are -1, 0, 1 or 2");
+    // the detection files group lines by class id, so two ids of one KITTI class would order
+    // that class's detections differently from the records
+    if (v >= 0 && seen[v]++)
+      return fail(SQDET_ERR_INVALID_ARG, name + ": two class ids map to the same KITTI class");
+    (k < 32 ? map.lo : map.hi) |= (uint64_t)(v + 1) << (2 * (k & 31));
+  }
+  if ((uintptr_t)scratch % 256)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch must be 256-byte aligned");
+  if ((uintptr_t)out % alignof(double) || (uintptr_t)offsets % alignof(int64_t) ||
+      (uintptr_t)objs % alignof(double) || (uintptr_t)dets % alignof(int32_t) ||
+      (uintptr_t)counts % alignof(int32_t))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": misaligned argument");
+  if (scratch_bytes_ < scratch_bytes(n, max_dets))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below sqdet_kitti_eval_scratch_bytes");
+  const int device = pointer_device(dets);
+  if (device < 0 || !device_range_ok(dets, (int64_t)n * max_dets * sizeof(sqdet_det), device) ||
+      !device_range_ok(counts, (int64_t)n * 4, device) ||
+      !device_range_ok(offsets, (int64_t)(n + 1) * 8, device) ||
+      (n_objects && !device_range_ok(objs, n_objects * (int64_t)sizeof(sqdet_kitti_obj), device)) ||
+      !device_range_ok(scratch, scratch_bytes_, device) ||
+      !device_range_ok(out, sizeof(sqdet_kitti_result), device))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": dets, counts, objs, offsets, scratch and out must "
+                                              "each lie inside one allocation on one device");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the records' device");
+  cudaStream_t st = (cudaStream_t)stream;
+  const Scratch s = carve(scratch, n, max_dets);
+  SQ_CUDA(cudaMemsetAsync(out, 0, sizeof(sqdet_kitti_result), st));
+  SQ_CUDA(cudaMemsetAsync(&out->status, 0xff, sizeof(out->status), st));
+  SQ_CUDA(cudaMemsetAsync(s.hist, 0, kCd * kBins * 4, st));
+  const int64_t recs = (int64_t)n * max_dets;
+  prepare_kernel<<<(unsigned)((recs + 255) / 256), 256, 0, st>>>(dets, counts, offsets, n_objects, n,
+                                                                 max_dets, map, s, out);
+  SQ_CHECK_LAUNCH("kitti prepare_kernel");
+  const unsigned warp_blocks = (unsigned)(((int64_t)n * kCd + kWarpsPerBlock - 1) / kWarpsPerBlock);
+  recall_kernel<<<warp_blocks, kWarpsPerBlock * 32, 0, st>>>(counts, objs, offsets, n_objects, n, max_dets, s, out);
+  SQ_CHECK_LAUNCH("kitti recall_kernel");
+  threshold_kernel<<<kCd, 1024, 0, st>>>(s, out);
+  SQ_CHECK_LAUNCH("kitti threshold_kernel");
+  pr_kernel<<<warp_blocks, kWarpsPerBlock * 32, 0, st>>>(counts, objs, offsets, n_objects, n, max_dets, s, out);
+  SQ_CHECK_LAUNCH("kitti pr_kernel");
+  sum_kernel<<<(kCd * kMaxThresholds + 127) / 128, 128, 0, st>>>(n, s, out);
+  SQ_CHECK_LAUNCH("kitti sum_kernel");
+  return SQDET_OK;
+}

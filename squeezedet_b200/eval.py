@@ -12,17 +12,17 @@ filtered (filter_prediction + NMS on original-image coordinates, eval.py:86-87) 
 on the same engine.  Two groups are in flight on the GPU while a thread pool decodes the next one
 with cv2.imread.  Corner format + score go into all_boxes[cls][image].  Then the KITTI detection
 files are written
-(src/dataset/kitti.py:100-127) and the reference's unmodified `evaluate_object` binary
-(built by oracle/build_kitti_eval.sh) is invoked and its stats_*_ap.txt parsed
-(kitti.py:129-159).  The TensorBoard summaries and the checkpoint-polling loop
-(eval.py:171-239) are not rebuilt.
+(src/dataset/kitti.py:100-127), and the records, uploaded once as one [N, max_dets] array, are
+scored on the GPU (squeezedet_b200.kitti, byte for byte the files of the KITTI devkit's
+`evaluate_object`, which src/dataset/kitti.py:129-136 runs) into stats_*.txt next to `data/`,
+whose APs are parsed as the reference parses them (kitti.py:138-159).  The TensorBoard summaries
+and the checkpoint-polling loop (eval.py:171-239) are not rebuilt.
 """
 from __future__ import annotations
 
 import argparse
 import collections
 import os
-import subprocess
 import time
 from concurrent.futures import ThreadPoolExecutor
 
@@ -100,8 +100,10 @@ def _charge(timer, seconds, images):
   timer.average_time = timer.total_time / timer.calls
 
 
+# where oracle/build_kitti_eval.sh puts the devkit's own scorer, against which the tests check
+# the GPU scorer's files; eval_once does not run it
 EVAL_TOOL = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'oracle',
-                         '_ref', 'evaluate_object')   # built by oracle/build_kitti_eval.sh
+                         '_ref', 'evaluate_object')
 
 
 def eval_once(flags):
@@ -135,12 +137,16 @@ def eval_once(flags):
   # one pinned result slot per group in flight (pinned, so the copies back stay asynchronous)
   dets_buf = [PinnedArray((k, model.max_dets), DET_DTYPE) for _ in range(2)]
   counts_buf = [PinnedArray((k,), np.int32) for _ in range(2)]
+  # every image's records, for the scorer
+  all_dets = np.zeros((num_images, model.max_dets), DET_DTYPE)
+  all_counts = np.zeros((num_images,), np.int32)
 
   def collect(gi):
     """The results of group gi, after its wait()."""
     dets, counts = dets_buf[gi & 1].array, counts_buf[gi & 1].array
     for j, i in enumerate(groups[gi]):
       _t['misc'].tic()
+      all_dets[i], all_counts[i] = dets[j], counts[j]
       per_class = detections_to_all_boxes(dets[j], int(counts[j]), None, mc.CLASSES)
       for c in range(mc.CLASSES):
         all_boxes[c][i] = per_class[c]
@@ -185,21 +191,20 @@ def eval_once(flags):
 
   det_dir = os.path.join(flags.eval_dir, 'detection_files_{:s}'.format('0'), 'data')
   result_dir = write_kitti_detections(det_dir, image_ids, mc.CLASS_NAMES, all_boxes)
-  tool = EVAL_TOOL
-  aps = names = None
-  if os.path.exists(tool):
-    cmd = ' '.join([tool, os.path.join(flags.data_path, 'training'),
-                    os.path.join(flags.data_path, 'ImageSets', flags.image_set + '.txt'),
-                    result_dir, str(num_images)])
-    print('Running: {}'.format(cmd))
-    subprocess.call(cmd, shell=True)
-    aps, names = parse_kitti_ap_files(result_dir, mc.CLASS_NAMES)
-    for ap, name in zip(aps, names):
-      print('    {}: {:.3f}'.format(name, ap))
-    print('    Mean average precision: {:.3f}'.format(float(np.mean(aps))))
+  from . import kitti
+  try:
+    labels = kitti.read_labels(os.path.join(flags.data_path, 'training', 'label_2'), image_ids)
+  except (OSError, ValueError) as e:
+    # as evaluate_object did: an error naming the file, no stats files, APs of 0
+    print('ERROR: Couldn\'t read the ground truth: {}'.format(e))
   else:
-    print('KITTI scorer binary not found ({}; build it with oracle/build_kitti_eval.sh); '
-          'detection files are in {}'.format(tool, det_dir))
+    scores = kitti.evaluate_device(all_dets, all_counts, mc.CLASS_NAMES, labels,
+                                   device='cuda:{:d}'.format(int(flags.gpu)))
+    kitti.write_stats(result_dir, scores)
+  aps, names = parse_kitti_ap_files(result_dir, mc.CLASS_NAMES)
+  for ap, name in zip(aps, names):
+    print('    {}: {:.3f}'.format(name, ap))
+  print('    Mean average precision: {:.3f}'.format(float(np.mean(aps))))
   return all_boxes, aps, names
 
 
