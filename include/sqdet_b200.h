@@ -702,6 +702,62 @@ int sqdet_kitti_eval(int n, int max_dets, const sqdet_det* dets, const int32_t* 
                      const int64_t* offsets, int64_t n_objects, void* scratch,
                      int64_t scratch_bytes, sqdet_kitti_result* out, void* stream);
 
+/* ---- KITTI detection error analysis of filtered records (no engine needed) ----------
+ * sqdet_kitti_analyze classifies the records of n images exactly as the reference's
+ * analyze_detections (src/dataset/kitti.py:182-296, restated in oracle/kitti_analysis.py) does
+ * the detection files eval.py writes from them.  Per image, the ground truth is every label line
+ * of an analyzed class, in file order; the detections are the records as read back from the file
+ * (corners rint(v * 100) / 100, scores k / 1000), ranked by score, then class id, then record
+ * index, and only the first G count, G the image's ground-truth count.  Each counted detection is
+ * matched to the first object of largest IoU: correct (the first such detection of that object),
+ * repeated, localization, classification or background error.
+ *
+ * The arguments are those of sqdet_kitti_eval, except that every class id must name a distinct
+ * analyzed class (class_map entries 0, 1 or 2, so classes <= 3), plus `lines`, a device buffer of
+ * line_capacity error lines: in image order, each image's loc / cls / bg detections in ranked
+ * order and then its missed objects in label order.  2 x (objects of the analyzed classes) lines
+ * always fit; lines past line_capacity are counted in out->n_lines but not written.  scratch:
+ * 256-byte aligned, sqdet_kitti_analyze_scratch_bytes(n, max_dets, n_objects) bytes.
+ * Everything runs on `stream`, with no host wait.
+ *
+ * Refused with SQDET_ERR_INVALID_ARG before any launch as sqdet_kitti_eval refuses, and for a
+ * class map with a -1 entry.  out->status is 16 * image + reason for the first image refused
+ * (-1 when none is): the scorer's reasons, a record with w < 0 or h < 0 (the engine writes none;
+ * its IoU union can be 0), or a label box of an analyzed class that is not finite or fails the
+ * reference's assertions x1 >= 0, x1 <= x2, y1 >= 0, y1 <= y2.                               */
+#define SQDET_KITTI_NEGATIVE_SIZE   7
+#define SQDET_KITTI_BAD_LABEL       8
+/* error line types */
+#define SQDET_KITTI_ERR_LOC         0
+#define SQDET_KITTI_ERR_CLS         1
+#define SQDET_KITTI_ERR_BG          2
+#define SQDET_KITTI_ERR_MISSED      3
+
+typedef struct sqdet_kitti_error_line {   /* one line of det_error_file.txt (56 bytes) */
+  int32_t image;
+  int32_t type;                    /* SQDET_KITTI_ERR_* */
+  int32_t cls;                     /* class id */
+  int32_t reserved;
+  double  x1, y1, x2, y2;          /* cx - w / 2., cy - h / 2., cx + w / 2., cy + h / 2. */
+  double  score;                   /* the read-back score, -1.0 for a missed object */
+} sqdet_kitti_error_line;
+
+typedef struct sqdet_kitti_analysis {
+  int64_t num_dets, num_objs;      /* counted detections; objects of the analyzed classes */
+  int64_t correct, loc, cls, bg, repeated;
+  int64_t detected;                /* objects a correct detection claimed */
+  int64_t n_lines;                 /* error lines, written or not */
+  int32_t status;
+  int32_t reserved;
+} sqdet_kitti_analysis;
+
+int64_t sqdet_kitti_analyze_scratch_bytes(int n, int max_dets, int64_t n_objects);
+int sqdet_kitti_analyze(int n, int max_dets, const sqdet_det* dets, const int32_t* counts,
+                        int classes, const int32_t* class_map, const sqdet_kitti_obj* objs,
+                        const int64_t* offsets, int64_t n_objects, void* scratch,
+                        int64_t scratch_bytes, sqdet_kitti_analysis* out,
+                        sqdet_kitti_error_line* lines, int64_t line_capacity, void* stream);
+
 /* ---- tiny device-memory helpers so a ctypes caller needs nothing else -------------- */
 int sqdet_malloc(int device, int64_t bytes, void** out_dev);
 int sqdet_free(int device, void* dev);

@@ -136,6 +136,9 @@ SIGNATURES = {
     'sqdet_encode_png': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp]),
     'sqdet_kitti_eval_scratch_bytes': (_i64, [_i, _i, _i64]),
     'sqdet_kitti_eval': (_i, [_i, _i, _vp, _vp, _i, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp]),
+    'sqdet_kitti_analyze_scratch_bytes': (_i64, [_i, _i, _i64]),
+    'sqdet_kitti_analyze': (_i, [_i, _i, _vp, _vp, _i, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp,
+                                 _i64, _vp]),
     'sqdet_jpeg_parse': (_i, [_vp, _i64, C.POINTER(JpegInfo)]),
     'sqdet_jpeg_decode_staging_bytes': (_i64, [_i, _vp, _vp]),
     'sqdet_jpeg_decode_scratch_bytes': (_i64, [_i, _vp, _vp]),

@@ -39,10 +39,12 @@ TYPES = ('Car', 'Pedestrian', 'Cyclist', 'Van', 'Person_sitting', 'Truck', 'Tram
 TYPE_P = (0.45, 0.08, 0.03, 0.05, 0.01, 0.02, 0.01, 0.02, 0.33)
 
 
-def synthetic_set(seed, n, dets=64, max_labels=13, min_labels=2):
+def synthetic_set(seed, n, dets=64, max_labels=13, min_labels=2, analyzable=False):
   """(labels, records): label file texts and DET_DTYPE record arrays of a seeded KITTI-like set: n images of min..max labels with KITTI's class mix, 1242x375, and
   `dets` records per image: some jittered around each car / pedestrian / cyclist label (at the
-  label's class or another), the rest anywhere."""
+  label's class or another), the rest anywhere.  With `analyzable`, car / pedestrian / cyclist
+  labels start at x1 >= 0, as the reference's detection analysis asserts (the same draws, so the
+  set is otherwise unchanged)."""
   rng = np.random.default_rng(seed)
   labels, records = [], []
   for _ in range(n):
@@ -53,6 +55,8 @@ def synthetic_set(seed, n, dets=64, max_labels=13, min_labels=2):
       w = float(rng.uniform(15, 300))
       h = float(rng.uniform(15, 200)) if rng.random() < 0.8 else float(rng.choice([25, 40]))
       x1, y1 = float(rng.uniform(-20, 1200)), float(rng.uniform(0, 340))
+      if analyzable and t in ('Car', 'Pedestrian', 'Cyclist'):
+        x1 = abs(x1)
       if t == 'DontCare':
         lines.append(label_line(t, x1, y1, x1 + w, y1 + h, trunc=-1, occ=-1, alpha=-10))
         continue

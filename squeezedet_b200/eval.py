@@ -15,8 +15,13 @@ files are written
 (src/dataset/kitti.py:100-127), and the records, uploaded once as one [N, max_dets] array, are
 scored on the GPU (squeezedet_b200.kitti, byte for byte the files of the KITTI devkit's
 `evaluate_object`, which src/dataset/kitti.py:129-136 runs) into stats_*.txt next to `data/`,
-whose APs are parsed as the reference parses them (kitti.py:138-159).  The TensorBoard summaries
-and the checkpoint-polling loop (eval.py:171-239) are not rebuilt.
+whose APs are parsed as the reference parses them (kitti.py:138-159).  Then, as eval.py:128-130
+does, the detections are analyzed on the GPU from the same records (kitti.analyze_device, line
+for line the reference's analyze_detections, kitti.py:182-296): the "Detection Analysis" block
+is printed and detection_files_0/error_analysis/det_error_file.txt written.  Where the reference
+divides by zero there (no counted detection or no object), the share prints as nan.  The
+TensorBoard summaries, the images visualize_detections draws for them (imdb.py:254-305) and the
+checkpoint-polling loop (eval.py:171-239) are not rebuilt.
 """
 from __future__ import annotations
 
@@ -192,6 +197,7 @@ def eval_once(flags):
   det_dir = os.path.join(flags.eval_dir, 'detection_files_{:s}'.format('0'), 'data')
   result_dir = write_kitti_detections(det_dir, image_ids, mc.CLASS_NAMES, all_boxes)
   from . import kitti
+  labels = None
   try:
     labels = kitti.read_labels(os.path.join(flags.data_path, 'training', 'label_2'), image_ids)
   except (OSError, ValueError) as e:
@@ -205,7 +211,31 @@ def eval_once(flags):
   for ap, name in zip(aps, names):
     print('    {}: {:.3f}'.format(name, ap))
   print('    Mean average precision: {:.3f}'.format(float(np.mean(aps))))
+  if labels is not None:
+    analyze(flags, image_ids, mc.CLASS_NAMES, all_dets, all_counts, labels, result_dir)
   return all_boxes, aps, names
+
+
+def analyze(flags, image_ids, class_names, all_dets, all_counts, labels, result_dir):
+  """eval.py:128-130: the detection analysis of every image's records, printed, and
+  <result_dir>/error_analysis/det_error_file.txt.  A label box the reference asserts against
+  prints an error naming the image, and no error file is written."""
+  from . import kitti
+  print('Analyzing detections...')
+  try:
+    stats, lines = kitti.analyze_device(all_dets, all_counts, class_names, labels,
+                                        device='cuda:{:d}'.format(int(flags.gpu)))
+  except ValueError as e:
+    msg = str(e)
+    if msg.startswith('image '):
+      k = int(msg.split(':')[0].split()[1])
+      msg = '{} ({}.txt){}'.format(msg.split(':')[0], image_ids[k], msg[msg.index(':'):])
+    print('ERROR: Couldn\'t analyze the detections: {}'.format(msg))
+    return None
+  print(kitti.analysis_text(stats), end='')
+  kitti.write_error_file(os.path.join(result_dir, 'error_analysis', 'det_error_file.txt'),
+                         image_ids, class_names, lines)
+  return stats
 
 
 def main(argv=None):

@@ -10,7 +10,14 @@ and the label files, with no detection file read back.
 The records are scored as the devkit scores the detection files eval.py writes from them
 (utils/viz.write_kitti_detections: corners with 2 decimals, the score with 3, alpha 0.0).  Class
 names match car, pedestrian and cyclist case-insensitively; other classes are never scored.  The
-devkit's gnuplot scripts and renders are not written.  No engine is needed."""
+devkit's gnuplot scripts and renders are not written.  No engine is needed.
+
+The detection error analysis the reference runs after the APs (analyze_detections, sqdet_kitti_
+analyze) comes from the same records and labels:
+
+  stats, lines = analyze_device(dets, counts, mc.CLASS_NAMES, labels)
+  print(analysis_text(stats))
+  write_error_file(det_error_file, image_ids, mc.CLASS_NAMES, lines)"""
 from __future__ import annotations
 
 import math
@@ -124,6 +131,22 @@ def average_precision(precision):
   return ap / 11.0
 
 
+ERROR_TYPES = ('loc', 'cls', 'bg', 'missed')          # SQDET_KITTI_ERR_*
+LINE_DTYPE = np.dtype([('image', '<i4'), ('type', '<i4'), ('cls', '<i4'), ('reserved', '<i4'),
+                       ('x1', '<f8'), ('y1', '<f8'), ('x2', '<f8'), ('y2', '<f8'),
+                       ('score', '<f8')])
+assert LINE_DTYPE.itemsize == 56            # sizeof(sqdet_kitti_error_line)
+COUNT_FIELDS = ('num_dets', 'num_objs', 'correct', 'loc', 'cls', 'bg', 'repeated', 'detected')
+ANALYSIS_DTYPE = np.dtype([(f, '<i8') for f in COUNT_FIELDS] +
+                          [('n_lines', '<i8'), ('status', '<i4'), ('reserved', '<i4')])
+assert ANALYSIS_DTYPE.itemsize == 80        # sizeof(sqdet_kitti_analysis)
+ANALYSIS_REASONS = dict(REASONS)
+del ANALYSIS_REASONS[6]
+ANALYSIS_REASONS[7] = 'a record has w < 0 or h < 0'
+ANALYSIS_REASONS[8] = ('a label box of an analyzed class is not finite or fails the reference\'s '
+                       'assertions x1 >= 0, x1 <= x2, y1 >= 0, y1 <= y2')
+
+
 def _records(dets, counts, device):
   """dets and counts as contiguous CUDA tensors: dets [n, max_dets] DET_DTYPE (numpy) or a CUDA
   tensor of those bytes with n rows; counts [n] int32."""
@@ -147,6 +170,44 @@ def _records(dets, counts, device):
   return d, c, n, max_dets
 
 
+def _cuda_device(dets, device):
+  import torch
+  if device is None:
+    device = dets.device if torch.is_tensor(dets) else torch.device('cuda', torch.cuda.current_device())
+  device = torch.device(device)
+  if device.type != 'cuda':
+    raise ValueError('the scorer runs on a CUDA device, got %s' % (device,))
+  return device
+
+
+def _cut_capacity(dets, counts):
+  """A numpy dets wider than 1024 cut to its largest count; ValueError names an image with more
+  than 1024 records."""
+  if isinstance(dets, np.ndarray) and dets.ndim == 2 and dets.shape[1] > MAX_DETS:
+    cnt = np.asarray(counts).reshape(-1)
+    over = np.nonzero(cnt > MAX_DETS)[0]
+    if len(over):
+      raise ValueError('image %d: %d records, and the scorer takes at most %d per image'
+                       % (over[0], cnt[over[0]], MAX_DETS))
+    dets = dets[:, :max(1, int(cnt.max()) if len(cnt) else 1)]
+  return dets
+
+
+def _upload(dets, counts, labels, device):
+  """Records, counts and labels on `device`, on the current stream: (dets, counts, max_dets,
+  n_objects, objs or None, offsets)."""
+  import torch
+  d, c, nd, max_dets = _records(dets, counts, device)
+  if nd != len(labels):
+    raise ValueError('%d images of records but %d of labels' % (nd, len(labels)))
+  if not 1 <= max_dets <= MAX_DETS:
+    raise ValueError('max_dets must be in [1, %d], got %d' % (MAX_DETS, max_dets))
+  n_obj = len(labels.objs)
+  objs = torch.from_numpy(labels.objs.view(np.uint8).reshape(-1)).to(device) if n_obj else None
+  offsets = torch.from_numpy(labels.offsets).to(device)
+  return d, c, max_dets, n_obj, objs, offsets
+
+
 def evaluate_device(dets, counts, class_names, labels, stream=None, device=None):
   """Scores n images -> {class name: (precision, aos, ap)} for each of car, pedestrian and
   cyclist that has a record anywhere, with precision and aos three 41-point curves (easy,
@@ -167,11 +228,7 @@ def evaluate_device(dets, counts, class_names, labels, stream=None, device=None)
   import torch
   from .jpeg import _torch_stream
   n = len(labels)
-  if device is None:
-    device = dets.device if torch.is_tensor(dets) else torch.device('cuda', torch.cuda.current_device())
-  device = torch.device(device)
-  if device.type != 'cuda':
-    raise ValueError('the scorer runs on a CUDA device, got %s' % (device,))
+  device = _cuda_device(dets, device)
   codes = [CLASSES.index(_fold(c)) if _fold(c) in CLASSES else -1 for c in class_names]
   if not 1 <= len(codes) <= 64:
     raise ValueError('class_names must name 1 to 64 classes')
@@ -179,24 +236,11 @@ def evaluate_device(dets, counts, class_names, labels, stream=None, device=None)
     raise ValueError('two class names name the same KITTI class: %r' % (list(class_names),))
   if n == 0:
     return {}
-  if isinstance(dets, np.ndarray) and dets.ndim == 2 and dets.shape[1] > MAX_DETS:
-    cnt = np.asarray(counts).reshape(-1)
-    over = np.nonzero(cnt > MAX_DETS)[0]
-    if len(over):
-      raise ValueError('image %d: %d records, and the scorer takes at most %d per image'
-                       % (over[0], cnt[over[0]], MAX_DETS))
-    dets = dets[:, :max(1, int(cnt.max()) if len(cnt) else 1)]
+  dets = _cut_capacity(dets, counts)
   lib = _lib.load()
   s = _torch_stream(stream, device)
   with torch.cuda.device(device), torch.cuda.stream(s):
-    d, c, nd, max_dets = _records(dets, counts, device)
-    if nd != n:
-      raise ValueError('%d images of records but %d of labels' % (nd, n))
-    if not 1 <= max_dets <= MAX_DETS:
-      raise ValueError('max_dets must be in [1, %d], got %d' % (MAX_DETS, max_dets))
-    n_obj = len(labels.objs)
-    objs = torch.from_numpy(labels.objs.view(np.uint8).reshape(-1)).to(device) if n_obj else None
-    offsets = torch.from_numpy(labels.offsets).to(device)
+    d, c, max_dets, n_obj, objs, offsets = _upload(dets, counts, labels, device)
     nbytes = lib.sqdet_kitti_eval_scratch_bytes(n, max_dets, n_obj)
     if nbytes < 0:
       raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
@@ -256,3 +300,103 @@ def write_stats(result_dir, scores):
     for rel, text in files.items():
       with open(os.path.join(result_dir, rel), 'w') as f:
         f.write(text)
+
+
+def analysis_stats(counts):
+  """The reference's `out` dict of analyze_detections from the counts (COUNT_FIELDS): the counts
+  as floats and the shares of detections and objects.  Where the reference divides by 0 and
+  raises ZeroDivisionError (no counted detection, or no object), the share is float('nan')."""
+  f = {k: float(counts[k]) for k in COUNT_FIELDS}
+
+  def share(a, b):
+    return a / b if b else float('nan')
+  return {'num of detections': f['num_dets'], 'num of objects': f['num_objs'],
+          '% correct detections': share(f['correct'], f['num_dets']),
+          '% localization error': share(f['loc'], f['num_dets']),
+          '% classification error': share(f['cls'], f['num_dets']),
+          '% background error': share(f['bg'], f['num_dets']),
+          '% repeated error': share(f['repeated'], f['num_dets']),
+          '% recall': share(f['detected'], f['num_objs'])}
+
+
+def analyze_device(dets, counts, class_names, labels, stream=None, device=None):
+  """The reference's detection error analysis (analyze_detections, src/dataset/kitti.py:182-296)
+  of n images -> (stats, lines): stats the reference's `out` dict (analysis_stats), lines a
+  LINE_DTYPE array of det_error_file.txt's lines in file order (write_error_file).
+
+  The arguments are evaluate_device's.  class_names must be distinct names among the lowercase
+  'car', 'pedestrian' and 'cyclist', as in every shipped config: the reference looks the lowercased
+  detection and label types up among them and fails on any other detection type.  Refused with
+  ValueError before any launch.  After the launch, ValueError names the first image with a record
+  evaluate_device refuses, a record with w < 0 or h < 0, or a label box of an analyzed class that
+  is not finite or fails the reference's assertions (x1 >= 0, x1 <= x2, y1 >= 0, y1 <= y2).
+
+  Runs on `stream` and waits for it at the end, for the counts and then the lines.  With no
+  images nothing is launched and every count is 0."""
+  import torch
+  from .jpeg import _torch_stream
+  n = len(labels)
+  device = _cuda_device(dets, device)
+  names = list(class_names)
+  if not 1 <= len(names) <= 3 or any(c not in CLASSES for c in names) or len(set(names)) < len(names):
+    raise ValueError('the analysis takes distinct class names among %r, got %r'
+                     % (CLASSES, names))
+  codes = [CLASSES.index(c) for c in names]
+  if n == 0:
+    return analysis_stats(dict.fromkeys(COUNT_FIELDS, 0)), np.zeros((0,), LINE_DTYPE)
+  dets = _cut_capacity(dets, counts)
+  capacity = 2 * int(np.isin(labels.objs['type'], codes).sum())
+  lib = _lib.load()
+  s = _torch_stream(stream, device)
+  with torch.cuda.device(device), torch.cuda.stream(s):
+    d, c, max_dets, n_obj, objs, offsets = _upload(dets, counts, labels, device)
+    nbytes = lib.sqdet_kitti_analyze_scratch_bytes(n, max_dets, n_obj)
+    if nbytes < 0:
+      raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
+    scratch = torch.empty((nbytes,), dtype=torch.uint8, device=device)
+    out = torch.empty((ANALYSIS_DTYPE.itemsize,), dtype=torch.uint8, device=device)
+    lines = torch.empty((max(capacity, 1) * LINE_DTYPE.itemsize,), dtype=torch.uint8, device=device)
+    cmap = np.array(codes, np.int32)
+    _lib.check(lib.sqdet_kitti_analyze(n, max_dets, d.data_ptr(), c.data_ptr(), len(codes),
+                                       cmap.ctypes.data, objs.data_ptr() if n_obj else None,
+                                       offsets.data_ptr(), n_obj, scratch.data_ptr(), nbytes,
+                                       out.data_ptr(), lines.data_ptr(), capacity, s.cuda_stream))
+    res = out.cpu().numpy().view(ANALYSIS_DTYPE)[0]
+    status = int(res['status'])
+    if status != -1:
+      raise ValueError('image %d: %s' % (status // 16,
+                                         ANALYSIS_REASONS.get(status % 16, 'unusable records')))
+    n_lines = int(res['n_lines'])
+    if n_lines > capacity:         # each image writes at most G detection and G missed lines
+      raise RuntimeError('%d error lines for a capacity of %d' % (n_lines, capacity))
+    got = lines[:n_lines * LINE_DTYPE.itemsize].cpu().numpy().view(LINE_DTYPE)
+  return analysis_stats(res), got
+
+
+def analysis_text(stats):
+  """The block analyze_detections prints, with its wording and '{}' formatting."""
+  rows = (('Number of detections', 'num of detections'), ('Number of objects', 'num of objects'),
+          ('Percentage of correct detections', '% correct detections'),
+          ('Percentage of localization error', '% localization error'),
+          ('Percentage of classification error', '% classification error'),
+          ('Percentage of background error', '% background error'),
+          ('Percentage of repeated detections', '% repeated error'), ('Recall', '% recall'))
+  return 'Detection Analysis:\n' + ''.join(
+      '    {}: {}\n'.format(label, stats[key]) for label, key in rows)
+
+
+def error_file_text(image_ids, class_names, lines):
+  """det_error_file.txt's text for analyze_device's lines: _save_detection's
+  '{:s} {:s} {:.1f} {:.1f} {:.1f} {:.1f} {:s} {:.3f}' per line."""
+  fmt = '{:s} {:s} {:.1f} {:.1f} {:.1f} {:.1f} {:s} {:.3f}\n'.format
+  return ''.join(fmt(image_ids[i], ERROR_TYPES[t], x1, y1, x2, y2, class_names[c], sc)
+                 for i, t, c, x1, y1, x2, y2, sc in zip(
+                     *(lines[f].tolist() for f in ('image', 'type', 'cls', 'x1', 'y1', 'x2', 'y2',
+                                                   'score'))))
+
+
+def write_error_file(path, image_ids, class_names, lines):
+  """Writes det_error_file.txt (error_file_text) at `path`, creating its directory."""
+  os.makedirs(os.path.dirname(path) or '.', exist_ok=True)
+  with open(path, 'w') as f:
+    f.write(error_file_text(image_ids, class_names, lines))
