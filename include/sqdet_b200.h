@@ -501,7 +501,7 @@ int sqdet_draw_dets(int n, int format, uint8_t* const* planes, const int64_t* pi
  *   cv2.imencode('.jpg', cv2.cvtColor(frame, code)[y:y+h, x:x+w], [IMWRITE_JPEG_QUALITY, quality])
  * with `code` the frame format's code of sqdet_forward_frames (BGR: no conversion): cv2's default
  * encoder, libjpeg-turbo's integer pipeline — baseline sequential, 4:2:0, Annex K Huffman tables
- * (not optimized), no restart markers, JFIF APP0 1.01 with 1:1 density, quantization tables of
+ * (not optimized), no restart markers (sqdet_encode_jpeg_params below takes cv2's other settings), JFIF APP0 1.01 with 1:1 density, quantization tables of
  * jpeg_quality_scaling(quality) clamped to 1..255.  Frames are laid out as sqdet_forward_frames
  * takes them.  Frame i's file goes to out_dev + i * cap and its length to lengths_dev[i]; a file
  * longer than cap gives lengths_dev[i] = -1 and unspecified bytes in that frame's slot, and the
@@ -530,6 +530,47 @@ int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int
                       const int32_t* heights, const int32_t* widths, const int32_t* crops,
                       int quality, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
                       void* scratch_dev, int64_t scratch_bytes, void* stream);
+
+/* ---- JPEG encoding with cv2's other IMWRITE_JPEG_* parameters ----------------------
+ * sqdet_encode_jpeg_params: sqdet_encode_jpeg with the file cv2.imencode('.jpg', crop, list)
+ * writes for the cv2 parameter list `params` stands for:
+ *   quality           IMWRITE_JPEG_QUALITY, 1..100
+ *   luma_quality      IMWRITE_JPEG_LUMA_QUALITY, 1..100 or -1 (unset): replaces quality
+ *   chroma_quality    IMWRITE_JPEG_CHROMA_QUALITY, 1..100 or -1: counts only with luma_quality
+ *                     (unset: the luma quality); when the two differ cv2 writes 4:4:4 whatever
+ *                     `sampling` says, and so does this
+ *   sampling          IMWRITE_JPEG_SAMPLING_FACTOR: 0x411111, 0x221111 (4:2:0, cv2's default),
+ *                     0x211111, 0x121111 or 0x111111 (luma h, v; Cb and Cr are 1x1)
+ *   optimize          IMWRITE_JPEG_OPTIMIZE, 0 or 1: each frame's own optimal Huffman tables
+ *   restart_interval  IMWRITE_JPEG_RST_INTERVAL, 0..65535 MCUs (0: no restart markers)
+ * cv2 clamps out-of-range values and falls back to 4:2:0 for another sampling; these functions
+ * refuse them with SQDET_ERR_INVALID_ARG instead (as they refuse a null params), and otherwise
+ * refuse what sqdet_encode_jpeg refuses.  Progressive files (IMWRITE_JPEG_PROGRESSIVE) are not
+ * written: encode those with cv2.
+ * sqdet_jpeg_max_bytes_params and sqdet_jpeg_scratch_bytes_params are the output capacity and
+ * scratch of those parameters (-1 when the parameters or sizes are refused).  Sampling, optimize
+ * and restart markers raise both: 4:4:4 codes three blocks per 8x8 pixels against 4:2:0's 1.5,
+ * optimized DC codes reach 16 + 11 bits, and each restart interval adds a padding byte and RSTn.
+ * sqdet_encode_jpeg, sqdet_jpeg_max_bytes and sqdet_jpeg_scratch_bytes are these with
+ * {quality, -1, -1, 0x221111, 0, 0} (quality 95 for the sizes).
+ * Optimized tables add two launches per group of 16 frames (symbol counts, then the tables) and
+ * restart markers two (each interval's first bit, then a scan); neither waits for the device. */
+typedef struct {
+  int32_t quality;
+  int32_t luma_quality;
+  int32_t chroma_quality;
+  int32_t sampling;
+  int32_t optimize;
+  int32_t restart_interval;
+} sqdet_jpeg_params;
+int64_t sqdet_jpeg_max_bytes_params(int h, int w, const sqdet_jpeg_params* params);
+int64_t sqdet_jpeg_scratch_bytes_params(int n, const int32_t* heights, const int32_t* widths,
+                                        const int32_t* crops, const sqdet_jpeg_params* params);
+int sqdet_encode_jpeg_params(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
+                             const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                             const sqdet_jpeg_params* params, uint8_t* out_dev, int64_t cap,
+                             int64_t* lengths_dev, void* scratch_dev, int64_t scratch_bytes,
+                             void* stream);
 
 /* ---- PNG encoding of frames in device memory (no engine needed) ---------------------
  * sqdet_encode_png: frame i's crop (x, y, w, h) becomes exactly the bytes of

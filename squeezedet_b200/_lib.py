@@ -61,6 +61,12 @@ class JpegInfo(C.Structure):
       [('scan_offset', C.c_int64)]
 
 
+class JpegParams(C.Structure):
+  """struct sqdet_jpeg_params."""
+  _fields_ = [(k, C.c_int32) for k in (
+      'quality', 'luma_quality', 'chroma_quality', 'sampling', 'optimize', 'restart_interval')]
+
+
 _vp, _i, _f, _i64 = C.c_void_p, C.c_int, C.c_float, C.c_int64
 _ip = C.POINTER(C.c_int)
 _i64p = C.POINTER(C.c_int64)
@@ -131,6 +137,10 @@ SIGNATURES = {
     'sqdet_jpeg_max_bytes': (_i64, [_i, _i]),
     'sqdet_jpeg_scratch_bytes': (_i64, [_i, _vp, _vp, _vp]),
     'sqdet_encode_jpeg': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i64, _vp, _vp, _i64, _vp]),
+    'sqdet_jpeg_max_bytes_params': (_i64, [_i, _i, C.POINTER(JpegParams)]),
+    'sqdet_jpeg_scratch_bytes_params': (_i64, [_i, _vp, _vp, _vp, C.POINTER(JpegParams)]),
+    'sqdet_encode_jpeg_params': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, C.POINTER(JpegParams), _vp,
+                                      _i64, _vp, _vp, _i64, _vp]),
     'sqdet_png_max_bytes': (_i64, [_i, _i]),
     'sqdet_png_scratch_bytes': (_i64, [_i, _vp, _vp, _vp]),
     'sqdet_encode_png': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp]),

@@ -33,7 +33,8 @@ from .bench_device_u8 import gpu_info
 FORMS = ('a_host_imencode', 'b_encode_jpeg_device')
 FRAME_W, FRAME_H, OVERLAP = 1920, 1080, 128
 QUALITY = 95
-KERNELS = ('transform_kernel', 'block_bits_kernel', 'scan_kernel', 'pack_kernel',
+SAMPLING_FACTORS = {'411': 0x411111, '420': 0x221111, '422': 0x211111, '440': 0x121111, '444': 0x111111}
+KERNELS = ('transform_kernel', 'hist_kernel', 'table_kernel', 'interval_kernel', 'block_bits_kernel', 'scan_kernel', 'pack_kernel',
            'count_ff_kernel', 'stuff_kernel')
 
 
@@ -44,7 +45,17 @@ def parse_args(argv=None):
   ap.add_argument('--warmup', type=int, default=3)
   ap.add_argument('--frames', type=int, default=2)
   ap.add_argument('--gpu', type=int, default=0)
+  # cv2's other JPEG parameters, passed alike to both forms; the defaults are cv2's
+  ap.add_argument('--sampling', default='420', choices=('411', '420', '422', '440', '444'))
+  ap.add_argument('--optimize', action='store_true')
+  ap.add_argument('--restart', type=int, default=0, help='restart interval in MCUs (0: none)')
   return ap.parse_args(argv)
+
+
+def jpeg_settings(args):
+  """encode_jpeg_device's keywords of the command line."""
+  return dict(quality=QUALITY, sampling=args.sampling, optimize=args.optimize,
+              restart_interval=args.restart)
 
 
 def measure_workload(args, name, model, fmt, clean, grid, torch):
@@ -56,6 +67,13 @@ def measure_workload(args, name, model, fmt, clean, grid, torch):
   stream = torch.cuda.Stream(device=clean[0].device)
   sptr = stream.cuda_stream
   work = [torch.empty_like(c) for c in clean]
+  settings = jpeg_settings(args)
+  cv2_params = [cv2.IMWRITE_JPEG_QUALITY, QUALITY,
+                cv2.IMWRITE_JPEG_SAMPLING_FACTOR, SAMPLING_FACTORS[args.sampling]]
+  if args.optimize:
+    cv2_params += [cv2.IMWRITE_JPEG_OPTIMIZE, 1]
+  if args.restart:
+    cv2_params += [cv2.IMWRITE_JPEG_RST_INTERVAL, args.restart]
 
   def drawn():
     with torch.cuda.stream(stream):
@@ -72,12 +90,12 @@ def measure_workload(args, name, model, fmt, clean, grid, torch):
         im = w.cpu().numpy()
         if fmt == 'nv12':
           im = cv2.cvtColor(im, cv2.COLOR_YUV2BGR_NV12)
-        files.append(cv2.imencode('.jpg', im, [cv2.IMWRITE_JPEG_QUALITY, QUALITY])[1].tobytes())
+        files.append(cv2.imencode('.jpg', im, cv2_params)[1].tobytes())
     return files
 
   def end_b():
     with torch.cuda.stream(stream):
-      data, lengths = encode_jpeg_device(work, fmt, quality=QUALITY, stream=stream)
+      data, lengths = encode_jpeg_device(work, fmt, stream=stream, **settings)
       return jpeg_bytes(data, lengths, stream=stream)
 
   ends = {FORMS[0]: end_a, FORMS[1]: end_b}
@@ -110,17 +128,19 @@ def measure_workload(args, name, model, fmt, clean, grid, torch):
   outs = []
   with profile(activities=[ProfilerActivity.CUDA]) as prof:
     for _ in range(calls):
-      outs.append(encode_jpeg_device(work, fmt, quality=QUALITY, stream=stream))
+      outs.append(encode_jpeg_device(work, fmt, stream=stream, **settings))
     stream.synchronize()
   evs = [ev for ev in prof.events() if ev.device_type == DeviceType.CUDA and
          any(k in ev.name for k in KERNELS + ('emset',))]
-  launches = calls * -(-n // 16) * (len(KERNELS) + 2)   # two scans and a memset per 16 frames
+  # per 16 frames: a memset and seven launches, two more with optimize and two with restart markers
+  launches = calls * -(-n // 16) * (8 + 2 * args.optimize + 2 * bool(args.restart))
   assert len(evs) >= launches * 9 // 10, 'found %d of %d encode launches' % (len(evs), launches)
   us = sum(ev.time_range.elapsed_us() for ev in evs) / calls
 
   row = {'workload': name, 'engine': '%dx%d b=%d' % (mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT,
                                                      mc.BATCH_SIZE),
          'frames': n, 'frame': '%dx%d %s' % (FRAME_W, FRAME_H, fmt), 'quality': QUALITY,
+         'sampling': args.sampling, 'optimize': args.optimize, 'restart': args.restart,
          'file_bytes_mean': float(np.mean([len(f) for f in want]))}
   for form in FORMS:
     row[form] = {'ms_per_frame_ending_median': 1e3 * float(np.median(ending[form])) / n,

@@ -1,27 +1,40 @@
-// Baseline JPEG encoding of uint8 frames in device memory (sqdet_encode_jpeg): frame i's crop,
-// converted to BGR as its format's cv2.cvtColor code does, becomes the bytes
-// cv2.imencode('.jpg', crop, [IMWRITE_JPEG_QUALITY, quality]) writes, bit for bit.  That is
-// libjpeg-turbo's default integer pipeline: 16-bit fixed-point YCbCr, 4:2:0 with edge replication
-// and the 1, 2 bias, jpeg_fdct_islow, quantization by 8 q, Annex K Huffman tables, no restart
-// markers.  oracle/jpeg.py restates it in numpy.
+// Baseline JPEG encoding of uint8 frames in device memory (sqdet_encode_jpeg_params): frame i's
+// crop, converted to BGR as its format's cv2.cvtColor code does, becomes the bytes
+// cv2.imencode('.jpg', crop, params) writes, bit for bit, for cv2's IMWRITE_JPEG_QUALITY,
+// _LUMA_QUALITY, _CHROMA_QUALITY, _SAMPLING_FACTOR, _OPTIMIZE and _RST_INTERVAL.  That is
+// libjpeg-turbo's integer pipeline: 16-bit fixed-point YCbCr; luma sampled 4x1, 2x2, 2x1, 1x2 or
+// 1x1 against 1x1 chroma, with edge replication and jcsample.c's downsampler of each; jpeg_fdct_islow;
+// quantization by 8 q; Annex K Huffman tables or, with optimize, each frame's own
+// jpeg_gen_optimal_table tables; restart markers every restart_interval MCUs.  oracle/jpeg.py
+// restates the defaults in numpy and oracle/jpeg_params.py the rest.
 //
 // The entropy-coded segment is one bit stream per frame, made parallel by knowing where each block's
 // codes start:
 //   1. transform    one thread per 8x8 block fetches its samples straight from the frame's planes
 //                   (frames.cuh), converts, downsamples, transforms and quantizes them, and
-//                   writes the quantized coefficients (natural order) to the scratch
+//                   writes the quantized coefficients (natural order) to the scratch; templated
+//                   over the sampling
+//   (optimize only)
+//   1a. hist        the symbol counts of the four tables (DC, AC x luma, chroma), per chunk in
+//                   shared memory, then added to the frame's 64-bit counts
+//   1b. table       per frame, one warp per table builds jpeg_gen_optimal_table's code lengths and
+//                   symbol order, and the canonical codes
 //   2. block_bits   the bit length of each block's codes: its DC difference (the previous block
 //                   of its component is another thread's) and its AC codes; sums per chunk of
 //                   kChunk blocks
 //   3. scan         per frame, the exclusive scan of the chunk sums: each chunk's first bit
+//   (restart markers only)
+//   3a. interval    each restart interval's first bit and its length in bytes (padded)
+//   3b. scan        per frame, their exclusive scan: each interval's first byte
 //   4. pack         each block scans its chunk for its own first bit and ORs its codes into the
 //                   frame's zeroed bit buffer (32-bit atomicOr: neighbours share only edge
-//                   words); the last block adds the 1-bit padding
-//   5. count_ff     the 0xFF bytes per kStuffChunk bytes of the stream
+//                   words); the last block of each interval adds the 1-bit padding
+//   5. count_ff     the 0xFF bytes (and 2 per RSTn marker) per kStuffChunk bytes of the stream
 //   6. scan         per frame, their exclusive scan
-//   7. stuff        each chunk copies its bytes to the output with a 0x00 after every 0xFF, and
-//                   the frame's first chunk writes the header (a host template with the frame's
-//                   height and width), EOI and the length, or -1 when the file does not fit
+//   7. stuff        each chunk copies its bytes to the output with a 0x00 after every 0xFF and
+//                   RSTn before each interval's first byte, and the frame's first chunk writes
+//                   the header (a host template with the frame's height, width and Huffman
+//                   tables filled in), EOI and the length, or -1 when the file does not fit
 // Frames run kJpegFramesPerLaunch at a time through these launches, reusing one scratch.
 #include <algorithm>
 #include <cstring>
@@ -37,9 +50,15 @@ constexpr int kStuffThreads = 256;
 constexpr int kStuffBytes = 16;        // bytes per stuffing thread
 constexpr int kStuffChunk = kStuffThreads * kStuffBytes;
 constexpr int kScanThreads = 1024;
-constexpr int kMaxBlockBits = 22 + 63 * 26;   // a chroma DC of category 11, 63 AC codes of 16 + 10 bits
-constexpr int kHeaderBytes = 623;
+// a chroma DC of category 11 (Annex K: an 11-bit code; optimized: up to 16 bits), 63 AC codes of
+// 16 + 10 bits
+constexpr int kMaxBlockBits = 22 + 63 * 26;
+constexpr int kMaxBlockBitsOpt = 27 + 63 * 26;
+constexpr int kPrefixBytes = 177;     // SOI, JFIF APP0, DQT x 2, SOF0
 constexpr int kSofSize = 163;         // the header's offset of SOF0's height (then its width)
+constexpr int kSosBytes = 14, kDriBytes = 6;
+constexpr int kHeaderBytes = 623;     // with the Annex K tables and no DRI; optimized tables are no longer
+constexpr int kTableThreads = 128;    // one warp per table
 
 // ---- Annex K tables ---------------------------------------------------------------------------
 constexpr uint8_t kStdLumaQ[64] = {
@@ -119,15 +138,30 @@ __constant__ uint8_t kZigzagDev[64] = {     // kZigzag, for device code
     35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51,
     58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
 
+// The tables as DHT writes them: bits[t][l] symbols of length l + 1 and the symbols in order, for
+// t = DC luma, AC luma, DC chroma, AC chroma; count[t] symbols in all.
+struct HuffSpec {
+  uint8_t bits[4][16];
+  uint8_t vals[4][256];
+  int16_t count[4];
+};
+// A frame's optimized tables: its codes and its DHT contents.
+struct FrameHuff {
+  HuffCodes c;
+  HuffSpec s;
+};
+
 // ---- per-frame geometry and scratch ---------------------------------------------------------------
 // One frame of a launch group: its crop, MCU grid and where its pieces of the scratch and output
-// are.  Blocks are numbered in stream order (per MCU: Y0 Y1 Y2 Y3 Cb Cr) from blk (a multiple of
-// kChunk); the chunk sums of its `chunks` block chunks start at csum and those of its `schunks`
-// stuffing chunks at ssum, each followed by one slot that the scan fills with the total.
+// are.  Blocks are numbered in stream order (per MCU: the luma blocks row by row, then Cb, Cr)
+// from blk (a multiple of kChunk); the chunk sums of its `chunks` block chunks start at csum,
+// those of its `schunks` stuffing chunks at ssum and those of its `ints` restart intervals at isum
+// (with restart markers only), each followed by one slot that the scan fills with the total.
 struct JpegGeom {
-  int h, w, mcu_cols, blocks;           // blocks = 6 * MCUs
-  int chunks, schunks;
-  int64_t blk, csum, ssum, words;       // words: the first 32-bit word of the bit buffer
+  int h, w, mcu_cols, blocks;           // blocks = MCUs * blocks per MCU
+  int chunks, schunks, ints;            // ints: restart intervals (1 without restart markers)
+  int64_t blk, csum, ssum, isum, ipos;  // ipos: the first of its intervals' first bits
+  int64_t words;                        // the first 32-bit word of the bit buffer
   uint8_t* out;
   int64_t* length;
 };
@@ -141,9 +175,14 @@ struct JpegParams {
   JpegGeom g[kJpegFramesPerLaunch];
   int16_t* coef;                        // [blocks][64], natural order
   uint32_t* bits;                       // [blocks]
-  int64_t* sums;                        // chunk sums of blocks and of stuffing chunks
+  int64_t* sums;                        // chunk sums of blocks, of stuffing chunks and of intervals
+  int64_t* ipos;                        // each interval's first bit, before padding
   uint32_t* stream;                     // bit buffers
+  unsigned long long* freq;             // [frame][4][256] symbol counts (optimize)
+  FrameHuff* huff;                      // [frame] (optimize)
   int64_t cap;
+  int hs, vs, luma, per;                // luma sampling factors, luma blocks and blocks per MCU
+  int rst;                              // MCUs per restart interval, 0 for none
 };
 
 // The reciprocal of each divisor 8 q (luma, chroma; natural order) as libjpeg-turbo builds it for
@@ -163,30 +202,43 @@ static_assert(sizeof(TransformParams<SQDET_FMT_I420>) <= 4096, "transform parame
 
 struct StuffParams {
   JpegParams p;
-  uint8_t header[kHeaderBytes];
+  HuffSpec std;                         // the Annex K tables
+  uint8_t prefix[kPrefixBytes];         // SOI .. SOF0, height and width 0
+  uint8_t suffix[kDriBytes + kSosBytes];  // DRI (with restart markers), SOS
+  int suffix_bytes;
 };
 static_assert(sizeof(StuffParams) <= 4096, "stuffing parameters exceed 4 KiB");
 
 __device__ __forceinline__ int nbits(int v) { return v ? 32 - __clz(abs(v)) : 0; }
 
-// Is block u (0..3 luma, 4, 5 chroma) of MCU m a luma block right of or below the image's blocks?
-__device__ __forceinline__ bool dummy_block(const JpegGeom& g, int m, int u) {
-  if (u >= 4) return false;
-  const int bx = (m % g.mcu_cols) * 2 + (u & 1), by = (m / g.mcu_cols) * 2 + (u >> 1);
+// Is block u (luma blocks 0 .. luma - 1 row by row, then Cb, Cr) of MCU m a luma block right of or
+// below the image's blocks?
+__device__ __forceinline__ bool dummy_block(const JpegParams& p, const JpegGeom& g, int m, int u) {
+  if (u >= p.luma) return false;
+  const int bx = (m % g.mcu_cols) * p.hs + u % p.hs, by = (m / g.mcu_cols) * p.vs + u / p.hs;
   return bx * 8 >= g.w || by * 8 >= g.h;
 }
 
 // The quantized DC that block b codes against: the previous block of its component in stream order,
-// a dummy block standing for the last real block before it (its DC is that block's), 0 at the start.
-__device__ int prev_dc(const JpegGeom& g, const int16_t* coef, int b) {
-  const int u = b % 6;
-  if (u >= 4) return b >= 6 ? coef[(int64_t)(b - 6) * 64] : 0;
-  for (int k = b - 1; k >= 0; --k) {
-    const int uk = k % 6;
-    if (uk >= 4) continue;
-    if (!dummy_block(g, k / 6, uk)) return coef[(int64_t)k * 64];
+// a dummy block standing for the last real block before it (its DC is that block's), 0 at the start
+// of the frame and of each restart interval.
+__device__ int prev_dc(const JpegParams& p, const JpegGeom& g, const int16_t* coef, int b) {
+  const int m = b / p.per, u = b - m * p.per;
+  const int first = p.rst ? (m - m % p.rst) * p.per : 0;     // the interval's first block
+  if (u >= p.luma) return b - p.per >= first ? coef[(int64_t)(b - p.per) * 64] : 0;
+  for (int k = b - 1; k >= first; --k) {
+    const int uk = k % p.per;
+    if (uk >= p.luma) continue;
+    if (!dummy_block(p, g, k / p.per, uk)) return coef[(int64_t)k * 64];
   }
   return 0;
+}
+
+// The code tables block_bits and pack read: the Annex K ones, or the frame's optimized ones.
+template <bool kOpt>
+__device__ __forceinline__ const HuffCodes& huff_codes_of(const JpegParams& p, int frame) {
+  if constexpr (kOpt) return p.huff[frame].c;
+  else return kHuff;
 }
 
 // ---- 1. transform -------------------------------------------------------------------------------
@@ -224,24 +276,26 @@ __device__ __forceinline__ int to_c(int b, int g, int r, bool cr) {
             : (-11059 * r - 21709 * g + 32768 * b + (128 << 16) + 32767) >> 16;
 }
 
-template <int F>
+// Luma HS x VS against 1x1 chroma: an MCU is 8 HS x 8 VS pixels.
+template <int F, int HS, int VS>
 __global__ void __launch_bounds__(kChunk) transform_kernel(const __grid_constant__ TransformParams<F> tp) {
+  constexpr int kLuma = HS * VS, kPer = kLuma + 2;
   const JpegGeom& g = tp.p.g[blockIdx.y];
   if ((int)blockIdx.x >= g.chunks) return;
   const int b = blockIdx.x * kChunk + threadIdx.x;
   const int64_t gb = g.blk + b;
   int blk[64];
-  const int m = b / 6, u = b % 6;
-  const bool real = b < g.blocks && !dummy_block(g, m, u);
+  const int m = b / kPer, u = b % kPer;
+  const bool real = b < g.blocks && !dummy_block(tp.p, g, m, u);
   if (b >= g.blocks) return;
   const auto taps_ = taps<F>(tp.f[blockIdx.y]);
   const int mx = m % g.mcu_cols, my = m / g.mcu_cols;
   if (!real) {
 #pragma unroll
     for (int i = 0; i < 64; ++i) blk[i] = 0;
-  } else if (u < 4) {
+  } else if (u < kLuma) {
     // luma: rows and columns past the crop repeat its last ones
-    const int y0 = my * 16 + (u >> 1) * 8, x0 = mx * 16 + (u & 1) * 8;
+    const int y0 = my * 8 * VS + (u / HS) * 8, x0 = mx * 8 * HS + (u % HS) * 8;
 #pragma unroll
     for (int r = 0; r < 8; ++r)
 #pragma unroll
@@ -251,23 +305,44 @@ __global__ void __launch_bounds__(kChunk) transform_kernel(const __grid_constant
         blk[r * 8 + c] = to_y(B, G, R) - 128;
       }
   } else {
-    // chroma: h2v2 of the full-size plane (last row repeated to a 2-row group, last column to the
-    // block's width), then the last downsampled row repeated to the MCU row
-    const bool cr = u == 5;
-    const int last_row = (g.h + 1) / 2 - 1;
+    // chroma: the full-size plane with its last row repeated to a VS-row group and its last column
+    // to the MCU's width, downsampled, then the last downsampled row repeated to the MCU row.
+    // h2v2 rounds with the bias 1, 2, 1, 2, ..., h2v1 with 0, 1, 0, 1, ..., int_downsample (4x1,
+    // 1x2) to nearest, halves up
+    const bool cr = u == kLuma + 1;
+    const int last_row = (g.h + VS - 1) / VS - 1;
 #pragma unroll 1
     for (int r = 0; r < 8; ++r) {
       const int dr = min(my * 8 + r, last_row);
-      const int ya = min(2 * dr, g.h - 1), yb = min(2 * dr + 1, g.h - 1);
+      if constexpr (HS == 2 && VS == 2) {
+        const int ya = min(2 * dr, g.h - 1), yb = min(2 * dr + 1, g.h - 1);
 #pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        const int xa = min(mx * 16 + 2 * c, g.w - 1), xb = min(mx * 16 + 2 * c + 1, g.w - 1);
-        int s = 0, B, G, R;
-        fetch_bgr(taps_, ya, xa, B, G, R); s += to_c(B, G, R, cr);
-        fetch_bgr(taps_, ya, xb, B, G, R); s += to_c(B, G, R, cr);
-        fetch_bgr(taps_, yb, xa, B, G, R); s += to_c(B, G, R, cr);
-        fetch_bgr(taps_, yb, xb, B, G, R); s += to_c(B, G, R, cr);
-        blk[r * 8 + c] = ((s + 1 + (c & 1)) >> 2) - 128;
+        for (int c = 0; c < 8; ++c) {
+          const int xa = min(mx * 16 + 2 * c, g.w - 1), xb = min(mx * 16 + 2 * c + 1, g.w - 1);
+          int s = 0, B, G, R;
+          fetch_bgr(taps_, ya, xa, B, G, R); s += to_c(B, G, R, cr);
+          fetch_bgr(taps_, ya, xb, B, G, R); s += to_c(B, G, R, cr);
+          fetch_bgr(taps_, yb, xa, B, G, R); s += to_c(B, G, R, cr);
+          fetch_bgr(taps_, yb, xb, B, G, R); s += to_c(B, G, R, cr);
+          blk[r * 8 + c] = ((s + 1 + (c & 1)) >> 2) - 128;
+        }
+      } else {
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          int s = 0;
+#pragma unroll
+          for (int i = 0; i < VS; ++i)
+#pragma unroll(HS == 4 ? 1 : HS)          // 4x1: 32 fetches per row unrolled spill
+            for (int j = 0; j < HS; ++j) {
+              int B, G, R;
+              fetch_bgr(taps_, min(VS * dr + i, g.h - 1), min(HS * (mx * 8 + c) + j, g.w - 1), B, G, R);
+              s += to_c(B, G, R, cr);
+            }
+          if constexpr (HS == 2) s = (s + (c & 1)) >> 1;
+          else if constexpr (kLuma == 4) s = (s + 2) >> 2;
+          else if constexpr (kLuma == 2) s = (s + 1) >> 1;
+          blk[r * 8 + c] = s - 128;
+        }
       }
     }
   }
@@ -278,7 +353,7 @@ __global__ void __launch_bounds__(kChunk) transform_kernel(const __grid_constant
     for (int c = 0; c < 8; ++c) fdct8<false>(blk + c, 8);
   }
   // quantize: libjpeg-turbo's reciprocal multiply by 1 / (8 q), sign restored
-  const int t = u >= 4;
+  const int t = u >= kLuma;
   int16_t z[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) {
@@ -291,14 +366,158 @@ __global__ void __launch_bounds__(kChunk) transform_kernel(const __grid_constant
   for (int i = 0; i < 8; ++i) o4[i] = reinterpret_cast<const int4*>(z)[i];
 }
 
+// ---- 1a. symbol counts (optimize) ----------------------------------------------------------------
+// Every Huffman symbol of block b, in stream order, to f(table, symbol): table 0 / 2 the DC of luma /
+// chroma, 1 / 3 their AC.
+template <typename Fn>
+__device__ __forceinline__ void block_symbols(const JpegParams& p, const JpegGeom& g, const int16_t* coef,
+                                              int b, Fn f) {
+  const int u = b % p.per, t = u >= p.luma ? 2 : 0;
+  const int16_t* z = coef + (int64_t)b * 64;
+  f(t, nbits(dummy_block(p, g, b / p.per, u) ? 0 : z[0] - prev_dc(p, g, coef, b)));
+  int run = 0;
+#pragma unroll 1
+  for (int k = 1; k < 64; ++k) {
+    const int v = z[kZigzagDev[k]];
+    if (v == 0) {
+      ++run;
+      continue;
+    }
+    for (; run > 15; run -= 16) f(t + 1, 0xF0);
+    f(t + 1, (run << 4) | nbits(v));
+    run = 0;
+  }
+  if (run) f(t + 1, 0);
+}
+
+__global__ void __launch_bounds__(kChunk) hist_kernel(const __grid_constant__ JpegParams p) {
+  __shared__ uint32_t count[4 * 256];
+  const JpegGeom& g = p.g[blockIdx.y];
+  if ((int)blockIdx.x >= g.chunks) return;
+  for (int i = threadIdx.x; i < 4 * 256; i += kChunk) count[i] = 0;
+  __syncthreads();
+  const int b = blockIdx.x * kChunk + threadIdx.x;
+  if (b < g.blocks)
+    block_symbols(p, g, p.coef + g.blk * 64, b, [&](int t, int sym) { atomicAdd(&count[t * 256 + sym], 1u); });
+  __syncthreads();
+  unsigned long long* freq = p.freq + (int64_t)blockIdx.y * 4 * 256;
+  for (int i = threadIdx.x; i < 4 * 256; i += kChunk)
+    if (count[i]) atomicAdd(freq + i, (unsigned long long)count[i]);
+}
+
+// ---- 1b. optimal tables (optimize) ----------------------------------------------------------------
+// The symbol with the smallest nonzero count other than `skip`, the larger symbol on ties (-1 for
+// none): one of jpeg_gen_optimal_table's searches, over the warp.
+__device__ __forceinline__ int warp_min_symbol(const unsigned long long* f, int skip, int lane) {
+  unsigned long long best = ~0ull;
+  int sym = -1;
+  for (int i = lane; i < 257; i += 32)
+    if (f[i] && i != skip && f[i] <= best) {
+      best = f[i];
+      sym = i;
+    }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const unsigned long long ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int os = __shfl_xor_sync(0xffffffffu, sym, o);
+    if (os >= 0 && (sym < 0 || ob < best || (ob == best && os > sym))) {
+      best = ob;
+      sym = os;
+    }
+  }
+  return sym;
+}
+
+// jpeg_gen_optimal_table (JPEG Annex K.2 with libjpeg's tie-breaking and the reserved symbol 256,
+// whose all-ones code no real symbol gets) of frame blockIdx.x's four tables, warp t building table
+// t, then its canonical codes.
+__global__ void __launch_bounds__(kTableThreads) table_kernel(const __grid_constant__ JpegParams p) {
+  __shared__ unsigned long long freq[4][257];
+  __shared__ int16_t size[4][257], others[4][257];
+  __shared__ int bits[4][33];
+  const int t = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  FrameHuff& fh = p.huff[blockIdx.x];
+  const unsigned long long* src = p.freq + ((int64_t)blockIdx.x * 4 + t) * 256;
+  unsigned long long* f = freq[t];
+  int16_t* sz = size[t];
+  int16_t* ot = others[t];
+  for (int i = lane; i < 257; i += 32) {
+    f[i] = i < 256 ? src[i] : 1;
+    sz[i] = 0;
+    ot[i] = -1;
+  }
+  for (int i = lane; i < 33; i += 32) bits[t][i] = 0;
+  __syncwarp();
+  for (;;) {
+    int c1 = warp_min_symbol(f, -1, lane);
+    int c2 = warp_min_symbol(f, c1, lane);
+    if (c2 < 0) break;
+    if (lane == 0) {
+      f[c1] += f[c2];
+      f[c2] = 0;
+      ++sz[c1];
+      while (ot[c1] >= 0) ++sz[c1 = ot[c1]];
+      ot[c1] = (int16_t)c2;
+      ++sz[c2];
+      while (ot[c2] >= 0) ++sz[c2 = ot[c2]];
+    }
+    __syncwarp();
+  }
+  if (lane == 0) {
+    int* nb = bits[t];
+    for (int i = 0; i < 257; ++i)
+      if (sz[i]) ++nb[min((int)sz[i], 32)];  // libjpeg refuses longer codes (2^31 symbols and more)
+    for (int i = 32; i > 16; --i)           // lengths above 16 moved up the tree
+      while (nb[i] > 0) {
+        int j = i - 2;
+        while (nb[j] == 0) --j;
+        nb[i] -= 2;
+        ++nb[i - 1];
+        nb[j + 1] += 2;
+        --nb[j];
+      }
+    int i = 16;
+    while (nb[i] == 0) --i;
+    --nb[i];                                // the reserved symbol's code
+    int count = 0;
+    for (int l = 1; l <= 16; ++l) {
+      fh.s.bits[t][l - 1] = (uint8_t)nb[l];
+      count += nb[l];
+    }
+    fh.s.count[t] = (int16_t)count;
+  }
+  __syncwarp();
+  // the symbols by (length before the limit, symbol)
+  for (int s = lane; s < 256; s += 32) {
+    if (!sz[s]) continue;
+    int rank = 0;
+    for (int u = 0; u < 256; ++u) rank += sz[u] && (sz[u] < sz[s] || (sz[u] == sz[s] && u < s));
+    fh.s.vals[t][rank] = (uint8_t)s;
+  }
+  __syncwarp();
+  if (lane == 0) {                          // canonical codes, as Annex C assigns them
+    const bool ac = t & 1;
+    uint16_t* code = ac ? fh.c.ac_code[t >> 1] : fh.c.dc_code[t >> 1];
+    uint8_t* len = ac ? fh.c.ac_len[t >> 1] : fh.c.dc_len[t >> 1];
+    int c = 0, k = 0;
+    for (int l = 1; l <= 16; ++l) {
+      for (int i = 0; i < fh.s.bits[t][l - 1]; ++i, ++k, ++c) {
+        code[fh.s.vals[t][k]] = (uint16_t)c;
+        len[fh.s.vals[t][k]] = (uint8_t)l;
+      }
+      c <<= 1;
+    }
+  }
+}
+
 // ---- 2. code lengths and chunk sums -------------------------------------------------------------
 // The bits of block b's codes: its DC difference (the block before it of its component is another
 // thread's), then its AC run/size codes with ZRLs and EOB.
-__device__ int block_bits(const JpegGeom& g, const int16_t* coef, int b) {
-  const int u = b % 6, t = u >= 4;
+__device__ __forceinline__ int block_bits(const JpegParams& p, const JpegGeom& g, const HuffCodes& H, const int16_t* coef, int b) {
+  const int u = b % p.per, t = u >= p.luma;
   const int16_t* z = coef + (int64_t)b * 64;
-  const int diff = dummy_block(g, b / 6, u) ? 0 : z[0] - prev_dc(g, coef, b);
-  int bits = kHuff.dc_len[t][nbits(diff)] + nbits(diff), run = 0;
+  const int diff = dummy_block(p, g, b / p.per, u) ? 0 : z[0] - prev_dc(p, g, coef, b);
+  int bits = H.dc_len[t][nbits(diff)] + nbits(diff), run = 0;
 #pragma unroll 4
   for (int k = 1; k < 64; ++k) {
     const int v = z[kZigzagDev[k]];
@@ -306,34 +525,36 @@ __device__ int block_bits(const JpegGeom& g, const int16_t* coef, int b) {
       ++run;
     } else {
       const int nb = nbits(v);
-      bits += (run >> 4) * kHuff.ac_len[t][0xF0] + kHuff.ac_len[t][((run & 15) << 4) | nb] + nb;
+      bits += (run >> 4) * H.ac_len[t][0xF0] + H.ac_len[t][((run & 15) << 4) | nb] + nb;
       run = 0;
     }
   }
-  return bits + (run ? kHuff.ac_len[t][0] : 0);
+  return bits + (run ? H.ac_len[t][0] : 0);
 }
 
+template <bool kOpt>
 __global__ void __launch_bounds__(kChunk) block_bits_kernel(const __grid_constant__ JpegParams p) {
   __shared__ int64_t warp[32];
   const JpegGeom& g = p.g[blockIdx.y];
   if ((int)blockIdx.x >= g.chunks) return;
   const int b = blockIdx.x * kChunk + threadIdx.x;
-  const int bits = b < g.blocks ? block_bits(g, p.coef + g.blk * 64, b) : 0;
+  const int bits = b < g.blocks ? block_bits(p, g, huff_codes_of<kOpt>(p, blockIdx.y), p.coef + g.blk * 64, b) : 0;
   p.bits[g.blk + b] = (uint32_t)bits;
   int64_t total;
   block_exclusive_scan(bits, warp, &total);
   if (threadIdx.x == 0) p.sums[g.csum + blockIdx.x] = total;
 }
 
-// ---- 3, 6. per-frame exclusive scans of chunk sums ------------------------------------------------
+// ---- 3, 3b, 6. per-frame exclusive scans of chunk sums ----------------------------------------------
+enum ScanOf { kScanBlocks, kScanStuffing, kScanIntervals };
 // Frame blockIdx.x's `count` chunk sums from sums[first] become their exclusive scan, and the slot
 // after them the total.
 __global__ void __launch_bounds__(kScanThreads) scan_kernel(const __grid_constant__ JpegParams p,
-                                                            int stuffing) {
+                                                            int which) {
   __shared__ int64_t warp[32];
   const JpegGeom& g = p.g[blockIdx.x];
-  int64_t* s = p.sums + (stuffing ? g.ssum : g.csum);
-  const int count = stuffing ? g.schunks : g.chunks;
+  int64_t* s = p.sums + (which == kScanBlocks ? g.csum : which == kScanStuffing ? g.ssum : g.isum);
+  const int count = which == kScanBlocks ? g.chunks : which == kScanStuffing ? g.schunks : g.ints;
   int64_t carry = 0;
   for (int base = 0; base < count; base += kScanThreads) {
     const int i = base + threadIdx.x;
@@ -344,6 +565,26 @@ __global__ void __launch_bounds__(kScanThreads) scan_kernel(const __grid_constan
     carry += total;
   }
   if (threadIdx.x == 0) s[count] = carry;
+}
+
+// ---- 3a. restart intervals --------------------------------------------------------------------------
+// The first bit of block b (b <= blocks) in the unpadded stream, from its chunk's first bit.
+__device__ int64_t block_first_bit(const JpegParams& p, const JpegGeom& g, int b) {
+  if (b == g.blocks) return p.sums[g.csum + g.chunks];
+  int64_t s = p.sums[g.csum + b / kChunk];
+  for (int k = b - b % kChunk; k < b; ++k) s += p.bits[g.blk + k];
+  return s;
+}
+
+// One thread per interval: its first bit, and its bytes once padded to a byte.
+__global__ void __launch_bounds__(kChunk) interval_kernel(const __grid_constant__ JpegParams p) {
+  const JpegGeom& g = p.g[blockIdx.y];
+  const int i = blockIdx.x * kChunk + threadIdx.x;
+  if (i >= g.ints) return;
+  const int first = i * p.rst * p.per, end = min(first + p.rst * p.per, g.blocks);
+  const int64_t a = block_first_bit(p, g, first), e = block_first_bit(p, g, end);
+  p.ipos[g.ipos + i] = a;
+  p.sums[g.isum + i] = (e - a + 7) >> 3;
 }
 
 // ---- 4. pack ------------------------------------------------------------------------------------
@@ -365,6 +606,7 @@ struct BitWriter {
   }
 };
 
+template <bool kOpt>
 __global__ void __launch_bounds__(kChunk) pack_kernel(const __grid_constant__ JpegParams p) {
   __shared__ int64_t warp[32];
   const JpegGeom& g = p.g[blockIdx.y];
@@ -373,15 +615,22 @@ __global__ void __launch_bounds__(kChunk) pack_kernel(const __grid_constant__ Jp
   const int64_t gb = g.blk + b;
   const int64_t bits = b < g.blocks ? p.bits[gb] : 0;
   int64_t total;
-  const int64_t pos = p.sums[g.csum + blockIdx.x] + block_exclusive_scan(bits, warp, &total);
+  int64_t pos = p.sums[g.csum + blockIdx.x] + block_exclusive_scan(bits, warp, &total);
   if (b >= g.blocks) return;
-  const int u = b % 6, t = u >= 4;
+  bool last = b == g.blocks - 1;          // the last block of its interval pads it to a byte
+  if (p.rst) {                            // from the interval's first bit to its first byte
+    const int span = p.rst * p.per, i = b / span;
+    pos += 8 * p.sums[g.isum + i] - p.ipos[g.ipos + i];
+    last |= (b + 1) % span == 0;
+  }
+  const HuffCodes& H = huff_codes_of<kOpt>(p, blockIdx.y);
+  const int u = b % p.per, t = u >= p.luma;
   BitWriter w{p.stream + g.words + (pos >> 5), 0, (int)(pos & 31)};
-  const bool dummy = dummy_block(g, b / 6, u);
+  const bool dummy = dummy_block(p, g, b / p.per, u);
   const int16_t* z = p.coef + gb * 64;
-  const int diff = dummy ? 0 : z[0] - prev_dc(g, p.coef + g.blk * 64, b);
+  const int diff = dummy ? 0 : z[0] - prev_dc(p, g, p.coef + g.blk * 64, b);
   const int dn = nbits(diff);
-  w.put(kHuff.dc_code[t][dn], kHuff.dc_len[t][dn]);
+  w.put(H.dc_code[t][dn], H.dc_len[t][dn]);
   if (dn) w.put((uint32_t)(diff < 0 ? diff - 1 : diff) & ((1u << dn) - 1), dn);
   int run = 0;
 #pragma unroll 1
@@ -391,15 +640,15 @@ __global__ void __launch_bounds__(kChunk) pack_kernel(const __grid_constant__ Jp
       ++run;
       continue;
     }
-    for (; run > 15; run -= 16) w.put(kHuff.ac_code[t][0xF0], kHuff.ac_len[t][0xF0]);
+    for (; run > 15; run -= 16) w.put(H.ac_code[t][0xF0], H.ac_len[t][0xF0]);
     const int nb = nbits(v), sym = (run << 4) | nb;
-    w.put(kHuff.ac_code[t][sym], kHuff.ac_len[t][sym]);
+    w.put(H.ac_code[t][sym], H.ac_len[t][sym]);
     w.put((uint32_t)(v < 0 ? v - 1 : v) & ((1u << nb) - 1), nb);
     run = 0;
   }
-  if (run) w.put(kHuff.ac_code[t][0], kHuff.ac_len[t][0]);
-  if (b == g.blocks - 1) {                  // 1-bits to the byte boundary
-    const int pad = (int)(-p.sums[g.csum + g.chunks] & 7);
+  if (run) w.put(H.ac_code[t][0], H.ac_len[t][0]);
+  if (last) {                               // 1-bits to the byte boundary
+    const int pad = (int)(-(pos + bits) & 7);
     if (pad) w.put((1u << pad) - 1, pad);
   }
   w.flush();
@@ -410,28 +659,71 @@ __device__ __forceinline__ uint8_t stream_byte(const uint32_t* words, int64_t j)
   return (uint8_t)(words[j >> 2] >> (24 - 8 * (j & 3)));
 }
 
+// The bytes of the frame's stream before stuffing.
+__device__ __forceinline__ int64_t stream_bytes(const JpegParams& p, const JpegGeom& g) {
+  return p.rst ? p.sums[g.isum + g.ints] : (p.sums[g.csum + g.chunks] + 7) >> 3;
+}
+
+// The first interval after the first (which has no marker) starting at byte `first` or later.
+__device__ int first_marker(const JpegParams& p, const JpegGeom& g, int64_t first) {
+  int lo = 1, hi = g.ints;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (p.sums[g.isum + mid] < first) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
 __global__ void __launch_bounds__(kStuffThreads) count_ff_kernel(const __grid_constant__ JpegParams p) {
   __shared__ int64_t warp[32];
   const JpegGeom& g = p.g[blockIdx.y];
   if ((int)blockIdx.x >= g.schunks) return;
-  const int64_t bytes = (p.sums[g.csum + g.chunks] + 7) >> 3;
+  const int64_t bytes = stream_bytes(p, g);
   const int64_t first = (int64_t)blockIdx.x * kStuffChunk + threadIdx.x * kStuffBytes;
   const uint32_t* words = p.stream + g.words;
   int ff = 0;
   for (int i = 0; i < kStuffBytes && first + i < bytes; ++i) ff += stream_byte(words, first + i) == 0xFF;
+  if (p.rst && first < bytes)               // RSTn: 2 bytes before an interval's first byte
+    for (int i = first_marker(p, g, first); i < g.ints && p.sums[g.isum + i] < first + kStuffBytes; ++i) ff += 2;
   int64_t total;
   block_exclusive_scan(ff, warp, &total);
   if (threadIdx.x == 0) p.sums[g.ssum + blockIdx.x] = total;
 }
 
 // ---- 7. stuff, header, EOI, length --------------------------------------------------------------
+// Byte i of the frame's header: the template's SOI .. SOF0 with the frame's height and width, the
+// four DHT segments of `hs`, then the template's DRI and SOS.
+__device__ uint8_t header_byte(const StuffParams& sp, const JpegGeom& g, const HuffSpec& hs, int i) {
+  if (i < kPrefixBytes) {
+    if (i < kSofSize || i >= kSofSize + 4) return sp.prefix[i];
+    const int v = i < kSofSize + 2 ? g.h : g.w;
+    return (uint8_t)(i & 1 ? v >> 8 : v);          // kSofSize is odd: the high byte first
+  }
+  i -= kPrefixBytes;
+  for (int t = 0; t < 4; ++t) {
+    const int len = 21 + hs.count[t];
+    if (i < len) {
+      if (i < 2) return i ? 0xC4 : 0xFF;
+      if (i < 4) return (uint8_t)(i == 2 ? (len - 2) >> 8 : len - 2);
+      if (i == 4) return (uint8_t)(((t & 1) << 4) | (t >> 1));
+      return i < 21 ? hs.bits[t][i - 5] : hs.vals[t][i - 21];
+    }
+    i -= len;
+  }
+  return sp.suffix[i];
+}
+
+template <bool kOpt>
 __global__ void __launch_bounds__(kStuffThreads) stuff_kernel(const __grid_constant__ StuffParams sp) {
   __shared__ int64_t warp[32];
   const JpegParams& p = sp.p;
   const JpegGeom& g = p.g[blockIdx.y];
   if ((int)blockIdx.x >= g.schunks) return;
-  const int64_t bytes = (p.sums[g.csum + g.chunks] + 7) >> 3;
-  const int64_t size = kHeaderBytes + bytes + p.sums[g.ssum + g.schunks] + 2;
+  const HuffSpec& hs = kOpt ? p.huff[blockIdx.y].s : sp.std;
+  const int header = kPrefixBytes + 84 + hs.count[0] + hs.count[1] + hs.count[2] + hs.count[3] + sp.suffix_bytes;
+  const int64_t bytes = stream_bytes(p, g);
+  const int64_t size = header + bytes + p.sums[g.ssum + g.schunks] + 2;
   if (blockIdx.x == 0 && threadIdx.x == 0) *g.length = size <= p.cap ? size : -1;
   if (size > p.cap) return;
   const int64_t first = (int64_t)blockIdx.x * kStuffChunk + threadIdx.x * kStuffBytes;
@@ -443,17 +735,24 @@ __global__ void __launch_bounds__(kStuffThreads) stuff_kernel(const __grid_const
     v[i] = first + i < bytes ? stream_byte(words, first + i) : 0;
     ff += first + i < bytes && v[i] == 0xFF;
   }
+  int marker = g.ints;
+  if (p.rst && first < bytes) {
+    marker = first_marker(p, g, first);
+    for (int i = marker; i < g.ints && p.sums[g.isum + i] < first + kStuffBytes; ++i) ff += 2;
+  }
   int64_t total;
-  int64_t o = kHeaderBytes + first + p.sums[g.ssum + blockIdx.x] + block_exclusive_scan(ff, warp, &total);
+  int64_t o = header + first + p.sums[g.ssum + blockIdx.x] + block_exclusive_scan(ff, warp, &total);
   for (int i = 0; i < kStuffBytes && first + i < bytes; ++i) {
+    if (marker < g.ints && p.sums[g.isum + marker] == first + i) {
+      g.out[o++] = 0xFF;
+      g.out[o++] = (uint8_t)(0xD0 + ((marker - 1) & 7));
+      ++marker;
+    }
     g.out[o++] = v[i];
     if (v[i] == 0xFF) g.out[o++] = 0;
   }
   if (blockIdx.x == 0) {
-    // the template with SOF0's height and width (bytes kSofSize.. of jpeg_header) filled in
-    const int hw[4] = {g.h >> 8, g.h & 255, g.w >> 8, g.w & 255};
-    for (int i = threadIdx.x; i < kHeaderBytes; i += kStuffThreads)
-      g.out[i] = i >= kSofSize && i < kSofSize + 4 ? (uint8_t)hw[i - kSofSize] : sp.header[i];
+    for (int i = threadIdx.x; i < header; i += kStuffThreads) g.out[i] = header_byte(sp, g, hs, i);
     if (threadIdx.x == 0) {
       g.out[size - 2] = 0xFF;
       g.out[size - 1] = 0xD9;
@@ -462,8 +761,46 @@ __global__ void __launch_bounds__(kStuffThreads) stuff_kernel(const __grid_const
 }
 
 // ---- host side -----------------------------------------------------------------------------------
-// The header of `quality` with height and width 0: SOI, JFIF APP0, DQT x 2, SOF0, DHT x 4, SOS.
-void jpeg_header(const uint16_t (&q)[2][64], uint8_t* out) {
+// What one call encodes with (cv2's parameters resolved): the luma and chroma qualities, the luma
+// sampling factors, optimized tables or not, and the restart interval in MCUs.
+struct Settings {
+  int lq, cq, hs, vs, optimize, rst;
+};
+constexpr Settings kDefaultSettings = {95, 95, 2, 2, 0, 0};
+
+// The parameters' settings, or a refusal naming the call: a quality outside [1, 100] (-1 leaves
+// luma_quality and chroma_quality unset), a sampling other than cv2's five, optimize other than 0
+// or 1, a restart interval outside [0, 65535].  As cv2: luma_quality replaces quality, chroma_quality
+// counts only with it, and two different ones make the file 4:4:4.
+int resolve_params(const std::string& name, const sqdet_jpeg_params* jp, Settings* s) {
+  if (!jp) return fail(SQDET_ERR_INVALID_ARG, name + ": null params");
+  if (jp->quality < 1 || jp->quality > 100) return fail(SQDET_ERR_INVALID_ARG, name + ": quality must be in [1, 100]");
+  for (int q : {jp->luma_quality, jp->chroma_quality})
+    if (q != -1 && (q < 1 || q > 100))
+      return fail(SQDET_ERR_INVALID_ARG, name + ": luma_quality and chroma_quality must be -1 or in [1, 100]");
+  const int f = jp->sampling;
+  if (f != 0x411111 && f != 0x221111 && f != 0x211111 && f != 0x121111 && f != 0x111111)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": sampling must be 0x411111, 0x221111, 0x211111, 0x121111 or 0x111111");
+  if (jp->optimize != 0 && jp->optimize != 1) return fail(SQDET_ERR_INVALID_ARG, name + ": optimize must be 0 or 1");
+  if (jp->restart_interval < 0 || jp->restart_interval > 65535)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": restart_interval must be in [0, 65535]");
+  s->hs = f >> 20;
+  s->vs = (f >> 16) & 15;
+  s->lq = s->cq = jp->quality;
+  if (jp->luma_quality != -1) {
+    s->lq = jp->luma_quality;
+    s->cq = jp->chroma_quality != -1 ? jp->chroma_quality : s->lq;
+    if (s->cq != s->lq) s->hs = s->vs = 1;
+  }
+  s->optimize = jp->optimize;
+  s->rst = jp->restart_interval;
+  return SQDET_OK;
+}
+
+// The header's template: SOI, JFIF APP0, DQT x 2 and SOF0 (height and width 0) into prefix, DRI
+// (with restart markers) and SOS into suffix; returns the suffix's bytes.
+int jpeg_header(const uint16_t (&q)[2][64], const Settings& st, uint8_t* prefix, uint8_t* suffix) {
+  uint8_t* out = prefix;
   int n = 0;
   auto put = [&](std::initializer_list<int> bytes) { for (int b : bytes) out[n++] = (uint8_t)b; };
   auto seg = [&](int marker, int len) { put({0xFF, marker, (len + 2) >> 8, (len + 2) & 255}); };
@@ -476,144 +813,204 @@ void jpeg_header(const uint16_t (&q)[2][64], uint8_t* out) {
     for (int k = 0; k < 64; ++k) out[n++] = (uint8_t)q[t][kZigzag[k]];
   }
   seg(0xC0, 15);                          // height and width at kSofSize, filled in per frame
-  put({8, 0, 0, 0, 0, 3, 1, 0x22, 0, 2, 0x11, 1, 3, 0x11, 1});
-  const uint8_t* bits[4] = {kDcLumaBits, kAcLumaBits, kDcChromaBits, kAcChromaBits};
-  const uint8_t* vals[4] = {kDcVals, kAcLumaVals, kDcVals, kAcChromaVals};
-  const int ids[4] = {0x00, 0x10, 0x01, 0x11};
-  for (int t = 0; t < 4; ++t) {
-    int count = 0;
-    for (int l = 0; l < 16; ++l) count += bits[t][l];
-    seg(0xC4, 17 + count);
-    put({ids[t]});
-    for (int l = 0; l < 16; ++l) out[n++] = bits[t][l];
-    for (int k = 0; k < count; ++k) out[n++] = vals[t][k];
+  put({8, 0, 0, 0, 0, 3, 1, st.hs << 4 | st.vs, 0, 2, 0x11, 1, 3, 0x11, 1});
+  out = suffix;
+  n = 0;
+  if (st.rst) {
+    seg(0xDD, 2);
+    put({st.rst >> 8, st.rst & 255});
   }
   seg(0xDA, 10);
   put({3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0});
+  return n;
+}
+
+// The Annex K tables as DHT writes them.
+HuffSpec std_spec() {
+  HuffSpec h{};
+  const uint8_t* bits[4] = {kDcLumaBits, kAcLumaBits, kDcChromaBits, kAcChromaBits};
+  const uint8_t* vals[4] = {kDcVals, kAcLumaVals, kDcVals, kAcChromaVals};
+  for (int t = 0; t < 4; ++t) {
+    int count = 0;
+    for (int l = 0; l < 16; ++l) count += h.bits[t][l] = bits[t][l];
+    for (int k = 0; k < count; ++k) h.vals[t][k] = vals[t][k];
+    h.count[t] = (int16_t)count;
+  }
+  return h;
 }
 
 // One frame's sizes in the scratch.
 struct FrameSizes {
-  int blocks, chunks, schunks;
-  int64_t words;
+  int blocks, chunks, schunks, ints;
+  int64_t bytes, words;                 // the stream's largest bytes before stuffing, its words
 };
-FrameSizes frame_sizes(int h, int w) {
+FrameSizes frame_sizes(int h, int w, const Settings& st) {
   FrameSizes s;
-  s.blocks = ((h + 15) / 16) * ((w + 15) / 16) * 6;
+  const int64_t mcus = (int64_t)((h + 8 * st.vs - 1) / (8 * st.vs)) * ((w + 8 * st.hs - 1) / (8 * st.hs));
+  s.blocks = (int)(mcus * (st.hs * st.vs + 2));
   s.chunks = (s.blocks + kChunk - 1) / kChunk;
-  const int64_t max_bytes = ((int64_t)s.blocks * kMaxBlockBits + 7) / 8;
-  s.schunks = (int)((max_bytes + kStuffChunk - 1) / kStuffChunk);
-  s.words = (max_bytes + 3) / 4 + 1;
+  s.ints = st.rst ? (int)((mcus + st.rst - 1) / st.rst) : 1;
+  // each interval is padded to a byte
+  s.bytes = ((int64_t)s.blocks * (st.optimize ? kMaxBlockBitsOpt : kMaxBlockBits) + 7) / 8 + (st.rst ? s.ints : 0);
+  s.schunks = (int)((s.bytes + kStuffChunk - 1) / kStuffChunk);
+  s.words = (s.bytes + 3) / 4 + 1;
   return s;
 }
 
 int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
 
-// The scratch of the frames [first, first + count): coefficients, bit lengths, chunk sums, bit
-// buffers, in that order.
+// The scratch of the frames [first, first + count): coefficients, bit lengths, chunk sums,
+// intervals' first bits, bit buffers, symbol counts and tables, in that order.
 struct GroupLayout {
-  int64_t coef, bits, sums, stream, total;
+  int64_t coef, bits, sums, ipos, stream, freq, huff, total;
 };
-GroupLayout group_layout(const FrameSource* fr, int first, int count, JpegGeom* g) {
-  int64_t blocks = 0, sums = 0, words = 0;
+GroupLayout group_layout(const FrameSource* fr, int first, int count, const Settings& st, JpegGeom* g) {
+  int64_t blocks = 0, sums = 0, ints = 0, words = 0;
   for (int i = 0; i < count; ++i) {
     const FrameSource& s = fr[first + i];
-    const FrameSizes z = frame_sizes(s.h, s.w);
+    const FrameSizes z = frame_sizes(s.h, s.w, st);
+    const int isums = st.rst ? z.ints + 1 : 0;
     if (g) {
       g[i].h = s.h;
       g[i].w = s.w;
-      g[i].mcu_cols = (s.w + 15) / 16;
+      g[i].mcu_cols = (s.w + 8 * st.hs - 1) / (8 * st.hs);
       g[i].blocks = z.blocks;
       g[i].chunks = z.chunks;
       g[i].schunks = z.schunks;
+      g[i].ints = z.ints;
       g[i].blk = blocks;
       g[i].csum = sums;
       g[i].ssum = sums + z.chunks + 1;
+      g[i].isum = sums + z.chunks + 1 + z.schunks + 1;
+      g[i].ipos = ints;
       g[i].words = words;
     }
     blocks += (int64_t)z.chunks * kChunk;
-    sums += z.chunks + 1 + z.schunks + 1;
+    sums += z.chunks + 1 + z.schunks + 1 + isums;
+    ints += st.rst ? z.ints : 0;
     words += z.words;
   }
   GroupLayout L;
   L.coef = 0;
   L.bits = L.coef + align256(blocks * 64 * 2);
   L.sums = L.bits + align256(blocks * 4);
-  L.stream = L.sums + align256(sums * 8);
-  L.total = L.stream + align256(words * 4);
+  L.ipos = L.sums + align256(sums * 8);
+  L.stream = L.ipos + align256(ints * 8);
+  L.freq = L.stream + align256(words * 4);
+  L.huff = L.freq + (st.optimize ? align256((int64_t)count * 4 * 256 * 8) : 0);
+  L.total = L.huff + (st.optimize ? align256((int64_t)count * sizeof(FrameHuff)) : 0);
   return L;
 }
 
+template <int F, int HS, int VS>
+void launch_transform(const dim3& grid, const TransformParams<F>& tp, cudaStream_t stream) {
+  transform_kernel<F, HS, VS><<<grid, kChunk, 0, stream>>>(tp);
+}
+
 template <int F>
-int launch_group(const PixFormat& pf, const FrameSource* fr, int first, int count,
-                 const QuantRecip& quant, const uint8_t* header, uint8_t* out, int64_t cap,
+int launch_group(const PixFormat& pf, const FrameSource* fr, int first, int count, const Settings& st,
+                 const QuantRecip& quant, const StuffParams& templ, uint8_t* out, int64_t cap,
                  int64_t* lengths, uint8_t* scratch, cudaStream_t stream) {
   TransformParams<F> tp;
   JpegParams& p = tp.p;
-  const GroupLayout L = group_layout(fr, first, count, p.g);
-  int max_chunks = 0, max_schunks = 0;
+  const GroupLayout L = group_layout(fr, first, count, st, p.g);
+  int max_chunks = 0, max_schunks = 0, max_ints = 0;
   for (int i = 0; i < count; ++i) {
     p.g[i].out = out + (int64_t)(first + i) * cap;
     p.g[i].length = lengths + first + i;
     tp.f[i] = frame_desc<kPlanes<F>>(pf, fr[first + i], fr[first + i].h, fr[first + i].w);
     max_chunks = std::max(max_chunks, p.g[i].chunks);
     max_schunks = std::max(max_schunks, p.g[i].schunks);
+    max_ints = std::max(max_ints, p.g[i].ints);
   }
   p.coef = reinterpret_cast<int16_t*>(scratch + L.coef);
   p.bits = reinterpret_cast<uint32_t*>(scratch + L.bits);
   p.sums = reinterpret_cast<int64_t*>(scratch + L.sums);
+  p.ipos = reinterpret_cast<int64_t*>(scratch + L.ipos);
   p.stream = reinterpret_cast<uint32_t*>(scratch + L.stream);
+  p.freq = reinterpret_cast<unsigned long long*>(scratch + L.freq);
+  p.huff = reinterpret_cast<FrameHuff*>(scratch + L.huff);
   p.cap = cap;
+  p.hs = st.hs;
+  p.vs = st.vs;
+  p.luma = st.hs * st.vs;
+  p.per = p.luma + 2;
+  p.rst = st.rst;
   tp.quant = quant;
-  SQ_CUDA(cudaMemsetAsync(p.stream, 0, (size_t)(L.total - L.stream), stream));
+  // the bit buffers and the symbol counts
+  SQ_CUDA(cudaMemsetAsync(p.stream, 0, (size_t)(L.huff - L.stream), stream));
   const dim3 grid((unsigned)max_chunks, (unsigned)count), sgrid((unsigned)max_schunks, (unsigned)count);
-  transform_kernel<F><<<grid, kChunk, 0, stream>>>(tp);
+  switch (st.hs * 16 + st.vs) {
+    case 0x41: launch_transform<F, 4, 1>(grid, tp, stream); break;
+    case 0x21: launch_transform<F, 2, 1>(grid, tp, stream); break;
+    case 0x12: launch_transform<F, 1, 2>(grid, tp, stream); break;
+    case 0x11: launch_transform<F, 1, 1>(grid, tp, stream); break;
+    default: launch_transform<F, 2, 2>(grid, tp, stream);
+  }
   SQ_CHECK_LAUNCH("jpeg transform_kernel");
-  block_bits_kernel<<<grid, kChunk, 0, stream>>>(p);
+  if (st.optimize) {
+    hist_kernel<<<grid, kChunk, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg hist_kernel");
+    table_kernel<<<(unsigned)count, kTableThreads, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg table_kernel");
+    block_bits_kernel<true><<<grid, kChunk, 0, stream>>>(p);
+  } else {
+    block_bits_kernel<false><<<grid, kChunk, 0, stream>>>(p);
+  }
   SQ_CHECK_LAUNCH("jpeg block_bits_kernel");
-  scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(p, 0);
+  scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(p, kScanBlocks);
   SQ_CHECK_LAUNCH("jpeg scan_kernel");
-  pack_kernel<<<grid, kChunk, 0, stream>>>(p);
+  if (st.rst) {
+    interval_kernel<<<dim3((unsigned)((max_ints + kChunk - 1) / kChunk), (unsigned)count), kChunk, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg interval_kernel");
+    scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(p, kScanIntervals);
+    SQ_CHECK_LAUNCH("jpeg scan_kernel");
+  }
+  if (st.optimize) pack_kernel<true><<<grid, kChunk, 0, stream>>>(p);
+  else pack_kernel<false><<<grid, kChunk, 0, stream>>>(p);
   SQ_CHECK_LAUNCH("jpeg pack_kernel");
   count_ff_kernel<<<sgrid, kStuffThreads, 0, stream>>>(p);
   SQ_CHECK_LAUNCH("jpeg count_ff_kernel");
-  scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(p, 1);
+  scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(p, kScanStuffing);
   SQ_CHECK_LAUNCH("jpeg scan_kernel");
-  StuffParams sp;
+  StuffParams sp = templ;
   sp.p = p;
-  memcpy(sp.header, header, kHeaderBytes);
-  stuff_kernel<<<sgrid, kStuffThreads, 0, stream>>>(sp);
+  if (st.optimize) stuff_kernel<true><<<sgrid, kStuffThreads, 0, stream>>>(sp);
+  else stuff_kernel<false><<<sgrid, kStuffThreads, 0, stream>>>(sp);
   SQ_CHECK_LAUNCH("jpeg stuff_kernel");
   return SQDET_OK;
 }
 
 // The largest file of an h x w crop.
-int64_t jpeg_max_bytes(int h, int w) {
-  const FrameSizes s = frame_sizes(h, w);
-  return kHeaderBytes + 2 * (((int64_t)s.blocks * kMaxBlockBits + 7) / 8) + 2;
+int64_t jpeg_max_bytes(int h, int w, const Settings& st) {
+  const FrameSizes s = frame_sizes(h, w, st);
+  // the header (optimized tables are no longer than Annex K's), the stream with every byte
+  // stuffed, RSTn between intervals, EOI
+  return kHeaderBytes + (st.rst ? kDriBytes : 0) + 2 * s.bytes + 2 * (int64_t)(s.ints - 1) + 2;
 }
 
 // The scratch the encode of the crops of `frames` needs.
-int64_t jpeg_scratch_bytes(const FrameSource* frames, int n) {
+int64_t jpeg_scratch_bytes(const FrameSource* frames, int n, const Settings& st) {
   int64_t most = 0;
   for (int first = 0; first < n; first += kJpegFramesPerLaunch)
-    most = std::max(most, group_layout(frames, first, std::min(kJpegFramesPerLaunch, n - first), nullptr).total);
+    most = std::max(most, group_layout(frames, first, std::min(kJpegFramesPerLaunch, n - first), st, nullptr).total);
   return most;
 }
 
 // The encode of the crops of `frames` (the frames' checks are the caller's).
-int launch_encode_jpeg(int format, const FrameSource* frames, int n, int quality, uint8_t* out,
+int launch_encode_jpeg(int format, const FrameSource* frames, int n, const Settings& st, uint8_t* out,
                        int64_t cap, int64_t* lengths, void* scratch, cudaStream_t stream) {
   const PixFormat* pf = pix_format(format);
   if (!pf) return fail(SQDET_ERR_INVALID_ARG, "sqdet_encode_jpeg: unknown format");
-  // jpeg_quality_scaling, then the standard tables scaled, rounded and clamped to 1..255
-  const int scale = quality < 50 ? 5000 / quality : 200 - 2 * quality;
+  // jpeg_quality_scaling of each table's quality, then the standard tables scaled, rounded and
+  // clamped to 1..255
+  const int scale[2] = {st.lq < 50 ? 5000 / st.lq : 200 - 2 * st.lq, st.cq < 50 ? 5000 / st.cq : 200 - 2 * st.cq};
   uint16_t q[2][64];
   QuantRecip quant;
   for (int i = 0; i < 64; ++i) {
     const uint8_t base[2] = {kStdLumaQ[i], kStdChromaQ[i]};
     for (int t = 0; t < 2; ++t) {
-      const int v = std::min(std::max((base[t] * scale + 50) / 100, 1), 255);
+      const int v = std::min(std::max((base[t] * scale[t] + 50) / 100, 1), 255);
       q[t][i] = (uint16_t)v;
       // compute_reciprocal of d = 8 v >= 8: r = 16 + floor(log2 d); a power of two drops a bit
       const uint32_t d = 8u * v;
@@ -634,22 +1031,23 @@ int launch_encode_jpeg(int format, const FrameSource* frames, int n, int quality
       quant.shift[t][i] = (uint8_t)r;
     }
   }
-  uint8_t header[kHeaderBytes];
-  jpeg_header(q, header);
+  StuffParams sp{};
+  sp.std = std_spec();
+  sp.suffix_bytes = jpeg_header(q, st, sp.prefix, sp.suffix);
   uint8_t* s = static_cast<uint8_t*>(scratch);
   for (int first = 0; first < n; first += kJpegFramesPerLaunch) {
     const int count = std::min(kJpegFramesPerLaunch, n - first);
     int rc;
     switch (format) {
 #define SQ_JPEG_CASE(F) \
-  case F: rc = launch_group<F>(*pf, frames, first, count, quant, header, out, cap, lengths, s, stream); break;
+  case F: rc = launch_group<F>(*pf, frames, first, count, st, quant, sp, out, cap, lengths, s, stream); break;
       SQ_JPEG_CASE(SQDET_FMT_BGR)
       SQ_JPEG_CASE(SQDET_FMT_RGB)
       SQ_JPEG_CASE(SQDET_FMT_BGRA)
       SQ_JPEG_CASE(SQDET_FMT_RGBA)
       SQ_JPEG_CASE(SQDET_FMT_RGB_PLANAR)
       SQ_JPEG_CASE(SQDET_FMT_NV12)
-      default: rc = launch_group<SQDET_FMT_I420>(*pf, frames, first, count, quant, header, out, cap, lengths, s, stream);
+      default: rc = launch_group<SQDET_FMT_I420>(*pf, frames, first, count, st, quant, sp, out, cap, lengths, s, stream);
 #undef SQ_JPEG_CASE
     }
     if (rc) return rc;
@@ -657,31 +1055,51 @@ int launch_encode_jpeg(int format, const FrameSource* frames, int n, int quality
   return SQDET_OK;
 }
 
+// sqdet_jpeg_params of cv2's defaults with `quality`.
+sqdet_jpeg_params default_params(int quality) {
+  return sqdet_jpeg_params{quality, -1, -1, 0x221111, 0, 0};
+}
+
 }  // namespace
 }  // namespace sqdet
 
 using namespace sqdet;
 
-int64_t sqdet_jpeg_max_bytes(int h, int w) {
+int64_t sqdet_jpeg_max_bytes_params(int h, int w, const sqdet_jpeg_params* params) {
+  Settings st;
+  if (resolve_params("sqdet_jpeg_max_bytes", params, &st)) return -1;
   if (h < 1 || w < 1 || h > kJpegMaxSide || w > kJpegMaxSide) {
     fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_max_bytes: h and w must be in [1, 65500]");
     return -1;
   }
-  return jpeg_max_bytes(h, w);
+  return jpeg_max_bytes(h, w, st);
+}
+
+int64_t sqdet_jpeg_max_bytes(int h, int w) {
+  const sqdet_jpeg_params d = default_params(kDefaultSettings.lq);
+  return sqdet_jpeg_max_bytes_params(h, w, &d);
+}
+
+int64_t sqdet_jpeg_scratch_bytes_params(int n, const int32_t* heights, const int32_t* widths,
+                                        const int32_t* crops, const sqdet_jpeg_params* params) {
+  std::vector<FrameSource> fr;
+  Settings st;
+  if (resolve_params("sqdet_jpeg_scratch_bytes", params, &st)) return -1;
+  if (encode_crops("sqdet_jpeg_scratch_bytes", "JPEG", kMaxJpegFrames, kJpegMaxSide, n, heights, widths, crops, fr))
+    return -1;
+  return jpeg_scratch_bytes(fr.data(), n, st);
 }
 
 int64_t sqdet_jpeg_scratch_bytes(int n, const int32_t* heights, const int32_t* widths,
                                  const int32_t* crops) {
-  std::vector<FrameSource> fr;
-  if (encode_crops("sqdet_jpeg_scratch_bytes", "JPEG", kMaxJpegFrames, kJpegMaxSide, n, heights, widths, crops, fr))
-    return -1;
-  return jpeg_scratch_bytes(fr.data(), n);
+  const sqdet_jpeg_params d = default_params(kDefaultSettings.lq);
+  return sqdet_jpeg_scratch_bytes_params(n, heights, widths, crops, &d);
 }
 
-int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
-                      const int32_t* heights, const int32_t* widths, const int32_t* crops,
-                      int quality, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
-                      void* scratch_dev, int64_t scratch_bytes, void* stream) {
+int sqdet_encode_jpeg_params(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
+                             const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                             const sqdet_jpeg_params* params, uint8_t* out_dev, int64_t cap,
+                             int64_t* lengths_dev, void* scratch_dev, int64_t scratch_bytes, void* stream) {
   const std::string name = "sqdet_encode_jpeg";
   const PixFormat* pf = pix_format(format);
   if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
@@ -690,14 +1108,16 @@ int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int
   std::vector<FrameSource> fr;
   int rc = encode_crops(name, "JPEG", kMaxJpegFrames, kJpegMaxSide, n, heights, widths, crops, fr);
   if (rc) return rc;
-  if (quality < 1 || quality > 100) return fail(SQDET_ERR_INVALID_ARG, name + ": quality must be in [1, 100]");
+  Settings st;
+  rc = resolve_params(name, params, &st);
+  if (rc) return rc;
   if (cap < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": cap must be at least 1");
   // the scratch holds int4, int64 and 32-bit atomic regions at 256-byte offsets from its start
   if ((uintptr_t)scratch_dev % 256)
     return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
   if ((uintptr_t)lengths_dev % alignof(int64_t))
     return fail(SQDET_ERR_INVALID_ARG, name + ": lengths_dev must be 8-byte aligned");
-  if (scratch_bytes < jpeg_scratch_bytes(fr.data(), n))
+  if (scratch_bytes < jpeg_scratch_bytes(fr.data(), n, st))
     return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below sqdet_jpeg_scratch_bytes");
   int device = kFrame0Device;
   rc = accept_frames(name, *pf, n, planes, pitches, heights, widths, crops, nullptr, &device, fr);
@@ -709,6 +1129,15 @@ int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int
                                               "device allocation on frame 0's device");
   DeviceGuard guard(device);
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
-  return launch_encode_jpeg(format, fr.data(), n, quality, out_dev, cap, lengths_dev, scratch_dev,
+  return launch_encode_jpeg(format, fr.data(), n, st, out_dev, cap, lengths_dev, scratch_dev,
                             (cudaStream_t)stream);
+}
+
+int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
+                      const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                      int quality, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
+                      void* scratch_dev, int64_t scratch_bytes, void* stream) {
+  const sqdet_jpeg_params d = default_params(quality);
+  return sqdet_encode_jpeg_params(n, format, planes, pitches, heights, widths, crops, &d, out_dev, cap,
+                                  lengths_dev, scratch_dev, scratch_bytes, stream);
 }

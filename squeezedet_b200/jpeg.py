@@ -20,12 +20,36 @@ def _first_tensor(f):
   return f[0] if isinstance(f, (tuple, list)) else f
 
 
-def max_bytes(h, w):
-  """The largest JPEG file of an h x w image (sqdet_jpeg_max_bytes).  Sides are at most 65500,
-  libjpeg's JPEG_MAX_DIMENSION, as for cv2.imencode."""
+# cv2's IMWRITE_JPEG_SAMPLING_FACTOR value of each sampling encode_jpeg_device takes
+SAMPLINGS = {'411': 0x411111, '420': 0x221111, '422': 0x211111, '440': 0x121111, '444': 0x111111}
+
+
+def jpeg_params(quality=95, sampling='420', optimize=False, restart_interval=0, luma_quality=None,
+                chroma_quality=None):
+  """The sqdet_jpeg_params of these settings, checked as the C ABI checks them: qualities in
+  [1, 100] (luma_quality and chroma_quality None when unset), sampling one of SAMPLINGS,
+  restart_interval in [0, 65535] MCUs.  cv2.imencode clamps values out of range instead."""
+  for name, q in (('quality', quality), ('luma_quality', luma_quality),
+                  ('chroma_quality', chroma_quality)):
+    if (q is not None or name == 'quality') and not 1 <= int(q) <= 100:
+      raise ValueError('%s must be in [1, 100], got %r' % (name, q))
+  if sampling not in SAMPLINGS:
+    raise ValueError('sampling must be one of %s, got %r' % (', '.join(SAMPLINGS), sampling))
+  if not 0 <= int(restart_interval) <= 65535:
+    raise ValueError('restart_interval must be in [0, 65535], got %r' % (restart_interval,))
+  return _lib.JpegParams(int(quality), -1 if luma_quality is None else int(luma_quality),
+                         -1 if chroma_quality is None else int(chroma_quality), SAMPLINGS[sampling],
+                         int(bool(optimize)), int(restart_interval))
+
+
+def max_bytes(h, w, **params):
+  """The largest JPEG file of an h x w image (sqdet_jpeg_max_bytes_params) with the keyword
+  settings of encode_jpeg_device.  Sides are at most 65500, libjpeg's JPEG_MAX_DIMENSION, as for
+  cv2.imencode."""
+  p = jpeg_params(**params)
   if not (1 <= int(h) <= 65500 and 1 <= int(w) <= 65500):
     raise ValueError('a JPEG is 1 to 65500 pixels wide and high, got %dx%d' % (w, h))
-  return int(_lib.load().sqdet_jpeg_max_bytes(int(h), int(w)))
+  return int(_lib.load().sqdet_jpeg_max_bytes_params(int(h), int(w), C.byref(p)))
 
 
 def _torch_stream(stream, device):
@@ -40,7 +64,8 @@ def _torch_stream(stream, device):
   return torch.cuda.default_stream(device) if raw == 0 else torch.cuda.ExternalStream(raw, device=device)
 
 
-def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None):
+def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None, *, sampling='420',
+                       optimize=False, restart_interval=0, luma_quality=None, chroma_quality=None):
   """-> (data [n, cap] uint8, lengths [n] int64), both on the frames' device: frame i's file is
   data[i, :lengths[i]], and lengths[i] is -1 if it did not fit cap = the largest file of the
   largest crop.  Asynchronous on `stream` (a torch.cuda.Stream, a raw cudaStream_t, or None for
@@ -52,21 +77,32 @@ def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None):
   take if every block had its longest codes and every byte were 0xFF (sqdet_jpeg_max_bytes, about
   20 MB for 1920 x 1080, whose quality-95 files of natural pictures are under 1 MB), and the
   scratch is about 17 MB per 1080p frame of each group of 16.  128 1080p frames take about 2.6 GB
-  of output; encode fewer frames per call where that matters."""
+  of output; encode fewer frames per call where that matters.
+
+  The keywords are cv2's other JPEG parameters, and the file is what cv2.imencode writes with them:
+  sampling ('411', '420', '422', '440' or '444': IMWRITE_JPEG_SAMPLING_FACTOR), optimize
+  (IMWRITE_JPEG_OPTIMIZE: each frame's own optimal Huffman tables), restart_interval
+  (IMWRITE_JPEG_RST_INTERVAL, in MCUs, 0 for none), luma_quality and chroma_quality
+  (IMWRITE_JPEG_LUMA_QUALITY / _CHROMA_QUALITY: luma_quality replaces quality, chroma_quality
+  counts only with it, and two different ones give 4:4:4 whatever `sampling` says).  4:4:4
+  doubles the worst-case sizes of 4:2:0.  Values cv2 would clamp raise ValueError.  Progressive
+  files are not written: use cv2.imencode with IMWRITE_JPEG_PROGRESSIVE for those."""
   import torch
   frames = list(frames)
   n = frame_count(frames, 128)
   if fmt not in PIXEL_FORMATS:
     raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
-  if not 1 <= int(quality) <= 100:
-    raise ValueError('quality must be in [1, 100], got %r' % (quality,))
+  settings = dict(quality=quality, sampling=sampling, optimize=optimize,
+                  restart_interval=restart_interval, luma_quality=luma_quality,
+                  chroma_quality=chroma_quality)
+  params = jpeg_params(**settings)
   device = getattr(_first_tensor(frames[0]), 'device', None)
   if getattr(device, 'type', None) != 'cuda':
     raise ValueError('frame 0: need a CUDA tensor, got %s' % (device,))
   planes, pitches, hs, ws, rects = pack_frames(frames, fmt, crops, device.index)
   lib = _lib.load()
-  cap = max(max_bytes(rects[4 * i + 3], rects[4 * i + 2]) for i in range(n))
-  scratch_bytes = lib.sqdet_jpeg_scratch_bytes(n, hs, ws, rects)
+  cap = max(max_bytes(rects[4 * i + 3], rects[4 * i + 2], **settings) for i in range(n))
+  scratch_bytes = lib.sqdet_jpeg_scratch_bytes_params(n, hs, ws, rects, C.byref(params))
   if scratch_bytes < 0:
     raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
   s = _torch_stream(stream, device)
@@ -76,9 +112,10 @@ def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None):
     data = torch.empty((n, cap), dtype=torch.uint8, device=device)
     lengths = torch.empty((n,), dtype=torch.int64, device=device)
     scratch = torch.empty((scratch_bytes,), dtype=torch.uint8, device=device)
-    _lib.check(lib.sqdet_encode_jpeg(n, PIXEL_FORMATS.index(fmt), planes, pitches, hs, ws, rects,
-                                     int(quality), data.data_ptr(), cap, lengths.data_ptr(),
-                                     scratch.data_ptr(), scratch_bytes, s.cuda_stream))
+    _lib.check(lib.sqdet_encode_jpeg_params(n, PIXEL_FORMATS.index(fmt), planes, pitches, hs, ws,
+                                            rects, C.byref(params), data.data_ptr(), cap,
+                                            lengths.data_ptr(), scratch.data_ptr(), scratch_bytes,
+                                            s.cuda_stream))
   return data, lengths
 
 
