@@ -22,6 +22,7 @@ Prints one JSON line with the card's name and power limit, read in the same run;
 from __future__ import annotations
 
 import argparse
+import dataclasses
 import json
 import time
 
@@ -30,7 +31,6 @@ import numpy as np
 from .bench_device_frames import make_model
 from .bench_device_u8 import gpu_info
 
-FORMS = ('a_host_imencode', 'b_encode_jpeg_device')
 FRAME_W, FRAME_H, OVERLAP = 1920, 1080, 128
 QUALITY = 95
 SAMPLING_FACTORS = {'411': 0x411111, '420': 0x221111, '422': 0x211111, '440': 0x121111, '444': 0x111111}
@@ -58,15 +58,28 @@ def jpeg_settings(args):
               restart_interval=args.restart)
 
 
-def measure_workload(args, name, model, fmt, clean, grid, torch):
+@dataclasses.dataclass
+class Encoder:
+  """What the benchmarks of the file encoders (this one, bench_png) differ in."""
+  name: str                 # 'jpeg': form (b) is encode_<name>_device, the benchmark bench_<name>
+  ext: str                  # cv2.imencode's extension
+  cv2_params: list          # cv2.imencode's parameters, the same settings as encode's
+  encode: object            # (frames, fmt, stream) -> (data, lengths) on the device
+  files: object             # (data, lengths, stream) -> the files as bytes objects
+  kernels: tuple            # the encode's kernels, as the profiler names them
+  launches: int             # the encode's launches and memsets per 16 frames
+  what: str                 # the files, as the workload names them
+  row: dict                 # the encoder's settings, as each row gives them
+  by_kernel: bool = False   # also give each kernel's device time
+
+  @property
+  def forms(self):
+    return ('a_host_imencode', 'b_encode_%s_device' % self.name)
+
+
+def jpeg_encoder(args):
   import cv2
   from .jpeg import encode_jpeg_device, jpeg_bytes
-  mc = model.mc
-  n = len(clean)
-  tiles = [(f,) + g for f in range(n) for g in grid]
-  stream = torch.cuda.Stream(device=clean[0].device)
-  sptr = stream.cuda_stream
-  work = [torch.empty_like(c) for c in clean]
   settings = jpeg_settings(args)
   cv2_params = [cv2.IMWRITE_JPEG_QUALITY, QUALITY,
                 cv2.IMWRITE_JPEG_SAMPLING_FACTOR, SAMPLING_FACTORS[args.sampling]]
@@ -74,6 +87,24 @@ def measure_workload(args, name, model, fmt, clean, grid, torch):
     cv2_params += [cv2.IMWRITE_JPEG_OPTIMIZE, 1]
   if args.restart:
     cv2_params += [cv2.IMWRITE_JPEG_RST_INTERVAL, args.restart]
+  # per 16 frames: a memset and seven launches, two more with optimize and two with restart markers
+  return Encoder('jpeg', '.jpg', cv2_params,
+                 lambda frames, fmt, stream: encode_jpeg_device(frames, fmt, stream=stream, **settings),
+                 jpeg_bytes, KERNELS, 8 + 2 * args.optimize + 2 * bool(args.restart),
+                 'JPEG quality %d files' % QUALITY,
+                 {'quality': QUALITY, 'sampling': args.sampling, 'optimize': args.optimize,
+                  'restart': args.restart})
+
+
+def measure_workload(enc, args, name, model, fmt, clean, grid, torch):
+  import cv2
+  forms = enc.forms
+  mc = model.mc
+  n = len(clean)
+  tiles = [(f,) + g for f in range(n) for g in grid]
+  stream = torch.cuda.Stream(device=clean[0].device)
+  sptr = stream.cuda_stream
+  work = [torch.empty_like(c) for c in clean]
 
   def drawn():
     with torch.cuda.stream(stream):
@@ -90,26 +121,26 @@ def measure_workload(args, name, model, fmt, clean, grid, torch):
         im = w.cpu().numpy()
         if fmt == 'nv12':
           im = cv2.cvtColor(im, cv2.COLOR_YUV2BGR_NV12)
-        files.append(cv2.imencode('.jpg', im, cv2_params)[1].tobytes())
+        files.append(cv2.imencode(enc.ext, im, enc.cv2_params)[1].tobytes())
     return files
 
   def end_b():
     with torch.cuda.stream(stream):
-      data, lengths = encode_jpeg_device(work, fmt, stream=stream, **settings)
-      return jpeg_bytes(data, lengths, stream=stream)
+      data, lengths = enc.encode(work, fmt, stream)
+      return enc.files(data, lengths, stream=stream)
 
-  ends = {FORMS[0]: end_a, FORMS[1]: end_b}
+  ends = {forms[0]: end_a, forms[1]: end_b}
   drawn()
   want = end_a()
   assert end_b() == want, '%s: the files differ' % name
-  for form in FORMS:
+  for form in forms:
     for _ in range(args.warmup):
       drawn()
       ends[form]()
-  step = {form: [] for form in FORMS}
-  ending = {form: [] for form in FORMS}
+  step = {form: [] for form in forms}
+  ending = {form: [] for form in forms}
   for r in range(args.rounds):
-    for form in (FORMS if r % 2 == 0 else FORMS[::-1]):
+    for form in (forms if r % 2 == 0 else forms[::-1]):
       for _ in range(args.steps):
         t0 = time.perf_counter()
         drawn()
@@ -128,35 +159,37 @@ def measure_workload(args, name, model, fmt, clean, grid, torch):
   outs = []
   with profile(activities=[ProfilerActivity.CUDA]) as prof:
     for _ in range(calls):
-      outs.append(encode_jpeg_device(work, fmt, stream=stream, **settings))
+      outs.append(enc.encode(work, fmt, stream))
     stream.synchronize()
+  names = enc.kernels + ('emset',)
   evs = [ev for ev in prof.events() if ev.device_type == DeviceType.CUDA and
-         any(k in ev.name for k in KERNELS + ('emset',))]
-  # per 16 frames: a memset and seven launches, two more with optimize and two with restart markers
-  launches = calls * -(-n // 16) * (8 + 2 * args.optimize + 2 * bool(args.restart))
+         any(k in ev.name for k in names)]
+  launches = calls * -(-n // 16) * enc.launches
   assert len(evs) >= launches * 9 // 10, 'found %d of %d encode launches' % (len(evs), launches)
   us = sum(ev.time_range.elapsed_us() for ev in evs) / calls
 
   row = {'workload': name, 'engine': '%dx%d b=%d' % (mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT,
                                                      mc.BATCH_SIZE),
-         'frames': n, 'frame': '%dx%d %s' % (FRAME_W, FRAME_H, fmt), 'quality': QUALITY,
-         'sampling': args.sampling, 'optimize': args.optimize, 'restart': args.restart,
+         'frames': n, 'frame': '%dx%d %s' % (FRAME_W, FRAME_H, fmt), **enc.row,
          'file_bytes_mean': float(np.mean([len(f) for f in want]))}
-  for form in FORMS:
+  for form in forms:
     row[form] = {'ms_per_frame_ending_median': 1e3 * float(np.median(ending[form])) / n,
                  'ms_per_frame_ending_min': 1e3 * min(ending[form]) / n,
                  'ms_per_frame_step_median': 1e3 * float(np.median(step[form])) / n}
   row['encode_kernels'] = {'us_per_frame_mean': us / n, 'calls_timed': calls}
+  if enc.by_kernel:
+    row['encode_kernels']['us_per_frame_by_kernel'] = {
+        k: sum(ev.time_range.elapsed_us() for ev in evs if k in ev.name) / calls / n for k in names}
   return row
 
 
-def measure(args):
+def measure(args, enc):
   import torch
   import torch.nn.functional as F
   from . import _lib
   from .utils.util import tile_grid
   if _lib.device_count() < 1:
-    raise SystemExit('bench_jpeg: no CUDA device visible; the engine has no CPU fallback')
+    raise SystemExit('bench_%s: no CUDA device visible; the engine has no CPU fallback' % enc.name)
   dev = torch.device('cuda', args.gpu)
   gen = torch.Generator(device=dev)
   gen.manual_seed(7)
@@ -172,22 +205,24 @@ def measure(args):
     grain = torch.randn((c, h, w), device=dev, generator=gen) * 4
     return (up + grain).clamp(0, 255).to(torch.uint8).permute(1, 2, 0).contiguous()
 
-  rows = [measure_workload(args, 'bgr_1080p', model, 'bgr',
+  rows = [measure_workload(enc, args, 'bgr_1080p', model, 'bgr',
                            [picture(FRAME_H, FRAME_W, 3) for _ in range(n)], grid, torch),
-          measure_workload(args, 'nv12_1080p', model, 'nv12',
+          measure_workload(enc, args, 'nv12_1080p', model, 'nv12',
                            [picture(FRAME_H * 3 // 2, FRAME_W, 1)[..., 0] for _ in range(n)],
                            grid, torch)]
   return {'workload': 'squeezeDet 1242x375, 1080p frames in device memory (smooth synthetic '
                       'pictures) as a tile_grid of 8 tiles (128 px overlap), detections drawn, '
-                      'then JPEG quality %d files on the host' % QUALITY,
+                      'then %s on the host' % enc.what,
           'gpu': gpu_info(args.gpu),
           'timer': 'host clock per step, split at a device synchronisation after the draw; '
                    'encode kernels: torch.profiler device durations of the calls, summed, per frame',
-          'rounds': args.rounds, 'steps': args.steps, 'forms': list(FORMS), 'rows': rows}
+          'rounds': args.rounds, 'steps': args.steps,
+          'forms': list(enc.forms), 'rows': rows}
 
 
 def main(argv=None):
-  print(json.dumps(measure(parse_args(argv))))
+  args = parse_args(argv)
+  print(json.dumps(measure(args, jpeg_encoder(args))))
 
 
 if __name__ == '__main__':

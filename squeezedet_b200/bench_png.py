@@ -12,7 +12,8 @@ Two frame formats: packed BGR and NV12.  Each step then ends one of two ways:
       (a PNG of these pictures is several MB, so the copy is a real part of the cost).
 The forms alternate within each round.  A step's time is split at a device synchronisation after
 the draw: `ending` is the encode and copy alone, `step` the whole step (a fresh copy of the frames,
-forward, draw, ending).  Every step's files of (b) are checked bitwise against (a)'s.
+forward, draw, ending).  Every step's files of (b) are checked bitwise against (a)'s.  The
+measurement is bench_jpeg's, with the PNG encoder.
 
 The encode kernels alone are timed in a separate pass under torch.profiler: the device durations of
 the encode_png_device calls' kernels and memsets, summed, per frame, also per kernel.
@@ -23,15 +24,9 @@ from __future__ import annotations
 
 import argparse
 import json
-import time
 
-import numpy as np
+from .bench_jpeg import Encoder, measure
 
-from .bench_device_frames import make_model
-from .bench_device_u8 import gpu_info
-
-FORMS = ('a_host_imencode', 'b_encode_png_device')
-FRAME_W, FRAME_H, OVERLAP = 1920, 1080, 128
 KERNELS = ('filter_kernel', 'mark_kernel', 'seg_scan_kernel', 'count_kernel', 'emit_kernel',
            'tree_kernel', 'frame_kernel', 'pack_kernel', 'idat_kernel')
 
@@ -46,130 +41,17 @@ def parse_args(argv=None):
   return ap.parse_args(argv)
 
 
-def measure_workload(args, name, model, fmt, clean, grid, torch):
-  import cv2
+def png_encoder():
   from .png import encode_png_device, png_bytes
-  mc = model.mc
-  n = len(clean)
-  tiles = [(f,) + g for f in range(n) for g in grid]
-  stream = torch.cuda.Stream(device=clean[0].device)
-  sptr = stream.cuda_stream
-  work = [torch.empty_like(c) for c in clean]
-
-  def drawn():
-    with torch.cuda.stream(stream):
-      for w, c in zip(work, clean):
-        w.copy_(c)
-    model.forward_device_tiles(work, fmt, tiles, stream=sptr)
-    model.draw_detections_device(work, fmt, which='tiles', stream=sptr)
-    stream.synchronize()
-
-  def end_a():
-    files = []
-    with torch.cuda.stream(stream):
-      for w in work:
-        im = w.cpu().numpy()
-        if fmt == 'nv12':
-          im = cv2.cvtColor(im, cv2.COLOR_YUV2BGR_NV12)
-        files.append(cv2.imencode('.png', im)[1].tobytes())
-    return files
-
-  def end_b():
-    with torch.cuda.stream(stream):
-      data, lengths = encode_png_device(work, fmt, stream=stream)
-      return png_bytes(data, lengths, stream=stream)
-
-  ends = {FORMS[0]: end_a, FORMS[1]: end_b}
-  drawn()
-  want = end_a()
-  assert end_b() == want, '%s: the files differ' % name
-  for form in FORMS:
-    for _ in range(args.warmup):
-      drawn()
-      ends[form]()
-  step = {form: [] for form in FORMS}
-  ending = {form: [] for form in FORMS}
-  for r in range(args.rounds):
-    for form in (FORMS if r % 2 == 0 else FORMS[::-1]):
-      for _ in range(args.steps):
-        t0 = time.perf_counter()
-        drawn()
-        t1 = time.perf_counter()
-        got = ends[form]()
-        t2 = time.perf_counter()
-        step[form].append(t2 - t0)
-        ending[form].append(t2 - t1)
-        assert got == want, '%s: the files of %s differ' % (name, form)
-
-  # the encode kernels alone, in a pass of their own under the profiler
-  from torch.autograd import DeviceType
-  from torch.profiler import ProfilerActivity, profile
-  drawn()
-  calls = 20
-  outs = []
-  with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    for _ in range(calls):
-      outs.append(encode_png_device(work, fmt, stream=stream))
-    stream.synchronize()
-  evs = [ev for ev in prof.events() if ev.device_type == DeviceType.CUDA and
-         any(k in ev.name for k in KERNELS + ('emset',))]
-  launches = calls * -(-n // 16) * (len(KERNELS) + 2)   # two scans and a memset per 16 frames
-  assert len(evs) >= launches * 9 // 10, 'found %d of %d encode launches' % (len(evs), launches)
-  us = sum(ev.time_range.elapsed_us() for ev in evs) / calls
-  per_kernel = {k: sum(ev.time_range.elapsed_us() for ev in evs if k in ev.name) / calls / n
-                for k in KERNELS + ('emset',)}
-
-  row = {'workload': name, 'engine': '%dx%d b=%d' % (mc.IMAGE_WIDTH, mc.IMAGE_HEIGHT,
-                                                     mc.BATCH_SIZE),
-         'frames': n, 'frame': '%dx%d %s' % (FRAME_W, FRAME_H, fmt),
-         'file_bytes_mean': float(np.mean([len(f) for f in want]))}
-  for form in FORMS:
-    row[form] = {'ms_per_frame_ending_median': 1e3 * float(np.median(ending[form])) / n,
-                 'ms_per_frame_ending_min': 1e3 * min(ending[form]) / n,
-                 'ms_per_frame_step_median': 1e3 * float(np.median(step[form])) / n}
-  row['encode_kernels'] = {'us_per_frame_mean': us / n, 'calls_timed': calls,
-                           'us_per_frame_by_kernel': per_kernel}
-  return row
-
-
-def measure(args):
-  import torch
-  import torch.nn.functional as F
-  from . import _lib
-  from .utils.util import tile_grid
-  if _lib.device_count() < 1:
-    raise SystemExit('bench_png: no CUDA device visible; the engine has no CPU fallback')
-  dev = torch.device('cuda', args.gpu)
-  gen = torch.Generator(device=dev)
-  gen.manual_seed(7)
-  grid = tile_grid(FRAME_W, FRAME_H, 1242, 375, OVERLAP)
-  assert len(grid) == 8, grid
-  n = args.frames
-  model = make_model(1242, 375, n * len(grid), args.gpu)
-
-  def picture(h, w, c):
-    """A smooth uint8 [h, w, c] picture: bilinear upsampled noise plus grain."""
-    low = torch.rand((1, c, h // 24, w // 24), device=dev, generator=gen) * 255
-    up = F.interpolate(low, size=(h, w), mode='bilinear', align_corners=False)[0]
-    grain = torch.randn((c, h, w), device=dev, generator=gen) * 4
-    return (up + grain).clamp(0, 255).to(torch.uint8).permute(1, 2, 0).contiguous()
-
-  rows = [measure_workload(args, 'bgr_1080p', model, 'bgr',
-                           [picture(FRAME_H, FRAME_W, 3) for _ in range(n)], grid, torch),
-          measure_workload(args, 'nv12_1080p', model, 'nv12',
-                           [picture(FRAME_H * 3 // 2, FRAME_W, 1)[..., 0] for _ in range(n)],
-                           grid, torch)]
-  return {'workload': 'squeezeDet 1242x375, 1080p frames in device memory (smooth synthetic '
-                      'pictures) as a tile_grid of 8 tiles (128 px overlap), detections drawn, '
-                      'then PNG files (cv2 defaults) on the host',
-          'gpu': gpu_info(args.gpu),
-          'timer': 'host clock per step, split at a device synchronisation after the draw; '
-                   'encode kernels: torch.profiler device durations of the calls, summed, per frame',
-          'rounds': args.rounds, 'steps': args.steps, 'forms': list(FORMS), 'rows': rows}
+  # two scans and a memset per 16 frames
+  return Encoder('png', '.png', [],
+                 lambda frames, fmt, stream: encode_png_device(frames, fmt, stream=stream),
+                 png_bytes, KERNELS, len(KERNELS) + 2, 'PNG files (cv2 defaults)', {},
+                 by_kernel=True)
 
 
 def main(argv=None):
-  print(json.dumps(measure(parse_args(argv))))
+  print(json.dumps(measure(parse_args(argv), png_encoder())))
 
 
 if __name__ == '__main__':

@@ -26,6 +26,28 @@ int  cuda_fail(cudaError_t err, const char* what);
     if (_e != cudaSuccess) return ::sqdet::cuda_fail(_e, what);         \
   } while (0)
 
+// ---- scratch layouts --------------------------------------------------------------------------
+inline int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
+
+// Regions of a scratch at 256-byte offsets from base, in the order they are taken.  A call's layout
+// is written once, taking from a Carver: with a null base it only counts the scratch size.
+struct Carver {
+  uint8_t* base = nullptr;
+  int64_t offset = 0;
+  // The offset of the next `bytes` bytes.
+  int64_t next(int64_t bytes) {
+    const int64_t at = offset;
+    offset += align256(bytes);
+    return at;
+  }
+  // The next `count` T (null when only counting).
+  template <class T>
+  T* take(int64_t count) {
+    const int64_t at = next(count * (int64_t)sizeof(T));
+    return base ? reinterpret_cast<T*>(base + at) : nullptr;
+  }
+};
+
 // ---- TF NHWC geometry (SURVEY App. A.1; tf.nn.conv2d / tf.nn.max_pool) ------------------
 struct Geom {
   int out, pad_before, pad_after;
@@ -124,13 +146,20 @@ bool device_range_ok(const void* p, int64_t bytes, int device);
 // The crop r = (x, y, w, h) of an H x W frame, or the whole frame when r is null, into s.x, s.y,
 // s.w and s.h; refuses an empty crop or one outside the frame, naming `which`.
 int check_crop(const std::string& which, int64_t H, int64_t W, const int32_t* r, FrameSource& s);
+// A frame encoder as its refusals name it: its call, its file format, the call that sizes its
+// scratch, and the most frames per call and pixels per crop side it takes.
+struct Encoder {
+  const char* call;
+  const char* file;
+  const char* scratch_call;
+  int max_frames, max_side;
+};
 // The crops of an encoder's n frames (heights[i] x widths[i], crops as check_crop takes them) into
-// fr, or a refusal naming the call: n outside [1, max_frames], an empty frame, a crop that
-// check_crop refuses, or one wider or higher than max_side, which the file `format` (its name, as
-// the message gives it) cannot hold.  Host arrays only: the encoders' size functions call it too.
-int encode_crops(const std::string& name, const char* format, int max_frames, int max_side, int n,
-                 const int32_t* heights, const int32_t* widths, const int32_t* crops,
-                 std::vector<FrameSource>& fr);
+// fr, or a refusal naming the call: n outside [1, enc.max_frames], an empty frame, a crop that
+// check_crop refuses, or one wider or higher than enc.max_side, which the file cannot hold.  Host
+// arrays only: the encoders' size functions call it too.
+int encode_crops(const std::string& name, const Encoder& enc, int n, const int32_t* heights,
+                 const int32_t* widths, const int32_t* crops, std::vector<FrameSource>& fr);
 // accept_frames' device: the one plane 0 of frame 0 is on.
 constexpr int kFrame0Device = -1;
 // Every check of n frames in format pf before any device work, filling fr or refusing with a

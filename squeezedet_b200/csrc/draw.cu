@@ -15,7 +15,7 @@
 #include <math.h>
 #include <stdint.h>
 #include <string.h>
-#include "common.cuh"
+#include "frames.cuh"
 
 #define SQDET_HERSHEY_SPACE __constant__
 #include "hershey_simplex.inc"
@@ -323,17 +323,9 @@ int launch_format(const FrameSource* frames, int n, const sqdet_det* dets, const
 int launch_draw_dets(int format, const FrameSource* frames, int n, const sqdet_det* dets,
                      const int32_t* counts, int max_dets, const DrawStyle& style,
                      cudaStream_t stream) {
-  switch (format) {
-    case SQDET_FMT_BGR: return launch_format<SQDET_FMT_BGR>(frames, n, dets, counts, max_dets, style, stream);
-    case SQDET_FMT_RGB: return launch_format<SQDET_FMT_RGB>(frames, n, dets, counts, max_dets, style, stream);
-    case SQDET_FMT_BGRA: return launch_format<SQDET_FMT_BGRA>(frames, n, dets, counts, max_dets, style, stream);
-    case SQDET_FMT_RGBA: return launch_format<SQDET_FMT_RGBA>(frames, n, dets, counts, max_dets, style, stream);
-    case SQDET_FMT_RGB_PLANAR:
-      return launch_format<SQDET_FMT_RGB_PLANAR>(frames, n, dets, counts, max_dets, style, stream);
-    case SQDET_FMT_NV12: return launch_format<SQDET_FMT_NV12>(frames, n, dets, counts, max_dets, style, stream);
-    case SQDET_FMT_I420: return launch_format<SQDET_FMT_I420>(frames, n, dets, counts, max_dets, style, stream);
-    default: return fail(SQDET_ERR_INVALID_ARG, "sqdet_draw_dets: unknown format");
-  }
+  return dispatch_format(format, [&](auto f) {
+    return launch_format<decltype(f)::value>(frames, n, dets, counts, max_dets, style, stream);
+  });
 }
 
 }  // namespace

@@ -11,8 +11,6 @@
 // work (accept_frames, device_range_ok), which every entry point taking device frames shares.
 #include <cuda.h>
 
-#include <algorithm>
-
 #include "frames.cuh"
 
 namespace sqdet {
@@ -163,24 +161,10 @@ int launch_resize_meansub_frames(int format, const FrameSource* frames, int n, f
       return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_frames: non-positive crop size");
   const long long blocks = ((long long)H * W + 255) / 256;
   if (blocks > 0x7fffffffLL) return fail(SQDET_ERR_INVALID_ARG, "resize_meansub_frames: image too large");
-  const auto b = (unsigned)blocks;
-  switch (format) {
-    case SQDET_FMT_BGR:
-      return launch_format<SQDET_FMT_BGR>(*pf, frames, n, dst, H, W, b, means, sub_first, scales_xy, stream);
-    case SQDET_FMT_RGB:
-      return launch_format<SQDET_FMT_RGB>(*pf, frames, n, dst, H, W, b, means, sub_first, scales_xy, stream);
-    case SQDET_FMT_BGRA:
-      return launch_format<SQDET_FMT_BGRA>(*pf, frames, n, dst, H, W, b, means, sub_first, scales_xy, stream);
-    case SQDET_FMT_RGBA:
-      return launch_format<SQDET_FMT_RGBA>(*pf, frames, n, dst, H, W, b, means, sub_first, scales_xy, stream);
-    case SQDET_FMT_RGB_PLANAR:
-      return launch_format<SQDET_FMT_RGB_PLANAR>(*pf, frames, n, dst, H, W, b, means, sub_first,
-                                                 scales_xy, stream);
-    case SQDET_FMT_NV12:
-      return launch_format<SQDET_FMT_NV12>(*pf, frames, n, dst, H, W, b, means, sub_first, scales_xy, stream);
-    default:
-      return launch_format<SQDET_FMT_I420>(*pf, frames, n, dst, H, W, b, means, sub_first, scales_xy, stream);
-  }
+  return dispatch_format(format, [&](auto f) {
+    return launch_format<decltype(f)::value>(*pf, frames, n, dst, H, W, (unsigned)blocks, means,
+                                             sub_first, scales_xy, stream);
+  });
 }
 
 // ---- frames and buffers from the caller ----------------------------------------------------------
@@ -227,21 +211,20 @@ int check_crop(const std::string& which, int64_t H, int64_t W, const int32_t* r,
   return SQDET_OK;
 }
 
-int encode_crops(const std::string& name, const char* format, int max_frames, int max_side, int n,
-                 const int32_t* heights, const int32_t* widths, const int32_t* crops,
-                 std::vector<FrameSource>& fr) {
+int encode_crops(const std::string& name, const Encoder& enc, int n, const int32_t* heights,
+                 const int32_t* widths, const int32_t* crops, std::vector<FrameSource>& fr) {
   if (!heights || !widths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  if (n < 1 || n > max_frames)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(max_frames) + "]");
+  if (n < 1 || n > enc.max_frames)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(enc.max_frames) + "]");
   fr.assign((size_t)n, FrameSource{});
   for (int i = 0; i < n; ++i) {
     const std::string which = name + ": frame " + std::to_string(i);
     if (heights[i] <= 0 || widths[i] <= 0) return fail(SQDET_ERR_INVALID_ARG, which + " is empty");
     const int rc = check_crop(which, heights[i], widths[i], crops ? crops + 4 * i : nullptr, fr[(size_t)i]);
     if (rc) return rc;
-    if (fr[(size_t)i].w > max_side || fr[(size_t)i].h > max_side)
-      return fail(SQDET_ERR_INVALID_ARG, which + ": a " + format + " is at most " +
-                                             std::to_string(max_side) + " pixels wide and high");
+    if (fr[(size_t)i].w > enc.max_side || fr[(size_t)i].h > enc.max_side)
+      return fail(SQDET_ERR_INVALID_ARG, which + ": a " + enc.file + " is at most " +
+                                             std::to_string(enc.max_side) + " pixels wide and high");
   }
   return SQDET_OK;
 }

@@ -2,11 +2,31 @@
 // read frames without writing a BGR copy (frames.cu: resize + mean subtraction into tensor 0;
 // jpeg.cu, png.cu: JPEG and PNG encoding).  A FrameDesc<P> holds a crop's P planes at its origin,
 // taps<F> turns it into the format's fetch, and each fetch converts to B, G, R as the format's
-// cv2.cvtColor code does.
+// cv2.cvtColor code does.  dispatch_format picks the instance of a format code for every launcher
+// of these kernels and draw.cu's, and encode_frames is the front end both encoders share.
 #pragma once
+#include <algorithm>
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace sqdet {
+
+// fn(std::integral_constant<int, F>{}) for the SQDET_FMT_* code F == format, whose result it
+// returns; a value outside SQDET_FMT_* is refused.
+template <class Fn>
+int dispatch_format(int format, Fn&& fn) {
+  switch (format) {
+    case SQDET_FMT_BGR: return fn(std::integral_constant<int, SQDET_FMT_BGR>{});
+    case SQDET_FMT_RGB: return fn(std::integral_constant<int, SQDET_FMT_RGB>{});
+    case SQDET_FMT_BGRA: return fn(std::integral_constant<int, SQDET_FMT_BGRA>{});
+    case SQDET_FMT_RGBA: return fn(std::integral_constant<int, SQDET_FMT_RGBA>{});
+    case SQDET_FMT_RGB_PLANAR: return fn(std::integral_constant<int, SQDET_FMT_RGB_PLANAR>{});
+    case SQDET_FMT_NV12: return fn(std::integral_constant<int, SQDET_FMT_NV12>{});
+    case SQDET_FMT_I420: return fn(std::integral_constant<int, SQDET_FMT_I420>{});
+    default: return fail(SQDET_ERR_INVALID_ARG, "unknown pixel format " + std::to_string(format));
+  }
+}
 
 // The taps of a packed uint8 frame of kBpp bytes per pixel whose row r starts at src + r * pitch
 // (any byte alignment), with B, G, R at byte offsets kB, kG, kR of a pixel (other bytes, such as
@@ -147,6 +167,62 @@ FrameDesc<P> frame_desc(const PixFormat& pf, const FrameSource& s, int H, int W)
   f.x_odd = s.x & 1;
   f.y_odd = s.y & 1;
   return f;
+}
+
+// ---- the front end of the frame encoders (jpeg.cu, png.cu) ---------------------------------------
+// Frames per launch of either encoder, whose descriptors travel in the parameter block.
+constexpr int kEncodeFramesPerLaunch = 16;
+
+// fn(first, count) for each group [first, first + count) of up to kEncodeFramesPerLaunch of n
+// frames, in order; returns the first nonzero result.
+template <class Fn>
+int for_each_group(int n, Fn&& fn) {
+  for (int first = 0; first < n; first += kEncodeFramesPerLaunch) {
+    const int rc = fn(first, std::min(kEncodeFramesPerLaunch, n - first));
+    if (rc) return rc;
+  }
+  return SQDET_OK;
+}
+
+// One call of an encoder: every check before any device work, in this order (format, null
+// arguments, encode_crops, the codec's settings, cap, scratch and lengths alignment, scratch_bytes,
+// accept_frames, the outputs' ranges), then launch(pf, frames) on frame 0's device.  settle(fr,
+// need) checks the codec's settings and sets the scratch the crops fr need, or returns a refusal.
+template <class Settle, class Launch>
+int encode_frames(const Encoder& enc, int n, int format, const uint8_t* const* planes,
+                  const int64_t* pitches, const int32_t* heights, const int32_t* widths,
+                  const int32_t* crops, uint8_t* out_dev, int64_t cap, int64_t* lengths_dev,
+                  void* scratch_dev, int64_t scratch_bytes, Settle&& settle, Launch&& launch) {
+  const std::string name = enc.call;
+  const PixFormat* pf = pix_format(format);
+  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
+  if (!planes || !heights || !widths || !out_dev || !lengths_dev || !scratch_dev)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  std::vector<FrameSource> fr;
+  int rc = encode_crops(name, enc, n, heights, widths, crops, fr);
+  if (rc) return rc;
+  int64_t need = 0;
+  rc = settle(fr, need);
+  if (rc) return rc;
+  if (cap < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": cap must be at least 1");
+  // the scratches hold int4, int64, 16-bit and 32-bit atomic regions at 256-byte offsets
+  if ((uintptr_t)scratch_dev % 256)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
+  if ((uintptr_t)lengths_dev % alignof(int64_t))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": lengths_dev must be 8-byte aligned");
+  if (scratch_bytes < need)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below " + enc.scratch_call);
+  int device = kFrame0Device;
+  rc = accept_frames(name, *pf, n, planes, pitches, heights, widths, crops, nullptr, &device, fr);
+  if (rc) return rc;
+  const bool out_fits = cap <= INT64_MAX / n && device_range_ok(out_dev, (int64_t)n * cap, device);
+  if (!out_fits || !device_range_ok(lengths_dev, (int64_t)n * 8, device) ||
+      !device_range_ok(scratch_dev, scratch_bytes, device))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": out_dev, lengths_dev or scratch_dev is not inside one "
+                                              "device allocation on frame 0's device");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
+  return launch(*pf, fr.data());
 }
 
 }  // namespace sqdet

@@ -35,8 +35,7 @@
 //                   RSTn before each interval's first byte, and the frame's first chunk writes
 //                   the header (a host template with the frame's height, width and Huffman
 //                   tables filled in), EOI and the length, or -1 when the file does not fit
-// Frames run kJpegFramesPerLaunch at a time through these launches, reusing one scratch.
-#include <algorithm>
+// Frames run kEncodeFramesPerLaunch at a time through these launches, reusing one scratch.
 #include <cstring>
 
 #include "frames.cuh"
@@ -165,14 +164,14 @@ struct JpegGeom {
   uint8_t* out;
   int64_t* length;
 };
-constexpr int kJpegFramesPerLaunch = 16;
-constexpr int kMaxJpegFrames = 128;     // frames per sqdet_encode_jpeg call
-// libjpeg-turbo's JPEG_MAX_DIMENSION: cv2.imencode refuses a longer side, and libjpeg does not
-// read a file whose SOF0 says one (its 16-bit fields would hold up to 65535)
+// 128 frames per sqdet_encode_jpeg call; sides up to libjpeg-turbo's JPEG_MAX_DIMENSION:
+// cv2.imencode refuses a longer side, and libjpeg does not read a file whose SOF0 says one (its
+// 16-bit fields would hold up to 65535)
 constexpr int kJpegMaxSide = 65500;
+constexpr Encoder kJpeg = {"sqdet_encode_jpeg", "JPEG", "sqdet_jpeg_scratch_bytes", 128, kJpegMaxSide};
 
 struct JpegParams {
-  JpegGeom g[kJpegFramesPerLaunch];
+  JpegGeom g[kEncodeFramesPerLaunch];
   int16_t* coef;                        // [blocks][64], natural order
   uint32_t* bits;                       // [blocks]
   int64_t* sums;                        // chunk sums of blocks, of stuffing chunks and of intervals
@@ -195,7 +194,7 @@ struct QuantRecip {
 template <int F>
 struct TransformParams {
   JpegParams p;
-  FrameDesc<kPlanes<F>> f[kJpegFramesPerLaunch];
+  FrameDesc<kPlanes<F>> f[kEncodeFramesPerLaunch];
   QuantRecip quant;
 };
 static_assert(sizeof(TransformParams<SQDET_FMT_I420>) <= 4096, "transform parameters exceed 4 KiB");
@@ -857,8 +856,6 @@ FrameSizes frame_sizes(int h, int w, const Settings& st) {
   return s;
 }
 
-int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
-
 // The scratch of the frames [first, first + count): coefficients, bit lengths, chunk sums,
 // intervals' first bits, bit buffers, symbol counts and tables, in that order.
 struct GroupLayout {
@@ -992,16 +989,17 @@ int64_t jpeg_max_bytes(int h, int w, const Settings& st) {
 // The scratch the encode of the crops of `frames` needs.
 int64_t jpeg_scratch_bytes(const FrameSource* frames, int n, const Settings& st) {
   int64_t most = 0;
-  for (int first = 0; first < n; first += kJpegFramesPerLaunch)
-    most = std::max(most, group_layout(frames, first, std::min(kJpegFramesPerLaunch, n - first), st, nullptr).total);
+  for_each_group(n, [&](int first, int count) {
+    most = std::max(most, group_layout(frames, first, count, st, nullptr).total);
+    return SQDET_OK;
+  });
   return most;
 }
 
-// The encode of the crops of `frames` (the frames' checks are the caller's).
-int launch_encode_jpeg(int format, const FrameSource* frames, int n, const Settings& st, uint8_t* out,
-                       int64_t cap, int64_t* lengths, void* scratch, cudaStream_t stream) {
-  const PixFormat* pf = pix_format(format);
-  if (!pf) return fail(SQDET_ERR_INVALID_ARG, "sqdet_encode_jpeg: unknown format");
+// The encode of the crops of `frames` in `format` (the frames' checks are the caller's).
+int launch_encode_jpeg(int format, const PixFormat& pf, const FrameSource* frames, int n,
+                       const Settings& st, uint8_t* out, int64_t cap, int64_t* lengths,
+                       void* scratch, cudaStream_t stream) {
   // jpeg_quality_scaling of each table's quality, then the standard tables scaled, rounded and
   // clamped to 1..255
   const int scale[2] = {st.lq < 50 ? 5000 / st.lq : 200 - 2 * st.lq, st.cq < 50 ? 5000 / st.cq : 200 - 2 * st.cq};
@@ -1035,24 +1033,12 @@ int launch_encode_jpeg(int format, const FrameSource* frames, int n, const Setti
   sp.std = std_spec();
   sp.suffix_bytes = jpeg_header(q, st, sp.prefix, sp.suffix);
   uint8_t* s = static_cast<uint8_t*>(scratch);
-  for (int first = 0; first < n; first += kJpegFramesPerLaunch) {
-    const int count = std::min(kJpegFramesPerLaunch, n - first);
-    int rc;
-    switch (format) {
-#define SQ_JPEG_CASE(F) \
-  case F: rc = launch_group<F>(*pf, frames, first, count, st, quant, sp, out, cap, lengths, s, stream); break;
-      SQ_JPEG_CASE(SQDET_FMT_BGR)
-      SQ_JPEG_CASE(SQDET_FMT_RGB)
-      SQ_JPEG_CASE(SQDET_FMT_BGRA)
-      SQ_JPEG_CASE(SQDET_FMT_RGBA)
-      SQ_JPEG_CASE(SQDET_FMT_RGB_PLANAR)
-      SQ_JPEG_CASE(SQDET_FMT_NV12)
-      default: rc = launch_group<SQDET_FMT_I420>(*pf, frames, first, count, st, quant, sp, out, cap, lengths, s, stream);
-#undef SQ_JPEG_CASE
-    }
-    if (rc) return rc;
-  }
-  return SQDET_OK;
+  return for_each_group(n, [&](int first, int count) {
+    return dispatch_format(format, [&](auto f) {
+      return launch_group<decltype(f)::value>(pf, frames, first, count, st, quant, sp, out, cap,
+                                              lengths, s, stream);
+    });
+  });
 }
 
 // sqdet_jpeg_params of cv2's defaults with `quality`.
@@ -1084,9 +1070,8 @@ int64_t sqdet_jpeg_scratch_bytes_params(int n, const int32_t* heights, const int
                                         const int32_t* crops, const sqdet_jpeg_params* params) {
   std::vector<FrameSource> fr;
   Settings st;
-  if (resolve_params("sqdet_jpeg_scratch_bytes", params, &st)) return -1;
-  if (encode_crops("sqdet_jpeg_scratch_bytes", "JPEG", kMaxJpegFrames, kJpegMaxSide, n, heights, widths, crops, fr))
-    return -1;
+  if (resolve_params(kJpeg.scratch_call, params, &st)) return -1;
+  if (encode_crops(kJpeg.scratch_call, kJpeg, n, heights, widths, crops, fr)) return -1;
   return jpeg_scratch_bytes(fr.data(), n, st);
 }
 
@@ -1100,37 +1085,18 @@ int sqdet_encode_jpeg_params(int n, int format, const uint8_t* const* planes, co
                              const int32_t* heights, const int32_t* widths, const int32_t* crops,
                              const sqdet_jpeg_params* params, uint8_t* out_dev, int64_t cap,
                              int64_t* lengths_dev, void* scratch_dev, int64_t scratch_bytes, void* stream) {
-  const std::string name = "sqdet_encode_jpeg";
-  const PixFormat* pf = pix_format(format);
-  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
-  if (!planes || !heights || !widths || !out_dev || !lengths_dev || !scratch_dev)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  std::vector<FrameSource> fr;
-  int rc = encode_crops(name, "JPEG", kMaxJpegFrames, kJpegMaxSide, n, heights, widths, crops, fr);
-  if (rc) return rc;
   Settings st;
-  rc = resolve_params(name, params, &st);
-  if (rc) return rc;
-  if (cap < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": cap must be at least 1");
-  // the scratch holds int4, int64 and 32-bit atomic regions at 256-byte offsets from its start
-  if ((uintptr_t)scratch_dev % 256)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
-  if ((uintptr_t)lengths_dev % alignof(int64_t))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": lengths_dev must be 8-byte aligned");
-  if (scratch_bytes < jpeg_scratch_bytes(fr.data(), n, st))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below sqdet_jpeg_scratch_bytes");
-  int device = kFrame0Device;
-  rc = accept_frames(name, *pf, n, planes, pitches, heights, widths, crops, nullptr, &device, fr);
-  if (rc) return rc;
-  const bool out_fits = cap <= INT64_MAX / n && device_range_ok(out_dev, (int64_t)n * cap, device);
-  if (!out_fits || !device_range_ok(lengths_dev, (int64_t)n * 8, device) ||
-      !device_range_ok(scratch_dev, scratch_bytes, device))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": out_dev, lengths_dev or scratch_dev is not inside one "
-                                              "device allocation on frame 0's device");
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
-  return launch_encode_jpeg(format, fr.data(), n, st, out_dev, cap, lengths_dev, scratch_dev,
-                            (cudaStream_t)stream);
+  auto settle = [&](const std::vector<FrameSource>& fr, int64_t& need) {
+    const int rc = resolve_params(kJpeg.call, params, &st);
+    if (!rc) need = jpeg_scratch_bytes(fr.data(), n, st);
+    return rc;
+  };
+  auto launch = [&](const PixFormat& pf, const FrameSource* fr) {
+    return launch_encode_jpeg(format, pf, fr, n, st, out_dev, cap, lengths_dev, scratch_dev,
+                              (cudaStream_t)stream);
+  };
+  return encode_frames(kJpeg, n, format, planes, pitches, heights, widths, crops, out_dev, cap,
+                       lengths_dev, scratch_dev, scratch_bytes, settle, launch);
 }
 
 int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int64_t* pitches,

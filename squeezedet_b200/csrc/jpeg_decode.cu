@@ -926,15 +926,11 @@ void build_tab(const uint8_t* bits, const uint8_t* vals, HuffTab& t) {
   memcpy(t.vals, vals, 256);
 }
 
-int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
-
 // One file's layout: sizes that follow from its headers alone.
 struct Layout {
   int mcu_cols, mcu_rows, mcus, bpm, restart, intervals, chunks, blocks, sub_max;
   int pw[3], ph[3];
   int64_t raw_len;
-  int64_t staging;                       // this file's tables and raw bytes
-  int64_t marks, coef, rest;             // its scratch: set to 0xFF, zeroed, and the rest
 };
 
 Layout layout(const Parsed& P, int64_t file_len, int sub_bits) {
@@ -964,28 +960,55 @@ Layout layout(const Parsed& P, int64_t file_len, int sub_bits) {
   L.raw_len = file_len - I.scan_offset;
   L.chunks = (int)std::max<int64_t>(1, (L.raw_len + kChunk - 1) / kChunk);
   L.sub_max = (int)((L.raw_len * 8 + sub_bits - 1) / sub_bits) + L.intervals;
-  L.staging = align256((int64_t)sizeof(HuffTab) * 6) + align256(L.raw_len + 16);
-  L.marks = 256 + align256((int64_t)(L.intervals + 1) * 4);          // terminator, ist
-  L.coef = align256((int64_t)L.blocks * 128);
-  int64_t s = 0;
-  s += align256((int64_t)(L.chunks + 1) * 8);                     // chunk sums
-  s += align256(L.raw_len + 16);                                  // clean stream, padded
-  s += align256((int64_t)(L.intervals + 1) * 4);                  // sbase
-  s += align256((int64_t)L.sub_max * 8) * 2;                      // entry, exit
-  s += align256((int64_t)L.sub_max * 16);                         // counts
-  for (int c = 0; c < I.components; ++c) s += align256((int64_t)L.pw[c] * L.ph[c]);
-  L.rest = s;
   return L;
 }
-
 
 // The whole call: parsed files, their layouts and where everything goes.
 struct Plan {
   std::vector<Parsed> parsed;
   std::vector<Layout> lay;
+  std::vector<DecFile> files;           // each file's regions, placed
   int64_t staging = 0, scratch = 0;
   int64_t marks = 0, marks_bytes = 0, coef = 0, coef_bytes = 0;
 };
+
+// Places every region of the call.  The staging holds the file descriptors, then each file's
+// Huffman tables and raw bytes (+16 zero bytes of padding); it is copied to the scratch's start.
+// After it in the scratch come every file's marks (a terminator, then ist), every file's
+// coefficients, and then each file's chunk sums, clean stream (padded), sbase, entry, exit, counts
+// and planes.
+void place(Plan& plan) {
+  const size_t n = plan.lay.size();
+  std::vector<DecFile>& fd = plan.files;
+  fd.assign(n, DecFile{});
+  Carver c;
+  c.next((int64_t)sizeof(DecFile) * (int64_t)n);
+  for (size_t i = 0; i < n; ++i) {
+    fd[i].tabs = c.next((int64_t)sizeof(HuffTab) * 6);
+    fd[i].raw = c.next(plan.lay[i].raw_len + 16);
+  }
+  plan.staging = plan.marks = c.offset;
+  for (size_t i = 0; i < n; ++i) {
+    fd[i].term = c.next(256);
+    fd[i].ist = c.next((int64_t)(plan.lay[i].intervals + 1) * 4);
+  }
+  plan.coef = c.offset;
+  plan.marks_bytes = plan.coef - plan.marks;
+  for (size_t i = 0; i < n; ++i) fd[i].coef = c.next((int64_t)plan.lay[i].blocks * 128);
+  plan.coef_bytes = c.offset - plan.coef;
+  for (size_t i = 0; i < n; ++i) {
+    const Layout& L = plan.lay[i];
+    fd[i].sums = c.next((int64_t)(L.chunks + 1) * 8);
+    fd[i].clean = c.next(L.raw_len + 16);
+    fd[i].sbase = c.next((int64_t)(L.intervals + 1) * 4);
+    fd[i].entry = c.next((int64_t)L.sub_max * 8);
+    fd[i].exit_ = c.next((int64_t)L.sub_max * 8);
+    fd[i].counts = c.next((int64_t)L.sub_max * 16);
+    for (int k = 0; k < plan.parsed[i].info.components; ++k)
+      fd[i].plane[k] = c.next((int64_t)L.pw[k] * L.ph[k]);
+  }
+  plan.scratch = c.offset;
+}
 
 // Parses every file; a refusal names the first file refused.
 int make_plan(const std::string& name, int n, const uint8_t* const* files, const int64_t* lengths,
@@ -1005,15 +1028,7 @@ int make_plan(const std::string& name, int n, const uint8_t* const* files, const
                                              kReasons[reason]);
     plan.lay[(size_t)i] = layout(plan.parsed[(size_t)i], lengths[i], g_sub_bits);
   }
-  int64_t st = align256((int64_t)sizeof(DecFile) * n);
-  for (const Layout& L : plan.lay) st += L.staging;
-  plan.staging = st;
-  plan.marks = st;
-  for (const Layout& L : plan.lay) plan.marks_bytes += L.marks;
-  plan.coef = plan.marks + plan.marks_bytes;
-  for (const Layout& L : plan.lay) plan.coef_bytes += L.coef;
-  plan.scratch = plan.coef + plan.coef_bytes;
-  for (const Layout& L : plan.lay) plan.scratch += L.rest;
+  place(plan);
   return SQDET_OK;
 }
 
@@ -1021,14 +1036,11 @@ int make_plan(const std::string& name, int n, const uint8_t* const* files, const
 void fill_staging(const Plan& plan, int n, const uint8_t* const* files, uint8_t* const* out,
                   const int64_t* pitch, uint8_t* stage) {
   DecFile* fd = reinterpret_cast<DecFile*>(stage);
-  int64_t so = align256((int64_t)sizeof(DecFile) * n);   // staging cursor
-  int64_t mo = plan.marks, co = plan.coef, ro = plan.coef + plan.coef_bytes;
   for (int i = 0; i < n; ++i) {
     const Parsed& P = plan.parsed[(size_t)i];
     const Layout& L = plan.lay[(size_t)i];
     const sqdet_jpeg_info& I = P.info;
-    DecFile f;
-    memset(&f, 0, sizeof(f));
+    DecFile f = plan.files[(size_t)i];
     f.h = I.coded_height;
     f.w = I.coded_width;
     f.oh = I.height;
@@ -1064,39 +1076,13 @@ void fill_staging(const Plan& plan, int n, const uint8_t* const* files, uint8_t*
       f.chh[c] = (int)(((int64_t)f.h * vc + vmax - 1) / vmax);
       for (int k = 0; k < 64; ++k) f.q[c][k] = (int16_t)P.qt[cp.tq][k];
     }
-    // staging: tables, raw bytes (+16 zero bytes of padding)
-    f.tabs = so;
-    HuffTab* tabs = reinterpret_cast<HuffTab*>(stage + so);
+    HuffTab* tabs = reinterpret_cast<HuffTab*>(stage + f.tabs);
     for (int c = 0; c < I.components; ++c) {
       build_tab(P.dc_bits[P.comp[c].td], P.dc_vals[P.comp[c].td], tabs[2 * c]);
       build_tab(P.ac_bits[P.comp[c].ta], P.ac_vals[P.comp[c].ta], tabs[2 * c + 1]);
     }
-    f.raw = so + align256((int64_t)sizeof(HuffTab) * 6);
     memcpy(stage + f.raw, files[i] + I.scan_offset, (size_t)L.raw_len);
     memset(stage + f.raw + L.raw_len, 0, 16);
-    so += L.staging;
-    // scratch
-    f.term = mo;
-    f.ist = mo + 256;
-    mo += L.marks;
-    f.coef = co;
-    co += L.coef;
-    f.sums = ro;
-    ro += align256((int64_t)(L.chunks + 1) * 8);
-    f.clean = ro;
-    ro += align256(L.raw_len + 16);
-    f.sbase = ro;
-    ro += align256((int64_t)(L.intervals + 1) * 4);
-    f.entry = ro;
-    ro += align256((int64_t)L.sub_max * 8);
-    f.exit_ = ro;
-    ro += align256((int64_t)L.sub_max * 8);
-    f.counts = ro;
-    ro += align256((int64_t)L.sub_max * 16);
-    for (int c = 0; c < I.components; ++c) {
-      f.plane[c] = ro;
-      ro += align256((int64_t)L.pw[c] * L.ph[c]);
-    }
     f.out = out[i];
     f.pitch = pitch[i];
     fd[i] = f;

@@ -48,24 +48,21 @@ struct Scratch {
   double* sim;          // [kCd][kMaxThresholds][n] per-image similarity
 };
 
-inline int64_t align256(int64_t b) { return (b + 255) & ~int64_t(255); }
-
-Scratch carve(void* base, int n, int max_dets) {
-  char* p = static_cast<char*>(base);
+Scratch carve(Carver& c, int n, int max_dets) {
   const int64_t recs = (int64_t)n * max_dets;
   Scratch s;
-  s.box = reinterpret_cast<double*>(p);  p += align256(recs * 32);
-  s.meta = reinterpret_cast<int32_t*>(p); p += align256(recs * 4);
-  s.hist = reinterpret_cast<int32_t*>(p); p += align256(kCd * kBins * 4);
-  s.thr = reinterpret_cast<int32_t*>(p);  p += align256(kCd * kMaxThresholds * 4);
-  s.sim = reinterpret_cast<double*>(p);
+  s.box = c.take<double>(recs * 4);
+  s.meta = c.take<int32_t>(recs);
+  s.hist = c.take<int32_t>(kCd * kBins);
+  s.thr = c.take<int32_t>(kCd * kMaxThresholds);
+  s.sim = c.take<double>((int64_t)kCd * kMaxThresholds * n);
   return s;
 }
 
 int64_t scratch_bytes(int n, int max_dets) {
-  const int64_t recs = (int64_t)n * max_dets;
-  return align256(recs * 32) + align256(recs * 4) + align256(kCd * kBins * 4) +
-         align256(kCd * kMaxThresholds * 4) + align256((int64_t)kCd * kMaxThresholds * n * 8);
+  Carver c;
+  carve(c, n, max_dets);
+  return c.offset;
 }
 
 __device__ __forceinline__ void refuse(sqdet_kitti_result* out, int image, int reason) {
@@ -398,22 +395,21 @@ struct AnalyzeScratch {
   int64_t* lines;       // [n] error lines, then the image's first line
 };
 
-AnalyzeScratch carve_analyze(void* base, int n, int max_dets, int64_t n_objects) {
-  char* p = static_cast<char*>(base);
+AnalyzeScratch carve_analyze(Carver& c, int n, int max_dets, int64_t n_objects) {
   const int64_t recs = (int64_t)n * max_dets;
   AnalyzeScratch s;
-  s.box = reinterpret_cast<double*>(p);     p += align256(recs * 32);
-  s.slot = reinterpret_cast<int32_t*>(p);   p += align256(recs * 4);
-  s.claim = reinterpret_cast<uint32_t*>(p); p += align256(n_objects * 4);
-  s.kept = reinterpret_cast<int32_t*>(p);   p += align256((int64_t)n * 4);
-  s.lines = reinterpret_cast<int64_t*>(p);
+  s.box = c.take<double>(recs * 4);
+  s.slot = c.take<int32_t>(recs);
+  s.claim = c.take<uint32_t>(n_objects);
+  s.kept = c.take<int32_t>(n);
+  s.lines = c.take<int64_t>(n);
   return s;
 }
 
 int64_t analyze_scratch_bytes(int n, int max_dets, int64_t n_objects) {
-  const int64_t recs = (int64_t)n * max_dets;
-  return align256(recs * 32) + align256(recs * 4) + align256(n_objects * 4) +
-         align256((int64_t)n * 4) + align256((int64_t)n * 8);
+  Carver c;
+  carve_analyze(c, n, max_dets, n_objects);
+  return c.offset;
 }
 
 __device__ __forceinline__ void refuse16(sqdet_kitti_analysis* out, int image, int reason) {
@@ -726,7 +722,8 @@ int sqdet_kitti_eval(int n, int max_dets, const sqdet_det* dets, const int32_t* 
   DeviceGuard guard(device);
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the records' device");
   cudaStream_t st = (cudaStream_t)stream;
-  const Scratch s = carve(scratch, n, max_dets);
+  Carver c{static_cast<uint8_t*>(scratch)};
+  const Scratch s = carve(c, n, max_dets);
   SQ_CUDA(cudaMemsetAsync(out, 0, sizeof(sqdet_kitti_result), st));
   SQ_CUDA(cudaMemsetAsync(&out->status, 0xff, sizeof(out->status), st));
   SQ_CUDA(cudaMemsetAsync(s.hist, 0, kCd * kBins * 4, st));
@@ -793,7 +790,8 @@ int sqdet_kitti_analyze(int n, int max_dets, const sqdet_det* dets, const int32_
   DeviceGuard guard(device);
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select the records' device");
   cudaStream_t st = (cudaStream_t)stream;
-  const AnalyzeScratch s = carve_analyze(scratch, n, max_dets, n_objects);
+  Carver c{static_cast<uint8_t*>(scratch)};
+  const AnalyzeScratch s = carve_analyze(c, n, max_dets, n_objects);
   SQ_CUDA(cudaMemsetAsync(out, 0, sizeof(sqdet_kitti_analysis), st));
   SQ_CUDA(cudaMemsetAsync(&out->status, 0xff, sizeof(out->status), st));
   rank_kernel<<<n, kAnalyzeThreads, 0, st>>>(dets, counts, objs, offsets, n_objects, max_dets,

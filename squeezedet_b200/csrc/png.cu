@@ -29,9 +29,7 @@
 //  10. idat         one CTA per IDAT chunk: its bytes and CRC-32 (per-thread CRCs of 32-byte
 //                   pieces combined by multiplication with x^(8 n) mod P); the first CTA writes the
 //                   signature and IHDR, the last IEND
-// Frames run kPngFramesPerLaunch at a time through these launches, reusing one scratch.
-#include <algorithm>
-
+// Frames run kEncodeFramesPerLaunch at a time through these launches, reusing one scratch.
 #include "frames.cuh"
 #include "scan.cuh"
 
@@ -52,9 +50,8 @@ constexpr int kIdatBytes = 8192;        // libpng's zbuffer: the IDAT data size
 constexpr int kIdatThreads = 256;
 constexpr int kCrcPiece = 32;           // bytes per thread of a chunk's CRC
 constexpr int kFrameThreads = 1024;
-constexpr int kMaxPngFrames = 128;      // frames per sqdet_encode_png call
 constexpr int kPngMaxSide = 1000000;    // libpng's PNG_USER_WIDTH_MAX / PNG_USER_HEIGHT_MAX
-constexpr int kPngFramesPerLaunch = 16;
+constexpr Encoder kPng = {"sqdet_encode_png", "PNG", "sqdet_png_scratch_bytes", 128, kPngMaxSide};
 constexpr int kLCodes = 286, kDCodes = 30, kBlCodes = 19, kEndBlock = 256;
 constexpr int kHeapSize = 2 * kLCodes + 1;
 constexpr int kFixedBytes = 8 + 25 + 12;  // signature, IHDR, IEND
@@ -153,7 +150,7 @@ struct FrameRec {
 };
 
 struct PngParams {
-  PngGeom g[kPngFramesPerLaunch];
+  PngGeom g[kEncodeFramesPerLaunch];
   uint8_t* data;                        // filtered streams
   int64_t* brk;                         // per segment: last run start, then the scanned run starts
   int64_t* cnt;                         // per segment: symbols, then the scanned first indices
@@ -168,7 +165,7 @@ struct PngParams {
 template <int F>
 struct FilterParams {
   PngParams p;
-  FrameDesc<kPlanes<F>> f[kPngFramesPerLaunch];
+  FrameDesc<kPlanes<F>> f[kEncodeFramesPerLaunch];
 };
 static_assert(sizeof(FilterParams<SQDET_FMT_I420>) <= 4096, "filter parameters exceed 4 KiB");
 
@@ -906,8 +903,6 @@ int64_t png_max_bytes(int h, int w) {
   return kFixedBytes + 12 * s.chunks + s.zmax;
 }
 
-int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
-
 // The scratch of the frames [first, first + count): filtered bytes, segment values (run starts,
 // symbol counts, Adler-32 terms), symbols, deflate blocks, frame records, zlib streams.
 struct GroupLayout {
@@ -1002,32 +997,21 @@ int launch_group(const PixFormat& pf, const FrameSource* fr, int first, int coun
 // The scratch the encode of the crops of `frames` needs.
 int64_t png_scratch_bytes(const FrameSource* frames, int n) {
   int64_t most = 0;
-  for (int first = 0; first < n; first += kPngFramesPerLaunch)
-    most = std::max(most, group_layout(frames, first, std::min(kPngFramesPerLaunch, n - first), nullptr).total);
+  for_each_group(n, [&](int first, int count) {
+    most = std::max(most, group_layout(frames, first, count, nullptr).total);
+    return SQDET_OK;
+  });
   return most;
 }
 
 int launch_encode_png(int format, const PixFormat& pf, const FrameSource* frames, int n, uint8_t* out,
                       int64_t cap, int64_t* lengths, void* scratch, cudaStream_t stream) {
   uint8_t* s = static_cast<uint8_t*>(scratch);
-  for (int first = 0; first < n; first += kPngFramesPerLaunch) {
-    const int count = std::min(kPngFramesPerLaunch, n - first);
-    int rc;
-    switch (format) {
-#define SQ_PNG_CASE(F) \
-  case F: rc = launch_group<F>(pf, frames, first, count, out, cap, lengths, s, stream); break;
-      SQ_PNG_CASE(SQDET_FMT_BGR)
-      SQ_PNG_CASE(SQDET_FMT_RGB)
-      SQ_PNG_CASE(SQDET_FMT_BGRA)
-      SQ_PNG_CASE(SQDET_FMT_RGBA)
-      SQ_PNG_CASE(SQDET_FMT_RGB_PLANAR)
-      SQ_PNG_CASE(SQDET_FMT_NV12)
-      default: rc = launch_group<SQDET_FMT_I420>(pf, frames, first, count, out, cap, lengths, s, stream);
-#undef SQ_PNG_CASE
-    }
-    if (rc) return rc;
-  }
-  return SQDET_OK;
+  return for_each_group(n, [&](int first, int count) {
+    return dispatch_format(format, [&](auto f) {
+      return launch_group<decltype(f)::value>(pf, frames, first, count, out, cap, lengths, s, stream);
+    });
+  });
 }
 
 }  // namespace
@@ -1046,8 +1030,7 @@ int64_t sqdet_png_max_bytes(int h, int w) {
 int64_t sqdet_png_scratch_bytes(int n, const int32_t* heights, const int32_t* widths,
                                 const int32_t* crops) {
   std::vector<FrameSource> fr;
-  if (encode_crops("sqdet_png_scratch_bytes", "PNG", kMaxPngFrames, kPngMaxSide, n, heights, widths, crops, fr))
-    return -1;
+  if (encode_crops(kPng.scratch_call, kPng, n, heights, widths, crops, fr)) return -1;
   return png_scratch_bytes(fr.data(), n);
 }
 
@@ -1055,32 +1038,14 @@ int sqdet_encode_png(int n, int format, const uint8_t* const* planes, const int6
                      const int32_t* heights, const int32_t* widths, const int32_t* crops,
                      uint8_t* out_dev, int64_t cap, int64_t* lengths_dev, void* scratch_dev,
                      int64_t scratch_bytes, void* stream) {
-  const std::string name = "sqdet_encode_png";
-  const PixFormat* pf = pix_format(format);
-  if (!pf) return fail(SQDET_ERR_INVALID_ARG, name + ": unknown format");
-  if (!planes || !heights || !widths || !out_dev || !lengths_dev || !scratch_dev)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  std::vector<FrameSource> fr;
-  int rc = encode_crops(name, "PNG", kMaxPngFrames, kPngMaxSide, n, heights, widths, crops, fr);
-  if (rc) return rc;
-  if (cap < 1) return fail(SQDET_ERR_INVALID_ARG, name + ": cap must be at least 1");
-  // the scratch holds int64, 16-bit and 32-bit atomic regions at 256-byte offsets from its start
-  if ((uintptr_t)scratch_dev % 256)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
-  if ((uintptr_t)lengths_dev % alignof(int64_t))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": lengths_dev must be 8-byte aligned");
-  if (scratch_bytes < png_scratch_bytes(fr.data(), n))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below sqdet_png_scratch_bytes");
-  int device = kFrame0Device;
-  rc = accept_frames(name, *pf, n, planes, pitches, heights, widths, crops, nullptr, &device, fr);
-  if (rc) return rc;
-  const bool out_fits = cap <= INT64_MAX / n && device_range_ok(out_dev, (int64_t)n * cap, device);
-  if (!out_fits || !device_range_ok(lengths_dev, (int64_t)n * 8, device) ||
-      !device_range_ok(scratch_dev, scratch_bytes, device))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": out_dev, lengths_dev or scratch_dev is not inside one "
-                                              "device allocation on frame 0's device");
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select frame 0's device");
-  return launch_encode_png(format, *pf, fr.data(), n, out_dev, cap, lengths_dev, scratch_dev,
-                           (cudaStream_t)stream);
+  auto settle = [&](const std::vector<FrameSource>& fr, int64_t& need) {
+    need = png_scratch_bytes(fr.data(), n);
+    return SQDET_OK;
+  };
+  auto launch = [&](const PixFormat& pf, const FrameSource* fr) {
+    return launch_encode_png(format, pf, fr, n, out_dev, cap, lengths_dev, scratch_dev,
+                             (cudaStream_t)stream);
+  };
+  return encode_frames(kPng, n, format, planes, pitches, heights, widths, crops, out_dev, cap,
+                       lengths_dev, scratch_dev, scratch_bytes, settle, launch);
 }

@@ -1,9 +1,12 @@
 """Frames in device memory as the library's frame calls take them (sqdet_forward_frames,
-sqdet_forward_tiles, sqdet_draw_dets, sqdet_encode_jpeg): the pixel formats, the C arrays of a
-batch of uint8 CUDA tensors, and the checks those calls share."""
+sqdet_forward_tiles, sqdet_draw_dets, sqdet_encode_jpeg, sqdet_encode_png): the pixel formats, the
+C arrays of a batch of uint8 CUDA tensors, the checks those calls share, and what the encoders
+share: the call itself, its stream and the copy-back of the files."""
 from __future__ import annotations
 
 import ctypes as C
+
+from . import _lib
 
 # The pixel formats, in SQDET_FMT_* order
 PIXEL_FORMATS = ('bgr', 'rgb', 'bgra', 'rgba', 'rgb_planar', 'nv12', 'i420')
@@ -53,6 +56,73 @@ def pack_frames(frames, fmt, crops, gpu_id):
     rects.extend(rect)
   return ((C.c_void_p * (3 * n))(*planes), (C.c_int64 * (3 * n))(*pitches),
           (C.c_int32 * n)(*hs), (C.c_int32 * n)(*ws), (C.c_int32 * (4 * n))(*rects))
+
+
+def first_tensor(f):
+  """Frame f's tensor, or its first plane's when f is a tuple of planes."""
+  return f[0] if isinstance(f, (tuple, list)) else f
+
+
+def torch_stream(stream, device):
+  """`stream` (a torch.cuda.Stream, a raw cudaStream_t, or None for torch's current stream on
+  `device`) as a torch stream, so that allocations can be ordered on it."""
+  import torch
+  if stream is None:
+    return torch.cuda.current_stream(device)
+  if isinstance(stream, torch.cuda.Stream):
+    return stream
+  raw = int(stream)
+  return torch.cuda.default_stream(device) if raw == 0 else torch.cuda.ExternalStream(raw, device=device)
+
+
+def encode_frames(frames, fmt, crops, stream, max_bytes, scratch_call, encode_call, settle=tuple):
+  """The files of an encoder (encode_jpeg_device, encode_png_device): the checks in this order
+  (1 to 128 frames, fmt, the codec's settings, frame 0 on a CUDA device, pack_frames), then cap =
+  max_bytes(h, w) of the largest crop, the scratch the C call `scratch_call` (n, heights, widths,
+  crops, *extra) gives and the C call `encode_call` (n, format, planes, pitches, heights, widths,
+  crops, *extra, data, cap, lengths, scratch, scratch_bytes, stream), where extra = settle() checks
+  the codec's settings and holds its further arguments to both calls."""
+  import torch
+  frames = list(frames)
+  n = frame_count(frames, 128)
+  if fmt not in PIXEL_FORMATS:
+    raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
+  extra = settle()
+  device = getattr(first_tensor(frames[0]), 'device', None)
+  if getattr(device, 'type', None) != 'cuda':
+    raise ValueError('frame 0: need a CUDA tensor, got %s' % (device,))
+  planes, pitches, hs, ws, rects = pack_frames(frames, fmt, crops, device.index)
+  lib = _lib.load()
+  cap = max(max_bytes(rects[4 * i + 3], rects[4 * i + 2]) for i in range(n))
+  nbytes = getattr(lib, scratch_call)(n, hs, ws, rects, *extra)
+  if nbytes < 0:
+    raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
+  s = torch_stream(stream, device)
+  # allocated on s: the caching allocator hands the scratch to a later allocation only in s's
+  # order, after the encode has finished with it
+  with torch.cuda.device(device), torch.cuda.stream(s):
+    data = torch.empty((n, cap), dtype=torch.uint8, device=device)
+    lengths = torch.empty((n,), dtype=torch.int64, device=device)
+    scratch = torch.empty((nbytes,), dtype=torch.uint8, device=device)
+    _lib.check(getattr(lib, encode_call)(n, PIXEL_FORMATS.index(fmt), planes, pitches, hs, ws,
+                                         rects, *extra, data.data_ptr(), cap, lengths.data_ptr(),
+                                         scratch.data_ptr(), nbytes, s.cuda_stream))
+  return data, lengths
+
+
+def file_bytes(data, lengths, stream=None):
+  """The files of an encoder's (data, lengths) as bytes objects, copying back only each file's own
+  bytes, in order after the work on `stream` (as the encoder takes it: pass the encode's stream).
+  ValueError for a frame whose file did not fit."""
+  import torch
+  with torch.cuda.device(data.device), torch.cuda.stream(torch_stream(stream, data.device)):
+    lens = lengths.cpu().tolist()
+    out = []
+    for i, n in enumerate(lens):
+      if n < 0:
+        raise ValueError('frame %d: the file did not fit the output capacity' % i)
+      out.append(data[i, :n].cpu().numpy().tobytes())
+  return out
 
 
 def _frame_planes(i, f, fmt, gpu_id):

@@ -13,12 +13,7 @@ from __future__ import annotations
 import ctypes as C
 
 from . import _lib
-from .frames import PIXEL_FORMATS, frame_count, pack_frames
-
-
-def _first_tensor(f):
-  return f[0] if isinstance(f, (tuple, list)) else f
-
+from .frames import encode_frames, file_bytes, torch_stream
 
 # cv2's IMWRITE_JPEG_SAMPLING_FACTOR value of each sampling encode_jpeg_device takes
 SAMPLINGS = {'411': 0x411111, '420': 0x221111, '422': 0x211111, '440': 0x121111, '444': 0x111111}
@@ -52,18 +47,6 @@ def max_bytes(h, w, **params):
   return int(_lib.load().sqdet_jpeg_max_bytes_params(int(h), int(w), C.byref(p)))
 
 
-def _torch_stream(stream, device):
-  """`stream` (a torch.cuda.Stream, a raw cudaStream_t, or None for torch's current stream on
-  `device`) as a torch stream, so that allocations can be ordered on it."""
-  import torch
-  if stream is None:
-    return torch.cuda.current_stream(device)
-  if isinstance(stream, torch.cuda.Stream):
-    return stream
-  raw = int(stream)
-  return torch.cuda.default_stream(device) if raw == 0 else torch.cuda.ExternalStream(raw, device=device)
-
-
 def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None, *, sampling='420',
                        optimize=False, restart_interval=0, luma_quality=None, chroma_quality=None):
   """-> (data [n, cap] uint8, lengths [n] int64), both on the frames' device: frame i's file is
@@ -87,51 +70,16 @@ def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None, *, samp
   counts only with it, and two different ones give 4:4:4 whatever `sampling` says).  4:4:4
   doubles the worst-case sizes of 4:2:0.  Values cv2 would clamp raise ValueError.  Progressive
   files are not written: use cv2.imencode with IMWRITE_JPEG_PROGRESSIVE for those."""
-  import torch
-  frames = list(frames)
-  n = frame_count(frames, 128)
-  if fmt not in PIXEL_FORMATS:
-    raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
   settings = dict(quality=quality, sampling=sampling, optimize=optimize,
                   restart_interval=restart_interval, luma_quality=luma_quality,
                   chroma_quality=chroma_quality)
-  params = jpeg_params(**settings)
-  device = getattr(_first_tensor(frames[0]), 'device', None)
-  if getattr(device, 'type', None) != 'cuda':
-    raise ValueError('frame 0: need a CUDA tensor, got %s' % (device,))
-  planes, pitches, hs, ws, rects = pack_frames(frames, fmt, crops, device.index)
-  lib = _lib.load()
-  cap = max(max_bytes(rects[4 * i + 3], rects[4 * i + 2], **settings) for i in range(n))
-  scratch_bytes = lib.sqdet_jpeg_scratch_bytes_params(n, hs, ws, rects, C.byref(params))
-  if scratch_bytes < 0:
-    raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
-  s = _torch_stream(stream, device)
-  # allocated on s: the caching allocator hands the scratch to a later allocation only in s's
-  # order, after the encode has finished with it
-  with torch.cuda.device(device), torch.cuda.stream(s):
-    data = torch.empty((n, cap), dtype=torch.uint8, device=device)
-    lengths = torch.empty((n,), dtype=torch.int64, device=device)
-    scratch = torch.empty((scratch_bytes,), dtype=torch.uint8, device=device)
-    _lib.check(lib.sqdet_encode_jpeg_params(n, PIXEL_FORMATS.index(fmt), planes, pitches, hs, ws,
-                                            rects, C.byref(params), data.data_ptr(), cap,
-                                            lengths.data_ptr(), scratch.data_ptr(), scratch_bytes,
-                                            s.cuda_stream))
-  return data, lengths
+  return encode_frames(frames, fmt, crops, stream, lambda h, w: max_bytes(h, w, **settings),
+                       'sqdet_jpeg_scratch_bytes_params', 'sqdet_encode_jpeg_params',
+                       lambda: (C.byref(jpeg_params(**settings)),))
 
 
-def jpeg_bytes(data, lengths, stream=None):
-  """The files of encode_jpeg_device's (data, lengths) as bytes objects, copying back only each
-  file's own bytes, in order after the work on `stream` (as encode_jpeg_device takes it: pass the
-  encode's stream).  ValueError for a frame whose file did not fit."""
-  import torch
-  with torch.cuda.device(data.device), torch.cuda.stream(_torch_stream(stream, data.device)):
-    lens = lengths.cpu().tolist()
-    out = []
-    for i, n in enumerate(lens):
-      if n < 0:
-        raise ValueError('frame %d: the file did not fit the output capacity' % i)
-      out.append(data[i, :n].cpu().numpy().tobytes())
-  return out
+# the files of encode_jpeg_device's (data, lengths)
+jpeg_bytes = file_bytes
 
 
 # ---- decoding ------------------------------------------------------------------------------------
@@ -229,7 +177,7 @@ def decode_jpeg_device(files, device, stream=None):
   scratch_bytes = lib.sqdet_jpeg_decode_scratch_bytes(n, ptrs, lens)
   if staging_bytes < 0 or scratch_bytes < 0:
     raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
-  s = _torch_stream(stream, device)
+  s = torch_stream(stream, device)
   staging = _staging.setdefault(device.index, _Staging())
   slot, buf = staging.get(staging_bytes)
   with torch.cuda.device(device), torch.cuda.stream(s):

@@ -26,6 +26,7 @@ import os
 import numpy as np
 
 from . import _lib
+from .frames import torch_stream
 
 CLASSES = ('car', 'pedestrian', 'cyclist')
 TYPE_CODES = {'car': 0, 'pedestrian': 1, 'cyclist': 2, 'van': 3, 'person_sitting': 4,
@@ -226,7 +227,6 @@ def evaluate_device(dets, counts, class_names, labels, stream=None, device=None)
   nothing is scored and no class is returned, as evaluate_object writes no stats for an empty
   set."""
   import torch
-  from .jpeg import _torch_stream
   n = len(labels)
   device = _cuda_device(dets, device)
   codes = [CLASSES.index(_fold(c)) if _fold(c) in CLASSES else -1 for c in class_names]
@@ -238,7 +238,7 @@ def evaluate_device(dets, counts, class_names, labels, stream=None, device=None)
     return {}
   dets = _cut_capacity(dets, counts)
   lib = _lib.load()
-  s = _torch_stream(stream, device)
+  s = torch_stream(stream, device)
   with torch.cuda.device(device), torch.cuda.stream(s):
     d, c, max_dets, n_obj, objs, offsets = _upload(dets, counts, labels, device)
     nbytes = lib.sqdet_kitti_eval_scratch_bytes(n, max_dets, n_obj)
@@ -334,7 +334,6 @@ def analyze_device(dets, counts, class_names, labels, stream=None, device=None):
   Runs on `stream` and waits for it at the end, for the counts and then the lines.  With no
   images nothing is launched and every count is 0."""
   import torch
-  from .jpeg import _torch_stream
   n = len(labels)
   device = _cuda_device(dets, device)
   names = list(class_names)
@@ -347,7 +346,7 @@ def analyze_device(dets, counts, class_names, labels, stream=None, device=None):
   dets = _cut_capacity(dets, counts)
   capacity = 2 * int(np.isin(labels.objs['type'], codes).sum())
   lib = _lib.load()
-  s = _torch_stream(stream, device)
+  s = torch_stream(stream, device)
   with torch.cuda.device(device), torch.cuda.stream(s):
     d, c, max_dets, n_obj, objs, offsets = _upload(dets, counts, labels, device)
     nbytes = lib.sqdet_kitti_analyze_scratch_bytes(n, max_dets, n_obj)

@@ -11,13 +11,12 @@ cv2.  No engine is needed."""
 from __future__ import annotations
 
 from . import _lib
-from .frames import PIXEL_FORMATS, frame_count, pack_frames
-from .jpeg import _first_tensor, _torch_stream, jpeg_bytes
+from .frames import encode_frames, file_bytes
 
 MAX_SIDE = 1000000        # libpng's PNG_USER_WIDTH_MAX / PNG_USER_HEIGHT_MAX
 
 # the files of encode_png_device's (data, lengths): the same per-file copy-back as JPEG's
-png_bytes = jpeg_bytes
+png_bytes = file_bytes
 
 
 def max_bytes(h, w):
@@ -40,28 +39,5 @@ def encode_png_device(frames, fmt, crops=None, stream=None):
   take if every filtered byte cost 9 bits (sqdet_png_max_bytes, about 7 MB for 1920 x 1080), and
   the scratch is about 26 MB per 1080p frame of each group of 16.  Sides above 1000000 raise
   ValueError before anything is allocated; cv2.imencode refuses them too."""
-  import torch
-  frames = list(frames)
-  n = frame_count(frames, 128)
-  if fmt not in PIXEL_FORMATS:
-    raise ValueError('fmt must be one of %s, got %r' % (', '.join(PIXEL_FORMATS), fmt))
-  device = getattr(_first_tensor(frames[0]), 'device', None)
-  if getattr(device, 'type', None) != 'cuda':
-    raise ValueError('frame 0: need a CUDA tensor, got %s' % (device,))
-  planes, pitches, hs, ws, rects = pack_frames(frames, fmt, crops, device.index)
-  lib = _lib.load()
-  cap = max(max_bytes(rects[4 * i + 3], rects[4 * i + 2]) for i in range(n))
-  scratch_bytes = lib.sqdet_png_scratch_bytes(n, hs, ws, rects)
-  if scratch_bytes < 0:
-    raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
-  s = _torch_stream(stream, device)
-  # allocated on s: the caching allocator hands the scratch to a later allocation only in s's
-  # order, after the encode has finished with it
-  with torch.cuda.device(device), torch.cuda.stream(s):
-    data = torch.empty((n, cap), dtype=torch.uint8, device=device)
-    lengths = torch.empty((n,), dtype=torch.int64, device=device)
-    scratch = torch.empty((scratch_bytes,), dtype=torch.uint8, device=device)
-    _lib.check(lib.sqdet_encode_png(n, PIXEL_FORMATS.index(fmt), planes, pitches, hs, ws, rects,
-                                    data.data_ptr(), cap, lengths.data_ptr(), scratch.data_ptr(),
-                                    scratch_bytes, s.cuda_stream))
-  return data, lengths
+  return encode_frames(frames, fmt, crops, stream, max_bytes, 'sqdet_png_scratch_bytes',
+                       'sqdet_encode_png')

@@ -1,5 +1,6 @@
 """sqdet_encode_jpeg and its size functions refuse bad arguments before any device work, so without
-a GPU too, and give the sizes the encoder needs."""
+a GPU too, and give the sizes the encoder needs.  The refusals both encoders share are in
+test_encode_abi."""
 import ctypes as C
 
 import numpy as np
@@ -8,7 +9,7 @@ import pytest
 from oracle import jpeg as ojpeg
 from squeezedet_b200 import _lib
 
-FMT_BGR, FMT_NV12 = 0, 5
+FMT_BGR = 0
 FAKE = 1 << 40            # never dereferenced: the argument checks come first
 
 
@@ -25,13 +26,11 @@ def host_planes(n=1):
   return p
 
 
-def encode(n=1, fmt=FMT_BGR, planes='host', h=16, w=16, crops=None, quality=95, out=FAKE, cap=1 << 20,
-           lengths=FAKE, scratch=FAKE, scratch_bytes=1 << 40):
+def encode(n=1, h=16, w=16, quality=95):
   lib = _lib.load()
-  hs, ws, cr = arrays(max(n, 1), h, w, crops)
-  pl = host_planes(max(n, 1)) if planes == 'host' else planes
-  return lib.sqdet_encode_jpeg(n, fmt, pl, None, hs, ws, cr, quality, out, cap, lengths, scratch,
-                               scratch_bytes, None)
+  hs, ws, _ = arrays(n, h, w)
+  return lib.sqdet_encode_jpeg(n, FMT_BGR, host_planes(n), None, hs, ws, None, quality, FAKE, 1 << 20,
+                               FAKE, FAKE, 1 << 40, None)
 
 
 def refused(rc, *words):
@@ -40,57 +39,12 @@ def refused(rc, *words):
   assert all(w.encode() in msg for w in words), msg
 
 
-def test_null_arguments():
-  lib = _lib.load()
-  hs, ws, _ = arrays()
-  pl = host_planes()
-  for args in [(None, None, hs, ws), (pl, None, None, ws), (pl, None, hs, None)]:
-    refused(lib.sqdet_encode_jpeg(1, FMT_BGR, *args, None, 95, FAKE, 100, FAKE, FAKE, 1 << 30, None), 'null')
-  refused(encode(out=None), 'null')
-  refused(encode(lengths=None), 'null')
-  refused(encode(scratch=None), 'null')
-
-
-def test_counts_format_quality_cap():
-  refused(encode(n=0), 'n must be in [1, 128]')
-  refused(encode(n=129), 'n must be in [1, 128]')
-  refused(encode(fmt=7), 'unknown format')
-  refused(encode(fmt=-1), 'unknown format')
+def test_quality_and_side():
+  """The refusals of sqdet_encode_jpeg's own: the quality, and sides past 65500.  The ones it shares
+  with sqdet_encode_png are in test_encode_abi."""
   refused(encode(quality=0), 'quality')
   refused(encode(quality=101), 'quality')
-  refused(encode(cap=0), 'cap')
-
-
-def test_frame_refusals():
-  refused(encode(h=0), 'frame 0 is empty')
-  refused(encode(crops=[0, 0, 0, 4]), 'empty crop')
-  refused(encode(crops=[10, 0, 8, 4]), 'crop outside the frame')
   refused(encode(h=70000, w=8), '65500')
-  refused(encode(fmt=FMT_NV12, h=15, w=16), 'even')
-  null_plane = (C.c_void_p * 3)(None, None, None)
-  refused(encode(planes=null_plane, fmt=FMT_BGR), 'null pointer')
-
-
-def test_misaligned_scratch_or_lengths():
-  """The scratch holds 16-byte vector, int64 and 32-bit atomic regions and lengths_dev int64s:
-  a misaligned pointer is refused rather than faulting a kernel."""
-  for off in (1, 8, 16, 128):
-    refused(encode(scratch=FAKE + off), 'scratch_dev must be 256-byte aligned')
-  for off in (1, 4):
-    refused(encode(lengths=FAKE + off), 'lengths_dev must be 8-byte aligned')
-  refused(encode(out=FAKE + 1), 'frame 0')        # out_dev may start at any byte
-
-
-def test_scratch_too_small():
-  lib = _lib.load()
-  hs, ws, _ = arrays()
-  need = lib.sqdet_jpeg_scratch_bytes(1, hs, ws, None)
-  refused(encode(scratch_bytes=need - 1), 'scratch_bytes')
-
-
-def test_memory_not_on_a_device():
-  """Host memory for the frames, the output or the scratch is refused, naming it."""
-  refused(encode(), 'frame 0', 'not inside one device allocation')
 
 
 def test_max_bytes():

@@ -1,5 +1,6 @@
 """sqdet_encode_png and its size functions refuse bad arguments before any device work, so without
-a GPU too, and give the sizes the encoder needs."""
+a GPU too, and give the sizes the encoder needs.  The refusals both encoders share are in
+test_encode_abi."""
 import ctypes as C
 
 import numpy as np
@@ -9,7 +10,7 @@ from oracle import png as opng
 from squeezedet_b200 import _lib
 from squeezedet_b200 import png as spng
 
-FMT_BGR, FMT_NV12 = 0, 5
+FMT_BGR = 0
 FAKE = 1 << 40            # never dereferenced: the argument checks come first
 
 
@@ -26,12 +27,11 @@ def host_planes(n=1):
   return p
 
 
-def encode(n=1, fmt=FMT_BGR, h=16, w=16, crops=None, out=FAKE, cap=1 << 20, lengths=FAKE,
-           scratch=FAKE, scratch_bytes=1 << 40):
+def encode(h=16, w=16, crops=None):
   lib = _lib.load()
-  hs, ws, cr = arrays(max(n, 1), h, w, crops)
-  return lib.sqdet_encode_png(n, fmt, host_planes(max(n, 1)), None, hs, ws, cr, out, cap, lengths,
-                              scratch, scratch_bytes, None)
+  hs, ws, cr = arrays(1, h, w, crops)
+  return lib.sqdet_encode_png(1, FMT_BGR, host_planes(), None, hs, ws, cr, FAKE, 1 << 20, FAKE, FAKE,
+                              1 << 40, None)
 
 
 def refused(rc, *words):
@@ -44,36 +44,6 @@ def test_symbols_declared():
   lib = _lib.load()
   for name in ('sqdet_png_max_bytes', 'sqdet_png_scratch_bytes', 'sqdet_encode_png'):
     assert name in _lib.SIGNATURES and getattr(lib, name)
-
-
-def test_null_arguments():
-  lib = _lib.load()
-  hs, ws, _ = arrays()
-  pl = host_planes()
-  for args in [(None, None, hs, ws), (pl, None, None, ws), (pl, None, hs, None)]:
-    refused(lib.sqdet_encode_png(1, FMT_BGR, *args, None, FAKE, 100, FAKE, FAKE, 1 << 30, None), 'null')
-  refused(encode(out=None), 'null')
-  refused(encode(lengths=None), 'null')
-  refused(encode(scratch=None), 'null')
-
-
-def test_counts_format_cap_alignment():
-  refused(encode(n=0), 'n must be in [1, 128]')
-  refused(encode(n=129), 'n must be in [1, 128]')
-  refused(encode(fmt=7), 'unknown format')
-  refused(encode(fmt=-1), 'unknown format')
-  refused(encode(cap=0), 'cap')
-  refused(encode(scratch=FAKE + 8), '256-byte aligned')
-  refused(encode(lengths=FAKE + 4), '8-byte aligned')
-  refused(encode(scratch_bytes=100), 'sqdet_png_scratch_bytes')
-
-
-def test_frame_refusals():
-  refused(encode(h=0), 'frame 0', 'empty')
-  refused(encode(crops=[10, 0, 10, 4]), 'crop outside the frame')
-  refused(encode(crops=[0, 0, 0, 4]), 'empty crop')
-  refused(encode(), 'not inside one device allocation')          # host memory is not a frame
-  refused(encode(fmt=FMT_NV12, h=15), 'even')
 
 
 def test_side_limits():
