@@ -545,8 +545,8 @@ int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int
  *   restart_interval  IMWRITE_JPEG_RST_INTERVAL, 0..65535 MCUs (0: no restart markers)
  * cv2 clamps out-of-range values and falls back to 4:2:0 for another sampling; these functions
  * refuse them with SQDET_ERR_INVALID_ARG instead (as they refuse a null params), and otherwise
- * refuse what sqdet_encode_jpeg refuses.  Progressive files (IMWRITE_JPEG_PROGRESSIVE) are not
- * written: encode those with cv2.
+ * refuse what sqdet_encode_jpeg refuses.  Progressive files (IMWRITE_JPEG_PROGRESSIVE) are
+ * sqdet_encode_jpeg_progressive's, below.
  * sqdet_jpeg_max_bytes_params and sqdet_jpeg_scratch_bytes_params are the output capacity and
  * scratch of those parameters (-1 when the parameters or sizes are refused).  Sampling, optimize
  * and restart markers raise both: 4:4:4 codes three blocks per 8x8 pixels against 4:2:0's 1.5,
@@ -571,6 +571,39 @@ int sqdet_encode_jpeg_params(int n, int format, const uint8_t* const* planes, co
                              const sqdet_jpeg_params* params, uint8_t* out_dev, int64_t cap,
                              int64_t* lengths_dev, void* scratch_dev, int64_t scratch_bytes,
                              void* stream);
+
+/* ---- progressive JPEG encoding ------------------------------------------------------
+ * sqdet_encode_jpeg_progressive: sqdet_encode_jpeg_params with the file cv2.imencode('.jpg', crop,
+ * list + [IMWRITE_JPEG_PROGRESSIVE, 1]) writes: SOF2 and jpeg_simple_progression's ten scans (DC
+ * first of Y, Cb, Cr; Y 1-5; Cr, Cb 1-63; Y 6-63; Y 1-63 refinement; DC refinement; Cr, Cb, Y
+ * 1-63 refinement), each with its own optimal Huffman tables, over the baseline file's quantized
+ * coefficients.  `optimize` is checked and has no effect, as in cv2: progressive tables are always
+ * optimal.  A restart interval counts MCUs in the two DC scans and blocks in the others, whose
+ * scans cover only the component's own blocks; one DRI sits before the first scan.  The refusals are
+ * sqdet_encode_jpeg_params'.
+ * sqdet_jpeg_max_bytes_progressive is the output capacity: 3055 bytes of headers (SOI .. SOF2 and
+ * ten DHT segments of at most 256 symbols, two three-component and eight one-component SOS), 6
+ * for the DRI with an interval, twice the bytes of the scans' longest data, 2 per RSTn (each
+ * scan's intervals but its first) and 2 for EOI.  A scan's longest data is ceil(units * bits / 8)
+ * plus a padding byte per interval, with units its blocks (the DC scans: every block of the MCUs;
+ * the others: the component's ceil(w_c / 8) x ceil(h_c / 8)) and bits per unit 27 for the DC first
+ * scan (16-bit code, 11 bits), 1 for the DC refinement, 26 n + 30 for a first AC scan of n
+ * coefficients (16 + 10 bits per coefficient, the EOBRUN code of 16 + 14 bits after the block) and
+ * 17 n + 30 for an AC refinement (16 + 1 bits per newly nonzero coefficient, a correction bit per
+ * other, the EOBRUN code; ZRLs cost at most a bit per zero).  Every byte may be stuffed.
+ * sqdet_jpeg_scratch_bytes_progressive is the scratch: the coefficients, four 32-bit words per
+ * unit of all ten scans, the bit buffers of those longest data, and per frame 11 x 256 64-bit
+ * symbol counts and its tables.  -1 when the parameters or sizes are refused.
+ * A group of 16 frames takes one memset and fourteen launches for all ten scans; none waits for the
+ * device. */
+int64_t sqdet_jpeg_max_bytes_progressive(int h, int w, const sqdet_jpeg_params* params);
+int64_t sqdet_jpeg_scratch_bytes_progressive(int n, const int32_t* heights, const int32_t* widths,
+                                             const int32_t* crops, const sqdet_jpeg_params* params);
+int sqdet_encode_jpeg_progressive(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
+                                  const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                                  const sqdet_jpeg_params* params, uint8_t* out_dev, int64_t cap,
+                                  int64_t* lengths_dev, void* scratch_dev, int64_t scratch_bytes,
+                                  void* stream);
 
 /* ---- PNG encoding of frames in device memory (no engine needed) ---------------------
  * sqdet_encode_png: frame i's crop (x, y, w, h) becomes exactly the bytes of

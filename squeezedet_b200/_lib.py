@@ -141,6 +141,10 @@ SIGNATURES = {
     'sqdet_jpeg_scratch_bytes_params': (_i64, [_i, _vp, _vp, _vp, C.POINTER(JpegParams)]),
     'sqdet_encode_jpeg_params': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, C.POINTER(JpegParams), _vp,
                                       _i64, _vp, _vp, _i64, _vp]),
+    'sqdet_jpeg_max_bytes_progressive': (_i64, [_i, _i, C.POINTER(JpegParams)]),
+    'sqdet_jpeg_scratch_bytes_progressive': (_i64, [_i, _vp, _vp, _vp, C.POINTER(JpegParams)]),
+    'sqdet_encode_jpeg_progressive': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, C.POINTER(JpegParams), _vp,
+                                           _i64, _vp, _vp, _i64, _vp]),
     'sqdet_png_max_bytes': (_i64, [_i, _i]),
     'sqdet_png_scratch_bytes': (_i64, [_i, _vp, _vp, _vp]),
     'sqdet_encode_png': (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _vp]),

@@ -35,7 +35,8 @@ FRAME_W, FRAME_H, OVERLAP = 1920, 1080, 128
 QUALITY = 95
 SAMPLING_FACTORS = {'411': 0x411111, '420': 0x221111, '422': 0x211111, '440': 0x121111, '444': 0x111111}
 KERNELS = ('transform_kernel', 'hist_kernel', 'table_kernel', 'interval_kernel', 'block_bits_kernel', 'scan_kernel', 'pack_kernel',
-           'count_ff_kernel', 'stuff_kernel')
+           'count_ff_kernel', 'stuff_kernel', 'prog_units_kernel', 'prog_eobrun_kernel', 'prog_table_kernel',
+           'prog_bits_kernel', 'prog_interval_kernel', 'prog_pack_kernel')
 
 
 def parse_args(argv=None):
@@ -49,13 +50,14 @@ def parse_args(argv=None):
   ap.add_argument('--sampling', default='420', choices=('411', '420', '422', '440', '444'))
   ap.add_argument('--optimize', action='store_true')
   ap.add_argument('--restart', type=int, default=0, help='restart interval in MCUs (0: none)')
+  ap.add_argument('--progressive', action='store_true', help='IMWRITE_JPEG_PROGRESSIVE')
   return ap.parse_args(argv)
 
 
 def jpeg_settings(args):
   """encode_jpeg_device's keywords of the command line."""
   return dict(quality=QUALITY, sampling=args.sampling, optimize=args.optimize,
-              restart_interval=args.restart)
+              restart_interval=args.restart, progressive=args.progressive)
 
 
 @dataclasses.dataclass
@@ -87,13 +89,17 @@ def jpeg_encoder(args):
     cv2_params += [cv2.IMWRITE_JPEG_OPTIMIZE, 1]
   if args.restart:
     cv2_params += [cv2.IMWRITE_JPEG_RST_INTERVAL, args.restart]
-  # per 16 frames: a memset and seven launches, two more with optimize and two with restart markers
+  if args.progressive:
+    cv2_params += [cv2.IMWRITE_JPEG_PROGRESSIVE, 1]
+  # per 16 frames: a memset and seven launches, two more with optimize and two with restart
+  # markers; progressive files take a memset and fourteen launches whatever the other settings
+  launches = 15 if args.progressive else 8 + 2 * args.optimize + 2 * bool(args.restart)
   return Encoder('jpeg', '.jpg', cv2_params,
                  lambda frames, fmt, stream: encode_jpeg_device(frames, fmt, stream=stream, **settings),
-                 jpeg_bytes, KERNELS, 8 + 2 * args.optimize + 2 * bool(args.restart),
-                 'JPEG quality %d files' % QUALITY,
+                 jpeg_bytes, KERNELS, launches,
+                 'JPEG quality %d%s files' % (QUALITY, ' progressive' if args.progressive else ''),
                  {'quality': QUALITY, 'sampling': args.sampling, 'optimize': args.optimize,
-                  'restart': args.restart})
+                  'restart': args.restart, 'progressive': args.progressive})
 
 
 def measure_workload(enc, args, name, model, fmt, clean, grid, torch):

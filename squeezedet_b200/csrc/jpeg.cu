@@ -36,6 +36,9 @@
 //                   the header (a host template with the frame's height, width and Huffman
 //                   tables filled in), EOI and the length, or -1 when the file does not fit
 // Frames run kEncodeFramesPerLaunch at a time through these launches, reusing one scratch.
+// Progressive files (sqdet_encode_jpeg_progressive) reuse the transform and then code the ten scans
+// of jpeg_simple_progression in launches P1-P7 below, every launch covering all scans of all frames
+// of the group; oracle/jpeg_progressive.py restates them.
 #include <cstring>
 
 #include "frames.cuh"
@@ -150,6 +153,18 @@ struct FrameHuff {
   HuffSpec s;
 };
 
+// A progressive frame's tables, by slot: scan s's table in slot s (scan 0's the DC luma one), scan
+// 0's DC chroma table in slot kChromaDcSlot; slot 6 (the DC refinement) stays empty.  The frame's
+// tail and symbol-block chunk sums (see prog_units_kernel) start at JpegGeom::tsum.
+constexpr int kScans = 10, kSlots = 11, kChromaDcSlot = 10;
+struct ProgHuff {
+  uint16_t code[kSlots][256];
+  uint8_t len[kSlots][256];
+  uint8_t bits[kSlots][16];
+  uint8_t vals[kSlots][256];
+  int16_t count[kSlots];
+};
+
 // ---- per-frame geometry and scratch ---------------------------------------------------------------
 // One frame of a launch group: its crop, MCU grid and where its pieces of the scratch and output
 // are.  Blocks are numbered in stream order (per MCU: the luma blocks row by row, then Cb, Cr)
@@ -161,6 +176,8 @@ struct JpegGeom {
   int chunks, schunks, ints;            // ints: restart intervals (1 without restart markers)
   int64_t blk, csum, ssum, isum, ipos;  // ipos: the first of its intervals' first bits
   int64_t words;                        // the first 32-bit word of the bit buffer
+  int64_t cblk, tsum;                   // progressive: the first block in coef (blk counts units) and
+                                        // the first tail chunk sum (the symbol-unit sums follow)
   uint8_t* out;
   int64_t* length;
 };
@@ -169,6 +186,8 @@ struct JpegGeom {
 // 16-bit fields would hold up to 65535)
 constexpr int kJpegMaxSide = 65500;
 constexpr Encoder kJpeg = {"sqdet_encode_jpeg", "JPEG", "sqdet_jpeg_scratch_bytes", 128, kJpegMaxSide};
+constexpr Encoder kJpegProg = {"sqdet_encode_jpeg_progressive", "JPEG", "sqdet_jpeg_scratch_bytes_progressive",
+                               128, kJpegMaxSide};
 
 struct JpegParams {
   JpegGeom g[kEncodeFramesPerLaunch];
@@ -179,6 +198,8 @@ struct JpegParams {
   uint32_t* stream;                     // bit buffers
   unsigned long long* freq;             // [frame][4][256] symbol counts (optimize)
   FrameHuff* huff;                      // [frame] (optimize)
+  uint32_t *flags, *pre, *flush;        // [units] (progressive)
+  ProgHuff* phuff;                      // [frame] (progressive)
   int64_t cap;
   int hs, vs, luma, per;                // luma sampling factors, luma blocks and blocks per MCU
   int rst;                              // MCUs per restart interval, 0 for none
@@ -205,6 +226,7 @@ struct StuffParams {
   uint8_t prefix[kPrefixBytes];         // SOI .. SOF0, height and width 0
   uint8_t suffix[kDriBytes + kSosBytes];  // DRI (with restart markers), SOS
   int suffix_bytes;
+  uint8_t sos[10][kSosBytes];           // progressive: each scan's SOS
 };
 static_assert(sizeof(StuffParams) <= 4096, "stuffing parameters exceed 4 KiB");
 
@@ -428,24 +450,17 @@ __device__ __forceinline__ int warp_min_symbol(const unsigned long long* f, int 
 }
 
 // jpeg_gen_optimal_table (JPEG Annex K.2 with libjpeg's tie-breaking and the reserved symbol 256,
-// whose all-ones code no real symbol gets) of frame blockIdx.x's four tables, warp t building table
-// t, then its canonical codes.
-__global__ void __launch_bounds__(kTableThreads) table_kernel(const __grid_constant__ JpegParams p) {
-  __shared__ unsigned long long freq[4][257];
-  __shared__ int16_t size[4][257], others[4][257];
-  __shared__ int bits[4][33];
-  const int t = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  FrameHuff& fh = p.huff[blockIdx.x];
-  const unsigned long long* src = p.freq + ((int64_t)blockIdx.x * 4 + t) * 256;
-  unsigned long long* f = freq[t];
-  int16_t* sz = size[t];
-  int16_t* ot = others[t];
+// whose all-ones code no real symbol gets) of the 256 counts at src, built by one warp in its shared
+// f, sz, ot (257 each) and nb (33), then its DHT contents (bits, vals, count) and canonical codes.
+__device__ __forceinline__ void optimal_table(const unsigned long long* src, unsigned long long* f, int16_t* sz,
+                                              int16_t* ot, int* nb, uint8_t* bits, uint8_t* vals,
+                                              int16_t* count, uint16_t* code, uint8_t* len, int lane) {
   for (int i = lane; i < 257; i += 32) {
     f[i] = i < 256 ? src[i] : 1;
     sz[i] = 0;
     ot[i] = -1;
   }
-  for (int i = lane; i < 33; i += 32) bits[t][i] = 0;
+  for (int i = lane; i < 33; i += 32) nb[i] = 0;
   __syncwarp();
   for (;;) {
     int c1 = warp_min_symbol(f, -1, lane);
@@ -463,7 +478,6 @@ __global__ void __launch_bounds__(kTableThreads) table_kernel(const __grid_const
     __syncwarp();
   }
   if (lane == 0) {
-    int* nb = bits[t];
     for (int i = 0; i < 257; ++i)
       if (sz[i]) ++nb[min((int)sz[i], 32)];  // libjpeg refuses longer codes (2^31 symbols and more)
     for (int i = 32; i > 16; --i)           // lengths above 16 moved up the tree
@@ -478,12 +492,12 @@ __global__ void __launch_bounds__(kTableThreads) table_kernel(const __grid_const
     int i = 16;
     while (nb[i] == 0) --i;
     --nb[i];                                // the reserved symbol's code
-    int count = 0;
+    int n = 0;
     for (int l = 1; l <= 16; ++l) {
-      fh.s.bits[t][l - 1] = (uint8_t)nb[l];
-      count += nb[l];
+      bits[l - 1] = (uint8_t)nb[l];
+      n += nb[l];
     }
-    fh.s.count[t] = (int16_t)count;
+    *count = (int16_t)n;
   }
   __syncwarp();
   // the symbols by (length before the limit, symbol)
@@ -491,22 +505,32 @@ __global__ void __launch_bounds__(kTableThreads) table_kernel(const __grid_const
     if (!sz[s]) continue;
     int rank = 0;
     for (int u = 0; u < 256; ++u) rank += sz[u] && (sz[u] < sz[s] || (sz[u] == sz[s] && u < s));
-    fh.s.vals[t][rank] = (uint8_t)s;
+    vals[rank] = (uint8_t)s;
   }
   __syncwarp();
   if (lane == 0) {                          // canonical codes, as Annex C assigns them
-    const bool ac = t & 1;
-    uint16_t* code = ac ? fh.c.ac_code[t >> 1] : fh.c.dc_code[t >> 1];
-    uint8_t* len = ac ? fh.c.ac_len[t >> 1] : fh.c.dc_len[t >> 1];
     int c = 0, k = 0;
     for (int l = 1; l <= 16; ++l) {
-      for (int i = 0; i < fh.s.bits[t][l - 1]; ++i, ++k, ++c) {
-        code[fh.s.vals[t][k]] = (uint16_t)c;
-        len[fh.s.vals[t][k]] = (uint8_t)l;
+      for (int i = 0; i < bits[l - 1]; ++i, ++k, ++c) {
+        code[vals[k]] = (uint16_t)c;
+        len[vals[k]] = (uint8_t)l;
       }
       c <<= 1;
     }
   }
+}
+
+// The optimal tables of frame blockIdx.x's four tables, warp t building table t.
+__global__ void __launch_bounds__(kTableThreads) table_kernel(const __grid_constant__ JpegParams p) {
+  __shared__ unsigned long long freq[4][257];
+  __shared__ int16_t size[4][257], others[4][257];
+  __shared__ int bits[4][33];
+  const int t = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  FrameHuff& fh = p.huff[blockIdx.x];
+  const bool ac = t & 1;
+  optimal_table(p.freq + ((int64_t)blockIdx.x * 4 + t) * 256, freq[t], size[t], others[t], bits[t],
+                fh.s.bits[t], fh.s.vals[t], &fh.s.count[t], ac ? fh.c.ac_code[t >> 1] : fh.c.dc_code[t >> 1],
+                ac ? fh.c.ac_len[t >> 1] : fh.c.dc_len[t >> 1], lane);
 }
 
 // ---- 2. code lengths and chunk sums -------------------------------------------------------------
@@ -653,14 +677,447 @@ __global__ void __launch_bounds__(kChunk) pack_kernel(const __grid_constant__ Jp
   w.flush();
 }
 
+// ---- progressive: ten scans ------------------------------------------------------------------------
+// jpeg_simple_progression for YCbCr, one 6-bit field per scan: Ss, Se, Ah, Al and the component (3:
+// all three, interleaved over the MCUs as the baseline scan is).
+constexpr uint64_t scan_fields(const int (&v)[kScans]) {
+  uint64_t r = 0;
+  for (int s = 0; s < kScans; ++s) r |= (uint64_t)v[s] << (6 * s);
+  return r;
+}
+constexpr uint64_t kScanSs = scan_fields({0, 1, 1, 1, 6, 1, 0, 1, 1, 1});
+constexpr uint64_t kScanSe = scan_fields({0, 5, 63, 63, 63, 63, 0, 63, 63, 63});
+constexpr uint64_t kScanAh = scan_fields({0, 0, 0, 0, 0, 2, 1, 1, 1, 1});
+constexpr uint64_t kScanAl = scan_fields({1, 2, 1, 1, 2, 1, 0, 0, 0, 0});
+constexpr uint64_t kScanComp = scan_fields({3, 0, 2, 1, 0, 0, 3, 2, 1, 0});
+__host__ __device__ __forceinline__ int scan_field(uint64_t f, int s) { return (int)(f >> (6 * s)) & 63; }
+constexpr int kEobrunMax = 0x7FFF;       // EOBRUN is emitted when it reaches this
+constexpr int kMaxBe = 1000 - 64 + 1;    // or when the buffered correction bits pass MAX_CORR_BITS - 64 + 1
+
+// The most bits one unit of scan s codes, with the EOBRUN flush after it (16 + 14 bits): a DC
+// difference of 16 + 11 bits; a refinement bit; 16 + 10 bits per first-scan coefficient (a ZRL
+// costs at most a bit per zero); 16 + 1 per newly nonzero refinement coefficient and 1 per other.
+__host__ __device__ inline int prog_max_unit_bits(int s) {
+  const int n = scan_field(kScanSe, s) - scan_field(kScanSs, s) + 1;
+  if (scan_field(kScanSs, s) == 0) return scan_field(kScanAh, s) ? 1 : 27;
+  return (scan_field(kScanAh, s) ? 17 : 26) * n + 30;
+}
+
+// A scan of an h x w frame: its units (the blocks it codes: every block of the MCUs for the DC
+// scans, the component's ceil(w_c / 8) x ceil(h_c / 8) blocks in raster order for the AC scans),
+// the frame's unit of its first (scans start at chunk boundaries), units per restart interval (all
+// of them without), its intervals and the frame's index of its first.
+struct ScanGeom {
+  int units, first, span, ints, iseg;
+};
+enum FindBy { kByScan, kByUnit, kByInterval };
+
+__host__ __device__ inline int scan_units(int h, int w, int hs, int vs, int s) {
+  const int mcus = ((h + 8 * vs - 1) / (8 * vs)) * ((w + 8 * hs - 1) / (8 * hs));
+  const int c = scan_field(kScanComp, s);
+  return c == 3 ? mcus * (hs * vs + 2) : c ? mcus : ((h + 7) >> 3) * ((w + 7) >> 3);
+}
+
+// The scan numbered i (kByScan), or holding the frame's unit (kByUnit) or interval (kByInterval) i,
+// and its geometry in q.  Scan kScans is the frame's end: q.first and q.iseg are its units (padded)
+// and intervals.
+__host__ __device__ __forceinline__ int find_scan(int h, int w, int hs, int vs, int rst, FindBy by, int i, ScanGeom& q) {
+  q = ScanGeom{0, 0, 0, 0, 0};
+  for (int k = 0;; ++k) {
+    q.units = k < kScans ? scan_units(h, w, hs, vs, k) : 0;
+    q.span = rst ? rst * (k < kScans && scan_field(kScanComp, k) == 3 ? hs * vs + 2 : 1) : (q.units ? q.units : 1);
+    q.ints = (q.units + q.span - 1) / q.span;
+    const int padded = (q.units + kChunk - 1) / kChunk * kChunk;
+    if (k == kScans || (by == kByScan ? k == i : by == kByUnit ? i < q.first + padded : i < q.iseg + q.ints)) return k;
+    q.first += padded;
+    q.iseg += q.ints;
+  }
+}
+__device__ __forceinline__ int find_scan(const JpegParams& p, const JpegGeom& g, FindBy by, int i, ScanGeom& q) {
+  return find_scan(g.h, g.w, p.hs, p.vs, p.rst, by, i, q);
+}
+
+// The block (stream order) of unit u of a scan of component c.
+__device__ __forceinline__ int unit_block(const JpegParams& p, const JpegGeom& g, int c, int u) {
+  if (c == 3) return u;
+  if (c) return u * p.per + p.luma + c - 1;
+  const int wib = (g.w + 7) >> 3, bx = u % wib, by = u / wib;
+  return ((by / p.vs) * g.mcu_cols + bx / p.hs) * p.per + (by % p.vs) * p.hs + bx % p.hs;
+}
+
+// The DC of block b: a dummy block's is the last real block's before it (its MCU's first luma block
+// is real), as libjpeg fills dummy blocks in for multi-scan files.
+__device__ __forceinline__ int eff_dc(const JpegParams& p, const JpegGeom& g, const int16_t* coef, int b) {
+  const int m = b / p.per;
+  int u = b - m * p.per;
+  while (dummy_block(p, g, m, u)) --u;
+  return coef[(int64_t)(m * p.per + u) * 64];
+}
+
+// What a unit leaves after its codes: whether it coded a symbol (so that a pending EOBRUN is
+// emitted before its codes), whether it adds one to EOBRUN, and its correction bits buffered behind
+// the run (refinement: the last `tail` bits of tail_bits).
+struct UnitEnd {
+  bool sym, eob;
+  int tail;
+  uint64_t tail_bits;
+};
+
+// Raw bits, at most 64, to f.
+template <class Fn>
+__device__ __forceinline__ void put_raw(Fn& f, uint64_t bits, int n) {
+  if (n > 32) f(-1, 0, (uint32_t)(bits >> 32), n - 32);
+  if (n) f(-1, 0, (uint32_t)bits, min(n, 32));
+}
+
+// The codes of unit u (the frame's index) of scan s (geometry q), in order, to f(slot, symbol,
+// extra bits, their length); slot -1: `extra` is raw bits.  EOBRUN flushes are not the unit's.
+template <class Fn>
+__device__ __forceinline__ UnitEnd unit_codes(const JpegParams& p, const JpegGeom& g, const int16_t* coef, int s,
+                              const ScanGeom& q, int u, Fn&& f) {
+  const int ss = scan_field(kScanSs, s), se = scan_field(kScanSe, s), ah = scan_field(kScanAh, s);
+  const int al = scan_field(kScanAl, s), c = scan_field(kScanComp, s);
+  const int local = u - q.first;
+  UnitEnd e{false, false, 0, 0};
+  if (ss == 0) {                          // DC: the point transform is an arithmetic shift
+    const int b = local, dc = eff_dc(p, g, coef, b) >> al;
+    if (ah) {
+      f(-1, 0, (uint32_t)dc & 1, 1);
+      return e;
+    }
+    const int m = b / p.per, k = b - m * p.per;
+    const int prev = k >= p.luma ? b - p.per : k ? b - 1 : b - p.per + p.luma - 1;
+    const int first = p.rst ? (m - m % p.rst) * p.per : 0;     // the interval's first block
+    const int diff = dc - (prev >= first ? eff_dc(p, g, coef, prev) >> al : 0), nb = nbits(diff);
+    f(k >= p.luma ? kChromaDcSlot : 0, nb, (uint32_t)(diff < 0 ? diff - 1 : diff) & ((1u << nb) - 1), nb);
+    e.sym = true;
+    return e;
+  }
+  const int16_t* z = coef + (int64_t)unit_block(p, g, c, local) * 64;
+  int run = 0;
+  if (!ah) {                              // AC first: |v| >> Al
+#pragma unroll 1
+    for (int k = ss; k <= se; ++k) {
+      const int v = z[kZigzagDev[k]], a = abs(v) >> al;
+      if (!a) {
+        ++run;
+        continue;
+      }
+      for (; run > 15; run -= 16) f(s, 0xF0, 0u, 0);
+      const int nb = nbits(a);
+      f(s, (run << 4) | nb, (uint32_t)(v < 0 ? ~a : a) & ((1u << nb) - 1), nb);
+      run = 0;
+      e.sym = true;
+    }
+    e.eob = run > 0;
+    return e;
+  }
+  // AC refinement: |v| >> Al == 1 is newly nonzero, larger values get a correction bit; runs count
+  // the coefficients still zero, and ZRLs past the last newly nonzero one fold into the EOB run
+  int eob = 0, br = 0;
+  uint64_t bb = 0;
+#pragma unroll 1
+  for (int k = ss; k <= se; ++k)
+    if ((abs(z[kZigzagDev[k]]) >> al) == 1) eob = k;
+#pragma unroll 1
+  for (int k = ss; k <= se; ++k) {
+    const int v = z[kZigzagDev[k]], a = abs(v) >> al;
+    if (!a) {
+      ++run;
+      continue;
+    }
+    for (; run > 15 && k <= eob; run -= 16) {
+      f(s, 0xF0, 0u, 0);
+      put_raw(f, bb, br);
+      bb = 0;
+      br = 0;
+      e.sym = true;
+    }
+    if (a > 1) {
+      bb = bb << 1 | (a & 1);
+      ++br;
+      continue;
+    }
+    f(s, (run << 4) | 1, (uint32_t)(v >= 0), 1);
+    put_raw(f, bb, br);
+    bb = 0;
+    br = run = 0;
+    e.sym = true;
+  }
+  e.eob = run > 0 || br > 0;
+  e.tail = br;
+  e.tail_bits = bb;
+  return e;
+}
+
+// The frame's tails (buffered correction bits) and symbol-coding units before unit k, from the
+// chunk sums at tsum (tails, then symbol units) and the in-chunk prefixes in pre.
+__device__ __forceinline__ int64_t tails_before(const JpegParams& p, const JpegGeom& g, int k) {
+  return p.sums[g.tsum + k / kChunk] + (k % kChunk ? p.pre[g.blk + k] & 0xFFFF : 0);
+}
+__device__ __forceinline__ int64_t syms_before(const JpegParams& p, const JpegGeom& g, int k) {
+  return p.sums[g.tsum + g.chunks + 1 + k / kChunk] + (k % kChunk ? p.pre[g.blk + k] >> 16 : 0);
+}
+
+// ---- P1. units: flags, prefixes, symbol counts -------------------------------------------------------
+// Grid (unit chunk, frame): each unit's UnitEnd as flags (sym | eob << 1 | tail << 2), the in-chunk
+// exclusive prefixes of tails and symbol units (pre: tails | syms << 16) and their chunk sums, and
+// the counts of the unit's own symbols.  A chunk lies in one scan, so it counts into at most two
+// tables (scan 0's DC luma and chroma).
+__global__ void __launch_bounds__(kChunk) prog_units_kernel(const __grid_constant__ JpegParams p) {
+  __shared__ uint32_t count[2][256];
+  __shared__ int64_t warp[32];
+  const JpegGeom& g = p.g[blockIdx.y];
+  if ((int)blockIdx.x >= g.chunks) return;
+  for (int i = threadIdx.x; i < 2 * 256; i += kChunk) count[i >> 8][i & 255] = 0;
+  __syncthreads();
+  const int u = blockIdx.x * kChunk + threadIdx.x;
+  ScanGeom q;
+  const int s = find_scan(p, g, kByUnit, u, q);
+  uint32_t flags = 0;
+  if (u - q.first < q.units) {
+    const UnitEnd e = unit_codes(p, g, p.coef + g.cblk * 64, s, q, u, [&](int slot, int sym, uint32_t, int) {
+      if (slot >= 0) atomicAdd(&count[slot == kChromaDcSlot][sym], 1u);
+    });
+    flags = (uint32_t)e.sym | (uint32_t)e.eob << 1 | (uint32_t)e.tail << 2;
+  }
+  p.flags[g.blk + u] = flags;
+  int64_t tails, syms;
+  const int64_t tb = block_exclusive_scan(flags >> 2, warp, &tails);
+  const int64_t sb = block_exclusive_scan(flags & 1, warp, &syms);
+  p.pre[g.blk + u] = (uint32_t)tb | (uint32_t)sb << 16;
+  if (threadIdx.x == 0) {
+    p.sums[g.tsum + blockIdx.x] = tails;
+    p.sums[g.tsum + g.chunks + 1 + blockIdx.x] = syms;
+  }
+  __syncthreads();
+  unsigned long long* freq = p.freq + (int64_t)blockIdx.y * kSlots * 256;
+  for (int i = threadIdx.x; i < 2 * 256; i += kChunk) {
+    const uint32_t n = count[i >> 8][i & 255];
+    if (n) atomicAdd(freq + (i >> 8 ? kChromaDcSlot : s) * 256 + (i & 255), (unsigned long long)n);
+  }
+}
+
+// ---- P2. EOBRUN flushes -------------------------------------------------------------------------------
+// A flush word: the EOBRUN emitted after a unit's codes and the correction bits buffered with it
+// (E | B << 15); 0 for none.  An AC scan's units that code a symbol, and each interval's first,
+// split it into segments whose other units code none.  The thread of the unit before a segment
+// (of its first unit, at an interval's start) walks it from flush to flush: each unit adds one
+// to EOBRUN and its tail to BE, a flush comes where EOBRUN reaches 0x7FFF (closed form) or BE
+// passes kMaxBe (a binary search on the tails' prefix sums), and the segment's end flushes what is
+// pending, before the next symbol or at the interval's end.  Its cost is its flushes.
+__global__ void __launch_bounds__(kChunk) prog_eobrun_kernel(const __grid_constant__ JpegParams p) {
+  __shared__ uint32_t count[256];
+  const JpegGeom& g = p.g[blockIdx.y];
+  if ((int)blockIdx.x >= g.chunks) return;
+  for (int i = threadIdx.x; i < 256; i += kChunk) count[i] = 0;
+  __syncthreads();
+  const int u = blockIdx.x * kChunk + threadIdx.x;
+  ScanGeom q;
+  const int s = find_scan(p, g, kByUnit, u, q);
+  const int local = u - q.first;
+  const uint32_t fl = local < q.units ? p.flags[g.blk + u] : 0;
+  if (scan_field(kScanSs, s) && local < q.units && ((fl & 1) || local % q.span == 0)) {
+    const int iend = q.first + min((local / q.span + 1) * q.span, q.units);
+    int E = 0, next = u;
+    int64_t B = 0;
+    if (fl & 1) {
+      E = (fl >> 1) & 1;
+      B = fl >> 2;
+      next = u + 1;
+    }
+    auto flush = [&](int k, int e, int64_t b) {
+      p.flush[g.blk + k] = (uint32_t)e | (uint32_t)b << 15;
+      atomicAdd(&count[(nbits(e) - 1) << 4], 1u);
+    };
+    // the segment's last unit: before the next unit coding a symbol, or the interval's last
+    const int64_t h0 = syms_before(p, g, u + 1);
+    int lo = u + 1, hi = iend;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (syms_before(p, g, mid + 1) > h0) hi = mid;
+      else lo = mid + 1;
+    }
+    const int e = lo - 1;
+    for (;;) {
+      const int64_t t0 = tails_before(p, g, next);
+      int k = next + (kEobrunMax - E) - 1;
+      if (B + tails_before(p, g, e + 1) - t0 > kMaxBe) {
+        int a = next, z = e;
+        while (a < z) {
+          const int mid = (a + z) >> 1;
+          if (B + tails_before(p, g, mid + 1) - t0 > kMaxBe) z = mid;
+          else a = mid + 1;
+        }
+        k = min(k, a);
+      }
+      if (k > e) break;
+      flush(k, E + k - next + 1, B + tails_before(p, g, k + 1) - t0);
+      E = 0;
+      B = 0;
+      next = k + 1;
+    }
+    E += e - next + 1;
+    if (E > 0) flush(e, E, B + tails_before(p, g, e + 1) - tails_before(p, g, next));
+  }
+  __syncthreads();
+  unsigned long long* freq = p.freq + ((int64_t)blockIdx.y * kSlots + s) * 256;
+  for (int i = threadIdx.x; i < 256; i += kChunk)
+    if (count[i]) atomicAdd(freq + i, (unsigned long long)count[i]);
+}
+
+// ---- P3. tables ---------------------------------------------------------------------------------------
+// Frame blockIdx.x's optimal tables, warp t building slot t's (none for the DC refinement).
+__global__ void __launch_bounds__(kSlots * 32) prog_table_kernel(const __grid_constant__ JpegParams p) {
+  __shared__ unsigned long long freq[kSlots][257];
+  __shared__ int16_t size[kSlots][257], others[kSlots][257];
+  __shared__ int bits[kSlots][33];
+  const int t = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (t == 6) return;
+  ProgHuff& h = p.phuff[blockIdx.x];
+  optimal_table(p.freq + ((int64_t)blockIdx.x * kSlots + t) * 256, freq[t], size[t], others[t], bits[t],
+                h.bits[t], h.vals[t], &h.count[t], h.code[t], h.len[t], lane);
+}
+
+// ---- P4. unit lengths and chunk sums -------------------------------------------------------------------
+// The bits of a flush word's EOBRUN code, its low bits and the buffered correction bits.
+__device__ __forceinline__ int flush_bits(const ProgHuff& h, int s, uint32_t fw) {
+  if (!fw) return 0;
+  const int nb = nbits((int)(fw & 0x7FFF)) - 1;
+  return h.len[s][nb << 4] + nb + (int)(fw >> 15);
+}
+
+__global__ void __launch_bounds__(kChunk) prog_bits_kernel(const __grid_constant__ JpegParams p) {
+  __shared__ int64_t warp[32];
+  const JpegGeom& g = p.g[blockIdx.y];
+  if ((int)blockIdx.x >= g.chunks) return;
+  const int u = blockIdx.x * kChunk + threadIdx.x;
+  ScanGeom q;
+  const int s = find_scan(p, g, kByUnit, u, q);
+  const ProgHuff& h = p.phuff[blockIdx.y];
+  int bits = 0;
+  if (u - q.first < q.units) {
+    unit_codes(p, g, p.coef + g.cblk * 64, s, q, u,
+               [&](int slot, int sym, uint32_t, int nb) { bits += (slot >= 0 ? h.len[slot][sym] : 0) + nb; });
+    bits += flush_bits(h, s, p.flush[g.blk + u]);
+  }
+  p.bits[g.blk + u] = (uint32_t)bits;
+  int64_t total;
+  block_exclusive_scan(bits, warp, &total);
+  if (threadIdx.x == 0) p.sums[g.csum + blockIdx.x] = total;
+}
+
+// ---- P5. intervals: one per restart interval of each scan (one per scan without) ------------------------
+__global__ void __launch_bounds__(kChunk) prog_interval_kernel(const __grid_constant__ JpegParams p) {
+  const JpegGeom& g = p.g[blockIdx.y];
+  const int i = blockIdx.x * kChunk + threadIdx.x;
+  if (i >= g.ints) return;
+  ScanGeom q;
+  find_scan(p, g, kByInterval, i, q);
+  const int j = i - q.iseg;
+  const int first = q.first + j * q.span, end = q.first + min((j + 1) * q.span, q.units);
+  const int64_t a = block_first_bit(p, g, first), e = block_first_bit(p, g, end);
+  p.ipos[g.ipos + i] = a;
+  p.sums[g.isum + i] = (e - a + 7) >> 3;
+}
+
+// ---- P6. pack --------------------------------------------------------------------------------------------
+// Each unit ORs in its codes, then its flush: the EOBRUN code and the tails of the run's units (the
+// last E units, each adding one), found by binary search on the tails' prefix sums; the last unit
+// of an interval pads it to a byte with 1-bits.
+// A unit's codes with the frame's tables (slot -1: raw bits) into a BitWriter.
+struct CodeWriter {
+  BitWriter w;
+  const ProgHuff& h;
+  __device__ __forceinline__ void operator()(int slot, int sym, uint32_t extra, int nb) {
+    if (slot >= 0) w.put(h.code[slot][sym], h.len[slot][sym]);
+    if (nb) w.put(extra, nb);
+  }
+};
+
+__global__ void __launch_bounds__(kChunk) prog_pack_kernel(const __grid_constant__ JpegParams p) {
+  __shared__ int64_t warp[32];
+  const JpegGeom& g = p.g[blockIdx.y];
+  if ((int)blockIdx.x >= g.chunks) return;
+  const int u = blockIdx.x * kChunk + threadIdx.x;
+  const int64_t bits = p.bits[g.blk + u];
+  int64_t total;
+  int64_t pos = p.sums[g.csum + blockIdx.x] + block_exclusive_scan(bits, warp, &total);
+  ScanGeom q;
+  const int s = find_scan(p, g, kByUnit, u, q);
+  const int local = u - q.first;
+  if (local >= q.units) return;
+  const int i = q.iseg + local / q.span;
+  pos += 8 * p.sums[g.isum + i] - p.ipos[g.ipos + i];
+  const bool last = local + 1 == q.units || (local + 1) % q.span == 0;
+  const ProgHuff& h = p.phuff[blockIdx.y];
+  const int16_t* coef = p.coef + g.cblk * 64;
+  CodeWriter put{{p.stream + g.words + (pos >> 5), 0, (int)(pos & 31)}, h};
+  unit_codes(p, g, coef, s, q, u, put);
+  const uint32_t fw = p.flush[g.blk + u];
+  if (fw) {
+    const int E = (int)(fw & 0x7FFF), nb = nbits(E) - 1;
+    put(s, nb << 4, (uint32_t)E & ((1u << nb) - 1), nb);
+    const int64_t end = tails_before(p, g, u + 1);
+    for (int k = u - E + 1; k <= u;) {
+      const int64_t t = tails_before(p, g, k);
+      if (t == end) break;
+      int lo = k, hi = u;                 // the first unit from k on with a tail
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (tails_before(p, g, mid + 1) > t) hi = mid;
+        else lo = mid + 1;
+      }
+      // its tail: the correction bits after its last newly nonzero coefficient (no code follows it)
+      const int16_t* z = coef + (int64_t)unit_block(p, g, scan_field(kScanComp, s), lo - q.first) * 64;
+      const int ss = scan_field(kScanSs, s), se = scan_field(kScanSe, s), al = scan_field(kScanAl, s);
+      int eob = 0;
+#pragma unroll 1
+      for (int j = ss; j <= se; ++j)
+        if ((abs(z[kZigzagDev[j]]) >> al) == 1) eob = j;
+#pragma unroll 1
+      for (int j = max(eob + 1, ss); j <= se; ++j) {
+        const int a = abs(z[kZigzagDev[j]]) >> al;
+        if (a > 1) put(-1, 0, (uint32_t)a & 1, 1);
+      }
+      k = lo + 1;
+    }
+  }
+  if (last) {                               // 1-bits to the byte boundary
+    const int pad = (int)(-(pos + bits) & 7);
+    if (pad) put.w.put((1u << pad) - 1, pad);
+  }
+  put.w.flush();
+}
+
+// ---- P7. markers between intervals ---------------------------------------------------------------------
+// A DHT segment of slot t's table as class/id `id`, byte i.
+__device__ __forceinline__ uint8_t dht_byte(const ProgHuff& h, int t, int id, int i) {
+  if (i < 2) return i ? 0xC4 : 0xFF;
+  const int len = 19 + h.count[t];
+  if (i < 4) return (uint8_t)(i == 2 ? len >> 8 : len);
+  if (i == 4) return (uint8_t)id;
+  return i < 21 ? h.bits[t][i - 5] : h.vals[t][i - 21];
+}
+
+// The bytes before interval i >= 1 of a progressive frame: RSTn within a scan, and at a scan's start
+// its DHT (AC scans) and SOS.
+__device__ __forceinline__ int prog_marker_bytes(const JpegParams& p, const JpegGeom& g, int i) {
+  ScanGeom q;
+  const int s = find_scan(p, g, kByInterval, i, q);
+  if (i > q.iseg) return 2;
+  return scan_field(kScanSs, s) ? 21 + p.phuff[blockIdx.y].count[s] + 10 : 14;
+}
+
 // ---- 5. 0xFF counts -----------------------------------------------------------------------------
 __device__ __forceinline__ uint8_t stream_byte(const uint32_t* words, int64_t j) {
   return (uint8_t)(words[j >> 2] >> (24 - 8 * (j & 3)));
 }
 
-// The bytes of the frame's stream before stuffing.
+// The bytes of the frame's stream before stuffing (progressive files always have intervals).
+template <bool kProg>
 __device__ __forceinline__ int64_t stream_bytes(const JpegParams& p, const JpegGeom& g) {
-  return p.rst ? p.sums[g.isum + g.ints] : (p.sums[g.csum + g.chunks] + 7) >> 3;
+  return kProg || p.rst ? p.sums[g.isum + g.ints] : (p.sums[g.csum + g.chunks] + 7) >> 3;
 }
 
 // The first interval after the first (which has no marker) starting at byte `first` or later.
@@ -674,17 +1131,19 @@ __device__ int first_marker(const JpegParams& p, const JpegGeom& g, int64_t firs
   return lo;
 }
 
+template <bool kProg>
 __global__ void __launch_bounds__(kStuffThreads) count_ff_kernel(const __grid_constant__ JpegParams p) {
   __shared__ int64_t warp[32];
   const JpegGeom& g = p.g[blockIdx.y];
   if ((int)blockIdx.x >= g.schunks) return;
-  const int64_t bytes = stream_bytes(p, g);
+  const int64_t bytes = stream_bytes<kProg>(p, g);
   const int64_t first = (int64_t)blockIdx.x * kStuffChunk + threadIdx.x * kStuffBytes;
   const uint32_t* words = p.stream + g.words;
   int ff = 0;
   for (int i = 0; i < kStuffBytes && first + i < bytes; ++i) ff += stream_byte(words, first + i) == 0xFF;
-  if (p.rst && first < bytes)               // RSTn: 2 bytes before an interval's first byte
-    for (int i = first_marker(p, g, first); i < g.ints && p.sums[g.isum + i] < first + kStuffBytes; ++i) ff += 2;
+  if ((kProg || p.rst) && first < bytes)    // RSTn: 2 bytes before an interval's first byte
+    for (int i = first_marker(p, g, first); i < g.ints && p.sums[g.isum + i] < first + kStuffBytes; ++i)
+      ff += kProg ? prog_marker_bytes(p, g, i) : 2;
   int64_t total;
   block_exclusive_scan(ff, warp, &total);
   if (threadIdx.x == 0) p.sums[g.ssum + blockIdx.x] = total;
@@ -693,7 +1152,7 @@ __global__ void __launch_bounds__(kStuffThreads) count_ff_kernel(const __grid_co
 // ---- 7. stuff, header, EOI, length --------------------------------------------------------------
 // Byte i of the frame's header: the template's SOI .. SOF0 with the frame's height and width, the
 // four DHT segments of `hs`, then the template's DRI and SOS.
-__device__ uint8_t header_byte(const StuffParams& sp, const JpegGeom& g, const HuffSpec& hs, int i) {
+__device__ __forceinline__ uint8_t header_byte(const StuffParams& sp, const JpegGeom& g, const HuffSpec& hs, int i) {
   if (i < kPrefixBytes) {
     if (i < kSofSize || i >= kSofSize + 4) return sp.prefix[i];
     const int v = i < kSofSize + 2 ? g.h : g.w;
@@ -713,15 +1172,50 @@ __device__ uint8_t header_byte(const StuffParams& sp, const JpegGeom& g, const H
   return sp.suffix[i];
 }
 
-template <bool kOpt>
+// A progressive file's header: the template's SOI .. SOF2, scan 0's two DHT segments, the
+// template's DRI and scan 0's SOS.
+__device__ __forceinline__ uint8_t prog_header_byte(const StuffParams& sp, const JpegGeom& g, const ProgHuff& h, int i) {
+  if (i < kPrefixBytes) return header_byte(sp, g, sp.std, i);
+  i -= kPrefixBytes;
+  for (int t = 0; t < 2; ++t) {
+    const int len = 21 + h.count[t ? kChromaDcSlot : 0];
+    if (i < len) return dht_byte(h, t ? kChromaDcSlot : 0, t, i);
+    i -= len;
+  }
+  return i < sp.suffix_bytes ? sp.suffix[i] : sp.sos[0][i - sp.suffix_bytes];
+}
+
+// Writes the bytes before interval i >= 1 of a progressive frame at out + o; returns the new o.
+__device__ __forceinline__ int64_t put_prog_marker(const StuffParams& sp, const JpegGeom& g, int i, int64_t o) {
+  ScanGeom q;
+  const int s = find_scan(sp.p, g, kByInterval, i, q);
+  if (i > q.iseg) {
+    g.out[o++] = 0xFF;
+    g.out[o++] = (uint8_t)(0xD0 + ((i - q.iseg - 1) & 7));
+    return o;
+  }
+  const int ss = scan_field(kScanSs, s);
+  if (ss) {
+    const ProgHuff& h = sp.p.phuff[blockIdx.y];
+    const int id = 0x10 | (scan_field(kScanComp, s) ? 1 : 0);
+    for (int k = 0; k < 21 + h.count[s]; ++k) g.out[o++] = dht_byte(h, s, id, k);
+  }
+  for (int k = 0; k < (ss ? 10 : 14); ++k) g.out[o++] = sp.sos[s][k];
+  return o;
+}
+
+template <bool kOpt, bool kProg = false>
 __global__ void __launch_bounds__(kStuffThreads) stuff_kernel(const __grid_constant__ StuffParams sp) {
   __shared__ int64_t warp[32];
   const JpegParams& p = sp.p;
   const JpegGeom& g = p.g[blockIdx.y];
   if ((int)blockIdx.x >= g.schunks) return;
   const HuffSpec& hs = kOpt ? p.huff[blockIdx.y].s : sp.std;
-  const int header = kPrefixBytes + 84 + hs.count[0] + hs.count[1] + hs.count[2] + hs.count[3] + sp.suffix_bytes;
-  const int64_t bytes = stream_bytes(p, g);
+  int header = kPrefixBytes + 84 + hs.count[0] + hs.count[1] + hs.count[2] + hs.count[3] + sp.suffix_bytes;
+  if constexpr (kProg)
+    header = kPrefixBytes + 42 + p.phuff[blockIdx.y].count[0] + p.phuff[blockIdx.y].count[kChromaDcSlot] +
+             sp.suffix_bytes + kSosBytes;
+  const int64_t bytes = stream_bytes<kProg>(p, g);
   const int64_t size = header + bytes + p.sums[g.ssum + g.schunks] + 2;
   if (blockIdx.x == 0 && threadIdx.x == 0) *g.length = size <= p.cap ? size : -1;
   if (size > p.cap) return;
@@ -735,23 +1229,32 @@ __global__ void __launch_bounds__(kStuffThreads) stuff_kernel(const __grid_const
     ff += first + i < bytes && v[i] == 0xFF;
   }
   int marker = g.ints;
-  if (p.rst && first < bytes) {
+  if ((kProg || p.rst) && first < bytes) {
     marker = first_marker(p, g, first);
-    for (int i = marker; i < g.ints && p.sums[g.isum + i] < first + kStuffBytes; ++i) ff += 2;
+    for (int i = marker; i < g.ints && p.sums[g.isum + i] < first + kStuffBytes; ++i)
+      ff += kProg ? prog_marker_bytes(p, g, i) : 2;
   }
   int64_t total;
   int64_t o = header + first + p.sums[g.ssum + blockIdx.x] + block_exclusive_scan(ff, warp, &total);
   for (int i = 0; i < kStuffBytes && first + i < bytes; ++i) {
     if (marker < g.ints && p.sums[g.isum + marker] == first + i) {
-      g.out[o++] = 0xFF;
-      g.out[o++] = (uint8_t)(0xD0 + ((marker - 1) & 7));
+      if constexpr (kProg) {
+        o = put_prog_marker(sp, g, marker, o);
+      } else {
+        g.out[o++] = 0xFF;
+        g.out[o++] = (uint8_t)(0xD0 + ((marker - 1) & 7));
+      }
       ++marker;
     }
-    g.out[o++] = v[i];
-    if (v[i] == 0xFF) g.out[o++] = 0;
+    // (progressive: the marker writes keep this loop rolled, so the byte is read again rather than
+    // indexing v, which would put v in local memory)
+    const uint8_t b = kProg ? stream_byte(words, first + i) : v[i];
+    g.out[o++] = b;
+    if (b == 0xFF) g.out[o++] = 0;
   }
   if (blockIdx.x == 0) {
-    for (int i = threadIdx.x; i < header; i += kStuffThreads) g.out[i] = header_byte(sp, g, hs, i);
+    for (int i = threadIdx.x; i < header; i += kStuffThreads)
+      g.out[i] = kProg ? prog_header_byte(sp, g, p.phuff[blockIdx.y], i) : header_byte(sp, g, hs, i);
     if (threadIdx.x == 0) {
       g.out[size - 2] = 0xFF;
       g.out[size - 1] = 0xD9;
@@ -761,11 +1264,11 @@ __global__ void __launch_bounds__(kStuffThreads) stuff_kernel(const __grid_const
 
 // ---- host side -----------------------------------------------------------------------------------
 // What one call encodes with (cv2's parameters resolved): the luma and chroma qualities, the luma
-// sampling factors, optimized tables or not, and the restart interval in MCUs.
+// sampling factors, optimized tables or not, the restart interval in MCUs, and progressive or not.
 struct Settings {
-  int lq, cq, hs, vs, optimize, rst;
+  int lq, cq, hs, vs, optimize, rst, prog;
 };
-constexpr Settings kDefaultSettings = {95, 95, 2, 2, 0, 0};
+constexpr Settings kDefaultSettings = {95, 95, 2, 2, 0, 0, 0};
 
 // The parameters' settings, or a refusal naming the call: a quality outside [1, 100] (-1 leaves
 // luma_quality and chroma_quality unset), a sampling other than cv2's five, optimize other than 0
@@ -793,11 +1296,13 @@ int resolve_params(const std::string& name, const sqdet_jpeg_params* jp, Setting
   }
   s->optimize = jp->optimize;
   s->rst = jp->restart_interval;
+  s->prog = 0;
   return SQDET_OK;
 }
 
-// The header's template: SOI, JFIF APP0, DQT x 2 and SOF0 (height and width 0) into prefix, DRI
-// (with restart markers) and SOS into suffix; returns the suffix's bytes.
+// The header's template: SOI, JFIF APP0, DQT x 2 and SOF0 (progressive: SOF2; height and width 0)
+// into prefix, DRI (with restart markers) and (baseline only) SOS into suffix; returns the suffix's
+// bytes.
 int jpeg_header(const uint16_t (&q)[2][64], const Settings& st, uint8_t* prefix, uint8_t* suffix) {
   uint8_t* out = prefix;
   int n = 0;
@@ -811,7 +1316,7 @@ int jpeg_header(const uint16_t (&q)[2][64], const Settings& st, uint8_t* prefix,
     put({t});
     for (int k = 0; k < 64; ++k) out[n++] = (uint8_t)q[t][kZigzag[k]];
   }
-  seg(0xC0, 15);                          // height and width at kSofSize, filled in per frame
+  seg(st.prog ? 0xC2 : 0xC0, 15);         // height and width at kSofSize, filled in per frame
   put({8, 0, 0, 0, 0, 3, 1, st.hs << 4 | st.vs, 0, 2, 0x11, 1, 3, 0x11, 1});
   out = suffix;
   n = 0;
@@ -819,9 +1324,29 @@ int jpeg_header(const uint16_t (&q)[2][64], const Settings& st, uint8_t* prefix,
     seg(0xDD, 2);
     put({st.rst >> 8, st.rst & 255});
   }
+  if (st.prog) return n;
   seg(0xDA, 10);
   put({3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0});
   return n;
+}
+
+// Each progressive scan's SOS: its components with their tables (DC first: the DC tables; AC: the
+// component's AC table; 0 for a table the scan does not use), Ss, Se, Ah << 4 | Al.
+void prog_sos(uint8_t (&sos)[kScans][kSosBytes]) {
+  for (int s = 0; s < kScans; ++s) {
+    const int c = scan_field(kScanComp, s), ss = scan_field(kScanSs, s), n = c == 3 ? 3 : 1;
+    uint8_t* o = sos[s];
+    int k = 0;
+    for (int v : {0xFF, 0xDA, 0, 6 + 2 * n, n}) o[k++] = (uint8_t)v;
+    for (int i = 0; i < n; ++i) {
+      const int comp = c == 3 ? i : c;
+      o[k++] = (uint8_t)(comp + 1);
+      o[k++] = (uint8_t)(ss ? (comp ? 0x01 : 0x00) : scan_field(kScanAh, s) || !comp ? 0x00 : 0x10);
+    }
+    o[k++] = (uint8_t)ss;
+    o[k++] = (uint8_t)scan_field(kScanSe, s);
+    o[k++] = (uint8_t)(scan_field(kScanAh, s) << 4 | scan_field(kScanAl, s));
+  }
 }
 
 // The Annex K tables as DHT writes them.
@@ -838,9 +1363,10 @@ HuffSpec std_spec() {
   return h;
 }
 
-// One frame's sizes in the scratch.
+// One frame's sizes in the scratch.  A progressive frame codes units, the blocks of each of its
+// scans (ScanGeom), in uchunks chunks; its ints are the intervals of all its scans.
 struct FrameSizes {
-  int blocks, chunks, schunks, ints;
+  int blocks, chunks, schunks, ints, uchunks;
   int64_t bytes, words;                 // the stream's largest bytes before stuffing, its words
 };
 FrameSizes frame_sizes(int h, int w, const Settings& st) {
@@ -849,8 +1375,20 @@ FrameSizes frame_sizes(int h, int w, const Settings& st) {
   s.blocks = (int)(mcus * (st.hs * st.vs + 2));
   s.chunks = (s.blocks + kChunk - 1) / kChunk;
   s.ints = st.rst ? (int)((mcus + st.rst - 1) / st.rst) : 1;
+  s.uchunks = s.chunks;
   // each interval is padded to a byte
   s.bytes = ((int64_t)s.blocks * (st.optimize ? kMaxBlockBitsOpt : kMaxBlockBits) + 7) / 8 + (st.rst ? s.ints : 0);
+  if (st.prog) {
+    ScanGeom q;
+    s.bytes = 0;
+    for (int k = 0; k < kScans; ++k) {
+      find_scan(h, w, st.hs, st.vs, st.rst, kByScan, k, q);
+      s.bytes += ((int64_t)q.units * prog_max_unit_bits(k) + 7) / 8 + q.ints;
+    }
+    find_scan(h, w, st.hs, st.vs, st.rst, kByScan, kScans, q);
+    s.uchunks = q.first / kChunk;
+    s.ints = q.iseg;
+  }
   s.schunks = (int)((s.bytes + kStuffChunk - 1) / kStuffChunk);
   s.words = (s.bytes + 3) / 4 + 1;
   return s;
@@ -858,16 +1396,35 @@ FrameSizes frame_sizes(int h, int w, const Settings& st) {
 
 // The scratch of the frames [first, first + count): coefficients, bit lengths, chunk sums,
 // intervals' first bits, bit buffers, symbol counts and tables, in that order.
+// A progressive frame's unit lengths, flags, prefixes and flush words follow the bit lengths, and
+// its tail and symbol-unit chunk sums the interval sums; g then describes the frame's units (blk,
+// blocks and chunks count units) and cblk its first block.
 struct GroupLayout {
-  int64_t coef, bits, sums, ipos, stream, freq, huff, total;
+  int64_t coef, bits, flags, pre, sums, ipos, flush, stream, freq, huff, total;
 };
 GroupLayout group_layout(const FrameSource* fr, int first, int count, const Settings& st, JpegGeom* g) {
-  int64_t blocks = 0, sums = 0, ints = 0, words = 0;
+  int64_t blocks = 0, units = 0, sums = 0, ints = 0, words = 0;
   for (int i = 0; i < count; ++i) {
     const FrameSource& s = fr[first + i];
     const FrameSizes z = frame_sizes(s.h, s.w, st);
-    const int isums = st.rst ? z.ints + 1 : 0;
-    if (g) {
+    const int isums = st.rst || st.prog ? z.ints + 1 : 0;
+    if (g && st.prog) {
+      g[i].h = s.h;
+      g[i].w = s.w;
+      g[i].mcu_cols = (s.w + 8 * st.hs - 1) / (8 * st.hs);
+      g[i].blocks = z.uchunks * kChunk;
+      g[i].chunks = z.uchunks;
+      g[i].schunks = z.schunks;
+      g[i].ints = z.ints;
+      g[i].blk = units;
+      g[i].cblk = blocks;
+      g[i].csum = sums;
+      g[i].ssum = sums + z.uchunks + 1;
+      g[i].isum = sums + z.uchunks + 1 + z.schunks + 1;
+      g[i].tsum = g[i].isum + isums;
+      g[i].ipos = ints;
+      g[i].words = words;
+    } else if (g) {
       g[i].h = s.h;
       g[i].w = s.w;
       g[i].mcu_cols = (s.w + 8 * st.hs - 1) / (8 * st.hs);
@@ -883,20 +1440,65 @@ GroupLayout group_layout(const FrameSource* fr, int first, int count, const Sett
       g[i].words = words;
     }
     blocks += (int64_t)z.chunks * kChunk;
-    sums += z.chunks + 1 + z.schunks + 1 + isums;
-    ints += st.rst ? z.ints : 0;
+    units += (int64_t)z.uchunks * kChunk;
+    sums += z.uchunks + 1 + z.schunks + 1 + isums + (st.prog ? 2 * (z.uchunks + 1) : 0);
+    ints += st.rst || st.prog ? z.ints : 0;
     words += z.words;
   }
+  const int64_t unit_words = st.prog ? align256(units * 4) : 0;
   GroupLayout L;
   L.coef = 0;
   L.bits = L.coef + align256(blocks * 64 * 2);
-  L.sums = L.bits + align256(blocks * 4);
+  L.flags = L.bits + align256(units * 4);
+  L.pre = L.flags + unit_words;
+  L.sums = L.pre + unit_words;
   L.ipos = L.sums + align256(sums * 8);
-  L.stream = L.ipos + align256(ints * 8);
+  L.flush = L.ipos + align256(ints * 8);
+  L.stream = L.flush + unit_words;
   L.freq = L.stream + align256(words * 4);
-  L.huff = L.freq + (st.optimize ? align256((int64_t)count * 4 * 256 * 8) : 0);
-  L.total = L.huff + (st.optimize ? align256((int64_t)count * sizeof(FrameHuff)) : 0);
+  L.huff = L.freq + (st.prog ? align256((int64_t)count * kSlots * 256 * 8)
+                             : st.optimize ? align256((int64_t)count * 4 * 256 * 8) : 0);
+  L.total = L.huff + (st.prog ? align256((int64_t)count * sizeof(ProgHuff))
+                              : st.optimize ? align256((int64_t)count * sizeof(FrameHuff)) : 0);
   return L;
+}
+
+// After the transform, a progressive group's ten scans: every launch runs all of them for every frame,
+// its grid over (unit chunk, frame) or (interval block, frame).  p describes the units.
+int launch_progressive(const JpegParams& p, const StuffParams& templ, int max_uchunks, int max_schunks,
+                       int max_ints, int count, cudaStream_t stream) {
+  const dim3 grid((unsigned)max_uchunks, (unsigned)count), sgrid((unsigned)max_schunks, (unsigned)count);
+  prog_units_kernel<<<grid, kChunk, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg prog_units_kernel");
+  JpegParams sums = p;                    // the tails' and then the symbol units' chunk sums
+  for (int k = 0; k < 2; ++k) {
+    for (int i = 0; i < count; ++i) sums.g[i].csum = p.g[i].tsum + k * (p.g[i].chunks + 1);
+    scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(sums, kScanBlocks);
+    SQ_CHECK_LAUNCH("jpeg scan_kernel");
+  }
+  prog_eobrun_kernel<<<grid, kChunk, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg prog_eobrun_kernel");
+  prog_table_kernel<<<(unsigned)count, kSlots * 32, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg prog_table_kernel");
+  prog_bits_kernel<<<grid, kChunk, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg prog_bits_kernel");
+  scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(p, kScanBlocks);
+  SQ_CHECK_LAUNCH("jpeg scan_kernel");
+  prog_interval_kernel<<<dim3((unsigned)((max_ints + kChunk - 1) / kChunk), (unsigned)count), kChunk, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg prog_interval_kernel");
+  scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(p, kScanIntervals);
+  SQ_CHECK_LAUNCH("jpeg scan_kernel");
+  prog_pack_kernel<<<grid, kChunk, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg prog_pack_kernel");
+  count_ff_kernel<true><<<sgrid, kStuffThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg count_ff_kernel");
+  scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(p, kScanStuffing);
+  SQ_CHECK_LAUNCH("jpeg scan_kernel");
+  StuffParams sp = templ;
+  sp.p = p;
+  stuff_kernel<false, true><<<sgrid, kStuffThreads, 0, stream>>>(sp);
+  SQ_CHECK_LAUNCH("jpeg stuff_kernel");
+  return SQDET_OK;
 }
 
 template <int F, int HS, int VS>
@@ -927,6 +1529,10 @@ int launch_group(const PixFormat& pf, const FrameSource* fr, int first, int coun
   p.stream = reinterpret_cast<uint32_t*>(scratch + L.stream);
   p.freq = reinterpret_cast<unsigned long long*>(scratch + L.freq);
   p.huff = reinterpret_cast<FrameHuff*>(scratch + L.huff);
+  p.flags = reinterpret_cast<uint32_t*>(scratch + L.flags);
+  p.pre = reinterpret_cast<uint32_t*>(scratch + L.pre);
+  p.flush = reinterpret_cast<uint32_t*>(scratch + L.flush);
+  p.phuff = reinterpret_cast<ProgHuff*>(scratch + L.huff);
   p.cap = cap;
   p.hs = st.hs;
   p.vs = st.vs;
@@ -934,8 +1540,21 @@ int launch_group(const PixFormat& pf, const FrameSource* fr, int first, int coun
   p.per = p.luma + 2;
   p.rst = st.rst;
   tp.quant = quant;
-  // the bit buffers and the symbol counts
-  SQ_CUDA(cudaMemsetAsync(p.stream, 0, (size_t)(L.huff - L.stream), stream));
+  // progressive: p describes the units and tp.p the blocks the transform writes
+  const JpegParams up = p;
+  const int max_uchunks = max_chunks;
+  if (st.prog) {
+    max_chunks = 0;
+    for (int i = 0; i < count; ++i) {
+      const FrameSizes z = frame_sizes(p.g[i].h, p.g[i].w, st);
+      p.g[i].blk = p.g[i].cblk;
+      p.g[i].blocks = z.blocks;
+      p.g[i].chunks = z.chunks;
+      max_chunks = std::max(max_chunks, z.chunks);
+    }
+  }
+  // the bit buffers, the symbol counts and (progressive) the flush words
+  SQ_CUDA(cudaMemsetAsync(scratch + L.flush, 0, (size_t)(L.huff - L.flush), stream));
   const dim3 grid((unsigned)max_chunks, (unsigned)count), sgrid((unsigned)max_schunks, (unsigned)count);
   switch (st.hs * 16 + st.vs) {
     case 0x41: launch_transform<F, 4, 1>(grid, tp, stream); break;
@@ -945,6 +1564,7 @@ int launch_group(const PixFormat& pf, const FrameSource* fr, int first, int coun
     default: launch_transform<F, 2, 2>(grid, tp, stream);
   }
   SQ_CHECK_LAUNCH("jpeg transform_kernel");
+  if (st.prog) return launch_progressive(up, templ, max_uchunks, max_schunks, max_ints, count, stream);
   if (st.optimize) {
     hist_kernel<<<grid, kChunk, 0, stream>>>(p);
     SQ_CHECK_LAUNCH("jpeg hist_kernel");
@@ -966,7 +1586,7 @@ int launch_group(const PixFormat& pf, const FrameSource* fr, int first, int coun
   if (st.optimize) pack_kernel<true><<<grid, kChunk, 0, stream>>>(p);
   else pack_kernel<false><<<grid, kChunk, 0, stream>>>(p);
   SQ_CHECK_LAUNCH("jpeg pack_kernel");
-  count_ff_kernel<<<sgrid, kStuffThreads, 0, stream>>>(p);
+  count_ff_kernel<false><<<sgrid, kStuffThreads, 0, stream>>>(p);
   SQ_CHECK_LAUNCH("jpeg count_ff_kernel");
   scan_kernel<<<(unsigned)count, kScanThreads, 0, stream>>>(p, kScanStuffing);
   SQ_CHECK_LAUNCH("jpeg scan_kernel");
@@ -978,9 +1598,18 @@ int launch_group(const PixFormat& pf, const FrameSource* fr, int first, int coun
   return SQDET_OK;
 }
 
+// The largest progressive header and scan preambles: SOI .. SOF2, ten DHT segments of at most 256
+// symbols (two before scan 0, one before each AC scan), two SOS of three components and eight of
+// one.
+constexpr int kProgHeaderBytes = kPrefixBytes + kScans * (21 + 256) + 2 * kSosBytes + 8 * (kSosBytes - 4);
+
 // The largest file of an h x w crop.
 int64_t jpeg_max_bytes(int h, int w, const Settings& st) {
   const FrameSizes s = frame_sizes(h, w, st);
+  // progressive: the headers, every scan's longest units with every interval padded, every byte
+  // stuffed, RSTn between the intervals of a scan, EOI
+  if (st.prog)
+    return kProgHeaderBytes + (st.rst ? kDriBytes : 0) + 2 * s.bytes + 2 * (int64_t)(s.ints - kScans) + 2;
   // the header (optimized tables are no longer than Annex K's), the stream with every byte
   // stuffed, RSTn between intervals, EOI
   return kHeaderBytes + (st.rst ? kDriBytes : 0) + 2 * s.bytes + 2 * (int64_t)(s.ints - 1) + 2;
@@ -1032,6 +1661,7 @@ int launch_encode_jpeg(int format, const PixFormat& pf, const FrameSource* frame
   StuffParams sp{};
   sp.std = std_spec();
   sp.suffix_bytes = jpeg_header(q, st, sp.prefix, sp.suffix);
+  if (st.prog) prog_sos(sp.sos);
   uint8_t* s = static_cast<uint8_t*>(scratch);
   return for_each_group(n, [&](int first, int count) {
     return dispatch_format(format, [&](auto f) {
@@ -1051,14 +1681,62 @@ sqdet_jpeg_params default_params(int quality) {
 
 using namespace sqdet;
 
-int64_t sqdet_jpeg_max_bytes_params(int h, int w, const sqdet_jpeg_params* params) {
+namespace sqdet {
+namespace {
+
+// The three entry points of baseline (prog 0) or progressive (prog 1) files.
+int64_t max_bytes_entry(int h, int w, const sqdet_jpeg_params* params, int prog) {
+  const std::string name = prog ? "sqdet_jpeg_max_bytes_progressive" : "sqdet_jpeg_max_bytes";
   Settings st;
-  if (resolve_params("sqdet_jpeg_max_bytes", params, &st)) return -1;
+  if (resolve_params(name, params, &st)) return -1;
+  st.prog = prog;
   if (h < 1 || w < 1 || h > kJpegMaxSide || w > kJpegMaxSide) {
-    fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_max_bytes: h and w must be in [1, 65500]");
+    fail(SQDET_ERR_INVALID_ARG, name + ": h and w must be in [1, 65500]");
     return -1;
   }
   return jpeg_max_bytes(h, w, st);
+}
+
+int64_t scratch_bytes_entry(int n, const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                            const sqdet_jpeg_params* params, int prog) {
+  const Encoder& enc = prog ? kJpegProg : kJpeg;
+  std::vector<FrameSource> fr;
+  Settings st;
+  if (resolve_params(enc.scratch_call, params, &st)) return -1;
+  st.prog = prog;
+  if (encode_crops(enc.scratch_call, enc, n, heights, widths, crops, fr)) return -1;
+  return jpeg_scratch_bytes(fr.data(), n, st);
+}
+
+int encode_entry(int n, int format, const uint8_t* const* planes, const int64_t* pitches, const int32_t* heights,
+                 const int32_t* widths, const int32_t* crops, const sqdet_jpeg_params* params, uint8_t* out_dev,
+                 int64_t cap, int64_t* lengths_dev, void* scratch_dev, int64_t scratch_bytes, void* stream,
+                 int prog) {
+  const Encoder& enc = prog ? kJpegProg : kJpeg;
+  Settings st;
+  auto settle = [&](const std::vector<FrameSource>& fr, int64_t& need) {
+    const int rc = resolve_params(enc.call, params, &st);
+    st.prog = prog;
+    if (!rc) need = jpeg_scratch_bytes(fr.data(), n, st);
+    return rc;
+  };
+  auto launch = [&](const PixFormat& pf, const FrameSource* fr) {
+    return launch_encode_jpeg(format, pf, fr, n, st, out_dev, cap, lengths_dev, scratch_dev,
+                              (cudaStream_t)stream);
+  };
+  return encode_frames(enc, n, format, planes, pitches, heights, widths, crops, out_dev, cap,
+                       lengths_dev, scratch_dev, scratch_bytes, settle, launch);
+}
+
+}  // namespace
+}  // namespace sqdet
+
+int64_t sqdet_jpeg_max_bytes_params(int h, int w, const sqdet_jpeg_params* params) {
+  return max_bytes_entry(h, w, params, 0);
+}
+
+int64_t sqdet_jpeg_max_bytes_progressive(int h, int w, const sqdet_jpeg_params* params) {
+  return max_bytes_entry(h, w, params, 1);
 }
 
 int64_t sqdet_jpeg_max_bytes(int h, int w) {
@@ -1068,11 +1746,12 @@ int64_t sqdet_jpeg_max_bytes(int h, int w) {
 
 int64_t sqdet_jpeg_scratch_bytes_params(int n, const int32_t* heights, const int32_t* widths,
                                         const int32_t* crops, const sqdet_jpeg_params* params) {
-  std::vector<FrameSource> fr;
-  Settings st;
-  if (resolve_params(kJpeg.scratch_call, params, &st)) return -1;
-  if (encode_crops(kJpeg.scratch_call, kJpeg, n, heights, widths, crops, fr)) return -1;
-  return jpeg_scratch_bytes(fr.data(), n, st);
+  return scratch_bytes_entry(n, heights, widths, crops, params, 0);
+}
+
+int64_t sqdet_jpeg_scratch_bytes_progressive(int n, const int32_t* heights, const int32_t* widths,
+                                             const int32_t* crops, const sqdet_jpeg_params* params) {
+  return scratch_bytes_entry(n, heights, widths, crops, params, 1);
 }
 
 int64_t sqdet_jpeg_scratch_bytes(int n, const int32_t* heights, const int32_t* widths,
@@ -1085,18 +1764,16 @@ int sqdet_encode_jpeg_params(int n, int format, const uint8_t* const* planes, co
                              const int32_t* heights, const int32_t* widths, const int32_t* crops,
                              const sqdet_jpeg_params* params, uint8_t* out_dev, int64_t cap,
                              int64_t* lengths_dev, void* scratch_dev, int64_t scratch_bytes, void* stream) {
-  Settings st;
-  auto settle = [&](const std::vector<FrameSource>& fr, int64_t& need) {
-    const int rc = resolve_params(kJpeg.call, params, &st);
-    if (!rc) need = jpeg_scratch_bytes(fr.data(), n, st);
-    return rc;
-  };
-  auto launch = [&](const PixFormat& pf, const FrameSource* fr) {
-    return launch_encode_jpeg(format, pf, fr, n, st, out_dev, cap, lengths_dev, scratch_dev,
-                              (cudaStream_t)stream);
-  };
-  return encode_frames(kJpeg, n, format, planes, pitches, heights, widths, crops, out_dev, cap,
-                       lengths_dev, scratch_dev, scratch_bytes, settle, launch);
+  return encode_entry(n, format, planes, pitches, heights, widths, crops, params, out_dev, cap, lengths_dev,
+                      scratch_dev, scratch_bytes, stream, 0);
+}
+
+int sqdet_encode_jpeg_progressive(int n, int format, const uint8_t* const* planes, const int64_t* pitches,
+                                  const int32_t* heights, const int32_t* widths, const int32_t* crops,
+                                  const sqdet_jpeg_params* params, uint8_t* out_dev, int64_t cap,
+                                  int64_t* lengths_dev, void* scratch_dev, int64_t scratch_bytes, void* stream) {
+  return encode_entry(n, format, planes, pitches, heights, widths, crops, params, out_dev, cap, lengths_dev,
+                      scratch_dev, scratch_bytes, stream, 1);
 }
 
 int sqdet_encode_jpeg(int n, int format, const uint8_t* const* planes, const int64_t* pitches,

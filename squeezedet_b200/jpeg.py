@@ -37,18 +37,20 @@ def jpeg_params(quality=95, sampling='420', optimize=False, restart_interval=0, 
                          int(bool(optimize)), int(restart_interval))
 
 
-def max_bytes(h, w, **params):
-  """The largest JPEG file of an h x w image (sqdet_jpeg_max_bytes_params) with the keyword
-  settings of encode_jpeg_device.  Sides are at most 65500, libjpeg's JPEG_MAX_DIMENSION, as for
-  cv2.imencode."""
+def max_bytes(h, w, progressive=False, **params):
+  """The largest JPEG file of an h x w image (sqdet_jpeg_max_bytes_params, or with progressive
+  sqdet_jpeg_max_bytes_progressive) with the keyword settings of encode_jpeg_device.  Sides are at
+  most 65500, libjpeg's JPEG_MAX_DIMENSION, as for cv2.imencode."""
   p = jpeg_params(**params)
   if not (1 <= int(h) <= 65500 and 1 <= int(w) <= 65500):
     raise ValueError('a JPEG is 1 to 65500 pixels wide and high, got %dx%d' % (w, h))
-  return int(_lib.load().sqdet_jpeg_max_bytes_params(int(h), int(w), C.byref(p)))
+  fn = 'sqdet_jpeg_max_bytes_progressive' if progressive else 'sqdet_jpeg_max_bytes_params'
+  return int(getattr(_lib.load(), fn)(int(h), int(w), C.byref(p)))
 
 
 def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None, *, sampling='420',
-                       optimize=False, restart_interval=0, luma_quality=None, chroma_quality=None):
+                       optimize=False, restart_interval=0, luma_quality=None, chroma_quality=None,
+                       progressive=False):
   """-> (data [n, cap] uint8, lengths [n] int64), both on the frames' device: frame i's file is
   data[i, :lengths[i]], and lengths[i] is -1 if it did not fit cap = the largest file of the
   largest crop.  Asynchronous on `stream` (a torch.cuda.Stream, a raw cudaStream_t, or None for
@@ -68,14 +70,21 @@ def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None, *, samp
   (IMWRITE_JPEG_RST_INTERVAL, in MCUs, 0 for none), luma_quality and chroma_quality
   (IMWRITE_JPEG_LUMA_QUALITY / _CHROMA_QUALITY: luma_quality replaces quality, chroma_quality
   counts only with it, and two different ones give 4:4:4 whatever `sampling` says).  4:4:4
-  doubles the worst-case sizes of 4:2:0.  Values cv2 would clamp raise ValueError.  Progressive
-  files are not written: use cv2.imencode with IMWRITE_JPEG_PROGRESSIVE for those."""
+  doubles the worst-case sizes of 4:2:0.  Values cv2 would clamp raise ValueError.
+
+  progressive=True writes what cv2.imencode writes with IMWRITE_JPEG_PROGRESSIVE as well
+  (sqdet_encode_jpeg_progressive): the same coefficients in jpeg_simple_progression's ten scans,
+  each with its own optimal tables, so optimize has no effect; a restart interval counts blocks in
+  the eight single-component scans.  Its worst-case cap is about 2.1 times the baseline one at
+  4:2:0.  decode_jpeg_device does not read these files; cv2.imdecode does."""
   settings = dict(quality=quality, sampling=sampling, optimize=optimize,
                   restart_interval=restart_interval, luma_quality=luma_quality,
                   chroma_quality=chroma_quality)
-  return encode_frames(frames, fmt, crops, stream, lambda h, w: max_bytes(h, w, **settings),
-                       'sqdet_jpeg_scratch_bytes_params', 'sqdet_encode_jpeg_params',
-                       lambda: (C.byref(jpeg_params(**settings)),))
+  kind = 'progressive' if progressive else 'params'
+  return encode_frames(frames, fmt, crops, stream,
+                       lambda h, w: max_bytes(h, w, progressive=progressive, **settings),
+                       'sqdet_jpeg_scratch_bytes_' + kind,
+                       'sqdet_encode_jpeg_' + kind, lambda: (C.byref(jpeg_params(**settings)),))
 
 
 # the files of encode_jpeg_device's (data, lengths)
