@@ -686,6 +686,11 @@ int sqdet_encode_png(int n, int format, const uint8_t* const* planes, const int6
 #define SQDET_JPEG_SAMPLING         8   /* other sampling layouts, multi-scan sequential files */
 #define SQDET_JPEG_SIZE             9   /* zero height or width */
 #define SQDET_JPEG_TOO_LARGE        10  /* a side above 65500 or more than 2^30 pixels, as coded */
+/* progressive entry points only (see below); each names what cv2.imdecode does with the file */
+#define SQDET_JPEG_BAD_PROGRESSION  11  /* scan script libjpeg rejects: cv2 returns None */
+#define SQDET_JPEG_BOGUS_PROGRESSION 12 /* scan script libjpeg warns on or overwrites: cv2 decodes it */
+#define SQDET_JPEG_SMOOTHED         13  /* libjpeg block-smooths it: cv2 decodes it */
+#define SQDET_JPEG_TOO_MANY_SCANS   14  /* more than 256 scans: cv2 decodes it */
 typedef struct {
   int32_t height, width;              /* of the decoded frame, after orientation */
   int32_t coded_height, coded_width;  /* as SOF gives them */
@@ -709,6 +714,65 @@ int sqdet_decode_jpeg(int n, const uint8_t* const* files_host, const int64_t* le
  * [32, 8192]; 0 restores the default 1024).  Process-wide; sizes from the functions above hold
  * for the value set when they were called.                                                    */
 int sqdet_jpeg_decode_set_subsequence_bits(int bits);
+
+/* ---- progressive JPEG decoding (no engine needed) ------------------------------------
+ * sqdet_decode_jpeg_progressive decodes SOF2 (progressive Huffman) files as well as every file
+ * sqdet_decode_jpeg decodes, in one batch, again exactly to cv2.imdecode's pixels; the sequential
+ * files of a batch decode to what sqdet_decode_jpeg gives them.  The four functions take the
+ * arguments of their plain counterparts, make the same argument checks and keep the same limits
+ * (1 to 128 files, 65500 per side, 2^30 pixels); sqdet_jpeg_decode_set_subsequence_bits applies
+ * to the sequential files.  The plain functions keep refusing SOF2 files.
+ *
+ * A progressive file holds its coefficients in several scans, each a band [Ss, Se] of one or
+ * more components at bit Al (Ah: the bit of the scan before, for a refinement).  cv2's
+ * libjpeg-turbo reads them all into a whole-image buffer and decodes that as a sequential file
+ * of those coefficients, so the sample path (IDCT, upsampling, colour, EXIF orientation) is the
+ * sequential one.  Refused besides the sequential refusals, each with what cv2 does:
+ *   SQDET_JPEG_BAD_PROGRESSION   libjpeg's JERR_BAD_PROGRESSION (a DC scan with Se != 0, an AC
+ *                                scan with Ss > Se, Se > 63 or several components, Ah != 0 with
+ *                                Al != Ah - 1, Al > 13): cv2 returns None
+ *   SQDET_JPEG_BOGUS_PROGRESSION libjpeg's JWRN_BOGUS_PROGRESSION (an AC scan before the
+ *                                component's DC, an Ah that is not the coefficient's last Al),
+ *                                and a second first scan (Ah = 0) of a coefficient: cv2 decodes
+ *   SQDET_JPEG_SMOOTHED          files libjpeg block-smooths, decided from the scan headers as
+ *                                jdcoefct.c's smoothing_ok decides: every component has DC bits
+ *                                and nonzero quantizers 0..9 of its latched table, and some
+ *                                coefficient 1..9 of some component is never coded or not coded
+ *                                down to bit 0.  Complete files are not smoothed
+ *   SQDET_JPEG_TOO_MANY_SCANS    more than 256 scans (libjpeg has no cap; a few header bytes
+ *                                must not size unbounded staging).  The scans past the cap are
+ *                                still checked, so a file libjpeg rejects or warns on is reported
+ *                                as such whatever its number of scans
+ * Still refused with their plain reasons: SOF6/SOF14 (hierarchical), SOF10 (arithmetic),
+ * multi-scan sequential files, and (SQDET_JPEG_SAMPLING, as the plain decoder refuses them) scans
+ * whose components are not in the frame's order or repeat one: libjpeg decodes some of these
+ * (Cr before Cb) and rejects others (Y, Cr, Cb); route them to cv2.imdecode.  A component's quantization table is the one in force at its
+ * first scan, as libjpeg latches it; DHT and DRI may change between scans, and an AC scan's
+ * restart interval counts blocks.
+ *
+ * status_dev[i] is negative, and only file i's pixels unspecified, for the corruptions of
+ * sqdet_decode_jpeg and, in a progressive scan, a run past Se, a refinement symbol of a size
+ * other than 1, or an EOBRUN past its restart interval.
+ *
+ * The host reads every scan's bytes to find the next header, removes their stuffing and splits
+ * them at their RSTn markers into the staging.  A scan's restart intervals are placed only as far
+ * as its markers reach (a scan with fewer markers than its DRI asks for is corrupt), so the
+ * staging follows the file's bytes, not its headers: at most 7 bytes per byte of the file (its
+ * clean data, and 4 + 8 bytes per restart interval, each of which takes at least the 2 bytes of
+ * its RSTn) plus about 5 KiB per scan for its tables and descriptor.  On the stream, with no host synchronisation: one launch decodes
+ * every first scan (Ah = 0) of every file, one warp per (scan, restart interval); one launch
+ * ORs in every DC refinement, one thread per block; one launch per depth of the longest chain of
+ * AC refinements of one component decodes those, one warp per (scan, restart interval); then
+ * the sequential IDCT and colour kernels.  A scan without restart markers is one lane's work. */
+int sqdet_jpeg_parse_progressive(const uint8_t* file, int64_t len, sqdet_jpeg_info* out);
+int64_t sqdet_jpeg_decode_staging_bytes_progressive(int n, const uint8_t* const* files_host,
+                                                    const int64_t* lengths);
+int64_t sqdet_jpeg_decode_scratch_bytes_progressive(int n, const uint8_t* const* files_host,
+                                                    const int64_t* lengths);
+int sqdet_decode_jpeg_progressive(int n, const uint8_t* const* files_host, const int64_t* lengths,
+                                  uint8_t* const* out_planes, const int64_t* out_pitches,
+                                  void* staging_pinned, int64_t staging_bytes, void* scratch_dev,
+                                  int64_t scratch_bytes, int32_t* status_dev, void* stream);
 
 /* ---- KITTI 2-D object scoring of filtered records (no engine needed) ---------------
  * sqdet_kitti_eval scores n images of records exactly as the KITTI devkit's evaluate_object does

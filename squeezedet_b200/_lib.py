@@ -158,6 +158,10 @@ SIGNATURES = {
     'sqdet_jpeg_decode_scratch_bytes': (_i64, [_i, _vp, _vp]),
     'sqdet_decode_jpeg': (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp]),
     'sqdet_jpeg_decode_set_subsequence_bits': (_i, [_i]),
+    'sqdet_jpeg_parse_progressive': (_i, [_vp, _i64, C.POINTER(JpegInfo)]),
+    'sqdet_jpeg_decode_staging_bytes_progressive': (_i64, [_i, _vp, _vp]),
+    'sqdet_jpeg_decode_scratch_bytes_progressive': (_i64, [_i, _vp, _vp]),
+    'sqdet_decode_jpeg_progressive': (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp]),
     'sqdet_malloc': (_i, [_i, _i64, C.POINTER(_vp)]),
     'sqdet_free': (_i, [_i, _vp]),
     'sqdet_malloc_host': (_i, [_i64, C.POINTER(_vp)]),

@@ -16,6 +16,10 @@ records of (b) are checked bitwise against (a)'s.
 The decode kernels alone are timed in a separate pass under torch.profiler: the device durations of
 the decode_jpeg_device calls' kernels, copies and memsets, summed, per frame.
 
+--progressive writes the files with IMWRITE_JPEG_PROGRESSIVE and decodes them with
+decode_jpeg_device(progressive=True); the kernel pass then also reports each kernel's share: the
+first scans, the DC refinements and the AC refinements separately.
+
 Prints one JSON line with the card's name and power limit, read in the same run; writes nothing.
 """
 from __future__ import annotations
@@ -36,6 +40,8 @@ QUALITY = 95
 KERNELS = ('destuff_count_kernel', 'scan_chunks_kernel', 'destuff_compact_kernel',
            'intervals_kernel', 'sync_tiles_kernel', 'sync_chain_kernel', 'scan_counts_kernel',
            'decode_write_kernel', 'idct_kernel', 'color_kernel')
+PROG_KERNELS = ('prog_seq_kernel', 'prog_dc_refine_kernel', 'idct_kernel', 'color_kernel',
+                'scatter_status_kernel')
 
 
 def parse_args(argv=None):
@@ -45,6 +51,7 @@ def parse_args(argv=None):
   ap.add_argument('--warmup', type=int, default=3)
   ap.add_argument('--frames', type=int, default=8)
   ap.add_argument('--gpu', type=int, default=0)
+  ap.add_argument('--progressive', action='store_true')
   return ap.parse_args(argv)
 
 
@@ -79,7 +86,7 @@ def measure_workload(args, name, model, files, torch):
     stream.synchronize()
 
   def form_b():
-    frames, status = decode_jpeg_device(files, dev, stream=stream)
+    frames, status = decode_jpeg_device(files, dev, stream=stream, progressive=args.progressive)
     model.forward_device_frames(frames, stream=stream.cuda_stream)
     stream.synchronize()
     return status
@@ -109,12 +116,14 @@ def measure_workload(args, name, model, files, torch):
   keep = []
   with profile(activities=[ProfilerActivity.CUDA]) as prof:
     for _ in range(calls):
-      keep.append(decode_jpeg_device(files, dev, stream=stream))
+      keep.append(decode_jpeg_device(files, dev, stream=stream, progressive=args.progressive))
     stream.synchronize()
+  names = PROG_KERNELS if args.progressive else KERNELS
   evs = [ev for ev in prof.events() if ev.device_type == DeviceType.CUDA and
-         any(k in ev.name for k in KERNELS + ('emset', 'emcpy', 'Memcpy', 'Memset'))]
-  kern = [ev for ev in evs if any(k in ev.name for k in KERNELS)]
-  assert len(kern) >= calls * len(KERNELS) * 9 // 10, 'found %d decode launches' % len(kern)
+         any(k in ev.name for k in names + ('emset', 'emcpy', 'Memcpy', 'Memset'))]
+  kern = [ev for ev in evs if any(k in ev.name for k in names)]
+  assert len(kern) >= calls * (3 if args.progressive else len(KERNELS)) * 9 // 10, \
+      'found %d decode launches' % len(kern)
   us = sum(ev.time_range.elapsed_us() for ev in evs) / calls
   us_k = sum(ev.time_range.elapsed_us() for ev in kern) / calls
   n = len(files)
@@ -124,6 +133,17 @@ def measure_workload(args, name, model, files, torch):
                  'ms_per_frame_step_min': 1e3 * min(step[form]) / n}
   row['decode_device'] = {'us_per_frame_kernels': us_k / n, 'us_per_frame_with_copy_and_memsets': us / n,
                           'calls_timed': calls}
+  if args.progressive:
+    # a call's first prog_seq_kernel decodes the first scans, its later ones the AC refinements
+    share = {}
+    prev = None
+    for ev in sorted(kern, key=lambda e: e.time_range.start):
+      k = next(k for k in names if k in ev.name)
+      if k == 'prog_seq_kernel':
+        k = 'ac_refine' if prev in ('prog_seq_kernel', 'prog_dc_refine_kernel', 'ac_refine') else 'first_scans'
+      share[k] = share.get(k, 0.0) + ev.time_range.elapsed_us() / calls / n
+      prev = k if k != 'first_scans' else 'prog_seq_kernel'
+    row['decode_device']['us_per_frame_by_kernel'] = share
   return row
 
 
@@ -137,12 +157,13 @@ def measure(args):
   model = make_model(1242, 375, args.frames, args.gpu)
   rows = []
   for name, (h, w) in (('kitti_1242x375', (375, 1242)), ('1080p', (1080, 1920))):
-    files = [cv2.imencode('.jpg', picture(h, w, rng), [cv2.IMWRITE_JPEG_QUALITY, QUALITY])[1].tobytes()
-             for _ in range(args.frames)]
+    params = [cv2.IMWRITE_JPEG_QUALITY, QUALITY] + ([cv2.IMWRITE_JPEG_PROGRESSIVE, 1] if args.progressive else [])
+    files = [cv2.imencode('.jpg', picture(h, w, rng), params)[1].tobytes() for _ in range(args.frames)]
     rows.append(measure_workload(args, name, model, files, torch))
-  return {'workload': 'squeezeDet 1242x375 forward_device_frames on JPEG files (quality 95, 4:2:0, '
+  kind = 'progressive ' if args.progressive else ''
+  return {'workload': 'squeezeDet 1242x375 forward_device_frames on %sJPEG files (quality 95, 4:2:0, '
                       'smooth synthetic pictures) decoded by a cv2.imdecode thread pool and '
-                      'uploaded, or by decode_jpeg_device',
+                      'uploaded, or by decode_jpeg_device' % kind,
           'gpu': gpu_info(args.gpu), 'cpu_threads': os.cpu_count(),
           'timer': 'host clock per step from the files on the host to a device synchronisation '
                    'after the forward; decode kernels: torch.profiler device durations, summed, per frame',

@@ -719,6 +719,8 @@ struct Parsed {
   bool have_q[4], have_dc[4], have_ac[4];
   uint8_t dc_bits[4][16], ac_bits[4][16];
   uint8_t dc_vals[4][256], ac_vals[4][256];
+  bool progressive;                    // SOF2 (parse with progressive = true only)
+  int64_t first_sos;                   // SOF2: the first SOS marker's offset
 };
 
 int u16(const uint8_t* b, int64_t i) { return (b[i] << 8) | b[i + 1]; }
@@ -759,7 +761,9 @@ int exif_orientation(const uint8_t* s, int64_t n) {
 const char* kReasons[] = {"ok", "malformed or truncated header", "progressive", "arithmetic coding",
                           "lossless", "not 8-bit samples", "not 1 or 3 components",
                           "RGB-coded", "unsupported sampling",
-                          "zero height or width", "larger than cv2 decodes"};
+                          "zero height or width", "larger than cv2 decodes",
+                          "scan script libjpeg rejects", "scan script libjpeg warns on or overwrites",
+                          "block-smoothed by libjpeg", "more than 256 scans"};
 
 // The largest file cv2.imdecode decodes: libjpeg's JPEG_MAX_DIMENSION per side, and cv2's default
 // CV_IO_MAX_IMAGE_PIXELS (it raises above that many pixels).
@@ -781,8 +785,9 @@ bool huff_ok(const uint8_t* bits, const uint8_t* vals, bool dc) {
   return true;
 }
 
-// The headers up to the first SOS; the reason (SQDET_JPEG_*) and what was read.
-int parse(const uint8_t* b, int64_t n, Parsed& P) {
+// The headers up to the first SOS; the reason (SQDET_JPEG_*) and what was read.  With
+// `progressive`, an SOF2 frame is read as SOF0's is and the first SOS is left to parse_scans.
+int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive = false) {
   memset(&P, 0, sizeof(P));
   sqdet_jpeg_info& I = P.info;
   I.orientation = 1;
@@ -802,12 +807,13 @@ int parse(const uint8_t* b, int64_t n, Parsed& P) {
     const uint8_t* body = b + i + 2;
     const int bn = len - 2;
     i += len;
-    if (m == 0xC2 || m == 0xC6 || m == 0xCA || m == 0xCE) return SQDET_JPEG_PROGRESSIVE;
+    if ((m == 0xC2 && !progressive) || m == 0xC6 || m == 0xCA || m == 0xCE) return SQDET_JPEG_PROGRESSIVE;
     if (m == 0xC9 || m == 0xCB || m == 0xCD || m == 0xCF) return SQDET_JPEG_ARITHMETIC;
     if (m == 0xC3 || m == 0xC7) return SQDET_JPEG_LOSSLESS;
     if (m == 0xC5) return SQDET_JPEG_PROGRESSIVE;
-    if (m == 0xC0 || m == 0xC1) {
+    if (m == 0xC0 || m == 0xC1 || m == 0xC2) {
       if (frame || bn < 6) return SQDET_JPEG_MALFORMED;
+      P.progressive = m == 0xC2;
       I.coded_height = u16(body, 1);
       I.coded_width = u16(body, 3);
       ncomp = body[5];
@@ -869,6 +875,20 @@ int parse(const uint8_t* b, int64_t n, Parsed& P) {
       adobe = body[11];
     } else if (m == 0xDA) {
       if (!frame || bn < 1) return SQDET_JPEG_MALFORMED;
+      if (P.progressive) {
+        if (ncomp == 3 && !jfif &&
+            (adobe >= 0 ? adobe == 0
+                        : P.comp[0].id == 'R' && P.comp[1].id == 'G' && P.comp[2].id == 'B'))
+          return SQDET_JPEG_COLOR_TRANSFORM;
+        P.first_sos = i - len - 2;
+        I.h_samp = ncomp == 1 ? 1 : P.comp[0].h;
+        I.v_samp = ncomp == 1 ? 1 : P.comp[0].v;
+        const bool swap = I.orientation >= 5;
+        I.height = swap ? I.coded_width : I.coded_height;
+        I.width = swap ? I.coded_height : I.coded_width;
+        I.supported = 1;
+        return SQDET_JPEG_OK;
+      }
       const int ns = body[0];
       if (bn != 4 + 2 * ns) return SQDET_JPEG_MALFORMED;
       if (ns != ncomp) return SQDET_JPEG_SAMPLING;
@@ -1032,6 +1052,47 @@ int make_plan(const std::string& name, int n, const uint8_t* const* files, const
   return SQDET_OK;
 }
 
+// The fields of a file's descriptor that follow from its frame header, its quantization tables
+// (as the components name them) included.
+void describe(const Parsed& P, const Layout& L, DecFile& f) {
+  const sqdet_jpeg_info& I = P.info;
+  f.h = I.coded_height;
+  f.w = I.coded_width;
+  f.oh = I.height;
+  f.ow = I.width;
+  f.ncomp = I.components;
+  f.orient = I.orientation;
+  f.mcu_cols = L.mcu_cols;
+  f.mcus = L.mcus;
+  f.bpm = L.bpm;
+  f.restart = L.restart;
+  f.intervals = L.intervals;
+  f.raw_len = (int32_t)L.raw_len;
+  f.chunks = L.chunks;
+  f.blocks = L.blocks;
+  f.sub_max = L.sub_max;
+  f.sub_bits = g_sub_bits;
+  int u = 0;
+  for (int c = 0; c < I.components; ++c) {
+    const Comp& cp = P.comp[c];
+    const int hc = I.components == 1 ? 1 : cp.h, vc = I.components == 1 ? 1 : cp.v;
+    f.ch[c] = (int8_t)hc;
+    f.cv[c] = (int8_t)vc;
+    for (int by = 0; by < vc; ++by)
+      for (int bx = 0; bx < hc; ++bx, ++u) {
+        f.bcomp[u] = (int8_t)c;
+        f.bdy[u] = (int8_t)by;
+        f.bdx[u] = (int8_t)bx;
+      }
+    f.pw[c] = L.pw[c];
+    f.ph[c] = L.ph[c];
+    const int hmax = I.components == 1 ? 1 : P.comp[0].h, vmax = I.components == 1 ? 1 : P.comp[0].v;
+    f.cw[c] = (int)(((int64_t)f.w * hc + hmax - 1) / hmax);
+    f.chh[c] = (int)(((int64_t)f.h * vc + vmax - 1) / vmax);
+    for (int k = 0; k < 64; ++k) f.q[c][k] = (int16_t)P.qt[cp.tq][k];
+  }
+}
+
 // Fills the staging (descriptors, tables, raw bytes) for outputs out/pitch.
 void fill_staging(const Plan& plan, int n, const uint8_t* const* files, uint8_t* const* out,
                   const int64_t* pitch, uint8_t* stage) {
@@ -1041,41 +1102,7 @@ void fill_staging(const Plan& plan, int n, const uint8_t* const* files, uint8_t*
     const Layout& L = plan.lay[(size_t)i];
     const sqdet_jpeg_info& I = P.info;
     DecFile f = plan.files[(size_t)i];
-    f.h = I.coded_height;
-    f.w = I.coded_width;
-    f.oh = I.height;
-    f.ow = I.width;
-    f.ncomp = I.components;
-    f.orient = I.orientation;
-    f.mcu_cols = L.mcu_cols;
-    f.mcus = L.mcus;
-    f.bpm = L.bpm;
-    f.restart = L.restart;
-    f.intervals = L.intervals;
-    f.raw_len = (int32_t)L.raw_len;
-    f.chunks = L.chunks;
-    f.blocks = L.blocks;
-    f.sub_max = L.sub_max;
-    f.sub_bits = g_sub_bits;
-    int u = 0;
-    for (int c = 0; c < I.components; ++c) {
-      const Comp& cp = P.comp[c];
-      const int hc = I.components == 1 ? 1 : cp.h, vc = I.components == 1 ? 1 : cp.v;
-      f.ch[c] = (int8_t)hc;
-      f.cv[c] = (int8_t)vc;
-      for (int by = 0; by < vc; ++by)
-        for (int bx = 0; bx < hc; ++bx, ++u) {
-          f.bcomp[u] = (int8_t)c;
-          f.bdy[u] = (int8_t)by;
-          f.bdx[u] = (int8_t)bx;
-        }
-      f.pw[c] = L.pw[c];
-      f.ph[c] = L.ph[c];
-      const int hmax = I.components == 1 ? 1 : P.comp[0].h, vmax = I.components == 1 ? 1 : P.comp[0].v;
-      f.cw[c] = (int)(((int64_t)f.w * hc + hmax - 1) / hmax);
-      f.chh[c] = (int)(((int64_t)f.h * vc + vmax - 1) / vmax);
-      for (int k = 0; k < 64; ++k) f.q[c][k] = (int16_t)P.qt[cp.tq][k];
-    }
+    describe(P, L, f);
     HuffTab* tabs = reinterpret_cast<HuffTab*>(stage + f.tabs);
     for (int c = 0; c < I.components; ++c) {
       build_tab(P.dc_bits[P.comp[c].td], P.dc_vals[P.comp[c].td], tabs[2 * c]);
@@ -1130,6 +1157,760 @@ int launch_decode(const Plan& plan, int n, uint8_t* stage, uint8_t* scratch, int
   return SQDET_OK;
 }
 
+// The decode calls' checks of everything but the files, in their order; info[i] is file i's.
+int check_decode_args(const std::string& name, int n, const sqdet_jpeg_info* const* info,
+                      uint8_t* const* out_planes, const int64_t* out_pitches, void* staging_pinned,
+                      int64_t staging_bytes, int64_t staging_need, void* scratch_dev,
+                      int64_t scratch_bytes, int64_t scratch_need, int32_t* status_dev,
+                      const char* staging_fn, const char* scratch_fn) {
+  if ((uintptr_t)scratch_dev % 256) return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
+  if ((uintptr_t)status_dev % alignof(int32_t))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": status_dev must be 4-byte aligned");
+  if (staging_bytes < staging_need)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": staging_bytes is below " + staging_fn);
+  if (scratch_bytes < scratch_need)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below " + scratch_fn);
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, staging_pinned) != cudaSuccess || attr.type != cudaMemoryTypeHost) {
+    (void)cudaGetLastError();
+    return fail(SQDET_ERR_INVALID_ARG, name + ": staging_pinned is not page-locked host memory");
+  }
+  if (!out_planes[0]) return fail(SQDET_ERR_INVALID_ARG, name + ": output 0 is null");
+  const int device = pointer_device(out_planes[0]);
+  if (device < 0) return fail(SQDET_ERR_INVALID_ARG, name + ": output 0 is not device memory");
+  for (int i = 0; i < n; ++i) {
+    const sqdet_jpeg_info& I = *info[i];
+    const std::string which = name + ": output " + std::to_string(i);
+    if (!out_planes[i]) return fail(SQDET_ERR_INVALID_ARG, which + " is null");
+    if (out_pitches[i] < 3 * (int64_t)I.width) return fail(SQDET_ERR_INVALID_ARG, which + ": pitch below 3 * width");
+    const int64_t bytes = (int64_t)(I.height - 1) * out_pitches[i] + 3 * (int64_t)I.width;
+    if (!device_range_ok(out_planes[i], bytes, device))
+      return fail(SQDET_ERR_INVALID_ARG, which + " is not inside one device allocation on output 0's device");
+  }
+  if (!device_range_ok(status_dev, (int64_t)n * 4, device) ||
+      !device_range_ok(scratch_dev, scratch_bytes, device))
+    return fail(SQDET_ERR_INVALID_ARG, name + ": status_dev or scratch_dev is not inside one device "
+                                              "allocation on output 0's device");
+  return SQDET_OK;
+}
+
+// ==== progressive (SOF2) files ============================================================
+// libjpeg reads every scan into a whole-image coefficient buffer and runs its output pass once
+// the file has ended, so a progressive file decodes to what a sequential file of the final
+// coefficients decodes to; idct_kernel and color_kernel run unchanged.  The host parses every
+// SOS with the tables in force at that point, removes the stuffing and splits each scan's data
+// at its RSTn markers, and packs it all into the staging.  Then, on the stream:
+//   1. prog_seq (first)  every first scan (Ah = 0, DC and AC) of every file: one warp per
+//                        (scan, restart interval) decodes it in order; first scans write disjoint
+//                        (component, coefficient) sets and read none, so they are independent
+//   2. prog_dc_refine    every DC refinement scan: one thread per block ORs bit Al into its DC
+//   3. prog_seq (refine) AC refinements, one launch per depth of the longest chain: the d-th
+//                        refinement scan of each component of each file, one warp per
+//                        (scan, interval), which keeps each block's nonzero coefficients as a
+//                        mask so a run and the correction bits it passes are found with
+//                        popcount and bit scans
+// then idct and color.  Every loop is bounded by host-known sizes; corrupt data sets a negative
+// status for its file only.
+constexpr int kMaxScans = 256;
+// one (scan, interval) per CTA of one warp, decoded by its first lane: items that shared a warp
+// would run their divergent walks one after another
+constexpr int kProgThreads = 32;
+constexpr int kScanPad = 32;          // zero bytes after each scan's clean data
+
+struct ProgScan {
+  int32_t file, ss, se, ah, al;
+  int32_t nb;                         // blocks per unit: the MCU's of the scan's components, or 1
+  int32_t units, per, intervals;      // units in the scan and per restart interval
+  int32_t cols;                       // one-component scans: the component's block columns
+  int32_t single, bad;                // one-component scan; an RSTn out of sequence or missing
+  int8_t bc[10], bu[10], bt[10];      // per block of a unit: component, block of the MCU, table
+  int64_t tabs, clean, ist;
+};
+
+struct ProgParams {
+  DecFile* f;
+  const ProgScan* sc;
+  const int2* items;                  // (scan, interval) or, for prog_dc_refine, (scan, 0)
+  int nitems;
+  uint8_t* s;
+  int32_t* status;
+};
+
+// The coefficient block of block j of unit u of scan S.
+__device__ __forceinline__ int64_t unit_block(const DecFile& f, const ProgScan& S, int u, int j) {
+  if (!S.single) return (int64_t)u * f.bpm + S.bu[j];
+  const int by = u / S.cols, bx = u - by * S.cols;
+  if (f.ncomp == 1) return (int64_t)by * f.mcu_cols + bx;
+  const int c = S.bc[0], h = f.ch[c], v = f.cv[c];
+  return ((int64_t)(by / v) * f.mcu_cols + bx / h) * f.bpm + S.bu[0] + (by % v) * h + bx % h;
+}
+
+__device__ __forceinline__ int16_t jcoef(int v) { return (int16_t)v; }
+
+// Reads one correction bit for each set bit of `corr` (zigzag positions, in order) and applies
+// it as decode_mcu_AC_refine does.
+__device__ __forceinline__ int corrections(const uint8_t* clean, int p, int16_t* blk, uint64_t corr,
+                                           int p1, int m1) {
+#pragma unroll 1
+  while (corr) {
+    const int take = min(__popcll(corr), 32);
+    const uint32_t w = peek32(clean, p);
+    p += take;
+#pragma unroll 1
+    for (int i = 0; i < take; ++i) {
+      const int k = __ffsll((long long)corr) - 1;
+      corr &= corr - 1;
+      if ((w >> (31 - i)) & 1) {
+        int16_t& c = blk[kNaturalDev[k]];
+        if ((c & p1) == 0) c = jcoef(c + (c >= 0 ? p1 : m1));
+      }
+    }
+  }
+  return p;
+}
+
+// One restart interval of a Huffman-coded scan; 0 or a negative status.
+__device__ int prog_interval(const DecFile& f, const ProgScan& S, const uint8_t* clean,
+                             const HuffTab* tabs, int16_t* coef, int u0, int u1, int p, int end) {
+  if (S.ss == 0) {                                       // DC first
+    int dc[3] = {0, 0, 0};
+#pragma unroll 1
+    for (int u = u0; u < u1; ++u) {
+#pragma unroll 1
+      for (int j = 0; j < S.nb; ++j) {
+        const uint32_t bits = peek32(clean, p);
+        int len;
+        const int s = huff_decode(tabs[S.bt[j]], bits, len);
+        if (!len) return -4;
+        const uint32_t extra = s ? (bits << len) >> (32 - s) : 0;
+        p += len + s;
+        const int c = S.bc[j];
+        dc[c] += extend(extra, s);
+        coef[unit_block(f, S, u, j) * 64] = jcoef((int)((unsigned)dc[c] << S.al));
+        if (p > end) return -7;
+      }
+    }
+    return 0;
+  }
+  const HuffTab& t = tabs[0];
+  int eobrun = 0;
+  if (S.ah == 0) {                                       // AC first
+#pragma unroll 1
+    for (int u = u0; u < u1; ++u) {
+      if (eobrun) {
+        --eobrun;
+        continue;
+      }
+      int16_t* blk = coef + unit_block(f, S, u, 0) * 64;
+#pragma unroll 1
+      for (int k = S.ss; k <= S.se;) {
+        const uint32_t bits = peek32(clean, p);
+        int len;
+        const int sym = huff_decode(t, bits, len);
+        if (!len) return -4;
+        const int r = sym >> 4, s = sym & 15;
+        if (s) {
+          k += r;
+          if (k > S.se) return -5;
+          blk[kNaturalDev[k]] = jcoef((int)((unsigned)extend((bits << len) >> (32 - s), s) << S.al));
+          p += len + s;
+          ++k;
+        } else if (r == 15) {
+          p += len;
+          k += 16;
+          if (k > S.se + 1) return -5;
+        } else {
+          eobrun = (1 << r) + (r ? (int)((bits << len) >> (32 - r)) : 0) - 1;
+          p += len + r;
+          break;
+        }
+        if (p > end) return -7;
+      }
+      if (p > end) return -7;
+    }
+    return eobrun ? -9 : 0;
+  }
+  // AC refinement
+  const int p1 = 1 << S.al, m1 = (int)(~0u << S.al);
+  const uint64_t band = (~0ull >> (63 - S.se)) & (~0ull << S.ss);
+#pragma unroll 1
+  for (int u = u0; u < u1; ++u) {
+    int16_t* blk = coef + unit_block(f, S, u, 0) * 64;
+    uint64_t nat = 0;                                    // nonzero coefficients, natural order
+    const int4* src = reinterpret_cast<const int4*>(blk);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int4 v = src[i];
+      const int32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        nat |= (uint64_t)((w[e] & 0xFFFF) != 0) << (8 * i + 2 * e);
+        nat |= (uint64_t)((w[e] >> 16) != 0) << (8 * i + 2 * e + 1);
+      }
+    }
+    uint64_t nz = 0;                                     // the same in zigzag order, in the band
+#pragma unroll 1
+    for (int k = S.ss; k <= S.se; ++k) nz |= ((nat >> kNaturalDev[k]) & 1) << k;
+    int k = S.ss;
+    if (eobrun == 0) {
+#pragma unroll 1
+      while (k <= S.se) {
+        const uint32_t bits = peek32(clean, p);
+        int len;
+        const int sym = huff_decode(t, bits, len);
+        if (!len) return -4;
+        int r = sym >> 4;
+        const int s = sym & 15;
+        p += len;
+        int val = 0;
+        if (s) {
+          if (s != 1) return -10;
+          val = (bits << len) >> 31 ? p1 : m1;
+          p += 1;
+        } else if (r != 15) {
+          eobrun = (1 << r) + (r ? (int)((bits << len) >> (32 - r)) : 0);
+          p += r;
+          break;
+        }
+        // the target is the (r + 1)-th coefficient still zero from k on; the nonzero ones
+        // before it take a correction bit each
+        uint64_t zeros = ~nz & band & (~0ull << k);
+        if (__popcll(zeros) <= r) return -5;
+#pragma unroll 1
+        for (; r > 0; --r) zeros &= zeros - 1;
+        const int target = __ffsll((long long)zeros) - 1;
+        p = corrections(clean, p, blk, nz & (~0ull << k) & ((1ull << target) - 1), p1, m1);
+        if (val) blk[kNaturalDev[target]] = jcoef(val);
+        k = target + 1;
+        if (p > end) return -7;
+      }
+    }
+    if (eobrun > 0) {
+      p = corrections(clean, p, blk, k < 64 ? nz & (~0ull << k) : 0, p1, m1);
+      --eobrun;
+    }
+    if (p > end) return -7;
+  }
+  return eobrun ? -9 : 0;
+}
+
+__global__ void __launch_bounds__(kProgThreads) prog_seq_kernel(ProgParams p) {
+  const int t = blockIdx.x;
+  if (threadIdx.x || t >= p.nitems) return;
+  const int2 it = p.items[t];
+  const ProgScan& S = p.sc[it.x];
+  const DecFile& f = p.f[S.file];
+  const int32_t* ist = reinterpret_cast<const int32_t*>(p.s + S.ist);
+  const int r = it.y, u0 = r * S.per, u1 = min(S.units, u0 + S.per);
+  const int rc = S.bad ? -2
+                       : prog_interval(f, S, p.s + S.clean, reinterpret_cast<const HuffTab*>(p.s + S.tabs),
+                                       reinterpret_cast<int16_t*>(p.s + f.coef), u0, u1, ist[r] * 8,
+                                       ist[r + 1] * 8);
+  if (rc) fail_file(p.status, S.file, rc);
+}
+
+// DC refinement: block g of the scan is bit g - (its interval's first block) of its interval.
+__global__ void __launch_bounds__(kPixThreads) prog_dc_refine_kernel(ProgParams p) {
+  const ProgScan& S = p.sc[p.items[blockIdx.y].x];
+  const DecFile& f = p.f[S.file];
+  const int g = blockIdx.x * kPixThreads + threadIdx.x;
+  if (g >= S.units * S.nb) return;
+  if (S.bad) {                       // its intervals past the markers present have no ist
+    fail_file(p.status, S.file, -2);
+    return;
+  }
+  const int u = g / S.nb, j = g - u * S.nb, r = u / S.per;
+  const int32_t* ist = reinterpret_cast<const int32_t*>(p.s + S.ist);
+  const int64_t bit = (int64_t)ist[r] * 8 + (int64_t)(g - r * S.per * S.nb);
+  if (bit >= (int64_t)ist[r + 1] * 8) {
+    fail_file(p.status, S.file, -7);
+    return;
+  }
+  if ((p.s[S.clean + (bit >> 3)] >> (7 - (bit & 7))) & 1) {
+    // two refinement scans of one DC may run at once: OR into the word that holds it
+    int16_t* dc = reinterpret_cast<int16_t*>(p.s + f.coef) + unit_block(f, S, u, j) * 64;
+    atomicOr(reinterpret_cast<unsigned int*>(dc), (unsigned)(1 << S.al));
+  }
+}
+
+// ---- host: every scan -------------------------------------------------------------------------
+struct PScan {
+  int ncomp, comp[3], ss, se, ah, al, restart;
+  uint8_t bits[3][16], vals[3][256];   // the tables in force at the scan
+  int64_t start, end;                  // its entropy-coded bytes
+  int64_t markers;                     // the RSTn markers among them
+};
+struct Prog {
+  std::vector<PScan> scans;
+  bool latched[3];
+  uint16_t q[3][64];
+};
+
+// The first byte at or after j that starts a marker other than RSTn (or n), and the RSTn markers
+// before it.
+int64_t data_end(const uint8_t* b, int64_t n, int64_t j, int64_t& markers) {
+  markers = 0;
+  for (; j < n; ++j) {
+    if (b[j] != 0xFF) continue;
+    if (j + 1 >= n) return j;
+    const int nx = b[j + 1];
+    if (nx >= 0xD0 && nx <= 0xD7) ++markers;
+    else if (!(nx == 0x00 || nx == 0xFF)) return j;
+  }
+  return n;
+}
+
+// jdcoefct.c's smoothing_ok at the output pass: whether libjpeg block-smooths the file.
+bool smoothed(int ncomp, const Prog& G, const int (*cbits)[64]) {
+  static const int kQ[10] = {0, 1, 8, 16, 9, 2, 3, 10, 17, 24};
+  bool useful = false;
+  for (int c = 0; c < ncomp; ++c) {
+    if (!G.latched[c] || cbits[c][0] < 0) return false;
+    for (int k : kQ)
+      if (G.q[c][k] == 0) return false;
+    for (int k = 1; k < 10; ++k) useful = useful || cbits[c][k] != 0;
+  }
+  return useful;
+}
+
+// The scans of an SOF2 file from its first SOS on (oracle/jpeg_decode_progressive.py restates
+// it): the reason (SQDET_JPEG_*) and every scan.
+int parse_scans(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
+  G.scans.clear();
+  memset(G.latched, 0, sizeof(G.latched));
+  memset(G.q, 0, sizeof(G.q));
+  const int ncomp = P.info.components;
+  int cbits[3][64];
+  for (auto& row : cbits)
+    for (int& x : row) x = -1;
+  bool bogus = false, too_many = false;
+  int restart = P.info.restart_interval;
+  int64_t i = P.first_sos;
+  for (;;) {
+    while (i + 1 < n && b[i] == 0xFF && b[i + 1] == 0xFF) ++i;
+    if (!G.scans.empty() && i >= n) break;               // no EOI: the image ends there
+    if (i + 2 > n || b[i] != 0xFF) return SQDET_JPEG_MALFORMED;
+    const int m = b[i + 1];
+    i += 2;
+    if (m == 0xD9 && !G.scans.empty()) break;
+    if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) return SQDET_JPEG_MALFORMED;
+    if (i + 2 > n) return SQDET_JPEG_MALFORMED;
+    const int len = u16(b, i);
+    if (len < 2 || i + len > n) return SQDET_JPEG_MALFORMED;
+    const uint8_t* body = b + i + 2;
+    const int bn = len - 2;
+    i += len;
+    if (m >= 0xC0 && m <= 0xCF && m != 0xC4 && m != 0xC8 && m != 0xCC) return SQDET_JPEG_MALFORMED;
+    if (m == 0xDB) {
+      for (int j = 0; j < bn;) {
+        const int pq = body[j] >> 4, tq = body[j] & 15, size = pq ? 128 : 64;
+        if (pq > 1 || tq > 3 || j + 1 + size > bn) return SQDET_JPEG_MALFORMED;
+        for (int k = 0; k < 64; ++k)
+          P.qt[tq][kNatural[k]] = pq ? (uint16_t)u16(body, j + 1 + 2 * k) : body[j + 1 + k];
+        P.have_q[tq] = true;
+        j += 1 + size;
+      }
+    } else if (m == 0xC4) {
+      for (int j = 0; j < bn;) {
+        if (j + 17 > bn) return SQDET_JPEG_MALFORMED;
+        const int tc = body[j] >> 4, th = body[j] & 15;
+        int cnt = 0;
+        for (int l = 0; l < 16; ++l) cnt += body[j + 1 + l];
+        if (tc > 1 || th > 3 || cnt > 256 || j + 17 + cnt > bn) return SQDET_JPEG_MALFORMED;
+        memcpy(tc ? P.ac_bits[th] : P.dc_bits[th], body + j + 1, 16);
+        memcpy(tc ? P.ac_vals[th] : P.dc_vals[th], body + j + 17, (size_t)cnt);
+        (tc ? P.have_ac : P.have_dc)[th] = true;
+        j += 17 + cnt;
+      }
+    } else if (m == 0xDD) {
+      if (bn != 2) return SQDET_JPEG_MALFORMED;
+      restart = u16(body, 0);
+    } else if (m == 0xDA) {
+      if (bn < 1) return SQDET_JPEG_MALFORMED;
+      const int ns = body[0];
+      if (bn != 4 + 2 * ns || ns < 1 || ns > 4) return SQDET_JPEG_MALFORMED;
+      PScan S{};
+      S.ncomp = ns;
+      int prev = -1;
+      for (int k = 0; k < ns; ++k) {
+        int c = 0;
+        while (c < ncomp && P.comp[c].id != body[1 + 2 * k]) ++c;
+        if (c == ncomp) return SQDET_JPEG_MALFORMED;
+        if (c <= prev) return SQDET_JPEG_SAMPLING;       // out of the frame's order, or repeated
+        prev = S.comp[k] = c;
+      }
+      S.ss = body[1 + 2 * ns];
+      S.se = body[2 + 2 * ns];
+      S.ah = body[3 + 2 * ns] >> 4;
+      S.al = body[3 + 2 * ns] & 15;
+      S.restart = restart;
+      for (int k = 0; k < ns; ++k) {                    // latch_quant_tables
+        const int c = S.comp[k];
+        if (G.latched[c]) continue;
+        if (!P.have_q[P.comp[c].tq]) return SQDET_JPEG_MALFORMED;
+        memcpy(G.q[c], P.qt[P.comp[c].tq], sizeof(G.q[c]));
+        G.latched[c] = true;
+      }
+      const bool dc_band = S.ss == 0;
+      const bool bad = dc_band ? S.se != 0 : (S.ss > S.se || S.se > 63 || ns != 1);
+      if ((S.ah != 0 && S.al != S.ah - 1) || S.al > 13 || bad) return SQDET_JPEG_BAD_PROGRESSION;
+      for (int k = 0; k < ns; ++k) {
+        int* cb = cbits[S.comp[k]];
+        if (!dc_band && cb[0] < 0) bogus = true;
+        for (int q = S.ss; q <= S.se; ++q) {
+          if (S.ah != std::max(cb[q], 0) || (S.ah == 0 && cb[q] >= 0)) bogus = true;
+          cb[q] = S.al;
+        }
+      }
+      for (int k = 0; k < ns; ++k) {
+        const int td = body[2 + 2 * k] >> 4, ta = body[2 + 2 * k] & 15;
+        if (dc_band && S.ah == 0) {
+          if (td > 3 || !P.have_dc[td] || !huff_ok(P.dc_bits[td], P.dc_vals[td], true))
+            return SQDET_JPEG_MALFORMED;
+          memcpy(S.bits[k], P.dc_bits[td], 16);
+          memcpy(S.vals[k], P.dc_vals[td], 256);
+        } else if (!dc_band) {
+          if (ta > 3 || !P.have_ac[ta] || !huff_ok(P.ac_bits[ta], P.ac_vals[ta], false))
+            return SQDET_JPEG_MALFORMED;
+          memcpy(S.bits[k], P.ac_bits[ta], 16);
+          memcpy(S.vals[k], P.ac_vals[ta], 256);
+        }
+      }
+      S.start = i;
+      S.end = data_end(b, n, i, S.markers);
+      i = S.end;
+      // past the cap the scans are still checked, so that a later one libjpeg rejects is
+      // reported as libjpeg reports it
+      if ((int)G.scans.size() == kMaxScans) too_many = true;
+      else G.scans.push_back(S);
+    }
+    // APPn, COM and anything else: skipped
+  }
+  if (too_many) return SQDET_JPEG_TOO_MANY_SCANS;
+  if (bogus) return SQDET_JPEG_BOGUS_PROGRESSION;
+  if (smoothed(ncomp, G, cbits)) return SQDET_JPEG_SMOOTHED;
+  P.info.scan_offset = G.scans[0].start;
+  return SQDET_JPEG_OK;
+}
+
+// sqdet_jpeg_parse_progressive's reading of a file: sequential files as parse() reads them.
+int parse_any(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
+  const int reason = parse(b, n, P, true);
+  if (reason || !P.progressive) return reason;
+  return parse_scans(b, n, P, G);
+}
+
+// The scan's geometry: its units, blocks per unit and restart interval in units.
+void scan_geometry(const Parsed& P, const Layout& L, const PScan& S, ProgScan& D) {
+  const int ncomp = P.info.components;
+  D.ss = S.ss;
+  D.se = S.se;
+  D.ah = S.ah;
+  D.al = S.al;
+  D.single = S.ncomp == 1;
+  int uoff[3] = {0, 0, 0};
+  for (int c = 1; c < ncomp; ++c) uoff[c] = uoff[c - 1] + P.comp[c - 1].h * P.comp[c - 1].v;
+  if (D.single) {
+    const int c = S.comp[0];
+    const int hc = ncomp == 1 ? 1 : P.comp[c].h, vc = ncomp == 1 ? 1 : P.comp[c].v;
+    const int hmax = ncomp == 1 ? 1 : P.comp[0].h, vmax = ncomp == 1 ? 1 : P.comp[0].v;
+    const int64_t cw = ((int64_t)P.info.coded_width * hc + hmax - 1) / hmax;
+    const int64_t chh = ((int64_t)P.info.coded_height * vc + vmax - 1) / vmax;
+    D.cols = (int)((cw + 7) / 8);
+    D.units = D.cols * (int)((chh + 7) / 8);
+    D.nb = 1;
+    D.bc[0] = (int8_t)c;
+    D.bu[0] = (int8_t)(ncomp == 1 ? 0 : uoff[c]);
+    D.bt[0] = 0;
+  } else {
+    D.units = L.mcus;
+    D.cols = L.mcu_cols;
+    int j = 0;
+    for (int k = 0; k < S.ncomp; ++k) {
+      const int c = S.comp[k];
+      for (int q = 0; q < P.comp[c].h * P.comp[c].v; ++q, ++j) {
+        D.bc[j] = (int8_t)c;
+        D.bu[j] = (int8_t)(uoff[c] + q);
+        D.bt[j] = (int8_t)k;
+      }
+    }
+    D.nb = j;
+  }
+  D.per = S.restart ? std::min(S.restart, D.units) : D.units;
+  // only the intervals the scan's markers delimit are placed, so that the staging follows the
+  // file's bytes and not its DRI; a scan with fewer markers than intervals is corrupt
+  const int64_t need = (D.units + D.per - 1) / D.per;
+  D.intervals = (int)std::min<int64_t>(need, S.markers + 1);
+  D.bad = D.intervals < need;
+}
+
+// A call of the progressive entry points: its sequential files go through the sequential
+// pipeline as a Plan of their own, its progressive files through the kernels above.
+struct PPlan {
+  std::vector<int> seq, prg;           // the call's indices of each kind of file
+  Plan base;                           // the sequential files
+  std::vector<Parsed> parsed;          // the progressive files
+  std::vector<Layout> lay;
+  std::vector<Prog> prog;
+  std::vector<DecFile> files;
+  std::vector<ProgScan> scans;
+  std::vector<int2> items;             // first-scan items, then DC refinements, then each depth's
+  int first = 0, dc_refine = 0;
+  std::vector<int> depth;              // AC refinement items per depth
+  int64_t scan_off = 0, item_off = 0, pstaging = 0, coef = 0, coef_bytes = 0, pscratch = 0;
+  int64_t stage_at = 0, scratch_at = 0, status_at = 0;   // the progressive part; the statuses
+  int64_t staging = 0, scratch = 0;
+};
+
+// Parses every file and places every region.  The staging holds the sequential files' staging,
+// then the progressive files': their descriptors, the scan descriptors, the work items, then per
+// scan its tables, interval starts and clean data.  The scratch holds the sequential files'
+// scratch, then the progressive staging's copy, their coefficients and sample planes, then one
+// status per file of the call.
+int make_pplan(const std::string& name, int n, const uint8_t* const* files, const int64_t* lengths,
+               PPlan& plan) {
+  if (!files || !lengths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (n < 1 || n > kMaxFiles)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxFiles) + "]");
+  for (int i = 0; i < n; ++i) {
+    if (!files[i]) return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + " is null");
+    if (lengths[i] < 4 || lengths[i] > kMaxFileBytes)
+      return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + ": length must be in [4, 2^28]");
+    Parsed P;
+    Prog G;
+    const int reason = parse_any(files[i], lengths[i], P, G);
+    if (reason)
+      return fail(SQDET_ERR_UNSUPPORTED, name + ": file " + std::to_string(i) + " is not supported: " +
+                                             kReasons[reason]);
+    const Layout L = layout(P, lengths[i], g_sub_bits);
+    if (P.progressive) {
+      plan.prg.push_back(i);
+      plan.parsed.push_back(P);
+      plan.lay.push_back(L);
+      plan.prog.push_back(std::move(G));
+    } else {
+      plan.seq.push_back(i);
+      plan.base.parsed.push_back(P);
+      plan.base.lay.push_back(L);
+    }
+  }
+  if (!plan.seq.empty()) place(plan.base);
+  // work items: first scans, DC refinements, then AC refinements by their depth in their
+  // component's chain
+  std::vector<std::vector<int2>> depth_items;
+  std::vector<int2> dcref;
+  for (size_t i = 0; i < plan.prg.size(); ++i) {
+    int chain[3] = {0, 0, 0};
+    for (const PScan& S : plan.prog[i].scans) {
+      ProgScan D{};
+      D.file = (int)i;
+      scan_geometry(plan.parsed[i], plan.lay[i], S, D);
+      const int si = (int)plan.scans.size();
+      plan.scans.push_back(D);
+      if (S.ah == 0) {
+        for (int r = 0; r < D.intervals; ++r) plan.items.push_back(make_int2(si, r));
+      } else if (S.ss == 0) {
+        dcref.push_back(make_int2(si, 0));
+      } else {
+        const int d = chain[S.comp[0]]++;
+        if ((int)depth_items.size() <= d) depth_items.resize((size_t)d + 1);
+        for (int r = 0; r < D.intervals; ++r) depth_items[(size_t)d].push_back(make_int2(si, r));
+      }
+    }
+  }
+  plan.first = (int)plan.items.size();
+  plan.items.insert(plan.items.end(), dcref.begin(), dcref.end());
+  plan.dc_refine = (int)dcref.size();
+  for (const auto& v : depth_items) {
+    plan.items.insert(plan.items.end(), v.begin(), v.end());
+    plan.depth.push_back((int)v.size());
+  }
+  const size_t np = plan.prg.size();
+  plan.files.assign(np, DecFile{});
+  Carver c;
+  c.next((int64_t)sizeof(DecFile) * (int64_t)np);
+  plan.scan_off = c.next((int64_t)sizeof(ProgScan) * (int64_t)plan.scans.size());
+  plan.item_off = c.next((int64_t)sizeof(int2) * (int64_t)plan.items.size());
+  int si = 0;
+  for (size_t i = 0; i < np; ++i)
+    for (const PScan& S : plan.prog[i].scans) {
+      ProgScan& D = plan.scans[(size_t)si++];
+      D.tabs = c.next((int64_t)sizeof(HuffTab) * S.ncomp);
+      D.ist = c.next((int64_t)(D.intervals + 1) * 4);
+      D.clean = c.next(S.end - S.start + kScanPad);
+    }
+  plan.pstaging = c.offset;
+  plan.coef = c.offset;
+  for (size_t i = 0; i < np; ++i) plan.files[i].coef = c.next((int64_t)plan.lay[i].blocks * 128);
+  plan.coef_bytes = c.offset - plan.coef;
+  for (size_t i = 0; i < np; ++i)
+    for (int k = 0; k < plan.parsed[i].info.components; ++k)
+      plan.files[i].plane[k] = c.next((int64_t)plan.lay[i].pw[k] * plan.lay[i].ph[k]);
+  plan.pscratch = c.offset;
+  Carver whole;
+  whole.next(plan.seq.empty() ? 0 : plan.base.staging);
+  plan.stage_at = whole.next(np ? plan.pstaging : 0);
+  plan.staging = whole.offset;
+  whole = Carver{};
+  whole.next(plan.seq.empty() ? 0 : plan.base.scratch);
+  plan.scratch_at = whole.next(np ? plan.pscratch : 0);
+  plan.status_at = whole.next((int64_t)n * 4);
+  plan.scratch = whole.offset;
+  return SQDET_OK;
+}
+
+// Removes the stuffing of a scan's bytes and splits them at its RSTn markers into clean (ist[r]:
+// where interval r starts); whether the markers are in sequence and none is missing.  Markers
+// after the last interval's are skipped, as libjpeg skips them.
+bool destuff_scan(const uint8_t* b, int64_t start, int64_t end, int intervals, uint8_t* clean,
+                  int32_t* ist) {
+  int64_t o = 0;
+  int r = 0;
+  bool ok = true;
+  ist[0] = 0;
+  for (int64_t j = start; j < end; ++j) {
+    if (b[j] != 0xFF) {
+      clean[o++] = b[j];
+      continue;
+    }
+    const int nx = j + 1 < end ? b[j + 1] : -1;
+    if (nx == 0x00) {
+      clean[o++] = 0xFF;
+      ++j;
+    } else if (nx >= 0xD0 && nx <= 0xD7) {
+      if (r + 1 < intervals) {
+        ok = ok && nx == 0xD0 + (r & 7);
+        ist[r + 1] = (int32_t)o;
+      }
+      ++r;
+      ++j;
+    }
+  }
+  for (int k = std::min(r + 1, intervals); k <= intervals; ++k) ist[k] = (int32_t)o;
+  return ok && r + 1 >= intervals;
+}
+
+void fill_pstaging(const PPlan& plan, const uint8_t* const* files, uint8_t* const* out,
+                   const int64_t* pitch, uint8_t* stage) {
+  if (!plan.seq.empty()) {
+    std::vector<const uint8_t*> f;
+    std::vector<uint8_t*> o;
+    std::vector<int64_t> pt;
+    for (int i : plan.seq) {
+      f.push_back(files[i]);
+      o.push_back(out[i]);
+      pt.push_back(pitch[i]);
+    }
+    fill_staging(plan.base, (int)plan.seq.size(), f.data(), o.data(), pt.data(), stage);
+  }
+  if (plan.prg.empty()) return;
+  stage += plan.stage_at;
+  DecFile* fd = reinterpret_cast<DecFile*>(stage);
+  ProgScan* sc = reinterpret_cast<ProgScan*>(stage + plan.scan_off);
+  int si = 0;
+  for (size_t i = 0; i < plan.prg.size(); ++i) {
+    const int k = plan.prg[i];
+    const Parsed& P = plan.parsed[i];
+    const Prog& G = plan.prog[i];
+    DecFile f = plan.files[i];
+    describe(P, plan.lay[i], f);
+    for (int c = 0; c < P.info.components; ++c)          // the tables latched at the first scans
+      for (int q = 0; q < 64; ++q) f.q[c][q] = G.latched[c] ? (int16_t)G.q[c][q] : 0;
+    f.out = out[k];
+    f.pitch = pitch[k];
+    fd[i] = f;
+    for (const PScan& S : G.scans) {
+      ProgScan D = plan.scans[(size_t)si];
+      HuffTab* tabs = reinterpret_cast<HuffTab*>(stage + D.tabs);
+      const bool coded = S.ss != 0 || S.ah == 0;
+      for (int t = 0; coded && t < (S.ss ? 1 : S.ncomp); ++t) build_tab(S.bits[t], S.vals[t], tabs[t]);
+      uint8_t* clean = stage + D.clean;
+      const bool ok = destuff_scan(files[k], S.start, S.end, D.intervals, clean,
+                                   reinterpret_cast<int32_t*>(stage + D.ist));
+      D.bad = D.bad || !ok;
+      const int32_t len = reinterpret_cast<int32_t*>(stage + D.ist)[D.intervals];
+      memset(clean + len, 0, (size_t)(S.end - S.start - len + kScanPad));
+      sc[si++] = D;
+    }
+  }
+  memcpy(stage + plan.item_off, plan.items.data(), sizeof(int2) * plan.items.size());
+}
+
+// The call's index of each status the two pipelines wrote: the sequential files', then the
+// progressive files'.
+struct StatusOrder {
+  int32_t n, at[kMaxFiles];
+};
+
+__global__ void scatter_status_kernel(const int32_t* tmp, StatusOrder o, int32_t* status) {
+  const int i = threadIdx.x;
+  if (i < o.n) status[o.at[i]] = tmp[i];
+}
+
+int launch_pdecode(const PPlan& plan, int n, uint8_t* stage, uint8_t* scratch, int32_t* status,
+                   cudaStream_t stream) {
+  int32_t* tmp = reinterpret_cast<int32_t*>(scratch + plan.status_at);
+  const int nb = (int)plan.seq.size(), np = (int)plan.prg.size();
+  if (nb) {
+    const int rc = launch_decode(plan.base, nb, stage, scratch, tmp, stream);
+    if (rc) return rc;
+  }
+  if (np) {
+    uint8_t* s = scratch + plan.scratch_at;
+    SQ_CUDA(cudaMemcpyAsync(s, stage + plan.stage_at, (size_t)plan.pstaging, cudaMemcpyHostToDevice, stream));
+    SQ_CUDA(cudaMemsetAsync(tmp + nb, 0, sizeof(int32_t) * (size_t)np, stream));
+    SQ_CUDA(cudaMemsetAsync(s + plan.coef, 0, (size_t)plan.coef_bytes, stream));
+    ProgParams pp{reinterpret_cast<DecFile*>(s), reinterpret_cast<const ProgScan*>(s + plan.scan_off),
+                  reinterpret_cast<const int2*>(s + plan.item_off), 0, s, tmp + nb};
+    if (plan.first) {
+      pp.nitems = plan.first;
+      prog_seq_kernel<<<(unsigned)plan.first, kProgThreads, 0, stream>>>(pp);
+      SQ_CHECK_LAUNCH("jpeg prog_seq_kernel (first scans)");
+    }
+    int at = plan.first;
+    if (plan.dc_refine) {
+      int max_blocks = 0;
+      for (int k = 0; k < plan.dc_refine; ++k) {
+        const ProgScan& S = plan.scans[(size_t)plan.items[(size_t)(at + k)].x];
+        max_blocks = std::max(max_blocks, S.units * S.nb);
+      }
+      ProgParams q = pp;
+      q.items += at;
+      q.nitems = plan.dc_refine;
+      prog_dc_refine_kernel<<<dim3((unsigned)((max_blocks + kPixThreads - 1) / kPixThreads), (unsigned)plan.dc_refine),
+                              kPixThreads, 0, stream>>>(q);
+      SQ_CHECK_LAUNCH("jpeg prog_dc_refine_kernel");
+      at += plan.dc_refine;
+    }
+    for (int d : plan.depth) {
+      ProgParams q = pp;
+      q.items += at;
+      q.nitems = d;
+      prog_seq_kernel<<<(unsigned)d, kProgThreads, 0, stream>>>(q);
+      SQ_CHECK_LAUNCH("jpeg prog_seq_kernel (AC refinements)");
+      at += d;
+    }
+    int max_blocks = 0;
+    int64_t max_pix = 0;
+    for (int i = 0; i < np; ++i) {
+      max_blocks = std::max(max_blocks, plan.lay[(size_t)i].blocks);
+      max_pix = std::max(max_pix, (int64_t)plan.parsed[(size_t)i].info.height * plan.parsed[(size_t)i].info.width);
+    }
+    DecParams p{reinterpret_cast<DecFile*>(s), s, tmp + nb};
+    idct_kernel<<<dim3((unsigned)((max_blocks + kPixThreads - 1) / kPixThreads), (unsigned)np), kPixThreads, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg idct_kernel");
+    color_kernel<<<dim3((unsigned)((max_pix + kPixThreads - 1) / kPixThreads), (unsigned)np), kPixThreads, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg color_kernel");
+  }
+  StatusOrder o{};
+  o.n = n;
+  for (int j = 0; j < nb; ++j) o.at[j] = plan.seq[(size_t)j];
+  for (int j = 0; j < np; ++j) o.at[nb + j] = plan.prg[(size_t)j];
+  scatter_status_kernel<<<1, kMaxFiles, 0, stream>>>(tmp, o, status);
+  SQ_CHECK_LAUNCH("jpeg scatter_status_kernel");
+  return SQDET_OK;
+}
+
 }  // namespace
 }  // namespace sqdet
 
@@ -1177,37 +1958,68 @@ int sqdet_decode_jpeg(int n, const uint8_t* const* files_host, const int64_t* le
   Plan plan;
   int rc = make_plan(name, n, files_host, lengths, plan);
   if (rc) return rc;
-  if ((uintptr_t)scratch_dev % 256) return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
-  if ((uintptr_t)status_dev % alignof(int32_t))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": status_dev must be 4-byte aligned");
-  if (staging_bytes < plan.staging)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": staging_bytes is below sqdet_jpeg_decode_staging_bytes");
-  if (scratch_bytes < plan.scratch)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_bytes is below sqdet_jpeg_decode_scratch_bytes");
-  cudaPointerAttributes attr;
-  if (cudaPointerGetAttributes(&attr, staging_pinned) != cudaSuccess || attr.type != cudaMemoryTypeHost) {
-    (void)cudaGetLastError();
-    return fail(SQDET_ERR_INVALID_ARG, name + ": staging_pinned is not page-locked host memory");
-  }
-  if (!out_planes[0]) return fail(SQDET_ERR_INVALID_ARG, name + ": output 0 is null");
-  const int device = pointer_device(out_planes[0]);
-  if (device < 0) return fail(SQDET_ERR_INVALID_ARG, name + ": output 0 is not device memory");
-  for (int i = 0; i < n; ++i) {
-    const sqdet_jpeg_info& I = plan.parsed[(size_t)i].info;
-    const std::string which = name + ": output " + std::to_string(i);
-    if (!out_planes[i]) return fail(SQDET_ERR_INVALID_ARG, which + " is null");
-    if (out_pitches[i] < 3 * (int64_t)I.width) return fail(SQDET_ERR_INVALID_ARG, which + ": pitch below 3 * width");
-    const int64_t bytes = (int64_t)(I.height - 1) * out_pitches[i] + 3 * (int64_t)I.width;
-    if (!device_range_ok(out_planes[i], bytes, device))
-      return fail(SQDET_ERR_INVALID_ARG, which + " is not inside one device allocation on output 0's device");
-  }
-  if (!device_range_ok(status_dev, (int64_t)n * 4, device) ||
-      !device_range_ok(scratch_dev, scratch_bytes, device))
-    return fail(SQDET_ERR_INVALID_ARG, name + ": status_dev or scratch_dev is not inside one device "
-                                              "allocation on output 0's device");
+  std::vector<const sqdet_jpeg_info*> info((size_t)n);
+  for (int i = 0; i < n; ++i) info[(size_t)i] = &plan.parsed[(size_t)i].info;
+  rc = check_decode_args(name, n, info.data(), out_planes, out_pitches, staging_pinned, staging_bytes,
+                         plan.staging, scratch_dev, scratch_bytes, plan.scratch, status_dev,
+                         "sqdet_jpeg_decode_staging_bytes", "sqdet_jpeg_decode_scratch_bytes");
+  if (rc) return rc;
   fill_staging(plan, n, files_host, out_planes, out_pitches, static_cast<uint8_t*>(staging_pinned));
-  DeviceGuard guard(device);
+  DeviceGuard guard(pointer_device(out_planes[0]));
   if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select output 0's device");
   return launch_decode(plan, n, static_cast<uint8_t*>(staging_pinned), static_cast<uint8_t*>(scratch_dev),
                        status_dev, (cudaStream_t)stream);
+}
+
+int sqdet_jpeg_parse_progressive(const uint8_t* file, int64_t len, sqdet_jpeg_info* out) {
+  if (!file || !out || len < 0)
+    return fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_parse_progressive: bad argument");
+  Parsed P;
+  Prog G;
+  const int reason = parse_any(file, len, P, G);
+  P.info.reason = reason;
+  if (reason) P.info.supported = 0;
+  *out = P.info;
+  if (reason)
+    return fail(SQDET_ERR_UNSUPPORTED, std::string("sqdet_jpeg_parse_progressive: not supported: ") + kReasons[reason]);
+  return SQDET_OK;
+}
+
+int64_t sqdet_jpeg_decode_staging_bytes_progressive(int n, const uint8_t* const* files_host,
+                                                    const int64_t* lengths) {
+  PPlan plan;
+  if (make_pplan("sqdet_jpeg_decode_staging_bytes_progressive", n, files_host, lengths, plan)) return -1;
+  return plan.staging;
+}
+
+int64_t sqdet_jpeg_decode_scratch_bytes_progressive(int n, const uint8_t* const* files_host,
+                                                    const int64_t* lengths) {
+  PPlan plan;
+  if (make_pplan("sqdet_jpeg_decode_scratch_bytes_progressive", n, files_host, lengths, plan)) return -1;
+  return plan.scratch;
+}
+
+int sqdet_decode_jpeg_progressive(int n, const uint8_t* const* files_host, const int64_t* lengths,
+                                  uint8_t* const* out_planes, const int64_t* out_pitches,
+                                  void* staging_pinned, int64_t staging_bytes, void* scratch_dev,
+                                  int64_t scratch_bytes, int32_t* status_dev, void* stream) {
+  const std::string name = "sqdet_decode_jpeg_progressive";
+  if (!out_planes || !out_pitches || !staging_pinned || !scratch_dev || !status_dev)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  PPlan plan;
+  int rc = make_pplan(name, n, files_host, lengths, plan);
+  if (rc) return rc;
+  std::vector<const sqdet_jpeg_info*> info((size_t)n);
+  for (size_t j = 0; j < plan.seq.size(); ++j) info[(size_t)plan.seq[j]] = &plan.base.parsed[j].info;
+  for (size_t j = 0; j < plan.prg.size(); ++j) info[(size_t)plan.prg[j]] = &plan.parsed[j].info;
+  rc = check_decode_args(name, n, info.data(), out_planes, out_pitches, staging_pinned, staging_bytes,
+                         plan.staging, scratch_dev, scratch_bytes, plan.scratch, status_dev,
+                         "sqdet_jpeg_decode_staging_bytes_progressive",
+                         "sqdet_jpeg_decode_scratch_bytes_progressive");
+  if (rc) return rc;
+  fill_pstaging(plan, files_host, out_planes, out_pitches, static_cast<uint8_t*>(staging_pinned));
+  DeviceGuard guard(pointer_device(out_planes[0]));
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select output 0's device");
+  return launch_pdecode(plan, n, static_cast<uint8_t*>(staging_pinned), static_cast<uint8_t*>(scratch_dev),
+                        status_dev, (cudaStream_t)stream);
 }

@@ -76,7 +76,7 @@ def encode_jpeg_device(frames, fmt, crops=None, quality=95, stream=None, *, samp
   (sqdet_encode_jpeg_progressive): the same coefficients in jpeg_simple_progression's ten scans,
   each with its own optimal tables, so optimize has no effect; a restart interval counts blocks in
   the eight single-component scans.  Its worst-case cap is about 2.1 times the baseline one at
-  4:2:0.  decode_jpeg_device does not read these files; cv2.imdecode does."""
+  4:2:0.  decode_jpeg_device(..., progressive=True) reads these files back."""
   settings = dict(quality=quality, sampling=sampling, optimize=optimize,
                   restart_interval=restart_interval, luma_quality=luma_quality,
                   chroma_quality=chroma_quality)
@@ -93,18 +93,21 @@ jpeg_bytes = file_bytes
 
 # ---- decoding ------------------------------------------------------------------------------------
 JPEG_TOO_LARGE = 10       # SQDET_JPEG_TOO_LARGE: past cv2's limits, so cv2.imdecode refuses it too
+JPEG_BAD_PROGRESSION = 11  # SQDET_JPEG_BAD_PROGRESSION: cv2.imdecode returns None
 
 
-def jpeg_info(file_bytes):
+def jpeg_info(file_bytes, progressive=False):
   """sqdet_jpeg_parse of one file -> dict: height and width of the decoded frame (after the EXIF
   orientation), coded_height, coded_width, components, h_samp, v_samp (luma sampling),
   orientation, restart_interval, supported (bool), reason (a SQDET_JPEG_* code) and reason_text
-  (the library's words for it).  Host only."""
+  (the library's words for it).  With progressive, sqdet_jpeg_parse_progressive: whether
+  decode_jpeg_device(..., progressive=True) decodes it.  Host only."""
   b = bytes(file_bytes)
   info = _lib.JpegInfo()
   buf = C.create_string_buffer(b, len(b))
   lib = _lib.load()
-  rc = lib.sqdet_jpeg_parse(buf, len(b), C.byref(info))
+  parse = lib.sqdet_jpeg_parse_progressive if progressive else lib.sqdet_jpeg_parse
+  rc = parse(buf, len(b), C.byref(info))
   if rc not in (_lib.OK, -3):
     _lib.check(rc)
   out = {k: int(getattr(info, k)) for k, _ in _lib.JpegInfo._fields_ if k != 'reserved'}
@@ -139,7 +142,7 @@ class _Staging:
 _staging = {}
 
 
-def decode_jpeg_device(files, device, stream=None):
+def decode_jpeg_device(files, device, stream=None, *, progressive=False):
   """JPEG files (bytes-like, on the host) -> (frames, status): frames[i] is a uint8 [H, W, 3] BGR
   CUDA tensor on `device` with exactly the pixels of cv2.imdecode(files[i], cv2.IMREAD_COLOR), and
   status an int32 [n] CUDA tensor, 0 where the file decoded and negative where its entropy-coded
@@ -157,7 +160,16 @@ def decode_jpeg_device(files, device, stream=None):
   stream): the frames, status and scratch are allocated on it, so read them on it or after
   synchronising it.  The files go to the device through two pinned staging buffers this module
   owns per device and uses in turn; a call waits (on the host) only until the call before the
-  previous one has finished on its stream."""
+  previous one has finished on its stream.
+
+  progressive=True (sqdet_decode_jpeg_progressive) decodes progressive (SOF2) files too, in the
+  same batch, again to exactly cv2.imdecode's pixels; the other files give the frames of the plain
+  call.  Besides the plain call's refusals it raises ValueError for a scan script libjpeg rejects
+  (cv2.imdecode returns None) or warns on or lets overwrite a coefficient, for a scan whose
+  components are out of the frame's order, for a file libjpeg would block-smooth (an incomplete
+  one: complete files, such as every file cv2 or encode_jpeg_device writes, are not smoothed) and
+  for more than 256 scans; route those to cv2.imdecode.  A progressive scan without restart
+  markers is decoded by one GPU lane, so these files decode much slower than sequential ones."""
   import torch
   files = [bytes(f) for f in files]
   n = len(files)
@@ -172,18 +184,19 @@ def decode_jpeg_device(files, device, stream=None):
   for i, f in enumerate(files):
     if len(f) < 4:
       raise ValueError('file %d: not a JPEG file (%d bytes)' % (i, len(f)))
-    info = jpeg_info(f)
+    info = jpeg_info(f, progressive)
     if not info['supported']:
       raise ValueError('file %d: not supported (%s); %s' % (
           i, info['reason_text'], 'nor does cv2.imdecode decode it'
-          if info['reason'] == JPEG_TOO_LARGE else 'decode it with cv2.imdecode'))
+          if info['reason'] in (JPEG_TOO_LARGE, JPEG_BAD_PROGRESSION) else 'decode it with cv2.imdecode'))
     infos.append(info)
   lib = _lib.load()
   bufs = [C.create_string_buffer(f, len(f)) for f in files]
   ptrs = (C.c_void_p * n)(*[C.addressof(b) for b in bufs])
   lens = (C.c_int64 * n)(*[len(f) for f in files])
-  staging_bytes = lib.sqdet_jpeg_decode_staging_bytes(n, ptrs, lens)
-  scratch_bytes = lib.sqdet_jpeg_decode_scratch_bytes(n, ptrs, lens)
+  kind = '_progressive' if progressive else ''
+  staging_bytes = getattr(lib, 'sqdet_jpeg_decode_staging_bytes' + kind)(n, ptrs, lens)
+  scratch_bytes = getattr(lib, 'sqdet_jpeg_decode_scratch_bytes' + kind)(n, ptrs, lens)
   if staging_bytes < 0 or scratch_bytes < 0:
     raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
   s = torch_stream(stream, device)
@@ -196,9 +209,9 @@ def decode_jpeg_device(files, device, stream=None):
     scratch = torch.empty((scratch_bytes,), dtype=torch.uint8, device=device)
     outs = (C.c_void_p * n)(*[t.data_ptr() for t in frames])
     pitches = (C.c_int64 * n)(*[3 * t.shape[1] for t in frames])
-    _lib.check(lib.sqdet_decode_jpeg(n, ptrs, lens, outs, pitches, buf.data_ptr(), buf.numel(),
-                                     scratch.data_ptr(), scratch_bytes, status.data_ptr(),
-                                     s.cuda_stream))
+    _lib.check(getattr(lib, 'sqdet_decode_jpeg' + kind)(
+        n, ptrs, lens, outs, pitches, buf.data_ptr(), buf.numel(), scratch.data_ptr(),
+        scratch_bytes, status.data_ptr(), s.cuda_stream))
     staging.events[slot] = torch.cuda.Event()
     staging.events[slot].record(s)
   return frames, status
