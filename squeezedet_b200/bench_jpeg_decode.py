@@ -40,8 +40,7 @@ QUALITY = 95
 KERNELS = ('destuff_count_kernel', 'scan_chunks_kernel', 'destuff_compact_kernel',
            'intervals_kernel', 'sync_tiles_kernel', 'sync_chain_kernel', 'scan_counts_kernel',
            'decode_write_kernel', 'idct_kernel', 'color_kernel')
-PROG_KERNELS = ('prog_seq_kernel', 'prog_dc_refine_kernel', 'idct_kernel', 'color_kernel',
-                'scatter_status_kernel')
+PROG_KERNELS = ('prog_seq_kernel', 'prog_dc_refine_kernel', 'idct_kernel', 'color_kernel')
 
 
 def parse_args(argv=None):

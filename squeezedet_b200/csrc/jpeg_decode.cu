@@ -36,6 +36,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "scan.cuh"
 
 namespace sqdet {
 
@@ -86,6 +87,7 @@ struct DecFile {
   int32_t pw[3], ph[3];                // padded plane width and height (whole blocks)
   int32_t cw[3], chh[3];               // component width and height in samples
   int16_t q[3][64];                    // dequantization, natural order (libjpeg's short multiplier)
+  int32_t index;                       // the file's index in the call: where its status goes
   int64_t raw, clean, sums, term, ist, sbase, entry, exit_, counts, coef, plane[3], tabs;
   uint8_t* out;
   int64_t pitch;
@@ -97,34 +99,8 @@ struct DecParams {
   int32_t* status;
 };
 
-__device__ __forceinline__ void fail_file(int32_t* status, int i, int code) { status[i] = code; }
-
-// ---- block-wide exclusive scan (blockDim.x a multiple of 32) ------------------------------------
-template <class T>
-__device__ T block_scan(T v, T* warp, T* total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  T x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const T y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp[wid] = x;
-  __syncthreads();
-  if (wid == 0) {
-    T w = lane < nw ? warp[lane] : T(0);
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const T y = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += y;
-    }
-    if (lane < nw) warp[lane] = w;
-  }
-  __syncthreads();
-  const T before = (wid ? warp[wid - 1] : T(0)) + x - v;
-  *total = warp[nw - 1];
-  __syncthreads();
-  return before;
+__device__ __forceinline__ void fail_file(int32_t* status, const DecFile& f, int code) {
+  status[f.index] = code;
 }
 
 // ---- 1. destuff counts ---------------------------------------------------------------------------
@@ -165,7 +141,7 @@ __global__ void __launch_bounds__(kChunkThreads) destuff_count_kernel(DecParams 
   }
   if (term != INT32_MAX) atomicMin(reinterpret_cast<uint32_t*>(p.s + f.term), (uint32_t)term);
   int64_t total;
-  block_scan<int64_t>(v, warp, &total);
+  block_exclusive_scan(v, warp, &total);
   if (threadIdx.x == 0) reinterpret_cast<int64_t*>(p.s + f.sums)[blockIdx.x] = total;
 }
 
@@ -179,7 +155,7 @@ __global__ void __launch_bounds__(kScanThreads) scan_chunks_kernel(DecParams p) 
     const int i = base + threadIdx.x;
     const int64_t v = i < f.chunks ? s[i] : 0;
     int64_t total;
-    const int64_t ex = block_scan<int64_t>(v, warp, &total);
+    const int64_t ex = block_exclusive_scan(v, warp, &total);
     if (i < f.chunks) s[i] = carry + ex;
     carry += total;
   }
@@ -207,7 +183,7 @@ __global__ void __launch_bounds__(kChunkThreads) destuff_compact_kernel(DecParam
     v += cls[i] == 0 ? 1 : cls[i] == 2 ? kRstOne : 0;
   }
   int64_t total;
-  const int64_t at = reinterpret_cast<const int64_t*>(p.s + f.sums)[blockIdx.x] + block_scan<int64_t>(v, warp, &total);
+  const int64_t at = reinterpret_cast<const int64_t*>(p.s + f.sums)[blockIdx.x] + block_exclusive_scan(v, warp, &total);
   int64_t o = at & (kRstOne - 1);
   int r = (int)(at >> 40);
   for (int i = 0; i < kChunkBytes; ++i) {
@@ -222,7 +198,7 @@ __global__ void __launch_bounds__(kChunkThreads) destuff_compact_kernel(DecParam
       // the r-th marker ends interval r and must be RST(r mod 8); markers after the last
       // interval's are skipped, as libjpeg skips them
       if (r + 1 < f.intervals) {
-        if (raw[j + 1] != 0xD0 + (r & 7)) fail_file(p.status, blockIdx.y, -2);
+        if (raw[j + 1] != 0xD0 + (r & 7)) fail_file(p.status, f, -2);
         ist[r + 1] = (int32_t)o;
       }
       ++r;
@@ -259,11 +235,11 @@ __global__ void __launch_bounds__(kScanThreads) intervals_kernel(DecParams p) {
       }
     }
     int32_t total;
-    const int32_t ex = block_scan<int32_t>(v, warp, &total);
+    const int32_t ex = block_exclusive_scan(v, warp, &total);
     if (r < f.intervals) sbase[r] = carry + ex;
     carry += total;
   }
-  if (bad) fail_file(p.status, i, -3);
+  if (bad) fail_file(p.status, f, -3);
   if (threadIdx.x == 0) sbase[f.intervals] = min(carry, f.sub_max);
 }
 
@@ -502,10 +478,10 @@ __global__ void __launch_bounds__(kScanThreads) scan_counts_kernel(DecParams p) 
     const int i = base + threadIdx.x;
     const int4 v = i < nsub ? c[i] : make_int4(0, 0, 0, 0);
     int4 ex, tot;
-    ex.x = block_scan<int32_t>(v.x, warp, &tot.x);
-    ex.y = block_scan<int32_t>(v.y, warp, &tot.y);
-    ex.z = block_scan<int32_t>(v.z, warp, &tot.z);
-    ex.w = block_scan<int32_t>(v.w, warp, &tot.w);
+    ex.x = block_exclusive_scan(v.x, warp, &tot.x);
+    ex.y = block_exclusive_scan(v.y, warp, &tot.y);
+    ex.z = block_exclusive_scan(v.z, warp, &tot.z);
+    ex.w = block_exclusive_scan(v.w, warp, &tot.w);
     if (i < nsub) c[i] = make_int4(carry.x + ex.x, carry.y + ex.y, carry.z + ex.z, carry.w + ex.w);
     carry = make_int4(carry.x + tot.x, carry.y + tot.y, carry.z + tot.z, carry.w + tot.w);
   }
@@ -527,7 +503,7 @@ __global__ void __launch_bounds__(kTile) decode_write_kernel(DecParams p) {
   Counts c{mine.x - base.x, {mine.y - base.y, mine.z - base.z, mine.w - base.w}};
   const int b0 = c.blocks;
   if (b0 < 0) {
-    fail_file(p.status, blockIdx.y, -6);
+    fail_file(p.status, f, -6);
     return;
   }
   State st = reinterpret_cast<const State*>(p.s + f.entry)[g];
@@ -541,11 +517,11 @@ __global__ void __launch_bounds__(kTile) decode_write_kernel(DecParams p) {
                            : 0;
   const int end_bits = max(ist[sub.r + 1], 0) * 8;
   if (rc) {
-    fail_file(p.status, blockIdx.y, rc);
+    fail_file(p.status, f, rc);
   } else if (st.p > end_bits) {
-    fail_file(p.status, blockIdx.y, -7);                 // ran off the interval's data
+    fail_file(p.status, f, -7);                          // ran off the interval's data
   } else if (sub.j == sub.nsub - 1 && b0 + c.blocks < interval_blocks) {
-    fail_file(p.status, blockIdx.y, -8);                 // too few blocks in the interval
+    fail_file(p.status, f, -8);                          // too few blocks in the interval
   }
   // data after an interval's last block is skipped, as libjpeg skips it before the next marker
 }
@@ -785,9 +761,70 @@ bool huff_ok(const uint8_t* bits, const uint8_t* vals, bool dc) {
   return true;
 }
 
+// One marker segment: its marker, where the marker starts and its body.
+struct Segment {
+  int m;
+  int64_t at;
+  const uint8_t* body;
+  int bn;
+};
+
+// Reads the marker segment at i, after any fill bytes, and moves i past it; the reason
+// (SQDET_JPEG_*).  A standalone marker (SOI, EOI, RSTn, TEM) or a length past the end is malformed.
+// With `eoi_ends`, the end of the data or an EOI there is not: it reads as s.m = EOI.
+int next_segment(const uint8_t* b, int64_t n, int64_t& i, bool eoi_ends, Segment& s) {
+  while (i + 1 < n && b[i] == 0xFF && b[i + 1] == 0xFF) ++i;
+  if (eoi_ends && i >= n) {
+    s.m = 0xD9;
+    return SQDET_JPEG_OK;
+  }
+  if (i + 2 > n || b[i] != 0xFF) return SQDET_JPEG_MALFORMED;
+  s.at = i;
+  s.m = b[i + 1];
+  i += 2;
+  if (eoi_ends && s.m == 0xD9) return SQDET_JPEG_OK;
+  if (s.m == 0xD8 || s.m == 0xD9 || (s.m >= 0xD0 && s.m <= 0xD7) || s.m == 0x01) return SQDET_JPEG_MALFORMED;
+  if (i + 2 > n) return SQDET_JPEG_MALFORMED;
+  const int len = u16(b, i);
+  if (len < 2 || i + len > n) return SQDET_JPEG_MALFORMED;
+  s.body = b + i + 2;
+  s.bn = len - 2;
+  i += len;
+  return SQDET_JPEG_OK;
+}
+
+// A DQT or DHT segment's tables into P; the reason.  Other segments are the caller's.
+int read_tables(const Segment& s, Parsed& P) {
+  const uint8_t* body = s.body;
+  const int bn = s.bn;
+  if (s.m == 0xDB) {
+    for (int j = 0; j < bn;) {
+      const int pq = body[j] >> 4, tq = body[j] & 15, size = pq ? 128 : 64;
+      if (pq > 1 || tq > 3 || j + 1 + size > bn) return SQDET_JPEG_MALFORMED;
+      for (int k = 0; k < 64; ++k)
+        P.qt[tq][kNatural[k]] = pq ? (uint16_t)u16(body, j + 1 + 2 * k) : body[j + 1 + k];
+      P.have_q[tq] = true;
+      j += 1 + size;
+    }
+  } else if (s.m == 0xC4) {
+    for (int j = 0; j < bn;) {
+      if (j + 17 > bn) return SQDET_JPEG_MALFORMED;
+      const int tc = body[j] >> 4, th = body[j] & 15;
+      int cnt = 0;
+      for (int l = 0; l < 16; ++l) cnt += body[j + 1 + l];
+      if (tc > 1 || th > 3 || cnt > 256 || j + 17 + cnt > bn) return SQDET_JPEG_MALFORMED;
+      memcpy(tc ? P.ac_bits[th] : P.dc_bits[th], body + j + 1, 16);
+      memcpy(tc ? P.ac_vals[th] : P.dc_vals[th], body + j + 17, (size_t)cnt);
+      (tc ? P.have_ac : P.have_dc)[th] = true;
+      j += 17 + cnt;
+    }
+  }
+  return SQDET_JPEG_OK;
+}
+
 // The headers up to the first SOS; the reason (SQDET_JPEG_*) and what was read.  With
 // `progressive`, an SOF2 frame is read as SOF0's is and the first SOS is left to parse_scans.
-int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive = false) {
+int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive) {
   memset(&P, 0, sizeof(P));
   sqdet_jpeg_info& I = P.info;
   I.orientation = 1;
@@ -796,17 +833,11 @@ int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive = false) {
   bool frame = false, exif = false, jfif = false;
   int64_t i = 2;
   for (;;) {
-    while (i + 1 < n && b[i] == 0xFF && b[i + 1] == 0xFF) ++i;
-    if (i + 2 > n || b[i] != 0xFF) return SQDET_JPEG_MALFORMED;
-    const int m = b[i + 1];
-    i += 2;
-    if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) return SQDET_JPEG_MALFORMED;
-    if (i + 2 > n) return SQDET_JPEG_MALFORMED;
-    const int len = u16(b, i);
-    if (len < 2 || i + len > n) return SQDET_JPEG_MALFORMED;
-    const uint8_t* body = b + i + 2;
-    const int bn = len - 2;
-    i += len;
+    Segment s;
+    if (const int r = next_segment(b, n, i, false, s)) return r;
+    if (const int r = read_tables(s, P)) return r;
+    const int m = s.m, bn = s.bn;
+    const uint8_t* body = s.body;
     if ((m == 0xC2 && !progressive) || m == 0xC6 || m == 0xCA || m == 0xCE) return SQDET_JPEG_PROGRESSIVE;
     if (m == 0xC9 || m == 0xCB || m == 0xCD || m == 0xCF) return SQDET_JPEG_ARITHMETIC;
     if (m == 0xC3 || m == 0xC7) return SQDET_JPEG_LOSSLESS;
@@ -842,27 +873,6 @@ int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive = false) {
         if (!luma_ok) return SQDET_JPEG_SAMPLING;
       }
       frame = true;
-    } else if (m == 0xDB) {
-      for (int j = 0; j < bn;) {
-        const int pq = body[j] >> 4, tq = body[j] & 15, size = pq ? 128 : 64;
-        if (pq > 1 || tq > 3 || j + 1 + size > bn) return SQDET_JPEG_MALFORMED;
-        for (int k = 0; k < 64; ++k)
-          P.qt[tq][kNatural[k]] = pq ? (uint16_t)u16(body, j + 1 + 2 * k) : body[j + 1 + k];
-        P.have_q[tq] = true;
-        j += 1 + size;
-      }
-    } else if (m == 0xC4) {
-      for (int j = 0; j < bn;) {
-        if (j + 17 > bn) return SQDET_JPEG_MALFORMED;
-        const int tc = body[j] >> 4, th = body[j] & 15;
-        int cnt = 0;
-        for (int l = 0; l < 16; ++l) cnt += body[j + 1 + l];
-        if (tc > 1 || th > 3 || cnt > 256 || j + 17 + cnt > bn) return SQDET_JPEG_MALFORMED;
-        memcpy(tc ? P.ac_bits[th] : P.dc_bits[th], body + j + 1, 16);
-        memcpy(tc ? P.ac_vals[th] : P.dc_vals[th], body + j + 17, (size_t)cnt);
-        (tc ? P.have_ac : P.have_dc)[th] = true;
-        j += 17 + cnt;
-      }
     } else if (m == 0xDD) {
       if (bn != 2) return SQDET_JPEG_MALFORMED;
       I.restart_interval = u16(body, 0);
@@ -875,45 +885,33 @@ int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive = false) {
       adobe = body[11];
     } else if (m == 0xDA) {
       if (!frame || bn < 1) return SQDET_JPEG_MALFORMED;
-      if (P.progressive) {
-        if (ncomp == 3 && !jfif &&
-            (adobe >= 0 ? adobe == 0
-                        : P.comp[0].id == 'R' && P.comp[1].id == 'G' && P.comp[2].id == 'B'))
-          return SQDET_JPEG_COLOR_TRANSFORM;
-        P.first_sos = i - len - 2;
-        I.h_samp = ncomp == 1 ? 1 : P.comp[0].h;
-        I.v_samp = ncomp == 1 ? 1 : P.comp[0].v;
-        const bool swap = I.orientation >= 5;
-        I.height = swap ? I.coded_width : I.coded_height;
-        I.width = swap ? I.coded_height : I.coded_width;
-        I.supported = 1;
-        return SQDET_JPEG_OK;
-      }
-      const int ns = body[0];
-      if (bn != 4 + 2 * ns) return SQDET_JPEG_MALFORMED;
-      if (ns != ncomp) return SQDET_JPEG_SAMPLING;
-      for (int k = 0; k < ns; ++k) {
-        Comp& c = P.comp[k];
-        if (body[1 + 2 * k] != c.id) return SQDET_JPEG_SAMPLING;
-        c.td = body[2 + 2 * k] >> 4;
-        c.ta = body[2 + 2 * k] & 15;
-        if (c.td > 3 || c.ta > 3 || !P.have_dc[c.td] || !P.have_ac[c.ta] || !P.have_q[c.tq])
-          return SQDET_JPEG_MALFORMED;
-        if (!huff_ok(P.dc_bits[c.td], P.dc_vals[c.td], true) || !huff_ok(P.ac_bits[c.ta], P.ac_vals[c.ta], false))
+      if (!P.progressive) {                 // the one scan of a sequential file
+        const int ns = body[0];
+        if (bn != 4 + 2 * ns) return SQDET_JPEG_MALFORMED;
+        if (ns != ncomp) return SQDET_JPEG_SAMPLING;
+        for (int k = 0; k < ns; ++k) {
+          Comp& c = P.comp[k];
+          if (body[1 + 2 * k] != c.id) return SQDET_JPEG_SAMPLING;
+          c.td = body[2 + 2 * k] >> 4;
+          c.ta = body[2 + 2 * k] & 15;
+          if (c.td > 3 || c.ta > 3 || !P.have_dc[c.td] || !P.have_ac[c.ta] || !P.have_q[c.tq])
+            return SQDET_JPEG_MALFORMED;
+          if (!huff_ok(P.dc_bits[c.td], P.dc_vals[c.td], true) || !huff_ok(P.ac_bits[c.ta], P.ac_vals[c.ta], false))
+            return SQDET_JPEG_MALFORMED;
+        }
+        if (body[1 + 2 * ns] != 0 || body[2 + 2 * ns] != 63 || body[3 + 2 * ns] != 0)
           return SQDET_JPEG_MALFORMED;
       }
-      if (body[1 + 2 * ns] != 0 || body[2 + 2 * ns] != 63 || body[3 + 2 * ns] != 0)
-        return SQDET_JPEG_MALFORMED;
       // libjpeg's colour space of 3 components: YCbCr after a JFIF APP0; else as an Adobe APP14's
       // transform says (0: RGB); else RGB for component ids 'R', 'G', 'B'
       if (ncomp == 3 && !jfif &&
           (adobe >= 0 ? adobe == 0
                       : P.comp[0].id == 'R' && P.comp[1].id == 'G' && P.comp[2].id == 'B'))
         return SQDET_JPEG_COLOR_TRANSFORM;
-      I.scan_offset = i;
-      I.h_samp = P.comp[0].h;
-      I.v_samp = P.comp[0].v;
-      if (ncomp == 1) I.h_samp = I.v_samp = 1;
+      if (P.progressive) P.first_sos = s.at;
+      else I.scan_offset = i;
+      I.h_samp = ncomp == 1 ? 1 : P.comp[0].h;
+      I.v_samp = ncomp == 1 ? 1 : P.comp[0].v;
       const bool swap = I.orientation >= 5;
       I.height = swap ? I.coded_width : I.coded_height;
       I.width = swap ? I.coded_height : I.coded_width;
@@ -983,75 +981,6 @@ Layout layout(const Parsed& P, int64_t file_len, int sub_bits) {
   return L;
 }
 
-// The whole call: parsed files, their layouts and where everything goes.
-struct Plan {
-  std::vector<Parsed> parsed;
-  std::vector<Layout> lay;
-  std::vector<DecFile> files;           // each file's regions, placed
-  int64_t staging = 0, scratch = 0;
-  int64_t marks = 0, marks_bytes = 0, coef = 0, coef_bytes = 0;
-};
-
-// Places every region of the call.  The staging holds the file descriptors, then each file's
-// Huffman tables and raw bytes (+16 zero bytes of padding); it is copied to the scratch's start.
-// After it in the scratch come every file's marks (a terminator, then ist), every file's
-// coefficients, and then each file's chunk sums, clean stream (padded), sbase, entry, exit, counts
-// and planes.
-void place(Plan& plan) {
-  const size_t n = plan.lay.size();
-  std::vector<DecFile>& fd = plan.files;
-  fd.assign(n, DecFile{});
-  Carver c;
-  c.next((int64_t)sizeof(DecFile) * (int64_t)n);
-  for (size_t i = 0; i < n; ++i) {
-    fd[i].tabs = c.next((int64_t)sizeof(HuffTab) * 6);
-    fd[i].raw = c.next(plan.lay[i].raw_len + 16);
-  }
-  plan.staging = plan.marks = c.offset;
-  for (size_t i = 0; i < n; ++i) {
-    fd[i].term = c.next(256);
-    fd[i].ist = c.next((int64_t)(plan.lay[i].intervals + 1) * 4);
-  }
-  plan.coef = c.offset;
-  plan.marks_bytes = plan.coef - plan.marks;
-  for (size_t i = 0; i < n; ++i) fd[i].coef = c.next((int64_t)plan.lay[i].blocks * 128);
-  plan.coef_bytes = c.offset - plan.coef;
-  for (size_t i = 0; i < n; ++i) {
-    const Layout& L = plan.lay[i];
-    fd[i].sums = c.next((int64_t)(L.chunks + 1) * 8);
-    fd[i].clean = c.next(L.raw_len + 16);
-    fd[i].sbase = c.next((int64_t)(L.intervals + 1) * 4);
-    fd[i].entry = c.next((int64_t)L.sub_max * 8);
-    fd[i].exit_ = c.next((int64_t)L.sub_max * 8);
-    fd[i].counts = c.next((int64_t)L.sub_max * 16);
-    for (int k = 0; k < plan.parsed[i].info.components; ++k)
-      fd[i].plane[k] = c.next((int64_t)L.pw[k] * L.ph[k]);
-  }
-  plan.scratch = c.offset;
-}
-
-// Parses every file; a refusal names the first file refused.
-int make_plan(const std::string& name, int n, const uint8_t* const* files, const int64_t* lengths,
-              Plan& plan) {
-  if (!files || !lengths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  if (n < 1 || n > kMaxFiles)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxFiles) + "]");
-  plan.parsed.resize((size_t)n);
-  plan.lay.resize((size_t)n);
-  for (int i = 0; i < n; ++i) {
-    if (!files[i]) return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + " is null");
-    if (lengths[i] < 4 || lengths[i] > kMaxFileBytes)
-      return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + ": length must be in [4, 2^28]");
-    const int reason = parse(files[i], lengths[i], plan.parsed[(size_t)i]);
-    if (reason)
-      return fail(SQDET_ERR_UNSUPPORTED, name + ": file " + std::to_string(i) + " is not supported: " +
-                                             kReasons[reason]);
-    plan.lay[(size_t)i] = layout(plan.parsed[(size_t)i], lengths[i], g_sub_bits);
-  }
-  place(plan);
-  return SQDET_OK;
-}
-
 // The fields of a file's descriptor that follow from its frame header, its quantization tables
 // (as the components name them) included.
 void describe(const Parsed& P, const Layout& L, DecFile& f) {
@@ -1093,76 +1022,12 @@ void describe(const Parsed& P, const Layout& L, DecFile& f) {
   }
 }
 
-// Fills the staging (descriptors, tables, raw bytes) for outputs out/pitch.
-void fill_staging(const Plan& plan, int n, const uint8_t* const* files, uint8_t* const* out,
-                  const int64_t* pitch, uint8_t* stage) {
-  DecFile* fd = reinterpret_cast<DecFile*>(stage);
-  for (int i = 0; i < n; ++i) {
-    const Parsed& P = plan.parsed[(size_t)i];
-    const Layout& L = plan.lay[(size_t)i];
-    const sqdet_jpeg_info& I = P.info;
-    DecFile f = plan.files[(size_t)i];
-    describe(P, L, f);
-    HuffTab* tabs = reinterpret_cast<HuffTab*>(stage + f.tabs);
-    for (int c = 0; c < I.components; ++c) {
-      build_tab(P.dc_bits[P.comp[c].td], P.dc_vals[P.comp[c].td], tabs[2 * c]);
-      build_tab(P.ac_bits[P.comp[c].ta], P.ac_vals[P.comp[c].ta], tabs[2 * c + 1]);
-    }
-    memcpy(stage + f.raw, files[i] + I.scan_offset, (size_t)L.raw_len);
-    memset(stage + f.raw + L.raw_len, 0, 16);
-    f.out = out[i];
-    f.pitch = pitch[i];
-    fd[i] = f;
-  }
-}
-
-int launch_decode(const Plan& plan, int n, uint8_t* stage, uint8_t* scratch, int32_t* status,
-                  cudaStream_t stream) {
-  int max_chunks = 0, max_tiles = 0, max_blocks = 0;
-  int64_t max_pix = 0;
-  for (int i = 0; i < n; ++i) {
-    const Layout& L = plan.lay[(size_t)i];
-    const sqdet_jpeg_info& I = plan.parsed[(size_t)i].info;
-    max_chunks = std::max(max_chunks, L.chunks);
-    max_tiles = std::max(max_tiles, (L.sub_max + kTile - 1) / kTile);
-    max_blocks = std::max(max_blocks, L.blocks);
-    max_pix = std::max(max_pix, (int64_t)I.height * I.width);
-  }
-  SQ_CUDA(cudaMemcpyAsync(scratch, stage, (size_t)plan.staging, cudaMemcpyHostToDevice, stream));
-  SQ_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t) * (size_t)n, stream));
-  SQ_CUDA(cudaMemsetAsync(scratch + plan.marks, 0xFF, (size_t)plan.marks_bytes, stream));
-  SQ_CUDA(cudaMemsetAsync(scratch + plan.coef, 0, (size_t)plan.coef_bytes, stream));
-  DecParams p{reinterpret_cast<DecFile*>(scratch), scratch, status};
-  const unsigned un = (unsigned)n;
-  destuff_count_kernel<<<dim3((unsigned)max_chunks, un), kChunkThreads, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg destuff_count_kernel");
-  scan_chunks_kernel<<<un, kScanThreads, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg scan_chunks_kernel");
-  destuff_compact_kernel<<<dim3((unsigned)max_chunks, un), kChunkThreads, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg destuff_compact_kernel");
-  intervals_kernel<<<un, kScanThreads, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg intervals_kernel");
-  sync_tiles_kernel<<<dim3((unsigned)max_tiles, un), kTile, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg sync_tiles_kernel");
-  sync_chain_kernel<<<un, kTile, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg sync_chain_kernel");
-  scan_counts_kernel<<<un, kScanThreads, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg scan_counts_kernel");
-  decode_write_kernel<<<dim3((unsigned)max_tiles, un), kTile, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg decode_write_kernel");
-  idct_kernel<<<dim3((unsigned)((max_blocks + kPixThreads - 1) / kPixThreads), un), kPixThreads, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg idct_kernel");
-  color_kernel<<<dim3((unsigned)((max_pix + kPixThreads - 1) / kPixThreads), un), kPixThreads, 0, stream>>>(p);
-  SQ_CHECK_LAUNCH("jpeg color_kernel");
-  return SQDET_OK;
-}
-
 // The decode calls' checks of everything but the files, in their order; info[i] is file i's.
 int check_decode_args(const std::string& name, int n, const sqdet_jpeg_info* const* info,
                       uint8_t* const* out_planes, const int64_t* out_pitches, void* staging_pinned,
                       int64_t staging_bytes, int64_t staging_need, void* scratch_dev,
                       int64_t scratch_bytes, int64_t scratch_need, int32_t* status_dev,
-                      const char* staging_fn, const char* scratch_fn) {
+                      const std::string& staging_fn, const std::string& scratch_fn) {
   if ((uintptr_t)scratch_dev % 256) return fail(SQDET_ERR_INVALID_ARG, name + ": scratch_dev must be 256-byte aligned");
   if ((uintptr_t)status_dev % alignof(int32_t))
     return fail(SQDET_ERR_INVALID_ARG, name + ": status_dev must be 4-byte aligned");
@@ -1406,7 +1271,8 @@ __global__ void __launch_bounds__(kProgThreads) prog_seq_kernel(ProgParams p) {
                        : prog_interval(f, S, p.s + S.clean, reinterpret_cast<const HuffTab*>(p.s + S.tabs),
                                        reinterpret_cast<int16_t*>(p.s + f.coef), u0, u1, ist[r] * 8,
                                        ist[r + 1] * 8);
-  if (rc) fail_file(p.status, S.file, rc);
+  // p.f[S.file] rather than f: with f here, ptxas gives the kernel 70 registers instead of 55
+  if (rc) fail_file(p.status, p.f[S.file], rc);
 }
 
 // DC refinement: block g of the scan is bit g - (its interval's first block) of its interval.
@@ -1416,14 +1282,14 @@ __global__ void __launch_bounds__(kPixThreads) prog_dc_refine_kernel(ProgParams 
   const int g = blockIdx.x * kPixThreads + threadIdx.x;
   if (g >= S.units * S.nb) return;
   if (S.bad) {                       // its intervals past the markers present have no ist
-    fail_file(p.status, S.file, -2);
+    fail_file(p.status, f, -2);
     return;
   }
   const int u = g / S.nb, j = g - u * S.nb, r = u / S.per;
   const int32_t* ist = reinterpret_cast<const int32_t*>(p.s + S.ist);
   const int64_t bit = (int64_t)ist[r] * 8 + (int64_t)(g - r * S.per * S.nb);
   if (bit >= (int64_t)ist[r + 1] * 8) {
-    fail_file(p.status, S.file, -7);
+    fail_file(p.status, f, -7);
     return;
   }
   if ((p.s[S.clean + (bit >> 3)] >> (7 - (bit & 7))) & 1) {
@@ -1487,42 +1353,14 @@ int parse_scans(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
   int restart = P.info.restart_interval;
   int64_t i = P.first_sos;
   for (;;) {
-    while (i + 1 < n && b[i] == 0xFF && b[i + 1] == 0xFF) ++i;
-    if (!G.scans.empty() && i >= n) break;               // no EOI: the image ends there
-    if (i + 2 > n || b[i] != 0xFF) return SQDET_JPEG_MALFORMED;
-    const int m = b[i + 1];
-    i += 2;
-    if (m == 0xD9 && !G.scans.empty()) break;
-    if (m == 0xD8 || m == 0xD9 || (m >= 0xD0 && m <= 0xD7) || m == 0x01) return SQDET_JPEG_MALFORMED;
-    if (i + 2 > n) return SQDET_JPEG_MALFORMED;
-    const int len = u16(b, i);
-    if (len < 2 || i + len > n) return SQDET_JPEG_MALFORMED;
-    const uint8_t* body = b + i + 2;
-    const int bn = len - 2;
-    i += len;
+    Segment s;
+    if (const int r = next_segment(b, n, i, !G.scans.empty(), s)) return r;
+    if (s.m == 0xD9) break;                              // EOI, or no EOI: the image ends there
+    if (const int r = read_tables(s, P)) return r;
+    const int m = s.m, bn = s.bn;
+    const uint8_t* body = s.body;
     if (m >= 0xC0 && m <= 0xCF && m != 0xC4 && m != 0xC8 && m != 0xCC) return SQDET_JPEG_MALFORMED;
-    if (m == 0xDB) {
-      for (int j = 0; j < bn;) {
-        const int pq = body[j] >> 4, tq = body[j] & 15, size = pq ? 128 : 64;
-        if (pq > 1 || tq > 3 || j + 1 + size > bn) return SQDET_JPEG_MALFORMED;
-        for (int k = 0; k < 64; ++k)
-          P.qt[tq][kNatural[k]] = pq ? (uint16_t)u16(body, j + 1 + 2 * k) : body[j + 1 + k];
-        P.have_q[tq] = true;
-        j += 1 + size;
-      }
-    } else if (m == 0xC4) {
-      for (int j = 0; j < bn;) {
-        if (j + 17 > bn) return SQDET_JPEG_MALFORMED;
-        const int tc = body[j] >> 4, th = body[j] & 15;
-        int cnt = 0;
-        for (int l = 0; l < 16; ++l) cnt += body[j + 1 + l];
-        if (tc > 1 || th > 3 || cnt > 256 || j + 17 + cnt > bn) return SQDET_JPEG_MALFORMED;
-        memcpy(tc ? P.ac_bits[th] : P.dc_bits[th], body + j + 1, 16);
-        memcpy(tc ? P.ac_vals[th] : P.dc_vals[th], body + j + 17, (size_t)cnt);
-        (tc ? P.have_ac : P.have_dc)[th] = true;
-        j += 17 + cnt;
-      }
-    } else if (m == 0xDD) {
+    if (m == 0xDD) {
       if (bn != 2) return SQDET_JPEG_MALFORMED;
       restart = u16(body, 0);
     } else if (m == 0xDA) {
@@ -1593,9 +1431,9 @@ int parse_scans(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
   return SQDET_JPEG_OK;
 }
 
-// sqdet_jpeg_parse_progressive's reading of a file: sequential files as parse() reads them.
-int parse_any(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
-  const int reason = parse(b, n, P, true);
+// A file as the entry points read it: with `progressive`, SOF2 files too, with their scans.
+int parse_file(const uint8_t* b, int64_t n, bool progressive, Parsed& P, Prog& G) {
+  const int reason = parse(b, n, P, progressive);
   if (reason || !P.progressive) return reason;
   return parse_scans(b, n, P, G);
 }
@@ -1644,121 +1482,6 @@ void scan_geometry(const Parsed& P, const Layout& L, const PScan& S, ProgScan& D
   D.bad = D.intervals < need;
 }
 
-// A call of the progressive entry points: its sequential files go through the sequential
-// pipeline as a Plan of their own, its progressive files through the kernels above.
-struct PPlan {
-  std::vector<int> seq, prg;           // the call's indices of each kind of file
-  Plan base;                           // the sequential files
-  std::vector<Parsed> parsed;          // the progressive files
-  std::vector<Layout> lay;
-  std::vector<Prog> prog;
-  std::vector<DecFile> files;
-  std::vector<ProgScan> scans;
-  std::vector<int2> items;             // first-scan items, then DC refinements, then each depth's
-  int first = 0, dc_refine = 0;
-  std::vector<int> depth;              // AC refinement items per depth
-  int64_t scan_off = 0, item_off = 0, pstaging = 0, coef = 0, coef_bytes = 0, pscratch = 0;
-  int64_t stage_at = 0, scratch_at = 0, status_at = 0;   // the progressive part; the statuses
-  int64_t staging = 0, scratch = 0;
-};
-
-// Parses every file and places every region.  The staging holds the sequential files' staging,
-// then the progressive files': their descriptors, the scan descriptors, the work items, then per
-// scan its tables, interval starts and clean data.  The scratch holds the sequential files'
-// scratch, then the progressive staging's copy, their coefficients and sample planes, then one
-// status per file of the call.
-int make_pplan(const std::string& name, int n, const uint8_t* const* files, const int64_t* lengths,
-               PPlan& plan) {
-  if (!files || !lengths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  if (n < 1 || n > kMaxFiles)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxFiles) + "]");
-  for (int i = 0; i < n; ++i) {
-    if (!files[i]) return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + " is null");
-    if (lengths[i] < 4 || lengths[i] > kMaxFileBytes)
-      return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + ": length must be in [4, 2^28]");
-    Parsed P;
-    Prog G;
-    const int reason = parse_any(files[i], lengths[i], P, G);
-    if (reason)
-      return fail(SQDET_ERR_UNSUPPORTED, name + ": file " + std::to_string(i) + " is not supported: " +
-                                             kReasons[reason]);
-    const Layout L = layout(P, lengths[i], g_sub_bits);
-    if (P.progressive) {
-      plan.prg.push_back(i);
-      plan.parsed.push_back(P);
-      plan.lay.push_back(L);
-      plan.prog.push_back(std::move(G));
-    } else {
-      plan.seq.push_back(i);
-      plan.base.parsed.push_back(P);
-      plan.base.lay.push_back(L);
-    }
-  }
-  if (!plan.seq.empty()) place(plan.base);
-  // work items: first scans, DC refinements, then AC refinements by their depth in their
-  // component's chain
-  std::vector<std::vector<int2>> depth_items;
-  std::vector<int2> dcref;
-  for (size_t i = 0; i < plan.prg.size(); ++i) {
-    int chain[3] = {0, 0, 0};
-    for (const PScan& S : plan.prog[i].scans) {
-      ProgScan D{};
-      D.file = (int)i;
-      scan_geometry(plan.parsed[i], plan.lay[i], S, D);
-      const int si = (int)plan.scans.size();
-      plan.scans.push_back(D);
-      if (S.ah == 0) {
-        for (int r = 0; r < D.intervals; ++r) plan.items.push_back(make_int2(si, r));
-      } else if (S.ss == 0) {
-        dcref.push_back(make_int2(si, 0));
-      } else {
-        const int d = chain[S.comp[0]]++;
-        if ((int)depth_items.size() <= d) depth_items.resize((size_t)d + 1);
-        for (int r = 0; r < D.intervals; ++r) depth_items[(size_t)d].push_back(make_int2(si, r));
-      }
-    }
-  }
-  plan.first = (int)plan.items.size();
-  plan.items.insert(plan.items.end(), dcref.begin(), dcref.end());
-  plan.dc_refine = (int)dcref.size();
-  for (const auto& v : depth_items) {
-    plan.items.insert(plan.items.end(), v.begin(), v.end());
-    plan.depth.push_back((int)v.size());
-  }
-  const size_t np = plan.prg.size();
-  plan.files.assign(np, DecFile{});
-  Carver c;
-  c.next((int64_t)sizeof(DecFile) * (int64_t)np);
-  plan.scan_off = c.next((int64_t)sizeof(ProgScan) * (int64_t)plan.scans.size());
-  plan.item_off = c.next((int64_t)sizeof(int2) * (int64_t)plan.items.size());
-  int si = 0;
-  for (size_t i = 0; i < np; ++i)
-    for (const PScan& S : plan.prog[i].scans) {
-      ProgScan& D = plan.scans[(size_t)si++];
-      D.tabs = c.next((int64_t)sizeof(HuffTab) * S.ncomp);
-      D.ist = c.next((int64_t)(D.intervals + 1) * 4);
-      D.clean = c.next(S.end - S.start + kScanPad);
-    }
-  plan.pstaging = c.offset;
-  plan.coef = c.offset;
-  for (size_t i = 0; i < np; ++i) plan.files[i].coef = c.next((int64_t)plan.lay[i].blocks * 128);
-  plan.coef_bytes = c.offset - plan.coef;
-  for (size_t i = 0; i < np; ++i)
-    for (int k = 0; k < plan.parsed[i].info.components; ++k)
-      plan.files[i].plane[k] = c.next((int64_t)plan.lay[i].pw[k] * plan.lay[i].ph[k]);
-  plan.pscratch = c.offset;
-  Carver whole;
-  whole.next(plan.seq.empty() ? 0 : plan.base.staging);
-  plan.stage_at = whole.next(np ? plan.pstaging : 0);
-  plan.staging = whole.offset;
-  whole = Carver{};
-  whole.next(plan.seq.empty() ? 0 : plan.base.scratch);
-  plan.scratch_at = whole.next(np ? plan.pscratch : 0);
-  plan.status_at = whole.next((int64_t)n * 4);
-  plan.scratch = whole.offset;
-  return SQDET_OK;
-}
-
 // Removes the stuffing of a scan's bytes and splits them at its RSTn markers into clean (ist[r]:
 // where interval r starts); whether the markers are in sequence and none is missing.  Markers
 // after the last interval's are skipped, as libjpeg skips them.
@@ -1790,42 +1513,172 @@ bool destuff_scan(const uint8_t* b, int64_t start, int64_t end, int intervals, u
   return ok && r + 1 >= intervals;
 }
 
-void fill_pstaging(const PPlan& plan, const uint8_t* const* files, uint8_t* const* out,
-                   const int64_t* pitch, uint8_t* stage) {
-  if (!plan.seq.empty()) {
-    std::vector<const uint8_t*> f;
-    std::vector<uint8_t*> o;
-    std::vector<int64_t> pt;
-    for (int i : plan.seq) {
-      f.push_back(files[i]);
-      o.push_back(out[i]);
-      pt.push_back(pitch[i]);
-    }
-    fill_staging(plan.base, (int)plan.seq.size(), f.data(), o.data(), pt.data(), stage);
+// ---- host: one call ------------------------------------------------------------------------------
+// One file of a call: its headers, its layout, its scans (progressive files) and its index in the
+// call.
+struct Input {
+  Parsed P;
+  Layout L;
+  Prog G;
+  int index;
+};
+
+// The whole call.  Its sequential files come first, so that the sequential stages' grids run over
+// the first nseq descriptors; the progressive stages reach theirs through the work items.
+struct Plan {
+  std::vector<Input> in;               // the sequential files, then the progressive ones
+  int nseq = 0;
+  std::vector<DecFile> files;          // in's descriptors, their regions placed
+  std::vector<ProgScan> scans;         // every scan of every progressive file, in order
+  std::vector<int2> items;             // first-scan items, then DC refinements, then each depth's
+  int first = 0, dc_refine = 0;
+  std::vector<int> depth;              // AC refinement items per depth
+  int64_t scan_off = 0, item_off = 0, staging = 0, scratch = 0;
+  int64_t marks = 0, marks_bytes = 0, coef = 0, coef_bytes = 0;
+};
+
+// Places every region of the call.  The staging holds the file descriptors, the scan descriptors
+// and the work items, then each sequential file's Huffman tables and raw bytes (+16 zero bytes of
+// padding), then each scan's tables, interval starts and clean data; it is copied to the scratch's
+// start.  After it in the scratch come the sequential files' marks (a terminator, then ist), every
+// file's coefficients, and then per file: a sequential file's chunk sums, clean stream (padded),
+// sbase, entry, exit and counts, and every file's planes.
+void place(Plan& plan) {
+  const size_t n = plan.in.size(), ns = (size_t)plan.nseq;
+  std::vector<DecFile>& fd = plan.files;
+  fd.assign(n, DecFile{});
+  Carver c;
+  c.next((int64_t)sizeof(DecFile) * (int64_t)n);
+  plan.scan_off = c.next((int64_t)sizeof(ProgScan) * (int64_t)plan.scans.size());
+  plan.item_off = c.next((int64_t)sizeof(int2) * (int64_t)plan.items.size());
+  for (size_t i = 0; i < ns; ++i) {
+    fd[i].tabs = c.next((int64_t)sizeof(HuffTab) * 6);
+    fd[i].raw = c.next(plan.in[i].L.raw_len + 16);
   }
-  if (plan.prg.empty()) return;
-  stage += plan.stage_at;
+  size_t si = 0;
+  for (size_t i = ns; i < n; ++i)
+    for (const PScan& S : plan.in[i].G.scans) {
+      ProgScan& D = plan.scans[si++];
+      D.tabs = c.next((int64_t)sizeof(HuffTab) * S.ncomp);
+      D.ist = c.next((int64_t)(D.intervals + 1) * 4);
+      D.clean = c.next(S.end - S.start + kScanPad);
+    }
+  plan.staging = plan.marks = c.offset;
+  for (size_t i = 0; i < ns; ++i) {
+    fd[i].term = c.next(256);
+    fd[i].ist = c.next((int64_t)(plan.in[i].L.intervals + 1) * 4);
+  }
+  plan.coef = c.offset;
+  plan.marks_bytes = plan.coef - plan.marks;
+  for (size_t i = 0; i < n; ++i) fd[i].coef = c.next((int64_t)plan.in[i].L.blocks * 128);
+  plan.coef_bytes = c.offset - plan.coef;
+  for (size_t i = 0; i < n; ++i) {
+    const Layout& L = plan.in[i].L;
+    if (i < ns) {
+      fd[i].sums = c.next((int64_t)(L.chunks + 1) * 8);
+      fd[i].clean = c.next(L.raw_len + 16);
+      fd[i].sbase = c.next((int64_t)(L.intervals + 1) * 4);
+      fd[i].entry = c.next((int64_t)L.sub_max * 8);
+      fd[i].exit_ = c.next((int64_t)L.sub_max * 8);
+      fd[i].counts = c.next((int64_t)L.sub_max * 16);
+    }
+    for (int k = 0; k < plan.in[i].P.info.components; ++k)
+      fd[i].plane[k] = c.next((int64_t)L.pw[k] * L.ph[k]);
+  }
+  plan.scratch = c.offset;
+}
+
+// Parses every file, SOF2 files too with `progressive`, and places every region; a refusal names
+// the first file refused.
+int make_plan(const std::string& name, int n, const uint8_t* const* files, const int64_t* lengths,
+              bool progressive, Plan& plan) {
+  if (!files || !lengths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  if (n < 1 || n > kMaxFiles)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxFiles) + "]");
+  plan.in.resize((size_t)n);
+  for (int i = 0; i < n; ++i) {
+    if (!files[i]) return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + " is null");
+    if (lengths[i] < 4 || lengths[i] > kMaxFileBytes)
+      return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + ": length must be in [4, 2^28]");
+    Input& in = plan.in[(size_t)i];
+    const int reason = parse_file(files[i], lengths[i], progressive, in.P, in.G);
+    if (reason)
+      return fail(SQDET_ERR_UNSUPPORTED, name + ": file " + std::to_string(i) + " is not supported: " +
+                                             kReasons[reason]);
+    in.L = layout(in.P, lengths[i], g_sub_bits);
+    in.index = i;
+  }
+  const auto prog = std::stable_partition(plan.in.begin(), plan.in.end(),
+                                          [](const Input& in) { return !in.P.progressive; });
+  plan.nseq = (int)(prog - plan.in.begin());
+  // work items: first scans, DC refinements, then AC refinements by their depth in their
+  // component's chain
+  std::vector<std::vector<int2>> depth_items;
+  std::vector<int2> dcref;
+  for (size_t i = (size_t)plan.nseq; i < plan.in.size(); ++i) {
+    int chain[3] = {0, 0, 0};
+    for (const PScan& S : plan.in[i].G.scans) {
+      ProgScan D{};
+      D.file = (int)i;
+      scan_geometry(plan.in[i].P, plan.in[i].L, S, D);
+      const int si = (int)plan.scans.size();
+      plan.scans.push_back(D);
+      if (S.ah == 0) {
+        for (int r = 0; r < D.intervals; ++r) plan.items.push_back(make_int2(si, r));
+      } else if (S.ss == 0) {
+        dcref.push_back(make_int2(si, 0));
+      } else {
+        const int d = chain[S.comp[0]]++;
+        if ((int)depth_items.size() <= d) depth_items.resize((size_t)d + 1);
+        for (int r = 0; r < D.intervals; ++r) depth_items[(size_t)d].push_back(make_int2(si, r));
+      }
+    }
+  }
+  plan.first = (int)plan.items.size();
+  plan.items.insert(plan.items.end(), dcref.begin(), dcref.end());
+  plan.dc_refine = (int)dcref.size();
+  for (const auto& v : depth_items) {
+    plan.items.insert(plan.items.end(), v.begin(), v.end());
+    plan.depth.push_back((int)v.size());
+  }
+  place(plan);
+  return SQDET_OK;
+}
+
+// Fills the staging (descriptors, tables, raw bytes, scans, work items) for outputs out/pitch.
+void fill_staging(const Plan& plan, const uint8_t* const* files, uint8_t* const* out,
+                  const int64_t* pitch, uint8_t* stage) {
   DecFile* fd = reinterpret_cast<DecFile*>(stage);
   ProgScan* sc = reinterpret_cast<ProgScan*>(stage + plan.scan_off);
-  int si = 0;
-  for (size_t i = 0; i < plan.prg.size(); ++i) {
-    const int k = plan.prg[i];
-    const Parsed& P = plan.parsed[i];
-    const Prog& G = plan.prog[i];
-    DecFile f = plan.files[i];
-    describe(P, plan.lay[i], f);
-    for (int c = 0; c < P.info.components; ++c)          // the tables latched at the first scans
-      for (int q = 0; q < 64; ++q) f.q[c][q] = G.latched[c] ? (int16_t)G.q[c][q] : 0;
-    f.out = out[k];
-    f.pitch = pitch[k];
-    fd[i] = f;
-    for (const PScan& S : G.scans) {
-      ProgScan D = plan.scans[(size_t)si];
+  size_t si = 0;
+  for (size_t j = 0; j < plan.in.size(); ++j) {
+    const Input& in = plan.in[j];
+    const Parsed& P = in.P;
+    const uint8_t* file = files[in.index];
+    DecFile f = plan.files[j];
+    describe(P, in.L, f);
+    f.index = in.index;
+    f.out = out[in.index];
+    f.pitch = pitch[in.index];
+    if (!P.progressive) {
+      HuffTab* tabs = reinterpret_cast<HuffTab*>(stage + f.tabs);
+      for (int c = 0; c < P.info.components; ++c) {
+        build_tab(P.dc_bits[P.comp[c].td], P.dc_vals[P.comp[c].td], tabs[2 * c]);
+        build_tab(P.ac_bits[P.comp[c].ta], P.ac_vals[P.comp[c].ta], tabs[2 * c + 1]);
+      }
+      memcpy(stage + f.raw, file + P.info.scan_offset, (size_t)in.L.raw_len);
+      memset(stage + f.raw + in.L.raw_len, 0, 16);
+    }
+    for (int c = 0; P.progressive && c < P.info.components; ++c)   // latched at the first scans
+      for (int q = 0; q < 64; ++q) f.q[c][q] = in.G.latched[c] ? (int16_t)in.G.q[c][q] : 0;
+    fd[j] = f;
+    for (const PScan& S : in.G.scans) {
+      ProgScan D = plan.scans[si];
       HuffTab* tabs = reinterpret_cast<HuffTab*>(stage + D.tabs);
       const bool coded = S.ss != 0 || S.ah == 0;
       for (int t = 0; coded && t < (S.ss ? 1 : S.ncomp); ++t) build_tab(S.bits[t], S.vals[t], tabs[t]);
       uint8_t* clean = stage + D.clean;
-      const bool ok = destuff_scan(files[k], S.start, S.end, D.intervals, clean,
+      const bool ok = destuff_scan(file, S.start, S.end, D.intervals, clean,
                                    reinterpret_cast<int32_t*>(stage + D.ist));
       D.bad = D.bad || !ok;
       const int32_t len = reinterpret_cast<int32_t*>(stage + D.ist)[D.intervals];
@@ -1833,111 +1686,155 @@ void fill_pstaging(const PPlan& plan, const uint8_t* const* files, uint8_t* cons
       sc[si++] = D;
     }
   }
-  memcpy(stage + plan.item_off, plan.items.data(), sizeof(int2) * plan.items.size());
+  std::copy(plan.items.begin(), plan.items.end(), reinterpret_cast<int2*>(stage + plan.item_off));
 }
 
-// The call's index of each status the two pipelines wrote: the sequential files', then the
-// progressive files'.
-struct StatusOrder {
-  int32_t n, at[kMaxFiles];
-};
-
-__global__ void scatter_status_kernel(const int32_t* tmp, StatusOrder o, int32_t* status) {
-  const int i = threadIdx.x;
-  if (i < o.n) status[o.at[i]] = tmp[i];
-}
-
-int launch_pdecode(const PPlan& plan, int n, uint8_t* stage, uint8_t* scratch, int32_t* status,
-                   cudaStream_t stream) {
-  int32_t* tmp = reinterpret_cast<int32_t*>(scratch + plan.status_at);
-  const int nb = (int)plan.seq.size(), np = (int)plan.prg.size();
-  if (nb) {
-    const int rc = launch_decode(plan.base, nb, stage, scratch, tmp, stream);
-    if (rc) return rc;
+// The call's launches: the sequential stages over the sequential files, the progressive stages
+// over the progressive files' scans, then the IDCT and colour over every file.
+int launch_decode(const Plan& plan, uint8_t* stage, uint8_t* scratch, int32_t* status,
+                  cudaStream_t stream) {
+  const int n = (int)plan.in.size(), ns = plan.nseq;
+  int max_chunks = 0, max_tiles = 0, max_blocks = 0;
+  int64_t max_pix = 0;
+  for (int i = 0; i < n; ++i) {
+    const Layout& L = plan.in[(size_t)i].L;
+    const sqdet_jpeg_info& I = plan.in[(size_t)i].P.info;
+    if (i < ns) {
+      max_chunks = std::max(max_chunks, L.chunks);
+      max_tiles = std::max(max_tiles, (L.sub_max + kTile - 1) / kTile);
+    }
+    max_blocks = std::max(max_blocks, L.blocks);
+    max_pix = std::max(max_pix, (int64_t)I.height * I.width);
   }
-  if (np) {
-    uint8_t* s = scratch + plan.scratch_at;
-    SQ_CUDA(cudaMemcpyAsync(s, stage + plan.stage_at, (size_t)plan.pstaging, cudaMemcpyHostToDevice, stream));
-    SQ_CUDA(cudaMemsetAsync(tmp + nb, 0, sizeof(int32_t) * (size_t)np, stream));
-    SQ_CUDA(cudaMemsetAsync(s + plan.coef, 0, (size_t)plan.coef_bytes, stream));
-    ProgParams pp{reinterpret_cast<DecFile*>(s), reinterpret_cast<const ProgScan*>(s + plan.scan_off),
-                  reinterpret_cast<const int2*>(s + plan.item_off), 0, s, tmp + nb};
-    if (plan.first) {
-      pp.nitems = plan.first;
-      prog_seq_kernel<<<(unsigned)plan.first, kProgThreads, 0, stream>>>(pp);
-      SQ_CHECK_LAUNCH("jpeg prog_seq_kernel (first scans)");
-    }
-    int at = plan.first;
-    if (plan.dc_refine) {
-      int max_blocks = 0;
-      for (int k = 0; k < plan.dc_refine; ++k) {
-        const ProgScan& S = plan.scans[(size_t)plan.items[(size_t)(at + k)].x];
-        max_blocks = std::max(max_blocks, S.units * S.nb);
-      }
-      ProgParams q = pp;
-      q.items += at;
-      q.nitems = plan.dc_refine;
-      prog_dc_refine_kernel<<<dim3((unsigned)((max_blocks + kPixThreads - 1) / kPixThreads), (unsigned)plan.dc_refine),
-                              kPixThreads, 0, stream>>>(q);
-      SQ_CHECK_LAUNCH("jpeg prog_dc_refine_kernel");
-      at += plan.dc_refine;
-    }
-    for (int d : plan.depth) {
-      ProgParams q = pp;
-      q.items += at;
-      q.nitems = d;
-      prog_seq_kernel<<<(unsigned)d, kProgThreads, 0, stream>>>(q);
-      SQ_CHECK_LAUNCH("jpeg prog_seq_kernel (AC refinements)");
-      at += d;
-    }
-    int max_blocks = 0;
-    int64_t max_pix = 0;
-    for (int i = 0; i < np; ++i) {
-      max_blocks = std::max(max_blocks, plan.lay[(size_t)i].blocks);
-      max_pix = std::max(max_pix, (int64_t)plan.parsed[(size_t)i].info.height * plan.parsed[(size_t)i].info.width);
-    }
-    DecParams p{reinterpret_cast<DecFile*>(s), s, tmp + nb};
-    idct_kernel<<<dim3((unsigned)((max_blocks + kPixThreads - 1) / kPixThreads), (unsigned)np), kPixThreads, 0, stream>>>(p);
-    SQ_CHECK_LAUNCH("jpeg idct_kernel");
-    color_kernel<<<dim3((unsigned)((max_pix + kPixThreads - 1) / kPixThreads), (unsigned)np), kPixThreads, 0, stream>>>(p);
-    SQ_CHECK_LAUNCH("jpeg color_kernel");
+  SQ_CUDA(cudaMemcpyAsync(scratch, stage, (size_t)plan.staging, cudaMemcpyHostToDevice, stream));
+  SQ_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t) * (size_t)n, stream));
+  if (ns) SQ_CUDA(cudaMemsetAsync(scratch + plan.marks, 0xFF, (size_t)plan.marks_bytes, stream));
+  SQ_CUDA(cudaMemsetAsync(scratch + plan.coef, 0, (size_t)plan.coef_bytes, stream));
+  const DecParams p{reinterpret_cast<DecFile*>(scratch), scratch, status};
+  if (ns) {
+    const unsigned un = (unsigned)ns;
+    destuff_count_kernel<<<dim3((unsigned)max_chunks, un), kChunkThreads, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg destuff_count_kernel");
+    scan_chunks_kernel<<<un, kScanThreads, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg scan_chunks_kernel");
+    destuff_compact_kernel<<<dim3((unsigned)max_chunks, un), kChunkThreads, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg destuff_compact_kernel");
+    intervals_kernel<<<un, kScanThreads, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg intervals_kernel");
+    sync_tiles_kernel<<<dim3((unsigned)max_tiles, un), kTile, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg sync_tiles_kernel");
+    sync_chain_kernel<<<un, kTile, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg sync_chain_kernel");
+    scan_counts_kernel<<<un, kScanThreads, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg scan_counts_kernel");
+    decode_write_kernel<<<dim3((unsigned)max_tiles, un), kTile, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg decode_write_kernel");
   }
-  StatusOrder o{};
-  o.n = n;
-  for (int j = 0; j < nb; ++j) o.at[j] = plan.seq[(size_t)j];
-  for (int j = 0; j < np; ++j) o.at[nb + j] = plan.prg[(size_t)j];
-  scatter_status_kernel<<<1, kMaxFiles, 0, stream>>>(tmp, o, status);
-  SQ_CHECK_LAUNCH("jpeg scatter_status_kernel");
+  const ProgParams pp{p.f, reinterpret_cast<const ProgScan*>(scratch + plan.scan_off),
+                      reinterpret_cast<const int2*>(scratch + plan.item_off), plan.first, scratch, status};
+  if (plan.first) {
+    prog_seq_kernel<<<(unsigned)plan.first, kProgThreads, 0, stream>>>(pp);
+    SQ_CHECK_LAUNCH("jpeg prog_seq_kernel (first scans)");
+  }
+  int at = plan.first;
+  if (plan.dc_refine) {
+    int dc_blocks = 0;
+    for (int k = 0; k < plan.dc_refine; ++k) {
+      const ProgScan& S = plan.scans[(size_t)plan.items[(size_t)(at + k)].x];
+      dc_blocks = std::max(dc_blocks, S.units * S.nb);
+    }
+    ProgParams q = pp;
+    q.items += at;
+    q.nitems = plan.dc_refine;
+    prog_dc_refine_kernel<<<dim3((unsigned)((dc_blocks + kPixThreads - 1) / kPixThreads), (unsigned)plan.dc_refine),
+                            kPixThreads, 0, stream>>>(q);
+    SQ_CHECK_LAUNCH("jpeg prog_dc_refine_kernel");
+    at += plan.dc_refine;
+  }
+  for (int d : plan.depth) {
+    ProgParams q = pp;
+    q.items += at;
+    q.nitems = d;
+    prog_seq_kernel<<<(unsigned)d, kProgThreads, 0, stream>>>(q);
+    SQ_CHECK_LAUNCH("jpeg prog_seq_kernel (AC refinements)");
+    at += d;
+  }
+  idct_kernel<<<dim3((unsigned)((max_blocks + kPixThreads - 1) / kPixThreads), (unsigned)n), kPixThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg idct_kernel");
+  color_kernel<<<dim3((unsigned)((max_pix + kPixThreads - 1) / kPixThreads), (unsigned)n), kPixThreads, 0, stream>>>(p);
+  SQ_CHECK_LAUNCH("jpeg color_kernel");
   return SQDET_OK;
 }
 
+// ---- entry points: the plain ones and their _progressive siblings ----------------------------------
+std::string entry_name(const char* plain, bool progressive) {
+  return std::string(plain) + (progressive ? "_progressive" : "");
+}
+
+int parse_entry(const uint8_t* file, int64_t len, sqdet_jpeg_info* out, bool progressive) {
+  const std::string name = entry_name("sqdet_jpeg_parse", progressive);
+  if (!file || !out || len < 0) return fail(SQDET_ERR_INVALID_ARG, name + ": bad argument");
+  Parsed P;
+  Prog G;
+  const int reason = parse_file(file, len, progressive, P, G);
+  P.info.reason = reason;
+  if (reason) P.info.supported = 0;
+  *out = P.info;
+  if (reason) return fail(SQDET_ERR_UNSUPPORTED, name + ": not supported: " + kReasons[reason]);
+  return SQDET_OK;
+}
+
+int64_t staging_bytes_entry(int n, const uint8_t* const* files, const int64_t* lengths, bool progressive) {
+  Plan plan;
+  if (make_plan(entry_name("sqdet_jpeg_decode_staging_bytes", progressive), n, files, lengths, progressive, plan))
+    return -1;
+  return plan.staging;
+}
+
+int64_t scratch_bytes_entry(int n, const uint8_t* const* files, const int64_t* lengths, bool progressive) {
+  Plan plan;
+  if (make_plan(entry_name("sqdet_jpeg_decode_scratch_bytes", progressive), n, files, lengths, progressive, plan))
+    return -1;
+  return plan.scratch;
+}
+
+int decode_entry(int n, const uint8_t* const* files_host, const int64_t* lengths, uint8_t* const* out_planes,
+                 const int64_t* out_pitches, void* staging_pinned, int64_t staging_bytes, void* scratch_dev,
+                 int64_t scratch_bytes, int32_t* status_dev, void* stream, bool progressive) {
+  const std::string name = entry_name("sqdet_decode_jpeg", progressive);
+  if (!out_planes || !out_pitches || !staging_pinned || !scratch_dev || !status_dev)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
+  Plan plan;
+  int rc = make_plan(name, n, files_host, lengths, progressive, plan);
+  if (rc) return rc;
+  std::vector<const sqdet_jpeg_info*> info((size_t)n);
+  for (const Input& in : plan.in) info[(size_t)in.index] = &in.P.info;
+  rc = check_decode_args(name, n, info.data(), out_planes, out_pitches, staging_pinned, staging_bytes,
+                         plan.staging, scratch_dev, scratch_bytes, plan.scratch, status_dev,
+                         entry_name("sqdet_jpeg_decode_staging_bytes", progressive),
+                         entry_name("sqdet_jpeg_decode_scratch_bytes", progressive));
+  if (rc) return rc;
+  fill_staging(plan, files_host, out_planes, out_pitches, static_cast<uint8_t*>(staging_pinned));
+  DeviceGuard guard(pointer_device(out_planes[0]));
+  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select output 0's device");
+  return launch_decode(plan, static_cast<uint8_t*>(staging_pinned), static_cast<uint8_t*>(scratch_dev),
+                       status_dev, (cudaStream_t)stream);
+}
 }  // namespace
 }  // namespace sqdet
 
 using namespace sqdet;
 
 int sqdet_jpeg_parse(const uint8_t* file, int64_t len, sqdet_jpeg_info* out) {
-  if (!file || !out || len < 0) return fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_parse: bad argument");
-  Parsed P;
-  const int reason = parse(file, len, P);
-  P.info.reason = reason;
-  if (reason) P.info.supported = 0;
-  *out = P.info;
-  if (reason)
-    return fail(SQDET_ERR_UNSUPPORTED, std::string("sqdet_jpeg_parse: not supported: ") + kReasons[reason]);
-  return SQDET_OK;
+  return parse_entry(file, len, out, false);
 }
 
 int64_t sqdet_jpeg_decode_staging_bytes(int n, const uint8_t* const* files_host, const int64_t* lengths) {
-  Plan plan;
-  if (make_plan("sqdet_jpeg_decode_staging_bytes", n, files_host, lengths, plan)) return -1;
-  return plan.staging;
+  return staging_bytes_entry(n, files_host, lengths, false);
 }
 
 int64_t sqdet_jpeg_decode_scratch_bytes(int n, const uint8_t* const* files_host, const int64_t* lengths) {
-  Plan plan;
-  if (make_plan("sqdet_jpeg_decode_scratch_bytes", n, files_host, lengths, plan)) return -1;
-  return plan.scratch;
+  return scratch_bytes_entry(n, files_host, lengths, false);
 }
 
 int sqdet_jpeg_decode_set_subsequence_bits(int bits) {
@@ -1952,74 +1849,28 @@ int sqdet_decode_jpeg(int n, const uint8_t* const* files_host, const int64_t* le
                       uint8_t* const* out_planes, const int64_t* out_pitches, void* staging_pinned,
                       int64_t staging_bytes, void* scratch_dev, int64_t scratch_bytes,
                       int32_t* status_dev, void* stream) {
-  const std::string name = "sqdet_decode_jpeg";
-  if (!out_planes || !out_pitches || !staging_pinned || !scratch_dev || !status_dev)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  Plan plan;
-  int rc = make_plan(name, n, files_host, lengths, plan);
-  if (rc) return rc;
-  std::vector<const sqdet_jpeg_info*> info((size_t)n);
-  for (int i = 0; i < n; ++i) info[(size_t)i] = &plan.parsed[(size_t)i].info;
-  rc = check_decode_args(name, n, info.data(), out_planes, out_pitches, staging_pinned, staging_bytes,
-                         plan.staging, scratch_dev, scratch_bytes, plan.scratch, status_dev,
-                         "sqdet_jpeg_decode_staging_bytes", "sqdet_jpeg_decode_scratch_bytes");
-  if (rc) return rc;
-  fill_staging(plan, n, files_host, out_planes, out_pitches, static_cast<uint8_t*>(staging_pinned));
-  DeviceGuard guard(pointer_device(out_planes[0]));
-  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select output 0's device");
-  return launch_decode(plan, n, static_cast<uint8_t*>(staging_pinned), static_cast<uint8_t*>(scratch_dev),
-                       status_dev, (cudaStream_t)stream);
+  return decode_entry(n, files_host, lengths, out_planes, out_pitches, staging_pinned, staging_bytes,
+                      scratch_dev, scratch_bytes, status_dev, stream, false);
 }
 
 int sqdet_jpeg_parse_progressive(const uint8_t* file, int64_t len, sqdet_jpeg_info* out) {
-  if (!file || !out || len < 0)
-    return fail(SQDET_ERR_INVALID_ARG, "sqdet_jpeg_parse_progressive: bad argument");
-  Parsed P;
-  Prog G;
-  const int reason = parse_any(file, len, P, G);
-  P.info.reason = reason;
-  if (reason) P.info.supported = 0;
-  *out = P.info;
-  if (reason)
-    return fail(SQDET_ERR_UNSUPPORTED, std::string("sqdet_jpeg_parse_progressive: not supported: ") + kReasons[reason]);
-  return SQDET_OK;
+  return parse_entry(file, len, out, true);
 }
 
 int64_t sqdet_jpeg_decode_staging_bytes_progressive(int n, const uint8_t* const* files_host,
                                                     const int64_t* lengths) {
-  PPlan plan;
-  if (make_pplan("sqdet_jpeg_decode_staging_bytes_progressive", n, files_host, lengths, plan)) return -1;
-  return plan.staging;
+  return staging_bytes_entry(n, files_host, lengths, true);
 }
 
 int64_t sqdet_jpeg_decode_scratch_bytes_progressive(int n, const uint8_t* const* files_host,
                                                     const int64_t* lengths) {
-  PPlan plan;
-  if (make_pplan("sqdet_jpeg_decode_scratch_bytes_progressive", n, files_host, lengths, plan)) return -1;
-  return plan.scratch;
+  return scratch_bytes_entry(n, files_host, lengths, true);
 }
 
 int sqdet_decode_jpeg_progressive(int n, const uint8_t* const* files_host, const int64_t* lengths,
                                   uint8_t* const* out_planes, const int64_t* out_pitches,
                                   void* staging_pinned, int64_t staging_bytes, void* scratch_dev,
                                   int64_t scratch_bytes, int32_t* status_dev, void* stream) {
-  const std::string name = "sqdet_decode_jpeg_progressive";
-  if (!out_planes || !out_pitches || !staging_pinned || !scratch_dev || !status_dev)
-    return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
-  PPlan plan;
-  int rc = make_pplan(name, n, files_host, lengths, plan);
-  if (rc) return rc;
-  std::vector<const sqdet_jpeg_info*> info((size_t)n);
-  for (size_t j = 0; j < plan.seq.size(); ++j) info[(size_t)plan.seq[j]] = &plan.base.parsed[j].info;
-  for (size_t j = 0; j < plan.prg.size(); ++j) info[(size_t)plan.prg[j]] = &plan.parsed[j].info;
-  rc = check_decode_args(name, n, info.data(), out_planes, out_pitches, staging_pinned, staging_bytes,
-                         plan.staging, scratch_dev, scratch_bytes, plan.scratch, status_dev,
-                         "sqdet_jpeg_decode_staging_bytes_progressive",
-                         "sqdet_jpeg_decode_scratch_bytes_progressive");
-  if (rc) return rc;
-  fill_pstaging(plan, files_host, out_planes, out_pitches, static_cast<uint8_t*>(staging_pinned));
-  DeviceGuard guard(pointer_device(out_planes[0]));
-  if (!guard.ok) return fail(SQDET_ERR_CUDA, "cannot select output 0's device");
-  return launch_pdecode(plan, n, static_cast<uint8_t*>(staging_pinned), static_cast<uint8_t*>(scratch_dev),
-                        status_dev, (cudaStream_t)stream);
+  return decode_entry(n, files_host, lengths, out_planes, out_pitches, staging_pinned, staging_bytes,
+                      scratch_dev, scratch_bytes, status_dev, stream, true);
 }

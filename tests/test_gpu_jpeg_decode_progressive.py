@@ -11,7 +11,7 @@ from squeezedet_b200 import _lib
 from squeezedet_b200.jpeg import decode_jpeg_device, encode_jpeg_device, jpeg_bytes
 
 from oracle import jpeg_decode_progressive as P
-from oracle.jpeg_decode import CorruptData
+from oracle.jpeg_decode import CorruptData, parse
 
 import jpeg_corpus as J
 from gpu_util import fetch_results
@@ -167,21 +167,31 @@ def corrupt(f, scan_index):
 
 
 def test_corrupt_scans_fail_only_their_file():
+  """Corrupt progressive and sequential files interleaved: each status lands at its file's index,
+  whichever stages decode the file."""
   rng = np.random.default_rng(13)
   good = [('good %d' % i, J.encode(J.content('smooth', 64, 96, 3, rng), PROG, 1)) for i in range(3)]
+  good.append(('good baseline', J.encode(J.content('smooth', 64, 96, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 90)))
   noise = J.encode(J.content('noise', 64, 96, 3, rng), PROG, 1, cv2.IMWRITE_JPEG_QUALITY, 100)
   # a first scan, a refinement and data that runs out inside the last scan (a file cut earlier
   # would miss whole scans, which libjpeg smooths, so it is refused)
   bad = [corrupt(noise, 1), corrupt(noise, 5), noise[:len(noise) - 300], W.with_dri(noise, 1)]
+  # baseline files: 0xFF 0x00 runs (all-ones bits, an invalid code) and an RSTn marker removed
+  junk = bytearray(J.encode(J.content('smooth', 64, 96, 3, rng), cv2.IMWRITE_JPEG_QUALITY, 90))
+  scan = parse(bytes(junk)).scan
+  junk[scan + 10:scan + 50] = b'\xff\x00' * 20
+  rst = J.encode(J.content('smooth', 64, 96, 3, rng), cv2.IMWRITE_JPEG_RST_INTERVAL, 2)
+  k = rst.index(b'\xff\xd1', parse(rst).scan)
+  bad += [bytes(junk), rst[:k] + rst[k + 2:]]
   for f in bad:                       # corrupt as the oracle sees it too
     with pytest.raises(CorruptData):
       P.decode(f)
-  files = [good[0][1], bad[0], good[1][1], bad[1], bad[2], good[2][1], bad[3]]
+  files = [good[0][1], bad[4], bad[0], good[3][1], good[1][1], bad[1], bad[5], bad[2], good[2][1], bad[3]]
   frames, status = decode_jpeg_device(files, DEV, progressive=True)
   st = status.cpu().numpy()
-  assert st[1] < 0 and st[3] < 0 and st[4] < 0 and st[6] < 0, st
-  for k, (name, f) in zip((0, 2, 5), good):
-    assert st[k] == 0
+  assert all(st[k] < 0 for k in (1, 2, 5, 6, 7, 9)), st
+  for k, (name, f) in zip((0, 4, 8, 3), good):
+    assert st[k] == 0, (name, st)
     assert np.array_equal(frames[k].cpu().numpy(), J.imdecode(f)), name
 
 
