@@ -692,7 +692,7 @@ int sqdet_encode_png(int n, int format, const uint8_t* const* planes, const int6
 #define SQDET_JPEG_SMOOTHED         13  /* libjpeg block-smooths it: cv2 decodes it */
 #define SQDET_JPEG_TOO_MANY_SCANS   14  /* more than 256 scans: cv2 decodes it */
 typedef struct {
-  int32_t height, width;              /* of the decoded frame, after orientation */
+  int32_t height, width;              /* of the decoded frame (reduced, see _params), after orientation */
   int32_t coded_height, coded_width;  /* as SOF gives them */
   int32_t components;                 /* 1 or 3 */
   int32_t h_samp, v_samp;             /* luma sampling factors (chroma is 1x1) */
@@ -773,6 +773,51 @@ int sqdet_decode_jpeg_progressive(int n, const uint8_t* const* files_host, const
                                   uint8_t* const* out_planes, const int64_t* out_pitches,
                                   void* staging_pinned, int64_t staging_bytes, void* scratch_dev,
                                   int64_t scratch_bytes, int32_t* status_dev, void* stream);
+
+/* ---- JPEG decoding with cv2's other colour reads: IMREAD_REDUCED_COLOR_2/4/8 ---------
+ * The _params functions take the arguments of their plain counterparts and a
+ * sqdet_jpeg_decode_params:
+ *   progressive  0: the files sqdet_decode_jpeg decodes; 1: those of sqdet_decode_jpeg_progressive
+ *   scale_denom  1, 2, 4 or 8: file i becomes exactly cv2.imdecode(file, IMREAD_REDUCED_COLOR_s)
+ *                with s = scale_denom (IMREAD_COLOR for 1); anything else is SQDET_ERR_INVALID_ARG
+ *   reserved     0
+ * The plain and _progressive functions are these with {0, 1} and {1, 1}.
+ *
+ * libjpeg-turbo decodes straight to the reduced size with scaled IDCTs; so does sqdet_decode_jpeg_params.
+ * The frame is ceil(coded_height / s) x ceil(coded_width / s) before the EXIF orientation, and
+ * sqdet_jpeg_info's height and width report it after the orientation.  Luma takes an m x m IDCT
+ * per 8 x 8 block, m = 8 / s (jpeg_idct_4x4 and jpeg_idct_2x2 as libjpeg-turbo's SSE2 code
+ * computes them, and jpeg_idct_1x1); a chroma component's IDCT doubles from m while it stays
+ * below 8 and libjpeg's divisibility rule holds, which 4:2:0 chroma meets (chroma at 2m, not
+ * upsampled) and the other samplings do not (chroma at m, upsampled).  Upsampling is fancy
+ * (h2v1 and h1v2 triangle filters) at 1/2 and 1/4 and replication at 1/8.  The coefficients are
+ * those of the full-size decode; the sample planes in the scratch shrink to the scaled size.
+ *
+ * Size limits: a coded side above 65500 is SQDET_JPEG_TOO_LARGE at any scale, as in libjpeg.
+ * cv2 applies CV_IO_MAX_IMAGE_PIXELS (2^30) to the reduced size: above it the reason is
+ * SQDET_JPEG_TOO_LARGE (cv2 refuses the file too).  A file of more than 2^30 coded pixels whose
+ * reduced size fits is SQDET_JPEG_CODED_TOO_LARGE, refused before any sizing: cv2 decodes it at
+ * that scale, but a few header bytes must not size gigabytes of coefficients (2 bytes per coded
+ * sample); route it to cv2.imdecode.                                                          */
+#define SQDET_JPEG_CODED_TOO_LARGE  15  /* more than 2^30 coded pixels, fewer reduced: cv2 decodes it */
+typedef struct {
+  int32_t progressive;
+  int32_t scale_denom;
+  int32_t reserved[2];
+} sqdet_jpeg_decode_params;
+int sqdet_jpeg_parse_params(const uint8_t* file, int64_t len, const sqdet_jpeg_decode_params* params,
+                            sqdet_jpeg_info* out);
+int64_t sqdet_jpeg_decode_staging_bytes_params(int n, const uint8_t* const* files_host,
+                                               const int64_t* lengths,
+                                               const sqdet_jpeg_decode_params* params);
+int64_t sqdet_jpeg_decode_scratch_bytes_params(int n, const uint8_t* const* files_host,
+                                               const int64_t* lengths,
+                                               const sqdet_jpeg_decode_params* params);
+int sqdet_decode_jpeg_params(int n, const uint8_t* const* files_host, const int64_t* lengths,
+                             const sqdet_jpeg_decode_params* params, uint8_t* const* out_planes,
+                             const int64_t* out_pitches, void* staging_pinned, int64_t staging_bytes,
+                             void* scratch_dev, int64_t scratch_bytes, int32_t* status_dev,
+                             void* stream);
 
 /* ---- KITTI 2-D object scoring of filtered records (no engine needed) ---------------
  * sqdet_kitti_eval scores n images of records exactly as the KITTI devkit's evaluate_object does

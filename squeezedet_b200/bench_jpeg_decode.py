@@ -5,7 +5,8 @@
 
 A SqueezeDet engine at 1242x375 (b = --frames) runs forward_device_frames on --frames JPEG files
 per step, quality 95, of smooth synthetic pictures (bilinear upsampled noise plus grain, as
-bench_jpeg makes them, seeded on the host).  Two workloads: 1242x375 files and 1920x1080 files.
+bench_jpeg makes them, seeded on the host).  Three workloads: 1242x375 files, 1920x1080 files and
+4000x3000 files, the size of a 12 MP camera's.
 Each step starts from the files' bytes on the host and ends one of two ways:
   (a) a thread pool of cv2.imdecode (one file per task, os.cpu_count() threads), the BGR frames
       uploaded, then forward_device_frames;
@@ -19,6 +20,10 @@ the decode_jpeg_device calls' kernels, copies and memsets, summed, per frame.
 --progressive writes the files with IMWRITE_JPEG_PROGRESSIVE and decodes them with
 decode_jpeg_device(progressive=True); the kernel pass then also reports each kernel's share: the
 first scans, the DC refinements and the AC refinements separately.
+
+--reduce s (2, 4 or 8) decodes at 1/s of the size: (a) with cv2.imdecode(f,
+IMREAD_REDUCED_COLOR_s), (b) with decode_jpeg_device(reduce=s); the forward resizes the smaller
+frames.  Each row reports the device bytes of a call: its frames and its decode scratch.
 
 Prints one JSON line with the card's name and power limit, read in the same run; writes nothing.
 """
@@ -51,6 +56,7 @@ def parse_args(argv=None):
   ap.add_argument('--frames', type=int, default=8)
   ap.add_argument('--gpu', type=int, default=0)
   ap.add_argument('--progressive', action='store_true')
+  ap.add_argument('--reduce', type=int, choices=(1, 2, 4, 8), default=1)
   return ap.parse_args(argv)
 
 
@@ -63,10 +69,13 @@ def picture(h, w, rng):
 
 
 def measure_workload(args, name, model, files, torch):
+  import ctypes as C
   import cv2
   from . import _lib
-  from .jpeg import decode_jpeg_device
+  from .jpeg import decode_jpeg_device, jpeg_info
   dev = torch.device('cuda', args.gpu)
+  flag = {1: cv2.IMREAD_COLOR, 2: cv2.IMREAD_REDUCED_COLOR_2, 4: cv2.IMREAD_REDUCED_COLOR_4,
+          8: cv2.IMREAD_REDUCED_COLOR_8}[args.reduce]
   lib = model._lib
   stream = torch.cuda.ExternalStream(lib.sqdet_engine_stream(model._engine), device=dev)
   pool = ThreadPoolExecutor(os.cpu_count() or 1)
@@ -78,14 +87,15 @@ def measure_workload(args, name, model, files, torch):
     return out
 
   def form_a():
-    imgs = list(pool.map(lambda f: cv2.imdecode(np.frombuffer(f, np.uint8), cv2.IMREAD_COLOR), files))
+    imgs = list(pool.map(lambda f: cv2.imdecode(np.frombuffer(f, np.uint8), flag), files))
     with torch.cuda.stream(stream):
       frames = [torch.from_numpy(im).to(dev, non_blocking=False) for im in imgs]
     model.forward_device_frames(frames, stream=stream.cuda_stream)
     stream.synchronize()
 
   def form_b():
-    frames, status = decode_jpeg_device(files, dev, stream=stream, progressive=args.progressive)
+    frames, status = decode_jpeg_device(files, dev, stream=stream, progressive=args.progressive,
+                                        reduce=args.reduce)
     model.forward_device_frames(frames, stream=stream.cuda_stream)
     stream.synchronize()
     return status
@@ -115,7 +125,8 @@ def measure_workload(args, name, model, files, torch):
   keep = []
   with profile(activities=[ProfilerActivity.CUDA]) as prof:
     for _ in range(calls):
-      keep.append(decode_jpeg_device(files, dev, stream=stream, progressive=args.progressive))
+      keep.append(decode_jpeg_device(files, dev, stream=stream, progressive=args.progressive,
+                                     reduce=args.reduce))
     stream.synchronize()
   names = PROG_KERNELS if args.progressive else KERNELS
   evs = [ev for ev in prof.events() if ev.device_type == DeviceType.CUDA and
@@ -132,6 +143,14 @@ def measure_workload(args, name, model, files, torch):
                  'ms_per_frame_step_min': 1e3 * min(step[form]) / n}
   row['decode_device'] = {'us_per_frame_kernels': us_k / n, 'us_per_frame_with_copy_and_memsets': us / n,
                           'calls_timed': calls}
+  infos = [jpeg_info(f, args.progressive, args.reduce) for f in files]
+  bufs = [C.create_string_buffer(f, len(f)) for f in files]
+  params = _lib.JpegDecodeParams(int(args.progressive), args.reduce)
+  scratch = lib.sqdet_jpeg_decode_scratch_bytes_params(
+      n, (C.c_void_p * n)(*[C.addressof(b) for b in bufs]), (C.c_int64 * n)(*map(len, files)), C.byref(params))
+  row['device_bytes_per_call'] = {'frames': sum(3 * i['height'] * i['width'] for i in infos),
+                                  'decode_scratch': int(scratch),
+                                  'frame_hw': [infos[0]['height'], infos[0]['width']]}
   if args.progressive:
     # a call's first prog_seq_kernel decodes the first scans, its later ones the AC refinements
     share = {}
@@ -155,14 +174,16 @@ def measure(args):
   rng = np.random.default_rng(7)
   model = make_model(1242, 375, args.frames, args.gpu)
   rows = []
-  for name, (h, w) in (('kitti_1242x375', (375, 1242)), ('1080p', (1080, 1920))):
+  for name, (h, w) in (('kitti_1242x375', (375, 1242)), ('1080p', (1080, 1920)),
+                       ('camera_4000x3000', (3000, 4000))):
     params = [cv2.IMWRITE_JPEG_QUALITY, QUALITY] + ([cv2.IMWRITE_JPEG_PROGRESSIVE, 1] if args.progressive else [])
     files = [cv2.imencode('.jpg', picture(h, w, rng), params)[1].tobytes() for _ in range(args.frames)]
     rows.append(measure_workload(args, name, model, files, torch))
   kind = 'progressive ' if args.progressive else ''
+  scale = ' at 1/%d (IMREAD_REDUCED_COLOR_%d)' % (args.reduce, args.reduce) if args.reduce > 1 else ''
   return {'workload': 'squeezeDet 1242x375 forward_device_frames on %sJPEG files (quality 95, 4:2:0, '
-                      'smooth synthetic pictures) decoded by a cv2.imdecode thread pool and '
-                      'uploaded, or by decode_jpeg_device' % kind,
+                      'smooth synthetic pictures) decoded%s by a cv2.imdecode thread pool and '
+                      'uploaded, or by decode_jpeg_device' % (kind, scale), 'reduce': args.reduce,
           'gpu': gpu_info(args.gpu), 'cpu_threads': os.cpu_count(),
           'timer': 'host clock per step from the files on the host to a device synchronisation '
                    'after the forward; decode kernels: torch.profiler device durations, summed, per frame',

@@ -1,7 +1,10 @@
 // Baseline / extended sequential JPEG decoding into BGR frames in device memory
 // (sqdet_decode_jpeg): file i becomes exactly cv2.imdecode(file_i, cv2.IMREAD_COLOR), which is
 // libjpeg-turbo's (SIMD) islow IDCT, fancy upsampling, fixed-point YCbCr->RGB and the EXIF orientation.
-// oracle/jpeg_decode.py restates it in numpy.
+// With a scale_denom s of 2, 4 or 8 (sqdet_decode_jpeg_params) it is cv2.imdecode(file_i,
+// IMREAD_REDUCED_COLOR_s): each component's scaled IDCT (8, 4, 2 or 1 samples a side, planned per
+// component as libjpeg plans it), then that scale's upsampling.  oracle/jpeg_decode.py restates the
+// full-size decode in numpy, oracle/jpeg_decode_reduced.py the reduced one.
 //
 // The host parses the headers, builds each file's Huffman lookup and quantization tables and
 // packs them with the raw entropy-coded bytes into the caller's pinned staging; one copy takes
@@ -25,9 +28,10 @@
 //                      per-component DC difference sums
 //   8. decode_write    each subsequence decodes again from its final entry state, with its first
 //                      block and DC predictors from the scan, and writes its coefficients
-//   9. idct            jpeg_idct_islow per 8x8 block (as libjpeg-turbo's SIMD code computes it)
-//                      into the component planes
-//  10. color           per output pixel: orientation, fancy upsampling, YCbCr->BGR
+//   9. idct            per 8x8 block, the component's planned IDCT: jpeg_idct_islow, _4x4 or _2x2
+//                      (as libjpeg-turbo's SIMD code computes them) or _1x1, into its plane
+//  10. color           per output pixel: orientation, the planned upsampling (fancy or
+//                      replicated), YCbCr->BGR
 // All loops are bounded by host-known sizes; a corrupt entropy-coded segment sets a negative
 // status for its file and nothing else.
 #include <algorithm>
@@ -84,6 +88,9 @@ struct DecFile {
   int32_t sub_bits;
   int8_t bcomp[10], bdy[10], bdx[10];  // per block of an MCU: component, block row and column in it
   int8_t ch[3], cv[3];                 // sampling factors
+  int8_t isz[3];                       // IDCT size: samples a side per block (8 at full size)
+  int8_t uh[3], uv[3];                 // upsampling factors to the frame
+  int8_t fancy;                        // fancy upsampling (off at 1/8)
   int32_t pw[3], ph[3];                // padded plane width and height (whole blocks)
   int32_t cw[3], chh[3];               // component width and height in samples
   int16_t q[3][64];                    // dequantization, natural order (libjpeg's short multiplier)
@@ -573,8 +580,104 @@ __device__ __forceinline__ void idct8(int* d, int stride, int shift) {
   d[4 * stride] = (t13 - a0 + rnd) >> shift;
 }
 
-// The SIMD islow's block: dequantization by a 16-bit multiply; the column pass saturated to 16
-// bits, or, when every AC coefficient is zero, the DC << 2 in 16 bits; the output clamped.
+// jidctred.c's constants, 13 fraction bits
+constexpr int F0_211 = 1730, F0_509 = 4176, F0_601 = 4926, F0_720 = 5906, F0_850 = 6967,
+              F1_061 = 8697, F1_272 = 10426, F1_451 = 11893, F2_172 = 17799, F3_624 = 29692;
+
+// 32-bit sums that wrap as the SIMD code's paddd does (they can pass 2^31 on 16-bit tables)
+__device__ __forceinline__ int wadd(int a, int b) { return (int)((unsigned)a + (unsigned)b); }
+__device__ __forceinline__ int wsub(int a, int b) { return (int)((unsigned)a - (unsigned)b); }
+__device__ __forceinline__ int wshl(int a, int s) { return (int)((unsigned)a << s); }
+
+// One 1-D pass of jpeg_idct_4x4 over d[0], d[stride], ... d[7 stride] (d[4 stride] unused), as
+// jsimd_idct_4x4_sse2 computes it: pmaddwd products of 16-bit inputs summed in 32 bits -> the
+// four outputs, descaled by `shift`.
+__device__ __forceinline__ void red4(const int* d, int stride, int shift, int* o) {
+  const int tmp0 = wshl(d[0], 14);
+  const int tmp2 = wsub(d[2 * stride] * F1_847, d[6 * stride] * F0_765);
+  const int t10 = wadd(tmp0, tmp2), t12 = wsub(tmp0, tmp2);
+  const int z1 = d[7 * stride], z2 = d[5 * stride], z3 = d[3 * stride], z4 = d[stride];
+  const int odd0 = wadd(wadd(z1 * -F0_211, z2 * F1_451), wadd(z3 * -F2_172, z4 * F1_061));
+  const int odd2 = wadd(wadd(z1 * -F0_509, z2 * -F0_601), wadd(z3 * F0_899, z4 * F2_562));
+  const int rnd = 1 << (shift - 1);
+  o[0] = wadd(wadd(t10, odd2), rnd) >> shift;
+  o[1] = wadd(wadd(t12, odd0), rnd) >> shift;
+  o[2] = wadd(wsub(t12, odd0), rnd) >> shift;
+  o[3] = wadd(wsub(t10, odd2), rnd) >> shift;
+}
+
+// jpeg_idct_2x2's odd part over d[stride], d[3 stride], d[5 stride], d[7 stride].
+__device__ __forceinline__ int red2_odd(const int* d, int stride) {
+  return wadd(wsub(d[stride] * F3_624, d[3 * stride] * F1_272),
+              wsub(d[5 * stride] * F0_850, d[7 * stride] * F0_720));
+}
+
+__device__ __forceinline__ uint32_t clamp_sample(int v) { return (uint32_t)(min(max(v, -128), 127) + 128); }
+
+// jpeg_idct_4x4 (jsimd_idct_4x4_sse2) of dequantized d[64] into a 4x4 block of the plane: a block
+// whose coefficient rows 1, 2, 3, 5, 6 and 7 are all zero takes row 0 << 2 (16-bit) as its column
+// pass, the others the column pass saturated to 16 bits; the row pass saturates to 8 bits.
+__device__ __forceinline__ void idct_4x4(int* d, bool ac, uint8_t* out, int pw) {
+  int ws[32];
+#pragma unroll
+  for (int col = 0; col < 8; ++col) {
+    int o[4];
+    if (ac) {
+      red4(d + col, 8, 12, o);
+#pragma unroll
+      for (int r = 0; r < 4; ++r) o[r] = s16(o[r]);
+    } else {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) o[r] = w16(d[col] << 2);
+    }
+#pragma unroll
+    for (int r = 0; r < 4; ++r) ws[8 * r + col] = o[r];
+  }
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    int o[4];
+    red4(ws + 8 * r, 1, 19, o);
+    uint32_t w = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) w |= clamp_sample(o[k]) << (8 * k);
+    *reinterpret_cast<uint32_t*>(out + (int64_t)r * pw) = w;
+  }
+}
+
+// jpeg_idct_2x2 (jsimd_idct_2x2_sse2) of dequantized d[64] into a 2x2 block: no zero test; the
+// column pass keeps column 0 in 32 bits and saturates columns 1, 3, 5 and 7 to 16; the row pass
+// shifts column 0 left in 32 bits (it wraps) and saturates the output to 8 bits.
+__device__ __forceinline__ void idct_2x2(const int* d, uint8_t* out, int pw) {
+  int ws[2][8];
+#pragma unroll
+  for (int col = 0; col < 8; ++col) {
+    if (col == 2 || col == 4 || col == 6) continue;
+    const int t10 = wshl(d[col], 15), t0 = red2_odd(d + col, 8);
+    const int a = wadd(wadd(t10, t0), 1 << 12) >> 13, b = wadd(wsub(t10, t0), 1 << 12) >> 13;
+    ws[0][col] = col ? s16(a) : a;
+    ws[1][col] = col ? s16(b) : b;
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int t10 = wshl(ws[r][0], 15), t0 = red2_odd(ws[r], 1);
+    const uint32_t lo = clamp_sample(wadd(wadd(t10, t0), 1 << 19) >> 20);
+    const uint32_t hi = clamp_sample(wadd(wsub(t10, t0), 1 << 19) >> 20);
+    *reinterpret_cast<uint16_t*>(out + (int64_t)r * pw) = (uint16_t)(lo | hi << 8);
+  }
+}
+
+// jpeg_idct_1x1 (C: libjpeg-turbo has no SIMD one): the DC times its quantizer (16-bit signed,
+// product exact), descaled by 3, through jidctred.c's range_limit[x & 1023].
+__device__ __forceinline__ uint8_t idct_1x1(int dc, int q) {
+  const int x = ((dc * q + 4) >> 3) & 1023;
+  return (uint8_t)(x < 128 ? x + 128 : x < 512 ? 255 : x < 896 ? 0 : x - 896);
+}
+
+// Each block through its component's planned IDCT.  8: the SIMD islow's block, dequantization by a
+// 16-bit multiply; the column pass saturated to 16 bits, or, when every AC coefficient is zero,
+// the DC << 2 in 16 bits; the output clamped.  4, 2, 1: the reduced ones above, which only the
+// kScaled instance has, so that a full-size decode keeps islow's registers and occupancy.
+template <bool kScaled>
 __global__ void __launch_bounds__(kPixThreads) idct_kernel(DecParams p) {
   const DecFile& f = p.f[blockIdx.y];
   const int b = blockIdx.x * kPixThreads + threadIdx.x;
@@ -591,15 +694,31 @@ __global__ void __launch_bounds__(kPixThreads) idct_kernel(DecParams p) {
     bx = mx * f.ch[c] + f.bdx[u];
   }
   const int4* src = reinterpret_cast<const int4*>(p.s + f.coef) + (int64_t)b * 8;
+  const int n = kScaled ? f.isz[c] : 8;
+  uint8_t* plane = p.s + f.plane[c];
+  const int pw = f.pw[c];
+  if (kScaled && n == 1) {
+    plane[(int64_t)by * pw + bx] = idct_1x1(reinterpret_cast<const int16_t*>(src)[0], f.q[c][0]);
+    return;
+  }
   int d[64];
-  int ac = 0;
+  int ac = 0, ac4 = 0;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int4 v = src[i];
     if (i) ac |= v.x | v.y | v.z | v.w;
+    if (kScaled && i && i != 4) ac4 |= v.x | v.y | v.z | v.w;
     const int16_t* h = reinterpret_cast<const int16_t*>(&v);
 #pragma unroll
     for (int e = 0; e < 8; ++e) d[8 * i + e] = w16((int)h[e] * (int)f.q[c][8 * i + e]);
+  }
+  if (kScaled && n == 4) {
+    idct_4x4(d, ac4 != 0, plane + (int64_t)by * 4 * pw + bx * 4, pw);
+    return;
+  }
+  if (kScaled && n == 2) {
+    idct_2x2(d, plane + (int64_t)by * 2 * pw + bx * 2, pw);
+    return;
   }
   if (ac) {
 #pragma unroll
@@ -612,8 +731,6 @@ __global__ void __launch_bounds__(kPixThreads) idct_kernel(DecParams p) {
   }
 #pragma unroll
   for (int row = 0; row < 8; ++row) idct8(d + 8 * row, 1, 18);
-  uint8_t* plane = p.s + f.plane[c];
-  const int pw = f.pw[c];
 #pragma unroll
   for (int row = 0; row < 8; ++row) {
     uint32_t w[2] = {0, 0};
@@ -627,12 +744,14 @@ __global__ void __launch_bounds__(kPixThreads) idct_kernel(DecParams p) {
 }
 
 // ---- 10. upsample, convert, orient ----------------------------------------------------------------------
-// Chroma of full-resolution pixel (y, x) from plane c (cw x chh samples) with sampling (fh, fv).
+// Chroma of frame pixel (y, x) from plane c (cw x chh samples) upsampled by (fh, fv): with `fancy`,
+// libjpeg's triangle filters where it has them (h2v1 and h2v2 on planes wider than 2 samples,
+// h1v2 always), replication otherwise.
 __device__ __forceinline__ int chroma_at(const uint8_t* pl, int pw, int cw, int chh, int fh, int fv,
-                                         int y, int x) {
-  const bool fancy_h = fh == 2 && cw > 2;
+                                         bool fancy, int y, int x) {
+  const bool fancy_h = fancy && fh == 2 && cw > 2;
   if (fh == 1 && fv == 1) return pl[(int64_t)y * pw + x];
-  if (fv == 2 && (fh == 1 || fancy_h)) {
+  if (fancy && fv == 2 && (fh == 1 || fancy_h)) {
     const int r = y >> 1, rn = (y & 1) ? min(r + 1, chh - 1) : max(r - 1, 0);
     if (fh == 1) return (3 * pl[(int64_t)r * pw + x] + pl[(int64_t)rn * pw + x] + 1 + (y & 1)) >> 2;
     const int cx = x >> 1, xn = (x & 1) ? min(cx + 1, cw - 1) : max(cx - 1, 0);
@@ -667,9 +786,9 @@ __global__ void __launch_bounds__(kPixThreads) color_kernel(DecParams p) {
   const int y = p.s[f.plane[0] + (int64_t)sy * f.pw[0] + sx];
   int b = y, g = y, r = y;
   if (f.ncomp == 3) {
-    const int fh = f.ch[0], fv = f.cv[0];
-    const int cb = chroma_at(p.s + f.plane[1], f.pw[1], f.cw[1], f.chh[1], fh, fv, sy, sx) - 128;
-    const int cr = chroma_at(p.s + f.plane[2], f.pw[2], f.cw[2], f.chh[2], fh, fv, sy, sx) - 128;
+    const int fh = f.uh[1], fv = f.uv[1];
+    const int cb = chroma_at(p.s + f.plane[1], f.pw[1], f.cw[1], f.chh[1], fh, fv, f.fancy, sy, sx) - 128;
+    const int cr = chroma_at(p.s + f.plane[2], f.pw[2], f.cw[2], f.chh[2], fh, fv, f.fancy, sy, sx) - 128;
     // jdcolor.c's tables: FIX(x) = x * 2^16 rounded
     r = y + ((91881 * cr + 32768) >> 16);
     b = y + ((116130 * cb + 32768) >> 16);
@@ -697,6 +816,7 @@ struct Parsed {
   uint8_t dc_vals[4][256], ac_vals[4][256];
   bool progressive;                    // SOF2 (parse with progressive = true only)
   int64_t first_sos;                   // SOF2: the first SOS marker's offset
+  int reduce;                          // the scale it decodes at: 1 / reduce
 };
 
 int u16(const uint8_t* b, int64_t i) { return (b[i] << 8) | b[i + 1]; }
@@ -733,13 +853,14 @@ int exif_orientation(const uint8_t* s, int64_t n) {
   return 1;
 }
 
-// jpeg.jpeg_info reports these words; oracle/jpeg_decode.py's REASONS are tested equal to them
+// jpeg.jpeg_info reports these words; the oracles' REASONS are tested equal to them
 const char* kReasons[] = {"ok", "malformed or truncated header", "progressive", "arithmetic coding",
                           "lossless", "not 8-bit samples", "not 1 or 3 components",
                           "RGB-coded", "unsupported sampling",
                           "zero height or width", "larger than cv2 decodes",
                           "scan script libjpeg rejects", "scan script libjpeg warns on or overwrites",
-                          "block-smoothed by libjpeg", "more than 256 scans"};
+                          "block-smoothed by libjpeg", "more than 256 scans",
+                          "more than 2^30 coded pixels, which cv2 decodes at this scale"};
 
 // The largest file cv2.imdecode decodes: libjpeg's JPEG_MAX_DIMENSION per side, and cv2's default
 // CV_IO_MAX_IMAGE_PIXELS (it raises above that many pixels).
@@ -822,10 +943,12 @@ int read_tables(const Segment& s, Parsed& P) {
   return SQDET_JPEG_OK;
 }
 
-// The headers up to the first SOS; the reason (SQDET_JPEG_*) and what was read.  With
-// `progressive`, an SOF2 frame is read as SOF0's is and the first SOS is left to parse_scans.
-int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive) {
+// The headers up to the first SOS, for a decode at scale 1 / reduce; the reason (SQDET_JPEG_*) and
+// what was read.  With `progressive`, an SOF2 frame is read as SOF0's is and the first SOS is left
+// to parse_scans.
+int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive, int reduce) {
   memset(&P, 0, sizeof(P));
+  P.reduce = reduce;
   sqdet_jpeg_info& I = P.info;
   I.orientation = 1;
   if (n < 4 || b[0] != 0xFF || b[1] != 0xD8) return SQDET_JPEG_MALFORMED;
@@ -861,9 +984,12 @@ int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive) {
         if (c.tq > 3 || c.h < 1 || c.h > 4 || c.v < 1 || c.v > 4) return SQDET_JPEG_MALFORMED;
       }
       if (I.coded_height == 0 || I.coded_width == 0) return SQDET_JPEG_SIZE;
-      if (I.coded_height > kMaxSide || I.coded_width > kMaxSide ||
-          (int64_t)I.coded_height * I.coded_width > kMaxPixels)
-        return SQDET_JPEG_TOO_LARGE;
+      // libjpeg's side limit holds at every scale; cv2's pixel limit is on the reduced size, but
+      // more coded pixels than that is refused before anything is sized from them
+      if (I.coded_height > kMaxSide || I.coded_width > kMaxSide) return SQDET_JPEG_TOO_LARGE;
+      if ((int64_t)I.coded_height * I.coded_width > kMaxPixels)
+        return (int64_t)((I.coded_height + reduce - 1) / reduce) * ((I.coded_width + reduce - 1) / reduce) > kMaxPixels
+                   ? SQDET_JPEG_TOO_LARGE : SQDET_JPEG_CODED_TOO_LARGE;
       if (ncomp == 3) {
         const int h = P.comp[0].h, v = P.comp[0].v;
         const bool luma_ok = (h == 1 && v == 1) || (h == 2 && v == 1) || (h == 1 && v == 2) ||
@@ -913,8 +1039,9 @@ int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive) {
       I.h_samp = ncomp == 1 ? 1 : P.comp[0].h;
       I.v_samp = ncomp == 1 ? 1 : P.comp[0].v;
       const bool swap = I.orientation >= 5;
-      I.height = swap ? I.coded_width : I.coded_height;
-      I.width = swap ? I.coded_height : I.coded_width;
+      const int rh = (I.coded_height + reduce - 1) / reduce, rw = (I.coded_width + reduce - 1) / reduce;
+      I.height = swap ? rw : rh;
+      I.width = swap ? rh : rw;
       I.supported = 1;
       return SQDET_JPEG_OK;
     }
@@ -944,9 +1071,11 @@ void build_tab(const uint8_t* bits, const uint8_t* vals, HuffTab& t) {
   memcpy(t.vals, vals, 256);
 }
 
-// One file's layout: sizes that follow from its headers alone.
+// One file's layout: sizes that follow from its headers alone.  isz, uh and uv are each
+// component's IDCT size and upsampling factors at the file's scale; pw and ph its plane's.
 struct Layout {
   int mcu_cols, mcu_rows, mcus, bpm, restart, intervals, chunks, blocks, sub_max;
+  int isz[3], uh[3], uv[3];
   int pw[3], ph[3];
   int64_t raw_len;
 };
@@ -955,21 +1084,23 @@ Layout layout(const Parsed& P, int64_t file_len, int sub_bits) {
   const sqdet_jpeg_info& I = P.info;
   Layout L{};
   const int H = I.coded_height, W = I.coded_width;
-  if (I.components == 1) {
-    L.mcu_cols = (W + 7) / 8;
-    L.mcu_rows = (H + 7) / 8;
-    L.bpm = 1;
-    L.pw[0] = L.mcu_cols * 8;
-    L.ph[0] = L.mcu_rows * 8;
-  } else {
-    const int hs = P.comp[0].h, vs = P.comp[0].v;
-    L.mcu_cols = (W + 8 * hs - 1) / (8 * hs);
-    L.mcu_rows = (H + 8 * vs - 1) / (8 * vs);
-    L.bpm = hs * vs + 2;
-    for (int c = 0; c < 3; ++c) {
-      L.pw[c] = L.mcu_cols * P.comp[c].h * 8;
-      L.ph[c] = L.mcu_rows * P.comp[c].v * 8;
-    }
+  const bool gray = I.components == 1;
+  const int hmax = gray ? 1 : P.comp[0].h, vmax = gray ? 1 : P.comp[0].v;
+  L.mcu_cols = (W + 8 * hmax - 1) / (8 * hmax);
+  L.mcu_rows = (H + 8 * vmax - 1) / (8 * vmax);
+  L.bpm = gray ? 1 : hmax * vmax + 2;
+  // jpeg_calc_output_dimensions: luma's IDCT is m = 8 / reduce; another component's doubles
+  // from m while below 8 and both divisibility conditions hold (4:2:0 chroma: 2m, the others m)
+  const int m = 8 / P.reduce;
+  for (int c = 0; c < I.components; ++c) {
+    const int h = gray ? 1 : P.comp[c].h, v = gray ? 1 : P.comp[c].v;
+    int n = m;
+    while (n < 8 && (hmax * m) % (h * n * 2) == 0 && (vmax * m) % (v * n * 2) == 0) n *= 2;
+    L.isz[c] = n;
+    L.uh[c] = hmax * m / (h * n);
+    L.uv[c] = vmax * m / (v * n);
+    L.pw[c] = L.mcu_cols * h * n;
+    L.ph[c] = L.mcu_rows * v * n;
   }
   L.mcus = L.mcu_cols * L.mcu_rows;
   L.blocks = L.mcus * L.bpm;
@@ -985,8 +1116,8 @@ Layout layout(const Parsed& P, int64_t file_len, int sub_bits) {
 // (as the components name them) included.
 void describe(const Parsed& P, const Layout& L, DecFile& f) {
   const sqdet_jpeg_info& I = P.info;
-  f.h = I.coded_height;
-  f.w = I.coded_width;
+  f.h = (I.coded_height + P.reduce - 1) / P.reduce;
+  f.w = (I.coded_width + P.reduce - 1) / P.reduce;
   f.oh = I.height;
   f.ow = I.width;
   f.ncomp = I.components;
@@ -1001,6 +1132,7 @@ void describe(const Parsed& P, const Layout& L, DecFile& f) {
   f.blocks = L.blocks;
   f.sub_max = L.sub_max;
   f.sub_bits = g_sub_bits;
+  f.fancy = P.reduce < 8;              // jinit_upsampler: fancy only while luma's IDCT is above 1
   int u = 0;
   for (int c = 0; c < I.components; ++c) {
     const Comp& cp = P.comp[c];
@@ -1013,11 +1145,15 @@ void describe(const Parsed& P, const Layout& L, DecFile& f) {
         f.bdy[u] = (int8_t)by;
         f.bdx[u] = (int8_t)bx;
       }
+    f.isz[c] = (int8_t)L.isz[c];
+    f.uh[c] = (int8_t)L.uh[c];
+    f.uv[c] = (int8_t)L.uv[c];
     f.pw[c] = L.pw[c];
     f.ph[c] = L.ph[c];
+    // libjpeg's downsampled_width / _height at this scale
     const int hmax = I.components == 1 ? 1 : P.comp[0].h, vmax = I.components == 1 ? 1 : P.comp[0].v;
-    f.cw[c] = (int)(((int64_t)f.w * hc + hmax - 1) / hmax);
-    f.chh[c] = (int)(((int64_t)f.h * vc + vmax - 1) / vmax);
+    f.cw[c] = (int)(((int64_t)I.coded_width * hc * L.isz[c] + 8 * hmax - 1) / (8 * hmax));
+    f.chh[c] = (int)(((int64_t)I.coded_height * vc * L.isz[c] + 8 * vmax - 1) / (8 * vmax));
     for (int k = 0; k < 64; ++k) f.q[c][k] = (int16_t)P.qt[cp.tq][k];
   }
 }
@@ -1431,9 +1567,16 @@ int parse_scans(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
   return SQDET_JPEG_OK;
 }
 
+// How a call decodes: SOF2 files too or not, and at which scale (1 / reduce).
+struct Mode {
+  bool progressive;
+  int reduce;
+  const char* suffix;                  // of the entry points' names in messages
+};
+
 // A file as the entry points read it: with `progressive`, SOF2 files too, with their scans.
-int parse_file(const uint8_t* b, int64_t n, bool progressive, Parsed& P, Prog& G) {
-  const int reason = parse(b, n, P, progressive);
+int parse_file(const uint8_t* b, int64_t n, const Mode& mode, Parsed& P, Prog& G) {
+  const int reason = parse(b, n, P, mode.progressive, mode.reduce);
   if (reason || !P.progressive) return reason;
   return parse_scans(b, n, P, G);
 }
@@ -1533,6 +1676,7 @@ struct Plan {
   std::vector<int2> items;             // first-scan items, then DC refinements, then each depth's
   int first = 0, dc_refine = 0;
   std::vector<int> depth;              // AC refinement items per depth
+  int reduce = 1;                      // every file's scale: 1 / reduce
   int64_t scan_off = 0, item_off = 0, staging = 0, scratch = 0;
   int64_t marks = 0, marks_bytes = 0, coef = 0, coef_bytes = 0;
 };
@@ -1591,17 +1735,18 @@ void place(Plan& plan) {
 // Parses every file, SOF2 files too with `progressive`, and places every region; a refusal names
 // the first file refused.
 int make_plan(const std::string& name, int n, const uint8_t* const* files, const int64_t* lengths,
-              bool progressive, Plan& plan) {
+              const Mode& mode, Plan& plan) {
   if (!files || !lengths) return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
   if (n < 1 || n > kMaxFiles)
     return fail(SQDET_ERR_INVALID_ARG, name + ": n must be in [1, " + std::to_string(kMaxFiles) + "]");
   plan.in.resize((size_t)n);
+  plan.reduce = mode.reduce;
   for (int i = 0; i < n; ++i) {
     if (!files[i]) return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + " is null");
     if (lengths[i] < 4 || lengths[i] > kMaxFileBytes)
       return fail(SQDET_ERR_INVALID_ARG, name + ": file " + std::to_string(i) + ": length must be in [4, 2^28]");
     Input& in = plan.in[(size_t)i];
-    const int reason = parse_file(files[i], lengths[i], progressive, in.P, in.G);
+    const int reason = parse_file(files[i], lengths[i], mode, in.P, in.G);
     if (reason)
       return fail(SQDET_ERR_UNSUPPORTED, name + ": file " + std::to_string(i) + " is not supported: " +
                                              kReasons[reason]);
@@ -1759,24 +1904,24 @@ int launch_decode(const Plan& plan, uint8_t* stage, uint8_t* scratch, int32_t* s
     SQ_CHECK_LAUNCH("jpeg prog_seq_kernel (AC refinements)");
     at += d;
   }
-  idct_kernel<<<dim3((unsigned)((max_blocks + kPixThreads - 1) / kPixThreads), (unsigned)n), kPixThreads, 0, stream>>>(p);
+  const dim3 idct_grid((unsigned)((max_blocks + kPixThreads - 1) / kPixThreads), (unsigned)n);
+  if (plan.reduce > 1) idct_kernel<true><<<idct_grid, kPixThreads, 0, stream>>>(p);
+  else idct_kernel<false><<<idct_grid, kPixThreads, 0, stream>>>(p);
   SQ_CHECK_LAUNCH("jpeg idct_kernel");
   color_kernel<<<dim3((unsigned)((max_pix + kPixThreads - 1) / kPixThreads), (unsigned)n), kPixThreads, 0, stream>>>(p);
   SQ_CHECK_LAUNCH("jpeg color_kernel");
   return SQDET_OK;
 }
 
-// ---- entry points: the plain ones and their _progressive siblings ----------------------------------
-std::string entry_name(const char* plain, bool progressive) {
-  return std::string(plain) + (progressive ? "_progressive" : "");
-}
+// ---- entry points: the plain ones, their _progressive siblings and the _params ones -------------------
+std::string entry_name(const char* plain, const Mode& mode) { return std::string(plain) + mode.suffix; }
 
-int parse_entry(const uint8_t* file, int64_t len, sqdet_jpeg_info* out, bool progressive) {
-  const std::string name = entry_name("sqdet_jpeg_parse", progressive);
+int parse_entry(const uint8_t* file, int64_t len, sqdet_jpeg_info* out, const Mode& mode) {
+  const std::string name = entry_name("sqdet_jpeg_parse", mode);
   if (!file || !out || len < 0) return fail(SQDET_ERR_INVALID_ARG, name + ": bad argument");
   Parsed P;
   Prog G;
-  const int reason = parse_file(file, len, progressive, P, G);
+  const int reason = parse_file(file, len, mode, P, G);
   P.info.reason = reason;
   if (reason) P.info.supported = 0;
   *out = P.info;
@@ -1784,35 +1929,35 @@ int parse_entry(const uint8_t* file, int64_t len, sqdet_jpeg_info* out, bool pro
   return SQDET_OK;
 }
 
-int64_t staging_bytes_entry(int n, const uint8_t* const* files, const int64_t* lengths, bool progressive) {
+int64_t staging_bytes_entry(int n, const uint8_t* const* files, const int64_t* lengths, const Mode& mode) {
   Plan plan;
-  if (make_plan(entry_name("sqdet_jpeg_decode_staging_bytes", progressive), n, files, lengths, progressive, plan))
+  if (make_plan(entry_name("sqdet_jpeg_decode_staging_bytes", mode), n, files, lengths, mode, plan))
     return -1;
   return plan.staging;
 }
 
-int64_t scratch_bytes_entry(int n, const uint8_t* const* files, const int64_t* lengths, bool progressive) {
+int64_t scratch_bytes_entry(int n, const uint8_t* const* files, const int64_t* lengths, const Mode& mode) {
   Plan plan;
-  if (make_plan(entry_name("sqdet_jpeg_decode_scratch_bytes", progressive), n, files, lengths, progressive, plan))
+  if (make_plan(entry_name("sqdet_jpeg_decode_scratch_bytes", mode), n, files, lengths, mode, plan))
     return -1;
   return plan.scratch;
 }
 
 int decode_entry(int n, const uint8_t* const* files_host, const int64_t* lengths, uint8_t* const* out_planes,
                  const int64_t* out_pitches, void* staging_pinned, int64_t staging_bytes, void* scratch_dev,
-                 int64_t scratch_bytes, int32_t* status_dev, void* stream, bool progressive) {
-  const std::string name = entry_name("sqdet_decode_jpeg", progressive);
+                 int64_t scratch_bytes, int32_t* status_dev, void* stream, const Mode& mode) {
+  const std::string name = entry_name("sqdet_decode_jpeg", mode);
   if (!out_planes || !out_pitches || !staging_pinned || !scratch_dev || !status_dev)
     return fail(SQDET_ERR_INVALID_ARG, name + ": null argument");
   Plan plan;
-  int rc = make_plan(name, n, files_host, lengths, progressive, plan);
+  int rc = make_plan(name, n, files_host, lengths, mode, plan);
   if (rc) return rc;
   std::vector<const sqdet_jpeg_info*> info((size_t)n);
   for (const Input& in : plan.in) info[(size_t)in.index] = &in.P.info;
   rc = check_decode_args(name, n, info.data(), out_planes, out_pitches, staging_pinned, staging_bytes,
                          plan.staging, scratch_dev, scratch_bytes, plan.scratch, status_dev,
-                         entry_name("sqdet_jpeg_decode_staging_bytes", progressive),
-                         entry_name("sqdet_jpeg_decode_scratch_bytes", progressive));
+                         entry_name("sqdet_jpeg_decode_staging_bytes", mode),
+                         entry_name("sqdet_jpeg_decode_scratch_bytes", mode));
   if (rc) return rc;
   fill_staging(plan, files_host, out_planes, out_pitches, static_cast<uint8_t*>(staging_pinned));
   DeviceGuard guard(pointer_device(out_planes[0]));
@@ -1820,21 +1965,38 @@ int decode_entry(int n, const uint8_t* const* files_host, const int64_t* lengths
   return launch_decode(plan, static_cast<uint8_t*>(staging_pinned), static_cast<uint8_t*>(scratch_dev),
                        status_dev, (cudaStream_t)stream);
 }
+
+constexpr Mode kPlain{false, 1, ""}, kProgressive{true, 1, "_progressive"};
+
+// A sqdet_jpeg_decode_params as a Mode; false (with the error set) when it is not one.
+bool params_mode(const char* plain, const sqdet_jpeg_decode_params* params, Mode& mode) {
+  const std::string name = std::string(plain) + "_params";
+  if (!params) return fail(SQDET_ERR_INVALID_ARG, name + ": params is null"), false;
+  const int s = params->scale_denom;
+  if (params->progressive != 0 && params->progressive != 1)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": progressive must be 0 or 1"), false;
+  if (s != 1 && s != 2 && s != 4 && s != 8)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": scale_denom must be 1, 2, 4 or 8"), false;
+  if (params->reserved[0] || params->reserved[1])
+    return fail(SQDET_ERR_INVALID_ARG, name + ": reserved must be 0"), false;
+  mode = Mode{params->progressive == 1, s, "_params"};
+  return true;
+}
 }  // namespace
 }  // namespace sqdet
 
 using namespace sqdet;
 
 int sqdet_jpeg_parse(const uint8_t* file, int64_t len, sqdet_jpeg_info* out) {
-  return parse_entry(file, len, out, false);
+  return parse_entry(file, len, out, kPlain);
 }
 
 int64_t sqdet_jpeg_decode_staging_bytes(int n, const uint8_t* const* files_host, const int64_t* lengths) {
-  return staging_bytes_entry(n, files_host, lengths, false);
+  return staging_bytes_entry(n, files_host, lengths, kPlain);
 }
 
 int64_t sqdet_jpeg_decode_scratch_bytes(int n, const uint8_t* const* files_host, const int64_t* lengths) {
-  return scratch_bytes_entry(n, files_host, lengths, false);
+  return scratch_bytes_entry(n, files_host, lengths, kPlain);
 }
 
 int sqdet_jpeg_decode_set_subsequence_bits(int bits) {
@@ -1850,21 +2012,21 @@ int sqdet_decode_jpeg(int n, const uint8_t* const* files_host, const int64_t* le
                       int64_t staging_bytes, void* scratch_dev, int64_t scratch_bytes,
                       int32_t* status_dev, void* stream) {
   return decode_entry(n, files_host, lengths, out_planes, out_pitches, staging_pinned, staging_bytes,
-                      scratch_dev, scratch_bytes, status_dev, stream, false);
+                      scratch_dev, scratch_bytes, status_dev, stream, kPlain);
 }
 
 int sqdet_jpeg_parse_progressive(const uint8_t* file, int64_t len, sqdet_jpeg_info* out) {
-  return parse_entry(file, len, out, true);
+  return parse_entry(file, len, out, kProgressive);
 }
 
 int64_t sqdet_jpeg_decode_staging_bytes_progressive(int n, const uint8_t* const* files_host,
                                                     const int64_t* lengths) {
-  return staging_bytes_entry(n, files_host, lengths, true);
+  return staging_bytes_entry(n, files_host, lengths, kProgressive);
 }
 
 int64_t sqdet_jpeg_decode_scratch_bytes_progressive(int n, const uint8_t* const* files_host,
                                                     const int64_t* lengths) {
-  return scratch_bytes_entry(n, files_host, lengths, true);
+  return scratch_bytes_entry(n, files_host, lengths, kProgressive);
 }
 
 int sqdet_decode_jpeg_progressive(int n, const uint8_t* const* files_host, const int64_t* lengths,
@@ -1872,5 +2034,39 @@ int sqdet_decode_jpeg_progressive(int n, const uint8_t* const* files_host, const
                                   void* staging_pinned, int64_t staging_bytes, void* scratch_dev,
                                   int64_t scratch_bytes, int32_t* status_dev, void* stream) {
   return decode_entry(n, files_host, lengths, out_planes, out_pitches, staging_pinned, staging_bytes,
-                      scratch_dev, scratch_bytes, status_dev, stream, true);
+                      scratch_dev, scratch_bytes, status_dev, stream, kProgressive);
+}
+
+int sqdet_jpeg_parse_params(const uint8_t* file, int64_t len, const sqdet_jpeg_decode_params* params,
+                            sqdet_jpeg_info* out) {
+  Mode mode;
+  if (!params_mode("sqdet_jpeg_parse", params, mode)) return SQDET_ERR_INVALID_ARG;
+  return parse_entry(file, len, out, mode);
+}
+
+int64_t sqdet_jpeg_decode_staging_bytes_params(int n, const uint8_t* const* files_host,
+                                               const int64_t* lengths,
+                                               const sqdet_jpeg_decode_params* params) {
+  Mode mode;
+  if (!params_mode("sqdet_jpeg_decode_staging_bytes", params, mode)) return -1;
+  return staging_bytes_entry(n, files_host, lengths, mode);
+}
+
+int64_t sqdet_jpeg_decode_scratch_bytes_params(int n, const uint8_t* const* files_host,
+                                               const int64_t* lengths,
+                                               const sqdet_jpeg_decode_params* params) {
+  Mode mode;
+  if (!params_mode("sqdet_jpeg_decode_scratch_bytes", params, mode)) return -1;
+  return scratch_bytes_entry(n, files_host, lengths, mode);
+}
+
+int sqdet_decode_jpeg_params(int n, const uint8_t* const* files_host, const int64_t* lengths,
+                             const sqdet_jpeg_decode_params* params, uint8_t* const* out_planes,
+                             const int64_t* out_pitches, void* staging_pinned, int64_t staging_bytes,
+                             void* scratch_dev, int64_t scratch_bytes, int32_t* status_dev,
+                             void* stream) {
+  Mode mode;
+  if (!params_mode("sqdet_decode_jpeg", params, mode)) return SQDET_ERR_INVALID_ARG;
+  return decode_entry(n, files_host, lengths, out_planes, out_pitches, staging_pinned, staging_bytes,
+                      scratch_dev, scratch_bytes, status_dev, stream, mode);
 }

@@ -94,20 +94,35 @@ jpeg_bytes = file_bytes
 # ---- decoding ------------------------------------------------------------------------------------
 JPEG_TOO_LARGE = 10       # SQDET_JPEG_TOO_LARGE: past cv2's limits, so cv2.imdecode refuses it too
 JPEG_BAD_PROGRESSION = 11  # SQDET_JPEG_BAD_PROGRESSION: cv2.imdecode returns None
+JPEG_CODED_TOO_LARGE = 15  # SQDET_JPEG_CODED_TOO_LARGE: cv2.imdecode decodes it at this scale
+# the scales decode_jpeg_device takes: cv2's IMREAD_COLOR and IMREAD_REDUCED_COLOR_2, _4 and _8
+REDUCTIONS = (1, 2, 4, 8)
 
 
-def jpeg_info(file_bytes, progressive=False):
+def _decode_call(progressive, reduce):
+  """(suffix of the C functions, their sqdet_jpeg_decode_params or None): the plain or
+  _progressive functions at full size, the _params ones at a reduced scale."""
+  if reduce not in REDUCTIONS:
+    raise ValueError('reduce must be one of %s, got %r' % (', '.join(map(str, REDUCTIONS)), reduce))
+  if reduce == 1:
+    return ('_progressive' if progressive else ''), None
+  return '_params', _lib.JpegDecodeParams(int(bool(progressive)), reduce)
+
+
+def jpeg_info(file_bytes, progressive=False, reduce=1):
   """sqdet_jpeg_parse of one file -> dict: height and width of the decoded frame (after the EXIF
-  orientation), coded_height, coded_width, components, h_samp, v_samp (luma sampling),
-  orientation, restart_interval, supported (bool), reason (a SQDET_JPEG_* code) and reason_text
-  (the library's words for it).  With progressive, sqdet_jpeg_parse_progressive: whether
-  decode_jpeg_device(..., progressive=True) decodes it.  Host only."""
+  orientation, and at scale 1 / reduce), coded_height, coded_width, components, h_samp, v_samp
+  (luma sampling), orientation, restart_interval, supported (bool), reason (a SQDET_JPEG_* code)
+  and reason_text (the library's words for it).  With progressive, sqdet_jpeg_parse_progressive:
+  whether decode_jpeg_device(..., progressive=True) decodes it; with reduce 2, 4 or 8,
+  sqdet_jpeg_parse_params: whether decode_jpeg_device(..., reduce=reduce) does.  Host only."""
+  kind, params = _decode_call(progressive, reduce)
   b = bytes(file_bytes)
   info = _lib.JpegInfo()
   buf = C.create_string_buffer(b, len(b))
   lib = _lib.load()
-  parse = lib.sqdet_jpeg_parse_progressive if progressive else lib.sqdet_jpeg_parse
-  rc = parse(buf, len(b), C.byref(info))
+  parse = getattr(lib, 'sqdet_jpeg_parse' + kind)
+  rc = parse(buf, len(b), *((C.byref(params),) if params else ()), C.byref(info))
   if rc not in (_lib.OK, -3):
     _lib.check(rc)
   out = {k: int(getattr(info, k)) for k, _ in _lib.JpegInfo._fields_ if k != 'reserved'}
@@ -142,7 +157,7 @@ class _Staging:
 _staging = {}
 
 
-def decode_jpeg_device(files, device, stream=None, *, progressive=False):
+def decode_jpeg_device(files, device, stream=None, *, progressive=False, reduce=1):
   """JPEG files (bytes-like, on the host) -> (frames, status): frames[i] is a uint8 [H, W, 3] BGR
   CUDA tensor on `device` with exactly the pixels of cv2.imdecode(files[i], cv2.IMREAD_COLOR), and
   status an int32 [n] CUDA tensor, 0 where the file decoded and negative where its entropy-coded
@@ -169,8 +184,16 @@ def decode_jpeg_device(files, device, stream=None, *, progressive=False):
   components are out of the frame's order, for a file libjpeg would block-smooth (an incomplete
   one: complete files, such as every file cv2 or encode_jpeg_device writes, are not smoothed) and
   for more than 256 scans; route those to cv2.imdecode.  A progressive scan without restart
-  markers is decoded by one GPU lane, so these files decode much slower than sequential ones."""
+  markers is decoded by one GPU lane, so these files decode much slower than sequential ones.
+
+  reduce=2, 4 or 8 (sqdet_decode_jpeg_params) decodes each file at that fraction of its size, to
+  exactly the pixels of cv2.imdecode(files[i], cv2.IMREAD_REDUCED_COLOR_<reduce>): a frame of
+  ceil(H / reduce) x ceil(W / reduce) before the orientation, from libjpeg's scaled IDCTs, so a
+  12 MP camera file takes a 2.3 MB frame at 1/4 instead of 36 MB.  The size limit then applies to
+  the reduced frame, as in cv2; a file of more than 2^30 coded pixels whose reduced frame fits
+  still raises ValueError, and cv2.imdecode decodes it.  Any other reduce raises ValueError."""
   import torch
+  kind, params = _decode_call(progressive, reduce)
   files = [bytes(f) for f in files]
   n = len(files)
   if not 1 <= n <= 128:
@@ -184,7 +207,7 @@ def decode_jpeg_device(files, device, stream=None, *, progressive=False):
   for i, f in enumerate(files):
     if len(f) < 4:
       raise ValueError('file %d: not a JPEG file (%d bytes)' % (i, len(f)))
-    info = jpeg_info(f, progressive)
+    info = jpeg_info(f, progressive, reduce)
     if not info['supported']:
       raise ValueError('file %d: not supported (%s); %s' % (
           i, info['reason_text'], 'nor does cv2.imdecode decode it'
@@ -194,9 +217,9 @@ def decode_jpeg_device(files, device, stream=None, *, progressive=False):
   bufs = [C.create_string_buffer(f, len(f)) for f in files]
   ptrs = (C.c_void_p * n)(*[C.addressof(b) for b in bufs])
   lens = (C.c_int64 * n)(*[len(f) for f in files])
-  kind = '_progressive' if progressive else ''
-  staging_bytes = getattr(lib, 'sqdet_jpeg_decode_staging_bytes' + kind)(n, ptrs, lens)
-  scratch_bytes = getattr(lib, 'sqdet_jpeg_decode_scratch_bytes' + kind)(n, ptrs, lens)
+  pargs = (C.byref(params),) if params else ()
+  staging_bytes = getattr(lib, 'sqdet_jpeg_decode_staging_bytes' + kind)(n, ptrs, lens, *pargs)
+  scratch_bytes = getattr(lib, 'sqdet_jpeg_decode_scratch_bytes' + kind)(n, ptrs, lens, *pargs)
   if staging_bytes < 0 or scratch_bytes < 0:
     raise _lib.SqdetError(-1, lib.sqdet_last_error().decode('utf-8', 'replace'))
   s = torch_stream(stream, device)
@@ -210,7 +233,7 @@ def decode_jpeg_device(files, device, stream=None, *, progressive=False):
     outs = (C.c_void_p * n)(*[t.data_ptr() for t in frames])
     pitches = (C.c_int64 * n)(*[3 * t.shape[1] for t in frames])
     _lib.check(getattr(lib, 'sqdet_decode_jpeg' + kind)(
-        n, ptrs, lens, outs, pitches, buf.data_ptr(), buf.numel(), scratch.data_ptr(),
+        n, ptrs, lens, *pargs, outs, pitches, buf.data_ptr(), buf.numel(), scratch.data_ptr(),
         scratch_bytes, status.data_ptr(), s.cuda_stream))
     staging.events[slot] = torch.cuda.Event()
     staging.events[slot].record(s)
