@@ -694,7 +694,7 @@ int sqdet_encode_png(int n, int format, const uint8_t* const* planes, const int6
 typedef struct {
   int32_t height, width;              /* of the decoded frame (reduced, see _params), after orientation */
   int32_t coded_height, coded_width;  /* as SOF gives them */
-  int32_t components;                 /* 1 or 3 */
+  int32_t components;                 /* 1 or 3 (4 too with any_layout) */
   int32_t h_samp, v_samp;             /* luma sampling factors (chroma is 1x1) */
   int32_t orientation;                /* EXIF Orientation 1..8 (1 without one) */
   int32_t restart_interval;           /* MCUs per restart interval, 0 for none */
@@ -818,6 +818,63 @@ int sqdet_decode_jpeg_params(int n, const uint8_t* const* files_host, const int6
                              const int64_t* out_pitches, void* staging_pinned, int64_t staging_bytes,
                              void* scratch_dev, int64_t scratch_bytes, int32_t* status_dev,
                              void* stream);
+
+/* ---- JPEG decoding of every colour space and sampling cv2.imdecode reads -------------
+ * The _options functions take the arguments of the _params ones with a
+ * sqdet_jpeg_decode_options in place of the params:
+ *   progressive, scale_denom  as in sqdet_jpeg_decode_params
+ *   any_layout   0: the files the _params functions decode (they are these functions with
+ *                any_layout = 0); 1: those and the layouts below; anything else is
+ *                SQDET_ERR_INVALID_ARG
+ *   reserved     0
+ * With any_layout = 1, file i is still exactly cv2.imdecode(file, IMREAD_COLOR or
+ * IMREAD_REDUCED_COLOR_s) and these Huffman-coded 8-bit files decode too:
+ *   colour space  as libjpeg's default_decompress_parms decides it.  3 components: YCbCr after a
+ *                 JFIF APP0, else RGB for an Adobe APP14 transform 0 (any other transform:
+ *                 YCbCr), else RGB for component ids 'R','G','B', else YCbCr.  RGB planes come out
+ *                 as they are (B, G, R = planes 2, 1, 0).  4 components: YCCK for an Adobe
+ *                 transform other than 0, else CMYK.  cv2 reads 4 components as libjpeg's CMYK
+ *                 (YCCK through ycck_cmyk_convert: C, M, Y = 255 - the clamped YCbCr->RGB of Y,
+ *                 Cb, Cr; K as coded) and converts each pixel with icvCvt_CMYK2BGR:
+ *                 B = K - ((255 - Y) * K >> 8), G from M, R from C; no Adobe inversion.
+ *   sampling      factors 1..4 with max_h / h and max_v / v integral for every component (the
+ *                 largest factors need not be component 0's) and at most 10 blocks in an
+ *                 interleaved MCU: a sequential file's scan, and each interleaved progressive
+ *                 scan.  Each component is upsampled as jinit_upsampler chooses from its scaled
+ *                 IDCT size: not at all when it has the frame's size; h2v1 and h2v2 by the
+ *                 triangle filters when fancy upsampling is on and its downsampled width is above
+ *                 2, by replication otherwise; h1v2 by the triangle filter when fancy upsampling
+ *                 is on; any other integral ratio by replication (int_upsample).  Fancy
+ *                 upsampling is on at scales 1, 1/2 and 1/4 and off at 1/8.  Upsampling comes
+ *                 before the colour conversion, whatever the colour space.
+ * Refused with any_layout = 1, each with what cv2 does:
+ *   SQDET_JPEG_BAD_SAMPLING   a ratio that is not integral, or more than 10 blocks in an
+ *                             interleaved MCU: libjpeg rejects the file and cv2 returns None
+ *   SQDET_JPEG_COMPONENTS     2 components, or more than 4: libjpeg has no conversion of them to
+ *                             BGR and cv2 returns None
+ * Arithmetic, lossless, 12-bit and multi-scan sequential files keep their refusals.  The plain,
+ * _progressive and _params functions keep refusing every file they refused before, with the
+ * same reasons.                                                                               */
+#define SQDET_JPEG_BAD_SAMPLING     16  /* any_layout: sampling libjpeg rejects: cv2 returns None */
+typedef struct {
+  int32_t progressive;
+  int32_t scale_denom;
+  int32_t any_layout;
+  int32_t reserved[5];
+} sqdet_jpeg_decode_options;
+int sqdet_jpeg_parse_options(const uint8_t* file, int64_t len, const sqdet_jpeg_decode_options* options,
+                             sqdet_jpeg_info* out);
+int64_t sqdet_jpeg_decode_staging_bytes_options(int n, const uint8_t* const* files_host,
+                                                const int64_t* lengths,
+                                                const sqdet_jpeg_decode_options* options);
+int64_t sqdet_jpeg_decode_scratch_bytes_options(int n, const uint8_t* const* files_host,
+                                                const int64_t* lengths,
+                                                const sqdet_jpeg_decode_options* options);
+int sqdet_decode_jpeg_options(int n, const uint8_t* const* files_host, const int64_t* lengths,
+                              const sqdet_jpeg_decode_options* options, uint8_t* const* out_planes,
+                              const int64_t* out_pitches, void* staging_pinned, int64_t staging_bytes,
+                              void* scratch_dev, int64_t scratch_bytes, int32_t* status_dev,
+                              void* stream);
 
 /* ---- KITTI 2-D object scoring of filtered records (no engine needed) ---------------
  * sqdet_kitti_eval scores n images of records exactly as the KITTI devkit's evaluate_object does

@@ -72,6 +72,12 @@ class JpegDecodeParams(C.Structure):
   _fields_ = [('progressive', C.c_int32), ('scale_denom', C.c_int32), ('reserved', C.c_int32 * 2)]
 
 
+class JpegDecodeOptions(C.Structure):
+  """struct sqdet_jpeg_decode_options."""
+  _fields_ = [('progressive', C.c_int32), ('scale_denom', C.c_int32), ('any_layout', C.c_int32),
+              ('reserved', C.c_int32 * 5)]
+
+
 _vp, _i, _f, _i64 = C.c_void_p, C.c_int, C.c_float, C.c_int64
 _ip = C.POINTER(C.c_int)
 _i64p = C.POINTER(C.c_int64)
@@ -172,6 +178,11 @@ SIGNATURES = {
     'sqdet_jpeg_decode_scratch_bytes_params': (_i64, [_i, _vp, _vp, C.POINTER(JpegDecodeParams)]),
     'sqdet_decode_jpeg_params': (_i, [_i, _vp, _vp, C.POINTER(JpegDecodeParams), _vp, _vp, _vp, _i64,
                                       _vp, _i64, _vp, _vp]),
+    'sqdet_jpeg_parse_options': (_i, [_vp, _i64, C.POINTER(JpegDecodeOptions), C.POINTER(JpegInfo)]),
+    'sqdet_jpeg_decode_staging_bytes_options': (_i64, [_i, _vp, _vp, C.POINTER(JpegDecodeOptions)]),
+    'sqdet_jpeg_decode_scratch_bytes_options': (_i64, [_i, _vp, _vp, C.POINTER(JpegDecodeOptions)]),
+    'sqdet_decode_jpeg_options': (_i, [_i, _vp, _vp, C.POINTER(JpegDecodeOptions), _vp, _vp, _vp, _i64,
+                                       _vp, _i64, _vp, _vp]),
     'sqdet_malloc': (_i, [_i, _i64, C.POINTER(_vp)]),
     'sqdet_free': (_i, [_i, _vp]),
     'sqdet_malloc_host': (_i, [_i64, C.POINTER(_vp)]),

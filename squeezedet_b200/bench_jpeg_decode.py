@@ -25,6 +25,10 @@ first scans, the DC refinements and the AC refinements separately.
 IMREAD_REDUCED_COLOR_s), (b) with decode_jpeg_device(reduce=s); the forward resizes the smaller
 frames.  Each row reports the device bytes of a call: its frames and its decode scratch.
 
+--layout cmyk or rgb writes the same pictures as Pillow's CMYK files (Adobe-inverted, 4:4:4, four
+components) or its RGB-coded files (keep_rgb: Adobe transform 0, 4:4:4), quality 95, and decodes
+them with decode_jpeg_device(any_layout=True); (a) is cv2.imdecode of the same files.
+
 Prints one JSON line with the card's name and power limit, read in the same run; writes nothing.
 """
 from __future__ import annotations
@@ -57,6 +61,7 @@ def parse_args(argv=None):
   ap.add_argument('--gpu', type=int, default=0)
   ap.add_argument('--progressive', action='store_true')
   ap.add_argument('--reduce', type=int, choices=(1, 2, 4, 8), default=1)
+  ap.add_argument('--layout', choices=('cmyk', 'rgb'), default=None)
   return ap.parse_args(argv)
 
 
@@ -66,6 +71,25 @@ def picture(h, w, rng):
   low = rng.uniform(0, 255, (max(h // 24, 2), max(w // 24, 2), 3)).astype(np.float32)
   up = cv2.resize(low, (w, h), interpolation=cv2.INTER_LINEAR)
   return np.clip(up + rng.normal(0, 4, (h, w, 3)), 0, 255).astype(np.uint8)
+
+
+def encode(img, args):
+  """A quality-95 JPEG of BGR img: cv2's (4:2:0), or with --layout Pillow's CMYK or RGB-coded one."""
+  import cv2
+  if args.layout is None:
+    params = [cv2.IMWRITE_JPEG_QUALITY, QUALITY] + ([cv2.IMWRITE_JPEG_PROGRESSIVE, 1] if args.progressive else [])
+    return cv2.imencode('.jpg', img, params)[1].tobytes()
+  import io
+  from PIL import Image
+  rgb = np.ascontiguousarray(img[..., ::-1])
+  if args.layout == 'cmyk':
+    im = Image.fromarray(np.concatenate([255 - rgb, np.zeros(rgb.shape[:2] + (1,), np.uint8)], axis=2), 'CMYK')
+    kw = {}
+  else:
+    im, kw = Image.fromarray(rgb, 'RGB'), {'keep_rgb': True}
+  buf = io.BytesIO()
+  im.save(buf, 'JPEG', quality=QUALITY, progressive=args.progressive, **kw)
+  return buf.getvalue()
 
 
 def measure_workload(args, name, model, files, torch):
@@ -95,7 +119,7 @@ def measure_workload(args, name, model, files, torch):
 
   def form_b():
     frames, status = decode_jpeg_device(files, dev, stream=stream, progressive=args.progressive,
-                                        reduce=args.reduce)
+                                        reduce=args.reduce, any_layout=args.layout is not None)
     model.forward_device_frames(frames, stream=stream.cuda_stream)
     stream.synchronize()
     return status
@@ -126,9 +150,9 @@ def measure_workload(args, name, model, files, torch):
   with profile(activities=[ProfilerActivity.CUDA]) as prof:
     for _ in range(calls):
       keep.append(decode_jpeg_device(files, dev, stream=stream, progressive=args.progressive,
-                                     reduce=args.reduce))
+                                     reduce=args.reduce, any_layout=args.layout is not None))
     stream.synchronize()
-  names = PROG_KERNELS if args.progressive else KERNELS
+  names = (PROG_KERNELS if args.progressive else KERNELS) + (('color_any_kernel',) if args.layout else ())
   evs = [ev for ev in prof.events() if ev.device_type == DeviceType.CUDA and
          any(k in ev.name for k in names + ('emset', 'emcpy', 'Memcpy', 'Memset'))]
   kern = [ev for ev in evs if any(k in ev.name for k in names)]
@@ -143,11 +167,11 @@ def measure_workload(args, name, model, files, torch):
                  'ms_per_frame_step_min': 1e3 * min(step[form]) / n}
   row['decode_device'] = {'us_per_frame_kernels': us_k / n, 'us_per_frame_with_copy_and_memsets': us / n,
                           'calls_timed': calls}
-  infos = [jpeg_info(f, args.progressive, args.reduce) for f in files]
+  infos = [jpeg_info(f, args.progressive, args.reduce, args.layout is not None) for f in files]
   bufs = [C.create_string_buffer(f, len(f)) for f in files]
-  params = _lib.JpegDecodeParams(int(args.progressive), args.reduce)
-  scratch = lib.sqdet_jpeg_decode_scratch_bytes_params(
-      n, (C.c_void_p * n)(*[C.addressof(b) for b in bufs]), (C.c_int64 * n)(*map(len, files)), C.byref(params))
+  options = _lib.JpegDecodeOptions(int(args.progressive), args.reduce, int(args.layout is not None))
+  scratch = lib.sqdet_jpeg_decode_scratch_bytes_options(
+      n, (C.c_void_p * n)(*[C.addressof(b) for b in bufs]), (C.c_int64 * n)(*map(len, files)), C.byref(options))
   row['device_bytes_per_call'] = {'frames': sum(3 * i['height'] * i['width'] for i in infos),
                                   'decode_scratch': int(scratch),
                                   'frame_hw': [infos[0]['height'], infos[0]['width']]}
@@ -176,14 +200,15 @@ def measure(args):
   rows = []
   for name, (h, w) in (('kitti_1242x375', (375, 1242)), ('1080p', (1080, 1920)),
                        ('camera_4000x3000', (3000, 4000))):
-    params = [cv2.IMWRITE_JPEG_QUALITY, QUALITY] + ([cv2.IMWRITE_JPEG_PROGRESSIVE, 1] if args.progressive else [])
-    files = [cv2.imencode('.jpg', picture(h, w, rng), params)[1].tobytes() for _ in range(args.frames)]
+    files = [encode(picture(h, w, rng), args) for _ in range(args.frames)]
     rows.append(measure_workload(args, name, model, files, torch))
-  kind = 'progressive ' if args.progressive else ''
+  kind = ('progressive ' if args.progressive else '') + \
+      {None: '', 'cmyk': "Pillow's CMYK ", 'rgb': "Pillow's RGB-coded "}[args.layout]
   scale = ' at 1/%d (IMREAD_REDUCED_COLOR_%d)' % (args.reduce, args.reduce) if args.reduce > 1 else ''
-  return {'workload': 'squeezeDet 1242x375 forward_device_frames on %sJPEG files (quality 95, 4:2:0, '
+  return {'workload': 'squeezeDet 1242x375 forward_device_frames on %sJPEG files (quality 95, %s, '
                       'smooth synthetic pictures) decoded%s by a cv2.imdecode thread pool and '
-                      'uploaded, or by decode_jpeg_device' % (kind, scale), 'reduce': args.reduce,
+                      'uploaded, or by decode_jpeg_device' % (kind, '4:4:4' if args.layout else '4:2:0', scale),
+          'reduce': args.reduce, 'layout': args.layout or 'ycc',
           'gpu': gpu_info(args.gpu), 'cpu_threads': os.cpu_count(),
           'timer': 'host clock per step from the files on the host to a device synchronisation '
                    'after the forward; decode kernels: torch.profiler device durations, summed, per frame',

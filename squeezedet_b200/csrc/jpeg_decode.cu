@@ -3,8 +3,11 @@
 // libjpeg-turbo's (SIMD) islow IDCT, fancy upsampling, fixed-point YCbCr->RGB and the EXIF orientation.
 // With a scale_denom s of 2, 4 or 8 (sqdet_decode_jpeg_params) it is cv2.imdecode(file_i,
 // IMREAD_REDUCED_COLOR_s): each component's scaled IDCT (8, 4, 2 or 1 samples a side, planned per
-// component as libjpeg plans it), then that scale's upsampling.  oracle/jpeg_decode.py restates the
-// full-size decode in numpy, oracle/jpeg_decode_reduced.py the reduced one.
+// component as libjpeg plans it), then that scale's upsampling.  With any_layout
+// (sqdet_decode_jpeg_options) also CMYK, YCCK and RGB-coded files and every sampling libjpeg
+// decodes: each component upsampled by its own factors, then its colour space converted as cv2
+// reads it.  oracle/jpeg_decode.py restates the full-size decode in numpy,
+// oracle/jpeg_decode_reduced.py the reduced one, oracle/jpeg_decode_layouts.py the other layouts.
 //
 // The host parses the headers, builds each file's Huffman lookup and quantization tables and
 // packs them with the raw entropy-coded bytes into the caller's pinned staging; one copy takes
@@ -31,7 +34,8 @@
 //   9. idct            per 8x8 block, the component's planned IDCT: jpeg_idct_islow, _4x4 or _2x2
 //                      (as libjpeg-turbo's SIMD code computes them) or _1x1, into its plane
 //  10. color           per output pixel: orientation, the planned upsampling (fancy or
-//                      replicated), YCbCr->BGR
+//                      replicated), YCbCr->BGR; color_any for the other layouts (launched only
+//                      when a call has one)
 // All loops are bounded by host-known sizes; a corrupt entropy-coded segment sets a negative
 // status for its file and nothing else.
 #include <algorithm>
@@ -80,22 +84,32 @@ struct HuffTab {
   uint8_t vals[256];
 };
 
+constexpr int kMaxComps = 4;
+constexpr int kMaxBlocks = 10;           // libjpeg's D_MAX_BLOCKS_IN_MCU
+
+// libjpeg's colour space of a file, as default_decompress_parms decides it
+enum Space : int8_t { kYcc = 0, kGray, kRgb, kCmyk, kYcck };
+
 // Everything the kernels know of one file.  Offsets are bytes from the scratch's start.
 struct DecFile {
   int32_t h, w, oh, ow, ncomp, orient;
   int32_t mcu_cols, mcus, bpm, restart, intervals;
   int32_t raw_len, chunks, blocks, sub_max;
   int32_t sub_bits;
-  int8_t bcomp[10], bdy[10], bdx[10];  // per block of an MCU: component, block row and column in it
-  int8_t ch[3], cv[3];                 // sampling factors
-  int8_t isz[3];                       // IDCT size: samples a side per block (8 at full size)
-  int8_t uh[3], uv[3];                 // upsampling factors to the frame
+  int8_t bcomp[kMaxBlocks], bdy[kMaxBlocks], bdx[kMaxBlocks];  // per block of an MCU: component,
+                                                               // block row and column in it
+  int8_t ch[kMaxComps], cv[kMaxComps];  // sampling factors
+  int8_t isz[kMaxComps];               // IDCT size: samples a side per block (8 at full size)
+  int8_t uh[kMaxComps], uv[kMaxComps];  // upsampling factors to the frame
   int8_t fancy;                        // fancy upsampling (off at 1/8)
-  int32_t pw[3], ph[3];                // padded plane width and height (whole blocks)
-  int32_t cw[3], chh[3];               // component width and height in samples
-  int16_t q[3][64];                    // dequantization, natural order (libjpeg's short multiplier)
+  int8_t space;                        // Space
+  int8_t general;                      // converted by color_any_kernel, not color_kernel
+  int32_t pw[kMaxComps], ph[kMaxComps];  // padded plane width and height (whole blocks)
+  int32_t cw[kMaxComps], chh[kMaxComps];  // component width and height in samples
+  int16_t q[kMaxComps][64];            // dequantization, natural order (libjpeg's short multiplier)
   int32_t index;                       // the file's index in the call: where its status goes
-  int64_t raw, clean, sums, term, ist, sbase, entry, exit_, counts, coef, plane[3], tabs;
+  int64_t raw, clean, sums, term, ist, sbase, entry, exit_, counts, coef, plane[kMaxComps], tabs;
+  int64_t counts3;                     // 4 components: component 3's DC sums beside counts
   uint8_t* out;
   int64_t pitch;
 };
@@ -288,7 +302,7 @@ __device__ __forceinline__ int extend(uint32_t v, int s) {
 }
 
 struct Counts {
-  int blocks, dc[3];
+  int blocks, dc[kMaxComps];
 };
 
 // Decodes from state st while st.p < end and fewer than block_limit blocks are complete.  kWrite:
@@ -386,7 +400,7 @@ __device__ void sync_rounds(const DecFile& f, const HuffTab* tabs, const uint8_t
   for (int round = 0; round < kTile; ++round) {
     if (dirty && valid) {
       State st = entry[t];
-      cnt = Counts{0, {0, 0, 0}};
+      cnt = Counts{0, {0, 0, 0, 0}};
       decode_run<false>(f, tabs, clean, st, sub.end, INT32_MAX, cnt, nullptr, 0, f.sub_bits + 64);
       exit_[t] = st;
     }
@@ -422,12 +436,13 @@ __global__ void __launch_bounds__(kTile) sync_tiles_kernel(DecParams p) {
   const bool valid = g < nsub;
   const Sub sub = valid ? locate(f, ist, sbase, g) : Sub{0, 0, 0, 0, 0};
   entry[threadIdx.x] = State{sub.start, 0};
-  Counts cnt{0, {0, 0, 0}};
+  Counts cnt{0, {0, 0, 0, 0}};
   sync_rounds(f, tabs, clean, sub, valid, true, entry, exit_, cnt, starts);
   if (valid) {
     reinterpret_cast<State*>(p.s + f.entry)[g] = entry[threadIdx.x];
     reinterpret_cast<State*>(p.s + f.exit_)[g] = exit_[threadIdx.x];
     reinterpret_cast<int4*>(p.s + f.counts)[g] = make_int4(cnt.blocks, cnt.dc[0], cnt.dc[1], cnt.dc[2]);
+    if (f.ncomp == 4) reinterpret_cast<int32_t*>(p.s + f.counts3)[g] = cnt.dc[3];
   }
 }
 
@@ -444,6 +459,7 @@ __global__ void __launch_bounds__(kTile) sync_chain_kernel(DecParams p) {
   State* gentry = reinterpret_cast<State*>(p.s + f.entry);
   State* gexit = reinterpret_cast<State*>(p.s + f.exit_);
   int4* gcounts = reinterpret_cast<int4*>(p.s + f.counts);
+  int32_t* gcounts3 = reinterpret_cast<int32_t*>(p.s + f.counts3);
   const int tiles = (f.sub_max + kTile - 1) / kTile;
 #pragma unroll 1
   for (int tile = 1; tile < tiles; ++tile) {
@@ -462,13 +478,14 @@ __global__ void __launch_bounds__(kTile) sync_chain_kernel(DecParams p) {
       exit_[threadIdx.x] = gexit[g];
     }
     const int4 c4 = valid ? gcounts[g] : make_int4(0, 0, 0, 0);
-    Counts cnt{c4.x, {c4.y, c4.z, c4.w}};
+    Counts cnt{c4.x, {c4.y, c4.z, c4.w, valid && f.ncomp == 4 ? gcounts3[g] : 0}};
     __syncthreads();
     sync_rounds(f, tabs, clean, sub, valid, threadIdx.x == 0, entry, exit_, cnt, starts);
     if (valid) {
       gentry[g] = entry[threadIdx.x];
       gexit[g] = exit_[threadIdx.x];
       gcounts[g] = make_int4(cnt.blocks, cnt.dc[0], cnt.dc[1], cnt.dc[2]);
+      if (f.ncomp == 4) gcounts3[g] = cnt.dc[3];
     }
     __syncthreads();
   }
@@ -492,6 +509,16 @@ __global__ void __launch_bounds__(kScanThreads) scan_counts_kernel(DecParams p) 
     if (i < nsub) c[i] = make_int4(carry.x + ex.x, carry.y + ex.y, carry.z + ex.z, carry.w + ex.w);
     carry = make_int4(carry.x + tot.x, carry.y + tot.y, carry.z + tot.z, carry.w + tot.w);
   }
+  if (f.ncomp != 4) return;                // uniform: one file per CTA
+  int32_t* c3 = reinterpret_cast<int32_t*>(p.s + f.counts3);
+  int32_t carry3 = 0;
+  for (int base = 0; base < nsub; base += kScanThreads) {
+    const int i = base + threadIdx.x;
+    int32_t tot;
+    const int32_t ex = block_exclusive_scan(i < nsub ? c3[i] : 0, warp, &tot);
+    if (i < nsub) c3[i] = carry3 + ex;
+    carry3 += tot;
+  }
 }
 
 // ---- 8. decode and write coefficients -----------------------------------------------------------------
@@ -507,7 +534,9 @@ __global__ void __launch_bounds__(kTile) decode_write_kernel(DecParams p) {
   const Sub sub = locate(f, ist, sbase, g);
   const int4 mine = counts[g], base = counts[sbase[sub.r]];
   const int interval_blocks = min(f.restart, f.mcus - sub.r * f.restart) * f.bpm;
-  Counts c{mine.x - base.x, {mine.y - base.y, mine.z - base.z, mine.w - base.w}};
+  const int32_t* counts3 = reinterpret_cast<const int32_t*>(p.s + f.counts3);
+  Counts c{mine.x - base.x, {mine.y - base.y, mine.z - base.z, mine.w - base.w,
+                             f.ncomp == 4 ? counts3[g] - counts3[sbase[sub.r]] : 0}};
   const int b0 = c.blocks;
   if (b0 < 0) {
     fail_file(p.status, f, -6);
@@ -767,12 +796,10 @@ __device__ __forceinline__ int chroma_at(const uint8_t* pl, int pw, int cw, int 
   return pl[(int64_t)(y / fv) * pw + x / fh];
 }
 
-__global__ void __launch_bounds__(kPixThreads) color_kernel(DecParams p) {
-  const DecFile& f = p.f[blockIdx.y];
-  const int64_t i = (int64_t)blockIdx.x * kPixThreads + threadIdx.x;
-  if (i >= (int64_t)f.oh * f.ow) return;
-  const int oy = (int)(i / f.ow), ox = (int)(i - (int64_t)oy * f.ow);
-  int sy = oy, sx = ox;
+// The decoded pixel (sy, sx) that output pixel (oy, ox) shows under the EXIF orientation.
+__device__ __forceinline__ void oriented_source(const DecFile& f, int oy, int ox, int& sy, int& sx) {
+  sy = oy;
+  sx = ox;
   switch (f.orient) {
     case 2: sx = f.w - 1 - ox; break;
     case 3: sy = f.h - 1 - oy; sx = f.w - 1 - ox; break;
@@ -783,19 +810,67 @@ __global__ void __launch_bounds__(kPixThreads) color_kernel(DecParams p) {
     case 8: sy = ox; sx = f.w - 1 - oy; break;
     default: break;
   }
+}
+
+// jdcolor.c's ycc_rgb_convert (tables FIX(x) = x * 2^16 rounded), cb and cr centred, clamped.
+__device__ __forceinline__ void ycc_rgb(int y, int cb, int cr, int& r, int& g, int& b) {
+  r = y + ((91881 * cr + 32768) >> 16);
+  b = y + ((116130 * cb + 32768) >> 16);
+  g = y + ((-22554 * cb + 32768 - 46802 * cr) >> 16);
+  r = min(max(r, 0), 255);
+  g = min(max(g, 0), 255);
+  b = min(max(b, 0), 255);
+}
+
+// Gray files and YCbCr files whose luma is not upsampled and whose two chroma planes share their
+// factors: every file the plain decoder takes.
+__global__ void __launch_bounds__(kPixThreads) color_kernel(DecParams p) {
+  const DecFile& f = p.f[blockIdx.y];
+  const int64_t i = (int64_t)blockIdx.x * kPixThreads + threadIdx.x;
+  if (f.general || i >= (int64_t)f.oh * f.ow) return;
+  const int oy = (int)(i / f.ow), ox = (int)(i - (int64_t)oy * f.ow);
+  int sy, sx;
+  oriented_source(f, oy, ox, sy, sx);
   const int y = p.s[f.plane[0] + (int64_t)sy * f.pw[0] + sx];
   int b = y, g = y, r = y;
   if (f.ncomp == 3) {
     const int fh = f.uh[1], fv = f.uv[1];
     const int cb = chroma_at(p.s + f.plane[1], f.pw[1], f.cw[1], f.chh[1], fh, fv, f.fancy, sy, sx) - 128;
     const int cr = chroma_at(p.s + f.plane[2], f.pw[2], f.cw[2], f.chh[2], fh, fv, f.fancy, sy, sx) - 128;
-    // jdcolor.c's tables: FIX(x) = x * 2^16 rounded
-    r = y + ((91881 * cr + 32768) >> 16);
-    b = y + ((116130 * cb + 32768) >> 16);
-    g = y + ((-22554 * cb + 32768 - 46802 * cr) >> 16);
-    r = min(max(r, 0), 255);
-    g = min(max(g, 0), 255);
-    b = min(max(b, 0), 255);
+    ycc_rgb(y, cb, cr, r, g, b);
+  }
+  uint8_t* o = f.out + (int64_t)oy * f.pitch + 3 * (int64_t)ox;
+  o[0] = (uint8_t)b;
+  o[1] = (uint8_t)g;
+  o[2] = (uint8_t)r;
+}
+
+// The other files (f.general): each component upsampled by its own factors (jinit_upsampler's
+// rule, chroma_at), then its colour space to BGR as cv2 reads it.  RGB: the planes as they are.
+// YCbCr: as above.  CMYK and YCCK: libjpeg's CMYK output (YCCK through ycck_cmyk_convert: C, M, Y
+// = 255 - the clamped YCbCr->RGB, K unchanged), then cv2's icvCvt_CMYK2BGR: B = K - ((255 - Y) *
+// K >> 8), and so on.
+__global__ void __launch_bounds__(kPixThreads) color_any_kernel(DecParams p) {
+  const DecFile& f = p.f[blockIdx.y];
+  const int64_t i = (int64_t)blockIdx.x * kPixThreads + threadIdx.x;
+  if (!f.general || i >= (int64_t)f.oh * f.ow) return;
+  const int oy = (int)(i / f.ow), ox = (int)(i - (int64_t)oy * f.ow);
+  int sy, sx;
+  oriented_source(f, oy, ox, sy, sx);
+  int v[kMaxComps] = {0, 0, 0, 0};
+#pragma unroll
+  for (int c = 0; c < kMaxComps; ++c)
+    if (c < f.ncomp)
+      v[c] = chroma_at(p.s + f.plane[c], f.pw[c], f.cw[c], f.chh[c], f.uh[c], f.uv[c], f.fancy, sy, sx);
+  int r = v[0], g = v[1], b = v[2];
+  if (f.space == kYcc || f.space == kYcck) ycc_rgb(v[0], v[1] - 128, v[2] - 128, r, g, b);
+  if (f.space == kCmyk || f.space == kYcck) {
+    const int k = v[3];
+    const int cc = f.space == kCmyk ? v[0] : 255 - r, m = f.space == kCmyk ? v[1] : 255 - g,
+              yy = f.space == kCmyk ? v[2] : 255 - b;
+    r = k - ((255 - cc) * k >> 8);
+    g = k - ((255 - m) * k >> 8);
+    b = k - ((255 - yy) * k >> 8);
   }
   uint8_t* o = f.out + (int64_t)oy * f.pitch + 3 * (int64_t)ox;
   o[0] = (uint8_t)b;
@@ -809,13 +884,16 @@ struct Comp {
 };
 struct Parsed {
   sqdet_jpeg_info info;
-  Comp comp[3];
+  Comp comp[kMaxComps];
+  int hmax, vmax;                      // the largest sampling factors (1 for gray)
+  Space space;
   uint16_t qt[4][64];                  // natural order
   bool have_q[4], have_dc[4], have_ac[4];
   uint8_t dc_bits[4][16], ac_bits[4][16];
   uint8_t dc_vals[4][256], ac_vals[4][256];
   bool progressive;                    // SOF2 (parse with progressive = true only)
   int64_t first_sos;                   // SOF2: the first SOS marker's offset
+  bool wide_mcu;                       // SOF2: more than 10 blocks in the frame's MCU
   int reduce;                          // the scale it decodes at: 1 / reduce
 };
 
@@ -860,7 +938,8 @@ const char* kReasons[] = {"ok", "malformed or truncated header", "progressive", 
                           "zero height or width", "larger than cv2 decodes",
                           "scan script libjpeg rejects", "scan script libjpeg warns on or overwrites",
                           "block-smoothed by libjpeg", "more than 256 scans",
-                          "more than 2^30 coded pixels, which cv2 decodes at this scale"};
+                          "more than 2^30 coded pixels, which cv2 decodes at this scale",
+                          "sampling libjpeg rejects"};
 
 // The largest file cv2.imdecode decodes: libjpeg's JPEG_MAX_DIMENSION per side, and cv2's default
 // CV_IO_MAX_IMAGE_PIXELS (it raises above that many pixels).
@@ -945,8 +1024,9 @@ int read_tables(const Segment& s, Parsed& P) {
 
 // The headers up to the first SOS, for a decode at scale 1 / reduce; the reason (SQDET_JPEG_*) and
 // what was read.  With `progressive`, an SOF2 frame is read as SOF0's is and the first SOS is left
-// to parse_scans.
-int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive, int reduce) {
+// to parse_scans.  With `any_layout`, 4 components, the RGB, CMYK and YCCK colour spaces and every
+// sampling libjpeg decodes are read too; the other sampling is SQDET_JPEG_BAD_SAMPLING.
+int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive, int reduce, bool any_layout) {
   memset(&P, 0, sizeof(P));
   P.reduce = reduce;
   sqdet_jpeg_info& I = P.info;
@@ -973,7 +1053,7 @@ int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive, int reduce) 
       ncomp = body[5];
       if (body[0] != 8) return SQDET_JPEG_PRECISION;
       if (bn != 6 + 3 * ncomp) return SQDET_JPEG_MALFORMED;
-      if (ncomp != 1 && ncomp != 3) return SQDET_JPEG_COMPONENTS;
+      if (ncomp != 1 && ncomp != 3 && !(any_layout && ncomp == 4)) return SQDET_JPEG_COMPONENTS;
       I.components = ncomp;
       for (int k = 0; k < ncomp; ++k) {
         Comp& c = P.comp[k];
@@ -990,7 +1070,22 @@ int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive, int reduce) 
       if ((int64_t)I.coded_height * I.coded_width > kMaxPixels)
         return (int64_t)((I.coded_height + reduce - 1) / reduce) * ((I.coded_width + reduce - 1) / reduce) > kMaxPixels
                    ? SQDET_JPEG_TOO_LARGE : SQDET_JPEG_CODED_TOO_LARGE;
-      if (ncomp == 3) {
+      P.hmax = P.vmax = 1;
+      int mcu_blocks = 0;
+      for (int k = 0; ncomp > 1 && k < ncomp; ++k) {
+        P.hmax = std::max(P.hmax, P.comp[k].h);
+        P.vmax = std::max(P.vmax, P.comp[k].v);
+        mcu_blocks += P.comp[k].h * P.comp[k].v;
+      }
+      if (ncomp > 1 && any_layout) {
+        // jinit_upsampler takes integral ratios only; a sequential file's one scan is
+        // interleaved, and jdinput.c's per_scan_setup allows 10 blocks per MCU
+        for (int k = 0; k < ncomp; ++k)
+          if (P.hmax % P.comp[k].h || P.vmax % P.comp[k].v) return SQDET_JPEG_BAD_SAMPLING;
+        // a progressive frame's MCU may be wider, if no interleaved scan is: parse_scans decides
+        if (m != 0xC2 && mcu_blocks > kMaxBlocks) return SQDET_JPEG_BAD_SAMPLING;
+        P.wide_mcu = mcu_blocks > kMaxBlocks;
+      } else if (ncomp == 3) {
         const int h = P.comp[0].h, v = P.comp[0].v;
         const bool luma_ok = (h == 1 && v == 1) || (h == 2 && v == 1) || (h == 1 && v == 2) ||
                              (h == 2 && v == 2) || (h == 4 && v == 1);
@@ -1029,11 +1124,16 @@ int parse(const uint8_t* b, int64_t n, Parsed& P, bool progressive, int reduce) 
           return SQDET_JPEG_MALFORMED;
       }
       // libjpeg's colour space of 3 components: YCbCr after a JFIF APP0; else as an Adobe APP14's
-      // transform says (0: RGB); else RGB for component ids 'R', 'G', 'B'
+      // transform says (0: RGB); else RGB for component ids 'R', 'G', 'B'.  Of 4: as an Adobe
+      // APP14's transform says (0: CMYK, anything else YCCK), CMYK without one
       if (ncomp == 3 && !jfif &&
           (adobe >= 0 ? adobe == 0
-                      : P.comp[0].id == 'R' && P.comp[1].id == 'G' && P.comp[2].id == 'B'))
-        return SQDET_JPEG_COLOR_TRANSFORM;
+                      : P.comp[0].id == 'R' && P.comp[1].id == 'G' && P.comp[2].id == 'B')) {
+        if (!any_layout) return SQDET_JPEG_COLOR_TRANSFORM;
+        P.space = kRgb;
+      } else {
+        P.space = ncomp == 1 ? kGray : ncomp == 3 ? kYcc : adobe > 0 ? kYcck : kCmyk;
+      }
       if (P.progressive) P.first_sos = s.at;
       else I.scan_offset = i;
       I.h_samp = ncomp == 1 ? 1 : P.comp[0].h;
@@ -1075,8 +1175,8 @@ void build_tab(const uint8_t* bits, const uint8_t* vals, HuffTab& t) {
 // component's IDCT size and upsampling factors at the file's scale; pw and ph its plane's.
 struct Layout {
   int mcu_cols, mcu_rows, mcus, bpm, restart, intervals, chunks, blocks, sub_max;
-  int isz[3], uh[3], uv[3];
-  int pw[3], ph[3];
+  int isz[kMaxComps], uh[kMaxComps], uv[kMaxComps];
+  int pw[kMaxComps], ph[kMaxComps];
   int64_t raw_len;
 };
 
@@ -1085,10 +1185,11 @@ Layout layout(const Parsed& P, int64_t file_len, int sub_bits) {
   Layout L{};
   const int H = I.coded_height, W = I.coded_width;
   const bool gray = I.components == 1;
-  const int hmax = gray ? 1 : P.comp[0].h, vmax = gray ? 1 : P.comp[0].v;
+  const int hmax = P.hmax, vmax = P.vmax;
   L.mcu_cols = (W + 8 * hmax - 1) / (8 * hmax);
   L.mcu_rows = (H + 8 * vmax - 1) / (8 * vmax);
-  L.bpm = gray ? 1 : hmax * vmax + 2;
+  L.bpm = 0;
+  for (int c = 0; c < I.components; ++c) L.bpm += gray ? 1 : P.comp[c].h * P.comp[c].v;
   // jpeg_calc_output_dimensions: luma's IDCT is m = 8 / reduce; another component's doubles
   // from m while below 8 and both divisibility conditions hold (4:2:0 chroma: 2m, the others m)
   const int m = 8 / P.reduce;
@@ -1112,6 +1213,13 @@ Layout layout(const Parsed& P, int64_t file_len, int sub_bits) {
   return L;
 }
 
+// Whether color_any_kernel converts the file: anything but gray and YCbCr with luma at the frame's
+// size and both chroma planes upsampled alike.
+bool general_layout(const Parsed& P, const Layout& L) {
+  return !(P.space == kGray || (P.space == kYcc && L.uh[0] == 1 && L.uv[0] == 1 &&
+                                L.uh[1] == L.uh[2] && L.uv[1] == L.uv[2]));
+}
+
 // The fields of a file's descriptor that follow from its frame header, its quantization tables
 // (as the components name them) included.
 void describe(const Parsed& P, const Layout& L, DecFile& f) {
@@ -1133,6 +1241,8 @@ void describe(const Parsed& P, const Layout& L, DecFile& f) {
   f.sub_max = L.sub_max;
   f.sub_bits = g_sub_bits;
   f.fancy = P.reduce < 8;              // jinit_upsampler: fancy only while luma's IDCT is above 1
+  f.space = P.space;
+  f.general = general_layout(P, L);
   int u = 0;
   for (int c = 0; c < I.components; ++c) {
     const Comp& cp = P.comp[c];
@@ -1151,7 +1261,7 @@ void describe(const Parsed& P, const Layout& L, DecFile& f) {
     f.pw[c] = L.pw[c];
     f.ph[c] = L.ph[c];
     // libjpeg's downsampled_width / _height at this scale
-    const int hmax = I.components == 1 ? 1 : P.comp[0].h, vmax = I.components == 1 ? 1 : P.comp[0].v;
+    const int hmax = P.hmax, vmax = P.vmax;
     f.cw[c] = (int)(((int64_t)I.coded_width * hc * L.isz[c] + 8 * hmax - 1) / (8 * hmax));
     f.chh[c] = (int)(((int64_t)I.coded_height * vc * L.isz[c] + 8 * vmax - 1) / (8 * vmax));
     for (int k = 0; k < 64; ++k) f.q[c][k] = (int16_t)P.qt[cp.tq][k];
@@ -1274,7 +1384,7 @@ __device__ __forceinline__ int corrections(const uint8_t* clean, int p, int16_t*
 __device__ int prog_interval(const DecFile& f, const ProgScan& S, const uint8_t* clean,
                              const HuffTab* tabs, int16_t* coef, int u0, int u1, int p, int end) {
   if (S.ss == 0) {                                       // DC first
-    int dc[3] = {0, 0, 0};
+    int dc[kMaxComps] = {0, 0, 0, 0};
 #pragma unroll 1
     for (int u = u0; u < u1; ++u) {
 #pragma unroll 1
@@ -1437,15 +1547,15 @@ __global__ void __launch_bounds__(kPixThreads) prog_dc_refine_kernel(ProgParams 
 
 // ---- host: every scan -------------------------------------------------------------------------
 struct PScan {
-  int ncomp, comp[3], ss, se, ah, al, restart;
-  uint8_t bits[3][16], vals[3][256];   // the tables in force at the scan
+  int ncomp, comp[kMaxComps], ss, se, ah, al, restart;
+  uint8_t bits[kMaxComps][16], vals[kMaxComps][256];   // the tables in force at the scan
   int64_t start, end;                  // its entropy-coded bytes
   int64_t markers;                     // the RSTn markers among them
 };
 struct Prog {
   std::vector<PScan> scans;
-  bool latched[3];
-  uint16_t q[3][64];
+  bool latched[kMaxComps];
+  uint16_t q[kMaxComps][64];
 };
 
 // The first byte at or after j that starts a marker other than RSTn (or n), and the RSTn markers
@@ -1482,7 +1592,7 @@ int parse_scans(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
   memset(G.latched, 0, sizeof(G.latched));
   memset(G.q, 0, sizeof(G.q));
   const int ncomp = P.info.components;
-  int cbits[3][64];
+  int cbits[kMaxComps][64];
   for (auto& row : cbits)
     for (int& x : row) x = -1;
   bool bogus = false, too_many = false;
@@ -1513,6 +1623,10 @@ int parse_scans(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
         if (c <= prev) return SQDET_JPEG_SAMPLING;       // out of the frame's order, or repeated
         prev = S.comp[k] = c;
       }
+      // jdinput.c's per_scan_setup: an interleaved scan's MCU is at most 10 blocks
+      int scan_blocks = 0;
+      for (int k = 0; ns > 1 && k < ns; ++k) scan_blocks += P.comp[S.comp[k]].h * P.comp[S.comp[k]].v;
+      if (scan_blocks > kMaxBlocks) return SQDET_JPEG_BAD_SAMPLING;
       S.ss = body[1 + 2 * ns];
       S.se = body[2 + 2 * ns];
       S.ah = body[3 + 2 * ns] >> 4;
@@ -1563,6 +1677,9 @@ int parse_scans(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
   if (too_many) return SQDET_JPEG_TOO_MANY_SCANS;
   if (bogus) return SQDET_JPEG_BOGUS_PROGRESSION;
   if (smoothed(ncomp, G, cbits)) return SQDET_JPEG_SMOOTHED;
+  // the coefficients are laid out in the frame's MCUs, of at most 10 blocks here; libjpeg decodes
+  // such a file, so it goes to cv2
+  if (P.wide_mcu) return SQDET_JPEG_SAMPLING;
   P.info.scan_offset = G.scans[0].start;
   return SQDET_JPEG_OK;
 }
@@ -1571,12 +1688,13 @@ int parse_scans(const uint8_t* b, int64_t n, Parsed& P, Prog& G) {
 struct Mode {
   bool progressive;
   int reduce;
+  bool any_layout;
   const char* suffix;                  // of the entry points' names in messages
 };
 
 // A file as the entry points read it: with `progressive`, SOF2 files too, with their scans.
 int parse_file(const uint8_t* b, int64_t n, const Mode& mode, Parsed& P, Prog& G) {
-  const int reason = parse(b, n, P, mode.progressive, mode.reduce);
+  const int reason = parse(b, n, P, mode.progressive, mode.reduce, mode.any_layout);
   if (reason || !P.progressive) return reason;
   return parse_scans(b, n, P, G);
 }
@@ -1589,12 +1707,12 @@ void scan_geometry(const Parsed& P, const Layout& L, const PScan& S, ProgScan& D
   D.ah = S.ah;
   D.al = S.al;
   D.single = S.ncomp == 1;
-  int uoff[3] = {0, 0, 0};
+  int uoff[kMaxComps] = {0, 0, 0, 0};
   for (int c = 1; c < ncomp; ++c) uoff[c] = uoff[c - 1] + P.comp[c - 1].h * P.comp[c - 1].v;
   if (D.single) {
     const int c = S.comp[0];
     const int hc = ncomp == 1 ? 1 : P.comp[c].h, vc = ncomp == 1 ? 1 : P.comp[c].v;
-    const int hmax = ncomp == 1 ? 1 : P.comp[0].h, vmax = ncomp == 1 ? 1 : P.comp[0].v;
+    const int hmax = P.hmax, vmax = P.vmax;
     const int64_t cw = ((int64_t)P.info.coded_width * hc + hmax - 1) / hmax;
     const int64_t chh = ((int64_t)P.info.coded_height * vc + vmax - 1) / vmax;
     D.cols = (int)((cw + 7) / 8);
@@ -1677,6 +1795,7 @@ struct Plan {
   int first = 0, dc_refine = 0;
   std::vector<int> depth;              // AC refinement items per depth
   int reduce = 1;                      // every file's scale: 1 / reduce
+  bool general = false;                // some file needs color_any_kernel
   int64_t scan_off = 0, item_off = 0, staging = 0, scratch = 0;
   int64_t marks = 0, marks_bytes = 0, coef = 0, coef_bytes = 0;
 };
@@ -1696,7 +1815,7 @@ void place(Plan& plan) {
   plan.scan_off = c.next((int64_t)sizeof(ProgScan) * (int64_t)plan.scans.size());
   plan.item_off = c.next((int64_t)sizeof(int2) * (int64_t)plan.items.size());
   for (size_t i = 0; i < ns; ++i) {
-    fd[i].tabs = c.next((int64_t)sizeof(HuffTab) * 6);
+    fd[i].tabs = c.next((int64_t)sizeof(HuffTab) * 2 * std::max(3, plan.in[i].P.info.components));
     fd[i].raw = c.next(plan.in[i].L.raw_len + 16);
   }
   size_t si = 0;
@@ -1725,6 +1844,7 @@ void place(Plan& plan) {
       fd[i].entry = c.next((int64_t)L.sub_max * 8);
       fd[i].exit_ = c.next((int64_t)L.sub_max * 8);
       fd[i].counts = c.next((int64_t)L.sub_max * 16);
+      if (plan.in[i].P.info.components == 4) fd[i].counts3 = c.next((int64_t)L.sub_max * 4);
     }
     for (int k = 0; k < plan.in[i].P.info.components; ++k)
       fd[i].plane[k] = c.next((int64_t)L.pw[k] * L.ph[k]);
@@ -1752,6 +1872,7 @@ int make_plan(const std::string& name, int n, const uint8_t* const* files, const
                                              kReasons[reason]);
     in.L = layout(in.P, lengths[i], g_sub_bits);
     in.index = i;
+    plan.general = plan.general || general_layout(in.P, in.L);
   }
   const auto prog = std::stable_partition(plan.in.begin(), plan.in.end(),
                                           [](const Input& in) { return !in.P.progressive; });
@@ -1761,7 +1882,7 @@ int make_plan(const std::string& name, int n, const uint8_t* const* files, const
   std::vector<std::vector<int2>> depth_items;
   std::vector<int2> dcref;
   for (size_t i = (size_t)plan.nseq; i < plan.in.size(); ++i) {
-    int chain[3] = {0, 0, 0};
+    int chain[kMaxComps] = {0, 0, 0, 0};
     for (const PScan& S : plan.in[i].G.scans) {
       ProgScan D{};
       D.file = (int)i;
@@ -1908,8 +2029,13 @@ int launch_decode(const Plan& plan, uint8_t* stage, uint8_t* scratch, int32_t* s
   if (plan.reduce > 1) idct_kernel<true><<<idct_grid, kPixThreads, 0, stream>>>(p);
   else idct_kernel<false><<<idct_grid, kPixThreads, 0, stream>>>(p);
   SQ_CHECK_LAUNCH("jpeg idct_kernel");
-  color_kernel<<<dim3((unsigned)((max_pix + kPixThreads - 1) / kPixThreads), (unsigned)n), kPixThreads, 0, stream>>>(p);
+  const dim3 pix_grid((unsigned)((max_pix + kPixThreads - 1) / kPixThreads), (unsigned)n);
+  color_kernel<<<pix_grid, kPixThreads, 0, stream>>>(p);
   SQ_CHECK_LAUNCH("jpeg color_kernel");
+  if (plan.general) {
+    color_any_kernel<<<pix_grid, kPixThreads, 0, stream>>>(p);
+    SQ_CHECK_LAUNCH("jpeg color_any_kernel");
+  }
   return SQDET_OK;
 }
 
@@ -1966,21 +2092,34 @@ int decode_entry(int n, const uint8_t* const* files_host, const int64_t* lengths
                        status_dev, (cudaStream_t)stream);
 }
 
-constexpr Mode kPlain{false, 1, ""}, kProgressive{true, 1, "_progressive"};
+constexpr Mode kPlain{false, 1, false, ""}, kProgressive{true, 1, false, "_progressive"};
 
-// A sqdet_jpeg_decode_params as a Mode; false (with the error set) when it is not one.
-bool params_mode(const char* plain, const sqdet_jpeg_decode_params* params, Mode& mode) {
-  const std::string name = std::string(plain) + "_params";
-  if (!params) return fail(SQDET_ERR_INVALID_ARG, name + ": params is null"), false;
-  const int s = params->scale_denom;
-  if (params->progressive != 0 && params->progressive != 1)
+// A sqdet_jpeg_decode_options as a Mode, its functions named with `suffix` in messages; false
+// (with the error set) when it is not one.
+bool options_mode(const char* plain, const char* suffix, const sqdet_jpeg_decode_options* o, Mode& mode) {
+  const std::string name = std::string(plain) + suffix;
+  if (!o) return fail(SQDET_ERR_INVALID_ARG, name + ": options is null"), false;
+  const int s = o->scale_denom;
+  if (o->progressive != 0 && o->progressive != 1)
     return fail(SQDET_ERR_INVALID_ARG, name + ": progressive must be 0 or 1"), false;
   if (s != 1 && s != 2 && s != 4 && s != 8)
     return fail(SQDET_ERR_INVALID_ARG, name + ": scale_denom must be 1, 2, 4 or 8"), false;
-  if (params->reserved[0] || params->reserved[1])
-    return fail(SQDET_ERR_INVALID_ARG, name + ": reserved must be 0"), false;
-  mode = Mode{params->progressive == 1, s, "_params"};
+  if (o->any_layout != 0 && o->any_layout != 1)
+    return fail(SQDET_ERR_INVALID_ARG, name + ": any_layout must be 0 or 1"), false;
+  for (const int32_t r : o->reserved)
+    if (r) return fail(SQDET_ERR_INVALID_ARG, name + ": reserved must be 0"), false;
+  mode = Mode{o->progressive == 1, s, o->any_layout == 1, suffix};
   return true;
+}
+
+// A sqdet_jpeg_decode_params as a Mode: the options {progressive, scale_denom, any_layout = 0}.
+bool params_mode(const char* plain, const sqdet_jpeg_decode_params* params, Mode& mode) {
+  if (!params) return fail(SQDET_ERR_INVALID_ARG, std::string(plain) + "_params: params is null"), false;
+  sqdet_jpeg_decode_options o{};
+  o.progressive = params->progressive;
+  o.scale_denom = params->scale_denom;
+  o.reserved[0] = params->reserved[0] | params->reserved[1];
+  return options_mode(plain, "_params", &o, mode);
 }
 }  // namespace
 }  // namespace sqdet
@@ -2067,6 +2206,40 @@ int sqdet_decode_jpeg_params(int n, const uint8_t* const* files_host, const int6
                              void* stream) {
   Mode mode;
   if (!params_mode("sqdet_decode_jpeg", params, mode)) return SQDET_ERR_INVALID_ARG;
+  return decode_entry(n, files_host, lengths, out_planes, out_pitches, staging_pinned, staging_bytes,
+                      scratch_dev, scratch_bytes, status_dev, stream, mode);
+}
+
+int sqdet_jpeg_parse_options(const uint8_t* file, int64_t len, const sqdet_jpeg_decode_options* options,
+                             sqdet_jpeg_info* out) {
+  Mode mode;
+  if (!options_mode("sqdet_jpeg_parse", "_options", options, mode)) return SQDET_ERR_INVALID_ARG;
+  return parse_entry(file, len, out, mode);
+}
+
+int64_t sqdet_jpeg_decode_staging_bytes_options(int n, const uint8_t* const* files_host,
+                                                const int64_t* lengths,
+                                                const sqdet_jpeg_decode_options* options) {
+  Mode mode;
+  if (!options_mode("sqdet_jpeg_decode_staging_bytes", "_options", options, mode)) return -1;
+  return staging_bytes_entry(n, files_host, lengths, mode);
+}
+
+int64_t sqdet_jpeg_decode_scratch_bytes_options(int n, const uint8_t* const* files_host,
+                                                const int64_t* lengths,
+                                                const sqdet_jpeg_decode_options* options) {
+  Mode mode;
+  if (!options_mode("sqdet_jpeg_decode_scratch_bytes", "_options", options, mode)) return -1;
+  return scratch_bytes_entry(n, files_host, lengths, mode);
+}
+
+int sqdet_decode_jpeg_options(int n, const uint8_t* const* files_host, const int64_t* lengths,
+                              const sqdet_jpeg_decode_options* options, uint8_t* const* out_planes,
+                              const int64_t* out_pitches, void* staging_pinned, int64_t staging_bytes,
+                              void* scratch_dev, int64_t scratch_bytes, int32_t* status_dev,
+                              void* stream) {
+  Mode mode;
+  if (!options_mode("sqdet_decode_jpeg", "_options", options, mode)) return SQDET_ERR_INVALID_ARG;
   return decode_entry(n, files_host, lengths, out_planes, out_pitches, staging_pinned, staging_bytes,
                       scratch_dev, scratch_bytes, status_dev, stream, mode);
 }

@@ -95,28 +95,34 @@ jpeg_bytes = file_bytes
 JPEG_TOO_LARGE = 10       # SQDET_JPEG_TOO_LARGE: past cv2's limits, so cv2.imdecode refuses it too
 JPEG_BAD_PROGRESSION = 11  # SQDET_JPEG_BAD_PROGRESSION: cv2.imdecode returns None
 JPEG_CODED_TOO_LARGE = 15  # SQDET_JPEG_CODED_TOO_LARGE: cv2.imdecode decodes it at this scale
+JPEG_COMPONENTS = 6       # SQDET_JPEG_COMPONENTS: with any_layout, cv2.imdecode returns None too
+JPEG_BAD_SAMPLING = 16    # SQDET_JPEG_BAD_SAMPLING: cv2.imdecode returns None
 # the scales decode_jpeg_device takes: cv2's IMREAD_COLOR and IMREAD_REDUCED_COLOR_2, _4 and _8
 REDUCTIONS = (1, 2, 4, 8)
 
 
-def _decode_call(progressive, reduce):
-  """(suffix of the C functions, their sqdet_jpeg_decode_params or None): the plain or
-  _progressive functions at full size, the _params ones at a reduced scale."""
+def _decode_call(progressive, reduce, any_layout=False):
+  """(suffix of the C functions, their sqdet_jpeg_decode_params / _options or None): the plain or
+  _progressive functions at full size, the _params ones at a reduced scale, the _options ones
+  with any_layout."""
   if reduce not in REDUCTIONS:
     raise ValueError('reduce must be one of %s, got %r' % (', '.join(map(str, REDUCTIONS)), reduce))
+  if any_layout:
+    return '_options', _lib.JpegDecodeOptions(int(bool(progressive)), reduce, 1)
   if reduce == 1:
     return ('_progressive' if progressive else ''), None
   return '_params', _lib.JpegDecodeParams(int(bool(progressive)), reduce)
 
 
-def jpeg_info(file_bytes, progressive=False, reduce=1):
+def jpeg_info(file_bytes, progressive=False, reduce=1, any_layout=False):
   """sqdet_jpeg_parse of one file -> dict: height and width of the decoded frame (after the EXIF
   orientation, and at scale 1 / reduce), coded_height, coded_width, components, h_samp, v_samp
   (luma sampling), orientation, restart_interval, supported (bool), reason (a SQDET_JPEG_* code)
   and reason_text (the library's words for it).  With progressive, sqdet_jpeg_parse_progressive:
   whether decode_jpeg_device(..., progressive=True) decodes it; with reduce 2, 4 or 8,
-  sqdet_jpeg_parse_params: whether decode_jpeg_device(..., reduce=reduce) does.  Host only."""
-  kind, params = _decode_call(progressive, reduce)
+  sqdet_jpeg_parse_params: whether decode_jpeg_device(..., reduce=reduce) does; with any_layout,
+  sqdet_jpeg_parse_options: whether decode_jpeg_device(..., any_layout=True) does.  Host only."""
+  kind, params = _decode_call(progressive, reduce, any_layout)
   b = bytes(file_bytes)
   info = _lib.JpegInfo()
   buf = C.create_string_buffer(b, len(b))
@@ -157,7 +163,7 @@ class _Staging:
 _staging = {}
 
 
-def decode_jpeg_device(files, device, stream=None, *, progressive=False, reduce=1):
+def decode_jpeg_device(files, device, stream=None, *, progressive=False, reduce=1, any_layout=False):
   """JPEG files (bytes-like, on the host) -> (frames, status): frames[i] is a uint8 [H, W, 3] BGR
   CUDA tensor on `device` with exactly the pixels of cv2.imdecode(files[i], cv2.IMREAD_COLOR), and
   status an int32 [n] CUDA tensor, 0 where the file decoded and negative where its entropy-coded
@@ -191,9 +197,17 @@ def decode_jpeg_device(files, device, stream=None, *, progressive=False, reduce=
   ceil(H / reduce) x ceil(W / reduce) before the orientation, from libjpeg's scaled IDCTs, so a
   12 MP camera file takes a 2.3 MB frame at 1/4 instead of 36 MB.  The size limit then applies to
   the reduced frame, as in cv2; a file of more than 2^30 coded pixels whose reduced frame fits
-  still raises ValueError, and cv2.imdecode decodes it.  Any other reduce raises ValueError."""
+  still raises ValueError, and cv2.imdecode decodes it.  Any other reduce raises ValueError.
+
+  any_layout=True (sqdet_decode_jpeg_options) decodes, besides those, the colour spaces and
+  samplings of every other Huffman-coded 8-bit file cv2.imdecode reads, again to exactly its
+  pixels, and combines with progressive and reduce: CMYK and YCCK files (4 components, as
+  Photoshop and Pillow write them), RGB-coded files (Adobe transform 0, or ids 'R', 'G', 'B'
+  without JFIF) and any sampling with integral ratios and at most 10 blocks per interleaved MCU.
+  Files libjpeg rejects (other sampling, 2 or more than 4 components) raise ValueError saying that
+  cv2.imdecode does not decode them either."""
   import torch
-  kind, params = _decode_call(progressive, reduce)
+  kind, params = _decode_call(progressive, reduce, any_layout)
   files = [bytes(f) for f in files]
   n = len(files)
   if not 1 <= n <= 128:
@@ -207,11 +221,13 @@ def decode_jpeg_device(files, device, stream=None, *, progressive=False, reduce=
   for i, f in enumerate(files):
     if len(f) < 4:
       raise ValueError('file %d: not a JPEG file (%d bytes)' % (i, len(f)))
-    info = jpeg_info(f, progressive, reduce)
+    info = jpeg_info(f, progressive, reduce, any_layout)
     if not info['supported']:
+      refused = (JPEG_TOO_LARGE, JPEG_BAD_PROGRESSION) + \
+          ((JPEG_COMPONENTS, JPEG_BAD_SAMPLING) if any_layout else ())
       raise ValueError('file %d: not supported (%s); %s' % (
           i, info['reason_text'], 'nor does cv2.imdecode decode it'
-          if info['reason'] in (JPEG_TOO_LARGE, JPEG_BAD_PROGRESSION) else 'decode it with cv2.imdecode'))
+          if info['reason'] in refused else 'decode it with cv2.imdecode'))
     infos.append(info)
   lib = _lib.load()
   bufs = [C.create_string_buffer(f, len(f)) for f in files]
